@@ -1,6 +1,6 @@
-# Build libb200gan.so (sm_100a only).  `make` here or __graft_entry__.build() -- same commands.
+# Build libb200gan.so (sm_90a, H100, only).  `make` here or __graft_entry__.build() -- same commands.
 NVCC ?= /usr/local/cuda/bin/nvcc
-ARCH := -gencode arch=compute_100a,code=sm_100a
+ARCH := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall,-Wno-unused-function -Xptxas -v
 SRC := gan_deeplearning4j_b200/csrc
 OUT := gan_deeplearning4j_b200/lib

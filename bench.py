@@ -1,11 +1,11 @@
 #!/usr/bin/env python
 """bench.py -- images/sec for the full adversarial G+D step (BASELINE.json metric) on synthetic 64x64x3 batches.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c2|c4|c5]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config c2|c4|c5] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one pass of the hot path (SURVEY.md 8d): x_fake = G(z_d); D update on (x_real, y_real)+(x_fake, y_fake);
-G update through D on z_g with labels 1 -- J:408-471 without I/O -- through libb200gan.so (hand-written sm_100a CUDA).
+G update through D on z_g with labels 1 -- J:408-471 without I/O -- through libb200gan.so (hand-written sm_90a CUDA for the H100).
 Workload at N=1: BASELINE configs[1] = 64x64x3 DCGAN, z=100, bf16, batch 128 per GPU (weak scaling: 128/GPU).
 
 `value`   : images/sec with inputs resident in HBM, per-step CUDA-event time on the launching stream, max over ranks.
@@ -18,7 +18,11 @@ Workload at N=1: BASELINE configs[1] = 64x64x3 DCGAN, z=100, bf16, batch 128 per
             separate bias / activation / BatchNorm / Adam passes; SURVEY.md 8d(i), P:104-108), pinned to the NumPy oracle by
             tests/test_oracle.py, on this box's physical cores at the SAME batch as the GPU arm.  B2G_CPU_ENGINE=torch|numpy select the
             oneDNN/MKL port or the NumPy oracle instead.
-`extra`   : short runs of the other BASELINE configurations (C4 128x128, C5 MLP-GAN) so that the driver's record carries them.
+`extra`   : short runs of the other BASELINE configurations (C4 128x128, C5 MLP-GAN) so that the record carries them.
+--dump-outputs DIR: after the timed steps, what the last timed step left for a caller -- its three losses and the updated G / D parameters --
+            as DIR/<name>.npy (float32), at most 64 MB in all: where the whole vectors would not fit (C4), a fixed-seed sample of each large
+            vector is written with its element indices (DIR/<name>_index.npy, float64).  Inputs and initial weights are seeded, so two builds
+            can be compared output for output.  --impl ours only.
 --impl reference: that CPU restatement IS the reference arm (DL4J itself cannot run: no JVM in the image; SURVEY.md 8c).
 """
 from __future__ import annotations
@@ -66,12 +70,13 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"], bf16_tflops_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback")
+    # NVIDIA's H100 SXM data sheet (dense bf16, HBM3 at 700 W): a ceiling, not a measured rate
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """SM clock / throttle reasons sampled DURING the timed region (B200_PROFILING.md).  NVML is polled from a thread every ~2 ms (the
-    driver's 20-step timed region is ~25 ms: `nvidia-smi -lms 20` yielded 0-1 samples there in round 1); nvidia-smi is the fallback."""
+    """SM clock / throttle reasons sampled DURING the timed region.  NVML is polled from a thread every ~2 ms: a short timed region
+    yields few samples at a coarser period."""
 
     def __init__(self, index):
         self.index, self.samples, self._stop, self._thr, self.nv = index, [], threading.Event(), None, None
@@ -280,19 +285,9 @@ def tensor_rooflines(b, ctx, cfg, batch, peaks):
     tot_ms = sum(r["ms"] * r["count"] for r in ok); tot_fl = sum(r["flops"] * r["count"] for r in ok)
     dom = max(ok, key=lambda r: r["ms"] * r["count"])
     ach = dom["flops"] / (dom["ms"] * 1e-3) / 1e12
-    prof = None
-    pj = os.path.join(ROOT, "profiles", "r02_ncu_dominant.json")          # dram bytes per launch of the dominant kernel from the committed `ncu --set full` capture
-    if os.path.exists(pj):
-        try:
-            prof = json.load(open(pj))
-        except Exception:
-            prof = None
     roof = {"bound": "tensor", "achieved": ach, "peak": peaks["bf16_tflops"], "unit": "TFLOP/s", "frac": ach / peaks["bf16_tflops"],
-            "traffic": ((prof or {}).get("workloads", {}).get(dom["name"]) or {}).get("dram_bytes_per_launch"),
-            "traffic_l2_to_sm": ((prof or {}).get("workloads", {}).get(dom["name"]) or {}).get("l2_to_sm_bytes_per_launch"),
-            "traffic_unit": "bytes/launch: `traffic` = ncu dram__bytes_read.sum + dram__bytes_write.sum, `traffic_l2_to_sm` = l1tex__m_xbar2l1tex_read_bytes.sum (profiles/r02_ncu_dominant.json, one `ncu --set full` launch of this workload)",
             "algorithmic_bytes": dom["bytes"], "kernel": f"{dom['kernel']}: {dom['name']}", "flops_per_launch": dom["flops"], "ms_per_launch": dom["ms"],
-            "share_of_tensor_time": dom["ms"] * dom["count"] / tot_ms, "peak_source": peaks["source"] + " (burst cuBLAS bf16)",
+            "share_of_tensor_time": dom["ms"] * dom["count"] / tot_ms, "peak_source": peaks["source"],
             "how": "the tensor-core launch with the largest time share of the step, timed alone with CUDA events on the library stream (10 launches, warm L2)"}
     fam = {"launches_per_step": sum(r["count"] for r in ok), "gflop_per_step": tot_fl / 1e9, "ms_per_step_if_serialised": tot_ms,
            "achieved_tflops": tot_fl / (tot_ms * 1e-3) / 1e12, "frac": tot_fl / (tot_ms * 1e-3) / 1e12 / peaks["bf16_tflops"],
@@ -338,6 +333,38 @@ def timed_resident_steps(ctx, gan, n, steps, warmup, barrier):
         step_ms.append(gan.last_step_ms())
     barrier()
     return step_ms
+
+
+DUMP_BUDGET_BYTES = 64 * 10**6     # everything --dump-outputs writes, .npy headers included
+DUMP_WHOLE_ELEMS = 4096           # arrays this small are always written whole
+NPY_HEADER_BYTES = 128
+
+
+def dump_plan(sizes, budget=DUMP_BUDGET_BYTES):
+    """{name: element count} -> {name: elements to write}.  Everything, if the whole float32 arrays fit the budget; otherwise the large arrays
+    keep the same fraction of their elements, each kept element costing 4 B of value and 8 B of float64 index."""
+    if sum(4 * n + NPY_HEADER_BYTES for n in sizes.values()) <= budget:
+        return dict(sizes)
+    small = {k: n for k, n in sizes.items() if n <= DUMP_WHOLE_ELEMS}
+    large = {k: n for k, n in sizes.items() if n > DUMP_WHOLE_ELEMS}
+    avail = budget - sum(4 * n + NPY_HEADER_BYTES for n in small.values()) - 2 * NPY_HEADER_BYTES * len(large)
+    frac = avail / (12 * sum(large.values()))
+    return dict(small, **{k: min(n, int(n * frac)) for k, n in large.items()})
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes {name: array} as float32 DIR/<name>.npy within DUMP_BUDGET_BYTES; a sampled array also gets DIR/<name>_index.npy (float64),
+    the sorted element indices drawn with a seed fixed per name, so that two builds' dumps compare element for element."""
+    import zlib
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: np.asarray(a, np.float32).ravel() for k, a in arrays.items()}
+    plan = dump_plan({k: a.size for k, a in arrays.items()})
+    for name, a in arrays.items():
+        if plan[name] < a.size:
+            idx = np.sort(np.random.default_rng(zlib.crc32(name.encode())).choice(a.size, plan[name], replace=False))
+            np.save(os.path.join(out_dir, name + "_index.npy"), idx.astype(np.float64))
+            a = a[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def run_ours(args, cfg, rank, world, local_rank):
@@ -402,6 +429,8 @@ def run_ours(args, cfg, rank, world, local_rank):
     launches = ctx.launch_count() - launches0; simt = G.simt_gemm_calls() + D.simt_gemm_calls() - simt0
     clocks = sampler.stop() if rank == 0 else None
     losses = gan.losses()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"losses": losses, "g_params": G.params(), "d_params": D.params()})
     total_ms = float(sum(step_ms))
     # ---- end to end through the host-buffer entry point
     lo = np.zeros(3, np.float32)
@@ -454,7 +483,7 @@ def run_ours(args, cfg, rank, world, local_rank):
                        "fake_bn": "inference (gen.output, J:420)", "cuda_graph": os.environ.get("B2G_GRAPH_NCCL", "1") != "0" or world == 1, "step": "G(z_d) -> D update on real|fake -> G update through D", **({"dp": dp_opts} if world > 1 else {})},
             "roofline": roof, "roofline_family": fam, "hbm": hbm,
             "step_roofline": {"algorithmic_gflop_per_image": F / 1e9, "achieved_tflops_per_gpu": step_tf, "peak": peaks["bf16_tflops_sustained"], "frac": step_tf / peaks["bf16_tflops_sustained"],
-                              "peak_source": peaks["source"] + " (sustained cuBLAS bf16)"},
+                              "peak_source": peaks["source"]},
             "cpu_baseline": cpu_base,
             "e2e": {"value": e2e_ips, "unit": unit, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
             "gpu_launches": int(launches), "launches_per_step": launches / max(1, args.steps), "simt_gemm_launches_per_step": simt / max(1, args.steps),
@@ -475,7 +504,11 @@ def main():
     ap.add_argument("--config", default="c2", choices=sorted(CONFIGS))
     ap.add_argument("--no-cpu", dest="no_cpu", action="store_true", help="skip the cpu_baseline leg (A/B runs of kernel switches; not for reported lines)")
     ap.add_argument("--no-extra", dest="no_extra", action="store_true", help="skip the short C4 / C5 runs appended under `extra`")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", metavar="DIR", default=None,
+                    help="write the last timed step's losses and updated parameters to DIR/<name>.npy (at most 64 MB; --impl ours)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes what the GPU path computed: it needs --impl ours")
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1")); local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     cfg = CONFIGS[args.config]
     if args.impl == "reference":

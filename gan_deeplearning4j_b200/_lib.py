@@ -1,7 +1,7 @@
 """ctypes binding of libb200gan.so -- the same C-ABI (include/b200gan.h) the JNI shim exposes to the Java facade.
 
 There is no CPU fallback: importing works anywhere (so that symbol/ABI tests run without a GPU), but every
-compute entry point needs the CUDA library and an sm_100 device and raises B200GanError otherwise.
+compute entry point needs the CUDA library and an sm_90 device and raises B200GanError otherwise.
 """
 from __future__ import annotations
 
@@ -112,7 +112,7 @@ def load():
     if _lib is not None:
         return _lib
     if not os.path.exists(LIB_PATH):
-        raise B200GanError(-7, f"{LIB_PATH} is missing: build it with `make` (nvcc, sm_100a). There is no CPU fallback.")
+        raise B200GanError(-7, f"{LIB_PATH} is missing: build it with `make` (nvcc, sm_90a). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH, mode=C.RTLD_GLOBAL)
     for name, (res, args) in PROTOTYPES.items():
         fn = getattr(lib, name)        # AttributeError if the library does not export a declared symbol

@@ -11,11 +11,11 @@ namespace b2g {
 
 #define LAUNCHED() do { ++::b2g::g_launch_count; } while (0)
 
-// Programmatic dependent launch (default on; B2G_PDL=0 disables; measured on B200 round 2: 1.116 -> 1.097 ms per C2 step): a kernel launched with the attribute may be SCHEDULED while its predecessor in the stream is
+// Programmatic dependent launch (default on; B2G_PDL=0 disables): a kernel launched with the attribute may be SCHEDULED while its predecessor in the stream is
 // still running (as soon as every predecessor CTA has exited or called pdl_trigger()), so the ~2 us launch latency and the successor's
 // prologue overlap the predecessor's tail; pdl_wait() -- the first thing every kernel of this library does before touching global memory --
-// blocks until the predecessor has completed and flushed.  Round 1 triggered at the top of EVERY kernel and measured a 5 % loss (waiting
-// successor CTAs held SM slots that the predecessor's later waves needed); here only single-wave kernels trigger early, all others
+// blocks until the predecessor has completed and flushed.  An early trigger in a multi-wave kernel lets waiting successor CTAs hold SM
+// slots that the predecessor's later waves need, so only single-wave kernels trigger early, all others
 // trigger implicitly when their CTAs exit.  Both instructions are no-ops for a launch without the attribute.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }

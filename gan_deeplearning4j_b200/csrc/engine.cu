@@ -84,7 +84,7 @@ struct LayerRT {
   ConvGeom geom{};                                             // conv-equivalent geometry (N filled per call)
   int64_t off_W = -1, n_W = 0, off_b = -1, off_gamma = -1, off_beta = -1, off_mean = -1, off_var = -1;
   int64_t off_W_bf = -1;                                       // bf16 operand copy [A][taps][B] (written by the updater itself); serves fprop, dgrad (MN-major tiles) and wgrad
-  int64_t off_Wps_bf = -1;                                     // packed [16][9][O] weights of the tcgen05 pixel-shuffle transposed conv (<= 4 image channels)
+  int64_t off_Wps_bf = -1;                                     // packed [16][9][O] weights of the tensor-core pixel-shuffle transposed conv (<= 4 image channels)
   int wA = 0, wTaps = 0, wB = 0;                               // internal weight layout [A][taps][B]
   void* out = nullptr; bool out_alias = false;
   void* probs = nullptr;                                       // OUTPUT / LOSS: sigmoid(logits)
@@ -96,7 +96,7 @@ struct LayerRT {
   bool stats_by_producer = false, bwd_premul = false;          // set per pass: the producing GEMM's epilogue has already filled acc_fwd / (acc_bwd and eps = dy')
   int fused_act = ACT_IDENTITY; float fused_alpha = 0.f;       // BN followed by an ActivationLayer
   bool act_fused_into_prev = false;
-  float* wg_part = nullptr; size_t wg_part_floats = 0;         // split-K partials of this layer's tcgen05 weight gradient (reduced by ONE k_reduce_multi per pass)
+  float* wg_part = nullptr; size_t wg_part_floats = 0;         // split-K partials of this layer's tensor-core weight gradient (reduced by ONE k_reduce_multi per pass)
   bool has_gemm() const { return d.type == B2G_LAYER_CONV2D || d.type == B2G_LAYER_DECONV2D || d.type == B2G_LAYER_DENSE || d.type == B2G_LAYER_OUTPUT; }
 };
 
@@ -274,7 +274,7 @@ static int32_t net_alloc(b2g_net* n) {
       scratch = std::max(scratch, k_tc_edge_wgrad_scratch_floats(g));
       scratch = std::max(scratch, k_colsum_scratch_floats(std::max(l.oc, l.ic)));
       max_w = std::max(max_w, (size_t)l.n_W);
-      // split-K partials of the tcgen05 weight gradients stay in a per-layer region until the pass's single k_reduce_multi launch
+      // split-K partials of the tensor-core weight gradients stay in a per-layer region until the pass's single k_reduce_multi launch
       if (n->prec == PREC_BF16 && n->ctx->tc_ok && !l.d.frozen) {
         l.wg_part_floats = std::max(k_tc_wgrad_scratch_floats(g), k_tc_edge_wgrad_scratch_floats(g));
         if (l.wg_part_floats) B2(dalloc(n, &l.wg_part, sizeof(float) * l.wg_part_floats));
@@ -383,11 +383,11 @@ static const void* w_ptr(const b2g_net* n, const LayerRT& l, int* wprec) {
   *wprec = PREC_F32; return n->params + l.off_W;
 }
 
-// tcgen05 versions of the <= 4-image-channel layers (B2G_NO_TC_EDGE=1 keeps the SIMT kernels of kernels_edge.cu)
+// tensor-core versions of the <= 4-image-channel layers (B2G_NO_TC_EDGE=1 keeps the SIMT kernels of kernels_edge.cu)
 static inline bool tc_on(const b2g_net* n) { return n->prec == PREC_BF16 && n->ctx->tc_ok; }
 static bool tc_edge_on(const b2g_net* n) { static int on = -1; if (on < 0) on = getenv("B2G_NO_TC_EDGE") ? 0 : 1; return on && tc_on(n); }
 static inline cudaStream_t fstream(const b2g_net* n) { return n->fwd_stream ? n->fwd_stream : n->ctx->stream; }
-// A BF16 net whose GEMM-shaped op has no tcgen05 kernel runs it on the SIMT kernels: counted (b2g_net_simt_gemm_calls, bench.py prints
+// A BF16 net whose GEMM-shaped op has no tensor-core kernel runs it on the SIMT kernels: counted (b2g_net_simt_gemm_calls, bench.py prints
 // it per step) so that a shape falling off the tensor-core path is visible, never silent.  The by-design skinny layers (<= 4 units on one
 // side, K = 100 G-first) are counted too.
 static inline void note_simt(b2g_net* n) { if (n->prec == PREC_BF16) ++n->simt_gemm_calls; }
@@ -401,7 +401,7 @@ static int32_t gemm_fprop(b2g_net* n, const LayerRT& l, const ConvGeom& g, const
   cudaStream_t s = fstream(n); int wp; const void* w = w_ptr(n, l, &wp);
   if (fused) *fused = false;
   if (scale) {       // folded epilogue: tensor-core or SIMT GEMM kernels only
-    if (tc_on(n) && tc_fprop_supported(g)) { TcEpi e{}; e.mode = EPI_PLAIN; e.scale = scale; return k_tc_fprop(g, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)out, act, alpha, s, &e) == 0 ? 0 : fail(B2G_ERR_CUDA, "tcgen05 fprop launch failed"); }
+    if (tc_on(n) && tc_fprop_supported(g)) { TcEpi e{}; e.mode = EPI_PLAIN; e.scale = scale; return k_tc_fprop(g, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)out, act, alpha, s, &e) == 0 ? 0 : fail(B2G_ERR_CUDA, "tensor-core fprop launch failed"); }
     note_simt(n); k_simt_fprop(n->prec, wp, g, x, w, bias, out, act, alpha, s, scale); return 0;
   }
   if (tc_edge_on(n) && tc_edge_conv_supported(g) && k_tc_edge_conv(g, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)out, act, alpha, s) == 0) return 0;
@@ -410,7 +410,7 @@ static int32_t gemm_fprop(b2g_net* n, const LayerRT& l, const ConvGeom& g, const
   if (tc_on(n) && tc_fprop_supported(g)) {
     if (fuse && k_tc_fprop(g, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)out, act, alpha, s, fuse) == 0) { if (fused) *fused = true; return 0; }
     if (k_tc_fprop(g, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)out, act, alpha, s) == 0) return 0;
-    return fail(B2G_ERR_CUDA, "tcgen05 fprop launch failed");
+    return fail(B2G_ERR_CUDA, "tensor-core fprop launch failed");
   }
   note_simt(n); k_simt_fprop(n->prec, wp, g, x, w, bias, out, act, alpha, s); return 0;
 }
@@ -419,13 +419,13 @@ static int32_t gemm_dgrad(b2g_net* n, const LayerRT& l, const ConvGeom& g, const
   cudaStream_t s = fstream(n); int wp; const void* w = w_ptr(n, l, &wp);
   if (fused) *fused = false;
   if (scale) {
-    if (tc_on(n) && tc_dgrad_supported(g) && !edge_deconv_small_c_supported(g)) { TcEpi e{}; e.mode = EPI_PLAIN; e.scale = scale; return k_tc_dgrad(g, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)dx, act, alpha, s, &e) == 0 ? 0 : fail(B2G_ERR_CUDA, "tcgen05 dgrad launch failed"); }
+    if (tc_on(n) && tc_dgrad_supported(g) && !edge_deconv_small_c_supported(g)) { TcEpi e{}; e.mode = EPI_PLAIN; e.scale = scale; return k_tc_dgrad(g, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)dx, act, alpha, s, &e) == 0 ? 0 : fail(B2G_ERR_CUDA, "tensor-core dgrad launch failed"); }
     note_simt(n); k_simt_dgrad(n->prec, wp, g, dy, w, bias, dx, act, alpha, s, scale); return 0;
   }
   if (tc_edge_on(n) && l.off_Wps_bf >= 0 && tc_deconv_ps_supported(g)) {
     const TcEpi* f = (fuse && fuse->mode == EPI_ACTBWD) ? fuse : nullptr;
     if (k_tc_deconv_ps(g, (const __nv_bfloat16*)dy, n->shadow + l.off_Wps_bf, bias, (__nv_bfloat16*)dx, act, alpha, s, f) == 0) { if (fused) *fused = f != nullptr; return 0; }
-    return fail(B2G_ERR_CUDA, "tcgen05 pixel-shuffle deconv launch failed");
+    return fail(B2G_ERR_CUDA, "tensor-core pixel-shuffle deconv launch failed");
   }
   if (edge_deconv_small_c_supported(g)) { note_simt(n); k_edge_deconv_small_c(n->prec, wp, g, dy, w, bias, dx, act, alpha, s); return 0; }
   if (dense_small_o_supported(g) && !bias && act == ACT_IDENTITY) { note_simt(n); k_dense_small_o_dgrad(n->prec, wp, g, dy, w, dx, s); return 0; }
@@ -436,13 +436,13 @@ static int32_t gemm_dgrad(b2g_net* n, const LayerRT& l, const ConvGeom& g, const
     if (tc_fprop_supported(t)) {
       if (fuse && k_tc_fprop(t, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)dx, act, alpha, s, fuse, 1) == 0) { if (fused) *fused = true; return 0; }
       if (k_tc_fprop(t, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)dx, act, alpha, s, nullptr, 1) == 0) return 0;
-      return fail(B2G_ERR_CUDA, "tcgen05 dense dgrad launch failed");
+      return fail(B2G_ERR_CUDA, "tensor-core dense dgrad launch failed");
     }
   }
   if (tc_on(n) && tc_dgrad_supported(g)) {
     if (fuse && k_tc_dgrad(g, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)dx, act, alpha, s, fuse) == 0) { if (fused) *fused = true; return 0; }
     if (k_tc_dgrad(g, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)dx, act, alpha, s) == 0) return 0;
-    return fail(B2G_ERR_CUDA, "tcgen05 dgrad launch failed");
+    return fail(B2G_ERR_CUDA, "tensor-core dgrad launch failed");
   }
   note_simt(n); k_simt_dgrad(n->prec, wp, g, dy, w, bias, dx, act, alpha, s); return 0;
 }
@@ -453,7 +453,7 @@ static int32_t gemm_wgrad(b2g_net* n, LayerRT& l, const ConvGeom& g, const void*
   if (dense_small_k_supported(g) && !(tc_on(n) && tc_wgrad_supported(g))) { note_simt(n); k_dense_small_k_wgrad(n->prec, g, x, dy, dw, s); return 0; }
   if (tc_on(n) && tc_wgrad_supported(g) && l.wg_part) {
     if (k_tc_wgrad(g, (const __nv_bfloat16*)x, (const __nv_bfloat16*)dy, dw, l.wg_part, l.wg_part_floats, 0, s, &n->pending) == 0) return 0;
-    return fail(B2G_ERR_CUDA, "tcgen05 wgrad launch failed");
+    return fail(B2G_ERR_CUDA, "tensor-core wgrad launch failed");
   }
   note_simt(n); k_simt_wgrad(n->prec, g, x, dy, dw, scratch, n->scratch_floats, 0, s); return 0;
 }
@@ -680,7 +680,7 @@ static int32_t net_allreduce_grads(b2g_net* n) {
     k_nhwc_to_nchw_f32(PREC_BF16, n->ar_buf, n->grads, 1, 1, (int)n->n_params, c->stream);
     return 0;
   }
-  if (n->p2p) {        // one kernel over NVLink peer memory instead of the NCCL ring (measured on 2 x B200: see DESIGN.md)
+  if (n->p2p) {        // one kernel over NVLink peer memory instead of the NCCL ring
     P2pArgs a{}; for (int r = 0; r < c->world; ++r) { a.grads[r] = n->p2p_peer_grads[r]; a.flags[r] = c->p2p_peer_flags[r]; }
     a.rank = c->rank; a.world = c->world; a.n = (size_t)n->n_params; a.state = c->p2p_state;
     k_p2p_allreduce(a, c->stream); CHECK_KERNELS(); return 0;
@@ -710,7 +710,7 @@ extern "C" int32_t b2g_ctx_create(int32_t device, b2g_ctx** out) {
   CU(cudaSetDevice(device));
   b2g_ctx* c = new b2g_ctx(); c->device = device;
   CU(cudaGetDeviceProperties(&c->prop, device));
-  if (c->prop.major != 10) { int mj = c->prop.major, mn = c->prop.minor; delete c; return fail(B2G_ERR_NO_DEVICE, "device is sm_%d%d; this library is built for sm_100a (B200) only", mj, mn); }
+  if (c->prop.major != 9) { int mj = c->prop.major, mn = c->prop.minor; delete c; return fail(B2G_ERR_NO_DEVICE, "device is sm_%d%d; this library is built for sm_90a (H100) only", mj, mn); }
   CU(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
   CU(cudaStreamCreateWithFlags(&c->side, cudaStreamNonBlocking)); CU(cudaStreamCreateWithFlags(&c->side2, cudaStreamNonBlocking));
   CU(cudaEventCreateWithFlags(&c->ev_a, cudaEventDisableTiming)); CU(cudaEventCreateWithFlags(&c->ev_b, cudaEventDisableTiming));
@@ -963,7 +963,7 @@ static int32_t gan_step_part2(b2g_gan* g, int N) {
   // x_real arrived (and was converted to the device layout) on the copy stream meanwhile; only the discriminator needs it
   // 3a (hoisted). The generator's train-mode forward on z_g depends only on G's parameters, which the D step does not touch: it runs on a
   // second stream -- on one GPU underneath the whole D step; with a communicator underneath the D gradient all-reduce + updater, where the
-  // SMs would otherwise idle on the network (measured on 2 x B200, round 2: the all-reduce pair costs ~0.17 ms per step when exposed).
+  // SMs would otherwise idle on the network.
   // (with sync_bn the generator's BatchNorm all-reduces must keep one issue order with the discriminator's on every rank: no hoisting)
   cudaStream_t s3 = (G->sync_bn || D->sync_bn) ? s : G->ctx->side2;
   const bool under_allreduce = G->ctx->comm && G->ctx->world > 1 && D->grad_allreduce && s3 != s;
@@ -1205,12 +1205,12 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   size_t na = kind == 1 ? ny : nx, nb = kind == 2 ? ny : nw, no = kind == 0 ? ny : kind == 1 ? nx : nw;
   const int oc = kind == 0 ? g.O : g.C;       // channels of the result (kinds 0 / 1)
   if (impl == 1) {
-    if (prec != PREC_BF16 || !c->tc_ok) return fail(B2G_ERR_UNSUPPORTED, "tcgen05 kernels need BF16 precision and a working tensor-map encoder");
+    if (prec != PREC_BF16 || !c->tc_ok) return fail(B2G_ERR_UNSUPPORTED, "tensor-core kernels need BF16 precision and a working tensor-map encoder");
     bool ok = kind == 0 ? tc_fprop_supported(g) : kind == 1 ? tc_dgrad_supported(g) : tc_wgrad_supported(g);
-    if (!ok) return fail(B2G_ERR_UNSUPPORTED, "no tcgen05 kernel for this shape");
+    if (!ok) return fail(B2G_ERR_UNSUPPORTED, "no tensor-core kernel for this shape");
   }
-  if (opt && (impl != 1 || kind == 2) && (opt->epi || opt->bias || opt->scale || opt->act)) return fail(B2G_ERR_UNSUPPORTED, "epilogue options apply to the tcgen05 fprop / dgrad kernels (impl 1, kind 0 / 1)");
-  // impl 2 = the SIMT skinny-layer kernels (kernels_edge.cu), impl 3 = their tcgen05 counterparts; both need <= 4 image channels (g.C)
+  if (opt && (impl != 1 || kind == 2) && (opt->epi || opt->bias || opt->scale || opt->act)) return fail(B2G_ERR_UNSUPPORTED, "epilogue options apply to the tensor-core fprop / dgrad kernels (impl 1, kind 0 / 1)");
+  // impl 2 = the SIMT skinny-layer kernels (kernels_edge.cu), impl 3 = their tensor-core counterparts; both need <= 4 image channels (g.C)
   if (impl == 2 || impl == 3) {
     bool ok = kind == 0 ? edge_conv_small_cin_supported(g) : kind == 1 ? edge_deconv_small_c_supported(g) : edge_wgrad_small_cin_supported(g);
     if (impl == 3) ok = ok && prec == PREC_BF16 && c->tc_ok && (kind == 0 ? tc_edge_conv_supported(g) : kind == 1 ? tc_deconv_ps_supported(g) : tc_edge_wgrad_supported(g));

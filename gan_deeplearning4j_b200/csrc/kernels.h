@@ -1,4 +1,4 @@
-// kernels.h -- launch wrappers of every CUDA kernel in libb200gan.so (sm_100a only).
+// kernels.h -- launch wrappers of every CUDA kernel in libb200gan.so (sm_90a only).
 // Host-callable, stream-ordered, no allocation.  "prec" selects the activation storage type
 // (PREC_F32 = DL4J-parity mode, PREC_BF16 = tensor-core mode); statistics, parameters, gradients and
 // updater state are always fp32.
@@ -23,6 +23,8 @@ struct ConvGeom {
 };
 
 extern uint64_t g_launch_count;   // every kernel launch of this library bumps it (bench evidence)
+// multiprocessor count of the current device (queried once per device): the one source every grid-sizing rule of the library uses
+int device_sm_count();
 
 // ---- layout ------------------------------------------------------------------------------------
 void k_nchw_f32_to_nhwc(int prec, const float* src, void* dst, int N, int C, int HW, cudaStream_t s);
@@ -50,7 +52,7 @@ void k_bn_bwd(int prec, const void* x, const void* eps_out, void* eps_in, int ro
               float* scratch, float* g_gamma, float* g_beta, int want_param_grads, cudaStream_t s);
 
 // Fused path (bf16, C % 8 == 0): the batch statistics live in 128-bit fixed-point accumulators acc[groups][2][2][C] (statistic, hi | lo,
-// channel; common.cuh sacc_add) that the producing tcgen05 GEMM fills from its epilogue (kernels_tc.cu EPI_STATS / EPI_BNBWD) or, where the
+// channel; common.cuh sacc_add) that the producing tensor-core GEMM fills from its epilogue (kernels_tc.cu EPI_STATS / EPI_BNBWD) or, where the
 // producer has no such epilogue, the *_stats_acc kernels below; the apply kernels derive mean / invstd (and the backward coefficients) from
 // them on the fly -- no partial buffers, no finalise launches.  The caller zeroes acc (one memset per pass).
 bool k_bn_vec_ok(int prec, int C);
@@ -153,12 +155,12 @@ bool dense_small_k_supported(const ConvGeom& g);         // 1x1 geometry, reduct
 void k_dense_small_k_dgrad(int prec, int wprec, const ConvGeom& g, const void* dy, const void* w, const float* bias, void* dx, int act, float alpha, cudaStream_t s);
 void k_dense_small_k_wgrad(int prec, const ConvGeom& g, const void* x, const void* dy, float* dw, cudaStream_t s);
 
-// ---- GEMM-shaped kernels, tcgen05 tensor cores (bf16 in, fp32 accumulate in TMEM) -------------------------
+// ---- GEMM-shaped kernels, wgmma tensor cores (bf16 in, fp32 accumulate in registers) -------------------------
 bool tc_fprop_supported(const ConvGeom& g);
 bool tc_dgrad_supported(const ConvGeom& g);
 bool tc_wgrad_supported(const ConvGeom& g);
 int  tc_init();   // resolves cuTensorMapEncodeTiled; 0 on success
-extern const char* g_tc_last_kernel;     // which tcgen05 kernel the most recent k_tc_* call dispatched (parity tests assert it)
+extern const char* g_tc_last_kernel;     // which tensor-core kernel the most recent k_tc_* call dispatched (parity tests assert it)
 // epilogue of the fprop / dgrad kernels (kernels_tc.cu): what happens between the fp32 accumulator and the bf16 store
 enum { EPI_PLAIN = 0, EPI_STATS = 1, EPI_BNBWD = 2, EPI_ACTBWD = 3 };
 struct TcEpi {
@@ -176,12 +178,12 @@ int k_tc_fprop(const ConvGeom& g, const __nv_bfloat16* x, const __nv_bfloat16* w
 int k_tc_dgrad(const ConvGeom& g, const __nv_bfloat16* dy, const __nv_bfloat16* w, const float* bias, __nv_bfloat16* dx, int act, float alpha, cudaStream_t s, const TcEpi* epi = nullptr);
 int k_tc_wgrad(const ConvGeom& g, const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, float* scratch, size_t scratch_floats, int accumulate, cudaStream_t s, ReduceList* defer = nullptr);
 size_t k_tc_wgrad_scratch_floats(const ConvGeom& g);
-// transposed conv 4x4 s2 p1 onto <= 4 image channels as one 3x3 tcgen05 conv over the 2x2 output blocks (weights packed by k_pack_deconv_ps)
+// transposed conv 4x4 s2 p1 onto <= 4 image channels as one 3x3 tensor-core conv over the 2x2 output blocks (weights packed by k_pack_deconv_ps)
 bool tc_deconv_ps_shape(const ConvGeom& g);          // geometry only (allocation time)
 bool tc_deconv_ps_supported(const ConvGeom& g);      // + the batch tiles into 128-pixel rows
 size_t k_tc_deconv_ps_weight_elems(const ConvGeom& g);
 void k_pack_deconv_ps(const float* w, __nv_bfloat16* wps, int O, int C, cudaStream_t s);
-// conv 4x4 s2 p1 from <= 4 image channels (fprop form) and its weight gradient: im2col rows built in shared memory by the CTA, tcgen05 MMAs
+// conv 4x4 s2 p1 from <= 4 image channels (fprop form) and its weight gradient: im2col rows built in shared memory by the CTA, wgmma MMAs
 bool tc_edge_conv_supported(const ConvGeom& g);
 bool tc_edge_wgrad_supported(const ConvGeom& g);
 size_t k_tc_edge_wgrad_scratch_floats(const ConvGeom& g);

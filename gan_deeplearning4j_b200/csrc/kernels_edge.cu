@@ -376,7 +376,7 @@ __global__ void __launch_bounds__(128) dense_small_k_wgrad_kernel(const T* __res
 // ------------------------------------------------------------------ (e') the same two GEMMs on warp-level tensor-core MMAs (bf16 operands) ---
 // out[n][c] = sum_o z[n][o] W[o][c] (N x 100 x 8192) and dW[o][c] = sum_n z[n][o] dOut[n][c] (100 x N x 8192) are 0.2 GFLOP each: the
 // SIMT kernels above spend ~18 us on instruction issue (ncu: 43 % issue-slot busy at 25 % occupancy).  mma.sync.m16n8k16 with ldmatrix
-// fragments cuts the instruction count ~10x; the tcgen05 path does not apply (reduction of 100 is not a multiple of 64 and the operand
+// fragments cuts the instruction count ~10x; the tensor-core path does not apply (reduction of 100 is not a multiple of 64 and the operand
 // rows are not 16-byte multiples for TMA).  Operands are staged once per CTA in shared memory, rows padded so that every ldmatrix
 // phase touches 8 distinct 16-byte bank groups.
 __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
@@ -514,7 +514,7 @@ bool dense_small_o_supported(const ConvGeom& g) { return g.KH == 1 && g.KW == 1 
 
 template <typename T, typename TW>
 static void launch_deconv_small_c(const ConvGeom& g, const void* dy, const void* w, const float* bias, void* dx, int act, float alpha, cudaStream_t s) {
-  long tot = (long)g.N * g.OH * g.OW; long blocks = (tot + 127) / 128; if (blocks > 148 * 8) blocks = 148 * 8;
+  long tot = (long)g.N * g.OH * g.OW; long blocks = (tot + 127) / 128; if (blocks > device_sm_count() * 8) blocks = device_sm_count() * 8;
   launch_pdl(edge_deconv_small_c_kernel<T, TW>, dim3((unsigned)blocks), dim3(128), (size_t)(16 * g.O * sizeof(float4)), s, (const T*)dy, (const TW*)w, bias, (T*)dx, g.N, g.OH, g.OW, g.O, g.C, act, alpha);
 }
 void k_edge_deconv_small_c(int prec, int wprec, const ConvGeom& g, const void* dy, const void* w, const float* bias, void* dx, int act, float alpha, cudaStream_t s) {
@@ -525,7 +525,7 @@ void k_edge_deconv_small_c(int prec, int wprec, const ConvGeom& g, const void* d
 }
 template <typename T, typename TW>
 static void launch_conv_small_cin(const ConvGeom& g, const void* x, const void* w, const float* bias, void* out, int act, float alpha, cudaStream_t s) {
-  long tot = (long)g.N * g.OH * (g.OW / 4) * (g.O / 16); long blocks = (tot + 127) / 128; if (blocks > 148 * 8) blocks = 148 * 8;
+  long tot = (long)g.N * g.OH * (g.OW / 4) * (g.O / 16); long blocks = (tot + 127) / 128; if (blocks > device_sm_count() * 8) blocks = device_sm_count() * 8;
   launch_pdl(edge_conv_small_cin_kernel<T, TW>, dim3((unsigned)blocks), dim3(128), (size_t)(16 * g.C * g.O * sizeof(float)), s, (const T*)x, (const TW*)w, bias, (T*)out, g.N, g.H, g.W, g.C, g.OH, g.OW, g.O, act, alpha);
 }
 void k_edge_conv_small_cin(int prec, int wprec, const ConvGeom& g, const void* x, const void* w, const float* bias, void* out, int act, float alpha, cudaStream_t s) {
@@ -534,7 +534,7 @@ void k_edge_conv_small_cin(int prec, int wprec, const ConvGeom& g, const void* x
   else launch_conv_small_cin<__nv_bfloat16, __nv_bfloat16>(g, x, w, bias, out, act, alpha, s);
   LAUNCHED();
 }
-static int edge_wgrad_ctas(const ConvGeom& g) { long P = (long)g.N * g.OH * g.OW; long c = 148 * 2; long cap = (P + 63) / 64; if (c > cap) c = cap; if (c < 1) c = 1; return (int)c; }
+static int edge_wgrad_ctas(const ConvGeom& g) { long P = (long)g.N * g.OH * g.OW; long c = device_sm_count() * 2; long cap = (P + 63) / 64; if (c > cap) c = cap; if (c < 1) c = 1; return (int)c; }
 size_t k_edge_wgrad_scratch_floats(const ConvGeom& g) { return edge_wgrad_small_cin_supported(g) ? (size_t)edge_wgrad_ctas(g) * g.O * 16 * g.C : 0; }
 void k_edge_wgrad_small_cin(int prec, const ConvGeom& g, const void* x, const void* dy, float* dw, float* scratch, int accumulate, cudaStream_t s) {
   const int ctas = edge_wgrad_ctas(g); const long P = (long)g.N * g.OH * g.OW; const int ppc = (int)((P + ctas - 1) / ctas);
@@ -575,7 +575,7 @@ void k_dense_small_o_fwd(int prec, int wprec, const ConvGeom& g, const void* x, 
   LAUNCHED();
 }
 void k_dense_small_o_dgrad(int prec, int wprec, const ConvGeom& g, const void* dy, const void* w, void* dx, cudaStream_t s) {
-  size_t tot = (size_t)g.N * (g.C / 8); int blocks = (int)((tot + 255) / 256); if (blocks > 148 * 8) blocks = 148 * 8;
+  size_t tot = (size_t)g.N * (g.C / 8); int blocks = (int)((tot + 255) / 256); if (blocks > device_sm_count() * 8) blocks = device_sm_count() * 8;
   if (prec == PREC_F32) launch_pdl(dense_small_o_dgrad_kernel<float, float>, dim3(blocks), dim3(256), (size_t)(0), s, (const float*)dy, (const float*)w, (float*)dx, g.N, g.C, g.O);
   else if (wprec == PREC_F32) launch_pdl(dense_small_o_dgrad_kernel<__nv_bfloat16, float>, dim3(blocks), dim3(256), (size_t)(0), s, (const __nv_bfloat16*)dy, (const float*)w, (__nv_bfloat16*)dx, g.N, g.C, g.O);
   else launch_pdl(dense_small_o_dgrad_kernel<__nv_bfloat16, __nv_bfloat16>, dim3(blocks), dim3(256), (size_t)(0), s, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)w, (__nv_bfloat16*)dx, g.N, g.C, g.O);

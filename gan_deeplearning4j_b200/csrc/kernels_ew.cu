@@ -4,7 +4,7 @@
 //
 // Semantics follow DL4J 1.0.0-beta3 as restated in oracle/dl4j_oracle.py (SURVEY.md section 8a rows
 // a3-a6, a8, a9); the reference call sites are J:123-125,132-134,141-144,159-163,201-202 where
-// J = /root/reference/Java/src/main/java/org/deeplearning4j/dl4jGANComputerVision.java.
+// J = Java/src/main/java/org/deeplearning4j/dl4jGANComputerVision.java of the reference repository.
 //
 // All of these are bandwidth-bound: threads are mapped so that a warp touches consecutive channels
 // (NHWC innermost), reductions are fixed-order two-stage (deterministic), nothing allocates.
@@ -52,8 +52,13 @@ __global__ void permute_kernel(const T* __restrict__ src, T* __restrict__ dst, i
     case ACT_LRELU: { constexpr int ACTC = ACT_LRELU; __VA_ARGS__; } break;                     \
     default: { constexpr int ACTC = -1; __VA_ARGS__; } break;                                   \
   }
-static inline int vec4_blocks(size_t n_vec) { size_t b = (n_vec + 1023) / 1024; if (b > 148 * 4) b = 148 * 4; if (b < 1) b = 1; return (int)b; }
-static inline int ew_blocks(size_t n, int per = 256) { size_t b = (n + per - 1) / per; if (b > 148 * 16) b = 148 * 16; if (b < 1) b = 1; return (int)b; }
+int device_sm_count() {
+  static int sms[64] = {}; int d = 0; cudaGetDevice(&d); if (d < 0 || d >= 64) d = 0;
+  if (!sms[d]) { int v = 0; cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, d); sms[d] = v > 0 ? v : 1; }
+  return sms[d];
+}
+static inline int vec4_blocks(size_t n_vec) { const size_t cap = (size_t)device_sm_count() * 4; size_t b = (n_vec + 1023) / 1024; if (b > cap) b = cap; if (b < 1) b = 1; return (int)b; }
+static inline int ew_blocks(size_t n, int per = 256) { const size_t cap = (size_t)device_sm_count() * 16; size_t b = (n + per - 1) / per; if (b > cap) b = cap; if (b < 1) b = 1; return (int)b; }
 
 void k_nchw_f32_to_nhwc(int prec, const float* src, void* dst, int N, int C, int HW, cudaStream_t s) {
   size_t n = (size_t)N * C * HW; if (!n) return;
@@ -373,7 +378,7 @@ void k_bn_bwd(int prec, const void* x, const void* eps_out, void* eps_in, int ro
 
 // ---------------------------------------------------------------- BatchNorm on 128-bit accumulators ----------------
 // north_star's "BatchNorm fused with its producer": the batch statistics arrive in acc[groups][2][2][C] (common.cuh sacc_add) from the
-// tcgen05 GEMM epilogues (kernels_tc.cu EPI_STATS / EPI_BNBWD) or from the *_stats_acc kernels below; the apply kernels turn them into
+// tensor-core GEMM epilogues (kernels_tc.cu EPI_STATS / EPI_BNBWD) or from the *_stats_acc kernels below; the apply kernels turn them into
 // per-channel coefficients in shared memory (once per block, in double) and stream the tensor once.  bf16, C % 8 == 0, 256 % (C/8) == 0.
 bool k_bn_vec_ok(int prec, int C) { return vec_ok(prec, C); }
 size_t k_bn_acc_elems(int C, int groups) { return (size_t)groups * 4 * C; }

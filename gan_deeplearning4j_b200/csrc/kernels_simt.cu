@@ -2,7 +2,7 @@
 //
 // These are (1) the fp32 "DL4J-parity" path (activations, weights and accumulation all fp32 -- the mode in
 // which whole-step activations/gradients are compared with the oracle to 1e-3 relative) and (2) the
-// correctness reference every tcgen05 kernel in kernels_tc.cu is checked against on the device, and
+// correctness reference every tensor-core kernel in kernels_tc.cu is checked against on the device, and
 // (3) the kernels for shapes the tensor-core path does not cover (5x5 reference convs, dense layers).
 //
 // One 64x64x16 tiled kernel, three gather rules (SURVEY.md section 8a rows a1, a2, a7):

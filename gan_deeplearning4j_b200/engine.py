@@ -241,7 +241,7 @@ class Net:
         check(self.lib.b2g_net_set_iteration(self.h, int(it)))
 
     def simt_gemm_calls(self) -> int:
-        """BF16 nets: GEMM-shaped operations that ran on the SIMT kernels instead of tcgen05 since creation."""
+        """BF16 nets: GEMM-shaped operations that ran on the SIMT kernels instead of the tensor-core kernels since creation."""
         v = C.c_uint64()
         check(self.lib.b2g_net_simt_gemm_calls(self.h, C.byref(v)))
         return v.value
@@ -309,7 +309,7 @@ class Gan:
 
 
 def test_conv(ctx: Context, kind: int, impl: int, precision: int, geom: Dict[str, int], a, b, out_size: int, iters: int = 1):
-    """Kernel-level hook: kind 0 fprop / 1 dgrad / 2 wgrad; impl 0 SIMT / 1 tcgen05. Returns (out, ms_per_iter)."""
+    """Kernel-level hook: kind 0 fprop / 1 dgrad / 2 wgrad; impl 0 SIMT / 1 tensor-core. Returns (out, ms_per_iter)."""
     g = _lib.ConvGeom(**geom)
     a, b = _f32(a).ravel(), _f32(b).ravel()
     out = np.empty(out_size, np.float32)
@@ -323,7 +323,7 @@ EPI_PLAIN, EPI_STATS, EPI_BNBWD, EPI_ACTBWD = 0, 1, 2, 3
 
 def test_conv_ex(ctx: Context, kind: int, geom: Dict[str, int], a, b, out_size: int, *, epi: int = 0, act: str = "identity", alpha: float = 0.0,
                  bias=None, scale=None, groups: int = 1, aux=None, aux2=None, iters: int = 1):
-    """tcgen05 fprop (kind 0) / dgrad (kind 1) with the epilogue the training step uses.  Returns (out, stats or None, kernel name, ms)."""
+    """Tensor-core fprop (kind 0) / dgrad (kind 1) with the epilogue the training step uses.  Returns (out, stats or None, kernel name, ms)."""
     g = _lib.ConvGeom(**geom)
     a, b = _f32(a).ravel(), _f32(b).ravel()
     out = np.empty(out_size, np.float32)

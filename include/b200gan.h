@@ -1,5 +1,5 @@
 /*
- * b200gan.h -- C-ABI of libb200gan.so: the B200-native (sm_100a) execution engine behind the DL4J
+ * b200gan.h -- C-ABI of libb200gan.so: the H100-native (sm_90a) execution engine behind the DL4J
  * ComputationGraph / Layer API used by hamaadshah/gan_deeplearning4j.
  *
  * This is the drop-in boundary (SURVEY.md section 8b): plain pointers and sizes, no C++/torch types.
@@ -7,7 +7,7 @@
  * it through the primitive-only JNI shim (jni/b200gan_jni.cpp); the Python host mirror
  * (gan_deeplearning4j_b200/) and every test reach the SAME functions through ctypes.
  *
- * J = /root/reference/Java/src/main/java/org/deeplearning4j/dl4jGANComputerVision.java
+ * J = Java/src/main/java/org/deeplearning4j/dl4jGANComputerVision.java of the reference repository
  *
  * Conventions
  *   - every function returns int32: 0 = OK, <0 = b2g_status error; text via b2g_last_error().
@@ -47,7 +47,7 @@ typedef enum {
   B2G_ERR_NCCL = -4,
   B2G_ERR_OOM = -5,
   B2G_ERR_UNSUPPORTED = -6,
-  B2G_ERR_NO_DEVICE = -7   /* no sm_100 device: there is NO CPU fallback */
+  B2G_ERR_NO_DEVICE = -7   /* no sm_90 device: there is NO CPU fallback */
 } b2g_status;
 
 /* Layer vocabulary = {what the reference file builds} U {what north_star names}. */
@@ -97,7 +97,7 @@ typedef struct {
 typedef struct {
   int32_t in_h, in_w, in_c;     /* InputType.convolutionalFlat(h,w,c) / convolutional; feedForward(n): h=w=1,c=n */
   int32_t max_batch;            /* largest minibatch any call will present */
-  int32_t precision;            /* b2g_precision: FP32 = DL4J-parity mode; BF16 = tcgen05 tensor-core mode */
+  int32_t precision;            /* b2g_precision: FP32 = DL4J-parity mode; BF16 = tensor-core mode */
   float grad_clip;              /* GradientNormalization.ClipElementWiseAbsoluteValue threshold (J:123-124); 0 = off */
   float xent_clip_eps;          /* LossBinaryXENT clipEps: 1e-5 = DL4J-exact, 0 = BCE-with-logits (north_star) */
   int32_t bn_groups;            /* >1: statistics per contiguous batch group (the GAN step runs real|fake as 2 groups) */
@@ -158,7 +158,7 @@ int32_t b2g_net_fit(b2g_net* net, const float* x, const float* y, int32_t batch,
  * configuration.json ("iterationCount"); a restore that drops it restarts Adam's bias correction with warm moments (J:606-618). */
 int32_t b2g_net_get_iteration(b2g_net* net, int64_t* out);
 int32_t b2g_net_set_iteration(b2g_net* net, int64_t iteration);
-/* BF16 nets: how many GEMM-shaped operations ran on the SIMT kernels instead of tcgen05 since creation (skinny layers by design, or a
+/* BF16 nets: how many GEMM-shaped operations ran on the SIMT kernels instead of the tensor-core kernels since creation (skinny layers by design, or a
  * shape the tensor-core kernels do not tile).  north_star: no silent fallback -- bench.py prints it per step. */
 int32_t b2g_net_simt_gemm_calls(b2g_net* net, uint64_t* out);
 
@@ -216,7 +216,7 @@ int32_t b2g_ctx_allreduce_test(b2g_ctx* ctx, float* host_inout, int64_t n);
 /* Run ONE hot-path kernel on caller-provided host tensors (NHWC, fp32 on host, rounded to bf16 on the
  * device when precision is BF16) and return the fp32 result; used by tests/ and the roofline bench.
  * kind: 0 = conv fprop, 1 = conv dgrad (= deconv fprop), 2 = conv wgrad.
- * impl: 0 = SIMT reference kernel, 1 = tcgen05 tensor-core kernel, 2 / 3 = skinny-layer (<= 4 image channels) SIMT / tcgen05 kernels,
+ * impl: 0 = SIMT reference kernel, 1 = tensor-core kernel, 2 / 3 = skinny-layer (<= 4 image channels) SIMT / tensor-core kernels,
  * 4 = dense 1x1-geometry kernels (B2G_ERR_UNSUPPORTED if the shape has none). */
 typedef struct {
   int32_t n, h, w, c;          /* conv input  (NHWC) */
@@ -226,7 +226,7 @@ typedef struct {
 int32_t b2g_test_conv(b2g_ctx* ctx, int32_t kind, int32_t impl, int32_t precision, const b2g_conv_geom* g,
                       const float* x_or_dy, const float* w_or_x, float* out, int32_t iters, float* ms_per_iter);
 /* The same with the epilogue the training step actually uses (impl 1, kind 0 / 1): bias, folded inference-BatchNorm scale, activation,
- * and the fused BatchNorm epilogues of kernels_tc.cu.  `kernel` returns the name of the tcgen05 kernel that was dispatched, so a parity
+ * and the fused BatchNorm epilogues of kernels_tc.cu.  `kernel` returns the name of the tensor-core kernel that was dispatched, so a parity
  * test can assert that it exercised the variant the benchmark runs (persistent MT=2, one-wave split-K, ...). */
 typedef struct {
   int32_t epi;            /* 0 plain; 1 + statistics (sum, sum of squares per group and channel) of the stored outputs;

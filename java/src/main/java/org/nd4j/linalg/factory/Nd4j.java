@@ -10,7 +10,7 @@ public final class Nd4j {
     private static final Random RNG = new Random(666);
     private Nd4j() {}
     public static void setDataType(DataBuffer.Type t) { if (t != DataBuffer.Type.FLOAT) throw new IllegalStateException("b200gan computes in fp32/bf16"); }
-    public static String getBackend() { return "b200gan (sm_100a, libb200gan.so v" + org.deeplearning4j.b200.Native.version() + ")"; }
+    public static String getBackend() { return "b200gan (sm_90a, libb200gan.so v" + org.deeplearning4j.b200.Native.version() + ")"; }
     public static MemoryManager getMemoryManager() { return new MemoryManager(); }
     public static final class MemoryManager { public void setAutoGcWindow(int ms) { /* device memory is one static arena per net */ } }
     private static long numel(long... s) { long n = 1; for (long v : s) n *= v; return n; }

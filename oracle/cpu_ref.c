@@ -1,6 +1,6 @@
 /* cpu_ref.c -- TEST / BENCH INFRASTRUCTURE, not product code (only tests/, bench.py's CPU legs and __graft_entry__.build() touch oracle/).
  *
- * A C + OpenMP restatement of how DL4J 1.0.0-beta3 with the nd4j-native CPU backend (P:104-108 of /root/reference/Java/pom.xml; the
+ * A C + OpenMP restatement of how DL4J 1.0.0-beta3 with the nd4j-native CPU backend (P:104-108 of the reference's Java/pom.xml; the
  * reference's "reference plumbing" configuration) executes the adversarial G+D step of J:408-471: NCHW fp32 activations, every layer
  * op-by-op -- explicit im2col buffer + SGEMM + separate bias / activation / BatchNorm passes, col2im scatter for the transposed
  * convolutions and the input gradients, a multi-pass Adam updater -- on all host cores.  DL4J itself cannot run here (no JVM, no jars:

@@ -295,13 +295,13 @@ def test_full_size_c2_step_properties(b200):
 
 
 # ------------------------------------------------------------------------------------------------
-# tcgen05 tensor-core kernels vs the oracle on bf16-rounded operands (and vs the SIMT kernel)
+# wgmma tensor-core kernels vs the oracle on bf16-rounded operands (and vs the SIMT kernel)
 # ------------------------------------------------------------------------------------------------
 TC_FPROP_CASES = [
     # n, h, w, c, o, k, s, p
     (2, 16, 16, 64, 64, 4, 2, 1),      # 8x8 out: two images per 128-row tile, BN=64
     (1, 32, 32, 64, 128, 4, 2, 1),     # 16x16 out: 8 rows of one image per tile, BN=128 (D2 shape, one image)
-    (8, 8, 8, 128, 256, 4, 2, 1),      # 4x4 out: eight images per tile, two 64-channel chunks, BN=256 (D4-like)
+    (8, 8, 8, 128, 256, 4, 2, 1),      # 4x4 out: eight images per tile, two 64-channel chunks, BN=128 (D4-like)
     (2, 8, 8, 64, 64, 3, 1, 1),        # stride 1
     (4, 9, 9, 64, 128, 5, 2, 0),       # reference-style 5x5 s2 p0, Truncate: 3x3 out ... not tileable -> must be refused
     (128, 1, 1, 128, 64, 1, 1, 0),     # dense layer as 1x1 conv
@@ -347,22 +347,30 @@ def test_tc_dgrad_phase_form_matches_oracle(b200, case):
 
 
 TC_WGRAD_CASES = [
-    # n, h, w, c, o  (4x4 s2 p1)
-    (4, 16, 16, 64, 128),     # 8x8 dy grid: one image per 64-pixel K-block, BNW=64
-    (2, 32, 32, 128, 128),    # 16x16 grid: 4 rows per K-block, BNW=128
-    (16, 8, 8, 256, 256),     # 4x4 grid: four images per K-block, BNW=256, two o-tiles
+    # n, h, w, c, o, k, s, p
+    (4, 16, 16, 64, 128, 4, 2, 1),     # 8x8 dy grid: one image per 64-pixel K-block, BNW=128
+    (2, 32, 32, 128, 128, 4, 2, 1),    # 16x16 grid: 4 rows per K-block, BNW=128
+    (16, 8, 8, 256, 256, 4, 2, 1),     # 4x4 grid: four images per K-block, BNW=128, two o-tiles
+    (4, 16, 16, 64, 128, 3, 1, 1),     # 3x3 s1: 9*64 = 576 columns are not a multiple of 128 -> BNW=64
 ]
 
 
 @pytest.mark.parametrize("case", TC_WGRAD_CASES)
 def test_tc_wgrad_mn_major_matches_oracle(b200, case):
     b, ctx = b200
-    n, h, w, c, oc = case
+    n, h, w, c, oc, k, s, p = case
     rng = np.random.default_rng(4)
-    x, wt, y, dy, dx, dw = _conv_ref(n, h, w, c, oc, 4, 2, 1, rng, bf16_round)
-    geom = dict(n=n, h=h, w=w, c=c, oh=h // 2, ow=w // 2, o=oc, kh=4, kw=4, sh=2, sw=2, ph=1, pw=1)
-    out, _ = b.test_conv(ctx, 2, 1, b.BF16, geom, x.transpose(0, 2, 3, 1), dy.transpose(0, 2, 3, 1), dw.size)
-    assert rel_err(out.reshape(oc, 4, 4, c), dw.transpose(0, 2, 3, 1)) < 1e-4     # fp32 accumulate, fp32 out: only summation order differs
+    x, wt, y, dy, dx, dw = _conv_ref(n, h, w, c, oc, k, s, p, rng, bf16_round)
+    oh, ow = y.shape[2], y.shape[3]
+    geom = dict(n=n, h=h, w=w, c=c, oh=oh, ow=ow, o=oc, kh=k, kw=k, sh=s, sw=s, ph=p, pw=p)
+    opts = b._lib.TestConvOpts()
+    import ctypes as C
+    out = np.empty(dw.size, np.float32); ms = C.c_float()
+    fp = lambda a: a.ctypes.data_as(C.POINTER(C.c_float))
+    xa, da = np.ascontiguousarray(x.transpose(0, 2, 3, 1).ravel(), np.float32), np.ascontiguousarray(dy.transpose(0, 2, 3, 1).ravel(), np.float32)
+    b.engine.check(ctx.lib.b2g_test_conv_ex(ctx.h, 2, 1, b.BF16, C.byref(b._lib.ConvGeom(**geom)), fp(xa), fp(da), fp(out), 1, C.byref(ms), C.byref(opts)))
+    assert rel_err(out.reshape(oc, k, k, c), dw.transpose(0, 2, 3, 1)) < 1e-4     # fp32 accumulate, fp32 out: only summation order differs
+    assert opts.kernel.decode() == ("tc_wgrad_kernel<64,4>" if (k * k * c) % 128 else "tc_wgrad_kernel<128,4>")
 
 
 TC_EDGE_CASES = [
@@ -376,7 +384,7 @@ TC_EDGE_CASES = [
 
 @pytest.mark.parametrize("case", TC_EDGE_CASES)
 def test_tc_skinny_layer_kernels_match_oracle(b200, case):
-    """tcgen05 versions of the <= 4-image-channel layers: transposed conv as ONE 3x3 conv over 2x2 output blocks (pixel-shuffle epilogue)."""
+    """Tensor-core versions of the <= 4-image-channel layers: transposed conv as ONE 3x3 conv over 2x2 output blocks (pixel-shuffle epilogue)."""
     b, ctx = b200
     n, h, w, c, oc = case
     rng = np.random.default_rng(5)

@@ -28,7 +28,7 @@ def pack_deconv_ps(w_int, O, C):
 
 
 def test_pixel_shuffle_form_of_the_transposed_conv_equals_deconvolution2d():
-    """The tcgen05 G-last forward computes ONE 3x3 s1 p1 conv with 16 = (py,px,c4) output columns over the deconv input and scatters
+    """The tensor-core G-last forward computes ONE 3x3 s1 p1 conv with 16 = (py,px,c4) output columns over the deconv input and scatters
     each pixel's 16 values to its 2x2 output block.  With the packed weights this must equal Deconvolution2D 4x4 s2 p1 (J:203-219 family)."""
     rng = np.random.default_rng(0)
     n, O, C, h = 2, 8, 3, 5                                  # deconv: O input channels on an h x h grid -> C channels on 2h x 2h
@@ -82,6 +82,32 @@ def test_bench_reference_arm_prints_the_contract_line():
     assert line["cpu_baseline"]["kind"] == "port" and line["cpu_baseline"]["value"] == line["value"] and line["cpu_baseline"]["cores"] >= 1
     assert line["e2e"] == {"value": line["value"], "unit": line["unit"], "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}
     assert line["value"] > 0
+
+
+def test_bench_dump_outputs_fit_64_mb_for_every_config(tmp_path):
+    """bench.py --dump-outputs at the real parameter counts of every benchmark config: at most 64 MB on disk, whole vectors where they fit,
+    otherwise a seeded sample whose float64 indices select the same elements on every run."""
+    import bench
+    from helpers import oracle_from_specs
+    for name, cfg in bench.CONFIGS.items():
+        gs, ds, gin, din = bench.build_specs(cfg)
+        ng = oracle_from_specs(gs, gin, dtype=np.float32).num_params()
+        nd = oracle_from_specs(ds, din, dtype=np.float32, flat_input=False).num_params()
+        arrays = {"losses": np.arange(3, dtype=np.float32), "g_params": np.arange(ng, dtype=np.float32), "d_params": np.arange(nd, dtype=np.float32)}
+        for run in ("a", "b"):
+            bench.dump_outputs(str(tmp_path / name / run), arrays)
+        files = sorted(os.listdir(tmp_path / name / "a"))
+        assert sum(os.path.getsize(tmp_path / name / "a" / f) for f in files) <= 64 * 10**6, name
+        whole = 4 * (ng + nd + 3) <= 64 * 10**6 - 3 * 128
+        assert files == (["d_params.npy", "g_params.npy", "losses.npy"] if whole else ["d_params.npy", "d_params_index.npy", "g_params.npy", "g_params_index.npy", "losses.npy"]), (name, files)
+        for f in files:
+            a, b = np.load(tmp_path / name / "a" / f), np.load(tmp_path / name / "b" / f)
+            assert a.dtype in (np.float32, np.float64) and np.array_equal(a, b), (name, f)
+        for v in ("g_params", "d_params"):
+            got = np.load(tmp_path / name / "a" / f"{v}.npy")
+            idx = np.load(tmp_path / name / "a" / f"{v}_index.npy").astype(np.int64) if not whole else np.arange(arrays[v].size)
+            np.testing.assert_array_equal(got, arrays[v][idx])          # arange values: each kept value names its own element
+        assert whole or name == "c4", name
 
 
 def test_checkpoint_container_round_trip_and_nd4j_stream_layout(tmp_path):

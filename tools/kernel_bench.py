@@ -13,7 +13,7 @@ import gan_deeplearning4j_b200 as b
 edge_only = "--edge-only" in sys.argv
 args = [a for a in sys.argv[1:] if not a.startswith("--")]
 n = int(args[0]) if args else 128
-peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 1590.0
+peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 989.0      # H100 SXM data-sheet dense bf16
 ctx = b.Context(0)
 rng = np.random.default_rng(0)
 # (name, kind, batch, h, w, c, o)  conv geometry 4x4 s2 p1; kind 0 fprop, 1 dgrad(=deconv fwd), 2 wgrad
@@ -22,7 +22,7 @@ for name, bt, h, c, o in (("D2", 2 * n, 32, 64, 128), ("D3", 2 * n, 16, 128, 256
     shapes += [(name + " fprop (D-step 2N)", 0, bt, h, h, c, o), (name + " wgrad (D-step 2N)", 2, bt, h, h, c, o), (name + " dgrad (G-step N)", 1, n, h, h, c, o)]
 for name, h, c, o in (("G2", 8, 256, 512), ("G3", 16, 128, 256), ("G4", 32, 64, 128)):   # conv-equivalent geometry of the transposed convs
     shapes += [(name + " fwd = dgrad form (N)", 1, n, h, h, c, o), (name + " wgrad (N)", 2, n, h, h, c, o), (name + " input-grad = fprop form (N)", 0, n, h, h, c, o)]
-# skinny layers (3 image channels): impl 2 = SIMT, impl 3 = tcgen05; (name, kind, batch)
+# skinny layers (3 image channels): impl 2 = SIMT, impl 3 = tensor cores; (name, kind, batch)
 edge = [("D1 fprop (D-step 2N)", 0, 2 * n), ("D1 wgrad (D-step 2N)", 2, 2 * n), ("D1 dgrad (G-step N)", 1, n),
         ("G5 fwd = dgrad form (N)", 1, n), ("G5 wgrad (N)", 2, n), ("G5 input-grad = fprop form (N)", 0, n)]
 edge_rows = []
@@ -58,7 +58,7 @@ for r in rows:
     print(f"| {r[0]} | {r[1]:.2f} | {r[2]:.1f} | {r[3]:.0f} | {r[4]:.2f} |")
 tot_f = sum(r[1] for r in rows); tot_t = sum(r[2] for r in rows if r[2] == r[2]) or 1.0
 print(f"| all | {tot_f:.1f} | {tot_t:.0f} | {tot_f / tot_t * 1e3:.0f} | {tot_f / tot_t * 1e3 / peak:.2f} |")
-print(f"\n| skinny layer (batch N={n}) | GFLOP | activation MB | SIMT us | tcgen05 us |\n|---|---|---|---|---|")
+print(f"\n| skinny layer (batch N={n}) | GFLOP | activation MB | SIMT us | tensor-core us |\n|---|---|---|---|---|")
 for r in edge_rows:
     print(f"| {r[0]} | {r[1]:.2f} | {r[2]:.1f} | {r[3]:.1f} | {r[4]:.1f} |")
 ctx.close()
