@@ -101,6 +101,9 @@ PROTOTYPES = {
     "b2g_test_conv": (_i32, [_vp, _i32, _i32, _i32, C.POINTER(ConvGeom), _fp, _fp, _fp, _i32, _fp]),
     "b2g_test_hbm_kernels": (_i32, [_vp, _i32, _i32, _i32, _fp]),
     "b2g_test_conv_ex": (_i32, [_vp, _i32, _i32, _i32, C.POINTER(ConvGeom), _fp, _fp, _fp, _i32, _fp, C.POINTER(TestConvOpts)]),
+    "b2g_test_bn": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _fp, _fp, _fp, _fp, _fp, _fp, _i32, C.c_float, C.c_float, C.c_float,
+                           _i32, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
+    "b2g_test_net_shadow": (_i32, [_vp, _i32, _i32, _fp, _i64]),
 }
 
 _lib = None

@@ -31,11 +31,10 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
-// 128-bit fixed-point accumulation of fp32 partial sums with two 64-bit integer atomics: hi counts units of 2^-10, lo the remainder in units
+// 128-bit fixed-point accumulation of fp32 / fp64 partial sums with two 64-bit integer atomics: hi counts units of 2^-10, lo the remainder in units
 // of 2^-60.  Integer addition commutes, so a sum of per-CTA partials is bit-identical whatever order the CTAs arrive in (fp32 / fp64 atomics
 // are not), it is exact to 2^-61 per addend, and it cannot overflow below |total| ~ 9e15.  hi_lo[idx] / hi_lo[stride + idx].
-__device__ __forceinline__ void sacc_add(unsigned long long* hi_lo, size_t stride, size_t idx, float s) {
-  const double d = (double)s;
+__device__ __forceinline__ void sacc_add(unsigned long long* hi_lo, size_t stride, size_t idx, double d) {
   const long long hi = __double2ll_rn(d * 1024.0);
   const double r = d - (double)hi * (1.0 / 1024.0);
   const long long lo = __double2ll_rn(r * 1152921504606846976.0);

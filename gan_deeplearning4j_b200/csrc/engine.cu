@@ -90,7 +90,7 @@ struct LayerRT {
   void* probs = nullptr;                                       // OUTPUT / LOSS: sigmoid(logits)
   uint8_t* argmax = nullptr;
   float* bn_mean = nullptr; float* bn_invstd = nullptr; float* bn_fold = nullptr;   // bn_fold: [scale | shift] for the inference-mode epilogue fold
-  float* bn_coef = nullptr;                                    // fused path: [groups][4][C] = scale, shift, mean, invstd of the latest train-mode forward
+  float* bn_coef = nullptr;                                    // fused path: [groups][4][C] = scale, beta, mean, invstd of the latest train-mode forward
   unsigned long long *acc_fwd = nullptr, *acc_bwd = nullptr;   // fused path: 128-bit statistics accumulators (forward: sum x, sum x^2; backward: sum dy', sum dy'*xhat)
   bool fwd_fused = false; int fwd_groups = 1;                  // the latest train-mode forward of this BatchNorm took the accumulator path (so must its backward)
   bool stats_by_producer = false, bwd_premul = false;          // set per pass: the producing GEMM's epilogue has already filled acc_fwd / (acc_bwd and eps = dy')
@@ -1285,6 +1285,89 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
 }
 extern "C" int32_t b2g_test_conv(b2g_ctx* c, int32_t kind, int32_t impl, int32_t precision, const b2g_conv_geom* gg, const float* a_host, const float* b_host, float* out, int32_t iters, float* ms_per_iter) {
   return b2g_test_conv_ex(c, kind, impl, precision, gg, a_host, b_host, out, iters, ms_per_iter, nullptr);
+}
+
+// One BatchNorm(+activation) forward and backward on [groups][rows][C] host tensors through the kernels the training step uses.
+// path 0: k_bn_stats -> k_bn_apply -> k_bn_bwd (fp32 or bf16); path 1: the 128-bit accumulator kernels, backward statistics from
+// k_bn_bwd_stats_acc; path 2: the accumulator kernels in the state the EPI_BNBWD epilogue leaves them (eps_out already holds dy' =
+// eps * act', the backward accumulator holds (sum dy', sum dy'*z)).  g_gamma / g_beta are in/out (accumulated into, as in a backward pass).
+extern "C" int32_t b2g_test_bn(b2g_ctx* c, int32_t precision, int32_t path, int32_t groups, int32_t rows, int32_t C, const float* x, const float* eps_out,
+                               const float* gamma, const float* beta, const float* run_mean, const float* run_var, int32_t act, float alpha, float eps, float decay,
+                               int32_t want_param_grads, float* y, float* eps_in, float* g_gamma, float* g_beta, float* g_mean, float* g_var, float* mean, float* invstd) {
+  if (!c || !x || !eps_out || !gamma || !beta || !run_mean || !run_var || !y || !eps_in || !g_gamma || !g_beta || !g_mean || !g_var || !mean || !invstd) return fail(B2G_ERR_ARG, "null");
+  if (groups < 1 || rows < 1 || C < 1 || path < 0 || path > 2) return fail(B2G_ERR_ARG, "bad BatchNorm test arguments");
+  const int prec = precision == B2G_PREC_BF16 ? PREC_BF16 : PREC_F32;
+  if (path != 0 && !k_bn_vec_ok(prec, C)) return fail(B2G_ERR_UNSUPPORTED, "the accumulator BatchNorm kernels need bf16 and C %% 8 == 0 with 256 %% (C/8) == 0 (C = %d)", C);
+  CU(cudaSetDevice(c->device)); cudaStream_t s = c->stream;
+  const size_t n = (size_t)groups * rows * C, gc = (size_t)groups * C, ts = prec_size(prec);
+  std::vector<void*> mem;
+  auto alloc = [&](void** p, size_t bytes) -> int32_t { *p = nullptr; CU(cudaMalloc(p, bytes)); mem.push_back(*p); return 0; };
+  auto release = [&]() { for (void* p : mem) cudaFree(p); mem.clear(); };
+  float *fx, *fe, *fo, *d_par, *d_grad, *d_stat, *scratch, *coef, *unit; void *tx, *te, *ty, *tei; unsigned long long* acc;
+  int32_t r = 0;
+  if ((r = alloc((void**)&fx, 4 * n)) || (r = alloc((void**)&fe, 4 * n)) || (r = alloc((void**)&fo, 4 * n)) || (r = alloc(&tx, ts * n)) || (r = alloc(&te, ts * n)) ||
+      (r = alloc(&ty, ts * n)) || (r = alloc(&tei, ts * n)) || (r = alloc((void**)&d_par, 4 * 4 * (size_t)C)) || (r = alloc((void**)&d_grad, 4 * 4 * (size_t)C)) ||
+      (r = alloc((void**)&d_stat, 4 * 2 * gc)) || (r = alloc((void**)&scratch, 4 * k_bn_scratch_floats(C, groups))) || (r = alloc((void**)&coef, 4 * 4 * gc)) ||
+      (r = alloc((void**)&unit, 4 * 4 * gc)) || (r = alloc((void**)&acc, 8 * 2 * k_bn_acc_elems(C, groups)))) { release(); return r; }
+  float *d_gamma = d_par, *d_beta = d_par + C, *d_rm = d_par + 2 * C, *d_rv = d_par + 3 * C;
+  float *d_gg = d_grad, *d_gb = d_grad + C, *d_gm = d_grad + 2 * C, *d_gv = d_grad + 3 * C, *d_mean = d_stat, *d_is = d_stat + gc;
+  unsigned long long *acc_f = acc, *acc_b = acc + k_bn_acc_elems(C, groups);
+  auto up = [&](float* d, const float* h, size_t k) { return cudaMemcpyAsync(d, h, 4 * k, cudaMemcpyHostToDevice, s); };
+  if (up(fx, x, n) || up(fe, eps_out, n) || up(d_gamma, gamma, C) || up(d_beta, beta, C) || up(d_rm, run_mean, C) || up(d_rv, run_var, C) ||
+      up(d_gg, g_gamma, C) || up(d_gb, g_beta, C) || cudaMemsetAsync(acc, 0, 8 * 2 * k_bn_acc_elems(C, groups), s)) { release(); return fail(B2G_ERR_CUDA, "BatchNorm test upload failed"); }
+  if (prec == PREC_BF16) { k_cast_f32_to_bf16(fx, (__nv_bfloat16*)tx, n, s); k_cast_f32_to_bf16(fe, (__nv_bfloat16*)te, n, s); }
+  else { cudaMemcpyAsync(tx, fx, 4 * n, cudaMemcpyDeviceToDevice, s); cudaMemcpyAsync(te, fe, 4 * n, cudaMemcpyDeviceToDevice, s); }
+  const int want = want_param_grads ? 1 : 0;
+  if (path == 0) {
+    k_bn_stats(prec, tx, rows, C, groups, scratch, d_mean, d_is, eps, d_rm, d_rv, d_gm, d_gv, decay, s);
+    k_bn_apply(prec, tx, ty, rows, C, groups, d_mean, d_is, d_gamma, d_beta, act, alpha, s);
+    k_bn_bwd(prec, tx, te, tei, rows, C, groups, d_mean, d_is, d_gamma, d_beta, act, alpha, scratch, d_gg, d_gb, want, s);
+  } else {
+    k_bn_stats_acc(tx, rows, C, groups, acc_f, s);
+    k_bn_apply_acc(tx, ty, rows, C, groups, acc_f, d_gamma, d_beta, act, alpha, eps, coef, d_rm, d_rv, d_gm, d_gv, decay, s, 1);
+    if (path == 1) k_bn_bwd_stats_acc(tx, te, rows, C, groups, coef, act, alpha, acc_b, s);
+    else {      // (scale 1, shift 0, mean 0, invstd 1) makes xhat = z: the accumulator receives (sum dy', sum dy'*z) exactly as the epilogue writes it
+      for (int g = 0; g < groups; ++g) for (int k = 0; k < 4; ++k) k_fill_f32(unit + (size_t)(g * 4 + k) * C, (k == 0 || k == 3) ? 1.f : 0.f, C, s);
+      k_bn_bwd_stats_acc(tx, te, rows, C, groups, unit, ACT_IDENTITY, 0.f, acc_b, s);
+    }
+    k_bn_bwd_apply_acc(tx, te, tei, rows, C, groups, coef, act, alpha, path == 2 ? 1 : 0, acc_b, d_gg, d_gb, want, s, 1);
+    for (int g = 0; g < groups; ++g) {
+      cudaMemcpyAsync(d_mean + (size_t)g * C, coef + (size_t)(g * 4 + 2) * C, 4 * C, cudaMemcpyDeviceToDevice, s);
+      cudaMemcpyAsync(d_is + (size_t)g * C, coef + (size_t)(g * 4 + 3) * C, 4 * C, cudaMemcpyDeviceToDevice, s);
+    }
+  }
+  auto down = [&](float* h, const void* t) -> int32_t {     // widen a T tensor to fp32 and copy it out
+    k_nhwc_to_nchw_f32(prec, t, fo, 1, 1, (int)n, s); CU(cudaMemcpyAsync(h, fo, 4 * n, cudaMemcpyDeviceToHost, s)); CU(cudaStreamSynchronize(s)); return 0;
+  };
+  if ((r = down(y, ty)) || (r = down(eps_in, tei))) { release(); return r; }
+  cudaError_t e = cudaSuccess;
+  float* hs[6] = {g_gamma, g_beta, g_mean, g_var, mean, invstd}; const float* ds[6] = {d_gg, d_gb, d_gm, d_gv, d_mean, d_is}; const size_t ks[6] = {(size_t)C, (size_t)C, (size_t)C, (size_t)C, gc, gc};
+  for (int k = 0; k < 6 && e == cudaSuccess; ++k) e = cudaMemcpyAsync(hs[k], ds[k], 4 * ks[k], cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  if (e == cudaSuccess) e = cudaGetLastError();
+  release();
+  if (e != cudaSuccess) return fail(B2G_ERR_CUDA, "BatchNorm test: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+// Copies one of the bf16 weight operands the updater keeps beside the fp32 master, widened to fp32: which = 0 the straight copy of W
+// (internal [A][taps][B] order), which = 1 the packed [(py,px,c)][(dyr,dxc)][O] operand of the pixel-shuffle transposed conv.
+extern "C" int32_t b2g_test_net_shadow(b2g_net* n, int32_t layer, int32_t which, float* out, int64_t count) {
+  if (!n || !out) return fail(B2G_ERR_ARG, "null");
+  if (layer < 0 || layer >= (int)n->L.size()) return fail(B2G_ERR_ARG, "layer %d out of range", layer);
+  if (n->prec != PREC_BF16) return fail(B2G_ERR_UNSUPPORTED, "FP32 nets keep no bf16 weight copies");
+  const LayerRT& l = n->L[layer];
+  int64_t off = -1, len = 0;
+  if (which == 0) { off = l.off_W_bf; len = l.n_W; }
+  else if (which == 1) { off = l.off_Wps_bf; len = (int64_t)k_tc_deconv_ps_weight_elems(l.geom); }
+  else return fail(B2G_ERR_ARG, "which = %d (0 straight copy, 1 pixel-shuffle operand)", which);
+  if (off < 0) return fail(B2G_ERR_UNSUPPORTED, "layer %d has no %s", layer, which ? "pixel-shuffle operand" : "bf16 weight copy");
+  if (count != len) return fail(B2G_ERR_SHAPE, "layer %d operand has %lld elements, %lld requested", layer, (long long)len, (long long)count);
+  CU(cudaSetDevice(n->ctx->device)); cudaStream_t s = n->ctx->stream;
+  if ((size_t)len > n->stage_floats) return fail(B2G_ERR_SHAPE, "operand larger than the staging buffer");
+  k_nhwc_to_nchw_f32(PREC_BF16, n->shadow + off, n->stage_f32, 1, 1, (int)len, s);
+  CU(cudaMemcpyAsync(out, n->stage_f32, sizeof(float) * len, cudaMemcpyDeviceToHost, s)); CU(cudaStreamSynchronize(s)); CHECK_KERNELS();
+  return 0;
 }
 
 // Times the HBM-bound kernels of the step in isolation (bench.py's `hbm` roofline entries): every launch is bracketed by its own CUDA events

@@ -58,11 +58,12 @@ void k_bn_bwd(int prec, const void* x, const void* eps_out, void* eps_in, int ro
 bool k_bn_vec_ok(int prec, int C);
 size_t k_bn_acc_elems(int C, int groups);                  // 64-bit words per accumulator set
 void k_bn_stats_acc(const void* x, int rows_per_group, int C, int groups, unsigned long long* acc, cudaStream_t s);
-// y = act(x*scale+shift); block 0 also leaves coef[groups][4][C] = {scale = gamma*invstd, shift = beta - mean*scale, mean, invstd} for the
+// y = act(x*scale+shift) with shift = beta - mean*scale; block 0 also leaves coef[groups][4][C] = {scale = gamma*invstd, beta, mean, invstd} for the
 // backward pass and (g_mean != null) the DL4J running-stat pseudo-gradients averaged over groups
 void k_bn_apply_acc(const void* x, void* y, int rows_per_group, int C, int groups, const unsigned long long* acc, const float* gamma, const float* beta,
                     int act, float alpha, float eps, float* coef, const float* run_mean, const float* run_var, float* g_mean, float* g_var, float decay, cudaStream_t s, int replicas = 1);
-// sum dy', sum dy'*xhat -> acc with dy' = eps_out * act'(x*scale+shift)   (producers without the EPI_BNBWD epilogue)
+// sum dy', sum dy'*xhat -> acc with dy' = eps_out * act'(z), z from kernels_ew.cu bn_pre_act: (x - mean)*scale + beta for tanh / sigmoid,
+// the forward's x*scale+shift for relu / leaky relu   (producers without the EPI_BNBWD epilogue)
 void k_bn_bwd_stats_acc(const void* x, const void* eps_out, int rows_per_group, int C, int groups, const float* coef, int act, float alpha, unsigned long long* acc, cudaStream_t s);
 // eps_in = scale * (dy' - mean(dy') - xhat*mean(dy'*xhat)).  premul = 0: eps_out is the raw epsilon and acc = (sum dy', sum dy'*xhat) from
 // k_bn_bwd_stats_acc; premul = 1: eps_out already holds dy' and acc = (sum dy', sum dy'*z) from the EPI_BNBWD epilogue, converted here in

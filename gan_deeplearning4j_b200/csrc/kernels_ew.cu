@@ -101,15 +101,20 @@ __device__ __forceinline__ uint4 pack8(const float (&v)[8]) {
   return u;
 }
 
+// The statistics are accumulated around a per-(group, channel) pivot k = the group's first row: sum (x-k) and sum (x-k)^2.  The one-pass
+// variance E[(x-k)^2] - E[x-k]^2 then loses nothing to cancellation when |mean| >> std (a constant channel gives exactly 0), which the
+// raw E[x^2] - E[x]^2 in fp32 partial sums does.  The pivots go to pivot[g*C + c] for the final kernel.
 template <typename T>
-__global__ void bn_stats_partial_kernel(const T* __restrict__ x, int rows, int C, int S, float* __restrict__ psum, float* __restrict__ psq) { pdl_enter();
+__global__ void bn_stats_partial_kernel(const T* __restrict__ x, int rows, int C, int S, float* __restrict__ psum, float* __restrict__ psq, float* __restrict__ pivot) { pdl_enter();
   int g = blockIdx.y;
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= S * C) return;
   int c = idx % C, sl = idx / C;
   const T* xg = x + (size_t)g * rows * C;
+  const float k = ldf(xg, c);
+  if (sl == 0) pivot[g * C + c] = k;
   float a = 0.f, b = 0.f;
-  for (int r = sl; r < rows; r += S) { float v = ldf(xg, (size_t)r * C + c); a += v; b = fmaf(v, v, b); }
+  for (int r = sl; r < rows; r += S) { float v = ldf(xg, (size_t)r * C + c) - k; a += v; b = fmaf(v, v, b); }
   psum[((size_t)g * S + sl) * C + c] = a; psq[((size_t)g * S + sl) * C + c] = b;
 }
 // bf16, C % 8 == 0, C <= 2048: a 256-thread block = (C/8 channel-octets) x TY row lanes reduces a contiguous chunk of rows
@@ -131,22 +136,27 @@ __device__ __forceinline__ void block_fold_write(float (&acc)[NV][8], int C, int
     for (int v = 0; v < NV; ++v) { float a = 0.f; for (int k = 0; k < TY; ++k) a += sred[v][k * C + c]; dst[v][row_off + c] = a; }
   }
 }
-__global__ void __launch_bounds__(256) bn_stats_partial_bf16x8_kernel(const uint4* __restrict__ x, int rows, int C, int S, float* __restrict__ psum, float* __restrict__ psq) { pdl_enter();
+__global__ void __launch_bounds__(256) bn_stats_partial_bf16x8_kernel(const uint4* __restrict__ x, int rows, int C, int S, float* __restrict__ psum, float* __restrict__ psq, float* __restrict__ pivot) { pdl_enter();
   const int g = blockIdx.y, C8 = C / 8, TY = 256 / C8, c8 = threadIdx.x % C8, ty = threadIdx.x / C8, sl = blockIdx.x;
   const int chunk = (rows + S - 1) / S, r0 = sl * chunk, r1 = min(rows, r0 + chunk);
   const uint4* xg = x + (size_t)g * rows * C8;
-  float acc[2][8];
+  float acc[2][8], k[8];
+  unpack8(xg[c8], k);       // pivot: row 0 of the group (see bn_stats_partial_kernel)
+  if (sl == 0 && ty == 0) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) pivot[g * C + c8 * 8 + j] = k[j];
+  }
 #pragma unroll
   for (int j = 0; j < 8; ++j) { acc[0][j] = 0.f; acc[1][j] = 0.f; }
 #pragma unroll 4
   for (int r = r0 + ty; r < r1; r += TY) { float v[8]; unpack8(xg[(size_t)r * C8 + c8], v);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) { acc[0][j] += v[j]; acc[1][j] = fmaf(v[j], v[j], acc[1][j]); } }
+    for (int j = 0; j < 8; ++j) { const float d = v[j] - k[j]; acc[0][j] += d; acc[1][j] = fmaf(d, d, acc[1][j]); } }
   float* const dst[2] = {psum, psq};
   block_fold_write<2>(acc, C, C8, c8, ty, TY, dst, ((size_t)g * S + sl) * C);
 }
 // stage 2: block = 32 adjacent channels x 16 slice lanes (coalesced 128-byte rows of the partial arrays), fixed-order tree in double
-__global__ void __launch_bounds__(1024) bn_stats_final_kernel(const float* __restrict__ psum, const float* __restrict__ psq, int rows, int C, int S, int groups, float eps,
+__global__ void __launch_bounds__(1024) bn_stats_final_kernel(const float* __restrict__ psum, const float* __restrict__ psq, const float* __restrict__ pivot, int rows, int C, int S, int groups, float eps,
                                       float* __restrict__ mean, float* __restrict__ invstd,
                                       const float* __restrict__ run_mean, const float* __restrict__ run_var, float* g_mean, float* g_var, float decay) { pdl_enter();
   __shared__ double sa[32][33], sb[32][33];      // 32 channels x 32 slice lanes: S <= 256 partial rows in ONE batch of 8 loads per thread
@@ -165,7 +175,7 @@ __global__ void __launch_bounds__(1024) bn_stats_final_kernel(const float* __res
     __syncthreads();
     if (ty == 0 && c < C) {
       for (int k = 1; k < 32; ++k) { a += sa[k][tx]; b += sb[k][tx]; }
-      const double mu = a / rows; double var = b / rows - mu * mu; if (var < 0) var = 0;
+      const double d = a / rows, mu = (double)pivot[g * C + c] + d; double var = b / rows - d * d; if (var < 0) var = 0;
       mean[g * C + c] = (float)mu; invstd[g * C + c] = (float)(1.0 / sqrt(var + (double)eps));
       if (g_mean) { acc_gm += (1.0 - decay) * ((double)run_mean[c] - mu); acc_gv += (1.0 - decay) * ((double)run_var[c] - var); }
     }
@@ -178,15 +188,15 @@ void k_bn_stats(int prec, const void* x, int rows, int C, int groups, float* scr
                 const float* run_mean, const float* run_var, float* g_mean, float* g_var, float decay, cudaStream_t s) {
   const bool vec = vec_ok(prec, C);
   int S = vec ? vec_blocks(rows, C) : pick_slices(rows, C);
-  float* psum = scratch; float* psq = scratch + (size_t)groups * S * C;
+  float* psum = scratch; float* psq = scratch + (size_t)groups * S * C; float* pivot = psq + (size_t)groups * S * C;
   if (vec) {
-    launch_pdl(bn_stats_partial_bf16x8_kernel, dim3(dim3(S, groups)), dim3(256), (size_t)(0), s, (const uint4*)x, rows, C, S, psum, psq);
+    launch_pdl(bn_stats_partial_bf16x8_kernel, dim3(dim3(S, groups)), dim3(256), (size_t)(0), s, (const uint4*)x, rows, C, S, psum, psq, pivot);
   } else {
     dim3 grid((S * C + 255) / 256, groups);
-    DISPATCH_PREC(prec, T, (launch_pdl(bn_stats_partial_kernel<T>, dim3(grid), dim3(256), (size_t)(0), s, (const T*)x, rows, C, S, psum, psq)));
+    DISPATCH_PREC(prec, T, (launch_pdl(bn_stats_partial_kernel<T>, dim3(grid), dim3(256), (size_t)(0), s, (const T*)x, rows, C, S, psum, psq, pivot)));
   }
   LAUNCHED();
-  launch_pdl(bn_stats_final_kernel, dim3((C + 31) / 32), dim3(1024), (size_t)(0), s, psum, psq, rows, C, S, groups, eps, mean, invstd, run_mean, run_var, g_mean, g_var, decay); LAUNCHED();
+  launch_pdl(bn_stats_final_kernel, dim3((C + 31) / 32), dim3(1024), (size_t)(0), s, psum, psq, (const float*)pivot, rows, C, S, groups, eps, mean, invstd, run_mean, run_var, g_mean, g_var, decay); LAUNCHED();
 }
 __global__ void bn_prep_infer_kernel(const float* __restrict__ rm, const float* __restrict__ rv, int C, int groups, float eps, float* mean, float* invstd) { pdl_enter();
   int i = blockIdx.x * blockDim.x + threadIdx.x; if (i >= C * groups) return;
@@ -383,9 +393,15 @@ void k_bn_bwd(int prec, const void* x, const void* eps_out, void* eps_in, int ro
 bool k_bn_vec_ok(int prec, int C) { return vec_ok(prec, C); }
 size_t k_bn_acc_elems(int C, int groups) { return (size_t)groups * 4 * C; }
 
-template <int NV>
-__device__ __forceinline__ void block_fold_acc(float (&acc)[NV][8], int C, int c8, int ty, int TY, unsigned long long* accbase /* statistic v at accbase + v*2*C */) {
-  __shared__ float sred[NV][2048];
+// The block fold runs in double.  bn_stats_acc_kernel also sums per thread in double: bn_apply_acc_kernel forms E[x^2] - E[x]^2, a difference
+// of large numbers when |mean| >> std, so this kernel's sum x^2 is not rounded to fp32 on its way into the 128-bit accumulators (the kernel is
+// bandwidth-bound; the double arithmetic is not on its critical path).  The backward per-thread sums stay fp32 (a few rows each); the fold
+// over up to 256 row lanes stays in double because with unit coefficients the same kernel accumulates (sum dy', sum dy'*z), whose conversion
+// to sum dy'*xhat cancels.  The EPI_STATS / EPI_BNBWD GEMM epilogues, the other producers of these accumulators, reduce in fp32 over each
+// 128-row tile.
+template <int NV, typename A>
+__device__ __forceinline__ void block_fold_acc(A (&acc)[NV][8], int C, int c8, int ty, int TY, unsigned long long* accbase /* statistic v at accbase + v*2*C */) {
+  __shared__ double sred[NV][2048];
 #pragma unroll
   for (int v = 0; v < NV; ++v)
 #pragma unroll
@@ -393,20 +409,20 @@ __device__ __forceinline__ void block_fold_acc(float (&acc)[NV][8], int C, int c
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
 #pragma unroll
-    for (int v = 0; v < NV; ++v) { float a = 0.f; for (int k = 0; k < TY; ++k) a += sred[v][k * C + c]; sacc_add(accbase + (size_t)v * 2 * C, (size_t)C, (size_t)c, a); }
+    for (int v = 0; v < NV; ++v) { double a = 0.0; for (int k = 0; k < TY; ++k) a += sred[v][k * C + c]; sacc_add(accbase + (size_t)v * 2 * C, (size_t)C, (size_t)c, a); }
   }
 }
 __global__ void __launch_bounds__(256) bn_stats_acc_kernel(const uint4* __restrict__ x, int rows, int C, int S, unsigned long long* __restrict__ accp) { pdl_enter();
   const int g = blockIdx.y, C8 = C / 8, TY = 256 / C8, c8 = threadIdx.x % C8, ty = threadIdx.x / C8, sl = blockIdx.x;
   const int chunk = (rows + S - 1) / S, r0 = sl * chunk, r1 = min(rows, r0 + chunk);
   const uint4* xg = x + (size_t)g * rows * C8;
-  float acc[2][8];
+  double acc[2][8];
 #pragma unroll
-  for (int j = 0; j < 8; ++j) { acc[0][j] = 0.f; acc[1][j] = 0.f; }
+  for (int j = 0; j < 8; ++j) { acc[0][j] = 0.0; acc[1][j] = 0.0; }
 #pragma unroll 4
   for (int r = r0 + ty; r < r1; r += TY) { float v[8]; unpack8(xg[(size_t)r * C8 + c8], v);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) { acc[0][j] += v[j]; acc[1][j] = fmaf(v[j], v[j], acc[1][j]); } }
+    for (int j = 0; j < 8; ++j) { acc[0][j] += v[j]; acc[1][j] = fma((double)v[j], (double)v[j], acc[1][j]); } }
   block_fold_acc<2>(acc, C, c8, ty, TY, accp + (size_t)g * 4 * C);
 }
 void k_bn_stats_acc(const void* x, int rows, int C, int groups, unsigned long long* acc, cudaStream_t s) {
@@ -414,7 +430,13 @@ void k_bn_stats_acc(const void* x, int rows, int C, int groups, unsigned long lo
   launch_pdl(bn_stats_acc_kernel, dim3(S, groups), dim3(256), (size_t)0, s, (const uint4*)x, rows, C, S, acc); LAUNCHED();
 }
 
-// dynamic shared memory: [groups][2][C] floats = (scale, shift)
+// dynamic shared memory: [groups][2][C] floats = (scale, shift).  coef rows: scale, beta, mean, invstd.
+// The backward kernels' pre-activation: the smooth activations need z's value, formed as (x - mean) * scale + beta (with |mean| >> std,
+// x * scale + shift loses the low bits of z to the rounding of shift); relu / leaky relu only need its sign, taken from the same
+// x * scale + shift the forward evaluated (shift recomputed bit for bit), so that act' and the stored output agree at the kink.
+__device__ __forceinline__ float bn_pre_act(int act, float x, float sc, float be, float mu) {
+  return (act == ACT_RELU || act == ACT_LRELU) ? fmaf(x, sc, fmaf(-mu, sc, be)) : fmaf(x - mu, sc, be);
+}
 template <int ACTC>
 __global__ void __launch_bounds__(256, 3) bn_apply_acc_kernel(const uint4* __restrict__ x, uint4* __restrict__ y, int rows, int C, int groups, const unsigned long long* __restrict__ accp,
                                                              const float* __restrict__ gamma, const float* __restrict__ beta, int act, float alpha, float eps, float* __restrict__ coef,
@@ -436,7 +458,7 @@ __global__ void __launch_bounds__(256, 3) bn_apply_acc_kernel(const uint4* __res
       const float is = (float)(1.0 / sqrt(var + (double)eps)), sc = gamma[c] * is, sh = fmaf(-(float)mu, sc, beta[c]);
       s_cf[(g * 2 + 0) * C + c] = sc; s_cf[(g * 2 + 1) * C + c] = sh;
       if (writer) {
-        coef[(size_t)(g * 4 + 0) * C + c] = sc; coef[(size_t)(g * 4 + 1) * C + c] = sh; coef[(size_t)(g * 4 + 2) * C + c] = (float)mu; coef[(size_t)(g * 4 + 3) * C + c] = is;
+        coef[(size_t)(g * 4 + 0) * C + c] = sc; coef[(size_t)(g * 4 + 1) * C + c] = beta[c]; coef[(size_t)(g * 4 + 2) * C + c] = (float)mu; coef[(size_t)(g * 4 + 3) * C + c] = is;
         if (g_mean) { agm += (1.0 - decay) * ((double)run_mean[c] - mu); agv += (1.0 - decay) * ((double)run_var[c] - var); }
       }
     }
@@ -481,14 +503,14 @@ __global__ void __launch_bounds__(256, 3) bn_bwd_stats_acc_kernel(const uint4* _
   const int g = blockIdx.y, C8 = C / 8, TY = 256 / C8, c8 = threadIdx.x % C8, ty = threadIdx.x / C8, sl = blockIdx.x;
   const int chunk = (rows + S - 1) / S, r0 = sl * chunk, r1 = min(rows, r0 + chunk);
   const uint4* xg = x + (size_t)g * rows * C8; const uint4* eg = eo + (size_t)g * rows * C8;
-  float sc[8], sh[8], mu[8], is[8], acc[2][8];
+  float sc[8], be[8], mu[8], is[8], acc[2][8];
 #pragma unroll
-  for (int j = 0; j < 8; ++j) { const int c = c8 * 8 + j; sc[j] = coef[(size_t)(g * 4 + 0) * C + c]; sh[j] = coef[(size_t)(g * 4 + 1) * C + c]; mu[j] = coef[(size_t)(g * 4 + 2) * C + c]; is[j] = coef[(size_t)(g * 4 + 3) * C + c]; acc[0][j] = 0.f; acc[1][j] = 0.f; }
+  for (int j = 0; j < 8; ++j) { const int c = c8 * 8 + j; sc[j] = coef[(size_t)(g * 4 + 0) * C + c]; be[j] = coef[(size_t)(g * 4 + 1) * C + c]; mu[j] = coef[(size_t)(g * 4 + 2) * C + c]; is[j] = coef[(size_t)(g * 4 + 3) * C + c]; acc[0][j] = 0.f; acc[1][j] = 0.f; }
 #pragma unroll 4
   for (int r = r0 + ty; r < r1; r += TY) {
     float xv[8], ev[8]; unpack8(xg[(size_t)r * C8 + c8], xv); unpack8(eg[(size_t)r * C8 + c8], ev);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) { const float xh = (xv[j] - mu[j]) * is[j]; const float dy = ev[j] * act_grad_from_pre(ACTC < 0 ? act : ACTC, fmaf(xv[j], sc[j], sh[j]), alpha); acc[0][j] += dy; acc[1][j] = fmaf(dy, xh, acc[1][j]); }
+    for (int j = 0; j < 8; ++j) { const float xh = (xv[j] - mu[j]) * is[j]; const float dy = ev[j] * act_grad_from_pre(ACTC < 0 ? act : ACTC, bn_pre_act(ACTC < 0 ? act : ACTC, xv[j], sc[j], be[j], mu[j]), alpha); acc[0][j] += dy; acc[1][j] = fmaf(dy, xh, acc[1][j]); }
   }
   block_fold_acc<2>(acc, C, c8, ty, TY, accp + (size_t)g * 4 * C);
 }
@@ -528,9 +550,9 @@ __global__ void __launch_bounds__(256, 2) bn_bwd_apply_acc_kernel(const uint4* _
   const int c0 = (int)(t0 % C8) * 8;
   bool preloaded = true;
   for (int g = 0; g < groups; ++g) {
-    float sc[8], sh[8], mu[8], is[8], k1[8], k2[8];
+    float sc[8], be[8], mu[8], is[8], k1[8], k2[8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) { const int c = c0 + j; sc[j] = coef[(size_t)(g * 4 + 0) * C + c]; sh[j] = coef[(size_t)(g * 4 + 1) * C + c]; mu[j] = coef[(size_t)(g * 4 + 2) * C + c]; is[j] = coef[(size_t)(g * 4 + 3) * C + c];
+    for (int j = 0; j < 8; ++j) { const int c = c0 + j; sc[j] = coef[(size_t)(g * 4 + 0) * C + c]; be[j] = coef[(size_t)(g * 4 + 1) * C + c]; mu[j] = coef[(size_t)(g * 4 + 2) * C + c]; is[j] = coef[(size_t)(g * 4 + 3) * C + c];
       k1[j] = s_k[(g * 2 + 0) * C + c]; k2[j] = s_k[(g * 2 + 1) * C + c]; }
     const uint4* xg = x + g * per_group; const uint4* eg = eo + g * per_group; uint4* ig = ei + g * per_group;
     for (size_t i = t0; i < per_group; i += 4 * stride) {
@@ -544,7 +566,7 @@ __global__ void __launch_bounds__(256, 2) bn_bwd_apply_acc_kernel(const uint4* _
         float xv[8], ev[8], o[8]; unpack8(xa[q], xv); unpack8(ea[q], ev);
 #pragma unroll
         for (int j = 0; j < 8; ++j) { const float xh = (xv[j] - mu[j]) * is[j];
-          const float dy = PREMUL ? ev[j] : ev[j] * act_grad_from_pre(ACTC < 0 ? act : ACTC, fmaf(xv[j], sc[j], sh[j]), alpha); o[j] = sc[j] * (dy - k1[j] - xh * k2[j]); }
+          const float dy = PREMUL ? ev[j] : ev[j] * act_grad_from_pre(ACTC < 0 ? act : ACTC, bn_pre_act(ACTC < 0 ? act : ACTC, xv[j], sc[j], be[j], mu[j]), alpha); o[j] = sc[j] * (dy - k1[j] - xh * k2[j]); }
         ig[i + q * stride] = pack8(o);
       }
     }

@@ -252,6 +252,14 @@ class Net:
         check(self.lib.b2g_test_hbm_kernels(self.h, rows, channels, iters, _fp(ms)))
         return [float(v) for v in ms]
 
+    def weight_operand(self, layer: int, which: int, size: int) -> np.ndarray:
+        """BF16 nets: the bf16 copy of layer `layer`'s W that the next forward reads (which = 0, internal [A][taps][B] order, `size` = W's
+        element count), or the packed pixel-shuffle operand [(py,px,c)][(dyr,dxc)][O] of the <= 4-channel transposed conv (which = 1,
+        `size` = 144 * O), widened to fp32."""
+        out = np.empty(size, np.float32)
+        check(self.lib.b2g_test_net_shadow(self.h, layer, which, _fp(out), out.size))
+        return out
+
     def input_gradient(self, batch: int) -> np.ndarray:
         out = np.empty((batch, int(np.prod(self.input_shape))), np.float32)
         check(self.lib.b2g_net_get_input_gradient(self.h, batch, _fp(out)))
@@ -340,3 +348,21 @@ def test_conv_ex(ctx: Context, kind: int, geom: Dict[str, int], a, b, out_size: 
     ms = C.c_float()
     check(ctx.lib.b2g_test_conv_ex(ctx.h, kind, 1, BF16, C.byref(g), _fp(a), _fp(b), _fp(out), iters, C.byref(ms), C.byref(o)))
     return out, stats, o.kernel.decode(), ms.value
+
+
+def test_bn(ctx: Context, precision: int, path: int, x, eps_out, gamma, beta, run_mean, run_var, *, act: str = "identity", alpha: float = 0.0,
+            eps: float = 1e-5, decay: float = 0.9, g_gamma=None, g_beta=None, want_param_grads: bool = True):
+    """One BatchNorm(+activation) forward and backward through the training-step kernels (b2g_test_bn).  x, eps_out: [groups, rows, C].
+    Returns a dict with y, eps_in ([groups, rows, C]), g_gamma, g_beta (accumulated into the given initial values), g_mean, g_var ([C]) and
+    mean, invstd ([groups, C])."""
+    x, e = _f32(x), _f32(eps_out)
+    groups, rows, ch = x.shape
+    par = [_f32(v).ravel() for v in (gamma, beta, run_mean, run_var)]
+    r = {k: np.empty(x.shape, np.float32) for k in ("y", "eps_in")}
+    r["g_gamma"] = _f32(np.zeros(ch) if g_gamma is None else g_gamma).copy()
+    r["g_beta"] = _f32(np.zeros(ch) if g_beta is None else g_beta).copy()
+    r.update({k: np.empty(ch, np.float32) for k in ("g_mean", "g_var")})
+    r.update({k: np.empty((groups, ch), np.float32) for k in ("mean", "invstd")})
+    check(ctx.lib.b2g_test_bn(ctx.h, precision, path, groups, rows, ch, _fp(x), _fp(e), *[_fp(v) for v in par], ACTS[act], alpha, eps, decay,
+                              int(want_param_grads), *[_fp(r[k]) for k in ("y", "eps_in", "g_gamma", "g_beta", "g_mean", "g_var", "mean", "invstd")]))
+    return r

@@ -249,6 +249,20 @@ int32_t b2g_test_conv_ex(b2g_ctx* ctx, int32_t kind, int32_t impl, int32_t preci
  * `net` (perturbs its parameters: bench only), ms[1] BatchNorm apply and ms[2] BatchNorm backward apply on a [rows x channels] bf16 tensor. */
 int32_t b2g_test_hbm_kernels(b2g_net* net, int32_t rows, int32_t channels, int32_t iters, float* ms3);
 
+/* One train-mode BatchNorm(+activation act) forward and backward on host tensors x, eps_out [groups*rows][C] (fp32; rounded to bf16 on the
+ * device when precision is BF16), through the kernels of the training step.  path 0: the two-stage kernels (fp32 or bf16, any C);
+ * 1: the 128-bit accumulator kernels (bf16, C % 8 == 0, 256 % (C/8) == 0, else B2G_ERR_UNSUPPORTED); 2: the accumulator kernels in the
+ * state the fused BatchNorm-backward GEMM epilogue leaves: eps_out must already be multiplied by act'.
+ * Out: y, eps_in [groups*rows][C]; g_gamma / g_beta [C] are accumulated into (untouched when want_param_grads = 0); g_mean / g_var [C] =
+ * the running-statistic pseudo-gradients averaged over groups; mean / invstd [groups][C]. */
+int32_t b2g_test_bn(b2g_ctx* ctx, int32_t precision, int32_t path, int32_t groups, int32_t rows, int32_t C, const float* x, const float* eps_out,
+                    const float* gamma, const float* beta, const float* run_mean, const float* run_var, int32_t act, float alpha, float eps, float decay,
+                    int32_t want_param_grads, float* y, float* eps_in, float* g_gamma, float* g_beta, float* g_mean, float* g_var, float* mean, float* invstd);
+/* BF16 nets: the bf16 weight operand the next forward reads instead of the fp32 master, widened to fp32 (n = its element count).
+ * which = 0: the straight copy of W in the internal [A][taps][B] order; 1: the packed [(py,px,c)][(dyr,dxc)][O] operand of the
+ * pixel-shuffle transposed conv onto <= 4 channels (B2G_ERR_UNSUPPORTED if the layer has none). */
+int32_t b2g_test_net_shadow(b2g_net* net, int32_t layer, int32_t which, float* out, int64_t n);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,9 +9,12 @@ semantics) on the same bf16-rounded operands:
 The oracle evaluates whole sampled images (first / last, a few in the middle, the real|fake group boundary) for
 fprop / dgrad, and the full batch in image chunks (the weight gradient is a sum over images) for wgrad.
 """
+import copy
+
 import numpy as np
 import pytest
 
+from helpers import bf16_round, check_bf16, inject_forward
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
@@ -25,18 +28,6 @@ def b200():
     ctx = b.Context(0)
     yield b, ctx
     ctx.close()
-
-
-def bf16_round(a):
-    import torch
-    return torch.tensor(np.asarray(a, np.float32)).to(torch.bfloat16).to(torch.float32).numpy()
-
-
-def check_bf16(got, ref, what):
-    got = np.asarray(got, np.float64); ref = np.asarray(ref, np.float64)
-    tol = 2.0 ** -8 * np.abs(ref) + 2e-3 * np.sqrt(np.mean(ref ** 2)) + 1e-30
-    bad = np.abs(got - ref) > tol
-    assert not bad.any(), f"{what}: {bad.sum()} of {bad.size} elements outside 2^-8|ref| + 2e-3 rms; worst |d|={np.abs(got - ref).max():.4g} rms={np.sqrt(np.mean(ref ** 2)):.4g}"
 
 
 def sample_images(n):
@@ -225,34 +216,6 @@ def _fro(a, b):
     return float(np.linalg.norm(a - b) / (np.linalg.norm(b) + 1e-30))
 
 
-def _inject_forward(onet, bnet, specs, x_in, batch, what):
-    """Runs the oracle net layer by layer, each layer on the GPU's activation of the layer below; checks every produced tensor."""
-    cur = np.asarray(x_in, np.float32)
-    shape = cur.shape
-    i = 0
-    while i < len(specs):
-        t = specs[i]["type"]; l = onet.layers[i]
-        fused = t == "batchnorm" and i + 1 < len(specs) and specs[i + 1]["type"] == "activation"
-        ref = l.forward(cur.reshape(shape), True)
-        if fused:       # the engine stores BatchNorm+activation as one tensor
-            ref = onet.layers[i + 1].forward(ref, True)
-        shape = ref.shape
-        if t in ("conv2d", "deconv2d", "dense", "batchnorm", "output"):
-            got = bnet.activation(i, batch).reshape(shape)
-            if t == "output":
-                got_cmp, ref_cmp = got, l._z.reshape(shape)          # the engine keeps the logits; the oracle's forward returns sigmoid(z)
-            else:
-                got_cmp, ref_cmp = got, ref
-            check_bf16(got_cmp, ref_cmp, f"{what} layer {i} ({specs[i].get('name', t)})")
-            cur = got if t != "output" else got                       # inject the GPU's tensor into the next layer
-            if t == "output":
-                l._z = got.reshape(l._z.shape).astype(l._z.dtype)
-        else:
-            cur = ref
-        i += 2 if fused else 1
-    return cur.reshape(shape)
-
-
 def _grads_by_tensor(onet, flat):
     out, off = {}, 0
     for li, l in enumerate(onet.layers):
@@ -305,7 +268,7 @@ def test_bf16_whole_step_layer_by_layer(b200, case):
         for l in net.layers:
             if l.has_params and "W" in l.params:
                 l.params["W"] = bf16_round(l.params["W"]).astype(np.float32)
-    _inject_forward(D, bD, ds, bf16_round(x2), 2 * n, "D (2N)")
+    inject_forward(D, bD, ds, bf16_round(x2), 2 * n, "D (2N)")
     loss_sum, eps = D.layers[-1].score_and_eps(y2.astype(np.float32))
     if isinstance(D.layers[-1], o.Output):
         eps = D.layers[-1].backward(eps)
@@ -327,8 +290,8 @@ def test_bf16_whole_step_layer_by_layer(b200, case):
         if l.has_params and "W" in l.params:
             l.params["W"] = bf16_round(l.params["W"]).astype(np.float32)
     assert np.abs(bD.params() - pD_before).max() > 0
-    xg = _inject_forward(G, bG, gs, bf16_round(data[2]), n, "G (train, z_g)")
-    _inject_forward(D, bD, ds, xg, n, "D (G step)")
+    xg = inject_forward(G, bG, gs, bf16_round(data[2]), n, "G (train, z_g)")
+    inject_forward(D, bD, ds, xg, n, "D (G step)")
     loss_sum, eps = D.layers[-1].score_and_eps(data[5].astype(np.float32))
     if isinstance(D.layers[-1], o.Output):
         eps = D.layers[-1].backward(eps)
@@ -374,3 +337,169 @@ def test_dense_kernels(b200, case):
     if oc <= 4:
         got, _ = b.test_conv(ctx, 0, 4, b.BF16, g, x, wt, n * oc)
         check_bf16(got.reshape(n, oc), x.astype(np.float64) @ wt.astype(np.float64).T, name + " fprop")
+
+
+# ------------------------------------------------------------------------------------------------
+# BF16 at ragged batches: which kernel a GEMM runs depends on the batch.  A tensor-core tile exists only when pick_row_tile (kernels_tc.cu)
+# finds one for the batch; the fused BatchNorm epilogues (EPI_STATS / EPI_BNBWD) also need every tile inside one statistics group
+# (tc_epi_ok: images per group % images per tile == 0).  Otherwise the SIMT kernels, or the tensor-core GEMM followed by the unfused
+# k_bn_stats_acc / k_bn_bwd_stats_acc, take over.  DCGAN 32x32, nf = 64, z = 16 (every channel count tensor-core eligible), per-net batches
+# N in {1, 3, 4, 8}: between them the layers of one step take all three routes.
+# ------------------------------------------------------------------------------------------------
+def _pick_row_tile(n, gh, gw, rows=128):
+    """Python mirror of kernels_tc.cu pick_row_tile: images per 128-row tile, or None when the batch has no tile."""
+    p = gh * gw
+    if gw > rows or rows % gw:
+        return None
+    if p >= rows:
+        return 1 if p % rows == 0 and gh % (rows // gw) == 0 else None
+    if rows % p or n % (rows // p):
+        return None
+    return rows // p
+
+
+SWEEP_SIZE, SWEEP_Z, SWEEP_NF = 32, 16, 64
+
+
+def _sweep_routes(n):
+    """Route of every GEMM of the generator's train forward (n images, one statistics group) and of the discriminator's pass of the D
+    update (2n images, two groups of n): "fused" (tensor core, BatchNorm statistics in the epilogue), "unfused" (tensor core, then
+    k_bn_stats_acc), "tc" (tensor core, no BatchNorm after it), "simt".  (net, layer name, route)"""
+    def bn_route(rows, groups, gh, gw):
+        nt = _pick_row_tile(rows, gh, gw)
+        if nt is None:
+            return "simt"
+        return "fused" if (rows // groups) % nt == 0 else "unfused"
+    out = [("G", "gen_deconv_1", "simt"),                          # z -> 4x4: the 1x1 problem with a 16-long reduction (dense_small_k, by design)
+           ("G", "gen_deconv_2", bn_route(n, 1, 4, 4)),             # conv-equivalent output grid = the 4x4 input map
+           ("G", "gen_deconv_3", bn_route(n, 1, 8, 8)),
+           ("G", "gen_deconv_4", "tc"),                             # pixel-shuffle conv over 16x16 blocks: a tile for every batch
+           ("D", "dis_conv_1", "tc"),                               # 3-channel edge conv
+           ("D", "dis_conv_2", bn_route(2 * n, 2, 8, 8)),
+           ("D", "dis_conv_3", bn_route(2 * n, 2, 4, 4)),
+           ("D", "dis_conv_4", "simt")]                             # the logit (one output unit, by design)
+    return out
+
+
+SWEEP_N = (1, 3, 4, 8)
+# Largest relative Frobenius error of any gradient tensor checked on injected activations, measured at N = 8 (every BatchNorm fused) on an
+# H100 80GB HBM3: 0.0364; bound = 2x that.  Every ragged N must meet the same bound: the fallback routes may not be less accurate than the
+# fused one (measured at N = 1 / 3 / 4: 0.0069 / 0.0061 / 0.0069).
+SWEEP_GRAD_FRO = 0.073
+# The D pass of the step (two BatchNorm groups of N: the unfused routes) is compared with the oracle run on its own, not on injected
+# activations, so rounding compounds through the layers and grows as the groups shrink.  Measured on the same H100: 0.051 / 0.080 / 0.090 /
+# 0.123 at N = 8 / 4 / 3 / 1; bound = 2x the largest.  A wrong route (statistics of the wrong group, a missing term) is off by O(1).
+SWEEP_STEP_D_FRO = 0.25
+
+
+def test_ragged_batch_route_table_covers_every_route():
+    routes = {r for n in SWEEP_N for _, _, r in _sweep_routes(n)}
+    assert {"fused", "unfused", "simt"} <= routes, routes
+    assert all(r == "fused" for _, name, r in _sweep_routes(8) if name in ("gen_deconv_2", "gen_deconv_3", "dis_conv_2", "dis_conv_3"))
+
+
+def _oracle_grads(onet):
+    out = {}
+    for li, l in enumerate(onet.layers):
+        if l.has_params:
+            for pname, _, _ in l.param_specs():
+                out[(li, pname)] = _flat_order(l, pname)
+    return out
+
+
+def _check_grads(got_flat, want, onet, specs, what, fro_bound, errs, injected=True):
+    """injected: the oracle ran on the GPU's own activations, so the running-statistic pseudo-gradients (1 - decay) * (running - batch
+    statistic) must match to 1e-4 relative; otherwise they are held to the Frobenius bound like every other gradient."""
+    got = _grads_by_tensor(onet, got_flat)
+    for (li, pname), gv in got.items():
+        ref = want[(li, pname)]
+        if injected and pname in ("mean", "var"):
+            e = float(np.abs(gv - ref).max() / (np.abs(ref).max() + 1e-30))
+            assert e <= 1e-4, (f"{what}: {specs[li].get('name')}.{pname}", e)
+            continue
+        fro = _fro(gv, ref); errs.append(fro)
+        if fro_bound is not None:
+            assert fro <= fro_bound, (f"{what}: {specs[li].get('name')}.{pname}", fro, fro_bound)
+
+
+@pytest.mark.parametrize("n", SWEEP_N)
+def test_bf16_ragged_batch_routes_layer_by_layer(b200, n):
+    b, ctx = b200
+    from gan_deeplearning4j_b200 import models as m
+    from helpers import oracle_from_specs, push_params, randomize
+    size, z, nf = SWEEP_SIZE, SWEEP_Z, SWEEP_NF
+    rng = np.random.default_rng(31 + n)
+    gs, ds, dshape = m.dcgan_generator(size, z, nf, 3), m.dcgan_discriminator(size, nf, 3), (3, size, size)
+    data = [np.asarray(a, np.float32) for a in o.synthetic_batch(n, size, 3, z, seed=40 + n)]
+    q = o.Quirks(xent_clip_eps=0.0)
+    G = oracle_from_specs(gs, (z,), quirks=q, dtype=np.float32, seed=1); D = oracle_from_specs(ds, dshape, quirks=q, dtype=np.float32, seed=2, flat_input=False)
+    randomize(G, rng); randomize(D, rng)
+    bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.BF16, xent_clip_eps=0.0)
+    bD = b.Net(ctx, ds, dshape, max_batch=2 * n, precision=b.BF16, xent_clip_eps=0.0, bn_groups=2)
+    push_params(G, bG); push_params(D, bD)
+    for net in (G, D):
+        for l in net.layers:
+            if l.has_params and "W" in l.params:
+                l.params["W"] = bf16_round(l.params["W"]).astype(np.float32)
+    routes = _sweep_routes(n)
+    errs = []
+    # ---- the SIMT count of a train-mode forward is the table's (the D pass and D.output see the same 2N rows)
+    x2 = np.concatenate([data[0], rng.uniform(-1, 1, data[0].shape).astype(np.float32)])
+    for net, tag, x in ((bG, "G", data[1]), (bD, "D", x2)):
+        s0 = net.simt_gemm_calls(); net.output(x, train=True)
+        assert net.simt_gemm_calls() - s0 == sum(r == "simt" for t, _, r in routes if t == tag), (tag, n, routes)
+    # ---- inference-mode slicing invariance: the first k images of a batch through the kernels of batch k (other routes, same inputs)
+    for net, specs, x in ((bG, gs, data[1]), (bD, ds, x2)):
+        full = net.output(x)
+        layers = [li for li, s in enumerate(specs) if s["type"] == "batchnorm" or
+                  (s["type"] in ("conv2d", "deconv2d", "dense") and not (li + 1 < len(specs) and specs[li + 1]["type"] == "batchnorm"))]
+        acts = {li: net.activation(li, x.shape[0]) for li in layers}
+        for k in sorted({1, max(1, x.shape[0] - 1)}):
+            if k == x.shape[0]:
+                continue
+            part = net.output(x[:k])
+            tol = lambda ref: 2 * 2.0 ** -8 * np.abs(ref) + 2e-3 * np.sqrt(np.mean(ref.astype(np.float64) ** 2)) + 1e-30
+            assert (np.abs(part - full[:k]) <= tol(full[:k])).all(), ("output", n, k)
+            for li in layers:
+                ref = acts[li][:k]
+                assert (np.abs(net.activation(li, k) - ref) <= tol(ref)).all(), (specs[li]["name"], n, k)
+    # ---- D's train pass on 2N images (one statistics group), layer by layer with injected activations; every gradient incl. mean / var
+    y2 = np.concatenate([data[3], data[4]])
+    bD.compute_gradient_and_score(x2, y2)
+    inject_forward(D, bD, ds, bf16_round(x2), 2 * n, f"D (2N = {2 * n})")
+    _, eps = D.layers[-1].score_and_eps(y2.astype(np.float32))
+    D.backward_from_prefix(eps)
+    _check_grads(bD.gradients(), _oracle_grads(D), D, ds, f"D train pass, N = {n}", SWEEP_GRAD_FRO, errs)
+    # ---- the adversarial step.  Its D pass runs 2N images as two BatchNorm groups (the unfused routes): its gradients are still in D's
+    # gradient buffer afterwards (the G step through D computes no D weight gradient); reference = the oracle on each group, summed
+    x_fake = bG.output(data[1])                                     # gen.output(z_d): what the step feeds D as fakes (same kernels, same params)
+    D0 = [copy.deepcopy(l) for l in D.layers]
+    gan = b.Gan(bG, bD, use_cuda_graph=False)
+    gan.step(*data)
+    want = {}
+    for gi, (xg_, yg_) in enumerate(((bf16_round(data[0]), data[3]), (bf16_round(x_fake.reshape(data[0].shape)), data[4]))):
+        D.layers = [copy.deepcopy(l) for l in D0]
+        cur = xg_.astype(np.float32)
+        for l in D.layers:
+            cur = l.forward(cur, True)
+        _, eps = D.layers[-1].score_and_eps(yg_.astype(np.float32))
+        D.backward_from_prefix(eps)
+        for key, v in _oracle_grads(D).items():
+            want[key] = want.get(key, 0) + (0.5 * v if key[1] in ("mean", "var") else v)
+    step_errs = []
+    _check_grads(bD.gradients(), want, D, ds, f"D pass of the step (two groups of N = {n})", SWEEP_STEP_D_FRO, step_errs, injected=False)
+    # ---- the generator step: G train forward on z_g and D forward on its output, injected; every G gradient incl. mean / var
+    D.layers = [copy.deepcopy(l) for l in D0]
+    D.set_params_flat(bD.params().astype(np.float32))
+    for l in D.layers:
+        if l.has_params and "W" in l.params:
+            l.params["W"] = bf16_round(l.params["W"]).astype(np.float32)
+    xg = inject_forward(G, bG, gs, bf16_round(data[2]), n, f"G (train, N = {n})")
+    inject_forward(D, bD, ds, xg, n, f"D (G step, N = {n})")
+    _, eps = D.layers[-1].score_and_eps(data[5].astype(np.float32))
+    eps_g = D.backward_from_prefix(eps).reshape(xg.shape)
+    for l in reversed(G.layers):
+        eps_g = l.backward(eps_g)
+    _check_grads(bG.gradients(), _oracle_grads(G), G, gs, f"G step, N = {n}", SWEEP_GRAD_FRO, errs)
+    print(f"ragged-batch sweep N={n}: largest relative Frobenius gradient error {max(errs):.4g} (injected), {max(step_errs):.4g} (D pass of the step)")
+    gan.close(); bG.close(); bD.close()

@@ -8,7 +8,7 @@ compared kernel-by-kernel against the oracle evaluated on the same bf16-rounded 
 import numpy as np
 import pytest
 
-from helpers import oracle_from_specs, push_params, randomize, rel_err
+from helpers import bf16_round, oracle_from_specs, pack_deconv_ps, push_params, randomize, rel_err, w_internal
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
@@ -207,11 +207,6 @@ def _params_of(spec, net):
 # ------------------------------------------------------------------------------------------------
 # bf16 / kernel-level parity
 # ------------------------------------------------------------------------------------------------
-def bf16_round(a):
-    import torch
-    return torch.tensor(np.asarray(a, np.float32)).to(torch.bfloat16).to(torch.float32).numpy()
-
-
 CONV_CASES = [
     # n, h, w, c, o, k, s, p
     (2, 8, 8, 16, 24, 4, 2, 1), (3, 7, 9, 5, 6, 5, 2, 0), (2, 14, 14, 8, 4, 5, 1, 2), (4, 1, 1, 20, 12, 1, 1, 0), (2, 4, 4, 32, 1, 4, 1, 0),
@@ -730,3 +725,116 @@ def test_single_process_parameter_averaging_matches_oracle(b200):
     assert diff.max() <= 2 * 0.002 + 1e-6 and (diff > 1e-5).mean() < 0.02, (diff.max(), (diff > 1e-5).mean())
     assert bnet.iteration() == 1
     bnet.close()
+
+
+# ------------------------------------------------------------------------------------------------
+# The bf16 weight operands a BF16 net's forward reads instead of the fp32 master: the straight copy of every GEMM weight, and the packed
+# [(py,px,c)][(dyr,dxc)][O] operand of the pixel-shuffle transposed conv onto <= 4 channels.  After an update the updater kernel writes both
+# itself (vector or scalar branch, through its own inverse of the packing map); setParam / setParams / parameter averaging rewrite them
+# from the master.  Either way they must equal the master rounded to nearest even, bit for bit.
+# ------------------------------------------------------------------------------------------------
+def _ps_operand_O(spec):
+    """O of the [O][4][4][C] weight when the layer's conv-equivalent is a 4x4 s2 p1 conv with C <= 4 image channels and O % 64 == 0 (the
+    transposed conv onto the image, and the input gradient of the conv that reads it), else 0."""
+    if tuple(spec.get("kernel", ())) != (4, 4) or tuple(spec.get("stride", ())) != (2, 2) or tuple(spec.get("padding", ())) != (1, 1):
+        return 0
+    O, C = (spec["n_in"], spec["n_out"]) if spec["type"] == "deconv2d" else (spec["n_out"], spec["n_in"])
+    return O if C <= 4 and O % 64 == 0 else 0
+
+
+def _check_weight_operands(b, net, specs, what):
+    packed = 0
+    for li, s in enumerate(specs):
+        if s["type"] not in ("conv2d", "deconv2d", "dense", "output"):
+            continue
+        k = s.get("kernel", (1, 1)); size = s["n_in"] * s["n_out"] * k[0] * k[1]
+        w = bf16_round(w_internal(s, net.get_param(s["name"], "W", size)))
+        assert np.array_equal(net.weight_operand(li, 0, size), w), f"{what}: bf16 copy of {s['name']}.W differs from the rounded master"
+        O = _ps_operand_O(s)
+        if O:
+            got = net.weight_operand(li, 1, 144 * O)
+            assert np.array_equal(got, pack_deconv_ps(w.reshape(O, 4, 4, -1))), f"{what}: packed pixel-shuffle operand of {s['name']}"
+            packed += 1
+        else:
+            with pytest.raises(b.B200GanError) as e:
+                net.weight_operand(li, 1, 144)
+            assert e.value.code == -6
+    return packed
+
+
+def test_bf16_gan_weight_operands_track_the_master(b200):
+    """DCGAN 32x32, nf = 64: G-last (64 -> 3) and D-first's input gradient run the pixel-shuffle tensor-core conv.  Three Gan.steps and a resident step replayed from the CUDA
+    graph; after each, every GEMM layer's bf16 operands of both nets equal the rounded fp32 master."""
+    b, ctx = b200
+    size, z, nf, n = 32, 16, 64, 8
+    G, D, bG, bD = _gan_pair(b, ctx, size, z, nf, n, b.BF16)
+    from gan_deeplearning4j_b200 import models as m
+    gs, ds = m.dcgan_generator(size, z, nf, 3, lr=2e-3), m.dcgan_discriminator(size, nf, 3, lr=2e-3)
+    assert _check_weight_operands(b, bG, gs, "G after set_params") == 1 and _check_weight_operands(b, bD, ds, "D after set_params") == 1
+    gan = b.Gan(bG, bD, use_cuda_graph=True)
+    data = [a.astype(np.float32) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
+    g0 = bG.params()
+    for it in range(3):
+        gan.step(*data)
+        assert _check_weight_operands(b, bG, gs, f"G after step {it + 1}") == 1
+        _check_weight_operands(b, bD, ds, f"D after step {it + 1}")
+    data2 = [a.astype(np.float32) for a in o.synthetic_batch(n, size, 3, z, seed=4)]
+    gan.upload(*data2); gan.step_resident(n); ctx.sync()
+    _check_weight_operands(b, bG, gs, "G after a resident step"); _check_weight_operands(b, bD, ds, "D after a resident step")
+    assert np.abs(bG.params() - g0).max() > 0
+    gan.close(); bG.close(); bD.close()
+
+
+def _ps_fit_specs(updater, ps_bias):
+    """A (64, 8, 8) map -> pixel-shuffle transposed conv to 3 channels -> conv -> whole-map conv -> logit.  With a bias the transposed conv's
+    W segment starts at flat offset 3 ([b | W]): the updater writes it from its scalar branch; without, from its 16-byte branch."""
+    return [{"type": "deconv2d", "name": "ps", "n_in": 64, "n_out": 3, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "has_bias": ps_bias,
+             "activation": "tanh", "updater": updater, "l2": 1e-3},
+            {"type": "conv2d", "name": "c1", "n_in": 3, "n_out": 64, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "activation": "lrelu", "alpha": 0.2,
+             "updater": updater, "l2": 1e-3},
+            {"type": "conv2d", "name": "c2", "n_in": 64, "n_out": 1, "kernel": (8, 8), "updater": updater, "l2": 1e-3},
+            {"type": "loss", "name": "loss"}]
+
+
+@pytest.mark.parametrize("ps_bias", [True, False], ids=["ps-W-at-offset-3", "ps-W-aligned"])
+@pytest.mark.parametrize("upd", ["sgd", "rmsprop", "adam"])
+def test_bf16_fit_weight_operands_track_the_master(b200, upd, ps_bias):
+    b, ctx = b200
+    from gan_deeplearning4j_b200 import models as m
+    u = {"sgd": m.sgd(0.05), "rmsprop": m.rmsprop(1e-3, 0.9, 1e-6), "adam": m.adam(1e-3)}[upd]
+    specs = _ps_fit_specs(u, ps_bias)
+    off = 0
+    for li, name, p, shape, _ in oracle_from_specs(specs, (64, 8, 8)).param_table():
+        if (name, p) == ("ps", "W"):
+            break
+        off += int(np.prod(shape))
+    assert off == (3 if ps_bias else 0)
+    net = b.Net(ctx, specs, (64, 8, 8), max_batch=6, precision=b.BF16, grad_clip=0.5)
+    rng = np.random.default_rng(8)
+    for it in range(3):
+        net.fit(rng.standard_normal((6, 64, 8, 8)).astype(np.float32), rng.uniform(0, 1, (6, 1)).astype(np.float32))
+        assert _check_weight_operands(b, net, specs, f"{upd} fit {it + 1}") == 2
+    net.close()
+
+
+def test_bf16_weight_operands_after_set_params_set_param_restore_and_averaging(b200, tmp_path):
+    """The host-side rewrites of the master: setParams (all layers), setParam of the packed layer alone (net_refresh_shadow's only_layer),
+    restore from a checkpoint, and single-process parameter averaging."""
+    b, ctx = b200
+    from gan_deeplearning4j_b200 import models as m, parallel
+    specs = _ps_fit_specs(m.adam(1e-3), True)
+    net = b.Net(ctx, specs, (64, 8, 8), max_batch=6, precision=b.BF16)
+    rng = np.random.default_rng(9)
+    net.set_params((0.05 * rng.standard_normal(net.num_params())).astype(np.float32))
+    _check_weight_operands(b, net, specs, "set_params")
+    net.set_param("ps", "W", (0.1 * rng.standard_normal(64 * 3 * 16)).astype(np.float32))
+    _check_weight_operands(b, net, specs, "set_param(ps, W)")
+    path = str(tmp_path / "ps.zip"); net.save(path)
+    other = b.Net(ctx, specs, (64, 8, 8), max_batch=6, precision=b.BF16, seed=5)
+    other.restore(path)
+    assert np.array_equal(other.params(), net.params())
+    _check_weight_operands(b, other, specs, "restore")
+    d = [(rng.standard_normal((6, 64, 8, 8)).astype(np.float32), rng.uniform(0, 1, (6, 1)).astype(np.float32)) for _ in range(2)]
+    parallel.fit_parameter_averaging(net, d, averaging_frequency=1)
+    _check_weight_operands(b, net, specs, "parameter averaging")
+    net.close(); other.close()

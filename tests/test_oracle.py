@@ -14,7 +14,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from helpers import randomize
+from helpers import pack_deconv_ps, randomize
 from oracle import dl4j_oracle as o
 
 
@@ -475,3 +475,25 @@ def test_golden_vectors_pin_the_oracle():
         assert set(stored.files) == set(fresh), fname
         for k in stored.files:
             np.testing.assert_allclose(fresh[k], stored[k], rtol=1e-9, atol=1e-12, err_msg=f"{fname}:{k}")
+
+
+@pytest.mark.parametrize("C", [1, 3, 4])
+def test_pixel_shuffle_packing_reproduces_the_transposed_conv(C):
+    """tests/helpers.pack_deconv_ps (the reference for the packed operand the BF16 updater writes), used as a 3x3 convolution over the 2x2
+    output blocks, is the 4x4 stride-2 pad-1 Deconvolution2D forward of the oracle: out[2Y+py, 2X+px, c] = sum over (dyr, dxc, o) of
+    P[py,px,c][dyr,dxc][o] * x[Y+dyr, X+dxc, o], with x zero outside the map."""
+    rng = np.random.default_rng(C)
+    n, O, H, W = 2, 6, 5, 7
+    lay = o.Deconv2D(O, C, (4, 4), (2, 2), (1, 1), has_bias=False); lay.init(rng, np.float64)
+    x = rng.standard_normal((n, O, H, W))
+    ref = lay.forward(x, True)                                                  # [n, C, 2H, 2W]
+    P = pack_deconv_ps(lay.params["W"].transpose(0, 2, 3, 1)).reshape(2, 2, 4, 3, 3, O)      # internal [O][4][4][C]
+    xp = np.pad(x.transpose(0, 2, 3, 1), ((0, 0), (1, 1), (1, 1), (0, 0)))        # NHWC, one zero row / column each side
+    got = np.zeros((n, H, 2, W, 2, 4))
+    for dyr in (-1, 0, 1):
+        for dxc in (-1, 0, 1):
+            win = xp[:, 1 + dyr:1 + dyr + H, 1 + dxc:1 + dxc + W, :]            # x[Y+dyr, X+dxc]
+            got += np.einsum("nyxo,pqco->nypxqc", win, P[:, :, :, dyr + 1, dxc + 1, :])
+    assert not got[..., C:].any()                                               # padded channels stay empty
+    got = got[..., :C].reshape(n, 2 * H, 2 * W, C).transpose(0, 3, 1, 2)
+    np.testing.assert_allclose(got, ref, rtol=1e-12, atol=1e-12)
