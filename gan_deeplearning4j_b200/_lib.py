@@ -81,6 +81,8 @@ PROTOTYPES = {
     "b2g_net_fit": (_i32, [_vp, _fp, _fp, _i32, _fp]),
     "b2g_net_get_iteration": (_i32, [_vp, C.POINTER(_i64)]),
     "b2g_net_set_iteration": (_i32, [_vp, _i64]),
+    "b2g_net_get_dropout_pass": (_i32, [_vp, C.POINTER(_i64)]),
+    "b2g_net_set_dropout_pass": (_i32, [_vp, _i64]),
     "b2g_net_simt_gemm_calls": (_i32, [_vp, C.POINTER(C.c_uint64)]),
     "b2g_gan_create": (_i32, [_vp, _vp, C.POINTER(GanConfig), _pvp]),
     "b2g_gan_destroy": (_i32, [_vp]),
@@ -104,6 +106,7 @@ PROTOTYPES = {
     "b2g_test_bn": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _fp, _fp, _fp, _fp, _fp, _fp, _i32, C.c_float, C.c_float, C.c_float,
                            _i32, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     "b2g_test_net_shadow": (_i32, [_vp, _i32, _i32, _fp, _i64]),
+    "b2g_test_dropout": (_i32, [_vp, _i32, C.c_uint64, _i32, _i32, _i64, _i32, _i32, _i32, _i32, C.c_float, _fp, _fp, _fp, _fp]),
 }
 
 _lib = None

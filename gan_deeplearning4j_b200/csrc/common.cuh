@@ -45,6 +45,20 @@ __device__ __forceinline__ double sacc_read(const unsigned long long* hi_lo, siz
   return (double)(long long)hi_lo[idx] * (1.0 / 1024.0) + (double)(long long)hi_lo[stride + idx] * (1.0 / 1152921504606846976.0);
 }
 
+// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC'11; the Random123 constants): a counter-based generator,
+// so a mask element's random word is a pure function of (counter, key) and needs no state beyond the counter the caller forms.
+struct Philox4 { uint32_t x[4]; };
+__device__ __forceinline__ Philox4 philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+    const uint32_t lo0 = 0xD2511F53u * c0, hi0 = __umulhi(0xD2511F53u, c0);
+    const uint32_t lo1 = 0xCD9E8D57u * c2, hi1 = __umulhi(0xCD9E8D57u, c2);
+    c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
+  }
+  return Philox4{{c0, c1, c2, c3}};
+}
+
 #define DISPATCH_PREC(prec, T, ...)                                   \
   do {                                                                \
     if ((prec) == ::b2g::PREC_F32) { using T = float; __VA_ARGS__; }  \

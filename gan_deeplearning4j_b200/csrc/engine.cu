@@ -97,6 +97,10 @@ struct LayerRT {
   int fused_act = ACT_IDENTITY; float fused_alpha = 0.f;       // BN followed by an ActivationLayer
   bool act_fused_into_prev = false;
   float* wg_part = nullptr; size_t wg_part_floats = 0;         // split-K partials of this layer's tensor-core weight gradient (reduced by ONE k_reduce_multi per pass)
+  // DropoutLayer: its own output buffer (never its input: the layer below differentiates from its own pre-dropout output) and the 1-bit
+  // keep mask of the latest train-mode forward; `out` is drop_buf after a masked forward and the input itself after a pass-through one
+  void* drop_buf = nullptr; uint32_t* drop_mask = nullptr; bool drop_live = false;
+  bool drop_active() const { return d.type == B2G_LAYER_DROPOUT && !d.frozen && d.act_alpha < 1.f; }   // FrozenLayer: test mode, identity
   bool has_gemm() const { return d.type == B2G_LAYER_CONV2D || d.type == B2G_LAYER_DECONV2D || d.type == B2G_LAYER_DENSE || d.type == B2G_LAYER_OUTPUT; }
 };
 
@@ -121,6 +125,8 @@ struct b2g_net {
   std::vector<cudaEvent_t> ev_fork, ev_done; cudaEvent_t ev_join = nullptr;
   unsigned long long* bn_acc = nullptr; size_t bn_acc_bytes = 0;  // every BatchNorm layer's accumulators, zeroed by one memset per train-mode forward
   unsigned* upd_ticket = nullptr;                                  // block-completion counter of the updater kernel (the last block bumps step_dev)
+  unsigned long long* drop_pass = nullptr;                         // dropout pass counter P (device): read by every dropout kernel of a train-mode pass
+  unsigned* drop_ticket = nullptr;                                 // block-completion counter of the pass's last dropout kernel (its last block bumps P)
   ReduceList pending{};                                            // split-K partial sums queued by this backward pass
   uint64_t simt_gemm_calls = 0;                                    // BF16 nets: GEMM-shaped ops that ran on the SIMT kernels (skinny / unsupported shapes) -- reported, never silent
   float* scratch = nullptr; size_t scratch_floats = 0;
@@ -225,6 +231,12 @@ static int32_t net_build(b2g_net* n, const b2g_layer_desc* layers, int32_t nl) {
         if ((size_t)d.pre_h * d.pre_w * d.pre_c != l.in_elems) return fail(B2G_ERR_SHAPE, "layer %s: FeedForwardToCnn(%d,%d,%d) != %zu features", d.name, d.pre_h, d.pre_w, d.pre_c, l.in_elems);
         l.oh = d.pre_h; l.ow = d.pre_w; l.oc = d.pre_c; break;
       case B2G_LAYER_CNN_TO_FF: l.oh = l.ow = 1; l.oc = h * w * ch; break;
+      case B2G_LAYER_DROPOUT:        // DropoutLayer.Builder(p): p = retain probability, carried in act_alpha; no parameters
+        if (!(d.act_alpha > 0.f && d.act_alpha <= 1.f)) return fail(B2G_ERR_ARG, "layer %s: dropout retain probability %g outside (0, 1]", d.name, (double)d.act_alpha);
+        l.oh = h; l.ow = w; l.oc = ch;
+        if ((uint64_t)c.max_batch * h * w * ch > (1ull << 34))     // checked before anything is allocated
+          return fail(B2G_ERR_UNSUPPORTED, "layer %s: a dropout pass of %llu elements exceeds the 2^34 the mask counter addresses", d.name, (unsigned long long)c.max_batch * h * w * ch);
+        break;
       default: return fail(B2G_ERR_ARG, "layer %d: unknown type %d", i, d.type);
     }
     l.out_elems = (size_t)l.oh * l.ow * l.oc;
@@ -252,6 +264,8 @@ static int32_t net_alloc(b2g_net* n) {
   B2(dalloc(n, &n->st0, sizeof(float) * n->n_params)); B2(dalloc(n, &n->st1, sizeof(float) * n->n_params));
   if (n->n_shadow) B2(dalloc(n, &n->shadow, sizeof(__nv_bfloat16) * n->n_shadow));
   B2(dalloc(n, &n->upd_ticket, sizeof(unsigned))); CU(cudaMemsetAsync(n->upd_ticket, 0, sizeof(unsigned), n->ctx->stream));
+  B2(dalloc(n, &n->drop_pass, sizeof(unsigned long long))); CU(cudaMemsetAsync(n->drop_pass, 0, sizeof(unsigned long long), n->ctx->stream));
+  B2(dalloc(n, &n->drop_ticket, sizeof(unsigned))); CU(cudaMemsetAsync(n->drop_ticket, 0, sizeof(unsigned), n->ctx->stream));
   B2(dalloc(n, &n->step_dev, sizeof(int))); B2(dalloc(n, &n->loss_dev, sizeof(float) * 8)); B2(dalloc(n, &n->l2_dev, sizeof(double)));
   B2(dalloc(n, &n->labels_dev, sizeof(float) * R * std::max<size_t>(1, n->L.back().out_elems)));
   B2(dalloc(n, (char**)&n->input, ts * R * n->in_elems));
@@ -263,6 +277,7 @@ static int32_t net_alloc(b2g_net* n) {
                  (l.d.type == B2G_LAYER_CNN_TO_FF && (l.ic == 1 || l.ih * l.iw == 1));
     l.out_alias = alias;
     if (!alias) B2(dalloc(n, (char**)&l.out, ts * R * l.out_elems));
+    if (l.d.type == B2G_LAYER_DROPOUT) { l.drop_buf = l.out; B2(dalloc(n, &l.drop_mask, sizeof(uint32_t) * (((size_t)R * l.out_elems + 31) / 32))); }
     if (l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS) B2(dalloc(n, (char**)&l.probs, ts * R * l.out_elems));
     if (l.d.type == B2G_LAYER_MAXPOOL) B2(dalloc(n, &l.argmax, (size_t)R * l.out_elems));
     if (l.d.type == B2G_LAYER_BATCHNORM) { B2(dalloc(n, &l.bn_fold, sizeof(float) * 2 * l.oc)); B2(dalloc(n, &l.bn_mean, sizeof(float) * G * l.oc)); B2(dalloc(n, &l.bn_invstd, sizeof(float) * G * l.oc)); scratch = std::max(scratch, k_bn_scratch_floats(l.oc, G));
@@ -458,6 +473,15 @@ static int32_t gemm_wgrad(b2g_net* n, LayerRT& l, const ConvGeom& g, const void*
   note_simt(n); k_simt_wgrad(n->prec, g, x, dy, dw, scratch, n->scratch_floats, 0, s); return 0;
 }
 
+// The mask inputs of a DropoutLayer (include/b200gan.h): key = the net's seed (0 -> 666, as for Xavier init), counter word 3 = chain index |
+// rank << 16.  The rank is fixed per context, so a captured graph may hold it; P is read by the kernel.
+static DropoutArgs make_dropout_args(uint64_t seed, int layer, int rank, float p) {
+  DropoutArgs a{}; a.seed = seed ? seed : 666; a.tag = (uint32_t)layer | ((uint32_t)rank << 16);
+  a.keep_all = p >= 1.f ? 1 : 0; a.threshold = a.keep_all ? 0u : (uint32_t)floor((double)p * 4294967296.0); a.scale = 1.0f / p;
+  return a;
+}
+static DropoutArgs dropout_args(const b2g_net* n, int layer) { return make_dropout_args(n->cfg.seed, layer, n->ctx->rank, n->L[layer].d.act_alpha); }
+
 // Runs layers [0, L) on `in` (T NHWC, rows examples). Returns pointer to the final activations.
 static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const void** result) {
   cudaStream_t s = fstream(n);
@@ -469,6 +493,9 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
   if (o.train && n->bn_acc) CU(cudaMemsetAsync(n->bn_acc, 0, n->bn_acc_bytes, s));
   static int fold_bn = -1; if (fold_bn < 0) { const char* e = getenv("B2G_FOLD_BN"); fold_bn = (e && e[0] == '0') ? 0 : 1; }
   static int fuse_bn = -1; if (fuse_bn < 0) { const char* e = getenv("B2G_FUSE_BN"); fuse_bn = (e && e[0] == '0') ? 0 : 1; }
+  // every masked DropoutLayer of a train-mode pass draws with the same pass counter P; the last one's kernel advances P on the device
+  int last_drop = -1;
+  if (o.train) for (size_t i = 0; i < n->L.size(); ++i) if (n->L[i].drop_active()) last_drop = (int)i;
   for (size_t i = 0; i < n->L.size(); ++i) {
     LayerRT& l = n->L[i]; const b2g_layer_desc& d = l.d;
     void* out = l.out;
@@ -518,6 +545,14 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
       case B2G_LAYER_LOSS: out = (void*)cur; break;
       case B2G_LAYER_FF_TO_CNN: if (l.out_alias) out = (void*)cur; else k_permute(n->prec, cur, out, R, l.oc, l.oh * l.ow, 1, s); break;
       case B2G_LAYER_CNN_TO_FF: if (l.out_alias) out = (void*)cur; else k_permute(n->prec, cur, out, R, l.ic, l.ih * l.iw, 0, s); break;
+      case B2G_LAYER_DROPOUT:
+        l.drop_live = o.train && l.drop_active();
+        if (l.drop_live) {
+          k_dropout_fwd(n->prec, cur, l.drop_buf, l.drop_mask, (size_t)R * l.out_elems, dropout_args(n, (int)i), n->drop_pass, n->drop_ticket, (int)i == last_drop, s);
+          out = l.drop_buf;
+        } else out = (void*)cur;       // inference, FrozenLayer or p = 1: the identity, no launch
+        l.out = out;
+        break;
     }
     if (fuse) n->L[i + 1].stats_by_producer = fused;
     if (l.out_alias) l.out = out;
@@ -648,6 +683,7 @@ static int32_t net_backward(b2g_net* n, const void* net_in, void* eps, int rows,
       case B2G_LAYER_UPSAMPLE2D: if (need_in) { void* nx = other(cur); k_upsample_bwd(n->prec, cur, nx, R, l.ih, l.iw, l.ic, d.k_h, s); cur = nx; } break;
       case B2G_LAYER_FF_TO_CNN: if (!l.out_alias && need_in) { void* nx = other(cur); k_permute(n->prec, cur, nx, R, l.oc, l.oh * l.ow, 0, s); cur = nx; } break;
       case B2G_LAYER_CNN_TO_FF: if (!l.out_alias && need_in) { void* nx = other(cur); k_permute(n->prec, cur, nx, R, l.ic, l.ih * l.iw, 1, s); cur = nx; } break;
+      case B2G_LAYER_DROPOUT: if (need_in && l.drop_live) k_dropout_bwd(n->prec, cur, cur, l.drop_mask, (size_t)R * l.out_elems, 1.0f / d.act_alpha, s); break;   // the forward's mask
     }
     if (i == n->ar_split_layer && want_wgrad && allreduce_follows && ar_overlap_on(n)) {
       // every gradient of layers >= i is queued (BN scale/shift on s, weights/biases on s2): all-reduce that tail on the comm stream now
@@ -1014,7 +1050,7 @@ extern "C" int32_t b2g_gan_create(b2g_net* gen, b2g_net* dis, const b2g_gan_conf
   if (gen->ctx != dis->ctx) return fail(B2G_ERR_ARG, "generator and discriminator live on different contexts");
   if (gen->prec != dis->prec) return fail(B2G_ERR_ARG, "generator and discriminator use different precisions");
   if (gen->L.back().out_elems != dis->in_elems) return fail(B2G_ERR_SHAPE, "generator output (%zu) != discriminator input (%zu)", gen->L.back().out_elems, dis->in_elems);
-  if (gen->L.back().out_alias) return fail(B2G_ERR_UNSUPPORTED, "generator must end in a layer that owns its output");
+  if (gen->L.back().out_alias || gen->L.back().d.type == B2G_LAYER_DROPOUT) return fail(B2G_ERR_UNSUPPORTED, "generator must end in a layer that owns its output");
   if (dis->L.back().d.type == B2G_LAYER_OUTPUT && dis->L.back().d.loss != B2G_LOSS_XENT) return fail(B2G_ERR_UNSUPPORTED, "the adversarial step needs a binary XENT discriminator");
   if (dis->cfg.bn_groups < 2 || dis->max_rows < 2) return fail(B2G_ERR_ARG, "discriminator must be created with bn_groups>=2 and max_batch = 2*N");
   int N = std::min(gen->max_rows, dis->max_rows / 2);
@@ -1118,6 +1154,16 @@ extern "C" int32_t b2g_net_get_iteration(b2g_net* n, int64_t* out) {
 extern "C" int32_t b2g_net_set_iteration(b2g_net* n, int64_t it) {
   if (!n || it < 0 || it > 0x7fffffff) return fail(B2G_ERR_ARG, "bad iteration"); CU(cudaSetDevice(n->ctx->device));
   int v = (int)it; CU(cudaMemcpyAsync(n->step_dev, &v, sizeof(int), cudaMemcpyHostToDevice, n->ctx->stream)); CU(cudaStreamSynchronize(n->ctx->stream)); return 0;
+}
+// The dropout pass counter P lives on the device for the same reason; a checkpoint carries it so that a resumed run draws the masks of an
+// uninterrupted one.
+extern "C" int32_t b2g_net_get_dropout_pass(b2g_net* n, int64_t* out) {
+  if (!n || !out) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
+  unsigned long long v = 0; CU(cudaMemcpyAsync(&v, n->drop_pass, sizeof(v), cudaMemcpyDeviceToHost, n->ctx->stream)); CU(cudaStreamSynchronize(n->ctx->stream)); *out = (int64_t)v; return 0;
+}
+extern "C" int32_t b2g_net_set_dropout_pass(b2g_net* n, int64_t pass) {
+  if (!n || pass < 0) return fail(B2G_ERR_ARG, "bad dropout pass"); CU(cudaSetDevice(n->ctx->device));
+  unsigned long long v = (unsigned long long)pass; CU(cudaMemcpyAsync(n->drop_pass, &v, sizeof(v), cudaMemcpyHostToDevice, n->ctx->stream)); CU(cudaStreamSynchronize(n->ctx->stream)); return 0;
 }
 extern "C" int32_t b2g_net_simt_gemm_calls(b2g_net* n, uint64_t* out) { if (!n || !out) return fail(B2G_ERR_ARG, "null"); *out = n->simt_gemm_calls; return 0; }
 
@@ -1347,6 +1393,48 @@ extern "C" int32_t b2g_test_bn(b2g_ctx* c, int32_t precision, int32_t path, int3
   if (e == cudaSuccess) e = cudaGetLastError();
   release();
   if (e != cudaSuccess) return fail(B2G_ERR_CUDA, "BatchNorm test: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+// One DropoutLayer forward (pass counter `pass`, advanced by the kernel) and backward on rows*h*w*c host tensors in NHWC element order,
+// through the kernels the training step uses.
+extern "C" int32_t b2g_test_dropout(b2g_ctx* c, int32_t precision, uint64_t seed, int32_t layer, int32_t rank, int64_t pass, int32_t rows, int32_t h, int32_t w, int32_t ch,
+                                    float p, const float* x, const float* dy, float* y, float* dx) {
+  if (!c || !x || !dy || !y || !dx) return fail(B2G_ERR_ARG, "null");
+  if (!(p > 0.f && p <= 1.f)) return fail(B2G_ERR_ARG, "dropout retain probability %g outside (0, 1]", (double)p);
+  if (rows < 1 || h < 1 || w < 1 || ch < 1 || layer < 0 || layer > 0xffff || rank < 0 || rank > 0xffff || pass < 0) return fail(B2G_ERR_ARG, "bad dropout test arguments");
+  const size_t n = (size_t)rows * h * w * ch;
+  if (n > 0x7fffffff) return fail(B2G_ERR_UNSUPPORTED, "the dropout test hook takes at most 2^31 - 1 elements (%zu)", n);
+  const int prec = precision == B2G_PREC_BF16 ? PREC_BF16 : PREC_F32; const size_t ts = prec_size(prec);
+  CU(cudaSetDevice(c->device)); cudaStream_t s = c->stream;
+  std::vector<void*> mem;
+  auto alloc = [&](void** q, size_t bytes) -> int32_t { *q = nullptr; CU(cudaMalloc(q, bytes)); mem.push_back(*q); return 0; };
+  auto release = [&]() { for (void* q : mem) cudaFree(q); mem.clear(); };
+  float *fx, *fe; void *tx, *te, *ty; uint32_t* mask; unsigned long long* dpass; unsigned* ticket; int32_t r = 0;
+  if ((r = alloc((void**)&fx, 4 * n)) || (r = alloc((void**)&fe, 4 * n)) || (r = alloc(&tx, ts * n)) || (r = alloc(&te, ts * n)) || (r = alloc(&ty, ts * n)) ||
+      (r = alloc((void**)&mask, 4 * ((n + 31) / 32))) || (r = alloc((void**)&dpass, sizeof(unsigned long long))) || (r = alloc((void**)&ticket, sizeof(unsigned)))) { release(); return r; }
+  const unsigned long long p0 = (unsigned long long)pass;
+  cudaError_t e = cudaMemcpyAsync(fx, x, 4 * n, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(fe, dy, 4 * n, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(dpass, &p0, sizeof(p0), cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = cudaMemsetAsync(ticket, 0, sizeof(unsigned), s);
+  if (e != cudaSuccess) { release(); return fail(B2G_ERR_CUDA, "dropout test upload: %s", cudaGetErrorString(e)); }
+  if (prec == PREC_BF16) { k_cast_f32_to_bf16(fx, (__nv_bfloat16*)tx, n, s); k_cast_f32_to_bf16(fe, (__nv_bfloat16*)te, n, s); }
+  else { cudaMemcpyAsync(tx, fx, 4 * n, cudaMemcpyDeviceToDevice, s); cudaMemcpyAsync(te, fe, 4 * n, cudaMemcpyDeviceToDevice, s); }
+  const DropoutArgs a = make_dropout_args(seed, layer, rank, p);
+  k_dropout_fwd(prec, tx, ty, mask, n, a, dpass, ticket, 1, s);
+  k_dropout_bwd(prec, te, te, mask, n, a.scale, s);
+  unsigned long long p1 = 0;
+  k_nhwc_to_nchw_f32(prec, ty, fx, 1, 1, (int)n, s);
+  k_nhwc_to_nchw_f32(prec, te, fe, 1, 1, (int)n, s);
+  e = cudaMemcpyAsync(y, fx, 4 * n, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(dx, fe, 4 * n, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&p1, dpass, sizeof(p1), cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  if (e == cudaSuccess) e = cudaGetLastError();
+  release();
+  if (e != cudaSuccess) return fail(B2G_ERR_CUDA, "dropout test: %s", cudaGetErrorString(e));
+  if (p1 != p0 + 1) return fail(B2G_ERR_CUDA, "dropout test: the forward left the pass counter at %llu, expected %llu", p1, p0 + 1);
   return 0;
 }
 

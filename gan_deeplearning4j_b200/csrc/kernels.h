@@ -81,6 +81,16 @@ void k_maxpool_bwd(int prec, const void* eps_out, const uint8_t* argmax, void* e
 void k_upsample_fwd(int prec, const void* x, void* y, int N, int H, int W, int C, int f, cudaStream_t s);
 void k_upsample_bwd(int prec, const void* eps_out, void* eps_in, int N, int H, int W, int C, int f, cudaStream_t s);
 
+// ---- dropout (DL4J DropoutLayer, inverted dropout; mask definition in include/b200gan.h) ----------------------------------------
+// Forward over the n elements of one pass (NHWC, element index e): y = x * (1/p) where kept, 0 where dropped, and the keep bits into
+// mask[e >> 5] bit (e & 31).  The random word of element e is Philox4x32-10(ctr = {e >> 2, lo32(P), hi32(P), tag}, key = {lo32(seed), hi32(seed)})[e & 3],
+// P = *pass read on the device.  bump_pass: the last block to finish advances *pass by one (ticket counter *ticket, reset by that block).
+// tag = layer | rank << 16; keep where the word < threshold = floor(p * 2^32), or everywhere when keep_all (p >= 1); scale = 1.0f / p
+struct DropoutArgs { uint64_t seed; uint32_t tag; uint32_t threshold; float scale; int keep_all; };
+void k_dropout_fwd(int prec, const void* x, void* y, uint32_t* mask, size_t n, const DropoutArgs& a, unsigned long long* pass, unsigned* ticket, int bump_pass, cudaStream_t s);
+// Backward: eps_in = eps_out * (1/p) where the forward kept the element, 0 elsewhere (eps_in may equal eps_out)
+void k_dropout_bwd(int prec, const void* eps_out, void* eps_in, const uint32_t* mask, size_t n, float scale, cudaStream_t s);
+
 // ---- loss ----------------------------------------------------------------------------------------------
 // LossBinaryXENT on logits z[rows] with labels y[rows]: dz = dL/dz (sum form, not /mb), loss_sums[g] = sum of losses per group.
 void k_xent(int prec, const void* z, const float* y, void* dz, float* loss_sums, int rows_per_group, int groups, float clip_eps, cudaStream_t s);

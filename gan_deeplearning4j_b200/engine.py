@@ -15,7 +15,7 @@ from . import _lib
 from ._lib import GanConfig, LayerDesc, NetConfig, check
 
 LAYER_TYPES = {"conv2d": 0, "deconv2d": 1, "batchnorm": 2, "dense": 3, "activation": 4, "maxpool": 5, "upsample2d": 6,
-               "output": 7, "loss": 8, "ff_to_cnn": 9, "cnn_to_ff": 10}
+               "output": 7, "loss": 8, "ff_to_cnn": 9, "cnn_to_ff": 10, "dropout": 11}
 ACTS = {"identity": 0, "tanh": 1, "sigmoid": 2, "relu": 3, "lrelu": 4}
 UPDATERS = {"sgd": 0, "rmsprop": 1, "adam": 2, "noop": 3}
 FP32, BF16 = 0, 1
@@ -41,6 +41,8 @@ def layer_desc(spec: Dict) -> LayerDesc:
     d.has_bias = 1 if spec.get("has_bias", True) else 0
     d.act = ACTS[spec.get("activation", "identity")]
     d.act_alpha = spec.get("alpha", 0.01)
+    if spec["type"] == "dropout":       # DropoutLayer.Builder(p): p = retain probability, carried in act_alpha
+        d.act_alpha = spec["p"]
     u = spec.get("updater") or {"kind": "sgd", "lr": 0.0}
     d.updater = UPDATERS[u["kind"]]
     d.lr = u.get("lr", 0.0)
@@ -173,7 +175,8 @@ class Net:
     def save(self, path, save_updater: bool = True):
         from . import serializer
         serializer.save_net(self, path, self.specs, self.input_shape, save_updater,
-                            {"precision": "bf16" if self.precision == BF16 else "fp32", "max_batch": self.max_batch, "iteration": self.iteration()})
+                            {"precision": "bf16" if self.precision == BF16 else "fp32", "max_batch": self.max_batch, "iteration": self.iteration(),
+                             "dropout_pass": self.dropout_pass()})
 
     def restore(self, path, load_updater: bool = True):
         """Loads parameters (and updater state) of a checkpoint written by save() into this net (same architecture)."""
@@ -239,6 +242,15 @@ class Net:
 
     def set_iteration(self, it: int):
         check(self.lib.b2g_net_set_iteration(self.h, int(it)))
+
+    def dropout_pass(self) -> int:
+        """The dropout pass counter P: train-mode forwards that applied a DropoutLayer mask; part of a checkpoint."""
+        v = C.c_int64()
+        check(self.lib.b2g_net_get_dropout_pass(self.h, C.byref(v)))
+        return v.value
+
+    def set_dropout_pass(self, p: int):
+        check(self.lib.b2g_net_set_dropout_pass(self.h, int(p)))
 
     def simt_gemm_calls(self) -> int:
         """BF16 nets: GEMM-shaped operations that ran on the SIMT kernels instead of the tensor-core kernels since creation."""
@@ -366,3 +378,14 @@ def test_bn(ctx: Context, precision: int, path: int, x, eps_out, gamma, beta, ru
     check(ctx.lib.b2g_test_bn(ctx.h, precision, path, groups, rows, ch, _fp(x), _fp(e), *[_fp(v) for v in par], ACTS[act], alpha, eps, decay,
                               int(want_param_grads), *[_fp(r[k]) for k in ("y", "eps_in", "g_gamma", "g_beta", "g_mean", "g_var", "mean", "invstd")]))
     return r
+
+
+def test_dropout(ctx: Context, precision: int, x, dy, p: float, *, seed: int = 666, layer: int = 0, rank: int = 0, pass_: int = 0):
+    """One DropoutLayer forward and backward through the training-step kernels (b2g_test_dropout).  x, dy: [rows, H, W, C] in the engine's NHWC
+    order (or [rows, F]).  Returns (y, dx) in the same shape."""
+    x, e = _f32(x), _f32(dy)
+    rows = x.shape[0]
+    h, w, c = (x.shape[1:] if x.ndim == 4 else (1, 1, int(np.prod(x.shape[1:]))))
+    y, dx = np.empty_like(x), np.empty_like(x)
+    check(ctx.lib.b2g_test_dropout(ctx.h, precision, seed, layer, rank, pass_, rows, h, w, c, p, _fp(x), _fp(e), _fp(y), _fp(dx)))
+    return y, dx

@@ -107,11 +107,15 @@ def mlp_generator(z=100, hidden=1024, d=256, lr=2e-4, beta1=0.5) -> List[Dict]:
             {"type": "dense", "name": "gen_dense_3", "n_out": d, "activation": "tanh", "updater": u()}]
 
 
-def mlp_discriminator(d=256, hidden=1024, lr=2e-4, beta1=0.5) -> List[Dict]:
+def mlp_discriminator(d=256, hidden=1024, lr=2e-4, beta1=0.5, dropout=None) -> List[Dict]:
+    """dropout = p: a DropoutLayer(p) (p = retain probability) after each hidden LeakyReLU, the DL4J MNIST GAN example's discriminator shape."""
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
-    return [{"type": "dense", "name": "dis_dense_1", "n_out": hidden, "activation": "lrelu", "alpha": 0.2, "updater": u()},
-            {"type": "dense", "name": "dis_dense_2", "n_out": hidden, "activation": "lrelu", "alpha": 0.2, "updater": u()},
-            {"type": "output", "name": "dis_output", "n_out": 1, "updater": u()}]
+    L = []
+    for i in (1, 2):
+        L.append({"type": "dense", "name": f"dis_dense_{i}", "n_out": hidden, "activation": "lrelu", "alpha": 0.2, "updater": u()})
+        if dropout is not None:
+            L.append({"type": "dropout", "name": f"dis_dropout_{i}", "p": dropout})
+    return L + [{"type": "output", "name": "dis_output", "n_out": 1, "updater": u()}]
 
 
 # algorithmic MACs per image of the conv/deconv/dense layers (SURVEY.md 8d: F = 2*(4*G_f + 8*D_f))

@@ -11,7 +11,7 @@ and `updaterState.bin` = `Nd4j.write(updater state view)`.  This module writes t
                      parameter order -- NOT DL4J's per-UpdaterBlock interleaving; a DL4J reader must regroup it
   configuration.json this library's layer specification (the arguments of b2g_net_create), NOT DL4J's Jackson schema: a Java user rebuilds the
                      graph with the same builder calls (the driver's own code, J:118-310) and loads the arrays
-  b200gan.json       precision, input shape, iteration counter
+  b200gan.json       precision, input shape, iteration counter, dropout pass counter
 
 `read_model` reads the container back (and accepts legacy int-length headers), so the library can resume training -- the reference can only save.
 """
@@ -99,4 +99,7 @@ def restore_into(net, path, load_updater: bool = True) -> Dict:
         # Adam's bias correction depends on the iteration count: warm moments with t = 1 would diverge from an uninterrupted run
         if "iteration" in m["meta"] and hasattr(net, "set_iteration"):
             net.set_iteration(int(m["meta"]["iteration"]))
+    # the DropoutLayer pass counter: a resumed run draws the masks an uninterrupted one would have drawn
+    if "dropout_pass" in m["meta"] and hasattr(net, "set_dropout_pass"):
+        net.set_dropout_pass(int(m["meta"]["dropout_pass"]))
     return m

@@ -62,8 +62,23 @@ typedef enum {
   B2G_LAYER_OUTPUT = 7,      /* OutputLayer.Builder(LossFunction.XENT).activation(SIGMOID).nOut() J:159-163,303-308 */
   B2G_LAYER_LOSS = 8,        /* LossLayer(XENT, sigmoid): loss on incoming logits (DCGAN D-last conv)              */
   B2G_LAYER_FF_TO_CNN = 9,   /* FeedForwardToCnnPreProcessor(h,w,c)                               J:200,255         */
-  B2G_LAYER_CNN_TO_FF = 10   /* CnnToFeedForwardPreProcessor (auto-inserted by setInputTypes, SURVEY.md 3.1)       */
+  B2G_LAYER_CNN_TO_FF = 10,  /* CnnToFeedForwardPreProcessor (auto-inserted by setInputTypes, SURVEY.md 3.1)       */
+  B2G_LAYER_DROPOUT = 11     /* DropoutLayer.Builder(p): p = RETAIN probability in (0, 1], carried in act_alpha; no parameters */
 } b2g_layer_type;
+
+/* DropoutLayer (inverted dropout, DL4J 1.0.0-beta3).  Train-mode forward y = x * m, m = 1/p (fp32 1.0f / p) with probability p, else 0;
+ * y = x * (1/p) is formed in fp32 and rounded once to the activation type, dropped elements are +0.  Backward dx = dy * m with the forward's
+ * mask (kept as one bit per element).  Inference (train = 0) and a frozen DropoutLayer (FrozenLayer = test mode) are the identity, launch
+ * nothing and b2g_net_get_activation returns the layer's input.
+ * The mask is a pure function of (S, r, L, P, e), so the same on every run and in both precisions:
+ *   S = b2g_net_config.seed (0 -> 666), r = the context's rank (0 without a communicator), L = the layer's index in the b2g_layer_desc array,
+ *   P = the net's dropout pass counter, e = ((row*H + h)*W + w)*C + c the element's NHWC index in the pass (row = position in the pass batch);
+ *   (x0,x1,x2,x3) = Philox4x32-10(ctr = {e >> 2, lo32(P), hi32(P), L | (r << 16)}, key = {lo32(S), hi32(S)})
+ *   keep(e) = p >= 1  ||  x[e & 3] < (uint32)floor(p * 2^32)
+ * P is a 64-bit word in device memory, 0 at b2g_net_create.  Every train-mode forward of a net with at least one masking DropoutLayer
+ * (train, not frozen, p < 1) uses the current P for all of them and then advances P by 1 on the device (so a replayed CUDA graph draws new
+ * masks); other forwards leave it unchanged.  In the GAN step D's real|fake pass (2N rows) uses P and the generator step's D pass P + 1.
+ * A pass may hold at most 2^34 elements (max_batch * layer size; B2G_ERR_UNSUPPORTED at b2g_net_create). */
 
 typedef enum {               /* org.nd4j.linalg.activations.Activation  J:126,162,215 */
   B2G_ACT_IDENTITY = 0, B2G_ACT_TANH = 1, B2G_ACT_SIGMOID = 2, B2G_ACT_RELU = 3, B2G_ACT_LRELU = 4
@@ -84,7 +99,7 @@ typedef struct {
   int32_t k_h, k_w, s_h, s_w, p_h, p_w;   /* conv / deconv / pool geometry; upsample factor in k_h */
   int32_t has_bias;             /* hasBias(true) default */
   int32_t act;                  /* b2g_activation */
-  float act_alpha;              /* ActivationLReLU alpha: DL4J default 0.01, DCGAN passes 0.2 */
+  float act_alpha;              /* ActivationLReLU alpha: DL4J default 0.01, DCGAN passes 0.2; DropoutLayer retain probability p */
   int32_t updater;              /* b2g_updater; "frozen" in the reference = RMSPROP with lr 0 (J:84) */
   float lr, beta1, beta2, eps;  /* RmsProp: beta1 = rmsDecay (ctor order lr, rmsDecay, epsilon; J:133 passes 1e-8, 1e-8) */
   float l2;                     /* .l2(1e-4) (J:125): weights only, applied AFTER the updater, not lr-scaled */
@@ -158,6 +173,10 @@ int32_t b2g_net_fit(b2g_net* net, const float* x, const float* y, int32_t batch,
  * configuration.json ("iterationCount"); a restore that drops it restarts Adam's bias correction with warm moments (J:606-618). */
 int32_t b2g_net_get_iteration(b2g_net* net, int64_t* out);
 int32_t b2g_net_set_iteration(b2g_net* net, int64_t iteration);
+/* The dropout pass counter P (see B2G_LAYER_DROPOUT); a checkpoint carries it so that a resumed run draws the masks of an uninterrupted one.
+ * Both are sync points, like get_iteration. */
+int32_t b2g_net_get_dropout_pass(b2g_net* net, int64_t* out);
+int32_t b2g_net_set_dropout_pass(b2g_net* net, int64_t pass);
 /* BF16 nets: how many GEMM-shaped operations ran on the SIMT kernels instead of the tensor-core kernels since creation (skinny layers by design, or a
  * shape the tensor-core kernels do not tile).  north_star: no silent fallback -- bench.py prints it per step. */
 int32_t b2g_net_simt_gemm_calls(b2g_net* net, uint64_t* out);
@@ -262,6 +281,11 @@ int32_t b2g_test_bn(b2g_ctx* ctx, int32_t precision, int32_t path, int32_t group
  * which = 0: the straight copy of W in the internal [A][taps][B] order; 1: the packed [(py,px,c)][(dyr,dxc)][O] operand of the
  * pixel-shuffle transposed conv onto <= 4 channels (B2G_ERR_UNSUPPORTED if the layer has none). */
 int32_t b2g_test_net_shadow(b2g_net* net, int32_t layer, int32_t which, float* out, int64_t n);
+/* One DropoutLayer forward and backward on host tensors x, dy of rows*h*w*c elements in NHWC element order (fp32; rounded to bf16 on the
+ * device when precision is BF16), through the kernels of the training step, with the mask of (seed, layer, rank, pass) as defined at
+ * B2G_LAYER_DROPOUT.  Out: y, dx (same order).  Fails unless the forward advanced its pass counter from pass to pass + 1. */
+int32_t b2g_test_dropout(b2g_ctx* ctx, int32_t precision, uint64_t seed, int32_t layer, int32_t rank, int64_t pass, int32_t rows, int32_t h, int32_t w,
+                         int32_t c, float p, const float* x, const float* dy, float* y, float* dx);
 
 #ifdef __cplusplus
 }

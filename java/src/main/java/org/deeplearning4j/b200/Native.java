@@ -28,6 +28,8 @@ public final class Native {
     public static native int netSetUpdaterState(long net, long hostAddr, long n);
     public static native int netGetIteration(long net, long outAddr);
     public static native int netSetIteration(long net, long iteration);
+    public static native int netGetDropoutPass(long net, long outAddr);
+    public static native int netSetDropoutPass(long net, long pass);
     public static native int netSimtGemmCalls(long net, long outAddr);
     public static native int netSetSyncBn(long net, int enabled);
     public static native int netSetGradPayloadBf16(long net, int enabled);

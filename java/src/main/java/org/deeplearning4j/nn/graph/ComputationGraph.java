@@ -52,6 +52,9 @@ public class ComputationGraph {
     /** BaseMultiLayerUpdater's iteration count (Adam's t - 1); part of a checkpoint and of the state a Spark worker starts from. */
     public long getIterationCount() { ByteBuffer o = Native.direct(8); Native.check(Native.netGetIteration(net, Native.address(o))); return o.getLong(0); }
     public void setIterationCount(long it) { Native.check(Native.netSetIteration(net, it)); }
+    /** The DropoutLayer pass counter (one per train-mode forward that masks); save it with the parameters to resume the same mask sequence. */
+    public long getDropoutPass() { ByteBuffer o = Native.direct(8); Native.check(Native.netGetDropoutPass(net, Native.address(o))); return o.getLong(0); }
+    public void setDropoutPass(long pass) { Native.check(Native.netSetDropoutPass(net, pass)); }
     public String configurationJson() {
         StringBuilder s = new StringBuilder("{\"format\": \"b200gan layer specs\", \"layers\": [");
         for (int i = 0; i < layers.size(); ++i) { Layer l = layers.get(i); s.append(i == 0 ? "" : ", ").append("{\"name\": \"").append(l.name).append("\", \"type\": ").append(l.type).append(", \"nIn\": ").append(l.nIn).append(", \"nOut\": ").append(l.nOut).append("}"); }

@@ -42,6 +42,8 @@ FN(netGetUpdaterState)(JNIEnv_*, jclass, jlong net, jlong hostAddr, jlong n) { r
 FN(netSetUpdaterState)(JNIEnv_*, jclass, jlong net, jlong hostAddr, jlong n) { return b2g_net_set_updater_state(P(b2g_net*, net), P(const float*, hostAddr), n); }
 FN(netGetIteration)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_get_iteration(P(b2g_net*, net), P(int64_t*, outAddr)); }
 FN(netSetIteration)(JNIEnv_*, jclass, jlong net, jlong it) { return b2g_net_set_iteration(P(b2g_net*, net), it); }
+FN(netGetDropoutPass)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_get_dropout_pass(P(b2g_net*, net), P(int64_t*, outAddr)); }
+FN(netSetDropoutPass)(JNIEnv_*, jclass, jlong net, jlong pass) { return b2g_net_set_dropout_pass(P(b2g_net*, net), pass); }
 FN(netSimtGemmCalls)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_simt_gemm_calls(P(b2g_net*, net), P(uint64_t*, outAddr)); }
 FN(netSetSyncBn)(JNIEnv_*, jclass, jlong net, jint enabled) { return b2g_net_set_sync_bn(P(b2g_net*, net), enabled); }
 FN(netSetGradPayloadBf16)(JNIEnv_*, jclass, jlong net, jint enabled) { return b2g_net_set_grad_payload_bf16(P(b2g_net*, net), enabled); }
