@@ -83,6 +83,7 @@ PROTOTYPES = {
     "b2g_net_set_iteration": (_i32, [_vp, _i64]),
     "b2g_net_get_dropout_pass": (_i32, [_vp, C.POINTER(_i64)]),
     "b2g_net_set_dropout_pass": (_i32, [_vp, _i64]),
+    "b2g_net_set_gradient_normalization": (_i32, [_vp, _i32, C.c_float]),
     "b2g_net_simt_gemm_calls": (_i32, [_vp, C.POINTER(C.c_uint64)]),
     "b2g_gan_create": (_i32, [_vp, _vp, C.POINTER(GanConfig), _pvp]),
     "b2g_gan_destroy": (_i32, [_vp]),

@@ -127,6 +127,12 @@ struct b2g_net {
   unsigned* upd_ticket = nullptr;                                  // block-completion counter of the updater kernel (the last block bumps step_dev)
   unsigned long long* drop_pass = nullptr;                         // dropout pass counter P (device): read by every dropout kernel of a train-mode pass
   unsigned* drop_ticket = nullptr;                                 // block-completion counter of the pass's last dropout kernel (its last block bumps P)
+  // L2 gradient normalization (b2g_net_set_gradient_normalization): mode, threshold and a generation bumped on every change (a captured GAN
+  // step holds the mode's launches, so it is re-captured when the generation differs); norm groups per layer and per segment; the norm
+  // kernel's per-chunk partial sums, block-completion counter and per-segment multipliers
+  int gn_mode = B2G_GN_NONE; float gn_threshold = 1.0f; uint64_t gn_gen = 0;
+  GnGroup *gn_layer_groups = nullptr, *gn_param_groups = nullptr; int gn_n_layer_groups = 0, gn_n_param_groups = 0;
+  double* gn_partial = nullptr; unsigned* gn_ticket = nullptr; float* gn_mult = nullptr;
   ReduceList pending{};                                            // split-K partial sums queued by this backward pass
   uint64_t simt_gemm_calls = 0;                                    // BF16 nets: GEMM-shaped ops that ran on the SIMT kernels (skinny / unsupported shapes) -- reported, never silent
   float* scratch = nullptr; size_t scratch_floats = 0;
@@ -332,13 +338,14 @@ static int32_t net_init_params_and_updater(b2g_net* n) {
   std::vector<float> hp(n->n_params, 0.f), h0(n->n_params, 0.f);
   uint64_t seed = n->cfg.seed ? n->cfg.seed : 666;
   std::vector<int64_t> l2o, l2l; std::vector<float> l2c;
+  std::vector<int> seg_layer;      // layer index of every segment (the norm groups of the PerLayer modes)
   for (auto& l : n->L) {
     const b2g_layer_desc& d = l.d;
     auto add_seg = [&](int64_t off, int64_t len, bool weight, bool noop) {
       if (d.frozen) return;      // FrozenLayer: no update, no l2 decay, no l2 score (calcL2() == 0)
       UpdSeg sg{}; sg.off = off; sg.len = len; sg.kind = noop ? 3 : updater_kind(d.updater);
       sg.lr = d.lr; sg.b1 = d.beta1; sg.b2 = d.beta2; sg.eps = d.eps; sg.l2 = weight ? d.l2 : 0.f; sg.clip = n->cfg.grad_clip; sg.div_mb = noop ? 0 : 1;
-      sg.off_bf = (weight && l.off_W_bf >= 0) ? l.off_W_bf : -1; sg.off_ps = (weight && l.off_Wps_bf >= 0) ? l.off_Wps_bf : -1; sg.ps_O = l.geom.O; sg.ps_C = l.geom.C; n->segs.push_back(sg);
+      sg.off_bf = (weight && l.off_W_bf >= 0) ? l.off_W_bf : -1; sg.off_ps = (weight && l.off_Wps_bf >= 0) ? l.off_Wps_bf : -1; sg.ps_O = l.geom.O; sg.ps_C = l.geom.C; n->segs.push_back(sg); seg_layer.push_back((int)(&l - n->L.data()));
       if (!noop && sg.kind == 1) for (int64_t i = 0; i < len; ++i) h0[off + i] = d.eps;     // RmsPropUpdater cache initialised to epsilon
       if (weight && d.l2 != 0.f) { l2o.push_back(off); l2l.push_back(len); l2c.push_back(0.5f * d.l2); }
     };
@@ -367,6 +374,23 @@ static int32_t net_init_params_and_updater(b2g_net* n) {
   CU(cudaMemcpyAsync(n->segs_dev, n->segs.data(), sizeof(UpdSeg) * n->segs.size(), cudaMemcpyHostToDevice, s));
   CU(cudaMemcpyAsync(n->chunk_seg_dev, cs.data(), sizeof(int32_t) * cs.size(), cudaMemcpyHostToDevice, s));
   CU(cudaMemcpyAsync(n->chunk_off_dev, co.data(), sizeof(int64_t) * co.size(), cudaMemcpyHostToDevice, s));
+  {  // L2 gradient normalization: norm groups over the chunk map (chunks follow segment order, segments follow layer order), partial sums, multipliers
+    const int ns = (int)n->segs.size();
+    std::vector<int32_t> seg_c0(ns + 1, n->nchunks);
+    for (int c = n->nchunks - 1; c >= 0; --c) seg_c0[cs[c]] = c;
+    std::vector<GnGroup> per_layer, per_param;
+    for (int i = 0; i < ns; ++i) {
+      per_param.push_back(GnGroup{seg_c0[i], seg_c0[i + 1], i, i + 1});
+      if (i > 0 && seg_layer[i] == seg_layer[i - 1]) { per_layer.back().chunk_end = seg_c0[i + 1]; per_layer.back().seg_end = i + 1; }
+      else per_layer.push_back(GnGroup{seg_c0[i], seg_c0[i + 1], i, i + 1});
+    }
+    n->gn_n_layer_groups = (int)per_layer.size(); n->gn_n_param_groups = (int)per_param.size();
+    B2(dalloc(n, &n->gn_layer_groups, sizeof(GnGroup) * std::max<size_t>(1, per_layer.size()))); B2(dalloc(n, &n->gn_param_groups, sizeof(GnGroup) * std::max<size_t>(1, per_param.size())));
+    B2(dalloc(n, &n->gn_partial, sizeof(double) * std::max(1, n->nchunks))); B2(dalloc(n, &n->gn_mult, sizeof(float) * std::max(1, ns)));
+    B2(dalloc(n, &n->gn_ticket, sizeof(unsigned))); CU(cudaMemsetAsync(n->gn_ticket, 0, sizeof(unsigned), s));
+    CU(cudaMemcpyAsync(n->gn_layer_groups, per_layer.data(), sizeof(GnGroup) * per_layer.size(), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(n->gn_param_groups, per_param.data(), sizeof(GnGroup) * per_param.size(), cudaMemcpyHostToDevice, s));
+  }
   n->n_l2 = (int)l2o.size();
   if (n->n_l2) {
     B2(dalloc(n, &n->l2_off_dev, sizeof(int64_t) * n->n_l2)); B2(dalloc(n, &n->l2_len_dev, sizeof(int64_t) * n->n_l2)); B2(dalloc(n, &n->l2_coef_dev, sizeof(float) * n->n_l2));
@@ -728,8 +752,18 @@ static int32_t net_update(b2g_net* n, int mb_local) {
   cudaStream_t s = n->ctx->stream; int W = n->ctx->comm ? n->ctx->world : 1;
   // BN running-stat pseudo-gradients are exempt from the minibatch division; under DP they are averaged over ranks
   if (!n->grad_allreduce) W = 1;     // parameter-averaging mode: purely local update
-  // one pass: /mb -> clip -> updater -> +l2*W -> theta -= g, the bf16 operand copies (straight and packed) and the iteration counter
-  k_updater(n->params, n->grads, n->st0, n->st1, n->segs_dev, n->chunk_seg_dev, n->chunk_off_dev, n->nchunks, 1.0f / ((float)mb_local * W), 1.0f / (float)W, n->step_dev, n->upd_ticket, n->shadow, s);
+  const float inv_mb = 1.0f / ((float)mb_local * W), inv_world = 1.0f / (float)W;
+  // L2 gradient normalization: one kernel takes the norms of the (all-reduced) gradient after /mb and leaves one multiplier per segment
+  const bool gn = n->gn_mode != B2G_GN_NONE;
+  if (gn) {
+    const bool per_layer = n->gn_mode == B2G_GN_RENORM_L2_LAYER || n->gn_mode == B2G_GN_CLIP_L2_LAYER;
+    const bool clip = n->gn_mode == B2G_GN_CLIP_L2_LAYER || n->gn_mode == B2G_GN_CLIP_L2_PARAM;
+    k_gradnorm(n->grads, n->segs_dev, n->chunk_seg_dev, n->chunk_off_dev, n->nchunks, per_layer ? n->gn_layer_groups : n->gn_param_groups,
+               per_layer ? n->gn_n_layer_groups : n->gn_n_param_groups, clip ? 1 : 0, n->gn_threshold, inv_mb, inv_world, n->gn_partial, n->gn_ticket, n->gn_mult, s);
+  }
+  // one pass: /mb -> [x multiplier] -> clip -> updater -> +l2*W -> theta -= g, the bf16 operand copies (straight and packed) and the iteration counter
+  k_updater(n->params, n->grads, n->st0, n->st1, n->segs_dev, n->chunk_seg_dev, n->chunk_off_dev, n->nchunks, inv_mb, inv_world, n->step_dev, n->upd_ticket, n->shadow,
+            gn ? n->gn_mult : nullptr, s);
   CHECK_KERNELS();
   return 0;
 }
@@ -959,6 +993,7 @@ struct b2g_gan {
   float* loss_dev = nullptr;              // [4]: d_real_sum, d_fake_sum, g_sum
   float* stage = nullptr; size_t stage_floats = 0;
   cudaGraph_t graph = nullptr, graph1 = nullptr; cudaGraphExec_t exec = nullptr, exec1 = nullptr; int graph_batch = 0; uint64_t graph_launches = 0, graph_simt_g = 0, graph_simt_d = 0;
+  uint64_t graph_gn_g = 0, graph_gn_d = 0;   // the nets' gradient-normalization generations the captured graph was made with
   cudaEvent_t ev0 = nullptr, ev1 = nullptr; float last_ms = 0.f; int last_batch = 1; bool nccl_warm = false;
   cudaStream_t copy_stream = nullptr; cudaEvent_t ev_x = nullptr; bool ev1_valid = false;   // x_real's H2D runs under the generator's forward
   std::vector<void*> allocs;
@@ -1105,7 +1140,7 @@ extern "C" int32_t b2g_gan_step_resident(b2g_gan* g, int32_t batch) {
   CU(cudaEventRecord(g->ev0, s));
   if (!use_graph) { B2(gan_step_part1(g, batch)); CU(cudaStreamWaitEvent(s, g->ev_x, 0)); B2(gan_step_part2(g, batch)); phase_report(s); }
   else {
-    if (!g->exec || g->graph_batch != batch) {
+    if (!g->exec || g->graph_batch != batch || g->graph_gn_g != g->G->gn_gen || g->graph_gn_d != g->D->gn_gen) {
       if (g->exec) { cudaGraphExecDestroy(g->exec); g->exec = nullptr; } if (g->graph) { cudaGraphDestroy(g->graph); g->graph = nullptr; }
       if (g->exec1) { cudaGraphExecDestroy(g->exec1); g->exec1 = nullptr; } if (g->graph1) { cudaGraphDestroy(g->graph1); g->graph1 = nullptr; }
       uint64_t before = g_launch_count; const uint64_t sg0 = g->G->simt_gemm_calls, sd0 = g->D->simt_gemm_calls;
@@ -1120,6 +1155,7 @@ extern "C" int32_t b2g_gan_step_resident(b2g_gan* g, int32_t batch) {
       g->graph_simt_g = g->G->simt_gemm_calls - sg0; g->graph_simt_d = g->D->simt_gemm_calls - sd0; g->G->simt_gemm_calls = sg0; g->D->simt_gemm_calls = sd0;
       if (r) return r; if (e != cudaSuccess) return fail(B2G_ERR_CUDA, "graph capture: %s", cudaGetErrorString(e));
       CU(cudaGraphInstantiate(&g->exec1, g->graph1, 0)); CU(cudaGraphInstantiate(&g->exec, g->graph, 0)); g->graph_batch = batch;
+      g->graph_gn_g = g->G->gn_gen; g->graph_gn_d = g->D->gn_gen;
     }
     CU(cudaGraphLaunch(g->exec1, s));
     CU(cudaStreamWaitEvent(s, g->ev_x, 0));
@@ -1164,6 +1200,19 @@ extern "C" int32_t b2g_net_get_dropout_pass(b2g_net* n, int64_t* out) {
 extern "C" int32_t b2g_net_set_dropout_pass(b2g_net* n, int64_t pass) {
   if (!n || pass < 0) return fail(B2G_ERR_ARG, "bad dropout pass"); CU(cudaSetDevice(n->ctx->device));
   unsigned long long v = (unsigned long long)pass; CU(cudaMemcpyAsync(n->drop_pass, &v, sizeof(v), cudaMemcpyHostToDevice, n->ctx->stream)); CU(cudaStreamSynchronize(n->ctx->stream)); return 0;
+}
+extern "C" int32_t b2g_net_set_gradient_normalization(b2g_net* n, int32_t mode, float threshold) {
+  if (!n) return fail(B2G_ERR_ARG, "null");
+  if (mode == B2G_GN_CLIP_ELEMENTWISE) return fail(B2G_ERR_ARG, "ClipElementWiseAbsoluteValue is b2g_net_config.grad_clip, set when the net is created");
+  if (mode != B2G_GN_NONE && mode != B2G_GN_RENORM_L2_LAYER && mode != B2G_GN_RENORM_L2_PARAM && mode != B2G_GN_CLIP_L2_LAYER && mode != B2G_GN_CLIP_L2_PARAM)
+    return fail(B2G_ERR_ARG, "unknown gradient normalization %d", mode);
+  if (mode != B2G_GN_NONE && n->cfg.grad_clip > 0.f)
+    return fail(B2G_ERR_ARG, "the net was created with grad_clip %g (ClipElementWiseAbsoluteValue): one gradient normalization per layer", (double)n->cfg.grad_clip);
+  const bool clip = mode == B2G_GN_CLIP_L2_LAYER || mode == B2G_GN_CLIP_L2_PARAM;
+  if (clip && !(threshold > 0.f && isfinite(threshold))) return fail(B2G_ERR_ARG, "gradient normalization threshold %g: the clip modes need a finite threshold > 0", (double)threshold);
+  if (!clip) threshold = 1.0f;      // the renormalize modes ignore it
+  if (mode != n->gn_mode || threshold != n->gn_threshold) { n->gn_mode = mode; n->gn_threshold = threshold; ++n->gn_gen; }
+  return 0;
 }
 extern "C" int32_t b2g_net_simt_gemm_calls(b2g_net* n, uint64_t* out) { if (!n || !out) return fail(B2G_ERR_ARG, "null"); *out = n->simt_gemm_calls; return 0; }
 
@@ -1473,7 +1522,7 @@ extern "C" int32_t b2g_test_hbm_kernels(b2g_net* n, int32_t rows, int32_t channe
   for (int which = 0; which < 3; ++which) for (int it = -1; it < iters; ++it) {
     B2(b2g_flush_l2(c));
     CU(cudaEventRecord(e0, s));
-    if (which == 0) k_updater(n->params, n->grads, n->st0, n->st1, n->segs_dev, n->chunk_seg_dev, n->chunk_off_dev, n->nchunks, 1.0f, 1.0f, n->step_dev, n->upd_ticket, n->shadow, s);
+    if (which == 0) k_updater(n->params, n->grads, n->st0, n->st1, n->segs_dev, n->chunk_seg_dev, n->chunk_off_dev, n->nchunks, 1.0f, 1.0f, n->step_dev, n->upd_ticket, n->shadow, nullptr, s);
     else if (which == 1) k_bn_apply_acc(x, y, rows, channels, 1, acc, gb, gb + channels, ACT_LRELU, 0.2f, 1e-5f, coef, gb + 2 * channels, gb + 3 * channels, nullptr, nullptr, 0.9f, s);
     else k_bn_bwd_apply_acc(x, e, y, rows, channels, 1, coef, ACT_LRELU, 0.2f, 1, acc, gb, gb + channels, 0, s);
     CU(cudaEventRecord(e1, s)); CU(cudaEventSynchronize(e1));

@@ -126,10 +126,24 @@ struct UpdSeg {            // one parameter tensor
   int ps_O, ps_C;
 };
 // The last block to finish bumps *step_dev (Adam's t) and resets *ticket: no separate counter kernel.
+// gn_mult (may be null): one fp32 multiplier per segment (k_gradnorm), applied to g right after the minibatch division.
 void k_updater(float* params, const float* grads, float* st0, float* st1, const UpdSeg* segs_dev, const int32_t* chunk_seg_dev,
                const int64_t* chunk_off_dev, int nchunks, float inv_mb, float inv_world, int* step_dev /* t = *step_dev + 1 */, unsigned* ticket,
-               __nv_bfloat16* shadow, cudaStream_t s);
+               __nv_bfloat16* shadow, const float* gn_mult, cudaStream_t s);
 static const int UPD_CHUNK = 4096;
+
+// ---- L2 gradient normalization (DL4J GradientNormalization.{Renormalize,Clip}L2Per{Layer,ParamType}; kernels_gradnorm.cu) ---------
+// A norm group is a run of updater segments: one layer's segments, or one segment.  Its chunks are [chunk_begin, chunk_end) of the updater's
+// chunk map, its segments [seg_begin, seg_end).
+struct GnGroup { int32_t chunk_begin, chunk_end, seg_begin, seg_end; };
+// One block per updater chunk: partial[c] = sum over the chunk of (double)(g * gscale)^2 (gscale = inv_mb, or inv_world for the BatchNorm
+// running-stat pseudo-gradients, as in the updater).  The last block to finish (ticket counter *ticket, reset by that block) folds the
+// partials of each group in chunk order, norm = sqrt(sum), and writes mult[s] for every segment s of the group, rounded to fp32 once:
+//   clip = 0 (renormalize): 1 / norm, or 1 / 1e-5 when norm == 0;   clip = 1: threshold / norm when norm > threshold, else 1.
+// The result does not depend on the order in which blocks run.
+void k_gradnorm(const float* grads, const UpdSeg* segs_dev, const int32_t* chunk_seg_dev, const int64_t* chunk_off_dev, int nchunks,
+                const GnGroup* groups_dev, int ngroups, int clip, float threshold, float inv_mb, float inv_world, double* partial, unsigned* ticket,
+                float* mult, cudaStream_t s);
 void k_fill_f32(float* p, float v, size_t n, cudaStream_t s);
 void k_scale_f32(float* p, float v, size_t n, cudaStream_t s);
 // Gradient all-reduce over NVLink peer memory (one process per GPU, buffers exchanged as CUDA IPC handles): ONE kernel per GPU does

@@ -947,8 +947,11 @@ void k_reduce_multi(const ReduceList& rl, cudaStream_t s) {
 
 // ---------------------------------------------------------------- updater -------------------------------
 // One pass over params: 28 B/param for Adam (read p,g,m,v; write p,m,v), 20 B/param RmsProp, +2 B bf16 shadow.
-__device__ __forceinline__ float upd_elem(const UpdSeg& sg, float g, float p, float& s0, float& s1, float gscale, float alpha_t) {
+// SCALED: the L2 gradient normalization multiplier of the segment (kernels_gradnorm.cu) follows the minibatch division
+template <bool SCALED>
+__device__ __forceinline__ float upd_elem(const UpdSeg& sg, float g, float p, float& s0, float& s1, float gscale, float alpha_t, float gmult) {
   g *= gscale;
+  if (SCALED) g *= gmult;
   if (sg.clip > 0.f) g = fminf(fmaxf(g, -sg.clip), sg.clip);
   float u;
   if (sg.kind == 0) u = sg.lr * g;
@@ -966,10 +969,13 @@ __device__ __forceinline__ void upd_shadow(const UpdSeg& sg, __nv_bfloat16* __re
     shadow[sg.off_ps + ((int64_t)((py * 8 + px * 4 + c) * 9 + (dyr + 1) * 3 + (dxc + 1))) * sg.ps_O + o] = pb;
   }
 }
+template <bool SCALED>
 __global__ void __launch_bounds__(256) updater_kernel(float* __restrict__ params, const float* __restrict__ grads, float* __restrict__ st0, float* __restrict__ st1,
                                                       const UpdSeg* __restrict__ segs, const int32_t* __restrict__ chunk_seg, const int64_t* __restrict__ chunk_off,
-                                                      float inv_mb, float inv_world, int* __restrict__ step, unsigned* __restrict__ ticket, __nv_bfloat16* __restrict__ shadow) { pdl_enter();
+                                                      float inv_mb, float inv_world, int* __restrict__ step, unsigned* __restrict__ ticket, __nv_bfloat16* __restrict__ shadow,
+                                                      const float* __restrict__ gn_mult) { pdl_enter();
   const UpdSeg sg = segs[chunk_seg[blockIdx.x]];
+  const float gmult = SCALED ? gn_mult[chunk_seg[blockIdx.x]] : 1.0f;
   const int64_t base = chunk_off[blockIdx.x];
   const int64_t end = min(base + (int64_t)UPD_CHUNK, sg.off + sg.len);
   const int t = *step + 1;
@@ -987,8 +993,8 @@ __global__ void __launch_bounds__(256) updater_kernel(float* __restrict__ params
 #pragma unroll
     for (int q = 0; q < 4; ++q) { const int64_t i = base + 4 * (threadIdx.x + q * (int64_t)blockDim.x); if (i >= end) continue;
       float4 p4;
-      p4.x = upd_elem(sg, gv[q].x, pv[q].x, s0[q].x, s1[q].x, gscale, alpha_t); p4.y = upd_elem(sg, gv[q].y, pv[q].y, s0[q].y, s1[q].y, gscale, alpha_t);
-      p4.z = upd_elem(sg, gv[q].z, pv[q].z, s0[q].z, s1[q].z, gscale, alpha_t); p4.w = upd_elem(sg, gv[q].w, pv[q].w, s0[q].w, s1[q].w, gscale, alpha_t);
+      p4.x = upd_elem<SCALED>(sg, gv[q].x, pv[q].x, s0[q].x, s1[q].x, gscale, alpha_t, gmult); p4.y = upd_elem<SCALED>(sg, gv[q].y, pv[q].y, s0[q].y, s1[q].y, gscale, alpha_t, gmult);
+      p4.z = upd_elem<SCALED>(sg, gv[q].z, pv[q].z, s0[q].z, s1[q].z, gscale, alpha_t, gmult); p4.w = upd_elem<SCALED>(sg, gv[q].w, pv[q].w, s0[q].w, s1[q].w, gscale, alpha_t, gmult);
       *reinterpret_cast<float4*>(params + i) = p4;
       if (has0) *reinterpret_cast<float4*>(st0 + i) = s0[q];
       if (has1) *reinterpret_cast<float4*>(st1 + i) = s1[q];
@@ -1006,7 +1012,7 @@ __global__ void __launch_bounds__(256) updater_kernel(float* __restrict__ params
         gv[q] = ok ? grads[i] : 0.f; pv[q] = ok ? params[i] : 0.f; s0[q] = (ok && has0) ? st0[i] : 0.f; s1[q] = (ok && has1) ? st1[i] : 0.f; }
 #pragma unroll
       for (int q = 0; q < 4; ++q) { const int64_t i = i0 + q * (int64_t)blockDim.x; if (i >= end) continue;
-        const float p = upd_elem(sg, gv[q], pv[q], s0[q], s1[q], gscale, alpha_t);
+        const float p = upd_elem<SCALED>(sg, gv[q], pv[q], s0[q], s1[q], gscale, alpha_t, gmult);
         params[i] = p; if (has0) st0[i] = s0[q]; if (has1) st1[i] = s1[q];
         if (sh) upd_shadow(sg, shadow, i, __float2bfloat16_rn(p));
       }
@@ -1021,9 +1027,11 @@ __global__ void __launch_bounds__(256) updater_kernel(float* __restrict__ params
   }
 }
 void k_updater(float* params, const float* grads, float* st0, float* st1, const UpdSeg* segs, const int32_t* chunk_seg, const int64_t* chunk_off,
-               int nchunks, float inv_mb, float inv_world, int* step_dev, unsigned* ticket, __nv_bfloat16* shadow, cudaStream_t s) {
+               int nchunks, float inv_mb, float inv_world, int* step_dev, unsigned* ticket, __nv_bfloat16* shadow, const float* gn_mult, cudaStream_t s) {
   if (!nchunks) return;
-  launch_pdl(updater_kernel, dim3(nchunks), dim3(256), (size_t)(0), s, params, grads, st0, st1, segs, chunk_seg, chunk_off, inv_mb, inv_world, step_dev, ticket, shadow); LAUNCHED();
+  if (gn_mult) launch_pdl(updater_kernel<true>, dim3(nchunks), dim3(256), (size_t)(0), s, params, grads, st0, st1, segs, chunk_seg, chunk_off, inv_mb, inv_world, step_dev, ticket, shadow, gn_mult);
+  else launch_pdl(updater_kernel<false>, dim3(nchunks), dim3(256), (size_t)(0), s, params, grads, st0, st1, segs, chunk_seg, chunk_off, inv_mb, inv_world, step_dev, ticket, shadow, gn_mult);
+  LAUNCHED();
 }
 __global__ void fill_f32_kernel(float* p, float v, size_t n) { pdl_enter();
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = v;

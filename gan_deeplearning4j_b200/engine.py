@@ -18,6 +18,9 @@ LAYER_TYPES = {"conv2d": 0, "deconv2d": 1, "batchnorm": 2, "dense": 3, "activati
                "output": 7, "loss": 8, "ff_to_cnn": 9, "cnn_to_ff": 10, "dropout": 11}
 ACTS = {"identity": 0, "tanh": 1, "sigmoid": 2, "relu": 3, "lrelu": 4}
 UPDATERS = {"sgd": 0, "rmsprop": 1, "adam": 2, "noop": 3}
+# DL4J GradientNormalization -> b2g_gradient_normalization (DL4J's ordinals).  ClipElementWiseAbsoluteValue is the `grad_clip` argument of Net.
+GRADIENT_NORMALIZATIONS = {"none": 0, "renormalize_l2_per_layer": 1, "renormalize_l2_per_param_type": 2, "clip_l2_per_layer": 4,
+                           "clip_l2_per_param_type": 5}
 FP32, BF16 = 0, 1
 
 
@@ -119,7 +122,8 @@ class Net:
     """b2g_net: a chain-shaped ComputationGraph (init / output / fit / getLayer(..).getParam/setParam; J:166-170,420-510)."""
 
     def __init__(self, ctx: Context, specs: Sequence[Dict], input_shape, max_batch: int, precision: int = FP32,
-                 grad_clip: float = 0.0, xent_clip_eps: float = 1e-5, bn_groups: int = 1, seed: int = 666):
+                 grad_clip: float = 0.0, xent_clip_eps: float = 1e-5, bn_groups: int = 1, seed: int = 666,
+                 gradient_normalization: str = "none", gradient_normalization_threshold: float = 1.0):
         self.ctx, self.lib, self.specs = ctx, ctx.lib, list(specs)
         c, h, w = input_shape if len(input_shape) == 3 else (input_shape[0], 1, 1)
         self.input_shape = tuple(input_shape)
@@ -134,6 +138,12 @@ class Net:
         self.n_params = n.value
         check(self.lib.b2g_net_output_size(self.h, C.byref(n)))
         self.out_elems = n.value
+        if gradient_normalization != "none":
+            try:
+                self.set_gradient_normalization(gradient_normalization, gradient_normalization_threshold)
+            except Exception:
+                self.close()
+                raise
 
     # --- parameters (DL4J flattened-view order) ---
     def num_params(self) -> int:
@@ -211,6 +221,14 @@ class Net:
         s = C.c_float()
         check(self.lib.b2g_net_fit(self.h, _fp(x), _fp(y), x.shape[0], C.byref(s)))
         return s.value
+
+    def set_gradient_normalization(self, mode: str, threshold: float = 1.0):
+        """DL4J's GradientNormalization for every layer of the net, applied from the next update on: "none", "renormalize_l2_per_layer",
+        "renormalize_l2_per_param_type", "clip_l2_per_layer" or "clip_l2_per_param_type" (the clip modes need a finite threshold > 0; the
+        renormalize modes ignore it).  ClipElementWiseAbsoluteValue is `grad_clip` at construction, and excludes the L2 modes."""
+        if mode not in GRADIENT_NORMALIZATIONS:
+            raise ValueError(f"unknown gradient normalization {mode!r}; one of {sorted(GRADIENT_NORMALIZATIONS)} (element-wise clipping is grad_clip)")
+        check(self.lib.b2g_net_set_gradient_normalization(self.h, GRADIENT_NORMALIZATIONS[mode], float(threshold)))
 
     def set_grad_allreduce(self, enabled: bool):
         """False = the reference's parameter-averaging mode: fit() updates locally, average_parameters() synchronises."""

@@ -177,6 +177,26 @@ int32_t b2g_net_set_iteration(b2g_net* net, int64_t iteration);
  * Both are sync points, like get_iteration. */
 int32_t b2g_net_get_dropout_pass(b2g_net* net, int64_t* out);
 int32_t b2g_net_set_dropout_pass(b2g_net* net, int64_t pass);
+/* GradientNormalization (DL4J 1.0.0-beta3 BaseMultiLayerUpdater.preApply; the values are DL4J's ordinals).  Set per net; it applies wherever the
+ * net's updater runs (b2g_net_fit, the D and G updates of b2g_gan_step, parameter-averaging mode) and takes effect at the next update.
+ * The order of one update is  g /= mb  ->  normalization  ->  updater  ->  + l2*W  ->  theta -= g,  where g /= mb is the division the updater
+ * already does (BatchNorm running-stat pseudo-gradients are not divided by mb; under a gradient all-reduce they are averaged over ranks).
+ *   RENORM_L2_LAYER (1):  g <- g / ||g_layer||_2, dividing by 1e-5 instead when the norm is exactly 0; the threshold is ignored.
+ *   RENORM_L2_PARAM (2):  the same per parameter tensor (W, b, gamma, beta, mean, var).
+ *   CLIP_ELEMENTWISE (3): not accepted here: it is b2g_net_config.grad_clip.
+ *   CLIP_L2_LAYER (4):    g <- g * threshold / ||g_layer||_2 when ||g_layer||_2 > threshold (a norm equal to the threshold is not scaled).
+ *   CLIP_L2_PARAM (5):    the same per parameter tensor.
+ * A layer is one b2g_layer_desc entry with parameters that is not frozen; its gradient is its whole contiguous range of the flattened vector,
+ * so a BatchNorm layer's mean/var pseudo-gradients count in its norm and are scaled with it (as grad_clip clips them).  The norm is summed in
+ * double over the fp32 values of g after the division, the multiplier is rounded to fp32 once and multiplied into g.  Under a gradient
+ * all-reduce the norm is that of the all-reduced gradient, so every rank derives the same multipliers.  b2g_net_get_gradients still returns
+ * the raw summed gradients.  An L2 mode adds one kernel launch per update; B2G_GN_NONE launches what a net without normalization launches. */
+typedef enum {
+  B2G_GN_NONE = 0, B2G_GN_RENORM_L2_LAYER = 1, B2G_GN_RENORM_L2_PARAM = 2, B2G_GN_CLIP_ELEMENTWISE = 3, B2G_GN_CLIP_L2_LAYER = 4, B2G_GN_CLIP_L2_PARAM = 5
+} b2g_gradient_normalization;
+/* mode in {0, 1, 2, 4, 5}; the clip modes need a finite threshold > 0.  B2G_ERR_ARG for mode 3 (use grad_clip), an unknown mode, a bad
+ * threshold, or an L2 mode on a net created with grad_clip > 0 (DL4J allows one mode per layer). */
+int32_t b2g_net_set_gradient_normalization(b2g_net* net, int32_t mode, float threshold);
 /* BF16 nets: how many GEMM-shaped operations ran on the SIMT kernels instead of the tensor-core kernels since creation (skinny layers by design, or a
  * shape the tensor-core kernels do not tile).  north_star: no silent fallback -- bench.py prints it per step. */
 int32_t b2g_net_simt_gemm_calls(b2g_net* net, uint64_t* out);

@@ -30,6 +30,7 @@ public final class Native {
     public static native int netSetIteration(long net, long iteration);
     public static native int netGetDropoutPass(long net, long outAddr);
     public static native int netSetDropoutPass(long net, long pass);
+    public static native int netSetGradientNormalization(long net, int mode, float threshold);
     public static native int netSimtGemmCalls(long net, long outAddr);
     public static native int netSetSyncBn(long net, int enabled);
     public static native int netSetGradPayloadBf16(long net, int enabled);

@@ -21,8 +21,15 @@ public class NeuralNetConfiguration {
         public Builder inferenceWorkspaceMode(WorkspaceMode m) { return this; }
         public Builder seed(long s) { seed = s; return this; }
         public Builder optimizationAlgo(OptimizationAlgorithm a) { return this; }
-        public Builder gradientNormalization(GradientNormalization g) { if (g == GradientNormalization.None) clip = 0f; else if (clip == 0f) clip = 1f; return this; }
-        public Builder gradientNormalizationThreshold(double t) { clip = (float) t; return this; }
+        /** The L2 mode (RenormalizeL2* / ClipL2*) and its threshold (DL4J's default 1.0); ClipElementWiseAbsoluteValue lives in `clip`. */
+        public GradientNormalization gradNorm = GradientNormalization.None; public float gradNormThreshold = 1f;
+        public Builder gradientNormalization(GradientNormalization g) {
+            if (g.isL2()) { gradNorm = g; clip = 0f; return this; }
+            gradNorm = GradientNormalization.None;
+            if (g == GradientNormalization.None) clip = 0f; else if (clip == 0f) clip = 1f;
+            return this;
+        }
+        public Builder gradientNormalizationThreshold(double t) { gradNormThreshold = (float) t; if (!gradNorm.isL2()) clip = (float) t; return this; }
         public Builder l2(double v) { l2 = (float) v; return this; }
         public Builder activation(Activation a) { act = a; return this; }
         public Builder weightInit(WeightInit w) { return this; }

@@ -5,6 +5,7 @@ import java.nio.ByteBuffer;
 import java.nio.FloatBuffer;
 import java.util.List;
 import org.deeplearning4j.b200.Native;
+import org.deeplearning4j.nn.conf.GradientNormalization;
 import org.deeplearning4j.nn.conf.NeuralNetConfiguration.ComputationGraphConfiguration;
 import org.deeplearning4j.nn.conf.layers.Layer;
 import org.nd4j.linalg.api.ndarray.INDArray;
@@ -24,6 +25,8 @@ public class ComputationGraph {
         ByteBuffer h = Native.direct(8);
         Native.check(Native.netCreate(Native.context(), Native.address(cfg), Native.address(desc), layers.size(), Native.address(h)));
         net = h.getLong(0);
+        GradientNormalization gn = conf.b.g.gradNorm;      // RenormalizeL2* / ClipL2*: on-device norms before every update
+        if (gn.isL2()) Native.check(Native.netSetGradientNormalization(net, gn.ordinal(), conf.b.g.gradNormThreshold));
     }
     public long handle() { return net; }
     public ComputationGraphConfiguration configuration() { return conf; }

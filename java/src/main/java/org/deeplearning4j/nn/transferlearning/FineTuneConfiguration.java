@@ -9,14 +9,17 @@ import org.nd4j.linalg.activations.Activation;
 import org.nd4j.linalg.learning.config.IUpdater;
 
 public class FineTuneConfiguration {
-    public float clip, l2; public Activation act = Activation.TANH; public IUpdater updater; public long seed = 666;
+    public float clip, l2; public GradientNormalization gradNorm = GradientNormalization.None; public float gradNormThreshold = 1f; public Activation act = Activation.TANH; public IUpdater updater; public long seed = 666;
     public static class Builder {
         private final FineTuneConfiguration c = new FineTuneConfiguration();
         public Builder trainingWorkspaceMode(WorkspaceMode m) { return this; }
         public Builder inferenceWorkspaceMode(WorkspaceMode m) { return this; }
         public Builder optimizationAlgo(OptimizationAlgorithm a) { return this; }
-        public Builder gradientNormalization(GradientNormalization g) { if (c.clip == 0f && g != GradientNormalization.None) c.clip = 1f; return this; }
-        public Builder gradientNormalizationThreshold(double t) { c.clip = (float) t; return this; }
+        public Builder gradientNormalization(GradientNormalization g) {
+            if (g.isL2()) { c.gradNorm = g; c.clip = 0f; return this; }
+            c.gradNorm = GradientNormalization.None; if (c.clip == 0f && g != GradientNormalization.None) c.clip = 1f; return this;
+        }
+        public Builder gradientNormalizationThreshold(double t) { c.gradNormThreshold = (float) t; if (!c.gradNorm.isL2()) c.clip = (float) t; return this; }
         public Builder activation(Activation a) { c.act = a; return this; }
         public Builder l2(double v) { c.l2 = (float) v; return this; }
         public Builder weightInit(WeightInit w) { return this; }

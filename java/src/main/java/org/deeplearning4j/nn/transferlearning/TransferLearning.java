@@ -21,6 +21,7 @@ public final class TransferLearning {
         public GraphBuilder addLayer(String name, Layer l, String... inputs) { l.name = name; added.add(l); return this; }
         public ComputationGraph build() {
             NeuralNetConfiguration.Builder b = new NeuralNetConfiguration.Builder().seed(ft.seed).gradientNormalizationThreshold(ft.clip).l2(ft.l2).activation(ft.act);
+            if (ft.gradNorm.isL2()) b.gradientNormalization(ft.gradNorm).gradientNormalizationThreshold(ft.gradNormThreshold);
             NeuralNetConfiguration.GraphBuilder g = b.graphBuilder().setInputTypes(src.configuration().b.in);
             boolean frozen = frozenUpTo != null;
             for (Layer l : src.configuration().b.layers) {

@@ -44,6 +44,7 @@ FN(netGetIteration)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net
 FN(netSetIteration)(JNIEnv_*, jclass, jlong net, jlong it) { return b2g_net_set_iteration(P(b2g_net*, net), it); }
 FN(netGetDropoutPass)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_get_dropout_pass(P(b2g_net*, net), P(int64_t*, outAddr)); }
 FN(netSetDropoutPass)(JNIEnv_*, jclass, jlong net, jlong pass) { return b2g_net_set_dropout_pass(P(b2g_net*, net), pass); }
+FN(netSetGradientNormalization)(JNIEnv_*, jclass, jlong net, jint mode, jfloat threshold) { return b2g_net_set_gradient_normalization(P(b2g_net*, net), mode, threshold); }
 FN(netSimtGemmCalls)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_simt_gemm_calls(P(b2g_net*, net), P(uint64_t*, outAddr)); }
 FN(netSetSyncBn)(JNIEnv_*, jclass, jlong net, jint enabled) { return b2g_net_set_sync_bn(P(b2g_net*, net), enabled); }
 FN(netSetGradPayloadBf16)(JNIEnv_*, jclass, jlong net, jint enabled) { return b2g_net_set_grad_payload_bf16(P(b2g_net*, net), enabled); }
