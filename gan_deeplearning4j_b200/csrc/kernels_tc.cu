@@ -6,15 +6,15 @@
 // and activation passes; SURVEY.md section 8a rows a1, a2; reference call sites J:135-150, 203-219) for the
 // DCGAN shapes of SURVEY.md Appendix B.
 //
-// One warp-specialised CTA of three warpgroups computes a 128 x BN output tile:
-//   warpgroup 0     TMA producer: one elected lane of warp 0 issues, per K-block, one 4-D tensor-map box for the activations (the
-//                   im2col gather is done by the TMA unit: traversal strides give the stride-2 sampling, out-of-bounds coordinates
-//                   give the zero padding) and the weight box(es), both landing 128B-swizzled in a STAGES-deep smem ring (mbarrier
-//                   expect_tx)
-//   warpgroups 1-2  consumers: each owns 64 accumulator rows and issues 4 x wgmma m64nNk16 per K-block straight from the swizzled
-//                   tiles via matrix descriptors, keeping one K-block in flight; after the main loop the accumulators are parked as
-//                   fp32 in the drained ring and the eight consumer warps run the epilogue (one thread = one output pixel): + bias,
-//                   activation, BatchNorm statistics, convert to bf16, 16-byte stores of the contiguous NHWC channel run
+// A persistent, warp-specialised CTA of five warpgroups (one per SM) walks 128 x BN output tiles:
+//   producer        one elected lane issues, per K-block, one 4-D tensor-map box for the activations (the im2col gather is done by the
+//                   TMA unit: traversal strides give the stride-2 sampling, out-of-bounds coordinates give the zero padding) and the
+//                   weight box(es), both landing 128B-swizzled in a STAGES-deep smem ring (mbarrier expect_tx), tile after tile
+//   2 consumers     each owns 64 accumulator rows and issues 4 x wgmma m64nNk16 per K-block straight from the swizzled tiles via
+//                   matrix descriptors, keeping one K-block in flight; at the end of a tile the accumulators are parked as fp32 in a
+//                   park buffer and the consumers go on with the next tile
+//   2 epilogue      one thread = one output pixel of the parked tile: + bias, activation, BatchNorm statistics, convert to bf16, 16-byte
+//                   stores of the contiguous NHWC channel run -- overlapping the next tile's MMAs
 // Modes: fprop (conv forward; also the input-gradient of a transposed conv) and dgrad (conv input-gradient = transposed
 // conv forward) in sub-pixel phase form: a 4x4 stride-2 pad-1 transposed conv is four 2x2 stride-1 convs, one per output
 // parity class, so no MAC is spent on inserted zeros and nothing is scattered.
@@ -160,9 +160,11 @@ struct TcConvParams {
   int imgs_per_group;
   const __nv_bfloat16* aux; // EPI_BNBWD / EPI_ACTBWD: the forward output whose act' multiplies the result   (same NHWC shape as `out`)
   const __nv_bfloat16* aux2;// EPI_BNBWD: the BatchNorm input z
+  int tiles_m, tiles_n, phases;   // work items: tile t = ((phase * tiles_n) + n tile) * tiles_m + m tile
 };
 
-static constexpr int TC_THREADS = 384;       // producer warpgroup + two consumer warpgroups
+static constexpr int TC_THREADS = 384;       // tc_wgrad_kernel: producer warpgroup + two consumer warpgroups
+static constexpr int TC_CONV_THREADS = 640;  // tc_conv_kernel: two MMA consumer warpgroups, two epilogue warpgroups, a producer warpgroup
 template <int BN, int STAGES, int EPI = EPI_PLAIN>
 struct TcSmem {
   static constexpr int A_BYTES = 128 * 128;        // 128 rows x 64 bf16
@@ -170,14 +172,19 @@ struct TcSmem {
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
   static constexpr int ACC_PITCH = BN + 4;         // floats per parked accumulator row: 16-byte row reads by 8 lanes hit 8 different bank groups
-  static_assert(128 * ACC_PITCH * 4 <= RING_BYTES, "the parked accumulators live in the drained ring");
-  static constexpr int BAR_OFF = RING_BYTES;
+  static constexpr int PARK_BYTES = 128 * ACC_PITCH * 4;
+  static constexpr int PARKS = BN >= 128 ? 1 : 2;  // accumulator park slots: two where shared memory allows (a 128-column tile has one)
+  static constexpr int PARK_OFF = RING_BYTES;
+  static constexpr int BAR_OFF = PARK_OFF + PARKS * PARK_BYTES;
   static constexpr int STAT_OFF = BAR_OFF + 256;
   static constexpr int STG_OFF = STAT_OFF + ((EPI == EPI_STATS || EPI == EPI_BNBWD) ? 4 * 2 * BN * 4 : 0);
   static constexpr int TOTAL = STG_OFF + (BN >= 32 ? 8 * 2048 : 0) + 1024;   // + barriers + statistics + epilogue staging + alignment slack
+  static_assert(TOTAL <= 227 * 1024, "one CTA per SM must fit the shared memory of an sm_90 SM");
 };
 
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }    // the eight consumer warps only
+__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }    // the eight epilogue warps only
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // column sums over the 32 lanes of a warp: on return lane l holds sum_lanes a[l] in a[0].  One butterfly level per template instance, so
 // that every index into `a` is a compile-time constant and the array stays in registers (a runtime loop over the level puts it on the stack).
@@ -199,8 +206,8 @@ __device__ __forceinline__ void warp_colsum32(float (&a)[32], int lane) { warp_c
 // A thread owns one accumulator row, but a warp instruction in which every lane touches its own row costs the load/store unit 32
 // wavefronts of 16 B each.  Global traffic therefore goes through a per-warp 2 KB staging area `stg` ([32 rows][4 x 16 B], XOR-swizzled so
 // that both access patterns are bank-conflict free): four lanes cover the 64 B of one row, a warp instruction covers 8 rows = 16 full
-// sectors.  The same transposition brings the auxiliary operands (forward output y, BN input z) in, and the loads for the next 32 columns
-// are issued before the arithmetic of the current ones so that their latency hides behind it.
+// sectors.  The same transposition brings the auxiliary operands (forward output y, BN input z) in, 32 columns at a time (loading the next
+// 32 ahead would keep 32 more registers live than the epilogue warpgroups have; their latency overlaps the next tile's MMAs instead).
 template <int BN, int EPI, bool AFFINE>
 __device__ __forceinline__ void epi_tile(const TcConvParams& p, const float* srow, size_t roff, int nb0, int group, float* sst, uint4* stg, int q, int lane, int ep_tid,
                                          int c_beg, int c_end) {
@@ -210,19 +217,18 @@ __device__ __forceinline__ void epi_tile(const TcConvParams& p, const float* sro
   size_t roff_i[4];                      // element offsets of the rows this lane serves in the transposed pattern: row i*8 + lane/4
 #pragma unroll
   for (int i = 0; i < 4; ++i) roff_i[i] = __shfl_sync(0xffffffffu, (unsigned long long)roff, i * 8 + sub) + cq * 8;
-  uint4 gy[4], gz[4];
-  if constexpr (EPI >= EPI_BNBWD) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) gy[i] = *reinterpret_cast<const uint4*>(p.aux + roff_i[i] + c_beg);
-  }
-  if constexpr (EPI == EPI_BNBWD) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i) gz[i] = *reinterpret_cast<const uint4*>(p.aux2 + roff_i[i] + c_beg);
-  }
 #pragma unroll 1
   for (int c0 = c_beg; c0 < c_end; c0 += 32) {
     uint32_t v[32];
-    uint4 ax[4], az[4];
+    uint4 gy[4], gz[4], ax[4], az[4];
+    if constexpr (EPI >= EPI_BNBWD) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) gy[i] = *reinterpret_cast<const uint4*>(p.aux + roff_i[i] + c0);
+    }
+    if constexpr (EPI == EPI_BNBWD) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) gz[i] = *reinterpret_cast<const uint4*>(p.aux2 + roff_i[i] + c0);
+    }
     if constexpr (EPI >= EPI_BNBWD) {
 #pragma unroll
       for (int i = 0; i < 4; ++i) { const int r = i * 8 + sub; stg[r * 4 + (cq ^ ((r >> 1) & 3))] = gy[i]; }
@@ -230,10 +236,6 @@ __device__ __forceinline__ void epi_tile(const TcConvParams& p, const float* sro
 #pragma unroll
       for (int j = 0; j < 4; ++j) ax[j] = stg[lane * 4 + (j ^ sx)];
       __syncwarp();
-      if (c0 + 32 < c_end) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) gy[i] = *reinterpret_cast<const uint4*>(p.aux + roff_i[i] + c0 + 32);
-      }
     }
     if constexpr (EPI == EPI_BNBWD) {
 #pragma unroll
@@ -242,10 +244,6 @@ __device__ __forceinline__ void epi_tile(const TcConvParams& p, const float* sro
 #pragma unroll
       for (int j = 0; j < 4; ++j) az[j] = stg[lane * 4 + (j ^ sx)];
       __syncwarp();
-      if (c0 + 32 < c_end) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) gz[i] = *reinterpret_cast<const uint4*>(p.aux2 + roff_i[i] + c0 + 32);
-      }
     }
 #pragma unroll
     for (int j = 0; j < 8; ++j) { const uint4 t = reinterpret_cast<const uint4*>(srow + c0)[j]; v[4 * j] = t.x; v[4 * j + 1] = t.y; v[4 * j + 2] = t.z; v[4 * j + 3] = t.w; }
@@ -369,79 +367,110 @@ __device__ __forceinline__ void tap_coords(const TcConvParams& p, int ta, int tb
   }
 }
 
-// One warp-specialised CTA per 128 x BN output tile.
+// Persistent and warp-specialised: CTA b walks the work items t = b, b + gridDim.x, ... (one 128 x BN output tile of one phase each).
+//   warpgroups 0-1  MMA consumers: 64 accumulator rows each; at the end of a tile's K loop they park the fp32 fragments in a park slot (not the
+//                   ring), arrive on "park full" and go straight on to the next tile
+//   warpgroups 2-3  epilogue: wait on "park full", run epi_tile (or the pixel-shuffle scatter) from the slot, arrive on "park empty"
+//   warpgroup 4     TMA producer (one warp): the K-blocks of all of the CTA's tiles as one stream through the ring, so the next tile's loads are in flight
+//                   before the current tile's K loop ends
+// so the epilogue of tile i runs while the MMAs of tile i+1 are issued.  The per-tile arithmetic and summation order are those of a
+// one-tile CTA: results do not depend on the grid size.
 // PS ("pixel shuffle", BN = 16): the 4x4 stride-2 pad-1 transposed conv onto <= 4 image channels (G-last forward, D1 input gradient) as ONE
 // 3x3 stride-1 pad-1 convolution whose 16 output columns are (py, px, c) = the 2x2 output block x 4 (padded) channels: the four
 // sub-pixel phases share every activation load (9 taps instead of 4 x 4), the packed weight [16][9][O] holds zeros where a
 // (tap, phase) pair does not meet; the epilogue scatters its 16 values to the 2x2 block of the NHWC image.
+// Registers per thread after setmaxnreg.  Each SM sub-partition holds one warp of every warpgroup and 64 KB of registers, so the launch
+// gives 96 per thread (16384 / (5 x 32), in steps of 8) and PRODUCER + 2 MMA + 2 EPI must stay within 5 x 96.  128 accumulator columns
+// need 96 in the MMA warpgroups (at 88 ptxas serialises the wgmmas).
+template <int BN>
+struct TcConvRegs {
+  static constexpr int LAUNCH = 96, PRODUCER = 24, MMA = BN >= 128 ? 96 : 64, EPI = BN >= 128 ? 128 : 160;
+  static_assert(PRODUCER + 2 * MMA + 2 * EPI <= 5 * LAUNCH, "setmaxnreg budget exceeds the launch allocation");
+};
 template <int BN, int STAGES, int EPI, bool AFFINE, bool PS = false>
-__global__ void __launch_bounds__(TC_THREADS, 1) tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcConvParams p) {
+__global__ void __launch_bounds__(TC_CONV_THREADS, 1) tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcConvParams p) {
   using S = TcSmem<BN, STAGES, EPI>;
+  using R = TcConvRegs<BN>;
   constexpr int NB = BN >= 64 ? BN / 64 : 1, NACC = BN >= 64 ? 32 : BN / 2;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
   const uint32_t bar_full = smem_base + S::BAR_OFF;                 // STAGES x 8 B
   const uint32_t bar_empty = bar_full + 8 * STAGES;                 // STAGES x 8 B
+  const uint32_t park_full = bar_empty + 8 * STAGES;                // PARKS x 8 B
+  const uint32_t park_empty = park_full + 8 * S::PARKS;             // PARKS x 8 B
   float* sst = reinterpret_cast<float*>(smem_gen + S::STAT_OFF);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  // tile coordinates
-  const int mt = blockIdx.x, nb0 = blockIdx.y * BN, phase = blockIdx.z;
-  const int py = phase >> 1, px = phase & 1;
-  int n0, y0;
-  if (p.Nt > 1) { n0 = mt * p.Nt; y0 = 0; } else { n0 = mt / p.tiles_y; y0 = (mt % p.tiles_y) * p.Ht; }
   const int num_kb = p.taps_h * p.taps_w * p.chunks;
+  const int tiles = p.tiles_m * p.tiles_n * p.phases;
+  // work item -> first output channel, phase, and the first image / row of its 128-row tile
+  auto tile_coords = [&](int t, int& nb0, int& phase, int& n0, int& y0) {
+    const int mt = t % p.tiles_m, r = t / p.tiles_m;
+    nb0 = (r % p.tiles_n) * BN; phase = r / p.tiles_n;
+    if (p.Nt > 1) { n0 = mt * p.Nt; y0 = 0; } else { n0 = mt / p.tiles_y; y0 = (mt % p.tiles_y) * p.Ht; }
+  };
 
   if (threadIdx.x == 0) {
     prefetch_map(&tmA); prefetch_map(&tmB);
     for (int s = 0; s < STAGES; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 8); }    // 8 consumer warps release a stage
+    for (int k = 0; k < S::PARKS; ++k) { mbar_init(park_full + 8 * k, 256); mbar_init(park_empty + 8 * k, 256); }   // every consumer / epilogue thread
     fence_mbar_init();
   }
   __syncthreads();
   pdl_wait();         // barrier init above overlaps the predecessor's tail; global memory is touched only below
 
-  if (warp == 0) {
-    // ===== TMA producer (converged warp, elected lane issues): no integer division inside the loop -- ring slot, channel chunk and tap advance as counters =====
-    const int ybase = p.mode == 0 ? y0 * p.SH : y0;
-    int s = 0, ch = 0, ta = 0, tb = 0; uint32_t ph = 0;
-    int ax, dy_, wtap; tap_coords(p, 0, 0, py, px, ax, dy_, wtap);
-    for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait(bar_empty + 8 * s, ph ^ 1);
-      if (elect_one_sync()) {
-        mbar_expect_tx(bar_full + 8 * s, S::STAGE_BYTES);
-        tma_load_4d(smem_base + s * S::STAGE_BYTES, &tmA, bar_full + 8 * s, ch * 64, ax, ybase + dy_, n0);
-        load_b_tile<BN>(p, &tmB, smem_base + s * S::STAGE_BYTES + S::A_BYTES, bar_full + 8 * s, ch, wtap, nb0);
+  if (warp >= 16) {
+    setmaxnreg_dec<R::PRODUCER>();
+    if (warp == 16) {
+      // ===== TMA producer (converged warp, elected lane issues): no integer division inside the K loop -- ring slot, channel chunk and tap advance as counters =====
+      int s = 0; uint32_t ph = 0;
+      for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+        int nb0, phase, n0, y0; tile_coords(t, nb0, phase, n0, y0);
+        const int py = phase >> 1, px = phase & 1;
+        const int ybase = p.mode == 0 ? y0 * p.SH : y0;
+        int ch = 0, ta = 0, tb = 0;
+        int ax, dy_, wtap; tap_coords(p, 0, 0, py, px, ax, dy_, wtap);
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(bar_empty + 8 * s, ph ^ 1);
+          if (elect_one_sync()) {
+            mbar_expect_tx(bar_full + 8 * s, S::STAGE_BYTES);
+            tma_load_4d(smem_base + s * S::STAGE_BYTES, &tmA, bar_full + 8 * s, ch * 64, ax, ybase + dy_, n0);
+            load_b_tile<BN>(p, &tmB, smem_base + s * S::STAGE_BYTES + S::A_BYTES, bar_full + 8 * s, ch, wtap, nb0);
+          }
+          __syncwarp();
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+          if (++ch == p.chunks) { ch = 0; if (++tb == p.taps_w) { tb = 0; ++ta; } tap_coords(p, ta, tb, py, px, ax, dy_, wtap); }
+        }
       }
-      __syncwarp();
-      if (++s == STAGES) { s = 0; ph ^= 1; }
-      if (++ch == p.chunks) { ch = 0; if (++tb == p.taps_w) { tb = 0; ++ta; } tap_coords(p, ta, tb, py, px, ax, dy_, wtap); }
     }
-  } else if (warp >= 4) {
-    // ===== consumers: warpgroup wg owns accumulator rows [64 wg, 64 wg + 64) =====
-    const int wg = (warp >> 2) - 1;
-    float acc[NB][NACC];
+  } else if (warp < 8) {
+    if constexpr (R::MMA < R::LAUNCH) setmaxnreg_dec<R::MMA>();
+    // ===== MMA consumers: warpgroup wg owns accumulator rows [64 wg, 64 wg + 64) =====
+    const int wg = warp >> 2;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    int s = 0, k = 0; uint32_t ph = 0, kph = 0;
+    for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+      float acc[NB][NACC];
 #pragma unroll
-    for (int nb = 0; nb < NB; ++nb)
+      for (int nb = 0; nb < NB; ++nb)
 #pragma unroll
-      for (int j = 0; j < NACC; ++j) acc[nb][j] = 0.f;
-    int s = 0, prev = -1; uint32_t ph = 0;
-    for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait(bar_full + 8 * s, ph);
-      wg_fence();
-      const uint32_t st = smem_base + s * S::STAGE_BYTES;
-      mma_kblock<BN, NB, NACC>(acc, st + wg * 8192, st + S::A_BYTES, PS ? 0 : p.b_mn);
-      wg_commit();
-      wg_wait<1>();                                   // the previous K-block's MMAs are done: its stage goes back to the producer
-      if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
-      prev = s;
-      if (++s == STAGES) { s = 0; ph ^= 1; }
-    }
-    wg_wait<0>();
-    epi_bar_sync();                                   // both warpgroups are done with the ring: it now holds the fp32 accumulators
-    float* park = reinterpret_cast<float*>(smem_gen);
-    {
-      const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        for (int j = 0; j < NACC; ++j) acc[nb][j] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(bar_full + 8 * s, ph);
+        wg_fence();
+        const uint32_t st = smem_base + s * S::STAGE_BYTES;
+        mma_kblock<BN, NB, NACC>(acc, st + wg * 8192, st + S::A_BYTES, PS ? 0 : p.b_mn);
+        wg_commit();
+        wg_wait<1>();                                   // the previous K-block's MMAs are done: its stage goes back to the producer
+        if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
+        prev = s;
+        if (++s == STAGES) { s = 0; ph ^= 1; }
+      }
+      wg_wait<0>();
+      if (lane == 0) mbar_arrive(bar_empty + 8 * prev);
+      mbar_wait(park_empty + 8 * k, kph ^ 1);           // the epilogue is done with the tile parked in this slot before
+      float* park = reinterpret_cast<float*>(smem_gen + S::PARK_OFF + k * S::PARK_BYTES);
 #pragma unroll
       for (int nb = 0; nb < NB; ++nb)
 #pragma unroll
@@ -450,50 +479,62 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_conv_kernel(const __grid_con
           *reinterpret_cast<float2*>(park + r0 * S::ACC_PITCH + col) = make_float2(acc[nb][4 * j], acc[nb][4 * j + 1]);
           *reinterpret_cast<float2*>(park + (r0 + 8) * S::ACC_PITCH + col) = make_float2(acc[nb][4 * j + 2], acc[nb][4 * j + 3]);
         }
+      mbar_arrive(park_full + 8 * k);
+      if (++k == S::PARKS) { k = 0; kph ^= 1; }
     }
-    epi_bar_sync();
-    // ===== epilogue: consumer warp cw serves rows [32 q, 32 q + 32) (q = cw % 4), column half cw / 4 =====
-    const int cw = warp - 4, q = cw & 3, half = cw >> 2;
+  } else {
+    setmaxnreg_inc<R::EPI>();
+    // ===== epilogue: warp ew serves parked rows [32 q, 32 q + 32) (q = ew % 4), column half ew / 4 =====
+    const int ew = warp - 8, q = ew & 3, half = ew >> 2;
     const int row = q * 32 + lane;
     const int img = row / (p.Ht * p.Wt), rem = row % (p.Ht * p.Wt), yy = rem / p.Wt, xx = rem % p.Wt;
-    const int n = n0 + img, gy = y0 + yy, gx = xx;
-    const float* srow = park + row * S::ACC_PITCH;
-    if constexpr (PS) {
-      if (half == 0) {
-        const int C = p.OC;
+    int k = 0; uint32_t kph = 0;
+    for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+      int nb0, phase, n0, y0; tile_coords(t, nb0, phase, n0, y0);
+      const int py = phase >> 1, px = phase & 1;
+      const int n = n0 + img, gy = y0 + yy, gx = xx;
+      mbar_wait(park_full + 8 * k, kph);
+      const float* srow = reinterpret_cast<const float*>(smem_gen + S::PARK_OFF + k * S::PARK_BYTES) + row * S::ACC_PITCH;
+      if constexpr (PS) {
+        if (half == 0) {
+          const int C = p.OC;
 #pragma unroll
-        for (int ppy = 0; ppy < 2; ++ppy) {
-          const size_t doff = (((size_t)n * p.outH + 2 * gy + ppy) * p.outW + 2 * gx) * C;
-          __nv_bfloat16* dst = p.out + doff;
-          float o[8];
-#pragma unroll
-          for (int ppx = 0; ppx < 2; ++ppx)
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              float a = srow[(ppy * 2 + ppx) * 4 + c];
-              if constexpr (EPI == EPI_ACTBWD) { if (c < C) a *= act_grad_from_out(p.act, __bfloat162float(p.aux[doff + ppx * C + c]), p.alpha); }
-              else { if (p.bias && c < C) a += p.bias[c]; a = act_fwd(p.act, a, p.alpha); }
-              o[ppx * 4 + c] = a;
-            }
-          if (C == 3) {         // 6 contiguous bf16 = three aligned 32-bit stores
-            __nv_bfloat162 h0 = __floats2bfloat162_rn(o[0], o[1]), h1 = __floats2bfloat162_rn(o[2], o[4]), h2 = __floats2bfloat162_rn(o[5], o[6]);
-            uint32_t* d32 = reinterpret_cast<uint32_t*>(dst);
-            d32[0] = *reinterpret_cast<uint32_t*>(&h0); d32[1] = *reinterpret_cast<uint32_t*>(&h1); d32[2] = *reinterpret_cast<uint32_t*>(&h2);
-          } else {
+          for (int ppy = 0; ppy < 2; ++ppy) {
+            const size_t doff = (((size_t)n * p.outH + 2 * gy + ppy) * p.outW + 2 * gx) * C;
+            __nv_bfloat16* dst = p.out + doff;
+            float o[8];
 #pragma unroll
             for (int ppx = 0; ppx < 2; ++ppx)
 #pragma unroll
-              for (int c = 0; c < 4; ++c) if (c < C) dst[ppx * C + c] = __float2bfloat16(o[ppx * 4 + c]);
+              for (int c = 0; c < 4; ++c) {
+                float a = srow[(ppy * 2 + ppx) * 4 + c];
+                if constexpr (EPI == EPI_ACTBWD) { if (c < C) a *= act_grad_from_out(p.act, __bfloat162float(p.aux[doff + ppx * C + c]), p.alpha); }
+                else { if (p.bias && c < C) a += p.bias[c]; a = act_fwd(p.act, a, p.alpha); }
+                o[ppx * 4 + c] = a;
+              }
+            if (C == 3) {         // 6 contiguous bf16 = three aligned 32-bit stores
+              __nv_bfloat162 h0 = __floats2bfloat162_rn(o[0], o[1]), h1 = __floats2bfloat162_rn(o[2], o[4]), h2 = __floats2bfloat162_rn(o[5], o[6]);
+              uint32_t* d32 = reinterpret_cast<uint32_t*>(dst);
+              d32[0] = *reinterpret_cast<uint32_t*>(&h0); d32[1] = *reinterpret_cast<uint32_t*>(&h1); d32[2] = *reinterpret_cast<uint32_t*>(&h2);
+            } else {
+#pragma unroll
+              for (int ppx = 0; ppx < 2; ++ppx)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) if (c < C) dst[ppx * C + c] = __float2bfloat16(o[ppx * 4 + c]);
+            }
           }
         }
+      } else {
+        size_t pix;
+        if (p.mode == 0) pix = ((size_t)n * p.outH + gy) * p.outW + gx;
+        else pix = ((size_t)n * p.outH + 2 * gy + py) * p.outW + 2 * gx + px;
+        const int group = p.imgs_per_group > 0 ? n0 / p.imgs_per_group : 0;
+        epi_tile<BN, EPI, AFFINE>(p, srow, pix * p.OC + nb0, nb0, group, sst, reinterpret_cast<uint4*>(smem_gen + S::STG_OFF) + ew * 128, q, lane,
+                                  (int)threadIdx.x - 256, half * (BN / 2), (half + 1) * (BN / 2));
+        if constexpr (EPI == EPI_STATS || EPI == EPI_BNBWD) epi_bar_sync();   // every epilogue warp has read sst before the next tile rewrites it
       }
-    } else {
-      size_t pix;
-      if (p.mode == 0) pix = ((size_t)n * p.outH + gy) * p.outW + gx;
-      else pix = ((size_t)n * p.outH + 2 * gy + py) * p.outW + 2 * gx + px;
-      const int group = p.imgs_per_group > 0 ? n0 / p.imgs_per_group : 0;
-      epi_tile<BN, EPI, AFFINE>(p, srow, pix * p.OC + nb0, nb0, group, sst, reinterpret_cast<uint4*>(smem_gen + S::STG_OFF) + cw * 128, q, lane, (int)threadIdx.x - 128,
-                                half * (BN / 2), (half + 1) * (BN / 2));
+      mbar_arrive(park_empty + 8 * k);
+      if (++k == S::PARKS) { k = 0; kph ^= 1; }
     }
   }
 }
@@ -537,28 +578,31 @@ bool tc_dgrad_supported(const ConvGeom& g) {
 // the fused BatchNorm epilogues need every 128-row tile inside one statistics group
 static bool tc_epi_ok(const TcEpi* e, int Nt) { return !e || e->mode == EPI_PLAIN || e->mode == EPI_ACTBWD || (e->imgs_per_group > 0 && e->imgs_per_group % Nt == 0 && e->acc); }
 
+// persistent grid: one CTA per SM, or one per work item when there are fewer
 template <int BN, int STAGES, int EPI, bool AFFINE, bool PS = false>
-static int launch_conv_e(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, dim3 grid, cudaStream_t s) {
+static int launch_conv_e(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, cudaStream_t s) {
   using S = TcSmem<BN, STAGES, EPI>;
   TC_SET_SMEM_ONCE((tc_conv_kernel<BN, STAGES, EPI, AFFINE, PS>), S::TOTAL);
-  launch_pdl(tc_conv_kernel<BN, STAGES, EPI, AFFINE, PS>, dim3(grid), dim3(TC_THREADS), (size_t)(S::TOTAL), s, tmA, tmB, p);
+  const long tiles = (long)p.tiles_m * p.tiles_n * p.phases;
+  const unsigned grid = (unsigned)std::min<long>(tiles, device_sm_count());
+  launch_pdl(tc_conv_kernel<BN, STAGES, EPI, AFFINE, PS>, dim3(grid), dim3(TC_CONV_THREADS), (size_t)(S::TOTAL), s, tmA, tmB, p);
   LAUNCHED();
   return cudaPeekAtLastError() == cudaSuccess ? 0 : -3;
 }
 template <int BN, int STAGES>
-static int launch_conv(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, dim3 grid, cudaStream_t s, const char* name) {
+static int launch_conv(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, cudaStream_t s, const char* name) {
   g_tc_last_kernel = name;
   switch (p.epi) {
-    case EPI_STATS: return launch_conv_e<BN, STAGES, EPI_STATS, false>(tmA, tmB, p, grid, s);
-    case EPI_BNBWD: return launch_conv_e<BN, STAGES, EPI_BNBWD, false>(tmA, tmB, p, grid, s);
-    case EPI_ACTBWD: return launch_conv_e<BN, STAGES, EPI_ACTBWD, false>(tmA, tmB, p, grid, s);
+    case EPI_STATS: return launch_conv_e<BN, STAGES, EPI_STATS, false>(tmA, tmB, p, s);
+    case EPI_BNBWD: return launch_conv_e<BN, STAGES, EPI_BNBWD, false>(tmA, tmB, p, s);
+    case EPI_ACTBWD: return launch_conv_e<BN, STAGES, EPI_ACTBWD, false>(tmA, tmB, p, s);
   }
-  return (p.scale && p.bias) ? launch_conv_e<BN, STAGES, EPI_PLAIN, true>(tmA, tmB, p, grid, s) : launch_conv_e<BN, STAGES, EPI_PLAIN, false>(tmA, tmB, p, grid, s);
+  return (p.scale && p.bias) ? launch_conv_e<BN, STAGES, EPI_PLAIN, true>(tmA, tmB, p, s) : launch_conv_e<BN, STAGES, EPI_PLAIN, false>(tmA, tmB, p, s);
 }
-static int dispatch_conv(int BN, const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, dim3 grid, cudaStream_t s) {
+static int dispatch_conv(int BN, const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, cudaStream_t s) {
   switch (BN) {
-    case 64: return launch_conv<64, 4>(tmA, tmB, p, grid, s, "tc_conv_kernel<64,4>");
-    case 128: return launch_conv<128, 4>(tmA, tmB, p, grid, s, "tc_conv_kernel<128,4>");
+    case 64: return launch_conv<64, 4>(tmA, tmB, p, s, "tc_conv_kernel<64,4>");
+    case 128: return launch_conv<128, 4>(tmA, tmB, p, s, "tc_conv_kernel<128,4>");
   }
   return -4;
 }
@@ -594,9 +638,9 @@ int k_tc_fprop(const ConvGeom& g, const __nv_bfloat16* x, const __nv_bfloat16* w
   cuuint32_t box[4] = {64, (cuuint32_t)(p.Wt * g.SW), (cuuint32_t)(p.Ht * g.SH), (cuuint32_t)p.Nt};
   cuuint32_t es[4] = {1, (cuuint32_t)g.SW, (cuuint32_t)g.SH, 1};
   if (make_map_bf16(&tmA, x, 4, dims, strides, box, es)) return -1;
-  dim3 grid((unsigned)(g.N * g.OH * g.OW / 128), (unsigned)(g.O / BN), 1);
+  p.tiles_m = g.N * g.OH * g.OW / 128; p.tiles_n = g.O / BN; p.phases = 1;
   if (w_mn ? weight_map(&tmB, w, g.C, 1, g.O, 64) : weight_map(&tmB, w, g.O, g.KH * g.KW, g.C, BN)) return -1;
-  return dispatch_conv(BN, tmA, tmB, p, grid, s);
+  return dispatch_conv(BN, tmA, tmB, p, s);
 }
 
 // conv input gradient = transposed-conv forward, 4x4 s2 p1, in sub-pixel phase form.  w is the STRAIGHT copy [O][16][C]: the reduction runs
@@ -615,8 +659,8 @@ int k_tc_dgrad(const ConvGeom& g, const __nv_bfloat16* dy, const __nv_bfloat16* 
   cuuint32_t es[4] = {1, 1, 1, 1};
   if (weight_map(&tmB, w, g.O, 16, g.C, 64)) return -1;
   if (make_map_bf16(&tmA, dy, 4, dims, strides, box, es)) return -1;
-  dim3 grid((unsigned)(g.N * g.OH * g.OW / 128), (unsigned)(g.C / BN), 4);
-  return dispatch_conv(BN, tmA, tmB, p, grid, s);
+  p.tiles_m = g.N * g.OH * g.OW / 128; p.tiles_n = g.C / BN; p.phases = 4;
+  return dispatch_conv(BN, tmA, tmB, p, s);
 }
 
 // ------------------------------------------------------------------ transposed conv onto <= 4 channels ------
@@ -649,9 +693,9 @@ int k_tc_deconv_ps(const ConvGeom& g, const __nv_bfloat16* dy, const __nv_bfloat
   cuuint32_t box[4] = {64, (cuuint32_t)p.Wt, (cuuint32_t)p.Ht, (cuuint32_t)p.Nt}; cuuint32_t es[4] = {1, 1, 1, 1};
   if (make_map_bf16(&tmA, dy, 4, dims, strides, box, es)) return -1;
   if (weight_map(&tmB, wps, 16, 9, g.O, 16)) return -1;
-  dim3 grid((unsigned)((long)g.N * g.OH * g.OW / 128), 1, 1);
+  p.tiles_m = (int)((long)g.N * g.OH * g.OW / 128); p.tiles_n = 1; p.phases = 1;
   g_tc_last_kernel = "tc_conv_kernel<16,4,PS>";
-  return p.epi == EPI_ACTBWD ? launch_conv_e<16, 4, EPI_ACTBWD, false, true>(tmA, tmB, p, grid, s) : launch_conv_e<16, 4, EPI_PLAIN, false, true>(tmA, tmB, p, grid, s);
+  return p.epi == EPI_ACTBWD ? launch_conv_e<16, 4, EPI_ACTBWD, false, true>(tmA, tmB, p, s) : launch_conv_e<16, 4, EPI_PLAIN, false, true>(tmA, tmB, p, s);
 }
 
 // ------------------------------------------------------------------ conv 4x4 s2 p1 FROM <= 4 image channels ------
