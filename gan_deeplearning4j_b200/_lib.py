@@ -42,9 +42,11 @@ class ConvGeom(C.Structure):
 
 
 class TestConvOpts(C.Structure):
-    """b2g_test_conv_opts: the epilogue a kernel-level parity test asks for, and the name of the kernel that ran."""
+    """b2g_test_conv_opts: the epilogue a kernel-level parity test asks for, the name of the kernel that ran, and the schedule controls
+    (forced tile width, grid cap, output poisoning, [C][O] dense weight operand)."""
     _fields_ = [("epi", C.c_int32), ("act", C.c_int32), ("alpha", C.c_float), ("bias", C.POINTER(C.c_float)), ("scale", C.POINTER(C.c_float)),
-                ("groups", C.c_int32), ("aux", C.POINTER(C.c_float)), ("aux2", C.POINTER(C.c_float)), ("stats", C.POINTER(C.c_double)), ("kernel", C.c_char * 64)]
+                ("groups", C.c_int32), ("aux", C.POINTER(C.c_float)), ("aux2", C.POINTER(C.c_float)), ("stats", C.POINTER(C.c_double)), ("kernel", C.c_char * 64),
+                ("bn", C.c_int32), ("max_ctas", C.c_int32), ("poison", C.c_int32), ("w_mn", C.c_int32)]
 
 
 _vp, _i32, _i64, _fp = C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_float)

@@ -1290,6 +1290,12 @@ extern "C" int32_t b2g_ctx_allreduce_test(b2g_ctx* c, float* host, int64_t n) {
 }
 
 // ------------------------------------------------------------------ kernel-level test hook ----------------
+// The tile-width / grid overrides of tc_conv_kernel hold for the hook's own launch loop only: reset right after it, and on every early return.
+struct TcTestSchedule {
+  TcTestSchedule(int bn, int max_ctas) { g_tc_test_bn = bn; g_tc_test_max_ctas = max_ctas; }
+  ~TcTestSchedule() { reset(); }
+  void reset() { g_tc_test_bn = 0; g_tc_test_max_ctas = 0; }
+};
 extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int32_t precision, const b2g_conv_geom* gg, const float* a_host, const float* b_host, float* out, int32_t iters, float* ms_per_iter,
                                     b2g_test_conv_opts* opt) {
   if (!c || !gg || !a_host || !b_host || !out) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(c->device));
@@ -1304,11 +1310,24 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
     bool ok = kind == 0 ? tc_fprop_supported(g) : kind == 1 ? tc_dgrad_supported(g) : tc_wgrad_supported(g);
     if (!ok) return fail(B2G_ERR_UNSUPPORTED, "no tensor-core kernel for this shape");
   }
-  if (opt && (impl != 1 || kind == 2) && (opt->epi || opt->bias || opt->scale || opt->act)) return fail(B2G_ERR_UNSUPPORTED, "epilogue options apply to the tensor-core fprop / dgrad kernels (impl 1, kind 0 / 1)");
+  const bool tc_conv = impl == 1 && kind != 2, ps = impl == 3 && kind == 1;     // the launches of tc_conv_kernel (ps: its pixel-shuffle form)
+  if (opt && !tc_conv && !ps && (opt->epi || opt->bias || opt->scale || opt->act))
+    return fail(B2G_ERR_UNSUPPORTED, "epilogue options apply to the tensor-core fprop / dgrad kernels (impl 1, kind 0 / 1) and the pixel-shuffle deconv (impl 3, kind 1)");
+  if (opt && ps && (opt->scale || (opt->epi != EPI_PLAIN && opt->epi != EPI_ACTBWD)))
+    return fail(B2G_ERR_UNSUPPORTED, "the pixel-shuffle deconv has bias, activation and the activation-backward epilogue only");
+  const int force_bn = opt ? opt->bn : 0, max_ctas = opt ? opt->max_ctas : 0;
+  const bool poison = opt && opt->poison, w_mn = opt && opt->w_mn;
+  if (force_bn && (!tc_conv || (force_bn != 64 && force_bn != 128) || oc % force_bn))
+    return fail(B2G_ERR_UNSUPPORTED, "bn %d: the tensor-core fprop / dgrad tile is 64 or 128 columns and must divide the %d output channels", force_bn, oc);
+  if (max_ctas < 0 || (max_ctas && !tc_conv && !ps)) return fail(B2G_ERR_UNSUPPORTED, "max_ctas %d: a grid cap applies to tc_conv_kernel launches only", max_ctas);
+  if (poison && kind == 2) return fail(B2G_ERR_UNSUPPORTED, "poison applies to the bf16 outputs of kinds 0 / 1");
+  if (w_mn && (impl != 1 || kind != 0 || g.KH != 1 || g.KW != 1)) return fail(B2G_ERR_UNSUPPORTED, "w_mn: the [C][O] weight operand exists for the 1x1 tensor-core fprop only");
   // impl 2 = the SIMT skinny-layer kernels (kernels_edge.cu), impl 3 = their tensor-core counterparts; both need <= 4 image channels (g.C)
   if (impl == 2 || impl == 3) {
     bool ok = kind == 0 ? edge_conv_small_cin_supported(g) : kind == 1 ? edge_deconv_small_c_supported(g) : edge_wgrad_small_cin_supported(g);
     if (impl == 3) ok = ok && prec == PREC_BF16 && c->tc_ok && (kind == 0 ? tc_edge_conv_supported(g) : kind == 1 ? tc_deconv_ps_supported(g) : tc_edge_wgrad_supported(g));
+    // the training step runs the pixel-shuffle deconv wherever tc_deconv_ps_supported holds, also where the SIMT kernel has no variant (O > 128)
+    if (ps) ok = prec == PREC_BF16 && c->tc_ok && tc_deconv_ps_supported(g);
     if (!ok) return fail(B2G_ERR_UNSUPPORTED, "no skinny-layer kernel (impl %d) for this shape", impl);
   }
   // impl 4 = the dense (1x1 geometry) SIMT kernels: <= 4 output units (D-last) or a short reduction (G-first in its dgrad form)
@@ -1323,7 +1342,7 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   else { CU(cudaMemcpyAsync(ta, fa, 4 * na, cudaMemcpyDeviceToDevice, s)); CU(cudaMemcpyAsync(tb, fb, 4 * nb, cudaMemcpyDeviceToDevice, s)); }
   if (impl == 3 && kind == 1) { CU(cudaMalloc(&wps, 2 * k_tc_deconv_ps_weight_elems(g))); k_pack_deconv_ps(fb, wps, g.O, g.C, s); }
   TcEpi epi{}; const TcEpi* pe = nullptr; const float* bias = nullptr; int act = 0; float alpha = 0.f; int groups = 1;
-  if (opt && impl == 1 && kind != 2) {
+  if (opt && (tc_conv || ps)) {
     groups = opt->groups > 0 ? opt->groups : 1; act = opt->act; alpha = opt->alpha;
     if (opt->bias) { CU(cudaMalloc(&d_bias, 4 * oc)); CU(cudaMemcpyAsync(d_bias, opt->bias, 4 * oc, cudaMemcpyHostToDevice, s)); bias = d_bias; }
     if (opt->scale) { CU(cudaMalloc(&d_scale, 4 * oc)); CU(cudaMemcpyAsync(d_scale, opt->scale, 4 * oc, cudaMemcpyHostToDevice, s)); }
@@ -1342,9 +1361,11 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   cudaEvent_t e0, e1; CU(cudaEventCreate(&e0)); CU(cudaEventCreate(&e1));
   int reps = iters < 1 ? 1 : iters; int rc = 0;
   g_tc_last_kernel = "";
+  TcTestSchedule schedule(force_bn, max_ctas);
   for (int it = -1; it < reps; ++it) {       // it = -1: warm-up
     if (it == 0) CU(cudaEventRecord(e0, s));
     if (d_acc) CU(cudaMemsetAsync(d_acc, 0, 8 * k_bn_acc_elems(oc, groups), s));
+    if (poison) CU(cudaMemsetAsync(to, 0xFF, ts * no, s));       // a tile this launch does not write reads back as NaN, not as the warm-up's values
     if (impl == 4) {
       const bool so = dense_small_o_supported(g);
       if (kind == 0) k_dense_small_o_fwd(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s);
@@ -1353,14 +1374,15 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
     }
     else if (impl >= 2) {
       if (kind == 0) { if (impl == 3) rc = k_tc_edge_conv(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, nullptr, (__nv_bfloat16*)to, 0, 0.f, s); else k_edge_conv_small_cin(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s); }
-      else if (kind == 1) { if (impl == 3) rc = k_tc_deconv_ps(g, (const __nv_bfloat16*)ta, wps, nullptr, (__nv_bfloat16*)to, 0, 0.f, s); else k_edge_deconv_small_c(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s); }
+      else if (kind == 1) { if (impl == 3) rc = k_tc_deconv_ps(g, (const __nv_bfloat16*)ta, wps, bias, (__nv_bfloat16*)to, act, alpha, s, pe); else k_edge_deconv_small_c(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s); }
       else { if (impl == 3) rc = k_tc_edge_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fo, nullptr, scratch, sc, 0, s); else k_edge_wgrad_small_cin(prec, g, ta, tb, fo, scratch, 0, s); }
     }
-    else if (kind == 0) { if (impl) rc = k_tc_fprop(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s, pe); else k_simt_fprop(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s); }
+    else if (kind == 0) { if (impl) rc = k_tc_fprop(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s, pe, w_mn ? 1 : 0); else k_simt_fprop(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s); }
     else if (kind == 1) { if (impl) rc = k_tc_dgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s, pe); else k_simt_dgrad(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s); }
     else { if (impl) rc = k_tc_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fo, scratch, sc, 0, s); else k_simt_wgrad(prec, g, ta, tb, fo, scratch, sc, 0, s); }
     if (rc) break;
   }
+  schedule.reset();
   CU(cudaEventRecord(e1, s));
   if (rc) return fail(B2G_ERR_CUDA, "tensor-core kernel launch failed (%d)", rc);
   if (opt) { strncpy(opt->kernel, g_tc_last_kernel, sizeof(opt->kernel) - 1); opt->kernel[sizeof(opt->kernel) - 1] = 0; }

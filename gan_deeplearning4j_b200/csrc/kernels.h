@@ -186,6 +186,9 @@ bool tc_dgrad_supported(const ConvGeom& g);
 bool tc_wgrad_supported(const ConvGeom& g);
 int  tc_init();   // resolves cuTensorMapEncodeTiled; 0 on success
 extern const char* g_tc_last_kernel;     // which tensor-core kernel the most recent k_tc_* call dispatched (parity tests assert it)
+// Schedule overrides of tc_conv_kernel, set only by the kernel-level test hook around its launches (0 = production choice):
+// g_tc_test_bn forces the 64- or 128-column tile, g_tc_test_max_ctas caps the persistent grid at min(work items, max_ctas)
+extern int g_tc_test_bn, g_tc_test_max_ctas;
 // epilogue of the fprop / dgrad kernels (kernels_tc.cu): what happens between the fp32 accumulator and the bf16 store
 enum { EPI_PLAIN = 0, EPI_STATS = 1, EPI_BNBWD = 2, EPI_ACTBWD = 3 };
 struct TcEpi {

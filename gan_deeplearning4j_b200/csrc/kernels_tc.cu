@@ -541,6 +541,7 @@ __global__ void __launch_bounds__(TC_CONV_THREADS, 1) tc_conv_kernel(const __gri
 
 // ------------------------------------------------------------------ host side ------------------------------
 const char* g_tc_last_kernel = "";       // name of the tensor-core kernel the most recent k_tc_* call dispatched (parity tests assert it)
+int g_tc_test_bn = 0, g_tc_test_max_ctas = 0;   // test-hook schedule overrides (kernels.h); production code never sets them
 static int tc_device() { int dev = 0; cudaGetDevice(&dev); return dev < 0 || dev >= 64 ? 0 : dev; }
 // cudaFuncAttributeMaxDynamicSharedMemorySize is per device: one flag per (kernel, device)
 #define TC_SET_SMEM_ONCE(kernel, bytes)                                                                                            \
@@ -558,6 +559,7 @@ static bool pick_row_tile(int N, int GH, int GW, int rows, int* Nt, int* Ht, int
 static int pick_bn(int OC) { return OC % 128 == 0 ? 128 : OC % 64 == 0 ? 64 : 0; }
 // Small layers (few M tiles) are latency-bound per CTA, not bandwidth-bound: prefer narrower N tiles until the grid covers the SMs.
 static int pick_bn_fill(int OC, long m_tiles_x_phases) {
+  if (g_tc_test_bn) return g_tc_test_bn;
   static int min_ctas = -1; if (min_ctas < 0) { const char* e = getenv("B2G_BN_MIN_CTAS"); min_ctas = e ? atoi(e) : 0; }
   const int target = min_ctas >= 1 ? min_ctas : device_sm_count();
   int bn = pick_bn(OC);
@@ -578,13 +580,13 @@ bool tc_dgrad_supported(const ConvGeom& g) {
 // the fused BatchNorm epilogues need every 128-row tile inside one statistics group
 static bool tc_epi_ok(const TcEpi* e, int Nt) { return !e || e->mode == EPI_PLAIN || e->mode == EPI_ACTBWD || (e->imgs_per_group > 0 && e->imgs_per_group % Nt == 0 && e->acc); }
 
-// persistent grid: one CTA per SM, or one per work item when there are fewer
+// persistent grid: one CTA per SM, or one per work item when there are fewer (a test may cap it at g_tc_test_max_ctas instead)
 template <int BN, int STAGES, int EPI, bool AFFINE, bool PS = false>
 static int launch_conv_e(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, cudaStream_t s) {
   using S = TcSmem<BN, STAGES, EPI>;
   TC_SET_SMEM_ONCE((tc_conv_kernel<BN, STAGES, EPI, AFFINE, PS>), S::TOTAL);
   const long tiles = (long)p.tiles_m * p.tiles_n * p.phases;
-  const unsigned grid = (unsigned)std::min<long>(tiles, device_sm_count());
+  const unsigned grid = (unsigned)std::min<long>(tiles, g_tc_test_max_ctas > 0 ? g_tc_test_max_ctas : device_sm_count());
   launch_pdl(tc_conv_kernel<BN, STAGES, EPI, AFFINE, PS>, dim3(grid), dim3(TC_CONV_THREADS), (size_t)(S::TOTAL), s, tmA, tmB, p);
   LAUNCHED();
   return cudaPeekAtLastError() == cudaSuccess ? 0 : -3;

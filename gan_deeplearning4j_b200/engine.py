@@ -360,14 +360,19 @@ EPI_PLAIN, EPI_STATS, EPI_BNBWD, EPI_ACTBWD = 0, 1, 2, 3
 
 
 def test_conv_ex(ctx: Context, kind: int, geom: Dict[str, int], a, b, out_size: int, *, epi: int = 0, act: str = "identity", alpha: float = 0.0,
-                 bias=None, scale=None, groups: int = 1, aux=None, aux2=None, iters: int = 1):
-    """Tensor-core fprop (kind 0) / dgrad (kind 1) with the epilogue the training step uses.  Returns (out, stats or None, kernel name, ms)."""
+                 bias=None, scale=None, groups: int = 1, aux=None, aux2=None, iters: int = 1, impl: int = 1, bn: int = 0, max_ctas: int = 0,
+                 poison: bool = False, w_mn: bool = False):
+    """Tensor-core fprop (kind 0) / dgrad (kind 1) with the epilogue the training step uses (impl 3, kind 1: the pixel-shuffle deconv, b = the
+    [O][4][4][C] weight).  bn forces the 64- / 128-column tile, max_ctas caps the persistent grid (0: production choice for both); poison
+    fills the output with bf16 NaN before every launch; w_mn (kind 0, 1x1): b is the [C][O] dense weight.
+    Returns (out, stats or None, kernel name, ms)."""
     g = _lib.ConvGeom(**geom)
     a, b = _f32(a).ravel(), _f32(b).ravel()
     out = np.empty(out_size, np.float32)
     oc = geom["o"] if kind == 0 else geom["c"]
     o = _lib.TestConvOpts()
     o.epi, o.act, o.alpha, o.groups = epi, ACTS[act], alpha, groups
+    o.bn, o.max_ctas, o.poison, o.w_mn = bn, max_ctas, int(poison), int(w_mn)
     keep = []
     for name, v in (("bias", bias), ("scale", scale), ("aux", aux), ("aux2", aux2)):
         if v is not None:
@@ -376,7 +381,7 @@ def test_conv_ex(ctx: Context, kind: int, geom: Dict[str, int], a, b, out_size: 
     if epi in (EPI_STATS, EPI_BNBWD):
         stats = np.zeros((groups, 2, oc), np.float64); o.stats = stats.ctypes.data_as(C.POINTER(C.c_double))
     ms = C.c_float()
-    check(ctx.lib.b2g_test_conv_ex(ctx.h, kind, 1, BF16, C.byref(g), _fp(a), _fp(b), _fp(out), iters, C.byref(ms), C.byref(o)))
+    check(ctx.lib.b2g_test_conv_ex(ctx.h, kind, impl, BF16, C.byref(g), _fp(a), _fp(b), _fp(out), iters, C.byref(ms), C.byref(o)))
     return out, stats, o.kernel.decode(), ms.value
 
 

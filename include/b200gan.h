@@ -265,8 +265,10 @@ typedef struct {
 int32_t b2g_test_conv(b2g_ctx* ctx, int32_t kind, int32_t impl, int32_t precision, const b2g_conv_geom* g,
                       const float* x_or_dy, const float* w_or_x, float* out, int32_t iters, float* ms_per_iter);
 /* The same with the epilogue the training step actually uses (impl 1, kind 0 / 1): bias, folded inference-BatchNorm scale, activation,
- * and the fused BatchNorm epilogues of kernels_tc.cu.  `kernel` returns the name of the tensor-core kernel that was dispatched, so a parity
- * test can assert that it exercised the variant the benchmark runs (persistent MT=2, one-wave split-K, ...). */
+ * and the fused BatchNorm epilogues of kernels_tc.cu; for the pixel-shuffle deconv (impl 3, kind 1) bias, activation and the
+ * activation-backward epilogue.  `kernel` returns the name of the tensor-core kernel that was dispatched, so a parity test can assert
+ * that it exercised the variant the benchmark runs.  bn / max_ctas / poison / w_mn let a test pin the tile width and the grid of the
+ * persistent kernel, see every element the measured launch left unwritten, and reach the dense input-gradient operand layout. */
 typedef struct {
   int32_t epi;            /* 0 plain; 1 + statistics (sum, sum of squares per group and channel) of the stored outputs;
                              2 BatchNorm-backward epilogue: out = acc * act'(aux) (aux = the BatchNorm+activation output y), statistics sum out, sum out*aux2
@@ -280,6 +282,11 @@ typedef struct {
   const float* aux2;      /* epi 2: the BatchNorm input z (same shape) */
   double* stats;          /* out (epi 1 / 2): [groups][2][C_out] */
   char kernel[64];        /* out */
+  /* Schedule controls of the persistent tensor-core conv kernel (impl 1 kind 0 / 1, and impl 3 kind 1 where noted); 0 = production. */
+  int32_t bn;             /* impl 1: force the 64- or 128-column tile (B2G_ERR_UNSUPPORTED unless C_out is a multiple of it) */
+  int32_t max_ctas;       /* impl 1 / impl 3 kind 1: grid = min(work items, max_ctas) instead of min(work items, SMs); may exceed the SM count */
+  int32_t poison;         /* kinds 0 / 1: fill the output with 0xFF bytes (bf16 NaN) before every launch, warm-up included */
+  int32_t w_mn;           /* impl 1 kind 0, 1x1 geometry: the weight operand is [C][O] (the dense input gradient's own [nOut][nIn] weight) */
 } b2g_test_conv_opts;
 int32_t b2g_test_conv_ex(b2g_ctx* ctx, int32_t kind, int32_t impl, int32_t precision, const b2g_conv_geom* g,
                          const float* x_or_dy, const float* w_or_x, float* out, int32_t iters, float* ms_per_iter, b2g_test_conv_opts* opts);

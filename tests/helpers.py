@@ -88,11 +88,16 @@ def bf16_round(a):
 
 def check_bf16(got, ref, what):
     """A bf16 tensor against its float64 reference: |got - ref| <= 2^-8 |ref| + 2e-3 rms(ref) elementwise (one bf16 rounding is 2^-9
-    relative; the rms term absorbs fp32 accumulation order on elements that cancel)."""
+    relative; the rms term absorbs fp32 accumulation order on elements that cancel).  A non-finite element of got fails."""
     got = np.asarray(got, np.float64); ref = np.asarray(ref, np.float64)
     tol = 2.0 ** -8 * np.abs(ref) + 2e-3 * np.sqrt(np.mean(ref ** 2)) + 1e-30
-    bad = np.abs(got - ref) > tol
-    assert not bad.any(), f"{what}: {bad.sum()} of {bad.size} elements outside 2^-8|ref| + 2e-3 rms; worst |d|={np.abs(got - ref).max():.4g} rms={np.sqrt(np.mean(ref ** 2)):.4g}"
+    d = np.abs(got - ref)
+    bad = ~(d <= tol)          # NaN compares False: a NaN or inf in got (or ref) is an error, not a pass
+    if bad.any():
+        fin = np.isfinite(d)
+        worst = d[fin].max() if fin.any() else float("nan")
+        raise AssertionError(f"{what}: {bad.sum()} of {bad.size} elements outside 2^-8|ref| + 2e-3 rms ({(~np.isfinite(got)).sum()} non-finite); "
+                             f"worst finite |d|={worst:.4g} rms={np.sqrt(np.mean(ref ** 2)):.4g}")
 
 
 def inject_forward(onet, bnet, specs, x_in, batch, what):

@@ -50,12 +50,16 @@ def test_struct_layouts_match_the_c_header(tmp_path):
     prog = tmp_path / "layout.c"
     prog.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "b200gan.h"\nint main(){'
                     'printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(b2g_layer_desc), offsetof(b2g_layer_desc,n_in), offsetof(b2g_layer_desc,updater),'
-                    ' offsetof(b2g_layer_desc,pre_c), sizeof(b2g_net_config), offsetof(b2g_net_config,seed), sizeof(b2g_gan_config), sizeof(b2g_conv_geom), offsetof(b2g_net_config,bn_groups));return 0;}')
+                    ' offsetof(b2g_layer_desc,pre_c), sizeof(b2g_net_config), offsetof(b2g_net_config,seed), sizeof(b2g_gan_config), sizeof(b2g_conv_geom), offsetof(b2g_net_config,bn_groups));'
+                    'printf("%zu %zu %zu %zu %zu %zu %zu\\n", sizeof(b2g_test_conv_opts), offsetof(b2g_test_conv_opts,stats), offsetof(b2g_test_conv_opts,kernel),'
+                    ' offsetof(b2g_test_conv_opts,bn), offsetof(b2g_test_conv_opts,max_ctas), offsetof(b2g_test_conv_opts,poison), offsetof(b2g_test_conv_opts,w_mn));return 0;}')
     exe = tmp_path / "layout"
     subprocess.run(["gcc", "-I", os.path.join(ROOT, "include"), str(prog), "-o", str(exe)], check=True)
     got = [int(v) for v in subprocess.run([str(exe)], capture_output=True, text=True).stdout.split()]
-    L, N = _lib.LayerDesc, _lib.NetConfig
-    assert got == [C.sizeof(L), L.n_in.offset, L.updater.offset, L.pre_c.offset, C.sizeof(N), N.seed.offset, C.sizeof(_lib.GanConfig), C.sizeof(_lib.ConvGeom), N.bn_groups.offset]
+    L, N, T = _lib.LayerDesc, _lib.NetConfig, _lib.TestConvOpts
+    assert got == [C.sizeof(L), L.n_in.offset, L.updater.offset, L.pre_c.offset, C.sizeof(N), N.seed.offset, C.sizeof(_lib.GanConfig), C.sizeof(_lib.ConvGeom), N.bn_groups.offset,
+                   C.sizeof(T), T.stats.offset, T.kernel.offset, T.bn.offset, T.max_ctas.offset, T.poison.offset, T.w_mn.offset]
+    assert (T.stats.offset, T.kernel.offset) == (56, 64)         # the fields older callers fill keep their offsets
 
 
 def test_no_device_fails_loudly_not_silently(lib):

@@ -6,16 +6,21 @@ which kernel ran (asserted), and the result is compared with the CPU oracle (ora
 semantics) on the same bf16-rounded operands:
     bf16 outputs:  |got - ref| <= 2^-8 |ref| + 2e-3 rms(ref)        (one bf16 rounding is 2^-9 relative; fp32 accumulation order)
     fp32 wgrad:    max|got - ref| <= 1e-4 max|ref|
-The oracle evaluates whole sampled images (first / last, a few in the middle, the real|fake group boundary) for
-fprop / dgrad, and the full batch in image chunks (the weight gradient is a sum over images) for wgrad.
+The tensor-core fprop / dgrad GEMMs are compared on every element of the whole batch with the float64 reference of tests/conv_ref.py
+(pinned to the oracle by tests/test_conv_ref.py), on an output poisoned with NaN before the launch, and their production epilogue is
+re-run at one CTA and at one CTA per tile (bit-identical).  The oracle evaluates whole sampled images (first / last, a few in the middle,
+the real|fake group boundary) for the edge kernels, and the full batch in image chunks (the weight gradient is a sum over images) for wgrad.
 """
 import copy
 
 import numpy as np
 import pytest
 
+import conv_ref
+import tc_schedule
 from helpers import bf16_round, check_bf16, inject_forward
 from oracle import dl4j_oracle as o
+from tc_schedule import pick_row_tile as _pick_row_tile
 
 pytestmark = pytest.mark.gpu
 
@@ -46,14 +51,38 @@ def act_fwd(name, z, alpha):
     return {"identity": lambda: z, "relu": lambda: np.maximum(z, 0), "lrelu": lambda: np.where(z > 0, z, alpha * z), "tanh": lambda: np.tanh(z)}[name]()
 
 
-# (name, batch, conv-input size h, c, o, expected kernel)   -- conv geometry 4x4 s2 p1: x [n,h,h,c] -> y [n,h/2,h/2,o]
+_REF = {}
+
+
+def _full_ref(key, fn):
+    """float64 GEMM of a whole batch (conv_ref), computed once per shape: every epilogue of a case shares its operands."""
+    if key not in _REF:
+        _REF[key] = fn()
+    return _REF[key]
+
+
+def _check_schedule_invariance(b, ctx, kind, g, a, wt, size, kw, out, stats, kernel, what):
+    """The production epilogue of a shape once more at one CTA (every tile through one CTA's rings and park slots) and at one CTA per tile:
+    output and statistics bit-identical to the production grid's."""
+    bn = int(kernel.split("<")[1].split(",")[0])
+    geo = tc_schedule.geometry("fprop" if kind == 0 else "dgrad", g["n"], g["h"], g["w"], g["c"], g["o"], 4, 2, 1, bn)
+    for mc in (1, geo["tiles"]):
+        o2, s2, k2, _ = b.test_conv_ex(ctx, kind, g, a, wt, size, poison=True, max_ctas=mc, **kw)
+        assert k2 == kernel, (what, mc, k2)
+        assert np.array_equal(o2.view(np.uint32), out.view(np.uint32)), f"{what}: max_ctas={mc} output differs from the production grid's"
+        if stats is not None:
+            assert np.array_equal(s2, stats), f"{what}: max_ctas={mc} statistics differ from the production grid's"
+
+
+# (name, batch, conv-input size h, c, o, expected kernel, the epilogue the step runs this GEMM with)
+# conv geometry 4x4 s2 p1: x [n,h,h,c] -> y [n,h/2,h/2,o]
 FPROP = [
-    ("D2 fprop, D step (2N, real|fake)", 2 * N, 32, 64, 128, "tc_conv_kernel<128,4>"),
-    ("D3 fprop, D step", 2 * N, 16, 128, 256, "tc_conv_kernel<128,4>"),
-    ("D4 fprop, D step", 2 * N, 8, 256, 512, "tc_conv_kernel<64,4>"),
-    ("D2 fprop, G step / G4 input gradient", N, 32, 64, 128, "tc_conv_kernel<128,4>"),
-    ("D3 fprop, G step / G3 input gradient", N, 16, 128, 256, "tc_conv_kernel<64,4>"),
-    ("D4 fprop, G step / G2 input gradient", N, 8, 256, 512, "tc_conv_kernel<64,4>"),
+    ("D2 fprop, D step (2N, real|fake)", 2 * N, 32, 64, 128, "tc_conv_kernel<128,4>", "stats"),
+    ("D3 fprop, D step", 2 * N, 16, 128, 256, "tc_conv_kernel<128,4>", "stats"),
+    ("D4 fprop, D step", 2 * N, 8, 256, 512, "tc_conv_kernel<64,4>", "stats"),
+    ("D2 fprop, G step / G4 input gradient", N, 32, 64, 128, "tc_conv_kernel<128,4>", "bnbwd_relu"),
+    ("D3 fprop, G step / G3 input gradient", N, 16, 128, 256, "tc_conv_kernel<64,4>", "bnbwd_relu"),
+    ("D4 fprop, G step / G2 input gradient", N, 8, 256, 512, "tc_conv_kernel<64,4>", "bnbwd_relu"),
 ]
 
 
@@ -61,49 +90,52 @@ FPROP = [
 @pytest.mark.parametrize("epi", ["stats", "bnbwd_relu", "plain_bias_lrelu"])
 def test_fprop_production_dispatch(b200, case, epi):
     """conv forward (D2-D4) with the BatchNorm statistics epilogue, and the same kernel as the generator's input-gradient GEMM with the
-    BatchNorm-backward epilogue (J:197-199 BatchNormalization + ReLU below each transposed conv)."""
+    BatchNorm-backward epilogue (J:197-199 BatchNormalization + ReLU below each transposed conv).  Every element of the whole batch against
+    the float64 reference; the output is poisoned (bf16 NaN) before each launch, so an unwritten tile fails."""
     b, ctx = b200
-    name, n, h, c, oc, kernel = case
+    name, n, h, c, oc, kernel, prod_epi = case
     rng = np.random.default_rng(11)
     x = bf16_round(rng.standard_normal((n, h, h, c))); wt = bf16_round(rng.standard_normal((oc, 4, 4, c)) / np.sqrt(16 * c))
     g = geom_of(n, h, c, oc); oh = h // 2
     groups = 2 if n == 2 * N else 1
-    idx = sample_images(n)
-    lay = conv_layer(c, oc, wt.transpose(0, 3, 1, 2))
-    ref = lay.forward(x[idx].transpose(0, 3, 1, 2).astype(np.float64), True).transpose(0, 2, 3, 1)        # [len(idx), oh, oh, oc]
+    ref = _full_ref(("fprop", name), lambda: conv_ref.conv2d(x, wt, 2, 1))        # [n, oh, oh, oc]
+    size = n * oh * oh * oc
     if epi == "stats":
-        out, stats, k, _ = b.test_conv_ex(ctx, 0, g, x, wt, n * oh * oh * oc, epi=b.EPI_STATS, groups=groups)
-        out = out.reshape(n, oh, oh, oc)
-        check_bf16(out[idx], ref, name)
+        kw = dict(epi=b.EPI_STATS, groups=groups)
+        out, stats, k, _ = b.test_conv_ex(ctx, 0, g, x, wt, size, poison=True, **kw)
+        check_bf16(out.reshape(n, oh, oh, oc), ref, name)
         # the statistics are those of the STORED bf16 tensor, per (group, channel): exact up to fp32 summation order inside a 128-row tile
         og = out.reshape(groups, -1, oc).astype(np.float64)
         np.testing.assert_allclose(stats[:, 0, :], og.sum(1), rtol=2e-5, atol=2e-3)
         np.testing.assert_allclose(stats[:, 1, :], (og ** 2).sum(1), rtol=2e-5, atol=2e-3)
     elif epi == "plain_bias_lrelu":
         bias = rng.standard_normal(oc).astype(np.float32) * 0.1
-        out, _, k, _ = b.test_conv_ex(ctx, 0, g, x, wt, n * oh * oh * oc, act="lrelu", alpha=0.2, bias=bias)
-        check_bf16(out.reshape(n, oh, oh, oc)[idx], act_fwd("lrelu", ref + bias.astype(np.float64), 0.2), name)
+        kw = dict(act="lrelu", alpha=0.2, bias=bias)
+        out, stats, k, _ = b.test_conv_ex(ctx, 0, g, x, wt, size, poison=True, **kw)
+        check_bf16(out.reshape(n, oh, oh, oc), act_fwd("lrelu", ref + bias.astype(np.float64), 0.2), name)
     else:
         # the GEMM result is the epsilon w.r.t. the output y of BatchNorm+ReLU; z = that BatchNorm's input: out = eps * relu'(y), statistics sum out, sum out*z
         z = bf16_round(rng.standard_normal((n, oh, oh, oc)))
         y = bf16_round(np.maximum(z * rng.uniform(0.5, 1.5, oc) + rng.standard_normal(oc) * 0.3, 0))
-        out, stats, k, _ = b.test_conv_ex(ctx, 0, g, x, wt, n * oh * oh * oc, epi=b.EPI_BNBWD, act="relu", groups=groups, aux=y, aux2=z)
-        out = out.reshape(n, oh, oh, oc)
-        check_bf16(out[idx], ref * (y[idx] > 0), name)
+        kw = dict(epi=b.EPI_BNBWD, act="relu", groups=groups, aux=y, aux2=z)
+        out, stats, k, _ = b.test_conv_ex(ctx, 0, g, x, wt, size, poison=True, **kw)
+        check_bf16(out.reshape(n, oh, oh, oc), ref * (y > 0), name)
         zg = z.reshape(groups, -1, oc).astype(np.float64); og = out.reshape(groups, -1, oc).astype(np.float64)
         np.testing.assert_allclose(stats[:, 0, :], og.sum(1), rtol=2e-5, atol=2e-3)
         np.testing.assert_allclose(stats[:, 1, :], (og * zg).sum(1), rtol=2e-5, atol=5e-3)
     assert k == kernel, f"{name}: dispatched {k}, the C2 step is expected to run {kernel}"
+    if epi == prod_epi:
+        _check_schedule_invariance(b, ctx, 0, g, x, wt, size, kw, out, stats, kernel, name)
 
 
 # conv geometry: dy [n,h/2,h/2,o] -> dx [n,h,h,c]  (= transposed-conv forward o -> c)
 DGRAD = [
-    ("D2 dgrad, D step (2N)", 2 * N, 32, 64, 128, "tc_conv_kernel<64,4>"),
-    ("D3 dgrad, D step", 2 * N, 16, 128, 256, "tc_conv_kernel<128,4>"),
-    ("D4 dgrad, D step", 2 * N, 8, 256, 512, "tc_conv_kernel<128,4>"),
-    ("G4 forward / D2 dgrad, G step (N)", N, 32, 64, 128, "tc_conv_kernel<64,4>"),
-    ("G3 forward / D3 dgrad, G step", N, 16, 128, 256, "tc_conv_kernel<128,4>"),
-    ("G2 forward / D4 dgrad, G step", N, 8, 256, 512, "tc_conv_kernel<64,4>"),
+    ("D2 dgrad, D step (2N)", 2 * N, 32, 64, 128, "tc_conv_kernel<64,4>", "actbwd_lrelu"),
+    ("D3 dgrad, D step", 2 * N, 16, 128, 256, "tc_conv_kernel<128,4>", "bnbwd_lrelu"),
+    ("D4 dgrad, D step", 2 * N, 8, 256, 512, "tc_conv_kernel<128,4>", "bnbwd_lrelu"),
+    ("G4 forward / D2 dgrad, G step (N)", N, 32, 64, 128, "tc_conv_kernel<64,4>", "stats"),
+    ("G3 forward / D3 dgrad, G step", N, 16, 128, 256, "tc_conv_kernel<128,4>", "stats"),
+    ("G2 forward / D4 dgrad, G step", N, 8, 256, 512, "tc_conv_kernel<64,4>", "stats"),
 ]
 
 
@@ -112,43 +144,46 @@ DGRAD = [
 def test_dgrad_production_dispatch(b200, case, epi):
     """Deconvolution2D forward = conv input gradient in sub-pixel phase form, weights read as MN-major tiles from the straight [O][16][C] copy:
     train-mode generator forward (statistics epilogue), inference-mode generator forward (folded BatchNorm + ReLU: gen.output, J:420),
-    discriminator input gradients with the BatchNorm-backward / LeakyReLU-backward epilogues."""
+    discriminator input gradients with the BatchNorm-backward / LeakyReLU-backward epilogues.  Whole batch, poisoned output, as above."""
     b, ctx = b200
-    name, n, h, c, oc, kernel = case
+    name, n, h, c, oc, kernel, prod_epi = case
     rng = np.random.default_rng(12)
     dy = bf16_round(rng.standard_normal((n, h // 2, h // 2, oc))); wt = bf16_round(rng.standard_normal((oc, 4, 4, c)) / np.sqrt(4 * oc))
     g = geom_of(n, h, c, oc)
     groups = 2 if n == 2 * N else 1
-    idx = sample_images(n)
-    lay = conv_layer(c, oc, wt.transpose(0, 3, 1, 2))
-    lay.forward(np.zeros((len(idx), c, h, h)), True)
-    ref = lay.backward(dy[idx].transpose(0, 3, 1, 2).astype(np.float64)).transpose(0, 2, 3, 1)           # [len(idx), h, h, c]
+    ref = _full_ref(("dgrad", name), lambda: conv_ref.conv2d_input_grad(dy, wt, (h, h), 2, 1))     # [n, h, h, c]
     size = n * h * h * c
+    stats = None
     if epi == "stats":
-        out, stats, k, _ = b.test_conv_ex(ctx, 1, g, dy, wt, size, epi=b.EPI_STATS, groups=groups)
-        out = out.reshape(n, h, h, c); check_bf16(out[idx], ref, name)
+        kw = dict(epi=b.EPI_STATS, groups=groups)
+        out, stats, k, _ = b.test_conv_ex(ctx, 1, g, dy, wt, size, poison=True, **kw)
+        check_bf16(out.reshape(n, h, h, c), ref, name)
         og = out.reshape(groups, -1, c).astype(np.float64)
         np.testing.assert_allclose(stats[:, 0, :], og.sum(1), rtol=2e-5, atol=2e-3)
         np.testing.assert_allclose(stats[:, 1, :], (og ** 2).sum(1), rtol=2e-5, atol=2e-3)
     elif epi == "affine_relu":
         scale = rng.uniform(0.5, 1.5, c).astype(np.float32); shift = (rng.standard_normal(c) * 0.2).astype(np.float32)
-        out, _, k, _ = b.test_conv_ex(ctx, 1, g, dy, wt, size, act="relu", bias=shift, scale=scale)
-        check_bf16(out.reshape(n, h, h, c)[idx], act_fwd("relu", ref * scale.astype(np.float64) + shift.astype(np.float64), 0.0), name)
+        kw = dict(act="relu", bias=shift, scale=scale)
+        out, _, k, _ = b.test_conv_ex(ctx, 1, g, dy, wt, size, poison=True, **kw)
+        check_bf16(out.reshape(n, h, h, c), act_fwd("relu", ref * scale.astype(np.float64) + shift.astype(np.float64), 0.0), name)
     elif epi == "actbwd_lrelu":
         a = bf16_round(rng.standard_normal((n, h, h, c)))
-        out, _, k, _ = b.test_conv_ex(ctx, 1, g, dy, wt, size, epi=b.EPI_ACTBWD, act="lrelu", alpha=0.2, aux=a)
-        check_bf16(out.reshape(n, h, h, c)[idx], ref * np.where(a[idx] > 0, 1.0, 0.2), name)
+        kw = dict(epi=b.EPI_ACTBWD, act="lrelu", alpha=0.2, aux=a)
+        out, _, k, _ = b.test_conv_ex(ctx, 1, g, dy, wt, size, poison=True, **kw)
+        check_bf16(out.reshape(n, h, h, c), ref * np.where(a > 0, 1.0, 0.2), name)
     else:
         z = bf16_round(rng.standard_normal((n, h, h, c)))
         u = z * rng.uniform(0.5, 1.5, c) + rng.standard_normal(c) * 0.3
         y = bf16_round(np.where(u > 0, u, 0.2 * u))
-        out, stats, k, _ = b.test_conv_ex(ctx, 1, g, dy, wt, size, epi=b.EPI_BNBWD, act="lrelu", alpha=0.2, groups=groups, aux=y, aux2=z)
-        out = out.reshape(n, h, h, c)
-        check_bf16(out[idx], ref * np.where(y[idx] > 0, 1.0, 0.2), name)
+        kw = dict(epi=b.EPI_BNBWD, act="lrelu", alpha=0.2, groups=groups, aux=y, aux2=z)
+        out, stats, k, _ = b.test_conv_ex(ctx, 1, g, dy, wt, size, poison=True, **kw)
+        check_bf16(out.reshape(n, h, h, c), ref * np.where(y > 0, 1.0, 0.2), name)
         zg = z.reshape(groups, -1, c).astype(np.float64); og = out.reshape(groups, -1, c).astype(np.float64)
         np.testing.assert_allclose(stats[:, 0, :], og.sum(1), rtol=2e-5, atol=2e-3)
         np.testing.assert_allclose(stats[:, 1, :], (og * zg).sum(1), rtol=2e-5, atol=5e-3)
     assert k == kernel, f"{name}: dispatched {k}, the C2 step is expected to run {kernel}"
+    if epi == prod_epi:
+        _check_schedule_invariance(b, ctx, 1, g, dy, wt, size, kw, out, stats, kernel, name)
 
 
 WGRAD = [
@@ -346,18 +381,6 @@ def test_dense_kernels(b200, case):
 # k_bn_stats_acc / k_bn_bwd_stats_acc, take over.  DCGAN 32x32, nf = 64, z = 16 (every channel count tensor-core eligible), per-net batches
 # N in {1, 3, 4, 8}: between them the layers of one step take all three routes.
 # ------------------------------------------------------------------------------------------------
-def _pick_row_tile(n, gh, gw, rows=128):
-    """Python mirror of kernels_tc.cu pick_row_tile: images per 128-row tile, or None when the batch has no tile."""
-    p = gh * gw
-    if gw > rows or rows % gw:
-        return None
-    if p >= rows:
-        return 1 if p % rows == 0 and gh % (rows // gw) == 0 else None
-    if rows % p or n % (rows // p):
-        return None
-    return rows // p
-
-
 SWEEP_SIZE, SWEEP_Z, SWEEP_NF = 32, 16, 64
 
 
