@@ -11,7 +11,7 @@ namespace b2g {
 
 #define LAUNCHED() do { ++::b2g::g_launch_count; } while (0)
 
-// Programmatic dependent launch (default on; B2G_PDL=0 disables): a kernel launched with the attribute may be SCHEDULED while its predecessor in the stream is
+// Programmatic dependent launch (launch_pdl sets the attribute on every launch): a kernel launched with the attribute may be SCHEDULED while its predecessor in the stream is
 // still running (as soon as every predecessor CTA has exited or called pdl_trigger()), so the ~2 us launch latency and the successor's
 // prologue overlap the predecessor's tail; pdl_wait() -- the first thing every kernel of this library does before touching global memory --
 // blocks until the predecessor has completed and flushed.  An early trigger in a multi-wave kernel lets waiting successor CTAs hold SM
@@ -21,13 +21,11 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 // elementwise / reduction kernels: their grids are one wave (<= 8 blocks of 256 threads per SM), so they let the successor in at once
 __device__ __forceinline__ void pdl_enter() { pdl_trigger(); pdl_wait(); }
-extern int g_pdl_enabled;     // -1 unknown, 0 off, 1 on
-inline bool pdl_on() { if (g_pdl_enabled < 0) { const char* e = getenv("B2G_PDL"); g_pdl_enabled = (e && e[0] == '0') ? 0 : 1; } return g_pdl_enabled == 1; }
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
   cudaLaunchConfig_t cfg{}; cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = stream;
   cudaLaunchAttribute at[1]; at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = pdl_on() ? 1 : 0;
+  cfg.attrs = at; cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 

@@ -247,7 +247,7 @@ static int32_t net_build(b2g_net* n, const b2g_layer_desc* layers, int32_t nl) {
     }
     l.out_elems = (size_t)l.oh * l.ow * l.oc;
     if (l.has_gemm() && n->prec == PREC_BF16) { l.off_W_bf = off_bf; off_bf += l.n_W; off_bf = (off_bf + 63) / 64 * 64;
-      if (n->ctx->tc_ok && tc_deconv_ps_shape(l.geom) && !getenv("B2G_NO_TC_EDGE")) { l.off_Wps_bf = off_bf; off_bf += (int64_t)k_tc_deconv_ps_weight_elems(l.geom); off_bf = (off_bf + 63) / 64 * 64; } }
+      if (n->ctx->tc_ok && tc_deconv_ps_shape(l.geom)) { l.off_Wps_bf = off_bf; off_bf += (int64_t)k_tc_deconv_ps_weight_elems(l.geom); off_bf = (off_bf + 63) / 64 * 64; } }
     h = l.oh; w = l.ow; ch = l.oc;
     n->L.push_back(l);
   }
@@ -422,9 +422,7 @@ static const void* w_ptr(const b2g_net* n, const LayerRT& l, int* wprec) {
   *wprec = PREC_F32; return n->params + l.off_W;
 }
 
-// tensor-core versions of the <= 4-image-channel layers (B2G_NO_TC_EDGE=1 keeps the SIMT kernels of kernels_edge.cu)
 static inline bool tc_on(const b2g_net* n) { return n->prec == PREC_BF16 && n->ctx->tc_ok; }
-static bool tc_edge_on(const b2g_net* n) { static int on = -1; if (on < 0) on = getenv("B2G_NO_TC_EDGE") ? 0 : 1; return on && tc_on(n); }
 static inline cudaStream_t fstream(const b2g_net* n) { return n->fwd_stream ? n->fwd_stream : n->ctx->stream; }
 // A BF16 net whose GEMM-shaped op has no tensor-core kernel runs it on the SIMT kernels: counted (b2g_net_simt_gemm_calls, bench.py prints
 // it per step) so that a shape falling off the tensor-core path is visible, never silent.  The by-design skinny layers (<= 4 units on one
@@ -443,7 +441,7 @@ static int32_t gemm_fprop(b2g_net* n, const LayerRT& l, const ConvGeom& g, const
     if (tc_on(n) && tc_fprop_supported(g)) { TcEpi e{}; e.mode = EPI_PLAIN; e.scale = scale; return k_tc_fprop(g, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)out, act, alpha, s, &e) == 0 ? 0 : fail(B2G_ERR_CUDA, "tensor-core fprop launch failed"); }
     note_simt(n); k_simt_fprop(n->prec, wp, g, x, w, bias, out, act, alpha, s, scale); return 0;
   }
-  if (tc_edge_on(n) && tc_edge_conv_supported(g) && k_tc_edge_conv(g, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)out, act, alpha, s) == 0) return 0;
+  if (tc_on(n) && tc_edge_conv_supported(g) && k_tc_edge_conv(g, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)out, act, alpha, s) == 0) return 0;
   if (edge_conv_small_cin_supported(g)) { note_simt(n); k_edge_conv_small_cin(n->prec, wp, g, x, w, bias, out, act, alpha, s); return 0; }
   if (dense_small_o_supported(g)) { note_simt(n); k_dense_small_o_fwd(n->prec, wp, g, x, w, bias, out, act, alpha, s); return 0; }
   if (tc_on(n) && tc_fprop_supported(g)) {
@@ -461,7 +459,7 @@ static int32_t gemm_dgrad(b2g_net* n, const LayerRT& l, const ConvGeom& g, const
     if (tc_on(n) && tc_dgrad_supported(g) && !edge_deconv_small_c_supported(g)) { TcEpi e{}; e.mode = EPI_PLAIN; e.scale = scale; return k_tc_dgrad(g, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)dx, act, alpha, s, &e) == 0 ? 0 : fail(B2G_ERR_CUDA, "tensor-core dgrad launch failed"); }
     note_simt(n); k_simt_dgrad(n->prec, wp, g, dy, w, bias, dx, act, alpha, s, scale); return 0;
   }
-  if (tc_edge_on(n) && l.off_Wps_bf >= 0 && tc_deconv_ps_supported(g)) {
+  if (tc_on(n) && l.off_Wps_bf >= 0 && tc_deconv_ps_supported(g)) {
     const TcEpi* f = (fuse && fuse->mode == EPI_ACTBWD) ? fuse : nullptr;
     if (k_tc_deconv_ps(g, (const __nv_bfloat16*)dy, n->shadow + l.off_Wps_bf, bias, (__nv_bfloat16*)dx, act, alpha, s, f) == 0) { if (fused) *fused = f != nullptr; return 0; }
     return fail(B2G_ERR_CUDA, "tensor-core pixel-shuffle deconv launch failed");
@@ -486,7 +484,7 @@ static int32_t gemm_dgrad(b2g_net* n, const LayerRT& l, const ConvGeom& g, const
   note_simt(n); k_simt_dgrad(n->prec, wp, g, dy, w, bias, dx, act, alpha, s); return 0;
 }
 static int32_t gemm_wgrad(b2g_net* n, LayerRT& l, const ConvGeom& g, const void* x, const void* dy, float* dw, cudaStream_t s, float* scratch, float* db = nullptr, bool* bias_done = nullptr) {
-  if (tc_edge_on(n) && tc_edge_wgrad_supported(g) && l.wg_part) { const int r = k_tc_edge_wgrad(g, (const __nv_bfloat16*)x, (const __nv_bfloat16*)dy, dw, db, l.wg_part, l.wg_part_floats, 0, s, &n->pending); if (r >= 0) { if (bias_done) *bias_done = r == 1; return 0; } }
+  if (tc_on(n) && tc_edge_wgrad_supported(g) && l.wg_part) { const int r = k_tc_edge_wgrad(g, (const __nv_bfloat16*)x, (const __nv_bfloat16*)dy, dw, db, l.wg_part, l.wg_part_floats, 0, s, &n->pending); if (r >= 0) { if (bias_done) *bias_done = r == 1; return 0; } }
   if (edge_wgrad_small_cin_supported(g)) { note_simt(n); k_edge_wgrad_small_cin(n->prec, g, x, dy, dw, scratch, 0, s); return 0; }
   if (dense_small_o_supported(g)) { note_simt(n); k_dense_small_o_wgrad(n->prec, g, x, dy, dw, scratch, 0, s); return 0; }
   if (dense_small_k_supported(g) && !(tc_on(n) && tc_wgrad_supported(g))) { note_simt(n); k_dense_small_k_wgrad(n->prec, g, x, dy, dw, s); return 0; }
@@ -515,8 +513,6 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
   n->last_rows = R;
   // every BatchNorm accumulator of the pass (forward statistics and the backward reductions that follow) starts from zero: one memset node
   if (o.train && n->bn_acc) CU(cudaMemsetAsync(n->bn_acc, 0, n->bn_acc_bytes, s));
-  static int fold_bn = -1; if (fold_bn < 0) { const char* e = getenv("B2G_FOLD_BN"); fold_bn = (e && e[0] == '0') ? 0 : 1; }
-  static int fuse_bn = -1; if (fuse_bn < 0) { const char* e = getenv("B2G_FUSE_BN"); fuse_bn = (e && e[0] == '0') ? 0 : 1; }
   // every masked DropoutLayer of a train-mode pass draws with the same pass counter P; the last one's kernel advances P on the device
   int last_drop = -1;
   if (o.train) for (size_t i = 0; i < n->L.size(); ++i) if (n->L[i].drop_active()) last_drop = (int)i;
@@ -529,7 +525,7 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
     // a 1x1-input deconv is computed as the 1x1 problem with taps*C output channels: its columns are not the BatchNorm's channels
     const bool remapped = d.type == B2G_LAYER_DECONV2D && l.geom.KH == 1 && l.geom.C != l.oc;
     // inference-mode (or frozen) BatchNorm right after a linear conv / deconv / dense: fold it, and its activation, into that GEMM's epilogue
-    if (fold_bn && gemm_then_bn && d.act == B2G_ACT_IDENTITY && (!o.train || n->L[i + 1].d.frozen) && !(i + 2 == n->L.size() && o.out_override) && !remapped) {
+    if (gemm_then_bn && d.act == B2G_ACT_IDENTITY && (!o.train || n->L[i + 1].d.frozen) && !(i + 2 == n->L.size() && o.out_override) && !remapped) {
       LayerRT& bn = n->L[i + 1];
       ConvGeom g = l.geom; g.N = R;
       k_bn_fold(n->params + bn.off_mean, n->params + bn.off_var, n->params + bn.off_gamma, n->params + bn.off_beta, bias, bn.oc, bn.d.bn_eps, bn.bn_fold, bn.bn_fold + bn.oc, s);
@@ -539,7 +535,7 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
     }
     // train-mode BatchNorm right after a GEMM: its batch statistics come out of the GEMM's epilogue (kernels_tc.cu EPI_STATS)
     TcEpi st{}; const TcEpi* fuse = nullptr; bool fused = false;
-    if (fuse_bn && gemm_then_bn && o.train && !n->L[i + 1].d.frozen && n->L[i + 1].bn_coef && !remapped && tc_on(n)) {
+    if (gemm_then_bn && o.train && !n->L[i + 1].d.frozen && n->L[i + 1].bn_coef && !remapped && tc_on(n)) {
       st.mode = EPI_STATS; st.acc = n->L[i + 1].acc_fwd; st.imgs_per_group = R / o.groups; fuse = &st;
     }
     switch (d.type) {
@@ -549,7 +545,7 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
         int rows_pg = (R / o.groups) * l.oh * l.ow;
         const bool bn_train = o.train && !d.frozen;      // FrozenLayer always activates in test mode
         l.fwd_fused = false;
-        if (bn_train && l.bn_coef && fuse_bn) {
+        if (bn_train && l.bn_coef) {
           if (!l.stats_by_producer) k_bn_stats_acc(cur, rows_pg, l.oc, o.groups, l.acc_fwd, s);
           const int reps = sync_bn_world(n);
           if (reps > 1) NC(g_nccl.ar(l.acc_fwd, l.acc_fwd, k_bn_acc_elems(l.oc, o.groups), /*ncclUint64*/ 5, /*ncclSum*/ 0, n->ctx->comm, s));      // integer sums: bit-identical on every rank
@@ -602,12 +598,9 @@ static void flush_pending_reduce(b2g_net* n, cudaStream_t s2) { if (n->pending.c
 // top_act_done: the epsilon handed in has already been multiplied by the last layer's act' (the mirror image of the above).
 static int32_t net_backward(b2g_net* n, const void* net_in, void* eps, int rows, int groups, bool want_wgrad, bool need_input_grad, bool allreduce_follows = false,
                             const TcEpi* input_act = nullptr, bool* input_act_done = nullptr, bool top_act_done = false) {
-  static int fork_on = -1; if (fork_on < 0) { const char* e = getenv("B2G_WGRAD_FORK"); fork_on = (e && e[0] == '0') ? 0 : 1; }
-  cudaStream_t s = n->ctx->stream, s2 = fork_on ? n->ctx->side : n->ctx->stream; const int R = rows;
+  cudaStream_t s = n->ctx->stream, s2 = n->ctx->side; const int R = rows;
   void* cur = eps;
   if (input_act_done) *input_act_done = false;
-  static int fuse_bn = -1; if (fuse_bn < 0) { const char* e = getenv("B2G_FUSE_BN"); fuse_bn = (e && e[0] == '0') ? 0 : 1; }
-  static int fuse_act = -1; if (fuse_act < 0) { const char* e = getenv("B2G_FUSE_ACTBWD"); fuse_act = (e && e[0] == '0') ? 0 : 1; }
   n->pending.count = 0;
   // Three epsilon buffers in rotation.  Weight gradients are forked to the side stream (they only READ delta and the layer
   // input), so the input-gradient chain -- the critical path -- never waits for them; a buffer still being read by a
@@ -635,13 +628,13 @@ static int32_t net_backward(b2g_net* n, const void* net_in, void* eps, int rows,
     *target = -1;
     if (!tc_on(n)) return false;
     int k = i - 1; while (k >= 0 && n->L[k].act_fused_into_prev) --k;
-    if (k < 0) { if (input_act && fuse_act) { *e = *input_act; *target = -2; return true; } return false; }
+    if (k < 0) { if (input_act) { *e = *input_act; *target = -2; return true; } return false; }
     LayerRT& b = n->L[k];
-    if (fuse_bn && b.d.type == B2G_LAYER_BATCHNORM && b.fwd_fused && !b.d.frozen && b.fwd_groups == groups) {
+    if (b.d.type == B2G_LAYER_BATCHNORM && b.fwd_fused && !b.d.frozen && b.fwd_groups == groups) {
       e->mode = EPI_BNBWD; e->acc = b.acc_bwd; e->imgs_per_group = R / groups; e->aux = (const __nv_bfloat16*)b.out; e->aux2 = (const __nv_bfloat16*)(k == 0 ? net_in : n->L[k - 1].out);
       e->act = b.fused_act; e->alpha = b.fused_alpha; *target = k; return true;
     }
-    if (fuse_act && k == i - 1 && b.has_gemm() && b.d.act != B2G_ACT_IDENTITY && b.d.type != B2G_LAYER_OUTPUT) {
+    if (k == i - 1 && b.has_gemm() && b.d.act != B2G_ACT_IDENTITY && b.d.type != B2G_LAYER_OUTPUT) {
       e->mode = EPI_ACTBWD; e->aux = (const __nv_bfloat16*)b.out; e->act = b.d.act; e->alpha = b.d.act_alpha; *target = k; return true;
     }
     return false;
@@ -690,8 +683,10 @@ static int32_t net_backward(b2g_net* n, const void* net_in, void* eps, int rows,
         // affine-only dy * gamma * invstd, not the batch-statistics form below.  The reference never differentiates through its frozen
         // trunk (J:335-370: only the new head trains), so that case is refused rather than computed wrongly.
         if (d.frozen) { if (need_in) return fail(B2G_ERR_UNSUPPORTED, "layer %d: a gradient through a frozen BatchNorm (trainable layer or input gradient below it) is not implemented", i); break; }
+        // an accumulator forward never writes bn_mean / bn_invstd: its backward is the accumulator path, over the forward's groups
+        if (l.fwd_fused && l.fwd_groups != groups) return fail(B2G_ERR_ARG, "layer %d: BatchNorm backward in %d groups after a forward in %d", i, groups, l.fwd_groups);
         int rows_pg = (R / groups) * l.oh * l.ow; void* nx = need_in ? other(cur) : nullptr;
-        if (l.fwd_fused && l.fwd_groups == groups) {
+        if (l.fwd_fused) {
           if (!l.bwd_premul) k_bn_bwd_stats_acc(lin, cur, rows_pg, l.oc, groups, l.bn_coef, l.fused_act, l.fused_alpha, l.acc_bwd, s);
           const int reps = sync_bn_world(n);
           if (reps > 1) NC(g_nccl.ar(l.acc_bwd, l.acc_bwd, k_bn_acc_elems(l.oc, groups), /*ncclUint64*/ 5, /*ncclSum*/ 0, n->ctx->comm, s));
@@ -999,22 +994,6 @@ struct b2g_gan {
   std::vector<void*> allocs;
 };
 
-// B2G_PHASES=1 (diagnostic, eager launches only -- events inside a captured graph carry no time): CUDA events on the main stream at the
-// phase boundaries of the step; b2g_gan_step_resident prints the intervals to stderr.  The side streams are not marked: an interval is the
-// main-stream critical path between two boundaries, including whatever it had to wait for.
-static bool phases_on() { static int v = -1; if (v < 0) { const char* e = getenv("B2G_PHASES"); v = (e && atoi(e)) ? 1 : 0; } return v == 1; }
-static cudaEvent_t g_ph_ev[24]; static const char* g_ph_name[24]; static int g_ph_n = 0;
-static void phase_mark(cudaStream_t s, const char* name) {
-  if (!phases_on()) return; cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone; cudaStreamIsCapturing(s, &st); if (st != cudaStreamCaptureStatusNone || g_ph_n >= 24) return;
-  if (!g_ph_ev[g_ph_n]) cudaEventCreate(&g_ph_ev[g_ph_n]);
-  cudaEventRecord(g_ph_ev[g_ph_n], s); g_ph_name[g_ph_n++] = name;
-}
-static void phase_report(cudaStream_t s) {
-  if (!phases_on() || g_ph_n < 2) { g_ph_n = 0; return; }
-  cudaStreamSynchronize(s); float tot = 0.f;
-  for (int i = 1; i < g_ph_n; ++i) { float ms = 0.f; cudaEventElapsedTime(&ms, g_ph_ev[i - 1], g_ph_ev[i]); tot += ms; fprintf(stderr, "[b2g phase] %-34s %8.1f us\n", g_ph_name[i], ms * 1e3f); }
-  fprintf(stderr, "[b2g phase] %-34s %8.1f us\n", "total", tot * 1e3f); g_ph_n = 0;
-}
 // part 1: x_fake = gen.output(z_d) -- needs nothing from the host but z_d.  part 2: everything that touches x_real.
 // They are two graphs so that the copy-stream event of x_real's H2D can be waited on between them (a captured stream may not
 // wait on work outside its capture).
@@ -1023,10 +1002,7 @@ static int32_t gan_step_part1(b2g_gan* g, int N) {
   const size_t ts = prec_size(D->prec);
   void* fake_dst = (char*)D->input + ts * (size_t)N * D->in_elems;
   FwdOpts og{N, 1, g->cfg.fake_bn_train != 0, false, fake_dst};
-  phase_mark(G->ctx->stream, "start");
-  int32_t r = net_forward(G, g->z_d, og, nullptr);
-  phase_mark(G->ctx->stream, "G forward (inference) on z_d");
-  return r;
+  return net_forward(G, g->z_d, og, nullptr);
 }
 static int32_t gan_step_part2(b2g_gan* g, int N) {
   b2g_net *G = g->G, *D = g->D; cudaStream_t s = G->ctx->stream;
@@ -1051,32 +1027,24 @@ static int32_t gan_step_part2(b2g_gan* g, int N) {
   CU(cudaMemsetAsync(D->grads, 0, sizeof(float) * D->n_params, s));
   const void* logits = nullptr; FwdOpts od{2 * N, 2, true, true, nullptr};
   B2(net_forward(D, D->input, od, &logits));
-  phase_mark(s, "D forward 2N (+hoisted G fwd fork)");
   k_xent(D->prec, logits, g->y_d, D->epsA, g->loss_dev, N, 2, D->cfg.xent_clip_eps, s);
   B2(net_backward(D, D->input, D->epsA, 2 * N, 2, true, false, /*allreduce_follows=*/true));
-  phase_mark(s, "D loss + backward 2N (join wgrad)");
   if (under_allreduce) B2(hoisted_g_forward());
   B2(net_allreduce_grads(D));
   B2(net_update(D, 2 * N));
-  phase_mark(s, "D all-reduce + update");
   // 3. G update through D on (z_g, y_gen) (J:465-471); D's parameters / running stats / updater state untouched
   CU(cudaStreamWaitEvent(s, G->ctx->ev_b, 0));
-  phase_mark(s, "wait for hoisted G train forward");
   FwdOpts od2{N, 1, true, false, nullptr};
   B2(net_forward(D, xg, od2, &logits));
-  phase_mark(s, "D forward N");
   k_xent(D->prec, logits, g->y_g, D->epsA, g->loss_dev + 2, N, 1, D->cfg.xent_clip_eps, s);
   // the generator's output activation (tanh) is differentiated inside D's last input-gradient kernel when that kernel can (EPI_ACTBWD)
   TcEpi ga{}; const LayerRT& gl = G->L.back(); bool ga_done = false;
   const bool ga_can = gl.has_gemm() && gl.d.act != B2G_ACT_IDENTITY && gl.d.type != B2G_LAYER_OUTPUT;
   if (ga_can) { ga.mode = EPI_ACTBWD; ga.aux = (const __nv_bfloat16*)xg; ga.act = gl.d.act; ga.alpha = gl.d.act_alpha; }
   B2(net_backward(D, xg, D->epsA, N, 1, false, true, false, ga_can ? &ga : nullptr, &ga_done));
-  phase_mark(s, "D input gradient N");
   B2(net_backward(G, g->z_g, D->input_grad, N, 1, true, false, /*allreduce_follows=*/true, nullptr, nullptr, ga_done));
-  phase_mark(s, "G backward (join wgrad)");
   B2(net_allreduce_grads(G));
   B2(net_update(G, N));
-  phase_mark(s, "G all-reduce + update");
   return 0;
 }
 
@@ -1138,7 +1106,7 @@ extern "C" int32_t b2g_gan_step_resident(b2g_gan* g, int32_t batch) {
   if (c->comm) g->nccl_warm = true;
   g->last_batch = batch;
   CU(cudaEventRecord(g->ev0, s));
-  if (!use_graph) { B2(gan_step_part1(g, batch)); CU(cudaStreamWaitEvent(s, g->ev_x, 0)); B2(gan_step_part2(g, batch)); phase_report(s); }
+  if (!use_graph) { B2(gan_step_part1(g, batch)); CU(cudaStreamWaitEvent(s, g->ev_x, 0)); B2(gan_step_part2(g, batch)); }
   else {
     if (!g->exec || g->graph_batch != batch || g->graph_gn_g != g->G->gn_gen || g->graph_gn_d != g->D->gn_gen) {
       if (g->exec) { cudaGraphExecDestroy(g->exec); g->exec = nullptr; } if (g->graph) { cudaGraphDestroy(g->graph); g->graph = nullptr; }

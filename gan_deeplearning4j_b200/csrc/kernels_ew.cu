@@ -16,7 +16,6 @@
 namespace b2g {
 
 uint64_t g_launch_count = 0;
-int g_pdl_enabled = -1;
 
 // ---------------------------------------------------------------- layout -----------------------------
 template <typename T>
@@ -136,25 +135,6 @@ __device__ __forceinline__ void block_fold_write(float (&acc)[NV][8], int C, int
     for (int v = 0; v < NV; ++v) { float a = 0.f; for (int k = 0; k < TY; ++k) a += sred[v][k * C + c]; dst[v][row_off + c] = a; }
   }
 }
-__global__ void __launch_bounds__(256) bn_stats_partial_bf16x8_kernel(const uint4* __restrict__ x, int rows, int C, int S, float* __restrict__ psum, float* __restrict__ psq, float* __restrict__ pivot) { pdl_enter();
-  const int g = blockIdx.y, C8 = C / 8, TY = 256 / C8, c8 = threadIdx.x % C8, ty = threadIdx.x / C8, sl = blockIdx.x;
-  const int chunk = (rows + S - 1) / S, r0 = sl * chunk, r1 = min(rows, r0 + chunk);
-  const uint4* xg = x + (size_t)g * rows * C8;
-  float acc[2][8], k[8];
-  unpack8(xg[c8], k);       // pivot: row 0 of the group (see bn_stats_partial_kernel)
-  if (sl == 0 && ty == 0) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) pivot[g * C + c8 * 8 + j] = k[j];
-  }
-#pragma unroll
-  for (int j = 0; j < 8; ++j) { acc[0][j] = 0.f; acc[1][j] = 0.f; }
-#pragma unroll 4
-  for (int r = r0 + ty; r < r1; r += TY) { float v[8]; unpack8(xg[(size_t)r * C8 + c8], v);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { const float d = v[j] - k[j]; acc[0][j] += d; acc[1][j] = fmaf(d, d, acc[1][j]); } }
-  float* const dst[2] = {psum, psq};
-  block_fold_write<2>(acc, C, C8, c8, ty, TY, dst, ((size_t)g * S + sl) * C);
-}
 // stage 2: block = 32 adjacent channels x 16 slice lanes (coalesced 128-byte rows of the partial arrays), fixed-order tree in double
 __global__ void __launch_bounds__(1024) bn_stats_final_kernel(const float* __restrict__ psum, const float* __restrict__ psq, const float* __restrict__ pivot, int rows, int C, int S, int groups, float eps,
                                       float* __restrict__ mean, float* __restrict__ invstd,
@@ -186,15 +166,10 @@ __global__ void __launch_bounds__(1024) bn_stats_final_kernel(const float* __res
 }
 void k_bn_stats(int prec, const void* x, int rows, int C, int groups, float* scratch, float* mean, float* invstd, float eps,
                 const float* run_mean, const float* run_var, float* g_mean, float* g_var, float decay, cudaStream_t s) {
-  const bool vec = vec_ok(prec, C);
-  int S = vec ? vec_blocks(rows, C) : pick_slices(rows, C);
+  const int S = pick_slices(rows, C);
   float* psum = scratch; float* psq = scratch + (size_t)groups * S * C; float* pivot = psq + (size_t)groups * S * C;
-  if (vec) {
-    launch_pdl(bn_stats_partial_bf16x8_kernel, dim3(dim3(S, groups)), dim3(256), (size_t)(0), s, (const uint4*)x, rows, C, S, psum, psq, pivot);
-  } else {
-    dim3 grid((S * C + 255) / 256, groups);
-    DISPATCH_PREC(prec, T, (launch_pdl(bn_stats_partial_kernel<T>, dim3(grid), dim3(256), (size_t)(0), s, (const T*)x, rows, C, S, psum, psq, pivot)));
-  }
+  dim3 grid((S * C + 255) / 256, groups);
+  DISPATCH_PREC(prec, T, (launch_pdl(bn_stats_partial_kernel<T>, dim3(grid), dim3(256), (size_t)(0), s, (const T*)x, rows, C, S, psum, psq, pivot)));
   LAUNCHED();
   launch_pdl(bn_stats_final_kernel, dim3((C + 31) / 32), dim3(1024), (size_t)(0), s, psum, psq, (const float*)pivot, rows, C, S, groups, eps, mean, invstd, run_mean, run_var, g_mean, g_var, decay); LAUNCHED();
 }
@@ -280,53 +255,6 @@ __global__ void bn_bwd_partial_kernel(const T* __restrict__ x, const T* __restri
   }
   p1[((size_t)g * S + sl) * C + c] = a; p2[((size_t)g * S + sl) * C + c] = b;
 }
-template <int ACTC>
-__global__ void __launch_bounds__(256, 3) bn_bwd_partial_bf16x8_kernel(const uint4* __restrict__ x, const uint4* __restrict__ eo, int rows, int C, int S, const float* __restrict__ mean,
-                                             const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta, int act, float alpha,
-                                             float* __restrict__ p1, float* __restrict__ p2) { pdl_enter();
-  const int g = blockIdx.y, C8 = C / 8, TY = 256 / C8, c8 = threadIdx.x % C8, ty = threadIdx.x / C8, sl = blockIdx.x;
-  const int chunk = (rows + S - 1) / S, r0 = sl * chunk, r1 = min(rows, r0 + chunk);
-  const uint4* xg = x + (size_t)g * rows * C8; const uint4* eg = eo + (size_t)g * rows * C8;
-  float mu[8], is[8], ga[8], be[8], acc[2][8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) { const int c = c8 * 8 + j; mu[j] = mean[g * C + c]; is[j] = invstd[g * C + c]; ga[j] = gamma[c]; be[j] = beta[c]; acc[0][j] = 0.f; acc[1][j] = 0.f; }
-#pragma unroll 4
-  for (int r = r0 + ty; r < r1; r += TY) {
-    float xv[8], ev[8]; unpack8(xg[(size_t)r * C8 + c8], xv); unpack8(eg[(size_t)r * C8 + c8], ev);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { const float xh = (xv[j] - mu[j]) * is[j]; const float dy = ev[j] * act_grad_from_pre(ACTC < 0 ? act : ACTC, fmaf(ga[j], xh, be[j]), alpha); acc[0][j] += dy; acc[1][j] = fmaf(dy, xh, acc[1][j]); }
-  }
-  float* const dst[2] = {p1, p2};
-  block_fold_write<2>(acc, C, C8, c8, ty, TY, dst, ((size_t)g * S + sl) * C);
-}
-template <int ACTC>
-__global__ void __launch_bounds__(256, 2) bn_bwd_apply_bf16x8_kernel(const uint4* __restrict__ x, const uint4* __restrict__ eo, uint4* __restrict__ ei, int rows, int C, int groups,
-                                           const float* __restrict__ mean, const float* __restrict__ invstd, const float* __restrict__ gamma,
-                                           const float* __restrict__ beta, int act, float alpha, const float* __restrict__ c1, const float* __restrict__ c2) { pdl_enter();
-  // same hoisting as bn_apply_bf16x8_kernel: one thread, one channel octet
-  const int C8 = C / 8; const size_t per_group = (size_t)rows * C8;
-  const size_t t0 = blockIdx.x * (size_t)blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
-  const int c0 = (int)(t0 % C8) * 8;
-  for (int g = 0; g < groups; ++g) {
-    float mu[8], is[8], ga[8], be[8], k1[8], k2[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) { const int k = g * C + c0 + j; mu[j] = mean[k]; is[j] = invstd[k]; ga[j] = gamma[c0 + j]; be[j] = beta[c0 + j]; k1[j] = c1[k]; k2[j] = c2[k]; }
-    const uint4* xg = x + g * per_group; const uint4* eg = eo + g * per_group; uint4* ig = ei + g * per_group;
-    for (size_t i = t0; i < per_group; i += 4 * stride) {
-      uint4 xa[4], ea[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) if (i + q * stride < per_group) { xa[q] = xg[i + q * stride]; ea[q] = eg[i + q * stride]; }
-#pragma unroll
-      for (int q = 0; q < 4; ++q) if (i + q * stride < per_group) {
-        float xv[8], ev[8], o[8]; unpack8(xa[q], xv); unpack8(ea[q], ev);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { const float xh = (xv[j] - mu[j]) * is[j];
-          const float dy = ev[j] * act_grad_from_pre(ACTC < 0 ? act : ACTC, fmaf(ga[j], xh, be[j]), alpha); o[j] = ga[j] * is[j] * (dy - k1[j] - xh * k2[j]); }
-        ig[i + q * stride] = pack8(o);
-      }
-    }
-  }
-}
 __global__ void __launch_bounds__(1024) bn_bwd_final_kernel(const float* __restrict__ p1, const float* __restrict__ p2, int rows, int C, int S, int groups,
                                     float* __restrict__ c1, float* __restrict__ c2, float* g_gamma, float* g_beta, int want) { pdl_enter();
   __shared__ double sa[32][33], sb[32][33];      // 32 channels x 32 slice lanes: S <= 256 partial rows in ONE batch of 8 loads per thread
@@ -366,21 +294,15 @@ __global__ void bn_bwd_apply_kernel(const T* __restrict__ x, const T* __restrict
 void k_bn_bwd(int prec, const void* x, const void* eps_out, void* eps_in, int rows, int C, int groups,
               const float* mean, const float* invstd, const float* gamma, const float* beta, int act, float alpha,
               float* scratch, float* g_gamma, float* g_beta, int want, cudaStream_t s) {
-  const bool vec = vec_ok(prec, C);
-  int S = vec ? vec_blocks(rows, C) : pick_slices(rows, C);
+  const int S = pick_slices(rows, C);
   float* p1 = scratch; float* p2 = p1 + (size_t)groups * S * C; float* c1 = p2 + (size_t)groups * S * C; float* c2 = c1 + (size_t)groups * C;
-  if (vec) {
-    DISPATCH_ACT(act, ACTC, launch_pdl(bn_bwd_partial_bf16x8_kernel<ACTC>, dim3(dim3(S, groups)), dim3(256), (size_t)(0), s, (const uint4*)x, (const uint4*)eps_out, rows, C, S, mean, invstd, gamma, beta, act, alpha, p1, p2));
-  } else {
-    dim3 grid((S * C + 255) / 256, groups);
-    DISPATCH_PREC(prec, T, (launch_pdl(bn_bwd_partial_kernel<T>, dim3(grid), dim3(256), (size_t)(0), s, (const T*)x, (const T*)eps_out, rows, C, S, mean, invstd, gamma, beta, act, alpha, p1, p2)));
-  }
+  dim3 grid((S * C + 255) / 256, groups);
+  DISPATCH_PREC(prec, T, (launch_pdl(bn_bwd_partial_kernel<T>, dim3(grid), dim3(256), (size_t)(0), s, (const T*)x, (const T*)eps_out, rows, C, S, mean, invstd, gamma, beta, act, alpha, p1, p2)));
   LAUNCHED();
   launch_pdl(bn_bwd_final_kernel, dim3((C + 31) / 32), dim3(1024), (size_t)(0), s, p1, p2, rows, C, S, groups, c1, c2, g_gamma, g_beta, want); LAUNCHED();
   if (eps_in) {
     size_t n = (size_t)rows * C * groups;
-    if (vec) { DISPATCH_ACT(act, ACTC, launch_pdl(bn_bwd_apply_bf16x8_kernel<ACTC>, dim3(vec4_blocks((size_t)rows * C / 8)), dim3(256), (size_t)(0), s, (const uint4*)x, (const uint4*)eps_out, (uint4*)eps_in, rows, C, groups, mean, invstd, gamma, beta, act, alpha, c1, c2)); }
-    else DISPATCH_PREC(prec, T, (launch_pdl(bn_bwd_apply_kernel<T>, dim3(ew_blocks(n)), dim3(256), (size_t)(0), s, (const T*)x, (const T*)eps_out, (T*)eps_in, rows, C, groups, mean, invstd, gamma, beta, act, alpha, c1, c2)));
+    DISPATCH_PREC(prec, T, (launch_pdl(bn_bwd_apply_kernel<T>, dim3(ew_blocks(n)), dim3(256), (size_t)(0), s, (const T*)x, (const T*)eps_out, (T*)eps_in, rows, C, groups, mean, invstd, gamma, beta, act, alpha, c1, c2)));
     LAUNCHED();
   }
 }

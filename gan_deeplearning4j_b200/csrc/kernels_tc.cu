@@ -560,8 +560,7 @@ static int pick_bn(int OC) { return OC % 128 == 0 ? 128 : OC % 64 == 0 ? 64 : 0;
 // Small layers (few M tiles) are latency-bound per CTA, not bandwidth-bound: prefer narrower N tiles until the grid covers the SMs.
 static int pick_bn_fill(int OC, long m_tiles_x_phases) {
   if (g_tc_test_bn) return g_tc_test_bn;
-  static int min_ctas = -1; if (min_ctas < 0) { const char* e = getenv("B2G_BN_MIN_CTAS"); min_ctas = e ? atoi(e) : 0; }
-  const int target = min_ctas >= 1 ? min_ctas : device_sm_count();
+  const int target = device_sm_count();
   int bn = pick_bn(OC);
   while (bn > 64 && m_tiles_x_phases * (OC / bn) < target) bn /= 2;
   return bn;
@@ -903,10 +902,7 @@ static bool edge_tile(const ConvGeom& g, int* Ht) {
 bool tc_edge_conv_supported(const ConvGeom& g) { int ht; return edge_tile(g, &ht) && g.O % 64 == 0; }
 bool tc_edge_wgrad_supported(const ConvGeom& g) { int ht; return edge_tile(g, &ht) && g.O == 64; }
 // CTA targets of the edge kernels: two waves for the weight gradient (split-K partials, fixed-order sum), eight for the forward
-static int tc_edge_wgrad_target() {
-  static int env = -1; if (env < 0) { const char* e = getenv("B2G_EDGE_WGRAD_CTAS"); env = e ? atoi(e) : 0; }
-  const int cap = 8 * device_sm_count(); return env >= 1 && env <= cap ? env : 2 * device_sm_count();
-}
+static int tc_edge_wgrad_target() { return 2 * device_sm_count(); }
 static int tc_edge_wgrad_ctas(const ConvGeom& g, int* tpc) {
   int ht = 1; edge_tile(g, &ht);
   const int tiles = g.N * (g.OH / ht), target = tc_edge_wgrad_target();
@@ -921,8 +917,7 @@ int k_tc_edge_conv(const ConvGeom& g, const __nv_bfloat16* x, const __nv_bfloat1
   p.tiles_total = g.N * p.tiles_y; p.act = act; p.alpha = alpha;
   const size_t smem = 1024 + 24576 + EDGE_SLAB_BYTES;
   TC_SET_SMEM_ONCE(tc_edge_conv_kernel, smem);
-  static int env = -1; if (env < 0) { const char* e = getenv("B2G_EDGE_CONV_CTAS"); env = e ? atoi(e) : 0; }
-  const int target = env >= 1 ? env : 8 * device_sm_count();
+  const int target = 8 * device_sm_count();
   p.tiles_per_cta = (p.tiles_total + target - 1) / target;
   launch_pdl(tc_edge_conv_kernel, dim3(dim3((unsigned)((p.tiles_total + p.tiles_per_cta - 1) / p.tiles_per_cta), (unsigned)(g.O / 64))), dim3(128), (size_t)(smem), s, p);
   LAUNCHED(); g_tc_last_kernel = "tc_edge_conv_kernel";
@@ -1060,10 +1055,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_wgrad_kernel(const __grid_co
 static int wgrad_bnw(const ConvGeom& g) { if (g.C % 64) return 0; const long cols = (long)g.KH * g.KW * g.C; return cols % 128 == 0 ? 128 : 64; }
 // CTA target of the split-K weight gradients: two thirds of a wave.  The weight-gradient kernels run on the side stream beside the
 // input-gradient chain, which keeps the remaining SMs; fewer CTAs also cut the fp32 partials the deferred reduce reads.
-static int wgrad_target() {
-  static int env = -1; if (env < 0) { const char* e = getenv("B2G_WGRAD_CTAS"); env = e ? atoi(e) : 0; }
-  return env >= 1 ? env : (2 * device_sm_count()) / 3;
-}
+static int wgrad_target() { return (2 * device_sm_count()) / 3; }
 // choose the split count so that the whole grid is at most wgrad_target() CTAs
 static int wgrad_splits_for(const ConvGeom& g, int o_tile) {
   const int bnw = wgrad_bnw(g); if (!bnw) return 1;

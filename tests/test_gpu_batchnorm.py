@@ -1,5 +1,5 @@
 """BatchNorm(+activation) kernels of the training step against a float64 reference, one kernel chain at a time (b2g_test_bn):
-    path 0  the two-stage kernels (k_bn_stats -> k_bn_apply -> k_bn_bwd), fp32 and bf16, vector and scalar variants;
+    path 0  the two-stage kernels (k_bn_stats -> k_bn_apply -> k_bn_bwd), fp32 and bf16, scalar kernels (bf16 apply 16-byte vectorised where C allows);
     path 1  the 128-bit accumulator kernels (k_bn_stats_acc -> k_bn_apply_acc -> k_bn_bwd_stats_acc -> k_bn_bwd_apply_acc);
     path 2  the accumulator kernels fed the way the fused BatchNorm-backward GEMM epilogue feeds them: eps already multiplied by act',
             backward statistics (sum dy', sum dy'*z) converted to (sum dy', sum dy'*xhat) in k_bn_bwd_apply_acc.
