@@ -1260,9 +1260,9 @@ extern "C" int32_t b2g_ctx_allreduce_test(b2g_ctx* c, float* host, int64_t n) {
 // ------------------------------------------------------------------ kernel-level test hook ----------------
 // The tile-width / grid overrides of tc_conv_kernel hold for the hook's own launch loop only: reset right after it, and on every early return.
 struct TcTestSchedule {
-  TcTestSchedule(int bn, int max_ctas) { g_tc_test_bn = bn; g_tc_test_max_ctas = max_ctas; }
+  TcTestSchedule(int bn, int max_ctas, int per_tap) { g_tc_test_bn = bn; g_tc_test_max_ctas = max_ctas; g_tc_test_per_tap = per_tap; }
   ~TcTestSchedule() { reset(); }
-  void reset() { g_tc_test_bn = 0; g_tc_test_max_ctas = 0; }
+  void reset() { g_tc_test_bn = 0; g_tc_test_max_ctas = 0; g_tc_test_per_tap = 0; }
 };
 extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int32_t precision, const b2g_conv_geom* gg, const float* a_host, const float* b_host, float* out, int32_t iters, float* ms_per_iter,
                                     b2g_test_conv_opts* opt) {
@@ -1284,7 +1284,8 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   if (opt && ps && (opt->scale || (opt->epi != EPI_PLAIN && opt->epi != EPI_ACTBWD)))
     return fail(B2G_ERR_UNSUPPORTED, "the pixel-shuffle deconv has bias, activation and the activation-backward epilogue only");
   const int force_bn = opt ? opt->bn : 0, max_ctas = opt ? opt->max_ctas : 0;
-  const bool poison = opt && opt->poison, w_mn = opt && opt->w_mn;
+  const bool poison = opt && opt->poison, w_mn = opt && opt->w_mn, per_tap = opt && opt->per_tap;
+  if (per_tap && !tc_conv) return fail(B2G_ERR_UNSUPPORTED, "per_tap applies to the tensor-core fprop / dgrad kernels (impl 1, kind 0 / 1)");
   if (force_bn && (!tc_conv || (force_bn != 64 && force_bn != 128) || oc % force_bn))
     return fail(B2G_ERR_UNSUPPORTED, "bn %d: the tensor-core fprop / dgrad tile is 64 or 128 columns and must divide the %d output channels", force_bn, oc);
   if (max_ctas < 0 || (max_ctas && !tc_conv && !ps)) return fail(B2G_ERR_UNSUPPORTED, "max_ctas %d: a grid cap applies to tc_conv_kernel launches only", max_ctas);
@@ -1328,8 +1329,8 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   }
   cudaEvent_t e0, e1; CU(cudaEventCreate(&e0)); CU(cudaEventCreate(&e1));
   int reps = iters < 1 ? 1 : iters; int rc = 0;
-  g_tc_last_kernel = "";
-  TcTestSchedule schedule(force_bn, max_ctas);
+  g_tc_last_kernel = ""; g_tc_last_slab = false;
+  TcTestSchedule schedule(force_bn, max_ctas, per_tap);
   for (int it = -1; it < reps; ++it) {       // it = -1: warm-up
     if (it == 0) CU(cudaEventRecord(e0, s));
     if (d_acc) CU(cudaMemsetAsync(d_acc, 0, 8 * k_bn_acc_elems(oc, groups), s));
@@ -1353,7 +1354,7 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   schedule.reset();
   CU(cudaEventRecord(e1, s));
   if (rc) return fail(B2G_ERR_CUDA, "tensor-core kernel launch failed (%d)", rc);
-  if (opt) { strncpy(opt->kernel, g_tc_last_kernel, sizeof(opt->kernel) - 1); opt->kernel[sizeof(opt->kernel) - 1] = 0; }
+  if (opt) { strncpy(opt->kernel, g_tc_last_kernel, sizeof(opt->kernel) - 1); opt->kernel[sizeof(opt->kernel) - 1] = 0; opt->slab = g_tc_last_slab; }
   if (kind != 2) { if (prec == PREC_BF16) { /* widen */ k_nhwc_to_nchw_f32(prec, to, fo, 1, 1, (int)no, s); } else CU(cudaMemcpyAsync(fo, to, 4 * no, cudaMemcpyDeviceToDevice, s)); }
   CU(cudaMemcpyAsync(out, fo, 4 * no, cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s)); CHECK_KERNELS();

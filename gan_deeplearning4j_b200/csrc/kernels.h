@@ -189,6 +189,10 @@ extern const char* g_tc_last_kernel;     // which tensor-core kernel the most re
 // Schedule overrides of tc_conv_kernel, set only by the kernel-level test hook around its launches (0 = production choice):
 // g_tc_test_bn forces the 64- or 128-column tile, g_tc_test_max_ctas caps the persistent grid at min(work items, max_ctas)
 extern int g_tc_test_bn, g_tc_test_max_ctas;
+// g_tc_test_per_tap keeps 4x4 s2 p1 fprop / dgrad on the per-tap activation loads; g_tc_last_slab: the most recent fprop / dgrad launch
+// loaded its activations as 2x2-tap slabs (kernels_tc.cu slab_tile)
+extern int g_tc_test_per_tap;
+extern bool g_tc_last_slab;
 // epilogue of the fprop / dgrad kernels (kernels_tc.cu): what happens between the fp32 accumulator and the bf16 store
 enum { EPI_PLAIN = 0, EPI_STATS = 1, EPI_BNBWD = 2, EPI_ACTBWD = 3 };
 struct TcEpi {

@@ -117,6 +117,20 @@ __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t 
         "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "l"(da), "l"(db), "n"(TA), "n"(TB));
 }
+// D[64 x 128] += A[64 x 16] B[16 x 128]: one instruction instead of two m64n64k16, so the A tile is read from shared memory once.  The
+// B descriptor spans both 64-column blocks (K-major: 128 rows, 8-row groups 1024 B apart; MN-major: the blocks LBO apart).  Fragment
+// d[4j + 2i + k], j < 16, of the n128 instruction = column block j / 8 of two n64 fragments: d0 = columns [0, 64), d1 = [64, 128), each
+// holding exactly what wgmma_n64 would (every output element sums the same 16 products).
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n128(float (&d0)[32], float (&d1)[32], uint64_t da, uint64_t db) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, 1, 1, 1, %66, %67;"
+      : "+f"(d0[0]), "+f"(d0[1]), "+f"(d0[2]), "+f"(d0[3]), "+f"(d0[4]), "+f"(d0[5]), "+f"(d0[6]), "+f"(d0[7]), "+f"(d0[8]), "+f"(d0[9]), "+f"(d0[10]), "+f"(d0[11]), "+f"(d0[12]), "+f"(d0[13]), "+f"(d0[14]), "+f"(d0[15]), "+f"(d0[16]), "+f"(d0[17]), "+f"(d0[18]), "+f"(d0[19]), "+f"(d0[20]), "+f"(d0[21]), "+f"(d0[22]), "+f"(d0[23]), "+f"(d0[24]), "+f"(d0[25]), "+f"(d0[26]), "+f"(d0[27]), "+f"(d0[28]), "+f"(d0[29]), "+f"(d0[30]), "+f"(d0[31]),
+        "+f"(d1[0]), "+f"(d1[1]), "+f"(d1[2]), "+f"(d1[3]), "+f"(d1[4]), "+f"(d1[5]), "+f"(d1[6]), "+f"(d1[7]), "+f"(d1[8]), "+f"(d1[9]), "+f"(d1[10]), "+f"(d1[11]), "+f"(d1[12]), "+f"(d1[13]), "+f"(d1[14]), "+f"(d1[15]), "+f"(d1[16]), "+f"(d1[17]), "+f"(d1[18]), "+f"(d1[19]), "+f"(d1[20]), "+f"(d1[21]), "+f"(d1[22]), "+f"(d1[23]), "+f"(d1[24]), "+f"(d1[25]), "+f"(d1[26]), "+f"(d1[27]), "+f"(d1[28]), "+f"(d1[29]), "+f"(d1[30]), "+f"(d1[31])
+      : "l"(da), "l"(db), "n"(TA), "n"(TB));
+}
 // the same with N = 16 (pixel-shuffle tile): d[4j + 2i + k], j < 2
 __device__ __forceinline__ void wgmma_n16(float (&d)[8], uint64_t da, uint64_t db) {
   asm volatile(
@@ -146,7 +160,10 @@ struct TcConvParams {
   int Nt, Ht, Wt;           // A-tile rows = Nt images x Ht rows x Wt cols of the row grid (Nt*Ht*Wt = 128)
   int GH, GW;               // row grid: conv output (fprop) / phase grid = dy spatial dims (dgrad)
   int tiles_y;              // GH / Ht
-  int taps_h, taps_w;       // K-loop taps: KH,KW (fprop) / 2,2 (dgrad phase)
+  int taps_h, taps_w;       // K-loop taps: KH,KW (fprop) / 2,2 (dgrad phase); slab path: row pairs (2 fprop, 1 dgrad) x column taps
+  int slab_bytes;           // slab path: bytes of one activation slab box, Nt x (Ht+1) x Wt rows of 128 B
+  int a_wg_bytes;           // slab path: offset of a consumer warpgroup's 64 A rows in the slab (64 rows, or one image's Ht+1 rows when Nt = 2)
+  int a_tap_bytes;          // slab path: offset of the upper tap of a row pair = one row of the row grid = Wt x 128 B
   int chunks;               // reduction channels / 64
   int KW, SH, SW, PH, PW;
   int OC;                   // output channels = row length of `out`
@@ -165,10 +182,13 @@ struct TcConvParams {
 
 static constexpr int TC_THREADS = 384;       // tc_wgrad_kernel: producer warpgroup + two consumer warpgroups
 static constexpr int TC_CONV_THREADS = 640;  // tc_conv_kernel: two MMA consumer warpgroups, two epilogue warpgroups, a producer warpgroup
-template <int BN, int STAGES, int EPI = EPI_PLAIN>
+// Slab path: a stage holds one activation slab of Nt x (Ht+1) x Wt rows (at most SLAB_ROWS: Ht = 8 rows of a 16-column grid, or two 8x8
+// images) and the weight tiles of the two taps that read it; at BN = 64 four such stages fit beside the two park slots
+static constexpr int SLAB_ROWS = 144;
+template <int BN, int STAGES, int EPI = EPI_PLAIN, bool SLAB = false>
 struct TcSmem {
-  static constexpr int A_BYTES = 128 * 128;        // 128 rows x 64 bf16
-  static constexpr int B_BYTES = BN * 128;
+  static constexpr int A_BYTES = (SLAB ? SLAB_ROWS : 128) * 128;   // 128 rows x 64 bf16 (per tap) / the slab
+  static constexpr int B_BYTES = (SLAB ? 2 : 1) * BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
   static constexpr int ACC_PITCH = BN + 4;         // floats per parked accumulator row: 16-byte row reads by 8 lanes hit 8 different bank groups
@@ -345,16 +365,20 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[NB][NACC], uint32_t a_sm
     const uint64_t bdesc = desc_kmajor_sw128(b_smem);
 #pragma unroll
     for (int k = 0; k < 4; ++k) wgmma_n16(acc[0], adesc + 2 * k, bdesc + 2 * k);
+  } else if constexpr (NB == 2) {
+    if (!b_mn) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_n128<0, 0>(acc[0], acc[1], adesc + 2 * k, desc_kmajor_sw128(b_smem) + 2 * k);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_n128<0, 1>(acc[0], acc[1], adesc + 2 * k, desc_mnmajor_sw128(b_smem + k * 2048, 8192));
+    }
   } else if (!b_mn) {
 #pragma unroll
-    for (int k = 0; k < 4; ++k)
-#pragma unroll
-      for (int nb = 0; nb < NB; ++nb) wgmma_n64<0, 0>(acc[nb], adesc + 2 * k, desc_kmajor_sw128(b_smem + nb * 8192) + 2 * k);
+    for (int k = 0; k < 4; ++k) wgmma_n64<0, 0>(acc[0], adesc + 2 * k, desc_kmajor_sw128(b_smem) + 2 * k);
   } else {
 #pragma unroll
-    for (int k = 0; k < 4; ++k)
-#pragma unroll
-      for (int nb = 0; nb < NB; ++nb) wgmma_n64<0, 1>(acc[nb], adesc + 2 * k, desc_mnmajor_sw128(b_smem + nb * 8192 + k * 2048, 8192));
+    for (int k = 0; k < 4; ++k) wgmma_n64<0, 1>(acc[0], adesc + 2 * k, desc_mnmajor_sw128(b_smem + k * 2048, 8192));
   }
 }
 __device__ __forceinline__ void tap_coords(const TcConvParams& p, int ta, int tb, int py, int px, int& ax, int& dy_, int& wtap) {
@@ -365,6 +389,14 @@ __device__ __forceinline__ void tap_coords(const TcConvParams& p, int ta, int tb
     const int sx = px == 0 ? (tb == 0 ? 1 : 3) : (tb == 0 ? 0 : 2), dxc = px == 0 ? (tb == 0 ? 0 : -1) : (tb == 0 ? 1 : 0);
     dy_ = dyr; ax = dxc; wtap = r * 4 + sx;
   }
+}
+// Slab path: K unit (pair ta, column tap tb) = two taps one row of the row grid apart that read the same slab, the lower one rows [0, Ht),
+// the upper one rows [1, Ht+1).  fprop 4x4 s2: taps (ta, tb) and (ta + 2, tb) (two input rows = one strided row); dgrad phase: taps (1, tb)
+// (dy row offset -1 / 0 for py = 0 / 1) and (0, tb) (0 / +1).  Both taps have the same column offset ax.
+__device__ __forceinline__ void slab_coords(const TcConvParams& p, int ta, int tb, int py, int px, int& ax, int& dy_, int& wlo, int& whi) {
+  int ax2, dy2;
+  tap_coords(p, p.mode == 0 ? ta : 1, tb, py, px, ax, dy_, wlo);
+  tap_coords(p, p.mode == 0 ? ta + 2 : 0, tb, py, px, ax2, dy2, whi);
 }
 
 // Persistent and warp-specialised: CTA b walks the work items t = b, b + gridDim.x, ... (one 128 x BN output tile of one phase each).
@@ -387,9 +419,13 @@ struct TcConvRegs {
   static constexpr int LAUNCH = 96, PRODUCER = 24, MMA = BN >= 128 ? 96 : 64, EPI = BN >= 128 ? 128 : 160;
   static_assert(PRODUCER + 2 * MMA + 2 * EPI <= 5 * LAUNCH, "setmaxnreg budget exceeds the launch allocation");
 };
-template <int BN, int STAGES, int EPI, bool AFFINE, bool PS = false>
+// SLAB (4x4 s2 p1 fprop and phase-form dgrad on grids with Wt % 8 == 0): a K unit loads one slab box -- Nt x (Ht+1) x Wt rows, one column
+// offset, one channel chunk -- and the two taps' weight tiles; the MMA warpgroups run the lower tap from the slab and the upper tap from a
+// descriptor Wt rows further in (a multiple of 1024 B: the SW128 pattern stays canonical).  Half the K units of the per-tap path, and
+// (Ht+1) Wt instead of 2 x 128 activation rows from L2 per two taps.
+template <int BN, int STAGES, int EPI, bool AFFINE, bool PS = false, bool SLAB = false>
 __global__ void __launch_bounds__(TC_CONV_THREADS, 1) tc_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const TcConvParams p) {
-  using S = TcSmem<BN, STAGES, EPI>;
+  using S = TcSmem<BN, STAGES, EPI, SLAB>;
   using R = TcConvRegs<BN>;
   constexpr int NB = BN >= 64 ? BN / 64 : 1, NACC = BN >= 64 ? 32 : BN / 2;
   extern __shared__ uint8_t smem_raw[];
@@ -429,17 +465,21 @@ __global__ void __launch_bounds__(TC_CONV_THREADS, 1) tc_conv_kernel(const __gri
         const int py = phase >> 1, px = phase & 1;
         const int ybase = p.mode == 0 ? y0 * p.SH : y0;
         int ch = 0, ta = 0, tb = 0;
-        int ax, dy_, wtap; tap_coords(p, 0, 0, py, px, ax, dy_, wtap);
+        int ax, dy_, wtap, wtap2 = 0;
+        auto coords = [&]() { if constexpr (SLAB) slab_coords(p, ta, tb, py, px, ax, dy_, wtap, wtap2); else tap_coords(p, ta, tb, py, px, ax, dy_, wtap); };
+        coords();
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(bar_empty + 8 * s, ph ^ 1);
           if (elect_one_sync()) {
-            mbar_expect_tx(bar_full + 8 * s, S::STAGE_BYTES);
-            tma_load_4d(smem_base + s * S::STAGE_BYTES, &tmA, bar_full + 8 * s, ch * 64, ax, ybase + dy_, n0);
-            load_b_tile<BN>(p, &tmB, smem_base + s * S::STAGE_BYTES + S::A_BYTES, bar_full + 8 * s, ch, wtap, nb0);
+            const uint32_t st = smem_base + s * S::STAGE_BYTES;
+            mbar_expect_tx(bar_full + 8 * s, SLAB ? p.slab_bytes + S::B_BYTES : S::STAGE_BYTES);
+            tma_load_4d(st, &tmA, bar_full + 8 * s, ch * 64, ax, ybase + dy_, n0);
+            load_b_tile<BN>(p, &tmB, st + S::A_BYTES, bar_full + 8 * s, ch, wtap, nb0);
+            if constexpr (SLAB) load_b_tile<BN>(p, &tmB, st + S::A_BYTES + BN * 128, bar_full + 8 * s, ch, wtap2, nb0);
           }
           __syncwarp();
           if (++s == STAGES) { s = 0; ph ^= 1; }
-          if (++ch == p.chunks) { ch = 0; if (++tb == p.taps_w) { tb = 0; ++ta; } tap_coords(p, ta, tb, py, px, ax, dy_, wtap); }
+          if (++ch == p.chunks) { ch = 0; if (++tb == p.taps_w) { tb = 0; ++ta; } coords(); }
         }
       }
     }
@@ -460,7 +500,13 @@ __global__ void __launch_bounds__(TC_CONV_THREADS, 1) tc_conv_kernel(const __gri
         mbar_wait(bar_full + 8 * s, ph);
         wg_fence();
         const uint32_t st = smem_base + s * S::STAGE_BYTES;
-        mma_kblock<BN, NB, NACC>(acc, st + wg * 8192, st + S::A_BYTES, PS ? 0 : p.b_mn);
+        if constexpr (SLAB) {
+          const uint32_t a = st + wg * p.a_wg_bytes;
+          mma_kblock<BN, NB, NACC>(acc, a, st + S::A_BYTES, p.b_mn);
+          mma_kblock<BN, NB, NACC>(acc, a + p.a_tap_bytes, st + S::A_BYTES + BN * 128, p.b_mn);
+        } else {
+          mma_kblock<BN, NB, NACC>(acc, st + wg * 8192, st + S::A_BYTES, PS ? 0 : p.b_mn);
+        }
         wg_commit();
         wg_wait<1>();                                   // the previous K-block's MMAs are done: its stage goes back to the producer
         if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);
@@ -541,7 +587,8 @@ __global__ void __launch_bounds__(TC_CONV_THREADS, 1) tc_conv_kernel(const __gri
 
 // ------------------------------------------------------------------ host side ------------------------------
 const char* g_tc_last_kernel = "";       // name of the tensor-core kernel the most recent k_tc_* call dispatched (parity tests assert it)
-int g_tc_test_bn = 0, g_tc_test_max_ctas = 0;   // test-hook schedule overrides (kernels.h); production code never sets them
+bool g_tc_last_slab = false;             // whether the most recent k_tc_fprop / k_tc_dgrad loaded its activations as slabs
+int g_tc_test_bn = 0, g_tc_test_max_ctas = 0, g_tc_test_per_tap = 0;   // test-hook schedule overrides (kernels.h); production code never sets them
 static int tc_device() { int dev = 0; cudaGetDevice(&dev); return dev < 0 || dev >= 64 ? 0 : dev; }
 // cudaFuncAttributeMaxDynamicSharedMemorySize is per device: one flag per (kernel, device)
 #define TC_SET_SMEM_ONCE(kernel, bytes)                                                                                            \
@@ -580,32 +627,49 @@ bool tc_dgrad_supported(const ConvGeom& g) {
 static bool tc_epi_ok(const TcEpi* e, int Nt) { return !e || e->mode == EPI_PLAIN || e->mode == EPI_ACTBWD || (e->imgs_per_group > 0 && e->imgs_per_group % Nt == 0 && e->acc); }
 
 // persistent grid: one CTA per SM, or one per work item when there are fewer (a test may cap it at g_tc_test_max_ctas instead)
-template <int BN, int STAGES, int EPI, bool AFFINE, bool PS = false>
+template <int BN, int STAGES, int EPI, bool AFFINE, bool PS = false, bool SLAB = false>
 static int launch_conv_e(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, cudaStream_t s) {
-  using S = TcSmem<BN, STAGES, EPI>;
-  TC_SET_SMEM_ONCE((tc_conv_kernel<BN, STAGES, EPI, AFFINE, PS>), S::TOTAL);
+  using S = TcSmem<BN, STAGES, EPI, SLAB>;
+  TC_SET_SMEM_ONCE((tc_conv_kernel<BN, STAGES, EPI, AFFINE, PS, SLAB>), S::TOTAL);
   const long tiles = (long)p.tiles_m * p.tiles_n * p.phases;
   const unsigned grid = (unsigned)std::min<long>(tiles, g_tc_test_max_ctas > 0 ? g_tc_test_max_ctas : device_sm_count());
-  launch_pdl(tc_conv_kernel<BN, STAGES, EPI, AFFINE, PS>, dim3(grid), dim3(TC_CONV_THREADS), (size_t)(S::TOTAL), s, tmA, tmB, p);
+  launch_pdl(tc_conv_kernel<BN, STAGES, EPI, AFFINE, PS, SLAB>, dim3(grid), dim3(TC_CONV_THREADS), (size_t)(S::TOTAL), s, tmA, tmB, p);
   LAUNCHED();
   return cudaPeekAtLastError() == cudaSuccess ? 0 : -3;
 }
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool SLAB>
 static int launch_conv(const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, cudaStream_t s, const char* name) {
-  g_tc_last_kernel = name;
+  g_tc_last_kernel = name; g_tc_last_slab = SLAB;
   switch (p.epi) {
-    case EPI_STATS: return launch_conv_e<BN, STAGES, EPI_STATS, false>(tmA, tmB, p, s);
-    case EPI_BNBWD: return launch_conv_e<BN, STAGES, EPI_BNBWD, false>(tmA, tmB, p, s);
-    case EPI_ACTBWD: return launch_conv_e<BN, STAGES, EPI_ACTBWD, false>(tmA, tmB, p, s);
+    case EPI_STATS: return launch_conv_e<BN, STAGES, EPI_STATS, false, false, SLAB>(tmA, tmB, p, s);
+    case EPI_BNBWD: return launch_conv_e<BN, STAGES, EPI_BNBWD, false, false, SLAB>(tmA, tmB, p, s);
+    case EPI_ACTBWD: return launch_conv_e<BN, STAGES, EPI_ACTBWD, false, false, SLAB>(tmA, tmB, p, s);
   }
-  return (p.scale && p.bias) ? launch_conv_e<BN, STAGES, EPI_PLAIN, true>(tmA, tmB, p, s) : launch_conv_e<BN, STAGES, EPI_PLAIN, false>(tmA, tmB, p, s);
+  return (p.scale && p.bias) ? launch_conv_e<BN, STAGES, EPI_PLAIN, true, false, SLAB>(tmA, tmB, p, s) : launch_conv_e<BN, STAGES, EPI_PLAIN, false, false, SLAB>(tmA, tmB, p, s);
 }
-static int dispatch_conv(int BN, const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, cudaStream_t s) {
-  switch (BN) {
-    case 64: return launch_conv<64, 4>(tmA, tmB, p, s, "tc_conv_kernel<64,4>");
-    case 128: return launch_conv<128, 4>(tmA, tmB, p, s, "tc_conv_kernel<128,4>");
+// The label names the tile width and ring depth; the slab instantiation shares it with the per-tap one, g_tc_last_slab tells them apart.
+static int dispatch_conv(int BN, bool slab, const CUtensorMap& tmA, const CUtensorMap& tmB, const TcConvParams& p, cudaStream_t s) {
+  switch (BN * 2 + slab) {
+    case 128: return launch_conv<64, 4, false>(tmA, tmB, p, s, "tc_conv_kernel<64,4>");
+    case 256: return launch_conv<128, 4, false>(tmA, tmB, p, s, "tc_conv_kernel<128,4>");
+    case 129: return launch_conv<64, 4, true>(tmA, tmB, p, s, "tc_conv_kernel<64,4>");
   }
   return -4;
+}
+// Slab path condition: 64-column tiles (at BN = 128 a stage is 50 KB and two fit beside the park slot: on H100 that ring starves the MMAs
+// and ran 30-70 % slower than the 4-stage per-tap ring), SW128-aligned row shifts (Wt % 8 == 0), and a slab whose rows map onto the
+// consumer warpgroups' 64-row halves: one image per tile with at least two rows, or two images (one per warpgroup); at most SLAB_ROWS rows.
+static bool slab_tile(const TcConvParams& p, int BN) {
+  if (g_tc_test_per_tap || BN != 64 || p.Wt % 8) return false;
+  if (!((p.Nt == 1 && p.Ht >= 2) || (p.Nt == 2 && p.Ht * p.Wt == 64))) return false;
+  return p.Nt * (p.Ht + 1) * p.Wt <= SLAB_ROWS;
+}
+static bool is_k4s2p1_geom(const ConvGeom& g) { return g.KH == 4 && g.KW == 4 && g.SH == 2 && g.SW == 2 && g.PH == 1 && g.PW == 1 && g.H == 2 * g.OH && g.W == 2 * g.OW; }
+static void set_slab(TcConvParams& p) {
+  p.taps_h = p.mode == 0 ? 2 : 1;       // row pairs; taps_w stays 4 (fprop) / 2 (dgrad)
+  p.slab_bytes = p.Nt * (p.Ht + 1) * p.Wt * 128;
+  p.a_wg_bytes = p.Nt == 1 ? 64 * 128 : (p.Ht + 1) * p.Wt * 128;
+  p.a_tap_bytes = p.Wt * 128;
 }
 
 // weights as a 3-D tensor [rows][taps][inner] (bf16, inner contiguous)
@@ -633,15 +697,17 @@ int k_tc_fprop(const ConvGeom& g, const __nv_bfloat16* x, const __nv_bfloat16* w
   p.GH = g.OH; p.GW = g.OW; p.tiles_y = g.OH / p.Ht; p.taps_h = g.KH; p.taps_w = g.KW; p.chunks = g.C / 64; p.KW = g.KW;
   p.SH = g.SH; p.SW = g.SW; p.PH = g.PH; p.PW = g.PW; p.OC = g.O; p.outH = g.OH; p.outW = g.OW; p.out = out; p.b_mn = w_mn;
   fill_epi(p, bias, act, alpha, epi);
+  const bool slab = is_k4s2p1_geom(g) && !w_mn && slab_tile(p, BN);
+  if (slab) set_slab(p);
   CUtensorMap tmA, tmB;
   cuuint64_t dims[4] = {(cuuint64_t)g.C, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)g.N};
   cuuint64_t strides[3] = {(cuuint64_t)g.C * 2, (cuuint64_t)g.W * g.C * 2, (cuuint64_t)g.H * g.W * g.C * 2};
-  cuuint32_t box[4] = {64, (cuuint32_t)(p.Wt * g.SW), (cuuint32_t)(p.Ht * g.SH), (cuuint32_t)p.Nt};
+  cuuint32_t box[4] = {64, (cuuint32_t)(p.Wt * g.SW), (cuuint32_t)((p.Ht + slab) * g.SH), (cuuint32_t)p.Nt};
   cuuint32_t es[4] = {1, (cuuint32_t)g.SW, (cuuint32_t)g.SH, 1};
   if (make_map_bf16(&tmA, x, 4, dims, strides, box, es)) return -1;
   p.tiles_m = g.N * g.OH * g.OW / 128; p.tiles_n = g.O / BN; p.phases = 1;
   if (w_mn ? weight_map(&tmB, w, g.C, 1, g.O, 64) : weight_map(&tmB, w, g.O, g.KH * g.KW, g.C, BN)) return -1;
-  return dispatch_conv(BN, tmA, tmB, p, s);
+  return dispatch_conv(BN, slab, tmA, tmB, p, s);
 }
 
 // conv input gradient = transposed-conv forward, 4x4 s2 p1, in sub-pixel phase form.  w is the STRAIGHT copy [O][16][C]: the reduction runs
@@ -653,19 +719,20 @@ int k_tc_dgrad(const ConvGeom& g, const __nv_bfloat16* dy, const __nv_bfloat16* 
   p.GH = g.OH; p.GW = g.OW; p.tiles_y = g.OH / p.Ht; p.taps_h = 2; p.taps_w = 2; p.chunks = g.O / 64; p.KW = 4;
   p.SH = 1; p.SW = 1; p.PH = 0; p.PW = 0; p.OC = g.C; p.outH = g.H; p.outW = g.W; p.out = dx; p.b_mn = 1;
   fill_epi(p, bias, act, alpha, epi);
+  const bool slab = slab_tile(p, BN);
+  if (slab) set_slab(p);
   CUtensorMap tmA, tmB;
   cuuint64_t dims[4] = {(cuuint64_t)g.O, (cuuint64_t)g.OW, (cuuint64_t)g.OH, (cuuint64_t)g.N};
   cuuint64_t strides[3] = {(cuuint64_t)g.O * 2, (cuuint64_t)g.OW * g.O * 2, (cuuint64_t)g.OH * g.OW * g.O * 2};
-  cuuint32_t box[4] = {64, (cuuint32_t)p.Wt, (cuuint32_t)p.Ht, (cuuint32_t)p.Nt};
+  cuuint32_t box[4] = {64, (cuuint32_t)p.Wt, (cuuint32_t)(p.Ht + slab), (cuuint32_t)p.Nt};
   cuuint32_t es[4] = {1, 1, 1, 1};
   if (weight_map(&tmB, w, g.O, 16, g.C, 64)) return -1;
   if (make_map_bf16(&tmA, dy, 4, dims, strides, box, es)) return -1;
   p.tiles_m = g.N * g.OH * g.OW / 128; p.tiles_n = g.C / BN; p.phases = 4;
-  return dispatch_conv(BN, tmA, tmB, p, s);
+  return dispatch_conv(BN, slab, tmA, tmB, p, s);
 }
 
 // ------------------------------------------------------------------ transposed conv onto <= 4 channels ------
-static bool is_k4s2p1_geom(const ConvGeom& g) { return g.KH == 4 && g.KW == 4 && g.SH == 2 && g.SW == 2 && g.PH == 1 && g.PW == 1 && g.H == 2 * g.OH && g.W == 2 * g.OW; }
 bool tc_deconv_ps_shape(const ConvGeom& g) { return is_k4s2p1_geom(g) && g.C >= 1 && g.C <= 4 && g.O % 64 == 0; }
 bool tc_deconv_ps_supported(const ConvGeom& g) { int a, b, c; return tc_deconv_ps_shape(g) && pick_row_tile(g.N, g.OH, g.OW, 128, &a, &b, &c); }
 size_t k_tc_deconv_ps_weight_elems(const ConvGeom& g) { return tc_deconv_ps_shape(g) ? (size_t)16 * 9 * g.O : 0; }
@@ -1027,9 +1094,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_wgrad_kernel(const __grid_co
       wg_fence();
       const uint32_t a = smem_base + s * S::STAGE_BYTES + wg * 8192, b = smem_base + s * S::STAGE_BYTES + S::A_BYTES;
 #pragma unroll
-      for (int k = 0; k < 4; ++k)     // 16 pixel rows per MMA = 2048 B down both tiles
-#pragma unroll
-        for (int nb = 0; nb < NB; ++nb) wgmma_n64<1, 1>(acc[nb], desc_mnmajor_sw128(a + k * 2048, 8192), desc_mnmajor_sw128(b + nb * 8192 + k * 2048, 8192));
+      for (int k = 0; k < 4; ++k) {   // 16 pixel rows per MMA = 2048 B down both tiles
+        if constexpr (NB == 2) wgmma_n128<1, 1>(acc[0], acc[1], desc_mnmajor_sw128(a + k * 2048, 8192), desc_mnmajor_sw128(b + k * 2048, 8192));
+        else wgmma_n64<1, 1>(acc[0], desc_mnmajor_sw128(a + k * 2048, 8192), desc_mnmajor_sw128(b + k * 2048, 8192));
+      }
       wg_commit();
       wg_wait<1>();
       if (prev >= 0 && lane == 0) mbar_arrive(bar_empty + 8 * prev);

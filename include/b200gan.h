@@ -287,6 +287,8 @@ typedef struct {
   int32_t max_ctas;       /* impl 1 / impl 3 kind 1: grid = min(work items, max_ctas) instead of min(work items, SMs); may exceed the SM count */
   int32_t poison;         /* kinds 0 / 1: fill the output with 0xFF bytes (bf16 NaN) before every launch, warm-up included */
   int32_t w_mn;           /* impl 1 kind 0, 1x1 geometry: the weight operand is [C][O] (the dense input gradient's own [nOut][nIn] weight) */
+  int32_t per_tap;        /* impl 1: load the activations one box per tap also where the 4x4 s2 p1 slab path applies */
+  int32_t slab;           /* out: 1 when the launch loaded its activations as slabs shared by two taps */
 } b2g_test_conv_opts;
 int32_t b2g_test_conv_ex(b2g_ctx* ctx, int32_t kind, int32_t impl, int32_t precision, const b2g_conv_geom* g,
                          const float* x_or_dy, const float* w_or_x, float* out, int32_t iters, float* ms_per_iter, b2g_test_conv_opts* opts);
