@@ -37,6 +37,13 @@ class GanConfig(C.Structure):
     _fields_ = [("fake_bn_train", C.c_int32), ("use_cuda_graph", C.c_int32)]
 
 
+class LrSchedule(C.Structure):
+    """b2g_lr_schedule: one DL4J ISchedule (kind, ScheduleType, its parameters, and a MapSchedule's entries, copied during the call)."""
+    _fields_ = [("kind", C.c_int32), ("type", C.c_int32), ("initial", C.c_double), ("gamma", C.c_double), ("power", C.c_double),
+                ("step", C.c_double), ("decay_rate", C.c_double), ("n_map", C.c_int32), ("map_keys", C.POINTER(C.c_int32)),
+                ("map_values", C.POINTER(C.c_double))]
+
+
 class ConvGeom(C.Structure):
     _fields_ = [(k, C.c_int32) for k in ("n", "h", "w", "c", "oh", "ow", "o", "kh", "kw", "sh", "sw", "ph", "pw")]
 
@@ -86,6 +93,10 @@ PROTOTYPES = {
     "b2g_net_get_dropout_pass": (_i32, [_vp, C.POINTER(_i64)]),
     "b2g_net_set_dropout_pass": (_i32, [_vp, _i64]),
     "b2g_net_set_gradient_normalization": (_i32, [_vp, _i32, C.c_float]),
+    "b2g_net_set_lr_schedule": (_i32, [_vp, C.c_char_p, C.POINTER(LrSchedule)]),
+    "b2g_net_get_learning_rate": (_i32, [_vp, C.c_char_p, _fp]),
+    "b2g_net_get_epoch": (_i32, [_vp, C.POINTER(_i64)]),
+    "b2g_net_set_epoch": (_i32, [_vp, _i64]),
     "b2g_net_simt_gemm_calls": (_i32, [_vp, C.POINTER(C.c_uint64)]),
     "b2g_gan_create": (_i32, [_vp, _vp, C.POINTER(GanConfig), _pvp]),
     "b2g_gan_destroy": (_i32, [_vp]),

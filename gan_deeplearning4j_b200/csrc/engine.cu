@@ -127,13 +127,22 @@ struct b2g_net {
   unsigned* upd_ticket = nullptr;                                  // block-completion counter of the updater kernel (the last block bumps step_dev)
   unsigned long long* drop_pass = nullptr;                         // dropout pass counter P (device): read by every dropout kernel of a train-mode pass
   unsigned* drop_ticket = nullptr;                                 // block-completion counter of the pass's last dropout kernel (its last block bumps P)
-  // L2 gradient normalization (b2g_net_set_gradient_normalization): mode, threshold and a generation bumped on every change (a captured GAN
-  // step holds the mode's launches, so it is re-captured when the generation differs); norm groups per layer and per segment; the norm
+  // Updater settings generation: bumped by every gradient-normalization or learning-rate-schedule change (a captured GAN step holds the
+  // launches and kernel instantiations those settings select, so it is re-captured when the generation differs)
+  uint64_t settings_gen = 0;
+  // L2 gradient normalization (b2g_net_set_gradient_normalization): mode and threshold; norm groups per layer and per segment; the norm
   // kernel's per-chunk partial sums, block-completion counter and per-segment multipliers
-  int gn_mode = B2G_GN_NONE; float gn_threshold = 1.0f; uint64_t gn_gen = 0;
+  int gn_mode = B2G_GN_NONE; float gn_threshold = 1.0f;
   GnGroup *gn_layer_groups = nullptr, *gn_param_groups = nullptr; int gn_n_layer_groups = 0, gn_n_param_groups = 0;
   double* gn_partial = nullptr; unsigned* gn_ticket = nullptr; float* gn_mult = nullptr;
-  ReduceList pending{};                                            // split-K partial sums queued by this backward pass
+  // Learning-rate schedules (b2g_net_set_lr_schedule): per layer on the host (MAP entries included), per segment on the device with the
+  // MAP entries in sched_map (reallocated when the entries outgrow it); sched_on = some segment has one (selects the scheduled updater);
+  // the epoch word EPOCH schedules read; a one-float result slot of b2g_net_get_learning_rate
+  struct LayerSched { UpdSched sc{}; std::vector<int32_t> keys; std::vector<double> vals; };
+  std::vector<LayerSched> layer_sched; std::vector<int> seg_layer;
+  UpdSched* sched_dev = nullptr; bool sched_on = false; void* sched_map = nullptr; size_t sched_map_bytes = 0;
+  int64_t* epoch_dev = nullptr; float* lr_out = nullptr;
+  ReduceList pending{};                                           // split-K partial sums queued by this backward pass
   uint64_t simt_gemm_calls = 0;                                    // BF16 nets: GEMM-shaped ops that ran on the SIMT kernels (skinny / unsupported shapes) -- reported, never silent
   float* scratch = nullptr; size_t scratch_floats = 0;
   float* loss_dev = nullptr;           // [8]
@@ -390,6 +399,12 @@ static int32_t net_init_params_and_updater(b2g_net* n) {
     B2(dalloc(n, &n->gn_ticket, sizeof(unsigned))); CU(cudaMemsetAsync(n->gn_ticket, 0, sizeof(unsigned), s));
     CU(cudaMemcpyAsync(n->gn_layer_groups, per_layer.data(), sizeof(GnGroup) * per_layer.size(), cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(n->gn_param_groups, per_param.data(), sizeof(GnGroup) * per_param.size(), cudaMemcpyHostToDevice, s));
+  }
+  {  // learning-rate schedules: none yet (every segment kind 0), epoch 0
+    n->seg_layer = seg_layer; n->layer_sched.assign(n->L.size(), b2g_net::LayerSched{});
+    B2(dalloc(n, &n->sched_dev, sizeof(UpdSched) * std::max<size_t>(1, n->segs.size()))); CU(cudaMemsetAsync(n->sched_dev, 0, sizeof(UpdSched) * std::max<size_t>(1, n->segs.size()), s));
+    B2(dalloc(n, &n->epoch_dev, sizeof(int64_t))); CU(cudaMemsetAsync(n->epoch_dev, 0, sizeof(int64_t), s));
+    B2(dalloc(n, &n->lr_out, sizeof(float)));
   }
   n->n_l2 = (int)l2o.size();
   if (n->n_l2) {
@@ -756,9 +771,10 @@ static int32_t net_update(b2g_net* n, int mb_local) {
     k_gradnorm(n->grads, n->segs_dev, n->chunk_seg_dev, n->chunk_off_dev, n->nchunks, per_layer ? n->gn_layer_groups : n->gn_param_groups,
                per_layer ? n->gn_n_layer_groups : n->gn_n_param_groups, clip ? 1 : 0, n->gn_threshold, inv_mb, inv_world, n->gn_partial, n->gn_ticket, n->gn_mult, s);
   }
-  // one pass: /mb -> [x multiplier] -> clip -> updater -> +l2*W -> theta -= g, the bf16 operand copies (straight and packed) and the iteration counter
+  // one pass: /mb -> [x multiplier] -> clip -> updater [at the scheduled lr] -> +l2*W -> theta -= g, the bf16 operand copies (straight and
+  // packed) and the iteration counter
   k_updater(n->params, n->grads, n->st0, n->st1, n->segs_dev, n->chunk_seg_dev, n->chunk_off_dev, n->nchunks, inv_mb, inv_world, n->step_dev, n->upd_ticket, n->shadow,
-            gn ? n->gn_mult : nullptr, s);
+            gn ? n->gn_mult : nullptr, n->sched_on ? n->sched_dev : nullptr, n->epoch_dev, s);
   CHECK_KERNELS();
   return 0;
 }
@@ -832,6 +848,7 @@ extern "C" int32_t b2g_net_destroy(b2g_net* n) {
   if (!n) return 0; cudaSetDevice(n->ctx->device); cudaStreamSynchronize(n->ctx->stream); cudaStreamSynchronize(n->ctx->side);
   for (auto e : n->ev_fork) if (e) cudaEventDestroy(e); for (auto e : n->ev_done) if (e) cudaEventDestroy(e); if (n->ev_join) cudaEventDestroy(n->ev_join);
   if (n->p2p) for (int r = 0; r < n->ctx->world; ++r) if (r != n->ctx->rank && n->p2p_peer_grads[r]) cudaIpcCloseMemHandle(n->p2p_peer_grads[r]);
+  if (n->sched_map) cudaFree(n->sched_map);
   for (void* p : n->allocs) cudaFree(p); delete n; return 0;
 }
 extern "C" int32_t b2g_net_num_params(b2g_net* n, int64_t* out) { if (!n || !out) return fail(B2G_ERR_ARG, "null"); *out = n->n_params; return 0; }
@@ -988,7 +1005,7 @@ struct b2g_gan {
   float* loss_dev = nullptr;              // [4]: d_real_sum, d_fake_sum, g_sum
   float* stage = nullptr; size_t stage_floats = 0;
   cudaGraph_t graph = nullptr, graph1 = nullptr; cudaGraphExec_t exec = nullptr, exec1 = nullptr; int graph_batch = 0; uint64_t graph_launches = 0, graph_simt_g = 0, graph_simt_d = 0;
-  uint64_t graph_gn_g = 0, graph_gn_d = 0;   // the nets' gradient-normalization generations the captured graph was made with
+  uint64_t graph_settings_g = 0, graph_settings_d = 0;   // the nets' updater settings generations the captured graph was made with
   cudaEvent_t ev0 = nullptr, ev1 = nullptr; float last_ms = 0.f; int last_batch = 1; bool nccl_warm = false;
   cudaStream_t copy_stream = nullptr; cudaEvent_t ev_x = nullptr; bool ev1_valid = false;   // x_real's H2D runs under the generator's forward
   std::vector<void*> allocs;
@@ -1108,7 +1125,7 @@ extern "C" int32_t b2g_gan_step_resident(b2g_gan* g, int32_t batch) {
   CU(cudaEventRecord(g->ev0, s));
   if (!use_graph) { B2(gan_step_part1(g, batch)); CU(cudaStreamWaitEvent(s, g->ev_x, 0)); B2(gan_step_part2(g, batch)); }
   else {
-    if (!g->exec || g->graph_batch != batch || g->graph_gn_g != g->G->gn_gen || g->graph_gn_d != g->D->gn_gen) {
+    if (!g->exec || g->graph_batch != batch || g->graph_settings_g != g->G->settings_gen || g->graph_settings_d != g->D->settings_gen) {
       if (g->exec) { cudaGraphExecDestroy(g->exec); g->exec = nullptr; } if (g->graph) { cudaGraphDestroy(g->graph); g->graph = nullptr; }
       if (g->exec1) { cudaGraphExecDestroy(g->exec1); g->exec1 = nullptr; } if (g->graph1) { cudaGraphDestroy(g->graph1); g->graph1 = nullptr; }
       uint64_t before = g_launch_count; const uint64_t sg0 = g->G->simt_gemm_calls, sd0 = g->D->simt_gemm_calls;
@@ -1123,7 +1140,7 @@ extern "C" int32_t b2g_gan_step_resident(b2g_gan* g, int32_t batch) {
       g->graph_simt_g = g->G->simt_gemm_calls - sg0; g->graph_simt_d = g->D->simt_gemm_calls - sd0; g->G->simt_gemm_calls = sg0; g->D->simt_gemm_calls = sd0;
       if (r) return r; if (e != cudaSuccess) return fail(B2G_ERR_CUDA, "graph capture: %s", cudaGetErrorString(e));
       CU(cudaGraphInstantiate(&g->exec1, g->graph1, 0)); CU(cudaGraphInstantiate(&g->exec, g->graph, 0)); g->graph_batch = batch;
-      g->graph_gn_g = g->G->gn_gen; g->graph_gn_d = g->D->gn_gen;
+      g->graph_settings_g = g->G->settings_gen; g->graph_settings_d = g->D->settings_gen;
     }
     CU(cudaGraphLaunch(g->exec1, s));
     CU(cudaStreamWaitEvent(s, g->ev_x, 0));
@@ -1179,8 +1196,101 @@ extern "C" int32_t b2g_net_set_gradient_normalization(b2g_net* n, int32_t mode, 
   const bool clip = mode == B2G_GN_CLIP_L2_LAYER || mode == B2G_GN_CLIP_L2_PARAM;
   if (clip && !(threshold > 0.f && isfinite(threshold))) return fail(B2G_ERR_ARG, "gradient normalization threshold %g: the clip modes need a finite threshold > 0", (double)threshold);
   if (!clip) threshold = 1.0f;      // the renormalize modes ignore it
-  if (mode != n->gn_mode || threshold != n->gn_threshold) { n->gn_mode = mode; n->gn_threshold = threshold; ++n->gn_gen; }
+  if (mode != n->gn_mode || threshold != n->gn_threshold) { n->gn_mode = mode; n->gn_threshold = threshold; ++n->settings_gen; }
   return 0;
+}
+
+// ------------------------------------------------------------------ learning-rate schedules ---------------
+// A layer has a learning rate when it is not frozen, has parameters and its updater is not NoOp: when it owns an updater segment that is not
+// a NoOp one (frozen layers own no segments; a NoOp updater and BatchNorm mean/var make NoOp segments).  The Python layer specs apply the same
+// rule (engine.py layer_has_lr); b2g_net_get_learning_rate reads the layer's first such segment.
+static int lr_segment(const b2g_net* n, int li) {
+  for (size_t i = 0; i < n->segs.size(); ++i) if (n->seg_layer[i] == li && n->segs[i].kind != 3) return (int)i;
+  return -1;
+}
+static bool layer_has_lr(const b2g_net* n, int li) { return lr_segment(n, li) >= 0; }
+static int32_t find_lr_layer(const b2g_net* n, const char* layer, int* li) {
+  for (size_t i = 0; i < n->L.size(); ++i) if (!strncmp(n->L[i].d.name, layer, B2G_NAME_LEN)) {
+    if (!layer_has_lr(n, (int)i)) return fail(B2G_ERR_ARG, "layer %s has no learning rate (frozen, no parameters, or NoOp)", layer);
+    *li = (int)i; return 0;
+  }
+  return fail(B2G_ERR_ARG, "no layer named %s", layer);
+}
+// Rebuilds the per-segment table from the per-layer schedules: MAP entries go to sched_map (values, then keys), every segment of a layer with
+// a learning rate carries the layer's schedule (the BatchNorm mean/var segments too; their NoOp update ignores it).
+static int32_t net_upload_schedules(b2g_net* n) {
+  cudaStream_t s = n->ctx->stream;
+  size_t nv = 0; for (auto& ls : n->layer_sched) nv += ls.vals.size();
+  const size_t bytes = nv * (sizeof(double) + sizeof(int32_t));
+  CU(cudaStreamSynchronize(s));                  // nothing in flight reads the old table or map
+  if (bytes > n->sched_map_bytes) {
+    if (n->sched_map) { cudaFree(n->sched_map); n->sched_map = nullptr; n->sched_map_bytes = 0; }
+    cudaError_t e = cudaMalloc(&n->sched_map, bytes);
+    if (e != cudaSuccess) { n->sched_map = nullptr; return fail(B2G_ERR_OOM, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); }
+    n->sched_map_bytes = bytes;
+  }
+  std::vector<char> host(bytes); double* dv = (double*)n->sched_map; int32_t* dk = (int32_t*)((char*)n->sched_map + nv * sizeof(double));
+  std::vector<UpdSched> per_layer(n->L.size()); size_t at = 0;
+  for (size_t li = 0; li < n->L.size(); ++li) {
+    const auto& ls = n->layer_sched[li]; per_layer[li] = ls.sc;
+    if (ls.sc.kind == B2G_SCHED_MAP) {
+      memcpy(host.data() + at * sizeof(double), ls.vals.data(), ls.vals.size() * sizeof(double));
+      memcpy(host.data() + nv * sizeof(double) + at * sizeof(int32_t), ls.keys.data(), ls.keys.size() * sizeof(int32_t));
+      per_layer[li].vals = dv + at; per_layer[li].keys = dk + at; at += ls.vals.size();
+    }
+  }
+  std::vector<UpdSched> seg(n->segs.size()); bool on = false;
+  for (size_t i = 0; i < n->segs.size(); ++i) { seg[i] = per_layer[n->seg_layer[i]]; on = on || seg[i].kind != B2G_SCHED_NONE; }
+  if (bytes) CU(cudaMemcpyAsync(n->sched_map, host.data(), bytes, cudaMemcpyHostToDevice, s));
+  if (!seg.empty()) CU(cudaMemcpyAsync(n->sched_dev, seg.data(), sizeof(UpdSched) * seg.size(), cudaMemcpyHostToDevice, s));
+  CU(cudaStreamSynchronize(s));
+  n->sched_on = on; ++n->settings_gen;
+  return 0;
+}
+extern "C" int32_t b2g_net_set_lr_schedule(b2g_net* n, const char* layer, const b2g_lr_schedule* s) {
+  if (!n) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
+  b2g_net::LayerSched ls;
+  if (s && s->kind != B2G_SCHED_NONE) {
+    if (s->kind < B2G_SCHED_EXPONENTIAL || s->kind > B2G_SCHED_MAP) return fail(B2G_ERR_ARG, "unknown schedule kind %d (PolySchedule is not supported)", s->kind);
+    if (s->type != B2G_SCHED_ITERATION && s->type != B2G_SCHED_EPOCH) return fail(B2G_ERR_ARG, "unknown schedule type %d", s->type);
+    if (!std::isfinite(s->initial) || !std::isfinite(s->gamma) || !std::isfinite(s->power) || !std::isfinite(s->step) || !std::isfinite(s->decay_rate))
+      return fail(B2G_ERR_ARG, "schedule parameters must be finite");
+    if (s->kind == B2G_SCHED_STEP && !(s->step > 0.0)) return fail(B2G_ERR_ARG, "StepSchedule step %g: must be > 0", s->step);
+    if (s->kind == B2G_SCHED_INVERSE && s->gamma < 0.0) return fail(B2G_ERR_ARG, "InverseSchedule gamma %g: must be >= 0", s->gamma);
+    UpdSched& sc = ls.sc; sc.kind = s->kind; sc.type = s->type;
+    sc.initial = s->initial; sc.gamma = s->gamma; sc.power = s->power; sc.step = s->step; sc.decay = s->decay_rate;
+    if (s->kind == B2G_SCHED_MAP) {
+      if (s->n_map < 1 || !s->map_keys || !s->map_values) return fail(B2G_ERR_ARG, "MapSchedule needs at least one entry");
+      bool has0 = false;
+      for (int j = 0; j < s->n_map; ++j) {
+        if (j > 0 && s->map_keys[j] <= s->map_keys[j - 1]) return fail(B2G_ERR_ARG, "MapSchedule keys must strictly increase");
+        if (!std::isfinite(s->map_values[j])) return fail(B2G_ERR_ARG, "MapSchedule values must be finite");
+        has0 = has0 || s->map_keys[j] == 0;
+      }
+      if (!has0) return fail(B2G_ERR_ARG, "MapSchedule has no value for key 0");
+      ls.keys.assign(s->map_keys, s->map_keys + s->n_map); ls.vals.assign(s->map_values, s->map_values + s->n_map); sc.n_map = s->n_map;
+    }
+  }
+  if (layer) { int li = 0; B2(find_lr_layer(n, layer, &li)); n->layer_sched[li] = ls; }
+  else for (size_t li = 0; li < n->L.size(); ++li) if (layer_has_lr(n, (int)li)) n->layer_sched[li] = ls;
+  return net_upload_schedules(n);
+}
+extern "C" int32_t b2g_net_get_learning_rate(b2g_net* n, const char* layer, float* out) {
+  if (!n || !layer || !out) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
+  int li = 0; B2(find_lr_layer(n, layer, &li));
+  const int seg = lr_segment(n, li);
+  k_sched_lr(n->segs_dev, n->sched_dev, seg, n->step_dev, n->epoch_dev, n->lr_out, n->ctx->stream); CHECK_KERNELS();
+  CU(cudaMemcpyAsync(out, n->lr_out, sizeof(float), cudaMemcpyDeviceToHost, n->ctx->stream)); CU(cudaStreamSynchronize(n->ctx->stream));
+  return 0;
+}
+// The epoch word lives on the device like the iteration counter: a replayed graph reads the value set last, no re-capture needed.
+extern "C" int32_t b2g_net_get_epoch(b2g_net* n, int64_t* out) {
+  if (!n || !out) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
+  int64_t v = 0; CU(cudaMemcpyAsync(&v, n->epoch_dev, sizeof(v), cudaMemcpyDeviceToHost, n->ctx->stream)); CU(cudaStreamSynchronize(n->ctx->stream)); *out = v; return 0;
+}
+extern "C" int32_t b2g_net_set_epoch(b2g_net* n, int64_t epoch) {
+  if (!n || epoch < 0) return fail(B2G_ERR_ARG, "bad epoch"); CU(cudaSetDevice(n->ctx->device));
+  CU(cudaMemcpyAsync(n->epoch_dev, &epoch, sizeof(epoch), cudaMemcpyHostToDevice, n->ctx->stream)); CU(cudaStreamSynchronize(n->ctx->stream)); return 0;
 }
 extern "C" int32_t b2g_net_simt_gemm_calls(b2g_net* n, uint64_t* out) { if (!n || !out) return fail(B2G_ERR_ARG, "null"); *out = n->simt_gemm_calls; return 0; }
 
@@ -1513,7 +1623,8 @@ extern "C" int32_t b2g_test_hbm_kernels(b2g_net* n, int32_t rows, int32_t channe
   for (int which = 0; which < 3; ++which) for (int it = -1; it < iters; ++it) {
     B2(b2g_flush_l2(c));
     CU(cudaEventRecord(e0, s));
-    if (which == 0) k_updater(n->params, n->grads, n->st0, n->st1, n->segs_dev, n->chunk_seg_dev, n->chunk_off_dev, n->nchunks, 1.0f, 1.0f, n->step_dev, n->upd_ticket, n->shadow, nullptr, s);
+    if (which == 0) k_updater(n->params, n->grads, n->st0, n->st1, n->segs_dev, n->chunk_seg_dev, n->chunk_off_dev, n->nchunks, 1.0f, 1.0f, n->step_dev, n->upd_ticket, n->shadow, nullptr,
+                              nullptr, nullptr, s);
     else if (which == 1) k_bn_apply_acc(x, y, rows, channels, 1, acc, gb, gb + channels, ACT_LRELU, 0.2f, 1e-5f, coef, gb + 2 * channels, gb + 3 * channels, nullptr, nullptr, 0.9f, s);
     else k_bn_bwd_apply_acc(x, e, y, rows, channels, 1, coef, ACT_LRELU, 0.2f, 1, acc, gb, gb + channels, 0, s);
     CU(cudaEventRecord(e1, s)); CU(cudaEventSynchronize(e1));

@@ -125,11 +125,23 @@ struct UpdSeg {            // one parameter tensor
   int64_t off_bf, off_ps;
   int ps_O, ps_C;
 };
+// Learning-rate schedule of one segment (b2g_lr_schedule; kind 0 = the segment's constant lr).  keys / vals: the MAP schedule's entries in
+// the net's device memory.  Kept beside UpdSeg, not in it, so that the unscheduled updater reads the segment table it always read.
+struct UpdSched {
+  int kind, type;          // b2g_schedule_kind, b2g_schedule_type
+  int n_map;
+  double initial, gamma, power, step, decay;
+  const int32_t* keys; const double* vals;
+};
 // The last block to finish bumps *step_dev (Adam's t) and resets *ticket: no separate counter kernel.
 // gn_mult (may be null): one fp32 multiplier per segment (k_gradnorm), applied to g right after the minibatch division.
+// sched (may be null): one UpdSched per segment; each block then takes its segment's lr from the schedule at iteration *step_dev (before the
+// increment) or at epoch *epoch_dev, both read from device memory.
 void k_updater(float* params, const float* grads, float* st0, float* st1, const UpdSeg* segs_dev, const int32_t* chunk_seg_dev,
                const int64_t* chunk_off_dev, int nchunks, float inv_mb, float inv_world, int* step_dev /* t = *step_dev + 1 */, unsigned* ticket,
-               __nv_bfloat16* shadow, const float* gn_mult, cudaStream_t s);
+               __nv_bfloat16* shadow, const float* gn_mult, const UpdSched* sched, const int64_t* epoch_dev, cudaStream_t s);
+// *out = the fp32 learning rate the updater kernel would use for segment seg at the current *step_dev / *epoch_dev (one thread, one launch)
+void k_sched_lr(const UpdSeg* segs_dev, const UpdSched* sched, int seg, const int* step_dev, const int64_t* epoch_dev, float* out, cudaStream_t s);
 static const int UPD_CHUNK = 4096;
 
 // ---- L2 gradient normalization (DL4J GradientNormalization.{Renormalize,Clip}L2Per{Layer,ParamType}; kernels_gradnorm.cu) ---------

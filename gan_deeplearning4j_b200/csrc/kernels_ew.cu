@@ -891,16 +891,41 @@ __device__ __forceinline__ void upd_shadow(const UpdSeg& sg, __nv_bfloat16* __re
     shadow[sg.off_ps + ((int64_t)((py * 8 + px * 4 + c) * 9 + (dyr + 1) * 3 + (dxc + 1))) * sg.ps_O + o] = pb;
   }
 }
-template <bool SCALED>
+// The learning rate of a segment at iteration `it` (the counter before this update's increment) / epoch `ep`: DL4J's ISchedule.valueAt in
+// double, rounded to fp32 once (include/b200gan.h, b2g_lr_schedule); kind 0 = the constant lr.
+__device__ float sched_lr(const UpdSched& sc, float lr, int it, long long ep) {
+  if (sc.kind == 0) return lr;
+  const long long ii = sc.type == 1 ? ep : (long long)it;
+  const double i = (double)ii;
+  double v;
+  if (sc.kind == 1) v = sc.initial * pow(sc.gamma, i);
+  else if (sc.kind == 2) v = sc.initial / pow(1.0 + sc.gamma * i, sc.power);
+  else if (sc.kind == 3) v = sc.initial / (1.0 + exp(-sc.gamma * (i - sc.step)));
+  else if (sc.kind == 4) v = sc.initial * pow(sc.decay, floor(i / sc.step));
+  else {          // MAP: the largest key <= i (keys strictly increase, keys[0] <= 0 <= i)
+    int lo = 0, hi = sc.n_map - 1;
+    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if ((long long)sc.keys[mid] <= ii) lo = mid; else hi = mid - 1; }
+    v = sc.vals[lo];
+  }
+  return (float)v;
+}
+// SCHED: the segment's lr comes from its schedule (thread 0 evaluates it once per block, at *step before the increment or at *epoch)
+template <bool SCALED, bool SCHED>
 __global__ void __launch_bounds__(256) updater_kernel(float* __restrict__ params, const float* __restrict__ grads, float* __restrict__ st0, float* __restrict__ st1,
                                                       const UpdSeg* __restrict__ segs, const int32_t* __restrict__ chunk_seg, const int64_t* __restrict__ chunk_off,
                                                       float inv_mb, float inv_world, int* __restrict__ step, unsigned* __restrict__ ticket, __nv_bfloat16* __restrict__ shadow,
-                                                      const float* __restrict__ gn_mult) { pdl_enter();
-  const UpdSeg sg = segs[chunk_seg[blockIdx.x]];
+                                                      const float* __restrict__ gn_mult, const UpdSched* __restrict__ sched, const int64_t* __restrict__ epoch) { pdl_enter();
+  UpdSeg sg = segs[chunk_seg[blockIdx.x]];
   const float gmult = SCALED ? gn_mult[chunk_seg[blockIdx.x]] : 1.0f;
   const int64_t base = chunk_off[blockIdx.x];
   const int64_t end = min(base + (int64_t)UPD_CHUNK, sg.off + sg.len);
   const int t = *step + 1;
+  if (SCHED) {
+    __shared__ float lr_s;
+    if (threadIdx.x == 0) lr_s = sched_lr(sched[chunk_seg[blockIdx.x]], sg.lr, t - 1, (long long)*epoch);
+    __syncthreads();
+    sg.lr = lr_s;
+  }
   float alpha_t = 0.f;
   if (sg.kind == 2) alpha_t = sg.lr * sqrtf(1.0f - powf(sg.b2, (float)t)) / (1.0f - powf(sg.b1, (float)t));
   const float gscale = sg.div_mb ? inv_mb : inv_world;     // BN running-stat pseudo-gradients: no /mb, mean over ranks
@@ -949,11 +974,19 @@ __global__ void __launch_bounds__(256) updater_kernel(float* __restrict__ params
   }
 }
 void k_updater(float* params, const float* grads, float* st0, float* st1, const UpdSeg* segs, const int32_t* chunk_seg, const int64_t* chunk_off,
-               int nchunks, float inv_mb, float inv_world, int* step_dev, unsigned* ticket, __nv_bfloat16* shadow, const float* gn_mult, cudaStream_t s) {
+               int nchunks, float inv_mb, float inv_world, int* step_dev, unsigned* ticket, __nv_bfloat16* shadow, const float* gn_mult,
+               const UpdSched* sched, const int64_t* epoch_dev, cudaStream_t s) {
   if (!nchunks) return;
-  if (gn_mult) launch_pdl(updater_kernel<true>, dim3(nchunks), dim3(256), (size_t)(0), s, params, grads, st0, st1, segs, chunk_seg, chunk_off, inv_mb, inv_world, step_dev, ticket, shadow, gn_mult);
-  else launch_pdl(updater_kernel<false>, dim3(nchunks), dim3(256), (size_t)(0), s, params, grads, st0, st1, segs, chunk_seg, chunk_off, inv_mb, inv_world, step_dev, ticket, shadow, gn_mult);
+  auto kern = gn_mult ? (sched ? updater_kernel<true, true> : updater_kernel<true, false>) : (sched ? updater_kernel<false, true> : updater_kernel<false, false>);
+  launch_pdl(kern, dim3(nchunks), dim3(256), (size_t)(0), s, params, grads, st0, st1, segs, chunk_seg, chunk_off, inv_mb, inv_world, step_dev, ticket, shadow, gn_mult,
+             sched, epoch_dev);
   LAUNCHED();
+}
+__global__ void sched_lr_kernel(const UpdSeg* segs, const UpdSched* sched, int seg, const int* step, const int64_t* epoch, float* out) {
+  if (threadIdx.x == 0 && blockIdx.x == 0) *out = sched_lr(sched[seg], segs[seg].lr, *step, (long long)*epoch);
+}
+void k_sched_lr(const UpdSeg* segs, const UpdSched* sched, int seg, const int* step_dev, const int64_t* epoch_dev, float* out, cudaStream_t s) {
+  sched_lr_kernel<<<1, 32, 0, s>>>(segs, sched, seg, step_dev, epoch_dev, out); LAUNCHED();
 }
 __global__ void fill_f32_kernel(float* p, float v, size_t n) { pdl_enter();
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] = v;

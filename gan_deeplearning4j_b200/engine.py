@@ -6,13 +6,15 @@ All tensors cross as NumPy fp32 arrays in DL4J layouts (NCHW / [N,F]; parameters
 """
 from __future__ import annotations
 
+import copy
 import ctypes as C
+import math
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
 from . import _lib
-from ._lib import GanConfig, LayerDesc, NetConfig, check
+from ._lib import GanConfig, LayerDesc, LrSchedule, NetConfig, check
 
 LAYER_TYPES = {"conv2d": 0, "deconv2d": 1, "batchnorm": 2, "dense": 3, "activation": 4, "maxpool": 5, "upsample2d": 6,
                "output": 7, "loss": 8, "ff_to_cnn": 9, "cnn_to_ff": 10, "dropout": 11}
@@ -21,7 +23,81 @@ UPDATERS = {"sgd": 0, "rmsprop": 1, "adam": 2, "noop": 3}
 # DL4J GradientNormalization -> b2g_gradient_normalization (DL4J's ordinals).  ClipElementWiseAbsoluteValue is the `grad_clip` argument of Net.
 GRADIENT_NORMALIZATIONS = {"none": 0, "renormalize_l2_per_layer": 1, "renormalize_l2_per_param_type": 2, "clip_l2_per_layer": 4,
                            "clip_l2_per_param_type": 5}
+# DL4J ISchedule -> b2g_schedule_kind / b2g_schedule_type (models.py builds the dicts: exponential_schedule, ..., map_schedule)
+SCHEDULE_KINDS = {"exponential": 1, "inverse": 2, "sigmoid": 3, "step": 4, "map": 5}
+SCHEDULE_TYPES = {"iteration": 0, "epoch": 1}
 FP32, BF16 = 0, 1
+
+
+def is_schedule(lr) -> bool:
+    return isinstance(lr, dict)
+
+
+def schedule_value(sched: Dict, i) -> float:
+    """ISchedule.valueAt in double at counter value i (the arithmetic of b2g_lr_schedule in include/b200gan.h; the device rounds it to fp32)."""
+    k, i = sched["schedule"], float(i)
+    if k == "exponential":
+        return sched["initial"] * math.pow(sched["gamma"], i)
+    if k == "inverse":
+        return sched["initial"] / math.pow(1.0 + sched["gamma"] * i, sched["power"])
+    if k == "sigmoid":
+        return sched["initial"] / (1.0 + math.exp(-sched["gamma"] * (i - sched["step"])))
+    if k == "step":
+        return sched["initial"] * math.pow(sched["decay_rate"], math.floor(i / sched["step"]))
+    if k == "map":
+        below = [(int(key), float(v)) for key, v in sched["values"] if int(key) <= i]
+        return max(below)[1] if below else 0.0          # no key <= i: the engine rejects such a map (it must hold key 0)
+    raise ValueError(f"unknown learning-rate schedule {k!r}")
+
+
+def constant_lr(lr) -> float:
+    """The float b2g_layer_desc.lr carries for an updater's lr: the number itself, or a schedule's value at 0 (what the Java facade's
+    updaters write for new Adam(ISchedule): schedule.valueAt(0, 0)).  The engine returns to it when the layer's schedule is cleared."""
+    return float(lr) if not is_schedule(lr) else float(schedule_value(lr, 0))
+
+
+def schedule_struct(sched: Optional[Dict]):
+    """A schedule dict (models.py) -> (b2g_lr_schedule, arrays it points into).  None -> kind NONE."""
+    s = LrSchedule()
+    if sched is None:
+        return s, ()
+    if sched.get("schedule") not in SCHEDULE_KINDS:
+        raise ValueError(f"unknown learning-rate schedule {sched.get('schedule')!r}; one of {sorted(SCHEDULE_KINDS)} (PolySchedule is not supported)")
+    if sched.get("type", "iteration") not in SCHEDULE_TYPES:
+        raise ValueError(f"unknown schedule type {sched.get('type')!r}; one of {sorted(SCHEDULE_TYPES)}")
+    s.kind, s.type = SCHEDULE_KINDS[sched["schedule"]], SCHEDULE_TYPES[sched.get("type", "iteration")]
+    s.initial, s.gamma, s.power = sched.get("initial", 0.0), sched.get("gamma", 0.0), sched.get("power", 0.0)
+    s.step, s.decay_rate = sched.get("step", 0.0), sched.get("decay_rate", 0.0)
+    keep = ()
+    if sched["schedule"] == "map":
+        pairs = [(int(k), float(v)) for k, v in sched["values"]]
+        keys = np.array([k for k, _ in pairs], np.int32); vals = np.array([v for _, v in pairs], np.float64)
+        s.n_map = len(pairs)
+        s.map_keys = keys.ctypes.data_as(C.POINTER(C.c_int32)); s.map_values = vals.ctypes.data_as(C.POINTER(C.c_double))
+        keep = (keys, vals)
+    return s, keep
+
+
+def layer_has_lr(spec: Dict) -> bool:
+    """A layer whose updater has a learning rate: it has parameters, is not frozen and its updater is not NoOp.  A spec without an updater
+    is Sgd with lr 0 (layer_desc), so it has one.  The engine applies the same rule (engine.cu layer_has_lr)."""
+    u = spec.get("updater") or {"kind": "sgd"}
+    return spec["type"] in ("conv2d", "deconv2d", "dense", "output", "batchnorm") and not spec.get("frozen", False) and u["kind"] != "noop"
+
+
+def follow_lr_schedule(specs: List[Dict], constant: List[float], schedule: Optional[Dict], layer: Optional[str] = None):
+    """Writes what b2g_net_set_lr_schedule(layer, schedule) did into the layer specs a checkpoint saves: the schedule, or (schedule None) the
+    layer's creation-time constant lr constant[i] the engine returns to.  layer None: every layer with a learning rate; a name: the first layer
+    of that name, as the engine looks it up."""
+    for i, sp in enumerate(specs):
+        if layer is not None and sp.get("name") != layer:
+            continue
+        if layer_has_lr(sp):
+            if not sp.get("updater"):
+                sp["updater"] = {"kind": "sgd", "lr": 0.0}
+            sp["updater"]["lr"] = copy.deepcopy(schedule) if schedule is not None else constant[i]
+        if layer is not None:
+            break
 
 
 def _fp(a: np.ndarray):
@@ -48,7 +124,7 @@ def layer_desc(spec: Dict) -> LayerDesc:
         d.act_alpha = spec["p"]
     u = spec.get("updater") or {"kind": "sgd", "lr": 0.0}
     d.updater = UPDATERS[u["kind"]]
-    d.lr = u.get("lr", 0.0)
+    d.lr = constant_lr(u.get("lr", 0.0))     # new Adam(ISchedule): the schedule itself is set after b2g_net_create
     if u["kind"] == "rmsprop":          # RmsProp(learningRate, rmsDecay, epsilon)
         d.beta1, d.beta2, d.eps = u.get("rms_decay", 0.95), 0.0, u.get("eps", 1e-8)
     else:
@@ -124,7 +200,9 @@ class Net:
     def __init__(self, ctx: Context, specs: Sequence[Dict], input_shape, max_batch: int, precision: int = FP32,
                  grad_clip: float = 0.0, xent_clip_eps: float = 1e-5, bn_groups: int = 1, seed: int = 666,
                  gradient_normalization: str = "none", gradient_normalization_threshold: float = 1.0):
-        self.ctx, self.lib, self.specs = ctx, ctx.lib, list(specs)
+        self.ctx, self.lib, self.specs = ctx, ctx.lib, copy.deepcopy(list(specs))
+        # each layer's b2g_layer_desc.lr: what the engine uses again when a schedule is cleared
+        self.lr_constants = [constant_lr((sp.get("updater") or {}).get("lr", 0.0)) for sp in self.specs]
         c, h, w = input_shape if len(input_shape) == 3 else (input_shape[0], 1, 1)
         self.input_shape = tuple(input_shape)
         cfg = NetConfig(h, w, c, max_batch, precision, grad_clip, xent_clip_eps, bn_groups, seed)
@@ -138,12 +216,16 @@ class Net:
         self.n_params = n.value
         check(self.lib.b2g_net_output_size(self.h, C.byref(n)))
         self.out_elems = n.value
-        if gradient_normalization != "none":
-            try:
+        try:
+            if gradient_normalization != "none":
                 self.set_gradient_normalization(gradient_normalization, gradient_normalization_threshold)
-            except Exception:
-                self.close()
-                raise
+            for sp in self.specs:         # an updater constructed with an ISchedule: new Adam(new StepSchedule(...))
+                lr = (sp.get("updater") or {}).get("lr", 0.0)
+                if is_schedule(lr) and layer_has_lr(sp):
+                    self.set_lr_schedule(lr, sp["name"])
+        except Exception:
+            self.close()
+            raise
 
     # --- parameters (DL4J flattened-view order) ---
     def num_params(self) -> int:
@@ -186,7 +268,7 @@ class Net:
         from . import serializer
         serializer.save_net(self, path, self.specs, self.input_shape, save_updater,
                             {"precision": "bf16" if self.precision == BF16 else "fp32", "max_batch": self.max_batch, "iteration": self.iteration(),
-                             "dropout_pass": self.dropout_pass()})
+                             "dropout_pass": self.dropout_pass(), "epoch": self.epoch()})
 
     def restore(self, path, load_updater: bool = True):
         """Loads parameters (and updater state) of a checkpoint written by save() into this net (same architecture)."""
@@ -229,6 +311,30 @@ class Net:
         if mode not in GRADIENT_NORMALIZATIONS:
             raise ValueError(f"unknown gradient normalization {mode!r}; one of {sorted(GRADIENT_NORMALIZATIONS)} (element-wise clipping is grad_clip)")
         check(self.lib.b2g_net_set_gradient_normalization(self.h, GRADIENT_NORMALIZATIONS[mode], float(threshold)))
+
+    def set_lr_schedule(self, schedule: Optional[Dict], layer: Optional[str] = None):
+        """ComputationGraph.setLearningRate(ISchedule) (layer None: every layer whose updater has a learning rate) or setLearningRate(layer,
+        ISchedule); schedule None = back to the layer's constant lr from creation (b2g_layer_desc.lr).  Applied from the next update on; the
+        specs a checkpoint writes follow (follow_lr_schedule)."""
+        s, _arrays = schedule_struct(schedule)       # _arrays: the MAP entries s points into, alive for the call
+        check(self.lib.b2g_net_set_lr_schedule(self.h, None if layer is None else layer.encode(), C.byref(s)))
+        follow_lr_schedule(self.specs, self.lr_constants, schedule, layer)
+
+    def learning_rate(self, layer: str) -> float:
+        """ComputationGraph.getLearningRate(layer): the fp32 learning rate the layer's next update uses (before Adam's bias correction),
+        evaluated on the device."""
+        v = C.c_float()
+        check(self.lib.b2g_net_get_learning_rate(self.h, layer.encode(), C.byref(v)))
+        return v.value
+
+    def epoch(self) -> int:
+        """The epoch count EPOCH schedules read (ComputationGraph.getEpochCount); part of a checkpoint."""
+        v = C.c_int64()
+        check(self.lib.b2g_net_get_epoch(self.h, C.byref(v)))
+        return v.value
+
+    def set_epoch(self, epoch: int):
+        check(self.lib.b2g_net_set_epoch(self.h, int(epoch)))
 
     def set_grad_allreduce(self, enabled: bool):
         """False = the reference's parameter-averaging mode: fit() updates locally, average_parameters() synchronises."""

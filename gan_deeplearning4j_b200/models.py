@@ -20,6 +20,37 @@ def sgd(lr):
     return {"kind": "sgd", "lr": lr}
 
 
+# ------------------------------------------------------------------ learning-rate schedules ------------
+# org.nd4j.linalg.schedule.*: pass one as an updater's lr (new Adam(ISchedule): adam(lr=step_schedule(2e-4, 0.5, 1000))) or to
+# Net.set_lr_schedule.  type = ScheduleType: "iteration" (the updater's iteration count) or "epoch" (Net.set_epoch).  The arithmetic is
+# stated at b2g_lr_schedule in include/b200gan.h.
+def exponential_schedule(initial, gamma, type="iteration"):
+    """ExponentialSchedule: initial * gamma^i."""
+    return {"schedule": "exponential", "type": type, "initial": initial, "gamma": gamma}
+
+
+def inverse_schedule(initial, gamma, power, type="iteration"):
+    """InverseSchedule: initial / (1 + gamma*i)^power."""
+    return {"schedule": "inverse", "type": type, "initial": initial, "gamma": gamma, "power": power}
+
+
+def sigmoid_schedule(initial, gamma, step_size, type="iteration"):
+    """SigmoidSchedule: initial / (1 + exp(-gamma*(i - step_size)))."""
+    return {"schedule": "sigmoid", "type": type, "initial": initial, "gamma": gamma, "step": step_size}
+
+
+def step_schedule(initial, decay_rate, step, type="iteration"):
+    """StepSchedule: initial * decay_rate^floor(i / step)."""
+    return {"schedule": "step", "type": type, "initial": initial, "decay_rate": decay_rate, "step": step}
+
+
+def map_schedule(values, type="iteration"):
+    """MapSchedule: the value at the largest key <= i; values = {int: float} or [(key, value), ...] and must hold key 0.  Stored as a list of
+    [key, value] pairs sorted by key (a JSON object would turn the keys into strings)."""
+    pairs = sorted((int(k), float(v)) for k, v in (values.items() if isinstance(values, dict) else values))
+    return {"schedule": "map", "type": type, "values": [[k, v] for k, v in pairs]}
+
+
 # ------------------------------------------------------------------ C1: the reference graphs ---------
 def reference_discriminator(lr=0.002, prefix="dis") -> List[Dict]:
     """J:118-165: BN -> Conv5x5 s2 (1->64) -> MaxPool 2x2 s1 -> Conv5x5 s2 (64->128) -> MaxPool -> Dense 1024 -> Output(1, sigmoid, XENT);

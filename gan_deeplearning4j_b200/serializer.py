@@ -10,8 +10,9 @@ and `updaterState.bin` = `Nd4j.write(updater state view)`.  This module writes t
   updaterState.bin   the updater state, same format.  Layout = this library's [state0 | state1] (RmsProp cache / Adam m, then Adam v), each in
                      parameter order -- NOT DL4J's per-UpdaterBlock interleaving; a DL4J reader must regroup it
   configuration.json this library's layer specification (the arguments of b2g_net_create), NOT DL4J's Jackson schema: a Java user rebuilds the
-                     graph with the same builder calls (the driver's own code, J:118-310) and loads the arrays
-  b200gan.json       precision, input shape, iteration counter, dropout pass counter
+                     graph with the same builder calls (the driver's own code, J:118-310) and loads the arrays.  An updater's learning-rate
+                     schedule is part of its spec (a MapSchedule as a list of [key, value] pairs)
+  b200gan.json       precision, input shape, iteration counter, dropout pass counter, epoch count
 
 `read_model` reads the container back (and accepts legacy int-length headers), so the library can resume training -- the reference can only save.
 """
@@ -102,4 +103,7 @@ def restore_into(net, path, load_updater: bool = True) -> Dict:
     # the DropoutLayer pass counter: a resumed run draws the masks an uninterrupted one would have drawn
     if "dropout_pass" in m["meta"] and hasattr(net, "set_dropout_pass"):
         net.set_dropout_pass(int(m["meta"]["dropout_pass"]))
+    # the epoch count EPOCH learning-rate schedules read
+    if "epoch" in m["meta"] and hasattr(net, "set_epoch"):
+        net.set_epoch(int(m["meta"]["epoch"]))
     return m

@@ -197,6 +197,43 @@ typedef enum {
 /* mode in {0, 1, 2, 4, 5}; the clip modes need a finite threshold > 0.  B2G_ERR_ARG for mode 3 (use grad_clip), an unknown mode, a bad
  * threshold, or an L2 mode on a net created with grad_clip > 0 (DL4J allows one mode per layer). */
 int32_t b2g_net_set_gradient_normalization(b2g_net* net, int32_t mode, float threshold);
+/* Learning-rate schedules (DL4J 1.0.0-beta3 org.nd4j.linalg.schedule.ISchedule; new Adam(ISchedule), ComputationGraph.setLearningRate(ISchedule)).
+ * A layer with a schedule updates with lr_i = (float)value(i) in place of b2g_layer_desc.lr; l2 is unchanged (applied after the updater, not
+ * lr-scaled).  value(i) is computed in double and rounded to fp32 once:
+ *   EXPONENTIAL (1): initial * pow(gamma, i)
+ *   INVERSE     (2): initial / pow(1 + gamma * i, power)
+ *   SIGMOID     (3): initial / (1 + exp(-gamma * (i - step)))                       (step = DL4J's stepSize)
+ *   STEP        (4): initial * pow(decay_rate, floor(i / step))                     (step a double > 0)
+ *   MAP         (5): map_values[j] for the largest map_keys[j] <= i                  (the keys strictly increase and contain 0)
+ * i is the net's iteration counter before this update's increment (b2g_net_get_iteration: 0 on the first update, Adam's t - 1) for
+ * type ITERATION, or the net's epoch word (b2g_net_get_epoch) for type EPOCH.  Both are read from device memory by the updater kernel, so a
+ * replayed CUDA graph uses the current values.  Sgd: u = lr_i * g.  RmsProp: u = lr_i * g / (sqrt(s) + eps).  Adam:
+ * alpha_t = lr_i * sqrt(1 - b2^t) / (1 - b1^t) in fp32 as without a schedule.  A schedule applies wherever the net's updater runs
+ * (b2g_net_fit, the D and G updates of b2g_gan_step, parameter-averaging mode) and adds no kernel launch.  PolySchedule is not supported. */
+typedef enum {
+  B2G_SCHED_NONE = 0, B2G_SCHED_EXPONENTIAL = 1, B2G_SCHED_INVERSE = 2, B2G_SCHED_SIGMOID = 3, B2G_SCHED_STEP = 4, B2G_SCHED_MAP = 5
+} b2g_schedule_kind;
+typedef enum { B2G_SCHED_ITERATION = 0, B2G_SCHED_EPOCH = 1 } b2g_schedule_type;   /* org.nd4j.linalg.schedule.ScheduleType */
+typedef struct {
+  int32_t kind, type;               /* b2g_schedule_kind, b2g_schedule_type */
+  double initial, gamma, power, step, decay_rate;   /* the fields a kind does not use are ignored but must be finite */
+  int32_t n_map;                    /* MAP: entries of map_keys / map_values (copied during the call) */
+  const int32_t* map_keys;
+  const double* map_values;
+} b2g_lr_schedule;
+/* ComputationGraph.setLearningRate(ISchedule) (layer NULL: every non-frozen layer whose updater has a learning rate, others are skipped) and
+ * setLearningRate(String, ISchedule) (layer named).  s NULL or kind NONE: back to the layer's constant lr.  Takes effect at the next update.
+ * B2G_ERR_ARG for an unknown kind or type, a non-finite parameter or map value, step <= 0 (STEP), gamma < 0 (INVERSE), a map that is empty,
+ * whose keys do not strictly increase or that has no key 0, and a named layer that does not exist, is frozen or has no learning rate (no
+ * parameters, or NoOp). */
+int32_t b2g_net_set_lr_schedule(b2g_net* net, const char* layer, const b2g_lr_schedule* s);
+/* ComputationGraph.getLearningRate(String): the fp32 learning rate the layer's next update will use (before Adam's bias correction), computed
+ * on the device by the function the updater kernel calls.  Sync point. */
+int32_t b2g_net_get_learning_rate(b2g_net* net, const char* layer, float* out);
+/* ComputationGraph.getEpochCount / setEpochCount: the 64-bit device word EPOCH schedules read, 0 at b2g_net_create.  The host sets it, nothing
+ * increments it; a new value takes effect at the next update, also in a replayed CUDA graph.  Sync points.  B2G_ERR_ARG for epoch < 0. */
+int32_t b2g_net_get_epoch(b2g_net* net, int64_t* out);
+int32_t b2g_net_set_epoch(b2g_net* net, int64_t epoch);
 /* BF16 nets: how many GEMM-shaped operations ran on the SIMT kernels instead of the tensor-core kernels since creation (skinny layers by design, or a
  * shape the tensor-core kernels do not tile).  north_star: no silent fallback -- bench.py prints it per step. */
 int32_t b2g_net_simt_gemm_calls(b2g_net* net, uint64_t* out);

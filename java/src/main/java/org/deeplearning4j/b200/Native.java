@@ -31,6 +31,10 @@ public final class Native {
     public static native int netGetDropoutPass(long net, long outAddr);
     public static native int netSetDropoutPass(long net, long pass);
     public static native int netSetGradientNormalization(long net, int mode, float threshold);
+    public static native int netSetLrSchedule(long net, long layerNameAddr, long scheduleAddr);   // layerNameAddr 0: every layer; scheduleAddr 0: constant lr
+    public static native int netGetLearningRate(long net, long layerNameAddr, long outAddr);
+    public static native int netGetEpoch(long net, long outAddr);
+    public static native int netSetEpoch(long net, long epoch);
     public static native int netSimtGemmCalls(long net, long outAddr);
     public static native int netSetSyncBn(long net, int enabled);
     public static native int netSetGradPayloadBf16(long net, int enabled);

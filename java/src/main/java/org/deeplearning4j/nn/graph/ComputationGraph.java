@@ -10,6 +10,7 @@ import org.deeplearning4j.nn.conf.NeuralNetConfiguration.ComputationGraphConfigu
 import org.deeplearning4j.nn.conf.layers.Layer;
 import org.nd4j.linalg.api.ndarray.INDArray;
 import org.nd4j.linalg.dataset.DataSet;
+import org.nd4j.linalg.schedule.ISchedule;
 
 public class ComputationGraph {
     private final ComputationGraphConfiguration conf; private long net; private List<Layer> layers; private int maxBatch = Integer.getInteger("b200gan.maxBatch", 1024);
@@ -27,7 +28,43 @@ public class ComputationGraph {
         net = h.getLong(0);
         GradientNormalization gn = conf.b.g.gradNorm;      // RenormalizeL2* / ClipL2*: on-device norms before every update
         if (gn.isL2()) Native.check(Native.netSetGradientNormalization(net, gn.ordinal(), conf.b.g.gradNormThreshold));
+        for (Layer l : layers)            // new Adam(ISchedule) / RmsProp(ISchedule) / Sgd(ISchedule): evaluated on the device at every update
+            if (l.updater != null && l.updater.lrSchedule() != null && hasLearningRate(l)) setLearningRate(l.name, l.updater.lrSchedule());
     }
+    /** The library's rule (include/b200gan.h, b2g_net_set_lr_schedule): parameters, not frozen, updater not NoOp. */
+    private static boolean hasLearningRate(Layer l) {
+        boolean params = l.type == 0 || l.type == 1 || l.type == 2 || l.type == 3 || l.type == 7;    // conv, deconv, BatchNorm, dense, output
+        return params && l.frozen == 0 && l.updater.kind() != 3;
+    }
+
+    /** setLearningRate(ISchedule): every layer whose updater has a learning rate, from the next update on (null: back to the constant lr). */
+    public void setLearningRate(ISchedule s) { applySchedule(null, s); }
+    public void setLearningRate(String layerName, ISchedule s) { applySchedule(layerName, s); }
+    private void applySchedule(String layerName, ISchedule s) {
+        ByteBuffer st = null, keys = null, vals = null;      // b2g_lr_schedule (72 bytes) and a MapSchedule's entries
+        if (s != null) {
+            int[] k = s.mapKeys(); double[] v = s.mapValues(); double[] p = s.parameters();
+            keys = Native.direct(4 * Math.max(1, k.length)); vals = Native.direct(8 * Math.max(1, v.length));
+            for (int i = 0; i < k.length; ++i) { keys.putInt(4 * i, k[i]); vals.putDouble(8 * i, v[i]); }
+            st = Native.direct(72);
+            st.putInt(0, s.kind()).putInt(4, s.getScheduleType().ordinal());
+            for (int i = 0; i < 5; ++i) st.putDouble(8 + 8 * i, p[i]);
+            st.putInt(48, k.length).putLong(56, Native.address(keys)).putLong(64, Native.address(vals));
+        }
+        ByteBuffer name = layerName == null ? null : Native.cstr(layerName);
+        Native.check(Native.netSetLrSchedule(net, name == null ? 0 : Native.address(name), st == null ? 0 : Native.address(st)));
+        java.lang.ref.Reference.reachabilityFence(st); java.lang.ref.Reference.reachabilityFence(keys); java.lang.ref.Reference.reachabilityFence(vals);
+        java.lang.ref.Reference.reachabilityFence(name);   // the native side reads these buffers only through their addresses
+    }
+    /** The learning rate the layer's next update uses (its schedule's value at the current iteration / epoch, or its constant lr). */
+    public double getLearningRate(String layerName) {
+        ByteBuffer o = Native.direct(4); ByteBuffer name = Native.cstr(layerName);
+        Native.check(Native.netGetLearningRate(net, Native.address(name), Native.address(o))); return o.getFloat(0);
+    }
+    /** The epoch count EPOCH schedules read.  Nothing increments it but incrementEpochCount / setEpochCount: call one at each epoch's end. */
+    public int getEpochCount() { ByteBuffer o = Native.direct(8); Native.check(Native.netGetEpoch(net, Native.address(o))); return (int) o.getLong(0); }
+    public void setEpochCount(int epochCount) { Native.check(Native.netSetEpoch(net, epochCount)); }
+    public void incrementEpochCount() { setEpochCount(getEpochCount() + 1); }
     public long handle() { return net; }
     public ComputationGraphConfiguration configuration() { return conf; }
     public long numParams() { ByteBuffer o = Native.direct(8); Native.check(Native.netNumParams(net, Native.address(o))); return o.getLong(0); }

@@ -45,6 +45,15 @@ FN(netSetIteration)(JNIEnv_*, jclass, jlong net, jlong it) { return b2g_net_set_
 FN(netGetDropoutPass)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_get_dropout_pass(P(b2g_net*, net), P(int64_t*, outAddr)); }
 FN(netSetDropoutPass)(JNIEnv_*, jclass, jlong net, jlong pass) { return b2g_net_set_dropout_pass(P(b2g_net*, net), pass); }
 FN(netSetGradientNormalization)(JNIEnv_*, jclass, jlong net, jint mode, jfloat threshold) { return b2g_net_set_gradient_normalization(P(b2g_net*, net), mode, threshold); }
+// scheduleAddr -> b2g_lr_schedule laid out by the facade in a direct ByteBuffer (0 = back to the constant lr); layerNameAddr 0 = every layer
+FN(netSetLrSchedule)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong scheduleAddr) {
+  return b2g_net_set_lr_schedule(P(b2g_net*, net), P(const char*, layerNameAddr), P(const b2g_lr_schedule*, scheduleAddr));
+}
+FN(netGetLearningRate)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong outAddr) {
+  return b2g_net_get_learning_rate(P(b2g_net*, net), P(const char*, layerNameAddr), P(float*, outAddr));
+}
+FN(netGetEpoch)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_get_epoch(P(b2g_net*, net), P(int64_t*, outAddr)); }
+FN(netSetEpoch)(JNIEnv_*, jclass, jlong net, jlong epoch) { return b2g_net_set_epoch(P(b2g_net*, net), epoch); }
 FN(netSimtGemmCalls)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_simt_gemm_calls(P(b2g_net*, net), P(uint64_t*, outAddr)); }
 FN(netSetSyncBn)(JNIEnv_*, jclass, jlong net, jint enabled) { return b2g_net_set_sync_bn(P(b2g_net*, net), enabled); }
 FN(netSetGradPayloadBf16)(JNIEnv_*, jclass, jlong net, jint enabled) { return b2g_net_set_grad_payload_bf16(P(b2g_net*, net), enabled); }
