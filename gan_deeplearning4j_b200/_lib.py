@@ -53,7 +53,23 @@ class TestConvOpts(C.Structure):
     (forced tile width, grid cap, output poisoning, [C][O] dense weight operand)."""
     _fields_ = [("epi", C.c_int32), ("act", C.c_int32), ("alpha", C.c_float), ("bias", C.POINTER(C.c_float)), ("scale", C.POINTER(C.c_float)),
                 ("groups", C.c_int32), ("aux", C.POINTER(C.c_float)), ("aux2", C.POINTER(C.c_float)), ("stats", C.POINTER(C.c_double)), ("kernel", C.c_char * 64),
-                ("bn", C.c_int32), ("max_ctas", C.c_int32), ("poison", C.c_int32), ("w_mn", C.c_int32), ("per_tap", C.c_int32), ("slab", C.c_int32)]
+                ("bn", C.c_int32), ("max_ctas", C.c_int32), ("poison", C.c_int32), ("w_mn", C.c_int32), ("per_tap", C.c_int32), ("slab", C.c_int32),
+                ("defer", C.c_int32), ("db", C.POINTER(C.c_float))]
+
+
+class EwReduceJob(C.Structure):
+    """b2g_ew_reduce_job: one split-K sum of a reduce list (offsets into one buffer); `wide` is set by the call."""
+    _fields_ = [("n", C.c_int64), ("stride", C.c_int64), ("src_off", C.c_int64), ("dst_off", C.c_int64), ("splits", C.c_int32), ("wide", C.c_int32)]
+
+
+class TestEwOpts(C.Structure):
+    """b2g_test_ew_opts: which reduction / loss / element-wise kernel wrapper to run, its sizes and options, and what ran."""
+    _fields_ = [("op", C.c_int32), ("n", C.c_int64), ("rows", C.c_int32), ("cols", C.c_int32), ("groups", C.c_int32), ("splits", C.c_int32),
+                ("stride", C.c_int64)] + [(k, C.c_int32) for k in ("N", "H", "W", "C", "KH", "KW", "SH", "SW", "act")] + [
+                ("alpha", C.c_float), ("clip_eps", C.c_float), ("offset", C.c_int32), ("in_place", C.c_int32), ("accumulate", C.c_int32),
+                ("poison", C.c_int32), ("n_jobs", C.c_int32), ("jobs", C.POINTER(EwReduceJob)), ("n_seg", C.c_int32),
+                ("seg_off", C.POINTER(C.c_int64)), ("seg_len", C.POINTER(C.c_int64)), ("seg_coef", C.POINTER(C.c_float)), ("sumsq", C.c_double),
+                ("kernel", C.c_char * 64)]
 
 
 _vp, _i32, _i64, _fp = C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_float)
@@ -121,6 +137,7 @@ PROTOTYPES = {
                            _i32, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     "b2g_test_net_shadow": (_i32, [_vp, _i32, _i32, _fp, _i64]),
     "b2g_test_dropout": (_i32, [_vp, _i32, C.c_uint64, _i32, _i32, _i64, _i32, _i32, _i32, _i32, C.c_float, _fp, _fp, _fp, _fp]),
+    "b2g_test_ew": (_i32, [_vp, _i32, C.POINTER(TestEwOpts), _fp, _fp, _fp, _fp, _fp]),
 }
 
 _lib = None

@@ -1401,6 +1401,9 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   if (max_ctas < 0 || (max_ctas && !tc_conv && !ps)) return fail(B2G_ERR_UNSUPPORTED, "max_ctas %d: a grid cap applies to tc_conv_kernel launches only", max_ctas);
   if (poison && kind == 2) return fail(B2G_ERR_UNSUPPORTED, "poison applies to the bf16 outputs of kinds 0 / 1");
   if (w_mn && (impl != 1 || kind != 0 || g.KH != 1 || g.KW != 1)) return fail(B2G_ERR_UNSUPPORTED, "w_mn: the [C][O] weight operand exists for the 1x1 tensor-core fprop only");
+  const bool defer = opt && opt->defer; float* db_host = opt ? opt->db : nullptr;
+  if (defer && !(kind == 2 && (impl == 1 || impl == 3))) return fail(B2G_ERR_UNSUPPORTED, "defer applies to the tensor-core weight gradients (kind 2, impl 1 / 3)");
+  if (db_host && !(kind == 2 && impl == 3)) return fail(B2G_ERR_UNSUPPORTED, "db is the edge tensor-core weight gradient's bias column (kind 2, impl 3)");
   // impl 2 = the SIMT skinny-layer kernels (kernels_edge.cu), impl 3 = their tensor-core counterparts; both need <= 4 image channels (g.C)
   if (impl == 2 || impl == 3) {
     bool ok = kind == 0 ? edge_conv_small_cin_supported(g) : kind == 1 ? edge_deconv_small_c_supported(g) : edge_wgrad_small_cin_supported(g);
@@ -1420,6 +1423,9 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   if (prec == PREC_BF16) { k_cast_f32_to_bf16(fa, (__nv_bfloat16*)ta, na, s); k_cast_f32_to_bf16(fb, (__nv_bfloat16*)tb, nb, s); }
   else { CU(cudaMemcpyAsync(ta, fa, 4 * na, cudaMemcpyDeviceToDevice, s)); CU(cudaMemcpyAsync(tb, fb, 4 * nb, cudaMemcpyDeviceToDevice, s)); }
   if (impl == 3 && kind == 1) { CU(cudaMalloc(&wps, 2 * k_tc_deconv_ps_weight_elems(g))); k_pack_deconv_ps(fb, wps, g.O, g.C, s); }
+  float* d_db = nullptr; int db_written = 0;
+  if (db_host) CU(cudaMalloc(&d_db, 4 * (size_t)g.O));
+  ReduceList rl{}; ReduceList* prl = defer ? &rl : nullptr;
   TcEpi epi{}; const TcEpi* pe = nullptr; const float* bias = nullptr; int act = 0; float alpha = 0.f; int groups = 1;
   if (opt && (tc_conv || ps)) {
     groups = opt->groups > 0 ? opt->groups : 1; act = opt->act; alpha = opt->alpha;
@@ -1454,17 +1460,29 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
     else if (impl >= 2) {
       if (kind == 0) { if (impl == 3) rc = k_tc_edge_conv(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, nullptr, (__nv_bfloat16*)to, 0, 0.f, s); else k_edge_conv_small_cin(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s); }
       else if (kind == 1) { if (impl == 3) rc = k_tc_deconv_ps(g, (const __nv_bfloat16*)ta, wps, bias, (__nv_bfloat16*)to, act, alpha, s, pe); else k_edge_deconv_small_c(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s); }
-      else { if (impl == 3) rc = k_tc_edge_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fo, nullptr, scratch, sc, 0, s); else k_edge_wgrad_small_cin(prec, g, ta, tb, fo, scratch, 0, s); }
+      else {
+        if (impl == 3) { rc = k_tc_edge_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fo, d_db, scratch, sc, 0, s, prl); if (rc >= 0) { db_written = rc; rc = 0; } }
+        else k_edge_wgrad_small_cin(prec, g, ta, tb, fo, scratch, 0, s);
+      }
     }
     else if (kind == 0) { if (impl) rc = k_tc_fprop(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s, pe, w_mn ? 1 : 0); else k_simt_fprop(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s); }
     else if (kind == 1) { if (impl) rc = k_tc_dgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s, pe); else k_simt_dgrad(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s); }
-    else { if (impl) rc = k_tc_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fo, scratch, sc, 0, s); else k_simt_wgrad(prec, g, ta, tb, fo, scratch, sc, 0, s); }
+    else { if (impl) rc = k_tc_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fo, scratch, sc, 0, s, prl); else k_simt_wgrad(prec, g, ta, tb, fo, scratch, sc, 0, s); }
     if (rc) break;
+    if (defer) {      // the backward pass's one reduce-list launch over the partials the wgrad kernel left in scratch
+      if (!rl.count) { rc = -4; break; }
+      k_reduce_multi(rl, s); rl.count = 0;
+    }
   }
   schedule.reset();
   CU(cudaEventRecord(e1, s));
+  if (rc == -4) return fail(B2G_ERR_CUDA, "defer: the weight gradient queued no reduction");
   if (rc) return fail(B2G_ERR_CUDA, "tensor-core kernel launch failed (%d)", rc);
   if (opt) { strncpy(opt->kernel, g_tc_last_kernel, sizeof(opt->kernel) - 1); opt->kernel[sizeof(opt->kernel) - 1] = 0; opt->slab = g_tc_last_slab; }
+  if (d_db) {
+    if (!db_written) { cudaFree(d_db); return fail(B2G_ERR_UNSUPPORTED, "the edge weight gradient produces no bias column for C = %d", g.C); }
+    CU(cudaMemcpyAsync(db_host, d_db, 4 * (size_t)g.O, cudaMemcpyDeviceToHost, s));
+  }
   if (kind != 2) { if (prec == PREC_BF16) { /* widen */ k_nhwc_to_nchw_f32(prec, to, fo, 1, 1, (int)no, s); } else CU(cudaMemcpyAsync(fo, to, 4 * no, cudaMemcpyDeviceToDevice, s)); }
   CU(cudaMemcpyAsync(out, fo, 4 * no, cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s)); CHECK_KERNELS();
@@ -1475,7 +1493,7 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   }
   float ms = 0.f; CU(cudaEventElapsedTime(&ms, e0, e1)); if (ms_per_iter) *ms_per_iter = ms / reps;
   cudaEventDestroy(e0); cudaEventDestroy(e1);
-  cudaFree(fa); cudaFree(fb); cudaFree(fo); cudaFree(scratch); cudaFree(ta); cudaFree(tb); cudaFree(to); if (wps) cudaFree(wps);
+  cudaFree(fa); cudaFree(fb); cudaFree(fo); cudaFree(scratch); cudaFree(ta); cudaFree(tb); cudaFree(to); if (wps) cudaFree(wps); if (d_db) cudaFree(d_db);
   if (d_bias) cudaFree(d_bias); if (d_scale) cudaFree(d_scale); if (d_coef) cudaFree(d_coef); if (d_auxf) cudaFree(d_auxf); if (d_aux) cudaFree(d_aux); if (d_aux2) cudaFree(d_aux2); if (d_acc) cudaFree(d_acc);
   return 0;
 }
@@ -1585,6 +1603,163 @@ extern "C" int32_t b2g_test_dropout(b2g_ctx* c, int32_t precision, uint64_t seed
   release();
   if (e != cudaSuccess) return fail(B2G_ERR_CUDA, "dropout test: %s", cudaGetErrorString(e));
   if (p1 != p0 + 1) return fail(B2G_ERR_CUDA, "dropout test: the forward left the pass counter at %llu, expected %llu", p1, p0 + 1);
+  return 0;
+}
+
+// One reduction / loss / element-wise kernel through its production wrapper on host tensors (include/b200gan.h, b2g_test_ew).  The kernel
+// names come from the wrappers (g_ew_last_kernel): this hook never decides which path a shape takes.
+namespace {
+struct EwMem {        // every allocation of one b2g_test_ew call, released on every return
+  std::vector<void*> v;
+  ~EwMem() { for (void* p : v) cudaFree(p); }
+};
+}  // namespace
+extern "C" int32_t b2g_test_ew(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, const float* in0, const float* in1, float* out0, float* out1, float* out2) {
+  if (!c || !o) return fail(B2G_ERR_ARG, "null");
+  const int prec = precision == B2G_PREC_BF16 ? PREC_BF16 : PREC_F32; const size_t ts = prec_size(prec);
+  const int off = o->offset;
+  if (off < 0 || off > 64) return fail(B2G_ERR_ARG, "offset %d outside [0, 64]", off);
+  if (o->poison && o->accumulate) return fail(B2G_ERR_ARG, "poison would overwrite the initial destination accumulate adds to");
+  CU(cudaSetDevice(c->device)); cudaStream_t s = c->stream;
+  EwMem mem;
+  // es-byte elements, `off` elements past a 256-byte aligned allocation
+  auto dev = [&](size_t count, size_t es, void** p) -> int32_t { void* b = nullptr; CU(cudaMalloc(&b, es * (count + off) + 16)); mem.v.push_back(b); *p = (char*)b + es * off; return 0; };
+  auto upF = [&](const float* h, size_t count, float** p) -> int32_t {
+    B2(dev(count, 4, (void**)p)); if (h) CU(cudaMemcpyAsync(*p, h, 4 * count, cudaMemcpyHostToDevice, s)); return 0; };
+  auto upT = [&](const float* h, size_t count, void** p) -> int32_t {        // fp32 host -> T (bf16: rounded on the device)
+    B2(dev(count, ts, p)); if (!h) return 0;
+    if (prec == PREC_F32) { CU(cudaMemcpyAsync(*p, h, 4 * count, cudaMemcpyHostToDevice, s)); return 0; }
+    float* f = nullptr; CU(cudaMalloc(&f, 4 * count)); mem.v.push_back(f);
+    CU(cudaMemcpyAsync(f, h, 4 * count, cudaMemcpyHostToDevice, s)); k_cast_f32_to_bf16(f, (__nv_bfloat16*)*p, count, s); return 0; };
+  auto downF = [&](float* h, const float* d, size_t count) -> int32_t { if (h) CU(cudaMemcpyAsync(h, d, 4 * count, cudaMemcpyDeviceToHost, s)); return 0; };
+  auto downT = [&](float* h, const void* d, size_t count) -> int32_t {      // T -> fp32 host
+    if (!h) return 0;
+    float* f = nullptr; CU(cudaMalloc(&f, 4 * count)); mem.v.push_back(f);
+    k_nhwc_to_nchw_f32(prec, d, f, 1, 1, (int)count, s); CU(cudaMemcpyAsync(h, f, 4 * count, cudaMemcpyDeviceToHost, s)); return 0; };
+  auto poison = [&](void* d, size_t bytes) -> int32_t { if (o->poison) CU(cudaMemsetAsync(d, 0xFF, bytes, s)); return 0; };     // fp32 and bf16 NaN
+  std::string names;
+  auto ran = [&]() { if (!names.empty()) names += ","; names += g_ew_last_kernel; g_ew_last_kernel = ""; };
+  const int64_t lim = 0x7fffffff;
+  g_ew_last_kernel = "";
+  switch (o->op) {
+    case B2G_EW_REDUCE_SPLITS: {
+      if (!in0 || o->n < 1 || o->n > lim || o->splits < 1 || o->stride < o->n || (o->accumulate && !in1)) return fail(B2G_ERR_ARG, "bad REDUCE_SPLITS arguments");
+      float *src = nullptr, *dst = nullptr; B2(upF(in0, (size_t)o->splits * o->stride, &src)); B2(upF(in1, (size_t)o->n, &dst)); B2(poison(dst, 4 * o->n));
+      k_reduce_splits(src, dst, (size_t)o->n, o->splits, (size_t)o->stride, o->accumulate ? 1 : 0, s); ran();
+      B2(downF(out0, dst, (size_t)o->n));
+      break;
+    }
+    case B2G_EW_REDUCE_MULTI: {
+      if (!in0 || o->n < 1 || o->n > lim || o->n_jobs < 1 || o->n_jobs > ReduceList::MAX_JOBS || !o->jobs) return fail(B2G_ERR_ARG, "bad REDUCE_MULTI arguments");
+      const b2g_ew_reduce_job* J = o->jobs;
+      auto src_end = [&](int i) { return J[i].src_off + (int64_t)(J[i].splits - 1) * J[i].stride + J[i].n; };
+      for (int i = 0; i < o->n_jobs; ++i) {
+        if (J[i].n < 1 || J[i].splits < 1 || J[i].stride < J[i].n || J[i].src_off < 0 || J[i].dst_off < 0 || src_end(i) > o->n || J[i].dst_off + J[i].n > o->n)
+          return fail(B2G_ERR_ARG, "reduce job %d outside the buffer", i);
+        for (int k = 0; k < o->n_jobs; ++k) {      // a destination shared with any source or another destination would race
+          const bool src_hit = J[i].dst_off < src_end(k) && J[k].src_off < J[i].dst_off + J[i].n;
+          const bool dst_hit = k != i && J[i].dst_off < J[k].dst_off + J[k].n && J[k].dst_off < J[i].dst_off + J[i].n;
+          if (src_hit || dst_hit) return fail(B2G_ERR_ARG, "reduce job %d's destination overlaps job %d", i, k);
+        }
+      }
+      float* buf = nullptr; B2(upF(in0, (size_t)o->n, &buf));
+      ReduceList rl{};
+      for (int i = 0; i < o->n_jobs; ++i) {
+        reduce_list_push(&rl, buf + J[i].src_off, buf + J[i].dst_off, J[i].n, J[i].splits, J[i].stride);
+        o->jobs[i].wide = rl.jobs[i].blocks < 0 ? 1 : 0;
+        B2(poison(buf + J[i].dst_off, 4 * (size_t)J[i].n));
+      }
+      if (rl.count != o->n_jobs) return fail(B2G_ERR_ARG, "the reduce list took %d of %d jobs", rl.count, o->n_jobs);
+      k_reduce_multi(rl, s); ran();
+      B2(downF(out0, buf, (size_t)o->n));
+      break;
+    }
+    case B2G_EW_COLSUM: {
+      if (!in0 || o->rows < 1 || o->cols < 1 || (int64_t)o->rows * o->cols > lim || (o->accumulate && !in1)) return fail(B2G_ERR_ARG, "bad COLSUM arguments");
+      void* x = nullptr; float *out = nullptr, *scratch = nullptr; B2(upT(in0, (size_t)o->rows * o->cols, &x)); B2(upF(in1, (size_t)o->cols, &out)); B2(poison(out, 4 * (size_t)o->cols));
+      CU(cudaMalloc(&scratch, 4 * k_colsum_scratch_floats(o->cols))); mem.v.push_back(scratch);
+      k_colsum(prec, x, o->rows, o->cols, scratch, out, o->accumulate ? 1 : 0, s); ran();
+      B2(downF(out0, out, (size_t)o->cols));
+      break;
+    }
+    case B2G_EW_XENT: {
+      const size_t n = (size_t)o->rows * o->groups;
+      if (!in0 || !in1 || o->rows < 1 || o->groups < 1 || (int64_t)n > lim) return fail(B2G_ERR_ARG, "bad XENT arguments");
+      void *z = nullptr, *dz = nullptr; float *y = nullptr, *loss = nullptr; B2(upT(in0, n, &z)); B2(upF(in1, n, &y)); B2(dev(n, ts, &dz)); B2(upF(nullptr, (size_t)o->groups, &loss));
+      B2(poison(dz, ts * n)); B2(poison(loss, 4 * (size_t)o->groups));
+      k_xent(prec, z, y, dz, loss, o->rows, o->groups, o->clip_eps, s); ran();
+      B2(downT(out0, dz, n)); B2(downF(out1, loss, (size_t)o->groups));
+      break;
+    }
+    case B2G_EW_SOFTMAX_XENT: {
+      const size_t n = (size_t)o->rows * o->cols;
+      if (!in0 || o->rows < 1 || o->cols < 1 || (int64_t)n > lim) return fail(B2G_ERR_ARG, "bad SOFTMAX_XENT arguments");
+      void *z = nullptr, *dz = nullptr, *p = nullptr; float *y = nullptr, *loss = nullptr; B2(upT(in0, n, &z)); if (in1) B2(upF(in1, n, &y));
+      B2(dev(n, ts, &dz)); B2(dev(n, ts, &p)); B2(upF(nullptr, 1, &loss));
+      B2(poison(dz, ts * n)); B2(poison(p, ts * n)); B2(poison(loss, 4));
+      k_softmax_xent(prec, z, y, y ? dz : nullptr, p, y ? loss : nullptr, o->rows, o->cols, s); ran();       // no labels: the inference call
+      B2(downT(out0, dz, n)); B2(downF(out1, loss, 1)); B2(downT(out2, p, n));
+      break;
+    }
+    case B2G_EW_ACT_FWD: case B2G_EW_ACT_BWD: {
+      const size_t n = (size_t)o->n; const bool bwd = o->op == B2G_EW_ACT_BWD;
+      if (!in0 || (bwd && !in1) || o->n < 1 || o->n > lim || o->act < B2G_ACT_IDENTITY || o->act > B2G_ACT_LRELU) return fail(B2G_ERR_ARG, "bad activation arguments");
+      void *a = nullptr, *e = nullptr, *r = nullptr; B2(upT(in0, n, &a));
+      if (bwd) B2(upT(in1, n, &e));
+      if (bwd && o->in_place) r = e;
+      else { B2(dev(n, ts, &r)); B2(poison(r, ts * n)); }
+      if (bwd) k_act_bwd_from_output(prec, a, e, r, n, o->act, o->alpha, s);      // in place: eps_in == eps_out, as the backward pass calls it
+      else k_act_fwd(prec, a, r, n, o->act, o->alpha, s);
+      ran();
+      B2(downT(out0, r, n));
+      break;
+    }
+    case B2G_EW_MAXPOOL: {
+      if (!in0 || !in1 || o->N < 1 || o->C < 1 || o->KH < 1 || o->KW < 1 || o->SH < 1 || o->SW < 1 || o->H < o->KH || o->W < o->KW || o->KH * o->KW > 255)
+        return fail(B2G_ERR_ARG, "bad MAXPOOL arguments");
+      const int OH = (o->H - o->KH) / o->SH + 1, OW = (o->W - o->KW) / o->SW + 1;
+      const size_t ni = (size_t)o->N * o->H * o->W * o->C, no = (size_t)o->N * OH * OW * o->C;
+      if (ni > (size_t)lim) return fail(B2G_ERR_ARG, "MAXPOOL input too large");
+      void *x = nullptr, *eo = nullptr, *y = nullptr, *ei = nullptr; uint8_t* arg = nullptr;
+      B2(upT(in0, ni, &x)); B2(upT(in1, no, &eo)); B2(dev(no, ts, &y)); B2(dev(ni, ts, &ei)); B2(dev(no, 1, (void**)&arg));
+      B2(poison(y, ts * no)); B2(poison(ei, ts * ni)); B2(poison(arg, no));        // 0xFF: no window of <= 255 elements has that argmax
+      k_maxpool_fwd(prec, x, y, arg, o->N, o->H, o->W, o->C, OH, OW, o->KH, o->KW, o->SH, o->SW, s); ran();
+      k_maxpool_bwd(prec, eo, arg, ei, o->N, o->H, o->W, o->C, OH, OW, o->KH, o->KW, o->SH, o->SW, s); ran();
+      B2(downT(out0, y, no)); B2(downT(out1, ei, ni));
+      if (out2) {
+        std::vector<uint8_t> h(no); CU(cudaMemcpyAsync(h.data(), arg, no, cudaMemcpyDeviceToHost, s)); CU(cudaStreamSynchronize(s));
+        for (size_t i = 0; i < no; ++i) out2[i] = (float)h[i];
+      }
+      break;
+    }
+    case B2G_EW_UPSAMPLE: {
+      const int f = o->KH;
+      if (!in0 || !in1 || o->N < 1 || o->H < 1 || o->W < 1 || o->C < 1 || f < 1) return fail(B2G_ERR_ARG, "bad UPSAMPLE arguments");
+      const size_t ni = (size_t)o->N * o->H * o->W * o->C, no = ni * f * f;
+      if (no > (size_t)lim) return fail(B2G_ERR_ARG, "UPSAMPLE output too large");
+      void *x = nullptr, *eo = nullptr, *y = nullptr, *ei = nullptr;
+      B2(upT(in0, ni, &x)); B2(upT(in1, no, &eo)); B2(dev(no, ts, &y)); B2(dev(ni, ts, &ei)); B2(poison(y, ts * no)); B2(poison(ei, ts * ni));
+      k_upsample_fwd(prec, x, y, o->N, o->H, o->W, o->C, f, s); ran();
+      k_upsample_bwd(prec, eo, ei, o->N, o->H, o->W, o->C, f, s); ran();
+      B2(downT(out0, y, no)); B2(downT(out1, ei, ni));
+      break;
+    }
+    case B2G_EW_SUMSQ: {
+      if (!in0 || o->n < 1 || o->n_seg < 1 || !o->seg_off || !o->seg_len || !o->seg_coef) return fail(B2G_ERR_ARG, "bad SUMSQ arguments");
+      for (int i = 0; i < o->n_seg; ++i)
+        if (o->seg_off[i] < 0 || o->seg_len[i] < 0 || o->seg_off[i] + o->seg_len[i] > o->n) return fail(B2G_ERR_ARG, "segment %d outside the tensor", i);
+      float *p = nullptr, *coef = nullptr; int64_t *so = nullptr, *sl = nullptr; double* res = nullptr;
+      B2(upF(in0, (size_t)o->n, &p)); B2(upF(o->seg_coef, (size_t)o->n_seg, &coef)); B2(dev((size_t)o->n_seg, 8, (void**)&so)); B2(dev((size_t)o->n_seg, 8, (void**)&sl)); B2(dev(1, 8, (void**)&res));
+      CU(cudaMemcpyAsync(so, o->seg_off, 8 * (size_t)o->n_seg, cudaMemcpyHostToDevice, s)); CU(cudaMemcpyAsync(sl, o->seg_len, 8 * (size_t)o->n_seg, cudaMemcpyHostToDevice, s));
+      B2(poison(res, 8));
+      k_sumsq_segments(p, so, sl, coef, o->n_seg, res, s); ran();
+      CU(cudaMemcpyAsync(&o->sumsq, res, 8, cudaMemcpyDeviceToHost, s));
+      break;
+    }
+    default: return fail(B2G_ERR_ARG, "unknown op %d", o->op);
+  }
+  CU(cudaStreamSynchronize(s)); CHECK_KERNELS();
+  strncpy(o->kernel, names.c_str(), sizeof(o->kernel) - 1); o->kernel[sizeof(o->kernel) - 1] = 0;
   return 0;
 }
 

@@ -23,6 +23,9 @@ struct ConvGeom {
 };
 
 extern uint64_t g_launch_count;   // every kernel launch of this library bumps it (bench evidence)
+// which kernel the most recent call of a reduction / loss / activation / pooling wrapper below dispatched (kernel-level tests assert it;
+// k_colsum names its first stage)
+extern const char* g_ew_last_kernel;
 // multiprocessor count of the current device (queried once per device): the one source every grid-sizing rule of the library uses
 int device_sm_count();
 

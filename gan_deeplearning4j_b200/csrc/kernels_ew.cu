@@ -16,6 +16,7 @@
 namespace b2g {
 
 uint64_t g_launch_count = 0;
+const char* g_ew_last_kernel = "";
 
 // ---------------------------------------------------------------- layout -----------------------------
 template <typename T>
@@ -567,6 +568,7 @@ __global__ void act_bwd_out_kernel(const T* __restrict__ a, const T* __restrict_
 }
 void k_act_fwd(int prec, const void* x, void* y, size_t n, int act, float alpha, cudaStream_t s) {
   if (!n) return; DISPATCH_PREC(prec, T, (launch_pdl(act_fwd_kernel<T>, dim3(ew_blocks(n)), dim3(256), (size_t)(0), s, (const T*)x, (T*)y, n, act, alpha))); LAUNCHED();
+  g_ew_last_kernel = "act_fwd_kernel";
 }
 // bf16, 16-byte vectors (n % 8 == 0): the D1 / G-last activation derivative runs over the largest tensors of the step
 template <int ACTC>
@@ -588,9 +590,11 @@ __global__ void __launch_bounds__(256, 4) act_bwd_out_bf16x8_kernel(const uint4*
 void k_act_bwd_from_output(int prec, const void* a, const void* eo, void* ei, size_t n, int act, float alpha, cudaStream_t s) {
   if (!n) return;
   if (prec == PREC_BF16 && n % 8 == 0 && ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(eo) | reinterpret_cast<uintptr_t>(ei)) & 15) == 0) {
-    DISPATCH_ACT(act, ACTC, launch_pdl(act_bwd_out_bf16x8_kernel<ACTC>, dim3(vec4_blocks(n / 8)), dim3(256), (size_t)0, s, (const uint4*)a, (const uint4*)eo, (uint4*)ei, n / 8, act, alpha)); LAUNCHED(); return;
+    DISPATCH_ACT(act, ACTC, launch_pdl(act_bwd_out_bf16x8_kernel<ACTC>, dim3(vec4_blocks(n / 8)), dim3(256), (size_t)0, s, (const uint4*)a, (const uint4*)eo, (uint4*)ei, n / 8, act, alpha)); LAUNCHED();
+    g_ew_last_kernel = "act_bwd_out_bf16x8_kernel"; return;
   }
   DISPATCH_PREC(prec, T, (launch_pdl(act_bwd_out_kernel<T>, dim3(ew_blocks(n)), dim3(256), (size_t)(0), s, (const T*)a, (const T*)eo, (T*)ei, n, act, alpha))); LAUNCHED();
+  g_ew_last_kernel = "act_bwd_out_kernel";
 }
 void k_sigmoid_out(int prec, const void* z, void* p, size_t n, cudaStream_t s) { k_act_fwd(prec, z, p, n, ACT_SIGMOID, 0.f, s); }
 
@@ -626,10 +630,12 @@ __global__ void maxpool_bwd_kernel(const T* __restrict__ eo, const uint8_t* __re
 void k_maxpool_fwd(int prec, const void* x, void* y, uint8_t* arg, int N, int H, int W, int C, int OH, int OW, int KH, int KW, int SH, int SW, cudaStream_t s) {
   size_t n = (size_t)N * OH * OW * C; if (!n) return;
   DISPATCH_PREC(prec, T, (launch_pdl(maxpool_fwd_kernel<T>, dim3(ew_blocks(n)), dim3(256), (size_t)(0), s, (const T*)x, (T*)y, arg, N, H, W, C, OH, OW, KH, KW, SH, SW))); LAUNCHED();
+  g_ew_last_kernel = "maxpool_fwd_kernel";
 }
 void k_maxpool_bwd(int prec, const void* eo, const uint8_t* arg, void* ei, int N, int H, int W, int C, int OH, int OW, int KH, int KW, int SH, int SW, cudaStream_t s) {
   size_t n = (size_t)N * H * W * C; if (!n) return;
   DISPATCH_PREC(prec, T, (launch_pdl(maxpool_bwd_kernel<T>, dim3(ew_blocks(n)), dim3(256), (size_t)(0), s, (const T*)eo, arg, (T*)ei, N, H, W, C, OH, OW, KH, KW, SH, SW))); LAUNCHED();
+  g_ew_last_kernel = "maxpool_bwd_kernel";
 }
 template <typename T>
 __global__ void upsample_fwd_kernel(const T* __restrict__ x, T* __restrict__ y, int N, int H, int W, int C, int f) { pdl_enter();
@@ -652,10 +658,12 @@ __global__ void upsample_bwd_kernel(const T* __restrict__ eo, T* __restrict__ ei
 void k_upsample_fwd(int prec, const void* x, void* y, int N, int H, int W, int C, int f, cudaStream_t s) {
   size_t n = (size_t)N * H * f * W * f * C; if (!n) return;
   DISPATCH_PREC(prec, T, (launch_pdl(upsample_fwd_kernel<T>, dim3(ew_blocks(n)), dim3(256), (size_t)(0), s, (const T*)x, (T*)y, N, H, W, C, f))); LAUNCHED();
+  g_ew_last_kernel = "upsample_fwd_kernel";
 }
 void k_upsample_bwd(int prec, const void* eo, void* ei, int N, int H, int W, int C, int f, cudaStream_t s) {
   size_t n = (size_t)N * H * W * C; if (!n) return;
   DISPATCH_PREC(prec, T, (launch_pdl(upsample_bwd_kernel<T>, dim3(ew_blocks(n)), dim3(256), (size_t)(0), s, (const T*)eo, (T*)ei, N, H, W, C, f))); LAUNCHED();
+  g_ew_last_kernel = "upsample_bwd_kernel";
 }
 
 // ---------------------------------------------------------------- XENT ---------------------------------
@@ -686,6 +694,7 @@ __global__ void xent_kernel(const T* __restrict__ z, const float* __restrict__ y
 }
 void k_xent(int prec, const void* z, const float* y, void* dz, float* loss_sums, int rows, int groups, float clip, cudaStream_t s) {
   DISPATCH_PREC(prec, T, (launch_pdl(xent_kernel<T>, dim3(groups), dim3(1024), (size_t)(0), s, (const T*)z, y, (T*)dz, loss_sums, rows, clip))); LAUNCHED();
+  g_ew_last_kernel = "xent_kernel";
 }
 
 // LossMCXENT with softmax (J:357-362), K classes per row: one thread per row, block-level loss sum
@@ -709,6 +718,7 @@ __global__ void softmax_xent_kernel(const T* __restrict__ z, const float* __rest
 }
 void k_softmax_xent(int prec, const void* z, const float* y, void* dz, void* p_out, float* loss_sums, int rows, int K, cudaStream_t s) {
   DISPATCH_PREC(prec, T, (launch_pdl(softmax_xent_kernel<T>, dim3(1), dim3(1024), (size_t)0, s, (const T*)z, y, (T*)dz, (T*)p_out, loss_sums, rows, K))); LAUNCHED();
+  g_ew_last_kernel = "softmax_xent_kernel";
 }
 
 // ---------------------------------------------------------------- column sum / misc reductions -----------
@@ -772,19 +782,20 @@ void k_colsum(int prec, const void* x, int rows, int C, float* scratch, float* o
   if (prec == PREC_BF16 && C >= 1 && C <= 4 && rows % 8 == 0 && rows >= 4096 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
     const size_t groups8 = (size_t)rows / 8; int S = (int)std::min<size_t>(256, (groups8 + 255) / 256);
     switch (C) {
-      case 1: launch_pdl(colsum_small_c_kernel<1>, dim3(S), dim3(256), (size_t)0, s, (const uint4*)x, groups8, scratch); break;
-      case 2: launch_pdl(colsum_small_c_kernel<2>, dim3(S), dim3(256), (size_t)0, s, (const uint4*)x, groups8, scratch); break;
-      case 3: launch_pdl(colsum_small_c_kernel<3>, dim3(S), dim3(256), (size_t)0, s, (const uint4*)x, groups8, scratch); break;
-      default: launch_pdl(colsum_small_c_kernel<4>, dim3(S), dim3(256), (size_t)0, s, (const uint4*)x, groups8, scratch); break;
+      case 1: launch_pdl(colsum_small_c_kernel<1>, dim3(S), dim3(256), (size_t)0, s, (const uint4*)x, groups8, scratch); g_ew_last_kernel = "colsum_small_c_kernel<1>"; break;
+      case 2: launch_pdl(colsum_small_c_kernel<2>, dim3(S), dim3(256), (size_t)0, s, (const uint4*)x, groups8, scratch); g_ew_last_kernel = "colsum_small_c_kernel<2>"; break;
+      case 3: launch_pdl(colsum_small_c_kernel<3>, dim3(S), dim3(256), (size_t)0, s, (const uint4*)x, groups8, scratch); g_ew_last_kernel = "colsum_small_c_kernel<3>"; break;
+      default: launch_pdl(colsum_small_c_kernel<4>, dim3(S), dim3(256), (size_t)0, s, (const uint4*)x, groups8, scratch); g_ew_last_kernel = "colsum_small_c_kernel<4>"; break;
     }
     LAUNCHED();
     launch_pdl(colsum_final_kernel, dim3(1), dim3(512), (size_t)(0), s, scratch, C, S, out, accumulate); LAUNCHED();
     return;
   }
-  const bool vec = vec_ok(prec, C);
+  // the 16-byte loads of the bf16x8 kernel need a 16-byte aligned x; any other x takes the element-wise kernel
+  const bool vec = vec_ok(prec, C) && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
   int S = vec ? vec_blocks(rows, C) : pick_slices(rows, C);
-  if (vec) launch_pdl(colsum_partial_bf16x8_kernel, dim3(S), dim3(256), (size_t)(0), s, (const uint4*)x, rows, C, S, scratch);
-  else DISPATCH_PREC(prec, T, (launch_pdl(colsum_partial_kernel<T>, dim3((S * C + 255) / 256), dim3(256), (size_t)(0), s, (const T*)x, rows, C, S, scratch)));
+  if (vec) { launch_pdl(colsum_partial_bf16x8_kernel, dim3(S), dim3(256), (size_t)(0), s, (const uint4*)x, rows, C, S, scratch); g_ew_last_kernel = "colsum_partial_bf16x8_kernel"; }
+  else { DISPATCH_PREC(prec, T, (launch_pdl(colsum_partial_kernel<T>, dim3((S * C + 255) / 256), dim3(256), (size_t)(0), s, (const T*)x, rows, C, S, scratch))); g_ew_last_kernel = "colsum_partial_kernel"; }
   LAUNCHED();
   launch_pdl(colsum_final_kernel, dim3((C + 31) / 32), dim3(512), (size_t)(0), s, scratch, C, S, out, accumulate); LAUNCHED();
 }
@@ -803,6 +814,7 @@ __global__ void sumsq_segments_kernel(const float* __restrict__ p, const int64_t
 }
 void k_sumsq_segments(const float* p, const int64_t* so, const int64_t* sl, const float* sc, int nseg, double* out, cudaStream_t s) {
   launch_pdl(sumsq_segments_kernel, dim3(1), dim3(1024), (size_t)(0), s, p, so, sl, sc, nseg, out); LAUNCHED();
+  g_ew_last_kernel = "sumsq_segments_kernel";
 }
 __global__ void reduce_splits_kernel(const float* __restrict__ src, float* __restrict__ dst, size_t n, int splits, size_t stride, int accumulate) { pdl_enter();
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -823,9 +835,11 @@ __global__ void reduce_splits_wide_kernel(const float* __restrict__ src, float* 
 }
 void k_reduce_splits(const float* src, float* dst, size_t n, int splits, size_t stride, int accumulate, cudaStream_t s) {
   if (n && splits >= 64 && n <= (1u << 16)) {
-    launch_pdl(reduce_splits_wide_kernel, dim3((unsigned)((n * 32 + 255) / 256)), dim3(256), (size_t)0, s, src, dst, n, splits, stride, accumulate); LAUNCHED(); return;
+    launch_pdl(reduce_splits_wide_kernel, dim3((unsigned)((n * 32 + 255) / 256)), dim3(256), (size_t)0, s, src, dst, n, splits, stride, accumulate); LAUNCHED();
+    g_ew_last_kernel = "reduce_splits_wide_kernel"; return;
   }
   if (!n) return; launch_pdl(reduce_splits_kernel, dim3(ew_blocks(n)), dim3(256), (size_t)(0), s, src, dst, n, splits, stride, accumulate); LAUNCHED();
+  g_ew_last_kernel = "reduce_splits_kernel";
 }
 
 // every split-K partial sum of a backward pass in ONE launch: block -> (job, chunk); few splits: a thread owns 4 consecutive outputs and walks
@@ -865,6 +879,7 @@ void k_reduce_multi(const ReduceList& rl, cudaStream_t s) {
   int blocks = 0; for (int i = 0; i < rl.count; ++i) blocks += abs(rl.jobs[i].blocks);
   if (!blocks) return;
   launch_pdl(reduce_multi_kernel, dim3(blocks), dim3(256), (size_t)0, s, rl); LAUNCHED();
+  g_ew_last_kernel = "reduce_multi_kernel";
 }
 
 // ---------------------------------------------------------------- updater -------------------------------

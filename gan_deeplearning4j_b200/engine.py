@@ -467,11 +467,13 @@ EPI_PLAIN, EPI_STATS, EPI_BNBWD, EPI_ACTBWD = 0, 1, 2, 3
 
 def test_conv_ex(ctx: Context, kind: int, geom: Dict[str, int], a, b, out_size: int, *, epi: int = 0, act: str = "identity", alpha: float = 0.0,
                  bias=None, scale=None, groups: int = 1, aux=None, aux2=None, iters: int = 1, impl: int = 1, bn: int = 0, max_ctas: int = 0,
-                 poison: bool = False, w_mn: bool = False, per_tap: bool = False, info: Optional[dict] = None):
+                 poison: bool = False, w_mn: bool = False, per_tap: bool = False, info: Optional[dict] = None, defer: bool = False, db=None):
     """Tensor-core fprop (kind 0) / dgrad (kind 1) with the epilogue the training step uses (impl 3, kind 1: the pixel-shuffle deconv, b = the
     [O][4][4][C] weight).  bn forces the 64- / 128-column tile, max_ctas caps the persistent grid (0: production choice for both); poison
     fills the output with bf16 NaN before every launch; w_mn (kind 0, 1x1): b is the [C][O] dense weight; per_tap keeps a 4x4 s2 p1 shape on
     one activation box per tap instead of the slabs two taps share.  info, if given, receives "slab": whether the launch used the slabs.
+    Weight gradients (kind 2, impl 1 / 3): defer queues the split-K sum and runs it as the backward pass's one reduce-list launch; db (impl 3,
+    a float32 array of O elements) receives the bias gradient the edge kernel computes beside dw.
     Returns (out, stats or None, kernel name, ms)."""
     g = _lib.ConvGeom(**geom)
     a, b = _f32(a).ravel(), _f32(b).ravel()
@@ -479,7 +481,10 @@ def test_conv_ex(ctx: Context, kind: int, geom: Dict[str, int], a, b, out_size: 
     oc = geom["o"] if kind == 0 else geom["c"]
     o = _lib.TestConvOpts()
     o.epi, o.act, o.alpha, o.groups = epi, ACTS[act], alpha, groups
-    o.bn, o.max_ctas, o.poison, o.w_mn, o.per_tap = bn, max_ctas, int(poison), int(w_mn), int(per_tap)
+    o.bn, o.max_ctas, o.poison, o.w_mn, o.per_tap, o.defer = bn, max_ctas, int(poison), int(w_mn), int(per_tap), int(defer)
+    if db is not None:
+        assert db.dtype == np.float32 and db.flags.c_contiguous
+        o.db = _fp(db)
     keep = []
     for name, v in (("bias", bias), ("scale", scale), ("aux", aux), ("aux2", aux2)):
         if v is not None:
@@ -521,3 +526,35 @@ def test_dropout(ctx: Context, precision: int, x, dy, p: float, *, seed: int = 6
     y, dx = np.empty_like(x), np.empty_like(x)
     check(ctx.lib.b2g_test_dropout(ctx.h, precision, seed, layer, rank, pass_, rows, h, w, c, p, _fp(x), _fp(e), _fp(y), _fp(dx)))
     return y, dx
+
+
+EW_OPS = {"reduce_splits": 0, "reduce_multi": 1, "colsum": 2, "xent": 3, "softmax_xent": 4, "act_fwd": 5, "act_bwd": 6, "maxpool": 7,
+          "upsample": 8, "sumsq": 9}
+
+
+def test_ew(ctx: Context, precision: int, op: str, in0, in1=None, out_sizes=(0, 0, 0), *, act: str = "identity", jobs=None, segments=None, **opts):
+    """One reduction / loss / element-wise kernel through its production wrapper (b2g_test_ew; operands per op in include/b200gan.h).
+    out_sizes: element counts of out0..out2 (0: not asked for).  opts: the b2g_test_ew_opts sizes and switches (n, rows, cols, groups, splits,
+    stride, N, H, W, C, KH, KW, SH, SW, alpha, clip_eps, offset, in_place, accumulate, poison).  jobs (reduce_multi): dicts of n, splits,
+    stride, src_off, dst_off.  segments (sumsq): (offsets, lengths, coefficients).
+    Returns ([out0, out1, out2] with None where not asked for, {"kernel": names, "sumsq": float, "wide": [per job]})."""
+    o = _lib.TestEwOpts()
+    o.op, o.act = EW_OPS[op], ACTS[act]
+    for k, v in opts.items():
+        setattr(o, k, int(v) if isinstance(v, bool) else v)
+    keep = []
+    if jobs is not None:
+        arr = (_lib.EwReduceJob * len(jobs))(*[_lib.EwReduceJob(j["n"], j["stride"], j["src_off"], j["dst_off"], j["splits"], 0) for j in jobs])
+        o.n_jobs, o.jobs = len(jobs), arr
+        keep.append(arr)
+    if segments is not None:
+        so, sl, sc = (np.ascontiguousarray(segments[0], np.int64), np.ascontiguousarray(segments[1], np.int64), _f32(segments[2]))
+        keep += [so, sl, sc]
+        o.n_seg = len(so)
+        o.seg_off, o.seg_len, o.seg_coef = so.ctypes.data_as(C.POINTER(C.c_int64)), sl.ctypes.data_as(C.POINTER(C.c_int64)), _fp(sc)
+    ins = [None if v is None else _f32(v).ravel() for v in (in0, in1)]
+    outs = [np.empty(k, np.float32) if k else None for k in out_sizes]
+    ptr = lambda a: None if a is None else _fp(a)
+    check(ctx.lib.b2g_test_ew(ctx.h, precision, C.byref(o), *[ptr(a) for a in ins], *[ptr(a) for a in outs]))
+    info = {"kernel": o.kernel.decode(), "sumsq": o.sumsq, "wide": [o.jobs[i].wide for i in range(o.n_jobs)] if jobs is not None else []}
+    return outs, info

@@ -326,6 +326,10 @@ typedef struct {
   int32_t w_mn;           /* impl 1 kind 0, 1x1 geometry: the weight operand is [C][O] (the dense input gradient's own [nOut][nIn] weight) */
   int32_t per_tap;        /* impl 1: load the activations one box per tap also where the 4x4 s2 p1 slab path applies */
   int32_t slab;           /* out: 1 when the launch loaded its activations as slabs shared by two taps */
+  /* kind 2, impl 1 / impl 3: queue the split-K reduction into a list and sum it with ONE reduce-list launch afterwards, as a backward pass
+   * does, instead of reducing right after the wgrad kernel */
+  int32_t defer;
+  float* db;              /* kind 2, impl 3, C < 4: out [O], the bias gradient (column sums of dy) the edge wgrad kernel produces beside dw; NULL: not asked */
 } b2g_test_conv_opts;
 int32_t b2g_test_conv_ex(b2g_ctx* ctx, int32_t kind, int32_t impl, int32_t precision, const b2g_conv_geom* g,
                          const float* x_or_dy, const float* w_or_x, float* out, int32_t iters, float* ms_per_iter, b2g_test_conv_opts* opts);
@@ -352,6 +356,51 @@ int32_t b2g_test_net_shadow(b2g_net* net, int32_t layer, int32_t which, float* o
  * B2G_LAYER_DROPOUT.  Out: y, dx (same order).  Fails unless the forward advanced its pass counter from pass to pass + 1. */
 int32_t b2g_test_dropout(b2g_ctx* ctx, int32_t precision, uint64_t seed, int32_t layer, int32_t rank, int64_t pass, int32_t rows, int32_t h, int32_t w,
                          int32_t c, float p, const float* x, const float* dy, float* y, float* dx);
+
+/* One reduction, loss or element-wise kernel of the training step on host tensors, through its production launch wrapper (tests).
+ * T tensors are fp32 on the host, rounded to bf16 on the device when precision is BF16 and widened back on the way out; the others are fp32.
+ *   REDUCE_SPLITS  in0 src [splits*stride] fp32, in1 dst's initial value [n]          -> out0 dst [n]            (n, splits, stride, accumulate)
+ *   REDUCE_MULTI   in0 one fp32 buffer [n]; the jobs index into it                    -> out0 the buffer [n]     (jobs, n_jobs)
+ *   COLSUM         in0 x [rows][cols] T, in1 out's initial value [cols]               -> out0 [cols]             (rows, cols, accumulate)
+ *   XENT           in0 logits [groups][rows] T, in1 labels fp32                       -> out0 dz T, out1 loss per group [groups]   (clip_eps)
+ *   SOFTMAX_XENT   in0 logits [rows][cols] T, in1 labels fp32 or NULL (inference: no labels, dz or loss passed to the kernel)
+ *                                                                                     -> out0 dz T, out1 loss [1], out2 probabilities T
+ *   ACT_FWD        in0 x [n] T                                                        -> out0 act(x) T           (act, alpha)
+ *   ACT_BWD        in0 a = the forward output [n] T, in1 eps_out [n] T                -> out0 eps_in T           (act, alpha, in_place)
+ *   MAXPOOL        in0 x [N][H][W][C] T, in1 eps_out [N][OH][OW][C] T (OH = (H-KH)/SH + 1, OW likewise)
+ *                                                                                     -> out0 y T, out1 eps_in T, out2 argmax (as float)
+ *   UPSAMPLE       in0 x [N][H][W][C] T, in1 eps_out [N][H*KH][W*KH][C] T (factor KH) -> out0 y T, out1 eps_in T
+ *   SUMSQ          in0 p [n] fp32, segments seg_off / seg_len / seg_coef              -> sumsq
+ * Every output buffer not asked for may be NULL. */
+typedef enum {
+  B2G_EW_REDUCE_SPLITS = 0, B2G_EW_REDUCE_MULTI = 1, B2G_EW_COLSUM = 2, B2G_EW_XENT = 3, B2G_EW_SOFTMAX_XENT = 4,
+  B2G_EW_ACT_FWD = 5, B2G_EW_ACT_BWD = 6, B2G_EW_MAXPOOL = 7, B2G_EW_UPSAMPLE = 8, B2G_EW_SUMSQ = 9
+} b2g_ew_op;
+typedef struct {          /* one split-K sum of a reduce list: dst[i] = sum_s src[s*stride + i], i < n, all offsets in elements of in0 */
+  int64_t n, stride, src_off, dst_off;
+  int32_t splits;
+  int32_t wide;           /* out: 1 when the list runs this job one warp per output, 0 when one thread per 4 outputs */
+} b2g_ew_reduce_job;
+typedef struct {
+  int32_t op;             /* b2g_ew_op */
+  int64_t n;              /* REDUCE_SPLITS outputs, REDUCE_MULTI buffer length, ACT_* / SUMSQ elements */
+  int32_t rows, cols;     /* COLSUM rows x channels; XENT rows per group; SOFTMAX_XENT rows x classes */
+  int32_t groups;         /* XENT */
+  int32_t splits; int64_t stride;       /* REDUCE_SPLITS */
+  int32_t N, H, W, C, KH, KW, SH, SW;  /* MAXPOOL input and window; UPSAMPLE input and factor KH */
+  int32_t act; float alpha;             /* ACT_*: b2g activation */
+  float clip_eps;                       /* XENT: 0 = BCE with logits */
+  int32_t offset;         /* every device operand starts this many elements past a 256-byte aligned address (reaches the misaligned fallbacks) */
+  int32_t in_place;       /* ACT_BWD: eps_in is eps_out's buffer, as the backward pass calls it */
+  int32_t accumulate;     /* REDUCE_SPLITS / COLSUM: add to the initial destination in1 */
+  int32_t poison;         /* fill every output with NaN before the launch: an element the kernel leaves unwritten reads back as NaN */
+  int32_t n_jobs; b2g_ew_reduce_job* jobs;                              /* REDUCE_MULTI: at most 24 */
+  int32_t n_seg; const int64_t* seg_off; const int64_t* seg_len; const float* seg_coef;   /* SUMSQ */
+  double sumsq;           /* out: SUMSQ's result */
+  char kernel[64];        /* out: the kernel each wrapper call dispatched, comma-separated in call order (MAXPOOL / UPSAMPLE: forward, backward);
+                             COLSUM names its first stage, the final stage is the same kernel on every path */
+} b2g_test_ew_opts;
+int32_t b2g_test_ew(b2g_ctx* ctx, int32_t precision, b2g_test_ew_opts* opts, const float* in0, const float* in1, float* out0, float* out1, float* out2);
 
 #ifdef __cplusplus
 }

@@ -52,14 +52,21 @@ def test_struct_layouts_match_the_c_header(tmp_path):
                     'printf("%zu %zu %zu %zu %zu %zu %zu %zu %zu\\n", sizeof(b2g_layer_desc), offsetof(b2g_layer_desc,n_in), offsetof(b2g_layer_desc,updater),'
                     ' offsetof(b2g_layer_desc,pre_c), sizeof(b2g_net_config), offsetof(b2g_net_config,seed), sizeof(b2g_gan_config), sizeof(b2g_conv_geom), offsetof(b2g_net_config,bn_groups));'
                     'printf("%zu %zu %zu %zu %zu %zu %zu\\n", sizeof(b2g_test_conv_opts), offsetof(b2g_test_conv_opts,stats), offsetof(b2g_test_conv_opts,kernel),'
-                    ' offsetof(b2g_test_conv_opts,bn), offsetof(b2g_test_conv_opts,max_ctas), offsetof(b2g_test_conv_opts,poison), offsetof(b2g_test_conv_opts,w_mn));return 0;}')
+                    ' offsetof(b2g_test_conv_opts,bn), offsetof(b2g_test_conv_opts,max_ctas), offsetof(b2g_test_conv_opts,poison), offsetof(b2g_test_conv_opts,w_mn));'
+                    'printf("%zu %zu %zu %zu\\n", offsetof(b2g_test_conv_opts,per_tap), offsetof(b2g_test_conv_opts,slab), offsetof(b2g_test_conv_opts,defer), offsetof(b2g_test_conv_opts,db));'
+                    'printf("%zu %zu %zu\\n", sizeof(b2g_ew_reduce_job), offsetof(b2g_ew_reduce_job,splits), offsetof(b2g_ew_reduce_job,wide));'
+                    + "".join(f'printf("%zu\\n", offsetof(b2g_test_ew_opts,{f}));' for f, _ in _lib.TestEwOpts._fields_) +
+                    'printf("%zu\\n", sizeof(b2g_test_ew_opts));return 0;}')
     exe = tmp_path / "layout"
     subprocess.run(["gcc", "-I", os.path.join(ROOT, "include"), str(prog), "-o", str(exe)], check=True)
     got = [int(v) for v in subprocess.run([str(exe)], capture_output=True, text=True).stdout.split()]
-    L, N, T = _lib.LayerDesc, _lib.NetConfig, _lib.TestConvOpts
+    L, N, T, E, J = _lib.LayerDesc, _lib.NetConfig, _lib.TestConvOpts, _lib.TestEwOpts, _lib.EwReduceJob
     assert got == [C.sizeof(L), L.n_in.offset, L.updater.offset, L.pre_c.offset, C.sizeof(N), N.seed.offset, C.sizeof(_lib.GanConfig), C.sizeof(_lib.ConvGeom), N.bn_groups.offset,
-                   C.sizeof(T), T.stats.offset, T.kernel.offset, T.bn.offset, T.max_ctas.offset, T.poison.offset, T.w_mn.offset]
-    assert (T.stats.offset, T.kernel.offset) == (56, 64)         # the fields older callers fill keep their offsets
+                   C.sizeof(T), T.stats.offset, T.kernel.offset, T.bn.offset, T.max_ctas.offset, T.poison.offset, T.w_mn.offset,
+                   T.per_tap.offset, T.slab.offset, T.defer.offset, T.db.offset, C.sizeof(J), J.splits.offset, J.wide.offset] + \
+        [getattr(E, f).offset for f, _ in E._fields_] + [C.sizeof(E)]
+    assert (T.stats.offset, T.kernel.offset, T.bn.offset, T.slab.offset) == (56, 64, 128, 148)       # the fields older callers fill keep their offsets
+    assert (T.defer.offset, T.db.offset) == (152, 160)
 
 
 def test_no_device_fails_loudly_not_silently(lib):
