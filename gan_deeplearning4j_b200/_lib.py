@@ -97,6 +97,7 @@ PROTOTYPES = {
     "b2g_net_get_params": (_i32, [_vp, _fp, _i64]),
     "b2g_net_set_params": (_i32, [_vp, _fp, _i64]),
     "b2g_net_get_gradients": (_i32, [_vp, _fp, _i64]),
+    "b2g_net_updater_state_size": (_i32, [_vp, C.POINTER(_i64)]),
     "b2g_net_get_updater_state": (_i32, [_vp, _fp, _i64]),
     "b2g_net_set_updater_state": (_i32, [_vp, _fp, _i64]),
     "b2g_net_output": (_i32, [_vp, _fp, _i32, _i32, _fp]),

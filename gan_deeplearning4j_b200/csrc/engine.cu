@@ -111,6 +111,8 @@ struct b2g_net {
   int prec = PREC_F32;
   int64_t n_params = 0;
   float *params = nullptr, *grads = nullptr, *st0 = nullptr, *st1 = nullptr;
+  float* st2 = nullptr;                // third updater state slot (AMSGrad's v-hat): only nets with an AMSGrad segment have it
+  bool upd_ext = false;                // some segment has a kind >= 4: the updater runs its extended instantiations
   __nv_bfloat16* shadow = nullptr; int64_t n_shadow = 0;
   std::vector<UpdSeg> segs; UpdSeg* segs_dev = nullptr; int32_t* chunk_seg_dev = nullptr; int64_t* chunk_off_dev = nullptr; int nchunks = 0;
   int64_t *l2_off_dev = nullptr, *l2_len_dev = nullptr; float* l2_coef_dev = nullptr; int n_l2 = 0;
@@ -340,7 +342,8 @@ static int32_t net_alloc(b2g_net* n) {
   return 0;
 }
 
-static int updater_kind(int u) { return u == B2G_UPD_SGD ? 0 : u == B2G_UPD_RMSPROP ? 1 : u == B2G_UPD_ADAM ? 2 : 3; }
+// b2g_updater values are the updater kernel's kinds (b2g_net_create has rejected any other value)
+static int updater_kind(int u) { return u; }
 
 static int32_t net_init_params_and_updater(b2g_net* n) {
   cudaStream_t s = n->ctx->stream;
@@ -355,7 +358,7 @@ static int32_t net_init_params_and_updater(b2g_net* n) {
       UpdSeg sg{}; sg.off = off; sg.len = len; sg.kind = noop ? 3 : updater_kind(d.updater);
       sg.lr = d.lr; sg.b1 = d.beta1; sg.b2 = d.beta2; sg.eps = d.eps; sg.l2 = weight ? d.l2 : 0.f; sg.clip = n->cfg.grad_clip; sg.div_mb = noop ? 0 : 1;
       sg.off_bf = (weight && l.off_W_bf >= 0) ? l.off_W_bf : -1; sg.off_ps = (weight && l.off_Wps_bf >= 0) ? l.off_Wps_bf : -1; sg.ps_O = l.geom.O; sg.ps_C = l.geom.C; n->segs.push_back(sg); seg_layer.push_back((int)(&l - n->L.data()));
-      if (!noop && sg.kind == 1) for (int64_t i = 0; i < len; ++i) h0[off + i] = d.eps;     // RmsPropUpdater cache initialised to epsilon
+      if (!noop && (sg.kind == 1 || sg.kind == 5)) for (int64_t i = 0; i < len; ++i) h0[off + i] = d.eps;     // RmsProp cache / AdaGrad history initialised to epsilon
       if (weight && d.l2 != 0.f) { l2o.push_back(off); l2l.push_back(len); l2c.push_back(0.5f * d.l2); }
     };
     if (l.has_gemm()) {
@@ -375,6 +378,9 @@ static int32_t net_init_params_and_updater(b2g_net* n) {
   CU(cudaMemcpyAsync(n->params, hp.data(), sizeof(float) * n->n_params, cudaMemcpyHostToDevice, s));
   CU(cudaMemcpyAsync(n->st0, h0.data(), sizeof(float) * n->n_params, cudaMemcpyHostToDevice, s));
   CU(cudaMemsetAsync(n->st1, 0, sizeof(float) * n->n_params, s)); CU(cudaMemsetAsync(n->grads, 0, sizeof(float) * n->n_params, s));
+  bool amsgrad = false;
+  for (const UpdSeg& sg : n->segs) { n->upd_ext = n->upd_ext || sg.kind >= 4; amsgrad = amsgrad || sg.kind == 8; }
+  if (amsgrad) { B2(dalloc(n, &n->st2, sizeof(float) * n->n_params)); CU(cudaMemsetAsync(n->st2, 0, sizeof(float) * n->n_params, s)); }
   CU(cudaMemsetAsync(n->step_dev, 0, sizeof(int), s));
   std::vector<int32_t> cs; std::vector<int64_t> co;
   for (size_t i = 0; i < n->segs.size(); ++i) for (int64_t o = n->segs[i].off; o < n->segs[i].off + n->segs[i].len; o += UPD_CHUNK) { cs.push_back((int32_t)i); co.push_back(o); }
@@ -773,8 +779,8 @@ static int32_t net_update(b2g_net* n, int mb_local) {
   }
   // one pass: /mb -> [x multiplier] -> clip -> updater [at the scheduled lr] -> +l2*W -> theta -= g, the bf16 operand copies (straight and
   // packed) and the iteration counter
-  k_updater(n->params, n->grads, n->st0, n->st1, n->segs_dev, n->chunk_seg_dev, n->chunk_off_dev, n->nchunks, inv_mb, inv_world, n->step_dev, n->upd_ticket, n->shadow,
-            gn ? n->gn_mult : nullptr, n->sched_on ? n->sched_dev : nullptr, n->epoch_dev, s);
+  k_updater(n->params, n->grads, n->st0, n->st1, n->st2, n->segs_dev, n->chunk_seg_dev, n->chunk_off_dev, n->nchunks, inv_mb, inv_world, n->step_dev, n->upd_ticket,
+            n->shadow, gn ? n->gn_mult : nullptr, n->sched_on ? n->sched_dev : nullptr, n->epoch_dev, n->upd_ext, s);
   CHECK_KERNELS();
   return 0;
 }
@@ -836,6 +842,8 @@ extern "C" int32_t b2g_net_create(b2g_ctx* ctx, const b2g_net_config* cfg, const
   if (!ctx || !cfg || !layers || nl < 1 || !out) return fail(B2G_ERR_ARG, "b2g_net_create: null/empty argument");
   if (cfg->max_batch < 1 || cfg->in_h < 1 || cfg->in_w < 1 || cfg->in_c < 1) return fail(B2G_ERR_ARG, "b2g_net_create: bad input type / max_batch");
   if (cfg->precision != B2G_PREC_FP32 && cfg->precision != B2G_PREC_BF16) return fail(B2G_ERR_ARG, "b2g_net_create: precision %d", cfg->precision);
+  for (int32_t i = 0; i < nl; ++i)
+    if (layers[i].updater < B2G_UPD_SGD || layers[i].updater > B2G_UPD_ADADELTA) return fail(B2G_ERR_ARG, "b2g_net_create: layer %d: unknown updater %d", i, layers[i].updater);
   CU(cudaSetDevice(ctx->device));
   b2g_net* n = new b2g_net(); n->ctx = ctx; n->cfg = *cfg; n->prec = cfg->precision == B2G_PREC_BF16 ? PREC_BF16 : PREC_F32;
   if (n->cfg.bn_groups < 1) n->cfg.bn_groups = 1;
@@ -914,15 +922,20 @@ extern "C" int32_t b2g_net_set_params(b2g_net* n, const float* host, int64_t cnt
   if (!n || !host) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device)); B2(write_flat(n, n->params, host, cnt)); net_refresh_shadow(n); CU(cudaStreamSynchronize(n->ctx->stream)); return 0;
 }
 extern "C" int32_t b2g_net_get_gradients(b2g_net* n, float* host, int64_t cnt) { if (!n || !host) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device)); return read_flat(n, n->grads, host, cnt); }
+// [state0 | state1], plus | state2 on nets with an AMSGrad segment
+static int64_t updater_state_size(const b2g_net* n) { return (n->st2 ? 3 : 2) * n->n_params; }
+extern "C" int32_t b2g_net_updater_state_size(b2g_net* n, int64_t* out) { if (!n || !out) return fail(B2G_ERR_ARG, "null"); *out = updater_state_size(n); return 0; }
 extern "C" int32_t b2g_net_get_updater_state(b2g_net* n, float* host, int64_t cnt) {
   if (!n || !host) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
-  if (cnt != 2 * n->n_params) return fail(B2G_ERR_SHAPE, "updater state has %lld elements", (long long)(2 * n->n_params));
-  B2(read_flat(n, n->st0, host, n->n_params)); return read_flat(n, n->st1, host + n->n_params, n->n_params);
+  if (cnt != updater_state_size(n)) return fail(B2G_ERR_SHAPE, "updater state has %lld elements", (long long)updater_state_size(n));
+  B2(read_flat(n, n->st0, host, n->n_params)); B2(read_flat(n, n->st1, host + n->n_params, n->n_params));
+  return n->st2 ? read_flat(n, n->st2, host + 2 * n->n_params, n->n_params) : 0;
 }
 extern "C" int32_t b2g_net_set_updater_state(b2g_net* n, const float* host, int64_t cnt) {
   if (!n || !host) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
-  if (cnt != 2 * n->n_params) return fail(B2G_ERR_SHAPE, "updater state has %lld elements", (long long)(2 * n->n_params));
-  B2(write_flat(n, n->st0, host, n->n_params)); return write_flat(n, n->st1, host + n->n_params, n->n_params);
+  if (cnt != updater_state_size(n)) return fail(B2G_ERR_SHAPE, "updater state has %lld elements", (long long)updater_state_size(n));
+  B2(write_flat(n, n->st0, host, n->n_params)); B2(write_flat(n, n->st1, host + n->n_params, n->n_params));
+  return n->st2 ? write_flat(n, n->st2, host + 2 * n->n_params, n->n_params) : 0;
 }
 
 // host NCHW fp32 -> device input buffer (T NHWC)
@@ -1201,17 +1214,17 @@ extern "C" int32_t b2g_net_set_gradient_normalization(b2g_net* n, int32_t mode, 
 }
 
 // ------------------------------------------------------------------ learning-rate schedules ---------------
-// A layer has a learning rate when it is not frozen, has parameters and its updater is not NoOp: when it owns an updater segment that is not
-// a NoOp one (frozen layers own no segments; a NoOp updater and BatchNorm mean/var make NoOp segments).  The Python layer specs apply the same
-// rule (engine.py layer_has_lr); b2g_net_get_learning_rate reads the layer's first such segment.
+// A layer has a learning rate when it is not frozen, has parameters and its updater is neither NoOp nor AdaDelta: when it owns an updater
+// segment of another kind (frozen layers own no segments; a NoOp updater and BatchNorm mean/var make NoOp segments; AdaDelta has no learning
+// rate).  The Python layer specs apply the same rule (engine.py layer_has_lr); b2g_net_get_learning_rate reads the layer's first such segment.
 static int lr_segment(const b2g_net* n, int li) {
-  for (size_t i = 0; i < n->segs.size(); ++i) if (n->seg_layer[i] == li && n->segs[i].kind != 3) return (int)i;
+  for (size_t i = 0; i < n->segs.size(); ++i) if (n->seg_layer[i] == li && n->segs[i].kind != 3 && n->segs[i].kind != 9) return (int)i;
   return -1;
 }
 static bool layer_has_lr(const b2g_net* n, int li) { return lr_segment(n, li) >= 0; }
 static int32_t find_lr_layer(const b2g_net* n, const char* layer, int* li) {
   for (size_t i = 0; i < n->L.size(); ++i) if (!strncmp(n->L[i].d.name, layer, B2G_NAME_LEN)) {
-    if (!layer_has_lr(n, (int)i)) return fail(B2G_ERR_ARG, "layer %s has no learning rate (frozen, no parameters, or NoOp)", layer);
+    if (!layer_has_lr(n, (int)i)) return fail(B2G_ERR_ARG, "layer %s has no learning rate (frozen, no parameters, NoOp or AdaDelta)", layer);
     *li = (int)i; return 0;
   }
   return fail(B2G_ERR_ARG, "no layer named %s", layer);
@@ -1354,8 +1367,8 @@ extern "C" int32_t b2g_net_average_parameters(b2g_net* n) {
   if (!n) return fail(B2G_ERR_ARG, "null"); b2g_ctx* c = n->ctx; CU(cudaSetDevice(c->device));
   if (!c->comm || c->world == 1) return 0;
   const float inv = 1.0f / (float)c->world; cudaStream_t s = c->stream;
-  float* bufs[3] = {n->params, n->st0, n->st1};
-  for (float* b : bufs) { NC(g_nccl.ar(b, b, (size_t)n->n_params, 7, 0, c->comm, s)); k_scale_f32(b, inv, (size_t)n->n_params, s); }
+  float* bufs[4] = {n->params, n->st0, n->st1, n->st2};
+  for (float* b : bufs) { if (!b) continue; NC(g_nccl.ar(b, b, (size_t)n->n_params, 7, 0, c->comm, s)); k_scale_f32(b, inv, (size_t)n->n_params, s); }
   net_refresh_shadow(n);
   CU(cudaStreamSynchronize(s)); return 0;
 }
@@ -1798,8 +1811,8 @@ extern "C" int32_t b2g_test_hbm_kernels(b2g_net* n, int32_t rows, int32_t channe
   for (int which = 0; which < 3; ++which) for (int it = -1; it < iters; ++it) {
     B2(b2g_flush_l2(c));
     CU(cudaEventRecord(e0, s));
-    if (which == 0) k_updater(n->params, n->grads, n->st0, n->st1, n->segs_dev, n->chunk_seg_dev, n->chunk_off_dev, n->nchunks, 1.0f, 1.0f, n->step_dev, n->upd_ticket, n->shadow, nullptr,
-                              nullptr, nullptr, s);
+    if (which == 0) k_updater(n->params, n->grads, n->st0, n->st1, n->st2, n->segs_dev, n->chunk_seg_dev, n->chunk_off_dev, n->nchunks, 1.0f, 1.0f, n->step_dev, n->upd_ticket,
+                              n->shadow, nullptr, nullptr, nullptr, n->upd_ext, s);
     else if (which == 1) k_bn_apply_acc(x, y, rows, channels, 1, acc, gb, gb + channels, ACT_LRELU, 0.2f, 1e-5f, coef, gb + 2 * channels, gb + 3 * channels, nullptr, nullptr, 0.9f, s);
     else k_bn_bwd_apply_acc(x, e, y, rows, channels, 1, coef, ACT_LRELU, 0.2f, 1, acc, gb, gb + channels, 0, s);
     CU(cudaEventRecord(e1, s)); CU(cudaEventSynchronize(e1));

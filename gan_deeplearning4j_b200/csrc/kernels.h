@@ -118,8 +118,8 @@ void k_reduce_multi(const ReduceList& rl, cudaStream_t s);
 // ---- updater (BaseMultiLayerUpdater + UpdaterBlock + params.subi, one pass) -----------------------------
 struct UpdSeg {            // one parameter tensor
   int64_t off, len;
-  int kind;                // 0 sgd, 1 rmsprop, 2 adam, 3 noop
-  float lr, b1, b2, eps;   // rmsprop: b1 = rmsDecay
+  int kind;                // b2g_updater: 0 sgd, 1 rmsprop, 2 adam, 3 noop, 4 nesterovs, 5 adagrad, 6 adamax, 7 nadam, 8 amsgrad, 9 adadelta
+  float lr, b1, b2, eps;   // rmsprop: b1 = rmsDecay; nesterovs: b1 = momentum; adadelta: b1 = rho (lr unused)
   float l2;                // post-updater, not lr-scaled (pre-beta4)
   float clip;              // elementwise clip threshold, 0 = off
   int div_mb;              // 0 for BN mean/var pseudo-gradients
@@ -140,9 +140,11 @@ struct UpdSched {
 // gn_mult (may be null): one fp32 multiplier per segment (k_gradnorm), applied to g right after the minibatch division.
 // sched (may be null): one UpdSched per segment; each block then takes its segment's lr from the schedule at iteration *step_dev (before the
 // increment) or at epoch *epoch_dev, both read from device memory.
-void k_updater(float* params, const float* grads, float* st0, float* st1, const UpdSeg* segs_dev, const int32_t* chunk_seg_dev,
+// ext: some segment has a kind >= 4 (then the extended instantiations run; every other net launches the kernels it always launched).  st2: the
+// third state slot (AMSGrad's v-hat), may be null when no segment is AMSGrad.
+void k_updater(float* params, const float* grads, float* st0, float* st1, float* st2, const UpdSeg* segs_dev, const int32_t* chunk_seg_dev,
                const int64_t* chunk_off_dev, int nchunks, float inv_mb, float inv_world, int* step_dev /* t = *step_dev + 1 */, unsigned* ticket,
-               __nv_bfloat16* shadow, const float* gn_mult, const UpdSched* sched, const int64_t* epoch_dev, cudaStream_t s);
+               __nv_bfloat16* shadow, const float* gn_mult, const UpdSched* sched, const int64_t* epoch_dev, bool ext, cudaStream_t s);
 // *out = the fp32 learning rate the updater kernel would use for segment seg at the current *step_dev / *epoch_dev (one thread, one launch)
 void k_sched_lr(const UpdSeg* segs_dev, const UpdSched* sched, int seg, const int* step_dev, const int64_t* epoch_dev, float* out, cudaStream_t s);
 static const int UPD_CHUNK = 4096;

@@ -883,10 +883,14 @@ void k_reduce_multi(const ReduceList& rl, cudaStream_t s) {
 }
 
 // ---------------------------------------------------------------- updater -------------------------------
-// One pass over params: 28 B/param for Adam (read p,g,m,v; write p,m,v), 20 B/param RmsProp, +2 B bf16 shadow.
+// One pass over params: 28 B/param for Adam (read p,g,m,v; write p,m,v), 20 B/param RmsProp, +2 B bf16 shadow.  EXT kinds: Nesterovs and
+// AdaGrad 20 B, AdaMax, Nadam and AdaDelta 28 B, AMSGrad 36 B (include/b200gan.h, b2g_updater, states each formula).
 // SCALED: the L2 gradient normalization multiplier of the segment (kernels_gradnorm.cu) follows the minibatch division
-template <bool SCALED>
-__device__ __forceinline__ float upd_elem(const UpdSeg& sg, float g, float p, float& s0, float& s1, float gscale, float alpha_t, float gmult) {
+// EXT: the kinds 4-9 besides 0-3 (a net that has one still has NoOp BatchNorm mean/var segments); s2 is AMSGrad's v-hat.  alpha_t: Adam's and
+// AMSGrad's lr * sqrt(1 - b2^t) / (1 - b1^t), AdaMax's and Nadam's lr / (1 - b1^t), per block.
+template <bool SCALED, bool EXT = false>
+__device__ __forceinline__ float upd_elem(const UpdSeg& sg, float g, float p, float& s0, float& s1, float gscale, float alpha_t, float gmult,
+                                          float* s2 = nullptr) {
   g *= gscale;
   if (SCALED) g *= gmult;
   if (sg.clip > 0.f) g = fminf(fmaxf(g, -sg.clip), sg.clip);
@@ -894,7 +898,16 @@ __device__ __forceinline__ float upd_elem(const UpdSeg& sg, float g, float p, fl
   if (sg.kind == 0) u = sg.lr * g;
   else if (sg.kind == 1) { s0 = sg.b1 * s0 + (1.0f - sg.b1) * g * g; u = sg.lr * g / (sqrtf(s0) + sg.eps); }
   else if (sg.kind == 2) { s0 = sg.b1 * s0 + (1.0f - sg.b1) * g; s1 = sg.b2 * s1 + (1.0f - sg.b2) * g * g; u = alpha_t * s0 / (sqrtf(s1) + sg.eps); }
-  else u = g;
+  else if (!EXT || sg.kind == 3) u = g;
+  else if (sg.kind == 4) { const float vp = s0; s0 = sg.b1 * s0 - sg.lr * g; u = sg.b1 * vp - (1.0f + sg.b1) * s0; }             // Nesterovs
+  else if (sg.kind == 5) { s0 = s0 + g * g; u = sg.lr * g / (sqrtf(s0) + sg.eps); }                                               // AdaGrad
+  else if (sg.kind == 6) { s0 = sg.b1 * s0 + (1.0f - sg.b1) * g; s1 = fmaxf(sg.b2 * s1, fabsf(g)) + 1e-32f; u = alpha_t * s0 / s1; }  // AdaMax
+  else if (sg.kind == 7) { s0 = sg.b1 * s0 + (1.0f - sg.b1) * g; s1 = sg.b2 * s1 + (1.0f - sg.b2) * g * g;                        // Nadam
+                           u = alpha_t * (sg.b1 * s0 + (1.0f - sg.b1) * g) / (sqrtf(s1) + sg.eps); }
+  else if (sg.kind == 8) { s0 = sg.b1 * s0 + (1.0f - sg.b1) * g; s1 = sg.b2 * s1 + (1.0f - sg.b2) * g * g; *s2 = fmaxf(*s2, s1);   // AMSGrad
+                           u = alpha_t * s0 / (sqrtf(*s2) + sg.eps); }
+  else { s0 = sg.b1 * s0 + (1.0f - sg.b1) * g * g; u = sqrtf(s1 + sg.eps) / sqrtf(s0 + sg.eps) * g;                              // AdaDelta
+         s1 = sg.b1 * s1 + (1.0f - sg.b1) * u * u; }
   if (sg.l2 != 0.f) u = fmaf(sg.l2, p, u);
   return p - u;
 }
@@ -925,11 +938,13 @@ __device__ float sched_lr(const UpdSched& sc, float lr, int it, long long ep) {
   return (float)v;
 }
 // SCHED: the segment's lr comes from its schedule (thread 0 evaluates it once per block, at *step before the increment or at *epoch)
-template <bool SCALED, bool SCHED>
+// EXT: kinds 4-9 (upd_elem); st2 (AMSGrad's v-hat, allocated only for nets with an AMSGrad segment) is read by EXT instantiations only
+template <bool SCALED, bool SCHED, bool EXT>
 __global__ void __launch_bounds__(256) updater_kernel(float* __restrict__ params, const float* __restrict__ grads, float* __restrict__ st0, float* __restrict__ st1,
                                                       const UpdSeg* __restrict__ segs, const int32_t* __restrict__ chunk_seg, const int64_t* __restrict__ chunk_off,
                                                       float inv_mb, float inv_world, int* __restrict__ step, unsigned* __restrict__ ticket, __nv_bfloat16* __restrict__ shadow,
-                                                      const float* __restrict__ gn_mult, const UpdSched* __restrict__ sched, const int64_t* __restrict__ epoch) { pdl_enter();
+                                                      const float* __restrict__ gn_mult, const UpdSched* __restrict__ sched, const int64_t* __restrict__ epoch,
+                                                      float* __restrict__ st2) { pdl_enter();
   UpdSeg sg = segs[chunk_seg[blockIdx.x]];
   const float gmult = SCALED ? gn_mult[chunk_seg[blockIdx.x]] : 1.0f;
   const int64_t base = chunk_off[blockIdx.x];
@@ -942,24 +957,42 @@ __global__ void __launch_bounds__(256) updater_kernel(float* __restrict__ params
     sg.lr = lr_s;
   }
   float alpha_t = 0.f;
-  if (sg.kind == 2) alpha_t = sg.lr * sqrtf(1.0f - powf(sg.b2, (float)t)) / (1.0f - powf(sg.b1, (float)t));
+  if (!EXT) {
+    if (sg.kind == 2) alpha_t = sg.lr * sqrtf(1.0f - powf(sg.b2, (float)t)) / (1.0f - powf(sg.b1, (float)t));
+  } else {
+    if (sg.kind == 2 || sg.kind == 8) alpha_t = sg.lr * sqrtf(1.0f - powf(sg.b2, (float)t)) / (1.0f - powf(sg.b1, (float)t));
+    else if (sg.kind == 6 || sg.kind == 7) alpha_t = sg.lr / (1.0f - powf(sg.b1, (float)t));
+  }
   const float gscale = sg.div_mb ? inv_mb : inv_world;     // BN running-stat pseudo-gradients: no /mb, mean over ranks
-  const bool has0 = sg.kind == 1 || sg.kind == 2, has1 = sg.kind == 2, sh = shadow && sg.off_bf >= 0;
+  // state slots each kind reads and writes: s0 every kind but Sgd / NoOp, s1 Adam / AdaMax / Nadam / AMSGrad / AdaDelta, s2 AMSGrad
+  const bool has0 = EXT ? (sg.kind != 0 && sg.kind != 3) : (sg.kind == 1 || sg.kind == 2);
+  const bool has1 = EXT ? (sg.kind == 2 || (sg.kind >= 6 && sg.kind <= 9)) : sg.kind == 2;
+  const bool has2 = EXT && sg.kind == 8, sh = shadow && sg.off_bf >= 0;
   if (((base | end) & 3) == 0 && (!sh || ((sg.off_bf + (base - sg.off)) & 3) == 0)) {
-    // 16-byte path: a full 4096-element chunk is four float4 per thread and array, all 16 loads issued before the first use
-    float4 gv[4], pv[4], s0[4], s1[4];
+    // 16-byte path: a full 4096-element chunk is four float4 per thread and array, all 16 loads issued before the first use (20 with v-hat)
+    float4 gv[4], pv[4], s0[4], s1[4], s2[EXT ? 4 : 1];
 #pragma unroll
     for (int q = 0; q < 4; ++q) { const int64_t i = base + 4 * (threadIdx.x + q * (int64_t)blockDim.x); const bool ok = i < end; const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
       gv[q] = ok ? *reinterpret_cast<const float4*>(grads + i) : z; pv[q] = ok ? *reinterpret_cast<const float4*>(params + i) : z;
-      s0[q] = (ok && has0) ? *reinterpret_cast<const float4*>(st0 + i) : z; s1[q] = (ok && has1) ? *reinterpret_cast<const float4*>(st1 + i) : z; }
+      s0[q] = (ok && has0) ? *reinterpret_cast<const float4*>(st0 + i) : z; s1[q] = (ok && has1) ? *reinterpret_cast<const float4*>(st1 + i) : z;
+      if (EXT) s2[EXT ? q : 0] = (ok && has2) ? *reinterpret_cast<const float4*>(st2 + i) : z; }
 #pragma unroll
     for (int q = 0; q < 4; ++q) { const int64_t i = base + 4 * (threadIdx.x + q * (int64_t)blockDim.x); if (i >= end) continue;
       float4 p4;
-      p4.x = upd_elem<SCALED>(sg, gv[q].x, pv[q].x, s0[q].x, s1[q].x, gscale, alpha_t, gmult); p4.y = upd_elem<SCALED>(sg, gv[q].y, pv[q].y, s0[q].y, s1[q].y, gscale, alpha_t, gmult);
-      p4.z = upd_elem<SCALED>(sg, gv[q].z, pv[q].z, s0[q].z, s1[q].z, gscale, alpha_t, gmult); p4.w = upd_elem<SCALED>(sg, gv[q].w, pv[q].w, s0[q].w, s1[q].w, gscale, alpha_t, gmult);
+      if (!EXT) {
+        p4.x = upd_elem<SCALED>(sg, gv[q].x, pv[q].x, s0[q].x, s1[q].x, gscale, alpha_t, gmult); p4.y = upd_elem<SCALED>(sg, gv[q].y, pv[q].y, s0[q].y, s1[q].y, gscale, alpha_t, gmult);
+        p4.z = upd_elem<SCALED>(sg, gv[q].z, pv[q].z, s0[q].z, s1[q].z, gscale, alpha_t, gmult); p4.w = upd_elem<SCALED>(sg, gv[q].w, pv[q].w, s0[q].w, s1[q].w, gscale, alpha_t, gmult);
+      } else {
+        float4& h = s2[EXT ? q : 0];
+        p4.x = upd_elem<SCALED, true>(sg, gv[q].x, pv[q].x, s0[q].x, s1[q].x, gscale, alpha_t, gmult, &h.x);
+        p4.y = upd_elem<SCALED, true>(sg, gv[q].y, pv[q].y, s0[q].y, s1[q].y, gscale, alpha_t, gmult, &h.y);
+        p4.z = upd_elem<SCALED, true>(sg, gv[q].z, pv[q].z, s0[q].z, s1[q].z, gscale, alpha_t, gmult, &h.z);
+        p4.w = upd_elem<SCALED, true>(sg, gv[q].w, pv[q].w, s0[q].w, s1[q].w, gscale, alpha_t, gmult, &h.w);
+      }
       *reinterpret_cast<float4*>(params + i) = p4;
       if (has0) *reinterpret_cast<float4*>(st0 + i) = s0[q];
       if (has1) *reinterpret_cast<float4*>(st1 + i) = s1[q];
+      if (EXT && has2) *reinterpret_cast<float4*>(st2 + i) = s2[EXT ? q : 0];
       if (sh) {
         const __nv_bfloat162 lo = __floats2bfloat162_rn(p4.x, p4.y), hi = __floats2bfloat162_rn(p4.z, p4.w);
         if (sg.off_ps < 0) *reinterpret_cast<uint2*>(shadow + sg.off_bf + (i - sg.off)) = make_uint2(*reinterpret_cast<const uint32_t*>(&lo), *reinterpret_cast<const uint32_t*>(&hi));
@@ -968,14 +1001,16 @@ __global__ void __launch_bounds__(256) updater_kernel(float* __restrict__ params
     }
   } else {
     for (int64_t i0 = base + threadIdx.x; i0 < end; i0 += 4 * blockDim.x) {
-      float gv[4], pv[4], s0[4], s1[4];
+      float gv[4], pv[4], s0[4], s1[4], s2[EXT ? 4 : 1];
 #pragma unroll
       for (int q = 0; q < 4; ++q) { const int64_t i = i0 + q * (int64_t)blockDim.x; const bool ok = i < end;
-        gv[q] = ok ? grads[i] : 0.f; pv[q] = ok ? params[i] : 0.f; s0[q] = (ok && has0) ? st0[i] : 0.f; s1[q] = (ok && has1) ? st1[i] : 0.f; }
+        gv[q] = ok ? grads[i] : 0.f; pv[q] = ok ? params[i] : 0.f; s0[q] = (ok && has0) ? st0[i] : 0.f; s1[q] = (ok && has1) ? st1[i] : 0.f;
+        if (EXT) s2[EXT ? q : 0] = (ok && has2) ? st2[i] : 0.f; }
 #pragma unroll
       for (int q = 0; q < 4; ++q) { const int64_t i = i0 + q * (int64_t)blockDim.x; if (i >= end) continue;
-        const float p = upd_elem<SCALED>(sg, gv[q], pv[q], s0[q], s1[q], gscale, alpha_t, gmult);
-        params[i] = p; if (has0) st0[i] = s0[q]; if (has1) st1[i] = s1[q];
+        const float p = EXT ? upd_elem<SCALED, true>(sg, gv[q], pv[q], s0[q], s1[q], gscale, alpha_t, gmult, &s2[EXT ? q : 0])
+                            : upd_elem<SCALED>(sg, gv[q], pv[q], s0[q], s1[q], gscale, alpha_t, gmult);
+        params[i] = p; if (has0) st0[i] = s0[q]; if (has1) st1[i] = s1[q]; if (EXT && has2) st2[i] = s2[EXT ? q : 0];
         if (sh) upd_shadow(sg, shadow, i, __float2bfloat16_rn(p));
       }
     }
@@ -988,13 +1023,16 @@ __global__ void __launch_bounds__(256) updater_kernel(float* __restrict__ params
     if (done == gridDim.x - 1) { *step = t; *ticket = 0u; __threadfence(); }
   }
 }
-void k_updater(float* params, const float* grads, float* st0, float* st1, const UpdSeg* segs, const int32_t* chunk_seg, const int64_t* chunk_off,
+void k_updater(float* params, const float* grads, float* st0, float* st1, float* st2, const UpdSeg* segs, const int32_t* chunk_seg, const int64_t* chunk_off,
                int nchunks, float inv_mb, float inv_world, int* step_dev, unsigned* ticket, __nv_bfloat16* shadow, const float* gn_mult,
-               const UpdSched* sched, const int64_t* epoch_dev, cudaStream_t s) {
+               const UpdSched* sched, const int64_t* epoch_dev, bool ext, cudaStream_t s) {
   if (!nchunks) return;
-  auto kern = gn_mult ? (sched ? updater_kernel<true, true> : updater_kernel<true, false>) : (sched ? updater_kernel<false, true> : updater_kernel<false, false>);
+  auto kern = ext ? (gn_mult ? (sched ? updater_kernel<true, true, true> : updater_kernel<true, false, true>)
+                             : (sched ? updater_kernel<false, true, true> : updater_kernel<false, false, true>))
+                  : (gn_mult ? (sched ? updater_kernel<true, true, false> : updater_kernel<true, false, false>)
+                             : (sched ? updater_kernel<false, true, false> : updater_kernel<false, false, false>));
   launch_pdl(kern, dim3(nchunks), dim3(256), (size_t)(0), s, params, grads, st0, st1, segs, chunk_seg, chunk_off, inv_mb, inv_world, step_dev, ticket, shadow, gn_mult,
-             sched, epoch_dev);
+             sched, epoch_dev, st2);
   LAUNCHED();
 }
 __global__ void sched_lr_kernel(const UpdSeg* segs, const UpdSched* sched, int seg, const int* step, const int64_t* epoch, float* out) {

@@ -19,7 +19,9 @@ from ._lib import GanConfig, LayerDesc, LrSchedule, NetConfig, check
 LAYER_TYPES = {"conv2d": 0, "deconv2d": 1, "batchnorm": 2, "dense": 3, "activation": 4, "maxpool": 5, "upsample2d": 6,
                "output": 7, "loss": 8, "ff_to_cnn": 9, "cnn_to_ff": 10, "dropout": 11}
 ACTS = {"identity": 0, "tanh": 1, "sigmoid": 2, "relu": 3, "lrelu": 4}
-UPDATERS = {"sgd": 0, "rmsprop": 1, "adam": 2, "noop": 3}
+UPDATERS = {"sgd": 0, "rmsprop": 1, "adam": 2, "noop": 3, "nesterovs": 4, "adagrad": 5, "adamax": 6, "nadam": 7, "amsgrad": 8, "adadelta": 9}
+# updaters without a learning rate: their layers take no schedule and have no getLearningRate
+NO_LR_UPDATERS = ("noop", "adadelta")
 # DL4J GradientNormalization -> b2g_gradient_normalization (DL4J's ordinals).  ClipElementWiseAbsoluteValue is the `grad_clip` argument of Net.
 GRADIENT_NORMALIZATIONS = {"none": 0, "renormalize_l2_per_layer": 1, "renormalize_l2_per_param_type": 2, "clip_l2_per_layer": 4,
                            "clip_l2_per_param_type": 5}
@@ -79,10 +81,10 @@ def schedule_struct(sched: Optional[Dict]):
 
 
 def layer_has_lr(spec: Dict) -> bool:
-    """A layer whose updater has a learning rate: it has parameters, is not frozen and its updater is not NoOp.  A spec without an updater
-    is Sgd with lr 0 (layer_desc), so it has one.  The engine applies the same rule (engine.cu layer_has_lr)."""
+    """A layer whose updater has a learning rate: it has parameters, is not frozen and its updater is neither NoOp nor AdaDelta.  A spec
+    without an updater is Sgd with lr 0 (layer_desc), so it has one.  The engine applies the same rule (engine.cu layer_has_lr)."""
     u = spec.get("updater") or {"kind": "sgd"}
-    return spec["type"] in ("conv2d", "deconv2d", "dense", "output", "batchnorm") and not spec.get("frozen", False) and u["kind"] != "noop"
+    return spec["type"] in ("conv2d", "deconv2d", "dense", "output", "batchnorm") and not spec.get("frozen", False) and u["kind"] not in NO_LR_UPDATERS
 
 
 def follow_lr_schedule(specs: List[Dict], constant: List[float], schedule: Optional[Dict], layer: Optional[str] = None):
@@ -127,6 +129,12 @@ def layer_desc(spec: Dict) -> LayerDesc:
     d.lr = constant_lr(u.get("lr", 0.0))     # new Adam(ISchedule): the schedule itself is set after b2g_net_create
     if u["kind"] == "rmsprop":          # RmsProp(learningRate, rmsDecay, epsilon)
         d.beta1, d.beta2, d.eps = u.get("rms_decay", 0.95), 0.0, u.get("eps", 1e-8)
+    elif u["kind"] == "nesterovs":      # Nesterovs(learningRate, momentum): momentum in beta1
+        d.beta1, d.beta2, d.eps = u.get("momentum", 0.9), 0.0, 0.0
+    elif u["kind"] == "adagrad":        # AdaGrad(learningRate, epsilon)
+        d.beta1, d.beta2, d.eps = 0.0, 0.0, u.get("eps", 1e-6)
+    elif u["kind"] == "adadelta":       # AdaDelta(rho, epsilon): rho in beta1, no learning rate
+        d.lr, d.beta1, d.beta2, d.eps = 0.0, u.get("rho", 0.95), 0.0, u.get("eps", 1e-6)
     else:
         d.beta1, d.beta2, d.eps = u.get("beta1", 0.9), u.get("beta2", 0.999), u.get("eps", 1e-8)
     d.l2 = spec.get("l2", 0.0)
@@ -254,8 +262,14 @@ class Net:
         check(self.lib.b2g_net_get_gradients(self.h, _fp(out), out.size))
         return out
 
+    def updater_state_size(self) -> int:
+        """Elements of the updater state: 2 x numParams ([state0 | state1]), 3 x numParams on a net with an AMSGrad layer (| state2)."""
+        n = C.c_int64()
+        check(self.lib.b2g_net_updater_state_size(self.h, C.byref(n)))
+        return n.value
+
     def updater_state(self) -> np.ndarray:
-        out = np.empty(2 * self.n_params, np.float32)
+        out = np.empty(self.updater_state_size(), np.float32)
         check(self.lib.b2g_net_get_updater_state(self.h, _fp(out), out.size))
         return out
 

@@ -20,6 +20,39 @@ def sgd(lr):
     return {"kind": "sgd", "lr": lr}
 
 
+# org.nd4j.linalg.learning.config.{Nesterovs, AdaGrad, AdaMax, Nadam, AMSGrad, AdaDelta, NoOp} with DL4J's defaults; the update each computes is
+# stated at b2g_updater in include/b200gan.h.  lr may be a schedule (below) for every kind but AdaDelta, which has no learning rate.
+def nesterovs(lr=0.1, momentum=0.9):
+    """new Nesterovs(learningRate, momentum)."""
+    return {"kind": "nesterovs", "lr": lr, "momentum": momentum}
+
+
+def adagrad(lr=0.1, eps=1e-6):
+    """new AdaGrad(learningRate, epsilon); the history starts at epsilon."""
+    return {"kind": "adagrad", "lr": lr, "eps": eps}
+
+
+def adamax(lr=1e-3, beta1=0.9, beta2=0.999, eps=1e-8):
+    return {"kind": "adamax", "lr": lr, "beta1": beta1, "beta2": beta2, "eps": eps}
+
+
+def nadam(lr=1e-3, beta1=0.9, beta2=0.999, eps=1e-8):
+    return {"kind": "nadam", "lr": lr, "beta1": beta1, "beta2": beta2, "eps": eps}
+
+
+def amsgrad(lr=1e-3, beta1=0.9, beta2=0.999, eps=1e-8):
+    return {"kind": "amsgrad", "lr": lr, "beta1": beta1, "beta2": beta2, "eps": eps}
+
+
+def adadelta(rho=0.95, eps=1e-6):
+    """new AdaDelta(rho, epsilon): no learning rate."""
+    return {"kind": "adadelta", "rho": rho, "eps": eps}
+
+
+def noop():
+    return {"kind": "noop"}
+
+
 # ------------------------------------------------------------------ learning-rate schedules ------------
 # org.nd4j.linalg.schedule.*: pass one as an updater's lr (new Adam(ISchedule): adam(lr=step_schedule(2e-4, 0.5, 1000))) or to
 # Net.set_lr_schedule.  type = ScheduleType: "iteration" (the updater's iteration count) or "epoch" (Net.set_epoch).  The arithmetic is

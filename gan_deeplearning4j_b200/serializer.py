@@ -8,7 +8,9 @@ and `updaterState.bin` = `Nd4j.write(updater state view)`.  This module writes t
                      writeUTF(dataType) | big-endian elements  (BaseDataBuffer.write of nd4j 1.0.0-beta3, allocation mode LONG_SHAPE; restated
                      from memory -- no JVM here to pin it: PARITY UNPINNED like the rest of the DL4J semantics, see DESIGN.md 1)
   updaterState.bin   the updater state, same format.  Layout = this library's [state0 | state1] (RmsProp cache / Adam m, then Adam v), each in
-                     parameter order -- NOT DL4J's per-UpdaterBlock interleaving; a DL4J reader must regroup it
+                     parameter order, and a third slot [state0 | state1 | state2] (AMSGrad's v-hat) when some layer uses AMSGrad; the slot
+                     each updater kind uses is stated at b2g_updater in include/b200gan.h -- NOT DL4J's per-UpdaterBlock interleaving; a DL4J
+                     reader must regroup it
   configuration.json this library's layer specification (the arguments of b2g_net_create), NOT DL4J's Jackson schema: a Java user rebuilds the
                      graph with the same builder calls (the driver's own code, J:118-310) and loads the arrays.  An updater's learning-rate
                      schedule is part of its spec (a MapSchedule as a list of [key, value] pairs)

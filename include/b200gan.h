@@ -84,8 +84,30 @@ typedef enum {               /* org.nd4j.linalg.activations.Activation  J:126,16
   B2G_ACT_IDENTITY = 0, B2G_ACT_TANH = 1, B2G_ACT_SIGMOID = 2, B2G_ACT_RELU = 3, B2G_ACT_LRELU = 4
 } b2g_activation;
 
-typedef enum {               /* org.nd4j.linalg.learning.config.*  J:133 (RmsProp), north_star (Adam) */
-  B2G_UPD_SGD = 0, B2G_UPD_RMSPROP = 1, B2G_UPD_ADAM = 2, B2G_UPD_NOOP = 3
+/* org.nd4j.linalg.learning.config.*  J:133 (RmsProp), north_star (Adam); the others as in DL4J 1.0.0-beta3 (recalled, parity unpinned like
+ * the rest of the DL4J semantics).  One update is  g /= mb -> [normalization] -> [clip] -> u = updater(g) -> u += l2*W -> theta -= u,  in fp32.
+ * t = iteration + 1 (b2g_net_get_iteration before the update's increment); lr = b2g_layer_desc.lr or the layer's schedule value (b2g_lr_schedule);
+ * the bias-correction factors are computed once per updater block in fp32.  Desc fields: beta1, beta2, eps as named, except where noted.
+ *   SGD (0)        u = lr*g
+ *   RMSPROP (1)    beta1 = rmsDecay.  s0 (init eps): s0 = b1*s0 + (1-b1)*g^2;  u = lr*g / (sqrt(s0) + eps)
+ *   ADAM (2)       s0 = m, s1 = v: m = b1*m + (1-b1)*g;  v = b2*v + (1-b2)*g^2;  u = alpha_t*m / (sqrt(v) + eps),  alpha_t = lr*sqrt(1-b2^t)/(1-b1^t)
+ *   NOOP (3)       u = g
+ *   NESTEROVS (4)  new Nesterovs(lr = 0.1, momentum = 0.9); beta1 = momentum.  s0 = v (init 0):  vPrev = v;  v = mu*v - lr*g;
+ *                  u = mu*vPrev - (1+mu)*v
+ *   ADAGRAD (5)    new AdaGrad(lr = 0.1, eps = 1e-6).  s0 = h (init eps):  h = h + g^2;  u = lr*g / (sqrt(h) + eps)
+ *   ADAMAX (6)     new AdaMax(lr = 1e-3, b1 = 0.9, b2 = 0.999, eps = 1e-8).  s0 = m, s1 = u_inf:  m = b1*m + (1-b1)*g;
+ *                  u_inf = max(b2*u_inf, |g|) + 1e-32 (stored back);  u = lr/(1-b1^t) * m / u_inf  (eps is not used)
+ *   NADAM (7)      new Nadam(lr = 1e-3, b1 = 0.9, b2 = 0.999, eps = 1e-8).  s0 = m, s1 = v:  m, v as Adam;
+ *                  u = lr/(1-b1^t) * (b1*m + (1-b1)*g) / (sqrt(v) + eps)  (v is not bias-corrected)
+ *   AMSGRAD (8)    new AMSGrad(lr = 1e-3, b1 = 0.9, b2 = 0.999, eps = 1e-8).  s0 = m, s1 = v, s2 = vhat:  m, v as Adam;  vhat = max(vhat, v);
+ *                  u = alpha_t*m / (sqrt(vhat) + eps), alpha_t as Adam
+ *   ADADELTA (9)   new AdaDelta(rho = 0.95, eps = 1e-6); beta1 = rho, lr is ignored (the layer has no learning rate).  s0 = msg, s1 = msdx:
+ *                  msg = rho*msg + (1-rho)*g^2;  u = sqrt(msdx + eps) / sqrt(msg + eps) * g;  msdx = rho*msdx + (1-rho)*u^2
+ * A layer with lr 0 takes a zero updater step (DL4J's fallback from alpha_t == 0 to eps is not restated).  BatchNorm mean/var always update
+ * through NOOP.  Any other value is B2G_ERR_ARG at b2g_net_create. */
+typedef enum {
+  B2G_UPD_SGD = 0, B2G_UPD_RMSPROP = 1, B2G_UPD_ADAM = 2, B2G_UPD_NOOP = 3, B2G_UPD_NESTEROVS = 4, B2G_UPD_ADAGRAD = 5, B2G_UPD_ADAMAX = 6,
+  B2G_UPD_NADAM = 7, B2G_UPD_AMSGRAD = 8, B2G_UPD_ADADELTA = 9
 } b2g_updater;
 
 typedef enum { B2G_PREC_FP32 = 0, B2G_PREC_BF16 = 1 } b2g_precision;
@@ -152,7 +174,9 @@ int32_t b2g_net_get_params(b2g_net* net, float* host, int64_t n);
 int32_t b2g_net_set_params(b2g_net* net, const float* host, int64_t n);
 /* ComputationGraph.gradient(): summed (not minibatch-divided) gradients of the last backward, DL4J order. */
 int32_t b2g_net_get_gradients(b2g_net* net, float* host, int64_t n);
-/* updater state (ModelSerializer updaterState.bin payload): [state0 | state1] each in params order. */
+/* updater state (ModelSerializer updaterState.bin payload): [state0 | state1] each in params order, plus | state2 (AMSGrad's vhat) on a net
+ * with an AMSGrad layer; b2g_net_updater_state_size gives the element count (2 or 3 x numParams).  Slots per kind: b2g_updater. */
+int32_t b2g_net_updater_state_size(b2g_net* net, int64_t* out);
 int32_t b2g_net_get_updater_state(b2g_net* net, float* host, int64_t n);
 int32_t b2g_net_set_updater_state(b2g_net* net, const float* host, int64_t n);
 /* ComputationGraph.output(x)[0] (J:170,420): inference mode (BN uses mean/var). x: [batch, in] NCHW fp32 host;
@@ -208,7 +232,8 @@ int32_t b2g_net_set_gradient_normalization(b2g_net* net, int32_t mode, float thr
  * i is the net's iteration counter before this update's increment (b2g_net_get_iteration: 0 on the first update, Adam's t - 1) for
  * type ITERATION, or the net's epoch word (b2g_net_get_epoch) for type EPOCH.  Both are read from device memory by the updater kernel, so a
  * replayed CUDA graph uses the current values.  Sgd: u = lr_i * g.  RmsProp: u = lr_i * g / (sqrt(s) + eps).  Adam:
- * alpha_t = lr_i * sqrt(1 - b2^t) / (1 - b1^t) in fp32 as without a schedule.  A schedule applies wherever the net's updater runs
+ * alpha_t = lr_i * sqrt(1 - b2^t) / (1 - b1^t) in fp32 as without a schedule; likewise lr_i replaces lr in every b2g_updater formula (AdaDelta
+ * has none and takes no schedule).  A schedule applies wherever the net's updater runs
  * (b2g_net_fit, the D and G updates of b2g_gan_step, parameter-averaging mode) and adds no kernel launch.  PolySchedule is not supported. */
 typedef enum {
   B2G_SCHED_NONE = 0, B2G_SCHED_EXPONENTIAL = 1, B2G_SCHED_INVERSE = 2, B2G_SCHED_SIGMOID = 3, B2G_SCHED_STEP = 4, B2G_SCHED_MAP = 5
@@ -225,7 +250,7 @@ typedef struct {
  * setLearningRate(String, ISchedule) (layer named).  s NULL or kind NONE: back to the layer's constant lr.  Takes effect at the next update.
  * B2G_ERR_ARG for an unknown kind or type, a non-finite parameter or map value, step <= 0 (STEP), gamma < 0 (INVERSE), a map that is empty,
  * whose keys do not strictly increase or that has no key 0, and a named layer that does not exist, is frozen or has no learning rate (no
- * parameters, or NoOp). */
+ * parameters, NoOp or AdaDelta). */
 int32_t b2g_net_set_lr_schedule(b2g_net* net, const char* layer, const b2g_lr_schedule* s);
 /* ComputationGraph.getLearningRate(String): the fp32 learning rate the layer's next update will use (before Adam's bias correction), computed
  * on the device by the function the updater kernel calls.  Sync point. */

@@ -24,6 +24,7 @@ public final class Native {
     public static native int netGetParam(long net, long layerNameAddr, long paramNameAddr, long hostAddr, long n);
     public static native int netGetParams(long net, long hostAddr, long n);
     public static native int netSetParams(long net, long hostAddr, long n);
+    public static native int netUpdaterStateSize(long net, long outAddr);
     public static native int netGetUpdaterState(long net, long hostAddr, long n);
     public static native int netSetUpdaterState(long net, long hostAddr, long n);
     public static native int netGetIteration(long net, long outAddr);

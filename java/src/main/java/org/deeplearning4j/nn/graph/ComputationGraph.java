@@ -31,10 +31,10 @@ public class ComputationGraph {
         for (Layer l : layers)            // new Adam(ISchedule) / RmsProp(ISchedule) / Sgd(ISchedule): evaluated on the device at every update
             if (l.updater != null && l.updater.lrSchedule() != null && hasLearningRate(l)) setLearningRate(l.name, l.updater.lrSchedule());
     }
-    /** The library's rule (include/b200gan.h, b2g_net_set_lr_schedule): parameters, not frozen, updater not NoOp. */
+    /** The library's rule (include/b200gan.h, b2g_net_set_lr_schedule): parameters, not frozen, updater neither NoOp nor AdaDelta. */
     private static boolean hasLearningRate(Layer l) {
         boolean params = l.type == 0 || l.type == 1 || l.type == 2 || l.type == 3 || l.type == 7;    // conv, deconv, BatchNorm, dense, output
-        return params && l.frozen == 0 && l.updater.kind() != 3;
+        return params && l.frozen == 0 && l.updater.kind() != 3 && l.updater.kind() != 9;
     }
 
     /** setLearningRate(ISchedule): every layer whose updater has a learning rate, from the next update on (null: back to the constant lr). */
@@ -85,8 +85,10 @@ public class ComputationGraph {
         Native.check(Native.netFit(net, Native.address(Native.floats(ds.getFeatures().data)), Native.address(Native.floats(ds.getLabels().data)), batch, Native.address(score)));
     }
     public INDArray params() { int n = (int) numParams(); FloatBuffer b = Native.direct(4 * n).asFloatBuffer(); Native.check(Native.netGetParams(net, Native.address(b), n)); float[] d = new float[n]; b.get(d); return new INDArray(d, 1, n); }
-    /** Updater state in the library's [state0 | state1] order (RmsProp cache / Adam m, then Adam v), 2 x numParams values. */
-    public INDArray updaterState() { int n = 2 * (int) numParams(); FloatBuffer b = Native.direct(4 * n).asFloatBuffer(); Native.check(Native.netGetUpdaterState(net, Native.address(b), n)); float[] d = new float[n]; b.get(d); return new INDArray(d, 1, n); }
+    /** Updater state in the library's [state0 | state1] order (RmsProp cache / Adam m, then Adam v), 2 x numParams values, plus | state2
+     *  (AMSGrad's v-hat) on a graph with an AMSGrad layer; the slots of every updater kind are stated at b2g_updater in include/b200gan.h. */
+    public long updaterStateSize() { ByteBuffer o = Native.direct(8); Native.check(Native.netUpdaterStateSize(net, Native.address(o))); return o.getLong(0); }
+    public INDArray updaterState() { int n = (int) updaterStateSize(); FloatBuffer b = Native.direct(4 * n).asFloatBuffer(); Native.check(Native.netGetUpdaterState(net, Native.address(b), n)); float[] d = new float[n]; b.get(d); return new INDArray(d, 1, n); }
     /** The layer list as JSON (this library's specification, not DL4J's Jackson schema) -- ModelSerializer's configuration.json entry. */
     public void setUpdaterState(INDArray st) { Native.check(Native.netSetUpdaterState(net, Native.address(Native.floats(st.data)), st.length())); }
     /** BaseMultiLayerUpdater's iteration count (Adam's t - 1); part of a checkpoint and of the state a Spark worker starts from. */

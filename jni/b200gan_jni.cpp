@@ -38,6 +38,7 @@ FN(netGetParam)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong paramNam
 }
 FN(netGetParams)(JNIEnv_*, jclass, jlong net, jlong hostAddr, jlong n) { return b2g_net_get_params(P(b2g_net*, net), P(float*, hostAddr), n); }
 FN(netSetParams)(JNIEnv_*, jclass, jlong net, jlong hostAddr, jlong n) { return b2g_net_set_params(P(b2g_net*, net), P(const float*, hostAddr), n); }
+FN(netUpdaterStateSize)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_updater_state_size(P(b2g_net*, net), P(int64_t*, outAddr)); }
 FN(netGetUpdaterState)(JNIEnv_*, jclass, jlong net, jlong hostAddr, jlong n) { return b2g_net_get_updater_state(P(b2g_net*, net), P(float*, hostAddr), n); }
 FN(netSetUpdaterState)(JNIEnv_*, jclass, jlong net, jlong hostAddr, jlong n) { return b2g_net_set_updater_state(P(b2g_net*, net), P(const float*, hostAddr), n); }
 FN(netGetIteration)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_get_iteration(P(b2g_net*, net), P(int64_t*, outAddr)); }
