@@ -69,7 +69,7 @@ class TestEwOpts(C.Structure):
                 ("alpha", C.c_float), ("clip_eps", C.c_float), ("offset", C.c_int32), ("in_place", C.c_int32), ("accumulate", C.c_int32),
                 ("poison", C.c_int32), ("n_jobs", C.c_int32), ("jobs", C.POINTER(EwReduceJob)), ("n_seg", C.c_int32),
                 ("seg_off", C.POINTER(C.c_int64)), ("seg_len", C.POINTER(C.c_int64)), ("seg_coef", C.POINTER(C.c_float)), ("sumsq", C.c_double),
-                ("kernel", C.c_char * 64)]
+                ("kernel", C.c_char * 64), ("loss", C.c_int32)]
 
 
 _vp, _i32, _i64, _fp = C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_float)

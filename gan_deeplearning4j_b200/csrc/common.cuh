@@ -43,6 +43,18 @@ __device__ __forceinline__ double sacc_read(const unsigned long long* hi_lo, siz
   return (double)(long long)hi_lo[idx] * (1.0 / 1024.0) + (double)(long long)hi_lo[stride + idx] * (1.0 / 1152921504606846976.0);
 }
 
+// Sum over the block in a fixed order: each thread's running sum, a xor butterfly inside the warp, the warp sums added in warp order by
+// thread 0.  Only thread 0's result is used.
+__device__ __forceinline__ double block_sum(double v, double* red) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double t = 0.0;
+  if (threadIdx.x == 0) for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w];
+  return t;
+}
+
 // Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC'11; the Random123 constants): a counter-based generator,
 // so a mask element's random word is a pure function of (counter, key) and needs no state beyond the counter the caller forms.
 struct Philox4 { uint32_t x[4]; };

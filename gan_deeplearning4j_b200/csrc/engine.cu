@@ -87,7 +87,8 @@ struct LayerRT {
   int64_t off_Wps_bf = -1;                                     // packed [16][9][O] weights of the tensor-core pixel-shuffle transposed conv (<= 4 image channels)
   int wA = 0, wTaps = 0, wB = 0;                               // internal weight layout [A][taps][B]
   void* out = nullptr; bool out_alias = false;
-  void* probs = nullptr;                                       // OUTPUT / LOSS: sigmoid(logits)
+  void* probs = nullptr;                                       // OUTPUT / LOSS: the output activation of the logits (sigmoid, softmax or loss_act)
+  int loss_act = ACT_IDENTITY; float loss_alpha = 0.f;         // OUTPUT / LOSS with loss codes 2-8: the activation the loss applies to z
   uint8_t* argmax = nullptr;
   float* bn_mean = nullptr; float* bn_invstd = nullptr; float* bn_fold = nullptr;   // bn_fold: [scale | shift] for the inference-mode epilogue fold
   float* bn_coef = nullptr;                                    // fused path: [groups][4][C] = scale, beta, mean, invstd of the latest train-mode forward
@@ -148,6 +149,7 @@ struct b2g_net {
   uint64_t simt_gemm_calls = 0;                                    // BF16 nets: GEMM-shaped ops that ran on the SIMT kernels (skinny / unsupported shapes) -- reported, never silent
   float* scratch = nullptr; size_t scratch_floats = 0;
   float* loss_dev = nullptr;           // [8]
+  double* loss_partial = nullptr; unsigned* loss_ticket = nullptr;   // k_loss's per-block sums and its ticket
   double* l2_dev = nullptr;
   void* input_grad = nullptr;          // where the last backward left d(loss)/d(input), or null
   int last_rows = 0;
@@ -185,6 +187,18 @@ static void w_internal_to_dl4j(const float* src, float* dst, int A, int B, int t
 }
 
 // ------------------------------------------------------------------ net construction --------------------
+// OUTPUT / LOSS layers: checks the loss code and keeps the activation a loss of codes 2-8 applies (b2g_loss); an OUTPUT layer's GEMM then runs
+// without an activation, as for XENT and MCXENT, whose activations are implied.
+static int32_t take_loss(LayerRT& l) {
+  b2g_layer_desc& d = l.d;
+  if (d.loss < B2G_LOSS_XENT || d.loss > B2G_LOSS_WASSERSTEIN) return fail(B2G_ERR_ARG, "layer %s: unknown loss %d", d.name, d.loss);
+  if (d.loss >= B2G_LOSS_MSE) {
+    if (d.act < B2G_ACT_IDENTITY || d.act > B2G_ACT_LRELU) return fail(B2G_ERR_ARG, "layer %s: unknown activation %d", d.name, d.act);
+    l.loss_act = d.act; l.loss_alpha = d.act_alpha;
+  }
+  if (d.type == B2G_LAYER_OUTPUT) d.act = B2G_ACT_IDENTITY;
+  return 0;
+}
 static int32_t net_build(b2g_net* n, const b2g_layer_desc* layers, int32_t nl) {
   const b2g_net_config& c = n->cfg;
   int h = c.in_h, w = c.in_w, ch = c.in_c;
@@ -229,7 +243,10 @@ static int32_t net_build(b2g_net* n, const b2g_layer_desc* layers, int32_t nl) {
         l.wA = d.n_out; l.wTaps = 1; l.wB = d.n_in;                        // 'f'-order [nIn,nOut] == row-major [nOut][nIn]
         l.off_W = off; l.n_W = (int64_t)d.n_in * d.n_out; off += l.n_W;    // DefaultParamInitializer: [W | b]
         if (d.has_bias) { l.off_b = off; off += d.n_out; }
-        if (d.type == B2G_LAYER_OUTPUT) { d.act = B2G_ACT_IDENTITY; if (d.loss == B2G_LOSS_XENT && d.n_out != 1) return fail(B2G_ERR_UNSUPPORTED, "layer %s: XENT output supports nOut=1 (use MCXENT for nOut>1)", d.name); }
+        if (d.type == B2G_LAYER_OUTPUT) {
+          B2(take_loss(l));      // the GEMM's epilogue stays identity: the loss applies the activation
+          if (d.loss == B2G_LOSS_XENT && d.n_out != 1) return fail(B2G_ERR_UNSUPPORTED, "layer %s: XENT output supports nOut=1 (use MCXENT for nOut>1)", d.name);
+        }
       } break;
       case B2G_LAYER_BATCHNORM: {
         d.n_in = d.n_out = ch; l.oh = h; l.ow = w; l.oc = ch;
@@ -243,7 +260,12 @@ static int32_t net_build(b2g_net* n, const b2g_layer_desc* layers, int32_t nl) {
         if (d.k_h * d.k_w > 255) return fail(B2G_ERR_UNSUPPORTED, "layer %s: pooling window too large", d.name);
         break;
       case B2G_LAYER_UPSAMPLE2D: if (d.k_h < 1) d.k_h = 2; l.oh = h * d.k_h; l.ow = w * d.k_h; l.oc = ch; break;
-      case B2G_LAYER_LOSS: l.oh = h; l.ow = w; l.oc = ch; if ((size_t)h * w * ch != 1) return fail(B2G_ERR_UNSUPPORTED, "layer %s: XENT loss needs one logit per example", d.name); break;
+      case B2G_LAYER_LOSS:
+        l.oh = h; l.ow = w; l.oc = ch; B2(take_loss(l));
+        if (d.loss == B2G_LOSS_MCXENT) return fail(B2G_ERR_UNSUPPORTED, "layer %s: MCXENT is supported on OutputLayer only", d.name);
+        if (d.loss == B2G_LOSS_XENT && (size_t)h * w * ch != 1) return fail(B2G_ERR_UNSUPPORTED, "layer %s: XENT loss needs one logit per example", d.name);
+        if ((h != 1 || w != 1) && (size_t)h * w * ch != 1) return fail(B2G_ERR_UNSUPPORTED, "layer %s: a loss on a %dx%d map is not supported (feed-forward input or one element per example)", d.name, h, w);
+        break;
       case B2G_LAYER_FF_TO_CNN:
         if ((size_t)d.pre_h * d.pre_w * d.pre_c != l.in_elems) return fail(B2G_ERR_SHAPE, "layer %s: FeedForwardToCnn(%d,%d,%d) != %zu features", d.name, d.pre_h, d.pre_w, d.pre_c, l.in_elems);
         l.oh = d.pre_h; l.ow = d.pre_w; l.oc = d.pre_c; break;
@@ -285,6 +307,11 @@ static int32_t net_alloc(b2g_net* n) {
   B2(dalloc(n, &n->drop_ticket, sizeof(unsigned))); CU(cudaMemsetAsync(n->drop_ticket, 0, sizeof(unsigned), n->ctx->stream));
   B2(dalloc(n, &n->step_dev, sizeof(int))); B2(dalloc(n, &n->loss_dev, sizeof(float) * 8)); B2(dalloc(n, &n->l2_dev, sizeof(double)));
   B2(dalloc(n, &n->labels_dev, sizeof(float) * R * std::max<size_t>(1, n->L.back().out_elems)));
+  {  // k_loss's per-block sums for one group of max_batch rows (fit) or two of max_batch / 2 (the GAN step's D pass)
+    const size_t per = n->L.back().out_elems;
+    B2(dalloc(n, &n->loss_partial, sizeof(double) * std::max(k_loss_blocks((size_t)R * per, 1), 2 * k_loss_blocks((size_t)(R / 2) * per, 2))));
+  }
+  B2(dalloc(n, &n->loss_ticket, sizeof(unsigned))); CU(cudaMemsetAsync(n->loss_ticket, 0, sizeof(unsigned), n->ctx->stream));
   B2(dalloc(n, (char**)&n->input, ts * R * n->in_elems));
   size_t max_act = n->in_elems, scratch = 1 << 16, max_w = 0, bn_acc_words = 0;
   for (auto& l : n->L) {
@@ -962,6 +989,9 @@ extern "C" int32_t b2g_net_output(b2g_net* n, const float* x, int32_t batch, int
   B2(net_forward(n, n->input, o, &res));
   LayerRT& l = n->L.back();
   if (l.d.type == B2G_LAYER_OUTPUT && l.d.loss == B2G_LOSS_MCXENT) { k_softmax_xent(n->prec, res, nullptr, nullptr, l.probs, nullptr, batch, l.oc, n->ctx->stream); res = l.probs; }
+  else if ((l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS) && l.d.loss >= B2G_LOSS_MSE) {      // a = act(z); identity: the logits themselves
+    if (l.loss_act != ACT_IDENTITY) { k_act_fwd(n->prec, res, l.probs, (size_t)batch * l.out_elems, l.loss_act, l.loss_alpha, n->ctx->stream); res = l.probs; }
+  }
   else if (l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS) { k_sigmoid_out(n->prec, res, l.probs, (size_t)batch * l.out_elems, n->ctx->stream); res = l.probs; }
   return download_act(n, res, batch, l.oc, l.oh * l.ow, out);
 }
@@ -971,16 +1001,21 @@ extern "C" int32_t b2g_net_get_activation(b2g_net* n, int32_t layer, int32_t bat
   return download_act(n, l.out, batch, l.oc, l.oh * l.ow, host);
 }
 
+// The loss of the net's last layer (b2g_loss) on its logits, one launch: dz = dL/dz, loss_sums[g] = the summed scores of group g's rows.  The only
+// place that dispatches on the loss: fit, computeGradientAndScore and both losses of the GAN step come here.  A net that does not end in an
+// OUTPUT or LOSS layer runs XENT.
 static void net_loss(b2g_net* n, const void* logits, const float* labels, void* dz, float* loss_sums, int rows_per_group, int groups) {
   const LayerRT& l = n->L.back();
-  if (l.d.type == B2G_LAYER_OUTPUT && l.d.loss == B2G_LOSS_MCXENT) k_softmax_xent(n->prec, logits, labels, dz, nullptr, loss_sums, rows_per_group * groups, l.oc, n->ctx->stream);
-  else k_xent(n->prec, logits, labels, dz, loss_sums, rows_per_group, groups, n->cfg.xent_clip_eps, n->ctx->stream);
+  const int loss = (l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS) ? l.d.loss : B2G_LOSS_XENT;
+  if (loss == B2G_LOSS_MCXENT) k_softmax_xent(n->prec, logits, labels, dz, nullptr, loss_sums, rows_per_group * groups, l.oc, n->ctx->stream);
+  else if (loss == B2G_LOSS_XENT) k_xent(n->prec, logits, labels, dz, loss_sums, rows_per_group, groups, n->cfg.xent_clip_eps, n->ctx->stream);
+  else k_loss(n->prec, loss, l.loss_act, l.loss_alpha, logits, labels, dz, loss_sums, rows_per_group, (int)l.out_elems, groups, n->loss_partial, n->loss_ticket, n->ctx->stream);
 }
 static int32_t train_pass(b2g_net* n, const float* x, const float* y, int batch, bool do_update, float* score) {
   cudaStream_t s = n->ctx->stream;
   if (batch < 1 || batch > n->max_rows) return fail(B2G_ERR_SHAPE, "batch %d outside [1,%d]", batch, n->max_rows);
   int lt = n->L.back().d.type;
-  if (lt != B2G_LAYER_OUTPUT && lt != B2G_LAYER_LOSS) return fail(B2G_ERR_UNSUPPORTED, "fit needs a net ending in OutputLayer/LossLayer (XENT)");
+  if (lt != B2G_LAYER_OUTPUT && lt != B2G_LAYER_LOSS) return fail(B2G_ERR_UNSUPPORTED, "fit needs a net ending in OutputLayer/LossLayer");
   B2(upload_input(n, x, batch, n->input));
   CU(cudaMemcpyAsync(n->labels_dev, y, sizeof(float) * batch * n->L.back().out_elems, cudaMemcpyHostToDevice, s));
   CU(cudaMemsetAsync(n->grads, 0, sizeof(float) * n->n_params, s));
@@ -1057,7 +1092,7 @@ static int32_t gan_step_part2(b2g_gan* g, int N) {
   CU(cudaMemsetAsync(D->grads, 0, sizeof(float) * D->n_params, s));
   const void* logits = nullptr; FwdOpts od{2 * N, 2, true, true, nullptr};
   B2(net_forward(D, D->input, od, &logits));
-  k_xent(D->prec, logits, g->y_d, D->epsA, g->loss_dev, N, 2, D->cfg.xent_clip_eps, s);
+  net_loss(D, logits, g->y_d, D->epsA, g->loss_dev, N, 2);
   B2(net_backward(D, D->input, D->epsA, 2 * N, 2, true, false, /*allreduce_follows=*/true));
   if (under_allreduce) B2(hoisted_g_forward());
   B2(net_allreduce_grads(D));
@@ -1066,7 +1101,7 @@ static int32_t gan_step_part2(b2g_gan* g, int N) {
   CU(cudaStreamWaitEvent(s, G->ctx->ev_b, 0));
   FwdOpts od2{N, 1, true, false, nullptr};
   B2(net_forward(D, xg, od2, &logits));
-  k_xent(D->prec, logits, g->y_g, D->epsA, g->loss_dev + 2, N, 1, D->cfg.xent_clip_eps, s);
+  net_loss(D, logits, g->y_g, D->epsA, g->loss_dev + 2, N, 1);
   // the generator's output activation (tanh) is differentiated inside D's last input-gradient kernel when that kernel can (EPI_ACTBWD)
   TcEpi ga{}; const LayerRT& gl = G->L.back(); bool ga_done = false;
   const bool ga_can = gl.has_gemm() && gl.d.act != B2G_ACT_IDENTITY && gl.d.type != B2G_LAYER_OUTPUT;
@@ -1084,7 +1119,12 @@ extern "C" int32_t b2g_gan_create(b2g_net* gen, b2g_net* dis, const b2g_gan_conf
   if (gen->prec != dis->prec) return fail(B2G_ERR_ARG, "generator and discriminator use different precisions");
   if (gen->L.back().out_elems != dis->in_elems) return fail(B2G_ERR_SHAPE, "generator output (%zu) != discriminator input (%zu)", gen->L.back().out_elems, dis->in_elems);
   if (gen->L.back().out_alias || gen->L.back().d.type == B2G_LAYER_DROPOUT) return fail(B2G_ERR_UNSUPPORTED, "generator must end in a layer that owns its output");
-  if (dis->L.back().d.type == B2G_LAYER_OUTPUT && dis->L.back().d.loss != B2G_LOSS_XENT) return fail(B2G_ERR_UNSUPPORTED, "the adversarial step needs a binary XENT discriminator");
+  {  // one output per example; XENT or a loss of codes 2-8 (the labels the caller uploads choose the objective)
+    const LayerRT& dl = dis->L.back();
+    const bool lossy = dl.d.type == B2G_LAYER_OUTPUT || dl.d.type == B2G_LAYER_LOSS;
+    if (lossy && dl.d.loss == B2G_LOSS_MCXENT) return fail(B2G_ERR_UNSUPPORTED, "the adversarial step needs a discriminator with one output per example (not MCXENT)");
+    if (lossy && dl.out_elems != 1) return fail(B2G_ERR_UNSUPPORTED, "the adversarial step needs a discriminator with one output per example, not %zu", dl.out_elems);
+  }
   if (dis->cfg.bn_groups < 2 || dis->max_rows < 2) return fail(B2G_ERR_ARG, "discriminator must be created with bn_groups>=2 and max_batch = 2*N");
   int N = std::min(gen->max_rows, dis->max_rows / 2);
   CU(cudaSetDevice(gen->ctx->device));
@@ -1712,6 +1752,18 @@ extern "C" int32_t b2g_test_ew(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* 
       B2(poison(dz, ts * n)); B2(poison(p, ts * n)); B2(poison(loss, 4));
       k_softmax_xent(prec, z, y, y ? dz : nullptr, p, y ? loss : nullptr, o->rows, o->cols, s); ran();       // no labels: the inference call
       B2(downT(out0, dz, n)); B2(downF(out1, loss, 1)); B2(downT(out2, p, n));
+      break;
+    }
+    case B2G_EW_LOSS: {
+      const size_t per = (size_t)o->rows * o->cols, n = per * o->groups;
+      if (!in0 || !in1 || o->rows < 1 || o->cols < 1 || o->groups < 1 || (int64_t)n > lim || o->loss < B2G_LOSS_MSE || o->loss > B2G_LOSS_WASSERSTEIN ||
+          o->act < B2G_ACT_IDENTITY || o->act > B2G_ACT_LRELU) return fail(B2G_ERR_ARG, "bad LOSS arguments");
+      void *z = nullptr, *dz = nullptr; float *y = nullptr, *loss = nullptr; double* partial = nullptr; unsigned* ticket = nullptr;
+      B2(upT(in0, n, &z)); B2(upF(in1, n, &y)); B2(dev(n, ts, &dz)); B2(upF(nullptr, (size_t)o->groups, &loss));
+      B2(dev((size_t)o->groups * k_loss_blocks(per, o->groups), 8, (void**)&partial)); B2(dev(1, 4, (void**)&ticket)); CU(cudaMemsetAsync(ticket, 0, 4, s));
+      B2(poison(dz, ts * n)); B2(poison(loss, 4 * (size_t)o->groups));
+      k_loss(prec, o->loss, o->act, o->alpha, z, y, dz, loss, o->rows, o->cols, o->groups, partial, ticket, s); ran();
+      B2(downT(out0, dz, n)); B2(downF(out1, loss, (size_t)o->groups));
       break;
     }
     case B2G_EW_ACT_FWD: case B2G_EW_ACT_BWD: {

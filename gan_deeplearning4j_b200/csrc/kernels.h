@@ -11,6 +11,7 @@ namespace b2g {
 
 enum Prec { PREC_F32 = 0, PREC_BF16 = 1 };
 enum Act { ACT_IDENTITY = 0, ACT_TANH = 1, ACT_SIGMOID = 2, ACT_RELU = 3, ACT_LRELU = 4 };
+enum Loss { LOSS_MSE = 2, LOSS_L1 = 3, LOSS_L2 = 4, LOSS_MAE = 5, LOSS_HINGE = 6, LOSS_SQUARED_HINGE = 7, LOSS_WASSERSTEIN = 8 };   // b2g_loss
 
 inline size_t prec_size(int prec) { return prec == PREC_F32 ? 4 : 2; }
 
@@ -100,6 +101,12 @@ void k_xent(int prec, const void* z, const float* y, void* dz, float* loss_sums,
 void k_sigmoid_out(int prec, const void* z, void* p, size_t n, cudaStream_t s);
 // LossMCXENT + softmax over K classes: dz = softmax(z) - y, loss_sums[0] = -sum y log clip(p, 1e-10); p_out optional (probabilities)
 void k_softmax_xent(int prec, const void* z, const float* y, void* dz, void* p_out, float* loss_sums, int rows, int K, cudaStream_t s);
+// LossMSE / L1 / L2 / MAE / Hinge / SquaredHinge / Wasserstein (b2g_loss 2-8) on a = act(z), z and y [groups][rows][n_out]: dz = dL/da * act'(a)
+// (sum form, not /mb), loss_sums[g] = the group's summed per-example scores.  One launch; the sums are bit-reproducible: partial
+// [groups * k_loss_blocks(rows * n_out, groups)] doubles and a ticket word (0 between launches) hold the per-block sums the last block folds.
+int k_loss_blocks(size_t n_per_group, int groups);
+void k_loss(int prec, int loss, int act, float alpha, const void* z, const float* y, void* dz, float* loss_sums, int rows_per_group, int n_out, int groups,
+            double* partial, unsigned* ticket, cudaStream_t s);
 
 // ---- reductions ------------------------------------------------------------------------------------
 // out[c] (+)= sum_rows x[row][c]

@@ -721,6 +721,72 @@ void k_softmax_xent(int prec, const void* z, const float* y, void* dz, void* p_o
   g_ew_last_kernel = "softmax_xent_kernel";
 }
 
+// ---------------------------------------------------------------- regression / margin losses ----------------
+// LossMSE, LossL1, LossL2, LossMAE, LossHinge, LossSquaredHinge and LossWasserstein as ILossFunction.computeGradient(labels, preOutput,
+// activationFn): a = act(z) in fp32, dz = dL/da * act'(a) with the derivative taken from a; formulas at b2g_loss (include/b200gan.h).
+// Group g's rows * n_out elements are split into k_loss_blocks() slices fixed by the shape, one block each (at most LOSS_MAX_GRID blocks in
+// all: one wave, so the kernel lets its successor in at once).  A block sums its elements' scores in double (its block_sum order is fixed) and
+// writes the sum to partial[]; the last block to finish folds each group's partials, one warp per group, each lane a strided subset in slice
+// order and then the warp's xor butterfly: the loss sums do not depend on the order the blocks ran in.
+constexpr int LOSS_THREADS = 256, LOSS_ELEMS_PER_BLOCK = 1024, LOSS_MAX_GRID = 1024;
+int k_loss_blocks(size_t n_per_group, int groups) {
+  const size_t b = (n_per_group + LOSS_ELEMS_PER_BLOCK - 1) / LOSS_ELEMS_PER_BLOCK;
+  return (int)std::min<size_t>(std::max<size_t>(b, 1), std::max(1, LOSS_MAX_GRID / groups));
+}
+template <typename T>
+__global__ void __launch_bounds__(LOSS_THREADS) loss_kernel(const T* __restrict__ z, const float* __restrict__ y, T* __restrict__ dz, float* __restrict__ loss_sums,
+                                                           size_t n_per_group, int n_out, int bpg, int loss, int act, float alpha, double* partial, unsigned* ticket) {
+  pdl_enter();
+  __shared__ double red[LOSS_THREADS / 32];
+  __shared__ int last;
+  const int g = blockIdx.x / bpg, b = blockIdx.x % bpg;
+  const float nf = (float)n_out;
+  double acc = 0.0;
+  for (size_t j = (size_t)b * LOSS_THREADS + threadIdx.x; j < n_per_group; j += (size_t)bpg * LOSS_THREADS) {
+    const size_t i = (size_t)g * n_per_group + j;
+    const float a = act_fwd(act, ldf(z, i), alpha), yi = y[i];
+    const double e = (double)a - (double)yi, m = 1.0 - (double)yi * (double)a;    // error a - y; hinge margin 1 - y a
+    double l; float ga;                                                              // this element's score (before / nOut) and dL/da
+    switch (loss) {
+      case LOSS_MSE: l = e * e; ga = 2.0f * (a - yi) / nf; break;
+      case LOSS_L2: l = e * e; ga = 2.0f * (a - yi); break;
+      case LOSS_L1: l = fabs(e); ga = (float)((a > yi) - (a < yi)); break;
+      case LOSS_MAE: l = fabs(e); ga = (float)((a > yi) - (a < yi)) / nf; break;
+      case LOSS_HINGE: l = fmax(m, 0.0); ga = m > 0.0 ? -yi : 0.f; break;
+      case LOSS_SQUARED_HINGE: l = m > 0.0 ? m * m : 0.0; ga = m > 0.0 ? -2.0f * yi * (float)m : 0.f; break;
+      default: l = (double)yi * (double)a; ga = yi / nf; break;                   // LOSS_WASSERSTEIN
+    }
+    acc += l;
+    stf(dz, i, ga * act_grad_from_out(act, a, alpha));
+  }
+  const double tot = block_sum(acc, red);
+  if (threadIdx.x == 0) {
+    partial[blockIdx.x] = tot;
+    __threadfence();
+    last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();      // every partial is visible: each writer fenced before taking its ticket
+  const bool per_out = loss == LOSS_MSE || loss == LOSS_MAE || loss == LOSS_WASSERSTEIN;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int gg = warp; gg < (int)(gridDim.x / bpg); gg += LOSS_THREADS / 32) {
+    double s = 0.0;
+    for (int k = lane; k < bpg; k += 32) s += __ldcg(partial + (size_t)gg * bpg + k);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) loss_sums[gg] = (float)(per_out ? s / n_out : s);
+  }
+  if (threadIdx.x == 0) { *ticket = 0u; __threadfence(); }
+}
+void k_loss(int prec, int loss, int act, float alpha, const void* z, const float* y, void* dz, float* loss_sums, int rows_per_group, int n_out, int groups,
+            double* partial, unsigned* ticket, cudaStream_t s) {
+  const size_t n = (size_t)rows_per_group * n_out; const int bpg = k_loss_blocks(n, groups);
+  DISPATCH_PREC(prec, T, (launch_pdl(loss_kernel<T>, dim3(groups * bpg), dim3(LOSS_THREADS), (size_t)0, s, (const T*)z, y, (T*)dz, loss_sums, n, n_out, bpg,
+                                     loss, act, alpha, partial, ticket))); LAUNCHED();
+  g_ew_last_kernel = "loss_kernel";
+}
+
 // ---------------------------------------------------------------- column sum / misc reductions -----------
 template <typename T>
 __global__ void colsum_partial_kernel(const T* __restrict__ x, int rows, int C, int S, float* __restrict__ p) { pdl_enter();

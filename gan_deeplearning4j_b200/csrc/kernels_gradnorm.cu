@@ -12,18 +12,6 @@ namespace b2g {
 
 __device__ __forceinline__ double sq(float g, float gscale) { const double v = (double)(g * gscale); return v * v; }
 
-// Sum over the block in a fixed order: each thread's running sum, a xor butterfly inside the warp, the 8 warp sums added in warp order by
-// thread 0.  Only thread 0's result is used.
-__device__ __forceinline__ double block_sum(double v, double* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double t = 0.0;
-  if (threadIdx.x == 0) for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += red[w];
-  return t;
-}
-
 __global__ void __launch_bounds__(256) gradnorm_kernel(const float* __restrict__ grads, const UpdSeg* __restrict__ segs, const int32_t* __restrict__ chunk_seg,
                                                        const int64_t* __restrict__ chunk_off, const GnGroup* __restrict__ groups, int ngroups, int clip,
                                                        float threshold, float inv_mb, float inv_world, double* partial, unsigned* ticket, float* __restrict__ mult) {

@@ -19,6 +19,8 @@ from ._lib import GanConfig, LayerDesc, LrSchedule, NetConfig, check
 LAYER_TYPES = {"conv2d": 0, "deconv2d": 1, "batchnorm": 2, "dense": 3, "activation": 4, "maxpool": 5, "upsample2d": 6,
                "output": 7, "loss": 8, "ff_to_cnn": 9, "cnn_to_ff": 10, "dropout": 11}
 ACTS = {"identity": 0, "tanh": 1, "sigmoid": 2, "relu": 3, "lrelu": 4}
+# LossFunctions.LossFunction -> b2g_loss.  XENT / MCXENT imply their sigmoid / softmax; the others apply the spec's "activation" (b2g_loss)
+LOSSES = {"xent": 0, "mcxent": 1, "mse": 2, "l1": 3, "l2": 4, "mae": 5, "hinge": 6, "squared_hinge": 7, "wasserstein": 8}
 UPDATERS = {"sgd": 0, "rmsprop": 1, "adam": 2, "noop": 3, "nesterovs": 4, "adagrad": 5, "adamax": 6, "nadam": 7, "amsgrad": 8, "adadelta": 9}
 # updaters without a learning rate: their layers take no schedule and have no getLearningRate
 NO_LR_UPDATERS = ("noop", "adadelta")
@@ -141,7 +143,7 @@ def layer_desc(spec: Dict) -> LayerDesc:
     d.bn_decay, d.bn_eps = spec.get("decay", 0.9), spec.get("eps", 1e-5)
     to = spec.get("to", (0, 0, 0))      # FeedForwardToCnnPreProcessor(h, w, c)
     d.pre_h, d.pre_w, d.pre_c = to
-    d.loss = {"xent": 0, "mcxent": 1}[spec.get("loss", "xent")]
+    d.loss = LOSSES[spec.get("loss", "xent")]
     d.frozen = 1 if spec.get("frozen", False) else 0
     return d
 
@@ -543,17 +545,18 @@ def test_dropout(ctx: Context, precision: int, x, dy, p: float, *, seed: int = 6
 
 
 EW_OPS = {"reduce_splits": 0, "reduce_multi": 1, "colsum": 2, "xent": 3, "softmax_xent": 4, "act_fwd": 5, "act_bwd": 6, "maxpool": 7,
-          "upsample": 8, "sumsq": 9}
+          "upsample": 8, "sumsq": 9, "loss": 10}
 
 
-def test_ew(ctx: Context, precision: int, op: str, in0, in1=None, out_sizes=(0, 0, 0), *, act: str = "identity", jobs=None, segments=None, **opts):
+def test_ew(ctx: Context, precision: int, op: str, in0, in1=None, out_sizes=(0, 0, 0), *, act: str = "identity", jobs=None, segments=None,
+            loss: str = "xent", **opts):
     """One reduction / loss / element-wise kernel through its production wrapper (b2g_test_ew; operands per op in include/b200gan.h).
     out_sizes: element counts of out0..out2 (0: not asked for).  opts: the b2g_test_ew_opts sizes and switches (n, rows, cols, groups, splits,
     stride, N, H, W, C, KH, KW, SH, SW, alpha, clip_eps, offset, in_place, accumulate, poison).  jobs (reduce_multi): dicts of n, splits,
-    stride, src_off, dst_off.  segments (sumsq): (offsets, lengths, coefficients).
+    stride, src_off, dst_off.  segments (sumsq): (offsets, lengths, coefficients).  loss (op "loss"): a LOSSES name of codes 2-8.
     Returns ([out0, out1, out2] with None where not asked for, {"kernel": names, "sumsq": float, "wide": [per job]})."""
     o = _lib.TestEwOpts()
-    o.op, o.act = EW_OPS[op], ACTS[act]
+    o.op, o.act, o.loss = EW_OPS[op], ACTS[act], LOSSES[loss]
     for k, v in opts.items():
         setattr(o, k, int(v) if isinstance(v, bool) else v)
     keep = []

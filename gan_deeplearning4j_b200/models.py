@@ -148,8 +148,18 @@ def dcgan_generator(size=64, z=100, nf=64, nc=3, lr=2e-4, beta1=0.5) -> List[Dic
     return L
 
 
-def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5) -> List[Dict]:
-    """Conv(4x4 s2 p1)+LeakyReLU(0.2); (Conv+BatchNorm+LeakyReLU)*; Conv(4x4 s1 p0) -> logit; XENT.  Input (nc,size,size)."""
+def _loss_keys(loss, out_activation) -> Dict:
+    """The spec keys of a discriminator's loss-bearing layer: none for XENT (today's specs), else the loss and the activation it applies."""
+    if loss == "xent":
+        if out_activation != "identity":
+            raise ValueError("XENT implies the sigmoid: out_activation applies to the losses other than XENT")
+        return {}
+    return {"loss": loss, "activation": out_activation}
+
+
+def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", out_activation="identity") -> List[Dict]:
+    """Conv(4x4 s2 p1)+LeakyReLU(0.2); (Conv+BatchNorm+LeakyReLU)*; Conv(4x4 s1 p0) -> logit; LossLayer(loss).  Input (nc,size,size).
+    loss: "xent" (sigmoid implied), or "mse" (least-squares GAN), "hinge", "wasserstein", ... applied to out_activation(logit)."""
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
     n_down = int(math.log2(size)) - 2
     L = [{"type": "conv2d", "name": "dis_conv_1", "n_in": nc, "n_out": nf, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "activation": "lrelu", "alpha": 0.2, "updater": u()}]
@@ -159,7 +169,7 @@ def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5) -> List[Dict]:
               {"type": "batchnorm", "name": f"dis_bn_{i + 2}", "updater": u()}, {"type": "activation", "name": f"dis_act_{i + 2}", "activation": "lrelu", "alpha": 0.2}]
         ch *= 2
     L += [{"type": "conv2d", "name": f"dis_conv_{n_down + 1}", "n_in": ch, "n_out": 1, "kernel": (4, 4), "stride": (1, 1), "padding": (0, 0), "updater": u()},
-          {"type": "loss", "name": "dis_loss"}]
+          dict({"type": "loss", "name": "dis_loss"}, **_loss_keys(loss, out_activation))]
     return L
 
 
@@ -171,15 +181,16 @@ def mlp_generator(z=100, hidden=1024, d=256, lr=2e-4, beta1=0.5) -> List[Dict]:
             {"type": "dense", "name": "gen_dense_3", "n_out": d, "activation": "tanh", "updater": u()}]
 
 
-def mlp_discriminator(d=256, hidden=1024, lr=2e-4, beta1=0.5, dropout=None) -> List[Dict]:
-    """dropout = p: a DropoutLayer(p) (p = retain probability) after each hidden LeakyReLU, the DL4J MNIST GAN example's discriminator shape."""
+def mlp_discriminator(d=256, hidden=1024, lr=2e-4, beta1=0.5, dropout=None, loss="xent", out_activation="identity") -> List[Dict]:
+    """dropout = p: a DropoutLayer(p) (p = retain probability) after each hidden LeakyReLU, the DL4J MNIST GAN example's discriminator shape.
+    loss / out_activation: the OutputLayer's loss, as for dcgan_discriminator."""
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
     L = []
     for i in (1, 2):
         L.append({"type": "dense", "name": f"dis_dense_{i}", "n_out": hidden, "activation": "lrelu", "alpha": 0.2, "updater": u()})
         if dropout is not None:
             L.append({"type": "dropout", "name": f"dis_dropout_{i}", "p": dropout})
-    return L + [{"type": "output", "name": "dis_output", "n_out": 1, "updater": u()}]
+    return L + [dict({"type": "output", "name": "dis_output", "n_out": 1, "updater": u()}, **_loss_keys(loss, out_activation))]
 
 
 # algorithmic MACs per image of the conv/deconv/dense layers (SURVEY.md 8d: F = 2*(4*G_f + 8*D_f))

@@ -60,7 +60,7 @@ typedef enum {
   B2G_LAYER_MAXPOOL = 5,     /* SubsamplingLayer.Builder(PoolingType.MAX).kernelSize().stride()   J:141-144,151-154 */
   B2G_LAYER_UPSAMPLE2D = 6,  /* Upsampling2D.Builder(size)                                        J:201-202,210-211 */
   B2G_LAYER_OUTPUT = 7,      /* OutputLayer.Builder(LossFunction.XENT).activation(SIGMOID).nOut() J:159-163,303-308 */
-  B2G_LAYER_LOSS = 8,        /* LossLayer(XENT, sigmoid): loss on incoming logits (DCGAN D-last conv)              */
+  B2G_LAYER_LOSS = 8,        /* LossLayer(loss): loss (b2g_loss) on the incoming pre-activations (DCGAN D-last conv) */
   B2G_LAYER_FF_TO_CNN = 9,   /* FeedForwardToCnnPreProcessor(h,w,c)                               J:200,255         */
   B2G_LAYER_CNN_TO_FF = 10,  /* CnnToFeedForwardPreProcessor (auto-inserted by setInputTypes, SURVEY.md 3.1)       */
   B2G_LAYER_DROPOUT = 11     /* DropoutLayer.Builder(p): p = RETAIN probability in (0, 1], carried in act_alpha; no parameters */
@@ -111,7 +111,27 @@ typedef enum {
 } b2g_updater;
 
 typedef enum { B2G_PREC_FP32 = 0, B2G_PREC_BF16 = 1 } b2g_precision;
-typedef enum { B2G_LOSS_XENT = 0, B2G_LOSS_MCXENT = 1 } b2g_loss;
+/* org.nd4j.linalg.lossfunctions.LossFunctions.LossFunction (DL4J 1.0.0-beta3 org.nd4j.linalg.lossfunctions.impl.*, recalled; parity unpinned like
+ * the rest of the DL4J semantics).  The loss of OUTPUT and LOSS layers (b2g_layer_desc.loss); any other value is B2G_ERR_ARG at b2g_net_create.
+ *   XENT (0)    LossBinaryXENT with the implied sigmoid, nOut = 1 (clipEps = b2g_net_config.xent_clip_eps); b2g_layer_desc.act is ignored
+ *   MCXENT (1)  LossMCXENT with the implied softmax, OUTPUT layers only (B2G_ERR_UNSUPPORTED on a LOSS layer); act is ignored
+ * Codes 2-8 act like ILossFunction.computeGradient(labels, preOutput, activationFn): the layer's pre-activation z, a = act(z) in fp32 with the
+ * layer's b2g_activation act (act_alpha = LeakyReLU's alpha), and dL/dz = dL/da * act'(a), the derivative taken from the output a.  Per example,
+ * over the outputs j < nOut (y = labels):
+ *   MSE (2)             score sum (a-y)^2 / nOut              dL/da = 2(a-y) / nOut
+ *   L1 (3)              score sum |a-y|                       dL/da = sign(a-y), sign(0) = 0
+ *   L2 (4)              score sum (a-y)^2                     dL/da = 2(a-y)
+ *   MAE (5)             score sum |a-y| / nOut                dL/da = sign(a-y) / nOut       (LossMAE = LossFunction.MEAN_ABSOLUTE_ERROR)
+ *   HINGE (6)           score sum max(0, 1 - y a)             dL/da = -y where 1 - y a > 0 (strictly), else 0     (labels +-1)
+ *   SQUARED_HINGE (7)   score sum max(0, 1 - y a)^2           dL/da = -2y max(0, 1 - y a)
+ *   WASSERSTEIN (8)     score sum y a / nOut                  dL/da = y / nOut
+ * The loss of a pass (or of a group of the GAN step) is the sum of its examples' scores, summed in double in an order fixed by the shape (the same
+ * bits on every run) and rounded to fp32 once; score = that sum / minibatch + the l2 term.  OUTPUT layers take any nOut; a LOSS layer needs a
+ * feed-forward input (H = W = 1) or one element per example (else B2G_ERR_UNSUPPORTED).  b2g_net_output returns a = act(z). */
+typedef enum {
+  B2G_LOSS_XENT = 0, B2G_LOSS_MCXENT = 1, B2G_LOSS_MSE = 2, B2G_LOSS_L1 = 3, B2G_LOSS_L2 = 4, B2G_LOSS_MAE = 5, B2G_LOSS_HINGE = 6,
+  B2G_LOSS_SQUARED_HINGE = 7, B2G_LOSS_WASSERSTEIN = 8
+} b2g_loss;
 
 /* One layer of a chain-shaped ComputationGraph (every graph in the reference is a chain, J:118-310). */
 typedef struct {
@@ -127,7 +147,7 @@ typedef struct {
   float l2;                     /* .l2(1e-4) (J:125): weights only, applied AFTER the updater, not lr-scaled */
   float bn_decay, bn_eps;       /* BatchNormalization defaults 0.9 / 1e-5 */
   int32_t pre_h, pre_w, pre_c;  /* FF_TO_CNN target shape */
-  int32_t loss;                 /* OUTPUT layer: 0 = LossFunction.XENT + sigmoid (J:159-163), 1 = MCXENT + softmax (J:357-362) */
+  int32_t loss;                 /* OUTPUT / LOSS layer: b2g_loss (0 = LossFunction.XENT + sigmoid J:159-163, 1 = MCXENT + softmax J:357-362, 2-8 on act) */
   int32_t frozen;               /* TransferLearning.setFeatureExtractor (J:350): FrozenLayer = test-mode forward, no gradient, no update */
 } b2g_layer_desc;
 
@@ -184,9 +204,9 @@ int32_t b2g_net_set_updater_state(b2g_net* net, const float* host, int64_t n);
 int32_t b2g_net_output(b2g_net* net, const float* x, int32_t batch, int32_t train, float* out);
 /* Activations of one layer from the most recent forward (parity tests): NCHW fp32. */
 int32_t b2g_net_get_activation(b2g_net* net, int32_t layer, int32_t batch, float* host);
-/* computeGradientAndScore(): train-mode forward, XENT loss vs labels y [batch,1], backprop.
+/* computeGradientAndScore(): train-mode forward, the last layer's loss (b2g_loss) vs labels y, backprop.
  * score = sum(loss)/batch + 0.5*l2*||W||^2 ; gradients stay on device (b2g_net_get_gradients).
- * Labels y are [batch, nOut] (nOut = 1 for XENT; one-hot rows for MCXENT). */
+ * Labels y are [batch, nOut] (nOut = 1 for XENT; one-hot rows for MCXENT; targets for codes 2-8). */
 int32_t b2g_net_compute_gradient_and_score(b2g_net* net, const float* x, const float* y, int32_t batch, float* score);
 /* epsilon w.r.t. the network input from the last backward (NCHW fp32; what the stacked gan graph feeds the generator). */
 int32_t b2g_net_get_input_gradient(b2g_net* net, int32_t batch, float* host);
@@ -266,7 +286,9 @@ int32_t b2g_net_simt_gemm_calls(b2g_net* net, uint64_t* out);
 /* ---------------------------------------------------------------- the fused GAN step -------------- */
 /* The adversarial iteration J:408-471 with dis / gan / gen sharing storage (the 28 setParam copies J:429-510
  * become aliasing): x_fake = G.output(z_d); D update on (x_real,y_real)+(x_fake,y_fake); G update through D on
- * (z_g, y_gen).  See oracle/dl4j_oracle.py::gan_step for the exact arithmetic. */
+ * (z_g, y_gen).  See oracle/dl4j_oracle.py::gan_step for the exact arithmetic.
+ * The discriminator ends in one output per example with loss XENT or one of codes 2-8 (b2g_loss; MCXENT is B2G_ERR_UNSUPPORTED); the caller's
+ * labels pick the objective: least-squares GAN 1 / 0 / 1 with MSE, hinge +1 / -1 / +1, Wasserstein the caller's sign convention. */
 typedef struct {
   int32_t fake_bn_train;   /* 0: x_fake from inference-mode BN (gen.output, J:420); 1: batch statistics */
   int32_t use_cuda_graph;  /* capture the whole step once and replay it */
@@ -396,10 +418,12 @@ int32_t b2g_test_dropout(b2g_ctx* ctx, int32_t precision, uint64_t seed, int32_t
  *                                                                                     -> out0 y T, out1 eps_in T, out2 argmax (as float)
  *   UPSAMPLE       in0 x [N][H][W][C] T, in1 eps_out [N][H*KH][W*KH][C] T (factor KH) -> out0 y T, out1 eps_in T
  *   SUMSQ          in0 p [n] fp32, segments seg_off / seg_len / seg_coef              -> sumsq
+ *   LOSS           in0 logits [groups][rows][cols] T, in1 labels fp32                 -> out0 dz T, out1 loss per group [groups]
+ *                                                                                        (loss = b2g_loss 2-8, cols = nOut, act, alpha)
  * Every output buffer not asked for may be NULL. */
 typedef enum {
   B2G_EW_REDUCE_SPLITS = 0, B2G_EW_REDUCE_MULTI = 1, B2G_EW_COLSUM = 2, B2G_EW_XENT = 3, B2G_EW_SOFTMAX_XENT = 4,
-  B2G_EW_ACT_FWD = 5, B2G_EW_ACT_BWD = 6, B2G_EW_MAXPOOL = 7, B2G_EW_UPSAMPLE = 8, B2G_EW_SUMSQ = 9
+  B2G_EW_ACT_FWD = 5, B2G_EW_ACT_BWD = 6, B2G_EW_MAXPOOL = 7, B2G_EW_UPSAMPLE = 8, B2G_EW_SUMSQ = 9, B2G_EW_LOSS = 10
 } b2g_ew_op;
 typedef struct {          /* one split-K sum of a reduce list: dst[i] = sum_s src[s*stride + i], i < n, all offsets in elements of in0 */
   int64_t n, stride, src_off, dst_off;
@@ -424,6 +448,7 @@ typedef struct {
   double sumsq;           /* out: SUMSQ's result */
   char kernel[64];        /* out: the kernel each wrapper call dispatched, comma-separated in call order (MAXPOOL / UPSAMPLE: forward, backward);
                              COLSUM names its first stage, the final stage is the same kernel on every path */
+  int32_t loss;           /* LOSS: b2g_loss 2-8 */
 } b2g_test_ew_opts;
 int32_t b2g_test_ew(b2g_ctx* ctx, int32_t precision, b2g_test_ew_opts* opts, const float* in0, const float* in1, float* out0, float* out1, float* out2);
 

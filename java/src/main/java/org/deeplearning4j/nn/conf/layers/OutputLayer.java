@@ -2,7 +2,8 @@ package org.deeplearning4j.nn.conf.layers;
 public final class OutputLayer {
     private OutputLayer() {}
     public static final class Builder extends Layer.Builder<Builder> {
-        public Builder(org.nd4j.linalg.lossfunctions.LossFunctions.LossFunction f) { l.type = 7; l.loss = f == org.nd4j.linalg.lossfunctions.LossFunctions.LossFunction.MCXENT ? 1 : 0; l.act = 0; }   // XENT+sigmoid (J:159-163) or MCXENT+softmax (J:357-362); the activation is implied by the loss   // J:159-163
+        // XENT+sigmoid (J:159-163) and MCXENT+softmax (J:357-362) imply their activation; the other losses apply .activation(..), identity by default
+        public Builder(org.nd4j.linalg.lossfunctions.LossFunctions.LossFunction f) { l.type = 7; l.loss = f.code; l.act = 0; }
         
     }
 }
