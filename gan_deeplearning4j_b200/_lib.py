@@ -50,11 +50,12 @@ class ConvGeom(C.Structure):
 
 class TestConvOpts(C.Structure):
     """b2g_test_conv_opts: the epilogue a kernel-level parity test asks for, the name of the kernel that ran, and the schedule controls
-    (forced tile width, grid cap, output poisoning, [C][O] dense weight operand)."""
+    (forced tile width, grid cap, output poisoning, [C][O] dense weight operand); the parameter offset of the SIMT / skinny-layer / dense
+    kernels' fp32 weight operand or gradient, and the split-K count they report."""
     _fields_ = [("epi", C.c_int32), ("act", C.c_int32), ("alpha", C.c_float), ("bias", C.POINTER(C.c_float)), ("scale", C.POINTER(C.c_float)),
                 ("groups", C.c_int32), ("aux", C.POINTER(C.c_float)), ("aux2", C.POINTER(C.c_float)), ("stats", C.POINTER(C.c_double)), ("kernel", C.c_char * 64),
                 ("bn", C.c_int32), ("max_ctas", C.c_int32), ("poison", C.c_int32), ("w_mn", C.c_int32), ("per_tap", C.c_int32), ("slab", C.c_int32),
-                ("defer", C.c_int32), ("db", C.POINTER(C.c_float))]
+                ("defer", C.c_int32), ("db", C.POINTER(C.c_float)), ("param_offset", C.c_int32), ("splits", C.c_int32)]
 
 
 class EwReduceJob(C.Structure):

@@ -1442,8 +1442,19 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
     if (!ok) return fail(B2G_ERR_UNSUPPORTED, "no tensor-core kernel for this shape");
   }
   const bool tc_conv = impl == 1 && kind != 2, ps = impl == 3 && kind == 1;     // the launches of tc_conv_kernel (ps: its pixel-shuffle form)
-  if (opt && !tc_conv && !ps && (opt->epi || opt->bias || opt->scale || opt->act))
-    return fail(B2G_ERR_UNSUPPORTED, "epilogue options apply to the tensor-core fprop / dgrad kernels (impl 1, kind 0 / 1) and the pixel-shuffle deconv (impl 3, kind 1)");
+  // the SIMT, skinny-layer and dense kernels; gemm_epi: those whose production wrapper takes bias / activation (k_dense_small_o_dgrad and the
+  // weight gradients have none: as in gemm_dgrad, a dense input gradient with an epilogue runs the short-reduction kernel)
+  const bool gemm = impl == 0 || impl == 2 || impl == 4;
+  const bool gemm_epi = gemm && kind != 2 && !(impl == 4 && kind == 1 && !dense_small_k_supported(g));
+  if (opt && gemm) {
+    if (opt->epi || (!gemm_epi && (opt->bias || opt->scale || opt->act)))
+      return fail(B2G_ERR_UNSUPPORTED, "impl %d kind %d: no epilogue (bias / activation: impl 0 / 2 kind 0 / 1, impl 4 kind 0 and the short-reduction kind 1; no fused BatchNorm epilogue)", impl, kind);
+    if (opt->scale && impl != 0) return fail(B2G_ERR_UNSUPPORTED, "scale applies to the SIMT fprop / dgrad (impl 0) and the tensor-core kernels");
+  }
+  else if (opt && !tc_conv && !ps && (opt->epi || opt->bias || opt->scale || opt->act))
+    return fail(B2G_ERR_UNSUPPORTED, "epilogue options apply to the tensor-core fprop / dgrad kernels (impl 1, kind 0 / 1), the pixel-shuffle deconv (impl 3, kind 1) and the SIMT / skinny-layer / dense kernels (impl 0 / 2 / 4)");
+  const int poff = opt ? opt->param_offset : 0;
+  if (poff < 0 || (poff && !gemm)) return fail(B2G_ERR_UNSUPPORTED, "param_offset %d: applies to the SIMT / skinny-layer / dense kernels (impl 0 / 2 / 4)", poff);
   if (opt && ps && (opt->scale || (opt->epi != EPI_PLAIN && opt->epi != EPI_ACTBWD)))
     return fail(B2G_ERR_UNSUPPORTED, "the pixel-shuffle deconv has bias, activation and the activation-backward epilogue only");
   const int force_bn = opt ? opt->bn : 0, max_ctas = opt ? opt->max_ctas : 0;
@@ -1452,7 +1463,7 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   if (force_bn && (!tc_conv || (force_bn != 64 && force_bn != 128) || oc % force_bn))
     return fail(B2G_ERR_UNSUPPORTED, "bn %d: the tensor-core fprop / dgrad tile is 64 or 128 columns and must divide the %d output channels", force_bn, oc);
   if (max_ctas < 0 || (max_ctas && !tc_conv && !ps)) return fail(B2G_ERR_UNSUPPORTED, "max_ctas %d: a grid cap applies to tc_conv_kernel launches only", max_ctas);
-  if (poison && kind == 2) return fail(B2G_ERR_UNSUPPORTED, "poison applies to the bf16 outputs of kinds 0 / 1");
+  if (poison && kind == 2 && !gemm) return fail(B2G_ERR_UNSUPPORTED, "poison applies to the outputs of kinds 0 / 1, and to the weight gradients of impl 0 / 2 / 4");
   if (w_mn && (impl != 1 || kind != 0 || g.KH != 1 || g.KW != 1)) return fail(B2G_ERR_UNSUPPORTED, "w_mn: the [C][O] weight operand exists for the 1x1 tensor-core fprop only");
   const bool defer = opt && opt->defer; float* db_host = opt ? opt->db : nullptr;
   if (defer && !(kind == 2 && (impl == 1 || impl == 3))) return fail(B2G_ERR_UNSUPPORTED, "defer applies to the tensor-core weight gradients (kind 2, impl 1 / 3)");
@@ -1470,8 +1481,13 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   float *fa = nullptr, *fb = nullptr, *fo = nullptr, *scratch = nullptr; void *ta = nullptr, *tb = nullptr, *to = nullptr; __nv_bfloat16* wps = nullptr;
   float *d_bias = nullptr, *d_scale = nullptr, *d_coef = nullptr, *d_auxf = nullptr; __nv_bfloat16 *d_aux = nullptr, *d_aux2 = nullptr; unsigned long long* d_acc = nullptr;
   size_t sc = std::max(std::max(std::max(k_simt_wgrad_scratch_floats(g), k_tc_wgrad_scratch_floats(g)), std::max(k_edge_wgrad_scratch_floats(g), k_tc_edge_wgrad_scratch_floats(g))), k_dense_small_o_wgrad_scratch_floats(g)) + 16;
-  CU(cudaMalloc(&fa, 4 * na)); CU(cudaMalloc(&fb, 4 * nb)); CU(cudaMalloc(&fo, 4 * no)); CU(cudaMalloc(&scratch, 4 * sc));
-  CU(cudaMalloc(&ta, ts * na)); CU(cudaMalloc(&tb, ts * nb)); CU(cudaMalloc(&to, ts * no));
+  // param_offset: the fp32 weight operand (FP32, kinds 0 / 1) and the weight gradient (kind 2) start poff elements past the 256-byte aligned
+  // cudaMalloc base, as W and dW do in a net's flattened parameter / gradient vectors
+  const size_t woff = (prec == PREC_F32 && kind != 2) ? (size_t)poff : 0, dwoff = kind == 2 ? (size_t)poff : 0;
+  CU(cudaMalloc(&fa, 4 * na)); CU(cudaMalloc(&fb, 4 * nb)); CU(cudaMalloc(&fo, 4 * (no + dwoff))); CU(cudaMalloc(&scratch, 4 * sc));
+  CU(cudaMalloc(&ta, ts * na)); CU(cudaMalloc(&tb, ts * nb + 4 * woff)); CU(cudaMalloc(&to, ts * no));
+  float* const fres = fo + dwoff;           // the fp32 result: dw (kind 2), or the widened output (kinds 0 / 1)
+  void* const tbase = tb; tb = (float*)tb + woff;
   CU(cudaMemcpyAsync(fa, a_host, 4 * na, cudaMemcpyHostToDevice, s)); CU(cudaMemcpyAsync(fb, b_host, 4 * nb, cudaMemcpyHostToDevice, s));
   if (prec == PREC_BF16) { k_cast_f32_to_bf16(fa, (__nv_bfloat16*)ta, na, s); k_cast_f32_to_bf16(fb, (__nv_bfloat16*)tb, nb, s); }
   else { CU(cudaMemcpyAsync(ta, fa, 4 * na, cudaMemcpyDeviceToDevice, s)); CU(cudaMemcpyAsync(tb, fb, 4 * nb, cudaMemcpyDeviceToDevice, s)); }
@@ -1496,31 +1512,37 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
     }
     if (opt->epi || opt->scale) pe = &epi;
   }
+  if (opt && gemm_epi) {
+    act = opt->act; alpha = opt->alpha;
+    if (opt->bias) { CU(cudaMalloc(&d_bias, 4 * oc)); CU(cudaMemcpyAsync(d_bias, opt->bias, 4 * oc, cudaMemcpyHostToDevice, s)); bias = d_bias; }
+    if (opt->scale) { CU(cudaMalloc(&d_scale, 4 * oc)); CU(cudaMemcpyAsync(d_scale, opt->scale, 4 * oc, cudaMemcpyHostToDevice, s)); }
+  }
   cudaEvent_t e0, e1; CU(cudaEventCreate(&e0)); CU(cudaEventCreate(&e1));
   int reps = iters < 1 ? 1 : iters; int rc = 0;
-  g_tc_last_kernel = ""; g_tc_last_slab = false;
+  g_tc_last_kernel = ""; g_tc_last_slab = false; g_gemm_last_kernel = ""; g_gemm_last_splits = 0;
   TcTestSchedule schedule(force_bn, max_ctas, per_tap);
   for (int it = -1; it < reps; ++it) {       // it = -1: warm-up
     if (it == 0) CU(cudaEventRecord(e0, s));
     if (d_acc) CU(cudaMemsetAsync(d_acc, 0, 8 * k_bn_acc_elems(oc, groups), s));
     if (poison) CU(cudaMemsetAsync(to, 0xFF, ts * no, s));       // a tile this launch does not write reads back as NaN, not as the warm-up's values
+    if (poison && kind == 2) { CU(cudaMemsetAsync(fres, 0xFF, 4 * no, s)); CU(cudaMemsetAsync(scratch, 0xFF, 4 * sc, s)); }   // fp32 NaN: dw and the split-K partials
     if (impl == 4) {
       const bool so = dense_small_o_supported(g);
-      if (kind == 0) k_dense_small_o_fwd(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s);
-      else if (kind == 1) { if (so) k_dense_small_o_dgrad(prec, prec, g, ta, tb, to, s); else k_dense_small_k_dgrad(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s); }
-      else { if (so) k_dense_small_o_wgrad(prec, g, ta, tb, fo, scratch, 0, s); else k_dense_small_k_wgrad(prec, g, ta, tb, fo, s); }
+      if (kind == 0) k_dense_small_o_fwd(prec, prec, g, ta, tb, bias, to, act, alpha, s);
+      else if (kind == 1) { if (so && !bias && !act) k_dense_small_o_dgrad(prec, prec, g, ta, tb, to, s); else k_dense_small_k_dgrad(prec, prec, g, ta, tb, bias, to, act, alpha, s); }
+      else { if (so) k_dense_small_o_wgrad(prec, g, ta, tb, fres, scratch, 0, s); else k_dense_small_k_wgrad(prec, g, ta, tb, fres, s); }
     }
     else if (impl >= 2) {
-      if (kind == 0) { if (impl == 3) rc = k_tc_edge_conv(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, nullptr, (__nv_bfloat16*)to, 0, 0.f, s); else k_edge_conv_small_cin(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s); }
-      else if (kind == 1) { if (impl == 3) rc = k_tc_deconv_ps(g, (const __nv_bfloat16*)ta, wps, bias, (__nv_bfloat16*)to, act, alpha, s, pe); else k_edge_deconv_small_c(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s); }
+      if (kind == 0) { if (impl == 3) rc = k_tc_edge_conv(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, nullptr, (__nv_bfloat16*)to, 0, 0.f, s); else k_edge_conv_small_cin(prec, prec, g, ta, tb, bias, to, act, alpha, s); }
+      else if (kind == 1) { if (impl == 3) rc = k_tc_deconv_ps(g, (const __nv_bfloat16*)ta, wps, bias, (__nv_bfloat16*)to, act, alpha, s, pe); else k_edge_deconv_small_c(prec, prec, g, ta, tb, bias, to, act, alpha, s); }
       else {
-        if (impl == 3) { rc = k_tc_edge_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fo, d_db, scratch, sc, 0, s, prl); if (rc >= 0) { db_written = rc; rc = 0; } }
-        else k_edge_wgrad_small_cin(prec, g, ta, tb, fo, scratch, 0, s);
+        if (impl == 3) { rc = k_tc_edge_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fres, d_db, scratch, sc, 0, s, prl); if (rc >= 0) { db_written = rc; rc = 0; } }
+        else k_edge_wgrad_small_cin(prec, g, ta, tb, fres, scratch, 0, s);
       }
     }
-    else if (kind == 0) { if (impl) rc = k_tc_fprop(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s, pe, w_mn ? 1 : 0); else k_simt_fprop(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s); }
-    else if (kind == 1) { if (impl) rc = k_tc_dgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s, pe); else k_simt_dgrad(prec, prec, g, ta, tb, nullptr, to, 0, 0.f, s); }
-    else { if (impl) rc = k_tc_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fo, scratch, sc, 0, s, prl); else k_simt_wgrad(prec, g, ta, tb, fo, scratch, sc, 0, s); }
+    else if (kind == 0) { if (impl) rc = k_tc_fprop(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s, pe, w_mn ? 1 : 0); else k_simt_fprop(prec, prec, g, ta, tb, bias, to, act, alpha, s, d_scale); }
+    else if (kind == 1) { if (impl) rc = k_tc_dgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s, pe); else k_simt_dgrad(prec, prec, g, ta, tb, bias, to, act, alpha, s, d_scale); }
+    else { if (impl) rc = k_tc_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fres, scratch, sc, 0, s, prl); else k_simt_wgrad(prec, g, ta, tb, fres, scratch, sc, 0, s); }
     if (rc) break;
     if (defer) {      // the backward pass's one reduce-list launch over the partials the wgrad kernel left in scratch
       if (!rl.count) { rc = -4; break; }
@@ -1531,13 +1553,16 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   CU(cudaEventRecord(e1, s));
   if (rc == -4) return fail(B2G_ERR_CUDA, "defer: the weight gradient queued no reduction");
   if (rc) return fail(B2G_ERR_CUDA, "tensor-core kernel launch failed (%d)", rc);
-  if (opt) { strncpy(opt->kernel, g_tc_last_kernel, sizeof(opt->kernel) - 1); opt->kernel[sizeof(opt->kernel) - 1] = 0; opt->slab = g_tc_last_slab; }
+  if (opt) {
+    strncpy(opt->kernel, gemm ? g_gemm_last_kernel : g_tc_last_kernel, sizeof(opt->kernel) - 1); opt->kernel[sizeof(opt->kernel) - 1] = 0; opt->slab = g_tc_last_slab;
+    opt->splits = gemm ? g_gemm_last_splits : 0;
+  }
   if (d_db) {
     if (!db_written) { cudaFree(d_db); return fail(B2G_ERR_UNSUPPORTED, "the edge weight gradient produces no bias column for C = %d", g.C); }
     CU(cudaMemcpyAsync(db_host, d_db, 4 * (size_t)g.O, cudaMemcpyDeviceToHost, s));
   }
   if (kind != 2) { if (prec == PREC_BF16) { /* widen */ k_nhwc_to_nchw_f32(prec, to, fo, 1, 1, (int)no, s); } else CU(cudaMemcpyAsync(fo, to, 4 * no, cudaMemcpyDeviceToDevice, s)); }
-  CU(cudaMemcpyAsync(out, fo, 4 * no, cudaMemcpyDeviceToHost, s));
+  CU(cudaMemcpyAsync(out, fres, 4 * no, cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s)); CHECK_KERNELS();
   if (d_acc && opt && opt->stats) {      // [groups][2][C] doubles from the [groups][2][2][C] hi | lo words
     std::vector<long long> h(k_bn_acc_elems(oc, groups)); CU(cudaMemcpy(h.data(), d_acc, 8 * h.size(), cudaMemcpyDeviceToHost));
@@ -1546,7 +1571,7 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   }
   float ms = 0.f; CU(cudaEventElapsedTime(&ms, e0, e1)); if (ms_per_iter) *ms_per_iter = ms / reps;
   cudaEventDestroy(e0); cudaEventDestroy(e1);
-  cudaFree(fa); cudaFree(fb); cudaFree(fo); cudaFree(scratch); cudaFree(ta); cudaFree(tb); cudaFree(to); if (wps) cudaFree(wps); if (d_db) cudaFree(d_db);
+  cudaFree(fa); cudaFree(fb); cudaFree(fo); cudaFree(scratch); cudaFree(ta); cudaFree(tbase); cudaFree(to); if (wps) cudaFree(wps); if (d_db) cudaFree(d_db);
   if (d_bias) cudaFree(d_bias); if (d_scale) cudaFree(d_scale); if (d_coef) cudaFree(d_coef); if (d_auxf) cudaFree(d_auxf); if (d_aux) cudaFree(d_aux); if (d_aux2) cudaFree(d_aux2); if (d_acc) cudaFree(d_acc);
   return 0;
 }

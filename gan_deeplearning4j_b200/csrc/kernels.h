@@ -186,6 +186,10 @@ void k_simt_dgrad(int prec, int wprec, const ConvGeom& g, const void* dy, const 
 // wgrad:  dw[o][r][s][c] = sum_pixels dy[pix][o] x[pix(r,s)][c]   (fp32 out, split-K scratch of k_simt_wgrad_scratch floats)
 void k_simt_wgrad(int prec, const ConvGeom& g, const void* x, const void* dy, float* dw, float* scratch, size_t scratch_floats, int accumulate, cudaStream_t s);
 size_t k_simt_wgrad_scratch_floats(const ConvGeom& g);
+// which SIMT / skinny-layer / dense kernel the most recent k_simt_* / k_edge_* / k_dense_* call below dispatched, and the number of split-K
+// partial sums it reduced (wgrad_splits, edge_wgrad_ctas, dense_wgrad_splits; 1 where the kernel has no split).  Kernel-level tests assert both.
+extern const char* g_gemm_last_kernel;
+extern int g_gemm_last_splits;
 
 // ---- skinny layers (kernels_edge.cu): <=4 image channels on one side, or <=4 output units ------------------
 bool edge_deconv_small_c_supported(const ConvGeom& g);   // dgrad form, g.C <= 4

@@ -338,8 +338,9 @@ __global__ void __launch_bounds__(128) dense_small_k_dgrad_kernel(const T* __res
   for (int r = 0; r < 8; ++r) if (n0 + r < N) st2(dx + (size_t)(n0 + r) * C + c, act_fwd(act, acc[r][0] + b0, alpha), act_fwd(act, acc[r][1] + b1, alpha));
 }
 // dw[o][c] = sum_n dy[n][o] * x[n][c]: thread = 2 adjacent c x 16 o, the whole batch reduced in the CTA (no split, deterministic);
-// rows are consumed 8 at a time so that eight global loads are in flight per thread
-template <typename T>
+// rows are consumed 8 at a time so that eight global loads are in flight per thread.  dw is a layer's slice of the flattened gradient vector,
+// at any element offset: ST2 (dw 8-byte aligned; C and c are even) stores each pair as one float2, otherwise as two floats.
+template <typename T, bool ST2>
 __global__ void __launch_bounds__(128) dense_small_k_wgrad_kernel(const T* __restrict__ x, const T* __restrict__ dy, float* __restrict__ dw, int N, int C, int O) { pdl_enter();
   __shared__ __align__(16) float sd[128][16];            // [n][o local]
   const int c = (blockIdx.x * 128 + threadIdx.x) * 2, o0 = blockIdx.y * 16;
@@ -369,7 +370,10 @@ __global__ void __launch_bounds__(128) dense_small_k_wgrad_kernel(const T* __res
     }
   }
 #pragma unroll
-  for (int j = 0; j < 16; ++j) if (o0 + j < O) st2(dw + (size_t)(o0 + j) * C + c, acc[j][0], acc[j][1]);
+  for (int j = 0; j < 16; ++j) if (o0 + j < O) {
+    float* p = dw + (size_t)(o0 + j) * C + c;
+    if constexpr (ST2) st2(p, acc[j][0], acc[j][1]); else { p[0] = acc[j][0]; p[1] = acc[j][1]; }
+  }
 }
 
 
@@ -516,6 +520,7 @@ template <typename T, typename TW>
 static void launch_deconv_small_c(const ConvGeom& g, const void* dy, const void* w, const float* bias, void* dx, int act, float alpha, cudaStream_t s) {
   long tot = (long)g.N * g.OH * g.OW; long blocks = (tot + 127) / 128; if (blocks > device_sm_count() * 8) blocks = device_sm_count() * 8;
   launch_pdl(edge_deconv_small_c_kernel<T, TW>, dim3((unsigned)blocks), dim3(128), (size_t)(16 * g.O * sizeof(float4)), s, (const T*)dy, (const TW*)w, bias, (T*)dx, g.N, g.OH, g.OW, g.O, g.C, act, alpha);
+  g_gemm_last_kernel = "edge_deconv_small_c_kernel"; g_gemm_last_splits = 1;
 }
 void k_edge_deconv_small_c(int prec, int wprec, const ConvGeom& g, const void* dy, const void* w, const float* bias, void* dx, int act, float alpha, cudaStream_t s) {
   if (prec == PREC_F32) launch_deconv_small_c<float, float>(g, dy, w, bias, dx, act, alpha, s);
@@ -527,6 +532,7 @@ template <typename T, typename TW>
 static void launch_conv_small_cin(const ConvGeom& g, const void* x, const void* w, const float* bias, void* out, int act, float alpha, cudaStream_t s) {
   long tot = (long)g.N * g.OH * (g.OW / 4) * (g.O / 16); long blocks = (tot + 127) / 128; if (blocks > device_sm_count() * 8) blocks = device_sm_count() * 8;
   launch_pdl(edge_conv_small_cin_kernel<T, TW>, dim3((unsigned)blocks), dim3(128), (size_t)(16 * g.C * g.O * sizeof(float)), s, (const T*)x, (const TW*)w, bias, (T*)out, g.N, g.H, g.W, g.C, g.OH, g.OW, g.O, act, alpha);
+  g_gemm_last_kernel = "edge_conv_small_cin_kernel"; g_gemm_last_splits = 1;
 }
 void k_edge_conv_small_cin(int prec, int wprec, const ConvGeom& g, const void* x, const void* w, const float* bias, void* out, int act, float alpha, cudaStream_t s) {
   if (prec == PREC_F32) launch_conv_small_cin<float, float>(g, x, w, bias, out, act, alpha, s);
@@ -536,23 +542,35 @@ void k_edge_conv_small_cin(int prec, int wprec, const ConvGeom& g, const void* x
 }
 static int edge_wgrad_ctas(const ConvGeom& g) { long P = (long)g.N * g.OH * g.OW; long c = device_sm_count() * 2; long cap = (P + 63) / 64; if (c > cap) c = cap; if (c < 1) c = 1; return (int)c; }
 size_t k_edge_wgrad_scratch_floats(const ConvGeom& g) { return edge_wgrad_small_cin_supported(g) ? (size_t)edge_wgrad_ctas(g) * g.O * 16 * g.C : 0; }
+// (64*O + 64*64) floats of dynamic shared memory: past the 48 KB default for O > 128.  The kernel is opted into the amount the largest
+// supported O (256) needs, once per (instantiation, device) -- the attribute is per device -- and only by a launch that needs more than 48 KB.
+static size_t edge_wgrad_smem(int O) { return (64 * (size_t)O + 64 * 64) * sizeof(float); }
+template <typename T> static void edge_wgrad_opt_in() {
+  static bool set_[64] = {}; int d = 0; cudaGetDevice(&d); if (d < 0 || d >= 64) d = 0;
+  if (!set_[d] && cudaFuncSetAttribute(edge_wgrad_small_cin_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)edge_wgrad_smem(256)) == cudaSuccess) set_[d] = true;
+}
 void k_edge_wgrad_small_cin(int prec, const ConvGeom& g, const void* x, const void* dy, float* dw, float* scratch, int accumulate, cudaStream_t s) {
   const int ctas = edge_wgrad_ctas(g); const long P = (long)g.N * g.OH * g.OW; const int ppc = (int)((P + ctas - 1) / ctas);
-  const size_t n = (size_t)g.O * 16 * g.C; const size_t smem = (64 * g.O + 64 * 64) * sizeof(float);
+  const size_t n = (size_t)g.O * 16 * g.C; const size_t smem = edge_wgrad_smem(g.O);
+  if (smem > 48 * 1024) DISPATCH_PREC(prec, T, (edge_wgrad_opt_in<T>()));
   DISPATCH_PREC(prec, T, (launch_pdl(edge_wgrad_small_cin_kernel<T>, dim3(ctas), dim3(2 * g.O), (size_t)(smem), s, (const T*)x, (const T*)dy, scratch, g.N, g.H, g.W, g.C, g.OH, g.OW, g.O, ppc))); LAUNCHED();
   k_reduce_splits(scratch, dw, n, ctas, n, accumulate, s);
+  g_gemm_last_kernel = "edge_wgrad_small_cin_kernel"; g_gemm_last_splits = ctas;
 }
 bool dense_small_k_supported(const ConvGeom& g) { return g.KH == 1 && g.KW == 1 && g.H == 1 && g.W == 1 && g.O >= 1 && g.O <= 128 && g.C % 256 == 0 && g.C >= 256; }
 void k_dense_small_k_dgrad(int prec, int wprec, const ConvGeom& g, const void* dy, const void* w, const float* bias, void* dx, int act, float alpha, cudaStream_t s) {
   dim3 grid(g.C / 256, (g.N + 7) / 8);
+  g_gemm_last_kernel = "dense_small_k_dgrad_kernel"; g_gemm_last_splits = 1;
   if (prec == PREC_F32) launch_pdl(dense_small_k_dgrad_kernel<float, float>, grid, dim3(128), (size_t)0, s, (const float*)dy, (const float*)w, bias, (float*)dx, g.N, g.C, g.O, act, alpha);
   else if (wprec == PREC_F32) launch_pdl(dense_small_k_dgrad_kernel<__nv_bfloat16, float>, grid, dim3(128), (size_t)0, s, (const __nv_bfloat16*)dy, (const float*)w, bias, (__nv_bfloat16*)dx, g.N, g.C, g.O, act, alpha);
-  else if ((reinterpret_cast<uintptr_t>(w) & 15) == 0 && (reinterpret_cast<uintptr_t>(dy) & 3) == 0 && (reinterpret_cast<uintptr_t>(dx) & 3) == 0)
+  else if ((reinterpret_cast<uintptr_t>(w) & 15) == 0 && (reinterpret_cast<uintptr_t>(dy) & 3) == 0 && (reinterpret_cast<uintptr_t>(dx) & 3) == 0) {
+    g_gemm_last_kernel = "dense_k_fwd_mma_kernel";
     switch ((g.O + 15) / 16) {
 #define B2G_DK_FWD(KT) case KT: launch_pdl(dense_k_fwd_mma_kernel<KT>, dim3(g.C / 64, (g.N + 63) / 64), dim3(128), (size_t)0, s, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)dx, g.N, g.C, g.O, act, alpha); break;
       B2G_DK_FWD(1) B2G_DK_FWD(2) B2G_DK_FWD(3) B2G_DK_FWD(4) B2G_DK_FWD(5) B2G_DK_FWD(6) B2G_DK_FWD(7) B2G_DK_FWD(8)
 #undef B2G_DK_FWD
     }
+  }
   else launch_pdl(dense_small_k_dgrad_kernel<__nv_bfloat16, __nv_bfloat16>, grid, dim3(128), (size_t)0, s, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)dx, g.N, g.C, g.O, act, alpha);
   LAUNCHED();
 }
@@ -564,22 +582,29 @@ void k_dense_small_k_wgrad(int prec, const ConvGeom& g, const void* x, const voi
       B2G_DK_WG(1) B2G_DK_WG(2) B2G_DK_WG(3) B2G_DK_WG(4) B2G_DK_WG(5) B2G_DK_WG(6) B2G_DK_WG(7) B2G_DK_WG(8)
 #undef B2G_DK_WG
     }
-    LAUNCHED(); return;
+    LAUNCHED(); g_gemm_last_kernel = "dense_k_wgrad_mma_kernel"; g_gemm_last_splits = 1; return;
   }
-  DISPATCH_PREC(prec, T, (launch_pdl(dense_small_k_wgrad_kernel<T>, grid, dim3(128), (size_t)0, s, (const T*)x, (const T*)dy, dw, g.N, g.C, g.O))); LAUNCHED();
+  if ((reinterpret_cast<uintptr_t>(dw) & 7) == 0) {
+    DISPATCH_PREC(prec, T, (launch_pdl(dense_small_k_wgrad_kernel<T, true>, grid, dim3(128), (size_t)0, s, (const T*)x, (const T*)dy, dw, g.N, g.C, g.O)));
+    g_gemm_last_kernel = "dense_small_k_wgrad_kernel<st2>";
+  } else {
+    DISPATCH_PREC(prec, T, (launch_pdl(dense_small_k_wgrad_kernel<T, false>, grid, dim3(128), (size_t)0, s, (const T*)x, (const T*)dy, dw, g.N, g.C, g.O)));
+    g_gemm_last_kernel = "dense_small_k_wgrad_kernel<st1>";
+  }
+  LAUNCHED(); g_gemm_last_splits = 1;
 }
 void k_dense_small_o_fwd(int prec, int wprec, const ConvGeom& g, const void* x, const void* w, const float* bias, void* out, int act, float alpha, cudaStream_t s) {
   if (prec == PREC_F32) launch_pdl(dense_small_o_fwd_kernel<float, float>, dim3(g.N), dim3(128), (size_t)(0), s, (const float*)x, (const float*)w, bias, (float*)out, g.C, g.O, act, alpha);
   else if (wprec == PREC_F32) launch_pdl(dense_small_o_fwd_kernel<__nv_bfloat16, float>, dim3(g.N), dim3(128), (size_t)(0), s, (const __nv_bfloat16*)x, (const float*)w, bias, (__nv_bfloat16*)out, g.C, g.O, act, alpha);
   else launch_pdl(dense_small_o_fwd_kernel<__nv_bfloat16, __nv_bfloat16>, dim3(g.N), dim3(128), (size_t)(0), s, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)out, g.C, g.O, act, alpha);
-  LAUNCHED();
+  LAUNCHED(); g_gemm_last_kernel = "dense_small_o_fwd_kernel"; g_gemm_last_splits = 1;
 }
 void k_dense_small_o_dgrad(int prec, int wprec, const ConvGeom& g, const void* dy, const void* w, void* dx, cudaStream_t s) {
   size_t tot = (size_t)g.N * (g.C / 8); int blocks = (int)((tot + 255) / 256); if (blocks > device_sm_count() * 8) blocks = device_sm_count() * 8;
   if (prec == PREC_F32) launch_pdl(dense_small_o_dgrad_kernel<float, float>, dim3(blocks), dim3(256), (size_t)(0), s, (const float*)dy, (const float*)w, (float*)dx, g.N, g.C, g.O);
   else if (wprec == PREC_F32) launch_pdl(dense_small_o_dgrad_kernel<__nv_bfloat16, float>, dim3(blocks), dim3(256), (size_t)(0), s, (const __nv_bfloat16*)dy, (const float*)w, (__nv_bfloat16*)dx, g.N, g.C, g.O);
   else launch_pdl(dense_small_o_dgrad_kernel<__nv_bfloat16, __nv_bfloat16>, dim3(blocks), dim3(256), (size_t)(0), s, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)w, (__nv_bfloat16*)dx, g.N, g.C, g.O);
-  LAUNCHED();
+  LAUNCHED(); g_gemm_last_kernel = "dense_small_o_dgrad_kernel"; g_gemm_last_splits = 1;
 }
 static int dense_wgrad_splits(const ConvGeom& g) { int sp = (g.N + 7) / 8; if (sp > 32) sp = 32; if (sp < 1) sp = 1; return sp; }
 size_t k_dense_small_o_wgrad_scratch_floats(const ConvGeom& g) { return dense_small_o_supported(g) ? (size_t)dense_wgrad_splits(g) * g.O * g.C : 0; }
@@ -588,6 +613,7 @@ void k_dense_small_o_wgrad(int prec, const ConvGeom& g, const void* x, const voi
   dim3 grid((g.C / 8 + 127) / 128, sp);
   DISPATCH_PREC(prec, T, (launch_pdl(dense_small_o_wgrad_kernel<T>, dim3(grid), dim3(128), (size_t)(0), s, (const T*)x, (const T*)dy, scratch, g.N, g.C, g.O, rps))); LAUNCHED();
   k_reduce_splits(scratch, dw, n, sp, n, accumulate, s);
+  g_gemm_last_kernel = "dense_small_o_wgrad_kernel"; g_gemm_last_splits = sp;
 }
 
 }  // namespace b2g

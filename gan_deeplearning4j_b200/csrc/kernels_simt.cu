@@ -16,6 +16,8 @@
 namespace b2g {
 
 static const int TM = 64, TN = 64, TK = 16;
+const char* g_gemm_last_kernel = "";
+int g_gemm_last_splits = 0;
 
 template <typename T, typename TW>
 struct FpropProb {
@@ -160,12 +162,14 @@ static void launch_fprop(const ConvGeom& g, const void* x, const void* w, const 
   FpropProb<T, TW> p{g, (const T*)x, (const TW*)w, bias, scale, (T*)out, act, alpha, g.N * g.OH * g.OW, g.O, g.KH * g.KW * g.C};
   dim3 grid((p.Ncols + TN - 1) / TN, (p.M + TM - 1) / TM, 1);
   launch_pdl(simt_gemm_kernel<FpropProb<T, TW>>, dim3(grid), dim3(256), (size_t)(0), s, p, p.K); LAUNCHED();
+  g_gemm_last_kernel = "simt_gemm_kernel<FpropProb>"; g_gemm_last_splits = 1;
 }
 template <typename T, typename TW>
 static void launch_dgrad(const ConvGeom& g, const void* dy, const void* w, const float* bias, const float* scale, void* dx, int act, float alpha, cudaStream_t s) {
   DgradProb<T, TW> p{g, (const T*)dy, (const TW*)w, bias, scale, (T*)dx, act, alpha, g.N * g.H * g.W, g.C, g.KH * g.KW * g.O};
   dim3 grid((p.Ncols + TN - 1) / TN, (p.M + TM - 1) / TM, 1);
   launch_pdl(simt_gemm_kernel<DgradProb<T, TW>>, dim3(grid), dim3(256), (size_t)(0), s, p, p.K); LAUNCHED();
+  g_gemm_last_kernel = "simt_gemm_kernel<DgradProb>"; g_gemm_last_splits = 1;
 }
 
 void k_simt_fprop(int prec, int wprec, const ConvGeom& g, const void* x, const void* w, const float* bias, void* out, int act, float alpha, cudaStream_t s, const float* scale) {
@@ -199,6 +203,7 @@ void k_simt_wgrad(int prec, const ConvGeom& g, const void* x, const void* dy, fl
   dim3 grid((int)((g.KH * g.KW * g.C + TN - 1) / TN), (g.O + TM - 1) / TM, sp);
   DISPATCH_PREC(prec, T, (launch_pdl(simt_gemm_kernel<WgradProb<T>>, dim3(grid), dim3(256), (size_t)(0), s, WgradProb<T>{g, (const T*)x, (const T*)dy, dst, n, g.O, g.KH * g.KW * g.C, P}, kps))); LAUNCHED();
   if (dst != dw) k_reduce_splits(dst, dw, n, sp, n, accumulate, s);
+  g_gemm_last_kernel = "simt_gemm_kernel<WgradProb>"; g_gemm_last_splits = sp;
 }
 
 }  // namespace b2g

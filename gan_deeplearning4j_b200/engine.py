@@ -483,13 +483,17 @@ EPI_PLAIN, EPI_STATS, EPI_BNBWD, EPI_ACTBWD = 0, 1, 2, 3
 
 def test_conv_ex(ctx: Context, kind: int, geom: Dict[str, int], a, b, out_size: int, *, epi: int = 0, act: str = "identity", alpha: float = 0.0,
                  bias=None, scale=None, groups: int = 1, aux=None, aux2=None, iters: int = 1, impl: int = 1, bn: int = 0, max_ctas: int = 0,
-                 poison: bool = False, w_mn: bool = False, per_tap: bool = False, info: Optional[dict] = None, defer: bool = False, db=None):
+                 poison: bool = False, w_mn: bool = False, per_tap: bool = False, info: Optional[dict] = None, defer: bool = False, db=None,
+                 precision: int = BF16, param_offset: int = 0):
     """Tensor-core fprop (kind 0) / dgrad (kind 1) with the epilogue the training step uses (impl 3, kind 1: the pixel-shuffle deconv, b = the
     [O][4][4][C] weight).  bn forces the 64- / 128-column tile, max_ctas caps the persistent grid (0: production choice for both); poison
-    fills the output with bf16 NaN before every launch; w_mn (kind 0, 1x1): b is the [C][O] dense weight; per_tap keeps a 4x4 s2 p1 shape on
-    one activation box per tap instead of the slabs two taps share.  info, if given, receives "slab": whether the launch used the slabs.
+    fills the output with NaN before every launch; w_mn (kind 0, 1x1): b is the [C][O] dense weight; per_tap keeps a 4x4 s2 p1 shape on
+    one activation box per tap instead of the slabs two taps share.  info, if given, receives "slab": whether the launch used the slabs, and
+    "splits": the split-K count of a SIMT / skinny-layer / dense kernel.
     Weight gradients (kind 2, impl 1 / 3): defer queues the split-K sum and runs it as the backward pass's one reduce-list launch; db (impl 3,
     a float32 array of O elements) receives the bias gradient the edge kernel computes beside dw.
+    The SIMT (impl 0), skinny-layer (impl 2) and dense (impl 4) kernels run in either precision with the bias / scale / activation their
+    production wrapper takes; param_offset puts their fp32 weight operand (FP32) or weight gradient that many elements past an aligned address.
     Returns (out, stats or None, kernel name, ms)."""
     g = _lib.ConvGeom(**geom)
     a, b = _f32(a).ravel(), _f32(b).ravel()
@@ -498,6 +502,7 @@ def test_conv_ex(ctx: Context, kind: int, geom: Dict[str, int], a, b, out_size: 
     o = _lib.TestConvOpts()
     o.epi, o.act, o.alpha, o.groups = epi, ACTS[act], alpha, groups
     o.bn, o.max_ctas, o.poison, o.w_mn, o.per_tap, o.defer = bn, max_ctas, int(poison), int(w_mn), int(per_tap), int(defer)
+    o.param_offset = param_offset
     if db is not None:
         assert db.dtype == np.float32 and db.flags.c_contiguous
         o.db = _fp(db)
@@ -509,9 +514,9 @@ def test_conv_ex(ctx: Context, kind: int, geom: Dict[str, int], a, b, out_size: 
     if epi in (EPI_STATS, EPI_BNBWD):
         stats = np.zeros((groups, 2, oc), np.float64); o.stats = stats.ctypes.data_as(C.POINTER(C.c_double))
     ms = C.c_float()
-    check(ctx.lib.b2g_test_conv_ex(ctx.h, kind, impl, BF16, C.byref(g), _fp(a), _fp(b), _fp(out), iters, C.byref(ms), C.byref(o)))
+    check(ctx.lib.b2g_test_conv_ex(ctx.h, kind, impl, precision, C.byref(g), _fp(a), _fp(b), _fp(out), iters, C.byref(ms), C.byref(o)))
     if info is not None:
-        info["slab"] = bool(o.slab)
+        info["slab"], info["splits"] = bool(o.slab), o.splits
     return out, stats, o.kernel.decode(), ms.value
 
 

@@ -377,6 +377,13 @@ typedef struct {
    * does, instead of reducing right after the wgrad kernel */
   int32_t defer;
   float* db;              /* kind 2, impl 3, C < 4: out [O], the bias gradient (column sums of dy) the edge wgrad kernel produces beside dw; NULL: not asked */
+  /* The SIMT (impl 0), skinny-layer (impl 2) and dense (impl 4) kernels take bias / act / alpha wherever their production wrapper does:
+   * impl 0 kind 0 / 1 (also scale), impl 2 kind 0 / 1, impl 4 kind 0 and kind 1 on the short-reduction kernel; never epi != 0.  poison
+   * applies to them for kinds 0 / 1 / 2 (kind 2: the fp32 dw is filled with 0xFF bytes, fp32 NaN).  `kernel` names the kernel they ran. */
+  int32_t param_offset;   /* impl 0 / 2 / 4: the fp32 weight operand (kinds 0 / 1; FP32 only -- the bf16 operand is a 64-element aligned copy) and the
+                             fp32 weight gradient (kind 2) start this many elements past a 256-byte aligned address, as a layer's W and dW do in the
+                             flattened parameter and gradient vectors */
+  int32_t splits;         /* out, impl 0 / 2 / 4: the number of split-K partial sums the kernel reduced (1 where it has no split) */
 } b2g_test_conv_opts;
 int32_t b2g_test_conv_ex(b2g_ctx* ctx, int32_t kind, int32_t impl, int32_t precision, const b2g_conv_geom* g,
                          const float* x_or_dy, const float* w_or_x, float* out, int32_t iters, float* ms_per_iter, b2g_test_conv_opts* opts);

@@ -48,6 +48,24 @@ def conv2d_input_grad(dy, w, hw, stride=1, pad=0):
     return xp[:, ph:ph + h, pw:pw + wd, :]
 
 
+def conv2d_weight_grad(x, dy, kh, kw, stride=1, pad=0):
+    """Adjoint of conv2d in w: x [N, H, W, C], dy [N, OH, OW, O] -> dw [O, KH, KW, C] = sum over (n, oy, ox) of dy times the input pixel each
+    tap reads (zero in the padding; rows / columns past the last window are read by no tap)."""
+    x = np.asarray(x, np.float64); dy = np.asarray(dy, np.float64)
+    (sh, sw), (ph, pw) = _pair(stride), _pair(pad)
+    n, h, wd, c = x.shape
+    n2, oh, ow, o = dy.shape
+    assert n == n2 and (oh, ow) == (out_size(h, kh, sh, ph), out_size(wd, kw, sw, pw)), (x.shape, dy.shape)
+    xp = np.zeros((n, max(h + 2 * ph, sh * (oh - 1) + kh), max(wd + 2 * pw, sw * (ow - 1) + kw), c))
+    xp[:, ph:ph + h, pw:pw + wd, :] = x
+    dw = np.zeros((o, kh, kw, c))
+    d2 = dy.reshape(-1, o)
+    for i in range(kh):
+        for j in range(kw):
+            dw[:, i, j, :] = d2.T @ xp[:, i:i + sh * (oh - 1) + 1:sh, j:j + sw * (ow - 1) + 1:sw, :].reshape(-1, c)
+    return dw
+
+
 def dense(x, w, w_mn=False):
     """x [N, C] -> [N, O]; w is [O][C] (a 1x1 conv's weight), or [C][O] when w_mn (a dense layer's [nOut][nIn] weight as the operand of its
     input gradient: C = nOut, O = nIn)."""

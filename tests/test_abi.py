@@ -54,6 +54,7 @@ def test_struct_layouts_match_the_c_header(tmp_path):
                     'printf("%zu %zu %zu %zu %zu %zu %zu\\n", sizeof(b2g_test_conv_opts), offsetof(b2g_test_conv_opts,stats), offsetof(b2g_test_conv_opts,kernel),'
                     ' offsetof(b2g_test_conv_opts,bn), offsetof(b2g_test_conv_opts,max_ctas), offsetof(b2g_test_conv_opts,poison), offsetof(b2g_test_conv_opts,w_mn));'
                     'printf("%zu %zu %zu %zu\\n", offsetof(b2g_test_conv_opts,per_tap), offsetof(b2g_test_conv_opts,slab), offsetof(b2g_test_conv_opts,defer), offsetof(b2g_test_conv_opts,db));'
+                    'printf("%zu %zu\\n", offsetof(b2g_test_conv_opts,param_offset), offsetof(b2g_test_conv_opts,splits));'
                     'printf("%zu %zu %zu\\n", sizeof(b2g_ew_reduce_job), offsetof(b2g_ew_reduce_job,splits), offsetof(b2g_ew_reduce_job,wide));'
                     + "".join(f'printf("%zu\\n", offsetof(b2g_test_ew_opts,{f}));' for f, _ in _lib.TestEwOpts._fields_) +
                     'printf("%zu\\n", sizeof(b2g_test_ew_opts));return 0;}')
@@ -63,10 +64,12 @@ def test_struct_layouts_match_the_c_header(tmp_path):
     L, N, T, E, J = _lib.LayerDesc, _lib.NetConfig, _lib.TestConvOpts, _lib.TestEwOpts, _lib.EwReduceJob
     assert got == [C.sizeof(L), L.n_in.offset, L.updater.offset, L.pre_c.offset, C.sizeof(N), N.seed.offset, C.sizeof(_lib.GanConfig), C.sizeof(_lib.ConvGeom), N.bn_groups.offset,
                    C.sizeof(T), T.stats.offset, T.kernel.offset, T.bn.offset, T.max_ctas.offset, T.poison.offset, T.w_mn.offset,
-                   T.per_tap.offset, T.slab.offset, T.defer.offset, T.db.offset, C.sizeof(J), J.splits.offset, J.wide.offset] + \
+                   T.per_tap.offset, T.slab.offset, T.defer.offset, T.db.offset, T.param_offset.offset, T.splits.offset,
+                   C.sizeof(J), J.splits.offset, J.wide.offset] + \
         [getattr(E, f).offset for f, _ in E._fields_] + [C.sizeof(E)]
     assert (T.stats.offset, T.kernel.offset, T.bn.offset, T.slab.offset) == (56, 64, 128, 148)       # the fields older callers fill keep their offsets
     assert (T.defer.offset, T.db.offset) == (152, 160)
+    assert (T.param_offset.offset, T.splits.offset, C.sizeof(T)) == (168, 172, 176)                 # appended after db
 
 
 def test_no_device_fails_loudly_not_silently(lib):

@@ -37,6 +37,36 @@ def test_conv_reference_matches_oracle_conv2d(case):
     np.testing.assert_allclose(got, dx, rtol=1e-12, atol=1e-12)
 
 
+# n, h, w, c, o, (kh, kw), (sh, sw), (ph, pw)
+WGRAD_CASES = [
+    (2, 8, 8, 3, 5, (4, 4), (2, 2), (1, 1)),       # the DCGAN 4x4 s2 p1
+    (2, 9, 11, 4, 3, (3, 5), (1, 2), (0, 2)),      # KH != KW, SH != SW, PH != PW
+    (3, 10, 10, 2, 4, (3, 3), (2, 2), (0, 0)),     # Truncate: the last input row / column is in no window
+    (2, 7, 9, 3, 2, (2, 3), (3, 2), (1, 0)),       # stride > kernel rows, Truncate columns
+    (2, 5, 6, 2, 3, (2, 2), (1, 1), (2, 3)),       # padding >= kernel: border outputs see only padding
+    (3, 1, 1, 7, 5, (1, 1), (1, 1), (0, 0)),       # dense as a 1x1 conv
+]
+
+
+@pytest.mark.parametrize("case", WGRAD_CASES, ids=[f"{c[1]}x{c[2]}_k{c[5][0]}x{c[5][1]}_s{c[6][0]}x{c[6][1]}_p{c[7][0]}x{c[7][1]}" for c in WGRAD_CASES])
+def test_weight_grad_reference_matches_oracle_conv2d(case):
+    """conv2d_weight_grad against the oracle's ConvolutionLayer weight gradient (im2col form), and against conv2d itself: <dy, conv2d(x, w)>
+    is linear in w, so its gradient in w is conv2d_weight_grad(x, dy)."""
+    n, h, w, c, oc, k, s, p = case
+    rng = np.random.default_rng(17)
+    x = rng.standard_normal((n, h, w, c)); wt = rng.standard_normal((oc,) + k + (c,))
+    lay = o.Conv2D(c, oc, k, s, p, has_bias=False); lay.init(np.random.default_rng(0), np.float64)
+    lay.params["W"] = wt.transpose(0, 3, 1, 2).copy()
+    y = lay.forward(x.transpose(0, 3, 1, 2), True).transpose(0, 2, 3, 1)
+    dy = rng.standard_normal(y.shape)
+    lay.backward(dy.transpose(0, 3, 1, 2))
+    got = conv_ref.conv2d_weight_grad(x, dy, k[0], k[1], s, p)
+    assert got.shape == wt.shape
+    np.testing.assert_allclose(got, lay.grads["W"].transpose(0, 2, 3, 1), rtol=1e-12, atol=1e-12)
+    e = np.zeros_like(wt); e.flat[rng.integers(wt.size)] = 1.0
+    np.testing.assert_allclose(np.sum(dy * conv_ref.conv2d(x, e, s, p)), np.sum(got * e), rtol=1e-12, atol=1e-12)
+
+
 def test_dense_reference_both_weight_layouts():
     rng = np.random.default_rng(8)
     x = rng.standard_normal((6, 5)); w = rng.standard_normal((3, 5))
