@@ -89,6 +89,9 @@ struct LayerRT {
   void* out = nullptr; bool out_alias = false;
   void* probs = nullptr;                                       // OUTPUT / LOSS: the output activation of the logits (sigmoid, softmax or loss_act)
   int loss_act = ACT_IDENTITY; float loss_alpha = 0.f;         // OUTPUT / LOSS with loss codes 2-8: the activation the loss applies to z
+  // b2g_activation codes 5-16 (kernels_act.cu): the layer's kind and alpha, moved out of d.act (which then reads identity, so no kernel that takes
+  // codes 0-4 ever sees them); ext_z: a GEMM layer's pre-activation z, from which both f and f' are computed
+  int ext_act = 0; float ext_alpha = 0.f; void* ext_z = nullptr;
   uint8_t* argmax = nullptr;
   float* bn_mean = nullptr; float* bn_invstd = nullptr; float* bn_fold = nullptr;   // bn_fold: [scale | shift] for the inference-mode epilogue fold
   float* bn_coef = nullptr;                                    // fused path: [groups][4][C] = scale, beta, mean, invstd of the latest train-mode forward
@@ -193,10 +196,23 @@ static int32_t take_loss(LayerRT& l) {
   b2g_layer_desc& d = l.d;
   if (d.loss < B2G_LOSS_XENT || d.loss > B2G_LOSS_WASSERSTEIN) return fail(B2G_ERR_ARG, "layer %s: unknown loss %d", d.name, d.loss);
   if (d.loss >= B2G_LOSS_MSE) {
-    if (d.act < B2G_ACT_IDENTITY || d.act > B2G_ACT_LRELU) return fail(B2G_ERR_ARG, "layer %s: unknown activation %d", d.name, d.act);
-    l.loss_act = d.act; l.loss_alpha = d.act_alpha;
+    if (d.act < B2G_ACT_IDENTITY || d.act > B2G_ACT_THRESHOLDEDRELU) return fail(B2G_ERR_ARG, "layer %s: unknown activation %d", d.name, d.act);
+    l.loss_act = d.act; l.loss_alpha = d.act_alpha;      // identity for codes 5-16 (take_act cleared d.act): net_loss applies ext_act
   }
   if (d.type == B2G_LAYER_OUTPUT) d.act = B2G_ACT_IDENTITY;
+  return 0;
+}
+// Layers whose activation is b2g_layer_desc.act: checks the code, and moves a code of 5-16 into ext_act / ext_alpha (d.act becomes identity).
+static int32_t take_act(LayerRT& l) {
+  b2g_layer_desc& d = l.d;
+  const bool lossy = d.type == B2G_LAYER_OUTPUT || d.type == B2G_LAYER_LOSS;
+  const bool has_act = d.type == B2G_LAYER_CONV2D || d.type == B2G_LAYER_DECONV2D || d.type == B2G_LAYER_DENSE || d.type == B2G_LAYER_ACTIVATION ||
+                       (lossy && d.loss >= B2G_LOSS_MSE && d.loss <= B2G_LOSS_WASSERSTEIN);
+  if (!has_act) return 0;
+  if (d.act < B2G_ACT_IDENTITY || d.act > B2G_ACT_THRESHOLDEDRELU) return fail(B2G_ERR_ARG, "layer %s: unknown activation %d", d.name, d.act);
+  if (!act_ext_kind(d.act)) return 0;
+  if (!std::isfinite(d.act_alpha)) return fail(B2G_ERR_ARG, "layer %s: activation %d needs a finite act_alpha, not %g", d.name, d.act, (double)d.act_alpha);
+  l.ext_act = d.act; l.ext_alpha = d.act_alpha; d.act = B2G_ACT_IDENTITY;
   return 0;
 }
 static int32_t net_build(b2g_net* n, const b2g_layer_desc* layers, int32_t nl) {
@@ -209,6 +225,7 @@ static int32_t net_build(b2g_net* n, const b2g_layer_desc* layers, int32_t nl) {
     l.ih = h; l.iw = w; l.ic = ch; l.in_elems = (size_t)h * w * ch;
     b2g_layer_desc& d = l.d;
     if (d.has_bias < 0) d.has_bias = 1;
+    B2(take_act(l));
     switch (d.type) {
       case B2G_LAYER_CONV2D: {
         if (d.n_in == 0) d.n_in = ch; if (d.n_in != ch) return fail(B2G_ERR_SHAPE, "layer %s: nIn %d != incoming channels %d", d.name, d.n_in, ch);
@@ -284,9 +301,9 @@ static int32_t net_build(b2g_net* n, const b2g_layer_desc* layers, int32_t nl) {
     h = l.oh; w = l.ow; ch = l.oc;
     n->L.push_back(l);
   }
-  // fuse BatchNormalization + ActivationLayer (north_star's BN+ReLU / BN+LeakyReLU)
+  // fuse BatchNormalization + ActivationLayer (north_star's BN+ReLU / BN+LeakyReLU); an ActivationLayer of codes 5-16 runs its own kernels
   for (size_t i = 0; i + 1 < n->L.size(); ++i)
-    if (n->L[i].d.type == B2G_LAYER_BATCHNORM && n->L[i + 1].d.type == B2G_LAYER_ACTIVATION) {
+    if (n->L[i].d.type == B2G_LAYER_BATCHNORM && n->L[i + 1].d.type == B2G_LAYER_ACTIVATION && !n->L[i + 1].ext_act) {
       n->L[i].fused_act = n->L[i + 1].d.act; n->L[i].fused_alpha = n->L[i + 1].d.act_alpha; n->L[i + 1].act_fused_into_prev = true;
     }
   int last = n->L.back().d.type;
@@ -323,6 +340,7 @@ static int32_t net_alloc(b2g_net* n) {
     if (!alias) B2(dalloc(n, (char**)&l.out, ts * R * l.out_elems));
     if (l.d.type == B2G_LAYER_DROPOUT) { l.drop_buf = l.out; B2(dalloc(n, &l.drop_mask, sizeof(uint32_t) * (((size_t)R * l.out_elems + 31) / 32))); }
     if (l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS) B2(dalloc(n, (char**)&l.probs, ts * R * l.out_elems));
+    if (l.ext_act && l.has_gemm() && l.d.type != B2G_LAYER_OUTPUT) B2(dalloc(n, (char**)&l.ext_z, ts * R * l.out_elems));
     if (l.d.type == B2G_LAYER_MAXPOOL) B2(dalloc(n, &l.argmax, (size_t)R * l.out_elems));
     if (l.d.type == B2G_LAYER_BATCHNORM) { B2(dalloc(n, &l.bn_fold, sizeof(float) * 2 * l.oc)); B2(dalloc(n, &l.bn_mean, sizeof(float) * G * l.oc)); B2(dalloc(n, &l.bn_invstd, sizeof(float) * G * l.oc)); scratch = std::max(scratch, k_bn_scratch_floats(l.oc, G));
       if (k_bn_vec_ok(n->prec, l.oc)) { B2(dalloc(n, &l.bn_coef, sizeof(float) * 4 * G * l.oc)); bn_acc_words += 2 * k_bn_acc_elems(l.oc, G); } }
@@ -573,7 +591,7 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
     // a 1x1-input deconv is computed as the 1x1 problem with taps*C output channels: its columns are not the BatchNorm's channels
     const bool remapped = d.type == B2G_LAYER_DECONV2D && l.geom.KH == 1 && l.geom.C != l.oc;
     // inference-mode (or frozen) BatchNorm right after a linear conv / deconv / dense: fold it, and its activation, into that GEMM's epilogue
-    if (gemm_then_bn && d.act == B2G_ACT_IDENTITY && (!o.train || n->L[i + 1].d.frozen) && !(i + 2 == n->L.size() && o.out_override) && !remapped) {
+    if (gemm_then_bn && d.act == B2G_ACT_IDENTITY && !l.ext_act && (!o.train || n->L[i + 1].d.frozen) && !(i + 2 == n->L.size() && o.out_override) && !remapped) {
       LayerRT& bn = n->L[i + 1];
       ConvGeom g = l.geom; g.N = R;
       k_bn_fold(n->params + bn.off_mean, n->params + bn.off_var, n->params + bn.off_gamma, n->params + bn.off_beta, bias, bn.oc, bn.d.bn_eps, bn.bn_fold, bn.bn_fold + bn.oc, s);
@@ -583,12 +601,15 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
     }
     // train-mode BatchNorm right after a GEMM: its batch statistics come out of the GEMM's epilogue (kernels_tc.cu EPI_STATS)
     TcEpi st{}; const TcEpi* fuse = nullptr; bool fused = false;
-    if (gemm_then_bn && o.train && !n->L[i + 1].d.frozen && n->L[i + 1].bn_coef && !remapped && tc_on(n)) {
+    // (not after an activation of codes 5-16: the BatchNorm's input is then a = f(z), not the GEMM's z)
+    if (gemm_then_bn && o.train && !n->L[i + 1].d.frozen && n->L[i + 1].bn_coef && !remapped && tc_on(n) && !l.ext_act) {
       st.mode = EPI_STATS; st.acc = n->L[i + 1].acc_fwd; st.imgs_per_group = R / o.groups; fuse = &st;
     }
+    // a GEMM layer with an activation of codes 5-16: the GEMM (identity epilogue) writes z into ext_z, then a = f(z)
+    void* gout = l.ext_z ? l.ext_z : out;
     switch (d.type) {
-      case B2G_LAYER_CONV2D: case B2G_LAYER_DENSE: case B2G_LAYER_OUTPUT: { ConvGeom g = l.geom; g.N = R; B2(gemm_fprop(n, l, g, cur, bias, out, d.act, d.act_alpha, nullptr, fuse, &fused)); } break;
-      case B2G_LAYER_DECONV2D: { ConvGeom g = l.geom; g.N = R; B2(gemm_dgrad(n, l, g, cur, bias, out, d.act, d.act_alpha, nullptr, fuse, &fused)); } break;
+      case B2G_LAYER_CONV2D: case B2G_LAYER_DENSE: case B2G_LAYER_OUTPUT: { ConvGeom g = l.geom; g.N = R; B2(gemm_fprop(n, l, g, cur, bias, gout, d.act, d.act_alpha, nullptr, fuse, &fused)); } break;
+      case B2G_LAYER_DECONV2D: { ConvGeom g = l.geom; g.N = R; B2(gemm_dgrad(n, l, g, cur, bias, gout, d.act, d.act_alpha, nullptr, fuse, &fused)); } break;
       case B2G_LAYER_BATCHNORM: {
         int rows_pg = (R / o.groups) * l.oh * l.ow;
         const bool bn_train = o.train && !d.frozen;      // FrozenLayer always activates in test mode
@@ -607,7 +628,11 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
         else k_bn_prep_infer(n->params + l.off_mean, n->params + l.off_var, l.oc, o.groups, d.bn_eps, l.bn_mean, l.bn_invstd, s);
         k_bn_apply(n->prec, cur, out, rows_pg, l.oc, o.groups, l.bn_mean, l.bn_invstd, n->params + l.off_gamma, n->params + l.off_beta, l.fused_act, l.fused_alpha, s);
       } break;
-      case B2G_LAYER_ACTIVATION: if (l.act_fused_into_prev) out = (void*)cur; else k_act_fwd(n->prec, cur, out, (size_t)R * l.out_elems, d.act, d.act_alpha, s); break;
+      case B2G_LAYER_ACTIVATION:
+        if (l.act_fused_into_prev) out = (void*)cur;
+        else if (l.ext_act) k_act_ext_fwd(n->prec, l.ext_act, l.ext_alpha, cur, out, (size_t)R * l.out_elems, s);
+        else k_act_fwd(n->prec, cur, out, (size_t)R * l.out_elems, d.act, d.act_alpha, s);
+        break;
       case B2G_LAYER_MAXPOOL: k_maxpool_fwd(n->prec, cur, out, l.argmax, R, l.ih, l.iw, l.ic, l.oh, l.ow, d.k_h, d.k_w, d.s_h, d.s_w, s); break;
       case B2G_LAYER_UPSAMPLE2D: k_upsample_fwd(n->prec, cur, out, R, l.ih, l.iw, l.ic, d.k_h, s); break;
       case B2G_LAYER_LOSS: out = (void*)cur; break;
@@ -622,6 +647,7 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
         l.out = out;
         break;
     }
+    if (l.ext_z) k_act_ext_fwd(n->prec, l.ext_act, l.ext_alpha, l.ext_z, out, (size_t)R * l.out_elems, s);
     if (fuse) n->L[i + 1].stats_by_producer = fused;
     if (l.out_alias) l.out = out;
     cur = out;
@@ -704,6 +730,7 @@ static int32_t net_backward(b2g_net* n, const void* net_in, void* eps, int rows,
       case B2G_LAYER_CONV2D: case B2G_LAYER_DENSE: case B2G_LAYER_OUTPUT: {
         ConvGeom g = l.geom; g.N = R;
         if (d.act != B2G_ACT_IDENTITY && !act_done[i]) k_act_bwd_from_output(n->prec, l.out, cur, cur, (size_t)R * l.out_elems, d.act, d.act_alpha, s);
+        if (l.ext_z) k_act_ext_bwd(n->prec, l.ext_act, l.ext_alpha, l.ext_z, cur, (size_t)R * l.out_elems, s);
         if (want_wgrad_l) {
           fork_wgrad(i, cur);
           bool bias_done = false;
@@ -717,6 +744,7 @@ static int32_t net_backward(b2g_net* n, const void* net_in, void* eps, int rows,
       case B2G_LAYER_DECONV2D: {
         ConvGeom g = l.geom; g.N = R;
         if (d.act != B2G_ACT_IDENTITY && !act_done[i]) k_act_bwd_from_output(n->prec, l.out, cur, cur, (size_t)R * l.out_elems, d.act, d.act_alpha, s);
+        if (l.ext_z) k_act_ext_bwd(n->prec, l.ext_act, l.ext_alpha, l.ext_z, cur, (size_t)R * l.out_elems, s);
         if (want_wgrad_l) {
           fork_wgrad(i, cur);
           B2(gemm_wgrad(n, l, g, /*conv input = deconv out grad*/ cur, /*conv dy = deconv input*/ lin, n->grads + l.off_W, s2, n->scratch2));
@@ -745,7 +773,10 @@ static int32_t net_backward(b2g_net* n, const void* net_in, void* eps, int rows,
                  n->scratch, n->grads + l.off_gamma, n->grads + l.off_beta, want_wgrad_l ? 1 : 0, s);
         if (need_in) cur = nx;
       } break;
-      case B2G_LAYER_ACTIVATION: if (!l.act_fused_into_prev) k_act_bwd_from_output(n->prec, l.out, cur, cur, (size_t)R * l.out_elems, d.act, d.act_alpha, s); break;
+      case B2G_LAYER_ACTIVATION:
+        if (l.ext_act) k_act_ext_bwd(n->prec, l.ext_act, l.ext_alpha, lin, cur, (size_t)R * l.out_elems, s);      // z = the layer's input
+        else if (!l.act_fused_into_prev) k_act_bwd_from_output(n->prec, l.out, cur, cur, (size_t)R * l.out_elems, d.act, d.act_alpha, s);
+        break;
       case B2G_LAYER_MAXPOOL: if (need_in) { void* nx = other(cur); k_maxpool_bwd(n->prec, cur, l.argmax, nx, R, l.ih, l.iw, l.ic, l.oh, l.ow, d.k_h, d.k_w, d.s_h, d.s_w, s); cur = nx; } break;
       case B2G_LAYER_UPSAMPLE2D: if (need_in) { void* nx = other(cur); k_upsample_bwd(n->prec, cur, nx, R, l.ih, l.iw, l.ic, d.k_h, s); cur = nx; } break;
       case B2G_LAYER_FF_TO_CNN: if (!l.out_alias && need_in) { void* nx = other(cur); k_permute(n->prec, cur, nx, R, l.oc, l.oh * l.ow, 0, s); cur = nx; } break;
@@ -990,7 +1021,8 @@ extern "C" int32_t b2g_net_output(b2g_net* n, const float* x, int32_t batch, int
   LayerRT& l = n->L.back();
   if (l.d.type == B2G_LAYER_OUTPUT && l.d.loss == B2G_LOSS_MCXENT) { k_softmax_xent(n->prec, res, nullptr, nullptr, l.probs, nullptr, batch, l.oc, n->ctx->stream); res = l.probs; }
   else if ((l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS) && l.d.loss >= B2G_LOSS_MSE) {      // a = act(z); identity: the logits themselves
-    if (l.loss_act != ACT_IDENTITY) { k_act_fwd(n->prec, res, l.probs, (size_t)batch * l.out_elems, l.loss_act, l.loss_alpha, n->ctx->stream); res = l.probs; }
+    if (l.ext_act) { k_act_ext_fwd(n->prec, l.ext_act, l.ext_alpha, res, l.probs, (size_t)batch * l.out_elems, n->ctx->stream); res = l.probs; }
+    else if (l.loss_act != ACT_IDENTITY) { k_act_fwd(n->prec, res, l.probs, (size_t)batch * l.out_elems, l.loss_act, l.loss_alpha, n->ctx->stream); res = l.probs; }
   }
   else if (l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS) { k_sigmoid_out(n->prec, res, l.probs, (size_t)batch * l.out_elems, n->ctx->stream); res = l.probs; }
   return download_act(n, res, batch, l.oc, l.oh * l.ow, out);
@@ -1009,6 +1041,12 @@ static void net_loss(b2g_net* n, const void* logits, const float* labels, void* 
   const int loss = (l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS) ? l.d.loss : B2G_LOSS_XENT;
   if (loss == B2G_LOSS_MCXENT) k_softmax_xent(n->prec, logits, labels, dz, nullptr, loss_sums, rows_per_group * groups, l.oc, n->ctx->stream);
   else if (loss == B2G_LOSS_XENT) k_xent(n->prec, logits, labels, dz, loss_sums, rows_per_group, groups, n->cfg.xent_clip_eps, n->ctx->stream);
+  else if (l.ext_act) {      // activation of codes 5-16: a = f(z) into probs, the loss on a with the identity, then dL/dz = dL/da * f'(z)
+    const size_t cnt = (size_t)rows_per_group * groups * l.out_elems;
+    k_act_ext_fwd(n->prec, l.ext_act, l.ext_alpha, logits, l.probs, cnt, n->ctx->stream);
+    k_loss(n->prec, loss, ACT_IDENTITY, 0.f, l.probs, labels, dz, loss_sums, rows_per_group, (int)l.out_elems, groups, n->loss_partial, n->loss_ticket, n->ctx->stream);
+    k_act_ext_bwd(n->prec, l.ext_act, l.ext_alpha, logits, dz, cnt, n->ctx->stream);
+  }
   else k_loss(n->prec, loss, l.loss_act, l.loss_alpha, logits, labels, dz, loss_sums, rows_per_group, (int)l.out_elems, groups, n->loss_partial, n->loss_ticket, n->ctx->stream);
 }
 static int32_t train_pass(b2g_net* n, const float* x, const float* y, int batch, bool do_update, float* score) {
@@ -1800,6 +1838,18 @@ extern "C" int32_t b2g_test_ew(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* 
       else { B2(dev(n, ts, &r)); B2(poison(r, ts * n)); }
       if (bwd) k_act_bwd_from_output(prec, a, e, r, n, o->act, o->alpha, s);      // in place: eps_in == eps_out, as the backward pass calls it
       else k_act_fwd(prec, a, r, n, o->act, o->alpha, s);
+      ran();
+      B2(downT(out0, r, n));
+      break;
+    }
+    case B2G_EW_ACT_EXT_FWD: case B2G_EW_ACT_EXT_BWD: {
+      const size_t n = (size_t)o->n; const bool bwd = o->op == B2G_EW_ACT_EXT_BWD;
+      if (!in0 || (bwd && !in1) || o->n < 1 || o->n > lim || !act_ext_kind(o->act) || !std::isfinite(o->alpha)) return fail(B2G_ERR_ARG, "bad activation arguments");
+      void *z = nullptr, *r = nullptr; B2(upT(in0, n, &z));
+      if (bwd) B2(upT(in1, n, &r));      // eps_out, overwritten in place with eps_in
+      else { B2(dev(n, ts, &r)); B2(poison(r, ts * n)); }
+      if (bwd) k_act_ext_bwd(prec, o->act, o->alpha, z, r, n, s);
+      else k_act_ext_fwd(prec, o->act, o->alpha, z, r, n, s);
       ran();
       B2(downT(out0, r, n));
       break;

@@ -10,7 +10,10 @@
 namespace b2g {
 
 enum Prec { PREC_F32 = 0, PREC_BF16 = 1 };
-enum Act { ACT_IDENTITY = 0, ACT_TANH = 1, ACT_SIGMOID = 2, ACT_RELU = 3, ACT_LRELU = 4 };
+enum Act { ACT_IDENTITY = 0, ACT_TANH = 1, ACT_SIGMOID = 2, ACT_RELU = 3, ACT_LRELU = 4,
+           // kernels_act.cu only: the GEMM epilogues, BatchNorm, loss and act_* kernels take codes 0-4 and treat any other code as identity
+           ACT_ELU = 5, ACT_SELU = 6, ACT_SOFTPLUS = 7, ACT_SOFTSIGN = 8, ACT_HARDTANH = 9, ACT_HARDSIGMOID = 10, ACT_RELU6 = 11, ACT_SWISH = 12,
+           ACT_CUBE = 13, ACT_RATIONALTANH = 14, ACT_RECTIFIEDTANH = 15, ACT_THRESHOLDEDRELU = 16, ACT_EXT_FIRST = ACT_ELU, ACT_EXT_LAST = ACT_THRESHOLDEDRELU };
 enum Loss { LOSS_MSE = 2, LOSS_L1 = 3, LOSS_L2 = 4, LOSS_MAE = 5, LOSS_HINGE = 6, LOSS_SQUARED_HINGE = 7, LOSS_WASSERSTEIN = 8 };   // b2g_loss
 
 inline size_t prec_size(int prec) { return prec == PREC_F32 ? 4 : 2; }
@@ -80,6 +83,11 @@ void k_bn_bwd_apply_acc(const void* x, const void* eps_out, void* eps_in, int ro
 void k_act_fwd(int prec, const void* x, void* y, size_t n, int act, float alpha, cudaStream_t s);
 // eps_in = eps_out * f'(.) evaluated from the layer OUTPUT a (tanh: 1-a^2, sigmoid: a(1-a), relu/lrelu: sign of a)
 void k_act_bwd_from_output(int prec, const void* a, const void* eps_out, void* eps_in, size_t n, int act, float alpha, cudaStream_t s);
+// b2g_activation codes 5-16 (kernels_act.cu; formulas in include/b200gan.h), one instantiation per kind: a = f(z); eps = eps * f'(z) in place.
+// alpha = ELU's alpha / ThresholdedReLU's theta.  A code outside 5-16 launches nothing.
+bool act_ext_kind(int act);
+void k_act_ext_fwd(int prec, int act, float alpha, const void* z, void* a, size_t n, cudaStream_t s);
+void k_act_ext_bwd(int prec, int act, float alpha, const void* z, void* eps, size_t n, cudaStream_t s);
 void k_maxpool_fwd(int prec, const void* x, void* y, uint8_t* argmax, int N, int H, int W, int C, int OH, int OW, int KH, int KW, int SH, int SW, cudaStream_t s);
 void k_maxpool_bwd(int prec, const void* eps_out, const uint8_t* argmax, void* eps_in, int N, int H, int W, int C, int OH, int OW, int KH, int KW, int SH, int SW, cudaStream_t s);
 void k_upsample_fwd(int prec, const void* x, void* y, int N, int H, int W, int C, int f, cudaStream_t s);

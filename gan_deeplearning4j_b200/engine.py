@@ -18,7 +18,11 @@ from ._lib import GanConfig, LayerDesc, LrSchedule, NetConfig, check
 
 LAYER_TYPES = {"conv2d": 0, "deconv2d": 1, "batchnorm": 2, "dense": 3, "activation": 4, "maxpool": 5, "upsample2d": 6,
                "output": 7, "loss": 8, "ff_to_cnn": 9, "cnn_to_ff": 10, "dropout": 11}
-ACTS = {"identity": 0, "tanh": 1, "sigmoid": 2, "relu": 3, "lrelu": 4}
+# org.nd4j.linalg.activations.Activation -> b2g_activation (codes 5-16: formulas at b2g_activation in include/b200gan.h)
+ACTS = {"identity": 0, "tanh": 1, "sigmoid": 2, "relu": 3, "lrelu": 4, "elu": 5, "selu": 6, "softplus": 7, "softsign": 8, "hardtanh": 9,
+        "hardsigmoid": 10, "relu6": 11, "swish": 12, "cube": 13, "rationaltanh": 14, "rectifiedtanh": 15, "thresholdedrelu": 16}
+# the spec's "alpha" when it has none: LeakyReLU's alpha 0.01, ELU's alpha and ThresholdedReLU's theta 1.0 (DL4J's defaults)
+ACT_ALPHA_DEFAULTS = {"elu": 1.0, "thresholdedrelu": 1.0}
 # LossFunctions.LossFunction -> b2g_loss.  XENT / MCXENT imply their sigmoid / softmax; the others apply the spec's "activation" (b2g_loss)
 LOSSES = {"xent": 0, "mcxent": 1, "mse": 2, "l1": 3, "l2": 4, "mae": 5, "hinge": 6, "squared_hinge": 7, "wasserstein": 8}
 UPDATERS = {"sgd": 0, "rmsprop": 1, "adam": 2, "noop": 3, "nesterovs": 4, "adagrad": 5, "adamax": 6, "nadam": 7, "amsgrad": 8, "adadelta": 9}
@@ -122,8 +126,9 @@ def layer_desc(spec: Dict) -> LayerDesc:
         k = (spec.get("size", 2), spec.get("size", 2))
     d.k_h, d.k_w, d.s_h, d.s_w, d.p_h, d.p_w = k[0], k[1], s[0], s[1], p[0], p[1]
     d.has_bias = 1 if spec.get("has_bias", True) else 0
-    d.act = ACTS[spec.get("activation", "identity")]
-    d.act_alpha = spec.get("alpha", 0.01)
+    act = spec.get("activation", "identity")
+    d.act = ACTS[act]
+    d.act_alpha = spec.get("alpha", ACT_ALPHA_DEFAULTS.get(act, 0.01))
     if spec["type"] == "dropout":       # DropoutLayer.Builder(p): p = retain probability, carried in act_alpha
         d.act_alpha = spec["p"]
     u = spec.get("updater") or {"kind": "sgd", "lr": 0.0}
@@ -550,12 +555,13 @@ def test_dropout(ctx: Context, precision: int, x, dy, p: float, *, seed: int = 6
 
 
 EW_OPS = {"reduce_splits": 0, "reduce_multi": 1, "colsum": 2, "xent": 3, "softmax_xent": 4, "act_fwd": 5, "act_bwd": 6, "maxpool": 7,
-          "upsample": 8, "sumsq": 9, "loss": 10}
+          "upsample": 8, "sumsq": 9, "loss": 10, "act_ext_fwd": 11, "act_ext_bwd": 12}
 
 
 def test_ew(ctx: Context, precision: int, op: str, in0, in1=None, out_sizes=(0, 0, 0), *, act: str = "identity", jobs=None, segments=None,
             loss: str = "xent", **opts):
     """One reduction / loss / element-wise kernel through its production wrapper (b2g_test_ew; operands per op in include/b200gan.h).
+    act_ext_fwd / act_ext_bwd (act: a name of codes 5-16): in0 = z, in1 = eps_out, out0 = f(z) / eps_out * f'(z).
     out_sizes: element counts of out0..out2 (0: not asked for).  opts: the b2g_test_ew_opts sizes and switches (n, rows, cols, groups, splits,
     stride, N, H, W, C, KH, KW, SH, SW, alpha, clip_eps, offset, in_place, accumulate, poison).  jobs (reduce_multi): dicts of n, splits,
     stride, src_off, dst_off.  segments (sumsq): (offsets, lengths, coefficients).  loss (op "loss"): a LOSSES name of codes 2-8.

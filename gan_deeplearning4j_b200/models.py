@@ -132,19 +132,28 @@ def reference_computer_vision(lr=0.002, n_classes=10) -> List[Dict]:
 
 
 # ------------------------------------------------------------------ C2-C4: DCGAN -----------------------
-def dcgan_generator(size=64, z=100, nf=64, nc=3, lr=2e-4, beta1=0.5) -> List[Dict]:
-    """ConvolutionTranspose2D(4x4)+BatchNorm+ReLU stack, tanh output (SURVEY.md Appendix B).  Input (z,)."""
+def _act(activation, alpha=None) -> Dict:
+    """The spec keys of an activation: LeakyReLU carries its alpha (0.2 when not given, the DCGAN value); another kind carries alpha only when
+    one is given (engine.layer_desc then fills DL4J's default)."""
+    if activation == "lrelu" and alpha is None:
+        alpha = 0.2
+    return {"activation": activation} if alpha is None else {"activation": activation, "alpha": alpha}
+
+
+def dcgan_generator(size=64, z=100, nf=64, nc=3, lr=2e-4, beta1=0.5, activation="relu", out_activation="tanh", alpha=None) -> List[Dict]:
+    """ConvolutionTranspose2D(4x4)+BatchNorm+ReLU stack, tanh output (SURVEY.md Appendix B).  Input (z,).
+    activation: the ActivationLayers' kind (any engine.ACTS name; alpha as in _act), out_activation: the last deconv's."""
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
     n_up = int(math.log2(size)) - 2
     ch = nf * 2 ** (n_up - 1)
     L = [{"type": "ff_to_cnn", "name": "gen_ff2cnn", "to": (1, 1, z)},
          {"type": "deconv2d", "name": "gen_deconv_1", "n_in": z, "n_out": ch, "kernel": (4, 4), "stride": (1, 1), "padding": (0, 0), "has_bias": False, "updater": u()},
-         {"type": "batchnorm", "name": "gen_bn_1", "updater": u()}, {"type": "activation", "name": "gen_act_1", "activation": "relu"}]
+         {"type": "batchnorm", "name": "gen_bn_1", "updater": u()}, dict({"type": "activation", "name": "gen_act_1"}, **_act(activation, alpha))]
     for i in range(n_up - 1):
         L += [{"type": "deconv2d", "name": f"gen_deconv_{i + 2}", "n_in": ch, "n_out": ch // 2, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "has_bias": False, "updater": u()},
-              {"type": "batchnorm", "name": f"gen_bn_{i + 2}", "updater": u()}, {"type": "activation", "name": f"gen_act_{i + 2}", "activation": "relu"}]
+              {"type": "batchnorm", "name": f"gen_bn_{i + 2}", "updater": u()}, dict({"type": "activation", "name": f"gen_act_{i + 2}"}, **_act(activation, alpha))]
         ch //= 2
-    L += [{"type": "deconv2d", "name": f"gen_deconv_{n_up + 1}", "n_in": ch, "n_out": nc, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "activation": "tanh", "updater": u()}]
+    L += [{"type": "deconv2d", "name": f"gen_deconv_{n_up + 1}", "n_in": ch, "n_out": nc, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "updater": u(), **_act(out_activation)}]
     return L
 
 
@@ -157,16 +166,17 @@ def _loss_keys(loss, out_activation) -> Dict:
     return {"loss": loss, "activation": out_activation}
 
 
-def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", out_activation="identity") -> List[Dict]:
+def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", out_activation="identity", activation="lrelu", alpha=None) -> List[Dict]:
     """Conv(4x4 s2 p1)+LeakyReLU(0.2); (Conv+BatchNorm+LeakyReLU)*; Conv(4x4 s1 p0) -> logit; LossLayer(loss).  Input (nc,size,size).
-    loss: "xent" (sigmoid implied), or "mse" (least-squares GAN), "hinge", "wasserstein", ... applied to out_activation(logit)."""
+    loss: "xent" (sigmoid implied), or "mse" (least-squares GAN), "hinge", "wasserstein", ... applied to out_activation(logit).
+    activation / alpha: the hidden activation in place of LeakyReLU(0.2) (as in _act)."""
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
     n_down = int(math.log2(size)) - 2
-    L = [{"type": "conv2d", "name": "dis_conv_1", "n_in": nc, "n_out": nf, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "activation": "lrelu", "alpha": 0.2, "updater": u()}]
+    L = [{"type": "conv2d", "name": "dis_conv_1", "n_in": nc, "n_out": nf, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), **_act(activation, alpha), "updater": u()}]
     ch = nf
     for i in range(n_down - 1):
         L += [{"type": "conv2d", "name": f"dis_conv_{i + 2}", "n_in": ch, "n_out": ch * 2, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "has_bias": False, "updater": u()},
-              {"type": "batchnorm", "name": f"dis_bn_{i + 2}", "updater": u()}, {"type": "activation", "name": f"dis_act_{i + 2}", "activation": "lrelu", "alpha": 0.2}]
+              {"type": "batchnorm", "name": f"dis_bn_{i + 2}", "updater": u()}, dict({"type": "activation", "name": f"dis_act_{i + 2}"}, **_act(activation, alpha))]
         ch *= 2
     L += [{"type": "conv2d", "name": f"dis_conv_{n_down + 1}", "n_in": ch, "n_out": 1, "kernel": (4, 4), "stride": (1, 1), "padding": (0, 0), "updater": u()},
           dict({"type": "loss", "name": "dis_loss"}, **_loss_keys(loss, out_activation))]
@@ -174,20 +184,22 @@ def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", o
 
 
 # ------------------------------------------------------------------ C5: MLP-GAN --------------------------
-def mlp_generator(z=100, hidden=1024, d=256, lr=2e-4, beta1=0.5) -> List[Dict]:
+def mlp_generator(z=100, hidden=1024, d=256, lr=2e-4, beta1=0.5, activation="relu", out_activation="tanh", alpha=None) -> List[Dict]:
+    """activation / alpha: the hidden layers' activation (as in _act); out_activation: the last layer's."""
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
-    return [{"type": "dense", "name": "gen_dense_1", "n_out": hidden, "activation": "relu", "updater": u()},
-            {"type": "dense", "name": "gen_dense_2", "n_out": hidden, "activation": "relu", "updater": u()},
-            {"type": "dense", "name": "gen_dense_3", "n_out": d, "activation": "tanh", "updater": u()}]
+    return [{"type": "dense", "name": "gen_dense_1", "n_out": hidden, **_act(activation, alpha), "updater": u()},
+            {"type": "dense", "name": "gen_dense_2", "n_out": hidden, **_act(activation, alpha), "updater": u()},
+            {"type": "dense", "name": "gen_dense_3", "n_out": d, **_act(out_activation), "updater": u()}]
 
 
-def mlp_discriminator(d=256, hidden=1024, lr=2e-4, beta1=0.5, dropout=None, loss="xent", out_activation="identity") -> List[Dict]:
+def mlp_discriminator(d=256, hidden=1024, lr=2e-4, beta1=0.5, dropout=None, loss="xent", out_activation="identity", activation="lrelu",
+                      alpha=None) -> List[Dict]:
     """dropout = p: a DropoutLayer(p) (p = retain probability) after each hidden LeakyReLU, the DL4J MNIST GAN example's discriminator shape.
-    loss / out_activation: the OutputLayer's loss, as for dcgan_discriminator."""
+    loss / out_activation: the OutputLayer's loss, as for dcgan_discriminator.  activation / alpha: the hidden activation (as in _act)."""
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
     L = []
     for i in (1, 2):
-        L.append({"type": "dense", "name": f"dis_dense_{i}", "n_out": hidden, "activation": "lrelu", "alpha": 0.2, "updater": u()})
+        L.append({"type": "dense", "name": f"dis_dense_{i}", "n_out": hidden, **_act(activation, alpha), "updater": u()})
         if dropout is not None:
             L.append({"type": "dropout", "name": f"dis_dropout_{i}", "p": dropout})
     return L + [dict({"type": "output", "name": "dis_output", "n_out": 1, "updater": u()}, **_loss_keys(loss, out_activation))]

@@ -80,8 +80,35 @@ typedef enum {
  * masks); other forwards leave it unchanged.  In the GAN step D's real|fake pass (2N rows) uses P and the generator step's D pass P + 1.
  * A pass may hold at most 2^34 elements (max_batch * layer size; B2G_ERR_UNSUPPORTED at b2g_net_create). */
 
-typedef enum {               /* org.nd4j.linalg.activations.Activation  J:126,162,215 */
-  B2G_ACT_IDENTITY = 0, B2G_ACT_TANH = 1, B2G_ACT_SIGMOID = 2, B2G_ACT_RELU = 3, B2G_ACT_LRELU = 4
+/* org.nd4j.linalg.activations.Activation  J:126,162,215.  Codes 0-4 as DL4J; LRELU's alpha = b2g_layer_desc.act_alpha.
+ * Codes 5-16 (DL4J 1.0.0-beta3 org.nd4j.linalg.activations.impl.*, recalled; parity unpinned like the rest of the DL4J semantics).  f and f' are
+ * computed in fp32 from the pre-activation z as stored (bf16 in a BF16 net: the GEMM's z is rounded once before f) with expf / expm1f / log1pf /
+ * tanhf, and the result is rounded once to the activation type.  The derivative is taken from z, as IActivation.backprop(in, epsilon) takes it:
+ *   ELU (5)             z >= 0 ? z : a*expm1(z)                           f' = z >= 0 ? 1 : a*e^z                    a = act_alpha (DL4J 1.0)
+ *   SELU (6)            l*(z > 0 ? z : s*expm1(z))                        f' = z > 0 ? l : l*s*e^z       l = 1.0507009873554805, s = 1.6732632423543772
+ *   SOFTPLUS (7)        max(z, 0) + log1p(e^-|z|)                         f' = sigmoid(z)
+ *   SOFTSIGN (8)        z / (1 + |z|)                                     f' = 1 / (1 + |z|)^2
+ *   HARDTANH (9)        min(1, max(-1, z))                                f' = 1 on -1 <= z <= 1, else 0
+ *   HARDSIGMOID (10)    min(1, max(0, 0.2z + 0.5))                        f' = 0.2 on -2.5 <= z <= 2.5, else 0
+ *   RELU6 (11)          min(max(z, 0), 6)                                 f' = 1 on 0 < z < 6, else 0
+ *   SWISH (12)          z*sigmoid(z)                                      f' = s*(1 + z*(1 - s)), s = sigmoid(z)
+ *   CUBE (13)           z^3                                               f' = 3z^2
+ *   RATIONALTANH (14)   y = 2z/3, A = 1 + |y| + y^2 + 1.41645*y^4:  1.7159*sgn(y)*(1 - 1/A)
+ *                                                                         f' = 1.7159*(2/3)*(1 + sgn(y)*(2y + 4*1.41645*y^3)) / A^2
+ *   RECTIFIEDTANH (15)  max(0, tanh z)                                    f' = z > 0 ? 1 - tanh^2 z : 0
+ *   THRESHOLDEDRELU (16) z > t ? z : 0                                    f' = z > t ? 1 : 0                         t = act_alpha (DL4J 1.0)
+ * Softplus and Swish use the overflow-safe forms above: DL4J's literal log(1 + e^z) and e^z(z + e^z + 1)/(e^z + 1)^2 overflow to inf / NaN in
+ * fp32 for large z; where those are finite the forms agree to rounding.  The Python and Java builders fill act_alpha = 1.0 for ELU and
+ * ThresholdedReLU when none is given; the C-ABI takes it as given and a non-finite act_alpha with codes 5-16 is B2G_ERR_ARG.
+ * Codes 0-16 are valid on CONV2D, DECONV2D, DENSE and ACTIVATION layers and on OUTPUT / LOSS layers with loss codes 2-8 (XENT / MCXENT ignore
+ * act); any other code there is B2G_ERR_ARG at b2g_net_create.  A GEMM layer with a code of 5-16 keeps its pre-activation z in a buffer of its own
+ * and applies f in a separate element-wise kernel; it is never fused into a GEMM or BatchNorm epilogue.
+ * Not provided: RRELU (random slopes per element in train mode), SOFTMAX as a hidden activation (implied by MCXENT), and GELU / MISH / PReLU
+ * (later DL4J versions). */
+typedef enum {
+  B2G_ACT_IDENTITY = 0, B2G_ACT_TANH = 1, B2G_ACT_SIGMOID = 2, B2G_ACT_RELU = 3, B2G_ACT_LRELU = 4,
+  B2G_ACT_ELU = 5, B2G_ACT_SELU = 6, B2G_ACT_SOFTPLUS = 7, B2G_ACT_SOFTSIGN = 8, B2G_ACT_HARDTANH = 9, B2G_ACT_HARDSIGMOID = 10,
+  B2G_ACT_RELU6 = 11, B2G_ACT_SWISH = 12, B2G_ACT_CUBE = 13, B2G_ACT_RATIONALTANH = 14, B2G_ACT_RECTIFIEDTANH = 15, B2G_ACT_THRESHOLDEDRELU = 16
 } b2g_activation;
 
 /* org.nd4j.linalg.learning.config.*  J:133 (RmsProp), north_star (Adam); the others as in DL4J 1.0.0-beta3 (recalled, parity unpinned like
@@ -127,7 +154,9 @@ typedef enum { B2G_PREC_FP32 = 0, B2G_PREC_BF16 = 1 } b2g_precision;
  *   WASSERSTEIN (8)     score sum y a / nOut                  dL/da = y / nOut
  * The loss of a pass (or of a group of the GAN step) is the sum of its examples' scores, summed in double in an order fixed by the shape (the same
  * bits on every run) and rounded to fp32 once; score = that sum / minibatch + the l2 term.  OUTPUT layers take any nOut; a LOSS layer needs a
- * feed-forward input (H = W = 1) or one element per example (else B2G_ERR_UNSUPPORTED).  b2g_net_output returns a = act(z). */
+ * feed-forward input (H = W = 1) or one element per example (else B2G_ERR_UNSUPPORTED).  b2g_net_output returns a = act(z).
+ * With an activation of codes 5-16 (b2g_activation) a = f(z) is formed by its own kernel and rounded to the activation type, the loss takes a
+ * with the identity, and dL/dz = dL/da * f'(z) with the derivative taken from z. */
 typedef enum {
   B2G_LOSS_XENT = 0, B2G_LOSS_MCXENT = 1, B2G_LOSS_MSE = 2, B2G_LOSS_L1 = 3, B2G_LOSS_L2 = 4, B2G_LOSS_MAE = 5, B2G_LOSS_HINGE = 6,
   B2G_LOSS_SQUARED_HINGE = 7, B2G_LOSS_WASSERSTEIN = 8
@@ -141,7 +170,8 @@ typedef struct {
   int32_t k_h, k_w, s_h, s_w, p_h, p_w;   /* conv / deconv / pool geometry; upsample factor in k_h */
   int32_t has_bias;             /* hasBias(true) default */
   int32_t act;                  /* b2g_activation */
-  float act_alpha;              /* ActivationLReLU alpha: DL4J default 0.01, DCGAN passes 0.2; DropoutLayer retain probability p */
+  float act_alpha;              /* ActivationLReLU alpha: DL4J default 0.01, DCGAN passes 0.2; ELU alpha / ThresholdedReLU theta (DL4J 1.0);
+                                   DropoutLayer retain probability p */
   int32_t updater;              /* b2g_updater; "frozen" in the reference = RMSPROP with lr 0 (J:84) */
   float lr, beta1, beta2, eps;  /* RmsProp: beta1 = rmsDecay (ctor order lr, rmsDecay, epsilon; J:133 passes 1e-8, 1e-8) */
   float l2;                     /* .l2(1e-4) (J:125): weights only, applied AFTER the updater, not lr-scaled */
@@ -427,10 +457,14 @@ int32_t b2g_test_dropout(b2g_ctx* ctx, int32_t precision, uint64_t seed, int32_t
  *   SUMSQ          in0 p [n] fp32, segments seg_off / seg_len / seg_coef              -> sumsq
  *   LOSS           in0 logits [groups][rows][cols] T, in1 labels fp32                 -> out0 dz T, out1 loss per group [groups]
  *                                                                                        (loss = b2g_loss 2-8, cols = nOut, act, alpha)
+ *   ACT_EXT_FWD    in0 z [n] T                                                        -> out0 f(z) T             (act = b2g_activation 5-16, alpha)
+ *   ACT_EXT_BWD    in0 z [n] T, in1 eps_out [n] T                                     -> out0 eps_out * f'(z) T, computed in place in eps_out's
+ *                                                                                        buffer as the backward pass calls it (act 5-16, alpha)
  * Every output buffer not asked for may be NULL. */
 typedef enum {
   B2G_EW_REDUCE_SPLITS = 0, B2G_EW_REDUCE_MULTI = 1, B2G_EW_COLSUM = 2, B2G_EW_XENT = 3, B2G_EW_SOFTMAX_XENT = 4,
-  B2G_EW_ACT_FWD = 5, B2G_EW_ACT_BWD = 6, B2G_EW_MAXPOOL = 7, B2G_EW_UPSAMPLE = 8, B2G_EW_SUMSQ = 9, B2G_EW_LOSS = 10
+  B2G_EW_ACT_FWD = 5, B2G_EW_ACT_BWD = 6, B2G_EW_MAXPOOL = 7, B2G_EW_UPSAMPLE = 8, B2G_EW_SUMSQ = 9, B2G_EW_LOSS = 10,
+  B2G_EW_ACT_EXT_FWD = 11, B2G_EW_ACT_EXT_BWD = 12
 } b2g_ew_op;
 typedef struct {          /* one split-K sum of a reduce list: dst[i] = sum_s src[s*stride + i], i < n, all offsets in elements of in0 */
   int64_t n, stride, src_off, dst_off;

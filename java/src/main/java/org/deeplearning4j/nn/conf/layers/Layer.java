@@ -3,6 +3,7 @@ package org.deeplearning4j.nn.conf.layers;
 
 import java.nio.ByteBuffer;
 import org.nd4j.linalg.activations.Activation;
+import org.nd4j.linalg.activations.IActivation;
 import org.nd4j.linalg.learning.config.IUpdater;
 
 public class Layer {
@@ -10,17 +11,19 @@ public class Layer {
     public int type, nIn, nOut, kH = 1, kW = 1, sH = 1, sW = 1, pH, pW, hasBias = 1, act = -1, preH, preW, preC, loss, frozen;
     public float alpha = 0.01f, l2 = Float.NaN, bnDecay = 0.9f, bnEps = 1e-5f;
     public IUpdater updater; public String name = "";
+    public boolean alphaSet;   // alpha given by leakyReluAlpha(..) or activation(IActivation); else ELU / ThresholdedReLU write DL4J's 1.0
 
     /** Serialise into the C struct layout (little-endian, no padding: every field is 4-byte aligned). */
     public void write(ByteBuffer b, Activation globalAct, float globalL2) {
         b.putInt(type); byte[] nm = name.getBytes(java.nio.charset.StandardCharsets.US_ASCII); byte[] fixed = new byte[64]; System.arraycopy(nm, 0, fixed, 0, Math.min(63, nm.length)); b.put(fixed);
         b.putInt(nIn).putInt(nOut).putInt(kH).putInt(kW).putInt(sH).putInt(sW).putInt(pH).putInt(pW).putInt(hasBias);
-        b.putInt(act >= 0 ? act : defaultAct(globalAct)).putFloat(alpha);
+        final int a = act >= 0 ? act : defaultAct(globalAct);
+        b.putInt(a).putFloat(!alphaSet && (a == Activation.ELU.code || a == Activation.THRESHOLDEDRELU.code) ? 1.0f : alpha);
         b.putInt(updater == null ? 0 : updater.kind()).putFloat(updater == null ? 0f : updater.lr()).putFloat(updater == null ? 0f : updater.beta1()).putFloat(updater == null ? 0f : updater.beta2()).putFloat(updater == null ? 1e-8f : updater.eps());
         b.putFloat(Float.isNaN(l2) ? globalL2 : l2).putFloat(bnDecay).putFloat(bnEps).putInt(preH).putInt(preW).putInt(preC).putInt(loss).putInt(frozen);
     }
     public Layer copy() { Layer c = new Layer(); c.type = type; c.nIn = nIn; c.nOut = nOut; c.kH = kH; c.kW = kW; c.sH = sH; c.sW = sW; c.pH = pH; c.pW = pW; c.hasBias = hasBias; c.act = act;
-        c.preH = preH; c.preW = preW; c.preC = preC; c.loss = loss; c.frozen = frozen; c.alpha = alpha; c.l2 = l2; c.bnDecay = bnDecay; c.bnEps = bnEps; c.updater = updater; c.name = name; return c; }
+        c.preH = preH; c.preW = preW; c.preC = preC; c.loss = loss; c.frozen = frozen; c.alpha = alpha; c.l2 = l2; c.bnDecay = bnDecay; c.bnEps = bnEps; c.updater = updater; c.name = name; c.alphaSet = alphaSet; return c; }
     protected int defaultAct(Activation g) { return g.code; }   // conv / dense inherit the global .activation(..) (J:126)
 
     @SuppressWarnings("unchecked")
@@ -34,7 +37,8 @@ public class Layer {
         public T hasBias(boolean b) { l.hasBias = b ? 1 : 0; return (T) this; }
         public T updater(IUpdater u) { l.updater = u; return (T) this; }
         public T activation(Activation a) { l.act = a.code; return (T) this; }
-        public T leakyReluAlpha(double a) { l.alpha = (float) a; return (T) this; }
+        public T activation(IActivation a) { l.act = a.code(); l.alpha = a.alpha(); l.alphaSet = true; return (T) this; }   // ActivationELU(alpha), ActivationThresholdedReLU(theta)
+        public T leakyReluAlpha(double a) { l.alpha = (float) a; l.alphaSet = true; return (T) this; }
         public T l2(double v) { l.l2 = (float) v; return (T) this; }
         public Layer build() { return l; }
     }
