@@ -73,6 +73,13 @@ class TestEwOpts(C.Structure):
                 ("kernel", C.c_char * 64), ("loss", C.c_int32)]
 
 
+class TestPoolOpts(C.Structure):
+    """b2g_test_pool_opts: which pooling kernels to run (pool2d / global), the kind, p, geometry and switches, and what ran."""
+    _fields_ = [("op", C.c_int32), ("pool", C.c_int32), ("pnorm", C.c_float)] + [
+                (k, C.c_int32) for k in ("N", "H", "W", "C", "KH", "KW", "SH", "SW", "PH", "PW", "offset", "poison")] + [
+                ("kernel", C.c_char * 64), ("splits", C.c_int32)]
+
+
 _vp, _i32, _i64, _fp = C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_float)
 _pvp = C.POINTER(C.c_void_p)
 
@@ -140,6 +147,7 @@ PROTOTYPES = {
     "b2g_test_net_shadow": (_i32, [_vp, _i32, _i32, _fp, _i64]),
     "b2g_test_dropout": (_i32, [_vp, _i32, C.c_uint64, _i32, _i32, _i64, _i32, _i32, _i32, _i32, C.c_float, _fp, _fp, _fp, _fp]),
     "b2g_test_ew": (_i32, [_vp, _i32, C.POINTER(TestEwOpts), _fp, _fp, _fp, _fp, _fp]),
+    "b2g_test_pool": (_i32, [_vp, _i32, C.POINTER(TestPoolOpts), _fp, _fp, _fp, _fp, _fp]),
 }
 
 _lib = None

@@ -93,6 +93,28 @@ void k_maxpool_bwd(int prec, const void* eps_out, const uint8_t* argmax, void* e
 void k_upsample_fwd(int prec, const void* x, void* y, int N, int H, int W, int C, int f, cudaStream_t s);
 void k_upsample_bwd(int prec, const void* eps_out, void* eps_in, int N, int H, int W, int C, int f, cudaStream_t s);
 
+// ---- average / sum / p-norm pooling (kernels_pool.cu; formulas and summation order at b2g_pooling in include/b200gan.h) ----------------
+// One instantiation per kind, precision and path (16-byte vectors when C is a multiple of the vector width and the tensors are aligned, else
+// per element).  pn = PNORM's p (a whole number >= 1; ignored by the other kinds).
+enum Pool { POOL_MAX = 0, POOL_AVG = 1, POOL_SUM = 2, POOL_PNORM = 3 };   // b2g_pooling
+// SubsamplingLayer AVG / SUM / PNORM, Truncate geometry with zero padding; MAX launches nothing (B2G_LAYER_MAXPOOL's kernels).  The backward
+// is the gather form; y = the forward's output (PNORM reads it and x).
+void k_pool2d_fwd(int prec, int kind, int pn, const void* x, void* y, int N, int H, int W, int C, int OH, int OW, int KH, int KW, int SH, int SW, int PH, int PW,
+                  cudaStream_t s);
+void k_pool2d_bwd(int prec, int kind, int pn, const void* eps_out, const void* x, const void* y, void* eps_in, int N, int H, int W, int C, int OH, int OW, int KH,
+                  int KW, int SH, int SW, int PH, int PW, cudaStream_t s);
+// GlobalPoolingLayer: x [N][HW][C] -> y [N][C], MAX also idx [N][C] (the pixel of the first maximum).  Where N x channel chunks gives too few
+// blocks the pixel range is split over k_global_pool_splits blocks (a function of the shape and of the vector path); their fp32 partials go to
+// part / part_idx ([N][splits][C]; k_global_pool_partial_elems for every batch up to max_rows) and the last block to finish folds them (ticket
+// word, 0 between launches).  One launch.
+int k_global_pool_splits(int prec, int N, int HW, int C, int vec);
+size_t k_global_pool_partial_elems(int prec, int max_rows, int HW, int C);
+void k_global_pool_fwd(int prec, int kind, int pn, const void* x, void* y, int32_t* idx, int N, int HW, int C, float* part, int32_t* part_idx, unsigned* ticket,
+                       cudaStream_t s);
+void k_global_pool_bwd(int prec, int kind, int pn, const void* eps_out, const void* x, const void* y, const int32_t* idx, void* eps_in, int N, int HW, int C,
+                       cudaStream_t s);
+extern int g_pool_last_splits;   // the split count of the most recent k_global_pool_fwd (kernel-level tests assert it)
+
 // ---- dropout (DL4J DropoutLayer, inverted dropout; mask definition in include/b200gan.h) ----------------------------------------
 // Forward over the n elements of one pass (NHWC, element index e): y = x * (1/p) where kept, 0 where dropped, and the keep bits into
 // mask[e >> 5] bit (e & 31).  The random word of element e is Philox4x32-10(ctr = {e >> 2, lo32(P), hi32(P), tag}, key = {lo32(seed), hi32(seed)})[e & 3],

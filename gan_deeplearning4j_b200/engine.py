@@ -17,7 +17,11 @@ from . import _lib
 from ._lib import GanConfig, LayerDesc, LrSchedule, NetConfig, check
 
 LAYER_TYPES = {"conv2d": 0, "deconv2d": 1, "batchnorm": 2, "dense": 3, "activation": 4, "maxpool": 5, "upsample2d": 6,
-               "output": 7, "loss": 8, "ff_to_cnn": 9, "cnn_to_ff": 10, "dropout": 11}
+               "output": 7, "loss": 8, "ff_to_cnn": 9, "cnn_to_ff": 10, "dropout": 11, "subsampling": 12, "global_pooling": 13}
+# org.deeplearning4j.nn.conf.layers.PoolingType -> b2g_pooling, carried in b2g_layer_desc.act of "subsampling" (avg / sum / pnorm; max is the
+# "maxpool" layer) and "global_pooling" (all four) specs; PNORM's p in act_alpha (formulas at b2g_pooling in include/b200gan.h)
+POOLINGS = {"max": 0, "avg": 1, "sum": 2, "pnorm": 3}
+GLOBAL_PNORM_DEFAULT = 2             # GlobalPoolingLayer.Builder().pnorm default
 # org.nd4j.linalg.activations.Activation -> b2g_activation (codes 5-16: formulas at b2g_activation in include/b200gan.h)
 ACTS = {"identity": 0, "tanh": 1, "sigmoid": 2, "relu": 3, "lrelu": 4, "elu": 5, "selu": 6, "softplus": 7, "softsign": 8, "hardtanh": 9,
         "hardsigmoid": 10, "relu6": 11, "swish": 12, "cube": 13, "rationaltanh": 14, "rectifiedtanh": 15, "thresholdedrelu": 16}
@@ -131,6 +135,9 @@ def layer_desc(spec: Dict) -> LayerDesc:
     d.act_alpha = spec.get("alpha", ACT_ALPHA_DEFAULTS.get(act, 0.01))
     if spec["type"] == "dropout":       # DropoutLayer.Builder(p): p = retain probability, carried in act_alpha
         d.act_alpha = spec["p"]
+    if spec["type"] in ("subsampling", "global_pooling"):      # the pooling kind in act, PNORM's p in act_alpha (0 = none given: refused)
+        d.act = POOLINGS[spec.get("pooling", "max")]
+        d.act_alpha = float(spec.get("pnorm", GLOBAL_PNORM_DEFAULT if spec["type"] == "global_pooling" else 0))
     u = spec.get("updater") or {"kind": "sgd", "lr": 0.0}
     d.updater = UPDATERS[u["kind"]]
     d.lr = constant_lr(u.get("lr", 0.0))     # new Adam(ISchedule): the schedule itself is set after b2g_net_create
@@ -586,3 +593,21 @@ def test_ew(ctx: Context, precision: int, op: str, in0, in1=None, out_sizes=(0, 
     check(ctx.lib.b2g_test_ew(ctx.h, precision, C.byref(o), *[ptr(a) for a in ins], *[ptr(a) for a in outs]))
     info = {"kernel": o.kernel.decode(), "sumsq": o.sumsq, "wide": [o.jobs[i].wide for i in range(o.n_jobs)] if jobs is not None else []}
     return outs, info
+
+
+POOL_TEST_OPS = {"pool2d": 0, "global_pool": 1}
+
+
+def test_pool(ctx: Context, precision: int, op: str, in0, in1, out_sizes=(0, 0, 0), *, pooling: str = "max", pnorm: float = 2.0, **opts):
+    """One pooling layer's forward and backward kernels through their production wrappers (b2g_test_pool; operands in include/b200gan.h).
+    op "pool2d" (pooling avg / sum / pnorm) or "global_pool" (any POOLINGS name); opts: N, H, W, C, KH, KW, SH, SW, PH, PW, offset, poison.
+    Returns ([out0, out1, out2] with None where not asked for, {"kernel": "forward,backward", "splits": int})."""
+    o = _lib.TestPoolOpts()
+    o.op, o.pool, o.pnorm = POOL_TEST_OPS[op], POOLINGS[pooling], float(pnorm)
+    for k, v in opts.items():
+        setattr(o, k, int(v))
+    ins = [_f32(v).ravel() for v in (in0, in1)]
+    outs = [np.empty(k, np.float32) if k else None for k in out_sizes]
+    ptr = lambda a: None if a is None else _fp(a)
+    check(ctx.lib.b2g_test_pool(ctx.h, precision, C.byref(o), *[ptr(a) for a in ins], *[ptr(a) for a in outs]))
+    return outs, {"kernel": o.kernel.decode(), "splits": o.splits}

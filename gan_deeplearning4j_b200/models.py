@@ -84,6 +84,34 @@ def map_schedule(values, type="iteration"):
     return {"schedule": "map", "type": type, "values": [[k, v] for k, v in pairs]}
 
 
+# ------------------------------------------------------------------ pooling layers ---------------------
+# SubsamplingLayer / GlobalPoolingLayer (b2g_pooling in include/b200gan.h).  SubsamplingLayer(MAX) is the "maxpool" spec (unpadded).
+def subsampling(pooling, kernel=(1, 1), stride=(2, 2), padding=(0, 0), pnorm=None, name="") -> Dict:
+    """new SubsamplingLayer.Builder(PoolingType.AVG / SUM / PNORM).kernelSize(kernel).stride(stride).padding(padding).pnorm(p) (DL4J's default
+    kernel 1x1, stride 2x2).  PNORM needs pnorm, a whole number >= 1."""
+    if pooling not in ("avg", "sum", "pnorm"):
+        raise ValueError(f"subsampling pooling {pooling!r}: one of avg, sum, pnorm (MAX is the 'maxpool' spec)")
+    spec = {"type": "subsampling", "name": name, "pooling": pooling, "kernel": tuple(kernel), "stride": tuple(stride), "padding": tuple(padding)}
+    if pooling == "pnorm":
+        if pnorm is None:
+            raise ValueError("PNORM subsampling needs pnorm (a whole number >= 1)")
+        spec["pnorm"] = int(pnorm)
+    return spec
+
+
+def global_pooling(pooling="max", pnorm=2, name="") -> Dict:
+    """new GlobalPoolingLayer.Builder(PoolingType).pnorm(p) (DL4J's defaults MAX, p = 2): [mb, C, H, W] -> [mb, C]."""
+    if pooling not in ("max", "avg", "sum", "pnorm"):
+        raise ValueError(f"global pooling {pooling!r}: one of max, avg, sum, pnorm")
+    spec = {"type": "global_pooling", "name": name, "pooling": pooling}
+    if pooling == "pnorm":
+        spec["pnorm"] = int(pnorm)
+    return spec
+
+
+_global_pooling_spec = global_pooling       # dcgan_discriminator's argument of the same name shadows the builder
+
+
 # ------------------------------------------------------------------ C1: the reference graphs ---------
 def reference_discriminator(lr=0.002, prefix="dis") -> List[Dict]:
     """J:118-165: BN -> Conv5x5 s2 (1->64) -> MaxPool 2x2 s1 -> Conv5x5 s2 (64->128) -> MaxPool -> Dense 1024 -> Output(1, sigmoid, XENT);
@@ -166,10 +194,13 @@ def _loss_keys(loss, out_activation) -> Dict:
     return {"loss": loss, "activation": out_activation}
 
 
-def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", out_activation="identity", activation="lrelu", alpha=None) -> List[Dict]:
+def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", out_activation="identity", activation="lrelu", alpha=None,
+                        global_pooling=None) -> List[Dict]:
     """Conv(4x4 s2 p1)+LeakyReLU(0.2); (Conv+BatchNorm+LeakyReLU)*; Conv(4x4 s1 p0) -> logit; LossLayer(loss).  Input (nc,size,size).
     loss: "xent" (sigmoid implied), or "mse" (least-squares GAN), "hinge", "wasserstein", ... applied to out_activation(logit).
-    activation / alpha: the hidden activation in place of LeakyReLU(0.2) (as in _act)."""
+    activation / alpha: the hidden activation in place of LeakyReLU(0.2) (as in _act).
+    global_pooling: a pooling kind ("sum" for the projected / ResNet-style head, "avg", "max", "pnorm"): GlobalPoolingLayer + OutputLayer(nOut 1,
+    loss) in place of the last conv and its LossLayer."""
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
     n_down = int(math.log2(size)) - 2
     L = [{"type": "conv2d", "name": "dis_conv_1", "n_in": nc, "n_out": nf, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), **_act(activation, alpha), "updater": u()}]
@@ -178,6 +209,9 @@ def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", o
         L += [{"type": "conv2d", "name": f"dis_conv_{i + 2}", "n_in": ch, "n_out": ch * 2, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "has_bias": False, "updater": u()},
               {"type": "batchnorm", "name": f"dis_bn_{i + 2}", "updater": u()}, dict({"type": "activation", "name": f"dis_act_{i + 2}"}, **_act(activation, alpha))]
         ch *= 2
+    if global_pooling is not None:
+        return L + [_global_pooling_spec(global_pooling, name="dis_global_pool"),
+                    dict({"type": "output", "name": "dis_output", "n_out": 1, "updater": u()}, **_loss_keys(loss, out_activation))]
     L += [{"type": "conv2d", "name": f"dis_conv_{n_down + 1}", "n_in": ch, "n_out": 1, "kernel": (4, 4), "stride": (1, 1), "padding": (0, 0), "updater": u()},
           dict({"type": "loss", "name": "dis_loss"}, **_loss_keys(loss, out_activation))]
     return L
@@ -223,6 +257,11 @@ def forward_macs(specs: List[Dict], input_shape) -> int:
             macs += c * h * w * s["n_out"]; c, h, w = s["n_out"], 1, 1
         elif t == "maxpool":
             k, st = s["kernel"], s.get("stride", (1, 1)); h, w = (h - k[0]) // st[0] + 1, (w - k[1]) // st[1] + 1
+        elif t == "subsampling":
+            k, st, p = s["kernel"], s.get("stride", (1, 1)), s.get("padding", (0, 0))
+            h, w = (h + 2 * p[0] - k[0]) // st[0] + 1, (w + 2 * p[1] - k[1]) // st[1] + 1
+        elif t == "global_pooling":
+            h, w = 1, 1
         elif t == "upsample2d":
             h, w = h * s.get("size", 2), w * s.get("size", 2)
         elif t == "ff_to_cnn":

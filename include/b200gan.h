@@ -63,7 +63,9 @@ typedef enum {
   B2G_LAYER_LOSS = 8,        /* LossLayer(loss): loss (b2g_loss) on the incoming pre-activations (DCGAN D-last conv) */
   B2G_LAYER_FF_TO_CNN = 9,   /* FeedForwardToCnnPreProcessor(h,w,c)                               J:200,255         */
   B2G_LAYER_CNN_TO_FF = 10,  /* CnnToFeedForwardPreProcessor (auto-inserted by setInputTypes, SURVEY.md 3.1)       */
-  B2G_LAYER_DROPOUT = 11     /* DropoutLayer.Builder(p): p = RETAIN probability in (0, 1], carried in act_alpha; no parameters */
+  B2G_LAYER_DROPOUT = 11,    /* DropoutLayer.Builder(p): p = RETAIN probability in (0, 1], carried in act_alpha; no parameters */
+  B2G_LAYER_SUBSAMPLING = 12,    /* SubsamplingLayer.Builder(PoolingType.AVG / SUM / PNORM).kernelSize().stride().padding().pnorm(): b2g_pooling */
+  B2G_LAYER_GLOBAL_POOLING = 13  /* GlobalPoolingLayer.Builder(PoolingType).pnorm(): b2g_pooling, output [mb, C] (H = W = 1)                 */
 } b2g_layer_type;
 
 /* DropoutLayer (inverted dropout, DL4J 1.0.0-beta3).  Train-mode forward y = x * m, m = 1/p (fp32 1.0f / p) with probability p, else 0;
@@ -79,6 +81,30 @@ typedef enum {
  * (train, not frozen, p < 1) uses the current P for all of them and then advances P by 1 on the device (so a replayed CUDA graph draws new
  * masks); other forwards leave it unchanged.  In the GAN step D's real|fake pass (2N rows) uses P and the generator step's D pass P + 1.
  * A pass may hold at most 2^34 elements (max_batch * layer size; B2G_ERR_UNSUPPORTED at b2g_net_create). */
+
+/* org.deeplearning4j.nn.conf.layers.PoolingType of SUBSAMPLING and GLOBAL_POOLING layers (DL4J 1.0.0-beta3, recalled; parity unpinned like the
+ * rest of the DL4J semantics).  The kind is carried in b2g_layer_desc.act (pooling layers have no activation), PNORM's p in act_alpha: a whole
+ * number >= 1 (DL4J's int pnorm; at most 1024).  SUBSAMPLING takes AVG, SUM and PNORM (MAX stays B2G_LAYER_MAXPOOL, unpadded); GLOBAL_POOLING
+ * takes all four.  B2G_ERR_ARG at b2g_net_create for another kind or a p that is not such a number; B2G_ERR_SHAPE for a SUBSAMPLING kernel or
+ * stride below 1, a padding below 0 or not smaller than the kernel, or an empty output.
+ *   SUBSAMPLING (Truncate): OH = (H + 2 ph - kh) / sh + 1, likewise OW; the window of output row oy is input rows oy*sh - ph ... + kh - 1, the
+ *   positions outside the input are zeros.  Per (example, output pixel, channel) the window's in-range elements are summed in fp32 in row-major
+ *   window order, then
+ *     AVG    y = sum / (kh*kw)       (the padding counts in the divisor)      dx += eps / (kh*kw)
+ *     SUM    y = sum                                                           dx += eps
+ *     PNORM  y = (sum |x|^p)^(1/p)                                             dx += eps * sign(x)|x|^(p-1) / max(y^(p-1), 1e-8)
+ *   The backward gathers: each input element sums, in fixed order (filter row, then column, ascending), eps (AVG / SUM) or eps / max(y^(p-1),
+ *   1e-8) (PNORM) of the windows that cover it, then divides by kh*kw (AVG) or multiplies by sign(x)|x|^(p-1) (PNORM), in fp32.
+ *   GLOBAL_POOLING: per (example, channel) over the H*W pixels to [mb, C] (collapseDimensions; [mb, C, 1, 1] is the same bytes):
+ *     MAX    y = the first maximum in row-major pixel order; dx = eps at that pixel, 0 elsewhere
+ *     AVG    y = sum / (H*W);  dx = eps / (H*W)        SUM  y = sum;  dx = eps
+ *     PNORM  y = (sum |x|^p)^(1/p);  dx = eps * sign(x)|x|^(p-1) / max(y^(p-1), 1e-8)
+ *   The pixel sum is in fp32 in an order fixed by the shape: lane t of a block takes pixels t, t + r, t + 2r, ... of its pixel range, the lanes
+ *   fold in lane order and, where a large map is split over blocks, the splits fold in split order (kernels_pool.cu gp_plan).
+ * Powers: |x|^p and y^(p-1) are exact products for p = 1, 2 and powf otherwise; the root is sqrtf for p = 2 and powf(s, 1.0f / p) for p >= 3.
+ * Every result is rounded once to the activation type.  The 1e-8 floor (SubsamplingLayer's default eps) keeps an all-zero window (after a
+ * ReLU) at 0 instead of 0/0; DL4J's GlobalPoolingLayer has no floor, so its NaN on a zero map is a deliberate deviation here. */
+typedef enum { B2G_POOL_MAX = 0, B2G_POOL_AVG = 1, B2G_POOL_SUM = 2, B2G_POOL_PNORM = 3 } b2g_pooling;
 
 /* org.nd4j.linalg.activations.Activation  J:126,162,215.  Codes 0-4 as DL4J; LRELU's alpha = b2g_layer_desc.act_alpha.
  * Codes 5-16 (DL4J 1.0.0-beta3 org.nd4j.linalg.activations.impl.*, recalled; parity unpinned like the rest of the DL4J semantics).  f and f' are
@@ -169,9 +195,9 @@ typedef struct {
   int32_t n_in, n_out;          /* channels / features (n_in may be 0 = infer, like setInputTypes) */
   int32_t k_h, k_w, s_h, s_w, p_h, p_w;   /* conv / deconv / pool geometry; upsample factor in k_h */
   int32_t has_bias;             /* hasBias(true) default */
-  int32_t act;                  /* b2g_activation */
+  int32_t act;                  /* b2g_activation; b2g_pooling on SUBSAMPLING / GLOBAL_POOLING layers */
   float act_alpha;              /* ActivationLReLU alpha: DL4J default 0.01, DCGAN passes 0.2; ELU alpha / ThresholdedReLU theta (DL4J 1.0);
-                                   DropoutLayer retain probability p */
+                                   DropoutLayer retain probability p; PNORM pooling's p */
   int32_t updater;              /* b2g_updater; "frozen" in the reference = RMSPROP with lr 0 (J:84) */
   float lr, beta1, beta2, eps;  /* RmsProp: beta1 = rmsDecay (ctor order lr, rmsDecay, epsilon; J:133 passes 1e-8, 1e-8) */
   float l2;                     /* .l2(1e-4) (J:125): weights only, applied AFTER the updater, not lr-scaled */
@@ -492,6 +518,26 @@ typedef struct {
   int32_t loss;           /* LOSS: b2g_loss 2-8 */
 } b2g_test_ew_opts;
 int32_t b2g_test_ew(b2g_ctx* ctx, int32_t precision, b2g_test_ew_opts* opts, const float* in0, const float* in1, float* out0, float* out1, float* out2);
+
+/* One pooling layer's forward and backward kernels (kernels_pool.cu) through their production wrappers on host tensors, as b2g_test_ew runs the
+ * other element-wise kernels (T tensors fp32 on the host, rounded to bf16 on the device when precision is BF16; offset and poison as there):
+ *   POOL2D       in0 x [N][H][W][C] T, in1 eps_out [N][OH][OW][C] T (b2g_pooling geometry with KH, KW, SH, SW, PH, PW; pool = AVG / SUM / PNORM)
+ *                                                                          -> out0 y T, out1 eps_in T (the backward reads the forward's y)
+ *   GLOBAL_POOL  in0 x [N][H][W][C] T, in1 eps_out [N][C] T (pool = any)  -> out0 y [N][C] T, out1 eps_in T, out2 MAX's pixel index (as float;
+ *                                                                             -1 for the other kinds)
+ * Every output buffer not asked for may be NULL. */
+typedef enum { B2G_TEST_POOL2D = 0, B2G_TEST_GLOBAL_POOL = 1 } b2g_test_pool_op;
+typedef struct {
+  int32_t op;             /* b2g_test_pool_op */
+  int32_t pool;           /* b2g_pooling */
+  float pnorm;            /* PNORM: p */
+  int32_t N, H, W, C, KH, KW, SH, SW, PH, PW;
+  int32_t offset;         /* every device operand starts this many elements past a 256-byte aligned address (reaches the per-element path) */
+  int32_t poison;         /* fill every output with NaN before the launch: an element the kernel leaves unwritten reads back as NaN */
+  char kernel[64];        /* out: forward, backward kernel */
+  int32_t splits;         /* out, GLOBAL_POOL: the number of blocks each example's pixel range was split over (1: no split) */
+} b2g_test_pool_opts;
+int32_t b2g_test_pool(b2g_ctx* ctx, int32_t precision, b2g_test_pool_opts* opts, const float* in0, const float* in1, float* out0, float* out1, float* out2);
 
 #ifdef __cplusplus
 }
