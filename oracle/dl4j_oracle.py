@@ -22,11 +22,22 @@ Reference call sites restated here (J = Java/src/main/java/org/deeplearning4j/dl
   * SubsamplingLayer MAX  J:141-144,151-154                     -> ``MaxPool``
   * DenseLayer            J:155-158,189-196                     -> ``Dense``
   * OutputLayer XENT      J:159-163,303-308                     -> ``Output`` / ``LossLayer``
-  * Activation.*          J:126,162,215                         -> ``ACTS``
+  * Activation.*          J:126,162,215                         -> ``act_forward`` / ``act_backward``
   * RmsProp/Adam, clip, l2  J:123-125,133...                    -> ``Net.apply_update``
   * fit / output loop     J:408-471                             -> ``Net.fit``, ``Net.output``, ``gan_iteration_reference``,
                                                                    ``gan_step`` (the aliased G+D step the CUDA path runs)
   * parameter averaging   J:325-333, Python/gan.ipynb:177-187   -> ``parameter_average``
+
+DL4J features the library offers beyond the reference's call sites, restated here from DL4J 1.0.0-beta3 (formulas at the named enum in
+include/b200gan.h):
+  * activations of b2g_activation codes 5-16       -> ``forward`` / ``derivative`` (reached through ``act_forward`` / ``act_backward``)
+  * losses of b2g_loss codes 2-8                   -> ``score_and_grad`` (``Output`` / ``LossLayer`` with a loss other than XENT)
+  * SubsamplingLayer AVG / SUM / PNORM, GlobalPoolingLayer (b2g_pooling)  -> ``Subsampling`` / ``GlobalPooling``
+  * DropoutLayer (B2G_LAYER_DROPOUT; the mask is the library's Philox draw) -> ``Dropout``, ``dropout_mask``
+  * the updaters of b2g_updater                    -> ``UpdaterCfg``, ``init_state``, ``update``
+  * L2 gradient normalization                      -> ``Net.set_gradient_normalization``, ``normalize``
+  * learning-rate schedules (ISchedule)            -> ``Net.set_lr_schedule``, ``value``, ``lr_at``
+``net_from_specs`` builds a Net from the layer specs the CUDA engine consumes.
 
 Layouts follow DL4J: activations NCHW, conv W [nOut,nIn,kH,kW] 'c' order flattened as [b | W],
 deconv W [nIn,nOut,kH,kW] flattened [b | W], dense W [nIn,nOut] 'f' order flattened [W | b],
@@ -35,6 +46,7 @@ BN [gamma | beta | mean | var].
 from __future__ import annotations
 
 import dataclasses
+import math
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -51,6 +63,24 @@ class Quirks:
     l2_after_updater: bool = True        # pre-beta4: g <- updater(g) ; g += l2*W   (not lr-scaled)
     rmsprop_cache_init_eps: bool = True  # RmsPropUpdater state initialised to epsilon
     adam_eps_outside: bool = True        # alpha_t*m/(sqrt(v)+eps), alpha_t = lr*sqrt(1-b2^t)/(1-b1^t)
+    # activations of codes 5-16
+    hardtanh_closed: bool = True             # HardTanh' = 1 on the CLOSED interval [-1, 1]
+    hardsigmoid_closed: bool = True          # HardSigmoid' = 0.2 on the CLOSED interval [-2.5, 2.5]
+    relu6_open: bool = True                  # ReLU6' = 1 on the OPEN interval (0, 6)
+    thresholded_relu_in_beta3: bool = True   # ActivationThresholdedReLU exists in 1.0.0-beta3 (False: the name is refused)
+    # losses of codes 2-8
+    wasserstein_per_output: bool = True      # LossWasserstein divides score and gradient by nOut (moot at nOut = 1)
+    # pooling
+    avg_include_pad_in_divisor: bool = True  # AVG divides by kh*kw, padding included (beta4 added the switch)
+    pnorm_denominator_floor: bool = True     # y^(p-1) floored at 1e-8 (SubsamplingLayer); global pooling: deliberate deviation
+    global_max_first_tie: bool = True        # global MAX routes eps to the FIRST maximum in row-major order (False: the last)
+    # updaters
+    adagrad_history_init_eps: bool = True    # AdaGrad's history starts at eps (else at 0)
+    adamax_floor_no_eps: bool = True         # AdaMax: u_inf gets + 1e-32 and the denominator has no eps (else u_inf + eps)
+    nadam_v_uncorrected: bool = True         # Nadam divides by sqrt(v) + eps (else by sqrt(v / (1-b2^t)) + eps)
+    # L2 gradient normalization
+    bn_stats_normalized: bool = True         # BatchNorm mean/var pseudo-gradients count in the layer's norm and are scaled
+    l2norm_zero_floor: float = 1e-5          # Renormalize divides by this instead of a zero norm
 
 
 DEFAULT_QUIRKS = Quirks()
@@ -68,7 +98,95 @@ def _sigmoid(z):
     return out
 
 
-def act_forward(name: str, z: np.ndarray, alpha: float = 0.01) -> np.ndarray:
+ACTS = ("identity", "tanh", "sigmoid", "relu", "lrelu")
+# b2g_activation codes 5-16, restated in float64 with f'(z) taken from the pre-activation z, as IActivation.backprop(in, epsilon) takes it
+EXT_ACTS = ("elu", "selu", "softplus", "softsign", "hardtanh", "hardsigmoid", "relu6", "swish", "cube", "rationaltanh", "rectifiedtanh",
+            "thresholdedrelu")
+ACT_CODES = {k: 5 + i for i, k in enumerate(EXT_ACTS)}
+ACT_ALPHA_DEFAULTS = {"elu": 1.0, "thresholdedrelu": 1.0}      # ELU's alpha, ThresholdedReLU's theta
+SELU_LAMBDA, SELU_ALPHA = 1.0507009873554805, 1.6732632423543772
+RT_A, RT_C = 1.7159, 1.41645
+
+
+def _check_ext(name, q):
+    if name not in EXT_ACTS:
+        raise ValueError(name)
+    if name == "thresholdedrelu" and not q.thresholded_relu_in_beta3:
+        raise ValueError("ThresholdedReLU is not part of DL4J 1.0.0-beta3 under Quirks.thresholded_relu_in_beta3 = False")
+
+
+def forward(name: str, z, alpha: float = None, q: Quirks = DEFAULT_QUIRKS) -> np.ndarray:
+    """f(z) in float64 of an activation of codes 5-16 (alpha None: the kind's default)."""
+    _check_ext(name, q)
+    z = np.asarray(z, np.float64)
+    a = ACT_ALPHA_DEFAULTS.get(name, 0.0) if alpha is None else float(alpha)
+    if name == "elu":
+        return np.where(z >= 0, z, a * np.expm1(np.minimum(z, 0)))
+    if name == "selu":
+        return SELU_LAMBDA * np.where(z > 0, z, SELU_ALPHA * np.expm1(np.minimum(z, 0)))
+    if name == "softplus":
+        return np.maximum(z, 0) + np.log1p(np.exp(-np.abs(z)))
+    if name == "softsign":
+        return z / (1 + np.abs(z))
+    if name == "hardtanh":
+        return np.clip(z, -1.0, 1.0)
+    if name == "hardsigmoid":
+        return np.clip(0.2 * z + 0.5, 0.0, 1.0)
+    if name == "relu6":
+        return np.clip(z, 0.0, 6.0)
+    if name == "swish":
+        return z * _sigmoid(z)
+    if name == "cube":
+        return z ** 3
+    if name == "rationaltanh":
+        y = 2.0 * z / 3.0
+        A = 1 + np.abs(y) + y * y + RT_C * y ** 4
+        return RT_A * np.sign(y) * (1 - 1 / A)
+    if name == "rectifiedtanh":
+        return np.maximum(0.0, np.tanh(z))
+    return np.where(z > a, z, 0.0)          # thresholdedrelu
+
+
+def derivative(name: str, z, alpha: float = None, q: Quirks = DEFAULT_QUIRKS) -> np.ndarray:
+    """f'(z) in float64 of an activation of codes 5-16."""
+    _check_ext(name, q)
+    z = np.asarray(z, np.float64)
+    a = ACT_ALPHA_DEFAULTS.get(name, 0.0) if alpha is None else float(alpha)
+    if name == "elu":
+        return np.where(z >= 0, 1.0, a * np.exp(np.minimum(z, 0)))
+    if name == "selu":
+        return np.where(z > 0, SELU_LAMBDA, SELU_LAMBDA * SELU_ALPHA * np.exp(np.minimum(z, 0)))
+    if name == "softplus":
+        return _sigmoid(z)
+    if name == "softsign":
+        return 1 / (1 + np.abs(z)) ** 2
+    if name == "hardtanh":
+        inside = (z >= -1) & (z <= 1) if q.hardtanh_closed else (z > -1) & (z < 1)
+        return np.where(inside, 1.0, 0.0)
+    if name == "hardsigmoid":
+        inside = (z >= -2.5) & (z <= 2.5) if q.hardsigmoid_closed else (z > -2.5) & (z < 2.5)
+        return np.where(inside, 0.2, 0.0)
+    if name == "relu6":
+        inside = (z > 0) & (z < 6) if q.relu6_open else (z >= 0) & (z <= 6)
+        return np.where(inside, 1.0, 0.0)
+    if name == "swish":
+        s = _sigmoid(z)
+        return s * (1 + z * (1 - s))
+    if name == "cube":
+        return 3 * z * z
+    if name == "rationaltanh":
+        y = 2.0 * z / 3.0
+        A = 1 + np.abs(y) + y * y + RT_C * y ** 4
+        return RT_A * (2.0 / 3.0) * (1 + np.sign(y) * (2 * y + 4 * RT_C * y ** 3)) / (A * A)
+    if name == "rectifiedtanh":
+        t = np.tanh(z)
+        return np.where(z > 0, 1 - t * t, 0.0)
+    return np.where(z > a, 1.0, 0.0)        # thresholdedrelu
+
+
+def act_forward(name: str, z: np.ndarray, alpha: float = 0.01, q: Quirks = DEFAULT_QUIRKS) -> np.ndarray:
+    if name in EXT_ACTS:
+        return forward(name, z, alpha, q)
     if name == "identity":
         return z
     if name == "tanh":
@@ -82,7 +200,9 @@ def act_forward(name: str, z: np.ndarray, alpha: float = 0.01) -> np.ndarray:
     raise ValueError(name)
 
 
-def act_backward(name: str, z: np.ndarray, eps: np.ndarray, alpha: float = 0.01) -> np.ndarray:
+def act_backward(name: str, z: np.ndarray, eps: np.ndarray, alpha: float = 0.01, q: Quirks = DEFAULT_QUIRKS) -> np.ndarray:
+    if name in EXT_ACTS:
+        return eps * derivative(name, z, alpha, q)
     if name == "identity":
         return eps
     if name == "tanh":
@@ -98,23 +218,39 @@ def act_backward(name: str, z: np.ndarray, eps: np.ndarray, alpha: float = 0.01)
     raise ValueError(name)
 
 
-ACTS = ("identity", "tanh", "sigmoid", "relu", "lrelu")
+# The layers call the activations through these bindings, so code that wraps the module's act_forward / act_backward for its own calls
+# does not change what a Net computes.
+_layer_act_forward, _layer_act_backward = act_forward, act_backward
 
 
 # --------------------------------------------------------------------------------------------------
-# Updater configs (org.nd4j.linalg.learning.config.{RmsProp,Adam,Sgd,NoOp})
+# Updaters (org.nd4j.linalg.learning.config.* / org.nd4j.linalg.learning.*Updater).  With t = iteration + 1:
+#   rmsprop    c = rho*c + (1-rho)*g^2;  u = lr*g / (sqrt(c) + eps)                       (c starts at eps)
+#   adam       m, v;  u = lr*sqrt(1-b2^t)/(1-b1^t) * m / (sqrt(v) + eps)
+#   nesterovs  vPrev = v;  v = mu*v - lr*g;  u = mu*vPrev - (1+mu)*v
+#   adagrad    h += g^2;  u = lr*g / (sqrt(h) + eps)                                   (h starts at eps)
+#   adamax     m = b1*m + (1-b1)*g;  u_inf = max(b2*u_inf, |g|) + 1e-32;  u = lr/(1-b1^t) * m / u_inf
+#   nadam      Adam's m, v;  u = lr * (b1*m + (1-b1)*g) / (1-b1^t) / (sqrt(v) + eps)
+#   amsgrad    Adam's m, v;  vhat = max(vhat, v);  u = lr*sqrt(1-b2^t)/(1-b1^t) * m / (sqrt(vhat) + eps)
+#   adadelta   msg = rho*msg + (1-rho)*g^2;  u = sqrt(msdx + eps)/sqrt(msg + eps) * g;  msdx = rho*msdx + (1-rho)*u^2   (no learning rate)
+#   sgd        u = lr*g;   noop  u = g
+# The state slots of a parameter are in the library's order (state0, state1, state2).
 # --------------------------------------------------------------------------------------------------
+EXT_UPDATERS = ("nesterovs", "adagrad", "adamax", "nadam", "amsgrad", "adadelta")
+N_STATE = {"sgd": 0, "noop": 0, "rmsprop": 1, "adam": 2, "nesterovs": 1, "adagrad": 1, "adamax": 2, "nadam": 2, "amsgrad": 3, "adadelta": 2}
+
+
 @dataclasses.dataclass
 class UpdaterCfg:
-    kind: str = "sgd"            # "sgd" | "rmsprop" | "adam" | "noop"
+    kind: str = "sgd"            # one of N_STATE
     lr: float = 1e-3
     rms_decay: float = 0.95      # NB: reference passes RmsProp(lr, 1e-8, 1e-8) => rms_decay = 1e-8 (J:133)
-    beta1: float = 0.9
+    beta1: float = 0.9           # Nesterovs' momentum and AdaDelta's rho, as in b2g_layer_desc
     beta2: float = 0.999
     eps: float = 1e-8
 
     def state_mult(self) -> int:
-        return {"sgd": 0, "noop": 0, "rmsprop": 1, "adam": 2}[self.kind]
+        return N_STATE[self.kind]
 
 
 def RmsProp(lr, rms_decay=0.95, eps=1e-8):
@@ -128,6 +264,178 @@ def Adam(lr=1e-3, beta1=0.9, beta2=0.999, eps=1e-8):
 
 def Sgd(lr):
     return UpdaterCfg("sgd", lr=lr)
+
+
+def updater_cfg(u) -> Optional[UpdaterCfg]:
+    """An updater spec dict (gan_deeplearning4j_b200.models) -> UpdaterCfg; a scheduled lr gives its value at 0, the constant the library
+    keeps for it."""
+    if u is None:
+        return None
+    k = u["kind"]
+    lr = u.get("lr", 0.0)
+    if isinstance(lr, dict):
+        lr = value(lr, 0)
+    if k == "rmsprop":
+        return RmsProp(lr, u.get("rms_decay", 0.95), u.get("eps", 1e-8))
+    if k == "adam":
+        return Adam(lr, u.get("beta1", 0.9), u.get("beta2", 0.999), u.get("eps", 1e-8))
+    if k == "sgd":
+        return Sgd(lr)
+    if k == "noop":
+        return UpdaterCfg("noop")
+    if k == "nesterovs":
+        return UpdaterCfg(k, lr=lr, beta1=u.get("momentum", 0.9))
+    if k == "adagrad":
+        return UpdaterCfg(k, lr=lr, eps=u.get("eps", 1e-6))
+    if k == "adadelta":
+        return UpdaterCfg(k, lr=0.0, beta1=u.get("rho", 0.95), eps=u.get("eps", 1e-6))
+    if k in ("adamax", "nadam", "amsgrad"):
+        return UpdaterCfg(k, lr=lr, beta1=u.get("beta1", 0.9), beta2=u.get("beta2", 0.999), eps=u.get("eps", 1e-8))
+    raise ValueError(f"unknown updater kind {k!r}")
+
+
+def init_state(u: UpdaterCfg, shape, dtype=np.float64, q: Quirks = DEFAULT_QUIRKS) -> List[np.ndarray]:
+    """The initial state slots of one parameter tensor."""
+    if u.kind == "rmsprop":
+        return [np.full(shape, u.eps if q.rmsprop_cache_init_eps else 0.0, dtype)]
+    st = [np.zeros(shape, dtype) for _ in range(N_STATE[u.kind])]
+    if u.kind == "adagrad" and q.adagrad_history_init_eps:
+        st[0][...] = u.eps
+    return st
+
+
+def update(u: UpdaterCfg, st, g, t: int, q: Quirks = DEFAULT_QUIRKS, lr: Optional[float] = None):
+    """The updater step u(g) of one parameter tensor at t = iteration + 1 and learning rate lr (None: u.lr); the state slots st are updated
+    in place."""
+    lr, b1, b2, eps = u.lr if lr is None else lr, u.beta1, u.beta2, u.eps
+    if u.kind == "noop":
+        return g
+    if u.kind == "sgd":
+        return lr * g
+    if u.kind == "rmsprop":
+        c = st[0]
+        c[...] = u.rms_decay * c + (1 - u.rms_decay) * g * g
+        return lr * g / (np.sqrt(c) + eps)
+    if u.kind == "adam":
+        m, v = st
+        m[...] = b1 * m + (1 - b1) * g
+        v[...] = b2 * v + (1 - b2) * g * g
+        if q.adam_eps_outside:
+            alpha_t = lr * np.sqrt(1 - b2 ** t) / (1 - b1 ** t)
+            return alpha_t * m / (np.sqrt(v) + eps)
+        return lr * (m / (1 - b1 ** t)) / (np.sqrt(v / (1 - b2 ** t)) + eps)
+    if u.kind == "nesterovs":
+        v = st[0]; v_prev = v.copy()
+        v[...] = b1 * v - lr * g
+        return b1 * v_prev - (1 + b1) * v
+    if u.kind == "adagrad":
+        h = st[0]
+        h[...] = h + g * g
+        return lr * g / (np.sqrt(h) + eps)
+    if u.kind == "adamax":
+        m, ui = st
+        m[...] = b1 * m + (1 - b1) * g
+        if q.adamax_floor_no_eps:
+            ui[...] = np.maximum(b2 * ui, np.abs(g)) + 1e-32
+            return lr / (1 - b1 ** t) * m / ui
+        ui[...] = np.maximum(b2 * ui, np.abs(g))
+        return lr / (1 - b1 ** t) * m / (ui + eps)
+    if u.kind in ("nadam", "amsgrad"):
+        m, v = st[0], st[1]
+        m[...] = b1 * m + (1 - b1) * g
+        v[...] = b2 * v + (1 - b2) * g * g
+        if u.kind == "nadam":
+            vv = v if q.nadam_v_uncorrected else v / (1 - b2 ** t)
+            return lr * (b1 * m + (1 - b1) * g) / (1 - b1 ** t) / (np.sqrt(vv) + eps)
+        vh = st[2]
+        vh[...] = np.maximum(vh, v)
+        return lr * np.sqrt(1 - b2 ** t) / (1 - b1 ** t) * m / (np.sqrt(vh) + eps)
+    if u.kind == "adadelta":
+        msg, msdx = st
+        msg[...] = b1 * msg + (1 - b1) * g * g
+        d = np.sqrt(msdx + eps) / np.sqrt(msg + eps) * g
+        msdx[...] = b1 * msdx + (1 - b1) * d * d
+        return d
+    raise ValueError(u.kind)
+
+
+# --------------------------------------------------------------------------------------------------
+# Learning-rate schedules (org.nd4j.linalg.schedule.ISchedule).  value(i) in double, i = the iteration count before the update's increment
+# (ITERATION) or the epoch count (EPOCH):
+#   exponential  initial * gamma^i                       inverse  initial / (1 + gamma*i)^power
+#   sigmoid      initial / (1 + exp(-gamma*(i - step)))  step     initial * decay_rate^floor(i / step)
+#   map          the value at the largest key <= i
+# The updater uses value(i) rounded to fp32 once in place of its constant lr.  The schedules are the dicts gan_deeplearning4j_b200.models
+# builds.
+# --------------------------------------------------------------------------------------------------
+def value(sched, i) -> float:
+    """ISchedule.valueAt in double for the schedule's own counter value i."""
+    k, i = sched["schedule"], float(i)
+    if k == "exponential":
+        return sched["initial"] * math.pow(sched["gamma"], i)
+    if k == "inverse":
+        return sched["initial"] / math.pow(1.0 + sched["gamma"] * i, sched["power"])
+    if k == "sigmoid":
+        return sched["initial"] / (1.0 + math.exp(-sched["gamma"] * (i - sched["step"])))
+    if k == "step":
+        return sched["initial"] * math.pow(sched["decay_rate"], math.floor(i / sched["step"]))
+    if k == "map":
+        best = None
+        for key, v in sched["values"]:
+            if key <= i and (best is None or key > best[0]):
+                best = (key, v)
+        assert best is not None, "a MapSchedule must hold key 0"
+        return float(best[1])
+    raise ValueError(k)
+
+
+def lr_at(sched, iteration: int, epoch: int) -> np.float32:
+    """The fp32 learning rate of an update at (iteration before the increment, epoch)."""
+    return np.float32(value(sched, epoch if sched.get("type", "iteration") == "epoch" else iteration))
+
+
+# --------------------------------------------------------------------------------------------------
+# L2 gradient normalization (BaseMultiLayerUpdater.preApply), between the division by mb and the updater:
+#   renormalize_l2_per_layer        g <- g / ||g_layer||  (a zero norm divides by `l2norm_zero_floor` instead; the threshold is ignored)
+#   renormalize_l2_per_param_type   the same per parameter tensor
+#   clip_l2_per_layer               g <- g * threshold / ||g_layer||  when ||g_layer|| > threshold
+#   clip_l2_per_param_type          the same per parameter tensor
+# A layer is one layer with parameters that is not frozen; its BatchNorm mean/var pseudo-gradients (not divided by mb) are inside its norm
+# and scaled with it when `bn_stats_normalized` holds.  The multiplier is rounded to fp32 once, as the library does.
+# --------------------------------------------------------------------------------------------------
+GRAD_NORMS = ("none", "renormalize_l2_per_layer", "renormalize_l2_per_param_type", "clip_l2_per_layer", "clip_l2_per_param_type")
+
+
+def multiplier(sumsq: float, mode: str, threshold: float, q: Quirks = DEFAULT_QUIRKS) -> np.float32:
+    """The fp32 multiplier of one norm group from its sum of squares."""
+    norm = math.sqrt(sumsq)
+    if mode.startswith("renormalize"):
+        return np.float32(1.0 / (norm if norm != 0.0 else q.l2norm_zero_floor))
+    thr = float(np.float32(threshold))
+    return np.float32(thr / norm) if norm > thr else np.float32(1.0)
+
+
+def norm_groups(net, g, mode, q: Quirks = DEFAULT_QUIRKS):
+    """The mode's norm groups over the divided gradients g: lists of (layer, param) keys, in parameter order."""
+    groups = {}
+    for (li, p) in g:
+        l = net.layers[li]
+        if p in l.noop_names() and not q.bn_stats_normalized:
+            continue
+        groups.setdefault(li if mode.endswith("per_layer") else (li, p), []).append((li, p))
+    return list(groups.values())
+
+
+def normalize(net, g, mode, threshold, q: Quirks = DEFAULT_QUIRKS):
+    """Applies the mode to the divided gradients g {(layer, param): g} (a new dict); also returns the groups' norms."""
+    out, norms = dict(g), []
+    for keys in norm_groups(net, g, mode, q):
+        ss = sum(float((np.asarray(g[k], np.float64) ** 2).sum()) for k in keys)
+        norms.append(math.sqrt(ss))
+        m = multiplier(ss, mode, threshold, q)
+        for k in keys:
+            out[k] = g[k] * float(m)
+    return out, norms
 
 
 # --------------------------------------------------------------------------------------------------
@@ -168,6 +476,7 @@ class Layer:
     updater: Optional[UpdaterCfg] = None
     l2: float = 0.0
     has_params = False
+    q: Quirks = DEFAULT_QUIRKS      # a Net gives its quirks to the layers that have none of their own
 
     def param_specs(self) -> List[Tuple[str, Tuple[int, ...], str]]:
         return []
@@ -231,10 +540,10 @@ class Conv2D(Layer):
         if self.has_bias:
             z2d = z2d + self.params["b"]
         self._z = z2d.reshape(n, oh, ow, self.n_out).transpose(0, 3, 1, 2)
-        return act_forward(self.activation, self._z, self.alpha)
+        return _layer_act_forward(self.activation, self._z, self.alpha, self.q)
 
     def backward(self, eps):
-        delta = act_backward(self.activation, self._z, eps, self.alpha)
+        delta = _layer_act_backward(self.activation, self._z, eps, self.alpha, self.q)
         n, o, oh, ow = delta.shape
         d2d = delta.transpose(0, 2, 3, 1).reshape(-1, o)
         self.grads["W"] = (d2d.T @ self._cols2d).reshape(self.params["W"].shape)
@@ -289,10 +598,10 @@ class Deconv2D(Layer):
         if self.has_bias:
             z = z + self.params["b"][None, :, None, None]
         self._z = z
-        return act_forward(self.activation, z, self.alpha)
+        return _layer_act_forward(self.activation, z, self.alpha, self.q)
 
     def backward(self, eps):
-        delta = act_backward(self.activation, self._z, eps, self.alpha)
+        delta = _layer_act_backward(self.activation, self._z, eps, self.alpha, self.q)
         n, c, h, w = self._x_shape
         dcols = np.ascontiguousarray(im2col(delta, *self.k, *self.s, *self.p)).reshape(n * h * w, -1)  # [pix, Cout*kH*kW]
         self.grads["W"] = (self._x2d.T @ dcols).reshape(self.params["W"].shape)
@@ -332,10 +641,10 @@ class Dense(Layer):
         self._z = x @ self.params["W"]
         if self.has_bias:
             self._z = self._z + self.params["b"]
-        return act_forward(self.activation, self._z, self.alpha)
+        return _layer_act_forward(self.activation, self._z, self.alpha, self.q)
 
     def backward(self, eps):
-        delta = act_backward(self.activation, self._z, eps, self.alpha)
+        delta = _layer_act_backward(self.activation, self._z, eps, self.alpha, self.q)
         self._delta = delta
         self.grads["W"] = self._x.T @ delta
         if self.has_bias:
@@ -408,10 +717,10 @@ class ActivationLayer(Layer):
 
     def forward(self, x, train):
         self._z = x
-        return act_forward(self.activation, x, self.alpha)
+        return _layer_act_forward(self.activation, x, self.alpha, self.q)
 
     def backward(self, eps):
-        return act_backward(self.activation, self._z, eps, self.alpha)
+        return _layer_act_backward(self.activation, self._z, eps, self.alpha, self.q)
 
 
 class MaxPool(Layer):
@@ -441,6 +750,141 @@ class MaxPool(Layer):
         dflat = np.zeros((n, oh, ow, c, kh * kw), dtype=eps.dtype)
         np.put_along_axis(dflat, self._arg[..., None], eps.transpose(0, 2, 3, 1)[..., None], -1)
         return col2im(dflat.reshape(n, oh, ow, c, kh, kw), self._x_shape, kh, kw, *self.s, 0, 0)
+
+
+# Average, sum and p-norm pooling (b2g_pooling), in float64.  Truncate geometry OH = (H + 2 ph - kh) / sh + 1; positions outside the input
+# are zero padding.
+#   AVG    y = window sum / (kh*kw)                dx += eps / (kh*kw)
+#   SUM    y = window sum                          dx += eps
+#   PNORM  y = (sum |x|^p)^(1/p)                   dx += eps * sign(x)|x|^(p-1) / max(y^(p-1), 1e-8)
+# GlobalPoolingLayer pools over H x W to [mb, C]; MAX routes eps to the first maximum in row-major pixel order.  The p-norm floor is
+# SubsamplingLayer's eps; DL4J's GlobalPoolingLayer has no floor (a zero map gives NaN there), so for global pooling the floor is a
+# deliberate deviation of the library, kept here as the default.
+POOLINGS = ("max", "avg", "sum", "pnorm")
+POOL_CODES = {k: i for i, k in enumerate(POOLINGS)}
+PNORM_EPS = 1e-8
+
+
+def _pnorm_den(y, p, q):
+    d = y ** (p - 1)
+    return np.maximum(d, PNORM_EPS) if q.pnorm_denominator_floor else d
+
+
+def _pnorm_num(x, p):
+    return np.sign(x) * np.abs(x) ** (p - 1)
+
+
+def pool2d_forward(kind, x, kernel, stride, padding, p=2, q: Quirks = DEFAULT_QUIRKS):
+    """x [N,C,H,W] float64 -> y [N,C,OH,OW]."""
+    (kh, kw), (sh, sw), (ph, pw) = kernel, stride, padding
+    cols = im2col(np.asarray(x, np.float64), kh, kw, sh, sw, ph, pw)          # [N,OH,OW,C,kh,kw], zero padded
+    if kind == "avg":
+        if q.avg_include_pad_in_divisor:
+            div = kh * kw
+        else:
+            div = im2col(np.ones((1, 1) + x.shape[2:]), kh, kw, sh, sw, ph, pw).sum((-2, -1))[0, :, :, 0][None, :, :, None]
+        y = cols.sum((-2, -1)) / div
+    elif kind == "sum":
+        y = cols.sum((-2, -1))
+    elif kind == "pnorm":
+        y = (np.abs(cols) ** p).sum((-2, -1)) ** (1.0 / p)
+    else:
+        raise ValueError(kind)
+    return y.transpose(0, 3, 1, 2)
+
+
+def pool2d_backward(kind, x, y, eps, kernel, stride, padding, p=2, q: Quirks = DEFAULT_QUIRKS):
+    """dL/dx [N,C,H,W] from eps = dL/dy [N,C,OH,OW] (y = the forward's output)."""
+    (kh, kw), (sh, sw), (ph, pw) = kernel, stride, padding
+    x = np.asarray(x, np.float64)
+    e = np.asarray(eps, np.float64).transpose(0, 2, 3, 1)[..., None, None]      # [N,OH,OW,C,1,1]
+    shape = e.shape[:4] + (kh, kw)
+    if kind == "avg":
+        if q.avg_include_pad_in_divisor:
+            dcols = np.broadcast_to(e / (kh * kw), shape)
+        else:
+            cnt = im2col(np.ones((1, 1) + x.shape[2:]), kh, kw, sh, sw, ph, pw).sum((-2, -1))[0, :, :, 0][None, :, :, None, None, None]
+            dcols = np.broadcast_to(e / cnt, shape)
+    elif kind == "sum":
+        dcols = np.broadcast_to(e, shape)
+    elif kind == "pnorm":
+        cols = im2col(x, kh, kw, sh, sw, ph, pw)
+        yy = np.asarray(y, np.float64).transpose(0, 2, 3, 1)[..., None, None]
+        dcols = e * _pnorm_num(cols, p) / _pnorm_den(yy, p, q)
+    else:
+        raise ValueError(kind)
+    return col2im(np.ascontiguousarray(dcols), x.shape, kh, kw, sh, sw, ph, pw)
+
+
+def global_forward(kind, x, p=2, q: Quirks = DEFAULT_QUIRKS):
+    """x [N,C,H,W] (or [N,C]) -> (y [N,C], MAX's row-major pixel index [N,C] or None)."""
+    x = np.asarray(x, np.float64)
+    f = x.reshape(x.shape[0], x.shape[1], -1)
+    if kind == "max":
+        idx = f.argmax(-1) if q.global_max_first_tie else f.shape[-1] - 1 - f[..., ::-1].argmax(-1)
+        return np.take_along_axis(f, idx[..., None], -1)[..., 0], idx
+    if kind == "avg":
+        return f.mean(-1), None
+    if kind == "sum":
+        return f.sum(-1), None
+    if kind == "pnorm":
+        return (np.abs(f) ** p).sum(-1) ** (1.0 / p), None
+    raise ValueError(kind)
+
+
+def global_backward(kind, x, y, idx, eps, p=2, q: Quirks = DEFAULT_QUIRKS):
+    x = np.asarray(x, np.float64)
+    f = x.reshape(x.shape[0], x.shape[1], -1)
+    e = np.asarray(eps, np.float64)[..., None]
+    if kind == "max":
+        d = np.zeros_like(f)
+        np.put_along_axis(d, idx[..., None], e, -1)
+    elif kind == "avg":
+        d = np.broadcast_to(e / f.shape[-1], f.shape)
+    elif kind == "sum":
+        d = np.broadcast_to(e, f.shape)
+    elif kind == "pnorm":
+        d = e * _pnorm_num(f, p) / _pnorm_den(np.asarray(y, np.float64)[..., None], p, q)
+    else:
+        raise ValueError(kind)
+    return np.ascontiguousarray(d).reshape(x.shape)
+
+
+class Subsampling(Layer):
+    """SubsamplingLayer.Builder(PoolingType.AVG / SUM / PNORM).kernelSize().stride().padding().pnorm()."""
+
+    def __init__(self, kind, kernel, stride=(1, 1), padding=(0, 0), p=2, name=""):
+        self.kind, self.k, self.s, self.pad, self.p, self.name = kind, tuple(kernel), tuple(stride), tuple(padding), p, name
+
+    def out_shape(self, s):
+        n, c, h, w = s
+        return (n, c, out_size(h, self.k[0], self.s[0], self.pad[0]), out_size(w, self.k[1], self.s[1], self.pad[1]))
+
+    def forward(self, x, train):
+        self._x = x
+        self._y = pool2d_forward(self.kind, x, self.k, self.s, self.pad, self.p, self.q)
+        return self._y
+
+    def backward(self, eps):
+        return pool2d_backward(self.kind, self._x, self._y, eps, self.k, self.s, self.pad, self.p, self.q)
+
+
+class GlobalPooling(Layer):
+    """GlobalPoolingLayer.Builder(PoolingType).pnorm(p): [N,C,H,W] -> [N,C]."""
+
+    def __init__(self, kind="max", p=2, name=""):
+        self.kind, self.p, self.name = kind, p, name
+
+    def out_shape(self, s):
+        return (s[0], s[1])
+
+    def forward(self, x, train):
+        self._x = x
+        self._y, self._idx = global_forward(self.kind, x, self.p, self.q)
+        return self._y
+
+    def backward(self, eps):
+        return global_backward(self.kind, self._x, self._y, self._idx, eps, self.p, self.q)
 
 
 class Upsample2D(Layer):
@@ -484,6 +928,87 @@ class Reshape(Layer):
         return eps.reshape(self._in_shape)
 
 
+# DropoutLayer.Builder(p), p = the RETAIN probability: training forward y = x * m, m = 1/p with probability p else 0; backward dx = dy * m;
+# inference and a FrozenLayer are the identity.  ND4J's random stream cannot be restated, so the mask is the CUDA library's own definition
+# (include/b200gan.h, B2G_LAYER_DROPOUT), restated exactly: parity with DL4J holds in distribution, with the library element for element.
+_M32 = np.uint64(0xFFFFFFFF)
+
+
+def philox4x32_10(ctr, key):
+    """Philox4x32-10 (Random123 constants), vectorised: ctr = 4 arrays / ints of 32-bit words, key = 2.  Returns the 4 output words (uint32)."""
+    c = [np.asarray(v, np.uint64) & _M32 for v in ctr]
+    k0, k1 = (np.uint64(int(v) & 0xFFFFFFFF) for v in key)
+    m0, m1, w0, w1, sh = np.uint64(0xD2511F53), np.uint64(0xCD9E8D57), np.uint64(0x9E3779B9), np.uint64(0xBB67AE85), np.uint64(32)
+    for r in range(10):
+        if r:
+            k0, k1 = (k0 + w0) & _M32, (k1 + w1) & _M32
+        p0, p1 = m0 * c[0], m1 * c[2]          # 32 x 32 -> 64-bit products, exact in uint64
+        c = [(p1 >> sh) ^ c[1] ^ k0, p1 & _M32, (p0 >> sh) ^ c[3] ^ k1, p0 & _M32]
+    return [v.astype(np.uint32) for v in c]
+
+
+def dropout_mask(seed, rank, layer, pass_, rows, h, w, c, p, row0=0):
+    """Keep mask of a DropoutLayer (True = kept) for rows [row0, row0 + rows) of pass `pass_`, returned NCHW [rows, c, h, w].  Element
+    e = ((row*h + y)*w + x)*c + ch (NHWC index in the pass) keeps iff p >= 1 or Philox4x32-10(ctr = {e >> 2, lo32(P), hi32(P), layer | rank << 16},
+    key = {lo32(S), hi32(S)})[e & 3] < floor(p * 2^32), with p taken as fp32 and S = seed (0 -> 666)."""
+    p = np.float32(p)
+    per = h * w * c
+    e0, e1 = row0 * per, (row0 + rows) * per
+    if p >= 1:
+        keep = np.ones(e1 - e0, bool)
+    else:
+        seed, pass_ = int(seed) or 666, int(pass_)
+        g = np.arange(e0 >> 2, ((e1 - 1) >> 2) + 1, dtype=np.uint64)
+        words = np.stack(philox4x32_10((g, pass_ & 0xFFFFFFFF, pass_ >> 32, int(layer) | (int(rank) << 16)), (seed & 0xFFFFFFFF, seed >> 32)), -1).ravel()
+        keep = words[e0 - 4 * (e0 >> 2):][:e1 - e0] < np.uint64(math.floor(float(p) * 2.0 ** 32))
+    return keep.reshape(rows, h, w, c).transpose(0, 3, 1, 2)
+
+
+class DropoutState:
+    """The mask inputs a net's DropoutLayers share: seed (the library's b2g_net_config.seed), rank, pass counter P, explicit draws.  Like the
+    library, the last masking DropoutLayer of a train-mode forward advances P once it has drawn its mask; `queue` holds explicit (pass, first
+    row) draws that replace the counter for the next forwards without advancing it."""
+
+    def __init__(self, seed=666, rank=0):
+        self.seed, self.rank, self.pass_, self.queue = seed, rank, 0, []
+
+    def current(self):
+        return self.queue[0] if self.queue else (self.pass_, 0)
+
+    def finish(self):          # end of a masking train-mode forward
+        if self.queue:
+            self.queue.pop(0)
+        else:
+            self.pass_ += 1
+
+
+class Dropout(Layer):
+    """DropoutLayer.Builder(p).  `index` = the layer's chain index in the CUDA library's layer array (the mask's L).  A Net shares its
+    DropoutState among its DropoutLayers."""
+
+    def __init__(self, p, name="", index=0, state=None, frozen=False):
+        self.p, self.name, self.index, self.state, self.frozen, self.last = float(np.float32(p)), name, index, state, frozen, False
+        self._m = None
+
+    def active(self):
+        return self.p < 1 and not self.frozen
+
+    def forward(self, x, train):
+        self._m = None
+        if not train or self.p >= 1:
+            return x
+        pass_, row0 = self.state.current()
+        _, c, h, w = x.shape if x.ndim == 4 else (x.shape[0], x.shape[1], 1, 1)
+        keep = dropout_mask(self.state.seed, self.state.rank, self.index, pass_, x.shape[0], h, w, c, self.p, row0).reshape(x.shape)
+        self._m = keep * x.dtype.type(np.float32(1) / np.float32(self.p))
+        if self.last:
+            self.state.finish()
+        return x * self._m
+
+    def backward(self, eps):
+        return eps if self._m is None else eps * self._m
+
+
 def xent_score_and_grad(z: np.ndarray, y: np.ndarray, clip_eps: float):
     """LossBinaryXENT with a sigmoid activation (J:159-163).  Returns (sum of per-example losses, dL/dz).
 
@@ -501,39 +1026,109 @@ def xent_score_and_grad(z: np.ndarray, y: np.ndarray, clip_eps: float):
     return loss.sum(), grad
 
 
+# Regression and margin losses (b2g_loss codes 2-8; org.nd4j.linalg.lossfunctions.impl.*).  Each is ILossFunction.computeGradient(labels,
+# preOutput, activationFn): a = act(z), dL/dz = dL/da * act'(a) with the derivative taken from the output a, per-example scores summed over
+# the nOut outputs:
+#   mse            sum (a-y)^2 / nOut          2(a-y) / nOut
+#   l1             sum |a-y|                   sign(a-y)              (sign(0) = 0)
+#   l2             sum (a-y)^2                 2(a-y)
+#   mae            sum |a-y| / nOut            sign(a-y) / nOut
+#   hinge          sum max(0, 1 - y a)         -y where 1 - y a > 0 (strictly), else 0
+#   squared_hinge  sum max(0, 1 - y a)^2       -2y max(0, 1 - y a)
+#   wasserstein    sum y a / nOut              y / nOut               (the / nOut: Quirks.wasserstein_per_output)
+# On an activation of codes 5-16 the loss takes a = f(z) with the identity and multiplies dL/da by f'(z).
+LOSSES = ("mse", "l1", "l2", "mae", "hinge", "squared_hinge", "wasserstein")
+LOSS_CODES = {"mse": 2, "l1": 3, "l2": 4, "mae": 5, "hinge": 6, "squared_hinge": 7, "wasserstein": 8}
+
+
+def act_grad_from_out(act: str, a: np.ndarray, alpha: float = 0.01) -> np.ndarray:
+    """f'(z) from the output a = f(z), as the library's act_grad_from_out takes it (LeakyReLU: sign(a) = sign(z) for alpha > 0)."""
+    if act == "identity":
+        return np.ones_like(a)
+    if act == "tanh":
+        return 1 - a * a
+    if act == "sigmoid":
+        return a * (1 - a)
+    if act == "relu":
+        return (a > 0).astype(a.dtype)
+    if act == "lrelu":
+        return np.where(a > 0, 1.0, alpha).astype(a.dtype)
+    raise ValueError(act)
+
+
+def per_output(loss: str, q: Quirks = DEFAULT_QUIRKS) -> bool:
+    """Whether the loss divides its score and gradient by nOut."""
+    return loss in ("mse", "mae") or (loss == "wasserstein" and q.wasserstein_per_output)
+
+
+def score_and_grad(loss: str, act: str, alpha: float, z: np.ndarray, y: np.ndarray, q: Quirks = DEFAULT_QUIRKS):
+    """z, y: [N, nOut].  Returns (sum over the N examples of the per-example scores, dL/dz [N, nOut])."""
+    if act in EXT_ACTS:
+        s, g = score_and_grad(loss, "identity", 0.0, forward(act, z, alpha, q), y, q)
+        return s, g * derivative(act, z, alpha, q)
+    a = act_forward(act, z, alpha)
+    e, m = a - y, 1 - y * a
+    if loss in ("mse", "l2"):
+        s, g = (e * e).sum(), 2 * e
+    elif loss in ("l1", "mae"):
+        s, g = np.abs(e).sum(), np.sign(e)
+    elif loss == "hinge":
+        s, g = np.maximum(m, 0).sum(), np.where(m > 0, -y, 0.0)
+    elif loss == "squared_hinge":
+        s, g = (np.maximum(m, 0) ** 2).sum(), -2 * y * np.maximum(m, 0)
+    elif loss == "wasserstein":
+        s, g = (y * a).sum(), y * np.ones_like(a)
+    else:
+        raise ValueError(loss)
+    if per_output(loss, q):
+        n = z.shape[1]
+        s, g = s / n, g / n
+    return float(s), g * act_grad_from_out(act, a, alpha)
+
+
+def _loss_score_and_grad(layer, z, y):
+    if layer.loss == "xent":
+        return xent_score_and_grad(z, y, layer.q.xent_clip_eps)
+    return score_and_grad(layer.loss, layer.loss_act, layer.loss_alpha, z, y, layer.q)
+
+
 class LossLayer(Layer):
-    """o.d.nn.conf.layers.LossLayer(XENT, sigmoid): loss on the incoming pre-activations, no parameters.
-    Accepts [N,1] or [N,1,1,1] (DCGAN D-last conv emits the logit)."""
+    """o.d.nn.conf.layers.LossLayer(loss, activation): the loss on activation(incoming pre-activations), no parameters.  XENT is on the
+    sigmoid.  Accepts [N,nOut] or [N,nOut,1,1] (DCGAN D-last conv emits the logit)."""
 
-    def __init__(self, name="", quirks: Quirks = DEFAULT_QUIRKS):
-        self.name, self.q = name, quirks
-
-    def init(self, rng, dtype):
-        super().init(rng, dtype)
+    def __init__(self, name="", quirks: Optional[Quirks] = None, loss="xent", activation="identity", alpha=0.01):
+        self.name, self.loss, self.loss_alpha = name, loss, alpha
+        if quirks is not None:
+            self.q = quirks
+        self.loss_act = "sigmoid" if loss == "xent" else activation
 
     def forward(self, x, train):
         self._z = x
-        return _sigmoid(x)
+        return _layer_act_forward(self.loss_act, x, self.loss_alpha, self.q)
 
     def score_and_eps(self, y):
         z = self._z
-        s, g = xent_score_and_grad(z.reshape(y.shape), y, self.q.xent_clip_eps)
+        s, g = _loss_score_and_grad(self, z.reshape(y.shape), y)
         return s, g.reshape(z.shape)
 
 
 class Output(Dense):
-    """OutputLayer(XENT).activation(SIGMOID).nOut(1) (J:159-163) = Dense + LossBinaryXENT."""
+    """OutputLayer.Builder(loss).activation(act).nOut(n) = Dense + the loss on act(z); XENT is on the sigmoid (J:159-163)."""
 
-    def __init__(self, n_in, n_out, updater=None, l2=0.0, name="", quirks: Quirks = DEFAULT_QUIRKS):
+    def __init__(self, n_in, n_out, updater=None, l2=0.0, name="", quirks: Optional[Quirks] = None, loss="xent", activation="identity",
+                 alpha=0.01):
         super().__init__(n_in, n_out, activation="identity", updater=updater, l2=l2, name=name)
-        self.q = quirks
+        if quirks is not None:
+            self.q = quirks
+        self.loss, self.loss_alpha = loss, alpha
+        self.loss_act = "sigmoid" if loss == "xent" else activation
 
     def forward(self, x, train):
-        z = super().forward(x, train)
-        return _sigmoid(z)
+        z = super().forward(x, train)          # the identity Dense: z; the loss applies the activation
+        return _layer_act_forward(self.loss_act, z, self.loss_alpha, self.q)
 
     def score_and_eps(self, y):
-        return xent_score_and_grad(self._z, y, self.q.xent_clip_eps)
+        return _loss_score_and_grad(self, self._z, y)
 
     def backward(self, eps):   # eps is already dL/dz
         self.grads["W"] = self._x.T @ eps
@@ -575,27 +1170,75 @@ class OutputSoftmax(Dense):
 # Network = ComputationGraph restricted to a chain (every graph in the reference is a chain).
 # --------------------------------------------------------------------------------------------------
 class Net:
+    """mask_seed, rank: the DropoutLayer masks' seed and rank (the library's b2g_net_config.seed and the replica's rank)."""
+
     def __init__(self, layers: Sequence[Layer], seed=666, dtype=np.float64, grad_clip: float = 0.0,
-                 quirks: Quirks = DEFAULT_QUIRKS):
+                 quirks: Quirks = DEFAULT_QUIRKS, mask_seed=666, rank=0):
         self.layers = list(layers)
         self.dtype = dtype
         self.grad_clip = grad_clip      # ClipElementWiseAbsoluteValue threshold (J:123-124); 0 = off
         self.q = quirks
-        self.iteration = 0
+        self.iteration = self.epoch = 0
+        self.gradient_normalization, self.gradient_normalization_threshold, self.grad_norm_last_norms = "none", 1.0, []
+        self.schedules: Dict[str, dict] = {}      # layer name -> schedule (None: the constant lr)
+        self.dropout = DropoutState(mask_seed, rank)
         rng = np.random.default_rng(seed)
         for l in self.layers:
+            if "q" not in vars(l):        # a layer built with its own quirks, or already in a net, keeps them
+                l.q = quirks
             l.init(rng, dtype)
+        drops = [l for l in self.layers if isinstance(l, Dropout)]
+        for l in drops:
+            l.state, l.last = self.dropout, False
+        active = [l for l in drops if l.active()]
+        if active:
+            active[-1].last = True
         self.state: Dict[Tuple[int, str], List[np.ndarray]] = {}
         for li, l in enumerate(self.layers):
             if not l.has_params:
                 continue
             u = l.updater or UpdaterCfg("sgd", 0.0)
             for pname, shape, _ in l.param_specs():
-                if u.kind == "rmsprop" and pname not in l.noop_names():
-                    init = u.eps if self.q.rmsprop_cache_init_eps else 0.0
-                    self.state[(li, pname)] = [np.full(shape, init, dtype)]
-                elif u.kind == "adam" and pname not in l.noop_names():
-                    self.state[(li, pname)] = [np.zeros(shape, dtype), np.zeros(shape, dtype)]
+                if N_STATE[u.kind] and pname not in l.noop_names():
+                    self.state[(li, pname)] = init_state(u, shape, dtype, self.q)
+
+    # ---- the library Net's settings ------------------------------------------------------------
+    def set_gradient_normalization(self, mode: str, threshold: float = 1.0):
+        """DL4J's GradientNormalization (one of GRAD_NORMS) for every layer, from the next update on."""
+        assert mode in GRAD_NORMS, mode
+        self.gradient_normalization, self.gradient_normalization_threshold = mode, threshold
+
+    def set_lr_schedule(self, schedule: Optional[dict], layer: Optional[str] = None):
+        """setLearningRate(ISchedule) (layer None: every layer whose updater has a learning rate) or setLearningRate(layer, ISchedule);
+        schedule None = back to the layer's constant lr."""
+        if layer is None:
+            names = [l.name for l in self.layers if l.has_params and l.updater is not None and l.updater.kind not in ("noop", "adadelta")]
+        else:
+            names = [layer]
+        for name in names:
+            self.schedules[name] = schedule
+
+    def learning_rate(self, layer: str) -> float:
+        """The learning rate the layer's next update uses: its schedule's fp32 value at the current iteration / epoch, else its constant."""
+        l = self.layer(layer)
+        return self._lr(l, l.updater)
+
+    def _lr(self, l: Layer, u: UpdaterCfg) -> float:
+        sched = self.schedules.get(l.name)
+        return float(lr_at(sched, self.iteration, self.epoch)) if sched is not None else u.lr
+
+    def set_epoch(self, epoch: int):
+        self.epoch = epoch
+
+    def dropout_pass(self) -> int:
+        """The dropout pass counter P: train-mode forwards that applied a DropoutLayer mask."""
+        return self.dropout.pass_
+
+    def set_dropout_pass(self, p: int):
+        self.dropout.pass_ = p
+
+    def _has_active_dropout(self) -> bool:
+        return any(isinstance(l, Dropout) and l.active() for l in self.layers)
 
     # ---- DL4J flattened parameter vector -------------------------------------------------------
     def param_table(self):
@@ -663,9 +1306,12 @@ class Net:
                     s += 0.5 * l.l2 * float((l.params[p].astype(np.float64) ** 2).sum())
         return s
 
-    def compute_gradient_and_score(self, x, y, collect=False):
-        """ComputationGraph.computeGradientAndScore: train-mode forward, XENT loss, backprop.
-        Gradients are minibatch *sums*; score = sum(loss)/mb + 0.5*l2*||W||^2."""
+    def compute_gradient_and_score(self, x, y, collect=False, pass_=None, row0=0):
+        """ComputationGraph.computeGradientAndScore: train-mode forward, loss, backprop.
+        Gradients are minibatch *sums*; score = sum(loss)/mb + 0.5*l2*||W||^2.
+        pass_: the DropoutLayers draw rows [row0, row0 + mb) of that pass, and the pass counter is left alone."""
+        if pass_ is not None and self._has_active_dropout():
+            self.dropout.queue.append((pass_, row0))
         out, acts = self.forward(x, train=True, collect=True)
         last = self.layers[-1]
         y = np.asarray(y, self.dtype)
@@ -693,38 +1339,29 @@ class Net:
 
     # ---- updater: BaseMultiLayerUpdater.update + UpdaterBlock + params.subi ----------------------
     def apply_update(self, mb: int, grads: Optional[Dict[Tuple[int, str], np.ndarray]] = None, frozen_from: Optional[int] = None):
-        """g/=mb -> clip -> updater -> +l2*W -> theta -= g.  (SURVEY.md section 8a row a9.)"""
+        """g/=mb -> L2 normalization -> clip -> updater at the layer's lr -> +l2*W -> theta -= g.  (SURVEY.md section 8a row a9.)"""
         t = self.iteration + 1
-        for li, l in enumerate(self.layers):
-            if not l.has_params or getattr(l, "frozen", False):     # FrozenLayer: no gradient, no update, no l2 decay
-                continue
-            u = l.updater or UpdaterCfg("sgd", 0.0)
-            for pname, shape, _ in l.param_specs():
+        live = [(li, l) for li, l in enumerate(self.layers)
+                if l.has_params and not getattr(l, "frozen", False)]     # FrozenLayer: no gradient, no update, no l2 decay
+        g_all = {}
+        for li, l in live:
+            for pname, _, _ in l.param_specs():
                 g = (grads[(li, pname)] if grads is not None else l.grads[pname]).astype(self.dtype).copy()
-                noop = pname in l.noop_names()
-                if not (noop and self.q.bn_stats_minibatch_exempt):
+                if not (pname in l.noop_names() and self.q.bn_stats_minibatch_exempt):
                     g = g / mb
+                g_all[(li, pname)] = g
+        if self.gradient_normalization != "none":
+            assert self.grad_clip == 0, "DL4J allows one gradient normalization per layer"
+            g_all, self.grad_norm_last_norms = normalize(self, g_all, self.gradient_normalization, self.gradient_normalization_threshold, self.q)
+        for li, l in live:
+            u = l.updater or UpdaterCfg("sgd", 0.0)
+            lr = self._lr(l, u)
+            for pname, _, _ in l.param_specs():
+                g = g_all[(li, pname)]
+                noop = pname in l.noop_names()
                 if self.grad_clip > 0 and (not noop or self.q.bn_stats_clipped):
                     g = np.clip(g, -self.grad_clip, self.grad_clip)
-                if noop or u.kind == "noop":
-                    upd = g
-                elif u.kind == "sgd":
-                    upd = u.lr * g
-                elif u.kind == "rmsprop":
-                    c = self.state[(li, pname)][0]
-                    c[...] = u.rms_decay * c + (1 - u.rms_decay) * g * g
-                    upd = u.lr * g / (np.sqrt(c) + u.eps)
-                elif u.kind == "adam":
-                    m, v = self.state[(li, pname)]
-                    m[...] = u.beta1 * m + (1 - u.beta1) * g
-                    v[...] = u.beta2 * v + (1 - u.beta2) * g * g
-                    if self.q.adam_eps_outside:
-                        alpha_t = u.lr * np.sqrt(1 - u.beta2 ** t) / (1 - u.beta1 ** t)
-                        upd = alpha_t * m / (np.sqrt(v) + u.eps)
-                    else:
-                        upd = u.lr * (m / (1 - u.beta1 ** t)) / (np.sqrt(v / (1 - u.beta2 ** t)) + u.eps)
-                else:
-                    raise ValueError(u.kind)
+                upd = g if noop else update(u, self.state.get((li, pname)), g, t, self.q, lr)
                 if l.l2 and pname in l.l2_names():
                     if self.q.l2_after_updater:
                         upd = upd + l.l2 * l.params[pname]
@@ -771,9 +1408,15 @@ def gan_step(G: Net, D: Net, x_real, z_d, z_g, y_real, y_fake, y_gen, fake_bn_tr
       3. G grads through D on z_g with labels y_gen (J:465-471): G and D both run train-mode BN; D's
          parameters, running stats and updater state are NOT touched (the reference's lr-0 "frozen" copy
          is overwritten from dis next iteration, J:429-460); one G updater step.
+    D's DropoutLayers draw as the library draws them, which runs the two D minibatches as one 2N-row pass: the real and fake minibatches are
+    rows [0, N) and [N, 2N) of pass P, and the G step's D pass is P + 1 (the counter ends at P + 2).
     Returns dict(loss_d_real, loss_d_fake, loss_g, x_fake).
     """
     n = x_real.shape[0]
+    if D._has_active_dropout():
+        P = D.dropout.pass_
+        D.dropout.queue += [(P, 0), (P, n)]
+        D.dropout.pass_ = P + 1
     x_fake = G.forward(z_d, train=fake_bn_train)
     # --- D step
     s_real = D.compute_gradient_and_score(x_real, y_real) - D.l2_score()
@@ -848,7 +1491,7 @@ def reference_discriminator(lr=0.002, dtype=np.float64, seed=666, prefix="dis", 
         MaxPool((2, 2), (1, 1), name=f"{prefix}_maxpool_layer_5"),
         Reshape((1152,), name=f"{prefix}_cnn2ff"),
         Dense(1152, 1024, "tanh", updater=u(), l2=1e-4, name=f"{prefix}_dense_layer_6"),
-        Output(1024, 1, updater=u(), l2=1e-4, name=f"{prefix}_output_layer_7", quirks=quirks),
+        Output(1024, 1, updater=u(), l2=1e-4, name=f"{prefix}_output_layer_7"),
     ]
     return Net(L, seed=seed, dtype=dtype, grad_clip=1.0, quirks=quirks)
 
@@ -924,7 +1567,7 @@ def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, dtype=np.float
               BatchNorm(ch * 2, updater=u(), name=f"dis_bn_{i + 2}"), ActivationLayer("lrelu", 0.2, name=f"dis_act_{i + 2}")]
         ch *= 2
     L += [Conv2D(ch, 1, (4, 4), (1, 1), (0, 0), updater=u(), name=f"dis_conv_{n_down + 1}"),
-          LossLayer(name="dis_loss", quirks=quirks)]
+          LossLayer(name="dis_loss")]
     return Net(L, seed=seed, dtype=dtype, quirks=quirks)
 
 
@@ -939,7 +1582,7 @@ def mlp_discriminator(d=256, hidden=1024, lr=2e-4, beta1=0.5, dtype=np.float64, 
     u = lambda: Adam(lr, beta1, 0.999, 1e-8)
     return Net([Dense(d, hidden, "lrelu", 0.2, updater=u(), name="dis_dense_1"),
                 Dense(hidden, hidden, "lrelu", 0.2, updater=u(), name="dis_dense_2"),
-                Output(hidden, 1, updater=u(), name="dis_output", quirks=quirks)], seed=seed, dtype=dtype, quirks=quirks)
+                Output(hidden, 1, updater=u(), name="dis_output")], seed=seed, dtype=dtype, quirks=quirks)
 
 
 def synthetic_batch(n, size=64, nc=3, z=100, seed=666, dtype=np.float32):
@@ -952,3 +1595,68 @@ def synthetic_batch(n, size=64, nc=3, z=100, seed=666, dtype=np.float32):
     y_fake = (0 + 0.05 * rng.standard_normal((n, 1))).astype(dtype)
     y_gen = np.ones((n, 1), dtype)
     return x, z_d, z_g, y_real, y_fake, y_gen
+
+
+# --------------------------------------------------------------------------------------------------
+# Layer specs (gan_deeplearning4j_b200.models / engine.LAYER_TYPES) -> Net
+# --------------------------------------------------------------------------------------------------
+def net_from_specs(specs, input_shape, *, quirks: Quirks = DEFAULT_QUIRKS, dtype=np.float64, seed=1, grad_clip=0.0, flat_input=True,
+                   mask_seed=666, rank=0) -> Net:
+    """The Net of the layer specs the CUDA engine consumes.  input_shape: (C,H,W) or (F,).  flat_input: prepend the convolutionalFlat
+    reshape (the oracle's layer indices are then the specs' + 1).  A spec's scheduled lr becomes the layer's schedule; its constant lr is
+    the schedule's value at 0, as the library keeps it.  An activation's alpha defaults as engine.layer_desc fills it.  A DropoutLayer's
+    mask index is its position in `specs` (the library's index).  mask_seed, rank: see Net."""
+    layers = []
+    shape = (1,) + tuple(input_shape)
+    if len(input_shape) == 3 and flat_input:
+        layers.append(Reshape(tuple(input_shape), name="in_reshape"))      # convolutionalFlat accepts [N,784] or [N,1,28,28]
+    schedules = {}
+    for i, s in enumerate(specs):
+        t, name = s["type"], s.get("name", "")
+        u = updater_cfg(s.get("updater"))
+        if u is not None and isinstance(s["updater"].get("lr"), dict) and u.kind != "noop":
+            schedules[name] = s["updater"]["lr"]
+        act = s.get("activation", "identity")
+        alpha = s.get("alpha", ACT_ALPHA_DEFAULTS.get(act, 0.01))
+        n_in = s.get("n_in") or (int(np.prod(shape[1:])) if t in ("dense", "output") else shape[1])
+        k, st, pad = s.get("kernel"), s.get("stride", (1, 1)), s.get("padding", (0, 0))
+        if t == "conv2d":
+            l = Conv2D(n_in, s["n_out"], k, st, pad, act, alpha, u, s.get("l2", 0.0), name, s.get("has_bias", True))
+        elif t == "deconv2d":
+            l = Deconv2D(n_in, s["n_out"], k, st, pad, act, alpha, u, s.get("l2", 0.0), name, s.get("has_bias", True))
+        elif t == "dense":
+            l = Dense(n_in, s["n_out"], act, alpha, u, s.get("l2", 0.0), name, s.get("has_bias", True))
+        elif t == "output" and s.get("loss", "xent") == "mcxent":
+            l = OutputSoftmax(n_in, s["n_out"], u, s.get("l2", 0.0), name)
+        elif t == "output":
+            l = Output(n_in, s["n_out"], u, s.get("l2", 0.0), name, loss=s.get("loss", "xent"), activation=act, alpha=alpha)
+        elif t == "loss":
+            l = LossLayer(name, loss=s.get("loss", "xent"), activation=act, alpha=alpha)
+        elif t == "batchnorm":
+            l = BatchNorm(shape[1], s.get("decay", 0.9), s.get("eps", 1e-5), u, name)
+        elif t == "activation":
+            l = ActivationLayer(act, alpha, name)
+        elif t == "maxpool":
+            l = MaxPool(k, st, name)
+        elif t == "subsampling":
+            l = Subsampling(s["pooling"], k, st, pad, s.get("pnorm", 0), name)
+        elif t == "global_pooling":
+            l = GlobalPooling(s.get("pooling", "max"), s.get("pnorm", 2), name)
+        elif t == "upsample2d":
+            l = Upsample2D(s.get("size", 2), name)
+        elif t == "dropout":
+            l = Dropout(s["p"], name, index=i)
+        elif t == "ff_to_cnn":
+            h, w, c = s["to"]; l = Reshape((c, h, w), name)
+        elif t == "cnn_to_ff":
+            l = Reshape((int(np.prod(shape[1:])),), name)
+        else:
+            raise ValueError(t)
+        if s.get("frozen", False):
+            l.frozen = True
+        layers.append(l)
+        shape = l.out_shape(shape)
+    net = Net(layers, seed=seed, dtype=dtype, grad_clip=grad_clip, quirks=quirks, mask_seed=mask_seed, rank=rank)
+    for name, sched in schedules.items():
+        net.set_lr_schedule(sched, name)
+    return net

@@ -16,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-from helpers import oracle_from_specs, randomize  # noqa: E402
+from helpers import randomize# noqa: E402
 from oracle import dl4j_oracle as o  # noqa: E402
 
 GAN_CFG = dict(size=16, z=12, nf=8, n=8, lr=2e-3, clip_eps=1e-5, seed_g=1, seed_d=2, seed_rand=5, seed_data=3, steps=3)
@@ -27,7 +27,7 @@ def gan_pair():
     c = GAN_CFG
     gs, ds = m.dcgan_generator(c["size"], c["z"], c["nf"], 3, lr=c["lr"]), m.dcgan_discriminator(c["size"], c["nf"], 3, lr=c["lr"])
     q = o.Quirks(xent_clip_eps=c["clip_eps"]); rng = np.random.default_rng(c["seed_rand"])
-    G = oracle_from_specs(gs, (c["z"],), quirks=q, seed=c["seed_g"]); D = oracle_from_specs(ds, (3, c["size"], c["size"]), quirks=q, seed=c["seed_d"])
+    G = o.net_from_specs(gs, (c["z"],), quirks=q, seed=c["seed_g"]); D = o.net_from_specs(ds, (3, c["size"], c["size"]), quirks=q, seed=c["seed_d"])
     randomize(G, rng); randomize(D, rng)
     return gs, ds, G, D
 

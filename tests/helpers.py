@@ -1,57 +1,5 @@
-"""Test-only glue: build the oracle's Net from the same layer specs the CUDA engine consumes."""
+"""Test-only utilities for comparing the oracle's nets (oracle.dl4j_oracle.net_from_specs) with the CUDA library's."""
 import numpy as np
-
-from oracle import dl4j_oracle as o
-
-
-def _upd(u):
-    if u is None:
-        return None
-    if u["kind"] == "rmsprop":
-        return o.RmsProp(u["lr"], u.get("rms_decay", 0.95), u.get("eps", 1e-8))
-    if u["kind"] == "adam":
-        return o.Adam(u["lr"], u.get("beta1", 0.9), u.get("beta2", 0.999), u.get("eps", 1e-8))
-    if u["kind"] == "sgd":
-        return o.Sgd(u["lr"])
-    return o.UpdaterCfg("noop")
-
-
-def oracle_from_specs(specs, input_shape, grad_clip=0.0, quirks=o.DEFAULT_QUIRKS, dtype=np.float64, seed=1, flat_input=True):
-    """input_shape: (C,H,W) or (F,).  flat_input: prepend the convolutionalFlat reshape (index shift +1)."""
-    layers = []
-    shape = (1,) + tuple(input_shape)
-    if len(input_shape) == 3 and flat_input:
-        layers.append(o.Reshape(tuple(input_shape), name="in_reshape"))      # convolutionalFlat accepts [N,784] or [N,1,28,28]
-    for s in specs:
-        t, name = s["type"], s.get("name", "")
-        u = _upd(s.get("updater"))
-        if t == "conv2d":
-            l = o.Conv2D(s.get("n_in") or shape[1], s["n_out"], s["kernel"], s.get("stride", (1, 1)), s.get("padding", (0, 0)), s.get("activation", "identity"), s.get("alpha", 0.01), u, s.get("l2", 0.0), name, s.get("has_bias", True))
-        elif t == "deconv2d":
-            l = o.Deconv2D(s.get("n_in") or shape[1], s["n_out"], s["kernel"], s.get("stride", (1, 1)), s.get("padding", (0, 0)), s.get("activation", "identity"), s.get("alpha", 0.01), u, s.get("l2", 0.0), name, s.get("has_bias", True))
-        elif t == "dense":
-            l = o.Dense(s.get("n_in") or shape[1], s["n_out"], s.get("activation", "identity"), s.get("alpha", 0.01), u, s.get("l2", 0.0), name, s.get("has_bias", True))
-        elif t == "output":
-            l = o.Output(s.get("n_in") or shape[1], s["n_out"], u, s.get("l2", 0.0), name, quirks)
-        elif t == "batchnorm":
-            l = o.BatchNorm(shape[1], s.get("decay", 0.9), s.get("eps", 1e-5), u, name)
-        elif t == "activation":
-            l = o.ActivationLayer(s["activation"], s.get("alpha", 0.01), name)
-        elif t == "maxpool":
-            l = o.MaxPool(s["kernel"], s.get("stride", (1, 1)), name)
-        elif t == "upsample2d":
-            l = o.Upsample2D(s.get("size", 2), name)
-        elif t == "loss":
-            l = o.LossLayer(name, quirks)
-        elif t == "ff_to_cnn":
-            h, w, c = s["to"]; l = o.Reshape((c, h, w), name)
-        elif t == "cnn_to_ff":
-            l = o.Reshape((int(np.prod(shape[1:])),), name)
-        else:
-            raise ValueError(t)
-        layers.append(l)
-        shape = l.out_shape(shape)
-    return o.Net(layers, seed=seed, dtype=dtype, grad_clip=grad_clip, quirks=quirks)
 
 
 def randomize(net, rng, scale=None):

@@ -1,11 +1,9 @@
-"""CPU checks of tests/activation_ref.py, the float64 restatement of b2g_activation codes 5-16: finite differences at GradientCheckUtil's
+"""CPU checks of the oracle's float64 restatement of b2g_activation codes 5-16: finite differences at GradientCheckUtil's
 tolerances, hand-computed values at and beside every boundary, float64 torch where torch has the same function, the quirk flags' reach, and the
 restatement through oracle layers and a loss (existing kinds unchanged)."""
 import numpy as np
 import pytest
 
-import activation_ref as ar
-import loss_ref as lr
 from helpers import randomize
 from oracle import dl4j_oracle as o
 
@@ -22,12 +20,12 @@ def _points(kind, rng):
     return z
 
 
-@pytest.mark.parametrize("kind", ar.KINDS)
+@pytest.mark.parametrize("kind", o.EXT_ACTS)
 def test_finite_differences(kind):
-    rng = np.random.default_rng(ar.CODES[kind])
+    rng = np.random.default_rng(o.ACT_CODES[kind])
     z = _points(kind, rng)
-    num = (ar.forward(kind, z + EPS) - ar.forward(kind, z - EPS)) / (2 * EPS)
-    ana = ar.derivative(kind, z)
+    num = (o.forward(kind, z + EPS) - o.forward(kind, z - EPS)) / (2 * EPS)
+    ana = o.derivative(kind, z)
     d = np.abs(num - ana)
     rel = d / np.maximum(np.abs(num) + np.abs(ana), 1e-300)
     assert np.all((rel <= MAX_REL) | (d <= MIN_ABS)), (kind, z[np.argmax(rel)], rel.max())
@@ -37,12 +35,12 @@ def test_finite_differences(kind):
 def test_finite_differences_with_alpha(kind):
     z = _points("selu", np.random.default_rng(3))
     z = z[np.abs(z - 0.37) > 10 * EPS]
-    num = (ar.forward(kind, z + EPS, 0.37) - ar.forward(kind, z - EPS, 0.37)) / (2 * EPS)
-    ana = ar.derivative(kind, z, 0.37)
+    num = (o.forward(kind, z + EPS, 0.37) - o.forward(kind, z - EPS, 0.37)) / (2 * EPS)
+    ana = o.derivative(kind, z, 0.37)
     assert np.all((np.abs(num - ana) <= MAX_REL * (np.abs(num) + np.abs(ana))) | (np.abs(num - ana) <= MIN_ABS))
 
 
-L, S = ar.SELU_LAMBDA, ar.SELU_ALPHA
+L, S = o.SELU_LAMBDA, o.SELU_ALPHA
 # (kind, alpha, z, f(z), f'(z)) at and beside the boundaries, by hand
 HAND = [
     ("elu", None, 0.0, 0.0, 1.0), ("elu", None, -1.0, np.e ** -1 - 1, np.e ** -1), ("elu", 0.5, -2.0, 0.5 * (np.e ** -2 - 1), 0.5 * np.e ** -2),
@@ -69,14 +67,14 @@ HAND = [
 
 @pytest.mark.parametrize("kind,alpha,z,f,df", HAND)
 def test_hand_computed_boundaries(kind, alpha, z, f, df):
-    assert ar.forward(kind, np.array([z]), alpha)[0] == pytest.approx(f, rel=1e-12, abs=1e-300)
-    assert ar.derivative(kind, np.array([z]), alpha)[0] == pytest.approx(df, rel=1e-12, abs=1e-300)
+    assert o.forward(kind, np.array([z]), alpha)[0] == pytest.approx(f, rel=1e-12, abs=1e-300)
+    assert o.derivative(kind, np.array([z]), alpha)[0] == pytest.approx(df, rel=1e-12, abs=1e-300)
 
 
 def test_no_overflow_where_the_function_is_finite():
     z = np.array([-1e4, -700.0, -100.0, 100.0, 700.0, 1e4])
-    for kind in ar.KINDS:
-        assert np.all(np.isfinite(ar.forward(kind, z))) and np.all(np.isfinite(ar.derivative(kind, z))), kind
+    for kind in o.EXT_ACTS:
+        assert np.all(np.isfinite(o.forward(kind, z))) and np.all(np.isfinite(o.derivative(kind, z))), kind
 
 
 @pytest.mark.parametrize("kind,fn", [("elu", "elu"), ("selu", "selu"), ("softplus", "softplus"), ("softsign", "softsign"),
@@ -88,34 +86,23 @@ def test_torch_float64_cross_check(kind, fn):
     t = torch.tensor(z, dtype=torch.float64, requires_grad=True)
     y = getattr(torch.nn.functional, fn)(t)
     y.sum().backward()
-    np.testing.assert_allclose(ar.forward(kind, z), y.detach().numpy(), rtol=1e-12, atol=1e-15)
-    np.testing.assert_allclose(ar.derivative(kind, z), t.grad.numpy(), rtol=1e-12, atol=1e-15)
+    np.testing.assert_allclose(o.forward(kind, z), y.detach().numpy(), rtol=1e-12, atol=1e-15)
+    np.testing.assert_allclose(o.derivative(kind, z), t.grad.numpy(), rtol=1e-12, atol=1e-15)
 
 
 def test_quirk_flags_move_only_their_boundaries():
     z = np.array([-2.5, -1.0, 0.0, 1.0, 2.5, 6.0, 3.0])
-    base = {k: ar.derivative(k, z) for k in ("hardtanh", "hardsigmoid", "relu6")}
+    base = {k: o.derivative(k, z) for k in ("hardtanh", "hardsigmoid", "relu6")}
     for field, kind, moved in (("hardtanh_closed", "hardtanh", [1, 3]), ("hardsigmoid_closed", "hardsigmoid", [0, 4]), ("relu6_open", "relu6", [2, 5])):
-        q = ar.ActQuirks(**{field: not getattr(ar.DEFAULT_ACT_QUIRKS, field)})
-        d = ar.derivative(kind, z, q=q)
+        q = o.Quirks(**{field: not getattr(o.DEFAULT_QUIRKS, field)})
+        d = o.derivative(kind, z, q=q)
         changed = np.nonzero(d != base[kind])[0].tolist()
         assert changed == moved, (field, changed)
     with pytest.raises(ValueError):
-        ar.forward("thresholdedrelu", z, q=ar.ActQuirks(thresholded_relu_in_beta3=False))
+        o.forward("thresholdedrelu", z, q=o.Quirks(thresholded_relu_in_beta3=False))
 
 
-def test_existing_kinds_go_to_the_oracle_bit_for_bit():
-    rng = np.random.default_rng(2)
-    z, e = rng.standard_normal(50), rng.standard_normal(50)
-    for k in o.ACTS:
-        assert np.array_equal(o.act_forward(k, z, 0.2), ar._orig["fwd"](k, z, 0.2))
-        assert np.array_equal(o.act_backward(k, z, e, 0.2), ar._orig["bwd"](k, z, e, 0.2))
-        s0, g0 = ar._orig["loss"]("mse", k, 0.2, z.reshape(5, 10), e.reshape(5, 10))
-        s1, g1 = lr.score_and_grad("mse", k, 0.2, z.reshape(5, 10), e.reshape(5, 10))
-        assert s0 == s1 and np.array_equal(g0, g1)
-
-
-@pytest.mark.parametrize("kind", ar.KINDS)
+@pytest.mark.parametrize("kind", o.EXT_ACTS)
 def test_net_gradient_through_layers_and_loss(kind):
     """Dense(kind) -> ActivationLayer(kind) -> Output(MSE on kind): the oracle net's parameter gradients against finite differences."""
     specs = [{"type": "dense", "name": "d1", "n_out": 5, "activation": kind},
@@ -123,7 +110,7 @@ def test_net_gradient_through_layers_and_loss(kind):
              {"type": "dense", "name": "d2", "n_out": 4},
              {"type": "activation", "name": "a2", "activation": kind},
              {"type": "output", "name": "out", "n_out": 3, "loss": "mse", "activation": kind}]
-    net = ar.oracle_from_specs(specs, (6,), seed=4)
+    net = o.net_from_specs(specs, (6,), seed=4)
     rng = np.random.default_rng(5)
     randomize(net, rng)          # non-zero biases: a row whose hidden units are all 0 would otherwise sit on the kink at z = 0
     x, y = rng.uniform(-1.2, 1.2, (7, 6)), rng.uniform(-1, 1, (7, 3))

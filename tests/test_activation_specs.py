@@ -6,8 +6,8 @@ import re
 import numpy as np
 import pytest
 
-import activation_ref as ar
 from gan_deeplearning4j_b200 import engine, models as m
+from oracle import dl4j_oracle as o
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 NAMES = ("IDENTITY", "TANH", "SIGMOID", "RELU", "LRELU", "ELU", "SELU", "SOFTPLUS", "SOFTSIGN", "HARDTANH", "HARDSIGMOID", "RELU6", "SWISH", "CUBE",
@@ -21,7 +21,7 @@ def test_codes_agree_across_header_kernels_engine_and_java():
     header = {k: int(v) for k, v in re.findall(r"B2G_ACT_(\w+) = (\d+)", body)}
     assert header == {n: i for i, n in enumerate(NAMES)}
     assert {k.upper(): v for k, v in engine.ACTS.items()} == header
-    assert {k: v for k, v in engine.ACTS.items() if v >= 5} == ar.CODES
+    assert {k: v for k, v in engine.ACTS.items() if v >= 5} == o.ACT_CODES
     kernels = open(os.path.join(ROOT, "gan_deeplearning4j_b200/csrc/kernels.h")).read()
     body = re.search(r"enum Act \{([^}]*)\}", kernels).group(1)
     assert {k: int(v) for k, v in re.findall(r"ACT_(\w+) = (\d+)", body)} == header
@@ -39,16 +39,16 @@ def test_java_parameterized_activations_and_default_alpha():
     assert "!alphaSet && (a == Activation.ELU.code || a == Activation.THRESHOLDEDRELU.code) ? 1.0f : alpha" in layer
 
 
-@pytest.mark.parametrize("kind", ar.KINDS)
+@pytest.mark.parametrize("kind", o.EXT_ACTS)
 def test_spec_to_descriptor(kind):
     for t in ("conv2d", "deconv2d", "dense", "activation"):
         d = engine.layer_desc({"type": t, "name": "l", "n_out": 2, "activation": kind})
-        assert d.act == ar.CODES[kind] and d.act_alpha == np.float32(ar.ALPHA_DEFAULTS.get(kind, 0.01))
+        assert d.act == o.ACT_CODES[kind] and d.act_alpha == np.float32(o.ACT_ALPHA_DEFAULTS.get(kind, 0.01))
         d = engine.layer_desc({"type": t, "name": "l", "n_out": 2, "activation": kind, "alpha": 0.3})
-        assert d.act == ar.CODES[kind] and d.act_alpha == np.float32(0.3)
+        assert d.act == o.ACT_CODES[kind] and d.act_alpha == np.float32(0.3)
     for t in ("output", "loss"):
         d = engine.layer_desc({"type": t, "name": "o", "n_out": 2, "loss": "mse", "activation": kind})
-        assert (d.loss, d.act) == (2, ar.CODES[kind])
+        assert (d.loss, d.act) == (2, o.ACT_CODES[kind])
     # LeakyReLU keeps its 0.01 default
     assert engine.layer_desc({"type": "dense", "name": "l", "n_out": 2, "activation": "lrelu"}).act_alpha == np.float32(0.01)
 

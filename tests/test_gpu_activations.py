@@ -1,14 +1,13 @@
 """The activations of b2g_activation codes 5-16 on the GPU: the act_ext kernels through their production wrappers (b2g_test_ew ops act_ext_fwd /
 act_ext_bwd) for every kind x precision x {vector, offset} path against float64 of the same stored z; FP32 nets with the new kinds in every
 placement (Dense -> Dense -> OutputLayer(MSE), Conv2D -> BatchNorm -> ActivationLayer -> Deconv2D -> BatchNorm -> LossLayer) against
-tests/activation_ref.py; BF16 16x16 DCGAN nets with ELU / SELU / Swish layer by layer on injected inputs; the FP32 GAN step (G: ELU hidden,
+the oracle's restatement; BF16 16x16 DCGAN nets with ELU / SELU / Swish layer by layer on injected inputs; the FP32 GAN step (G: ELU hidden,
 HardTanh output; D: SELU) against the oracle's gan_step in graph replay and eager mode with its launches per step; and the argument checks."""
 import ctypes as C
 
 import numpy as np
 import pytest
 
-import activation_ref as ar
 from helpers import bf16_round, check_bf16, push_params, randomize, rel_err
 from oracle import dl4j_oracle as o
 
@@ -42,13 +41,13 @@ def _inputs(n, rng):
 
 @pytest.mark.parametrize("offset", [0, 3])
 @pytest.mark.parametrize("prec", ["fp32", "bf16"])
-@pytest.mark.parametrize("kind", ar.KINDS)
+@pytest.mark.parametrize("kind", o.EXT_ACTS)
 def test_kernels_against_float64(b200, kind, prec, offset):
     """f and eps * f' within one rounding of the output type (2^-8 relative for bf16, the bound of the other bf16 tests) plus the fp32
     evaluation's few units of 2^-24 on the terms it combines; no inf / NaN anywhere, no element left unwritten (the outputs are poisoned)."""
     b, ctx = b200
     p = b.FP32 if prec == "fp32" else b.BF16
-    rng = np.random.default_rng(ar.CODES[kind] * 7 + offset)
+    rng = np.random.default_rng(o.ACT_CODES[kind] * 7 + offset)
     z = _inputs(4099, rng)
     e = rng.uniform(-2, 2, z.size).astype(np.float32)
     alpha = 0.75 if kind in ("elu", "thresholdedrelu") else 0.0
@@ -58,8 +57,8 @@ def test_kernels_against_float64(b200, kind, prec, offset):
     (fwd, _, _), info_f = b.test_ew(ctx, p, "act_ext_fwd", z, None, (z.size, 0, 0), act=kind, alpha=alpha, n=z.size, offset=offset, poison=True)
     (bwd, _, _), info_b = b.test_ew(ctx, p, "act_ext_bwd", z, e, (z.size, 0, 0), act=kind, alpha=alpha, n=z.size, offset=offset)
     assert info_f["kernel"] == f"act_ext_fwd_kernel<{kind}>" and info_b["kernel"] == f"act_ext_bwd_kernel<{kind}>"
-    f_ref = ar.forward(kind, zs, alpha)
-    d_ref = es * ar.derivative(kind, zs, alpha)
+    f_ref = o.forward(kind, zs, alpha)
+    d_ref = es * o.derivative(kind, zs, alpha)
     for got, ref, scale, what in ((fwd, f_ref, 1.0, "f"), (bwd, d_ref, np.abs(es), "eps*f'")):
         assert np.isfinite(got).all(), (kind, prec, what, "non-finite")
         tol = u_out * np.abs(ref) + 16 * U * (np.abs(ref) + scale)
@@ -93,14 +92,14 @@ def _conv(kind):
 
 
 @pytest.mark.parametrize("net", ["mlp", "conv"])
-@pytest.mark.parametrize("kind", ar.KINDS)
+@pytest.mark.parametrize("kind", o.EXT_ACTS)
 def test_fp32_nets_match_oracle(b200, kind, net):
     """Every activation, every gradient, the score, the post-update parameters and b2g_net_output (inference: the BatchNorm after a GEMM of a new
     kind is not folded into it; train mode: batch statistics) within DESIGN 1's 1e-3."""
     b, ctx = b200
     specs, shape, n_out = (_mlp if net == "mlp" else _conv)(kind)
-    rng = np.random.default_rng(ar.CODES[kind])
-    onet = ar.oracle_from_specs(specs, shape, seed=2, flat_input=False); randomize(onet, rng)
+    rng = np.random.default_rng(o.ACT_CODES[kind])
+    onet = o.net_from_specs(specs, shape, seed=2, flat_input=False); randomize(onet, rng)
     bnet = b.Net(ctx, specs, shape, max_batch=6, precision=b.FP32)
     push_params(onet, bnet)
     r = 0.5 if kind == "cube" and net == "mlp" else 1.5
@@ -126,7 +125,7 @@ def _check_ext_gemm(got, ref, z, kind, what):
     """A GEMM layer of a new kind in bf16: its z is rounded to bf16 once before f (b2g_activation), so beside check_bf16's bound on a the
     rounding of z moves the result by up to |f'(z)| 2^-8 |z|."""
     got, ref, z = (np.asarray(v, np.float64) for v in (got, ref, z))
-    tol = 2.0 ** -8 * (np.abs(ref) + np.abs(ar.derivative(kind, z) * z)) + 2e-3 * np.sqrt(np.mean(ref ** 2))
+    tol = 2.0 ** -8 * (np.abs(ref) + np.abs(o.derivative(kind, z) * z)) + 2e-3 * np.sqrt(np.mean(ref ** 2))
     bad = ~(np.abs(got - ref) <= tol)
     assert not bad.any(), (what, int(bad.sum()), bad.size, float(np.abs(got - ref)[bad].max()))
 
@@ -144,7 +143,7 @@ def test_bf16_dcgan_layers_on_injected_inputs(b200, kind):
              (m.dcgan_discriminator(16, 64, 3, activation=kind), m.dcgan_discriminator(16, 64, 3), (3, 16, 16))]
     for specs, base, shape in cases:
         x = bf16_round(rng.uniform(-1, 1, (n,) + shape))
-        onet = ar.oracle_from_specs(specs, shape, seed=3, flat_input=False); randomize(onet, rng)
+        onet = o.net_from_specs(specs, shape, seed=3, flat_input=False); randomize(onet, rng)
         for l in onet.layers:          # the tensor-core path reads bf16 weights: the oracle takes the same operands
             if l.has_params and "W" in l.params:
                 l.params["W"] = bf16_round(l.params["W"]).astype(np.float64)
@@ -160,7 +159,7 @@ def test_bf16_dcgan_layers_on_injected_inputs(b200, kind):
                         break
                     ref = l.forward(cur, True)
                     got = bnet.activation(i, n).reshape(ref.shape)
-                    if sp[i]["type"] != "activation" and sp[i].get("activation") in ar.KINDS:
+                    if sp[i]["type"] != "activation" and sp[i].get("activation") in o.EXT_ACTS:
                         _check_ext_gemm(got, ref, l._z, sp[i]["activation"], f"{kind} {sp[i]['name']}")
                     else:
                         check_bf16(got, ref, f"{kind} {sp[i]['name']}")
@@ -206,7 +205,7 @@ def test_fp32_gan_step_matches_oracle(b200):
     counts = {}
     for graph in (True, False):
         rng = np.random.default_rng(5)
-        G = ar.oracle_from_specs(gs, (z,), seed=1); D = ar.oracle_from_specs(ds, (3, size, size), seed=2)
+        G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
         randomize(G, rng); randomize(D, rng)
         bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
         bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2)

@@ -9,8 +9,7 @@ import sys
 import numpy as np
 import pytest
 
-import dropout_ref as dr
-from helpers import bf16_round, oracle_from_specs, push_params, randomize, rel_err
+from helpers import bf16_round, push_params, randomize, rel_err
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
@@ -37,7 +36,7 @@ def test_dropout_kernels_match_the_oracle_mask_exactly(b200, prec, n, p):
     dy = (rng.uniform(0.5, 2.0, n) * rng.choice([-1.0, 1.0], n)).astype(np.float32).reshape(1, 1, 1, n)
     seed, layer, rank, pass_ = 1234567890123, 5, 3, (1 << 32) + 17
     y, dx = b.test_dropout(ctx, P, x, dy, p, seed=seed, layer=layer, rank=rank, pass_=pass_)
-    keep = dr.dropout_mask(seed, rank, layer, pass_, 1, 1, 1, n, p).ravel()
+    keep = o.dropout_mask(seed, rank, layer, pass_, 1, 1, 1, n, p).ravel()
     assert np.array_equal(y.ravel() != 0, keep) and np.array_equal(dx.ravel() != 0, keep)
     s = np.float32(1) / np.float32(p)
     rnd = bf16_round if prec == "bf16" else (lambda a: np.asarray(a, np.float32))
@@ -81,7 +80,7 @@ def test_fp32_chain_matches_oracle_under_identical_masks(b200):
     b, ctx = b200
     specs = _chain_specs()
     rng = np.random.default_rng(3)
-    onet = dr.oracle_from_specs(specs, (3, 8, 8), mask_seed=41, seed=2); randomize(onet, rng)
+    onet = o.net_from_specs(specs, (3, 8, 8), mask_seed=41, seed=2); randomize(onet, rng)
     bnet = b.Net(ctx, specs, (3, 8, 8), max_batch=6, precision=b.FP32, seed=41)
     push_params(onet, bnet)
     x = rng.uniform(-1, 1, (6, 3, 8, 8)); y = rng.uniform(0, 1, (6, 1))
@@ -110,7 +109,7 @@ def test_inference_and_frozen_dropout_are_the_identity(b200):
     b, ctx = b200
     rng = np.random.default_rng(4)
     plain, drop, frozen = _chain_specs(with_dropout=False), _chain_specs(), _chain_specs(frozen=True)
-    onet = oracle_from_specs(plain, (3, 8, 8), seed=2); randomize(onet, rng)
+    onet = o.net_from_specs(plain, (3, 8, 8), seed=2); randomize(onet, rng)
     x = rng.uniform(-1, 1, (6, 3, 8, 8)); y = rng.uniform(0, 1, (6, 1))
     nets = [b.Net(ctx, s, (3, 8, 8), max_batch=6, precision=b.FP32) for s in (plain, drop, frozen)]
     for n in nets:
@@ -174,7 +173,7 @@ def _dcgan_d_with_dropout(size, nf, lr, p):
 
 def _bf16_grad_err(b, ctx, specs, in_shape, n, seed, rng_seed):
     rng = np.random.default_rng(rng_seed)
-    onet = dr.oracle_from_specs(specs, in_shape, mask_seed=seed, quirks=o.Quirks(xent_clip_eps=0.0), seed=2); randomize(onet, rng)
+    onet = o.net_from_specs(specs, in_shape, mask_seed=seed, quirks=o.Quirks(xent_clip_eps=0.0), seed=2); randomize(onet, rng)
     bnet = b.Net(ctx, specs, in_shape, max_batch=n, precision=b.BF16, xent_clip_eps=0.0, seed=seed)
     push_params(onet, bnet)
     x = rng.uniform(-1, 1, (n,) + tuple(in_shape)); y = rng.uniform(0, 1, (n, 1))
@@ -204,7 +203,7 @@ def _fp32_dcgan_with_dropout(b, ctx, n, p=0.7):
     size, z, nf = 16, 12, 8
     gs, ds = m.dcgan_generator(size, z, nf, 3, lr=2e-3), _dcgan_d_with_dropout(size, nf, 2e-3, p)
     rng = np.random.default_rng(5)
-    G = oracle_from_specs(gs, (z,), seed=1); D = dr.oracle_from_specs(ds, (3, size, size), mask_seed=667, seed=2)
+    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), mask_seed=667, seed=2)
     randomize(G, rng); randomize(D, rng)
     bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
     bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2, seed=667)
@@ -223,7 +222,7 @@ def test_fp32_gan_step_with_dropout_graph_eager_and_oracle(b200):
         drop = [i for i, s in enumerate(ds) if s["type"] == "dropout"]
         masks, losses = [], []
         for it in range(3):
-            r = dr.gan_step(G, D, *data)
+            r = o.gan_step(G, D, *data)
             lo = gan.step(*data); losses.append(lo)
             want = np.array([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]])
             assert np.all(np.abs(lo - want) < TOL * np.maximum(1, np.abs(want))), (graph, it, lo, want)

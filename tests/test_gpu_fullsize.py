@@ -279,7 +279,7 @@ def test_bf16_whole_step_layer_by_layer(b200, case):
     (ten bf16-rounded epsilon tensors deep), cosine >= 0.999."""
     b, ctx = b200
     from gan_deeplearning4j_b200 import models as m
-    from helpers import oracle_from_specs, push_params, randomize
+    from helpers import push_params, randomize
     name, size, z, nf, n = case
     rng = np.random.default_rng(21)
     if name == "c5":        # MLP-GAN (BASELINE configs[4]): dense tensor-core path, samples of d = 256 features
@@ -290,7 +290,7 @@ def test_bf16_whole_step_layer_by_layer(b200, case):
         gs, ds, dshape = m.dcgan_generator(size, z, nf, 3), m.dcgan_discriminator(size, nf, 3), (3, size, size)
         data = [np.asarray(a, np.float32) for a in o.synthetic_batch(n, size, 3, z, seed=5)]
     q = o.Quirks(xent_clip_eps=0.0)
-    G = oracle_from_specs(gs, (z,), quirks=q, dtype=np.float32, seed=1); D = oracle_from_specs(ds, dshape, quirks=q, dtype=np.float32, seed=2, flat_input=False)
+    G = o.net_from_specs(gs, (z,), quirks=q, dtype=np.float32, seed=1); D = o.net_from_specs(ds, dshape, quirks=q, dtype=np.float32, seed=2, flat_input=False)
     randomize(G, rng); randomize(D, rng)
     bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.BF16, xent_clip_eps=0.0)
     bD = b.Net(ctx, ds, dshape, max_batch=2 * n, precision=b.BF16, xent_clip_eps=0.0, bn_groups=2)
@@ -449,13 +449,13 @@ def _check_grads(got_flat, want, onet, specs, what, fro_bound, errs, injected=Tr
 def test_bf16_ragged_batch_routes_layer_by_layer(b200, n):
     b, ctx = b200
     from gan_deeplearning4j_b200 import models as m
-    from helpers import oracle_from_specs, push_params, randomize
+    from helpers import push_params, randomize
     size, z, nf = SWEEP_SIZE, SWEEP_Z, SWEEP_NF
     rng = np.random.default_rng(31 + n)
     gs, ds, dshape = m.dcgan_generator(size, z, nf, 3), m.dcgan_discriminator(size, nf, 3), (3, size, size)
     data = [np.asarray(a, np.float32) for a in o.synthetic_batch(n, size, 3, z, seed=40 + n)]
     q = o.Quirks(xent_clip_eps=0.0)
-    G = oracle_from_specs(gs, (z,), quirks=q, dtype=np.float32, seed=1); D = oracle_from_specs(ds, dshape, quirks=q, dtype=np.float32, seed=2, flat_input=False)
+    G = o.net_from_specs(gs, (z,), quirks=q, dtype=np.float32, seed=1); D = o.net_from_specs(ds, dshape, quirks=q, dtype=np.float32, seed=2, flat_input=False)
     randomize(G, rng); randomize(D, rng)
     bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.BF16, xent_clip_eps=0.0)
     bD = b.Net(ctx, ds, dshape, max_batch=2 * n, precision=b.BF16, xent_clip_eps=0.0, bn_groups=2)

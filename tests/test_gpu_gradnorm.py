@@ -1,4 +1,4 @@
-"""L2 gradient normalization on the GPU: FP32 fit and the fused GAN step against the oracle restatement (tests/gradnorm_ref.py) for all four
+"""L2 gradient normalization on the GPU: FP32 fit and the fused GAN step against the oracle's restatement for all four
 modes, eager against CUDA-graph replay bit for bit (a mode change re-captures), the bf16 weight copies after normalized updates, launch counts,
 argument checks and two ranks."""
 import copy
@@ -10,9 +10,7 @@ import sys
 import numpy as np
 import pytest
 
-import dropout_ref as dr
-import gradnorm_ref as gnr
-from helpers import bf16_round, oracle_from_specs, pack_deconv_ps, push_params, randomize, rel_err, w_internal
+from helpers import bf16_round, pack_deconv_ps, push_params, randomize, rel_err, w_internal
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
@@ -86,15 +84,15 @@ def test_fp32_fit_matches_oracle(b200, kind, upd, mode):
     b, ctx = b200
     specs, shape = _specs(kind, upd)
     rng = np.random.default_rng(11)
-    onet = oracle_from_specs(specs, shape, seed=2); randomize(onet, rng)
+    onet = o.net_from_specs(specs, shape, seed=2); randomize(onet, rng)
     n = 6
     xs = [rng.uniform(-1, 1, (n,) + shape) for _ in range(3)]; ys = [rng.uniform(0, 1, (n, 1)) for _ in range(3)]
     thr = 1.0
     if mode.startswith("clip"):        # dry run: the first update's group norms
-        probe = gnr.enable(copy.deepcopy(onet), mode, 1e30)
+        probe = copy.deepcopy(onet); probe.set_gradient_normalization(mode, 1e30)
         probe.fit(xs[0], ys[0])
         thr = _threshold_between(probe.grad_norm_last_norms)
-    gnr.enable(onet, mode, thr)
+    onet.set_gradient_normalization(mode, thr)
     bnet = b.Net(ctx, specs, shape, max_batch=n, precision=b.FP32, gradient_normalization=mode, gradient_normalization_threshold=thr)
     push_params(onet, bnet)
     clipped = []
@@ -113,9 +111,9 @@ def _fp32_dcgan(b, ctx, n, gmode, dmode, gthr=1.0, dthr=1.0):
     size, z, nf = 16, 12, 8
     gs, ds = m.dcgan_generator(size, z, nf, 3, lr=2e-3), m.dcgan_discriminator(size, nf, 3, lr=2e-3)
     rng = np.random.default_rng(5)
-    G = oracle_from_specs(gs, (z,), seed=1); D = oracle_from_specs(ds, (3, size, size), seed=2)
+    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
     randomize(G, rng); randomize(D, rng)
-    gnr.enable(G, gmode, gthr); gnr.enable(D, dmode, dthr)
+    G.set_gradient_normalization(gmode, gthr); D.set_gradient_normalization(dmode, dthr)
     bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32, gradient_normalization=gmode, gradient_normalization_threshold=gthr)
     bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2, gradient_normalization=dmode, gradient_normalization_threshold=dthr)
     push_params(G, bG); push_params(D, bD)
@@ -152,16 +150,16 @@ def test_fp32_gan_step_matches_oracle(b200, mode):
 
 def test_mnist_example_configuration_with_dropout(b200):
     """DL4J's MNIST GAN example: mlp_generator + mlp_discriminator(dropout=0.5), RenormalizeL2PerLayer on both nets, FP32, under the masks of
-    tests/dropout_ref.py."""
+    the oracle's dropout_mask."""
     b, ctx = b200
     from gan_deeplearning4j_b200 import models as m
     n, z, hid, d = 16, 24, 64, 48
     gs, ds = m.mlp_generator(z, hid, d, lr=1e-3), m.mlp_discriminator(d, hid, lr=1e-3, dropout=0.5)
     rng = np.random.default_rng(9)
-    G = oracle_from_specs(gs, (z,), seed=1); D = dr.oracle_from_specs(ds, (d,), mask_seed=667, seed=2)
+    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (d,), mask_seed=667, seed=2)
     randomize(G, rng); randomize(D, rng)
     mode = "renormalize_l2_per_layer"
-    gnr.enable(G, mode); gnr.enable(D, mode)
+    G.set_gradient_normalization(mode); D.set_gradient_normalization(mode)
     bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32, gradient_normalization=mode)
     bD = b.Net(ctx, ds, (d,), max_batch=2 * n, precision=b.FP32, bn_groups=2, seed=667, gradient_normalization=mode)
     push_params(G, bG); push_params(D, bD)
@@ -169,7 +167,7 @@ def test_mnist_example_configuration_with_dropout(b200):
     data = [rng.uniform(-1, 1, (n, d)), rng.uniform(-1, 1, (n, z)), rng.uniform(-1, 1, (n, z)),
             1 + 0.05 * rng.standard_normal((n, 1)), 0.05 * rng.standard_normal((n, 1)), np.ones((n, 1))]
     for it in range(3):
-        r = dr.gan_step(G, D, *data)
+        r = o.gan_step(G, D, *data)
         lo = gan.step(*data)
         want = np.array([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]])
         assert np.all(np.abs(lo - want) < TOL * np.maximum(1, np.abs(want))), (it, lo, want)

@@ -1,11 +1,10 @@
 """DL4J's MSE, L1, L2, MAE, Hinge, SquaredHinge and Wasserstein losses on the GPU: the loss kernel through its production wrapper (b2g_test_ew op
 "loss") for every loss x activation x precision against float64, FP32 fit and output of an MLP OutputLayer(MSE, nOut = 7) and a conv net ending
-in LossLayer(HINGE) against tests/loss_ref.py, the FP32 GAN step (least-squares, hinge, Wasserstein) against the oracle's gan_step, BF16 graph
+in LossLayer(HINGE) against the oracle's score_and_grad, the FP32 GAN step (least-squares, hinge, Wasserstein) against the oracle's gan_step, BF16 graph
 replay against eager with the XENT discriminator's launch counts, the argument checks and checkpoint / resume."""
 import numpy as np
 import pytest
 
-import loss_ref as lr
 from helpers import bf16_round, push_params, randomize, rel_err
 from oracle import dl4j_oracle as o
 
@@ -35,7 +34,7 @@ SHAPES = [(1, 1, 1, 0), (127, 3, 2, 1), (127, 256, 1, 3), (8192, 1, 2, 0), (8192
 def _dlda_and_sens(loss, act, a, y, n_out, alpha):
     """float64 dL/da (with the / nOut), and |d(dL/dz)/da| = |g' h| + |g h'| (h = act'(a)): how far dz moves per unit error in a."""
     e, m = a - y, 1 - y * a
-    per = 1.0 / n_out if lr.per_output(loss) else 1.0
+    per = 1.0 / n_out if o.per_output(loss) else 1.0
     if loss in ("mse", "l2"):
         g, gp = 2 * e * per, np.full_like(a, 2 * per)
     elif loss in ("l1", "mae"):
@@ -46,7 +45,7 @@ def _dlda_and_sens(loss, act, a, y, n_out, alpha):
         g, gp = -2 * y * np.maximum(m, 0), np.where(m > 0, 2 * y * y, 0.0)
     else:
         g, gp = y * per, np.zeros_like(a)
-    h = lr.act_grad_from_out(act, a, alpha)
+    h = o.act_grad_from_out(act, a, alpha)
     hp = {"tanh": -2 * a, "sigmoid": 1 - 2 * a}.get(act, np.zeros_like(a))
     return g, np.abs(gp * h) + np.abs(g * hp)
 
@@ -72,13 +71,13 @@ def _run(b, ctx, prec, loss, act, z, y, rows, n_out, groups, offset, alpha=0.2, 
 
 @pytest.mark.parametrize("prec", ["fp32", "bf16"])
 @pytest.mark.parametrize("act", ACTS)
-@pytest.mark.parametrize("loss", lr.LOSSES)
+@pytest.mark.parametrize("loss", o.LOSSES)
 def test_loss_kernel_against_float64(b200, loss, act, prec):
     """dz within one bf16 ulp (bf16) or 8u (|dz| + sens (|a| + 1)) (fp32, sens = |d dz / da|: a = act(z) carries a few ulp of tanhf / expf and
     each later operation one rounding); loss sums within 2u|S| + 8u sum |dL/da| (|a| + 1); no poisoned element survives."""
     b, ctx = b200
     P = b.BF16 if prec == "bf16" else b.FP32
-    rng = np.random.default_rng(lr.CODES[loss] * 100 + ACTS.index(act) * 10 + P)
+    rng = np.random.default_rng(o.LOSS_CODES[loss] * 100 + ACTS.index(act) * 10 + P)
     for rows, n_out, groups, offset in SHAPES:
         shape = (groups * rows, n_out)
         z = rng.uniform(-3, 3, shape).astype(np.float32); y = _labels(loss, rng, shape).astype(np.float32)
@@ -89,7 +88,7 @@ def test_loss_kernel_against_float64(b200, loss, act, prec):
         a = o.act_forward(act, zd, 0.2)
         y64 = y.astype(np.float64)
         g, sens = _dlda_and_sens(loss, act, a, y64, n_out, 0.2)
-        ref = g * lr.act_grad_from_out(act, a, 0.2)
+        ref = g * o.act_grad_from_out(act, a, 0.2)
         ok = ~_near_kink(loss, a, y64)
         d = np.abs(dz.reshape(shape) - ref)
         if P == b.BF16:
@@ -101,18 +100,18 @@ def test_loss_kernel_against_float64(b200, loss, act, prec):
         assert not bad.any(), (loss, act, prec, rows, n_out, groups, int(bad.sum()), float(d[bad].max()))
         for gi in range(groups):
             sl = slice(gi * rows, (gi + 1) * rows)
-            s_ref, _ = lr.score_and_grad(loss, act, 0.2, zd[sl], y64[sl])
+            s_ref, _ = o.score_and_grad(loss, act, 0.2, zd[sl], y64[sl])
             bound = 2 * U * abs(s_ref) + 8 * U * float((np.abs(g[sl]) * (np.abs(a[sl]) + 1)).sum()) + 1e-30
             assert abs(sums[gi] - s_ref) <= bound, (loss, act, prec, rows, n_out, groups, gi, sums[gi], s_ref, bound)
 
 
 @pytest.mark.parametrize("prec", ["fp32", "bf16"])
-@pytest.mark.parametrize("loss", lr.LOSSES)
+@pytest.mark.parametrize("loss", o.LOSSES)
 def test_small_integers_give_exact_sums(b200, loss, prec):
     """Small-integer z and y, identity: every score is an integer summed exactly in double, then divided by nOut once and rounded to fp32."""
     b, ctx = b200
     P = b.BF16 if prec == "bf16" else b.FP32
-    rng = np.random.default_rng(lr.CODES[loss] + 50 * P)
+    rng = np.random.default_rng(o.LOSS_CODES[loss] + 50 * P)
     for rows, n_out, groups, offset in SHAPES:
         shape = (groups * rows, n_out)
         z = rng.integers(-4, 5, shape).astype(np.float32)
@@ -124,10 +123,10 @@ def test_small_integers_give_exact_sums(b200, loss, prec):
             e, m = z64[sl] - y64[sl], 1 - y64[sl] * z64[sl]
             raw = {"mse": (e * e).sum(), "l2": (e * e).sum(), "l1": np.abs(e).sum(), "mae": np.abs(e).sum(), "hinge": np.maximum(m, 0).sum(),
                    "squared_hinge": (np.maximum(m, 0) ** 2).sum(), "wasserstein": (y64[sl] * z64[sl]).sum()}[loss]
-            want = np.float32(raw / n_out if lr.per_output(loss) else raw)
+            want = np.float32(raw / n_out if o.per_output(loss) else raw)
             assert sums[gi] == want, (loss, prec, rows, n_out, groups, gi, sums[gi], want)
         if loss in ("l1", "mae", "hinge"):        # the kinks: a = y gives 0, a margin of exactly 0 gives 0
-            _, ref = lr.score_and_grad(loss, "identity", 0.0, z64, y64)
+            _, ref = o.score_and_grad(loss, "identity", 0.0, z64, y64)
             assert np.array_equal(dz.reshape(shape), (bf16_round(ref) if P == b.BF16 else ref.astype(np.float32)))
 
 
@@ -166,7 +165,7 @@ def test_fp32_fit_matches_oracle(b200, net):
     b, ctx = b200
     specs, shape = _mlp(net.split("_")[1]) if net.startswith("mlp") else _conv_hinge()
     rng = np.random.default_rng(3)
-    onet = lr.oracle_from_specs(specs, shape, seed=2); randomize(onet, rng)
+    onet = o.net_from_specs(specs, shape, seed=2); randomize(onet, rng)
     bnet = b.Net(ctx, specs, shape, max_batch=6, precision=b.FP32)
     push_params(onet, bnet)
     n_out = 7 if net.startswith("mlp") else 2
@@ -206,7 +205,7 @@ def test_fp32_gan_step_matches_oracle(b200, kind):
     size, z, nf, n, lr_ = 16, 12, 8, 8, 2e-3
     gs, ds = m.dcgan_generator(size, z, nf, 3, lr=lr_), m.dcgan_discriminator(size, nf, 3, lr=lr_, loss=loss, out_activation=act)
     rng = np.random.default_rng(5)
-    G = lr.oracle_from_specs(gs, (z,), seed=1); D = lr.oracle_from_specs(ds, (3, size, size), seed=2)
+    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
     randomize(G, rng); randomize(D, rng)
     bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
     bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2)
@@ -270,7 +269,7 @@ def test_launches_per_step_equal_the_xent_discriminators(b200):
         gan.close(); G.close(); D.close()
         return out, losses
 
-    for loss in ("xent",) + lr.LOSSES:
+    for loss in ("xent",) + o.LOSSES:
         ys = (1.0, -1.0, 1.0) if loss in ("hinge", "squared_hinge", "wasserstein") else (1.0, 0.0, 1.0)
         c2, l2 = per_step(m.dcgan_generator(64, 100, 64, 3), m.dcgan_discriminator(64, 64, 3, loss=loss), (100,), (3, 64, 64), 128, ys)
         c5, l5 = per_step(m.mlp_generator(128, 1024, 256), m.mlp_discriminator(256, 1024, loss=loss), (128,), (256,), 8192, ys)

@@ -8,7 +8,7 @@ compared kernel-by-kernel against the oracle evaluated on the same bf16-rounded 
 import numpy as np
 import pytest
 
-from helpers import bf16_round, oracle_from_specs, pack_deconv_ps, push_params, randomize, rel_err, w_internal
+from helpers import bf16_round, pack_deconv_ps, push_params, randomize, rel_err, w_internal
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
@@ -46,7 +46,7 @@ def test_fp32_every_layer_activations_gradients_and_update(b200, act):
     b, ctx = b200
     specs = every_layer_specs(act)
     rng = np.random.default_rng(0)
-    onet = oracle_from_specs(specs, (3, 9, 9), grad_clip=1.0); randomize(onet, rng)
+    onet = o.net_from_specs(specs, (3, 9, 9), grad_clip=1.0); randomize(onet, rng)
     bnet = b.Net(ctx, specs, (3, 9, 9), max_batch=6, precision=b.FP32, grad_clip=1.0)
     assert bnet.num_params() == onet.num_params()
     push_params(onet, bnet)
@@ -91,7 +91,7 @@ def _gan_pair(b, ctx, size, z, nf, batch, precision, clip_eps=1e-5):
     gs, ds = m.dcgan_generator(size, z, nf, 3, lr=2e-3), m.dcgan_discriminator(size, nf, 3, lr=2e-3)
     q = o.Quirks(xent_clip_eps=clip_eps)
     rng = np.random.default_rng(5)
-    G = oracle_from_specs(gs, (z,), quirks=q, seed=1); D = oracle_from_specs(ds, (3, size, size), quirks=q, seed=2)
+    G = o.net_from_specs(gs, (z,), quirks=q, seed=1); D = o.net_from_specs(ds, (3, size, size), quirks=q, seed=2)
     randomize(G, rng); randomize(D, rng)
     bG = b.Net(ctx, gs, (z,), max_batch=batch, precision=precision, xent_clip_eps=clip_eps)
     bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * batch, precision=precision, xent_clip_eps=clip_eps, bn_groups=2)
@@ -147,7 +147,7 @@ def test_fp32_reference_graphs_replay_J408_510(b200):
     from gan_deeplearning4j_b200 import models as m
     n, z = 8, 2
     dis_s, gen_s, gan_s = m.reference_discriminator(0.002), m.reference_generator(0.0, z), m.reference_gan(0.004, z)
-    odis = oracle_from_specs(dis_s, (1, 28, 28), 1.0, seed=1, flat_input=False); ogen = oracle_from_specs(gen_s, (z,), 1.0, seed=2); ogan = oracle_from_specs(gan_s, (z,), 1.0, seed=3)
+    odis = o.net_from_specs(dis_s, (1, 28, 28), grad_clip=1.0, seed=1, flat_input=False); ogen = o.net_from_specs(gen_s, (z,), grad_clip=1.0, seed=2); ogan = o.net_from_specs(gan_s, (z,), grad_clip=1.0, seed=3)
     ng = len(gen_s)
     mk = lambda s, shp, mb: b.Net(ctx, s, shp, max_batch=mb, precision=b.FP32, grad_clip=1.0)
     bdis, bw0, bw1, bgen, bgan = mk(dis_s, (1, 28, 28), n), mk(dis_s, (1, 28, 28), n), mk(dis_s, (1, 28, 28), n), mk(gen_s, (z,), n), mk(gan_s, (z,), n)
@@ -416,7 +416,7 @@ def test_edge_layers_dcgan_ends(b200, prec):
     gs, ds = m.dcgan_generator(size, z, nf, 3, lr=1e-3), m.dcgan_discriminator(size, nf, 3, lr=1e-3)
     q = o.Quirks(xent_clip_eps=0.0)
     rng = np.random.default_rng(11)
-    G = oracle_from_specs(gs, (z,), quirks=q, seed=1); D = oracle_from_specs(ds, (3, size, size), quirks=q, seed=2)
+    G = o.net_from_specs(gs, (z,), quirks=q, seed=1); D = o.net_from_specs(ds, (3, size, size), quirks=q, seed=2)
     randomize(G, rng); randomize(D, rng)
     bG = b.Net(ctx, gs, (z,), max_batch=n, precision=P, xent_clip_eps=0.0)
     bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=P, xent_clip_eps=0.0, bn_groups=2)
@@ -470,7 +470,7 @@ def test_mlp_gan_step_matches_oracle(b200, prec):
     gs, ds = m.mlp_generator(z, hid, d, lr=1e-3), m.mlp_discriminator(d, hid, lr=1e-3)
     q = o.Quirks(xent_clip_eps=0.0)
     rng = np.random.default_rng(21)
-    G = oracle_from_specs(gs, (z,), quirks=q, seed=1); D = oracle_from_specs(ds, (d,), quirks=q, seed=2)
+    G = o.net_from_specs(gs, (z,), quirks=q, seed=1); D = o.net_from_specs(ds, (d,), quirks=q, seed=2)
     randomize(G, rng); randomize(D, rng)
     bG = b.Net(ctx, gs, (z,), max_batch=n, precision=P, xent_clip_eps=0.0)
     bD = b.Net(ctx, ds, (d,), max_batch=2 * n, precision=P, xent_clip_eps=0.0, bn_groups=2)
@@ -549,7 +549,7 @@ def test_boundary_error_codes(b200):
         b.Net(ctx, [{"type": "dense", "name": "d", "n_out": 4}], (8,), max_batch=2).fit(np.zeros((2, 8)), np.zeros((2, 1)))
     assert e.value.code == -6
     # ragged batches: every batch size from 1 up to max works and matches the oracle (falls back to non-tiled kernels)
-    onet = oracle_from_specs(specs, (3, 16, 16)); push_params(onet, net)
+    onet = o.net_from_specs(specs, (3, 16, 16)); push_params(onet, net)
     for bs in (1, 3, 4):
         x = np.random.default_rng(bs).uniform(-1, 1, (bs, 3, 16, 16))
         assert rel_err(net.output(x), onet.output(x).reshape(bs, -1)) < TOL
@@ -561,7 +561,7 @@ def test_fp32_transfer_learning_head_matches_oracle(b200):
     b, ctx = b200
     from gan_deeplearning4j_b200 import models as m
     n = 8
-    odis = oracle_from_specs(m.reference_discriminator(), (1, 28, 28), 1.0, seed=1, flat_input=False)
+    odis = o.net_from_specs(m.reference_discriminator(), (1, 28, 28), grad_clip=1.0, seed=1, flat_input=False)
     rng = np.random.default_rng(3); randomize(odis, rng)
     ocv = o.reference_computer_vision(odis)
     specs = m.reference_computer_vision()
@@ -712,7 +712,7 @@ def test_single_process_parameter_averaging_matches_oracle(b200):
     from gan_deeplearning4j_b200 import models as m, parallel
     specs = m.reference_discriminator(0.002)
     rng = np.random.default_rng(17)
-    onet = oracle_from_specs(specs, (1, 28, 28), grad_clip=1.0); randomize(onet, rng)
+    onet = o.net_from_specs(specs, (1, 28, 28), grad_clip=1.0); randomize(onet, rng)
     bnet = b.Net(ctx, specs, (1, 28, 28), max_batch=8, precision=b.FP32, grad_clip=1.0)
     push_params(onet, bnet)
     d = [(rng.uniform(0, 1, (8, 1, 28, 28)), 1 + 0.05 * rng.standard_normal((8, 1))), (rng.uniform(0, 1, (8, 1, 28, 28)), 0.05 * rng.standard_normal((8, 1)))]
@@ -804,7 +804,7 @@ def test_bf16_fit_weight_operands_track_the_master(b200, upd, ps_bias):
     u = {"sgd": m.sgd(0.05), "rmsprop": m.rmsprop(1e-3, 0.9, 1e-6), "adam": m.adam(1e-3)}[upd]
     specs = _ps_fit_specs(u, ps_bias)
     off = 0
-    for li, name, p, shape, _ in oracle_from_specs(specs, (64, 8, 8)).param_table():
+    for li, name, p, shape, _ in o.net_from_specs(specs, (64, 8, 8)).param_table():
         if (name, p) == ("ps", "W"):
             break
         off += int(np.prod(shape))

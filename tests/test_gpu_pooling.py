@@ -1,5 +1,5 @@
 """Average, sum and p-norm pooling on the GPU: the pool2d / global_pool kernels through their production wrappers (b2g_test_ew ops pool2d /
-global_pool) against tests/pooling_ref.py in both precisions on the vector, C % 8 != 0 and misaligned paths, with poisoned outputs and a global
+global_pool) against the oracle's restatement in both precisions on the vector, C % 8 != 0 and misaligned paths, with poisoned outputs and a global
 map large enough to be split over blocks; fp32 AVG / SUM forwards bit for bit against an fp32 emulation of the documented summation order; FP32
 nets with every kind against the float64 oracle over 3 fit iterations (one of them a ragged batch); BF16 nets layer by layer; the BF16 GAN step
 with a global-pooling-head discriminator (graph replay == eager, two fresh nets equal, bit for bit); launches per pass; argument checks."""
@@ -8,7 +8,6 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import pooling_ref as pr
 from helpers import bf16_round, check_bf16, push_params, randomize, rel_err
 from oracle import dl4j_oracle as o
 
@@ -59,7 +58,7 @@ def test_pool2d_kernels_against_float64(b200, kind, p, prec, path):
     P = b.FP32 if prec == "fp32" else b.BF16
     c, off = PATHS[path]
     u_out = U if P == b.FP32 else 2.0 ** -8
-    rng = np.random.default_rng(pr.CODES[kind] * 10 + p)
+    rng = np.random.default_rng(o.POOL_CODES[kind] * 10 + p)
     for (kh, kw), (sh, sw), (ph, pw), h, w in [((3, 3), (2, 2), (1, 1), 9, 7), ((2, 3), (3, 1), (1, 2), 7, 6)]:
         n = 3
         oh, ow = (h + 2 * ph - kh) // sh + 1, (w + 2 * pw - kw) // sw + 1
@@ -71,12 +70,12 @@ def test_pool2d_kernels_against_float64(b200, kind, p, prec, path):
         xs, es = (x, e) if P == b.FP32 else (bf16_round(x), bf16_round(e))
         xs, es = _nchw(xs.astype(np.float64)), _nchw(es.astype(np.float64))
         geo = ((kh, kw), (sh, sw), (ph, pw))
-        y_ref = pr.pool2d_forward(kind, xs, *geo, p)
-        y_mag = y_ref if kind == "pnorm" else pr.pool2d_forward(kind, np.abs(xs), *geo, p)
+        y_ref = o.pool2d_forward(kind, xs, *geo, p)
+        y_mag = y_ref if kind == "pnorm" else o.pool2d_forward(kind, np.abs(xs), *geo, p)
         _within(_nchw(y.reshape(n, oh, ow, c)), y_ref, y_mag, u_out, 32, (kind, p, prec, path, "y"))
         y_dev = _nchw(y.reshape(n, oh, ow, c).astype(np.float64))          # the backward reads the stored y
-        dx_ref = pr.pool2d_backward(kind, xs, y_dev, es, *geo, p)
-        dx_mag = pr.pool2d_backward(kind, np.abs(xs), y_dev, np.abs(es), *geo, p)
+        dx_ref = o.pool2d_backward(kind, xs, y_dev, es, *geo, p)
+        dx_mag = o.pool2d_backward(kind, np.abs(xs), y_dev, np.abs(es), *geo, p)
         _within(_nchw(dx.reshape(n, h, w, c)), dx_ref, dx_mag, u_out, 64, (kind, p, prec, path, "dx"))
 
 
@@ -103,7 +102,7 @@ def test_global_kernels_against_float64(b200, kind, p, prec, path, shape):
     c, off = PATHS[path]
     u_out = U if P == b.FP32 else 2.0 ** -8
     n, h, w = (5, 4, 3) if shape == "small" else (2, 64, 48)
-    rng = np.random.default_rng(pr.CODES[kind] * 10 + p + (shape == "split"))
+    rng = np.random.default_rng(o.POOL_CODES[kind] * 10 + p + (shape == "split"))
     x = rng.uniform(-2, 2, (n, h, w, c)).astype(np.float32)
     e = rng.uniform(-2, 2, (n, c)).astype(np.float32)
     (y, dx, idx), info = b.test_pool(ctx, P, "global_pool", x, e, (n * c, n * h * w * c, n * c), pooling=kind, N=n, H=h, W=w, C=c, pnorm=float(p),
@@ -113,16 +112,16 @@ def test_global_kernels_against_float64(b200, kind, p, prec, path, shape):
     assert info["splits"] == want_splits and (want_splits > 1) == (shape == "split"), (info, want_splits)
     xs, es = (x, e) if P == b.FP32 else (bf16_round(x), bf16_round(e))
     xs, es = _nchw(xs.astype(np.float64)), es.astype(np.float64)
-    y_ref, i_ref = pr.global_forward(kind, xs, p)
+    y_ref, i_ref = o.global_forward(kind, xs, p)
     if kind == "max":
         assert np.array_equal(idx.reshape(n, c), i_ref) and np.array_equal(y.reshape(n, c), y_ref), (kind, prec, path, shape)
     else:
         assert (idx == -1).all()
-        y_mag = y_ref if kind == "pnorm" else pr.global_forward(kind, np.abs(xs), p)[0]
+        y_mag = y_ref if kind == "pnorm" else o.global_forward(kind, np.abs(xs), p)[0]
         _within(y.reshape(n, c), y_ref, y_mag, u_out, 128, (kind, p, prec, path, shape, "y"))
     y_dev = y.reshape(n, c).astype(np.float64)
-    dx_ref = pr.global_backward(kind, xs, y_dev, i_ref, es, p)
-    dx_mag = pr.global_backward(kind, np.abs(xs), y_dev, i_ref, np.abs(es), p)
+    dx_ref = o.global_backward(kind, xs, y_dev, i_ref, es, p)
+    dx_mag = o.global_backward(kind, np.abs(xs), y_dev, i_ref, np.abs(es), p)
     _within(_nchw(dx.reshape(n, h, w, c)), dx_ref, dx_mag, u_out, 8, (kind, p, prec, path, shape, "dx"))
 
 
@@ -214,8 +213,8 @@ def test_fp32_nets_match_oracle(b200, net, pool, p):
     the second on a ragged batch of 5 (max_batch 6)."""
     b, ctx = b200
     specs, shape = (_sub_net if net == "sub" else _global_net)(pool, p)
-    rng = np.random.default_rng(pr.CODES[pool] * 10 + p)
-    onet = pr.oracle_from_specs(specs, shape, seed=2, flat_input=False); randomize(onet, rng)
+    rng = np.random.default_rng(o.POOL_CODES[pool] * 10 + p)
+    onet = o.net_from_specs(specs, shape, seed=2, flat_input=False); randomize(onet, rng)
     bnet = b.Net(ctx, specs, shape, max_batch=6, precision=b.FP32)
     push_params(onet, bnet)
     for it, mb in enumerate((6, 5, 6)):
@@ -250,10 +249,10 @@ def test_bf16_nets_layer_by_layer(b200, pool, p):
               {"type": "conv2d", "name": "c2", "n_out": 128, "kernel": (3, 3), "stride": (1, 1), "padding": (1, 1), "has_bias": False},
               {"type": "batchnorm", "name": "bn2"}, {"type": "activation", "name": "a2", "activation": "lrelu", "alpha": 0.2},
               dict(m.global_pooling(pool, p), name="g"), {"type": "output", "name": "out", "n_out": 1}]
-    rng = np.random.default_rng(pr.CODES[pool])
+    rng = np.random.default_rng(o.POOL_CODES[pool])
     for specs in (m.dcgan_discriminator(16, 64, 3, global_pooling=pool), specs2):
         x = bf16_round(rng.uniform(-1, 1, (n, 3, 16, 16)))
-        onet = pr.oracle_from_specs(specs, (3, 16, 16), seed=3, flat_input=False); randomize(onet, rng)
+        onet = o.net_from_specs(specs, (3, 16, 16), seed=3, flat_input=False); randomize(onet, rng)
         for l in onet.layers:
             if l.has_params and "W" in l.params:
                 l.params["W"] = bf16_round(l.params["W"]).astype(np.float64)
@@ -296,7 +295,7 @@ def test_bf16_gan_step_with_global_pooling_head_is_reproducible(b200, pool):
     ds = m.dcgan_discriminator(size, nf, 3, lr=2e-4, global_pooling=pool)
     data = [a.astype(np.float32) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
     rng = np.random.default_rng(5)
-    G = pr.oracle_from_specs(gs, (z,), seed=1); D = pr.oracle_from_specs(ds, (3, size, size), seed=2)
+    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
     randomize(G, rng); randomize(D, rng)
     runs = [_gan_run(b, ctx, gs, ds, G, D, data, n, size, z, graph) for graph in (True, False, True)]
     for a, c in ((runs[0], runs[1]), (runs[0], runs[2])):
@@ -324,7 +323,7 @@ def test_fp32_gan_step_with_global_pooling_head_matches_oracle(b200):
     ds = m.dcgan_discriminator(size, nf, 3, lr=lr_, global_pooling="sum")
     data = [a.astype(np.float64) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
     rng = np.random.default_rng(5)
-    G = pr.oracle_from_specs(gs, (z,), seed=1); D = pr.oracle_from_specs(ds, (3, size, size), seed=2)
+    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
     randomize(G, rng); randomize(D, rng)
     bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
     bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2)

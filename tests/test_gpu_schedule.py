@@ -1,4 +1,4 @@
-"""Learning-rate schedules on the GPU: the device-evaluated rate of every kind and type against tests/schedule_ref.py, FP32 fit and the fused
+"""Learning-rate schedules on the GPU: the device-evaluated rate of every kind and type against the oracle's lr_at, FP32 fit and the fused
 GAN step against the oracle, CUDA-graph replay against eager bit for bit (an epoch change without a re-capture, a schedule change with one),
 identity schedules, checkpoint / resume, the bf16 weight copies, launch counts and argument checks."""
 import copy
@@ -6,7 +6,6 @@ import copy
 import numpy as np
 import pytest
 
-import schedule_ref as sr
 from helpers import bf16_round, pack_deconv_ps, push_params, randomize, rel_err, w_internal
 from oracle import dl4j_oracle as o
 
@@ -89,7 +88,7 @@ def test_learning_rate_of_every_kind_matches_the_restatement(b200, type_):
         for c in counters:
             other = 7 + c % 5                      # the counter the schedule does not read must not matter
             net.set_iteration(c if type_ == "iteration" else other); net.set_epoch(c if type_ == "epoch" else other)
-            got, want = net.learning_rate("d2"), sr.lr_at(sched, c if type_ == "iteration" else other, c if type_ == "epoch" else other)
+            got, want = net.learning_rate("d2"), o.lr_at(sched, c if type_ == "iteration" else other, c if type_ == "epoch" else other)
             assert _f32_close(got, want), (sched, c, got, want)
             assert net.learning_rate("d1") == np.float32(0.02)        # unscheduled layers keep their constant lr
     net.set_lr_schedule(None, "d2")
@@ -103,7 +102,7 @@ def _fit_run(b, ctx, kind, upd, sched_name):
     sched = m.step_schedule(lr0, 0.5, 3) if sched_name == "step" else m.map_schedule({0: lr0, 2: 0.3 * lr0, 5: 0.6 * lr0})
     specs, shape = _specs(kind, upd, sched)
     rng = np.random.default_rng(11)
-    onet = sr.oracle_from_specs(specs, shape, seed=2); randomize(onet, rng)
+    onet = o.net_from_specs(specs, shape, seed=2); randomize(onet, rng)
     bnet = b.Net(ctx, specs, shape, max_batch=6, precision=b.FP32)
     push_params(onet, bnet)
     return onet, bnet, shape, rng
@@ -119,7 +118,7 @@ def test_fp32_fit_matches_oracle(b200, kind, upd, sched_name):
     for it in range(8):
         x, y = rng.uniform(-1, 1, (6,) + shape), rng.uniform(0, 1, (6, 1))
         name = onet.layers[-1].name
-        assert _f32_close(bnet.learning_rate(name), sr.lr_at(onet.lr_schedules[name], onet.iteration, 0))
+        assert _f32_close(bnet.learning_rate(name), onet.learning_rate(name))
         seen.add(float(bnet.learning_rate(name)))
         onet.fit(x, y); bnet.fit(x, y)
         _compare(onet, bnet, (kind, upd, sched_name, it))
@@ -132,7 +131,7 @@ def test_set_and_clear_mid_run_take_effect_at_the_next_update(b200):
     m = _m()
     specs, shape = _specs("mlp", "adam", 1e-2)
     rng = np.random.default_rng(3)
-    onet = sr.oracle_from_specs(specs, shape, seed=2); randomize(onet, rng)
+    onet = o.net_from_specs(specs, shape, seed=2); randomize(onet, rng)
     bnet = b.Net(ctx, specs, shape, max_batch=6, precision=b.FP32)
     push_params(onet, bnet)
     names = ["d1", "d2", "out"]
@@ -143,9 +142,9 @@ def test_set_and_clear_mid_run_take_effect_at_the_next_update(b200):
             layer, sched = change
             sched = None if sched == "clear" else sched
             bnet.set_lr_schedule(sched, None if layer == "all" else layer)
-            sr.set_schedule(onet, sched, names if layer == "all" else [layer])
+            onet.set_lr_schedule(sched, None if layer == "all" else layer)
         if it == 5:
-            bnet.set_epoch(4); onet.epoch = 4
+            bnet.set_epoch(4); onet.set_epoch(4)
         x, y = rng.uniform(-1, 1, (6,) + shape), rng.uniform(0, 1, (6, 1))
         onet.fit(x, y); bnet.fit(x, y)
         _compare(onet, bnet, ("plan", it))
@@ -158,7 +157,7 @@ def _fp32_dcgan(b, ctx, n, gsched, dsched):
     size, z, nf = 16, 12, 8
     gs, ds = m.dcgan_generator(size, z, nf, 3, lr=gsched), m.dcgan_discriminator(size, nf, 3, lr=dsched)
     rng = np.random.default_rng(5)
-    G = sr.oracle_from_specs(gs, (z,), seed=1); D = sr.oracle_from_specs(ds, (3, size, size), seed=2)
+    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
     randomize(G, rng); randomize(D, rng)
     bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
     bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2)

@@ -23,7 +23,7 @@ import numpy as np
 import pytest
 
 import conv_ref
-from helpers import bf16_round, oracle_from_specs, push_params, randomize, rel_err
+from helpers import bf16_round, push_params, randomize, rel_err
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
@@ -352,7 +352,7 @@ def test_hook_refuses_epilogues_the_wrappers_lack(b200):
 # ------------------------------------------------------------------ (4) through the engine --------------------------------------------------
 def _fp32_grads_and_fit(b, ctx, specs, in_shape, x, y, prec):
     rng = np.random.default_rng(2)
-    onet = oracle_from_specs(specs, in_shape, quirks=o.Quirks(xent_clip_eps=0.0)); randomize(onet, rng)
+    onet = o.net_from_specs(specs, in_shape, quirks=o.Quirks(xent_clip_eps=0.0)); randomize(onet, rng)
     bnet = b.Net(ctx, specs, in_shape, max_batch=x.shape[0], precision=prec, xent_clip_eps=0.0)
     push_params(onet, bnet)
     s_o = onet.compute_gradient_and_score(x, y); s_b = bnet.compute_gradient_and_score(x, y)
@@ -415,7 +415,7 @@ def test_dcgan_with_192_filters_steps(b200, prec):
     gs, ds = m.dcgan_generator(size, z, nf, 3, lr=1e-3), m.dcgan_discriminator(size, nf, 3, lr=1e-3)
     q = o.Quirks(xent_clip_eps=0.0)
     rng = np.random.default_rng(13)
-    G = oracle_from_specs(gs, (z,), quirks=q, seed=1); D = oracle_from_specs(ds, (3, size, size), quirks=q, seed=2)
+    G = o.net_from_specs(gs, (z,), quirks=q, seed=1); D = o.net_from_specs(ds, (3, size, size), quirks=q, seed=2)
     randomize(G, rng); randomize(D, rng)
     bG = b.Net(ctx, gs, (z,), max_batch=n, precision=P, xent_clip_eps=0.0)
     bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=P, xent_clip_eps=0.0, bn_groups=2)

@@ -1,4 +1,4 @@
-"""DL4J's Nesterovs, AdaGrad, AdaMax, Nadam, AMSGrad and AdaDelta on the GPU: FP32 fit of every kind against tests/updater_ref.py on an MLP and a
+"""DL4J's Nesterovs, AdaGrad, AdaMax, Nadam, AMSGrad and AdaDelta on the GPU: FP32 fit of every kind against the oracle on an MLP and a
 conv+BatchNorm net (parameters and every state slot), a net that mixes kinds per layer, odd widths (the scalar path), gradient normalization
 and schedules, the FP32 GAN step against the oracle, BF16 graph replay against eager and the bf16 weight copies, AMSGrad checkpoint / resume,
 parameter averaging, launch counts and argument checks."""
@@ -11,14 +11,13 @@ import sys
 import numpy as np
 import pytest
 
-import updater_ref as ur
 from helpers import bf16_round, pack_deconv_ps, push_params, randomize, rel_err, w_internal
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TOL = 1e-3
-KINDS = ur.KINDS
+KINDS = o.EXT_UPDATERS
 
 
 @pytest.fixture(scope="module")
@@ -124,7 +123,9 @@ def _bounds(specs):
 
 def _fit_and_compare(b, ctx, specs, shape, steps=6, grad_clip=0.5, seed=11, **net_kw):
     rng = np.random.default_rng(seed)
-    onet = ur.oracle_from_specs(specs, shape, seed=2, grad_clip=grad_clip, grad_norm=net_kw.pop("oracle_grad_norm", None)); randomize(onet, rng)
+    onet = o.net_from_specs(specs, shape, seed=2, grad_clip=grad_clip); randomize(onet, rng)
+    if "oracle_grad_norm" in net_kw:
+        onet.set_gradient_normalization(*net_kw.pop("oracle_grad_norm"))
     bnet = b.Net(ctx, specs, shape, max_batch=6, precision=b.FP32, grad_clip=grad_clip, **net_kw)
     push_params(onet, bnet)
     for it in range(steps):
@@ -204,7 +205,7 @@ def _fp32_dcgan(b, ctx, n, gkind, dkind):
     gs = [dict(s, updater=_upd(gkind)) if s.get("updater") else s for s in gs]
     ds = [dict(s, updater=_upd(dkind)) if s.get("updater") else s for s in ds]
     rng = np.random.default_rng(5)
-    G = ur.oracle_from_specs(gs, (z,), seed=1); D = ur.oracle_from_specs(ds, (3, size, size), seed=2)
+    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
     randomize(G, rng); randomize(D, rng)
     bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
     bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2)
@@ -327,7 +328,7 @@ def test_single_process_parameter_averaging_with_amsgrad_matches_oracle(b200):
     from gan_deeplearning4j_b200 import parallel
     specs, shape = _specs("mlp", "amsgrad")
     rng = np.random.default_rng(17)
-    onet = ur.oracle_from_specs(specs, shape, seed=2, grad_clip=0.5); randomize(onet, rng)
+    onet = o.net_from_specs(specs, shape, seed=2, grad_clip=0.5); randomize(onet, rng)
     bnet = b.Net(ctx, specs, shape, max_batch=8, precision=b.FP32, grad_clip=0.5)
     push_params(onet, bnet)
     for rnd in range(2):

@@ -1,4 +1,4 @@
-"""The L2 gradient normalization restatement (tests/gradnorm_ref.py) against hand-computed answers on tiny layers, and the plumbing of the mode
+"""The oracle's L2 gradient normalization against hand-computed answers on tiny layers, and the plumbing of the mode
 names through the C header, the ctypes binding, the Java enum and the JNI shim.  CPU only."""
 import copy
 import os
@@ -9,7 +9,6 @@ import sys
 import numpy as np
 import pytest
 
-import gradnorm_ref as gnr
 from oracle import dl4j_oracle as o
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -24,7 +23,8 @@ def _dense(l2=0.0, lr=1.0):
 
 
 def _update(net, mode, threshold, grads, mb, **q):
-    gnr.enable(net, mode, threshold, gnr.GradNormQuirks(**q))
+    net.q = o.Quirks(**q)
+    net.set_gradient_normalization(mode, threshold)
     net.apply_update(mb, grads=grads)
     return net
 
@@ -53,8 +53,8 @@ def test_multiplier_is_rounded_to_fp32_once():
     net = _update(_dense(), "renormalize_l2_per_layer", 1.0, G, 2)
     m = np.float32(1.0 / 13.0)
     assert -net.layers[0].params["W"][1, 0] == 4.0 * float(m)
-    assert gnr.multiplier(169.0, "clip_l2_per_layer", 13.0) == 1.0 and gnr.multiplier(169.0 * 1.01, "clip_l2_per_layer", 13.0) < 1.0
-    assert gnr.multiplier(169.0 * 1.01, "clip_l2_per_layer", 13.0) == np.float32(13.0 / np.sqrt(169.0 * 1.01))
+    assert o.multiplier(169.0, "clip_l2_per_layer", 13.0) == 1.0 and o.multiplier(169.0 * 1.01, "clip_l2_per_layer", 13.0) < 1.0
+    assert o.multiplier(169.0 * 1.01, "clip_l2_per_layer", 13.0) == np.float32(13.0 / np.sqrt(169.0 * 1.01))
 
 
 def test_zero_gradient_under_renormalize_moves_only_by_l2():
@@ -68,7 +68,7 @@ def test_zero_gradient_under_renormalize_moves_only_by_l2():
         assert np.all(np.isfinite(net.layers[0].params["W"]))
         np.testing.assert_array_equal(net.layers[0].params["W"].ravel(), [2.0 * 0.9, -4.0 * 0.9])     # W - l2 * W, no gradient part
         np.testing.assert_array_equal(net.layers[0].params["b"], [3.0])                               # no l2 on b
-    assert gnr.multiplier(0.0, "renormalize_l2_per_layer", 1.0) == np.float32(1e5)
+    assert o.multiplier(0.0, "renormalize_l2_per_layer", 1.0) == np.float32(1e5)
 
 
 def _bn_net():
@@ -111,7 +111,8 @@ def test_frozen_layers_are_left_out_and_gan_step_picks_the_mode_up():
     rng = np.random.default_rng(0)
     base = o.Net([o.Dense(3, 4, "tanh", updater=o.Sgd(0.1), name="a"), o.Output(4, 1, updater=o.Sgd(0.1), name="out")], seed=3)
     x, y = rng.uniform(-1, 1, (5, 3)), rng.uniform(0, 1, (5, 1))
-    plain, normed = copy.deepcopy(base), gnr.enable(copy.deepcopy(base), "renormalize_l2_per_layer")
+    plain, normed = copy.deepcopy(base), copy.deepcopy(base)
+    normed.set_gradient_normalization("renormalize_l2_per_layer")
     plain.fit(x, y); normed.fit(x, y)
     assert len(normed.grad_norm_last_norms) == 2
     d_plain = base.params_flat() - plain.params_flat()
@@ -120,7 +121,8 @@ def test_frozen_layers_are_left_out_and_gan_step_picks_the_mode_up():
     for sl in (slice(0, 16), slice(16, 21)):
         np.testing.assert_allclose(np.linalg.norm(d_norm[sl]), 0.1, rtol=1e-6)
         np.testing.assert_allclose(d_norm[sl] / np.linalg.norm(d_norm[sl]), d_plain[sl] / np.linalg.norm(d_plain[sl]), rtol=1e-9)
-    frozen = gnr.enable(copy.deepcopy(base), "renormalize_l2_per_layer")
+    frozen = copy.deepcopy(base)
+    frozen.set_gradient_normalization("renormalize_l2_per_layer")
     frozen.layers[0].frozen = True
     frozen.compute_gradient_and_score(x, y)
     frozen.apply_update(5)
@@ -139,7 +141,7 @@ def test_mode_names_match_header_java_and_python():
     assert h == {"NONE": 0, "RENORM_L2_LAYER": 1, "RENORM_L2_PARAM": 2, "CLIP_ELEMENTWISE": 3, "CLIP_L2_LAYER": 4, "CLIP_L2_PARAM": 5}
     assert GRADIENT_NORMALIZATIONS == {"none": 0, "renormalize_l2_per_layer": 1, "renormalize_l2_per_param_type": 2, "clip_l2_per_layer": 4,
                                        "clip_l2_per_param_type": 5}
-    assert set(GRADIENT_NORMALIZATIONS) == set(gnr.MODES)
+    assert set(GRADIENT_NORMALIZATIONS) == set(o.GRAD_NORMS)
     java = open(os.path.join(ROOT, "java/src/main/java/org/deeplearning4j/nn/conf/GradientNormalization.java")).read()
     names = re.search(r"enum GradientNormalization \{\s*([^;}]*)", java).group(1).replace(" ", "").replace("\n", "").split(",")
     assert names == ["None", "RenormalizeL2PerLayer", "RenormalizeL2PerParamType", "ClipElementWiseAbsoluteValue", "ClipL2PerLayer", "ClipL2PerParamType"]

@@ -88,11 +88,11 @@ def test_bench_dump_outputs_fit_64_mb_for_every_config(tmp_path):
     """bench.py --dump-outputs at the real parameter counts of every benchmark config: at most 64 MB on disk, whole vectors where they fit,
     otherwise a seeded sample whose float64 indices select the same elements on every run."""
     import bench
-    from helpers import oracle_from_specs
+    
     for name, cfg in bench.CONFIGS.items():
         gs, ds, gin, din = bench.build_specs(cfg)
-        ng = oracle_from_specs(gs, gin, dtype=np.float32).num_params()
-        nd = oracle_from_specs(ds, din, dtype=np.float32, flat_input=False).num_params()
+        ng = o.net_from_specs(gs, gin, dtype=np.float32).num_params()
+        nd = o.net_from_specs(ds, din, dtype=np.float32, flat_input=False).num_params()
         arrays = {"losses": np.arange(3, dtype=np.float32), "g_params": np.arange(ng, dtype=np.float32), "d_params": np.arange(nd, dtype=np.float32)}
         for run in ("a", "b"):
             bench.dump_outputs(str(tmp_path / name / run), arrays)

@@ -18,8 +18,9 @@ from helpers import pack_deconv_ps, randomize
 from oracle import dl4j_oracle as o
 
 
-def fd_check(net, x, y, eps=1e-6, max_rel=1e-3, min_abs=1e-8, n_probe=60, seed=0):
-    net.compute_gradient_and_score(x, y)
+def fd_check(net, x, y, eps=1e-6, max_rel=1e-3, min_abs=1e-8, n_probe=60, seed=0, **kw):
+    """kw: passed to compute_gradient_and_score (pass_ pins the DropoutLayer masks)."""
+    net.compute_gradient_and_score(x, y, **kw)
     mb = x.shape[0]
     g = net.grads_flat() / mb
     # l2 contributes l2*W to d(score)/dW; add analytically (DL4J's check includes it via the score)
@@ -40,8 +41,8 @@ def fd_check(net, x, y, eps=1e-6, max_rel=1e-3, min_abs=1e-8, n_probe=60, seed=0
     idx = rng.choice(np.flatnonzero(mask), size=min(n_probe, mask.sum()), replace=False)
     worst = 0.0
     for i in idx:
-        pp = p0.copy(); pp[i] += eps; net.set_params_flat(pp); sp = net.compute_gradient_and_score(x, y)
-        pm = p0.copy(); pm[i] -= eps; net.set_params_flat(pm); sm = net.compute_gradient_and_score(x, y)
+        pp = p0.copy(); pp[i] += eps; net.set_params_flat(pp); sp = net.compute_gradient_and_score(x, y, **kw)
+        pm = p0.copy(); pm[i] -= eps; net.set_params_flat(pm); sm = net.compute_gradient_and_score(x, y, **kw)
         num = (sp - sm) / (2 * eps)
         ana = g[i] + l2[i] * p0[i]
         if abs(num - ana) < min_abs:
@@ -80,6 +81,30 @@ def test_finite_differences_every_layer(act):
             l.params["gamma"] = rng.uniform(0.5, 1.5, l.n)
             l.params["beta"] = rng.uniform(-0.5, 0.5, l.n)
     fd_check(net, x, y)
+
+
+def test_finite_differences_of_a_net_composing_the_later_features():
+    """One net_from_specs net mixing an ELU conv, AVG subsampling with padding, a DropoutLayer (pinned to one pass), AdaGrad / Nesterovs on a
+    step schedule and an MSE output on Softsign: GradientCheckUtil's tolerances, then two fits through the one update pipeline."""
+    from gan_deeplearning4j_b200 import models as m
+    sched = m.step_schedule(0.05, 0.5, 1)
+    specs = [{"type": "conv2d", "name": "c1", "n_out": 4, "kernel": (3, 3), "padding": (1, 1), "activation": "elu", "updater": m.adagrad(sched), "l2": 1e-3},
+             {"type": "subsampling", "name": "s", "pooling": "avg", "kernel": (2, 2), "stride": (2, 2), "padding": (1, 1)},
+             {"type": "cnn_to_ff", "name": "ff"},
+             {"type": "dropout", "name": "drop", "p": 0.7},
+             {"type": "dense", "name": "d1", "n_out": 6, "activation": "swish", "updater": m.nesterovs(sched, 0.9)},
+             {"type": "output", "name": "out", "n_out": 3, "loss": "mse", "activation": "softsign", "updater": m.adam(1e-2)}]
+    net = o.net_from_specs(specs, (2, 5, 5), seed=4, flat_input=False)
+    rng = np.random.default_rng(7)
+    randomize(net, rng)
+    x, y = rng.uniform(-1, 1, (4, 2, 5, 5)), rng.uniform(-1, 1, (4, 3))
+    fd_check(net, x, y, pass_=0)
+    assert net.dropout_pass() == 0 and net.layers[3].index == 3
+    p0 = net.params_flat().copy()
+    net.fit(x, y); net.fit(x, y)
+    assert net.iteration == 2 and net.dropout_pass() == 2
+    assert net.learning_rate("c1") == net.learning_rate("d1") == np.float32(0.0125) and net.learning_rate("out") == 1e-2
+    assert len(net.state[(0, "W")]) == 1 and np.all(np.isfinite(net.params_flat())) and not np.any(net.params_flat() == p0)
 
 
 def test_finite_differences_dcgan_tiny():

@@ -1,4 +1,4 @@
-"""CPU checks of the learning-rate schedules: the restatement (tests/schedule_ref.py) against hand-computed values at and around the
+"""CPU checks of the learning-rate schedules: the oracle's restatement against hand-computed values at and around the
 boundaries, identity schedules leave the oracle bit-identical, the updater-spec builders, and the boundary (header enums, ctypes layout of
 b2g_lr_schedule against the C compiler, bound and exported symbols)."""
 import copy
@@ -12,45 +12,45 @@ import sys
 import numpy as np
 import pytest
 
-import schedule_ref as sr
-from helpers import oracle_from_specs
+
 from gan_deeplearning4j_b200 import models as m
+from oracle import dl4j_oracle as o
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def test_exponential_and_inverse():
     e = m.exponential_schedule(0.1, 0.9)
-    assert sr.value(e, 0) == 0.1 and sr.value(e, 1) == 0.1 * 0.9 and sr.value(e, 3) == 0.1 * 0.9 ** 3
+    assert o.value(e, 0) == 0.1 and o.value(e, 1) == 0.1 * 0.9 and o.value(e, 3) == 0.1 * 0.9 ** 3
     inv = m.inverse_schedule(0.2, 0.5, 2.0)
-    assert sr.value(inv, 0) == 0.2 and sr.value(inv, 2) == 0.2 / 4.0 and sr.value(inv, 6) == 0.2 / 16.0
-    assert sr.lr_at(e, 3, 0) == np.float32(0.1 * 0.9 ** 3) and sr.lr_at(e, 3, 0).dtype == np.float32
+    assert o.value(inv, 0) == 0.2 and o.value(inv, 2) == 0.2 / 4.0 and o.value(inv, 6) == 0.2 / 16.0
+    assert o.lr_at(e, 3, 0) == np.float32(0.1 * 0.9 ** 3) and o.lr_at(e, 3, 0).dtype == np.float32
 
 
 def test_sigmoid_at_and_around_its_step_size():
     s = m.sigmoid_schedule(0.4, 2.0, 10)
-    assert sr.value(s, 10) == 0.2                                   # exactly half at i = stepSize
-    assert sr.value(s, 9) == 0.4 / (1 + math.exp(2.0)) < 0.2 < sr.value(s, 11) == 0.4 / (1 + math.exp(-2.0))
-    assert sr.value(s, 0) < sr.value(s, 5) < sr.value(s, 10) < sr.value(s, 100) <= 0.4
+    assert o.value(s, 10) == 0.2                                   # exactly half at i = stepSize
+    assert o.value(s, 9) == 0.4 / (1 + math.exp(2.0)) < 0.2 < o.value(s, 11) == 0.4 / (1 + math.exp(-2.0))
+    assert o.value(s, 0) < o.value(s, 5) < o.value(s, 10) < o.value(s, 100) <= 0.4
 
 
 def test_step_at_multiples_of_step():
     s = m.step_schedule(0.08, 0.5, 3)
-    assert [sr.value(s, i) for i in range(10)] == [0.08] * 3 + [0.04] * 3 + [0.02] * 3 + [0.01]
+    assert [o.value(s, i) for i in range(10)] == [0.08] * 3 + [0.04] * 3 + [0.02] * 3 + [0.01]
     frac = m.step_schedule(1.0, 0.1, 2.5)                          # step is a double: floor(i / 2.5)
-    assert [sr.value(frac, i) for i in range(8)] == [1.0, 1.0, 1.0, 0.1, 0.1, 0.1 ** 2, 0.1 ** 2, 0.1 ** 2]
+    assert [o.value(frac, i) for i in range(8)] == [1.0, 1.0, 1.0, 0.1, 0.1, 0.1 ** 2, 0.1 ** 2, 0.1 ** 2]
 
 
 def test_map_at_and_between_keys():
     s = m.map_schedule({10: 0.01, 0: 0.1, 3: 0.05})
     assert s["values"] == [[0, 0.1], [3, 0.05], [10, 0.01]]       # sorted [key, value] pairs (JSON-safe)
-    assert [sr.value(s, i) for i in (0, 1, 2, 3, 4, 9, 10, 11, 10 ** 6)] == [0.1, 0.1, 0.1, 0.05, 0.05, 0.05, 0.01, 0.01, 0.01]
+    assert [o.value(s, i) for i in (0, 1, 2, 3, 4, 9, 10, 11, 10 ** 6)] == [0.1, 0.1, 0.1, 0.05, 0.05, 0.05, 0.01, 0.01, 0.01]
     assert m.map_schedule([(0, 1.0), (5, 2.0)])["values"] == [[0, 1.0], [5, 2.0]]
 
 
 def test_type_selects_the_counter():
     it, ep = m.step_schedule(1.0, 0.5, 1), m.step_schedule(1.0, 0.5, 1, type="epoch")
-    assert sr.lr_at(it, 3, 1) == np.float32(0.125) and sr.lr_at(ep, 3, 1) == np.float32(0.5)
+    assert o.lr_at(it, 3, 1) == np.float32(0.125) and o.lr_at(ep, 3, 1) == np.float32(0.5)
 
 
 def _mlp(lr):
@@ -63,12 +63,12 @@ def _mlp(lr):
 def test_identity_schedules_leave_the_oracle_bit_identical(identity):
     lr = float(np.float32(3e-3))         # the engine's constant lr is fp32; a schedule's value is rounded to fp32 too
     sched = m.exponential_schedule(lr, 1.0) if identity == "exponential" else m.map_schedule({0: lr})
-    plain = oracle_from_specs(_mlp(lr), (5,), seed=4)
+    plain = o.net_from_specs(_mlp(lr), (5,), seed=4)
     specs = copy.deepcopy(_mlp(lr))
     for s in specs:
         s["updater"]["lr"] = sched
-    wrapped = sr.oracle_from_specs(specs, (5,), seed=4)
-    assert set(wrapped.lr_schedules) == {"d1", "d2", "out"}
+    wrapped = o.net_from_specs(specs, (5,), seed=4)
+    assert set(wrapped.schedules) == {"d1", "d2", "out"}
     rng = np.random.default_rng(0)
     for _ in range(4):
         x, y = rng.uniform(-1, 1, (6, 5)), rng.uniform(0, 1, (6, 1))
@@ -83,7 +83,7 @@ def test_wrapped_oracle_uses_the_scheduled_rate_per_update():
     """SGD with a StepSchedule: each update moves the output bias by exactly lr_i * g (no l2 on biases)."""
     sched = m.step_schedule(0.5, 0.5, 2)
     specs = [{"type": "output", "name": "out", "n_out": 1, "updater": m.sgd(sched)}]
-    net = sr.oracle_from_specs(specs, (3,), seed=2)
+    net = o.net_from_specs(specs, (3,), seed=2)
     rng = np.random.default_rng(1)
     for it in range(5):
         x, y = rng.uniform(-1, 1, (4, 3)), rng.uniform(0, 1, (4, 1))
@@ -92,21 +92,21 @@ def test_wrapped_oracle_uses_the_scheduled_rate_per_update():
         g = net.layers[0].grads["b"] / 4
         net.apply_update(4)
         np.testing.assert_allclose(b0 - net.layers[0].params["b"], float(np.float32(0.5 * 0.5 ** (it // 2))) * g, rtol=1e-12)
-    sr.set_schedule(net, None, ["out"])
+    net.set_lr_schedule(None, "out")
     assert net.iteration == 5
     net.compute_gradient_and_score(x, y); net.apply_update(4)
-    assert net.layers[0].updater.lr == 0.5                      # back to the constant lr
+    assert net.learning_rate("out") == 0.5                      # back to the constant lr
 
 
 def test_epoch_schedules_follow_the_epoch_word():
     specs = [{"type": "output", "name": "out", "n_out": 1, "updater": m.sgd(m.map_schedule({0: 0.1, 2: 0.01}, type="epoch"))}]
-    net = sr.oracle_from_specs(specs, (3,), seed=2)
+    net = o.net_from_specs(specs, (3,), seed=2)
     x, y = np.ones((2, 3)), np.ones((2, 1))
     lrs = []
     for ep in (0, 1, 2, 5, 0):
-        net.epoch = ep
+        net.set_epoch(ep)
+        lrs.append(net.learning_rate("out"))
         net.compute_gradient_and_score(x, y); net.apply_update(2)
-        lrs.append(net.layers[0].updater.lr)
     assert lrs == [float(np.float32(v)) for v in (0.1, 0.1, 0.01, 0.01, 0.1)]
 
 

@@ -6,8 +6,8 @@ import math
 
 import numpy as np
 
-import schedule_ref as sr
 from gan_deeplearning4j_b200 import engine, models as m
+from oracle import dl4j_oracle as o
 
 
 def _schedules():
@@ -17,13 +17,13 @@ def _schedules():
 
 def test_constant_lr_is_the_value_at_zero_for_every_kind():
     for s in _schedules():
-        assert engine.constant_lr(s) == engine.schedule_value(s, 0) == sr.value(s, 0), s
+        assert engine.constant_lr(s) == engine.schedule_value(s, 0) == o.value(s, 0), s
     assert engine.constant_lr(m.sigmoid_schedule(0.4, 2.0, 10)) == 0.4 / (1 + math.exp(20.0))      # not `initial`
     assert engine.layer_desc({"type": "dense", "name": "d", "n_out": 2, "updater": m.sgd(m.sigmoid_schedule(0.4, 0.5, 1))}).lr == \
         np.float32(0.4 / (1 + math.exp(0.5)))
     for s in _schedules():
         for i in (0, 1, 2, 3, 7, 10, 11, 250):
-            assert engine.schedule_value(s, i) == sr.value(s, i), (s, i)
+            assert engine.schedule_value(s, i) == o.value(s, i), (s, i)
 
 
 def _specs():

@@ -1,6 +1,6 @@
-"""CPU checks of the updater restatement (tests/updater_ref.py): hand-computed answers over three steps for every new kind, float64 agreement
-with torch.optim where the two forms are the same update, the existing kinds unchanged by the wrapper (alone and stacked with gradient
-normalization and schedules), the quirk flags, mixed-kind nets and parameter averaging of the new state."""
+"""CPU checks of the oracle's updaters: hand-computed answers over three steps for every new kind, float64 agreement with torch.optim where
+the two forms are the same update, the spec builder's existing kinds against a hand-built net (alone and with gradient normalization and
+schedules), the quirk flags, mixed-kind nets and parameter averaging of the new state."""
 import copy
 import math
 
@@ -8,10 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-import gradnorm_ref as gr
-import schedule_ref as sr
-import updater_ref as ur
-from helpers import oracle_from_specs, randomize
+from helpers import randomize
 from gan_deeplearning4j_b200 import models as m
 from oracle import dl4j_oracle as o
 
@@ -35,8 +32,8 @@ KNOWN = {
 BUILDERS = {"nesterovs": m.nesterovs, "adagrad": m.adagrad, "adamax": m.adamax, "nadam": m.nadam, "amsgrad": m.amsgrad, "adadelta": m.adadelta}
 
 
-def _scalar_net(upd, quirks=ur.DEFAULT_UPDATER_QUIRKS, **kw):
-    net = ur.oracle_from_specs([{"type": "dense", "name": "d", "n_out": 1, "has_bias": False, "updater": upd}], (1,), quirks=quirks, **kw)
+def _scalar_net(upd, quirks=o.DEFAULT_QUIRKS, **kw):
+    net = o.net_from_specs([{"type": "dense", "name": "d", "n_out": 1, "has_bias": False, "updater": upd}], (1,), quirks=quirks, **kw)
     net.layers[0].params["W"] = np.ones((1, 1))
     return net
 
@@ -45,13 +42,13 @@ def _step(net, g, mb=2):
     net.apply_update(mb, grads={(0, "W"): np.full((1, 1), g * mb)})
 
 
-@pytest.mark.parametrize("kind", ur.KINDS)
+@pytest.mark.parametrize("kind", o.EXT_UPDATERS)
 def test_known_answers_over_three_steps(kind):
     net = _scalar_net(BUILDERS[kind]())
     for it, (g, want) in enumerate(zip(G3, KNOWN[kind])):
         _step(net, g)
         got = (float(net.layers[0].params["W"][0, 0]),) + tuple(float(s[0, 0]) for s in net.state[(0, "W")])
-        assert len(got) == len(want) == 1 + ur.N_STATE[kind]
+        assert len(got) == len(want) == 1 + o.N_STATE[kind]
         assert np.allclose(got, want, rtol=1e-10, atol=0), (kind, it, got, want)
     assert net.iteration == 3
 
@@ -66,9 +63,9 @@ def _torch_run(opt_fn, g_seq, p0):
 
 
 def _ref_run(u, g_seq, p0):
-    p, st = np.array(p0, np.float64), ur.init_state(u, np.shape(p0))
+    p, st = np.array(p0, np.float64), o.init_state(u, np.shape(p0))
     for t, g in enumerate(g_seq, 1):
-        p = p - ur.update(u, st, np.asarray(g, np.float64), t)
+        p = p - o.update(u, st, np.asarray(g, np.float64), t)
     return p
 
 
@@ -79,11 +76,11 @@ def test_float64_agreement_with_torch_optim(case):
     rng = np.random.default_rng(7)
     g_seq, p0 = [rng.standard_normal(13) for _ in range(6)], rng.standard_normal(13)
     if case == "nesterovs":
-        u, fn = ur.updater_cfg(m.nesterovs(0.05, 0.8)), lambda ps: torch.optim.SGD(ps, lr=0.05, momentum=0.8, nesterov=True)
+        u, fn = o.updater_cfg(m.nesterovs(0.05, 0.8)), lambda ps: torch.optim.SGD(ps, lr=0.05, momentum=0.8, nesterov=True)
     elif case == "adagrad":
-        u, fn = ur.updater_cfg(m.adagrad(0.1, 1e-6)), lambda ps: torch.optim.Adagrad(ps, lr=0.1, initial_accumulator_value=1e-6, eps=1e-6)
+        u, fn = o.updater_cfg(m.adagrad(0.1, 1e-6)), lambda ps: torch.optim.Adagrad(ps, lr=0.1, initial_accumulator_value=1e-6, eps=1e-6)
     else:
-        u, fn = ur.updater_cfg(m.adadelta(0.9, 1e-6)), lambda ps: torch.optim.Adadelta(ps, lr=1.0, rho=0.9, eps=1e-6)
+        u, fn = o.updater_cfg(m.adadelta(0.9, 1e-6)), lambda ps: torch.optim.Adadelta(ps, lr=1.0, rho=0.9, eps=1e-6)
     got, want = _ref_run(u, g_seq, p0), _torch_run(fn, g_seq, p0)
     assert np.allclose(got, want, rtol=1e-12, atol=1e-14), (case, np.abs(got - want).max())
 
@@ -113,15 +110,22 @@ def _same(a, b):
 
 @pytest.mark.parametrize("stack", ["plain", "gradnorm+schedule"])
 def test_existing_kinds_are_bit_identical_through_the_wrapper(stack):
+    """The spec builder's nets of the existing kinds against the same net built by hand ("plain") and against schedules and a normalization
+    mode set through the Net's methods."""
     sched = m.exponential_schedule(1e-2, 0.9)
     specs = _old_specs(sched if stack != "plain" else 1e-2)
     rng = np.random.default_rng(1)
     if stack == "plain":
-        a = oracle_from_specs(specs, (6,), seed=4, grad_clip=0.5)
-        b = ur.oracle_from_specs(specs, (6,), seed=4, grad_clip=0.5)
+        a = o.Net([o.Dense(6, 16, "tanh", updater=o.Adam(1e-2), l2=1e-3, name="d1"), o.BatchNorm(16, updater=o.RmsProp(1e-2, 0.9, 1e-8), name="bn"),
+                   o.Dense(16, 8, "lrelu", 0.2, updater=o.Sgd(0.05), name="d2"), o.Dense(8, 8, "tanh", updater=o.UpdaterCfg("noop"), name="d3"),
+                   o.Output(8, 1, updater=o.Adam(2e-3), name="out")], seed=4, grad_clip=0.5)
+        b = o.net_from_specs(specs, (6,), seed=4, grad_clip=0.5)
     else:
-        a = sr.enable(gr.enable(oracle_from_specs(sr.constant_specs(specs), (6,), seed=4), "clip_l2_per_layer", 0.3), sr.scheduled_layers(specs))
-        b = ur.oracle_from_specs(specs, (6,), grad_norm=("clip_l2_per_layer", 0.3), seed=4)
+        a = o.net_from_specs(_old_specs(o.value(sched, 0)), (6,), seed=4)
+        a.set_lr_schedule(sched, "d1")
+        b = o.net_from_specs(specs, (6,), seed=4)
+        for net in (a, b):
+            net.set_gradient_normalization("clip_l2_per_layer", 0.3)
     randomize(a, rng); b.set_params_flat(a.params_flat())
     _same(_fit(a, 4), _fit(b, 4))
 
@@ -139,17 +143,17 @@ def test_mixed_net_updates_each_layer_by_its_own_kind():
     update() says, the BatchNorm mean/var through NoOp, and the iteration advances once."""
     specs = _mixed_specs()
     rng = np.random.default_rng(2)
-    a = ur.oracle_from_specs(specs, (6,), seed=4, grad_clip=0.7)
+    a = o.net_from_specs(specs, (6,), seed=4, grad_clip=0.7)
     randomize(a, rng)
-    plain_specs = [dict(s, updater=m.noop()) if s["updater"]["kind"] in ur.KINDS else s for s in specs]
-    b = oracle_from_specs(plain_specs, (6,), seed=4, grad_clip=0.7); b.set_params_flat(a.params_flat())
+    plain_specs = [dict(s, updater=m.noop()) if s["updater"]["kind"] in o.EXT_UPDATERS else s for s in specs]
+    b = o.net_from_specs(plain_specs, (6,), seed=4, grad_clip=0.7); b.set_params_flat(a.params_flat())
     grads = {(li, p): 3 * rng.standard_normal(sh) for li, l in enumerate(a.layers) for p, sh, _ in l.param_specs()}
     before = {k: a.layers[k[0]].params[k[1]].copy() for k in grads}
     a.apply_update(4, grads=copy.deepcopy(grads)); b.apply_update(4, grads=copy.deepcopy(grads))
     assert a.iteration == b.iteration == 1
     for (li, p), g in grads.items():
         l = a.layers[li]
-        if l.updater.kind not in ur.KINDS:
+        if l.updater.kind not in o.EXT_UPDATERS:
             assert np.array_equal(l.params[p], b.layers[li].params[p]), (li, p)
             continue
         gd = g if p in l.noop_names() else g / 4
@@ -158,7 +162,7 @@ def test_mixed_net_updates_each_layer_by_its_own_kind():
             want = before[(li, p)] - gd
             assert (li, p) not in a.state
         else:
-            upd = ur.update(l.updater, ur.init_state(l.updater, g.shape), gd, 1)
+            upd = o.update(l.updater, o.init_state(l.updater, g.shape), gd, 1)
             want = before[(li, p)] - (upd + (l.l2 * before[(li, p)] if l.l2 and p in l.l2_names() else 0))
         assert np.allclose(l.params[p], want, rtol=1e-14, atol=1e-15), (li, p)
 
@@ -166,7 +170,8 @@ def test_mixed_net_updates_each_layer_by_its_own_kind():
 def test_schedules_and_gradient_normalization_reach_the_new_kinds():
     sched = m.step_schedule(0.1, 0.5, 1)
     specs = [{"type": "dense", "name": "d", "n_out": 3, "has_bias": False, "updater": m.nesterovs(sched, 0.9)}]
-    net = ur.oracle_from_specs(specs, (2,), grad_norm=("renormalize_l2_per_layer", 1.0), seed=1)
+    net = o.net_from_specs(specs, (2,), seed=1)
+    net.set_gradient_normalization("renormalize_l2_per_layer", 1.0)
     w = net.layers[0].params["W"].copy()
     v = np.zeros_like(w)
     rng = np.random.default_rng(5)
@@ -182,7 +187,7 @@ def test_schedules_and_gradient_normalization_reach_the_new_kinds():
 
 def test_parameter_average_averages_the_new_state():
     specs = _mixed_specs()
-    nets = [_fit(ur.oracle_from_specs(specs, (6,), seed=4), 2, seed=s) for s in (1, 2)]
+    nets = [_fit(o.net_from_specs(specs, (6,), seed=4), 2, seed=s) for s in (1, 2)]
     want = {k: [(x + y) / 2 for x, y in zip(nets[0].state[k], nets[1].state[k])] for k in nets[0].state}
     assert len(nets[0].state[(0, "W")]) == 3            # AMSGrad's three slots are all there
     into = copy.deepcopy(nets[0])
@@ -194,17 +199,17 @@ def test_parameter_average_averages_the_new_state():
 def test_each_quirk_flag_changes_what_it_should():
     g = np.array([0.3, -2.0, 0.0])
     def run(kind, q, hp, steps=2):
-        u = ur.updater_cfg(BUILDERS[kind](**hp))
-        st = ur.init_state(u, g.shape, q=q)
+        u = o.updater_cfg(BUILDERS[kind](**hp))
+        st = o.init_state(u, g.shape, q=q)
         init = [s.copy() for s in st]
-        us = [ur.update(u, st, g, t, q) for t in range(1, steps + 1)]
+        us = [o.update(u, st, g, t, q) for t in range(1, steps + 1)]
         return init, us, st
-    base = ur.DEFAULT_UPDATER_QUIRKS
+    base = o.DEFAULT_QUIRKS
     flags = {"adagrad_history_init_eps": ("adagrad", {}), "adamax_floor_no_eps": ("adamax", {"eps": 0.1}),
              "nadam_v_uncorrected": ("nadam", {})}
     for flag, (kind, hp) in flags.items():
-        q = ur.UpdaterQuirks(**{flag: not getattr(base, flag)})
-        for other in ur.KINDS:                          # the flag leaves every other kind alone, bit for bit
+        q = o.Quirks(**{flag: not getattr(base, flag)})
+        for other in o.EXT_UPDATERS:                          # the flag leaves every other kind alone, bit for bit
             if other != kind:
                 a, b = run(other, base, {}), run(other, q, {})
                 assert all(np.array_equal(x, y) for x, y in zip(a[1], b[1])), (flag, other)

@@ -14,8 +14,7 @@ import torch.distributed as dist
 
 import gan_deeplearning4j_b200 as b
 from gan_deeplearning4j_b200 import models as m, parallel
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-from dropout_ref import dropout_mask  # noqa: E402  (the test suite's NumPy restatement of the mask)
+from oracle.dl4j_oracle import dropout_mask  # noqa: E402  (the oracle's NumPy restatement of the mask)
 
 rank, world, local = parallel.env_rank_world()
 torch.cuda.set_device(local)
