@@ -1504,11 +1504,12 @@ extern "C" int32_t b2g_ctx_allreduce_test(b2g_ctx* c, float* host, int64_t n) {
 }
 
 // ------------------------------------------------------------------ kernel-level test hook ----------------
-// The tile-width / grid overrides of tc_conv_kernel hold for the hook's own launch loop only: reset right after it, and on every early return.
+// The tile-width / grid / split-count overrides of the tensor-core kernels hold for the hook's own launch loop only: reset right after it, and on
+// every early return.
 struct TcTestSchedule {
-  TcTestSchedule(int bn, int max_ctas, int per_tap) { g_tc_test_bn = bn; g_tc_test_max_ctas = max_ctas; g_tc_test_per_tap = per_tap; }
+  TcTestSchedule(int bn, int max_ctas, int per_tap, int splits) { g_tc_test_bn = bn; g_tc_test_max_ctas = max_ctas; g_tc_test_per_tap = per_tap; g_tc_test_splits = splits; }
   ~TcTestSchedule() { reset(); }
-  void reset() { g_tc_test_bn = 0; g_tc_test_max_ctas = 0; g_tc_test_per_tap = 0; }
+  void reset() { g_tc_test_bn = 0; g_tc_test_max_ctas = 0; g_tc_test_per_tap = 0; g_tc_test_splits = 0; }
 };
 extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int32_t precision, const b2g_conv_geom* gg, const float* a_host, const float* b_host, float* out, int32_t iters, float* ms_per_iter,
                                     b2g_test_conv_opts* opt) {
@@ -1525,6 +1526,7 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
     if (!ok) return fail(B2G_ERR_UNSUPPORTED, "no tensor-core kernel for this shape");
   }
   const bool tc_conv = impl == 1 && kind != 2, ps = impl == 3 && kind == 1;     // the launches of tc_conv_kernel (ps: its pixel-shuffle form)
+  const bool edge_fwd = impl == 3 && kind == 0, tc_wg = kind == 2 && (impl == 1 || impl == 3);   // tc_edge_conv_kernel; the tensor-core weight gradients
   // the SIMT, skinny-layer and dense kernels; gemm_epi: those whose production wrapper takes bias / activation (k_dense_small_o_dgrad and the
   // weight gradients have none: as in gemm_dgrad, a dense input gradient with an epilogue runs the short-reduction kernel)
   const bool gemm = impl == 0 || impl == 2 || impl == 4;
@@ -1534,10 +1536,12 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
       return fail(B2G_ERR_UNSUPPORTED, "impl %d kind %d: no epilogue (bias / activation: impl 0 / 2 kind 0 / 1, impl 4 kind 0 and the short-reduction kind 1; no fused BatchNorm epilogue)", impl, kind);
     if (opt->scale && impl != 0) return fail(B2G_ERR_UNSUPPORTED, "scale applies to the SIMT fprop / dgrad (impl 0) and the tensor-core kernels");
   }
-  else if (opt && !tc_conv && !ps && (opt->epi || opt->bias || opt->scale || opt->act))
-    return fail(B2G_ERR_UNSUPPORTED, "epilogue options apply to the tensor-core fprop / dgrad kernels (impl 1, kind 0 / 1), the pixel-shuffle deconv (impl 3, kind 1) and the SIMT / skinny-layer / dense kernels (impl 0 / 2 / 4)");
+  else if (opt && !tc_conv && !ps && !edge_fwd && (opt->epi || opt->bias || opt->scale || opt->act))
+    return fail(B2G_ERR_UNSUPPORTED, "epilogue options apply to the tensor-core fprop / dgrad kernels (impl 1, kind 0 / 1), the tensor-core skinny-layer conv and pixel-shuffle deconv (impl 3, kind 0 / 1) and the SIMT / skinny-layer / dense kernels (impl 0 / 2 / 4)");
+  if (opt && edge_fwd && (opt->epi || opt->scale)) return fail(B2G_ERR_UNSUPPORTED, "the tensor-core skinny-layer conv has bias and activation only");
   const int poff = opt ? opt->param_offset : 0;
-  if (poff < 0 || (poff && !gemm)) return fail(B2G_ERR_UNSUPPORTED, "param_offset %d: applies to the SIMT / skinny-layer / dense kernels (impl 0 / 2 / 4)", poff);
+  if (poff < 0 || (poff && !gemm && !tc_wg))
+    return fail(B2G_ERR_UNSUPPORTED, "param_offset %d: applies to the SIMT / skinny-layer / dense kernels (impl 0 / 2 / 4) and the tensor-core weight gradients (kind 2, impl 1 / 3)", poff);
   if (opt && ps && (opt->scale || (opt->epi != EPI_PLAIN && opt->epi != EPI_ACTBWD)))
     return fail(B2G_ERR_UNSUPPORTED, "the pixel-shuffle deconv has bias, activation and the activation-backward epilogue only");
   const int force_bn = opt ? opt->bn : 0, max_ctas = opt ? opt->max_ctas : 0;
@@ -1545,8 +1549,10 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   if (per_tap && !tc_conv) return fail(B2G_ERR_UNSUPPORTED, "per_tap applies to the tensor-core fprop / dgrad kernels (impl 1, kind 0 / 1)");
   if (force_bn && (!tc_conv || (force_bn != 64 && force_bn != 128) || oc % force_bn))
     return fail(B2G_ERR_UNSUPPORTED, "bn %d: the tensor-core fprop / dgrad tile is 64 or 128 columns and must divide the %d output channels", force_bn, oc);
-  if (max_ctas < 0 || (max_ctas && !tc_conv && !ps)) return fail(B2G_ERR_UNSUPPORTED, "max_ctas %d: a grid cap applies to tc_conv_kernel launches only", max_ctas);
-  if (poison && kind == 2 && !gemm) return fail(B2G_ERR_UNSUPPORTED, "poison applies to the outputs of kinds 0 / 1, and to the weight gradients of impl 0 / 2 / 4");
+  if (max_ctas < 0 || (max_ctas && !tc_conv && !ps && !edge_fwd))
+    return fail(B2G_ERR_UNSUPPORTED, "max_ctas %d: a grid cap applies to tc_conv_kernel and tc_edge_conv_kernel launches only", max_ctas);
+  const int force_splits = opt ? opt->splits : 0;
+  if (force_splits < 0 || (force_splits && !tc_wg)) return fail(B2G_ERR_UNSUPPORTED, "splits %d: a forced split count applies to the tensor-core weight gradients (kind 2, impl 1 / 3)", force_splits);
   if (w_mn && (impl != 1 || kind != 0 || g.KH != 1 || g.KW != 1)) return fail(B2G_ERR_UNSUPPORTED, "w_mn: the [C][O] weight operand exists for the 1x1 tensor-core fprop only");
   const bool defer = opt && opt->defer; float* db_host = opt ? opt->db : nullptr;
   if (defer && !(kind == 2 && (impl == 1 || impl == 3))) return fail(B2G_ERR_UNSUPPORTED, "defer applies to the tensor-core weight gradients (kind 2, impl 1 / 3)");
@@ -1564,6 +1570,8 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   float *fa = nullptr, *fb = nullptr, *fo = nullptr, *scratch = nullptr; void *ta = nullptr, *tb = nullptr, *to = nullptr; __nv_bfloat16* wps = nullptr;
   float *d_bias = nullptr, *d_scale = nullptr, *d_coef = nullptr, *d_auxf = nullptr; __nv_bfloat16 *d_aux = nullptr, *d_aux2 = nullptr; unsigned long long* d_acc = nullptr;
   size_t sc = std::max(std::max(std::max(k_simt_wgrad_scratch_floats(g), k_tc_wgrad_scratch_floats(g)), std::max(k_edge_wgrad_scratch_floats(g), k_tc_edge_wgrad_scratch_floats(g))), k_dense_small_o_wgrad_scratch_floats(g)) + 16;
+  // a forced split count needs room for that many partials: [splits][dw] (tc_wgrad_kernel), [ctas][dw] + [ctas][db] with ctas <= splits (tc_edge_wgrad_kernel)
+  if (force_splits) sc = std::max(sc, (size_t)force_splits * (impl == 1 ? nw : (size_t)64 * 16 * g.C + 64) + 16);
   // param_offset: the fp32 weight operand (FP32, kinds 0 / 1) and the weight gradient (kind 2) start poff elements past the 256-byte aligned
   // cudaMalloc base, as W and dW do in a net's flattened parameter / gradient vectors
   const size_t woff = (prec == PREC_F32 && kind != 2) ? (size_t)poff : 0, dwoff = kind == 2 ? (size_t)poff : 0;
@@ -1575,11 +1583,11 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   if (prec == PREC_BF16) { k_cast_f32_to_bf16(fa, (__nv_bfloat16*)ta, na, s); k_cast_f32_to_bf16(fb, (__nv_bfloat16*)tb, nb, s); }
   else { CU(cudaMemcpyAsync(ta, fa, 4 * na, cudaMemcpyDeviceToDevice, s)); CU(cudaMemcpyAsync(tb, fb, 4 * nb, cudaMemcpyDeviceToDevice, s)); }
   if (impl == 3 && kind == 1) { CU(cudaMalloc(&wps, 2 * k_tc_deconv_ps_weight_elems(g))); k_pack_deconv_ps(fb, wps, g.O, g.C, s); }
-  float* d_db = nullptr; int db_written = 0;
-  if (db_host) CU(cudaMalloc(&d_db, 4 * (size_t)g.O));
+  float *d_db = nullptr, *dbres = nullptr; int db_written = 0;
+  if (db_host) { CU(cudaMalloc(&d_db, 4 * ((size_t)g.O + dwoff))); dbres = d_db + dwoff; }      // db sits poff elements past the aligned base, as dw does
   ReduceList rl{}; ReduceList* prl = defer ? &rl : nullptr;
   TcEpi epi{}; const TcEpi* pe = nullptr; const float* bias = nullptr; int act = 0; float alpha = 0.f; int groups = 1;
-  if (opt && (tc_conv || ps)) {
+  if (opt && (tc_conv || ps || edge_fwd)) {
     groups = opt->groups > 0 ? opt->groups : 1; act = opt->act; alpha = opt->alpha;
     if (opt->bias) { CU(cudaMalloc(&d_bias, 4 * oc)); CU(cudaMemcpyAsync(d_bias, opt->bias, 4 * oc, cudaMemcpyHostToDevice, s)); bias = d_bias; }
     if (opt->scale) { CU(cudaMalloc(&d_scale, 4 * oc)); CU(cudaMemcpyAsync(d_scale, opt->scale, 4 * oc, cudaMemcpyHostToDevice, s)); }
@@ -1602,13 +1610,14 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   }
   cudaEvent_t e0, e1; CU(cudaEventCreate(&e0)); CU(cudaEventCreate(&e1));
   int reps = iters < 1 ? 1 : iters; int rc = 0;
-  g_tc_last_kernel = ""; g_tc_last_slab = false; g_gemm_last_kernel = ""; g_gemm_last_splits = 0;
-  TcTestSchedule schedule(force_bn, max_ctas, per_tap);
+  g_tc_last_kernel = ""; g_tc_last_slab = false; g_tc_last_splits = 0; g_gemm_last_kernel = ""; g_gemm_last_splits = 0;
+  TcTestSchedule schedule(force_bn, max_ctas, per_tap, force_splits);
   for (int it = -1; it < reps; ++it) {       // it = -1: warm-up
     if (it == 0) CU(cudaEventRecord(e0, s));
     if (d_acc) CU(cudaMemsetAsync(d_acc, 0, 8 * k_bn_acc_elems(oc, groups), s));
     if (poison) CU(cudaMemsetAsync(to, 0xFF, ts * no, s));       // a tile this launch does not write reads back as NaN, not as the warm-up's values
     if (poison && kind == 2) { CU(cudaMemsetAsync(fres, 0xFF, 4 * no, s)); CU(cudaMemsetAsync(scratch, 0xFF, 4 * sc, s)); }   // fp32 NaN: dw and the split-K partials
+    if (poison && dbres) CU(cudaMemsetAsync(dbres, 0xFF, 4 * (size_t)g.O, s));
     if (impl == 4) {
       const bool so = dense_small_o_supported(g);
       if (kind == 0) k_dense_small_o_fwd(prec, prec, g, ta, tb, bias, to, act, alpha, s);
@@ -1616,10 +1625,10 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
       else { if (so) k_dense_small_o_wgrad(prec, g, ta, tb, fres, scratch, 0, s); else k_dense_small_k_wgrad(prec, g, ta, tb, fres, s); }
     }
     else if (impl >= 2) {
-      if (kind == 0) { if (impl == 3) rc = k_tc_edge_conv(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, nullptr, (__nv_bfloat16*)to, 0, 0.f, s); else k_edge_conv_small_cin(prec, prec, g, ta, tb, bias, to, act, alpha, s); }
+      if (kind == 0) { if (impl == 3) rc = k_tc_edge_conv(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s); else k_edge_conv_small_cin(prec, prec, g, ta, tb, bias, to, act, alpha, s); }
       else if (kind == 1) { if (impl == 3) rc = k_tc_deconv_ps(g, (const __nv_bfloat16*)ta, wps, bias, (__nv_bfloat16*)to, act, alpha, s, pe); else k_edge_deconv_small_c(prec, prec, g, ta, tb, bias, to, act, alpha, s); }
       else {
-        if (impl == 3) { rc = k_tc_edge_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fres, d_db, scratch, sc, 0, s, prl); if (rc >= 0) { db_written = rc; rc = 0; } }
+        if (impl == 3) { rc = k_tc_edge_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fres, dbres, scratch, sc, 0, s, prl); if (rc >= 0) { db_written = rc; rc = 0; } }
         else k_edge_wgrad_small_cin(prec, g, ta, tb, fres, scratch, 0, s);
       }
     }
@@ -1638,11 +1647,11 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   if (rc) return fail(B2G_ERR_CUDA, "tensor-core kernel launch failed (%d)", rc);
   if (opt) {
     strncpy(opt->kernel, gemm ? g_gemm_last_kernel : g_tc_last_kernel, sizeof(opt->kernel) - 1); opt->kernel[sizeof(opt->kernel) - 1] = 0; opt->slab = g_tc_last_slab;
-    opt->splits = gemm ? g_gemm_last_splits : 0;
+    opt->splits = gemm ? g_gemm_last_splits : tc_wg ? g_tc_last_splits : 0;
   }
   if (d_db) {
     if (!db_written) { cudaFree(d_db); return fail(B2G_ERR_UNSUPPORTED, "the edge weight gradient produces no bias column for C = %d", g.C); }
-    CU(cudaMemcpyAsync(db_host, d_db, 4 * (size_t)g.O, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(db_host, dbres, 4 * (size_t)g.O, cudaMemcpyDeviceToHost, s));
   }
   if (kind != 2) { if (prec == PREC_BF16) { /* widen */ k_nhwc_to_nchw_f32(prec, to, fo, 1, 1, (int)no, s); } else CU(cudaMemcpyAsync(fo, to, 4 * no, cudaMemcpyDeviceToDevice, s)); }
   CU(cudaMemcpyAsync(out, fres, 4 * no, cudaMemcpyDeviceToHost, s));

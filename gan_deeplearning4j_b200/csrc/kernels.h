@@ -251,6 +251,10 @@ extern int g_tc_test_bn, g_tc_test_max_ctas;
 // loaded its activations as 2x2-tap slabs (kernels_tc.cu slab_tile)
 extern int g_tc_test_per_tap;
 extern bool g_tc_last_slab;
+// g_tc_test_splits forces the split count of the weight gradients: tc_wgrad_kernel's grid.x (any value >= 1; splits past the last K-block are
+// empty) and tc_edge_wgrad_kernel's CTA target (tiles_per_cta = ceil(tiles / splits)); g_tc_test_max_ctas is tc_edge_conv_kernel's CTA target
+// the same way.  g_tc_last_splits: the split count the most recent k_tc_wgrad / k_tc_edge_wgrad launched
+extern int g_tc_test_splits, g_tc_last_splits;
 // epilogue of the fprop / dgrad kernels (kernels_tc.cu): what happens between the fp32 accumulator and the bf16 store
 enum { EPI_PLAIN = 0, EPI_STATS = 1, EPI_BNBWD = 2, EPI_ACTBWD = 3 };
 struct TcEpi {

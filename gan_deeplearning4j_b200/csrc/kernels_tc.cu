@@ -588,7 +588,8 @@ __global__ void __launch_bounds__(TC_CONV_THREADS, 1) tc_conv_kernel(const __gri
 // ------------------------------------------------------------------ host side ------------------------------
 const char* g_tc_last_kernel = "";       // name of the tensor-core kernel the most recent k_tc_* call dispatched (parity tests assert it)
 bool g_tc_last_slab = false;             // whether the most recent k_tc_fprop / k_tc_dgrad loaded its activations as slabs
-int g_tc_test_bn = 0, g_tc_test_max_ctas = 0, g_tc_test_per_tap = 0;   // test-hook schedule overrides (kernels.h); production code never sets them
+int g_tc_test_bn = 0, g_tc_test_max_ctas = 0, g_tc_test_per_tap = 0, g_tc_test_splits = 0;   // test-hook schedule overrides (kernels.h); production code never sets them
+int g_tc_last_splits = 0;                // split count of the most recent k_tc_wgrad / k_tc_edge_wgrad launch
 static int tc_device() { int dev = 0; cudaGetDevice(&dev); return dev < 0 || dev >= 64 ? 0 : dev; }
 // cudaFuncAttributeMaxDynamicSharedMemorySize is per device: one flag per (kernel, device)
 #define TC_SET_SMEM_ONCE(kernel, bytes)                                                                                            \
@@ -972,7 +973,7 @@ bool tc_edge_wgrad_supported(const ConvGeom& g) { int ht; return edge_tile(g, &h
 static int tc_edge_wgrad_target() { return 2 * device_sm_count(); }
 static int tc_edge_wgrad_ctas(const ConvGeom& g, int* tpc) {
   int ht = 1; edge_tile(g, &ht);
-  const int tiles = g.N * (g.OH / ht), target = tc_edge_wgrad_target();
+  const int tiles = g.N * (g.OH / ht), target = g_tc_test_splits > 0 ? g_tc_test_splits : tc_edge_wgrad_target();
   const int per = (tiles + target - 1) / target; *tpc = per < 1 ? 1 : per;
   return (tiles + *tpc - 1) / *tpc;
 }
@@ -984,7 +985,7 @@ int k_tc_edge_conv(const ConvGeom& g, const __nv_bfloat16* x, const __nv_bfloat1
   p.tiles_total = g.N * p.tiles_y; p.act = act; p.alpha = alpha;
   const size_t smem = 1024 + 24576 + EDGE_SLAB_BYTES;
   TC_SET_SMEM_ONCE(tc_edge_conv_kernel, smem);
-  const int target = 8 * device_sm_count();
+  const int target = g_tc_test_max_ctas > 0 ? g_tc_test_max_ctas : 8 * device_sm_count();
   p.tiles_per_cta = (p.tiles_total + target - 1) / target;
   launch_pdl(tc_edge_conv_kernel, dim3(dim3((unsigned)((p.tiles_total + p.tiles_per_cta - 1) / p.tiles_per_cta), (unsigned)(g.O / 64))), dim3(128), (size_t)(smem), s, p);
   LAUNCHED(); g_tc_last_kernel = "tc_edge_conv_kernel";
@@ -1002,7 +1003,7 @@ int k_tc_edge_wgrad(const ConvGeom& g, const __nv_bfloat16* x, const __nv_bfloat
   const size_t smem = 1024 + 32768 + EDGE_SLAB_BYTES;
   TC_SET_SMEM_ONCE(tc_edge_wgrad_kernel, smem);
   launch_pdl(tc_edge_wgrad_kernel, dim3(dim3((unsigned)ctas)), dim3(128), (size_t)(smem), s, p);
-  LAUNCHED(); g_tc_last_kernel = "tc_edge_wgrad_kernel";
+  LAUNCHED(); g_tc_last_kernel = "tc_edge_wgrad_kernel"; g_tc_last_splits = ctas;
   if (cudaPeekAtLastError() != cudaSuccess) return -3;
   reduce_or_defer(defer, scratch, dw, n, ctas, n, accumulate, s);
   if (p.part_b) reduce_or_defer(defer, p.part_b, db, 64, ctas, 64, accumulate, s);
@@ -1130,7 +1131,7 @@ static int wgrad_splits_for(const ConvGeom& g, int o_tile) {
   long tiles = (long)(g.O / o_tile) * (g.KH * g.KW * g.C / bnw), kbt = (long)g.N * g.OH * g.OW / 64;
   long sp = wgrad_target() / tiles, cap = kbt / 8; if (cap < 1) cap = 1; if (sp > cap) sp = cap; if (sp < 1) sp = 1; return (int)sp;
 }
-static int tc_wgrad_splits(const ConvGeom& g) { return wgrad_splits_for(g, 128); }
+static int tc_wgrad_splits(const ConvGeom& g) { return g_tc_test_splits > 0 ? g_tc_test_splits : wgrad_splits_for(g, 128); }
 bool tc_wgrad_supported(const ConvGeom& g) {
   int a, b, c;
   return g.O % 128 == 0 && wgrad_bnw(g) != 0 && g.SH >= 1 && g.SH <= 2 && g.SW == g.SH && ((long)g.N * g.OH * g.OW) % 64 == 0 &&
@@ -1177,6 +1178,7 @@ int k_tc_wgrad(const ConvGeom& g, const __nv_bfloat16* x, const __nv_bfloat16* d
   dim3 grid((unsigned)splits, (unsigned)(p.taps * g.C / BNW), (unsigned)(g.O / 128));
   const int rc = BNW == 64 ? launch_wgrad<64, 4>(tmDy, tmX, p, grid, s, "tc_wgrad_kernel<64,4>") : launch_wgrad<128, 4>(tmDy, tmX, p, grid, s, "tc_wgrad_kernel<128,4>");
   if (rc) return rc;
+  g_tc_last_splits = splits;
   reduce_or_defer(defer, scratch, dw, n, splits, n, accumulate, s);
   return 0;
 }

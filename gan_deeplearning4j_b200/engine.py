@@ -496,14 +496,18 @@ EPI_PLAIN, EPI_STATS, EPI_BNBWD, EPI_ACTBWD = 0, 1, 2, 3
 def test_conv_ex(ctx: Context, kind: int, geom: Dict[str, int], a, b, out_size: int, *, epi: int = 0, act: str = "identity", alpha: float = 0.0,
                  bias=None, scale=None, groups: int = 1, aux=None, aux2=None, iters: int = 1, impl: int = 1, bn: int = 0, max_ctas: int = 0,
                  poison: bool = False, w_mn: bool = False, per_tap: bool = False, info: Optional[dict] = None, defer: bool = False, db=None,
-                 precision: int = BF16, param_offset: int = 0):
+                 precision: int = BF16, param_offset: int = 0, splits: int = 0):
     """Tensor-core fprop (kind 0) / dgrad (kind 1) with the epilogue the training step uses (impl 3, kind 1: the pixel-shuffle deconv, b = the
     [O][4][4][C] weight).  bn forces the 64- / 128-column tile, max_ctas caps the persistent grid (0: production choice for both); poison
     fills the output with NaN before every launch; w_mn (kind 0, 1x1): b is the [C][O] dense weight; per_tap keeps a 4x4 s2 p1 shape on
     one activation box per tap instead of the slabs two taps share.  info, if given, receives "slab": whether the launch used the slabs, and
-    "splits": the split-K count of a SIMT / skinny-layer / dense kernel.
+    "splits": the split-K count of a SIMT / skinny-layer / dense kernel or of a tensor-core weight gradient.
+    The tensor-core skinny-layer conv (impl 3, kind 0) takes bias and act / alpha, and max_ctas as its CTA target (tiles per CTA =
+    ceil(tiles / max_ctas)).
     Weight gradients (kind 2, impl 1 / 3): defer queues the split-K sum and runs it as the backward pass's one reduce-list launch; db (impl 3,
-    a float32 array of O elements) receives the bias gradient the edge kernel computes beside dw.
+    a float32 array of O elements) receives the bias gradient the edge kernel computes beside dw; splits forces the split count (impl 1:
+    the grid's split dimension, trailing splits may be empty; impl 3: the CTA target, tiles per CTA = ceil(tiles / splits)); poison fills
+    dw, db and the partials with NaN before every launch; param_offset puts dw and db that many elements past an aligned address.
     The SIMT (impl 0), skinny-layer (impl 2) and dense (impl 4) kernels run in either precision with the bias / scale / activation their
     production wrapper takes; param_offset puts their fp32 weight operand (FP32) or weight gradient that many elements past an aligned address.
     Returns (out, stats or None, kernel name, ms)."""
@@ -514,7 +518,7 @@ def test_conv_ex(ctx: Context, kind: int, geom: Dict[str, int], a, b, out_size: 
     o = _lib.TestConvOpts()
     o.epi, o.act, o.alpha, o.groups = epi, ACTS[act], alpha, groups
     o.bn, o.max_ctas, o.poison, o.w_mn, o.per_tap, o.defer = bn, max_ctas, int(poison), int(w_mn), int(per_tap), int(defer)
-    o.param_offset = param_offset
+    o.param_offset, o.splits = param_offset, splits
     if db is not None:
         assert db.dtype == np.float32 and db.flags.c_contiguous
         o.db = _fp(db)

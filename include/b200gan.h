@@ -406,7 +406,7 @@ int32_t b2g_test_conv(b2g_ctx* ctx, int32_t kind, int32_t impl, int32_t precisio
                       const float* x_or_dy, const float* w_or_x, float* out, int32_t iters, float* ms_per_iter);
 /* The same with the epilogue the training step actually uses (impl 1, kind 0 / 1): bias, folded inference-BatchNorm scale, activation,
  * and the fused BatchNorm epilogues of kernels_tc.cu; for the pixel-shuffle deconv (impl 3, kind 1) bias, activation and the
- * activation-backward epilogue.  `kernel` returns the name of the tensor-core kernel that was dispatched, so a parity test can assert
+ * activation-backward epilogue; for the skinny-layer conv forward (impl 3, kind 0) bias and activation.  `kernel` returns the name of the tensor-core kernel that was dispatched, so a parity test can assert
  * that it exercised the variant the benchmark runs.  bn / max_ctas / poison / w_mn let a test pin the tile width and the grid of the
  * persistent kernel, see every element the measured launch left unwritten, and reach the dense input-gradient operand layout. */
 typedef struct {
@@ -422,10 +422,13 @@ typedef struct {
   const float* aux2;      /* epi 2: the BatchNorm input z (same shape) */
   double* stats;          /* out (epi 1 / 2): [groups][2][C_out] */
   char kernel[64];        /* out */
-  /* Schedule controls of the persistent tensor-core conv kernel (impl 1 kind 0 / 1, and impl 3 kind 1 where noted); 0 = production. */
+  /* Schedule controls of the persistent tensor-core conv kernel (impl 1 kind 0 / 1, and impl 3 kind 0 / 1 where noted); 0 = production. */
   int32_t bn;             /* impl 1: force the 64- or 128-column tile (B2G_ERR_UNSUPPORTED unless C_out is a multiple of it) */
-  int32_t max_ctas;       /* impl 1 / impl 3 kind 1: grid = min(work items, max_ctas) instead of min(work items, SMs); may exceed the SM count */
-  int32_t poison;         /* kinds 0 / 1: fill the output with 0xFF bytes (bf16 NaN) before every launch, warm-up included */
+  int32_t max_ctas;       /* impl 1 / impl 3 kind 1: grid = min(work items, max_ctas) instead of min(work items, SMs); may exceed the SM count.
+                             impl 3 kind 0: the CTA target of the skinny-layer conv, tiles_per_cta = ceil(tiles / max_ctas) instead of
+                             ceil(tiles / (8 x SMs)) */
+  int32_t poison;         /* kinds 0 / 1: fill the output with 0xFF bytes (bf16 NaN) before every launch, warm-up included; kind 2 impl 1 / 3:
+                             dw, db and the split-K partials with fp32 NaN */
   int32_t w_mn;           /* impl 1 kind 0, 1x1 geometry: the weight operand is [C][O] (the dense input gradient's own [nOut][nIn] weight) */
   int32_t per_tap;        /* impl 1: load the activations one box per tap also where the 4x4 s2 p1 slab path applies */
   int32_t slab;           /* out: 1 when the launch loaded its activations as slabs shared by two taps */
@@ -438,8 +441,11 @@ typedef struct {
    * applies to them for kinds 0 / 1 / 2 (kind 2: the fp32 dw is filled with 0xFF bytes, fp32 NaN).  `kernel` names the kernel they ran. */
   int32_t param_offset;   /* impl 0 / 2 / 4: the fp32 weight operand (kinds 0 / 1; FP32 only -- the bf16 operand is a 64-element aligned copy) and the
                              fp32 weight gradient (kind 2) start this many elements past a 256-byte aligned address, as a layer's W and dW do in the
-                             flattened parameter and gradient vectors */
-  int32_t splits;         /* out, impl 0 / 2 / 4: the number of split-K partial sums the kernel reduced (1 where it has no split) */
+                             flattened parameter and gradient vectors.  Kind 2 impl 1 / 3: dw and db, in the immediate and the deferred reduction */
+  int32_t splits;         /* out, impl 0 / 2 / 4: the number of split-K partial sums the kernel reduced (1 where it has no split).
+                             in / out, kind 2 impl 1 / 3: in, force the split count (0 = production): tc_wgrad_kernel's grid.x, any value >= 1
+                             (splits past the last K-block are empty), or tc_edge_wgrad_kernel's CTA target (tiles_per_cta = ceil(tiles / splits));
+                             out, the count launched */
 } b2g_test_conv_opts;
 int32_t b2g_test_conv_ex(b2g_ctx* ctx, int32_t kind, int32_t impl, int32_t precision, const b2g_conv_geom* g,
                          const float* x_or_dy, const float* w_or_x, float* out, int32_t iters, float* ms_per_iter, b2g_test_conv_opts* opts);

@@ -341,31 +341,7 @@ def test_tc_dgrad_phase_form_matches_oracle(b200, case):
     assert rel_err(out.reshape(n, h, w, c), dx.transpose(0, 2, 3, 1)) < 1e-2
 
 
-TC_WGRAD_CASES = [
-    # n, h, w, c, o, k, s, p
-    (4, 16, 16, 64, 128, 4, 2, 1),     # 8x8 dy grid: one image per 64-pixel K-block, BNW=128
-    (2, 32, 32, 128, 128, 4, 2, 1),    # 16x16 grid: 4 rows per K-block, BNW=128
-    (16, 8, 8, 256, 256, 4, 2, 1),     # 4x4 grid: four images per K-block, BNW=128, two o-tiles
-    (4, 16, 16, 64, 128, 3, 1, 1),     # 3x3 s1: 9*64 = 576 columns are not a multiple of 128 -> BNW=64
-]
-
-
-@pytest.mark.parametrize("case", TC_WGRAD_CASES)
-def test_tc_wgrad_mn_major_matches_oracle(b200, case):
-    b, ctx = b200
-    n, h, w, c, oc, k, s, p = case
-    rng = np.random.default_rng(4)
-    x, wt, y, dy, dx, dw = _conv_ref(n, h, w, c, oc, k, s, p, rng, bf16_round)
-    oh, ow = y.shape[2], y.shape[3]
-    geom = dict(n=n, h=h, w=w, c=c, oh=oh, ow=ow, o=oc, kh=k, kw=k, sh=s, sw=s, ph=p, pw=p)
-    opts = b._lib.TestConvOpts()
-    import ctypes as C
-    out = np.empty(dw.size, np.float32); ms = C.c_float()
-    fp = lambda a: a.ctypes.data_as(C.POINTER(C.c_float))
-    xa, da = np.ascontiguousarray(x.transpose(0, 2, 3, 1).ravel(), np.float32), np.ascontiguousarray(dy.transpose(0, 2, 3, 1).ravel(), np.float32)
-    b.engine.check(ctx.lib.b2g_test_conv_ex(ctx.h, 2, 1, b.BF16, C.byref(b._lib.ConvGeom(**geom)), fp(xa), fp(da), fp(out), 1, C.byref(ms), C.byref(opts)))
-    assert rel_err(out.reshape(oc, k, k, c), dw.transpose(0, 2, 3, 1)) < 1e-4     # fp32 accumulate, fp32 out: only summation order differs
-    assert opts.kernel.decode() == ("tc_wgrad_kernel<64,4>" if (k * k * c) % 128 else "tc_wgrad_kernel<128,4>")
+# the tensor-core weight gradients are checked at every split schedule, bit for bit on integer operands, in tests/test_gpu_tc_wgrad.py
 
 
 TC_EDGE_CASES = [
