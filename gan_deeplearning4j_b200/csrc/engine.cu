@@ -209,7 +209,7 @@ static int32_t take_loss(LayerRT& l) {
 // Layers whose activation is b2g_layer_desc.act: checks the code, and moves a code of 5-16 into ext_act / ext_alpha (d.act becomes identity).
 static int32_t take_act(LayerRT& l) {
   b2g_layer_desc& d = l.d;
-  const bool lossy = d.type == B2G_LAYER_OUTPUT || d.type == B2G_LAYER_LOSS;
+  const bool lossy = d.type == B2G_LAYER_OUTPUT || d.type == B2G_LAYER_LOSS || d.type == B2G_LAYER_CNN_LOSS;
   const bool has_act = d.type == B2G_LAYER_CONV2D || d.type == B2G_LAYER_DECONV2D || d.type == B2G_LAYER_DENSE || d.type == B2G_LAYER_ACTIVATION ||
                        (lossy && d.loss >= B2G_LOSS_MSE && d.loss <= B2G_LOSS_WASSERSTEIN);
   if (!has_act) return 0;
@@ -311,6 +311,8 @@ static int32_t net_build(b2g_net* n, const b2g_layer_desc* layers, int32_t nl) {
         if (d.loss == B2G_LOSS_XENT && (size_t)h * w * ch != 1) return fail(B2G_ERR_UNSUPPORTED, "layer %s: XENT loss needs one logit per example", d.name);
         if ((h != 1 || w != 1) && (size_t)h * w * ch != 1) return fail(B2G_ERR_UNSUPPORTED, "layer %s: a loss on a %dx%d map is not supported (feed-forward input or one element per example)", d.name, h, w);
         break;
+      case B2G_LAYER_CNN_LOSS:       // CnnLossLayer: the rows are the N*H*W pixels, the columns the C channels (NHWC: the buffer as it is)
+        l.oh = h; l.ow = w; l.oc = ch; B2(take_loss(l)); break;
       case B2G_LAYER_FF_TO_CNN:
         if ((size_t)d.pre_h * d.pre_w * d.pre_c != l.in_elems) return fail(B2G_ERR_SHAPE, "layer %s: FeedForwardToCnn(%d,%d,%d) != %zu features", d.name, d.pre_h, d.pre_w, d.pre_c, l.in_elems);
         l.oh = d.pre_h; l.ow = d.pre_w; l.oc = d.pre_c; break;
@@ -354,20 +356,22 @@ static int32_t net_alloc(b2g_net* n) {
   B2(dalloc(n, &n->labels_dev, sizeof(float) * R * std::max<size_t>(1, n->L.back().out_elems)));
   {  // k_loss's per-block sums for one group of max_batch rows (fit) or two of max_batch / 2 (the GAN step's D pass)
     const size_t per = n->L.back().out_elems;
-    B2(dalloc(n, &n->loss_partial, sizeof(double) * std::max(k_loss_blocks((size_t)R * per, 1), 2 * k_loss_blocks((size_t)(R / 2) * per, 2))));
+    // CnnLossLayer: every slicing of kernels_cnnloss.cu and loss_kernel stays within LOSS_MAX_GRID = 1024 blocks
+    const int cnn = n->L.back().d.type == B2G_LAYER_CNN_LOSS ? 1024 : 0;
+    B2(dalloc(n, &n->loss_partial, sizeof(double) * std::max(cnn, std::max(k_loss_blocks((size_t)R * per, 1), 2 * k_loss_blocks((size_t)(R / 2) * per, 2)))));
   }
   B2(dalloc(n, &n->loss_ticket, sizeof(unsigned))); CU(cudaMemsetAsync(n->loss_ticket, 0, sizeof(unsigned), n->ctx->stream));
   B2(dalloc(n, (char**)&n->input, ts * R * n->in_elems));
   size_t max_act = n->in_elems, scratch = 1 << 16, max_w = 0, bn_acc_words = 0;
   for (auto& l : n->L) {
     max_act = std::max(max_act, std::max(l.in_elems, l.out_elems));
-    bool alias = l.act_fused_into_prev || l.d.type == B2G_LAYER_LOSS ||
+    bool alias = l.act_fused_into_prev || l.d.type == B2G_LAYER_LOSS || l.d.type == B2G_LAYER_CNN_LOSS ||
                  (l.d.type == B2G_LAYER_FF_TO_CNN && (l.oc == 1 || l.oh * l.ow == 1)) ||
                  (l.d.type == B2G_LAYER_CNN_TO_FF && (l.ic == 1 || l.ih * l.iw == 1));
     l.out_alias = alias;
     if (!alias) B2(dalloc(n, (char**)&l.out, ts * R * l.out_elems));
     if (l.d.type == B2G_LAYER_DROPOUT) { l.drop_buf = l.out; B2(dalloc(n, &l.drop_mask, sizeof(uint32_t) * (((size_t)R * l.out_elems + 31) / 32))); }
-    if (l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS) B2(dalloc(n, (char**)&l.probs, ts * R * l.out_elems));
+    if (l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS || l.d.type == B2G_LAYER_CNN_LOSS) B2(dalloc(n, (char**)&l.probs, ts * R * l.out_elems));
     if (l.ext_act && l.has_gemm() && l.d.type != B2G_LAYER_OUTPUT) B2(dalloc(n, (char**)&l.ext_z, ts * R * l.out_elems));
     if (l.d.type == B2G_LAYER_MAXPOOL) B2(dalloc(n, &l.argmax, (size_t)R * l.out_elems));
     if (l.d.type == B2G_LAYER_GLOBAL_POOLING) {
@@ -390,7 +394,7 @@ static int32_t net_alloc(b2g_net* n) {
       max_w = std::max(max_w, (size_t)l.n_W);
       // split-K partials of the tensor-core weight gradients stay in a per-layer region until the pass's single k_reduce_multi launch
       if (n->prec == PREC_BF16 && n->ctx->tc_ok && !l.d.frozen) {
-        l.wg_part_floats = std::max(k_tc_wgrad_scratch_floats(g), k_tc_edge_wgrad_scratch_floats(g));
+        l.wg_part_floats = std::max(std::max(k_tc_wgrad_scratch_floats(g), k_tc_edge_wgrad_scratch_floats(g)), k_head_wgrad_scratch_floats(g));
         if (l.wg_part_floats) B2(dalloc(n, &l.wg_part, sizeof(float) * l.wg_part_floats));
       }
     }
@@ -552,6 +556,7 @@ static int32_t gemm_fprop(b2g_net* n, const LayerRT& l, const ConvGeom& g, const
     if (k_tc_fprop(g, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)out, act, alpha, s) == 0) return 0;
     return fail(B2G_ERR_CUDA, "tensor-core fprop launch failed");
   }
+  if (n->prec == PREC_BF16 && head_conv_supported(g)) { k_head_fwd(g, (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)out, act, alpha, s); return 0; }
   note_simt(n); k_simt_fprop(n->prec, wp, g, x, w, bias, out, act, alpha, s); return 0;
 }
 static int32_t gemm_dgrad(b2g_net* n, const LayerRT& l, const ConvGeom& g, const void* dy, const float* bias, void* dx, int act, float alpha,
@@ -584,6 +589,7 @@ static int32_t gemm_dgrad(b2g_net* n, const LayerRT& l, const ConvGeom& g, const
     if (k_tc_dgrad(g, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)dx, act, alpha, s) == 0) return 0;
     return fail(B2G_ERR_CUDA, "tensor-core dgrad launch failed");
   }
+  if (n->prec == PREC_BF16 && head_conv_supported(g)) { k_head_dgrad(g, (const __nv_bfloat16*)dy, (const __nv_bfloat16*)w, bias, (__nv_bfloat16*)dx, act, alpha, s); return 0; }
   note_simt(n); k_simt_dgrad(n->prec, wp, g, dy, w, bias, dx, act, alpha, s); return 0;
 }
 static int32_t gemm_wgrad(b2g_net* n, LayerRT& l, const ConvGeom& g, const void* x, const void* dy, float* dw, cudaStream_t s, float* scratch, float* db = nullptr, bool* bias_done = nullptr) {
@@ -594,6 +600,10 @@ static int32_t gemm_wgrad(b2g_net* n, LayerRT& l, const ConvGeom& g, const void*
   if (tc_on(n) && tc_wgrad_supported(g) && l.wg_part) {
     if (k_tc_wgrad(g, (const __nv_bfloat16*)x, (const __nv_bfloat16*)dy, dw, l.wg_part, l.wg_part_floats, 0, s, &n->pending) == 0) return 0;
     return fail(B2G_ERR_CUDA, "tensor-core wgrad launch failed");
+  }
+  if (n->prec == PREC_BF16 && head_conv_supported(g) && l.wg_part) {
+    if (k_head_wgrad(g, (const __nv_bfloat16*)x, (const __nv_bfloat16*)dy, dw, l.wg_part, l.wg_part_floats, 0, s, &n->pending) == 0) return 0;
+    return fail(B2G_ERR_CUDA, "few-output conv weight gradient: partials larger than the layer's region");
   }
   note_simt(n); k_simt_wgrad(n->prec, g, x, dy, dw, scratch, n->scratch_floats, 0, s); return 0;
 }
@@ -674,7 +684,7 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
       case B2G_LAYER_SUBSAMPLING: k_pool2d_fwd(n->prec, l.pool, l.pnorm, cur, out, R, l.ih, l.iw, l.ic, l.oh, l.ow, d.k_h, d.k_w, d.s_h, d.s_w, d.p_h, d.p_w, s); break;
       case B2G_LAYER_GLOBAL_POOLING: k_global_pool_fwd(n->prec, l.pool, l.pnorm, cur, out, l.pool_idx, R, l.ih * l.iw, l.ic, l.pool_part, l.pool_part_idx, l.pool_ticket, s); break;
       case B2G_LAYER_UPSAMPLE2D: k_upsample_fwd(n->prec, cur, out, R, l.ih, l.iw, l.ic, d.k_h, s); break;
-      case B2G_LAYER_LOSS: out = (void*)cur; break;
+      case B2G_LAYER_LOSS: case B2G_LAYER_CNN_LOSS: out = (void*)cur; break;
       case B2G_LAYER_FF_TO_CNN: if (l.out_alias) out = (void*)cur; else k_permute(n->prec, cur, out, R, l.oc, l.oh * l.ow, 1, s); break;
       case B2G_LAYER_CNN_TO_FF: if (l.out_alias) out = (void*)cur; else k_permute(n->prec, cur, out, R, l.ic, l.ih * l.iw, 0, s); break;
       case B2G_LAYER_DROPOUT:
@@ -765,7 +775,7 @@ static int32_t net_backward(b2g_net* n, const void* net_in, void* eps, int rows,
     if (!need_in) for (int j = 0; j < i; ++j) if (!n->L[j].d.frozen && (n->L[j].has_gemm() || n->L[j].d.type == B2G_LAYER_BATCHNORM)) need_in = true;
     const bool want_wgrad_l = want_wgrad && !d.frozen;
     switch (d.type) {
-      case B2G_LAYER_LOSS: break;
+      case B2G_LAYER_LOSS: case B2G_LAYER_CNN_LOSS: break;
       case B2G_LAYER_CONV2D: case B2G_LAYER_DENSE: case B2G_LAYER_OUTPUT: {
         ConvGeom g = l.geom; g.N = R;
         if (d.act != B2G_ACT_IDENTITY && !act_done[i]) k_act_bwd_from_output(n->prec, l.out, cur, cur, (size_t)R * l.out_elems, d.act, d.act_alpha, s);
@@ -1064,7 +1074,15 @@ extern "C" int32_t b2g_net_output(b2g_net* n, const float* x, int32_t batch, int
   const void* res = nullptr; FwdOpts o{batch, 1, train != 0, false, nullptr};
   B2(net_forward(n, n->input, o, &res));
   LayerRT& l = n->L.back();
-  if (l.d.type == B2G_LAYER_OUTPUT && l.d.loss == B2G_LOSS_MCXENT) { k_softmax_xent(n->prec, res, nullptr, nullptr, l.probs, nullptr, batch, l.oc, n->ctx->stream); res = l.probs; }
+  if (l.d.type == B2G_LAYER_CNN_LOSS && l.d.loss == B2G_LOSS_MCXENT) {      // the per-pixel softmax
+    k_cnn_softmax_xent(n->prec, res, nullptr, nullptr, l.probs, nullptr, batch * l.oh * l.ow, l.oc, 1, nullptr, nullptr, n->ctx->stream); res = l.probs;
+  }
+  else if (l.d.type == B2G_LAYER_CNN_LOSS && l.d.loss == B2G_LOSS_XENT) { k_sigmoid_out(n->prec, res, l.probs, (size_t)batch * l.out_elems, n->ctx->stream); res = l.probs; }
+  else if (l.d.type == B2G_LAYER_CNN_LOSS) {      // a = act(z), as on a LOSS layer
+    if (l.ext_act) { k_act_ext_fwd(n->prec, l.ext_act, l.ext_alpha, res, l.probs, (size_t)batch * l.out_elems, n->ctx->stream); res = l.probs; }
+    else if (l.loss_act != ACT_IDENTITY) { k_act_fwd(n->prec, res, l.probs, (size_t)batch * l.out_elems, l.loss_act, l.loss_alpha, n->ctx->stream); res = l.probs; }
+  }
+  else if (l.d.type == B2G_LAYER_OUTPUT && l.d.loss == B2G_LOSS_MCXENT) { k_softmax_xent(n->prec, res, nullptr, nullptr, l.probs, nullptr, batch, l.oc, n->ctx->stream); res = l.probs; }
   else if ((l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS) && l.d.loss >= B2G_LOSS_MSE) {      // a = act(z); identity: the logits themselves
     if (l.ext_act) { k_act_ext_fwd(n->prec, l.ext_act, l.ext_alpha, res, l.probs, (size_t)batch * l.out_elems, n->ctx->stream); res = l.probs; }
     else if (l.loss_act != ACT_IDENTITY) { k_act_fwd(n->prec, res, l.probs, (size_t)batch * l.out_elems, l.loss_act, l.loss_alpha, n->ctx->stream); res = l.probs; }
@@ -1083,6 +1101,19 @@ extern "C" int32_t b2g_net_get_activation(b2g_net* n, int32_t layer, int32_t bat
 // OUTPUT or LOSS layer runs XENT.
 static void net_loss(b2g_net* n, const void* logits, const float* labels, void* dz, float* loss_sums, int rows_per_group, int groups) {
   const LayerRT& l = n->L.back();
+  if (l.d.type == B2G_LAYER_CNN_LOSS) {      // rows = the group's pixels, columns = the channels
+    const int px = rows_per_group * l.oh * l.ow; cudaStream_t s = n->ctx->stream;
+    if (l.d.loss == B2G_LOSS_XENT) k_cnn_xent(n->prec, logits, labels, dz, loss_sums, (size_t)rows_per_group * l.out_elems, groups, n->cfg.xent_clip_eps, n->loss_partial, n->loss_ticket, s);
+    else if (l.d.loss == B2G_LOSS_MCXENT) k_cnn_softmax_xent(n->prec, logits, labels, dz, nullptr, loss_sums, px, l.oc, groups, n->loss_partial, n->loss_ticket, s);
+    else if (l.ext_act) {
+      const size_t cnt = (size_t)rows_per_group * groups * l.out_elems;
+      k_act_ext_fwd(n->prec, l.ext_act, l.ext_alpha, logits, l.probs, cnt, s);
+      k_loss(n->prec, l.d.loss, ACT_IDENTITY, 0.f, l.probs, labels, dz, loss_sums, px, l.oc, groups, n->loss_partial, n->loss_ticket, s);
+      k_act_ext_bwd(n->prec, l.ext_act, l.ext_alpha, logits, dz, cnt, s);
+    }
+    else k_loss(n->prec, l.d.loss, l.loss_act, l.loss_alpha, logits, labels, dz, loss_sums, px, l.oc, groups, n->loss_partial, n->loss_ticket, s);
+    return;
+  }
   const int loss = (l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS) ? l.d.loss : B2G_LOSS_XENT;
   if (loss == B2G_LOSS_MCXENT) k_softmax_xent(n->prec, logits, labels, dz, nullptr, loss_sums, rows_per_group * groups, l.oc, n->ctx->stream);
   else if (loss == B2G_LOSS_XENT) k_xent(n->prec, logits, labels, dz, loss_sums, rows_per_group, groups, n->cfg.xent_clip_eps, n->ctx->stream);
@@ -1094,13 +1125,26 @@ static void net_loss(b2g_net* n, const void* logits, const float* labels, void* 
   }
   else k_loss(n->prec, loss, l.loss_act, l.loss_alpha, logits, labels, dz, loss_sums, rows_per_group, (int)l.out_elems, groups, n->loss_partial, n->loss_ticket, n->ctx->stream);
 }
+// host labels [batch][out_elems] -> dst on s.  A CnnLossLayer's labels are NCHW: permuted to the engine's NHWC through `stage` when C > 1 and
+// the map is wider than one pixel (otherwise the two orders coincide).
+static int32_t upload_labels(b2g_net* n, const float* y, int batch, float* dst, float* stage, cudaStream_t s) {
+  const LayerRT& l = n->L.back(); const size_t cnt = (size_t)batch * l.out_elems;
+  if (l.d.type == B2G_LAYER_CNN_LOSS && l.oc > 1 && l.oh * l.ow > 1) {
+    if (cnt > n->stage_floats) return fail(B2G_ERR_SHAPE, "labels larger than staging");
+    CU(cudaMemcpyAsync(stage, y, sizeof(float) * cnt, cudaMemcpyHostToDevice, s));
+    k_nchw_f32_to_nhwc(PREC_F32, stage, dst, batch, l.oc, l.oh * l.ow, s);
+    return 0;
+  }
+  CU(cudaMemcpyAsync(dst, y, sizeof(float) * cnt, cudaMemcpyHostToDevice, s));
+  return 0;
+}
 static int32_t train_pass(b2g_net* n, const float* x, const float* y, int batch, bool do_update, float* score) {
   cudaStream_t s = n->ctx->stream;
   if (batch < 1 || batch > n->max_rows) return fail(B2G_ERR_SHAPE, "batch %d outside [1,%d]", batch, n->max_rows);
   int lt = n->L.back().d.type;
-  if (lt != B2G_LAYER_OUTPUT && lt != B2G_LAYER_LOSS) return fail(B2G_ERR_UNSUPPORTED, "fit needs a net ending in OutputLayer/LossLayer");
+  if (lt != B2G_LAYER_OUTPUT && lt != B2G_LAYER_LOSS && lt != B2G_LAYER_CNN_LOSS) return fail(B2G_ERR_UNSUPPORTED, "fit needs a net ending in OutputLayer/LossLayer/CnnLossLayer");
   B2(upload_input(n, x, batch, n->input));
-  CU(cudaMemcpyAsync(n->labels_dev, y, sizeof(float) * batch * n->L.back().out_elems, cudaMemcpyHostToDevice, s));
+  B2(upload_labels(n, y, batch, n->labels_dev, n->stage_f32, s));
   CU(cudaMemsetAsync(n->grads, 0, sizeof(float) * n->n_params, s));
   const void* logits = nullptr; FwdOpts o{batch, 1, true, true, nullptr};
   B2(net_forward(n, n->input, o, &logits));
@@ -1132,7 +1176,7 @@ struct b2g_gan {
   b2g_net *G = nullptr, *D = nullptr; b2g_gan_config cfg{};
   int N = 0;                              // per-step batch (D sees 2N)
   void *z_d = nullptr, *z_g = nullptr;    // T [N][z]
-  float *y_d = nullptr, *y_g = nullptr;   // [2N] = y_real | y_fake ; [N]
+  float *y_d = nullptr, *y_g = nullptr;   // [2N][oe] = y_real | y_fake ; [N][oe]  (oe = the discriminator's outputs per example, NHWC)
   float* loss_dev = nullptr;              // [4]: d_real_sum, d_fake_sum, g_sum
   float* stage = nullptr; size_t stage_floats = 0;
   cudaGraph_t graph = nullptr, graph1 = nullptr; cudaGraphExec_t exec = nullptr, exec1 = nullptr; int graph_batch = 0; uint64_t graph_launches = 0, graph_simt_g = 0, graph_simt_d = 0;
@@ -1205,6 +1249,8 @@ extern "C" int32_t b2g_gan_create(b2g_net* gen, b2g_net* dis, const b2g_gan_conf
   {  // one output per example; XENT or a loss of codes 2-8 (the labels the caller uploads choose the objective)
     const LayerRT& dl = dis->L.back();
     const bool lossy = dl.d.type == B2G_LAYER_OUTPUT || dl.d.type == B2G_LAYER_LOSS;
+    if (dl.d.type == B2G_LAYER_CNN_LOSS && dl.d.loss == B2G_LOSS_MCXENT)
+      return fail(B2G_ERR_UNSUPPORTED, "the adversarial step needs a CnnLossLayer discriminator with XENT or a loss of codes 2-8 (not MCXENT: one label per patch)");
     if (lossy && dl.d.loss == B2G_LOSS_MCXENT) return fail(B2G_ERR_UNSUPPORTED, "the adversarial step needs a discriminator with one output per example (not MCXENT)");
     if (lossy && dl.out_elems != 1) return fail(B2G_ERR_UNSUPPORTED, "the adversarial step needs a discriminator with one output per example, not %zu", dl.out_elems);
   }
@@ -1215,7 +1261,8 @@ extern "C" int32_t b2g_gan_create(b2g_net* gen, b2g_net* dis, const b2g_gan_conf
   const size_t ts = prec_size(gen->prec);
   auto al = [&](void** p, size_t bytes) -> int32_t { cudaError_t e = cudaMalloc(p, bytes ? bytes : 16); if (e != cudaSuccess) return fail(B2G_ERR_OOM, "cudaMalloc: %s", cudaGetErrorString(e)); g->allocs.push_back(*p); return 0; };
   int32_t r = al(&g->z_d, ts * N * gen->in_elems); if (!r) r = al(&g->z_g, ts * N * gen->in_elems);
-  if (!r) r = al((void**)&g->y_d, sizeof(float) * 2 * N); if (!r) r = al((void**)&g->y_g, sizeof(float) * N); if (!r) r = al((void**)&g->loss_dev, sizeof(float) * 4);
+  const size_t oe = dis->L.back().out_elems;      // labels per example: 1, or a CnnLossLayer discriminator's patch map
+  if (!r) r = al((void**)&g->y_d, sizeof(float) * 2 * N * oe); if (!r) r = al((void**)&g->y_g, sizeof(float) * N * oe); if (!r) r = al((void**)&g->loss_dev, sizeof(float) * 4);
   g->stage_floats = (size_t)N * std::max(dis->in_elems, gen->in_elems); if (!r) r = al((void**)&g->stage, sizeof(float) * g->stage_floats);
   if (!r) { if (cudaEventCreate(&g->ev0) != cudaSuccess || cudaEventCreate(&g->ev1) != cudaSuccess || cudaEventCreateWithFlags(&g->ev_x, cudaEventDisableTiming) != cudaSuccess ||
                 cudaStreamCreateWithFlags(&g->copy_stream, cudaStreamNonBlocking) != cudaSuccess) r = fail(B2G_ERR_CUDA, "cudaEventCreate failed"); }
@@ -1243,9 +1290,11 @@ extern "C" int32_t b2g_gan_upload(b2g_gan* g, const float* x_real, const float* 
   k_nchw_f32_to_nhwc(G->prec, G->stage_f32, g->z_d, batch, G->cfg.in_c, G->cfg.in_h * G->cfg.in_w, s);
   CU(cudaMemcpyAsync(D->stage_f32, z_g, sizeof(float) * nz, cudaMemcpyHostToDevice, s));
   k_nchw_f32_to_nhwc(G->prec, D->stage_f32, g->z_g, batch, G->cfg.in_c, G->cfg.in_h * G->cfg.in_w, s);
-  CU(cudaMemcpyAsync(g->y_d, y_real, sizeof(float) * batch, cudaMemcpyHostToDevice, s));
-  CU(cudaMemcpyAsync(g->y_d + batch, y_fake, sizeof(float) * batch, cudaMemcpyHostToDevice, s));
-  CU(cudaMemcpyAsync(g->y_g, y_gen, sizeof(float) * batch, cudaMemcpyHostToDevice, s));
+  // [batch][oe] each (NCHW for a CnnLossLayer; D's staging buffer is free again once z_g's conversion above has run on s)
+  const size_t oe = D->L.back().out_elems;
+  B2(upload_labels(D, y_real, batch, g->y_d, D->stage_f32, s));
+  B2(upload_labels(D, y_fake, batch, g->y_d + (size_t)batch * oe, D->stage_f32, s));
+  B2(upload_labels(D, y_gen, batch, g->y_g, D->stage_f32, s));
   CHECK_KERNELS();
   return 0;
 }
@@ -1529,7 +1578,9 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   const bool edge_fwd = impl == 3 && kind == 0, tc_wg = kind == 2 && (impl == 1 || impl == 3);   // tc_edge_conv_kernel; the tensor-core weight gradients
   // the SIMT, skinny-layer and dense kernels; gemm_epi: those whose production wrapper takes bias / activation (k_dense_small_o_dgrad and the
   // weight gradients have none: as in gemm_dgrad, a dense input gradient with an epilogue runs the short-reduction kernel)
-  const bool gemm = impl == 0 || impl == 2 || impl == 4;
+  const bool gemm = impl == 0 || impl == 2 || impl == 4 || impl == 5;
+  // impl 5 = the few-output conv kernels (kernels_head.cu), BF16 only
+  if (impl == 5 && (prec != PREC_BF16 || !head_conv_supported(g))) return fail(B2G_ERR_UNSUPPORTED, "no few-output conv kernel (impl 5: BF16, O <= 4, C %% 8 == 0, k x k) for this shape");
   const bool gemm_epi = gemm && kind != 2 && !(impl == 4 && kind == 1 && !dense_small_k_supported(g));
   if (opt && gemm) {
     if (opt->epi || (!gemm_epi && (opt->bias || opt->scale || opt->act)))
@@ -1552,11 +1603,12 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   if (max_ctas < 0 || (max_ctas && !tc_conv && !ps && !edge_fwd))
     return fail(B2G_ERR_UNSUPPORTED, "max_ctas %d: a grid cap applies to tc_conv_kernel and tc_edge_conv_kernel launches only", max_ctas);
   const int force_splits = opt ? opt->splits : 0;
-  if (force_splits < 0 || (force_splits && !tc_wg)) return fail(B2G_ERR_UNSUPPORTED, "splits %d: a forced split count applies to the tensor-core weight gradients (kind 2, impl 1 / 3)", force_splits);
+  const bool head_wg = impl == 5 && kind == 2;
+  if (force_splits < 0 || (force_splits && !tc_wg && !head_wg)) return fail(B2G_ERR_UNSUPPORTED, "splits %d: a forced split count applies to the tensor-core weight gradients (kind 2, impl 1 / 3)", force_splits);
   if (w_mn && (impl != 1 || kind != 0 || g.KH != 1 || g.KW != 1)) return fail(B2G_ERR_UNSUPPORTED, "w_mn: the [C][O] weight operand exists for the 1x1 tensor-core fprop only");
   const bool defer = opt && opt->defer; float* db_host = opt ? opt->db : nullptr;
   if (defer && !(kind == 2 && (impl == 1 || impl == 3))) return fail(B2G_ERR_UNSUPPORTED, "defer applies to the tensor-core weight gradients (kind 2, impl 1 / 3)");
-  if (db_host && !(kind == 2 && impl == 3)) return fail(B2G_ERR_UNSUPPORTED, "db is the edge tensor-core weight gradient's bias column (kind 2, impl 3)");
+  if (db_host && !(kind == 2 && (impl == 3 || impl == 5))) return fail(B2G_ERR_UNSUPPORTED, "db is the edge tensor-core weight gradient's bias column (kind 2, impl 3)");
   // impl 2 = the SIMT skinny-layer kernels (kernels_edge.cu), impl 3 = their tensor-core counterparts; both need <= 4 image channels (g.C)
   if (impl == 2 || impl == 3) {
     bool ok = kind == 0 ? edge_conv_small_cin_supported(g) : kind == 1 ? edge_deconv_small_c_supported(g) : edge_wgrad_small_cin_supported(g);
@@ -1571,7 +1623,8 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   float *d_bias = nullptr, *d_scale = nullptr, *d_coef = nullptr, *d_auxf = nullptr; __nv_bfloat16 *d_aux = nullptr, *d_aux2 = nullptr; unsigned long long* d_acc = nullptr;
   size_t sc = std::max(std::max(std::max(k_simt_wgrad_scratch_floats(g), k_tc_wgrad_scratch_floats(g)), std::max(k_edge_wgrad_scratch_floats(g), k_tc_edge_wgrad_scratch_floats(g))), k_dense_small_o_wgrad_scratch_floats(g)) + 16;
   // a forced split count needs room for that many partials: [splits][dw] (tc_wgrad_kernel), [ctas][dw] + [ctas][db] with ctas <= splits (tc_edge_wgrad_kernel)
-  if (force_splits) sc = std::max(sc, (size_t)force_splits * (impl == 1 ? nw : (size_t)64 * 16 * g.C + 64) + 16);
+  if (force_splits) sc = std::max(sc, (size_t)force_splits * (impl == 1 || impl == 5 ? nw : (size_t)64 * 16 * g.C + 64) + 16);
+  if (impl == 5) sc = std::max(sc, std::max(k_head_wgrad_scratch_floats(g), k_colsum_scratch_floats(g.O)) + 16);
   // param_offset: the fp32 weight operand (FP32, kinds 0 / 1) and the weight gradient (kind 2) start poff elements past the 256-byte aligned
   // cudaMalloc base, as W and dW do in a net's flattened parameter / gradient vectors
   const size_t woff = (prec == PREC_F32 && kind != 2) ? (size_t)poff : 0, dwoff = kind == 2 ? (size_t)poff : 0;
@@ -1618,7 +1671,17 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
     if (poison) CU(cudaMemsetAsync(to, 0xFF, ts * no, s));       // a tile this launch does not write reads back as NaN, not as the warm-up's values
     if (poison && kind == 2) { CU(cudaMemsetAsync(fres, 0xFF, 4 * no, s)); CU(cudaMemsetAsync(scratch, 0xFF, 4 * sc, s)); }   // fp32 NaN: dw and the split-K partials
     if (poison && dbres) CU(cudaMemsetAsync(dbres, 0xFF, 4 * (size_t)g.O, s));
-    if (impl == 4) {
+    if (impl == 5) {      // the weight gradient's split sums as the backward pass runs them: one reduce-list launch; db = the column sums of dy
+      if (kind == 0) k_head_fwd(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s);
+      else if (kind == 1) k_head_dgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s);
+      else {
+        ReduceList hl{};
+        if (k_head_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fres, scratch, sc, force_splits, s, &hl)) { rc = -5; break; }
+        const int hs = g_gemm_last_splits; k_reduce_multi(hl, s); g_gemm_last_splits = hs;
+        if (dbres) { k_colsum(PREC_BF16, tb, g.N * g.OH * g.OW, g.O, scratch, dbres, 0, s); db_written = 1; }
+      }
+    }
+    else if (impl == 4) {
       const bool so = dense_small_o_supported(g);
       if (kind == 0) k_dense_small_o_fwd(prec, prec, g, ta, tb, bias, to, act, alpha, s);
       else if (kind == 1) { if (so && !bias && !act) k_dense_small_o_dgrad(prec, prec, g, ta, tb, to, s); else k_dense_small_k_dgrad(prec, prec, g, ta, tb, bias, to, act, alpha, s); }
@@ -1644,6 +1707,7 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
   schedule.reset();
   CU(cudaEventRecord(e1, s));
   if (rc == -4) return fail(B2G_ERR_CUDA, "defer: the weight gradient queued no reduction");
+  if (rc == -5) return fail(B2G_ERR_ARG, "splits %d: the partials do not fit the scratch", force_splits);
   if (rc) return fail(B2G_ERR_CUDA, "tensor-core kernel launch failed (%d)", rc);
   if (opt) {
     strncpy(opt->kernel, gemm ? g_gemm_last_kernel : g_tc_last_kernel, sizeof(opt->kernel) - 1); opt->kernel[sizeof(opt->kernel) - 1] = 0; opt->slab = g_tc_last_slab;
@@ -1884,6 +1948,23 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
       B2(poison(dz, ts * n)); B2(poison(loss, 4 * (size_t)o->groups));
       k_loss(prec, o->loss, o->act, o->alpha, z, y, dz, loss, o->rows, o->cols, o->groups, partial, ticket, s); ran();
       B2(downT(out0, dz, n)); B2(downF(out1, loss, (size_t)o->groups));
+      break;
+    }
+    case B2G_EW_CNN_XENT: case B2G_EW_CNN_SOFTMAX_XENT: {
+      const bool sm = o->op == B2G_EW_CNN_SOFTMAX_XENT;
+      const size_t per = (size_t)o->rows * o->cols, n = per * o->groups;
+      if (!in0 || (!in1 && !sm) || o->rows < 1 || o->cols < 1 || o->groups < 1 || (int64_t)n > lim) return fail(B2G_ERR_ARG, "bad CNN loss arguments");
+      const int bpg = sm ? k_cnn_softmax_blocks(o->rows, o->groups) : k_loss_blocks(per, o->groups);
+      void *z = nullptr, *dz = nullptr, *p = nullptr; float *y = nullptr, *loss = nullptr; double* partial = nullptr; unsigned* ticket = nullptr;
+      B2(upT(in0, n, &z)); if (in1) B2(upF(in1, n, &y)); B2(dev(n, ts, &dz)); B2(dev(n, ts, &p)); B2(upF(nullptr, (size_t)o->groups, &loss));
+      B2(dev((size_t)o->groups * bpg, 8, (void**)&partial)); B2(dev(1, 4, (void**)&ticket)); CU(cudaMemsetAsync(ticket, 0, 4, s));
+      B2(poison(dz, ts * n)); B2(poison(p, ts * n)); B2(poison(loss, 4 * (size_t)o->groups));
+      if (sm) k_cnn_softmax_xent(prec, z, y, y ? dz : nullptr, p, y ? loss : nullptr, o->rows, o->cols, o->groups, partial, ticket, s);     // no labels: the inference call
+      else k_cnn_xent(prec, z, y, dz, loss, per, o->groups, o->clip_eps, partial, ticket, s);
+      ran();
+      B2(downT(out0, dz, n)); B2(downF(out1, loss, (size_t)o->groups)); if (sm) B2(downT(out2, p, n));
+      unsigned t = 1; CU(cudaMemcpyAsync(&t, ticket, 4, cudaMemcpyDeviceToHost, s)); CU(cudaStreamSynchronize(s));
+      if (t != 0) return fail(B2G_ERR_CUDA, "CNN loss: the kernel left its ticket word at %u", t);
       break;
     }
     case B2G_EW_ACT_FWD: case B2G_EW_ACT_BWD: {

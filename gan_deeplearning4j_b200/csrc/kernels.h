@@ -137,6 +137,15 @@ void k_softmax_xent(int prec, const void* z, const float* y, void* dz, void* p_o
 int k_loss_blocks(size_t n_per_group, int groups);
 void k_loss(int prec, int loss, int act, float alpha, const void* z, const float* y, void* dz, float* loss_sums, int rows_per_group, int n_out, int groups,
             double* partial, unsigned* ticket, cudaStream_t s);
+// CnnLossLayer (kernels_cnnloss.cu; summation orders stated there): sigmoid XENT over groups x n_per_group elements, and softmax MCXENT over
+// the C channels of groups x rows_per_group NHWC pixels (y = null: the inference call, p_out only).  dz in the sum form, loss_sums[g] = group
+// g's summed scores.  partial: [groups * k_loss_blocks(n_per_group, groups)] (XENT) / [groups * k_cnn_softmax_blocks(rows_per_group, groups)]
+// (MCXENT) doubles, at most 1024; ticket: 0 between launches.
+void k_cnn_xent(int prec, const void* z, const float* y, void* dz, float* loss_sums, size_t n_per_group, int groups, float clip_eps, double* partial,
+                unsigned* ticket, cudaStream_t s);
+int k_cnn_softmax_blocks(int rows_per_group, int groups);
+void k_cnn_softmax_xent(int prec, const void* z, const float* y, void* dz, void* p_out, float* loss_sums, int rows_per_group, int C, int groups,
+                        double* partial, unsigned* ticket, cudaStream_t s);
 
 // ---- reductions ------------------------------------------------------------------------------------
 // out[c] (+)= sum_rows x[row][c]
@@ -237,6 +246,18 @@ size_t k_dense_small_o_wgrad_scratch_floats(const ConvGeom& g);
 bool dense_small_k_supported(const ConvGeom& g);         // 1x1 geometry, reduction g.O <= 128, g.C % 256 == 0 (DCGAN G-first: z -> 4x4 map)
 void k_dense_small_k_dgrad(int prec, int wprec, const ConvGeom& g, const void* dy, const void* w, const float* bias, void* dx, int act, float alpha, cudaStream_t s);
 void k_dense_small_k_wgrad(int prec, const ConvGeom& g, const void* x, const void* dy, float* dw, cudaStream_t s);
+
+// ---- few-output conv, BF16 nets (kernels_head.cu): k x k conv (KH*KW > 1, KH, KW <= 7, stride 1-2, 0 <= pad < kernel) from C % 8 == 0
+// channels onto O <= 4 on a map wider than one pixel (the PatchGAN head).  w: the bf16 weight copy [O][taps][C].  Forward and input gradient
+// take bias / activation (codes 0-4); the weight gradient writes fp32 partials [splits][O][taps][C] into part (k_head_wgrad_scratch_floats for
+// the production split count; force_splits > 0 forces a count, splits past the last pixel are empty) and queues their sum into defer, or
+// sums them at once when defer is null.  Returns -1 when part is too small.
+bool head_conv_supported(const ConvGeom& g);
+size_t k_head_wgrad_scratch_floats(const ConvGeom& g);
+void k_head_fwd(const ConvGeom& g, const __nv_bfloat16* x, const __nv_bfloat16* w, const float* bias, __nv_bfloat16* out, int act, float alpha, cudaStream_t s);
+void k_head_dgrad(const ConvGeom& g, const __nv_bfloat16* dy, const __nv_bfloat16* w, const float* bias, __nv_bfloat16* dx, int act, float alpha, cudaStream_t s);
+int k_head_wgrad(const ConvGeom& g, const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, float* part, size_t part_floats, int force_splits, cudaStream_t s,
+                 ReduceList* defer);
 
 // ---- GEMM-shaped kernels, wgmma tensor cores (bf16 in, fp32 accumulate in registers) -------------------------
 bool tc_fprop_supported(const ConvGeom& g);

@@ -17,7 +17,8 @@ from . import _lib
 from ._lib import GanConfig, LayerDesc, LrSchedule, NetConfig, check
 
 LAYER_TYPES = {"conv2d": 0, "deconv2d": 1, "batchnorm": 2, "dense": 3, "activation": 4, "maxpool": 5, "upsample2d": 6,
-               "output": 7, "loss": 8, "ff_to_cnn": 9, "cnn_to_ff": 10, "dropout": 11, "subsampling": 12, "global_pooling": 13}
+               "output": 7, "loss": 8, "ff_to_cnn": 9, "cnn_to_ff": 10, "dropout": 11, "subsampling": 12, "global_pooling": 13,
+               "cnn_loss": 14}
 # org.deeplearning4j.nn.conf.layers.PoolingType -> b2g_pooling, carried in b2g_layer_desc.act of "subsampling" (avg / sum / pnorm; max is the
 # "maxpool" layer) and "global_pooling" (all four) specs; PNORM's p in act_alpha (formulas at b2g_pooling in include/b200gan.h)
 POOLINGS = {"max": 0, "avg": 1, "sum": 2, "pnorm": 3}
@@ -445,8 +446,23 @@ class Gan:
         check(self.lib.b2g_gan_create(gen.h, dis.h, C.byref(cfg), C.byref(h)))
         self.h = h
 
+    def _args(self, x_real, z_d, z_g, y_real, y_fake, y_gen):
+        """fp32 arrays; each label vector becomes [N, out_elems] of the discriminator (NCHW for a CnnLossLayer patch map): per-image labels
+        ([N] or [N, 1]) are broadcast over the map."""
+        x = _f32(x_real)
+        n, oe = x.shape[0], self.dis.out_elems
+        ys = []
+        for name, y in (("y_real", y_real), ("y_fake", y_fake), ("y_gen", y_gen)):
+            y = _f32(y).reshape(n, -1)
+            if y.shape[1] == 1 and oe > 1:
+                y = np.ascontiguousarray(np.broadcast_to(y, (n, oe)))
+            if y.shape[1] != oe:
+                raise ValueError(f"{name}: {y.shape[1]} labels per example; the discriminator has {oe} outputs per example (or pass one per image)")
+            ys.append(y)
+        return [x, _f32(z_d), _f32(z_g)] + ys
+
     def step(self, x_real, z_d, z_g, y_real, y_fake, y_gen):
-        a = [_f32(v) for v in (x_real, z_d, z_g, y_real, y_fake, y_gen)]
+        a = self._args(x_real, z_d, z_g, y_real, y_fake, y_gen)
         losses = np.zeros(3, np.float32)
         check(self.lib.b2g_gan_step(self.h, *[_fp(v) for v in a], a[0].shape[0], _fp(losses)))
         return losses
@@ -457,7 +473,7 @@ class Gan:
         check(self.lib.b2g_gan_step(self.h, *args, batch, _fp(losses)))
 
     def upload(self, x_real, z_d, z_g, y_real, y_fake, y_gen):
-        a = [_f32(v) for v in (x_real, z_d, z_g, y_real, y_fake, y_gen)]
+        a = self._args(x_real, z_d, z_g, y_real, y_fake, y_gen)
         check(self.lib.b2g_gan_upload(self.h, *[_fp(v) for v in a], a[0].shape[0]))
         self.gen.ctx.sync()
 
@@ -566,7 +582,8 @@ def test_dropout(ctx: Context, precision: int, x, dy, p: float, *, seed: int = 6
 
 
 EW_OPS = {"reduce_splits": 0, "reduce_multi": 1, "colsum": 2, "xent": 3, "softmax_xent": 4, "act_fwd": 5, "act_bwd": 6, "maxpool": 7,
-          "upsample": 8, "sumsq": 9, "loss": 10, "act_ext_fwd": 11, "act_ext_bwd": 12}
+          "upsample": 8, "sumsq": 9, "loss": 10, "act_ext_fwd": 11, "act_ext_bwd": 12,
+          "cnn_xent": 13, "cnn_softmax_xent": 14}
 
 
 def test_ew(ctx: Context, precision: int, op: str, in0, in1=None, out_sizes=(0, 0, 0), *, act: str = "identity", jobs=None, segments=None,

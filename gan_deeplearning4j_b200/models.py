@@ -112,6 +112,21 @@ def global_pooling(pooling="max", pnorm=2, name="") -> Dict:
 _global_pooling_spec = global_pooling       # dcgan_discriminator's argument of the same name shadows the builder
 
 
+# ------------------------------------------------------------------ per-pixel loss ---------------------
+def cnn_loss(loss="xent", activation="identity", name="", alpha=None) -> Dict:
+    """new CnnLossLayer.Builder(LossFunction).activation(act): the loss on every pixel of a [mb, C, H, W] map, labels [mb, C, H, W]
+    (B2G_LAYER_CNN_LOSS in include/b200gan.h).  XENT implies a sigmoid per element, MCXENT a softmax over the channels of each pixel; the
+    others apply `activation`."""
+    if loss not in ("xent", "mcxent", "mse", "l1", "l2", "mae", "hinge", "squared_hinge", "wasserstein"):
+        raise ValueError(f"unknown loss {loss!r}")
+    if loss in ("xent", "mcxent") and activation != "identity":
+        raise ValueError(f"{loss.upper()} implies its activation: activation applies to the losses other than XENT and MCXENT")
+    spec = {"type": "cnn_loss", "name": name, "loss": loss}
+    if loss not in ("xent", "mcxent"):
+        spec.update(_act(activation, alpha))
+    return spec
+
+
 # ------------------------------------------------------------------ C1: the reference graphs ---------
 def reference_discriminator(lr=0.002, prefix="dis") -> List[Dict]:
     """J:118-165: BN -> Conv5x5 s2 (1->64) -> MaxPool 2x2 s1 -> Conv5x5 s2 (64->128) -> MaxPool -> Dense 1024 -> Output(1, sigmoid, XENT);
@@ -195,14 +210,21 @@ def _loss_keys(loss, out_activation) -> Dict:
 
 
 def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", out_activation="identity", activation="lrelu", alpha=None,
-                        global_pooling=None) -> List[Dict]:
+                        global_pooling=None, patch=False) -> List[Dict]:
     """Conv(4x4 s2 p1)+LeakyReLU(0.2); (Conv+BatchNorm+LeakyReLU)*; Conv(4x4 s1 p0) -> logit; LossLayer(loss).  Input (nc,size,size).
     loss: "xent" (sigmoid implied), or "mse" (least-squares GAN), "hinge", "wasserstein", ... applied to out_activation(logit).
     activation / alpha: the hidden activation in place of LeakyReLU(0.2) (as in _act).
     global_pooling: a pooling kind ("sum" for the projected / ResNet-style head, "avg", "max", "pnorm"): GlobalPoolingLayer + OutputLayer(nOut 1,
-    loss) in place of the last conv and its LossLayer."""
+    loss) in place of the last conv and its LossLayer.
+    patch: a PatchGAN critic -- the down-sampling stages stop at the max(4, size/16) map (at most four stride-2 convs), and a 3x3 s1 p1 conv onto
+    1 channel and a CnnLossLayer(loss) take the place of the last conv and its LossLayer: one logit and one label per patch (a 4x4 map up to
+    64x64, 8x8 at 128x128)."""
+    if patch and global_pooling is not None:
+        raise ValueError("patch and global_pooling are two different heads")
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
     n_down = int(math.log2(size)) - 2
+    if patch:
+        n_down = min(n_down, 4)
     L = [{"type": "conv2d", "name": "dis_conv_1", "n_in": nc, "n_out": nf, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), **_act(activation, alpha), "updater": u()}]
     ch = nf
     for i in range(n_down - 1):
@@ -212,6 +234,9 @@ def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", o
     if global_pooling is not None:
         return L + [_global_pooling_spec(global_pooling, name="dis_global_pool"),
                     dict({"type": "output", "name": "dis_output", "n_out": 1, "updater": u()}, **_loss_keys(loss, out_activation))]
+    if patch:
+        return L + [{"type": "conv2d", "name": f"dis_conv_{n_down + 1}", "n_in": ch, "n_out": 1, "kernel": (3, 3), "stride": (1, 1), "padding": (1, 1), "updater": u()},
+                    dict({"type": "cnn_loss", "name": "dis_loss"}, **_loss_keys(loss, out_activation))]
     L += [{"type": "conv2d", "name": f"dis_conv_{n_down + 1}", "n_in": ch, "n_out": 1, "kernel": (4, 4), "stride": (1, 1), "padding": (0, 0), "updater": u()},
           dict({"type": "loss", "name": "dis_loss"}, **_loss_keys(loss, out_activation))]
     return L

@@ -65,7 +65,8 @@ typedef enum {
   B2G_LAYER_CNN_TO_FF = 10,  /* CnnToFeedForwardPreProcessor (auto-inserted by setInputTypes, SURVEY.md 3.1)       */
   B2G_LAYER_DROPOUT = 11,    /* DropoutLayer.Builder(p): p = RETAIN probability in (0, 1], carried in act_alpha; no parameters */
   B2G_LAYER_SUBSAMPLING = 12,    /* SubsamplingLayer.Builder(PoolingType.AVG / SUM / PNORM).kernelSize().stride().padding().pnorm(): b2g_pooling */
-  B2G_LAYER_GLOBAL_POOLING = 13  /* GlobalPoolingLayer.Builder(PoolingType).pnorm(): b2g_pooling, output [mb, C] (H = W = 1)                 */
+  B2G_LAYER_GLOBAL_POOLING = 13, /* GlobalPoolingLayer.Builder(PoolingType).pnorm(): b2g_pooling, output [mb, C] (H = W = 1)                 */
+  B2G_LAYER_CNN_LOSS = 14        /* CnnLossLayer.Builder(LossFunction).activation(..): the loss per pixel of a [mb, C, H, W] map; no parameters  */
 } b2g_layer_type;
 
 /* DropoutLayer (inverted dropout, DL4J 1.0.0-beta3).  Train-mode forward y = x * m, m = 1/p (fp32 1.0f / p) with probability p, else 0;
@@ -182,7 +183,25 @@ typedef enum { B2G_PREC_FP32 = 0, B2G_PREC_BF16 = 1 } b2g_precision;
  * bits on every run) and rounded to fp32 once; score = that sum / minibatch + the l2 term.  OUTPUT layers take any nOut; a LOSS layer needs a
  * feed-forward input (H = W = 1) or one element per example (else B2G_ERR_UNSUPPORTED).  b2g_net_output returns a = act(z).
  * With an activation of codes 5-16 (b2g_activation) a = f(z) is formed by its own kernel and rounded to the activation type, the loss takes a
- * with the identity, and dL/dz = dL/da * f'(z) with the derivative taken from z. */
+ * with the identity, and dL/dz = dL/da * f'(z) with the derivative taken from z.
+ *
+ * B2G_LAYER_CNN_LOSS (DL4J 1.0.0-beta3 CnnLossLayer, recalled; parity unpinned like the rest of the DL4J semantics).  No parameters.
+ *   Rows and columns: the input is the layer below's [N, C, H, W]; the rows are its N*H*W pixels and the columns its C channels (DL4J's
+ *   reshape4dTo2d, which in the engine's NHWC layout is the buffer as it is).  A 1x1 map is accepted and then equals a LOSS layer on the same
+ *   values.
+ *   XENT (0): a sigmoid on every element, any C; the per-element formulas and xent_clip_eps are those of XENT above; act is ignored.
+ *   MCXENT (1): a softmax over the C channels of each pixel; score -sum_c y log(clamp(p, 1e-10, 1 - 1e-10)) (the log in double), dz = p - y;
+ *   act is ignored.
+ *   Codes 2-8: on a = act(z) with activation codes 0-16, exactly as on LOSS layers, with nOut = C (MSE, MAE and WASSERSTEIN divide by the
+ *   channel count, not by C*H*W).
+ *   Score = (sum of the row scores over all N*H*W rows) / N + the l2 term: CnnLossLayer.computeScore divides by the minibatch, not by the
+ *   pixel count.  dz is not divided; the updater's division by the minibatch is the only one.  The sums are taken in double in an order
+ *   fixed by the shape (kernels_cnnloss.cu for XENT / MCXENT, loss_kernel for codes 2-8) and rounded to fp32 once.
+ *   Labels: [N, C, H, W] fp32 in DL4J's NCHW order, b2g_net_output_size elements per example (fit, computeGradientAndScore and the GAN step).
+ *   b2g_net_output returns the activated map in NCHW: the sigmoid (XENT), the per-pixel softmax (MCXENT) or act(z).
+ *   Not supported: label masks, per-output weights, and the NHWC CNN2DFormat of later DL4J versions.
+ *   The adversarial step (b2g_gan_create) takes a discriminator ending in CNN_LOSS with XENT or codes 2-8 (a PatchGAN critic: one logit and
+ *   one label per patch); MCXENT there is B2G_ERR_UNSUPPORTED. */
 typedef enum {
   B2G_LOSS_XENT = 0, B2G_LOSS_MCXENT = 1, B2G_LOSS_MSE = 2, B2G_LOSS_L1 = 3, B2G_LOSS_L2 = 4, B2G_LOSS_MAE = 5, B2G_LOSS_HINGE = 6,
   B2G_LOSS_SQUARED_HINGE = 7, B2G_LOSS_WASSERSTEIN = 8
@@ -447,6 +466,10 @@ typedef struct {
                              (splits past the last K-block are empty), or tc_edge_wgrad_kernel's CTA target (tiles_per_cta = ceil(tiles / splits));
                              out, the count launched */
 } b2g_test_conv_opts;
+/* impl 5: the few-output conv kernels of BF16 nets (a k x k conv, KH*KW > 1, KH, KW <= 7, stride 1-2, 0 <= pad < kernel, from C % 8 == 0
+ * channels onto O <= 4 on a map wider than one pixel; B2G_ERR_UNSUPPORTED otherwise): bias / act / poison as impl 2 takes them; kind 2 runs the
+ * weight gradient's split sums as one reduce-list launch, takes splits (forced count, splits past the last pixel are empty), param_offset and
+ * db (the column sums of dy, as the training step forms the bias gradient). */
 int32_t b2g_test_conv_ex(b2g_ctx* ctx, int32_t kind, int32_t impl, int32_t precision, const b2g_conv_geom* g,
                          const float* x_or_dy, const float* w_or_x, float* out, int32_t iters, float* ms_per_iter, b2g_test_conv_opts* opts);
 
@@ -492,11 +515,15 @@ int32_t b2g_test_dropout(b2g_ctx* ctx, int32_t precision, uint64_t seed, int32_t
  *   ACT_EXT_FWD    in0 z [n] T                                                        -> out0 f(z) T             (act = b2g_activation 5-16, alpha)
  *   ACT_EXT_BWD    in0 z [n] T, in1 eps_out [n] T                                     -> out0 eps_out * f'(z) T, computed in place in eps_out's
  *                                                                                        buffer as the backward pass calls it (act 5-16, alpha)
+ *   CNN_XENT       in0 logits [groups][rows][cols] T (NHWC pixels x channels), in1 labels fp32
+ *                                                                                     -> out0 dz T, out1 loss per group [groups]   (clip_eps)
+ *   CNN_SOFTMAX_XENT  in0 logits [groups][rows][cols] T, in1 labels fp32 or NULL (inference: probabilities only)
+ *                                                                                     -> out0 dz T, out1 loss per group [groups], out2 probabilities T
  * Every output buffer not asked for may be NULL. */
 typedef enum {
   B2G_EW_REDUCE_SPLITS = 0, B2G_EW_REDUCE_MULTI = 1, B2G_EW_COLSUM = 2, B2G_EW_XENT = 3, B2G_EW_SOFTMAX_XENT = 4,
   B2G_EW_ACT_FWD = 5, B2G_EW_ACT_BWD = 6, B2G_EW_MAXPOOL = 7, B2G_EW_UPSAMPLE = 8, B2G_EW_SUMSQ = 9, B2G_EW_LOSS = 10,
-  B2G_EW_ACT_EXT_FWD = 11, B2G_EW_ACT_EXT_BWD = 12
+  B2G_EW_ACT_EXT_FWD = 11, B2G_EW_ACT_EXT_BWD = 12, B2G_EW_CNN_XENT = 13, B2G_EW_CNN_SOFTMAX_XENT = 14
 } b2g_ew_op;
 typedef struct {          /* one split-K sum of a reduce list: dst[i] = sum_s src[s*stride + i], i < n, all offsets in elements of in0 */
   int64_t n, stride, src_off, dst_off;
@@ -506,8 +533,8 @@ typedef struct {          /* one split-K sum of a reduce list: dst[i] = sum_s sr
 typedef struct {
   int32_t op;             /* b2g_ew_op */
   int64_t n;              /* REDUCE_SPLITS outputs, REDUCE_MULTI buffer length, ACT_* / SUMSQ elements */
-  int32_t rows, cols;     /* COLSUM rows x channels; XENT rows per group; SOFTMAX_XENT rows x classes */
-  int32_t groups;         /* XENT */
+  int32_t rows, cols;     /* COLSUM rows x channels; XENT rows per group; SOFTMAX_XENT rows x classes; CNN_* pixels per group x channels */
+  int32_t groups;         /* XENT, LOSS, CNN_* */
   int32_t splits; int64_t stride;       /* REDUCE_SPLITS */
   int32_t N, H, W, C, KH, KW, SH, SW;  /* MAXPOOL input and window; UPSAMPLE input and factor KH */
   int32_t act; float alpha;             /* ACT_*: b2g activation */

@@ -20,6 +20,7 @@ public final class Native {
     public static native int netCreate(long ctx, long cfgAddr, long layersAddr, int n, long outHandleAddr);
     public static native int netDestroy(long net);
     public static native int netNumParams(long net, long outAddr);
+    public static native int netOutputSize(long net, long outAddr);
     public static native int netSetParam(long net, long layerNameAddr, long paramNameAddr, long hostAddr, long n);
     public static native int netGetParam(long net, long layerNameAddr, long paramNameAddr, long hostAddr, long n);
     public static native int netGetParams(long net, long hostAddr, long n);

@@ -67,6 +67,8 @@ public class ComputationGraph {
     public void incrementEpochCount() { setEpochCount(getEpochCount() + 1); }
     public long handle() { return net; }
     public ComputationGraphConfiguration configuration() { return conf; }
+    /** Outputs per example of the last layer (b2g_net_output_size): 1 for a one-logit discriminator, C*H*W after a CnnLossLayer. */
+    public long outputSize() { ByteBuffer o = Native.direct(8); Native.check(Native.netOutputSize(net, Native.address(o))); return o.getLong(0); }
     public long numParams() { ByteBuffer o = Native.direct(8); Native.check(Native.netNumParams(net, Native.address(o))); return o.getLong(0); }
     public String summary() { StringBuilder s = new StringBuilder("b200gan ComputationGraph, params=" + numParams() + "\n"); for (Layer l : layers) s.append("  ").append(l.name).append(" type=").append(l.type).append(" nOut=").append(l.nOut).append("\n"); return s.toString(); }
 

@@ -30,6 +30,7 @@ FN(netCreate)(JNIEnv_*, jclass, jlong ctx, jlong cfgAddr, jlong layersAddr, jint
 }
 FN(netDestroy)(JNIEnv_*, jclass, jlong net) { return b2g_net_destroy(P(b2g_net*, net)); }
 FN(netNumParams)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_num_params(P(b2g_net*, net), P(int64_t*, outAddr)); }
+FN(netOutputSize)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_output_size(P(b2g_net*, net), P(int64_t*, outAddr)); }
 FN(netSetParam)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong paramNameAddr, jlong hostAddr, jlong n) {
   return b2g_net_set_param(P(b2g_net*, net), P(const char*, layerNameAddr), P(const char*, paramNameAddr), P(const float*, hostAddr), n);
 }
