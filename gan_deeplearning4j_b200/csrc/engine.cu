@@ -108,6 +108,10 @@ struct LayerRT {
   // DropoutLayer: its own output buffer (never its input: the layer below differentiates from its own pre-dropout output) and the 1-bit
   // keep mask of the latest train-mode forward; `out` is drop_buf after a masked forward and the input itself after a pass-through one
   void* drop_buf = nullptr; uint32_t* drop_mask = nullptr; bool drop_live = false;
+  // ELEMENTWISE / MERGE (include/b200gan.h): the skip source j (d.pre_h), the input order (d.pre_w), and whether this vertex is the first
+  // consumer of j the backward visits (it writes j's accumulator; the later ones add).  A skip source: its consumer count and fp32 accumulator.
+  int vsrc = -1, vorder = 0; bool vfirst = false;
+  int n_skip = 0; float* skip_acc = nullptr;
   bool drop_active() const { return d.type == B2G_LAYER_DROPOUT && !d.frozen && d.act_alpha < 1.f; }   // FrozenLayer: test mode, identity
   bool has_gemm() const { return d.type == B2G_LAYER_CONV2D || d.type == B2G_LAYER_DECONV2D || d.type == B2G_LAYER_DENSE || d.type == B2G_LAYER_OUTPUT; }
 };
@@ -323,6 +327,19 @@ static int32_t net_build(b2g_net* n, const b2g_layer_desc* layers, int32_t nl) {
         if ((uint64_t)c.max_batch * h * w * ch > (1ull << 34))     // checked before anything is allocated
           return fail(B2G_ERR_UNSUPPORTED, "layer %s: a dropout pass of %llu elements exceeds the 2^34 the mask counter addresses", d.name, (unsigned long long)c.max_batch * h * w * ch);
         break;
+      case B2G_LAYER_ELEMENTWISE: case B2G_LAYER_MERGE: {      // the spine (entry i-1) and a skip source j = pre_h, in the order pre_w
+        const int j = d.pre_h;
+        if (j < 0 || j >= i) return fail(B2G_ERR_ARG, "layer %s: skip source %d outside [0, %d)", d.name, j, i);
+        if (d.pre_w != 0 && d.pre_w != 1) return fail(B2G_ERR_ARG, "layer %s: input order %d (0 = spine first, 1 = skip first)", d.name, d.pre_w);
+        if (d.type == B2G_LAYER_ELEMENTWISE && (d.act < B2G_EW_OP_ADD || d.act > B2G_EW_OP_MAX)) return fail(B2G_ERR_ARG, "layer %s: unknown element-wise op %d", d.name, d.act);
+        const LayerRT& src = n->L[j];
+        if (src.d.type == B2G_LAYER_LOSS || src.d.type == B2G_LAYER_CNN_LOSS || src.d.type == B2G_LAYER_OUTPUT)
+          return fail(B2G_ERR_UNSUPPORTED, "layer %s: skip source %s is a loss-bearing layer", d.name, src.d.name);
+        if (src.oh != h || src.ow != w || (d.type == B2G_LAYER_ELEMENTWISE && src.oc != ch))
+          return fail(B2G_ERR_SHAPE, "layer %s: inputs [%d,%d,%d] (spine) and [%d,%d,%d] (%s) do not match", d.name, ch, h, w, src.oc, src.oh, src.ow, src.d.name);
+        l.vsrc = j; l.vorder = d.pre_w;
+        l.oh = h; l.ow = w; l.oc = d.type == B2G_LAYER_MERGE ? ch + src.oc : ch;
+      } break;
       default: return fail(B2G_ERR_ARG, "layer %d: unknown type %d", i, d.type);
     }
     l.out_elems = (size_t)l.oh * l.ow * l.oc;
@@ -331,9 +348,15 @@ static int32_t net_build(b2g_net* n, const b2g_layer_desc* layers, int32_t nl) {
     h = l.oh; w = l.ow; ch = l.oc;
     n->L.push_back(l);
   }
-  // fuse BatchNormalization + ActivationLayer (north_star's BN+ReLU / BN+LeakyReLU); an ActivationLayer of codes 5-16 runs its own kernels
+  // skip sources: consumer counts, and the first consumer in backward order (the highest index) of each
+  for (int i = (int)n->L.size() - 1; i >= 0; --i) {
+    LayerRT& l = n->L[i];
+    if (l.vsrc >= 0) { l.vfirst = n->L[l.vsrc].n_skip == 0; ++n->L[l.vsrc].n_skip; }
+  }
+  // fuse BatchNormalization + ActivationLayer (north_star's BN+ReLU / BN+LeakyReLU); an ActivationLayer of codes 5-16 runs its own kernels.
+  // Not where the BatchNorm is a skip source: its vertex reads the BatchNorm's own output and hands it an epsilon w.r.t. that output.
   for (size_t i = 0; i + 1 < n->L.size(); ++i)
-    if (n->L[i].d.type == B2G_LAYER_BATCHNORM && n->L[i + 1].d.type == B2G_LAYER_ACTIVATION && !n->L[i + 1].ext_act) {
+    if (n->L[i].d.type == B2G_LAYER_BATCHNORM && !n->L[i].n_skip && n->L[i + 1].d.type == B2G_LAYER_ACTIVATION && !n->L[i + 1].ext_act) {
       n->L[i].fused_act = n->L[i + 1].d.act; n->L[i].fused_alpha = n->L[i + 1].d.act_alpha; n->L[i + 1].act_fused_into_prev = true;
     }
   int last = n->L.back().d.type;
@@ -374,6 +397,7 @@ static int32_t net_alloc(b2g_net* n) {
     if (l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS || l.d.type == B2G_LAYER_CNN_LOSS) B2(dalloc(n, (char**)&l.probs, ts * R * l.out_elems));
     if (l.ext_act && l.has_gemm() && l.d.type != B2G_LAYER_OUTPUT) B2(dalloc(n, (char**)&l.ext_z, ts * R * l.out_elems));
     if (l.d.type == B2G_LAYER_MAXPOOL) B2(dalloc(n, &l.argmax, (size_t)R * l.out_elems));
+    if (l.n_skip) B2(dalloc(n, &l.skip_acc, sizeof(float) * R * l.out_elems));
     if (l.d.type == B2G_LAYER_GLOBAL_POOLING) {
       if (l.pool == B2G_POOL_MAX) B2(dalloc(n, &l.pool_idx, sizeof(int32_t) * R * l.oc));
       const size_t part = k_global_pool_partial_elems(n->prec, R, l.ih * l.iw, l.ic);
@@ -638,7 +662,9 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
     // a 1x1-input deconv is computed as the 1x1 problem with taps*C output channels: its columns are not the BatchNorm's channels
     const bool remapped = d.type == B2G_LAYER_DECONV2D && l.geom.KH == 1 && l.geom.C != l.oc;
     // inference-mode (or frozen) BatchNorm right after a linear conv / deconv / dense: fold it, and its activation, into that GEMM's epilogue
-    if (gemm_then_bn && d.act == B2G_ACT_IDENTITY && !l.ext_act && (!o.train || n->L[i + 1].d.frozen) && !(i + 2 == n->L.size() && o.out_override) && !remapped) {
+    // (not when the GEMM is a skip source: the fold never writes the GEMM's own output, which its vertex reads)
+    if (gemm_then_bn && d.act == B2G_ACT_IDENTITY && !l.ext_act && (!o.train || n->L[i + 1].d.frozen) && !(i + 2 == n->L.size() && o.out_override) && !remapped &&
+        !l.n_skip) {
       LayerRT& bn = n->L[i + 1];
       ConvGeom g = l.geom; g.N = R;
       k_bn_fold(n->params + bn.off_mean, n->params + bn.off_var, n->params + bn.off_gamma, n->params + bn.off_beta, bias, bn.oc, bn.d.bn_eps, bn.bn_fold, bn.bn_fold + bn.oc, s);
@@ -695,6 +721,15 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
         } else out = (void*)cur;       // inference, FrozenLayer or p = 1: the identity, no launch
         l.out = out;
         break;
+      case B2G_LAYER_ELEMENTWISE: {
+        const void* sk = n->L[l.vsrc].out;
+        k_vertex_ew_fwd(n->prec, d.act, l.vorder ? sk : cur, l.vorder ? cur : sk, out, (size_t)R * l.out_elems, s);
+      } break;
+      case B2G_LAYER_MERGE: {
+        const LayerRT& src = n->L[l.vsrc]; const size_t px = (size_t)R * l.oh * l.ow;
+        if (l.vorder) k_merge_fwd(n->prec, src.out, cur, out, px, src.oc, l.ic, s);
+        else k_merge_fwd(n->prec, cur, src.out, out, px, l.ic, src.oc, s);
+      } break;
     }
     if (l.ext_z) k_act_ext_fwd(n->prec, l.ext_act, l.ext_alpha, l.ext_z, out, (size_t)R * l.out_elems, s);
     if (fuse) n->L[i + 1].stats_by_producer = fused;
@@ -752,6 +787,8 @@ static int32_t net_backward(b2g_net* n, const void* net_in, void* eps, int rows,
     if (!tc_on(n)) return false;
     int k = i - 1; while (k >= 0 && n->L[k].act_fused_into_prev) --k;
     if (k < 0) { if (input_act) { *e = *input_act; *target = -2; return true; } return false; }
+    // a skip source in [k, i) still waits for its vertices' share, added at the top of its own backward: nothing may be premultiplied before that
+    for (int m = k; m < i; ++m) if (n->L[m].n_skip) return false;
     LayerRT& b = n->L[k];
     if (b.d.type == B2G_LAYER_BATCHNORM && b.fwd_fused && !b.d.frozen && b.fwd_groups == groups) {
       e->mode = EPI_BNBWD; e->acc = b.acc_bwd; e->imgs_per_group = R / groups; e->aux = (const __nv_bfloat16*)b.out; e->aux2 = (const __nv_bfloat16*)(k == 0 ? net_in : n->L[k - 1].out);
@@ -774,8 +811,20 @@ static int32_t net_backward(b2g_net* n, const void* net_in, void* eps, int rows,
     bool need_in = need_input_grad;
     if (!need_in) for (int j = 0; j < i; ++j) if (!n->L[j].d.frozen && (n->L[j].has_gemm() || n->L[j].d.type == B2G_LAYER_BATCHNORM)) need_in = true;
     const bool want_wgrad_l = want_wgrad && !d.frozen;
+    // a skip source: its vertices' shares join the spine epsilon before anything of its own backward runs
+    if (l.skip_acc) k_skip_add(n->prec, cur, l.skip_acc, (size_t)R * l.out_elems, s);
     switch (d.type) {
       case B2G_LAYER_LOSS: case B2G_LAYER_CNN_LOSS: break;
+      case B2G_LAYER_ELEMENTWISE:      // the spine's share in place, the skip's into the source's accumulator; PRODUCT / MAX read both inputs
+        if (need_in) k_vertex_ew_bwd(n->prec, d.act, l.vorder, cur, lin, n->L[l.vsrc].out, n->L[l.vsrc].skip_acc, l.vfirst ? 0 : 1, (size_t)R * l.out_elems, s);
+        break;
+      case B2G_LAYER_MERGE:
+        if (need_in) {
+          const LayerRT& src = n->L[l.vsrc]; void* nx = other(cur);
+          k_merge_bwd(n->prec, cur, nx, src.skip_acc, (size_t)R * l.oh * l.ow, l.vorder ? src.oc : l.ic, l.vorder ? l.ic : src.oc, l.vorder == 0, l.vfirst ? 0 : 1, s);
+          cur = nx;
+        }
+        break;
       case B2G_LAYER_CONV2D: case B2G_LAYER_DENSE: case B2G_LAYER_OUTPUT: {
         ConvGeom g = l.geom; g.N = R;
         if (d.act != B2G_ACT_IDENTITY && !act_done[i]) k_act_bwd_from_output(n->prec, l.out, cur, cur, (size_t)R * l.out_elems, d.act, d.act_alpha, s);
@@ -1965,6 +2014,42 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
       B2(downT(out0, dz, n)); B2(downF(out1, loss, (size_t)o->groups)); if (sm) B2(downT(out2, p, n));
       unsigned t = 1; CU(cudaMemcpyAsync(&t, ticket, 4, cudaMemcpyDeviceToHost, s)); CU(cudaStreamSynchronize(s));
       if (t != 0) return fail(B2G_ERR_CUDA, "CNN loss: the kernel left its ticket word at %u", t);
+      break;
+    }
+    case B2G_EW_VERTEX_FWD: case B2G_EW_VERTEX_BWD: case B2G_EW_SKIP_ADD: {
+      const size_t n = (size_t)o->n; const int order = o->groups;
+      if (!in0 || !in1 || o->n < 1 || o->n > lim) return fail(B2G_ERR_ARG, "bad vertex arguments");
+      if (o->op != B2G_EW_SKIP_ADD && (o->act < B2G_EW_OP_ADD || o->act > B2G_EW_OP_MAX || (order != 0 && order != 1))) return fail(B2G_ERR_ARG, "bad vertex op / order");
+      if (o->op == B2G_EW_VERTEX_FWD) {
+        void *a = nullptr, *b = nullptr, *y = nullptr; B2(upT(in0, n, &a)); B2(upT(in1, n, &b)); B2(dev(n, ts, &y)); B2(poison(y, ts * n));
+        k_vertex_ew_fwd(prec, o->act, order ? b : a, order ? a : b, y, n, s); ran();
+        B2(downT(out0, y, n));
+      } else if (o->op == B2G_EW_VERTEX_BWD) {
+        void *sp = nullptr, *sk = nullptr, *e = nullptr; float* acc = nullptr;
+        B2(upT(in0, n, &sp)); B2(upT(in0 + n, n, &sk)); B2(upT(in1, n, &e)); B2(upF(o->accumulate ? in1 + n : nullptr, n, &acc)); B2(poison(acc, 4 * n));
+        k_vertex_ew_bwd(prec, o->act, order, e, sp, sk, acc, o->accumulate ? 1 : 0, n, s); ran();
+        B2(downT(out0, e, n)); B2(downF(out1, acc, n));
+      } else {
+        void* e = nullptr; float* acc = nullptr; B2(upT(in0, n, &e)); B2(upF(in1, n, &acc));
+        k_skip_add(prec, e, acc, n, s); ran();
+        B2(downT(out0, e, n));
+      }
+      break;
+    }
+    case B2G_EW_MERGE_FWD: case B2G_EW_MERGE_BWD: {
+      const int Cs = o->cols, Ck = o->C, order = o->groups; const size_t P = (size_t)o->rows, nt = P * (Cs + Ck);
+      if (!in0 || (!in1 && (o->op == B2G_EW_MERGE_FWD || o->accumulate)) || o->rows < 1 || Cs < 1 || Ck < 1 || (order != 0 && order != 1) || nt > (size_t)lim)
+        return fail(B2G_ERR_ARG, "bad merge arguments");
+      if (o->op == B2G_EW_MERGE_FWD) {
+        void *a = nullptr, *b = nullptr, *y = nullptr; B2(upT(in0, P * Cs, &a)); B2(upT(in1, P * Ck, &b)); B2(dev(nt, ts, &y)); B2(poison(y, ts * nt));
+        if (order) k_merge_fwd(prec, b, a, y, P, Ck, Cs, s); else k_merge_fwd(prec, a, b, y, P, Cs, Ck, s);
+        ran(); B2(downT(out0, y, nt));
+      } else {
+        void *e = nullptr, *d = nullptr; float* acc = nullptr;
+        B2(upT(in0, nt, &e)); B2(dev(P * Cs, ts, &d)); B2(upF(o->accumulate ? in1 : nullptr, P * Ck, &acc)); B2(poison(d, ts * P * Cs)); B2(poison(acc, 4 * P * Ck));
+        k_merge_bwd(prec, e, d, acc, P, order ? Ck : Cs, order ? Cs : Ck, order == 0, o->accumulate ? 1 : 0, s); ran();
+        B2(downT(out0, d, P * Cs)); B2(downF(out1, acc, P * Ck));
+      }
       break;
     }
     case B2G_EW_ACT_FWD: case B2G_EW_ACT_BWD: {

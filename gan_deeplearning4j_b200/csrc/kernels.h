@@ -147,6 +147,20 @@ int k_cnn_softmax_blocks(int rows_per_group, int groups);
 void k_cnn_softmax_xent(int prec, const void* z, const float* y, void* dz, void* p_out, float* loss_sums, int rows_per_group, int C, int groups,
                         double* partial, unsigned* ticket, cudaStream_t s);
 
+// ---- skip-connection vertices (kernels_graph.cu; semantics at b2g_elementwise_op in include/b200gan.h) ----------------------------
+// One launch each.  a, b: the vertex's inputs in its input order.  The fp32 accumulator acc of a skip source is written (accumulate = 0, the
+// first contributor of a backward pass) or added to (1).
+enum VertexOp { VERTEX_ADD = 0, VERTEX_SUBTRACT = 1, VERTEX_PRODUCT = 2, VERTEX_AVERAGE = 3, VERTEX_MAX = 4 };   // b2g_elementwise_op
+void k_vertex_ew_fwd(int prec, int op, const void* a, const void* b, void* y, size_t n, cudaStream_t s);
+// eps (w.r.t. the vertex output) becomes the spine's share in place; the skip's share goes to acc.  order 0: inputs (spine, skip), 1: (skip, spine)
+void k_vertex_ew_bwd(int prec, int op, int order, void* eps, const void* spine, const void* skip, float* acc, int accumulate, size_t n, cudaStream_t s);
+// y [P][Ca + Cb] = concat(a [P][Ca], b [P][Cb]) per pixel (NHWC channel concat; [N][F] vectors with P = N)
+void k_merge_fwd(int prec, const void* a, const void* b, void* y, size_t P, int Ca, int Cb, cudaStream_t s);
+// eps [P][Ca + Cb] -> the spine's slice into dst (T), the skip's into acc (fp32).  spine_first: the spine is the first input
+void k_merge_bwd(int prec, const void* eps, void* dst, float* acc, size_t P, int Ca, int Cb, int spine_first, int accumulate, cudaStream_t s);
+// eps = eps + acc in fp32, rounded once to T (the skip gradient joining the spine at its source)
+void k_skip_add(int prec, void* eps, const float* acc, size_t n, cudaStream_t s);
+
 // ---- reductions ------------------------------------------------------------------------------------
 // out[c] (+)= sum_rows x[row][c]
 void k_colsum(int prec, const void* x, int rows, int C, float* scratch, float* out, int accumulate, cudaStream_t s);

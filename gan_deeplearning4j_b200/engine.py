@@ -18,7 +18,10 @@ from ._lib import GanConfig, LayerDesc, LrSchedule, NetConfig, check
 
 LAYER_TYPES = {"conv2d": 0, "deconv2d": 1, "batchnorm": 2, "dense": 3, "activation": 4, "maxpool": 5, "upsample2d": 6,
                "output": 7, "loss": 8, "ff_to_cnn": 9, "cnn_to_ff": 10, "dropout": 11, "subsampling": 12, "global_pooling": 13,
-               "cnn_loss": 14}
+               "cnn_loss": 14, "elementwise": 15, "merge": 16}
+# ElementWiseVertex.Op -> b2g_elementwise_op, carried in b2g_layer_desc.act of "elementwise" specs (semantics in include/b200gan.h)
+ELEMENTWISE_OPS = {"add": 0, "subtract": 1, "product": 2, "average": 3, "max": 4}
+VERTEX_TYPES = ("elementwise", "merge")
 # org.deeplearning4j.nn.conf.layers.PoolingType -> b2g_pooling, carried in b2g_layer_desc.act of "subsampling" (avg / sum / pnorm; max is the
 # "maxpool" layer) and "global_pooling" (all four) specs; PNORM's p in act_alpha (formulas at b2g_pooling in include/b200gan.h)
 POOLINGS = {"max": 0, "avg": 1, "sum": 2, "pnorm": 3}
@@ -121,7 +124,42 @@ def _f32(a) -> np.ndarray:
     return np.ascontiguousarray(a, dtype=np.float32)
 
 
-def layer_desc(spec: Dict) -> LayerDesc:
+def resolve_vertices(specs: Sequence[Dict]) -> List[Optional[tuple]]:
+    """Each vertex spec's ("inputs": [name, name]) as (j, order): j the index of the skip source, order 0 when the inputs are (spine, j) and 1
+    when they are (j, spine); None for the other specs.  The spine is the previous spec.  ValueError for a graph that is not spine plus skip:
+    a vertex without exactly two inputs, neither of them the previous spec, a name that is not an earlier spec or names several, the net input
+    as an input, or a loss-bearing source."""
+    out: List[Optional[tuple]] = []
+    for i, sp in enumerate(specs):
+        if sp["type"] not in VERTEX_TYPES:
+            out.append(None)
+            continue
+        name, inputs = sp.get("name", ""), list(sp.get("inputs", ()))
+        if len(inputs) != 2:
+            raise ValueError(f"vertex {name!r}: needs exactly two inputs, got {inputs}")
+        if i == 0:
+            raise ValueError(f"vertex {name!r}: the net input cannot be a vertex input")
+        if sp["type"] == "elementwise" and sp.get("op") not in ELEMENTWISE_OPS:
+            raise ValueError(f"vertex {name!r}: unknown op {sp.get('op')!r}; one of {sorted(ELEMENTWISE_OPS)}")
+        earlier = [s.get("name", "") for s in specs[:i]]
+        spine = earlier[-1]
+        if inputs[0] == spine:
+            order, other = 0, inputs[1]
+        elif inputs[1] == spine:
+            order, other = 1, inputs[0]
+        else:
+            raise ValueError(f"vertex {name!r}: one input must be the previous layer {spine!r} (spine plus skip), got {inputs}")
+        hits = [j for j, nm in enumerate(earlier) if nm == other]
+        if len(hits) != 1:
+            raise ValueError(f"vertex {name!r}: input {other!r} names {len(hits)} earlier layers (needs exactly one)")
+        if specs[hits[0]]["type"] in ("loss", "cnn_loss", "output"):
+            raise ValueError(f"vertex {name!r}: input {other!r} is a loss-bearing layer")
+        out.append((hits[0], order))
+    return out
+
+
+def layer_desc(spec: Dict, skip: Optional[tuple] = None) -> LayerDesc:
+    """skip: the vertex's (j, order) from resolve_vertices."""
     d = LayerDesc()
     d.type = LAYER_TYPES[spec["type"]]
     d.name = spec.get("name", "").encode()[:63]
@@ -158,6 +196,9 @@ def layer_desc(spec: Dict) -> LayerDesc:
     d.pre_h, d.pre_w, d.pre_c = to
     d.loss = LOSSES[spec.get("loss", "xent")]
     d.frozen = 1 if spec.get("frozen", False) else 0
+    if spec["type"] in VERTEX_TYPES:       # the op in act, the skip source and the input order in pre_h / pre_w
+        d.act = ELEMENTWISE_OPS[spec["op"]] if spec["type"] == "elementwise" else 0
+        d.pre_h, d.pre_w = skip
     return d
 
 
@@ -218,7 +259,7 @@ def comm_unique_id() -> bytes:
 
 
 class Net:
-    """b2g_net: a chain-shaped ComputationGraph (init / output / fit / getLayer(..).getParam/setParam; J:166-170,420-510)."""
+    """b2g_net: a spine-plus-skip ComputationGraph (init / output / fit / getLayer(..).getParam/setParam; J:166-170,420-510)."""
 
     def __init__(self, ctx: Context, specs: Sequence[Dict], input_shape, max_batch: int, precision: int = FP32,
                  grad_clip: float = 0.0, xent_clip_eps: float = 1e-5, bn_groups: int = 1, seed: int = 666,
@@ -229,7 +270,7 @@ class Net:
         c, h, w = input_shape if len(input_shape) == 3 else (input_shape[0], 1, 1)
         self.input_shape = tuple(input_shape)
         cfg = NetConfig(h, w, c, max_batch, precision, grad_clip, xent_clip_eps, bn_groups, seed)
-        arr = (LayerDesc * len(specs))(*[layer_desc(s) for s in specs])
+        arr = (LayerDesc * len(specs))(*[layer_desc(s, v) for s, v in zip(specs, resolve_vertices(specs))])
         hnd = C.c_void_p()
         check(self.lib.b2g_net_create(ctx.h, C.byref(cfg), arr, len(specs), C.byref(hnd)))
         self.h = hnd
@@ -583,19 +624,20 @@ def test_dropout(ctx: Context, precision: int, x, dy, p: float, *, seed: int = 6
 
 EW_OPS = {"reduce_splits": 0, "reduce_multi": 1, "colsum": 2, "xent": 3, "softmax_xent": 4, "act_fwd": 5, "act_bwd": 6, "maxpool": 7,
           "upsample": 8, "sumsq": 9, "loss": 10, "act_ext_fwd": 11, "act_ext_bwd": 12,
-          "cnn_xent": 13, "cnn_softmax_xent": 14}
+          "cnn_xent": 13, "cnn_softmax_xent": 14, "vertex_fwd": 15, "vertex_bwd": 16, "merge_fwd": 17, "merge_bwd": 18, "skip_add": 19}
 
 
 def test_ew(ctx: Context, precision: int, op: str, in0, in1=None, out_sizes=(0, 0, 0), *, act: str = "identity", jobs=None, segments=None,
             loss: str = "xent", **opts):
     """One reduction / loss / element-wise kernel through its production wrapper (b2g_test_ew; operands per op in include/b200gan.h).
+    vertex_fwd / vertex_bwd: act is an ELEMENTWISE_OPS name and groups the input order.
     act_ext_fwd / act_ext_bwd (act: a name of codes 5-16): in0 = z, in1 = eps_out, out0 = f(z) / eps_out * f'(z).
     out_sizes: element counts of out0..out2 (0: not asked for).  opts: the b2g_test_ew_opts sizes and switches (n, rows, cols, groups, splits,
     stride, N, H, W, C, KH, KW, SH, SW, alpha, clip_eps, offset, in_place, accumulate, poison).  jobs (reduce_multi): dicts of n, splits,
     stride, src_off, dst_off.  segments (sumsq): (offsets, lengths, coefficients).  loss (op "loss"): a LOSSES name of codes 2-8.
     Returns ([out0, out1, out2] with None where not asked for, {"kernel": names, "sumsq": float, "wide": [per job]})."""
     o = _lib.TestEwOpts()
-    o.op, o.act, o.loss = EW_OPS[op], ACTS[act], LOSSES[loss]
+    o.op, o.act, o.loss = EW_OPS[op], ELEMENTWISE_OPS[act] if op in ("vertex_fwd", "vertex_bwd") else ACTS[act], LOSSES[loss]
     for k, v in opts.items():
         setattr(o, k, int(v) if isinstance(v, bool) else v)
     keep = []

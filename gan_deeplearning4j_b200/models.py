@@ -127,6 +127,63 @@ def cnn_loss(loss="xent", activation="identity", name="", alpha=None) -> Dict:
     return spec
 
 
+# ------------------------------------------------------------------ skip connections -------------------
+# ElementWiseVertex / MergeVertex (B2G_LAYER_ELEMENTWISE / B2G_LAYER_MERGE in include/b200gan.h).  A vertex's inputs are layer names: one of them
+# must be the layer right before it (the spine), the other any earlier layer (engine.resolve_vertices).
+def elementwise(op, inputs, name="") -> Dict:
+    """graphBuilder.addVertex(name, new ElementWiseVertex(Op), inputs...): op one of add, subtract, product, average, max."""
+    if op not in ("add", "subtract", "product", "average", "max"):
+        raise ValueError(f"unknown ElementWiseVertex op {op!r}")
+    if len(inputs) != 2:
+        raise ValueError("an ElementWiseVertex here takes exactly two inputs")
+    return {"type": "elementwise", "name": name, "op": op, "inputs": list(inputs)}
+
+
+def merge(inputs, name="") -> Dict:
+    """graphBuilder.addVertex(name, new MergeVertex(), inputs...): the two inputs concatenated along the channels (features), in input order."""
+    if len(inputs) != 2:
+        raise ValueError("a MergeVertex here takes exactly two inputs")
+    return {"type": "merge", "name": name, "inputs": list(inputs)}
+
+
+def residual_block(prefix, ch, skip, lr=2e-4, beta1=0.5, activation="relu", alpha=None) -> List[Dict]:
+    """An identity residual block on the ch-channel map of layer `skip`, which must be the layer right before the block:
+    conv3x3 -> BatchNorm -> act -> conv3x3 -> BatchNorm -> ElementWiseVertex(Add)(., skip) -> act (the convolutions stride 1, pad 1, no bias)."""
+    u = lambda: adam(lr, beta1, 0.999, 1e-8)
+    conv = lambda k: {"type": "conv2d", "name": f"{prefix}_conv_{k}", "n_in": ch, "n_out": ch, "kernel": (3, 3), "stride": (1, 1), "padding": (1, 1),
+                      "has_bias": False, "updater": u()}
+    return [conv(1), {"type": "batchnorm", "name": f"{prefix}_bn_1", "updater": u()}, dict({"type": "activation", "name": f"{prefix}_act_1"}, **_act(activation, alpha)),
+            conv(2), {"type": "batchnorm", "name": f"{prefix}_bn_2", "updater": u()},
+            elementwise("add", [f"{prefix}_bn_2", skip], name=f"{prefix}_add"), dict({"type": "activation", "name": f"{prefix}_act_2"}, **_act(activation, alpha))]
+
+
+def unet(size=64, nc=3, n_classes=2, nf=32, depth=2, loss="mcxent", lr=1e-3, beta1=0.9, activation="relu", alpha=None) -> List[Dict]:
+    """A U-Net segmentation net (Ronneberger et al. 2015) of `depth` levels into a CnnLossLayer.  Input (nc, size, size), labels [n_classes,
+    size, size].  Level k (channels nf * 2^k): conv3x3 -> BatchNorm -> act, then MaxPool 2x2 s2; the bottom: conv3x3 -> BatchNorm -> act; on the
+    way up Deconvolution2D 4x4 s2 p1 -> MergeVertex(up, level k's act) -> conv3x3 -> BatchNorm -> act; last a 1x1 conv onto n_classes and
+    CnnLossLayer(loss)."""
+    if size % (2 ** depth):
+        raise ValueError(f"size {size} is not divisible by 2^depth = {2 ** depth}")
+    u = lambda: adam(lr, beta1, 0.999, 1e-8)
+    conv_bn_act = lambda name, c_in, c_out: [
+        {"type": "conv2d", "name": f"{name}_conv", "n_in": c_in, "n_out": c_out, "kernel": (3, 3), "stride": (1, 1), "padding": (1, 1), "has_bias": False, "updater": u()},
+        {"type": "batchnorm", "name": f"{name}_bn", "updater": u()}, dict({"type": "activation", "name": f"{name}_act"}, **_act(activation, alpha))]
+    L, c = [], nc
+    for k in range(depth):
+        L += conv_bn_act(f"unet_enc{k}", c, nf * 2 ** k) + [{"type": "maxpool", "name": f"unet_pool{k}", "kernel": (2, 2), "stride": (2, 2)}]
+        c = nf * 2 ** k
+    L += conv_bn_act("unet_mid", c, nf * 2 ** depth)
+    c = nf * 2 ** depth
+    for k in reversed(range(depth)):
+        ck = nf * 2 ** k
+        L += [{"type": "deconv2d", "name": f"unet_up{k}", "n_in": c, "n_out": ck, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "updater": u()},
+              merge([f"unet_up{k}", f"unet_enc{k}_act"], name=f"unet_merge{k}")]
+        L += conv_bn_act(f"unet_dec{k}", 2 * ck, ck)
+        c = ck
+    return L + [{"type": "conv2d", "name": "unet_head", "n_in": c, "n_out": n_classes, "kernel": (1, 1), "stride": (1, 1), "padding": (0, 0), "updater": u()},
+                cnn_loss(loss, name="unet_loss")]
+
+
 # ------------------------------------------------------------------ C1: the reference graphs ---------
 def reference_discriminator(lr=0.002, prefix="dis") -> List[Dict]:
     """J:118-165: BN -> Conv5x5 s2 (1->64) -> MaxPool 2x2 s1 -> Conv5x5 s2 (64->128) -> MaxPool -> Dense 1024 -> Output(1, sigmoid, XENT);
@@ -183,19 +240,24 @@ def _act(activation, alpha=None) -> Dict:
     return {"activation": activation} if alpha is None else {"activation": activation, "alpha": alpha}
 
 
-def dcgan_generator(size=64, z=100, nf=64, nc=3, lr=2e-4, beta1=0.5, activation="relu", out_activation="tanh", alpha=None) -> List[Dict]:
+def dcgan_generator(size=64, z=100, nf=64, nc=3, lr=2e-4, beta1=0.5, activation="relu", out_activation="tanh", alpha=None,
+                    residual=False) -> List[Dict]:
     """ConvolutionTranspose2D(4x4)+BatchNorm+ReLU stack, tanh output (SURVEY.md Appendix B).  Input (z,).
-    activation: the ActivationLayers' kind (any engine.ACTS name; alpha as in _act), out_activation: the last deconv's."""
+    activation: the ActivationLayers' kind (any engine.ACTS name; alpha as in _act), out_activation: the last deconv's.
+    residual: one identity residual_block after each up-sampling stage (a ResNet-style generator)."""
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
     n_up = int(math.log2(size)) - 2
     ch = nf * 2 ** (n_up - 1)
+    block = lambda k, c: residual_block(f"gen_res_{k}", c, f"gen_act_{k}", lr, beta1, activation, alpha) if residual else []
     L = [{"type": "ff_to_cnn", "name": "gen_ff2cnn", "to": (1, 1, z)},
          {"type": "deconv2d", "name": "gen_deconv_1", "n_in": z, "n_out": ch, "kernel": (4, 4), "stride": (1, 1), "padding": (0, 0), "has_bias": False, "updater": u()},
          {"type": "batchnorm", "name": "gen_bn_1", "updater": u()}, dict({"type": "activation", "name": "gen_act_1"}, **_act(activation, alpha))]
+    L += block(1, ch)
     for i in range(n_up - 1):
         L += [{"type": "deconv2d", "name": f"gen_deconv_{i + 2}", "n_in": ch, "n_out": ch // 2, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "has_bias": False, "updater": u()},
               {"type": "batchnorm", "name": f"gen_bn_{i + 2}", "updater": u()}, dict({"type": "activation", "name": f"gen_act_{i + 2}"}, **_act(activation, alpha))]
         ch //= 2
+        L += block(i + 2, ch)
     L += [{"type": "deconv2d", "name": f"gen_deconv_{n_up + 1}", "n_in": ch, "n_out": nc, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "updater": u(), **_act(out_activation)}]
     return L
 
@@ -210,7 +272,7 @@ def _loss_keys(loss, out_activation) -> Dict:
 
 
 def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", out_activation="identity", activation="lrelu", alpha=None,
-                        global_pooling=None, patch=False) -> List[Dict]:
+                        global_pooling=None, patch=False, residual=False) -> List[Dict]:
     """Conv(4x4 s2 p1)+LeakyReLU(0.2); (Conv+BatchNorm+LeakyReLU)*; Conv(4x4 s1 p0) -> logit; LossLayer(loss).  Input (nc,size,size).
     loss: "xent" (sigmoid implied), or "mse" (least-squares GAN), "hinge", "wasserstein", ... applied to out_activation(logit).
     activation / alpha: the hidden activation in place of LeakyReLU(0.2) (as in _act).
@@ -218,19 +280,23 @@ def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", o
     loss) in place of the last conv and its LossLayer.
     patch: a PatchGAN critic -- the down-sampling stages stop at the max(4, size/16) map (at most four stride-2 convs), and a 3x3 s1 p1 conv onto
     1 channel and a CnnLossLayer(loss) take the place of the last conv and its LossLayer: one logit and one label per patch (a 4x4 map up to
-    64x64, 8x8 at 128x128)."""
+    64x64, 8x8 at 128x128).
+    residual: one identity residual_block after each down-sampling stage (a ResNet-style critic)."""
     if patch and global_pooling is not None:
         raise ValueError("patch and global_pooling are two different heads")
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
     n_down = int(math.log2(size)) - 2
     if patch:
         n_down = min(n_down, 4)
+    block = lambda k, c, skip: residual_block(f"dis_res_{k}", c, skip, lr, beta1, activation, alpha) if residual else []
     L = [{"type": "conv2d", "name": "dis_conv_1", "n_in": nc, "n_out": nf, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), **_act(activation, alpha), "updater": u()}]
     ch = nf
+    L += block(1, ch, "dis_conv_1")
     for i in range(n_down - 1):
         L += [{"type": "conv2d", "name": f"dis_conv_{i + 2}", "n_in": ch, "n_out": ch * 2, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "has_bias": False, "updater": u()},
               {"type": "batchnorm", "name": f"dis_bn_{i + 2}", "updater": u()}, dict({"type": "activation", "name": f"dis_act_{i + 2}"}, **_act(activation, alpha))]
         ch *= 2
+        L += block(i + 2, ch, f"dis_act_{i + 2}")
     if global_pooling is not None:
         return L + [_global_pooling_spec(global_pooling, name="dis_global_pool"),
                     dict({"type": "output", "name": "dis_output", "n_out": 1, "updater": u()}, **_loss_keys(loss, out_activation))]
@@ -267,9 +333,14 @@ def mlp_discriminator(d=256, hidden=1024, lr=2e-4, beta1=0.5, dropout=None, loss
 # algorithmic MACs per image of the conv/deconv/dense layers (SURVEY.md 8d: F = 2*(4*G_f + 8*D_f))
 def forward_macs(specs: List[Dict], input_shape) -> int:
     c, h, w = input_shape if len(input_shape) == 3 else (input_shape[0], 1, 1)
+    from .engine import resolve_vertices
     macs = 0
-    for s in specs:
+    skips = resolve_vertices(specs)      # the merge vertices' sources by index, as b2g_net_create receives them (ValueError if not spine plus skip)
+    channels = []                        # each layer's output channels
+    for i, s in enumerate(specs):
         t = s["type"]
+        if t == "merge":
+            c += channels[skips[i][0]]
         if t == "conv2d":
             k, st, p = s["kernel"], s.get("stride", (1, 1)), s.get("padding", (0, 0))
             h, w = (h - k[0] + 2 * p[0]) // st[0] + 1, (w - k[1] + 2 * p[1]) // st[1] + 1
@@ -293,4 +364,5 @@ def forward_macs(specs: List[Dict], input_shape) -> int:
             h, w, c = s["to"]
         elif t == "cnn_to_ff":
             c, h, w = c * h * w, 1, 1
+        channels.append(c)
     return macs

@@ -66,8 +66,40 @@ typedef enum {
   B2G_LAYER_DROPOUT = 11,    /* DropoutLayer.Builder(p): p = RETAIN probability in (0, 1], carried in act_alpha; no parameters */
   B2G_LAYER_SUBSAMPLING = 12,    /* SubsamplingLayer.Builder(PoolingType.AVG / SUM / PNORM).kernelSize().stride().padding().pnorm(): b2g_pooling */
   B2G_LAYER_GLOBAL_POOLING = 13, /* GlobalPoolingLayer.Builder(PoolingType).pnorm(): b2g_pooling, output [mb, C] (H = W = 1)                 */
-  B2G_LAYER_CNN_LOSS = 14        /* CnnLossLayer.Builder(LossFunction).activation(..): the loss per pixel of a [mb, C, H, W] map; no parameters  */
+  B2G_LAYER_CNN_LOSS = 14,       /* CnnLossLayer.Builder(LossFunction).activation(..): the loss per pixel of a [mb, C, H, W] map; no parameters  */
+  B2G_LAYER_ELEMENTWISE = 15,    /* ElementWiseVertex(Op) of the spine and an earlier entry's output: b2g_elementwise_op; no parameters       */
+  B2G_LAYER_MERGE = 16           /* MergeVertex: concatenation of the two inputs along dimension 1 (channels / features); no parameters        */
 } b2g_layer_type;
+
+/* Spine-plus-skip graphs (DL4J 1.0.0-beta3 ElementWiseVertex / MergeVertex, recalled; parity unpinned like the rest of the DL4J semantics).
+ * Entry i of the b2g_layer_desc array takes entry i-1's output as its input (entry 0 the net input): the spine.  ELEMENTWISE and MERGE
+ * entries take a second input, the output of an earlier entry j (0 <= j < i), carried in fields these types do not otherwise use:
+ *   act    ELEMENTWISE: the b2g_elementwise_op
+ *   pre_h  j, the skip source
+ *   pre_w  the input order: 0 = (spine, j), 1 = (j, spine) -- DL4J's addVertex("m", v, "enc2", "dec3") in either order.  Only SUBTRACT and MAX's
+ *          tie rule depend on it for ELEMENTWISE; for MERGE it is the channel order of the concatenation.
+ * Every entry still depends on its predecessor, so the array order is the graph's only topological order: DL4J's flattened parameter vector
+ * (topological order) is the array order as for a chain, and the vertices have no parameters.
+ *   ELEMENTWISE: both inputs have the same shape.  y = a + b | a - b | a * b | (a + b) * 0.5 | (a >= b ? a : b) on the inputs (a, b) in input
+ *     order, in fp32, rounded once to the activation type.  Backward with e = the epsilon w.r.t. y:  ADD da = db = e;  SUBTRACT da = e,
+ *     db = -e;  PRODUCT da = e*b, db = e*a;  AVERAGE da = db = e*0.5;  MAX e to the larger input, a tie to the first input (a), 0 to the other.
+ *   MERGE: the inputs have the same H and W; the output has C_a + C_b channels, a's first ([N, F] vectors: the features, in DL4J's order after
+ *     CNN_TO_FF).  In the NHWC layout this is a per-pixel channel concat; its backward splits the epsilon into the two channel slices.
+ *   Gradient at a skip source j: each source has an fp32 buffer [max_batch][its output elements].  The backward visits entries in descending
+ *   order; a vertex writes the skip input's share of its epsilon into the buffer if it is the first (highest) consumer of j and adds it (fp32)
+ *   otherwise, so the order is fixed.  At the top of entry j's backward the buffer is added to the spine epsilon (fp32 sum, rounded once to
+ *   the activation type) before j's own backward runs.
+ *   Launches: one per vertex in the forward; one per vertex plus one per skip source in the backward.  A net without vertices launches what a
+ *   chain always launched.  The fusions that assume one consumer are not taken where the consumer set is larger: a BatchNorm that is a skip
+ *   source is not fused with the ActivationLayer after it, an inference-mode BatchNorm is not folded into a GEMM that is a skip source, and a
+ *   GEMM's input gradient does not premultiply a BatchNorm / activation derivative of a layer that still waits for a skip share.
+ *   B2G_ERR_ARG at b2g_net_create for j outside [0, i), an unknown op or an order outside {0, 1}; B2G_ERR_SHAPE for mismatched shapes;
+ *   B2G_ERR_UNSUPPORTED for a skip source of type LOSS, CNN_LOSS or OUTPUT.
+ *   Not provided: layers on the skip branch (projection shortcuts), vertices of more than two inputs, the net input as a vertex input, and the
+ *   Subset / Scale / Shift / L2 / Stack / Preprocessor vertices. */
+typedef enum {
+  B2G_EW_OP_ADD = 0, B2G_EW_OP_SUBTRACT = 1, B2G_EW_OP_PRODUCT = 2, B2G_EW_OP_AVERAGE = 3, B2G_EW_OP_MAX = 4   /* ElementWiseVertex.Op order */
+} b2g_elementwise_op;
 
 /* DropoutLayer (inverted dropout, DL4J 1.0.0-beta3).  Train-mode forward y = x * m, m = 1/p (fp32 1.0f / p) with probability p, else 0;
  * y = x * (1/p) is formed in fp32 and rounded once to the activation type, dropped elements are +0.  Backward dx = dy * m with the forward's
@@ -207,7 +239,7 @@ typedef enum {
   B2G_LOSS_SQUARED_HINGE = 7, B2G_LOSS_WASSERSTEIN = 8
 } b2g_loss;
 
-/* One layer of a chain-shaped ComputationGraph (every graph in the reference is a chain, J:118-310). */
+/* One layer of a spine-plus-skip ComputationGraph (every graph in the reference is a chain, J:118-310; vertices: B2G_LAYER_ELEMENTWISE). */
 typedef struct {
   int32_t type;                 /* b2g_layer_type */
   char name[B2G_NAME_LEN];      /* DL4J vertex name, e.g. "dis_conv2d_layer_2" */
@@ -519,11 +551,22 @@ int32_t b2g_test_dropout(b2g_ctx* ctx, int32_t precision, uint64_t seed, int32_t
  *                                                                                     -> out0 dz T, out1 loss per group [groups]   (clip_eps)
  *   CNN_SOFTMAX_XENT  in0 logits [groups][rows][cols] T, in1 labels fp32 or NULL (inference: probabilities only)
  *                                                                                     -> out0 dz T, out1 loss per group [groups], out2 probabilities T
+ * The skip-connection vertices (B2G_LAYER_ELEMENTWISE; act = b2g_elementwise_op, groups = the input order 0 / 1, accumulate = add to the
+ * accumulator instead of writing it):
+ *   VERTEX_FWD     in0 spine [n] T, in1 skip [n] T                                    -> out0 y [n] T
+ *   VERTEX_BWD     in0 [spine | skip] [2n] T (the forward inputs), in1 [eps [n] T | acc [n] fp32] (acc: the accumulator's initial value, read
+ *                  when accumulate)                                                   -> out0 the spine's epsilon T (eps's buffer, in place),
+ *                                                                                        out1 acc [n] fp32
+ *   MERGE_FWD      in0 spine [rows][cols] T, in1 skip [rows][C] T                     -> out0 y [rows][cols + C] T (input order: groups)
+ *   MERGE_BWD      in0 eps [rows][cols + C] T, in1 acc's initial value [rows][C] fp32 (when accumulate)
+ *                                                                                     -> out0 the spine's slice [rows][cols] T, out1 acc [rows][C]
+ *   SKIP_ADD       in0 eps [n] T, in1 acc [n] fp32                                    -> out0 eps + acc T (in place)
  * Every output buffer not asked for may be NULL. */
 typedef enum {
   B2G_EW_REDUCE_SPLITS = 0, B2G_EW_REDUCE_MULTI = 1, B2G_EW_COLSUM = 2, B2G_EW_XENT = 3, B2G_EW_SOFTMAX_XENT = 4,
   B2G_EW_ACT_FWD = 5, B2G_EW_ACT_BWD = 6, B2G_EW_MAXPOOL = 7, B2G_EW_UPSAMPLE = 8, B2G_EW_SUMSQ = 9, B2G_EW_LOSS = 10,
-  B2G_EW_ACT_EXT_FWD = 11, B2G_EW_ACT_EXT_BWD = 12, B2G_EW_CNN_XENT = 13, B2G_EW_CNN_SOFTMAX_XENT = 14
+  B2G_EW_ACT_EXT_FWD = 11, B2G_EW_ACT_EXT_BWD = 12, B2G_EW_CNN_XENT = 13, B2G_EW_CNN_SOFTMAX_XENT = 14,
+  B2G_EW_VERTEX_FWD = 15, B2G_EW_VERTEX_BWD = 16, B2G_EW_MERGE_FWD = 17, B2G_EW_MERGE_BWD = 18, B2G_EW_SKIP_ADD = 19
 } b2g_ew_op;
 typedef struct {          /* one split-K sum of a reduce list: dst[i] = sum_s src[s*stride + i], i < n, all offsets in elements of in0 */
   int64_t n, stride, src_off, dst_off;

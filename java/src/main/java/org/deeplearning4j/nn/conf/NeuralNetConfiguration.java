@@ -1,5 +1,5 @@
 // new NeuralNetConfiguration.Builder()....graphBuilder().addInputs().setInputTypes().addLayer().inputPreProcessor().setOutputs().build()  (J:118-165)
-// Collects the chain into b2g_net_config + b2g_layer_desc[]; CnnToFeedForward is auto-inserted before the first dense layer after
+// Collects the graph (a chain, or spine plus skip vertices) into b2g_net_config + b2g_layer_desc[]; CnnToFeedForward is auto-inserted before the first dense layer after
 // a convolutional one, as setInputTypes does in DL4J (SURVEY.md 3.1).
 package org.deeplearning4j.nn.conf;
 
@@ -39,10 +39,14 @@ public class NeuralNetConfiguration {
     public static class GraphBuilder {
         final Builder g; final List<Layer> layers = new ArrayList<>(); final Map<String, FeedForwardToCnnPreProcessor> pre = new HashMap<>(); InputType in;
         GraphBuilder(Builder g) { this.g = g; }
-        public GraphBuilder addInputs(String... names) { return this; }
         public GraphBuilder setInputTypes(InputType... t) { in = t[0]; return this; }
         public GraphBuilder inputPreProcessor(String layer, FeedForwardToCnnPreProcessor p) { pre.put(layer, p); return this; }
-        public GraphBuilder addLayer(String name, Layer l, String... inputs) { l.name = name; layers.add(l); return this; }   // chain graphs only (every graph in the reference is a chain)
+        final Map<String, String[]> inputsOf = new HashMap<>(); final List<String> graphInputs = new ArrayList<>(); boolean hasVertex = false;
+        public GraphBuilder addInputs(String... names) { for (String n : names) graphInputs.add(n); return this; }
+        /** A layer's input is the entry before it (the spine); in a graph with vertices that is checked at build(). */
+        public GraphBuilder addLayer(String name, Layer l, String... inputs) { l.name = name; layers.add(l); inputsOf.put(name, inputs.clone()); return this; }
+        /** ElementWiseVertex / MergeVertex: one input must be the entry right before the vertex, the other an earlier one (spine plus skip). */
+        public GraphBuilder addVertex(String name, Layer v, String... inputs) { v.name = name; layers.add(v); inputsOf.put(name, inputs.clone()); hasVertex = true; return this; }
         public GraphBuilder setOutputs(String... names) { return this; }
         public ComputationGraphConfiguration build() { return new ComputationGraphConfiguration(this); }
     }
@@ -58,6 +62,30 @@ public class NeuralNetConfiguration {
                 if (p != null) { Layer r = new Layer(); r.type = 9; r.name = l.name + "_ff2cnn"; r.preH = p.h; r.preW = p.w; r.preC = p.c; r.act = 0; out.add(r); cnn = true; }
                 if (cnn && (l.type == 3 || l.type == 7)) { Layer r = new Layer(); r.type = 10; r.name = l.name + "_cnn2ff"; r.act = 0; out.add(r); cnn = false; }
                 out.add(l);
+            }
+            // A graph with vertices is resolved and checked: every layer's input must be the layer added before it (the graph input for the
+            // first), so nothing sits on a skip branch, and each vertex's inputs become (skip source index in preH, input order in preW).
+            // IllegalStateException for anything but spine plus skip.  Graphs without vertices are the chains they always were.
+            if (!b.hasVertex) return out;
+            for (int k = 0; k < b.layers.size(); ++k) {
+                Layer l = b.layers.get(k); String[] ins = b.inputsOf.get(l.name);
+                if (l.type == 15 || l.type == 16) continue;
+                String prev = k == 0 ? null : b.layers.get(k - 1).name;
+                boolean ok = ins.length == 0 || (ins.length == 1 && (k == 0 ? b.graphInputs.contains(ins[0]) : ins[0].equals(prev)));
+                if (!ok) throw new IllegalStateException("layer " + l.name + ": its input must be " + (k == 0 ? "the graph input" : prev)
+                                                         + " (spine plus skip; layers on a skip branch are not supported)");
+            }
+            for (int i = 0; i < out.size(); ++i) {
+                Layer v = out.get(i); String[] ins = b.inputsOf.get(v.name);
+                if (v.type != 15 && v.type != 16) continue;
+                if (ins == null || ins.length != 2 || i == 0) throw new IllegalStateException("vertex " + v.name + ": needs two inputs, one of them the layer before it");
+                String spine = out.get(i - 1).name; int order; String other;
+                if (ins[0].equals(spine)) { order = 0; other = ins[1]; } else if (ins[1].equals(spine)) { order = 1; other = ins[0]; }
+                else throw new IllegalStateException("vertex " + v.name + ": one input must be " + spine + " (spine plus skip)");
+                int j = -1;
+                for (int k = 0; k < i; ++k) if (out.get(k).name.equals(other)) { if (j >= 0) throw new IllegalStateException("vertex " + v.name + ": " + other + " is ambiguous"); j = k; }
+                if (j < 0) throw new IllegalStateException("vertex " + v.name + ": " + other + " is not an earlier layer");
+                v.preH = j; v.preW = order;
             }
             return out;
         }
