@@ -1593,15 +1593,48 @@ extern "C" int32_t b2g_net_average_parameters(b2g_net* n) {
   net_refresh_shadow(n);
   CU(cudaStreamSynchronize(s)); return 0;
 }
+
+// ------------------------------------------------------------------ test hooks ----------------------------
+namespace {
+// Every device buffer and event of one test-hook call, released on every return.  Copies run on stream s; T is the call's precision.
+struct HookMem {
+  cudaStream_t s; int prec;
+  std::vector<void*> bufs; std::vector<cudaEvent_t> events;
+  HookMem(cudaStream_t s_, int prec_) : s(s_), prec(prec_) {}
+  HookMem(const HookMem&) = delete; HookMem& operator=(const HookMem&) = delete;
+  ~HookMem() { for (void* p : bufs) cudaFree(p); for (cudaEvent_t e : events) cudaEventDestroy(e); }
+  // count es-byte elements, off elements past a 256-byte aligned allocation (as a layer's W and dW sit in the flattened parameter vectors)
+  int32_t dev(size_t count, size_t es, void** p, size_t off = 0) {
+    void* b = nullptr; *p = nullptr; CU(cudaMalloc(&b, es * (count + off) + 16)); bufs.push_back(b); *p = (char*)b + es * off; return 0; }
+  // fp32 host -> fp32 device; h null: the buffer only
+  int32_t upF(const float* h, size_t count, float** p, size_t off = 0) {
+    B2(dev(count, 4, (void**)p, off)); if (h) CU(cudaMemcpyAsync(*p, h, 4 * count, cudaMemcpyHostToDevice, s)); return 0; }
+  // fp32 device -> T device (bf16: rounded)
+  int32_t toT(const float* f, void* t, size_t count) {
+    if (prec == PREC_F32) CU(cudaMemcpyAsync(t, f, 4 * count, cudaMemcpyDeviceToDevice, s)); else k_cast_f32_to_bf16(f, (__nv_bfloat16*)t, count, s); return 0; }
+  // fp32 host -> T device (bf16: rounded on the device from an fp32 copy); h null: the buffer only
+  int32_t upT(const float* h, size_t count, void** p, size_t off = 0) {
+    B2(dev(count, prec_size(prec), p, off)); if (!h) return 0;
+    if (prec == PREC_F32) { CU(cudaMemcpyAsync(*p, h, 4 * count, cudaMemcpyHostToDevice, s)); return 0; }
+    float* f = nullptr; B2(upF(h, count, &f)); return toT(f, *p, count); }
+  // fp32 device -> host; h null: nothing
+  int32_t downF(float* h, const float* d, size_t count) { if (h) CU(cudaMemcpyAsync(h, d, 4 * count, cudaMemcpyDeviceToHost, s)); return 0; }
+  // T device -> fp32 host (bf16: widened on the device into an fp32 copy); h null: nothing
+  int32_t downT(float* h, const void* d, size_t count) {
+    if (!h || prec == PREC_F32) return downF(h, (const float*)d, count);
+    float* f = nullptr; B2(upF(nullptr, count, &f)); k_nhwc_to_nchw_f32(prec, d, f, 1, 1, (int)count, s); return downF(h, f, count); }
+  int32_t event(cudaEvent_t* e) { CU(cudaEventCreate(e)); events.push_back(*e); return 0; }
+};
+}  // namespace
+
 extern "C" int32_t b2g_ctx_allreduce_test(b2g_ctx* c, float* host, int64_t n) {
   if (!c || !host || n < 1) return fail(B2G_ERR_ARG, "null"); if (!c->comm) return fail(B2G_ERR_NCCL, "no communicator"); CU(cudaSetDevice(c->device));
-  float* d = nullptr; CU(cudaMalloc(&d, sizeof(float) * n));
-  CU(cudaMemcpyAsync(d, host, sizeof(float) * n, cudaMemcpyHostToDevice, c->stream));
+  HookMem m(c->stream, PREC_F32); float* d = nullptr;
+  B2(m.upF(host, (size_t)n, &d));
   NC(g_nccl.ar(d, d, (size_t)n, 7, 0, c->comm, c->stream));
-  CU(cudaMemcpyAsync(host, d, sizeof(float) * n, cudaMemcpyDeviceToHost, c->stream)); CU(cudaStreamSynchronize(c->stream)); cudaFree(d); return 0;
+  B2(m.downF(host, d, (size_t)n)); CU(cudaStreamSynchronize(c->stream)); return 0;
 }
 
-// ------------------------------------------------------------------ kernel-level test hook ----------------
 // The tile-width / grid / split-count overrides of the tensor-core kernels hold for the hook's own launch loop only: reset right after it, and on
 // every early return.
 struct TcTestSchedule {
@@ -1609,146 +1642,151 @@ struct TcTestSchedule {
   ~TcTestSchedule() { reset(); }
   void reset() { g_tc_test_bn = 0; g_tc_test_max_ctas = 0; g_tc_test_per_tap = 0; g_tc_test_splits = 0; }
 };
+// What b2g_test_conv_ex takes for one (impl, kind): the precision and shapes its kernel runs, and the options it accepts.  Bits 1-3 of opts
+// are the fused epilogues EPI_STATS / EPI_BNBWD / EPI_ACTBWD; bit 0 stands for an epi value no kernel has.
+enum : unsigned { CO_STATS = 1u << EPI_STATS, CO_BNBWD = 1u << EPI_BNBWD, CO_ACTBWD = 1u << EPI_ACTBWD, CO_BIAS_ACT = 1u << 4, CO_SCALE = 1u << 5,
+                  CO_POFF = 1u << 6, CO_BN = 1u << 7, CO_MAX_CTAS = 1u << 8, CO_PER_TAP = 1u << 9, CO_W_MN = 1u << 10, CO_SPLITS = 1u << 11,
+                  CO_DEFER = 1u << 12, CO_DB = 1u << 13 };
+struct ConvHookImpl {
+  const char* kernel;                 // names the kernels in a refusal
+  bool bf16, tma;                     // BF16 only; needs the tensor-map encoder (c->tc_ok)
+  struct { bool (*shape)(const ConvGeom&); unsigned opts; } kind[3];      // fprop, dgrad, wgrad: the geometries it runs, the options it takes
+};
+static bool any_shape(const ConvGeom&) { return true; }
+static bool dense_bwd_shape(const ConvGeom& g) { return dense_small_o_supported(g) || dense_small_k_supported(g); }
+static bool tc_edge_conv_shape(const ConvGeom& g) { return edge_conv_small_cin_supported(g) && tc_edge_conv_supported(g); }
+static bool tc_edge_wgrad_shape(const ConvGeom& g) { return edge_wgrad_small_cin_supported(g) && tc_edge_wgrad_supported(g); }
+static const unsigned CO_TC = CO_STATS | CO_BNBWD | CO_ACTBWD | CO_BIAS_ACT | CO_SCALE | CO_BN | CO_MAX_CTAS | CO_PER_TAP;
+static const ConvHookImpl kConvHook[6] = {
+  {"SIMT kernel", false, false, {{any_shape, CO_BIAS_ACT | CO_SCALE | CO_POFF}, {any_shape, CO_BIAS_ACT | CO_SCALE | CO_POFF}, {any_shape, CO_POFF}}},
+  {"tensor-core kernel (BF16, a working tensor-map encoder)", true, true,
+   {{tc_fprop_supported, CO_TC | CO_W_MN}, {tc_dgrad_supported, CO_TC}, {tc_wgrad_supported, CO_POFF | CO_SPLITS | CO_DEFER}}},
+  {"skinny-layer kernel (<= 4 image channels)", false, false,
+   {{edge_conv_small_cin_supported, CO_BIAS_ACT | CO_POFF}, {edge_deconv_small_c_supported, CO_BIAS_ACT | CO_POFF}, {edge_wgrad_small_cin_supported, CO_POFF}}},
+  // kind 1 is the pixel-shuffle deconv: the training step runs it wherever tc_deconv_ps_supported holds, also where the SIMT kernel has no
+  // variant (O > 128)
+  {"skinny-layer tensor-core kernel (BF16, <= 4 image channels, a working tensor-map encoder)", true, true,
+   {{tc_edge_conv_shape, CO_BIAS_ACT | CO_MAX_CTAS}, {tc_deconv_ps_supported, CO_ACTBWD | CO_BIAS_ACT | CO_MAX_CTAS},
+    {tc_edge_wgrad_shape, CO_POFF | CO_SPLITS | CO_DEFER | CO_DB}}},
+  {"dense kernel (1x1 geometry: <= 4 output units, or a short reduction in the input / weight gradient)", false, false,
+   {{dense_small_o_supported, CO_BIAS_ACT | CO_POFF}, {dense_bwd_shape, CO_BIAS_ACT | CO_POFF}, {dense_bwd_shape, CO_POFF}}},
+  {"few-output conv kernel (BF16, O <= 4, C % 8 == 0, k x k)", true, false,
+   {{head_conv_supported, CO_BIAS_ACT | CO_POFF}, {head_conv_supported, CO_BIAS_ACT | CO_POFF}, {head_conv_supported, CO_POFF | CO_SPLITS | CO_DB}}},
+};
+static constexpr int ik(int impl, int kind) { return 3 * impl + kind; }
+
 extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int32_t precision, const b2g_conv_geom* gg, const float* a_host, const float* b_host, float* out, int32_t iters, float* ms_per_iter,
                                     b2g_test_conv_opts* opt) {
-  if (!c || !gg || !a_host || !b_host || !out) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(c->device));
+  if (!c || !gg || !a_host || !b_host || !out) return fail(B2G_ERR_ARG, "null");
+  if (kind < 0 || kind > 2 || impl < 0 || impl > 5) return fail(B2G_ERR_ARG, "kind %d / impl %d: kind is 0-2, impl 0-5", kind, impl);
+  CU(cudaSetDevice(c->device));
   cudaStream_t s = c->stream; int prec = precision == B2G_PREC_BF16 ? PREC_BF16 : PREC_F32; size_t ts = prec_size(prec);
   ConvGeom g{gg->n, gg->h, gg->w, gg->c, gg->oh, gg->ow, gg->o, gg->kh, gg->kw, gg->sh, gg->sw, gg->ph, gg->pw};
   size_t nx = (size_t)g.N * g.H * g.W * g.C, ny = (size_t)g.N * g.OH * g.OW * g.O, nw = (size_t)g.O * g.KH * g.KW * g.C;
   // operands: kind 0: a = x (NHWC), b = w [O][KH][KW][C] -> out y ; kind 1: a = dy, b = w -> out dx ; kind 2: a = x, b = dy -> out dw (fp32)
   size_t na = kind == 1 ? ny : nx, nb = kind == 2 ? ny : nw, no = kind == 0 ? ny : kind == 1 ? nx : nw;
   const int oc = kind == 0 ? g.O : g.C;       // channels of the result (kinds 0 / 1)
-  if (impl == 1) {
-    if (prec != PREC_BF16 || !c->tc_ok) return fail(B2G_ERR_UNSUPPORTED, "tensor-core kernels need BF16 precision and a working tensor-map encoder");
-    bool ok = kind == 0 ? tc_fprop_supported(g) : kind == 1 ? tc_dgrad_supported(g) : tc_wgrad_supported(g);
-    if (!ok) return fail(B2G_ERR_UNSUPPORTED, "no tensor-core kernel for this shape");
-  }
-  const bool tc_conv = impl == 1 && kind != 2, ps = impl == 3 && kind == 1;     // the launches of tc_conv_kernel (ps: its pixel-shuffle form)
-  const bool edge_fwd = impl == 3 && kind == 0, tc_wg = kind == 2 && (impl == 1 || impl == 3);   // tc_edge_conv_kernel; the tensor-core weight gradients
-  // the SIMT, skinny-layer and dense kernels; gemm_epi: those whose production wrapper takes bias / activation (k_dense_small_o_dgrad and the
-  // weight gradients have none: as in gemm_dgrad, a dense input gradient with an epilogue runs the short-reduction kernel)
-  const bool gemm = impl == 0 || impl == 2 || impl == 4 || impl == 5;
-  // impl 5 = the few-output conv kernels (kernels_head.cu), BF16 only
-  if (impl == 5 && (prec != PREC_BF16 || !head_conv_supported(g))) return fail(B2G_ERR_UNSUPPORTED, "no few-output conv kernel (impl 5: BF16, O <= 4, C %% 8 == 0, k x k) for this shape");
-  const bool gemm_epi = gemm && kind != 2 && !(impl == 4 && kind == 1 && !dense_small_k_supported(g));
-  if (opt && gemm) {
-    if (opt->epi || (!gemm_epi && (opt->bias || opt->scale || opt->act)))
-      return fail(B2G_ERR_UNSUPPORTED, "impl %d kind %d: no epilogue (bias / activation: impl 0 / 2 kind 0 / 1, impl 4 kind 0 and the short-reduction kind 1; no fused BatchNorm epilogue)", impl, kind);
-    if (opt->scale && impl != 0) return fail(B2G_ERR_UNSUPPORTED, "scale applies to the SIMT fprop / dgrad (impl 0) and the tensor-core kernels");
-  }
-  else if (opt && !tc_conv && !ps && !edge_fwd && (opt->epi || opt->bias || opt->scale || opt->act))
-    return fail(B2G_ERR_UNSUPPORTED, "epilogue options apply to the tensor-core fprop / dgrad kernels (impl 1, kind 0 / 1), the tensor-core skinny-layer conv and pixel-shuffle deconv (impl 3, kind 0 / 1) and the SIMT / skinny-layer / dense kernels (impl 0 / 2 / 4)");
-  if (opt && edge_fwd && (opt->epi || opt->scale)) return fail(B2G_ERR_UNSUPPORTED, "the tensor-core skinny-layer conv has bias and activation only");
-  const int poff = opt ? opt->param_offset : 0;
-  if (poff < 0 || (poff && !gemm && !tc_wg))
-    return fail(B2G_ERR_UNSUPPORTED, "param_offset %d: applies to the SIMT / skinny-layer / dense kernels (impl 0 / 2 / 4) and the tensor-core weight gradients (kind 2, impl 1 / 3)", poff);
-  if (opt && ps && (opt->scale || (opt->epi != EPI_PLAIN && opt->epi != EPI_ACTBWD)))
-    return fail(B2G_ERR_UNSUPPORTED, "the pixel-shuffle deconv has bias, activation and the activation-backward epilogue only");
-  const int force_bn = opt ? opt->bn : 0, max_ctas = opt ? opt->max_ctas : 0;
-  const bool poison = opt && opt->poison, w_mn = opt && opt->w_mn, per_tap = opt && opt->per_tap;
-  if (per_tap && !tc_conv) return fail(B2G_ERR_UNSUPPORTED, "per_tap applies to the tensor-core fprop / dgrad kernels (impl 1, kind 0 / 1)");
-  if (force_bn && (!tc_conv || (force_bn != 64 && force_bn != 128) || oc % force_bn))
-    return fail(B2G_ERR_UNSUPPORTED, "bn %d: the tensor-core fprop / dgrad tile is 64 or 128 columns and must divide the %d output channels", force_bn, oc);
-  if (max_ctas < 0 || (max_ctas && !tc_conv && !ps && !edge_fwd))
-    return fail(B2G_ERR_UNSUPPORTED, "max_ctas %d: a grid cap applies to tc_conv_kernel and tc_edge_conv_kernel launches only", max_ctas);
-  const int force_splits = opt ? opt->splits : 0;
-  const bool head_wg = impl == 5 && kind == 2;
-  if (force_splits < 0 || (force_splits && !tc_wg && !head_wg)) return fail(B2G_ERR_UNSUPPORTED, "splits %d: a forced split count applies to the tensor-core weight gradients (kind 2, impl 1 / 3)", force_splits);
-  if (w_mn && (impl != 1 || kind != 0 || g.KH != 1 || g.KW != 1)) return fail(B2G_ERR_UNSUPPORTED, "w_mn: the [C][O] weight operand exists for the 1x1 tensor-core fprop only");
-  const bool defer = opt && opt->defer; float* db_host = opt ? opt->db : nullptr;
-  if (defer && !(kind == 2 && (impl == 1 || impl == 3))) return fail(B2G_ERR_UNSUPPORTED, "defer applies to the tensor-core weight gradients (kind 2, impl 1 / 3)");
-  if (db_host && !(kind == 2 && (impl == 3 || impl == 5))) return fail(B2G_ERR_UNSUPPORTED, "db is the edge tensor-core weight gradient's bias column (kind 2, impl 3)");
-  // impl 2 = the SIMT skinny-layer kernels (kernels_edge.cu), impl 3 = their tensor-core counterparts; both need <= 4 image channels (g.C)
-  if (impl == 2 || impl == 3) {
-    bool ok = kind == 0 ? edge_conv_small_cin_supported(g) : kind == 1 ? edge_deconv_small_c_supported(g) : edge_wgrad_small_cin_supported(g);
-    if (impl == 3) ok = ok && prec == PREC_BF16 && c->tc_ok && (kind == 0 ? tc_edge_conv_supported(g) : kind == 1 ? tc_deconv_ps_supported(g) : tc_edge_wgrad_supported(g));
-    // the training step runs the pixel-shuffle deconv wherever tc_deconv_ps_supported holds, also where the SIMT kernel has no variant (O > 128)
-    if (ps) ok = prec == PREC_BF16 && c->tc_ok && tc_deconv_ps_supported(g);
-    if (!ok) return fail(B2G_ERR_UNSUPPORTED, "no skinny-layer kernel (impl %d) for this shape", impl);
-  }
-  // impl 4 = the dense (1x1 geometry) SIMT kernels: <= 4 output units (D-last) or a short reduction (G-first in its dgrad form)
-  if (impl == 4 && !(dense_small_o_supported(g) || (dense_small_k_supported(g) && kind != 0))) return fail(B2G_ERR_UNSUPPORTED, "no dense kernel for this shape");
-  float *fa = nullptr, *fb = nullptr, *fo = nullptr, *scratch = nullptr; void *ta = nullptr, *tb = nullptr, *to = nullptr; __nv_bfloat16* wps = nullptr;
-  float *d_bias = nullptr, *d_scale = nullptr, *d_coef = nullptr, *d_auxf = nullptr; __nv_bfloat16 *d_aux = nullptr, *d_aux2 = nullptr; unsigned long long* d_acc = nullptr;
+  const ConvHookImpl& im = kConvHook[impl];
+  if ((im.bf16 && prec != PREC_BF16) || (im.tma && !c->tc_ok) || !im.kind[kind].shape(g))
+    return fail(B2G_ERR_UNSUPPORTED, "impl %d kind %d: no %s for this shape", impl, kind, im.kernel);
+  const b2g_test_conv_opts none{}; const b2g_test_conv_opts& o = opt ? *opt : none;
+  const struct { unsigned flag; bool set; const char* what; } asked[] = {
+    {o.epi >= EPI_STATS && o.epi <= EPI_ACTBWD ? 1u << o.epi : 1u, o.epi != 0,
+     "fused epilogue (epi 1-3: the tensor-core fprop / dgrad, impl 1 kind 0 / 1; epi 3: the pixel-shuffle deconv, impl 3 kind 1)"},
+    {CO_BIAS_ACT, o.bias || o.act, "bias / activation (kinds 0 / 1; impl 4 kind 1 on its short-reduction kernel)"},
+    {CO_SCALE, o.scale != nullptr, "scale (the SIMT and tensor-core fprop / dgrad, impl 0 / 1 kind 0 / 1)"},
+    {CO_POFF, o.param_offset != 0, "param_offset (impl 0 / 2 / 4 / 5, and the tensor-core weight gradients, impl 1 / 3 kind 2)"},
+    {CO_BN, o.bn != 0, "bn (the tile width of the tensor-core fprop / dgrad, impl 1 kind 0 / 1)"},
+    {CO_MAX_CTAS, o.max_ctas != 0, "max_ctas (a grid cap of tc_conv_kernel and tc_edge_conv_kernel launches, impl 1 / 3 kind 0 / 1)"},
+    {CO_PER_TAP, o.per_tap != 0, "per_tap (the tensor-core fprop / dgrad, impl 1 kind 0 / 1)"},
+    {CO_W_MN, o.w_mn != 0, "w_mn (the [C][O] weight operand of the 1x1 tensor-core fprop, impl 1 kind 0)"},
+    {CO_SPLITS, o.splits != 0, "splits (a forced split count of the weight gradients of impl 1 / 3 / 5)"},
+    {CO_DEFER, o.defer != 0, "defer (the tensor-core weight gradients, impl 1 / 3 kind 2)"},
+    {CO_DB, o.db != nullptr, "db (the bias column of the edge tensor-core and few-output weight gradients, impl 3 / 5 kind 2)"},
+  };
+  for (const auto& a : asked) if (a.set && !(im.kind[kind].opts & a.flag)) return fail(B2G_ERR_UNSUPPORTED, "impl %d kind %d takes no %s", impl, kind, a.what);
+  if (o.param_offset < 0 || o.max_ctas < 0 || o.splits < 0)
+    return fail(B2G_ERR_UNSUPPORTED, "param_offset %d, max_ctas %d, splits %d: none may be negative", o.param_offset, o.max_ctas, o.splits);
+  if (o.bn && ((o.bn != 64 && o.bn != 128) || oc % o.bn))
+    return fail(B2G_ERR_UNSUPPORTED, "bn %d: the tensor-core fprop / dgrad tile is 64 or 128 columns and must divide the %d output channels", o.bn, oc);
+  // as in gemm_dgrad, a dense input gradient with an epilogue runs the short-reduction kernel
+  if (impl == 4 && kind == 1 && (o.bias || o.act) && !dense_small_k_supported(g))
+    return fail(B2G_ERR_UNSUPPORTED, "impl 4 kind 1: bias / activation run on the short-reduction kernel only, which has no variant for this shape");
+  if (o.w_mn && (g.KH != 1 || g.KW != 1)) return fail(B2G_ERR_UNSUPPORTED, "w_mn: the [C][O] weight operand exists for the 1x1 tensor-core fprop only");
+  const bool gemm = impl == 0 || impl == 2 || impl >= 4, tc_wg = kind == 2 && (impl == 1 || impl == 3);    // which globals name the launch
+  const int force_splits = o.splits;
   size_t sc = std::max(std::max(std::max(k_simt_wgrad_scratch_floats(g), k_tc_wgrad_scratch_floats(g)), std::max(k_edge_wgrad_scratch_floats(g), k_tc_edge_wgrad_scratch_floats(g))), k_dense_small_o_wgrad_scratch_floats(g)) + 16;
   // a forced split count needs room for that many partials: [splits][dw] (tc_wgrad_kernel), [ctas][dw] + [ctas][db] with ctas <= splits (tc_edge_wgrad_kernel)
   if (force_splits) sc = std::max(sc, (size_t)force_splits * (impl == 1 || impl == 5 ? nw : (size_t)64 * 16 * g.C + 64) + 16);
   if (impl == 5) sc = std::max(sc, std::max(k_head_wgrad_scratch_floats(g), k_colsum_scratch_floats(g.O)) + 16);
-  // param_offset: the fp32 weight operand (FP32, kinds 0 / 1) and the weight gradient (kind 2) start poff elements past the 256-byte aligned
-  // cudaMalloc base, as W and dW do in a net's flattened parameter / gradient vectors
-  const size_t woff = (prec == PREC_F32 && kind != 2) ? (size_t)poff : 0, dwoff = kind == 2 ? (size_t)poff : 0;
-  CU(cudaMalloc(&fa, 4 * na)); CU(cudaMalloc(&fb, 4 * nb)); CU(cudaMalloc(&fo, 4 * (no + dwoff))); CU(cudaMalloc(&scratch, 4 * sc));
-  CU(cudaMalloc(&ta, ts * na)); CU(cudaMalloc(&tb, ts * nb + 4 * woff)); CU(cudaMalloc(&to, ts * no));
-  float* const fres = fo + dwoff;           // the fp32 result: dw (kind 2), or the widened output (kinds 0 / 1)
-  void* const tbase = tb; tb = (float*)tb + woff;
-  CU(cudaMemcpyAsync(fa, a_host, 4 * na, cudaMemcpyHostToDevice, s)); CU(cudaMemcpyAsync(fb, b_host, 4 * nb, cudaMemcpyHostToDevice, s));
-  if (prec == PREC_BF16) { k_cast_f32_to_bf16(fa, (__nv_bfloat16*)ta, na, s); k_cast_f32_to_bf16(fb, (__nv_bfloat16*)tb, nb, s); }
-  else { CU(cudaMemcpyAsync(ta, fa, 4 * na, cudaMemcpyDeviceToDevice, s)); CU(cudaMemcpyAsync(tb, fb, 4 * nb, cudaMemcpyDeviceToDevice, s)); }
-  if (impl == 3 && kind == 1) { CU(cudaMalloc(&wps, 2 * k_tc_deconv_ps_weight_elems(g))); k_pack_deconv_ps(fb, wps, g.O, g.C, s); }
-  float *d_db = nullptr, *dbres = nullptr; int db_written = 0;
-  if (db_host) { CU(cudaMalloc(&d_db, 4 * ((size_t)g.O + dwoff))); dbres = d_db + dwoff; }      // db sits poff elements past the aligned base, as dw does
-  ReduceList rl{}; ReduceList* prl = defer ? &rl : nullptr;
-  TcEpi epi{}; const TcEpi* pe = nullptr; const float* bias = nullptr; int act = 0; float alpha = 0.f; int groups = 1;
-  if (opt && (tc_conv || ps || edge_fwd)) {
-    groups = opt->groups > 0 ? opt->groups : 1; act = opt->act; alpha = opt->alpha;
-    if (opt->bias) { CU(cudaMalloc(&d_bias, 4 * oc)); CU(cudaMemcpyAsync(d_bias, opt->bias, 4 * oc, cudaMemcpyHostToDevice, s)); bias = d_bias; }
-    if (opt->scale) { CU(cudaMalloc(&d_scale, 4 * oc)); CU(cudaMemcpyAsync(d_scale, opt->scale, 4 * oc, cudaMemcpyHostToDevice, s)); }
-    epi.mode = opt->epi; epi.scale = d_scale; epi.imgs_per_group = g.N / groups; epi.act = opt->act; epi.alpha = opt->alpha;
-    if (opt->epi == EPI_STATS || opt->epi == EPI_BNBWD) { CU(cudaMalloc(&d_acc, 8 * k_bn_acc_elems(oc, groups))); epi.acc = d_acc; }
-    if (opt->epi == EPI_BNBWD || opt->epi == EPI_ACTBWD) {
-      if (!opt->aux) return fail(B2G_ERR_ARG, "epilogue %d needs aux", opt->epi);
-      CU(cudaMalloc(&d_auxf, 4 * no)); CU(cudaMalloc(&d_aux, 2 * no)); CU(cudaMemcpyAsync(d_auxf, opt->aux, 4 * no, cudaMemcpyHostToDevice, s)); k_cast_f32_to_bf16(d_auxf, d_aux, no, s); epi.aux = d_aux;
-    }
-    if (opt->epi == EPI_BNBWD) {      // aux = the BatchNorm(+activation) output y, aux2 = its input z
-      if (!opt->aux2) return fail(B2G_ERR_ARG, "epilogue 2 needs aux2 (the BatchNorm input z)");
-      CU(cudaMalloc(&d_coef, 4 * no)); CU(cudaMalloc(&d_aux2, 2 * no)); CU(cudaMemcpyAsync(d_coef, opt->aux2, 4 * no, cudaMemcpyHostToDevice, s)); k_cast_f32_to_bf16(d_coef, d_aux2, no, s); epi.aux2 = d_aux2;
-    }
-    if (opt->epi || opt->scale) pe = &epi;
+  // param_offset: the fp32 weight operand (FP32, kinds 0 / 1) and the weight gradient and db (kind 2) start param_offset elements past the
+  // 256-byte aligned base of their allocation, as W and dW do in a net's flattened parameter / gradient vectors
+  const size_t woff = (prec == PREC_F32 && kind != 2) ? (size_t)o.param_offset : 0, dwoff = kind == 2 ? (size_t)o.param_offset : 0;
+  // the fp32 copies, then the T operands: the layout bench.py's per-kernel times rest on (a different order moves some by ~3% on an H100)
+  HookMem m(s, prec);
+  float *fa, *fb, *fres, *scratch, *dbres = nullptr, *bias = nullptr, *scale = nullptr; void *ta, *tb, *to; __nv_bfloat16* wps = nullptr;
+  B2(m.upF(a_host, na, &fa)); B2(m.upF(b_host, nb, &fb)); B2(m.upF(nullptr, no, &fres, dwoff)); B2(m.upF(nullptr, sc, &scratch));
+  B2(m.dev(na, ts, &ta)); B2(m.dev(nb, ts, &tb, woff)); B2(m.dev(no, ts, &to)); B2(m.toT(fa, ta, na)); B2(m.toT(fb, tb, nb));
+  if (impl == 3 && kind == 1) { B2(m.dev(k_tc_deconv_ps_weight_elems(g), 2, (void**)&wps)); k_pack_deconv_ps(fb, wps, g.O, g.C, s); }    // its packed weight operand
+  if (o.db) B2(m.upF(nullptr, g.O, &dbres, dwoff));
+  if (o.bias) B2(m.upF(o.bias, oc, &bias));
+  if (o.scale) B2(m.upF(o.scale, oc, &scale));
+  const int groups = o.groups > 0 ? o.groups : 1, act = o.act; const float alpha = o.alpha;
+  TcEpi epi{}; unsigned long long* d_acc = nullptr;
+  epi.mode = o.epi; epi.scale = scale; epi.imgs_per_group = g.N / groups; epi.act = act; epi.alpha = alpha;
+  if (o.epi == EPI_STATS || o.epi == EPI_BNBWD) { B2(m.dev(k_bn_acc_elems(oc, groups), 8, (void**)&d_acc)); epi.acc = d_acc; }
+  if (o.epi == EPI_BNBWD || o.epi == EPI_ACTBWD) {
+    if (!o.aux) return fail(B2G_ERR_ARG, "epilogue %d needs aux", o.epi);
+    void* aux = nullptr; B2(m.upT(o.aux, no, &aux)); epi.aux = (const __nv_bfloat16*)aux;
   }
-  if (opt && gemm_epi) {
-    act = opt->act; alpha = opt->alpha;
-    if (opt->bias) { CU(cudaMalloc(&d_bias, 4 * oc)); CU(cudaMemcpyAsync(d_bias, opt->bias, 4 * oc, cudaMemcpyHostToDevice, s)); bias = d_bias; }
-    if (opt->scale) { CU(cudaMalloc(&d_scale, 4 * oc)); CU(cudaMemcpyAsync(d_scale, opt->scale, 4 * oc, cudaMemcpyHostToDevice, s)); }
+  if (o.epi == EPI_BNBWD) {      // aux = the BatchNorm(+activation) output y, aux2 = its input z
+    if (!o.aux2) return fail(B2G_ERR_ARG, "epilogue 2 needs aux2 (the BatchNorm input z)");
+    void* aux2 = nullptr; B2(m.upT(o.aux2, no, &aux2)); epi.aux2 = (const __nv_bfloat16*)aux2;
   }
-  cudaEvent_t e0, e1; CU(cudaEventCreate(&e0)); CU(cudaEventCreate(&e1));
-  int reps = iters < 1 ? 1 : iters; int rc = 0;
+  const TcEpi* pe = o.epi || o.scale ? &epi : nullptr;
+  const __nv_bfloat16 *ba = (const __nv_bfloat16*)ta, *bb = (const __nv_bfloat16*)tb; __nv_bfloat16* bo = (__nv_bfloat16*)to;
+  ReduceList rl{}; ReduceList* prl = o.defer ? &rl : nullptr;
+  cudaEvent_t e0, e1; B2(m.event(&e0)); B2(m.event(&e1));
+  int reps = iters < 1 ? 1 : iters; int rc = 0, db_written = 0;
   g_tc_last_kernel = ""; g_tc_last_slab = false; g_tc_last_splits = 0; g_gemm_last_kernel = ""; g_gemm_last_splits = 0;
-  TcTestSchedule schedule(force_bn, max_ctas, per_tap, force_splits);
+  TcTestSchedule schedule(o.bn, o.max_ctas, o.per_tap != 0, force_splits);
   for (int it = -1; it < reps; ++it) {       // it = -1: warm-up
     if (it == 0) CU(cudaEventRecord(e0, s));
     if (d_acc) CU(cudaMemsetAsync(d_acc, 0, 8 * k_bn_acc_elems(oc, groups), s));
-    if (poison) CU(cudaMemsetAsync(to, 0xFF, ts * no, s));       // a tile this launch does not write reads back as NaN, not as the warm-up's values
-    if (poison && kind == 2) { CU(cudaMemsetAsync(fres, 0xFF, 4 * no, s)); CU(cudaMemsetAsync(scratch, 0xFF, 4 * sc, s)); }   // fp32 NaN: dw and the split-K partials
-    if (poison && dbres) CU(cudaMemsetAsync(dbres, 0xFF, 4 * (size_t)g.O, s));
-    if (impl == 5) {      // the weight gradient's split sums as the backward pass runs them: one reduce-list launch; db = the column sums of dy
-      if (kind == 0) k_head_fwd(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s);
-      else if (kind == 1) k_head_dgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s);
-      else {
+    if (o.poison) CU(cudaMemsetAsync(to, 0xFF, ts * no, s));       // a tile this launch does not write reads back as NaN, not as the warm-up's values
+    if (o.poison && kind == 2) { CU(cudaMemsetAsync(fres, 0xFF, 4 * no, s)); CU(cudaMemsetAsync(scratch, 0xFF, 4 * sc, s)); }   // fp32 NaN: dw and the split-K partials
+    if (o.poison && dbres) CU(cudaMemsetAsync(dbres, 0xFF, 4 * (size_t)g.O, s));
+    switch (ik(impl, kind)) {
+      case ik(0, 0): k_simt_fprop(prec, prec, g, ta, tb, bias, to, act, alpha, s, scale); break;
+      case ik(0, 1): k_simt_dgrad(prec, prec, g, ta, tb, bias, to, act, alpha, s, scale); break;
+      case ik(0, 2): k_simt_wgrad(prec, g, ta, tb, fres, scratch, sc, 0, s); break;
+      case ik(1, 0): rc = k_tc_fprop(g, ba, bb, bias, bo, act, alpha, s, pe, o.w_mn ? 1 : 0); break;
+      case ik(1, 1): rc = k_tc_dgrad(g, ba, bb, bias, bo, act, alpha, s, pe); break;
+      case ik(1, 2): rc = k_tc_wgrad(g, ba, bb, fres, scratch, sc, 0, s, prl); break;
+      case ik(2, 0): k_edge_conv_small_cin(prec, prec, g, ta, tb, bias, to, act, alpha, s); break;
+      case ik(2, 1): k_edge_deconv_small_c(prec, prec, g, ta, tb, bias, to, act, alpha, s); break;
+      case ik(2, 2): k_edge_wgrad_small_cin(prec, g, ta, tb, fres, scratch, 0, s); break;
+      case ik(3, 0): rc = k_tc_edge_conv(g, ba, bb, bias, bo, act, alpha, s); break;
+      case ik(3, 1): rc = k_tc_deconv_ps(g, ba, wps, bias, bo, act, alpha, s, pe); break;
+      case ik(3, 2): rc = k_tc_edge_wgrad(g, ba, bb, fres, dbres, scratch, sc, 0, s, prl); if (rc >= 0) { db_written = rc; rc = 0; } break;
+      case ik(4, 0): k_dense_small_o_fwd(prec, prec, g, ta, tb, bias, to, act, alpha, s); break;
+      case ik(4, 1):
+        if (dense_small_o_supported(g) && !bias && !act) k_dense_small_o_dgrad(prec, prec, g, ta, tb, to, s);
+        else k_dense_small_k_dgrad(prec, prec, g, ta, tb, bias, to, act, alpha, s);
+        break;
+      case ik(4, 2): if (dense_small_o_supported(g)) k_dense_small_o_wgrad(prec, g, ta, tb, fres, scratch, 0, s); else k_dense_small_k_wgrad(prec, g, ta, tb, fres, s); break;
+      case ik(5, 0): k_head_fwd(g, ba, bb, bias, bo, act, alpha, s); break;
+      case ik(5, 1): k_head_dgrad(g, ba, bb, bias, bo, act, alpha, s); break;
+      case ik(5, 2): {      // the weight gradient's split sums as the backward pass runs them: one reduce-list launch; db = the column sums of dy
         ReduceList hl{};
-        if (k_head_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fres, scratch, sc, force_splits, s, &hl)) { rc = -5; break; }
+        if (k_head_wgrad(g, ba, bb, fres, scratch, sc, force_splits, s, &hl)) { rc = -5; break; }
         const int hs = g_gemm_last_splits; k_reduce_multi(hl, s); g_gemm_last_splits = hs;
         if (dbres) { k_colsum(PREC_BF16, tb, g.N * g.OH * g.OW, g.O, scratch, dbres, 0, s); db_written = 1; }
+        break;
       }
     }
-    else if (impl == 4) {
-      const bool so = dense_small_o_supported(g);
-      if (kind == 0) k_dense_small_o_fwd(prec, prec, g, ta, tb, bias, to, act, alpha, s);
-      else if (kind == 1) { if (so && !bias && !act) k_dense_small_o_dgrad(prec, prec, g, ta, tb, to, s); else k_dense_small_k_dgrad(prec, prec, g, ta, tb, bias, to, act, alpha, s); }
-      else { if (so) k_dense_small_o_wgrad(prec, g, ta, tb, fres, scratch, 0, s); else k_dense_small_k_wgrad(prec, g, ta, tb, fres, s); }
-    }
-    else if (impl >= 2) {
-      if (kind == 0) { if (impl == 3) rc = k_tc_edge_conv(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s); else k_edge_conv_small_cin(prec, prec, g, ta, tb, bias, to, act, alpha, s); }
-      else if (kind == 1) { if (impl == 3) rc = k_tc_deconv_ps(g, (const __nv_bfloat16*)ta, wps, bias, (__nv_bfloat16*)to, act, alpha, s, pe); else k_edge_deconv_small_c(prec, prec, g, ta, tb, bias, to, act, alpha, s); }
-      else {
-        if (impl == 3) { rc = k_tc_edge_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fres, dbres, scratch, sc, 0, s, prl); if (rc >= 0) { db_written = rc; rc = 0; } }
-        else k_edge_wgrad_small_cin(prec, g, ta, tb, fres, scratch, 0, s);
-      }
-    }
-    else if (kind == 0) { if (impl) rc = k_tc_fprop(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s, pe, w_mn ? 1 : 0); else k_simt_fprop(prec, prec, g, ta, tb, bias, to, act, alpha, s, d_scale); }
-    else if (kind == 1) { if (impl) rc = k_tc_dgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, bias, (__nv_bfloat16*)to, act, alpha, s, pe); else k_simt_dgrad(prec, prec, g, ta, tb, bias, to, act, alpha, s, d_scale); }
-    else { if (impl) rc = k_tc_wgrad(g, (const __nv_bfloat16*)ta, (const __nv_bfloat16*)tb, fres, scratch, sc, 0, s, prl); else k_simt_wgrad(prec, g, ta, tb, fres, scratch, sc, 0, s); }
     if (rc) break;
-    if (defer) {      // the backward pass's one reduce-list launch over the partials the wgrad kernel left in scratch
+    if (o.defer) {      // the backward pass's one reduce-list launch over the partials the wgrad kernel left in scratch
       if (!rl.count) { rc = -4; break; }
       k_reduce_multi(rl, s); rl.count = 0;
     }
@@ -1762,22 +1800,18 @@ extern "C" int32_t b2g_test_conv_ex(b2g_ctx* c, int32_t kind, int32_t impl, int3
     strncpy(opt->kernel, gemm ? g_gemm_last_kernel : g_tc_last_kernel, sizeof(opt->kernel) - 1); opt->kernel[sizeof(opt->kernel) - 1] = 0; opt->slab = g_tc_last_slab;
     opt->splits = gemm ? g_gemm_last_splits : tc_wg ? g_tc_last_splits : 0;
   }
-  if (d_db) {
-    if (!db_written) { cudaFree(d_db); return fail(B2G_ERR_UNSUPPORTED, "the edge weight gradient produces no bias column for C = %d", g.C); }
-    CU(cudaMemcpyAsync(db_host, dbres, 4 * (size_t)g.O, cudaMemcpyDeviceToHost, s));
+  if (o.db) {
+    if (!db_written) return fail(B2G_ERR_UNSUPPORTED, "the edge weight gradient produces no bias column for C = %d", g.C);
+    B2(m.downF(o.db, dbres, g.O));
   }
-  if (kind != 2) { if (prec == PREC_BF16) { /* widen */ k_nhwc_to_nchw_f32(prec, to, fo, 1, 1, (int)no, s); } else CU(cudaMemcpyAsync(fo, to, 4 * no, cudaMemcpyDeviceToDevice, s)); }
-  CU(cudaMemcpyAsync(out, fres, 4 * no, cudaMemcpyDeviceToHost, s));
+  B2(kind == 2 ? m.downF(out, fres, no) : m.downT(out, to, no));
   CU(cudaStreamSynchronize(s)); CHECK_KERNELS();
-  if (d_acc && opt && opt->stats) {      // [groups][2][C] doubles from the [groups][2][2][C] hi | lo words
+  if (d_acc && o.stats) {      // [groups][2][C] doubles from the [groups][2][2][C] hi | lo words
     std::vector<long long> h(k_bn_acc_elems(oc, groups)); CU(cudaMemcpy(h.data(), d_acc, 8 * h.size(), cudaMemcpyDeviceToHost));
     for (int gi = 0; gi < groups; ++gi) for (int st = 0; st < 2; ++st) for (int ch = 0; ch < oc; ++ch)
-      opt->stats[((size_t)gi * 2 + st) * oc + ch] = (double)h[((size_t)(gi * 2 + st) * 2 + 0) * oc + ch] / 1024.0 + (double)h[((size_t)(gi * 2 + st) * 2 + 1) * oc + ch] / 1152921504606846976.0;
+      o.stats[((size_t)gi * 2 + st) * oc + ch] = (double)h[((size_t)(gi * 2 + st) * 2 + 0) * oc + ch] / 1024.0 + (double)h[((size_t)(gi * 2 + st) * 2 + 1) * oc + ch] / 1152921504606846976.0;
   }
   float ms = 0.f; CU(cudaEventElapsedTime(&ms, e0, e1)); if (ms_per_iter) *ms_per_iter = ms / reps;
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  cudaFree(fa); cudaFree(fb); cudaFree(fo); cudaFree(scratch); cudaFree(ta); cudaFree(tbase); cudaFree(to); if (wps) cudaFree(wps); if (d_db) cudaFree(d_db);
-  if (d_bias) cudaFree(d_bias); if (d_scale) cudaFree(d_scale); if (d_coef) cudaFree(d_coef); if (d_auxf) cudaFree(d_auxf); if (d_aux) cudaFree(d_aux); if (d_aux2) cudaFree(d_aux2); if (d_acc) cudaFree(d_acc);
   return 0;
 }
 extern "C" int32_t b2g_test_conv(b2g_ctx* c, int32_t kind, int32_t impl, int32_t precision, const b2g_conv_geom* gg, const float* a_host, const float* b_host, float* out, int32_t iters, float* ms_per_iter) {
@@ -1796,24 +1830,15 @@ extern "C" int32_t b2g_test_bn(b2g_ctx* c, int32_t precision, int32_t path, int3
   const int prec = precision == B2G_PREC_BF16 ? PREC_BF16 : PREC_F32;
   if (path != 0 && !k_bn_vec_ok(prec, C)) return fail(B2G_ERR_UNSUPPORTED, "the accumulator BatchNorm kernels need bf16 and C %% 8 == 0 with 256 %% (C/8) == 0 (C = %d)", C);
   CU(cudaSetDevice(c->device)); cudaStream_t s = c->stream;
-  const size_t n = (size_t)groups * rows * C, gc = (size_t)groups * C, ts = prec_size(prec);
-  std::vector<void*> mem;
-  auto alloc = [&](void** p, size_t bytes) -> int32_t { *p = nullptr; CU(cudaMalloc(p, bytes)); mem.push_back(*p); return 0; };
-  auto release = [&]() { for (void* p : mem) cudaFree(p); mem.clear(); };
-  float *fx, *fe, *fo, *d_par, *d_grad, *d_stat, *scratch, *coef, *unit; void *tx, *te, *ty, *tei; unsigned long long* acc;
-  int32_t r = 0;
-  if ((r = alloc((void**)&fx, 4 * n)) || (r = alloc((void**)&fe, 4 * n)) || (r = alloc((void**)&fo, 4 * n)) || (r = alloc(&tx, ts * n)) || (r = alloc(&te, ts * n)) ||
-      (r = alloc(&ty, ts * n)) || (r = alloc(&tei, ts * n)) || (r = alloc((void**)&d_par, 4 * 4 * (size_t)C)) || (r = alloc((void**)&d_grad, 4 * 4 * (size_t)C)) ||
-      (r = alloc((void**)&d_stat, 4 * 2 * gc)) || (r = alloc((void**)&scratch, 4 * k_bn_scratch_floats(C, groups))) || (r = alloc((void**)&coef, 4 * 4 * gc)) ||
-      (r = alloc((void**)&unit, 4 * 4 * gc)) || (r = alloc((void**)&acc, 8 * 2 * k_bn_acc_elems(C, groups)))) { release(); return r; }
-  float *d_gamma = d_par, *d_beta = d_par + C, *d_rm = d_par + 2 * C, *d_rv = d_par + 3 * C;
-  float *d_gg = d_grad, *d_gb = d_grad + C, *d_gm = d_grad + 2 * C, *d_gv = d_grad + 3 * C, *d_mean = d_stat, *d_is = d_stat + gc;
-  unsigned long long *acc_f = acc, *acc_b = acc + k_bn_acc_elems(C, groups);
-  auto up = [&](float* d, const float* h, size_t k) { return cudaMemcpyAsync(d, h, 4 * k, cudaMemcpyHostToDevice, s); };
-  if (up(fx, x, n) || up(fe, eps_out, n) || up(d_gamma, gamma, C) || up(d_beta, beta, C) || up(d_rm, run_mean, C) || up(d_rv, run_var, C) ||
-      up(d_gg, g_gamma, C) || up(d_gb, g_beta, C) || cudaMemsetAsync(acc, 0, 8 * 2 * k_bn_acc_elems(C, groups), s)) { release(); return fail(B2G_ERR_CUDA, "BatchNorm test upload failed"); }
-  if (prec == PREC_BF16) { k_cast_f32_to_bf16(fx, (__nv_bfloat16*)tx, n, s); k_cast_f32_to_bf16(fe, (__nv_bfloat16*)te, n, s); }
-  else { cudaMemcpyAsync(tx, fx, 4 * n, cudaMemcpyDeviceToDevice, s); cudaMemcpyAsync(te, fe, 4 * n, cudaMemcpyDeviceToDevice, s); }
+  const size_t n = (size_t)groups * rows * C, gc = (size_t)groups * C, ts = prec_size(prec), na = k_bn_acc_elems(C, groups);
+  HookMem m(s, prec);
+  float *d_gamma, *d_beta, *d_rm, *d_rv, *d_gg, *d_gb, *d_gm, *d_gv, *d_mean, *d_is, *scratch, *coef, *unit; void *tx, *te, *ty, *tei; unsigned long long* acc;
+  B2(m.upT(x, n, &tx)); B2(m.upT(eps_out, n, &te)); B2(m.dev(n, ts, &ty)); B2(m.dev(n, ts, &tei));
+  B2(m.upF(gamma, C, &d_gamma)); B2(m.upF(beta, C, &d_beta)); B2(m.upF(run_mean, C, &d_rm)); B2(m.upF(run_var, C, &d_rv));
+  B2(m.upF(g_gamma, C, &d_gg)); B2(m.upF(g_beta, C, &d_gb)); B2(m.upF(nullptr, C, &d_gm)); B2(m.upF(nullptr, C, &d_gv));
+  B2(m.upF(nullptr, gc, &d_mean)); B2(m.upF(nullptr, gc, &d_is)); B2(m.upF(nullptr, k_bn_scratch_floats(C, groups), &scratch));
+  B2(m.upF(nullptr, 4 * gc, &coef)); B2(m.upF(nullptr, 4 * gc, &unit)); B2(m.dev(2 * na, 8, (void**)&acc)); CU(cudaMemsetAsync(acc, 0, 8 * 2 * na, s));
+  unsigned long long *acc_f = acc, *acc_b = acc + na;
   const int want = want_param_grads ? 1 : 0;
   if (path == 0) {
     k_bn_stats(prec, tx, rows, C, groups, scratch, d_mean, d_is, eps, d_rm, d_rv, d_gm, d_gv, decay, s);
@@ -1833,17 +1858,10 @@ extern "C" int32_t b2g_test_bn(b2g_ctx* c, int32_t precision, int32_t path, int3
       cudaMemcpyAsync(d_is + (size_t)g * C, coef + (size_t)(g * 4 + 3) * C, 4 * C, cudaMemcpyDeviceToDevice, s);
     }
   }
-  auto down = [&](float* h, const void* t) -> int32_t {     // widen a T tensor to fp32 and copy it out
-    k_nhwc_to_nchw_f32(prec, t, fo, 1, 1, (int)n, s); CU(cudaMemcpyAsync(h, fo, 4 * n, cudaMemcpyDeviceToHost, s)); CU(cudaStreamSynchronize(s)); return 0;
-  };
-  if ((r = down(y, ty)) || (r = down(eps_in, tei))) { release(); return r; }
-  cudaError_t e = cudaSuccess;
-  float* hs[6] = {g_gamma, g_beta, g_mean, g_var, mean, invstd}; const float* ds[6] = {d_gg, d_gb, d_gm, d_gv, d_mean, d_is}; const size_t ks[6] = {(size_t)C, (size_t)C, (size_t)C, (size_t)C, gc, gc};
-  for (int k = 0; k < 6 && e == cudaSuccess; ++k) e = cudaMemcpyAsync(hs[k], ds[k], 4 * ks[k], cudaMemcpyDeviceToHost, s);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  if (e == cudaSuccess) e = cudaGetLastError();
-  release();
-  if (e != cudaSuccess) return fail(B2G_ERR_CUDA, "BatchNorm test: %s", cudaGetErrorString(e));
+  B2(m.downT(y, ty, n)); B2(m.downT(eps_in, tei, n));
+  B2(m.downF(g_gamma, d_gg, C)); B2(m.downF(g_beta, d_gb, C)); B2(m.downF(g_mean, d_gm, C)); B2(m.downF(g_var, d_gv, C));
+  B2(m.downF(mean, d_mean, gc)); B2(m.downF(invstd, d_is, gc));
+  CU(cudaStreamSynchronize(s)); CHECK_KERNELS();
   return 0;
 }
 
@@ -1858,45 +1876,24 @@ extern "C" int32_t b2g_test_dropout(b2g_ctx* c, int32_t precision, uint64_t seed
   if (n > 0x7fffffff) return fail(B2G_ERR_UNSUPPORTED, "the dropout test hook takes at most 2^31 - 1 elements (%zu)", n);
   const int prec = precision == B2G_PREC_BF16 ? PREC_BF16 : PREC_F32; const size_t ts = prec_size(prec);
   CU(cudaSetDevice(c->device)); cudaStream_t s = c->stream;
-  std::vector<void*> mem;
-  auto alloc = [&](void** q, size_t bytes) -> int32_t { *q = nullptr; CU(cudaMalloc(q, bytes)); mem.push_back(*q); return 0; };
-  auto release = [&]() { for (void* q : mem) cudaFree(q); mem.clear(); };
-  float *fx, *fe; void *tx, *te, *ty; uint32_t* mask; unsigned long long* dpass; unsigned* ticket; int32_t r = 0;
-  if ((r = alloc((void**)&fx, 4 * n)) || (r = alloc((void**)&fe, 4 * n)) || (r = alloc(&tx, ts * n)) || (r = alloc(&te, ts * n)) || (r = alloc(&ty, ts * n)) ||
-      (r = alloc((void**)&mask, 4 * ((n + 31) / 32))) || (r = alloc((void**)&dpass, sizeof(unsigned long long))) || (r = alloc((void**)&ticket, sizeof(unsigned)))) { release(); return r; }
+  HookMem m(s, prec);
+  void *tx, *te, *ty; uint32_t* mask; unsigned long long* dpass; unsigned* ticket;
   const unsigned long long p0 = (unsigned long long)pass;
-  cudaError_t e = cudaMemcpyAsync(fx, x, 4 * n, cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(fe, dy, 4 * n, cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(dpass, &p0, sizeof(p0), cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) e = cudaMemsetAsync(ticket, 0, sizeof(unsigned), s);
-  if (e != cudaSuccess) { release(); return fail(B2G_ERR_CUDA, "dropout test upload: %s", cudaGetErrorString(e)); }
-  if (prec == PREC_BF16) { k_cast_f32_to_bf16(fx, (__nv_bfloat16*)tx, n, s); k_cast_f32_to_bf16(fe, (__nv_bfloat16*)te, n, s); }
-  else { cudaMemcpyAsync(tx, fx, 4 * n, cudaMemcpyDeviceToDevice, s); cudaMemcpyAsync(te, fe, 4 * n, cudaMemcpyDeviceToDevice, s); }
+  B2(m.upT(x, n, &tx)); B2(m.upT(dy, n, &te)); B2(m.dev(n, ts, &ty)); B2(m.dev((n + 31) / 32, 4, (void**)&mask));
+  B2(m.dev(1, sizeof(p0), (void**)&dpass)); B2(m.dev(1, sizeof(unsigned), (void**)&ticket));
+  CU(cudaMemcpyAsync(dpass, &p0, sizeof(p0), cudaMemcpyHostToDevice, s)); CU(cudaMemsetAsync(ticket, 0, sizeof(unsigned), s));
   const DropoutArgs a = make_dropout_args(seed, layer, rank, p);
   k_dropout_fwd(prec, tx, ty, mask, n, a, dpass, ticket, 1, s);
   k_dropout_bwd(prec, te, te, mask, n, a.scale, s);
   unsigned long long p1 = 0;
-  k_nhwc_to_nchw_f32(prec, ty, fx, 1, 1, (int)n, s);
-  k_nhwc_to_nchw_f32(prec, te, fe, 1, 1, (int)n, s);
-  e = cudaMemcpyAsync(y, fx, 4 * n, cudaMemcpyDeviceToHost, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(dx, fe, 4 * n, cudaMemcpyDeviceToHost, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&p1, dpass, sizeof(p1), cudaMemcpyDeviceToHost, s);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  if (e == cudaSuccess) e = cudaGetLastError();
-  release();
-  if (e != cudaSuccess) return fail(B2G_ERR_CUDA, "dropout test: %s", cudaGetErrorString(e));
+  B2(m.downT(y, ty, n)); B2(m.downT(dx, te, n)); CU(cudaMemcpyAsync(&p1, dpass, sizeof(p1), cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s)); CHECK_KERNELS();
   if (p1 != p0 + 1) return fail(B2G_ERR_CUDA, "dropout test: the forward left the pass counter at %llu, expected %llu", p1, p0 + 1);
   return 0;
 }
 
 // One reduction / loss / element-wise kernel through its production wrapper on host tensors (include/b200gan.h, b2g_test_ew).  The kernel
 // names come from the wrappers (g_ew_last_kernel): this hook never decides which path a shape takes.
-namespace {
-struct EwMem {        // every allocation of one b2g_test_ew call, released on every return
-  std::vector<void*> v;
-  ~EwMem() { for (void* p : v) cudaFree(p); }
-};
-}  // namespace
 // b2g_test_pool runs through the same code as two private ops, its own options in po (null for every b2g_test_ew call)
 enum { EW_POOL2D = 100, EW_GLOBAL_POOL = 101 };
 static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, b2g_test_pool_opts* po, const float* in0, const float* in1, float* out0,
@@ -1907,21 +1904,7 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
   if (off < 0 || off > 64) return fail(B2G_ERR_ARG, "offset %d outside [0, 64]", off);
   if (o->poison && o->accumulate) return fail(B2G_ERR_ARG, "poison would overwrite the initial destination accumulate adds to");
   CU(cudaSetDevice(c->device)); cudaStream_t s = c->stream;
-  EwMem mem;
-  // es-byte elements, `off` elements past a 256-byte aligned allocation
-  auto dev = [&](size_t count, size_t es, void** p) -> int32_t { void* b = nullptr; CU(cudaMalloc(&b, es * (count + off) + 16)); mem.v.push_back(b); *p = (char*)b + es * off; return 0; };
-  auto upF = [&](const float* h, size_t count, float** p) -> int32_t {
-    B2(dev(count, 4, (void**)p)); if (h) CU(cudaMemcpyAsync(*p, h, 4 * count, cudaMemcpyHostToDevice, s)); return 0; };
-  auto upT = [&](const float* h, size_t count, void** p) -> int32_t {        // fp32 host -> T (bf16: rounded on the device)
-    B2(dev(count, ts, p)); if (!h) return 0;
-    if (prec == PREC_F32) { CU(cudaMemcpyAsync(*p, h, 4 * count, cudaMemcpyHostToDevice, s)); return 0; }
-    float* f = nullptr; CU(cudaMalloc(&f, 4 * count)); mem.v.push_back(f);
-    CU(cudaMemcpyAsync(f, h, 4 * count, cudaMemcpyHostToDevice, s)); k_cast_f32_to_bf16(f, (__nv_bfloat16*)*p, count, s); return 0; };
-  auto downF = [&](float* h, const float* d, size_t count) -> int32_t { if (h) CU(cudaMemcpyAsync(h, d, 4 * count, cudaMemcpyDeviceToHost, s)); return 0; };
-  auto downT = [&](float* h, const void* d, size_t count) -> int32_t {      // T -> fp32 host
-    if (!h) return 0;
-    float* f = nullptr; CU(cudaMalloc(&f, 4 * count)); mem.v.push_back(f);
-    k_nhwc_to_nchw_f32(prec, d, f, 1, 1, (int)count, s); CU(cudaMemcpyAsync(h, f, 4 * count, cudaMemcpyDeviceToHost, s)); return 0; };
+  HookMem m(s, prec);
   auto poison = [&](void* d, size_t bytes) -> int32_t { if (o->poison) CU(cudaMemsetAsync(d, 0xFF, bytes, s)); return 0; };     // fp32 and bf16 NaN
   std::string names;
   auto ran = [&]() { if (!names.empty()) names += ","; names += g_ew_last_kernel; g_ew_last_kernel = ""; };
@@ -1930,9 +1913,9 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
   switch (o->op) {
     case B2G_EW_REDUCE_SPLITS: {
       if (!in0 || o->n < 1 || o->n > lim || o->splits < 1 || o->stride < o->n || (o->accumulate && !in1)) return fail(B2G_ERR_ARG, "bad REDUCE_SPLITS arguments");
-      float *src = nullptr, *dst = nullptr; B2(upF(in0, (size_t)o->splits * o->stride, &src)); B2(upF(in1, (size_t)o->n, &dst)); B2(poison(dst, 4 * o->n));
+      float *src = nullptr, *dst = nullptr; B2(m.upF(in0, (size_t)o->splits * o->stride, &src, off)); B2(m.upF(in1, (size_t)o->n, &dst, off)); B2(poison(dst, 4 * o->n));
       k_reduce_splits(src, dst, (size_t)o->n, o->splits, (size_t)o->stride, o->accumulate ? 1 : 0, s); ran();
-      B2(downF(out0, dst, (size_t)o->n));
+      B2(m.downF(out0, dst, (size_t)o->n));
       break;
     }
     case B2G_EW_REDUCE_MULTI: {
@@ -1948,7 +1931,7 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
           if (src_hit || dst_hit) return fail(B2G_ERR_ARG, "reduce job %d's destination overlaps job %d", i, k);
         }
       }
-      float* buf = nullptr; B2(upF(in0, (size_t)o->n, &buf));
+      float* buf = nullptr; B2(m.upF(in0, (size_t)o->n, &buf, off));
       ReduceList rl{};
       for (int i = 0; i < o->n_jobs; ++i) {
         reduce_list_push(&rl, buf + J[i].src_off, buf + J[i].dst_off, J[i].n, J[i].splits, J[i].stride);
@@ -1957,34 +1940,34 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
       }
       if (rl.count != o->n_jobs) return fail(B2G_ERR_ARG, "the reduce list took %d of %d jobs", rl.count, o->n_jobs);
       k_reduce_multi(rl, s); ran();
-      B2(downF(out0, buf, (size_t)o->n));
+      B2(m.downF(out0, buf, (size_t)o->n));
       break;
     }
     case B2G_EW_COLSUM: {
       if (!in0 || o->rows < 1 || o->cols < 1 || (int64_t)o->rows * o->cols > lim || (o->accumulate && !in1)) return fail(B2G_ERR_ARG, "bad COLSUM arguments");
-      void* x = nullptr; float *out = nullptr, *scratch = nullptr; B2(upT(in0, (size_t)o->rows * o->cols, &x)); B2(upF(in1, (size_t)o->cols, &out)); B2(poison(out, 4 * (size_t)o->cols));
-      CU(cudaMalloc(&scratch, 4 * k_colsum_scratch_floats(o->cols))); mem.v.push_back(scratch);
+      void* x = nullptr; float *out = nullptr, *scratch = nullptr; B2(m.upT(in0, (size_t)o->rows * o->cols, &x, off)); B2(m.upF(in1, (size_t)o->cols, &out, off)); B2(poison(out, 4 * (size_t)o->cols));
+      B2(m.upF(nullptr, k_colsum_scratch_floats(o->cols), &scratch));
       k_colsum(prec, x, o->rows, o->cols, scratch, out, o->accumulate ? 1 : 0, s); ran();
-      B2(downF(out0, out, (size_t)o->cols));
+      B2(m.downF(out0, out, (size_t)o->cols));
       break;
     }
     case B2G_EW_XENT: {
       const size_t n = (size_t)o->rows * o->groups;
       if (!in0 || !in1 || o->rows < 1 || o->groups < 1 || (int64_t)n > lim) return fail(B2G_ERR_ARG, "bad XENT arguments");
-      void *z = nullptr, *dz = nullptr; float *y = nullptr, *loss = nullptr; B2(upT(in0, n, &z)); B2(upF(in1, n, &y)); B2(dev(n, ts, &dz)); B2(upF(nullptr, (size_t)o->groups, &loss));
+      void *z = nullptr, *dz = nullptr; float *y = nullptr, *loss = nullptr; B2(m.upT(in0, n, &z, off)); B2(m.upF(in1, n, &y, off)); B2(m.dev(n, ts, &dz, off)); B2(m.upF(nullptr, (size_t)o->groups, &loss, off));
       B2(poison(dz, ts * n)); B2(poison(loss, 4 * (size_t)o->groups));
       k_xent(prec, z, y, dz, loss, o->rows, o->groups, o->clip_eps, s); ran();
-      B2(downT(out0, dz, n)); B2(downF(out1, loss, (size_t)o->groups));
+      B2(m.downT(out0, dz, n)); B2(m.downF(out1, loss, (size_t)o->groups));
       break;
     }
     case B2G_EW_SOFTMAX_XENT: {
       const size_t n = (size_t)o->rows * o->cols;
       if (!in0 || o->rows < 1 || o->cols < 1 || (int64_t)n > lim) return fail(B2G_ERR_ARG, "bad SOFTMAX_XENT arguments");
-      void *z = nullptr, *dz = nullptr, *p = nullptr; float *y = nullptr, *loss = nullptr; B2(upT(in0, n, &z)); if (in1) B2(upF(in1, n, &y));
-      B2(dev(n, ts, &dz)); B2(dev(n, ts, &p)); B2(upF(nullptr, 1, &loss));
+      void *z = nullptr, *dz = nullptr, *p = nullptr; float *y = nullptr, *loss = nullptr; B2(m.upT(in0, n, &z, off)); if (in1) B2(m.upF(in1, n, &y, off));
+      B2(m.dev(n, ts, &dz, off)); B2(m.dev(n, ts, &p, off)); B2(m.upF(nullptr, 1, &loss, off));
       B2(poison(dz, ts * n)); B2(poison(p, ts * n)); B2(poison(loss, 4));
       k_softmax_xent(prec, z, y, y ? dz : nullptr, p, y ? loss : nullptr, o->rows, o->cols, s); ran();       // no labels: the inference call
-      B2(downT(out0, dz, n)); B2(downF(out1, loss, 1)); B2(downT(out2, p, n));
+      B2(m.downT(out0, dz, n)); B2(m.downF(out1, loss, 1)); B2(m.downT(out2, p, n));
       break;
     }
     case B2G_EW_LOSS: {
@@ -1992,11 +1975,11 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
       if (!in0 || !in1 || o->rows < 1 || o->cols < 1 || o->groups < 1 || (int64_t)n > lim || o->loss < B2G_LOSS_MSE || o->loss > B2G_LOSS_WASSERSTEIN ||
           o->act < B2G_ACT_IDENTITY || o->act > B2G_ACT_LRELU) return fail(B2G_ERR_ARG, "bad LOSS arguments");
       void *z = nullptr, *dz = nullptr; float *y = nullptr, *loss = nullptr; double* partial = nullptr; unsigned* ticket = nullptr;
-      B2(upT(in0, n, &z)); B2(upF(in1, n, &y)); B2(dev(n, ts, &dz)); B2(upF(nullptr, (size_t)o->groups, &loss));
-      B2(dev((size_t)o->groups * k_loss_blocks(per, o->groups), 8, (void**)&partial)); B2(dev(1, 4, (void**)&ticket)); CU(cudaMemsetAsync(ticket, 0, 4, s));
+      B2(m.upT(in0, n, &z, off)); B2(m.upF(in1, n, &y, off)); B2(m.dev(n, ts, &dz, off)); B2(m.upF(nullptr, (size_t)o->groups, &loss, off));
+      B2(m.dev((size_t)o->groups * k_loss_blocks(per, o->groups), 8, (void**)&partial, off)); B2(m.dev(1, 4, (void**)&ticket, off)); CU(cudaMemsetAsync(ticket, 0, 4, s));
       B2(poison(dz, ts * n)); B2(poison(loss, 4 * (size_t)o->groups));
       k_loss(prec, o->loss, o->act, o->alpha, z, y, dz, loss, o->rows, o->cols, o->groups, partial, ticket, s); ran();
-      B2(downT(out0, dz, n)); B2(downF(out1, loss, (size_t)o->groups));
+      B2(m.downT(out0, dz, n)); B2(m.downF(out1, loss, (size_t)o->groups));
       break;
     }
     case B2G_EW_CNN_XENT: case B2G_EW_CNN_SOFTMAX_XENT: {
@@ -2005,13 +1988,13 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
       if (!in0 || (!in1 && !sm) || o->rows < 1 || o->cols < 1 || o->groups < 1 || (int64_t)n > lim) return fail(B2G_ERR_ARG, "bad CNN loss arguments");
       const int bpg = sm ? k_cnn_softmax_blocks(o->rows, o->groups) : k_loss_blocks(per, o->groups);
       void *z = nullptr, *dz = nullptr, *p = nullptr; float *y = nullptr, *loss = nullptr; double* partial = nullptr; unsigned* ticket = nullptr;
-      B2(upT(in0, n, &z)); if (in1) B2(upF(in1, n, &y)); B2(dev(n, ts, &dz)); B2(dev(n, ts, &p)); B2(upF(nullptr, (size_t)o->groups, &loss));
-      B2(dev((size_t)o->groups * bpg, 8, (void**)&partial)); B2(dev(1, 4, (void**)&ticket)); CU(cudaMemsetAsync(ticket, 0, 4, s));
+      B2(m.upT(in0, n, &z, off)); if (in1) B2(m.upF(in1, n, &y, off)); B2(m.dev(n, ts, &dz, off)); B2(m.dev(n, ts, &p, off)); B2(m.upF(nullptr, (size_t)o->groups, &loss, off));
+      B2(m.dev((size_t)o->groups * bpg, 8, (void**)&partial, off)); B2(m.dev(1, 4, (void**)&ticket, off)); CU(cudaMemsetAsync(ticket, 0, 4, s));
       B2(poison(dz, ts * n)); B2(poison(p, ts * n)); B2(poison(loss, 4 * (size_t)o->groups));
       if (sm) k_cnn_softmax_xent(prec, z, y, y ? dz : nullptr, p, y ? loss : nullptr, o->rows, o->cols, o->groups, partial, ticket, s);     // no labels: the inference call
       else k_cnn_xent(prec, z, y, dz, loss, per, o->groups, o->clip_eps, partial, ticket, s);
       ran();
-      B2(downT(out0, dz, n)); B2(downF(out1, loss, (size_t)o->groups)); if (sm) B2(downT(out2, p, n));
+      B2(m.downT(out0, dz, n)); B2(m.downF(out1, loss, (size_t)o->groups)); if (sm) B2(m.downT(out2, p, n));
       unsigned t = 1; CU(cudaMemcpyAsync(&t, ticket, 4, cudaMemcpyDeviceToHost, s)); CU(cudaStreamSynchronize(s));
       if (t != 0) return fail(B2G_ERR_CUDA, "CNN loss: the kernel left its ticket word at %u", t);
       break;
@@ -2021,18 +2004,18 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
       if (!in0 || !in1 || o->n < 1 || o->n > lim) return fail(B2G_ERR_ARG, "bad vertex arguments");
       if (o->op != B2G_EW_SKIP_ADD && (o->act < B2G_EW_OP_ADD || o->act > B2G_EW_OP_MAX || (order != 0 && order != 1))) return fail(B2G_ERR_ARG, "bad vertex op / order");
       if (o->op == B2G_EW_VERTEX_FWD) {
-        void *a = nullptr, *b = nullptr, *y = nullptr; B2(upT(in0, n, &a)); B2(upT(in1, n, &b)); B2(dev(n, ts, &y)); B2(poison(y, ts * n));
+        void *a = nullptr, *b = nullptr, *y = nullptr; B2(m.upT(in0, n, &a, off)); B2(m.upT(in1, n, &b, off)); B2(m.dev(n, ts, &y, off)); B2(poison(y, ts * n));
         k_vertex_ew_fwd(prec, o->act, order ? b : a, order ? a : b, y, n, s); ran();
-        B2(downT(out0, y, n));
+        B2(m.downT(out0, y, n));
       } else if (o->op == B2G_EW_VERTEX_BWD) {
         void *sp = nullptr, *sk = nullptr, *e = nullptr; float* acc = nullptr;
-        B2(upT(in0, n, &sp)); B2(upT(in0 + n, n, &sk)); B2(upT(in1, n, &e)); B2(upF(o->accumulate ? in1 + n : nullptr, n, &acc)); B2(poison(acc, 4 * n));
+        B2(m.upT(in0, n, &sp, off)); B2(m.upT(in0 + n, n, &sk, off)); B2(m.upT(in1, n, &e, off)); B2(m.upF(o->accumulate ? in1 + n : nullptr, n, &acc, off)); B2(poison(acc, 4 * n));
         k_vertex_ew_bwd(prec, o->act, order, e, sp, sk, acc, o->accumulate ? 1 : 0, n, s); ran();
-        B2(downT(out0, e, n)); B2(downF(out1, acc, n));
+        B2(m.downT(out0, e, n)); B2(m.downF(out1, acc, n));
       } else {
-        void* e = nullptr; float* acc = nullptr; B2(upT(in0, n, &e)); B2(upF(in1, n, &acc));
+        void* e = nullptr; float* acc = nullptr; B2(m.upT(in0, n, &e, off)); B2(m.upF(in1, n, &acc, off));
         k_skip_add(prec, e, acc, n, s); ran();
-        B2(downT(out0, e, n));
+        B2(m.downT(out0, e, n));
       }
       break;
     }
@@ -2041,40 +2024,40 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
       if (!in0 || (!in1 && (o->op == B2G_EW_MERGE_FWD || o->accumulate)) || o->rows < 1 || Cs < 1 || Ck < 1 || (order != 0 && order != 1) || nt > (size_t)lim)
         return fail(B2G_ERR_ARG, "bad merge arguments");
       if (o->op == B2G_EW_MERGE_FWD) {
-        void *a = nullptr, *b = nullptr, *y = nullptr; B2(upT(in0, P * Cs, &a)); B2(upT(in1, P * Ck, &b)); B2(dev(nt, ts, &y)); B2(poison(y, ts * nt));
+        void *a = nullptr, *b = nullptr, *y = nullptr; B2(m.upT(in0, P * Cs, &a, off)); B2(m.upT(in1, P * Ck, &b, off)); B2(m.dev(nt, ts, &y, off)); B2(poison(y, ts * nt));
         if (order) k_merge_fwd(prec, b, a, y, P, Ck, Cs, s); else k_merge_fwd(prec, a, b, y, P, Cs, Ck, s);
-        ran(); B2(downT(out0, y, nt));
+        ran(); B2(m.downT(out0, y, nt));
       } else {
         void *e = nullptr, *d = nullptr; float* acc = nullptr;
-        B2(upT(in0, nt, &e)); B2(dev(P * Cs, ts, &d)); B2(upF(o->accumulate ? in1 : nullptr, P * Ck, &acc)); B2(poison(d, ts * P * Cs)); B2(poison(acc, 4 * P * Ck));
+        B2(m.upT(in0, nt, &e, off)); B2(m.dev(P * Cs, ts, &d, off)); B2(m.upF(o->accumulate ? in1 : nullptr, P * Ck, &acc, off)); B2(poison(d, ts * P * Cs)); B2(poison(acc, 4 * P * Ck));
         k_merge_bwd(prec, e, d, acc, P, order ? Ck : Cs, order ? Cs : Ck, order == 0, o->accumulate ? 1 : 0, s); ran();
-        B2(downT(out0, d, P * Cs)); B2(downF(out1, acc, P * Ck));
+        B2(m.downT(out0, d, P * Cs)); B2(m.downF(out1, acc, P * Ck));
       }
       break;
     }
     case B2G_EW_ACT_FWD: case B2G_EW_ACT_BWD: {
       const size_t n = (size_t)o->n; const bool bwd = o->op == B2G_EW_ACT_BWD;
       if (!in0 || (bwd && !in1) || o->n < 1 || o->n > lim || o->act < B2G_ACT_IDENTITY || o->act > B2G_ACT_LRELU) return fail(B2G_ERR_ARG, "bad activation arguments");
-      void *a = nullptr, *e = nullptr, *r = nullptr; B2(upT(in0, n, &a));
-      if (bwd) B2(upT(in1, n, &e));
+      void *a = nullptr, *e = nullptr, *r = nullptr; B2(m.upT(in0, n, &a, off));
+      if (bwd) B2(m.upT(in1, n, &e, off));
       if (bwd && o->in_place) r = e;
-      else { B2(dev(n, ts, &r)); B2(poison(r, ts * n)); }
+      else { B2(m.dev(n, ts, &r, off)); B2(poison(r, ts * n)); }
       if (bwd) k_act_bwd_from_output(prec, a, e, r, n, o->act, o->alpha, s);      // in place: eps_in == eps_out, as the backward pass calls it
       else k_act_fwd(prec, a, r, n, o->act, o->alpha, s);
       ran();
-      B2(downT(out0, r, n));
+      B2(m.downT(out0, r, n));
       break;
     }
     case B2G_EW_ACT_EXT_FWD: case B2G_EW_ACT_EXT_BWD: {
       const size_t n = (size_t)o->n; const bool bwd = o->op == B2G_EW_ACT_EXT_BWD;
       if (!in0 || (bwd && !in1) || o->n < 1 || o->n > lim || !act_ext_kind(o->act) || !std::isfinite(o->alpha)) return fail(B2G_ERR_ARG, "bad activation arguments");
-      void *z = nullptr, *r = nullptr; B2(upT(in0, n, &z));
-      if (bwd) B2(upT(in1, n, &r));      // eps_out, overwritten in place with eps_in
-      else { B2(dev(n, ts, &r)); B2(poison(r, ts * n)); }
+      void *z = nullptr, *r = nullptr; B2(m.upT(in0, n, &z, off));
+      if (bwd) B2(m.upT(in1, n, &r, off));      // eps_out, overwritten in place with eps_in
+      else { B2(m.dev(n, ts, &r, off)); B2(poison(r, ts * n)); }
       if (bwd) k_act_ext_bwd(prec, o->act, o->alpha, z, r, n, s);
       else k_act_ext_fwd(prec, o->act, o->alpha, z, r, n, s);
       ran();
-      B2(downT(out0, r, n));
+      B2(m.downT(out0, r, n));
       break;
     }
     case B2G_EW_MAXPOOL: {
@@ -2084,11 +2067,11 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
       const size_t ni = (size_t)o->N * o->H * o->W * o->C, no = (size_t)o->N * OH * OW * o->C;
       if (ni > (size_t)lim) return fail(B2G_ERR_ARG, "MAXPOOL input too large");
       void *x = nullptr, *eo = nullptr, *y = nullptr, *ei = nullptr; uint8_t* arg = nullptr;
-      B2(upT(in0, ni, &x)); B2(upT(in1, no, &eo)); B2(dev(no, ts, &y)); B2(dev(ni, ts, &ei)); B2(dev(no, 1, (void**)&arg));
+      B2(m.upT(in0, ni, &x, off)); B2(m.upT(in1, no, &eo, off)); B2(m.dev(no, ts, &y, off)); B2(m.dev(ni, ts, &ei, off)); B2(m.dev(no, 1, (void**)&arg, off));
       B2(poison(y, ts * no)); B2(poison(ei, ts * ni)); B2(poison(arg, no));        // 0xFF: no window of <= 255 elements has that argmax
       k_maxpool_fwd(prec, x, y, arg, o->N, o->H, o->W, o->C, OH, OW, o->KH, o->KW, o->SH, o->SW, s); ran();
       k_maxpool_bwd(prec, eo, arg, ei, o->N, o->H, o->W, o->C, OH, OW, o->KH, o->KW, o->SH, o->SW, s); ran();
-      B2(downT(out0, y, no)); B2(downT(out1, ei, ni));
+      B2(m.downT(out0, y, no)); B2(m.downT(out1, ei, ni));
       if (out2) {
         std::vector<uint8_t> h(no); CU(cudaMemcpyAsync(h.data(), arg, no, cudaMemcpyDeviceToHost, s)); CU(cudaStreamSynchronize(s));
         for (size_t i = 0; i < no; ++i) out2[i] = (float)h[i];
@@ -2105,11 +2088,11 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
       const size_t ni = (size_t)o->N * o->H * o->W * o->C, no = (size_t)o->N * OH * OW * o->C;
       if (ni > (size_t)lim || no > (size_t)lim) return fail(B2G_ERR_ARG, "POOL2D tensors too large");
       void *x = nullptr, *eo = nullptr, *y = nullptr, *ei = nullptr;
-      B2(upT(in0, ni, &x)); B2(upT(in1, no, &eo)); B2(dev(no, ts, &y)); B2(dev(ni, ts, &ei)); B2(poison(y, ts * no)); B2(poison(ei, ts * ni));
+      B2(m.upT(in0, ni, &x, off)); B2(m.upT(in1, no, &eo, off)); B2(m.dev(no, ts, &y, off)); B2(m.dev(ni, ts, &ei, off)); B2(poison(y, ts * no)); B2(poison(ei, ts * ni));
       const int pn = po->pool == B2G_POOL_PNORM ? (int)po->pnorm : 0;
       k_pool2d_fwd(prec, po->pool, pn, x, y, o->N, o->H, o->W, o->C, OH, OW, o->KH, o->KW, o->SH, o->SW, po->PH, po->PW, s); ran();
       k_pool2d_bwd(prec, po->pool, pn, eo, x, y, ei, o->N, o->H, o->W, o->C, OH, OW, o->KH, o->KW, o->SH, o->SW, po->PH, po->PW, s); ran();
-      B2(downT(out0, y, no)); B2(downT(out1, ei, ni));
+      B2(m.downT(out0, y, no)); B2(m.downT(out1, ei, ni));
       break;
     }
     case EW_GLOBAL_POOL: {
@@ -2121,15 +2104,15 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
       const size_t ni = (size_t)o->N * HW * o->C, no = (size_t)o->N * o->C;
       if (ni > (size_t)lim) return fail(B2G_ERR_ARG, "GLOBAL_POOL input too large");
       void *x = nullptr, *eo = nullptr, *y = nullptr, *ei = nullptr; int32_t *idx = nullptr, *part_idx = nullptr; float* part = nullptr; unsigned* ticket = nullptr;
-      B2(upT(in0, ni, &x)); B2(upT(in1, no, &eo)); B2(dev(no, ts, &y)); B2(dev(ni, ts, &ei)); B2(dev(no, 4, (void**)&idx));
+      B2(m.upT(in0, ni, &x, off)); B2(m.upT(in1, no, &eo, off)); B2(m.dev(no, ts, &y, off)); B2(m.dev(ni, ts, &ei, off)); B2(m.dev(no, 4, (void**)&idx, off));
       const size_t np = std::max<size_t>(1, k_global_pool_partial_elems(prec, o->N, HW, o->C));
-      B2(dev(np, 4, (void**)&part)); B2(dev(np, 4, (void**)&part_idx)); B2(dev(1, 4, (void**)&ticket)); CU(cudaMemsetAsync(ticket, 0, 4, s));
+      B2(m.dev(np, 4, (void**)&part, off)); B2(m.dev(np, 4, (void**)&part_idx, off)); B2(m.dev(1, 4, (void**)&ticket, off)); CU(cudaMemsetAsync(ticket, 0, 4, s));
       B2(poison(y, ts * no)); B2(poison(ei, ts * ni)); B2(poison(idx, 4 * no));      // 0xFF..: index -1, no pixel
       const int pn = po->pool == B2G_POOL_PNORM ? (int)po->pnorm : 0;
       k_global_pool_fwd(prec, po->pool, pn, x, y, po->pool == B2G_POOL_MAX ? idx : nullptr, o->N, HW, o->C, part, part_idx, ticket, s); ran();
       po->splits = g_pool_last_splits;
       k_global_pool_bwd(prec, po->pool, pn, eo, x, y, idx, ei, o->N, HW, o->C, s); ran();
-      B2(downT(out0, y, no)); B2(downT(out1, ei, ni));
+      B2(m.downT(out0, y, no)); B2(m.downT(out1, ei, ni));
       if (out2) {
         std::vector<int32_t> h(no); CU(cudaMemcpyAsync(h.data(), idx, 4 * no, cudaMemcpyDeviceToHost, s)); CU(cudaStreamSynchronize(s));
         for (size_t i = 0; i < no; ++i) out2[i] = (float)h[i];
@@ -2144,10 +2127,10 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
       const size_t ni = (size_t)o->N * o->H * o->W * o->C, no = ni * f * f;
       if (no > (size_t)lim) return fail(B2G_ERR_ARG, "UPSAMPLE output too large");
       void *x = nullptr, *eo = nullptr, *y = nullptr, *ei = nullptr;
-      B2(upT(in0, ni, &x)); B2(upT(in1, no, &eo)); B2(dev(no, ts, &y)); B2(dev(ni, ts, &ei)); B2(poison(y, ts * no)); B2(poison(ei, ts * ni));
+      B2(m.upT(in0, ni, &x, off)); B2(m.upT(in1, no, &eo, off)); B2(m.dev(no, ts, &y, off)); B2(m.dev(ni, ts, &ei, off)); B2(poison(y, ts * no)); B2(poison(ei, ts * ni));
       k_upsample_fwd(prec, x, y, o->N, o->H, o->W, o->C, f, s); ran();
       k_upsample_bwd(prec, eo, ei, o->N, o->H, o->W, o->C, f, s); ran();
-      B2(downT(out0, y, no)); B2(downT(out1, ei, ni));
+      B2(m.downT(out0, y, no)); B2(m.downT(out1, ei, ni));
       break;
     }
     case B2G_EW_SUMSQ: {
@@ -2155,7 +2138,7 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
       for (int i = 0; i < o->n_seg; ++i)
         if (o->seg_off[i] < 0 || o->seg_len[i] < 0 || o->seg_off[i] + o->seg_len[i] > o->n) return fail(B2G_ERR_ARG, "segment %d outside the tensor", i);
       float *p = nullptr, *coef = nullptr; int64_t *so = nullptr, *sl = nullptr; double* res = nullptr;
-      B2(upF(in0, (size_t)o->n, &p)); B2(upF(o->seg_coef, (size_t)o->n_seg, &coef)); B2(dev((size_t)o->n_seg, 8, (void**)&so)); B2(dev((size_t)o->n_seg, 8, (void**)&sl)); B2(dev(1, 8, (void**)&res));
+      B2(m.upF(in0, (size_t)o->n, &p, off)); B2(m.upF(o->seg_coef, (size_t)o->n_seg, &coef, off)); B2(m.dev((size_t)o->n_seg, 8, (void**)&so, off)); B2(m.dev((size_t)o->n_seg, 8, (void**)&sl, off)); B2(m.dev(1, 8, (void**)&res, off));
       CU(cudaMemcpyAsync(so, o->seg_off, 8 * (size_t)o->n_seg, cudaMemcpyHostToDevice, s)); CU(cudaMemcpyAsync(sl, o->seg_len, 8 * (size_t)o->n_seg, cudaMemcpyHostToDevice, s));
       B2(poison(res, 8));
       k_sumsq_segments(p, so, sl, coef, o->n_seg, res, s); ran();
@@ -2212,9 +2195,11 @@ extern "C" int32_t b2g_test_hbm_kernels(b2g_net* n, int32_t rows, int32_t channe
   if (!n || !ms3 || rows < 8 || iters < 1) return fail(B2G_ERR_ARG, "bad arguments"); b2g_ctx* c = n->ctx; CU(cudaSetDevice(c->device)); cudaStream_t s = c->stream;
   if (!k_bn_vec_ok(PREC_BF16, channels)) return fail(B2G_ERR_UNSUPPORTED, "channels %d not supported by the vector BatchNorm kernels", channels);
   const size_t ne = (size_t)rows * channels; __nv_bfloat16 *x = nullptr, *e = nullptr, *y = nullptr; float *coef = nullptr, *gb = nullptr; unsigned long long* acc = nullptr;
-  CU(cudaMalloc(&x, 2 * ne)); CU(cudaMalloc(&e, 2 * ne)); CU(cudaMalloc(&y, 2 * ne)); CU(cudaMalloc(&coef, 4 * 4 * channels)); CU(cudaMalloc(&gb, 4 * 4 * channels)); CU(cudaMalloc(&acc, 8 * k_bn_acc_elems(channels, 1)));
+  HookMem m(s, PREC_BF16);
+  B2(m.dev(ne, 2, (void**)&x)); B2(m.dev(ne, 2, (void**)&e)); B2(m.dev(ne, 2, (void**)&y)); B2(m.upF(nullptr, 4 * (size_t)channels, &coef)); B2(m.upF(nullptr, 4 * (size_t)channels, &gb));
+  B2(m.dev(k_bn_acc_elems(channels, 1), 8, (void**)&acc));
   CU(cudaMemsetAsync(x, 0x3c, 2 * ne, s)); CU(cudaMemsetAsync(e, 0x3c, 2 * ne, s)); CU(cudaMemsetAsync(acc, 0, 8 * k_bn_acc_elems(channels, 1), s)); k_fill_f32(coef, 1.0f, 4 * channels, s); k_fill_f32(gb, 1.0f, 4 * channels, s);
-  cudaEvent_t e0, e1; CU(cudaEventCreate(&e0)); CU(cudaEventCreate(&e1));
+  cudaEvent_t e0, e1; B2(m.event(&e0)); B2(m.event(&e1));
   ms3[0] = ms3[1] = ms3[2] = 0.f;
   for (int which = 0; which < 3; ++which) for (int it = -1; it < iters; ++it) {
     B2(b2g_flush_l2(c));
@@ -2227,6 +2212,5 @@ extern "C" int32_t b2g_test_hbm_kernels(b2g_net* n, int32_t rows, int32_t channe
     float ms = 0.f; CU(cudaEventElapsedTime(&ms, e0, e1)); if (it >= 0) ms3[which] += ms / iters;
   }
   CHECK_KERNELS();
-  cudaEventDestroy(e0); cudaEventDestroy(e1); cudaFree(x); cudaFree(e); cudaFree(y); cudaFree(coef); cudaFree(gb); cudaFree(acc);
   return 0;
 }
