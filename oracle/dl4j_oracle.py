@@ -37,6 +37,8 @@ include/b200gan.h):
   * the updaters of b2g_updater                    -> ``UpdaterCfg``, ``init_state``, ``update``
   * L2 gradient normalization                      -> ``Net.set_gradient_normalization``, ``normalize``
   * learning-rate schedules (ISchedule)            -> ``Net.set_lr_schedule``, ``value``, ``lr_at``
+  * CnnLossLayer (B2G_LAYER_CNN_LOSS)              -> ``CnnLossLayer``
+  * ElementWiseVertex / MergeVertex (b2g_elementwise_op) -> ``ElementWiseVertex`` / ``MergeVertex``, the skip edges of ``Net``
 ``net_from_specs`` builds a Net from the layer specs the CUDA engine consumes.
 
 Layouts follow DL4J: activations NCHW, conv W [nOut,nIn,kH,kW] 'c' order flattened as [b | W],
@@ -81,6 +83,8 @@ class Quirks:
     # L2 gradient normalization
     bn_stats_normalized: bool = True         # BatchNorm mean/var pseudo-gradients count in the layer's norm and are scaled
     l2norm_zero_floor: float = 1e-5          # Renormalize divides by this instead of a zero norm
+    # CnnLossLayer.computeScore: score /= getInputMiniBatchSize() (True); False: the row mean over N*H*W (score and gradient / (H*W) more)
+    cnn_loss_score_per_minibatch: bool = True
 
 
 DEFAULT_QUIRKS = Quirks()
@@ -1112,6 +1116,56 @@ class LossLayer(Layer):
         return s, g.reshape(z.shape)
 
 
+def to_rows(a):
+    """[N, C, H, W] -> [N*H*W, C] (pixel-major, channel-minor: the engine's NHWC buffer)."""
+    return np.ascontiguousarray(np.moveaxis(a, 1, -1)).reshape(-1, a.shape[1])
+
+
+def from_rows(r, shape):
+    n, c, h, w = shape
+    return np.ascontiguousarray(r.reshape(n, h, w, c).transpose(0, 3, 1, 2))
+
+
+def softmax_channels(z):
+    """The softmax over dimension 1: the classes of [N, C] rows, the channels of each pixel of an [N, C, H, W] map."""
+    e = np.exp(z - z.max(1, keepdims=True))
+    return e / e.sum(1, keepdims=True)
+
+
+class CnnLossLayer(LossLayer):
+    """CnnLossLayer.Builder(loss).activation(act) (B2G_LAYER_CNN_LOSS): no parameters.  The [N, C, H, W] map becomes [N*H*W, C] rows
+    (reshape4dTo2d), each row takes the loss of LossLayer / Output, and the score is summed over the rows.  forward returns the activated map
+    (sigmoid for XENT, the per-pixel softmax over the channels for MCXENT, act otherwise).  The score's divisor, the minibatch rather than the
+    pixel count, is a medium-confidence recall behind Quirks.cnn_loss_score_per_minibatch."""
+
+    def __init__(self, name="", quirks: Optional[Quirks] = None, loss="xent", activation="identity", alpha=0.01):
+        super().__init__(name, quirks, loss, activation, alpha)
+        if loss == "mcxent":
+            self.loss_act = "softmax"
+
+    def forward(self, x, train):
+        x = np.asarray(x)
+        if x.ndim == 2:                       # a feed-forward input is the 1x1 map
+            x = x.reshape(x.shape + (1, 1))
+        self._z = x
+        if self.loss == "mcxent":
+            return softmax_channels(x)
+        return _layer_act_forward(self.loss_act, x, self.loss_alpha, self.q)
+
+    def score_and_eps(self, y):
+        z = self._z
+        zr, yr = to_rows(z), to_rows(np.asarray(y, z.dtype).reshape(z.shape))
+        if self.loss == "mcxent":
+            s, g = mcxent_softmax_score_and_grad(zr, yr)
+        else:
+            s, g = _loss_score_and_grad(self, zr, yr)
+        g = from_rows(g, z.shape)
+        if not self.q.cnn_loss_score_per_minibatch:
+            hw = z.shape[2] * z.shape[3]
+            s, g = s / hw, g / hw
+        return float(s), g
+
+
 class Output(Dense):
     """OutputLayer.Builder(loss).activation(act).nOut(n) = Dense + the loss on act(z); XENT is on the sigmoid (J:159-163)."""
 
@@ -1153,9 +1207,7 @@ class OutputSoftmax(Dense):
         super().__init__(n_in, n_out, activation="identity", updater=updater, l2=l2, name=name)
 
     def forward(self, x, train):
-        z = super().forward(x, train)
-        e = np.exp(z - z.max(1, keepdims=True))
-        return e / e.sum(1, keepdims=True)
+        return softmax_channels(super().forward(x, train))
 
     def score_and_eps(self, y):
         return mcxent_softmax_score_and_grad(self._z, y)
@@ -1167,7 +1219,86 @@ class OutputSoftmax(Dense):
 
 
 # --------------------------------------------------------------------------------------------------
-# Network = ComputationGraph restricted to a chain (every graph in the reference is a chain).
+# Graph vertices (B2G_LAYER_ELEMENTWISE / B2G_LAYER_MERGE, semantics at b2g_elementwise_op in include/b200gan.h).  A vertex reads the
+# spine (the layer before it) and the output of an earlier layer, its skip source `src` (an index into the Net's layers).  order 0: the
+# inputs are (spine, skip); order 1: (skip, spine).  forward(x_spine, x_skip, train); backward(eps) -> (eps_spine, eps_skip).
+# --------------------------------------------------------------------------------------------------
+EW_OPS = ("add", "subtract", "product", "average", "max")
+
+
+def ew_forward(op, a, b):
+    if op == "add":
+        return a + b
+    if op == "subtract":
+        return a - b
+    if op == "product":
+        return a * b
+    if op == "average":
+        return (a + b) * 0.5
+    return np.where(a >= b, a, b)           # a tie takes the first input
+
+
+def ew_backward(op, e, a, b):
+    """(dL/da, dL/db) of ew_forward; MAX sends e to the larger input, a tie to the first."""
+    if op == "add":
+        return e, e
+    if op == "subtract":
+        return e, -e
+    if op == "product":
+        return e * b, e * a
+    if op == "average":
+        return e * 0.5, e * 0.5
+    first = a >= b
+    return np.where(first, e, 0.0), np.where(first, 0.0, e)
+
+
+class Vertex(Layer):
+    def __init__(self, src, order, name=""):
+        self.src, self.order, self.name = src, order, name
+
+    def out_shape(self, s, s_skip):
+        return s
+
+
+class ElementWiseVertex(Vertex):
+    """new ElementWiseVertex(op): no parameters."""
+
+    def __init__(self, op, src, order, name=""):
+        if op not in EW_OPS:
+            raise ValueError(op)
+        super().__init__(src, order, name)
+        self.op = op
+
+    def forward(self, x, skip, train):
+        self._a, self._b = (x, skip) if self.order == 0 else (skip, x)
+        return ew_forward(self.op, self._a, self._b)
+
+    def backward(self, eps):
+        da, db = ew_backward(self.op, eps, self._a, self._b)
+        return (da, db) if self.order == 0 else (db, da)
+
+
+class MergeVertex(Vertex):
+    """new MergeVertex(): the inputs concatenated along dimension 1 in input order; no parameters."""
+
+    def out_shape(self, s, s_skip):
+        return (s[0], s[1] + s_skip[1]) + tuple(s[2:])
+
+    def forward(self, x, skip, train):
+        first, second = (x, skip) if self.order == 0 else (skip, x)
+        self._c = first.shape[1]
+        return np.concatenate((first, second), axis=1)
+
+    def backward(self, eps):
+        first, second = eps[:, :self._c], eps[:, self._c:]
+        spine, skip = (first, second) if self.order == 0 else (second, first)
+        return np.ascontiguousarray(spine), np.ascontiguousarray(skip)
+
+
+# --------------------------------------------------------------------------------------------------
+# Network = ComputationGraph as a spine plus skip edges: layer i reads layer i-1's output, and a vertex also reads its skip source's.
+# (Every graph in the reference is a chain.)  The backward walks the spine in reverse; a vertex leaves the skip input's share of its epsilon
+# in the source's accumulator, which joins the spine epsilon when the walk reaches the source.
 # --------------------------------------------------------------------------------------------------
 class Net:
     """mask_seed, rank: the DropoutLayer masks' seed and rank (the library's b2g_net_config.seed and the replica's rank)."""
@@ -1182,6 +1313,7 @@ class Net:
         self.gradient_normalization, self.gradient_normalization_threshold, self.grad_norm_last_norms = "none", 1.0, []
         self.schedules: Dict[str, dict] = {}      # layer name -> schedule (None: the constant lr)
         self.dropout = DropoutState(mask_seed, rank)
+        self._skip_acc: Dict[int, np.ndarray] = {}    # skip source index -> the skip shares the current backward has met
         rng = np.random.default_rng(seed)
         for l in self.layers:
             if "q" not in vars(l):        # a layer built with its own quirks, or already in a net, keeps them
@@ -1274,29 +1406,43 @@ class Net:
 
     # ---- forward / backward --------------------------------------------------------------------
     def forward(self, x, train: bool, collect: bool = False):
+        self._skip_acc = {}
         acts = []
         a = np.asarray(x, self.dtype)
         for l in self.layers:
             # FrozenLayer (TransferLearning.setFeatureExtractor, J:350) always runs its layer in test mode
-            a = l.forward(a, train and not getattr(l, "frozen", False))
-            if collect:
-                acts.append(a)
+            t = train and not getattr(l, "frozen", False)
+            a = l.forward(a, acts[l.src], t) if isinstance(l, Vertex) else l.forward(a, t)
+            acts.append(a)
         return (a, acts) if collect else a
 
     def output(self, x):
         """ComputationGraph.output(x): inference mode => BatchNorm uses its mean/var parameters (J:420)."""
         return self.forward(x, train=False)
 
-    def backward_from(self, eps, stop_at: int = 0, collect: bool = False):
-        """Back-propagate eps (w.r.t. the output of the last non-loss layer handled by the caller)."""
+    def _backward(self, eps, lo: int, hi: int, collect: bool):
+        """The backward walk: layers hi-1 down to lo, LossLayers left to the caller.  A vertex's skip share goes into its source's accumulator
+        (the first consumer visited writes it, later ones add); a source adds its accumulator to the spine epsilon before its own backward."""
         epss = []
-        for l in reversed(self.layers[stop_at:]):
+        for i in range(hi - 1, lo - 1, -1):
+            l = self.layers[i]
             if isinstance(l, LossLayer):
                 continue
-            eps = l.backward(eps)
+            acc = self._skip_acc.pop(i, None)
+            if acc is not None:
+                eps = eps + acc.reshape(eps.shape)
+            if isinstance(l, Vertex):
+                eps, g = l.backward(eps)
+                self._skip_acc[l.src] = self._skip_acc[l.src] + g if l.src in self._skip_acc else g
+            else:
+                eps = l.backward(eps)
             if collect:
                 epss.append(eps)
         return (eps, epss[::-1]) if collect else eps
+
+    def backward_from(self, eps, stop_at: int = 0, collect: bool = False):
+        """Back-propagate eps (w.r.t. the output of the last non-loss layer handled by the caller)."""
+        return self._backward(eps, stop_at, len(self.layers), collect)
 
     def l2_score(self):
         s = 0.0
@@ -1313,29 +1459,26 @@ class Net:
         if pass_ is not None and self._has_active_dropout():
             self.dropout.queue.append((pass_, row0))
         out, acts = self.forward(x, train=True, collect=True)
-        last = self.layers[-1]
-        y = np.asarray(y, self.dtype)
-        loss_sum, eps = last.score_and_eps(y)
-        mb = x.shape[0]
-        if isinstance(last, (Output, OutputSoftmax)):
-            eps_in = last.backward(eps)
-            eps_in, epss = self.backward_from_prefix(eps_in, collect=True)
-        else:
-            eps_in, epss = self.backward_from_prefix(eps, collect=True)
-        score = float(loss_sum) / mb + self.l2_score()
+        loss_sum, eps_in, epss = self._loss_backward(y)
+        score = float(loss_sum) / x.shape[0] + self.l2_score()
         if collect:
             return score, acts, epss, eps_in
         return score
 
+    def _loss_backward(self, y):
+        """After a forward: the last layer's score on labels y, then the backward of its own parameters (an OutputLayer's) and the prefix.
+        Returns (loss sum, eps at the prefix's input, the prefix's epsilons)."""
+        last = self.layers[-1]
+        loss_sum, eps = last.score_and_eps(np.asarray(y, self.dtype))
+        if last.has_params:
+            eps = last.backward(eps)
+        return (loss_sum,) + self.backward_from_prefix(eps, collect=True)
+
     def backward_from_prefix(self, eps, collect=False):
         """Backprop through all layers except the final loss-bearing one; stops at the frozen feature extractor."""
-        epss = []
-        for l in reversed(self.layers[:-1]):
-            if getattr(l, "frozen", False):
-                break
-            eps = l.backward(eps)
-            epss.append(eps)
-        return (eps, epss[::-1]) if collect else eps
+        hi = len(self.layers) - 1
+        lo = max((i + 1 for i in range(hi) if getattr(self.layers[i], "frozen", False)), default=0)
+        return self._backward(eps, lo, hi, collect)
 
     # ---- updater: BaseMultiLayerUpdater.update + UpdaterBlock + params.subi ----------------------
     def apply_update(self, mb: int, grads: Optional[Dict[Tuple[int, str], np.ndarray]] = None, frozen_from: Optional[int] = None):
@@ -1435,15 +1578,9 @@ def gan_step(G: Net, D: Net, x_real, z_d, z_g, y_real, y_fake, y_gen, fake_bn_tr
     # --- G step (through D, D untouched)
     xg = G.forward(z_g, train=True)
     D.forward(xg, train=True)
-    last = D.layers[-1]
-    loss_sum, eps = last.score_and_eps(np.asarray(y_gen, D.dtype))
-    if isinstance(last, Output):
-        eps = last.backward(eps)
     d_params_before = {(li, p): l.params[p] for li, l in enumerate(D.layers) if l.has_params for p, _, _ in l.param_specs()}
-    eps_x = D.backward_from_prefix(eps)
-    eps_g = eps_x.reshape(xg.shape)
-    for l in reversed(G.layers):
-        eps_g = l.backward(eps_g)
+    loss_sum, eps_x, _ = D._loss_backward(y_gen)
+    G.backward_from(eps_x.reshape(xg.shape))
     G.apply_update(n)
     for (li, p), v in d_params_before.items():
         D.layers[li].params[p] = v
@@ -1605,11 +1742,13 @@ def net_from_specs(specs, input_shape, *, quirks: Quirks = DEFAULT_QUIRKS, dtype
     """The Net of the layer specs the CUDA engine consumes.  input_shape: (C,H,W) or (F,).  flat_input: prepend the convolutionalFlat
     reshape (the oracle's layer indices are then the specs' + 1).  A spec's scheduled lr becomes the layer's schedule; its constant lr is
     the schedule's value at 0, as the library keeps it.  An activation's alpha defaults as engine.layer_desc fills it.  A DropoutLayer's
-    mask index is its position in `specs` (the library's index).  mask_seed, rank: see Net."""
+    mask index is its position in `specs` (the library's index).  A vertex's inputs are resolved by vertex_inputs.  mask_seed, rank: see Net."""
     layers = []
     shape = (1,) + tuple(input_shape)
     if len(input_shape) == 3 and flat_input:
         layers.append(Reshape(tuple(input_shape), name="in_reshape"))      # convolutionalFlat accepts [N,784] or [N,1,28,28]
+    shapes = [shape] * len(layers)          # each layer's output shape
+    skips = vertex_inputs(specs, len(layers))
     schedules = {}
     for i, s in enumerate(specs):
         t, name = s["type"], s.get("name", "")
@@ -1632,6 +1771,14 @@ def net_from_specs(specs, input_shape, *, quirks: Quirks = DEFAULT_QUIRKS, dtype
             l = Output(n_in, s["n_out"], u, s.get("l2", 0.0), name, loss=s.get("loss", "xent"), activation=act, alpha=alpha)
         elif t == "loss":
             l = LossLayer(name, loss=s.get("loss", "xent"), activation=act, alpha=alpha)
+        elif t == "cnn_loss":
+            if i != len(specs) - 1:
+                raise ValueError("a cnn_loss spec must be the last layer")
+            l = CnnLossLayer(name, loss=s.get("loss", "xent"), activation=act, alpha=alpha)
+        elif t == "elementwise":
+            l = ElementWiseVertex(s["op"], *skips[i], name)
+        elif t == "merge":
+            l = MergeVertex(*skips[i], name)
         elif t == "batchnorm":
             l = BatchNorm(shape[1], s.get("decay", 0.9), s.get("eps", 1e-5), u, name)
         elif t == "activation":
@@ -1655,8 +1802,29 @@ def net_from_specs(specs, input_shape, *, quirks: Quirks = DEFAULT_QUIRKS, dtype
         if s.get("frozen", False):
             l.frozen = True
         layers.append(l)
-        shape = l.out_shape(shape)
+        shape = l.out_shape(shape, shapes[l.src]) if isinstance(l, Vertex) else l.out_shape(shape)
+        shapes.append(shape)
     net = Net(layers, seed=seed, dtype=dtype, grad_clip=grad_clip, quirks=quirks, mask_seed=mask_seed, rank=rank)
     for name, sched in schedules.items():
         net.set_lr_schedule(sched, name)
     return net
+
+
+def vertex_inputs(specs, off=0):
+    """Each vertex spec's "inputs" as (j, order): j the skip source's layer index (its position in the specs + off), order 0 when the inputs
+    are (spine, source) and 1 when they are (source, spine); None for the other specs.  The spine is the previous spec and the source the one
+    earlier spec of the other name.  ValueError for any other graph."""
+    out = []
+    for i, s in enumerate(specs):
+        if s["type"] not in ("elementwise", "merge"):
+            out.append(None)
+            continue
+        inputs, earlier = list(s.get("inputs", ())), [p.get("name", "") for p in specs[:i]]
+        if len(inputs) != 2 or not earlier or earlier[-1] not in inputs:
+            raise ValueError(f"vertex {s.get('name', '')!r}: inputs {inputs} are not the previous layer and one skip source")
+        order = 0 if inputs[0] == earlier[-1] else 1
+        hits = [j for j, name in enumerate(earlier) if name == inputs[1 - order]]
+        if len(hits) != 1:
+            raise ValueError(f"vertex {s.get('name', '')!r}: input {inputs[1 - order]!r} names {len(hits)} earlier layers (needs exactly one)")
+        out.append((hits[0] + off, order))
+    return out

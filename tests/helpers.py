@@ -28,6 +28,45 @@ def rel_err(a, b):
     return float(np.abs(a - b).max() / (np.abs(b).max() + 1e-30))
 
 
+def pclose(got, want, bound, tol=2e-3):
+    """Every element within tol of want's largest magnitude; else every element within bound and at most 2% of them beyond tol."""
+    d = np.abs(np.asarray(got, np.float64) - np.asarray(want, np.float64))
+    if d.max() < tol * np.abs(want).max():
+        return True
+    return d.max() <= bound and (d > tol * np.abs(want).max()).mean() <= 0.02
+
+
+def gan_step_parity(b, ctx, gs, ds, G, D, data, labels, lr, what, tol=1e-3):
+    """The FP32 adversarial step of the library against the oracle's, on copies of the oracle nets G, D (specs gs, ds): over 3 steps on data
+    (x_real, z_d, z_g and per-image labels), oracle gan_step with `labels` and Gan.step agree on the losses within tol and on both nets'
+    parameters by pclose at 2 lr, once captured as a CUDA graph and once eager; the two runs agree bit for bit.  The discriminator has one
+    output per label of an image."""
+    import copy
+    from oracle import dl4j_oracle as o
+    n, size, z = data[0].shape[0], data[0].shape[-1], data[1].shape[1]
+    results = {}
+    for graph in (True, False):
+        Gc, Dc = copy.deepcopy(G), copy.deepcopy(D)
+        bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
+        bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2)
+        assert bD.out_elems == labels[0][0].size
+        push_params(Gc, bG); push_params(Dc, bD)
+        gan = b.Gan(bG, bD, use_cuda_graph=graph)
+        ls = []
+        for it in range(3):
+            r = o.gan_step(Gc, Dc, *data[:3], *labels)
+            lo = gan.step(*data)
+            ls.append(lo)
+            want = np.array([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]])
+            assert np.all(np.abs(lo - want) < tol * np.maximum(1, np.abs(want))), (what, graph, it, lo, want)
+            assert pclose(bD.params(), Dc.params_flat(), 2 * lr), (what, it, "D", rel_err(bD.params(), Dc.params_flat()))
+            assert pclose(bG.params(), Gc.params_flat(), 2 * lr), (what, it, "G", rel_err(bG.params(), Gc.params_flat()))
+        results[graph] = (np.array(ls), bG.params(), bD.params())
+        gan.close(); bG.close(); bD.close()
+    for u, v in zip(results[True], results[False]):
+        assert np.array_equal(u, v), "graph replay == eager"
+
+
 def bf16_round(a):
     """fp32 -> bf16 -> fp32 with round-to-nearest-even, the rounding of the kernels' __float2bfloat16_rn."""
     import torch

@@ -1,4 +1,4 @@
-"""CnnLossLayer on the CPU: the restatement (tests/cnn_loss_ref.py) against finite differences at GradientCheckUtil's tolerances, alone and in
+"""CnnLossLayer on the CPU: the oracle's CnnLossLayer against finite differences at GradientCheckUtil's tolerances, alone and in
 conv -> [BN ->] act -> conv -> CnnLossLayer nets with odd H / W and in the adversarial step; float64 torch; hand-computed answers on a 2x2
 map; the 1x1 map against LossLayer; the layer specs, the PatchGAN discriminator builder and the codes shared with the header."""
 import copy
@@ -8,7 +8,6 @@ import re
 import numpy as np
 import pytest
 
-from cnn_loss_ref import CnnLossLayer, CnnQuirks, net_from_specs, to_rows
 from helpers import randomize
 from oracle import dl4j_oracle as o
 
@@ -31,7 +30,7 @@ def _labels(kind, rng, shape):
 
 
 def _layer(loss, act):
-    l = CnnLossLayer("cl", loss=loss, activation=act)
+    l = o.CnnLossLayer("cl", loss=loss, activation=act)
     l.init(None, np.float64)
     return l
 
@@ -72,7 +71,7 @@ def test_net_finite_differences(loss, act, kind, n_out, bn):
     if loss == "mcxent" and n_out == 1:
         pytest.skip("a softmax over one channel is constant")
     specs = _net(n_out, bn, loss, act)
-    net = net_from_specs(specs, (2, 7, 5), seed=4, flat_input=False)
+    net = o.net_from_specs(specs, (2, 7, 5), seed=4, flat_input=False)
     rng = np.random.default_rng(n_out * 7 + bn)
     randomize(net, rng)
     x = rng.uniform(-1, 1, (3, 2, 7, 5))
@@ -95,7 +94,7 @@ def _patch_gan(loss="xent"):
     size, z, nf = 16, 6, 4
     gs = m.dcgan_generator(size, z, nf, 3, lr=1e-2)
     ds = m.dcgan_discriminator(size, nf, 3, lr=1e-2, loss=loss, patch=True)
-    G = net_from_specs(gs, (z,), seed=1); D = net_from_specs(ds, (3, size, size), seed=2)
+    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
     rng = np.random.default_rng(5)
     randomize(G, rng); randomize(D, rng)
     return G, D, z, size
@@ -171,7 +170,7 @@ def test_hand_computed_2x2():
     assert np.isclose(s, 4 * np.log(2)) and np.allclose(g, 0.5 - y)       # 4 pixels, each -log 1/2
     lay = _layer("mse", "identity"); lay.forward(z, True); s, g = lay.score_and_eps(y)
     assert np.isclose(s, 4 * 1 / 2) and np.allclose(g, (0 - y) * 2 / 2)    # per pixel (1^2 + 0^2) / C
-    lay = CnnLossLayer("cl", loss="mse", cq=CnnQuirks(cnn_loss_score_per_minibatch=False)); lay.init(None, np.float64)
+    lay = o.CnnLossLayer("cl", o.Quirks(cnn_loss_score_per_minibatch=False), loss="mse"); lay.init(None, np.float64)
     lay.forward(z, True); s2, g2 = lay.score_and_eps(y)
     assert np.isclose(s2, s / 4) and np.allclose(g2, g / 4)
 
@@ -190,7 +189,7 @@ def test_1x1_map_equals_loss_layer(loss, act, kind):
 
 def test_rows_are_the_nhwc_buffer():
     a = np.arange(2 * 3 * 2 * 2).reshape(2, 3, 2, 2)
-    assert np.array_equal(to_rows(a).ravel(), a.transpose(0, 2, 3, 1).ravel())
+    assert np.array_equal(o.to_rows(a).ravel(), a.transpose(0, 2, 3, 1).ravel())
 
 
 # ------------------------------------------------------------------ specs ------------------------------------------------------------
@@ -223,7 +222,7 @@ def test_patch_discriminator_shapes_and_parameter_counts(size, side):
     full, patch = m.dcgan_discriminator(size, nf, 3), m.dcgan_discriminator(size, nf, 3, patch=True)
     assert full[:len(patch) - 2] == patch[:-2]
     assert patch[-2]["kernel"] == (3, 3) and patch[-2]["padding"] == (1, 1) and patch[-2]["n_out"] == 1 and patch[-1]["type"] == "cnn_loss"
-    D = net_from_specs(patch, (3, size, size), flat_input=False)
+    D = o.net_from_specs(patch, (3, size, size), flat_input=False)
     out = D.forward(np.zeros((2, 3, size, size)), train=False)
     assert out.shape == (2, 1, side, side)
     ch = patch[-2]["n_in"]
@@ -236,4 +235,4 @@ def test_patch_discriminator_shapes_and_parameter_counts(size, side):
 
 def test_cnn_loss_must_be_last():
     with pytest.raises(ValueError):
-        net_from_specs([{"type": "cnn_loss", "name": "a"}, {"type": "cnn_loss", "name": "b"}], (1, 2, 2), flat_input=False)
+        o.net_from_specs([{"type": "cnn_loss", "name": "a"}, {"type": "cnn_loss", "name": "b"}], (1, 2, 2), flat_input=False)

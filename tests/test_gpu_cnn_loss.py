@@ -1,15 +1,12 @@
 """CnnLossLayer on the GPU: the per-pixel loss kernels (b2g_test_ew ops cnn_xent / cnn_softmax_xent) against fp32 / float64 emulations of their
 documented formulas and order, on one block and many, groups 1 and 2, C in {1, 3, 5, 16}, aligned and odd offsets, poisoned outputs -- the
-vector and scalar paths give the same bits and so do two runs; FP32 nets ending in CnnLossLayer against the oracle's restatement
-(tests/cnn_loss_ref.py) over 3 fit iterations; a BF16 net; the adversarial step with a PatchGAN discriminator against the oracle, graph replay
+vector and scalar paths give the same bits and so do two runs; FP32 nets ending in CnnLossLayer against the oracle over 3 fit iterations; a
+BF16 net; the adversarial step with a PatchGAN discriminator against the oracle, graph replay
 against eager, per-image labels against the same labels as maps, and the refusals."""
-import copy
-
 import numpy as np
 import pytest
 
-from cnn_loss_ref import net_from_specs
-from helpers import bf16_round, check_bf16, push_params, randomize, rel_err
+from helpers import bf16_round, check_bf16, gan_step_parity, push_params, randomize, rel_err
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
@@ -155,7 +152,7 @@ def test_fp32_nets_match_oracle(b200, loss, act, c):
     b, ctx = b200
     specs, shape = _specs(loss, act, c)
     rng = np.random.default_rng(c * 13 + len(loss))
-    onet = net_from_specs(specs, shape, seed=2, flat_input=False); randomize(onet, rng)
+    onet = o.net_from_specs(specs, shape, seed=2, flat_input=False); randomize(onet, rng)
     bnet = b.Net(ctx, specs, shape, max_batch=6, precision=b.FP32)
     push_params(onet, bnet)
     assert bnet.out_elems == c * 5 * 4
@@ -181,7 +178,7 @@ def test_bf16_nets_match_oracle_loosely(b200, loss, act, c):
     specs, shape = _specs(loss, act, c)
     specs[0]["n_out"] = 64
     rng = np.random.default_rng(7)
-    onet = net_from_specs(specs, shape, seed=2, flat_input=False); randomize(onet, rng)
+    onet = o.net_from_specs(specs, shape, seed=2, flat_input=False); randomize(onet, rng)
     for l in onet.layers:
         if l.has_params and "W" in l.params:
             l.params["W"] = bf16_round(l.params["W"]).astype(np.float64)
@@ -203,22 +200,15 @@ def _patch_setup(loss, size=16, z=12, nf=8, lr=2e-3):
     gs = m.dcgan_generator(size, z, nf, 3, lr=lr)
     ds = m.dcgan_discriminator(size, nf, 3, lr=lr, loss=loss, patch=True)
     rng = np.random.default_rng(5)
-    G = net_from_specs(gs, (z,), seed=1); D = net_from_specs(ds, (3, size, size), seed=2)
+    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
     randomize(G, rng); randomize(D, rng)
     return gs, ds, G, D
-
-
-def _pclose(got, want, bound, tol=2 * TOL):
-    d = np.abs(np.asarray(got, np.float64) - np.asarray(want, np.float64))
-    if d.max() < tol * np.abs(want).max():
-        return True
-    return d.max() <= bound and (d > tol * np.abs(want).max()).mean() <= 0.02
 
 
 @pytest.mark.parametrize("loss", ["xent", "mse"])
 def test_fp32_patch_gan_step_matches_oracle(b200, loss):
     """A 16x16 DCGAN with a 4x4-patch discriminator (XENT; MSE with labels 1 / 0 / 1): losses and both nets' parameters over 3 steps; graph
-    replay equals the eager step bit for bit."""
+    replay equals the eager step bit for bit.  Gan.step takes the per-image labels and broadcasts them over the patch map."""
     b, ctx = b200
     size, z, n, lr_ = 16, 12, 8, 2e-3
     gs, ds, G, D = _patch_setup(loss)
@@ -226,27 +216,7 @@ def test_fp32_patch_gan_step_matches_oracle(b200, loss):
     if loss == "mse":
         data[3], data[4], data[5] = np.ones((n, 1)), np.zeros((n, 1)), np.ones((n, 1))
     maps = [np.broadcast_to(v.reshape(n, 1, 1, 1), (n, 1, 4, 4)).copy() for v in data[3:]]
-    G0, D0 = copy.deepcopy(G), copy.deepcopy(D)
-    results = {}
-    for graph in (True, False):
-        Gc, Dc = copy.deepcopy(G0), copy.deepcopy(D0)
-        bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
-        bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2)
-        push_params(Gc, bG); push_params(Dc, bD)
-        gan = b.Gan(bG, bD, use_cuda_graph=graph)
-        ls = []
-        for it in range(3):
-            r = o.gan_step(Gc, Dc, *data[:3], *maps)
-            lo = gan.step(*data)                   # per-image labels, broadcast over the patch map by Gan.step
-            ls.append(lo)
-            want = np.array([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]])
-            assert np.all(np.abs(lo - want) < TOL * np.maximum(1, np.abs(want))), (loss, graph, it, lo, want)
-            assert _pclose(bD.params(), Dc.params_flat(), 2 * lr_), (loss, it, "D", rel_err(bD.params(), Dc.params_flat()))
-            assert _pclose(bG.params(), Gc.params_flat(), 2 * lr_), (loss, it, "G", rel_err(bG.params(), Gc.params_flat()))
-        results[graph] = (np.array(ls), bG.params(), bD.params())
-        gan.close(); bG.close(); bD.close()
-    for u, v in zip(results[True], results[False]):
-        assert np.array_equal(u, v), "graph replay == eager"
+    gan_step_parity(b, ctx, gs, ds, G, D, data, maps, lr_, loss)
 
 
 def _bf16_run(b, ctx, gs, ds, G, D, data, n, size, z, graph=True, steps=2):
@@ -276,7 +246,7 @@ def test_bf16_patch_step_head_adds_no_simt_calls_and_label_broadcast(b200):
     simt = {}
     for patch in (False, True):
         ds = m.dcgan_discriminator(size, nf, 3, patch=patch)
-        G = net_from_specs(gs, (z,), seed=1); D = net_from_specs(ds, (3, size, size), seed=2)
+        G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
         randomize(G, rng); randomize(D, rng)
         out, simt[patch] = _bf16_run(b, ctx, gs, ds, G, D, data, n, size, z)
         assert np.isfinite(out[0]).all()

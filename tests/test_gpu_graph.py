@@ -1,15 +1,12 @@
 """Spine-plus-skip graphs on the GPU: the vertex kernels (b2g_test_ew ops vertex_fwd / vertex_bwd / merge_fwd / merge_bwd / skip_add) bit for
 bit against fp32 / bf16 emulations on the vector and scalar paths with poisoned outputs, written and accumulated; FP32 residual, U-Net,
-shared-source and feed-forward merge nets against the float64 restatement (tests/graph_ref.py) over fit iterations; BF16 nets, one per
+shared-source and feed-forward merge nets against the float64 oracle over fit iterations; BF16 nets, one per
 single-consumer fusion the engine turns off at a skip source; the adversarial step with residual nets against oracle gan_step, graph replay
 against eager; and the launch budget."""
-import copy
-
 import numpy as np
 import pytest
 
-import graph_ref as gr
-from helpers import bf16_round, push_params, randomize, rel_err
+from helpers import bf16_round, gan_step_parity, push_params, randomize, rel_err
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
@@ -38,12 +35,12 @@ def _t(a, bf):
 def _ew_ref(op, a, b):
     """ew_forward in fp32 (every op is one fp32 operation on the inputs, AVERAGE (a + b) * 0.5)."""
     a, b = a.astype(np.float32), b.astype(np.float32)
-    return gr.ew_forward(op, a, b).astype(np.float32)
+    return o.ew_forward(op, a, b).astype(np.float32)
 
 
 @pytest.mark.parametrize("prec", [0, 1])
 @pytest.mark.parametrize("offset,n", [(0, 4096 + 24), (0, 4096 + 3), (1, 1000 + 3)])
-@pytest.mark.parametrize("op", gr.OPS)
+@pytest.mark.parametrize("op", o.EW_OPS)
 def test_elementwise_kernels_bit_exact(b200, prec, offset, n, op):
     b, ctx = b200
     bf = prec == b.BF16
@@ -58,7 +55,7 @@ def test_elementwise_kernels_bit_exact(b200, prec, offset, n, op):
         (y, _, _), info = b.test_ew(ctx, prec, "vertex_fwd", sp, sk, (n, 0, 0), act=op, n=n, groups=order, offset=offset, poison=True)
         assert info["kernel"] == f"vertex_ew_fwd_kernel<{vec}>"
         assert np.array_equal(y, _t(_ew_ref(op, a, c), bf)), (op, order)
-        da, db = gr.ew_backward(op, e, a, c)
+        da, db = o.ew_backward(op, e, a, c)
         da, db = da.astype(np.float32), db.astype(np.float32)
         sp_share, sk_share = (da, db) if order == 0 else (db, da)
         for accumulate in (0, 1):
@@ -148,7 +145,7 @@ def test_fp32_graph_nets_match_oracle(b200, kind):
     b, ctx = b200
     specs, shape, loss = _nets(kind)
     rng = np.random.default_rng(21)
-    onet = gr.net_from_specs(specs, shape, seed=2, flat_input=False); randomize(onet, rng)
+    onet = o.net_from_specs(specs, shape, seed=2, flat_input=False); randomize(onet, rng)
     bnet = b.Net(ctx, specs, shape, max_batch=6, precision=b.FP32)
     push_params(onet, bnet)
     for it, mb in enumerate((6, 5, 6)):
@@ -172,7 +169,7 @@ def test_fp32_graph_nets_match_oracle(b200, kind):
 
 def _bf16_pair(b, ctx, specs, shape, seed=7, batch=8):
     rng = np.random.default_rng(seed)
-    onet = gr.net_from_specs(specs, shape, seed=2, flat_input=False); randomize(onet, rng)
+    onet = o.net_from_specs(specs, shape, seed=2, flat_input=False); randomize(onet, rng)
     for l in onet.layers:
         if l.has_params and "W" in l.params:
             l.params["W"] = bf16_round(l.params["W"]).astype(np.float64)
@@ -239,16 +236,9 @@ def _gan_setup(size=16, z=12, nf=8, lr=2e-3, patch=False):
     gs = m.dcgan_generator(size, z, nf, 3, lr=lr, residual=True)
     ds = m.dcgan_discriminator(size, nf, 3, lr=lr, residual=True, patch=patch)
     rng = np.random.default_rng(5)
-    G = gr.net_from_specs(gs, (z,), seed=1); D = gr.net_from_specs(ds, (3, size, size), seed=2)
+    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
     randomize(G, rng); randomize(D, rng)
     return gs, ds, G, D
-
-
-def _pclose(got, want, bound, tol=2 * TOL):
-    d = np.abs(np.asarray(got, np.float64) - np.asarray(want, np.float64))
-    if d.max() < tol * np.abs(want).max():
-        return True
-    return d.max() <= bound and (d > tol * np.abs(want).max()).mean() <= 0.02
 
 
 @pytest.mark.parametrize("patch", [False, True])
@@ -257,29 +247,8 @@ def test_fp32_residual_gan_step_matches_oracle(b200, patch):
     size, z, n, lr_ = 16, 12, 8, 2e-3
     gs, ds, G, D = _gan_setup(patch=patch)
     data = [a.astype(np.float64) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
-    oe = 16 if patch else 1
     labels = [np.broadcast_to(v.reshape(n, 1, 1, 1), (n, 1, 4, 4)).copy() if patch else v for v in data[3:]]
-    results = {}
-    for graph in (True, False):
-        Gc, Dc = copy.deepcopy(G), copy.deepcopy(D)
-        bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
-        bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2)
-        assert bD.out_elems == oe
-        push_params(Gc, bG); push_params(Dc, bD)
-        gan = b.Gan(bG, bD, use_cuda_graph=graph)
-        ls = []
-        for it in range(3):
-            r = o.gan_step(Gc, Dc, *data[:3], *labels)
-            lo = gan.step(*data)
-            ls.append(lo)
-            want = np.array([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]])
-            assert np.all(np.abs(lo - want) < TOL * np.maximum(1, np.abs(want))), (patch, graph, it, lo, want)
-            assert _pclose(bD.params(), Dc.params_flat(), 2 * lr_), (patch, it, "D", rel_err(bD.params(), Dc.params_flat()))
-            assert _pclose(bG.params(), Gc.params_flat(), 2 * lr_), (patch, it, "G", rel_err(bG.params(), Gc.params_flat()))
-        results[graph] = (np.array(ls), bG.params(), bD.params())
-        gan.close(); bG.close(); bD.close()
-    for u, v in zip(results[True], results[False]):
-        assert np.array_equal(u, v), "graph replay == eager"
+    gan_step_parity(b, ctx, gs, ds, G, D, data, labels, lr_, patch)
 
 
 def test_bf16_residual_gan_step_runs_and_replays(b200):

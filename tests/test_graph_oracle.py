@@ -1,5 +1,6 @@
-"""ElementWiseVertex / MergeVertex on the CPU: the float64 restatement (tests/graph_ref.py) against finite differences at GradientCheckUtil's
-tolerances and against torch.autograd, and the specs, builders and refusals of the Python host layer."""
+"""ElementWiseVertex / MergeVertex on the CPU: the oracle's vertices and skip edges against finite differences at GradientCheckUtil's
+tolerances and against torch.autograd, the oracle's vertex resolution against the library's, and the specs, builders and refusals of the
+Python host layer."""
 import numpy as np
 import pytest
 import torch
@@ -7,8 +8,6 @@ import torch
 from gan_deeplearning4j_b200 import engine as E
 from gan_deeplearning4j_b200 import models as m
 from oracle import dl4j_oracle as o
-
-import graph_ref as gr
 
 FD_EPS, MAX_REL, MIN_ABS = 1e-6, 1e-3, 1e-8      # GradientCheckUtil.checkGradients(..., 1e-6, 1e-3, 1e-8, ...)
 
@@ -66,11 +65,11 @@ def onehot_map(rng, n, c, h, w):
     return np.moveaxis(np.eye(c)[lab], -1, 1)
 
 
-@pytest.mark.parametrize("op", gr.OPS)
+@pytest.mark.parametrize("op", o.EW_OPS)
 @pytest.mark.parametrize("order", [0, 1])
 def test_elementwise_finite_differences(op, order):
     rng = np.random.default_rng(1)
-    net = gr.net_from_specs(ff_graph(op, order=order), (4,))
+    net = o.net_from_specs(ff_graph(op, order=order), (4,))
     x, y = rng.standard_normal((5, 4)), rng.standard_normal((5, 3))
     fd_check(net, x, y, rng, n_check=10 ** 6)
 
@@ -78,28 +77,28 @@ def test_elementwise_finite_differences(op, order):
 @pytest.mark.parametrize("order", [0, 1])
 def test_merge_finite_differences(order):
     rng = np.random.default_rng(2)
-    net = gr.net_from_specs(ff_graph("merge", order=order), (4,))
+    net = o.net_from_specs(ff_graph("merge", order=order), (4,))
     x, y = rng.standard_normal((5, 4)), rng.standard_normal((5, 3))
     fd_check(net, x, y, rng, n_check=10 ** 6)
 
 
-@pytest.mark.parametrize("op", gr.OPS)
+@pytest.mark.parametrize("op", o.EW_OPS)
 def test_vertex_on_its_own_predecessor_exact_ties(op):
     """j = i - 1: both inputs are the same tensor, so MAX ties on every element (all of e goes to the first input; the sum is e either way)."""
     rng = np.random.default_rng(3)
-    net = gr.net_from_specs(ff_graph(op, src="d2"), (4,))
+    net = o.net_from_specs(ff_graph(op, src="d2"), (4,))
     x, y = rng.standard_normal((5, 4)), rng.standard_normal((5, 3))
     fd_check(net, x, y, rng, n_check=10 ** 6)
 
 
 def test_max_tie_rule():
     a = np.array([1.0, 2.0, 3.0]); b = np.array([1.0, 5.0, 0.0]); e = np.array([10.0, 20.0, 30.0])
-    da, db = gr.ew_backward("max", e, a, b)
+    da, db = o.ew_backward("max", e, a, b)
     assert list(da) == [10.0, 0.0, 30.0] and list(db) == [0.0, 20.0, 0.0]
-    v = gr.ElementWiseVertex("max", 0, 1, gr.GraphState())      # order 1: (skip, spine) -> the tie goes to the skip input
-    v.gstate.outs[0] = a
-    v.forward(b, True)
-    assert list(v.backward(e)) == [0.0, 20.0, 0.0] and list(v.gstate.acc[0]) == [10.0, 0.0, 30.0]
+    v = o.ElementWiseVertex("max", 0, 1)      # order 1: (skip, spine) -> the tie goes to the skip input
+    v.forward(b, a, True)
+    spine, skip = v.backward(e)
+    assert list(spine) == [0.0, 20.0, 0.0] and list(skip) == [10.0, 0.0, 30.0]
 
 
 @pytest.mark.parametrize("builder,shape,loss", [
@@ -112,7 +111,7 @@ def test_conv_graph_finite_differences(builder, shape, loss):
         specs = m.unet(size=shape[1], nc=shape[0], n_classes=3, nf=2, depth=2, loss=loss)
     else:
         specs = shared_source_net()
-    net = gr.net_from_specs(specs, shape)
+    net = o.net_from_specs(specs, shape)
     n = 3
     x = rng.standard_normal((n,) + shape)
     out = net.forward(x, True)
@@ -122,7 +121,7 @@ def test_conv_graph_finite_differences(builder, shape, loss):
 
 def test_unet_shapes_and_macs():
     specs = m.unet(size=16, nc=3, n_classes=4, nf=8, depth=2)
-    net = gr.net_from_specs(specs, (3, 16, 16))
+    net = o.net_from_specs(specs, (3, 16, 16))
     out = net.forward(np.zeros((2, 3, 16, 16)), False)
     assert out.shape == (2, 4, 16, 16)
     merges = [s for s in specs if s["type"] == "merge"]
@@ -134,17 +133,21 @@ def test_unet_shapes_and_macs():
     assert macs == enc + dec
 
 
-def test_torch_autograd_agrees():
-    """A dense graph with every op (and a merge) in float64: the restatement's gradients against torch.autograd's."""
-    rng = np.random.default_rng(5)
+def every_op_net():
+    """d1 -> d2 -> one vertex of each op on d1 (the input order alternating) -> merge with d1 -> d3 -> output(mse)."""
     specs = [dense("d1", 6), dense("d2", 6, "sigmoid")]
     prev = "d2"
-    for k, op in enumerate(gr.OPS):
+    for k, op in enumerate(o.EW_OPS):
         specs += [m.elementwise(op, [prev, "d1"] if k % 2 == 0 else ["d1", prev], name=f"v{k}")]
         prev = f"v{k}"
-    specs += [m.merge(["d1", prev], name="mg"), dense("d3", 5),
-              {"type": "output", "name": "out", "n_out": 3, "loss": "mse", "activation": "identity", "updater": m.sgd(0.1)}]
-    net = gr.net_from_specs(specs, (4,))
+    return specs + [m.merge(["d1", prev], name="mg"), dense("d3", 5),
+                    {"type": "output", "name": "out", "n_out": 3, "loss": "mse", "activation": "identity", "updater": m.sgd(0.1)}]
+
+
+def test_torch_autograd_agrees():
+    """A dense graph with every op (and a merge) in float64: the oracle's gradients against torch.autograd's."""
+    rng = np.random.default_rng(5)
+    net = o.net_from_specs(every_op_net(), (4,))
     x, y = rng.standard_normal((5, 4)), rng.standard_normal((5, 3))
     net.compute_gradient_and_score(x, y)
     g = net.grads_flat()
@@ -152,7 +155,7 @@ def test_torch_autograd_agrees():
     P = {l.name: {k: torch.tensor(v, requires_grad=True) for k, v in l.params.items()} for l in Ls if l.has_params}
     d = lambda h, nm: h @ P[nm]["W"] + P[nm]["b"]
     h1 = torch.tanh(d(torch.tensor(x), "d1")); h = torch.sigmoid(d(h1, "d2"))
-    for k, op in enumerate(gr.OPS):
+    for k, op in enumerate(o.EW_OPS):
         a, b = (h, h1) if k % 2 == 0 else (h1, h)
         h = {"add": a + b, "subtract": a - b, "product": a * b, "average": (a + b) * 0.5, "max": torch.where(a >= b, a, b)}[op]
     h = torch.tanh(d(torch.cat([h1, h], 1), "d3"))
@@ -164,21 +167,23 @@ def test_torch_autograd_agrees():
 
 
 def test_chain_nets_unchanged_by_the_walk():
-    """A net without vertices built through the graph builder computes bit for bit what the oracle's own builder computes."""
-    specs = m.dcgan_discriminator(16, 4, 3)
-    a = gr.net_from_specs(specs, (3, 16, 16))
-    b = o.net_from_specs(specs, (3, 16, 16))
-    b.set_params_flat(a.params_flat())
+    """On a net without vertices, the Net's backward walk computes bit for bit what a plain loop over the layers computes."""
+    net = o.net_from_specs(m.dcgan_discriminator(16, 4, 3), (3, 16, 16))
     rng = np.random.default_rng(6)
     x, y = rng.standard_normal((4, 3, 16, 16)), rng.uniform(0, 1, (4, 1))
-    assert a.compute_gradient_and_score(x, y) == b.compute_gradient_and_score(x, y)
-    assert np.array_equal(a.grads_flat(), b.grads_flat())
+    score, _, _, eps_in = net.compute_gradient_and_score(x, y, collect=True)
+    walked = net.grads_flat()
+    loss_sum, eps = net.layers[-1].score_and_eps(y)      # the layers still hold the forward's inputs
+    for l in reversed(net.layers[:-1]):
+        eps = l.backward(eps)
+    assert score == float(loss_sum) / x.shape[0] + net.l2_score()
+    assert np.array_equal(walked, net.grads_flat()) and np.array_equal(eps_in, eps)
 
 
 def test_residual_gan_step_on_the_oracle():
-    """oracle.gan_step's three backward walks (backward_from_prefix and the generator's inline loop) run through the vertices."""
-    G = gr.net_from_specs(m.dcgan_generator(16, 8, 4, 3, residual=True), (8,))
-    D = gr.net_from_specs(m.dcgan_discriminator(16, 4, 3, residual=True), (3, 16, 16))
+    """oracle.gan_step's backward walks (the discriminator's prefix and the generator) run through the vertices."""
+    G = o.net_from_specs(m.dcgan_generator(16, 8, 4, 3, residual=True), (8,))
+    D = o.net_from_specs(m.dcgan_discriminator(16, 4, 3, residual=True), (3, 16, 16))
     data = [a.astype(np.float64) for a in o.synthetic_batch(4, 16, 3, 8, seed=3)]
     p0 = G.params_flat().copy()
     r = o.gan_step(G, D, *data)
@@ -217,6 +222,23 @@ def test_resolve_vertices():
     v = m.elementwise("max", ["a", "b"], name="v")
     d = E.layer_desc(v, E.resolve_vertices(base + [v])[2])
     assert (d.type, d.act, d.pre_h, d.pre_w) == (15, 4, 0, 1)
+
+
+def test_oracle_resolves_vertices_as_the_library_does():
+    """The oracle resolves every graph the tests build to the library's (j, order), and shifts j past the convolutionalFlat reshape."""
+    from test_gpu_graph import _guard_net, _nets
+    graphs = [residual_net(), shared_source_net(), every_op_net(), m.unet(size=8, nc=2, n_classes=3, nf=2, depth=2, loss="mcxent"),
+              m.unet(size=16, nc=3, n_classes=4, nf=8, depth=2)]
+    graphs += [ff_graph(v, order=order) for v in o.EW_OPS + ("merge",) for order in (0, 1)] + [ff_graph(v, src="d2") for v in o.EW_OPS]
+    graphs += [_nets(kind)[0] for kind in ("residual", "unet", "shared", "ff_merge")] + [_guard_net(g)[0] for g in ("bn_act", "fold", "bwd")]
+    for size, z, nf in ((16, 8, 4), (16, 12, 8), (32, 16, 8)):
+        graphs += [m.dcgan_generator(size, z, nf, 3, residual=True)]
+        graphs += [m.dcgan_discriminator(size, nf, 3, residual=True, patch=patch) for patch in (False, True)]
+    for specs in graphs:
+        want = E.resolve_vertices(specs)
+        assert any(want)
+        assert o.vertex_inputs(specs) == want
+        assert o.vertex_inputs(specs, 1) == [None if r is None else (r[0] + 1, r[1]) for r in want]
 
 
 @pytest.mark.parametrize("bad,msg", [
