@@ -1,5 +1,31 @@
-"""Test-only utilities for comparing the oracle's nets (oracle.dl4j_oracle.net_from_specs) with the CUDA library's."""
+"""Test-only utilities for comparing the oracle's nets (oracle.dl4j_oracle.net_from_specs) with the CUDA library's.
+
+- b200: the module-scoped fixture (b, ctx), the library and a Context on device 0.  A test module imports it (from helpers import b200),
+  which registers it in that module, so every module gets its own Context.
+- Builders: mlp_convbn_specs (the small MLP and conv + BatchNorm nets), oracle_gan_pair / fp32_gan_pair (the 16x16 DCGAN pair of the
+  oracle, and of the library with the oracle's parameters), bf16_gan (the BF16 pair of the launch-count tests).
+- Comparisons: pclose, compare_params_and_state, assert_close_up_to_sign_flips, gan_step_parity, check_bf16, inject_forward and
+  check_weight_operands; launches_per_step counts a GAN step's kernel launches; run_two_ranks runs a tools/ script on two GPUs."""
+import json
+import os
+import subprocess
+import sys
+
 import numpy as np
+import pytest
+
+from oracle import dl4j_oracle as o
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+@pytest.fixture(scope="module")
+def b200():
+    """(b, ctx): the library and a Context on device 0, closed when the module's tests are done."""
+    import gan_deeplearning4j_b200 as b
+    ctx = b.Context(0)
+    yield b, ctx
+    ctx.close()
 
 
 def randomize(net, rng, scale=None):
@@ -28,12 +54,133 @@ def rel_err(a, b):
     return float(np.abs(a - b).max() / (np.abs(b).max() + 1e-30))
 
 
-def pclose(got, want, bound, tol=2e-3):
-    """Every element within tol of want's largest magnitude; else every element within bound and at most 2% of them beyond tol."""
+def pclose(got, want, bound, tol=2e-3, step=0.0):
+    """Every element within tol of the scale, max(want's largest magnitude, step); else every element within bound and at most 2% of them
+    beyond tol.  step floors the scale: a parameter tensor that an update cancelled down to near zero (a one-element bias after one step) is
+    measured against one update step, not against its own size."""
     d = np.abs(np.asarray(got, np.float64) - np.asarray(want, np.float64))
-    if d.max() < tol * np.abs(want).max():
+    scale = max(np.abs(want).max(), step)
+    if d.max() < tol * scale:
         return True
-    return d.max() <= bound and (d > tol * np.abs(want).max()).mean() <= 0.02
+    return d.max() <= bound and (d > tol * scale).mean() <= 0.02
+
+
+def state_flat(onet, k):
+    """The oracle's updater state slot k flattened like b2g_net_get_updater_state (zeros where a parameter has none)."""
+    out = []
+    for li, _, p, shape, order in onet.param_table():
+        st = onet.state.get((li, p))
+        out.append((st[k] if st is not None and k < len(st) else np.zeros(shape)).ravel(order=order.upper()))
+    return np.concatenate(out)
+
+
+def compare_params_and_state(onet, bnet, what, tol, bounds=None):
+    """The library net's parameters and every updater state slot (2 or 3) against the oracle's, tensor by tensor, by pclose.  bounds: {layer
+    name: the lr-step exemption bound of its updater}; a layer without one has none.  A slot the oracle holds at zero is zero on the device."""
+    bounds = bounds or {}
+    p_b, p_o = bnet.params(), onet.params_flat()
+    st = bnet.updater_state(); n = bnet.num_params()
+    slots = st.size // n
+    assert slots in (2, 3)
+    s_o = [state_flat(onet, k) for k in range(slots)]
+    off = 0
+    for li, name, pn, shape, _ in onet.param_table():
+        k = int(np.prod(shape)); sl = slice(off, off + k)
+        bound = bounds.get(name, 0.0)
+        assert pclose(p_b[sl], p_o[sl], bound, tol, bound / 2), (what, name, pn, rel_err(p_b[sl], p_o[sl]))
+        for j in range(slots):
+            b_st, o_st = st[j * n:(j + 1) * n][sl], s_o[j][sl]
+            if np.abs(o_st).max() > 0:
+                assert pclose(b_st, o_st, np.inf if bound else 0.0, tol), (what, name, pn, "state", j, rel_err(b_st, o_st))
+            else:
+                assert np.all(b_st == 0), (what, name, pn, "state", j)
+        off += k
+
+
+def assert_close_up_to_sign_flips(got, want, lr, tol):
+    """An update of lr * g / (|g| + eps) (Adam's first step; RmsProp with rmsDecay = eps = 1e-8 on every step) is about lr * sign(g): an
+    element whose gradient is numerically zero may land one lr step apart.  Every difference within 2 lr (and a 1 % margin), and fewer than
+    2 % of the elements beyond tol of want's largest magnitude."""
+    d = np.abs(np.asarray(got, np.float64) - np.asarray(want, np.float64))
+    assert d.max() <= 2.02 * lr, d.max()
+    assert (d > tol * np.abs(want).max()).mean() < 2e-2, (d > tol * np.abs(want).max()).mean()
+
+
+def mlp_convbn_specs(kind, updater):
+    """(specs, input shape) of the 64 -> 256 -> 128 -> 1 MLP ("mlp": W of 8 chunks, every segment 16-byte aligned) or the conv + BatchNorm
+    net ("convbn") on 3x8x8; updater() gives each layer with parameters its updater spec."""
+    if kind == "mlp":
+        return [{"type": "dense", "name": "d1", "n_out": 256, "activation": "tanh", "updater": updater(), "l2": 1e-3},
+                {"type": "dense", "name": "d2", "n_out": 128, "activation": "lrelu", "alpha": 0.2, "updater": updater()},
+                {"type": "output", "name": "out", "n_out": 1, "updater": updater()}], (64,)
+    assert kind == "convbn", kind
+    return ([{"type": "conv2d", "name": "c1", "n_out": 8, "kernel": (3, 3), "stride": (2, 2), "padding": (1, 1), "updater": updater()},
+             {"type": "activation", "name": "a1", "activation": "lrelu", "alpha": 0.2},
+             {"type": "conv2d", "name": "c2", "n_out": 12, "kernel": (3, 3), "stride": (1, 1), "padding": (1, 1), "has_bias": False, "updater": updater()},
+             {"type": "batchnorm", "name": "bn2", "updater": updater()}, {"type": "activation", "name": "a2", "activation": "tanh"},
+             {"type": "cnn_to_ff", "name": "flat"},
+             {"type": "dense", "name": "fc", "n_out": 10, "activation": "tanh", "updater": updater()},
+             {"type": "output", "name": "out", "n_out": 1, "updater": updater()}], (3, 8, 8))
+
+
+def oracle_gan_pair(gs, ds, size=16, z=12, quirks=o.DEFAULT_QUIRKS, mask_seed=666):
+    """The oracle's G (specs gs, seed 1, on a z-vector) and D (specs ds, seed 2, on 3 x size x size images), both randomized from
+    default_rng(5), G first.  quirks: both nets'; mask_seed: D's dropout masks."""
+    rng = np.random.default_rng(5)
+    G = o.net_from_specs(gs, (z,), quirks=quirks, seed=1)
+    D = o.net_from_specs(ds, (3, size, size), quirks=quirks, seed=2, mask_seed=mask_seed)
+    randomize(G, rng); randomize(D, rng)
+    return G, D
+
+
+def fp32_gan_pair(b, ctx, gs, ds, n, size=16, z=12, quirks=o.DEFAULT_QUIRKS, mask_seed=666, g_kw=None, d_kw=None, **kw):
+    """oracle_gan_pair, the library's G (batch n) and D (batch 2n, two BatchNorm groups) holding its parameters, and the float64
+    synthetic_batch(n, size, 3, z, seed=3): (G, D, bG, bD, data).  kw: b.Net options of both library nets (precision, FP32 unless given;
+    xent_clip_eps); g_kw / d_kw: of one of them (seed, gradient_normalization)."""
+    G, D = oracle_gan_pair(gs, ds, size, z, quirks, mask_seed)
+    kw.setdefault("precision", b.FP32)
+    bG = b.Net(ctx, gs, (z,), max_batch=n, **kw, **(g_kw or {}))
+    bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, bn_groups=2, **kw, **(d_kw or {}))
+    push_params(G, bG); push_params(D, bD)
+    data = [a.astype(np.float64) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
+    return G, D, bG, bD, data
+
+
+def bf16_gan(b, ctx, gs, ds, gin, din, n):
+    """The BF16 G (input shape gin, batch n, seed 666) and D (din, batch 2n, two BatchNorm groups, seed 667) of the launch-count tests, on
+    BCE-with-logits (xent_clip_eps 0) like bench.py."""
+    G = b.Net(ctx, gs, gin, max_batch=n, precision=b.BF16, xent_clip_eps=0.0, seed=666)
+    D = b.Net(ctx, ds, din, max_batch=2 * n, precision=b.BF16, xent_clip_eps=0.0, bn_groups=2, seed=667)
+    return G, D
+
+
+def launches_per_step(ctx, gan, n):
+    """Kernel launches per resident GAN step of batch n on the uploaded data: the mean over three steps after two warm-up steps."""
+    for _ in range(2):
+        gan.step_resident(n)
+    ctx.sync(); l0 = ctx.launch_count()
+    for _ in range(3):
+        gan.step_resident(n)
+    ctx.sync()
+    return (ctx.launch_count() - l0) / 3
+
+
+def run_two_ranks(script, out_json, port, env=None, timeout=600):
+    """tools/<script> out_json on two ranks of one node under torch.distributed.run (master 127.0.0.1:port); the JSON it wrote.  Skips the
+    test on a machine with fewer than two GPUs."""
+    try:
+        import torch
+        gpus = torch.cuda.device_count()
+    except Exception:
+        gpus = 0
+    if gpus < 2:
+        pytest.skip("needs two GPUs")
+    out = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
+                          "--master-port", str(port), os.path.join(ROOT, "tools", script), str(out_json)],
+                         capture_output=True, text=True, timeout=timeout, env=env, cwd=ROOT)
+    assert out.returncode == 0, out.stdout[-800:] + out.stderr[-1500:]
+    with open(out_json) as f:
+        return json.load(f)
 
 
 def gan_step_parity(b, ctx, gs, ds, G, D, data, labels, lr, what, tol=1e-3):
@@ -42,7 +189,6 @@ def gan_step_parity(b, ctx, gs, ds, G, D, data, labels, lr, what, tol=1e-3):
     parameters by pclose at 2 lr, once captured as a CUDA graph and once eager; the two runs agree bit for bit.  The discriminator has one
     output per label of an image."""
     import copy
-    from oracle import dl4j_oracle as o
     n, size, z = data[0].shape[0], data[0].shape[-1], data[1].shape[1]
     results = {}
     for graph in (True, False):
@@ -148,3 +294,35 @@ def pack_deconv_ps(w):
                     if 0 <= s < 4:
                         out[py, px, :C, dyr + 1, dxc + 1, :] = w[:, r, s, :].T
     return out.ravel()
+
+
+def _ps_operand_O(spec):
+    """O of the [O][4][4][C] weight when the layer's conv-equivalent is a 4x4 s2 p1 conv with C <= 4 image channels and O % 64 == 0 (the
+    transposed conv onto the image, and the input gradient of the conv that reads it), else 0."""
+    if tuple(spec.get("kernel", ())) != (4, 4) or tuple(spec.get("stride", ())) != (2, 2) or tuple(spec.get("padding", ())) != (1, 1):
+        return 0
+    O, C = (spec["n_in"], spec["n_out"]) if spec["type"] == "deconv2d" else (spec["n_out"], spec["n_in"])
+    return O if C <= 4 and O % 64 == 0 else 0
+
+
+def check_weight_operands(b, net, specs, what):
+    """The bf16 weight operands a BF16 net's forward reads instead of the fp32 master: every GEMM layer's straight copy of W, and the packed
+    pixel-shuffle operand of a layer that has one, equal the master rounded to nearest even, bit for bit; a layer without one refuses the
+    request with B2G_ERR_UNSUPPORTED (-6).  Returns how many packed operands were checked."""
+    packed = 0
+    for li, s in enumerate(specs):
+        if s["type"] not in ("conv2d", "deconv2d", "dense", "output"):
+            continue
+        k = s.get("kernel", (1, 1)); size = s["n_in"] * s["n_out"] * k[0] * k[1]
+        w = bf16_round(w_internal(s, net.get_param(s["name"], "W", size)))
+        assert np.array_equal(net.weight_operand(li, 0, size), w), f"{what}: bf16 copy of {s['name']}.W differs from the rounded master"
+        O = _ps_operand_O(s)
+        if O:
+            got = net.weight_operand(li, 1, 144 * O)
+            assert np.array_equal(got, pack_deconv_ps(w.reshape(O, 4, 4, -1))), f"{what}: packed pixel-shuffle operand of {s['name']}"
+            packed += 1
+        else:
+            with pytest.raises(b.B200GanError) as e:
+                net.weight_operand(li, 1, 144)
+            assert e.value.code == -6
+    return packed

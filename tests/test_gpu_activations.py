@@ -8,25 +8,13 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from helpers import bf16_round, check_bf16, push_params, randomize, rel_err
+from gan_deeplearning4j_b200 import models as m
+from helpers import b200, bf16_round, check_bf16, fp32_gan_pair, launches_per_step, pclose, push_params, randomize, rel_err
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
 U = 2.0 ** -24
-
-
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
-
-
-def _m():
-    from gan_deeplearning4j_b200 import models as m
-    return m
 
 
 # ------------------------------------------------------------------ the kernels against float64 -----------------------------------------
@@ -74,14 +62,12 @@ def _lr(kind, lr, conv=False):
 
 
 def _mlp(kind):
-    m = _m()
     return [{"type": "dense", "name": "d1", "n_out": 24, "activation": kind, "updater": m.sgd(_lr(kind, 0.05)), "l2": 1e-3},
             {"type": "dense", "name": "d2", "n_out": 16, "activation": kind, "updater": m.adam(_lr(kind, 1e-2))},
             {"type": "output", "name": "out", "n_out": 5, "loss": "mse", "activation": kind, "updater": m.sgd(_lr(kind, 0.05))}], (12,), 5
 
 
 def _conv(kind):
-    m = _m()
     return [{"type": "conv2d", "name": "c1", "n_out": 8, "kernel": (3, 3), "stride": (2, 2), "padding": (1, 1), "activation": kind, "updater": m.sgd(_lr(kind, 0.05, True))},
             {"type": "batchnorm", "name": "bn1", "updater": m.sgd(_lr(kind, 0.05, True))},
             {"type": "activation", "name": "a1", "activation": kind},
@@ -136,7 +122,6 @@ def test_bf16_dcgan_layers_on_injected_inputs(b200, kind):
     own input to it (check_bf16; a GEMM of a new kind also allows the rounding of its stored z, _check_ext_gemm), and the same number of SIMT
     GEMM calls as the ReLU / LeakyReLU nets: the GEMMs stay on tensor cores."""
     b, ctx = b200
-    m = _m()
     n, z = 16, 32
     rng = np.random.default_rng(9)
     cases = [(m.dcgan_generator(16, z, 64, 3, activation=kind), m.dcgan_generator(16, z, 64, 3), (z,)),
@@ -170,25 +155,6 @@ def test_bf16_dcgan_layers_on_injected_inputs(b200, kind):
 
 
 # ------------------------------------------------------------------ the fused GAN step, FP32 --------------------------------------------
-def _close(got, want, bound, tol=2 * TOL):
-    """Within tol of max |want|, or DESIGN 1's sign-like first-step allowance: every difference <= bound and at most 2 % of elements beyond tol."""
-    d = np.abs(np.asarray(got, np.float64) - np.asarray(want, np.float64))
-    if d.max() < tol * np.abs(want).max():
-        return True
-    return d.max() <= bound and (d > tol * np.abs(want).max()).mean() <= 0.02
-
-
-def _launches_per_step(b, ctx, gan, n, data):
-    gan.upload(*data)
-    for _ in range(2):
-        gan.step_resident(n)
-    ctx.sync(); l0 = ctx.launch_count()
-    for _ in range(3):
-        gan.step_resident(n)
-    ctx.sync()
-    return (ctx.launch_count() - l0) / 3
-
-
 # launches per FP32 16x16 step (nf 8, z 12, batch 8) of the ELU / HardTanh generator with the SELU discriminator, and of the same nets on
 # ReLU / tanh and LeakyReLU (DESIGN.md 3.1: 14 more): per G forward (2 a step) 3 act_ext_fwd, per D forward (2) 2; G backward 2 more launches (its
 # unfused ActivationLayers; HardTanh's act_ext_bwd replaces tanh's), each D backward 1 more (its unfused ActivationLayer)
@@ -197,33 +163,28 @@ EXTRA_LAUNCHES = 2 * 3 + 2 * 2 + 2 + 2 * 1
 
 def test_fp32_gan_step_matches_oracle(b200):
     b, ctx = b200
-    m = _m()
     size, z, nf, n, lr_ = 16, 12, 8, 8, 2e-3
     gs = m.dcgan_generator(size, z, nf, 3, lr=lr_, activation="elu", out_activation="hardtanh")
     ds = m.dcgan_discriminator(size, nf, 3, lr=lr_, activation="selu")
-    data = [a.astype(np.float64) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
     counts = {}
     for graph in (True, False):
-        rng = np.random.default_rng(5)
-        G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
-        randomize(G, rng); randomize(D, rng)
-        bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
-        bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2)
-        push_params(G, bG); push_params(D, bD)
+        G, D, bG, bD, data = fp32_gan_pair(b, ctx, gs, ds, n)
         gan = b.Gan(bG, bD, use_cuda_graph=graph)
         for it in range(3):
             r = o.gan_step(G, D, *data)
             lo = gan.step(*data)
             want = np.array([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]])
             assert np.all(np.abs(lo - want) < TOL * np.maximum(1, np.abs(want))), (graph, it, lo, want)
-            assert _close(bD.params(), D.params_flat(), 2 * lr_), (graph, it, "D", rel_err(bD.params(), D.params_flat()))
-            assert _close(bG.params(), G.params_flat(), 2 * lr_), (graph, it, "G", rel_err(bG.params(), G.params_flat()))
-        counts[graph] = _launches_per_step(b, ctx, gan, n, [a.astype(np.float32) for a in data])
+            assert pclose(bD.params(), D.params_flat(), 2 * lr_), (graph, it, "D", rel_err(bD.params(), D.params_flat()))
+            assert pclose(bG.params(), G.params_flat(), 2 * lr_), (graph, it, "G", rel_err(bG.params(), G.params_flat()))
+        gan.upload(*[a.astype(np.float32) for a in data])
+        counts[graph] = launches_per_step(ctx, gan, n)
         gan.close(); bG.close(); bD.close()
     bG = b.Net(ctx, m.dcgan_generator(size, z, nf, 3, lr=lr_), (z,), max_batch=n, precision=b.FP32)
     bD = b.Net(ctx, m.dcgan_discriminator(size, nf, 3, lr=lr_), (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2)
     gan = b.Gan(bG, bD, use_cuda_graph=True)
-    base = _launches_per_step(b, ctx, gan, n, [a.astype(np.float32) for a in data])
+    gan.upload(*[a.astype(np.float32) for a in data])
+    base = launches_per_step(ctx, gan, n)
     gan.close(); bG.close(); bD.close()
     assert counts[True] == counts[False] == base + EXTRA_LAUNCHES, (counts, base)
 

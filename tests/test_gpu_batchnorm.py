@@ -14,20 +14,12 @@ of fp32 inputs at |m|/s = 100 within 2e-5, the measured bound of an fp32 batch m
 import numpy as np
 import pytest
 
-from helpers import bf16_round, check_bf16
+from helpers import b200, bf16_round, check_bf16
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
 
 ALPHA = 0.2
-
-
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
 
 
 def act_fwd(act, z):

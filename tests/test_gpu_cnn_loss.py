@@ -6,24 +6,12 @@ against eager, per-image labels against the same labels as maps, and the refusal
 import numpy as np
 import pytest
 
-from helpers import bf16_round, check_bf16, gan_step_parity, push_params, randomize, rel_err
+from gan_deeplearning4j_b200 import models as m
+from helpers import b200, bf16_round, check_bf16, gan_step_parity, oracle_gan_pair, push_params, randomize, rel_err
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
-
-
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
-
-
-def _m():
-    from gan_deeplearning4j_b200 import models as m
-    return m
 
 
 # ------------------------------------------------------------------ the loss kernels -----------------------------------------------------
@@ -137,7 +125,6 @@ def _labels(loss, rng, shape):
 
 
 def _specs(loss, act, c):
-    m = _m()
     return [{"type": "conv2d", "name": "c1", "n_out": 8, "kernel": (3, 3), "stride": (1, 1), "padding": (1, 1), "has_bias": False, "updater": m.sgd(0.05)},
             {"type": "batchnorm", "name": "bn1", "updater": m.sgd(0.05)},
             {"type": "activation", "name": "a1", "activation": "lrelu", "alpha": 0.2},
@@ -195,23 +182,14 @@ def test_bf16_nets_match_oracle_loosely(b200, loss, act, c):
 
 
 # ------------------------------------------------------------------ the adversarial step -------------------------------------------------
-def _patch_setup(loss, size=16, z=12, nf=8, lr=2e-3):
-    m = _m()
-    gs = m.dcgan_generator(size, z, nf, 3, lr=lr)
-    ds = m.dcgan_discriminator(size, nf, 3, lr=lr, loss=loss, patch=True)
-    rng = np.random.default_rng(5)
-    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
-    randomize(G, rng); randomize(D, rng)
-    return gs, ds, G, D
-
-
 @pytest.mark.parametrize("loss", ["xent", "mse"])
 def test_fp32_patch_gan_step_matches_oracle(b200, loss):
     """A 16x16 DCGAN with a 4x4-patch discriminator (XENT; MSE with labels 1 / 0 / 1): losses and both nets' parameters over 3 steps; graph
     replay equals the eager step bit for bit.  Gan.step takes the per-image labels and broadcasts them over the patch map."""
     b, ctx = b200
     size, z, n, lr_ = 16, 12, 8, 2e-3
-    gs, ds, G, D = _patch_setup(loss)
+    gs, ds = m.dcgan_generator(size, z, 8, 3, lr=lr_), m.dcgan_discriminator(size, 8, 3, lr=lr_, loss=loss, patch=True)
+    G, D = oracle_gan_pair(gs, ds, size, z)
     data = [a.astype(np.float64) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
     if loss == "mse":
         data[3], data[4], data[5] = np.ones((n, 1)), np.zeros((n, 1)), np.ones((n, 1))
@@ -238,7 +216,6 @@ def test_bf16_patch_step_head_adds_no_simt_calls_and_label_broadcast(b200):
     kernels count, the patch head's few-output kernels do not.  Per-image labels broadcast by Gan.step give the same bits as the same labels as
     full maps."""
     b, ctx = b200
-    m = _m()
     size, z, nf, n = 64, 100, 64, 16
     gs = m.dcgan_generator(size, z, nf, 3)
     data = [a.astype(np.float32) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
@@ -263,7 +240,6 @@ def test_bf16_head_conv_adds_no_simt_calls(b200):
     """BatchNorm -> the 3x3 s1 p1 head onto 1 channel -> CnnLossLayer: the head's forward, weight gradient and input gradient (the BatchNorm
     below is trainable) all run on the few-output kernels."""
     b, ctx = b200
-    m = _m()
     specs = [{"type": "batchnorm", "name": "bn", "updater": m.sgd(0.01)},
              {"type": "conv2d", "name": "head", "n_out": 1, "kernel": (3, 3), "stride": (1, 1), "padding": (1, 1), "updater": m.sgd(0.01)},
              dict(m.cnn_loss("xent"), name="cl")]
@@ -369,7 +345,6 @@ def test_loss_sums_count_every_element(b200, shape, prec):
 
 def test_refusals(b200):
     b, ctx = b200
-    m = _m()
     size, z, nf, n = 16, 12, 8, 4
     bG = b.Net(ctx, m.dcgan_generator(size, z, nf, 3), (z,), max_batch=n, precision=b.FP32)
     ds = m.dcgan_discriminator(size, nf, 3, patch=True)

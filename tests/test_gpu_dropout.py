@@ -1,28 +1,15 @@
 """DropoutLayer on the GPU: the dropout kernels against the oracle's mask element for element, FP32 nets against the oracle under identical
 masks, BF16 nets against the same nets without dropout, the identity cases, the device pass counter (eager, CUDA graph, checkpoint) and
 two ranks."""
-import json
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
-from helpers import bf16_round, push_params, randomize, rel_err
+from gan_deeplearning4j_b200 import models as m
+from helpers import b200, bf16_round, fp32_gan_pair, push_params, randomize, rel_err, run_two_ranks
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
 
 
 @pytest.mark.parametrize("p", [0.5, 0.9, 1.0])
@@ -63,7 +50,6 @@ def test_dropout_rejects_bad_arguments(b200):
 
 
 def _chain_specs(p=0.7, frozen=False, with_dropout=True):
-    from gan_deeplearning4j_b200 import models as m
     u = m.adam(1e-2)
     drop = lambda name: [{"type": "dropout", "name": name, "p": p, "frozen": frozen}] if with_dropout else []
     return ([{"type": "conv2d", "name": "c1", "n_out": 8, "kernel": (3, 3), "stride": (2, 2), "padding": (1, 1), "updater": u},
@@ -162,7 +148,6 @@ def test_pass_counter_and_checkpoint_resume(b200, tmp_path):
 
 
 def _dcgan_d_with_dropout(size, nf, lr, p):
-    from gan_deeplearning4j_b200 import models as m
     out = []
     for s in m.dcgan_discriminator(size, nf, 3, lr=lr):
         out.append(s)
@@ -188,7 +173,6 @@ def test_bf16_nets_with_dropout_track_the_oracle(b200):
     identical masks stays within 2x that of the same nets without dropout.  The DCGAN D puts DropoutLayers between the fused BatchNorm
     epilogues and the next GEMM (the BatchNorm backward then runs the accumulator kernels on its own)."""
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m
     cases = [("mlp", m.mlp_discriminator(128, 256, lr=1e-3), m.mlp_discriminator(128, 256, lr=1e-3, dropout=0.5), (128,), 256),
              ("dcgan32", m.dcgan_discriminator(32, 64, 3, lr=1e-3), _dcgan_d_with_dropout(32, 64, 1e-3, 0.5), (3, 32, 32), 8)]
     for name, plain, drop, shape, n in cases:
@@ -198,26 +182,13 @@ def test_bf16_nets_with_dropout_track_the_oracle(b200):
         assert e1 <= 2 * e0, (name, e0, e1)
 
 
-def _fp32_dcgan_with_dropout(b, ctx, n, p=0.7):
-    from gan_deeplearning4j_b200 import models as m
-    size, z, nf = 16, 12, 8
-    gs, ds = m.dcgan_generator(size, z, nf, 3, lr=2e-3), _dcgan_d_with_dropout(size, nf, 2e-3, p)
-    rng = np.random.default_rng(5)
-    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), mask_seed=667, seed=2)
-    randomize(G, rng); randomize(D, rng)
-    bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
-    bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2, seed=667)
-    push_params(G, bG); push_params(D, bD)
-    data = [a.astype(np.float64) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
-    return G, D, bG, bD, ds, data
-
-
 def test_fp32_gan_step_with_dropout_graph_eager_and_oracle(b200):
     b, ctx = b200
     n = 8
+    gs, ds = m.dcgan_generator(16, 12, 8, 3, lr=2e-3), _dcgan_d_with_dropout(16, 8, 2e-3, 0.7)
     runs = []
     for graph in (False, True):
-        G, D, bG, bD, ds, data = _fp32_dcgan_with_dropout(b, ctx, n)
+        G, D, bG, bD, data = fp32_gan_pair(b, ctx, gs, ds, n, mask_seed=667, d_kw=dict(seed=667))
         gan = b.Gan(bG, bD, use_cuda_graph=graph)
         drop = [i for i, s in enumerate(ds) if s["type"] == "dropout"]
         masks, losses = [], []
@@ -248,15 +219,5 @@ def test_fp32_gan_step_with_dropout_graph_eager_and_oracle(b200):
 
 
 def test_two_ranks_share_parameters_but_not_masks(tmp_path):
-    try:
-        import torch
-        gpus = torch.cuda.device_count()
-    except Exception:
-        gpus = 0
-    if gpus < 2:
-        pytest.skip("needs two GPUs")
-    out = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1", "--master-port", "29547",
-                          os.path.join(ROOT, "tools", "dropout_dp_check.py"), str(tmp_path / "dropout_dp.json")], capture_output=True, text=True, timeout=600, cwd=ROOT)
-    assert out.returncode == 0, out.stdout[-800:] + out.stderr[-1500:]
-    d = json.load(open(tmp_path / "dropout_dp.json"))
+    d = run_two_ranks("dropout_dp_check.py", tmp_path / "dropout_dp.json", 29547)
     assert d["world"] == 2 and d["d_params_identical"] is True and d["dropout_activations_differ"] is True and d["masks_match_oracle"] is True

@@ -8,19 +8,11 @@ import numpy as np
 import pytest
 
 import ew_ref as er
-from helpers import bf16_round
+from helpers import b200, bf16_round
 
 pytestmark = pytest.mark.gpu
 PRECS = ["fp32", "bf16"]
 U = 2.0 ** -24          # fp32 unit roundoff
-
-
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
 
 
 def _P(b, prec):

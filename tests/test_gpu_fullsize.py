@@ -18,21 +18,13 @@ import pytest
 
 import conv_ref
 import tc_schedule
-from helpers import bf16_round, check_bf16, inject_forward
+from helpers import b200, bf16_round, check_bf16, inject_forward
 from oracle import dl4j_oracle as o
 from tc_schedule import pick_row_tile as _pick_row_tile
 
 pytestmark = pytest.mark.gpu
 
 N = 128     # C2 per-GPU batch; the D step runs 2N
-
-
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
 
 
 def sample_images(n):

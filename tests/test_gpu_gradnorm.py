@@ -2,72 +2,27 @@
 modes, eager against CUDA-graph replay bit for bit (a mode change re-captures), the bf16 weight copies after normalized updates, launch counts,
 argument checks and two ranks."""
 import copy
-import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
-from helpers import bf16_round, pack_deconv_ps, push_params, randomize, rel_err, w_internal
+from gan_deeplearning4j_b200 import models as m
+from helpers import (b200, bf16_gan, check_weight_operands, compare_params_and_state, fp32_gan_pair, launches_per_step, mlp_convbn_specs,
+                     push_params, randomize, run_two_ranks)
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 L2_MODES = ("renormalize_l2_per_layer", "renormalize_l2_per_param_type", "clip_l2_per_layer", "clip_l2_per_param_type")
 
 
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
-
-
 def _specs(kind, upd):
-    from gan_deeplearning4j_b200 import models as m
-    u = m.sgd(0.05) if upd == "sgd" else m.adam(1e-2)
-    if kind == "mlp":          # 64 -> 256 -> 128 -> 1: W of 8 chunks, every segment 16-byte aligned
-        return [{"type": "dense", "name": "d1", "n_out": 256, "activation": "tanh", "updater": u, "l2": 1e-3},
-                {"type": "dense", "name": "d2", "n_out": 128, "activation": "lrelu", "alpha": 0.2, "updater": u},
-                {"type": "output", "name": "out", "n_out": 1, "updater": u}], (64,)
+    u = lambda: m.sgd(0.05) if upd == "sgd" else m.adam(1e-2)
     if kind == "ragged":       # 7 -> 999 -> 33 -> 1: segments at offsets 6993, 7992, ... (not multiples of 4): the scalar branches
-        return [{"type": "dense", "name": "d1", "n_out": 999, "activation": "tanh", "updater": u},
-                {"type": "dense", "name": "d2", "n_out": 33, "activation": "relu", "updater": u, "l2": 1e-3},
-                {"type": "output", "name": "out", "n_out": 1, "updater": u}], (7,)
-    return ([{"type": "conv2d", "name": "c1", "n_out": 8, "kernel": (3, 3), "stride": (2, 2), "padding": (1, 1), "updater": u},
-             {"type": "activation", "name": "a1", "activation": "lrelu", "alpha": 0.2},
-             {"type": "conv2d", "name": "c2", "n_out": 12, "kernel": (3, 3), "stride": (1, 1), "padding": (1, 1), "has_bias": False, "updater": u},
-             {"type": "batchnorm", "name": "bn2", "updater": u}, {"type": "activation", "name": "a2", "activation": "tanh"},
-             {"type": "cnn_to_ff", "name": "flat"},
-             {"type": "dense", "name": "fc", "n_out": 10, "activation": "tanh", "updater": u},
-             {"type": "output", "name": "out", "n_out": 1, "updater": u}], (3, 8, 8))
-
-
-def _state_flat(onet, k):
-    """The oracle's updater state k (Adam m / v) flattened like b2g_net_get_updater_state (zeros where a parameter has none)."""
-    out = []
-    for li, _, p, shape, order in onet.param_table():
-        st = onet.state.get((li, p))
-        out.append((st[k] if st is not None and k < len(st) else np.zeros(shape)).ravel(order=order.upper()))
-    return np.concatenate(out)
-
-
-def _compare(onet, bnet, what, tol=TOL):
-    p_b, p_o = bnet.params(), onet.params_flat()
-    st = bnet.updater_state(); n = bnet.num_params()
-    s0, s1 = _state_flat(onet, 0), _state_flat(onet, 1)
-    off = 0
-    for li, name, pn, shape, _ in onet.param_table():
-        k = int(np.prod(shape)); sl = slice(off, off + k)
-        assert rel_err(p_b[sl], p_o[sl]) < tol, (what, name, pn, rel_err(p_b[sl], p_o[sl]))
-        for b_st, o_st in ((st[:n][sl], s0[sl]), (st[n:][sl], s1[sl])):
-            if np.abs(o_st).max() > 0:
-                assert rel_err(b_st, o_st) < tol, (what, name, pn, "state")
-        off += k
+        return [{"type": "dense", "name": "d1", "n_out": 999, "activation": "tanh", "updater": u()},
+                {"type": "dense", "name": "d2", "n_out": 33, "activation": "relu", "updater": u(), "l2": 1e-3},
+                {"type": "output", "name": "out", "n_out": 1, "updater": u()}], (7,)
+    return mlp_convbn_specs(kind, u)
 
 
 def _threshold_between(norms):
@@ -100,30 +55,24 @@ def test_fp32_fit_matches_oracle(b200, kind, upd, mode):
         onet.fit(xs[it], ys[it]); bnet.fit(xs[it], ys[it])
         if mode.startswith("clip"):
             clipped += [nm > thr for nm in onet.grad_norm_last_norms]
-        _compare(onet, bnet, (kind, upd, mode, it))
+        compare_params_and_state(onet, bnet, (kind, upd, mode, it), TOL)
     if mode.startswith("clip"):
         assert any(clipped) and not all(clipped), clipped
     bnet.close()
 
 
-def _fp32_dcgan(b, ctx, n, gmode, dmode, gthr=1.0, dthr=1.0):
-    from gan_deeplearning4j_b200 import models as m
-    size, z, nf = 16, 12, 8
-    gs, ds = m.dcgan_generator(size, z, nf, 3, lr=2e-3), m.dcgan_discriminator(size, nf, 3, lr=2e-3)
-    rng = np.random.default_rng(5)
-    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
-    randomize(G, rng); randomize(D, rng)
+def _normalized_pair(b, ctx, n, gmode, dmode, gthr=1.0, dthr=1.0):
+    """fp32_gan_pair of the 16x16 DCGAN with G's gradient normalization (mode, threshold) gmode, gthr and D's dmode, dthr on both sides."""
+    gs, ds = m.dcgan_generator(16, 12, 8, 3, lr=2e-3), m.dcgan_discriminator(16, 8, 3, lr=2e-3)
+    G, D, bG, bD, data = fp32_gan_pair(b, ctx, gs, ds, n, g_kw=dict(gradient_normalization=gmode, gradient_normalization_threshold=gthr),
+                                       d_kw=dict(gradient_normalization=dmode, gradient_normalization_threshold=dthr))
     G.set_gradient_normalization(gmode, gthr); D.set_gradient_normalization(dmode, dthr)
-    bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32, gradient_normalization=gmode, gradient_normalization_threshold=gthr)
-    bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2, gradient_normalization=dmode, gradient_normalization_threshold=dthr)
-    push_params(G, bG); push_params(D, bD)
-    data = [a.astype(np.float64) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
     return G, D, bG, bD, data
 
 
 def _gan_norms(b, ctx, n, mode):
     """The group norms of the first step's D and G updates (oracle), for a threshold between them."""
-    G, D, bG, bD, data = _fp32_dcgan(b, ctx, n, mode, mode, 1e30, 1e30)
+    G, D, bG, bD, data = _normalized_pair(b, ctx, n, mode, mode, 1e30, 1e30)
     bG.close(); bD.close()
     o.gan_step(G, D, *data)
     return G.grad_norm_last_norms, D.grad_norm_last_norms
@@ -137,14 +86,14 @@ def test_fp32_gan_step_matches_oracle(b200, mode):
     if mode.startswith("clip"):
         gn, dn = _gan_norms(b, ctx, n, mode)
         gthr, dthr = _threshold_between(gn), _threshold_between(dn)
-    G, D, bG, bD, data = _fp32_dcgan(b, ctx, n, mode, mode, gthr, dthr)
+    G, D, bG, bD, data = _normalized_pair(b, ctx, n, mode, mode, gthr, dthr)
     gan = b.Gan(bG, bD, use_cuda_graph=True)
     for it in range(3):
         r = o.gan_step(G, D, *data)
         lo = gan.step(*data)
         want = np.array([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]])
         assert np.all(np.abs(lo - want) < TOL * np.maximum(1, np.abs(want))), (mode, it, lo, want)
-        _compare(D, bD, (mode, it, "D"), 2 * TOL); _compare(G, bG, (mode, it, "G"), 2 * TOL)
+        compare_params_and_state(D, bD, (mode, it, "D"), 2 * TOL); compare_params_and_state(G, bG, (mode, it, "G"), 2 * TOL)
     gan.close(); bG.close(); bD.close()
 
 
@@ -152,7 +101,6 @@ def test_mnist_example_configuration_with_dropout(b200):
     """DL4J's MNIST GAN example: mlp_generator + mlp_discriminator(dropout=0.5), RenormalizeL2PerLayer on both nets, FP32, under the masks of
     the oracle's dropout_mask."""
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m
     n, z, hid, d = 16, 24, 64, 48
     gs, ds = m.mlp_generator(z, hid, d, lr=1e-3), m.mlp_discriminator(d, hid, lr=1e-3, dropout=0.5)
     rng = np.random.default_rng(9)
@@ -171,7 +119,7 @@ def test_mnist_example_configuration_with_dropout(b200):
         lo = gan.step(*data)
         want = np.array([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]])
         assert np.all(np.abs(lo - want) < TOL * np.maximum(1, np.abs(want))), (it, lo, want)
-        _compare(D, bD, (it, "D"), 2 * TOL); _compare(G, bG, (it, "G"), 2 * TOL)
+        compare_params_and_state(D, bD, (it, "D"), 2 * TOL); compare_params_and_state(G, bG, (it, "G"), 2 * TOL)
         assert len(D.grad_norm_last_norms) == 3 and len(G.grad_norm_last_norms) == 3
     gan.close(); bG.close(); bD.close()
 
@@ -184,7 +132,7 @@ def test_graph_replay_matches_eager_and_recaptures_on_a_mode_change(b200):
     plan = [("renormalize_l2_per_layer", 1.0)] * 2 + [("clip_l2_per_param_type", 0.05)] * 2 + [("none", 1.0)] + [("clip_l2_per_layer", 0.2)] * 2
     runs = []
     for graph in (False, True):
-        G, D, bG, bD, data = _fp32_dcgan(b, ctx, n, "none", "none")
+        G, D, bG, bD, data = _normalized_pair(b, ctx, n, "none", "none")
         gan = b.Gan(bG, bD, use_cuda_graph=graph)
         losses, launches = [], []
         for mode, thr in plan:
@@ -206,28 +154,16 @@ def test_launch_counts(b200):
     """C2 (bench.py's DCGAN 64x64, bf16, batch 128) launches 83 kernels per step without a mode, 85 with an L2 mode on both nets (one norm
     kernel per update); fit adds exactly one launch."""
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m
     n = 128
-    G = b.Net(ctx, m.dcgan_generator(64, 100, 64, 3), (100,), max_batch=n, precision=b.BF16, xent_clip_eps=0.0, seed=666)
-    D = b.Net(ctx, m.dcgan_discriminator(64, 64, 3), (3, 64, 64), max_batch=2 * n, precision=b.BF16, xent_clip_eps=0.0, bn_groups=2, seed=667)
+    G, D = bf16_gan(b, ctx, m.dcgan_generator(64, 100, 64, 3), m.dcgan_discriminator(64, 64, 3), (100,), (3, 64, 64), n)
     gan = b.Gan(G, D, use_cuda_graph=True)
     rng = np.random.default_rng(1)
     gan.upload(rng.uniform(-1, 1, (n, 3, 64, 64)), rng.uniform(-1, 1, (n, 100)), rng.uniform(-1, 1, (n, 100)), np.ones((n, 1)), np.zeros((n, 1)), np.ones((n, 1)))
-
-    def per_step():
-        for _ in range(2):
-            gan.step_resident(n)
-        ctx.sync(); l0 = ctx.launch_count()
-        for _ in range(3):
-            gan.step_resident(n)
-        ctx.sync()
-        return (ctx.launch_count() - l0) / 3
-
-    assert per_step() == 83
+    assert launches_per_step(ctx, gan, n) == 83
     G.set_gradient_normalization("clip_l2_per_layer", 1.0); D.set_gradient_normalization("renormalize_l2_per_layer")
-    assert per_step() == 85
+    assert launches_per_step(ctx, gan, n) == 85
     G.set_gradient_normalization("none"); D.set_gradient_normalization("none")
-    assert per_step() == 83
+    assert launches_per_step(ctx, gan, n) == 83
     gan.close(); G.close(); D.close()
     specs, shape = _specs("mlp", "adam")
     net = b.Net(ctx, specs, shape, max_batch=4, precision=b.FP32)
@@ -240,23 +176,10 @@ def test_launch_counts(b200):
     net.close()
 
 
-def _check_weight_operands(net, specs, what):
-    for li, s in enumerate(specs):
-        if s["type"] not in ("conv2d", "deconv2d", "dense", "output"):
-            continue
-        k = s.get("kernel", (1, 1)); size = s["n_in"] * s["n_out"] * k[0] * k[1]
-        w = bf16_round(w_internal(s, net.get_param(s["name"], "W", size)))
-        assert np.array_equal(net.weight_operand(li, 0, size), w), f"{what}: bf16 copy of {s['name']}.W"
-        O, C = (s["n_in"], s["n_out"]) if s["type"] == "deconv2d" else (s["n_out"], s["n_in"])
-        if tuple(k) == (4, 4) and tuple(s.get("stride", ())) == (2, 2) and tuple(s.get("padding", ())) == (1, 1) and C <= 4 and O % 64 == 0:
-            assert np.array_equal(net.weight_operand(li, 1, 144 * O), pack_deconv_ps(w.reshape(O, 4, 4, -1))), f"{what}: packed operand of {s['name']}"
-
-
 def test_bf16_weight_copies_track_the_master(b200):
     """BF16 DCGAN 32x32 (G-last on the pixel-shuffle operand) with L2 modes through graph steps, and a fit net whose pixel-shuffle W sits at
     flat offset 3 (the updater's scalar branch): every bf16 weight copy equals the rounded fp32 master."""
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m
     size, z, nf, n = 32, 16, 64, 8
     gs, ds = m.dcgan_generator(size, z, nf, 3, lr=2e-3), m.dcgan_discriminator(size, nf, 3, lr=2e-3)
     G = b.Net(ctx, gs, (z,), max_batch=n, precision=b.BF16, xent_clip_eps=0.0, gradient_normalization="renormalize_l2_per_layer")
@@ -267,7 +190,7 @@ def test_bf16_weight_copies_track_the_master(b200):
     g0 = G.params()
     for it in range(3):
         gan.step(*data)
-        _check_weight_operands(G, gs, f"G step {it}"); _check_weight_operands(D, ds, f"D step {it}")
+        check_weight_operands(b, G, gs, f"G step {it}"); check_weight_operands(b, D, ds, f"D step {it}")
     assert np.abs(G.params() - g0).max() > 0
     gan.close(); G.close(); D.close()
     u = m.adam(1e-3)
@@ -282,7 +205,7 @@ def test_bf16_weight_copies_track_the_master(b200):
         net = b.Net(ctx, specs, (64, 8, 8), max_batch=6, precision=b.BF16, gradient_normalization=mode, gradient_normalization_threshold=0.05)
         for it in range(3):
             net.fit(rng.standard_normal((6, 64, 8, 8)).astype(np.float32), rng.uniform(0, 1, (6, 1)).astype(np.float32))
-            _check_weight_operands(net, specs, f"{mode} fit {it}")
+            check_weight_operands(b, net, specs, f"{mode} fit {it}")
         net.close()
 
 
@@ -316,15 +239,5 @@ def test_rejections(b200):
 
 
 def test_two_ranks_match_one_gpu(tmp_path):
-    try:
-        import torch
-        gpus = torch.cuda.device_count()
-    except Exception:
-        gpus = 0
-    if gpus < 2:
-        pytest.skip("needs two GPUs")
-    out = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1", "--master-port", "29549",
-                          os.path.join(ROOT, "tools", "gradnorm_dp_check.py"), str(tmp_path / "gradnorm_dp.json")], capture_output=True, text=True, timeout=600, cwd=ROOT)
-    assert out.returncode == 0, out.stdout[-800:] + out.stderr[-1500:]
-    d = json.load(open(tmp_path / "gradnorm_dp.json"))
+    d = run_two_ranks("gradnorm_dp_check.py", tmp_path / "gradnorm_dp.json", 29549)
     assert d["world"] == 2 and d["params_identical_across_ranks"] is True and d["max_rel_err_vs_one_gpu"] < 1e-5

@@ -6,24 +6,12 @@ against eager; and the launch budget."""
 import numpy as np
 import pytest
 
-from helpers import bf16_round, gan_step_parity, push_params, randomize, rel_err
+from gan_deeplearning4j_b200 import models as m
+from helpers import b200, bf16_round, gan_step_parity, oracle_gan_pair, push_params, randomize, rel_err
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
-
-
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
-
-
-def _m():
-    from gan_deeplearning4j_b200 import models as m
-    return m
 
 
 # ------------------------------------------------------------------ the vertex kernels ---------------------------------------------------
@@ -106,17 +94,16 @@ def test_skip_add_bit_exact(b200, prec, offset, n):
 
 # ------------------------------------------------------------------ nets against the oracle ---------------------------------------------
 def _dense(name, n_out, act="tanh", lr=0.05):
-    return {"type": "dense", "name": name, "n_out": n_out, "activation": act, "updater": _m().adam(lr)}
+    return {"type": "dense", "name": name, "n_out": n_out, "activation": act, "updater": m.adam(lr)}
 
 
 def _conv(name, c_in, c_out, k=3, s=1, p=1, act="identity", lr=0.01):
     return {"type": "conv2d", "name": name, "n_in": c_in, "n_out": c_out, "kernel": (k, k), "stride": (s, s), "padding": (p, p), "activation": act,
-            "has_bias": False, "updater": _m().adam(lr)}
+            "has_bias": False, "updater": m.adam(lr)}
 
 
 def _nets(kind, ch=8):
     """(specs, input shape, loss) of the graphs the parity tests run."""
-    m = _m()
     if kind == "residual":
         return ([_conv("stem", 3, ch, act="tanh")] + m.residual_block("rb", ch, "stem", lr=0.01) +
                 [_conv("head", ch, 2, k=1, p=0), m.cnn_loss("mse", name="loss")], (3, 8, 8), "mse")
@@ -129,7 +116,7 @@ def _nets(kind, ch=8):
     if kind == "ff_merge":
         return ([_dense("d1", 16), _dense("d2", 24, "sigmoid"), m.merge(["d1", "d2"], name="mg"), _dense("d3", 12),
                  m.elementwise("average", ["d3", "d3"], name="av"),
-                 {"type": "output", "name": "out", "n_out": 3, "loss": "mse", "activation": "identity", "updater": _m().adam(0.05)}], (10,), "mse")
+                 {"type": "output", "name": "out", "n_out": 3, "loss": "mse", "activation": "identity", "updater": m.adam(0.05)}], (10,), "mse")
     raise ValueError(kind)
 
 
@@ -204,7 +191,6 @@ def test_bf16_graph_nets_match_oracle_loosely(b200, kind):
 
 # One BF16 net per single-consumer fusion the engine turns off at a skip source; each would compute another function with the fusion on.
 def _guard_net(guard, ch=64):
-    m = _m()
     u = lambda: m.adam(0.01)
     if guard == "bn_act":           # the BatchNorm is the source: fused with its ReLU, the vertex would read relu(bn) for bn
         body = [_conv("c1", 3, ch), {"type": "batchnorm", "name": "bn1", "updater": u()}, {"type": "activation", "name": "a1", "activation": "relu"},
@@ -231,21 +217,16 @@ def test_bf16_fusion_guards(b200, guard):
 
 
 # ------------------------------------------------------------------ the adversarial step -------------------------------------------------
-def _gan_setup(size=16, z=12, nf=8, lr=2e-3, patch=False):
-    m = _m()
-    gs = m.dcgan_generator(size, z, nf, 3, lr=lr, residual=True)
-    ds = m.dcgan_discriminator(size, nf, 3, lr=lr, residual=True, patch=patch)
-    rng = np.random.default_rng(5)
-    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
-    randomize(G, rng); randomize(D, rng)
-    return gs, ds, G, D
+def _residual(size=16, z=12, nf=8, patch=False):
+    return m.dcgan_generator(size, z, nf, 3, lr=2e-3, residual=True), m.dcgan_discriminator(size, nf, 3, lr=2e-3, residual=True, patch=patch)
 
 
 @pytest.mark.parametrize("patch", [False, True])
 def test_fp32_residual_gan_step_matches_oracle(b200, patch):
     b, ctx = b200
     size, z, n, lr_ = 16, 12, 8, 2e-3
-    gs, ds, G, D = _gan_setup(patch=patch)
+    gs, ds = _residual(patch=patch)
+    G, D = oracle_gan_pair(gs, ds, size, z)
     data = [a.astype(np.float64) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
     labels = [np.broadcast_to(v.reshape(n, 1, 1, 1), (n, 1, 4, 4)).copy() if patch else v for v in data[3:]]
     gan_step_parity(b, ctx, gs, ds, G, D, data, labels, lr_, patch)
@@ -254,7 +235,8 @@ def test_fp32_residual_gan_step_matches_oracle(b200, patch):
 def test_bf16_residual_gan_step_runs_and_replays(b200):
     b, ctx = b200
     size, z, n = 32, 16, 16
-    gs, ds, G, D = _gan_setup(size=size, z=z, nf=64)
+    gs, ds = _residual(size, z, 64)
+    G, D = oracle_gan_pair(gs, ds, size, z)
     data = [a.astype(np.float32) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
     out = {}
     for graph in (True, False):
@@ -273,7 +255,6 @@ def test_launch_budget(b200):
     """A vertex costs one launch in the forward; in the backward one plus one per skip source.  The same net with an identity ActivationLayer
     in the vertex's place (one launch each way) is the yardstick."""
     b, ctx = b200
-    m = _m()
     out = {"type": "output", "name": "out", "n_out": 3, "loss": "mse", "activation": "identity", "updater": m.sgd(0.1)}
     base = [_dense("d1", 16), _dense("d2", 16)]
     vert = base + [m.elementwise("add", ["d2", "d1"], name="v"), _dense("d3", 8), out]
@@ -297,7 +278,6 @@ def test_residual_gan_step_launch_budget(b200):
     G forward twice (x_fake, then the G step), D forward twice and backward twice (D step, then the G step through D), G backward once.  FP32,
     so no tensor-core epilogue fusion (the guards' business) enters either count."""
     b, ctx = b200
-    m = _m()
     size, z, nf, n = 16, 12, 8, 8
     gs = m.dcgan_generator(size, z, nf, 3, residual=True)
     ds = m.dcgan_discriminator(size, nf, 3, residual=True)

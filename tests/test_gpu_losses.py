@@ -5,26 +5,14 @@ replay against eager with the XENT discriminator's launch counts, the argument c
 import numpy as np
 import pytest
 
-from helpers import bf16_round, push_params, randomize, rel_err
+from gan_deeplearning4j_b200 import models as m
+from helpers import b200, bf16_gan, bf16_round, fp32_gan_pair, launches_per_step, pclose, push_params, randomize, rel_err
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
 U = 2.0 ** -24            # fp32 unit roundoff
 ACTS = o.ACTS
-
-
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
-
-
-def _m():
-    from gan_deeplearning4j_b200 import models as m
-    return m
 
 
 # ------------------------------------------------------------------ the kernel against float64 ------------------------------------------
@@ -145,13 +133,11 @@ def test_multi_block_sums_are_bit_reproducible(b200, prec):
 
 # ------------------------------------------------------------------ FP32 fit and output against the oracle -------------------------------
 def _mlp(act):
-    m = _m()
     return [{"type": "dense", "name": "d1", "n_out": 32, "activation": "tanh", "updater": m.sgd(0.05), "l2": 1e-3},
             {"type": "output", "name": "out", "n_out": 7, "loss": "mse", "activation": act, "updater": m.sgd(0.05)}], (16,)
 
 
 def _conv_hinge():
-    m = _m()
     return [{"type": "conv2d", "name": "c1", "n_out": 8, "kernel": (3, 3), "stride": (2, 2), "padding": (1, 1), "activation": "lrelu", "alpha": 0.2,
              "updater": m.sgd(0.05), "l2": 1e-3},
             {"type": "conv2d", "name": "c2", "n_out": 6, "kernel": (3, 3), "stride": (1, 1), "padding": (1, 1), "has_bias": False, "updater": m.sgd(0.05)},
@@ -189,28 +175,13 @@ GAN_LOSSES = {"lsgan": ("mse", "identity", (1.0, 0.0, 1.0)), "hinge": ("hinge", 
               "wasserstein": ("wasserstein", "identity", (-1.0, 1.0, -1.0))}
 
 
-def _close(got, want, bound, tol=2 * TOL):
-    """Within tol of max |want|, or DESIGN 1's sign-like first-step allowance: every difference <= bound and at most 2 % of elements beyond tol."""
-    d = np.abs(np.asarray(got, np.float64) - np.asarray(want, np.float64))
-    if d.max() < tol * np.abs(want).max():
-        return True
-    return d.max() <= bound and (d > tol * np.abs(want).max()).mean() <= 0.02
-
-
 @pytest.mark.parametrize("kind", list(GAN_LOSSES))
 def test_fp32_gan_step_matches_oracle(b200, kind):
     b, ctx = b200
-    m = _m()
     loss, act, (yr, yf, yg) = GAN_LOSSES[kind]
-    size, z, nf, n, lr_ = 16, 12, 8, 8, 2e-3
-    gs, ds = m.dcgan_generator(size, z, nf, 3, lr=lr_), m.dcgan_discriminator(size, nf, 3, lr=lr_, loss=loss, out_activation=act)
-    rng = np.random.default_rng(5)
-    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
-    randomize(G, rng); randomize(D, rng)
-    bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
-    bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2)
-    push_params(G, bG); push_params(D, bD)
-    x, zd, zg, _, _, _ = [a.astype(np.float64) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
+    n, lr_ = 8, 2e-3
+    gs, ds = m.dcgan_generator(16, 12, 8, 3, lr=lr_), m.dcgan_discriminator(16, 8, 3, lr=lr_, loss=loss, out_activation=act)
+    G, D, bG, bD, (x, zd, zg, _, _, _) = fp32_gan_pair(b, ctx, gs, ds, n)
     ys = [np.full((n, 1), v) for v in (yr, yf, yg)]
     gan = b.Gan(bG, bD, use_cuda_graph=True)
     for it in range(3):
@@ -218,25 +189,18 @@ def test_fp32_gan_step_matches_oracle(b200, kind):
         lo = gan.step(x, zd, zg, *ys)
         want = np.array([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]])
         assert np.all(np.abs(lo - want) < TOL * np.maximum(1, np.abs(want))), (kind, it, lo, want)
-        assert _close(bD.params(), D.params_flat(), 2 * lr_), (kind, it, "D", rel_err(bD.params(), D.params_flat()))
-        assert _close(bG.params(), G.params_flat(), 2 * lr_), (kind, it, "G", rel_err(bG.params(), G.params_flat()))
+        assert pclose(bD.params(), D.params_flat(), 2 * lr_), (kind, it, "D", rel_err(bD.params(), D.params_flat()))
+        assert pclose(bG.params(), G.params_flat(), 2 * lr_), (kind, it, "G", rel_err(bG.params(), G.params_flat()))
     gan.close(); bG.close(); bD.close()
-
-
-def _bf16_gan(b, ctx, gs, ds, gin, din, n):
-    G = b.Net(ctx, gs, gin, max_batch=n, precision=b.BF16, xent_clip_eps=0.0, seed=666)
-    D = b.Net(ctx, ds, din, max_batch=2 * n, precision=b.BF16, xent_clip_eps=0.0, bn_groups=2, seed=667)
-    return G, D
 
 
 def test_bf16_graph_replay_matches_eager(b200):
     b, ctx = b200
-    m = _m()
     n = 8
     for loss, (yr, yf, yg) in (("mse", (1.0, 0.0, 1.0)), ("hinge", (1.0, -1.0, 1.0))):
         runs = []
         for graph in (False, True):
-            G, D = _bf16_gan(b, ctx, m.dcgan_generator(32, 16, 64, 3), m.dcgan_discriminator(32, 64, 3, loss=loss), (16,), (3, 32, 32), n)
+            G, D = bf16_gan(b, ctx, m.dcgan_generator(32, 16, 64, 3), m.dcgan_discriminator(32, 64, 3, loss=loss), (16,), (3, 32, 32), n)
             data = [a.astype(np.float32) for a in o.synthetic_batch(n, 32, 3, 16, seed=3)][:3] + [np.full((n, 1), v, np.float32) for v in (yr, yf, yg)]
             gan = b.Gan(G, D, use_cuda_graph=graph)
             losses = np.array([gan.step(*data) for _ in range(4)])
@@ -250,21 +214,14 @@ def test_bf16_graph_replay_matches_eager(b200):
 def test_launches_per_step_equal_the_xent_discriminators(b200):
     """C2 (DCGAN 64x64, bf16, batch 128) launches 83 kernels per step and a C5-shaped MLP-GAN 46, with D on XENT and on every new loss."""
     b, ctx = b200
-    m = _m()
     rng = np.random.default_rng(1)
 
     def per_step(gs, ds, gin, din, n, ys):
-        G, D = _bf16_gan(b, ctx, gs, ds, gin, din, n)
+        G, D = bf16_gan(b, ctx, gs, ds, gin, din, n)
         gan = b.Gan(G, D, use_cuda_graph=True)
         gan.upload(rng.uniform(-1, 1, (n,) + tuple(din)), rng.uniform(-1, 1, (n,) + tuple(gin)), rng.uniform(-1, 1, (n,) + tuple(gin)),
                    *[np.full((n, 1), v) for v in ys])
-        for _ in range(2):
-            gan.step_resident(n)
-        ctx.sync(); l0 = ctx.launch_count()
-        for _ in range(3):
-            gan.step_resident(n)
-        ctx.sync()
-        out = (ctx.launch_count() - l0) / 3
+        out = launches_per_step(ctx, gan, n)
         losses = gan.losses()
         gan.close(); G.close(); D.close()
         return out, losses
@@ -296,7 +253,6 @@ def _create(b, ctx, specs, shape, mutate=None, **cfg_kw):
 
 def test_rejections(b200):
     b, ctx = b200
-    m = _m()
     specs, shape = _mlp("identity")
     for bad in (9, -1, 100):
         def mut(d, bad=bad): d[-1].loss = bad
@@ -332,7 +288,6 @@ def test_rejections(b200):
 def test_mse_output_checkpoint_resume_is_bit_identical(b200, tmp_path):
     b, ctx = b200
     from gan_deeplearning4j_b200 import serializer
-    m = _m()
     specs = [{"type": "dense", "name": "d1", "n_out": 32, "activation": "tanh", "updater": m.adam(2e-3)},
              {"type": "output", "name": "out", "n_out": 7, "loss": "mse", "activation": "sigmoid", "updater": m.adam(2e-3)}]
     rng = np.random.default_rng(4)

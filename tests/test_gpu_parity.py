@@ -8,7 +8,8 @@ compared kernel-by-kernel against the oracle evaluated on the same bf16-rounded 
 import numpy as np
 import pytest
 
-from helpers import bf16_round, pack_deconv_ps, push_params, randomize, rel_err, w_internal
+from gan_deeplearning4j_b200 import models as m
+from helpers import (assert_close_up_to_sign_flips, b200, bf16_round, check_weight_operands, fp32_gan_pair, push_params, randomize, rel_err)
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
@@ -16,16 +17,7 @@ pytestmark = pytest.mark.gpu
 TOL = 1e-3   # north_star: "within 1e-3 relative fp32"
 
 
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
-
-
 def every_layer_specs(act="tanh"):
-    from gan_deeplearning4j_b200 import models as m
     u = m.adam(1e-2)
     return [
         {"type": "batchnorm", "name": "bn0", "updater": u},
@@ -86,26 +78,16 @@ def test_fp32_every_layer_activations_gradients_and_update(b200, act):
     bnet.close()
 
 
-def _gan_pair(b, ctx, size, z, nf, batch, precision, clip_eps=1e-5):
-    from gan_deeplearning4j_b200 import models as m
-    gs, ds = m.dcgan_generator(size, z, nf, 3, lr=2e-3), m.dcgan_discriminator(size, nf, 3, lr=2e-3)
-    q = o.Quirks(xent_clip_eps=clip_eps)
-    rng = np.random.default_rng(5)
-    G = o.net_from_specs(gs, (z,), quirks=q, seed=1); D = o.net_from_specs(ds, (3, size, size), quirks=q, seed=2)
-    randomize(G, rng); randomize(D, rng)
-    bG = b.Net(ctx, gs, (z,), max_batch=batch, precision=precision, xent_clip_eps=clip_eps)
-    bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * batch, precision=precision, xent_clip_eps=clip_eps, bn_groups=2)
-    push_params(G, bG); push_params(D, bD)
-    return G, D, bG, bD
+def _dcgan(size, z, nf):
+    return m.dcgan_generator(size, z, nf, 3, lr=2e-3), m.dcgan_discriminator(size, nf, 3, lr=2e-3)
 
 
 @pytest.mark.parametrize("fake_bn_train", [False, True])
 def test_fp32_gan_step_matches_oracle(b200, fake_bn_train):
     b, ctx = b200
-    size, z, nf, n = 16, 12, 8, 8
-    G, D, bG, bD = _gan_pair(b, ctx, size, z, nf, n, b.FP32)
+    n = 8
+    G, D, bG, bD, data = fp32_gan_pair(b, ctx, *_dcgan(16, 12, 8), n)
     gan = b.Gan(bG, bD, fake_bn_train=fake_bn_train, use_cuda_graph=False)
-    data = [a.astype(np.float64) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
     for it in range(3):
         r = o.gan_step(G, D, *data, fake_bn_train=fake_bn_train)
         losses = gan.step(*data)
@@ -124,11 +106,11 @@ def test_fp32_gan_step_matches_oracle(b200, fake_bn_train):
 
 def test_cuda_graph_replay_equals_eager(b200):
     b, ctx = b200
-    size, z, nf, n = 16, 12, 8, 8
-    data = o.synthetic_batch(n, size, 3, z, seed=4)
+    n = 8
+    data = o.synthetic_batch(n, 16, 3, 12, seed=4)
     outs = []
     for graph in (False, True):
-        G, D, bG, bD = _gan_pair(b, ctx, size, z, nf, n, b.FP32)
+        _, _, bG, bD, _ = fp32_gan_pair(b, ctx, *_dcgan(16, 12, 8), n)
         gan = b.Gan(bG, bD, use_cuda_graph=graph)
         gan.upload(*data)
         for _ in range(3):
@@ -144,7 +126,6 @@ def test_fp32_reference_graphs_replay_J408_510(b200):
     """The reference file's own graphs (C1) driven exactly like the Java loop body: dis fit by two parameter-averaged
     workers, 12 D->gan copies, gan fit, 16 gan->gen copies -- through getParam/setParam/fit/output only."""
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m
     n, z = 8, 2
     dis_s, gen_s, gan_s = m.reference_discriminator(0.002), m.reference_generator(0.0, z), m.reference_gan(0.004, z)
     odis = o.net_from_specs(dis_s, (1, 28, 28), grad_clip=1.0, seed=1, flat_input=False); ogen = o.net_from_specs(gen_s, (z,), grad_clip=1.0, seed=2); ogan = o.net_from_specs(gan_s, (z,), grad_clip=1.0, seed=3)
@@ -167,7 +148,7 @@ def test_fp32_reference_graphs_replay_J408_510(b200):
     assert abs(s0 - r["score_d_real"]) < TOL * abs(r["score_d_real"]) and abs(s1 - r["score_d_fake"]) < TOL * abs(r["score_d_fake"])
     bdis.set_params(0.5 * (bw0.params() + bw1.params()))                      # ParameterAveragingTrainingMaster: params AND updater state
     bdis.set_updater_state(0.5 * (bw0.updater_state() + bw1.updater_state()))
-    _assert_close_up_to_sign_flips(bdis.params(), odis.params_flat(), lr=0.002)
+    assert_close_up_to_sign_flips(bdis.params(), odis.params_flat(), 0.002, TOL)
     for s in dis_s:                                                           # J:429-460
         for p, cnt in _params_of(s, bdis):
             bgan.set_param(s["name"].replace("dis_", "gan_dis_", 1), p, bdis.get_param(s["name"], p, cnt))
@@ -176,19 +157,10 @@ def test_fp32_reference_graphs_replay_J408_510(b200):
     for s in gen_s:                                                           # J:474-510
         for p, cnt in _params_of(s, bgen):
             bgen.set_param(s["name"], p, bgan.get_param(s["name"].replace("gen_", "gan_", 1), p, cnt))
-    _assert_close_up_to_sign_flips(bgen.params(), ogen.params_flat(), lr=0.004)
-    _assert_close_up_to_sign_flips(bgan.params(), ogan.params_flat(), lr=0.004)
+    assert_close_up_to_sign_flips(bgen.params(), ogen.params_flat(), 0.004, TOL)
+    assert_close_up_to_sign_flips(bgan.params(), ogan.params_flat(), 0.004, TOL)
     for nn in (bdis, bw0, bw1, bgen, bgan):
         nn.close()
-
-
-def _assert_close_up_to_sign_flips(got, want, lr):
-    """The reference runs RmsProp(lr, rmsDecay=1e-8, eps=1e-8) (J:133): the update is lr*sign(g) for every |g| >~ 1e-8, so an element
-    whose gradient is numerically zero can legitimately land on the other side by one lr step. Everything else must match to TOL."""
-    d = np.abs(np.asarray(got, np.float64) - np.asarray(want, np.float64))
-    scale = np.abs(want).max()
-    assert d.max() <= 2.02 * lr, d.max()
-    assert (d > TOL * scale).mean() < 2e-2, (d > TOL * scale).mean()
 
 
 def _params_of(spec, net):
@@ -247,10 +219,9 @@ def test_simt_conv_kernels_match_oracle(b200, case, prec):
 def test_bf16_gan_step_tracks_oracle(b200):
     """End to end in tensor-core mode: same step, bf16 activations/weights, fp32 accumulation and master weights."""
     b, ctx = b200
-    size, z, nf, n = 16, 12, 8, 16
-    G, D, bG, bD = _gan_pair(b, ctx, size, z, nf, n, b.BF16, clip_eps=0.0)
+    n = 16
+    G, D, bG, bD, data = fp32_gan_pair(b, ctx, *_dcgan(16, 12, 8), n, quirks=o.Quirks(xent_clip_eps=0.0), precision=b.BF16, xent_clip_eps=0.0)
     gan = b.Gan(bG, bD, use_cuda_graph=False)
-    data = [a.astype(np.float64) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
     r = o.gan_step(G, D, *data)
     losses = gan.step(*data)
     assert abs(losses[0] - r["loss_d_real"]) < 0.05 and abs(losses[1] - r["loss_d_fake"]) < 0.05 and abs(losses[2] - r["loss_g"]) < 0.05
@@ -261,7 +232,6 @@ def test_bf16_gan_step_tracks_oracle(b200):
 def test_full_size_c2_step_properties(b200):
     """BASELINE config C2 (64x64x3, z=100, batch 128) at full size: size-independent properties."""
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m
     n = 128
     gs, ds = m.dcgan_generator(64, 100, 64, 3), m.dcgan_discriminator(64, 64, 3)
     bG = b.Net(ctx, gs, (100,), max_batch=n, precision=b.BF16, xent_clip_eps=0.0)
@@ -385,7 +355,6 @@ def test_edge_layers_dcgan_ends(b200, prec):
     """D1 (3->64 conv), G-last (64->3 transposed conv + tanh), D-last (full-window conv -> 1 logit), G-first (z -> 4x4)
     at a size where every specialised kernel engages; fp32 vs oracle to TOL, bf16 vs oracle loosely."""
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m
     P = b.BF16 if prec == "bf16" else b.FP32
     tol = 4e-2 if prec == "bf16" else TOL
     size, z, nf, n = 32, 16, 64, 8          # G: z->(4x4x256)->8x8x128->16x16x64->32x32x3 ; D: 32->16x16x64->8x8x128->4x4x256->1
@@ -428,7 +397,7 @@ def test_edge_layers_dcgan_ends(b200, prec):
                 if p in ("mean", "var"):
                     assert rel_err(p_b[off:off + k], p_o[off:off + k]) < 2 * TOL, (name, p)
                 else:     # Adam's first step is lr*g/(|g|+eps'): elements with a numerically-zero gradient may land one step apart
-                    _assert_close_up_to_sign_flips(p_b[off:off + k], p_o[off:off + k], lr=1e-3)
+                    assert_close_up_to_sign_flips(p_b[off:off + k], p_o[off:off + k], 1e-3, TOL)
                 off += k
     gan.close(); bG.close(); bD.close()
 
@@ -440,7 +409,6 @@ def test_edge_layers_dcgan_ends(b200, prec):
 def test_mlp_gan_step_matches_oracle(b200, prec):
     """Dense layers + OutputLayer(XENT): fp32 to TOL; bf16 at tensor-core-eligible sizes (batch 128, widths multiple of 128) loosely."""
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m
     P = b.BF16 if prec == "bf16" else b.FP32
     n, z, hid, d = 128, 128, 256, 128
     gs, ds = m.mlp_generator(z, hid, d, lr=1e-3), m.mlp_discriminator(d, hid, lr=1e-3)
@@ -466,15 +434,14 @@ def test_mlp_gan_step_matches_oracle(b200, prec):
     want = np.array([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]])
     assert np.all(np.abs(losses - want) < tol * np.maximum(1.0, np.abs(want))), (losses, want)
     if prec == "fp32":
-        _assert_close_up_to_sign_flips(bD.params(), D.params_flat(), lr=1e-3)
-        _assert_close_up_to_sign_flips(bG.params(), G.params_flat(), lr=1e-3)
+        assert_close_up_to_sign_flips(bD.params(), D.params_flat(), 1e-3, TOL)
+        assert_close_up_to_sign_flips(bG.params(), G.params_flat(), 1e-3, TOL)
     gan.close(); bG.close(); bD.close()
 
 
 def test_full_size_c4_and_c5_steps_run(b200):
     """BASELINE configs[3] (128x128x3, 32 per GPU) and configs[4] (MLP-GAN d=256, batch 8192) at full size: finite, learning, in range."""
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m
     for name, gs, ds, gin, din, n in (("c4", m.dcgan_generator(128), m.dcgan_discriminator(128), (100,), (3, 128, 128), 32),
                                      ("c5", m.mlp_generator(128, 1024, 256), m.mlp_discriminator(256, 1024), (128,), (256,), 8192)):
         bG = b.Net(ctx, gs, gin, max_batch=n, precision=b.BF16, xent_clip_eps=0.0)
@@ -500,7 +467,6 @@ def test_full_size_c4_and_c5_steps_run(b200):
 # ------------------------------------------------------------------------------------------------
 def test_boundary_error_codes(b200):
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m
     specs = m.dcgan_discriminator(16, 8, 3)
     net = b.Net(ctx, specs, (3, 16, 16), max_batch=4, precision=b.FP32)
     with pytest.raises(b.B200GanError) as e:                     # batch larger than max_batch
@@ -535,7 +501,6 @@ def test_boundary_error_codes(b200):
 def test_fp32_transfer_learning_head_matches_oracle(b200):
     """SURVEY 8f #3 (J:337-364, 512-545): frozen D trunk + BatchNormalization(1024) + OutputLayer(MCXENT, softmax, 10)."""
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m
     n = 8
     odis = o.net_from_specs(m.reference_discriminator(), (1, 28, 28), grad_clip=1.0, seed=1, flat_input=False)
     rng = np.random.default_rng(3); randomize(odis, rng)
@@ -569,7 +534,7 @@ def test_fp32_transfer_learning_head_matches_oracle(b200):
     for li, name, p, shape, _ in ocv.param_table():
         k = int(np.prod(shape))
         if name in ("dis_batch", "dis_output_layer_7"):
-            _assert_close_up_to_sign_flips(p1[off:off + k], ocv.params_flat()[off:off + k], lr=0.002)
+            assert_close_up_to_sign_flips(p1[off:off + k], ocv.params_flat()[off:off + k], 0.002, TOL)
         else:
             assert np.array_equal(p1[off:off + k], p0[off:off + k]), (name, p)  # not even l2-decayed
         off += k
@@ -601,7 +566,6 @@ def test_fp32_gan_step_matches_golden_fixture(b200):
     """The same step against the committed fixture tests/golden/gan_step_dcgan16.npz (inputs, initial parameters, and the oracle's losses and
     parameters after each of 3 steps; tests/golden/make_golden.py): the CUDA path is compared with fixed bytes, not with a live oracle run."""
     import os
-    from gan_deeplearning4j_b200 import models as m
     b, ctx = b200
     gold = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "gan_step_dcgan16.npz"))
     size, z, nf, n = 16, 12, 8, 8
@@ -623,7 +587,6 @@ def test_checkpoint_resume_equals_uninterrupted_run(b200, tmp_path):
     """ModelSerializer.writeModel / restore (J:606-618) with the updater state AND the iteration counter: N steps, save, restore into a
     fresh net, M more steps == N+M uninterrupted steps, bit for bit (Adam's bias correction depends on t: ADVICE round 1)."""
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m
     specs = m.dcgan_discriminator(16, 8, 3, lr=1e-2)
     rng = np.random.default_rng(9)
     xs = [rng.uniform(-1, 1, (8, 3, 16, 16)).astype(np.float32) for _ in range(5)]; ys = [rng.uniform(0, 1, (8, 1)).astype(np.float32) for _ in range(5)]
@@ -656,7 +619,6 @@ def test_xavier_init_statistics(b200):
     """WeightInit.XAVIER (J:127): W ~ N(0, 2/(fanIn+fanOut)) with conv fanIn = nIn*kH*kW, fanOut = nOut*kH*kW/(sH*sW); biases 0;
     BatchNorm gamma 1, beta 0, mean 0, var 1 -- the formula the oracle's Layer.init restates (dl4j_oracle.Conv2D.fans)."""
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m
     for specs, shape, onet in ((m.dcgan_discriminator(64, 64, 3), (3, 64, 64), o.dcgan_discriminator(64, 64, 3)), (m.dcgan_generator(64, 100, 64, 3), (100,), o.dcgan_generator(64, 100, 64, 3))):
         net = b.Net(ctx, specs, shape, max_batch=2, precision=b.FP32, seed=666)
         other = b.Net(ctx, specs, shape, max_batch=2, precision=b.FP32, seed=667)
@@ -685,7 +647,7 @@ def test_single_process_parameter_averaging_matches_oracle(b200):
     one minibatch each, parameters AND updater state averaged -- against the oracle's parameter_average of two fitted copies (FP32 mode)."""
     import copy
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m, parallel
+    from gan_deeplearning4j_b200 import parallel
     specs = m.reference_discriminator(0.002)
     rng = np.random.default_rng(17)
     onet = o.net_from_specs(specs, (1, 28, 28), grad_clip=1.0); randomize(onet, rng)
@@ -709,54 +671,23 @@ def test_single_process_parameter_averaging_matches_oracle(b200):
 # itself (vector or scalar branch, through its own inverse of the packing map); setParam / setParams / parameter averaging rewrite them
 # from the master.  Either way they must equal the master rounded to nearest even, bit for bit.
 # ------------------------------------------------------------------------------------------------
-def _ps_operand_O(spec):
-    """O of the [O][4][4][C] weight when the layer's conv-equivalent is a 4x4 s2 p1 conv with C <= 4 image channels and O % 64 == 0 (the
-    transposed conv onto the image, and the input gradient of the conv that reads it), else 0."""
-    if tuple(spec.get("kernel", ())) != (4, 4) or tuple(spec.get("stride", ())) != (2, 2) or tuple(spec.get("padding", ())) != (1, 1):
-        return 0
-    O, C = (spec["n_in"], spec["n_out"]) if spec["type"] == "deconv2d" else (spec["n_out"], spec["n_in"])
-    return O if C <= 4 and O % 64 == 0 else 0
-
-
-def _check_weight_operands(b, net, specs, what):
-    packed = 0
-    for li, s in enumerate(specs):
-        if s["type"] not in ("conv2d", "deconv2d", "dense", "output"):
-            continue
-        k = s.get("kernel", (1, 1)); size = s["n_in"] * s["n_out"] * k[0] * k[1]
-        w = bf16_round(w_internal(s, net.get_param(s["name"], "W", size)))
-        assert np.array_equal(net.weight_operand(li, 0, size), w), f"{what}: bf16 copy of {s['name']}.W differs from the rounded master"
-        O = _ps_operand_O(s)
-        if O:
-            got = net.weight_operand(li, 1, 144 * O)
-            assert np.array_equal(got, pack_deconv_ps(w.reshape(O, 4, 4, -1))), f"{what}: packed pixel-shuffle operand of {s['name']}"
-            packed += 1
-        else:
-            with pytest.raises(b.B200GanError) as e:
-                net.weight_operand(li, 1, 144)
-            assert e.value.code == -6
-    return packed
-
-
 def test_bf16_gan_weight_operands_track_the_master(b200):
     """DCGAN 32x32, nf = 64: G-last (64 -> 3) and D-first's input gradient run the pixel-shuffle tensor-core conv.  Three Gan.steps and a resident step replayed from the CUDA
     graph; after each, every GEMM layer's bf16 operands of both nets equal the rounded fp32 master."""
     b, ctx = b200
     size, z, nf, n = 32, 16, 64, 8
-    G, D, bG, bD = _gan_pair(b, ctx, size, z, nf, n, b.BF16)
-    from gan_deeplearning4j_b200 import models as m
-    gs, ds = m.dcgan_generator(size, z, nf, 3, lr=2e-3), m.dcgan_discriminator(size, nf, 3, lr=2e-3)
-    assert _check_weight_operands(b, bG, gs, "G after set_params") == 1 and _check_weight_operands(b, bD, ds, "D after set_params") == 1
+    gs, ds = _dcgan(size, z, nf)
+    _, _, bG, bD, data = fp32_gan_pair(b, ctx, gs, ds, n, size, z, precision=b.BF16)
+    assert check_weight_operands(b, bG, gs, "G after set_params") == 1 and check_weight_operands(b, bD, ds, "D after set_params") == 1
     gan = b.Gan(bG, bD, use_cuda_graph=True)
-    data = [a.astype(np.float32) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
     g0 = bG.params()
     for it in range(3):
         gan.step(*data)
-        assert _check_weight_operands(b, bG, gs, f"G after step {it + 1}") == 1
-        _check_weight_operands(b, bD, ds, f"D after step {it + 1}")
+        assert check_weight_operands(b, bG, gs, f"G after step {it + 1}") == 1
+        check_weight_operands(b, bD, ds, f"D after step {it + 1}")
     data2 = [a.astype(np.float32) for a in o.synthetic_batch(n, size, 3, z, seed=4)]
     gan.upload(*data2); gan.step_resident(n); ctx.sync()
-    _check_weight_operands(b, bG, gs, "G after a resident step"); _check_weight_operands(b, bD, ds, "D after a resident step")
+    check_weight_operands(b, bG, gs, "G after a resident step"); check_weight_operands(b, bD, ds, "D after a resident step")
     assert np.abs(bG.params() - g0).max() > 0
     gan.close(); bG.close(); bD.close()
 
@@ -776,7 +707,6 @@ def _ps_fit_specs(updater, ps_bias):
 @pytest.mark.parametrize("upd", ["sgd", "rmsprop", "adam"])
 def test_bf16_fit_weight_operands_track_the_master(b200, upd, ps_bias):
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m
     u = {"sgd": m.sgd(0.05), "rmsprop": m.rmsprop(1e-3, 0.9, 1e-6), "adam": m.adam(1e-3)}[upd]
     specs = _ps_fit_specs(u, ps_bias)
     off = 0
@@ -789,7 +719,7 @@ def test_bf16_fit_weight_operands_track_the_master(b200, upd, ps_bias):
     rng = np.random.default_rng(8)
     for it in range(3):
         net.fit(rng.standard_normal((6, 64, 8, 8)).astype(np.float32), rng.uniform(0, 1, (6, 1)).astype(np.float32))
-        assert _check_weight_operands(b, net, specs, f"{upd} fit {it + 1}") == 2
+        assert check_weight_operands(b, net, specs, f"{upd} fit {it + 1}") == 2
     net.close()
 
 
@@ -797,20 +727,20 @@ def test_bf16_weight_operands_after_set_params_set_param_restore_and_averaging(b
     """The host-side rewrites of the master: setParams (all layers), setParam of the packed layer alone (net_refresh_shadow's only_layer),
     restore from a checkpoint, and single-process parameter averaging."""
     b, ctx = b200
-    from gan_deeplearning4j_b200 import models as m, parallel
+    from gan_deeplearning4j_b200 import parallel
     specs = _ps_fit_specs(m.adam(1e-3), True)
     net = b.Net(ctx, specs, (64, 8, 8), max_batch=6, precision=b.BF16)
     rng = np.random.default_rng(9)
     net.set_params((0.05 * rng.standard_normal(net.num_params())).astype(np.float32))
-    _check_weight_operands(b, net, specs, "set_params")
+    check_weight_operands(b, net, specs, "set_params")
     net.set_param("ps", "W", (0.1 * rng.standard_normal(64 * 3 * 16)).astype(np.float32))
-    _check_weight_operands(b, net, specs, "set_param(ps, W)")
+    check_weight_operands(b, net, specs, "set_param(ps, W)")
     path = str(tmp_path / "ps.zip"); net.save(path)
     other = b.Net(ctx, specs, (64, 8, 8), max_batch=6, precision=b.BF16, seed=5)
     other.restore(path)
     assert np.array_equal(other.params(), net.params())
-    _check_weight_operands(b, other, specs, "restore")
+    check_weight_operands(b, other, specs, "restore")
     d = [(rng.standard_normal((6, 64, 8, 8)).astype(np.float32), rng.uniform(0, 1, (6, 1)).astype(np.float32)) for _ in range(2)]
     parallel.fit_parameter_averaging(net, d, averaging_frequency=1)
-    _check_weight_operands(b, net, specs, "parameter averaging")
+    check_weight_operands(b, net, specs, "parameter averaging")
     net.close(); other.close()

@@ -8,25 +8,13 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from helpers import bf16_round, check_bf16, push_params, randomize, rel_err
+from gan_deeplearning4j_b200 import models as m
+from helpers import b200, bf16_round, check_bf16, fp32_gan_pair, oracle_gan_pair, pclose, push_params, randomize, rel_err
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
 U = 2.0 ** -24
-
-
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
-
-
-def _m():
-    from gan_deeplearning4j_b200 import models as m
-    return m
 
 
 def _nchw(a_nhwc):
@@ -184,7 +172,6 @@ def test_fp32_forward_bit_identical_to_the_documented_order(b200, kind):
 
 # ------------------------------------------------------------------ FP32 nets against the oracle ----------------------------------------
 def _sub_net(pool, p):
-    m = _m()
     return [{"type": "conv2d", "name": "c1", "n_out": 8, "kernel": (3, 3), "stride": (1, 1), "padding": (1, 1), "activation": "tanh", "updater": m.sgd(0.05)},
             dict(m.subsampling(pool, (3, 3), (2, 2), (1, 1), pnorm=p if pool == "pnorm" else None), name="s1"),
             {"type": "conv2d", "name": "c2", "n_out": 6, "kernel": (2, 2), "stride": (1, 1), "activation": "tanh", "updater": m.adam(1e-2)},
@@ -194,7 +181,6 @@ def _sub_net(pool, p):
 
 
 def _global_net(pool, p):
-    m = _m()
     return [{"type": "conv2d", "name": "c1", "n_out": 8, "kernel": (3, 3), "stride": (2, 2), "padding": (1, 1), "activation": "tanh", "updater": m.sgd(0.05)},
             {"type": "batchnorm", "name": "bn1", "updater": m.sgd(0.05)},
             {"type": "activation", "name": "a1", "activation": "lrelu", "alpha": 0.2},
@@ -241,7 +227,6 @@ def test_bf16_nets_layer_by_layer(b200, pool, p):
     """A 16x16 DCGAN discriminator with a global-pooling head, and a conv -> subsampling -> conv -> global net: each layer against the oracle's
     layer run on the GPU's own input to it (check_bf16)."""
     b, ctx = b200
-    m = _m()
     n = 16
     sub = "avg" if pool == "max" else pool
     specs2 = [{"type": "conv2d", "name": "c1", "n_out": 64, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "activation": "lrelu", "alpha": 0.2},
@@ -289,14 +274,11 @@ def test_bf16_gan_step_with_global_pooling_head_is_reproducible(b200, pool):
     """Graph replay equals eager execution and two fresh nets equal each other, bit for bit (the split global-pooling reduction folds in a fixed
     order); the losses stay finite and near the FP32 oracle's first step."""
     b, ctx = b200
-    m = _m()
     size, z, nf, n = 32, 16, 32, 16
     gs = m.dcgan_generator(size, z, nf, 3, lr=2e-4)
     ds = m.dcgan_discriminator(size, nf, 3, lr=2e-4, global_pooling=pool)
     data = [a.astype(np.float32) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
-    rng = np.random.default_rng(5)
-    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
-    randomize(G, rng); randomize(D, rng)
+    G, D = oracle_gan_pair(gs, ds, size, z)
     runs = [_gan_run(b, ctx, gs, ds, G, D, data, n, size, z, graph) for graph in (True, False, True)]
     for a, c in ((runs[0], runs[1]), (runs[0], runs[2])):
         for u, v in zip(a, c):
@@ -307,35 +289,20 @@ def test_bf16_gan_step_with_global_pooling_head_is_reproducible(b200, pool):
     assert np.all(np.abs(runs[0][0][0] - want) < 0.1 * np.maximum(1, np.abs(want))), (runs[0][0][0], want)
 
 
-def _close(got, want, bound, tol=2 * TOL):
-    """Within tol of max |want|, or DESIGN 1's sign-like first-step allowance: every difference <= bound and at most 2 % of elements beyond tol."""
-    d = np.abs(np.asarray(got, np.float64) - np.asarray(want, np.float64))
-    if d.max() < tol * np.abs(want).max():
-        return True
-    return d.max() <= bound and (d > tol * np.abs(want).max()).mean() <= 0.02
-
-
 def test_fp32_gan_step_with_global_pooling_head_matches_oracle(b200):
     b, ctx = b200
-    m = _m()
-    size, z, nf, n, lr_ = 16, 12, 8, 8, 2e-3
-    gs = m.dcgan_generator(size, z, nf, 3, lr=lr_)
-    ds = m.dcgan_discriminator(size, nf, 3, lr=lr_, global_pooling="sum")
-    data = [a.astype(np.float64) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
-    rng = np.random.default_rng(5)
-    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
-    randomize(G, rng); randomize(D, rng)
-    bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
-    bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2)
-    push_params(G, bG); push_params(D, bD)
+    n, lr_ = 8, 2e-3
+    gs = m.dcgan_generator(16, 12, 8, 3, lr=lr_)
+    ds = m.dcgan_discriminator(16, 8, 3, lr=lr_, global_pooling="sum")
+    G, D, bG, bD, data = fp32_gan_pair(b, ctx, gs, ds, n)
     gan = b.Gan(bG, bD, use_cuda_graph=True)
     for it in range(3):
         r = o.gan_step(G, D, *data)
         lo = gan.step(*data)
         want = np.array([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]])
         assert np.all(np.abs(lo - want) < TOL * np.maximum(1, np.abs(want))), (it, lo, want)
-        assert _close(bD.params(), D.params_flat(), 2 * lr_), (it, "D", rel_err(bD.params(), D.params_flat()))
-        assert _close(bG.params(), G.params_flat(), 2 * lr_), (it, "G", rel_err(bG.params(), G.params_flat()))
+        assert pclose(bD.params(), D.params_flat(), 2 * lr_), (it, "D", rel_err(bD.params(), D.params_flat()))
+        assert pclose(bG.params(), G.params_flat(), 2 * lr_), (it, "G", rel_err(bG.params(), G.params_flat()))
     gan.close(); bG.close(); bD.close()
 
 
@@ -358,7 +325,6 @@ def test_launches_per_pass(b200):
     the same net fed the pooled features directly, and a global / subsampling layer in the middle against MAXPOOL of the same geometry (one
     launch each way)."""
     b, ctx = b200
-    m = _m()
     head = lambda: [{"type": "dense", "name": "d", "n_out": 5, "activation": "tanh", "updater": m.sgd(0.1)},
                     {"type": "output", "name": "o", "n_out": 3, "loss": "mse", "updater": m.sgd(0.1)}]
     conv = lambda frozen=False: {"type": "conv2d", "name": "c", "n_out": 8, "kernel": (3, 3), "padding": (1, 1), "activation": "tanh", "updater": m.sgd(0.1),
@@ -388,7 +354,6 @@ def test_launches_per_pass(b200):
 def test_rejections(b200):
     b, ctx = b200
     from gan_deeplearning4j_b200 import engine, _lib
-    m = _m()
 
     def create(spec_list, mutate=None, shape=(4, 6, 6)):
         descs = [engine.layer_desc(s) for s in spec_list]

@@ -6,62 +6,18 @@ import copy
 import numpy as np
 import pytest
 
-from helpers import bf16_round, pack_deconv_ps, push_params, randomize, rel_err, w_internal
+from gan_deeplearning4j_b200 import models as m
+from helpers import (b200, bf16_gan, check_weight_operands, compare_params_and_state, fp32_gan_pair, launches_per_step, mlp_convbn_specs,
+                     push_params, randomize)
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
 
 
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
-
-
-def _m():
-    from gan_deeplearning4j_b200 import models as m
-    return m
-
-
 def _specs(kind, upd, lr):
-    m = _m()
     mk = {"sgd": lambda: m.sgd(copy.deepcopy(lr)), "rmsprop": lambda: m.rmsprop(copy.deepcopy(lr), 0.9, 1e-8), "adam": lambda: m.adam(copy.deepcopy(lr))}[upd]
-    if kind == "mlp":
-        return [{"type": "dense", "name": "d1", "n_out": 256, "activation": "tanh", "updater": mk(), "l2": 1e-3},
-                {"type": "dense", "name": "d2", "n_out": 128, "activation": "lrelu", "alpha": 0.2, "updater": mk()},
-                {"type": "output", "name": "out", "n_out": 1, "updater": mk()}], (64,)
-    return ([{"type": "conv2d", "name": "c1", "n_out": 8, "kernel": (3, 3), "stride": (2, 2), "padding": (1, 1), "updater": mk()},
-             {"type": "activation", "name": "a1", "activation": "lrelu", "alpha": 0.2},
-             {"type": "conv2d", "name": "c2", "n_out": 12, "kernel": (3, 3), "stride": (1, 1), "padding": (1, 1), "has_bias": False, "updater": mk()},
-             {"type": "batchnorm", "name": "bn2", "updater": mk()}, {"type": "activation", "name": "a2", "activation": "tanh"},
-             {"type": "cnn_to_ff", "name": "flat"},
-             {"type": "dense", "name": "fc", "n_out": 10, "activation": "tanh", "updater": mk()},
-             {"type": "output", "name": "out", "n_out": 1, "updater": mk()}], (3, 8, 8))
-
-
-def _state_flat(onet, k):
-    out = []
-    for li, _, p, shape, order in onet.param_table():
-        st = onet.state.get((li, p))
-        out.append((st[k] if st is not None and k < len(st) else np.zeros(shape)).ravel(order=order.upper()))
-    return np.concatenate(out)
-
-
-def _compare(onet, bnet, what, tol=TOL):
-    p_b, p_o = bnet.params(), onet.params_flat()
-    st = bnet.updater_state(); n = bnet.num_params()
-    s0, s1 = _state_flat(onet, 0), _state_flat(onet, 1)
-    off = 0
-    for li, name, pn, shape, _ in onet.param_table():
-        k = int(np.prod(shape)); sl = slice(off, off + k)
-        assert rel_err(p_b[sl], p_o[sl]) < tol, (what, name, pn, rel_err(p_b[sl], p_o[sl]))
-        for b_st, o_st in ((st[:n][sl], s0[sl]), (st[n:][sl], s1[sl])):
-            if np.abs(o_st).max() > 0:
-                assert rel_err(b_st, o_st) < tol, (what, name, pn, "state")
-        off += k
+    return mlp_convbn_specs(kind, mk)
 
 
 def _f32_close(got, want) -> bool:
@@ -71,7 +27,6 @@ def _f32_close(got, want) -> bool:
 
 
 def _all_schedules(type_):
-    m = _m()
     return [m.exponential_schedule(0.1, 0.97, type=type_), m.inverse_schedule(0.1, 0.01, 0.75, type=type_),
             m.sigmoid_schedule(0.1, 0.05, 10, type=type_), m.step_schedule(0.1, 0.5, 10, type=type_), m.step_schedule(0.3, 0.7, 2.5, type=type_),
             m.map_schedule({0: 0.1, 10: 0.05, 100: 0.01, 12345: 1e-4}, type=type_)]
@@ -97,7 +52,6 @@ def test_learning_rate_of_every_kind_matches_the_restatement(b200, type_):
 
 
 def _fit_run(b, ctx, kind, upd, sched_name):
-    m = _m()
     lr0 = 0.05 if upd == "sgd" else 1e-2
     sched = m.step_schedule(lr0, 0.5, 3) if sched_name == "step" else m.map_schedule({0: lr0, 2: 0.3 * lr0, 5: 0.6 * lr0})
     specs, shape = _specs(kind, upd, sched)
@@ -121,14 +75,13 @@ def test_fp32_fit_matches_oracle(b200, kind, upd, sched_name):
         assert _f32_close(bnet.learning_rate(name), onet.learning_rate(name))
         seen.add(float(bnet.learning_rate(name)))
         onet.fit(x, y); bnet.fit(x, y)
-        _compare(onet, bnet, (kind, upd, sched_name, it))
+        compare_params_and_state(onet, bnet, (kind, upd, sched_name, it), TOL)
     assert len(seen) == 3, seen                    # the run crossed two schedule boundaries
     bnet.close()
 
 
 def test_set_and_clear_mid_run_take_effect_at_the_next_update(b200):
     b, ctx = b200
-    m = _m()
     specs, shape = _specs("mlp", "adam", 1e-2)
     rng = np.random.default_rng(3)
     onet = o.net_from_specs(specs, shape, seed=2); randomize(onet, rng)
@@ -147,43 +100,28 @@ def test_set_and_clear_mid_run_take_effect_at_the_next_update(b200):
             bnet.set_epoch(4); onet.set_epoch(4)
         x, y = rng.uniform(-1, 1, (6,) + shape), rng.uniform(0, 1, (6, 1))
         onet.fit(x, y); bnet.fit(x, y)
-        _compare(onet, bnet, ("plan", it))
+        compare_params_and_state(onet, bnet, ("plan", it), TOL)
     assert bnet.learning_rate("d2") == np.float32(1e-2)
     bnet.close()
 
 
-def _fp32_dcgan(b, ctx, n, gsched, dsched):
-    m = _m()
-    size, z, nf = 16, 12, 8
-    gs, ds = m.dcgan_generator(size, z, nf, 3, lr=gsched), m.dcgan_discriminator(size, nf, 3, lr=dsched)
-    rng = np.random.default_rng(5)
-    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
-    randomize(G, rng); randomize(D, rng)
-    bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
-    bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2)
-    push_params(G, bG); push_params(D, bD)
-    data = [a.astype(np.float64) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
-    return G, D, bG, bD, data
-
-
 def test_fp32_gan_step_matches_oracle(b200):
     b, ctx = b200
-    m = _m()
     n = 8
-    G, D, bG, bD, data = _fp32_dcgan(b, ctx, n, m.exponential_schedule(2e-3, 0.8), m.step_schedule(2e-3, 0.5, 2))
+    gs, ds = m.dcgan_generator(16, 12, 8, 3, lr=m.exponential_schedule(2e-3, 0.8)), m.dcgan_discriminator(16, 8, 3, lr=m.step_schedule(2e-3, 0.5, 2))
+    G, D, bG, bD, data = fp32_gan_pair(b, ctx, gs, ds, n)
     gan = b.Gan(bG, bD, use_cuda_graph=True)
     for it in range(5):
         r = o.gan_step(G, D, *data)
         lo = gan.step(*data)
         want = np.array([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]])
         assert np.all(np.abs(lo - want) < TOL * np.maximum(1, np.abs(want))), (it, lo, want)
-        _compare(D, bD, (it, "D"), 2 * TOL); _compare(G, bG, (it, "G"), 2 * TOL)
+        compare_params_and_state(D, bD, (it, "D"), 2 * TOL); compare_params_and_state(G, bG, (it, "G"), 2 * TOL)
     assert _f32_close(bD.learning_rate("dis_conv_1"), 2e-3 * 0.25) and _f32_close(bG.learning_rate("gen_deconv_1"), 2e-3 * 0.8 ** 5)
     gan.close(); bG.close(); bD.close()
 
 
 def _bf16_dcgan(b, ctx, n, size=32, gsched=2e-3, dsched=2e-3):
-    m = _m()
     z, nf = 16, 64
     gs, ds = m.dcgan_generator(size, z, nf, 3, lr=gsched), m.dcgan_discriminator(size, nf, 3, lr=dsched)
     G = b.Net(ctx, gs, (z,), max_batch=n, precision=b.BF16, xent_clip_eps=0.0)
@@ -196,7 +134,6 @@ def test_graph_replay_matches_eager_with_epoch_and_schedule_changes(b200):
     """BF16 GAN steps, eager and from CUDA graphs: an EPOCH schedule on G whose epoch changes between replays (no re-capture needed), and a
     schedule set on D mid-run and cleared again (re-captures).  Losses, parameters and updater state agree bit for bit."""
     b, ctx = b200
-    m = _m()
     n = 8
     gsched = m.step_schedule(2e-3, 0.5, 1, type="epoch")
     runs = []
@@ -221,7 +158,6 @@ def test_graph_replay_matches_eager_with_epoch_and_schedule_changes(b200):
 
 def test_identity_schedules_are_bit_identical_to_none_through_the_graph(b200):
     b, ctx = b200
-    m = _m()
     n = 8
     runs = []
     for g_lr, d_lr in ((2e-3, 2e-3), (m.exponential_schedule(2e-3, 1.0), m.map_schedule({0: 2e-3}, type="epoch"))):
@@ -239,7 +175,6 @@ def test_checkpoint_resume_is_bit_identical(b200, tmp_path):
     """Save after k fits (the schedules live in the checkpoint's specs, the epoch in its metadata), restore into a fresh net built from the
     checkpoint's specs, continue: the same parameters and state as an uninterrupted run."""
     b, ctx = b200
-    m = _m()
     from gan_deeplearning4j_b200 import serializer
     specs, shape = _specs("mlp", "adam", m.step_schedule(1e-2, 0.5, 2))
     rng = np.random.default_rng(4)
@@ -273,27 +208,14 @@ def test_checkpoint_resume_is_bit_identical(b200, tmp_path):
         net.close()
 
 
-def _check_weight_operands(net, specs, what):
-    for li, s in enumerate(specs):
-        if s["type"] not in ("conv2d", "deconv2d", "dense", "output"):
-            continue
-        k = s.get("kernel", (1, 1)); size = s["n_in"] * s["n_out"] * k[0] * k[1]
-        w = bf16_round(w_internal(s, net.get_param(s["name"], "W", size)))
-        assert np.array_equal(net.weight_operand(li, 0, size), w), f"{what}: bf16 copy of {s['name']}.W"
-        O, C = (s["n_in"], s["n_out"]) if s["type"] == "deconv2d" else (s["n_out"], s["n_in"])
-        if tuple(k) == (4, 4) and tuple(s.get("stride", ())) == (2, 2) and tuple(s.get("padding", ())) == (1, 1) and C <= 4 and O % 64 == 0:
-            assert np.array_equal(net.weight_operand(li, 1, 144 * O), pack_deconv_ps(w.reshape(O, 4, 4, -1))), f"{what}: packed operand of {s['name']}"
-
-
 def test_bf16_weight_copies_track_the_master(b200):
     b, ctx = b200
-    m = _m()
     gs, ds, G, D, data = _bf16_dcgan(b, ctx, 8, gsched=m.sigmoid_schedule(4e-3, 0.5, 2), dsched=m.map_schedule({0: 2e-3, 2: 5e-3}))
     gan = b.Gan(G, D, use_cuda_graph=True)
     g0 = G.params()
     for it in range(4):
         gan.step(*data)
-        _check_weight_operands(G, gs, f"G step {it}"); _check_weight_operands(D, ds, f"D step {it}")
+        check_weight_operands(b, G, gs, f"G step {it}"); check_weight_operands(b, D, ds, f"D step {it}")
     assert np.abs(G.params() - g0).max() > 0
     gan.close(); G.close(); D.close()
 
@@ -301,28 +223,16 @@ def test_bf16_weight_copies_track_the_master(b200):
 def test_launch_counts(b200):
     """C2 (bench.py's DCGAN 64x64, bf16, batch 128) launches 83 kernels per step with and without schedules; fit launches the same."""
     b, ctx = b200
-    m = _m()
     n = 128
-    G = b.Net(ctx, m.dcgan_generator(64, 100, 64, 3), (100,), max_batch=n, precision=b.BF16, xent_clip_eps=0.0, seed=666)
-    D = b.Net(ctx, m.dcgan_discriminator(64, 64, 3), (3, 64, 64), max_batch=2 * n, precision=b.BF16, xent_clip_eps=0.0, bn_groups=2, seed=667)
+    G, D = bf16_gan(b, ctx, m.dcgan_generator(64, 100, 64, 3), m.dcgan_discriminator(64, 64, 3), (100,), (3, 64, 64), n)
     gan = b.Gan(G, D, use_cuda_graph=True)
     rng = np.random.default_rng(1)
     gan.upload(rng.uniform(-1, 1, (n, 3, 64, 64)), rng.uniform(-1, 1, (n, 100)), rng.uniform(-1, 1, (n, 100)), np.ones((n, 1)), np.zeros((n, 1)), np.ones((n, 1)))
-
-    def per_step():
-        for _ in range(2):
-            gan.step_resident(n)
-        ctx.sync(); l0 = ctx.launch_count()
-        for _ in range(3):
-            gan.step_resident(n)
-        ctx.sync()
-        return (ctx.launch_count() - l0) / 3
-
-    assert per_step() == 83
+    assert launches_per_step(ctx, gan, n) == 83
     G.set_lr_schedule(m.exponential_schedule(2e-4, 0.999)); D.set_lr_schedule(m.map_schedule({0: 2e-4, 3: 1e-4}, type="epoch"))
-    assert per_step() == 83
+    assert launches_per_step(ctx, gan, n) == 83
     G.set_lr_schedule(None); D.set_lr_schedule(None)
-    assert per_step() == 83
+    assert launches_per_step(ctx, gan, n) == 83
     gan.close(); G.close(); D.close()
     specs, shape = _specs("mlp", "adam", 1e-3)
     net = b.Net(ctx, specs, shape, max_batch=4, precision=b.FP32)
@@ -339,7 +249,6 @@ def test_rejections(b200):
     b, ctx = b200
     import ctypes as C
     from gan_deeplearning4j_b200 import _lib
-    m = _m()
     specs = [{"type": "dense", "name": "d1", "n_out": 8, "activation": "tanh", "updater": m.adam(1e-3), "frozen": True},
              {"type": "dense", "name": "d2", "n_out": 8, "activation": "tanh", "updater": {"kind": "noop"}},
              {"type": "activation", "name": "act", "activation": "relu"},

@@ -7,16 +7,9 @@ import numpy as np
 import pytest
 
 from gan_deeplearning4j_b200 import engine
+from helpers import b200
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
 
 
 def _specs():

@@ -23,21 +23,14 @@ import numpy as np
 import pytest
 
 import conv_ref
-from helpers import bf16_round, push_params, randomize, rel_err
+from gan_deeplearning4j_b200 import models as m
+from helpers import assert_close_up_to_sign_flips, b200, bf16_round, push_params, randomize, rel_err
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
 
 U = 2.0 ** -24
 TOL = 1e-3          # the FP32 DL4J-parity bar of tests/test_gpu_parity.py
-
-
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx, ctx.device_info()["sm_count"]
-    ctx.close()
 
 
 def geom(n, h, w, c, oc, k=(1, 1), s=(1, 1), p=(0, 0)):
@@ -165,7 +158,7 @@ SIMT_GEOMS = {
 @pytest.mark.parametrize("prec", ["fp32", "bf16"])
 @pytest.mark.parametrize("name", list(SIMT_GEOMS))
 def test_simt_kernel_geometries(b200, name, prec):
-    b, ctx, _ = b200
+    b, ctx = b200
     g = geom(*SIMT_GEOMS[name])
     rng = np.random.default_rng(zlib.crc32(name.encode()))
     for exact in (True, False):
@@ -185,7 +178,7 @@ EPILOGUES = [(a, True, True) for a in ("identity", "tanh", "sigmoid", "relu", "l
 @pytest.mark.parametrize("epi", EPILOGUES, ids=[f"{a}{'_bias' if bb else ''}{'_scale' if s else ''}" for a, bb, s in EPILOGUES])
 def test_simt_kernel_epilogues(b200, epi, prec):
     """act(acc * scale + bias), every activation with and without bias and scale, on fprop and dgrad (the (acc + bias) * scale order fails)."""
-    b, ctx, _ = b200
+    b, ctx = b200
     act, bias, scale = epi
     g = geom(*SIMT_GEOMS["asym"])
     rng = np.random.default_rng(3)
@@ -204,7 +197,7 @@ TILE_CASES = [(TILE_N[(i + j) % 5], c, TILE_O[(i + j) % 7]) for i, c in enumerat
 @pytest.mark.parametrize("prec", ["fp32", "bf16"])
 @pytest.mark.parametrize("case", TILE_CASES, ids=[f"n{n}_c{c}_o{oc}" for n, c, oc in TILE_CASES])
 def test_simt_kernel_tile_remainders(b200, case, prec):
-    b, ctx, _ = b200
+    b, ctx = b200
     n, c, oc = case
     g = geom(n, 1, 1, c, oc)
     rng = np.random.default_rng(n * 1000 + c * 10 + oc)
@@ -225,7 +218,7 @@ WGRAD_REGIMES = {
 @pytest.mark.parametrize("prec", ["fp32", "bf16"])
 @pytest.mark.parametrize("name", list(WGRAD_REGIMES))
 def test_simt_wgrad_split_regimes(b200, name, prec):
-    b, ctx, _ = b200
+    b, ctx = b200
     args, want = WGRAD_REGIMES[name]
     g = geom(*args)
     assert simt_wgrad_splits(g) == want
@@ -243,7 +236,8 @@ def edge_geom(n, oh, ow, c, oc):
 @pytest.mark.parametrize("c", [1, 2, 3, 4])
 def test_edge_deconv_small_c(b200, c, prec):
     """G-last's forward: transposed conv onto C <= 4 channels, bias + tanh; H != W, N = 1, and a batch whose grid-stride loop takes two passes."""
-    b, ctx, sms = b200
+    b, ctx = b200
+    sms = ctx.device_info()["sm_count"]
     rng = np.random.default_rng(20 + c)
     passes = 8 * sms * 128                                 # positions one pass of the capped grid covers
     for oc in (8, 24, 128):
@@ -261,7 +255,8 @@ def test_edge_deconv_small_c(b200, c, prec):
 @pytest.mark.parametrize("c", [1, 2, 3, 4])
 def test_edge_conv_small_cin(b200, c, prec):
     """D1's forward: conv from C <= 4 channels, bias + lrelu; O = 192 at C = 4 is exactly the 48 KB shared-memory predicate."""
-    b, ctx, sms = b200
+    b, ctx = b200
+    sms = ctx.device_info()["sm_count"]
     rng = np.random.default_rng(30 + c)
     for oc in (16, 48) + ((192,) if c == 4 else ()):
         for n, oh, ow in ((1, 3, 4), (2, 5, 8)):
@@ -278,7 +273,8 @@ def test_edge_conv_small_cin(b200, c, prec):
 def test_edge_wgrad_small_cin(b200, oc, prec):
     """D1 / G-last weight gradient at every C <= 4: one CTA with a 15-pixel tail, and a multi-CTA batch.  O = 136 and 256 need more than
     48 KB of dynamic shared memory."""
-    b, ctx, sms = b200
+    b, ctx = b200
+    sms = ctx.device_info()["sm_count"]
     rng = np.random.default_rng(40 + oc)
     for c in (1, 2, 3, 4):
         for n, oh, ow in ((1, 3, 5), (4, 8, 12)):
@@ -299,7 +295,7 @@ SMALL_O_CASES = [(SMALL_O_N[(oc + ci + j) % 5], c, oc) for oc in (1, 2, 3, 4) fo
 def test_dense_small_o(b200, case, prec):
     """<= 4 output units: forward with bias + activation, input gradient, split weight gradient; W / dW at an odd offset (load8_any's
     scalar path) and aligned."""
-    b, ctx, _ = b200
+    b, ctx = b200
     n, c, oc = case
     g = geom(n, 1, 1, c, oc)
     rng = np.random.default_rng(n * 7 + c + oc)
@@ -320,7 +316,7 @@ SMALL_K_CASES = [(SMALL_K_N[(3 * i + ci) % 8], c, oc) for i, oc in enumerate((1,
 def test_dense_small_k(b200, case, prec):
     """Reduction of <= 128 (G-first): the input-gradient form with bias + activation and the weight gradient.  dW at an odd element offset
     is not 8-byte aligned: the SIMT kernel then stores scalars, and BF16 takes it instead of the mma.sync kernel."""
-    b, ctx, _ = b200
+    b, ctx = b200
     n, c, oc = case
     g = geom(n, 1, 1, c, oc)
     rng = np.random.default_rng(n * 13 + c + oc)
@@ -339,7 +335,7 @@ def test_dense_small_k(b200, case, prec):
 
 
 def test_hook_refuses_epilogues_the_wrappers_lack(b200):
-    b, ctx, _ = b200
+    b, ctx = b200
     x = np.ones(8 * 24, np.float32); w = np.ones(24, np.float32); dy = np.ones(8, np.float32)
     g = geom(8, 1, 1, 24, 1)
     for kind, a, bb, size, kw in ((1, dy, w, 8 * 24, dict(bias=np.ones(24))), (1, dy, w, 8 * 24, dict(act="tanh")), (2, x, dy, 24, dict(act="relu")),
@@ -376,7 +372,6 @@ def _fp32_grads_and_fit(b, ctx, specs, in_shape, x, y, prec):
 
 
 def _bug1_nets():
-    from gan_deeplearning4j_b200 import models as m
     u = m.sgd(0.1)
     head = [{"type": "conv2d", "name": "c", "n_out": 5, "kernel": (4, 4), "stride": (1, 1), "padding": (0, 0), "activation": "tanh", "updater": u},
             {"type": "cnn_to_ff", "name": "flat"}, {"type": "output", "name": "out", "n_out": 1, "updater": u}]
@@ -391,25 +386,17 @@ def _bug1_nets():
 @pytest.mark.parametrize("prec", ["fp32", "bf16"])
 @pytest.mark.parametrize("net", ["full_window_conv_head", "dense_after_1x1_conv"])
 def test_dense_small_k_wgrad_at_odd_parameter_offset_through_the_engine(b200, net, prec):
-    b, ctx, _ = b200
+    b, ctx = b200
     specs, in_shape, n_out = _bug1_nets()[net]
     rng = np.random.default_rng(9)
     x = rng.uniform(-1, 1, (8,) + in_shape); y = rng.uniform(0, 1, (8, n_out))
     _fp32_grads_and_fit(b, ctx, specs, in_shape, x, y, b.FP32 if prec == "fp32" else b.BF16)
 
 
-def _assert_close_up_to_sign_flips(got, want, lr):
-    """Adam's first step is lr * g / (|g| + eps): an element whose gradient is numerically zero may land one lr step apart."""
-    d = np.abs(np.asarray(got, np.float64) - np.asarray(want, np.float64))
-    assert d.max() <= 2.02 * lr, d.max()
-    assert (d > TOL * np.abs(want).max()).mean() < 2e-2
-
-
 @pytest.mark.parametrize("prec", ["fp32", "bf16"])
 def test_dcgan_with_192_filters_steps(b200, prec):
     """D1 with 192 filters and G-last from 192 channels: edge_wgrad_small_cin at O = 192 needs 64 KB of dynamic shared memory."""
-    b, ctx, _ = b200
-    from gan_deeplearning4j_b200 import models as m
+    b, ctx = b200
     P = b.BF16 if prec == "bf16" else b.FP32
     size, z, nf, n = 16, 12, 192, 8
     gs, ds = m.dcgan_generator(size, z, nf, 3, lr=1e-3), m.dcgan_discriminator(size, nf, 3, lr=1e-3)
@@ -447,6 +434,6 @@ def test_dcgan_with_192_filters_steps(b200, prec):
                 if p in ("mean", "var"):
                     assert rel_err(p_b[off:off + k], p_o[off:off + k]) < 2 * TOL, (name, p)
                 else:
-                    _assert_close_up_to_sign_flips(p_b[off:off + k], p_o[off:off + k], lr=1e-3)
+                    assert_close_up_to_sign_flips(p_b[off:off + k], p_o[off:off + k], 1e-3, TOL)
                 off += k
     gan.close(); bG.close(); bD.close()

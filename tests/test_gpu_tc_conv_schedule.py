@@ -23,7 +23,7 @@ import pytest
 
 import conv_ref
 import tc_schedule as ts
-from helpers import bf16_round, check_bf16
+from helpers import b200, bf16_round, check_bf16
 
 Case = collections.namedtuple("Case", "name kind n h w c o k s p groups tiles num_kb")
 # kind: fprop (conv forward, 1x1 dense included), dgrad (4x4 s2 p1 input gradient in phase form: c = dx channels, o = dy channels), ps (the
@@ -106,14 +106,6 @@ def test_schedule_table_reaches_every_corner():
 
 
 # ------------------------------------------------------------------------------------------------ GPU
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
-
-
 _OPERANDS = {}
 
 

@@ -24,7 +24,7 @@ import pytest
 
 import conv_ref
 import test_gpu_tc_conv_schedule as sched
-from helpers import bf16_round, check_bf16
+from helpers import b200, bf16_round, check_bf16
 
 SLAB_ROWS = 144
 SMS = 132
@@ -199,14 +199,6 @@ def operands(case):
         gemm = conv_ref.conv2d_input_grad(a, wt, (h, w), 2, 1)
     _OPERANDS[case.name] = (geom, a, wt, gemm.shape, gemm)
     return _OPERANDS[case.name]
-
-
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
 
 
 @pytest.mark.gpu

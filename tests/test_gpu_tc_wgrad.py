@@ -32,7 +32,7 @@ import pytest
 
 import conv_ref
 import tc_schedule as ts
-from helpers import bf16_round, check_bf16, rel_err
+from helpers import b200, bf16_round, check_bf16, rel_err
 
 SMS = ts.SMS                 # H100 SXM
 STAGES = 4                   # TMA ring depth of tc_wgrad_kernel<BNW, 4>
@@ -219,14 +219,6 @@ def test_table_reaches_every_corner():
 
 
 # ------------------------------------------------------------------------------------------------ GPU
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx, ctx.device_info()["sm_count"]
-    ctx.close()
-
-
 def ints(rng, values, shape):
     return rng.choice(np.array(values, np.float32), shape)
 
@@ -246,7 +238,8 @@ def wgrad_geom(case):
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", WGRAD_CASES, ids=[c.name for c in WGRAD_CASES])
 def test_tc_wgrad_exact_at_every_split(b200, case):
-    b, ctx, sms = b200
+    b, ctx = b200
+    sms = ctx.device_info()["sm_count"]
     g = wgrad_geom(case)
     rng = np.random.default_rng(zlib.crc32(case.name.encode()))
     x = ints(rng, [-3, -2, -1, 1, 2, 3], (case.n, case.h, case.w, case.c))
@@ -277,7 +270,8 @@ def edge_geom(c, g, o=64):
 @pytest.mark.gpu
 @pytest.mark.parametrize("c,g", EDGE_CASES, ids=[f"C{c}-{g.name}" for c, g in EDGE_CASES])
 def test_tc_edge_wgrad_exact_at_every_cta_count(b200, c, g):
-    b, ctx, sms = b200
+    b, ctx = b200
+    sms = ctx.device_info()["sm_count"]
     geom = edge_geom(c, g)
     rng = np.random.default_rng(zlib.crc32(f"wgrad C{c} {g.name}".encode()))
     x = ints(rng, [-3, -2, -1, 1, 2, 3], (g.n, g.h, g.w, c))
@@ -344,7 +338,8 @@ def edge_act_emulated(kw, acc):
 @pytest.mark.gpu
 @pytest.mark.parametrize("c,g", EDGE_CASES, ids=[f"C{c}-{g.name}" for c, g in EDGE_CASES])
 def test_tc_edge_conv_epilogues_at_every_cta_count(b200, c, g):
-    b, ctx, sms = b200
+    b, ctx = b200
+    sms = ctx.device_info()["sm_count"]
     rng = np.random.default_rng(zlib.crc32(f"conv C{c} {g.name}".encode()))
     g = conv_geom(g)
     for o in EDGE_OUT:

@@ -8,19 +8,11 @@ import numpy as np
 import pytest
 
 import conv_ref
-from helpers import bf16_round, rel_err
+from helpers import b200, bf16_round, rel_err
 
 pytestmark = pytest.mark.gpu
 
 UNSUPPORTED, ARG = -6, -1
-
-
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
 
 
 def geom(n, h, w, c, o, k=4, s=2, p=1):

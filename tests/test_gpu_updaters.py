@@ -3,39 +3,22 @@ conv+BatchNorm net (parameters and every state slot), a net that mixes kinds per
 and schedules, the FP32 GAN step against the oracle, BF16 graph replay against eager and the bf16 weight copies, AMSGrad checkpoint / resume,
 parameter averaging, launch counts and argument checks."""
 import copy
-import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
-from helpers import bf16_round, pack_deconv_ps, push_params, randomize, rel_err, w_internal
+from gan_deeplearning4j_b200 import models as m
+from helpers import (b200, bf16_gan, check_weight_operands, compare_params_and_state, fp32_gan_pair, launches_per_step, mlp_convbn_specs,
+                     push_params, randomize, run_two_ranks)
 from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TOL = 1e-3
 KINDS = o.EXT_UPDATERS
 
 
-@pytest.fixture(scope="module")
-def b200():
-    import gan_deeplearning4j_b200 as b
-    ctx = b.Context(0)
-    yield b, ctx
-    ctx.close()
-
-
-def _m():
-    from gan_deeplearning4j_b200 import models as m
-    return m
-
-
 def _upd(kind, lr=None):
     """One updater spec of `kind` at test-sized hyperparameters (lr may be a schedule; AdaDelta has none)."""
-    m = _m()
     lr = copy.deepcopy(lr)
     if kind == "nesterovs":
         return m.nesterovs(0.02 if lr is None else lr, 0.9)
@@ -60,61 +43,19 @@ def _specs(net, kinds):
     ks = [kinds] if isinstance(kinds, str) else list(kinds)
     it = iter(ks * 8)
     u = lambda: _upd(next(it))
-    if net == "mlp":
-        return [{"type": "dense", "name": "d1", "n_out": 256, "activation": "tanh", "updater": u(), "l2": 1e-3},
-                {"type": "dense", "name": "d2", "n_out": 128, "activation": "lrelu", "alpha": 0.2, "updater": u()},
-                {"type": "output", "name": "out", "n_out": 1, "updater": u()}], (64,)
     if net == "odd":          # every segment length odd: the updater's scalar path
         return [{"type": "dense", "name": "d1", "n_out": 37, "activation": "tanh", "updater": u(), "l2": 1e-3},
                 {"type": "dense", "name": "d2", "n_out": 23, "activation": "lrelu", "alpha": 0.2, "updater": u()},
                 {"type": "output", "name": "out", "n_out": 1, "updater": u()}], (13,)
-    return ([{"type": "conv2d", "name": "c1", "n_out": 8, "kernel": (3, 3), "stride": (2, 2), "padding": (1, 1), "updater": u(), "l2": 1e-3},
-             {"type": "activation", "name": "a1", "activation": "lrelu", "alpha": 0.2},
-             {"type": "conv2d", "name": "c2", "n_out": 12, "kernel": (3, 3), "stride": (1, 1), "padding": (1, 1), "has_bias": False, "updater": u()},
-             {"type": "batchnorm", "name": "bn2", "updater": u()}, {"type": "activation", "name": "a2", "activation": "tanh"},
-             {"type": "cnn_to_ff", "name": "flat"},
-             {"type": "dense", "name": "fc", "n_out": 10, "activation": "tanh", "updater": u()},
-             {"type": "output", "name": "out", "n_out": 1, "updater": u()}], (3, 8, 8))
+    specs, shape = mlp_convbn_specs(net, u)
+    if net == "convbn":
+        specs[0]["l2"] = 1e-3
+    return specs, shape
 
 
-def _state_flat(onet, k):
-    out = []
-    for li, _, p, shape, order in onet.param_table():
-        st = onet.state.get((li, p))
-        out.append((st[k] if st is not None and k < len(st) else np.zeros(shape)).ravel(order=order.upper()))
-    return np.concatenate(out)
-
-
-def _close(got, want, bound, tol, step=0.0):
-    """Within tol relative to max(|want|, step) -- a parameter tensor whose update cancelled it down to near zero (a one-element bias after
-    one step) is measured against one update step, not against its own size -- or the bounded lr-step exemption: every difference <= bound
-    and at most 2 % of the elements beyond tol."""
-    d = np.abs(np.asarray(got, np.float64) - np.asarray(want, np.float64))
-    scale = max(float(np.abs(want).max()), step)
-    if d.max() < tol * scale:
-        return True
-    return d.max() <= bound and (d > tol * scale).mean() <= 0.02
-
-
-def _compare(onet, bnet, what, bounds, tol=TOL):
-    """Parameters and every state slot of every parameter tensor; bounds: {layer name: exemption bound of its kind}."""
-    p_b, p_o = bnet.params(), onet.params_flat()
-    st = bnet.updater_state(); n = bnet.num_params()
-    slots = st.size // n
-    assert slots in (2, 3)
-    s_o = [_state_flat(onet, k) for k in range(slots)]
-    off = 0
-    for li, name, pn, shape, _ in onet.param_table():
-        k = int(np.prod(shape)); sl = slice(off, off + k)
-        bound = bounds.get(name, 0.0)
-        assert _close(p_b[sl], p_o[sl], bound, tol, bound / 2), (what, name, pn, rel_err(p_b[sl], p_o[sl]))
-        for j in range(slots):
-            b_st, o_st = st[j * n:(j + 1) * n][sl], s_o[j][sl]
-            if np.abs(o_st).max() > 0:
-                assert _close(b_st, o_st, np.inf if bound else 0.0, tol), (what, name, pn, "state", j, rel_err(b_st, o_st))
-            else:
-                assert np.all(b_st == 0), (what, name, pn, "state", j)
-        off += k
+def _with_kind(specs, kind):
+    """specs with every updater replaced by one of `kind`; Adam's specs as they are."""
+    return specs if kind == "adam" else [dict(s, updater=_upd(kind)) if s.get("updater") else s for s in specs]
 
 
 def _bounds(specs):
@@ -131,7 +72,7 @@ def _fit_and_compare(b, ctx, specs, shape, steps=6, grad_clip=0.5, seed=11, **ne
     for it in range(steps):
         x, y = rng.uniform(-1, 1, (6,) + shape), rng.uniform(0, 1, (6, 1))
         onet.fit(x, y); bnet.fit(x, y)
-        _compare(onet, bnet, it, _bounds(specs))
+        compare_params_and_state(onet, bnet, it, TOL, _bounds(specs))
     assert bnet.iteration() == steps
     return onet, bnet
 
@@ -151,7 +92,6 @@ def test_fp32_fit_mixed_kinds_per_layer(b200):
     specs, shape = _specs("convbn", ["amsgrad", "nesterovs", "adadelta", "adamax", "nadam", "adagrad"])
     _, bnet = _fit_and_compare(b, ctx, specs, shape, steps=5)
     bnet.close()
-    m = _m()
     specs, shape = _specs("mlp", "adagrad")
     specs[0]["updater"], specs[2]["updater"] = m.adam(2e-3), m.sgd(0.05)      # existing kinds beside a new one, one updater pass
     _, bnet = _fit_and_compare(b, ctx, specs, shape, steps=4)
@@ -169,7 +109,6 @@ def test_fp32_fit_odd_widths_take_the_scalar_path(b200, kind):
 @pytest.mark.parametrize("kind", KINDS)
 def test_clip_l2_per_layer_and_exponential_schedule(b200, kind):
     b, ctx = b200
-    m = _m()
     specs, shape = _specs("mlp", kind)
     if kind != "adadelta":
         for s in specs:
@@ -183,7 +122,6 @@ def test_clip_l2_per_layer_and_exponential_schedule(b200, kind):
 
 def test_adadelta_refuses_a_learning_rate_schedule(b200):
     b, ctx = b200
-    m = _m()
     specs, shape = _specs("mlp", ["adadelta", "adam", "adadelta"])
     net = b.Net(ctx, specs, shape, max_batch=4)
     for layer in ("d1", "out"):
@@ -198,40 +136,24 @@ def test_adadelta_refuses_a_learning_rate_schedule(b200):
     net.close()
 
 
-def _fp32_dcgan(b, ctx, n, gkind, dkind):
-    m = _m()
-    size, z, nf = 16, 12, 8
-    gs, ds = m.dcgan_generator(size, z, nf, 3), m.dcgan_discriminator(size, nf, 3)
-    gs = [dict(s, updater=_upd(gkind)) if s.get("updater") else s for s in gs]
-    ds = [dict(s, updater=_upd(dkind)) if s.get("updater") else s for s in ds]
-    rng = np.random.default_rng(5)
-    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
-    randomize(G, rng); randomize(D, rng)
-    bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
-    bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2)
-    push_params(G, bG); push_params(D, bD)
-    data = [a.astype(np.float64) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
-    return gs, ds, G, D, bG, bD, data
-
-
 def test_fp32_gan_step_matches_oracle(b200):
     """G on Nesterovs, D on AMSGrad (three state slots), CUDA-graph replay after the first step."""
     b, ctx = b200
     n = 8
-    gs, ds, G, D, bG, bD, data = _fp32_dcgan(b, ctx, n, "nesterovs", "amsgrad")
+    gs, ds = _with_kind(m.dcgan_generator(16, 12, 8, 3), "nesterovs"), _with_kind(m.dcgan_discriminator(16, 8, 3), "amsgrad")
+    G, D, bG, bD, data = fp32_gan_pair(b, ctx, gs, ds, n)
     gan = b.Gan(bG, bD, use_cuda_graph=True)
     for it in range(5):
         r = o.gan_step(G, D, *data)
         lo = gan.step(*data)
         want = np.array([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]])
         assert np.all(np.abs(lo - want) < TOL * np.maximum(1, np.abs(want))), (it, lo, want)
-        _compare(D, bD, (it, "D"), _bounds(ds), 2 * TOL); _compare(G, bG, (it, "G"), _bounds(gs), 2 * TOL)
+        compare_params_and_state(D, bD, (it, "D"), 2 * TOL, _bounds(ds)); compare_params_and_state(G, bG, (it, "G"), 2 * TOL, _bounds(gs))
     assert bD.updater_state_size() == 3 * bD.num_params() and bG.updater_state_size() == 2 * bG.num_params()
     gan.close(); bG.close(); bD.close()
 
 
 def _bf16_dcgan(b, ctx, n, gkinds, dkinds, size=32):
-    m = _m()
     z, nf = 16, 64
     gs, ds = m.dcgan_generator(size, z, nf, 3), m.dcgan_discriminator(size, nf, 3)
     for specs, kinds in ((gs, gkinds), (ds, dkinds)):
@@ -263,22 +185,6 @@ def test_bf16_graph_replay_matches_eager(b200):
     assert np.abs(runs[0][1]).max() > 0 and runs[0][5] == 5
 
 
-def _check_weight_operands(net, specs, what):
-    """Every bf16 weight copy equals the bf16-rounded master weight; returns how many packed pixel-shuffle operands were checked."""
-    packed = 0
-    for li, s in enumerate(specs):
-        if s["type"] not in ("conv2d", "deconv2d", "dense", "output"):
-            continue
-        k = s.get("kernel", (1, 1)); size = s["n_in"] * s["n_out"] * k[0] * k[1]
-        w = bf16_round(w_internal(s, net.get_param(s["name"], "W", size)))
-        assert np.array_equal(net.weight_operand(li, 0, size), w), f"{what}: bf16 copy of {s['name']}.W"
-        O, C = (s["n_in"], s["n_out"]) if s["type"] == "deconv2d" else (s["n_out"], s["n_in"])
-        if tuple(k) == (4, 4) and tuple(s.get("stride", ())) == (2, 2) and tuple(s.get("padding", ())) == (1, 1) and C <= 4 and O % 64 == 0:
-            assert np.array_equal(net.weight_operand(li, 1, 144 * O), pack_deconv_ps(w.reshape(O, 4, 4, -1))), f"{what}: packed operand of {s['name']}"
-            packed += 1
-    return packed
-
-
 def test_bf16_weight_copies_track_the_master(b200):
     b, ctx = b200
     for gk, dk in ((GK, DK), (("amsgrad",), ("adadelta", "nesterovs"))):
@@ -287,8 +193,8 @@ def test_bf16_weight_copies_track_the_master(b200):
         g0 = G.params()
         for it in range(3):
             gan.step(*data)
-            assert _check_weight_operands(G, gs, f"G step {it}") == 1      # G's last layer: the packed pixel-shuffle operand
-            _check_weight_operands(D, ds, f"D step {it}")
+            assert check_weight_operands(b, G, gs, f"G step {it}") == 1      # G's last layer: the packed pixel-shuffle operand
+            check_weight_operands(b, D, ds, f"D step {it}")
         assert np.abs(G.params() - g0).max() > 0
         gan.close(); G.close(); D.close()
 
@@ -337,7 +243,7 @@ def test_single_process_parameter_averaging_with_amsgrad_matches_oracle(b200):
         w0.fit(*d[0]); w1.fit(*d[1])
         o.parameter_average([w0, w1], onet); onet.iteration = w0.iteration
         parallel.fit_parameter_averaging(bnet, d, averaging_frequency=10)
-        _compare(onet, bnet, ("averaging", rnd), _bounds(specs))
+        compare_params_and_state(onet, bnet, ("averaging", rnd), TOL, _bounds(specs))
     assert bnet.iteration() == 2
     bnet.close()
 
@@ -345,31 +251,20 @@ def test_single_process_parameter_averaging_with_amsgrad_matches_oracle(b200):
 def test_launch_counts_do_not_change(b200):
     """C2 (bench.py's DCGAN 64x64, bf16, batch 128) launches 83 kernels per step and a C5-shaped MLP-GAN 46, with Adam and with every new kind."""
     b, ctx = b200
-    m = _m()
     rng = np.random.default_rng(1)
 
     def per_step(gs, ds, gin, din, n):
-        G = b.Net(ctx, gs, gin, max_batch=n, precision=b.BF16, xent_clip_eps=0.0, seed=666)
-        D = b.Net(ctx, ds, din, max_batch=2 * n, precision=b.BF16, xent_clip_eps=0.0, bn_groups=2, seed=667)
+        G, D = bf16_gan(b, ctx, gs, ds, gin, din, n)
         gan = b.Gan(G, D, use_cuda_graph=True)
         x = rng.uniform(-1, 1, (n,) + tuple(din))
         gan.upload(x, rng.uniform(-1, 1, (n,) + tuple(gin)), rng.uniform(-1, 1, (n,) + tuple(gin)), np.ones((n, 1)), np.zeros((n, 1)), np.ones((n, 1)))
-        for _ in range(2):
-            gan.step_resident(n)
-        ctx.sync(); l0 = ctx.launch_count()
-        for _ in range(3):
-            gan.step_resident(n)
-        ctx.sync()
-        out = (ctx.launch_count() - l0) / 3
+        out = launches_per_step(ctx, gan, n)
         gan.close(); G.close(); D.close()
         return out
 
-    def kind_of(specs, kind):
-        return specs if kind == "adam" else [dict(s, updater=_upd(kind)) if s.get("updater") else s for s in specs]
-
     for kind in ("adam",) + KINDS:
-        assert per_step(kind_of(m.dcgan_generator(64, 100, 64, 3), kind), kind_of(m.dcgan_discriminator(64, 64, 3), kind), (100,), (3, 64, 64), 128) == 83, kind
-        assert per_step(kind_of(m.mlp_generator(128, 1024, 256), kind), kind_of(m.mlp_discriminator(256, 1024), kind), (128,), (256,), 8192) == 46, kind
+        assert per_step(_with_kind(m.dcgan_generator(64, 100, 64, 3), kind), _with_kind(m.dcgan_discriminator(64, 64, 3), kind), (100,), (3, 64, 64), 128) == 83, kind
+        assert per_step(_with_kind(m.mlp_generator(128, 1024, 256), kind), _with_kind(m.mlp_discriminator(256, 1024), kind), (128,), (256,), 8192) == 46, kind
 
 
 def test_rejections(b200):
@@ -396,16 +291,6 @@ def test_rejections(b200):
 
 
 def test_two_ranks_average_every_state_slot(tmp_path):
-    try:
-        import torch
-        gpus = torch.cuda.device_count()
-    except Exception:
-        gpus = 0
-    if gpus < 2:
-        pytest.skip("needs two GPUs")
-    out = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1", "--master-port", "29551",
-                          os.path.join(ROOT, "tools", "updater_dp_check.py"), str(tmp_path / "updater_dp.json")], capture_output=True, text=True, timeout=600, cwd=ROOT)
-    assert out.returncode == 0, out.stdout[-800:] + out.stderr[-1500:]
-    d = json.load(open(tmp_path / "updater_dp.json"))
+    d = run_two_ranks("updater_dp_check.py", tmp_path / "updater_dp.json", 29551)
     assert d["world"] == 2 and d["state_slots"] == 3 and d["ranks_differed"] is True
     assert d["max_rel_err_params"] < 1e-6 and max(d["max_rel_err_slot"]) < 1e-6
