@@ -44,6 +44,11 @@ class LrSchedule(C.Structure):
                 ("map_values", C.POINTER(C.c_double))]
 
 
+class Constraint(C.Structure):
+    """b2g_constraint: one DL4J LayerConstraint on one parameter tensor (kind, DL4J dimensions as a bit mask, bounds, MinMaxNorm's rate)."""
+    _fields_ = [("kind", C.c_int32), ("dims_mask", C.c_int32), ("max_norm", C.c_double), ("min_norm", C.c_double), ("rate", C.c_double)]
+
+
 class ConvGeom(C.Structure):
     _fields_ = [(k, C.c_int32) for k in ("n", "h", "w", "c", "oh", "ow", "o", "kh", "kw", "sh", "sw", "ph", "pw")]
 
@@ -119,6 +124,8 @@ PROTOTYPES = {
     "b2g_net_set_dropout_pass": (_i32, [_vp, _i64]),
     "b2g_net_set_gradient_normalization": (_i32, [_vp, _i32, C.c_float]),
     "b2g_net_set_lr_schedule": (_i32, [_vp, C.c_char_p, C.POINTER(LrSchedule)]),
+    "b2g_net_set_constraints": (_i32, [_vp, C.c_char_p, C.c_char_p, C.POINTER(Constraint), _i32]),
+    "b2g_net_apply_constraints": (_i32, [_vp]),
     "b2g_net_get_learning_rate": (_i32, [_vp, C.c_char_p, _fp]),
     "b2g_net_get_epoch": (_i32, [_vp, C.POINTER(_i64)]),
     "b2g_net_set_epoch": (_i32, [_vp, _i64]),

@@ -156,6 +156,13 @@ struct b2g_net {
   std::vector<LayerSched> layer_sched; std::vector<int> seg_layer;
   UpdSched* sched_dev = nullptr; bool sched_on = false; void* sched_map = nullptr; size_t sched_map_bytes = 0;
   int64_t* epoch_dev = nullptr; float* lr_out = nullptr;
+  // Weight constraints (b2g_net_set_constraints): each constrained tensor's layer, parameter and list; the plan, rebuilt by every set: round r
+  // is the r-th constraint of every tensor, its one-pass / element-wise jobs [j0, j1) in one launch and its two-pass jobs [t0, t1) in a norm
+  // and a scale launch; the jobs' device table, the two-pass partials and multipliers (cudaMalloc'd per plan) and the norm kernel's ticket
+  struct ConTensor { int layer; char param[8]; std::vector<b2g_constraint> list; };
+  struct ConRound { int j0, j1, onepass_blocks, t0, t1, norm_blocks, scale_blocks; };
+  std::vector<ConTensor> con; std::vector<ConRound> con_rounds;
+  ConJob* con_jobs = nullptr; double* con_partial = nullptr; float* con_mult = nullptr; unsigned* con_ticket = nullptr;
   ReduceList pending{};                                           // split-K partial sums queued by this backward pass
   uint64_t simt_gemm_calls = 0;                                    // BF16 nets: GEMM-shaped ops that ran on the SIMT kernels (skinny / unsupported shapes) -- reported, never silent
   float* scratch = nullptr; size_t scratch_floats = 0;
@@ -926,6 +933,13 @@ static int32_t net_allreduce_grads(b2g_net* n) {
   NC(g_nccl.ar(n->grads, n->grads, (size_t)n->n_params, /*ncclFloat32*/ 7, /*ncclSum*/ 0, c->comm, c->stream));
   return 0;
 }
+// The constraint rounds of the net's plan, in order; a net without constraints launches nothing
+static void net_launch_constraints(b2g_net* n, cudaStream_t s) {
+  for (const auto& r : n->con_rounds) {
+    k_constraint_onepass(n->params, n->shadow, n->con_jobs, r.j0, r.j1, r.onepass_blocks, s);
+    k_constraint_twopass(n->params, n->shadow, n->con_jobs, r.t0, r.t1, r.norm_blocks, r.scale_blocks, n->con_partial, n->con_ticket, n->con_mult, s);
+  }
+}
 static int32_t net_update(b2g_net* n, int mb_local) {
   cudaStream_t s = n->ctx->stream; int W = n->ctx->comm ? n->ctx->world : 1;
   // BN running-stat pseudo-gradients are exempt from the minibatch division; under DP they are averaged over ranks
@@ -943,6 +957,7 @@ static int32_t net_update(b2g_net* n, int mb_local) {
   // packed) and the iteration counter
   k_updater(n->params, n->grads, n->st0, n->st1, n->st2, n->segs_dev, n->chunk_seg_dev, n->chunk_off_dev, n->nchunks, inv_mb, inv_world, n->step_dev, n->upd_ticket,
             n->shadow, gn ? n->gn_mult : nullptr, n->sched_on ? n->sched_dev : nullptr, n->epoch_dev, n->upd_ext, s);
+  net_launch_constraints(n, s);      // applyConstraints after the step (StochasticGradientDescent.optimize)
   CHECK_KERNELS();
   return 0;
 }
@@ -1019,6 +1034,7 @@ extern "C" int32_t b2g_net_destroy(b2g_net* n) {
   for (auto e : n->ev_fork) if (e) cudaEventDestroy(e); for (auto e : n->ev_done) if (e) cudaEventDestroy(e); if (n->ev_join) cudaEventDestroy(n->ev_join);
   if (n->p2p) for (int r = 0; r < n->ctx->world; ++r) if (r != n->ctx->rank && n->p2p_peer_grads[r]) cudaIpcCloseMemHandle(n->p2p_peer_grads[r]);
   if (n->sched_map) cudaFree(n->sched_map);
+  cudaFree(n->con_jobs); cudaFree(n->con_partial); cudaFree(n->con_mult);
   for (void* p : n->allocs) cudaFree(p); delete n; return 0;
 }
 extern "C" int32_t b2g_net_num_params(b2g_net* n, int64_t* out) { if (!n || !out) return fail(B2G_ERR_ARG, "null"); *out = n->n_params; return 0; }
@@ -1432,6 +1448,120 @@ extern "C" int32_t b2g_net_set_gradient_normalization(b2g_net* n, int32_t mode, 
   if (!clip) threshold = 1.0f;      // the renormalize modes ignore it
   if (mode != n->gn_mode || threshold != n->gn_threshold) { n->gn_mode = mode; n->gn_threshold = threshold; ++n->settings_gen; }
   return 0;
+}
+
+// ------------------------------------------------------------------ weight constraints --------------------
+// A parameter's internal axes [A][kH][kW][B] and where its DL4J dimensions land on them (b2g_constraint): conv W [nOut, nIn, kH, kW] and deconv
+// W [nIn, nOut, kH, kW] are [A][taps][B] with dims (0, 1, 2, 3) -> (A, B, kH, kW); dense / output W [nIn, nOut] is [nOut][nIn] = [A][B] with
+// dims (0, 1) -> (B, A); a [1, n] vector is [1][n] with dims (0, 1) -> (A, B).
+struct ConAxes { int ax[4]; int map[4]; int rank; };
+static ConAxes con_axes(const b2g_net* n, const ParamRef& r, const char* param) {
+  const LayerRT& l = n->L[r.layer];
+  ConAxes c{};
+  if (!strcmp(param, "W") && (l.d.type == B2G_LAYER_CONV2D || l.d.type == B2G_LAYER_DECONV2D)) c = ConAxes{{l.wA, l.d.k_h, l.d.k_w, l.wB}, {0, 3, 1, 2}, 4};
+  else if (!strcmp(param, "W")) c = ConAxes{{l.wA, 1, 1, l.wB}, {3, 0, 0, 0}, 2};
+  else c = ConAxes{{1, 1, 1, (int)r.len}, {0, 3, 0, 0}, 2};
+  return c;
+}
+// Rebuilds the job plan from n->con (include/b200gan.h for the rules, kernels.h ConJob for the paths).  Frozen layers' tensors are skipped.
+static int32_t net_build_constraints(b2g_net* n) {
+  cudaStream_t s = n->ctx->stream;
+  CU(cudaStreamSynchronize(s));                  // nothing in flight reads the old plan
+  cudaFree(n->con_jobs); cudaFree(n->con_partial); cudaFree(n->con_mult);
+  n->con_jobs = nullptr; n->con_partial = nullptr; n->con_mult = nullptr; n->con_rounds.clear();
+  std::vector<ConJob> jobs; int64_t parts = 0, mults = 0;
+  for (int round = 0; round < 4; ++round) {
+    std::vector<ConJob> one, two;
+    for (const auto& t : n->con) {
+      if ((int)t.list.size() <= round || n->L[t.layer].d.frozen) continue;     // FrozenLayer: no update, no constraint
+      const b2g_constraint& k = t.list[round];
+      const LayerRT& l = n->L[t.layer];
+      ParamRef r; B2(find_param(n, l.d.name, t.param, &r));
+      const ConAxes a = con_axes(n, r, t.param);
+      bool red[4] = {false, false, false, false};
+      for (int d = 0; d < a.rank; ++d) if (!k.dims_mask || (k.dims_mask >> d) & 1) red[a.map[d]] = true;
+      // [K0][R0][K1][R1][K2]: the runs of kept / reduced axes (size-1 axes dropped); a kept innermost run after a reduced one is K2 (strided
+      // groups, lane per group), the other runs fill K0, R0, K1, R1 in order
+      int run_f[4], run_n[4], nr = 0;
+      for (int x = 0; x < 4; ++x) {
+        if (a.ax[x] == 1) continue;
+        const int f = red[x] ? 1 : 0;
+        if (nr && run_f[nr - 1] == f) run_n[nr - 1] *= a.ax[x];
+        else { run_f[nr] = f; run_n[nr] = a.ax[x]; ++nr; }
+      }
+      int slot[5] = {1, 1, 1, 1, 1};
+      if (nr >= 2 && run_f[nr - 1] == 0) slot[4] = run_n[--nr];
+      for (int i = 0, si = -1; i < nr; ++i) { si = si < 0 ? run_f[i] : si + 1; slot[si] = run_n[i]; }
+      ConJob j{};
+      const bool w = !strcmp(t.param, "W");
+      j.sg.off = r.off; j.sg.len = r.len; j.sg.off_bf = (w && l.off_W_bf >= 0) ? l.off_W_bf : -1; j.sg.off_ps = (w && l.off_Wps_bf >= 0) ? l.off_Wps_bf : -1;
+      j.sg.ps_O = l.geom.O; j.sg.ps_C = l.geom.C;
+      j.kind = k.kind; j.max_norm = k.max_norm; j.min_norm = k.min_norm; j.rate = k.kind == B2G_CONSTRAINT_MIN_MAX_NORM ? k.rate : 1.0;
+      j.K0 = slot[0]; j.R0 = slot[1]; j.K1 = slot[2]; j.R1 = slot[3]; j.K2 = slot[4]; j.groups = j.K0 * j.K1 * j.K2; j.R = j.R0 * j.R1;
+      j.chunks = 1;
+      if (k.kind == B2G_CONSTRAINT_NON_NEGATIVE) { j.path = CON_ELEMWISE; j.blocks = (int)((r.len + CON_CHUNK - 1) / CON_CHUNK); one.push_back(j); }
+      else if (j.K2 == 1 && j.R <= CON_CHUNK) { j.path = CON_ONEPASS; j.blocks = j.groups; one.push_back(j); }
+      else {
+        j.path = CON_TWOPASS;
+        if (j.K2 == 1) { j.chunks = (j.R + CON_CHUNK - 1) / CON_CHUNK; j.blocks = j.groups * j.chunks; }
+        else { j.chunks = (j.R + CON_SCHUNK - 1) / CON_SCHUNK; j.blocks = j.K0 * j.K1 * ((j.K2 + 31) / 32) * j.chunks; }
+        j.blocks2 = (int)((r.len + CON_CHUNK - 1) / CON_CHUNK);
+        j.part_begin = parts; parts += (int64_t)j.groups * j.chunks; j.mult_begin = mults; mults += j.groups;
+        two.push_back(j);
+      }
+    }
+    if (one.empty() && two.empty()) break;
+    b2g_net::ConRound rd{};
+    rd.j0 = (int)jobs.size();
+    for (auto& j : one) { j.blk_begin = rd.onepass_blocks; rd.onepass_blocks += j.blocks; jobs.push_back(j); }
+    rd.j1 = rd.t0 = (int)jobs.size();
+    for (auto& j : two) { j.blk_begin = rd.norm_blocks; rd.norm_blocks += j.blocks; j.blk2_begin = rd.scale_blocks; rd.scale_blocks += j.blocks2; jobs.push_back(j); }
+    rd.t1 = (int)jobs.size();
+    n->con_rounds.push_back(rd);
+  }
+  if (!jobs.empty()) {
+    CU(cudaMalloc(&n->con_jobs, sizeof(ConJob) * jobs.size()));
+    CU(cudaMalloc(&n->con_partial, sizeof(double) * std::max<int64_t>(1, parts))); CU(cudaMalloc(&n->con_mult, sizeof(float) * std::max<int64_t>(1, mults)));
+    if (!n->con_ticket) { B2(dalloc(n, &n->con_ticket, sizeof(unsigned))); CU(cudaMemsetAsync(n->con_ticket, 0, sizeof(unsigned), s)); }
+    CU(cudaMemcpyAsync(n->con_jobs, jobs.data(), sizeof(ConJob) * jobs.size(), cudaMemcpyHostToDevice, s));
+    CU(cudaStreamSynchronize(s));
+  }
+  ++n->settings_gen;
+  return 0;
+}
+extern "C" int32_t b2g_net_set_constraints(b2g_net* n, const char* layer, const char* param, const b2g_constraint* list, int32_t cnt) {
+  if (!n || !layer || !param || cnt < 0 || (cnt > 0 && !list)) return fail(B2G_ERR_ARG, "b2g_net_set_constraints: null argument or negative count");
+  if (cnt > 4) return fail(B2G_ERR_ARG, "%s.%s: %d constraints, at most 4 per tensor", layer, param, cnt);
+  CU(cudaSetDevice(n->ctx->device));
+  ParamRef r; B2(find_param(n, layer, param, &r));
+  const ConAxes a = con_axes(n, r, param);
+  for (int i = 0; i < cnt; ++i) {
+    const b2g_constraint& k = list[i];
+    if (k.kind < B2G_CONSTRAINT_MAX_NORM || k.kind > B2G_CONSTRAINT_NON_NEGATIVE) return fail(B2G_ERR_ARG, "%s.%s: unknown constraint kind %d", layer, param, k.kind);
+    if (k.dims_mask < 0 || (k.dims_mask >> a.rank) != 0) return fail(B2G_ERR_ARG, "%s.%s: dims mask 0x%x outside the parameter's %d dimensions", layer, param, k.dims_mask, a.rank);
+    const bool maxk = k.kind == B2G_CONSTRAINT_MAX_NORM || k.kind == B2G_CONSTRAINT_MIN_MAX_NORM, mink = k.kind == B2G_CONSTRAINT_MIN_MAX_NORM;
+    if (maxk && !(std::isfinite(k.max_norm) && k.max_norm >= 0.0)) return fail(B2G_ERR_ARG, "%s.%s: max norm %g is not finite and >= 0", layer, param, k.max_norm);
+    if (mink && !(std::isfinite(k.min_norm) && k.min_norm >= 0.0)) return fail(B2G_ERR_ARG, "%s.%s: min norm %g is not finite and >= 0", layer, param, k.min_norm);
+    if (mink && k.min_norm > k.max_norm) return fail(B2G_ERR_ARG, "%s.%s: min norm %g > max norm %g", layer, param, k.min_norm, k.max_norm);
+    if (mink && !(k.rate >= 0.0 && k.rate <= 1.0)) return fail(B2G_ERR_ARG, "%s.%s: rate %g outside [0, 1]", layer, param, k.rate);
+  }
+  size_t at = 0;
+  while (at < n->con.size() && !(n->con[at].layer == r.layer && !strcmp(n->con[at].param, param))) ++at;
+  if (at == n->con.size()) {
+    if (!cnt) return 0;
+    b2g_net::ConTensor t{}; t.layer = r.layer; snprintf(t.param, sizeof(t.param), "%s", param);
+    n->con.push_back(t);
+    std::sort(n->con.begin(), n->con.end(), [&](const b2g_net::ConTensor& x, const b2g_net::ConTensor& y) {
+      ParamRef px, py; find_param(n, n->L[x.layer].d.name, x.param, &px); find_param(n, n->L[y.layer].d.name, y.param, &py); return px.off < py.off; });
+    at = 0; while (!(n->con[at].layer == r.layer && !strcmp(n->con[at].param, param))) ++at;
+  }
+  if (cnt) n->con[at].list.assign(list, list + cnt); else n->con.erase(n->con.begin() + at);
+  return net_build_constraints(n);
+}
+extern "C" int32_t b2g_net_apply_constraints(b2g_net* n) {
+  if (!n) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
+  net_launch_constraints(n, n->ctx->stream); CHECK_KERNELS();
+  CU(cudaStreamSynchronize(n->ctx->stream)); return 0;
 }
 
 // ------------------------------------------------------------------ learning-rate schedules ---------------

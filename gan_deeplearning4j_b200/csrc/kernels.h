@@ -188,6 +188,16 @@ struct UpdSeg {            // one parameter tensor
   int64_t off_bf, off_ps;
   int ps_O, ps_C;
 };
+// Writes the bf16 value pb of parameter element i (an index into the flattened vector, inside sg) to its slot(s) of the bf16 weight operands:
+// the straight copy, and the packed pixel-shuffle operand where sg has one.  Shared by the updater and the weight constraints.
+__device__ __forceinline__ void upd_shadow(const UpdSeg& sg, __nv_bfloat16* __restrict__ shadow, int64_t i, __nv_bfloat16 pb) {
+  shadow[sg.off_bf + (i - sg.off)] = pb;
+  if (sg.off_ps >= 0) {       // [O][4][4][C] element -> its one slot of the packed [(py,px,c4)][(dyr,dxc)][O] pixel-shuffle operand (kernels_tc.cu pack_deconv_ps_kernel)
+    const int e = (int)(i - sg.off), c = e % sg.ps_C, tap = (e / sg.ps_C) % 16, o = e / (sg.ps_C * 16), r = tap >> 2, sx = tap & 3;
+    const int py = (r == 0 || r == 2) ? 1 : 0, dyr = r == 3 ? -1 : r == 0 ? 1 : 0, px = (sx == 0 || sx == 2) ? 1 : 0, dxc = sx == 3 ? -1 : sx == 0 ? 1 : 0;
+    shadow[sg.off_ps + ((int64_t)((py * 8 + px * 4 + c) * 9 + (dyr + 1) * 3 + (dxc + 1))) * sg.ps_O + o] = pb;
+  }
+}
 // Learning-rate schedule of one segment (b2g_lr_schedule; kind 0 = the segment's constant lr).  keys / vals: the MAP schedule's entries in
 // the net's device memory.  Kept beside UpdSeg, not in it, so that the unscheduled updater reads the segment table it always read.
 struct UpdSched {
@@ -221,6 +231,32 @@ struct GnGroup { int32_t chunk_begin, chunk_end, seg_begin, seg_end; };
 void k_gradnorm(const float* grads, const UpdSeg* segs_dev, const int32_t* chunk_seg_dev, const int64_t* chunk_off_dev, int nchunks,
                 const GnGroup* groups_dev, int ngroups, int clip, float threshold, float inv_mb, float inv_world, double* partial, unsigned* ticket,
                 float* mult, cudaStream_t s);
+// ---- weight constraints (DL4J LayerConstraint: MaxNorm, MinMaxNorm, UnitNorm, NonNegative; kernels_constraint.cu) ----------------------
+// One job = one constraint on one parameter tensor.  The tensor (internal layout, an UpdSeg for its place and bf16 operands; off_bf < 0: none)
+// is viewed as [K0][R0][K1][R1][K2]: a group is one (k0, k1, k2), its elements (r0, r1) in that order, j = r0*R1 + r1 < R.  K2 > 1 exactly
+// when the tensor's innermost axis is kept (the groups are strided: a deconv W per output unit, a conv W over {0}, a dense W over {1}).
+//   CON_ONEPASS  (K2 == 1, R <= CON_CHUNK): one block per group; reads the group once into registers, scales, writes.
+//   CON_TWOPASS  the rest: a norm launch of per-chunk double partials whose last block folds them into one multiplier per group, then a scale
+//                launch over the tensor.  K2 == 1: one block per (group, chunk of CON_CHUNK j's);  K2 > 1: one block per (k0, k1, tile of 32
+//                k2, chunk of CON_SCHUNK j's), lane l of each warp reading group k2 = 32 tile + l (consecutive addresses).
+//   CON_ELEMWISE NonNegative: one block per CON_CHUNK elements.
+// blk_begin / blocks: the job's blocks in its one-pass or norm launch; blk2_begin / blocks2: in its scale launch; partials at
+// partial[part_begin + g*chunks + c], multipliers at mult[mult_begin + g].
+enum { CON_ONEPASS = 0, CON_TWOPASS = 1, CON_ELEMWISE = 2 };
+static const int CON_CHUNK = 4096, CON_SCHUNK = 256;
+struct ConJob {
+  UpdSeg sg;
+  int kind, path;           // b2g_constraint_kind, CON_*
+  double max_norm, min_norm, rate;
+  int K0, R0, K1, R1, K2, groups, R;
+  int blk_begin, blocks, blk2_begin, blocks2, chunks;
+  int64_t part_begin, mult_begin;
+};
+// jobs[j0, j1) of one round, all of them of CON_ONEPASS / CON_ELEMWISE paths, in ONE launch of `blocks` blocks
+void k_constraint_onepass(float* params, __nv_bfloat16* shadow, const ConJob* jobs, int j0, int j1, int blocks, cudaStream_t s);
+// jobs[j0, j1) of one round, all CON_TWOPASS: the norm launch (norm_blocks) then the scale launch (scale_blocks)
+void k_constraint_twopass(float* params, __nv_bfloat16* shadow, const ConJob* jobs, int j0, int j1, int norm_blocks, int scale_blocks, double* partial,
+                          unsigned* ticket, float* mult, cudaStream_t s);
 void k_fill_f32(float* p, float v, size_t n, cudaStream_t s);
 void k_scale_f32(float* p, float v, size_t n, cudaStream_t s);
 // Gradient all-reduce over NVLink peer memory (one process per GPU, buffers exchanged as CUDA IPC handles): ONE kernel per GPU does

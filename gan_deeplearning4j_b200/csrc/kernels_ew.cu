@@ -977,14 +977,6 @@ __device__ __forceinline__ float upd_elem(const UpdSeg& sg, float g, float p, fl
   if (sg.l2 != 0.f) u = fmaf(sg.l2, p, u);
   return p - u;
 }
-__device__ __forceinline__ void upd_shadow(const UpdSeg& sg, __nv_bfloat16* __restrict__ shadow, int64_t i, __nv_bfloat16 pb) {
-  shadow[sg.off_bf + (i - sg.off)] = pb;
-  if (sg.off_ps >= 0) {       // [O][4][4][C] element -> its one slot of the packed [(py,px,c4)][(dyr,dxc)][O] pixel-shuffle operand (kernels_tc.cu pack_deconv_ps_kernel)
-    const int e = (int)(i - sg.off), c = e % sg.ps_C, tap = (e / sg.ps_C) % 16, o = e / (sg.ps_C * 16), r = tap >> 2, sx = tap & 3;
-    const int py = (r == 0 || r == 2) ? 1 : 0, dyr = r == 3 ? -1 : r == 0 ? 1 : 0, px = (sx == 0 || sx == 2) ? 1 : 0, dxc = sx == 3 ? -1 : sx == 0 ? 1 : 0;
-    shadow[sg.off_ps + ((int64_t)((py * 8 + px * 4 + c) * 9 + (dyr + 1) * 3 + (dxc + 1))) * sg.ps_O + o] = pb;
-  }
-}
 // The learning rate of a segment at iteration `it` (the counter before this update's increment) / epoch `ep`: DL4J's ISchedule.valueAt in
 // double, rounded to fp32 once (include/b200gan.h, b2g_lr_schedule); kind 0 = the constant lr.
 __device__ float sched_lr(const UpdSched& sc, float lr, int it, long long ep) {

@@ -116,6 +116,53 @@ def follow_lr_schedule(specs: List[Dict], constant: List[float], schedule: Optio
             break
 
 
+# org.deeplearning4j.nn.conf.constraint.* -> b2g_constraint_kind (models.py builds the dicts: max_norm, min_max_norm, unit_norm, non_negative)
+CONSTRAINT_KINDS = {"max_norm": 0, "min_max_norm": 1, "unit_norm": 2, "non_negative": 3}
+CONSTRAINT_ON = ("all", "weights", "bias")      # also the order a layer's lists apply in: constrainAllParameters, Weights, Bias
+GEMM_TYPES = ("conv2d", "deconv2d", "dense", "output")
+
+
+def constraint_params(spec: Dict, on: str) -> List[str]:
+    """The parameters a constraint with target `on` applies to on a layer of this spec (DL4J initializeConstraints): "weights" is W of a
+    conv2d / deconv2d / dense / output layer (nothing on BatchNorm, whose weight keys are empty); "bias" is b where the layer has one; "all"
+    is every parameter, BatchNorm's gamma, beta, mean and var included.  Layers without parameters and FrozenLayers get nothing."""
+    if on not in CONSTRAINT_ON:
+        raise ValueError(f"constraint target {on!r}; one of {list(CONSTRAINT_ON)}")
+    t, bias = spec["type"], spec.get("has_bias", True)
+    if spec.get("frozen", False):
+        return []
+    if t in GEMM_TYPES:
+        return {"weights": ["W"], "bias": ["b"] if bias else [], "all": (["b", "W"] if bias else ["W"])}[on]
+    if t == "batchnorm":
+        return ["gamma", "beta", "mean", "var"] if on == "all" else []
+    return []
+
+
+def constraint_struct(c: Dict):
+    """A constraint dict (models.py) -> b2g_constraint."""
+    if c.get("constraint") not in CONSTRAINT_KINDS:
+        raise ValueError(f"unknown constraint {c.get('constraint')!r}; one of {sorted(CONSTRAINT_KINDS)}")
+    s = _lib.Constraint()
+    s.kind = CONSTRAINT_KINDS[c["constraint"]]
+    s.dims_mask = sum(1 << int(d) for d in set(c.get("dims", ())))
+    s.max_norm, s.min_norm, s.rate = c.get("max", 0.0), c.get("min", 0.0), c.get("rate", 1.0)
+    return s
+
+
+def resolve_constraints(spec: Dict) -> Dict[str, List[Dict]]:
+    """A layer spec's "constraints" as parameter name -> the ordered list each tensor runs: all-parameter constraints, then weight, then bias
+    constraints, each in the order given."""
+    out: Dict[str, List[Dict]] = {}
+    for c in spec.get("constraints", ()):
+        constraint_params(spec, c.get("on", "weights"))          # rejects an unknown target
+    for on in CONSTRAINT_ON:
+        for c in spec.get("constraints", ()):
+            if c.get("on", "weights") == on:
+                for p in constraint_params(spec, on):
+                    out.setdefault(p, []).append(c)
+    return out
+
+
 def _fp(a: np.ndarray):
     return a.ctypes.data_as(C.POINTER(C.c_float))
 
@@ -263,8 +310,16 @@ class Net:
 
     def __init__(self, ctx: Context, specs: Sequence[Dict], input_shape, max_batch: int, precision: int = FP32,
                  grad_clip: float = 0.0, xent_clip_eps: float = 1e-5, bn_groups: int = 1, seed: int = 666,
-                 gradient_normalization: str = "none", gradient_normalization_threshold: float = 1.0):
+                 gradient_normalization: str = "none", gradient_normalization_threshold: float = 1.0,
+                 constraints: Optional[Sequence[Dict]] = None):
+        """constraints: the global builder's constraints (models.max_norm, ...), for every layer whose own "constraints" reach none of its
+        parameters (none given, or e.g. only bias constraints on a BatchNorm), as DL4J's builder fills them in; the specs the net keeps (and a
+        checkpoint saves) carry them per layer."""
         self.ctx, self.lib, self.specs = ctx, ctx.lib, copy.deepcopy(list(specs))
+        if constraints:
+            for sp in self.specs:
+                if sp["type"] in GEMM_TYPES + ("batchnorm",) and not resolve_constraints(sp):
+                    sp["constraints"] = copy.deepcopy(list(constraints))
         # each layer's b2g_layer_desc.lr: what the engine uses again when a schedule is cleared
         self.lr_constants = [constant_lr((sp.get("updater") or {}).get("lr", 0.0)) for sp in self.specs]
         c, h, w = input_shape if len(input_shape) == 3 else (input_shape[0], 1, 1)
@@ -287,6 +342,9 @@ class Net:
                 lr = (sp.get("updater") or {}).get("lr", 0.0)
                 if is_schedule(lr) and layer_has_lr(sp):
                     self.set_lr_schedule(lr, sp["name"])
+            for sp in self.specs:
+                if sp.get("constraints"):
+                    self._push_constraints(sp, {})
         except Exception:
             self.close()
             raise
@@ -389,6 +447,34 @@ class Net:
         s, _arrays = schedule_struct(schedule)       # _arrays: the MAP entries s points into, alive for the call
         check(self.lib.b2g_net_set_lr_schedule(self.h, None if layer is None else layer.encode(), C.byref(s)))
         follow_lr_schedule(self.specs, self.lr_constants, schedule, layer)
+
+    def _push_constraints(self, spec: Dict, before: Dict[str, List[Dict]]):
+        now = resolve_constraints(spec)
+        for p in sorted(set(now) | set(before)):
+            lst = now.get(p, [])
+            arr = (_lib.Constraint * max(1, len(lst)))(*[constraint_struct(c) for c in lst])
+            check(self.lib.b2g_net_set_constraints(self.h, spec["name"].encode(), p.encode(), arr, len(lst)))
+
+    def set_constraints(self, constraints: Optional[Sequence[Dict]], layer: Optional[str] = None):
+        """Replaces the "constraints" of one layer's spec (layer None: of every layer with parameters), as Layer.Builder.constrainWeights /
+        constrainBias / constrainAllParameters would have set them; None or [] removes them.  Applied from the next update on (a captured GAN
+        step is re-captured); the specs a checkpoint writes follow."""
+        for sp in self.specs:
+            if (layer is not None and sp.get("name") != layer) or sp["type"] not in GEMM_TYPES + ("batchnorm",):
+                continue
+            before = resolve_constraints(sp)
+            new = dict(sp, constraints=copy.deepcopy(list(constraints or [])))
+            resolve_constraints(new)                    # validates before anything changes
+            sp["constraints"] = new["constraints"]
+            if not sp["constraints"]:
+                del sp["constraints"]
+            self._push_constraints(sp, before)
+            if layer is not None:
+                break
+
+    def apply_constraints(self):
+        """Model.applyConstraints: every constraint of the net once, now (the updates apply them by themselves)."""
+        check(self.lib.b2g_net_apply_constraints(self.h))
 
     def learning_rate(self, layer: str) -> float:
         """ComputationGraph.getLearningRate(layer): the fp32 learning rate the layer's next update uses (before Adam's bias correction),

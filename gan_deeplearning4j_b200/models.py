@@ -84,6 +84,32 @@ def map_schedule(values, type="iteration"):
     return {"schedule": "map", "type": type, "values": [[k, v] for k, v in pairs]}
 
 
+# ------------------------------------------------------------------ weight constraints -----------------
+# org.deeplearning4j.nn.conf.constraint.*: put them in a layer spec's "constraints" list (Layer.Builder.constrainWeights / constrainBias /
+# constrainAllParameters) or pass them as Net(..., constraints=[...]) (the global builder's: a layer whose own list reaches none of its
+# parameters takes them).  dims are DL4J dimensions of the parameter (conv W [nOut, nIn, kH, kW], deconv W [nIn, nOut, kH, kW], dense W
+# [nIn, nOut], vectors [1, n]); the norm is taken over them once per index of the others, () = over everything.  on: "weights", "bias" or
+# "all".  Arithmetic at b2g_constraint in include/b200gan.h.
+def max_norm(max, dims, on="weights") -> Dict:
+    """new MaxNormConstraint(maxNorm, dimensions...)."""
+    return {"constraint": "max_norm", "max": float(max), "dims": [int(d) for d in dims], "on": on}
+
+
+def min_max_norm(min, max, dims, rate=1.0, on="weights") -> Dict:
+    """new MinMaxNormConstraint(min, max, rate, dimensions...) (rate 1.0: MinMaxNormConstraint(min, max, dimensions...))."""
+    return {"constraint": "min_max_norm", "min": float(min), "max": float(max), "rate": float(rate), "dims": [int(d) for d in dims], "on": on}
+
+
+def unit_norm(dims, on="weights") -> Dict:
+    """new UnitNormConstraint(dimensions...)."""
+    return {"constraint": "unit_norm", "dims": [int(d) for d in dims], "on": on}
+
+
+def non_negative(on="weights") -> Dict:
+    """new NonNegativeConstraint()."""
+    return {"constraint": "non_negative", "on": on}
+
+
 # ------------------------------------------------------------------ pooling layers ---------------------
 # SubsamplingLayer / GlobalPoolingLayer (b2g_pooling in include/b200gan.h).  SubsamplingLayer(MAX) is the "maxpool" spec (unpadded).
 def subsampling(pooling, kernel=(1, 1), stride=(2, 2), padding=(0, 0), pnorm=None, name="") -> Dict:

@@ -348,6 +348,48 @@ typedef enum {
 /* mode in {0, 1, 2, 4, 5}; the clip modes need a finite threshold > 0.  B2G_ERR_ARG for mode 3 (use grad_clip), an unknown mode, a bad
  * threshold, or an L2 mode on a net created with grad_clip > 0 (DL4J allows one mode per layer). */
 int32_t b2g_net_set_gradient_normalization(b2g_net* net, int32_t mode, float threshold);
+/* Weight constraints (DL4J 1.0.0-beta3 org.deeplearning4j.nn.conf.constraint.*, Layer.Builder.constrainWeights / constrainBias /
+ * constrainAllParameters, recalled; parity unpinned like the rest of the DL4J semantics; the Keras constraints of the same names agree).
+ * A constraint acts on one parameter tensor in DL4J's shape: conv W [nOut, nIn, kH, kW], deconv W [nIn, nOut, kH, kW], dense / output W
+ * [nIn, nOut], and b, gamma, beta, mean, var [1, n].  Bit d of dims_mask is dimension d of that shape (conv / deconv W: d < 4, others d < 2).
+ * The L2 norm is taken over the set dimensions once per index of the remaining ones (a group); dims_mask 0 reduces over everything, as
+ * norm2() does.  norm = sqrt of the sum of squares in double over the fp32 values, in an order fixed by the shape (kernels_constraint.cu);
+ * the multiplier m is computed in double, rounded to fp32 once, and each element of the group becomes the fp32 product w * m.  eps = 1e-6
+ * (BaseConstraint.DEFAULT_EPSILON):
+ *   MAX_NORM (0)       m = clip(norm, 0, max_norm) / (norm + eps)     (a group under the bound still shrinks by norm / (norm + eps))
+ *   MIN_MAX_NORM (1)   m = (rate * clip(norm, min_norm, max_norm) + (1 - rate) * norm) / (norm + eps)
+ *   UNIT_NORM (2)      m = 1 / norm; an all-zero group is left as it is (DL4J divides by 0 and gives NaN: a deliberate deviation, as the
+ *                      PNORM floor at b2g_pooling)
+ *   NON_NEGATIVE (3)   w = w < 0 ? +0 : w, element-wise; -0.0 and NaN stay (replaceWhere(.., 0, lessThan(0))); dims_mask is not used
+ * Fields a kind does not use are ignored (rate is read by MIN_MAX_NORM only).
+ * When: after theta -= u of every update the net's updater runs (b2g_net_fit, the D update and the G update of b2g_gan_step, local fits in
+ * parameter-averaging mode) -- DL4J's applyConstraints after the step -- and in b2g_net_apply_constraints (Model.applyConstraints).  Never after
+ * b2g_net_average_parameters, set_param(s) or compute_gradient_and_score.  The G step leaves D untouched, constraints included.  A FrozenLayer
+ * (b2g_layer_desc.frozen) is never constrained; a layer with lr 0 is.  The bf16 weight operands of a BF16 net are rewritten with the fp32
+ * result, so they stay bf16(master).
+ * Order: a tensor's constraints run in list order; the callers put a layer's constrainAllParameters list first, then constrainWeights (W of
+ * CONV2D, DECONV2D, DENSE, OUTPUT; nothing on BATCHNORM), then constrainBias (b where the layer has one), each in the order given.  A layer
+ * whose own lists reach none of its parameters (none given, or only constrainBias on a BatchNorm) takes the global builder's lists, as DL4J's
+ * NeuralNetConfiguration.Builder fills them in.
+ * Launches per update: round r is the r-th constraint of every constrained tensor.  A tensor whose innermost stored axis (conv W: nIn and
+ * deconv W: nOut, both DL4J dimension 1; dense W: nIn, dimension 0; a vector: n, dimension 1) is reduced and whose groups hold at most 4096
+ * elements is one-pass, as is NonNegative; every other tensor (larger groups, or the innermost axis kept:
+ * strided groups such as a deconv W per output unit, dims {0, 2, 3}) takes two launches.  A round launches 1 kernel if it has a one-pass
+ * tensor, plus 2 if it has a two-launch tensor.  A net without constraints launches what it always launched. */
+typedef enum {
+  B2G_CONSTRAINT_MAX_NORM = 0, B2G_CONSTRAINT_MIN_MAX_NORM = 1, B2G_CONSTRAINT_UNIT_NORM = 2, B2G_CONSTRAINT_NON_NEGATIVE = 3
+} b2g_constraint_kind;
+typedef struct {
+  int32_t kind;                   /* b2g_constraint_kind */
+  int32_t dims_mask;              /* bit d = DL4J dimension d of the parameter */
+  double max_norm, min_norm, rate;
+} b2g_constraint;
+/* Replaces the constraint list of one tensor (param in {"W","b","gamma","beta","mean","var"}); n = 0 clears it.  Takes effect at the next update
+ * (a captured GAN step is re-captured).  B2G_ERR_ARG for an unknown kind, layer or parameter, a dims bit outside the parameter's rank, a bound
+ * that is not finite and >= 0, min_norm > max_norm, a rate outside [0, 1], or more than 4 constraints. */
+int32_t b2g_net_set_constraints(b2g_net* net, const char* layer, const char* param, const b2g_constraint* list, int32_t n);
+/* Model.applyConstraints(iteration, epoch): every constraint once, now, as after an update.  Sync point. */
+int32_t b2g_net_apply_constraints(b2g_net* net);
 /* Learning-rate schedules (DL4J 1.0.0-beta3 org.nd4j.linalg.schedule.ISchedule; new Adam(ISchedule), ComputationGraph.setLearningRate(ISchedule)).
  * A layer with a schedule updates with lr_i = (float)value(i) in place of b2g_layer_desc.lr; l2 is unchanged (applied after the updater, not
  * lr-scaled).  value(i) is computed in double and rounded to fp32 once:

@@ -34,6 +34,8 @@ public final class Native {
     public static native int netSetDropoutPass(long net, long pass);
     public static native int netSetGradientNormalization(long net, int mode, float threshold);
     public static native int netSetLrSchedule(long net, long layerNameAddr, long scheduleAddr);   // layerNameAddr 0: every layer; scheduleAddr 0: constant lr
+    public static native int netSetConstraints(long net, long layerNameAddr, long paramNameAddr, long constraintsAddr, int n);   // b2g_constraint[n]
+    public static native int netApplyConstraints(long net);
     public static native int netGetLearningRate(long net, long layerNameAddr, long outAddr);
     public static native int netGetEpoch(long net, long outAddr);
     public static native int netSetEpoch(long net, long epoch);

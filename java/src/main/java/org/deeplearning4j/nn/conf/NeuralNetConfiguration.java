@@ -8,6 +8,7 @@ import java.util.HashMap;
 import java.util.List;
 import java.util.Map;
 import org.deeplearning4j.nn.api.OptimizationAlgorithm;
+import org.deeplearning4j.nn.api.layers.LayerConstraint;
 import org.deeplearning4j.nn.conf.inputs.InputType;
 import org.deeplearning4j.nn.conf.layers.Layer;
 import org.deeplearning4j.nn.conf.preprocessor.FeedForwardToCnnPreProcessor;
@@ -33,6 +34,11 @@ public class NeuralNetConfiguration {
         public Builder l2(double v) { l2 = (float) v; return this; }
         public Builder activation(Activation a) { act = a; return this; }
         public Builder weightInit(WeightInit w) { return this; }
+        /** The global constraints: a layer whose own lists reach none of its parameters takes these. */
+        public List<LayerConstraint> constrainAll, constrainW, constrainB;
+        public Builder constrainAllParameters(LayerConstraint... c) { constrainAll = List.of(c); return this; }
+        public Builder constrainWeights(LayerConstraint... c) { constrainW = List.of(c); return this; }
+        public Builder constrainBias(LayerConstraint... c) { constrainB = List.of(c); return this; }
         public GraphBuilder graphBuilder() { return new GraphBuilder(this); }
     }
 

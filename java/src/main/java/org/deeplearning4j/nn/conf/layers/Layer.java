@@ -2,6 +2,8 @@
 package org.deeplearning4j.nn.conf.layers;
 
 import java.nio.ByteBuffer;
+import java.util.List;
+import org.deeplearning4j.nn.api.layers.LayerConstraint;
 import org.nd4j.linalg.activations.Activation;
 import org.nd4j.linalg.activations.IActivation;
 import org.nd4j.linalg.learning.config.IUpdater;
@@ -11,6 +13,8 @@ public class Layer {
     public int type, nIn, nOut, kH = 1, kW = 1, sH = 1, sW = 1, pH, pW, hasBias = 1, act = -1, preH, preW, preC, loss, frozen;
     public float alpha = 0.01f, l2 = Float.NaN, bnDecay = 0.9f, bnEps = 1e-5f;
     public IUpdater updater; public String name = "";
+    /** constrainAllParameters / constrainWeights / constrainBias; all null: the global builder's lists apply. */
+    public List<LayerConstraint> constrainAll, constrainW, constrainB;
     public boolean alphaSet;   // alpha given by leakyReluAlpha(..) or activation(IActivation); else ELU / ThresholdedReLU write DL4J's 1.0
 
     /** Serialise into the C struct layout (little-endian, no padding: every field is 4-byte aligned). */
@@ -23,7 +27,8 @@ public class Layer {
         b.putFloat(Float.isNaN(l2) ? globalL2 : l2).putFloat(bnDecay).putFloat(bnEps).putInt(preH).putInt(preW).putInt(preC).putInt(loss).putInt(frozen);
     }
     public Layer copy() { Layer c = new Layer(); c.type = type; c.nIn = nIn; c.nOut = nOut; c.kH = kH; c.kW = kW; c.sH = sH; c.sW = sW; c.pH = pH; c.pW = pW; c.hasBias = hasBias; c.act = act;
-        c.preH = preH; c.preW = preW; c.preC = preC; c.loss = loss; c.frozen = frozen; c.alpha = alpha; c.l2 = l2; c.bnDecay = bnDecay; c.bnEps = bnEps; c.updater = updater; c.name = name; c.alphaSet = alphaSet; return c; }
+        c.preH = preH; c.preW = preW; c.preC = preC; c.loss = loss; c.frozen = frozen; c.alpha = alpha; c.l2 = l2; c.bnDecay = bnDecay; c.bnEps = bnEps; c.updater = updater; c.name = name; c.alphaSet = alphaSet;
+        c.constrainAll = constrainAll; c.constrainW = constrainW; c.constrainB = constrainB; return c; }
     protected int defaultAct(Activation g) { return g.code; }   // conv / dense inherit the global .activation(..) (J:126)
 
     @SuppressWarnings("unchecked")
@@ -40,6 +45,9 @@ public class Layer {
         public T activation(IActivation a) { l.act = a.code(); l.alpha = a.alpha(); l.alphaSet = true; return (T) this; }   // ActivationELU(alpha), ActivationThresholdedReLU(theta)
         public T leakyReluAlpha(double a) { l.alpha = (float) a; l.alphaSet = true; return (T) this; }
         public T l2(double v) { l.l2 = (float) v; return (T) this; }
+        public T constrainAllParameters(LayerConstraint... c) { l.constrainAll = List.of(c); return (T) this; }
+        public T constrainWeights(LayerConstraint... c) { l.constrainW = List.of(c); return (T) this; }
+        public T constrainBias(LayerConstraint... c) { l.constrainB = List.of(c); return (T) this; }
         public Layer build() { return l; }
     }
 }

@@ -5,6 +5,7 @@ import java.nio.ByteBuffer;
 import java.nio.FloatBuffer;
 import java.util.List;
 import org.deeplearning4j.b200.Native;
+import org.deeplearning4j.nn.api.layers.LayerConstraint;
 import org.deeplearning4j.nn.conf.GradientNormalization;
 import org.deeplearning4j.nn.conf.NeuralNetConfiguration.ComputationGraphConfiguration;
 import org.deeplearning4j.nn.conf.layers.Layer;
@@ -30,7 +31,49 @@ public class ComputationGraph {
         if (gn.isL2()) Native.check(Native.netSetGradientNormalization(net, gn.ordinal(), conf.b.g.gradNormThreshold));
         for (Layer l : layers)            // new Adam(ISchedule) / RmsProp(ISchedule) / Sgd(ISchedule): evaluated on the device at every update
             if (l.updater != null && l.updater.lrSchedule() != null && hasLearningRate(l)) setLearningRate(l.name, l.updater.lrSchedule());
+        for (Layer l : layers) applyConstraints(l);
     }
+    /** The parameters a constrainAllParameters / constrainWeights / constrainBias list reaches on a layer (the library's rule, include/b200gan.h
+     *  b2g_constraint, and engine.py constraint_params): weights = W of conv, deconv, dense and output layers, nothing on BatchNorm; bias = b
+     *  where the layer has one; all = every parameter, BatchNorm's gamma, beta, mean and var included. */
+    static String[] constrainedParams(Layer l, String on) {
+        boolean gemm = l.type == 0 || l.type == 1 || l.type == 3 || l.type == 7;
+        if (gemm && on.equals("weights")) return new String[] { "W" };
+        if (gemm && on.equals("bias")) return l.hasBias != 0 ? new String[] { "b" } : new String[0];
+        if (gemm && on.equals("all")) return l.hasBias != 0 ? new String[] { "b", "W" } : new String[] { "W" };
+        if (l.type == 2 && on.equals("all")) return new String[] { "gamma", "beta", "mean", "var" };
+        return new String[0];
+    }
+    /** Each tensor's list runs all-parameter, then weight, then bias constraints.  A layer whose own lists reach none of its parameters takes
+     *  the global builder's lists (DL4J's NeuralNetConfiguration.Builder fills them in when the layer's resolved constraints are empty). */
+    private void applyConstraints(Layer l) {
+        java.util.Map<String, List<LayerConstraint>> per = constraintsByParam(l, l.constrainAll, l.constrainW, l.constrainB);
+        if (per.isEmpty()) per = constraintsByParam(l, conf.b.g.constrainAll, conf.b.g.constrainW, conf.b.g.constrainB);
+        for (java.util.Map.Entry<String, List<LayerConstraint>> e : per.entrySet()) {
+            List<LayerConstraint> cs = e.getValue();
+            ByteBuffer b = Native.direct(32 * cs.size());          // b2g_constraint[]: kind, dims_mask, max_norm, min_norm, rate (32 bytes)
+            for (int i = 0; i < cs.size(); ++i) {
+                LayerConstraint c = cs.get(i);
+                b.putInt(32 * i, c.kind()).putInt(32 * i + 4, c.dimsMask()).putDouble(32 * i + 8, c.maxNorm()).putDouble(32 * i + 16, c.minNorm())
+                 .putDouble(32 * i + 24, c.rate());
+            }
+            ByteBuffer name = Native.cstr(l.name), param = Native.cstr(e.getKey());
+            Native.check(Native.netSetConstraints(net, Native.address(name), Native.address(param), Native.address(b), cs.size()));
+            java.lang.ref.Reference.reachabilityFence(b); java.lang.ref.Reference.reachabilityFence(name); java.lang.ref.Reference.reachabilityFence(param);
+        }
+    }
+    private static java.util.Map<String, List<LayerConstraint>> constraintsByParam(Layer l, List<LayerConstraint> all, List<LayerConstraint> w,
+                                                                                   List<LayerConstraint> b) {
+        List<List<LayerConstraint>> lists = java.util.Arrays.asList(all, w, b);
+        String[] on = { "all", "weights", "bias" };
+        java.util.Map<String, List<LayerConstraint>> per = new java.util.LinkedHashMap<>();
+        for (int k = 0; k < 3; ++k)
+            if (lists.get(k) != null)
+                for (String p : constrainedParams(l, on[k])) for (LayerConstraint c : lists.get(k)) per.computeIfAbsent(p, x -> new java.util.ArrayList<>()).add(c);
+        return per;
+    }
+    /** Model.applyConstraints(iteration, epoch): every constraint once, now (fit applies them after each update by itself). */
+    public void applyConstraints(int iteration, int epoch) { Native.check(Native.netApplyConstraints(net)); }
     /** The library's rule (include/b200gan.h, b2g_net_set_lr_schedule): parameters, not frozen, updater neither NoOp nor AdaDelta. */
     private static boolean hasLearningRate(Layer l) {
         boolean params = l.type == 0 || l.type == 1 || l.type == 2 || l.type == 3 || l.type == 7;    // conv, deconv, BatchNorm, dense, output

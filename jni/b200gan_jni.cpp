@@ -51,6 +51,11 @@ FN(netSetGradientNormalization)(JNIEnv_*, jclass, jlong net, jint mode, jfloat t
 FN(netSetLrSchedule)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong scheduleAddr) {
   return b2g_net_set_lr_schedule(P(b2g_net*, net), P(const char*, layerNameAddr), P(const b2g_lr_schedule*, scheduleAddr));
 }
+// constraintsAddr -> b2g_constraint[n] laid out by the facade in a direct ByteBuffer; n = 0 clears the tensor's list
+FN(netSetConstraints)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong paramNameAddr, jlong constraintsAddr, jint n) {
+  return b2g_net_set_constraints(P(b2g_net*, net), P(const char*, layerNameAddr), P(const char*, paramNameAddr), P(const b2g_constraint*, constraintsAddr), n);
+}
+FN(netApplyConstraints)(JNIEnv_*, jclass, jlong net) { return b2g_net_apply_constraints(P(b2g_net*, net)); }
 FN(netGetLearningRate)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong outAddr) {
   return b2g_net_get_learning_rate(P(b2g_net*, net), P(const char*, layerNameAddr), P(float*, outAddr));
 }
