@@ -1,7 +1,7 @@
 // kernels_constraint.cu -- DL4J's weight constraints (LayerConstraint: MaxNormConstraint, MinMaxNormConstraint, UnitNormConstraint,
 // NonNegativeConstraint), applied to the fp32 master parameters after the updater, with the bf16 weight operands (straight and packed
 // pixel-shuffle copies) rewritten through upd_shadow.  Semantics: include/b200gan.h (b2g_constraint); the job plan: kernels.h (ConJob) and
-// engine.cu (net_build_constraints); restatement and exact emulation of this order: tests/constraint_ref.py.
+// engine.cu (net_build_constraints); restatement: oracle/dl4j_oracle.py; exact emulation of this order: tests/ew_ref.py.
 //
 // Summation order of a group's squared norm, in double over (double)w * (double)w (exact), fixed by the shape and not by the grid:
 //   K2 == 1 (the innermost axis reduced): the group's j's are cut into chunks of CON_CHUNK; in a chunk, thread t of 256 sums j = chunk_base + t + 256 q

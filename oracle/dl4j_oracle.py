@@ -39,6 +39,8 @@ include/b200gan.h):
   * learning-rate schedules (ISchedule)            -> ``Net.set_lr_schedule``, ``value``, ``lr_at``
   * CnnLossLayer (B2G_LAYER_CNN_LOSS)              -> ``CnnLossLayer``
   * ElementWiseVertex / MergeVertex (b2g_elementwise_op) -> ``ElementWiseVertex`` / ``MergeVertex``, the skip edges of ``Net``
+  * weight constraints (b2g_constraint)            -> ``constraint_multiplier``, ``apply_constraint``, ``constraints_by_param``,
+                                                      ``Net.set_constraints`` / ``apply_constraints``
 ``net_from_specs`` builds a Net from the layer specs the CUDA engine consumes.
 
 Layouts follow DL4J: activations NCHW, conv W [nOut,nIn,kH,kW] 'c' order flattened as [b | W],
@@ -85,6 +87,9 @@ class Quirks:
     l2norm_zero_floor: float = 1e-5          # Renormalize divides by this instead of a zero norm
     # CnnLossLayer.computeScore: score /= getInputMiniBatchSize() (True); False: the row mean over N*H*W (score and gradient / (H*W) more)
     cnn_loss_score_per_minibatch: bool = True
+    # weight constraints
+    constraint_eps: float = 1e-6                  # BaseConstraint.DEFAULT_EPSILON
+    unit_norm_zero_group_unchanged: bool = True   # UnitNorm leaves an all-zero group as it is (DL4J: 0/0 = NaN)
 
 
 DEFAULT_QUIRKS = Quirks()
@@ -440,6 +445,63 @@ def normalize(net, g, mode, threshold, q: Quirks = DEFAULT_QUIRKS):
         for k in keys:
             out[k] = g[k] * float(m)
     return out, norms
+
+
+# --------------------------------------------------------------------------------------------------
+# Weight constraints (LayerConstraint: MaxNorm, MinMaxNorm, UnitNorm, NonNegative; the dicts of models.max_norm, ...).  They run after
+# theta -= u in every update (``Net.apply_update``), never on a FrozenLayer, and never after averaging, set_params_flat or
+# compute_gradient_and_score.
+# --------------------------------------------------------------------------------------------------
+CONSTRAINT_KINDS = ("max_norm", "min_max_norm", "unit_norm", "non_negative")
+CONSTRAINT_ON = ("all", "weights", "bias")      # also the order a tensor's lists apply in: constrainAllParameters, Weights, Bias
+
+
+def constraint_multiplier(c: Dict, norm, q: Quirks = DEFAULT_QUIRKS):
+    """The fp32 multiplier of a group of L2 norm `norm` (float64 arrays), computed in double and rounded once."""
+    norm = np.asarray(norm, np.float64)
+    eps = q.constraint_eps
+    k = c["constraint"]
+    if k == "max_norm":
+        m = np.minimum(norm, c["max"]) / (norm + eps)
+    elif k == "min_max_norm":
+        rate = c.get("rate", 1.0)
+        m = (rate * np.minimum(np.maximum(norm, c["min"]), c["max"]) + (1.0 - rate) * norm) / (norm + eps)
+    elif k == "unit_norm":
+        with np.errstate(divide="ignore", invalid="ignore"):
+            m = 1.0 / norm
+        if q.unit_norm_zero_group_unchanged:
+            m = np.where(norm == 0.0, 1.0, m)
+    else:
+        raise ValueError(k)
+    return m.astype(np.float32)
+
+
+def apply_constraint(w: np.ndarray, c: Dict, q: Quirks = DEFAULT_QUIRKS) -> np.ndarray:
+    """One constraint on one parameter in its DL4J shape ([n] vectors as [1, n]; float64 or float32)."""
+    dt = w.dtype
+    if c["constraint"] == "non_negative":
+        return np.where(w < 0, np.zeros((), dt), w)
+    if w.ndim == 1:                    # b, gamma, beta, mean, var: DL4J's [1, n]
+        return apply_constraint(w.reshape(1, -1), c, q).reshape(w.shape)
+    dims = tuple(sorted(set(c.get("dims", ())))) or tuple(range(w.ndim))
+    norm = np.sqrt((w.astype(np.float64) ** 2).sum(axis=dims, keepdims=True))
+    return (w * constraint_multiplier(c, norm, q).astype(dt)).astype(dt)
+
+
+def constraints_by_param(layer: Layer, constraints: Sequence[Dict]) -> Dict[str, List[Dict]]:
+    """One layer's constraints as parameter name -> the ordered list its tensor runs (DL4J initializeConstraints): on a layer with parameters
+    that is not frozen, "weights" reaches W, "bias" b and "all" every parameter, where the layer has them; each list runs the all-parameter
+    constraints, then the weight, then the bias ones, each in the order given.  ValueError for an unknown target or kind."""
+    for c in constraints:
+        if c.get("on", "weights") not in CONSTRAINT_ON or c.get("constraint") not in CONSTRAINT_KINDS:
+            raise ValueError(f"constraint {c!r}: targets {CONSTRAINT_ON}, kinds {CONSTRAINT_KINDS}")
+    names = [p for p, _, _ in layer.param_specs()] if layer.has_params and not getattr(layer, "frozen", False) else []
+    reach = {"all": names, "weights": [p for p in names if p == "W"], "bias": [p for p in names if p == "b"]}
+    out: Dict[str, List[Dict]] = {}
+    for c in sorted(constraints, key=lambda c: CONSTRAINT_ON.index(c.get("on", "weights"))):    # stable: the given order within a target
+        for p in reach[c.get("on", "weights")]:
+            out.setdefault(p, []).append(c)
+    return out
 
 
 # --------------------------------------------------------------------------------------------------
@@ -1312,6 +1374,7 @@ class Net:
         self.iteration = self.epoch = 0
         self.gradient_normalization, self.gradient_normalization_threshold, self.grad_norm_last_norms = "none", 1.0, []
         self.schedules: Dict[str, dict] = {}      # layer name -> schedule (None: the constant lr)
+        self.layer_constraints: Dict[str, Dict[str, List[Dict]]] = {}     # layer name -> parameter -> its ordered constraints
         self.dropout = DropoutState(mask_seed, rank)
         self._skip_acc: Dict[int, np.ndarray] = {}    # skip source index -> the skip shares the current backward has met
         rng = np.random.default_rng(seed)
@@ -1361,6 +1424,20 @@ class Net:
 
     def set_epoch(self, epoch: int):
         self.epoch = epoch
+
+    def set_constraints(self, constraints: Optional[Sequence[Dict]], layer: Optional[str] = None):
+        """Replaces the constraints of one layer (layer None: of every layer with parameters), as Layer.Builder.constrainWeights /
+        constrainBias / constrainAllParameters would have set them; None or [] removes them.  Applied from the next update on."""
+        new = {l.name: constraints_by_param(l, list(constraints or ())) for l in self.layers if l.has_params and layer in (None, l.name)}
+        self.layer_constraints = {name: per for name, per in {**self.layer_constraints, **new}.items() if per}      # new: all validated
+
+    def apply_constraints(self):
+        """Model.applyConstraints: each live (not frozen) layer's tensors, each through its list in order."""
+        for l in self.layers:
+            if l.name in self.layer_constraints and not getattr(l, "frozen", False):
+                for p, lst in self.layer_constraints[l.name].items():
+                    for c in lst:
+                        l.params[p] = apply_constraint(l.params[p], c, self.q)
 
     def dropout_pass(self) -> int:
         """The dropout pass counter P: train-mode forwards that applied a DropoutLayer mask."""
@@ -1482,7 +1559,7 @@ class Net:
 
     # ---- updater: BaseMultiLayerUpdater.update + UpdaterBlock + params.subi ----------------------
     def apply_update(self, mb: int, grads: Optional[Dict[Tuple[int, str], np.ndarray]] = None, frozen_from: Optional[int] = None):
-        """g/=mb -> L2 normalization -> clip -> updater at the layer's lr -> +l2*W -> theta -= g.  (SURVEY.md section 8a row a9.)"""
+        """g/=mb -> L2 normalization -> clip -> updater at the layer's lr -> +l2*W -> theta -= g -> constraints.  (SURVEY.md 8a row a9.)"""
         t = self.iteration + 1
         live = [(li, l) for li, l in enumerate(self.layers)
                 if l.has_params and not getattr(l, "frozen", False)]     # FrozenLayer: no gradient, no update, no l2 decay
@@ -1512,6 +1589,8 @@ class Net:
                         raise NotImplementedError("only the pre-beta4 post-updater l2 form is restated")
                 l.params[pname] = (l.params[pname] - upd).astype(self.dtype)
         self.iteration += 1
+        if self.layer_constraints:
+            self.apply_constraints()
 
     def fit(self, x, y):
         """ComputationGraph.fit(DataSet) for one minibatch (Solver -> StochasticGradientDescent.optimize)."""
@@ -1738,12 +1817,14 @@ def synthetic_batch(n, size=64, nc=3, z=100, seed=666, dtype=np.float32):
 # Layer specs (gan_deeplearning4j_b200.models / engine.LAYER_TYPES) -> Net
 # --------------------------------------------------------------------------------------------------
 def net_from_specs(specs, input_shape, *, quirks: Quirks = DEFAULT_QUIRKS, dtype=np.float64, seed=1, grad_clip=0.0, flat_input=True,
-                   mask_seed=666, rank=0) -> Net:
+                   mask_seed=666, rank=0, constraints: Optional[Sequence[Dict]] = None) -> Net:
     """The Net of the layer specs the CUDA engine consumes.  input_shape: (C,H,W) or (F,).  flat_input: prepend the convolutionalFlat
     reshape (the oracle's layer indices are then the specs' + 1).  A spec's scheduled lr becomes the layer's schedule; its constant lr is
     the schedule's value at 0, as the library keeps it.  An activation's alpha defaults as engine.layer_desc fills it.  A DropoutLayer's
-    mask index is its position in `specs` (the library's index).  A vertex's inputs are resolved by vertex_inputs.  mask_seed, rank: see Net."""
-    layers = []
+    mask index is its position in `specs` (the library's index).  A vertex's inputs are resolved by vertex_inputs.  mask_seed, rank: see Net.
+    A spec's "constraints" are its layer's; constraints: the global builder's, for every layer whose own reach none of its parameters, as
+    DL4J's builder fills them in."""
+    layers, by_layer = [], {}
     shape = (1,) + tuple(input_shape)
     if len(input_shape) == 3 and flat_input:
         layers.append(Reshape(tuple(input_shape), name="in_reshape"))      # convolutionalFlat accepts [N,784] or [N,1,28,28]
@@ -1801,12 +1882,16 @@ def net_from_specs(specs, input_shape, *, quirks: Quirks = DEFAULT_QUIRKS, dtype
             raise ValueError(t)
         if s.get("frozen", False):
             l.frozen = True
+        per = constraints_by_param(l, s.get("constraints", ())) or constraints_by_param(l, constraints or ())
+        if per:
+            by_layer[name] = per
         layers.append(l)
         shape = l.out_shape(shape, shapes[l.src]) if isinstance(l, Vertex) else l.out_shape(shape)
         shapes.append(shape)
     net = Net(layers, seed=seed, dtype=dtype, grad_clip=grad_clip, quirks=quirks, mask_seed=mask_seed, rank=rank)
     for name, sched in schedules.items():
         net.set_lr_schedule(sched, name)
+    net.layer_constraints = by_layer
     return net
 
 

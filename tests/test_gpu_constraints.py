@@ -1,6 +1,6 @@
 """DL4J's weight constraints on the device (b2g_net_set_constraints / apply_constraints, kernels_constraint.cu): every kind and dims pattern
-bit for bit against the emulation of the documented summation order (constraint_ref.device_apply), fit and the FP32 GAN step against the
-oracle, the bf16 weight operands after constrained updates, and the launches a constraint adds."""
+bit for bit against the emulation of the documented summation order (ew_ref.device_apply), fit and the FP32 GAN step against the oracle,
+the bf16 weight operands after constrained updates, and the launches a constraint adds."""
 import copy
 
 import numpy as np
@@ -9,7 +9,7 @@ import pytest
 from helpers import (b200, bf16_gan, check_weight_operands, gan_step_parity, launches_per_step, oracle_gan_pair, pclose, push_params, rel_err,  # noqa: F401
                      run_two_ranks)
 from oracle import dl4j_oracle as o
-import constraint_ref as cr
+import ew_ref as er
 from gan_deeplearning4j_b200 import models as m
 
 pytestmark = pytest.mark.gpu
@@ -51,7 +51,7 @@ def _check_apply(b, ctx, specs, shape, cases, rng):
             before = _tensors(specs, shape, p0)
             targets = b.engine.constraint_params(next(s for s in specs if s["name"] == layer), on)
             kind = {p: KIND[layer] if p == "W" else "vector" for p in targets}
-            s, _ = cr.group_sums(kind[targets[0]], before[(layer, targets[0])], dims)
+            s, _ = er.group_sums(kind[targets[0]], before[(layer, targets[0])], dims)
             for c in _kinds(rng, np.sqrt(s)):
                 c = dict(c, dims=list(dims), on=on)
                 net.set_params(p0)
@@ -59,7 +59,7 @@ def _check_apply(b, ctx, specs, shape, cases, rng):
                 net.apply_constraints()
                 got = _tensors(specs, shape, net.params())
                 for k, v in got.items():
-                    want = cr.device_apply(kind[k[1]], before[k], c) if k[0] == layer and k[1] in targets else before[k]   # nothing else moves
+                    want = er.device_apply(kind[k[1]], before[k], c) if k[0] == layer and k[1] in targets else before[k]   # nothing else moves
                     bad = v.view(np.uint32) != want.view(np.uint32)
                     assert not bad.any(), (layer, k, dims, c, int(bad.sum()), bad.size)
                 net.set_constraints(None, layer)
@@ -84,11 +84,11 @@ def _fit_parity(b, ctx, updater):
             sp["updater"] = copy.deepcopy(updater)
     cons = [m.max_norm(0.6, (1, 2, 3)), m.non_negative(on="bias")]
     rng = np.random.default_rng(3)
-    on = o.net_from_specs(specs, (3, 16, 16), seed=2)
+    on = o.net_from_specs(specs, (3, 16, 16), seed=2, constraints=cons)
     from helpers import randomize
     randomize(on, rng)
-    cr.constrain(on, specs, cons)
     bn = b.Net(ctx, specs, (3, 16, 16), max_batch=8, constraints=cons)
+    assert {sp["name"]: r for sp in bn.specs if (r := b.engine.resolve_constraints(sp))} == on.layer_constraints      # the global rule
     push_params(on, bn)
     x = rng.uniform(-1, 1, (8, 3 * 16 * 16)); y = rng.integers(0, 2, (8, 1)).astype(np.float64)
     for it in range(3):
@@ -125,7 +125,6 @@ def test_wasserstein_gan_step_parity_with_max_norm_critic(b200):
     b, ctx = b200
     gs, ds = _wgan_specs([m.max_norm(0.5, (1, 2, 3))], [m.max_norm(0.8, (0, 2, 3))])
     G, D = oracle_gan_pair(gs, ds)
-    cr.constrain(G, gs); cr.constrain(D, ds)
     data = [a.astype(np.float64) for a in o.synthetic_batch(8, 16, 3, 12, seed=3)]
     gan_step_parity(b, ctx, gs, ds, G, D, data[:3] + WGAN_LABELS, WGAN_LABELS, 2e-3, "wgan max-norm")
 
@@ -134,7 +133,6 @@ def test_changing_a_constraint_recaptures_the_graph(b200):
     b, ctx = b200
     gs, ds = _wgan_specs([m.max_norm(0.5, (1, 2, 3))])
     G, D = oracle_gan_pair(gs, ds)
-    cr.constrain(G, gs); cr.constrain(D, ds)
     data = [a.astype(np.float64) for a in o.synthetic_batch(8, 16, 3, 12, seed=3)]
     bG = b.Net(ctx, gs, (12,), max_batch=8); bD = b.Net(ctx, ds, (3, 16, 16), max_batch=16, bn_groups=2)
     push_params(G, bG); push_params(D, bD)
@@ -143,8 +141,7 @@ def test_changing_a_constraint_recaptures_the_graph(b200):
     for it in range(4):
         if it == 2:
             bD.set_constraints(tighter)
-            ds2 = [dict(sp, constraints=tighter) if sp["type"] == "conv2d" else sp for sp in ds]
-            cr.constrain(D, ds2)
+            D.set_constraints(tighter)
         o.gan_step(G, D, *data[:3], *WGAN_LABELS)
         gan.step(*data[:3], *WGAN_LABELS)
         assert pclose(bD.params(), D.params_flat(), 4e-3), (it, rel_err(bD.params(), D.params_flat()))
@@ -174,25 +171,18 @@ def _bf16_run(b, ctx, d_cons, g_cons, steps=3):
     return gs, ds, G, D, gan, n
 
 
-def _expected_launches(specs, cons):
-    """Per update of one net: 1 if some tensor has a NonNegative or a contiguous group of <= 4096, + 2 if some tensor has another group
-    (one constraint per tensor here: one round)."""
-    from gan_deeplearning4j_b200.engine import resolve_constraints
-    one = two = False
-    for sp in specs:
-        for p, lst in resolve_constraints(dict(sp, constraints=cons) if sp["type"] in ("conv2d", "deconv2d", "dense", "output") else sp).items():
-            c = lst[0]
-            if c["constraint"] == "non_negative":
-                one = True
-                continue
-            k = sp.get("kernel", (1, 1))
-            shape = (sp["n_out"], k[0], k[1], sp["n_in"]) if sp["type"] == "conv2d" else (sp["n_in"], k[0], k[1], sp["n_out"])
-            K0, R0, K1, R1, K2 = cr.plan("conv", shape, tuple(c["dims"]))
-            if K2 == 1 and R0 * R1 <= cr.CHUNK:
-                one = True
-            else:
-                two = True
-    return int(one) + 2 * int(two)
+def _expected_launches(specs, input_shape, cons):
+    """Per update of one net given the global constraints cons: 1 if some tensor has a NonNegative or a one-pass group, + 2 if some tensor has
+    a two-launch group (one constraint per tensor here: one round)."""
+    net = o.net_from_specs(specs, input_shape)
+    net.set_constraints(cons)
+    paths = set()
+    for name, per in net.layer_constraints.items():
+        l = net.layer(name)
+        for p, (c,) in per.items():
+            kind = "vector" if p != "W" else "dense" if isinstance(l, o.Dense) else "conv"
+            paths.add("one-pass" if c["constraint"] == "non_negative" else er.constraint_path(kind, l.params[p].shape, c["dims"]))
+    return ("one-pass" in paths) + 2 * ("two-launch" in paths)
 
 
 def test_bf16_operands_follow_the_constrained_master_and_launch_counts(b200):
@@ -203,7 +193,7 @@ def test_bf16_operands_follow_the_constrained_master_and_launch_counts(b200):
     # deconvs, strided groups (two launches; the last deconv's scale pass writes the packed pixel-shuffle operand)
     d_cons, g_cons = [m.max_norm(1.0, ())], [m.max_norm(0.8, (0, 2, 3))]
     gs, ds, G0, D0, gan0, n0 = _bf16_run(b, ctx, None, None)
-    assert _expected_launches(ds, d_cons) == 3 and _expected_launches(gs, g_cons) == 2       # every path runs
+    assert _expected_launches(ds, (3, 32, 32), d_cons) == 3 and _expected_launches(gs, (16,), g_cons) == 2       # every path runs
     gan0.close(); G0.close(); D0.close()
     runs = []
     for _ in range(2):
@@ -213,7 +203,7 @@ def test_bf16_operands_follow_the_constrained_master_and_launch_counts(b200):
         runs.append((G.params(), D.params(), n))
         gan.close(); G.close(); D.close()
     assert np.array_equal(runs[0][0], runs[1][0]) and np.array_equal(runs[0][1], runs[1][1])
-    assert runs[0][2] == n0 + _expected_launches(ds, d_cons) + _expected_launches(gs, g_cons), (n0, runs[0][2])
+    assert runs[0][2] == n0 + _expected_launches(ds, (3, 32, 32), d_cons) + _expected_launches(gs, (16,), g_cons), (n0, runs[0][2])
 
 
 def test_two_ranks_match_one_gpu(tmp_path):
