@@ -165,8 +165,8 @@ def launches_per_step(ctx, gan, n):
     return (ctx.launch_count() - l0) / 3
 
 
-def run_two_ranks(script, out_json, port, env=None, timeout=600):
-    """tools/<script> out_json on two ranks of one node under torch.distributed.run (master 127.0.0.1:port); the JSON it wrote.  Skips the
+def run_two_ranks(script, out_json, port, env=None, timeout=600, args=()):
+    """tools/<script> out_json *args on two ranks of one node under torch.distributed.run (master 127.0.0.1:port); the JSON it wrote.  Skips the
     test on a machine with fewer than two GPUs."""
     try:
         import torch
@@ -176,7 +176,7 @@ def run_two_ranks(script, out_json, port, env=None, timeout=600):
     if gpus < 2:
         pytest.skip("needs two GPUs")
     out = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
-                          "--master-port", str(port), os.path.join(ROOT, "tools", script), str(out_json)],
+                          "--master-port", str(port), os.path.join(ROOT, "tools", script), str(out_json), *args],
                          capture_output=True, text=True, timeout=timeout, env=env, cwd=ROOT)
     assert out.returncode == 0, out.stdout[-800:] + out.stderr[-1500:]
     with open(out_json) as f:

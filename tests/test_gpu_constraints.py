@@ -207,5 +207,5 @@ def test_bf16_operands_follow_the_constrained_master_and_launch_counts(b200):
 
 
 def test_two_ranks_match_one_gpu(tmp_path):
-    d = run_two_ranks("constraint_dp_check.py", tmp_path / "constraint_dp.json", 29563)
+    d = run_two_ranks("dp_check.py", tmp_path / "constraint_dp.json", 29563, args=("constraint",))
     assert d["world"] == 2 and d["params_identical_across_ranks"] is True and d["max_rel_err_vs_one_gpu"] < 1e-5

@@ -219,5 +219,5 @@ def test_fp32_gan_step_with_dropout_graph_eager_and_oracle(b200):
 
 
 def test_two_ranks_share_parameters_but_not_masks(tmp_path):
-    d = run_two_ranks("dropout_dp_check.py", tmp_path / "dropout_dp.json", 29547)
+    d = run_two_ranks("dp_check.py", tmp_path / "dropout_dp.json", 29547, args=("dropout",))
     assert d["world"] == 2 and d["d_params_identical"] is True and d["dropout_activations_differ"] is True and d["masks_match_oracle"] is True

@@ -239,5 +239,5 @@ def test_rejections(b200):
 
 
 def test_two_ranks_match_one_gpu(tmp_path):
-    d = run_two_ranks("gradnorm_dp_check.py", tmp_path / "gradnorm_dp.json", 29549)
+    d = run_two_ranks("dp_check.py", tmp_path / "gradnorm_dp.json", 29549, args=("gradnorm",))
     assert d["world"] == 2 and d["params_identical_across_ranks"] is True and d["max_rel_err_vs_one_gpu"] < 1e-5

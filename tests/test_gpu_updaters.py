@@ -291,6 +291,6 @@ def test_rejections(b200):
 
 
 def test_two_ranks_average_every_state_slot(tmp_path):
-    d = run_two_ranks("updater_dp_check.py", tmp_path / "updater_dp.json", 29551)
+    d = run_two_ranks("dp_check.py", tmp_path / "updater_dp.json", 29551, args=("updater",))
     assert d["world"] == 2 and d["state_slots"] == 3 and d["ranks_differed"] is True
     assert d["max_rel_err_params"] < 1e-6 and max(d["max_rel_err_slot"]) < 1e-6
