@@ -127,6 +127,8 @@ PROTOTYPES = {
     "b2g_net_set_constraints": (_i32, [_vp, C.c_char_p, C.c_char_p, C.POINTER(Constraint), _i32]),
     "b2g_net_apply_constraints": (_i32, [_vp]),
     "b2g_net_get_learning_rate": (_i32, [_vp, C.c_char_p, _fp]),
+    "b2g_net_set_dropout_schedule": (_i32, [_vp, C.c_char_p, C.POINTER(LrSchedule)]),
+    "b2g_net_get_dropout_value": (_i32, [_vp, C.c_char_p, _fp]),
     "b2g_net_get_epoch": (_i32, [_vp, C.POINTER(_i64)]),
     "b2g_net_set_epoch": (_i32, [_vp, _i64]),
     "b2g_net_simt_gemm_calls": (_i32, [_vp, C.POINTER(C.c_uint64)]),
@@ -153,6 +155,7 @@ PROTOTYPES = {
                            _i32, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     "b2g_test_net_shadow": (_i32, [_vp, _i32, _i32, _fp, _i64]),
     "b2g_test_dropout": (_i32, [_vp, _i32, C.c_uint64, _i32, _i32, _i64, _i32, _i32, _i32, _i32, C.c_float, _fp, _fp, _fp, _fp]),
+    "b2g_test_dropout_kind": (_i32, [_vp, _i32, _i32, C.c_uint64, _i32, _i32, _i64, _i32, _i32, _i32, _i32, C.c_float, _fp, _fp, _fp, _fp]),
     "b2g_test_ew": (_i32, [_vp, _i32, C.POINTER(TestEwOpts), _fp, _fp, _fp, _fp, _fp]),
     "b2g_test_pool": (_i32, [_vp, _i32, C.POINTER(TestPoolOpts), _fp, _fp, _fp, _fp, _fp]),
 }

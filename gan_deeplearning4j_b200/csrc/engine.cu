@@ -108,11 +108,21 @@ struct LayerRT {
   // DropoutLayer: its own output buffer (never its input: the layer below differentiates from its own pre-dropout output) and the 1-bit
   // keep mask of the latest train-mode forward; `out` is drop_buf after a masked forward and the input itself after a pass-through one
   void* drop_buf = nullptr; uint32_t* drop_mask = nullptr; bool drop_live = false;
+  // the other kinds (b2g_dropout_kind in d.act): the mask is per element (ALPHA), per (row, channel) (SPATIAL) or absent (Gaussian kinds);
+  // drop_rec: the P and value of the latest forward (GAUSSIAN_DROPOUT's backward draws m again from them; a scheduled backward takes the
+  // forward's value).  drop_sched: b2g_net_set_dropout_schedule gave the layer a schedule, held on the device in drop_sched_dev (MAP entries
+  // in drop_map); such a layer is stochastic whatever its value
+  NoiseRec* drop_rec = nullptr; UpdSched* drop_sched_dev = nullptr; bool drop_sched = false; void* drop_map = nullptr;
   // ELEMENTWISE / MERGE (include/b200gan.h): the skip source j (d.pre_h), the input order (d.pre_w), and whether this vertex is the first
   // consumer of j the backward visits (it writes j's accumulator; the later ones add).  A skip source: its consumer count and fp32 accumulator.
   int vsrc = -1, vorder = 0; bool vfirst = false;
   int n_skip = 0; float* skip_acc = nullptr;
-  bool drop_active() const { return d.type == B2G_LAYER_DROPOUT && !d.frozen && d.act_alpha < 1.f; }   // FrozenLayer: test mode, identity
+  // a stochastic DropoutLayer: train mode draws from the pass counter.  FrozenLayer: test mode, identity; p = 1, rate = 0, stddev = 0: identity
+  bool drop_active() const {
+    if (d.type != B2G_LAYER_DROPOUT || d.frozen) return false;
+    if (drop_sched) return true;
+    return d.act == B2G_DROPOUT_GAUSSIAN_DROPOUT || d.act == B2G_DROPOUT_GAUSSIAN_NOISE ? d.act_alpha > 0.f : d.act_alpha < 1.f;
+  }
   bool has_gemm() const { return d.type == B2G_LAYER_CONV2D || d.type == B2G_LAYER_DECONV2D || d.type == B2G_LAYER_DENSE || d.type == B2G_LAYER_OUTPUT; }
 };
 
@@ -328,12 +338,21 @@ static int32_t net_build(b2g_net* n, const b2g_layer_desc* layers, int32_t nl) {
         if ((size_t)d.pre_h * d.pre_w * d.pre_c != l.in_elems) return fail(B2G_ERR_SHAPE, "layer %s: FeedForwardToCnn(%d,%d,%d) != %zu features", d.name, d.pre_h, d.pre_w, d.pre_c, l.in_elems);
         l.oh = d.pre_h; l.ow = d.pre_w; l.oc = d.pre_c; break;
       case B2G_LAYER_CNN_TO_FF: l.oh = l.ow = 1; l.oc = h * w * ch; break;
-      case B2G_LAYER_DROPOUT:        // DropoutLayer.Builder(p): p = retain probability, carried in act_alpha; no parameters
-        if (!(d.act_alpha > 0.f && d.act_alpha <= 1.f)) return fail(B2G_ERR_ARG, "layer %s: dropout retain probability %g outside (0, 1]", d.name, (double)d.act_alpha);
+      case B2G_LAYER_DROPOUT: {      // DropoutLayer.Builder(IDropout): the b2g_dropout_kind in act, its value (p, rate, stddev) in act_alpha; no parameters
+        const float v = d.act_alpha;
+        switch (d.act) {
+          case B2G_DROPOUT: case B2G_DROPOUT_ALPHA: case B2G_DROPOUT_SPATIAL:
+            if (!(v > 0.f && v <= 1.f)) return fail(B2G_ERR_ARG, "layer %s: dropout retain probability %g outside (0, 1]", d.name, (double)v);
+            break;
+          case B2G_DROPOUT_GAUSSIAN_DROPOUT: if (!(v >= 0.f && v < 1.f)) return fail(B2G_ERR_ARG, "layer %s: GaussianDropout rate %g outside [0, 1)", d.name, (double)v); break;
+          case B2G_DROPOUT_GAUSSIAN_NOISE: if (!(v >= 0.f && std::isfinite(v))) return fail(B2G_ERR_ARG, "layer %s: GaussianNoise stddev %g not finite and >= 0", d.name, (double)v); break;
+          default: return fail(B2G_ERR_ARG, "layer %s: unknown dropout kind %d", d.name, d.act);
+        }
+        if (d.act == B2G_DROPOUT_SPATIAL && h == 1 && w == 1) return fail(B2G_ERR_SHAPE, "layer %s: SpatialDropout needs a convolutional [H, W, C] input, not a feed-forward one", d.name);
         l.oh = h; l.ow = w; l.oc = ch;
         if ((uint64_t)c.max_batch * h * w * ch > (1ull << 34))     // checked before anything is allocated
           return fail(B2G_ERR_UNSUPPORTED, "layer %s: a dropout pass of %llu elements exceeds the 2^34 the mask counter addresses", d.name, (unsigned long long)c.max_batch * h * w * ch);
-        break;
+      } break;
       case B2G_LAYER_ELEMENTWISE: case B2G_LAYER_MERGE: {      // the spine (entry i-1) and a skip source j = pre_h, in the order pre_w
         const int j = d.pre_h;
         if (j < 0 || j >= i) return fail(B2G_ERR_ARG, "layer %s: skip source %d outside [0, %d)", d.name, j, i);
@@ -400,7 +419,13 @@ static int32_t net_alloc(b2g_net* n) {
                  (l.d.type == B2G_LAYER_CNN_TO_FF && (l.ic == 1 || l.ih * l.iw == 1));
     l.out_alias = alias;
     if (!alias) B2(dalloc(n, (char**)&l.out, ts * R * l.out_elems));
-    if (l.d.type == B2G_LAYER_DROPOUT) { l.drop_buf = l.out; B2(dalloc(n, &l.drop_mask, sizeof(uint32_t) * (((size_t)R * l.out_elems + 31) / 32))); }
+    if (l.d.type == B2G_LAYER_DROPOUT) {
+      l.drop_buf = l.out;
+      const size_t bits = l.d.act == B2G_DROPOUT_SPATIAL ? (size_t)R * l.oc : l.d.act == B2G_DROPOUT || l.d.act == B2G_DROPOUT_ALPHA ? (size_t)R * l.out_elems : 0;
+      if (bits) B2(dalloc(n, &l.drop_mask, sizeof(uint32_t) * ((bits + 31) / 32)));
+      B2(dalloc(n, &l.drop_rec, sizeof(NoiseRec))); CU(cudaMemsetAsync(l.drop_rec, 0, sizeof(NoiseRec), n->ctx->stream));
+      B2(dalloc(n, &l.drop_sched_dev, sizeof(UpdSched))); CU(cudaMemsetAsync(l.drop_sched_dev, 0, sizeof(UpdSched), n->ctx->stream));
+    }
     if (l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS || l.d.type == B2G_LAYER_CNN_LOSS) B2(dalloc(n, (char**)&l.probs, ts * R * l.out_elems));
     if (l.ext_act && l.has_gemm() && l.d.type != B2G_LAYER_OUTPUT) B2(dalloc(n, (char**)&l.ext_z, ts * R * l.out_elems));
     if (l.d.type == B2G_LAYER_MAXPOOL) B2(dalloc(n, &l.argmax, (size_t)R * l.out_elems));
@@ -553,7 +578,8 @@ static void net_refresh_shadow(b2g_net* n, int only_layer = -1) {
 }
 
 // ------------------------------------------------------------------ forward / backward -------------------
-struct FwdOpts { int rows; int groups; bool train; bool update_running; void* out_override; };
+// sched_step / sched_epoch: the counters scheduled DropoutLayers read (null: the net's own)
+struct FwdOpts { int rows; int groups; bool train; bool update_running; void* out_override; const int* sched_step = nullptr; const int64_t* sched_epoch = nullptr; };
 
 static const void* w_ptr(const b2g_net* n, const LayerRT& l, int* wprec) {
   if (n->prec == PREC_BF16) { *wprec = PREC_BF16; return n->shadow + l.off_W_bf; }
@@ -647,6 +673,22 @@ static DropoutArgs make_dropout_args(uint64_t seed, int layer, int rank, float p
   return a;
 }
 static DropoutArgs dropout_args(const b2g_net* n, int layer) { return make_dropout_args(n->cfg.seed, layer, n->ctx->rank, n->L[layer].d.act_alpha); }
+// The same inputs for the other kinds, with the kernels' constants derived from the value v (b2g_dropout_kind): sigma, AlphaDropout's a, b
+// and a', SpatialDropout's 1/p, and the Bernoulli threshold.  hw, C: the layer's map.
+static NoiseArgs make_noise_args(uint64_t seed, int layer, int rank, int kind, float v, int hw, int C) {
+  NoiseArgs a{}; a.seed = seed ? seed : 666; a.tag = (uint32_t)layer | ((uint32_t)rank << 16); a.hw = hw; a.C = C; a.value = v;
+  noise_derive(kind, v, a);
+  return a;
+}
+static NoiseArgs noise_args(const b2g_net* n, int layer) {
+  const LayerRT& l = n->L[layer];
+  return make_noise_args(n->cfg.seed, layer, n->ctx->rank, l.d.act, l.d.act_alpha, l.oh * l.ow, l.oc);
+}
+// The schedule inputs of a layer's kernels: its schedule (null when it has none) at the counters of the pass (the net's own, or in the GAN
+// step's generator pass the generator's)
+static NoiseSched noise_sched(const b2g_net* n, const LayerRT& l, const int* step, const int64_t* epoch) {
+  return NoiseSched{l.drop_sched ? l.drop_sched_dev : nullptr, step ? step : n->step_dev, epoch ? epoch : n->epoch_dev};
+}
 
 // Runs layers [0, L) on `in` (T NHWC, rows examples). Returns pointer to the final activations.
 static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const void** result) {
@@ -657,7 +699,7 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
   n->last_rows = R;
   // every BatchNorm accumulator of the pass (forward statistics and the backward reductions that follow) starts from zero: one memset node
   if (o.train && n->bn_acc) CU(cudaMemsetAsync(n->bn_acc, 0, n->bn_acc_bytes, s));
-  // every masked DropoutLayer of a train-mode pass draws with the same pass counter P; the last one's kernel advances P on the device
+  // every stochastic DropoutLayer of a train-mode pass draws with the same pass counter P; the last one's kernel advances P on the device
   int last_drop = -1;
   if (o.train) for (size_t i = 0; i < n->L.size(); ++i) if (n->L[i].drop_active()) last_drop = (int)i;
   for (size_t i = 0; i < n->L.size(); ++i) {
@@ -723,9 +765,11 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
       case B2G_LAYER_DROPOUT:
         l.drop_live = o.train && l.drop_active();
         if (l.drop_live) {
-          k_dropout_fwd(n->prec, cur, l.drop_buf, l.drop_mask, (size_t)R * l.out_elems, dropout_args(n, (int)i), n->drop_pass, n->drop_ticket, (int)i == last_drop, s);
+          if (d.act == B2G_DROPOUT && !l.drop_sched) k_dropout_fwd(n->prec, cur, l.drop_buf, l.drop_mask, (size_t)R * l.out_elems, dropout_args(n, (int)i), n->drop_pass, n->drop_ticket, (int)i == last_drop, s);
+          else k_noise_fwd(n->prec, d.act, cur, l.drop_buf, l.drop_mask, l.drop_rec, (size_t)R * l.out_elems, noise_args(n, (int)i),
+                           noise_sched(n, l, o.sched_step, o.sched_epoch), n->drop_pass, n->drop_ticket, (int)i == last_drop, s);
           out = l.drop_buf;
-        } else out = (void*)cur;       // inference, FrozenLayer or p = 1: the identity, no launch
+        } else out = (void*)cur;       // inference, FrozenLayer, p = 1, rate = 0 or stddev = 0: the identity, no launch
         l.out = out;
         break;
       case B2G_LAYER_ELEMENTWISE: {
@@ -892,7 +936,12 @@ static int32_t net_backward(b2g_net* n, const void* net_in, void* eps, int rows,
       case B2G_LAYER_UPSAMPLE2D: if (need_in) { void* nx = other(cur); k_upsample_bwd(n->prec, cur, nx, R, l.ih, l.iw, l.ic, d.k_h, s); cur = nx; } break;
       case B2G_LAYER_FF_TO_CNN: if (!l.out_alias && need_in) { void* nx = other(cur); k_permute(n->prec, cur, nx, R, l.oc, l.oh * l.ow, 0, s); cur = nx; } break;
       case B2G_LAYER_CNN_TO_FF: if (!l.out_alias && need_in) { void* nx = other(cur); k_permute(n->prec, cur, nx, R, l.ic, l.ih * l.iw, 1, s); cur = nx; } break;
-      case B2G_LAYER_DROPOUT: if (need_in && l.drop_live) k_dropout_bwd(n->prec, cur, cur, l.drop_mask, (size_t)R * l.out_elems, 1.0f / d.act_alpha, s); break;   // the forward's mask
+      case B2G_LAYER_DROPOUT:       // the forward's mask (GAUSSIAN_DROPOUT: its P; GAUSSIAN_NOISE: the identity, no launch)
+        if (need_in && l.drop_live) {
+          if (d.act == B2G_DROPOUT && !l.drop_sched) k_dropout_bwd(n->prec, cur, cur, l.drop_mask, (size_t)R * l.out_elems, 1.0f / d.act_alpha, s);
+          else k_noise_bwd(n->prec, d.act, cur, cur, l.drop_mask, l.drop_rec, (size_t)R * l.out_elems, noise_args(n, i), noise_sched(n, l, nullptr, nullptr), s);
+        }
+        break;
     }
     if (i == n->ar_split_layer && want_wgrad && allreduce_follows && ar_overlap_on(n)) {
       // every gradient of layers >= i is queued (BN scale/shift on s, weights/biases on s2): all-reduce that tail on the comm stream now
@@ -1034,6 +1083,7 @@ extern "C" int32_t b2g_net_destroy(b2g_net* n) {
   for (auto e : n->ev_fork) if (e) cudaEventDestroy(e); for (auto e : n->ev_done) if (e) cudaEventDestroy(e); if (n->ev_join) cudaEventDestroy(n->ev_join);
   if (n->p2p) for (int r = 0; r < n->ctx->world; ++r) if (r != n->ctx->rank && n->p2p_peer_grads[r]) cudaIpcCloseMemHandle(n->p2p_peer_grads[r]);
   if (n->sched_map) cudaFree(n->sched_map);
+  for (auto& l : n->L) if (l.drop_map) cudaFree(l.drop_map);
   cudaFree(n->con_jobs); cudaFree(n->con_partial); cudaFree(n->con_mult);
   for (void* p : n->allocs) cudaFree(p); delete n; return 0;
 }
@@ -1291,7 +1341,8 @@ static int32_t gan_step_part2(b2g_gan* g, int N) {
   B2(net_update(D, 2 * N));
   // 3. G update through D on (z_g, y_gen) (J:465-471); D's parameters / running stats / updater state untouched
   CU(cudaStreamWaitEvent(s, G->ctx->ev_b, 0));
-  FwdOpts od2{N, 1, true, false, nullptr};
+  // a scheduled DropoutLayer of D reads G's counters here: this pass belongs to the generator's fit (the stacked gan graph counts its own)
+  FwdOpts od2{N, 1, true, false, nullptr, G->step_dev, G->epoch_dev};
   B2(net_forward(D, xg, od2, &logits));
   net_loss(D, logits, g->y_g, D->epsA, g->loss_dev + 2, N, 1);
   // the generator's output activation (tanh) is differentiated inside D's last input-gradient kernel when that kernel can (EPI_ACTBWD)
@@ -1611,8 +1662,8 @@ static int32_t net_upload_schedules(b2g_net* n) {
   n->sched_on = on; ++n->settings_gen;
   return 0;
 }
-extern "C" int32_t b2g_net_set_lr_schedule(b2g_net* n, const char* layer, const b2g_lr_schedule* s) {
-  if (!n) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
+// A b2g_lr_schedule checked and copied (null or NONE: no schedule); shared by the learning-rate and the DropoutLayer schedules
+static int32_t parse_schedule(const b2g_lr_schedule* s, b2g_net::LayerSched* out) {
   b2g_net::LayerSched ls;
   if (s && s->kind != B2G_SCHED_NONE) {
     if (s->kind < B2G_SCHED_EXPONENTIAL || s->kind > B2G_SCHED_MAP) return fail(B2G_ERR_ARG, "unknown schedule kind %d (PolySchedule is not supported)", s->kind);
@@ -1635,6 +1686,12 @@ extern "C" int32_t b2g_net_set_lr_schedule(b2g_net* n, const char* layer, const 
       ls.keys.assign(s->map_keys, s->map_keys + s->n_map); ls.vals.assign(s->map_values, s->map_values + s->n_map); sc.n_map = s->n_map;
     }
   }
+  *out = ls;
+  return 0;
+}
+extern "C" int32_t b2g_net_set_lr_schedule(b2g_net* n, const char* layer, const b2g_lr_schedule* s) {
+  if (!n) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
+  b2g_net::LayerSched ls; B2(parse_schedule(s, &ls));
   if (layer) { int li = 0; B2(find_lr_layer(n, layer, &li)); n->layer_sched[li] = ls; }
   else for (size_t li = 0; li < n->L.size(); ++li) if (layer_has_lr(n, (int)li)) n->layer_sched[li] = ls;
   return net_upload_schedules(n);
@@ -1644,6 +1701,49 @@ extern "C" int32_t b2g_net_get_learning_rate(b2g_net* n, const char* layer, floa
   int li = 0; B2(find_lr_layer(n, layer, &li));
   const int seg = lr_segment(n, li);
   k_sched_lr(n->segs_dev, n->sched_dev, seg, n->step_dev, n->epoch_dev, n->lr_out, n->ctx->stream); CHECK_KERNELS();
+  CU(cudaMemcpyAsync(out, n->lr_out, sizeof(float), cudaMemcpyDeviceToHost, n->ctx->stream)); CU(cudaStreamSynchronize(n->ctx->stream));
+  return 0;
+}
+// ------------------------------------------------------------------ DropoutLayer schedules (b2g_net_set_dropout_schedule) ---------------
+static int32_t find_dropout_layer(const b2g_net* n, const char* layer, int* li) {
+  for (size_t i = 0; i < n->L.size(); ++i) if (!strncmp(n->L[i].d.name, layer, B2G_NAME_LEN)) {
+    if (n->L[i].d.type != B2G_LAYER_DROPOUT) return fail(B2G_ERR_ARG, "layer %s is not a DropoutLayer", layer);
+    *li = (int)i; return 0;
+  }
+  return fail(B2G_ERR_ARG, "no layer named %s", layer);
+}
+// The layer's schedule to its device slot, MAP entries (values, then keys) to a buffer of its own
+static int32_t upload_dropout_schedule(b2g_net* n, LayerRT& l, const b2g_net::LayerSched& ls) {
+  cudaStream_t s = n->ctx->stream;
+  CU(cudaStreamSynchronize(s));                  // nothing in flight reads the old schedule or map
+  if (l.drop_map) { CU(cudaFree(l.drop_map)); l.drop_map = nullptr; }
+  UpdSched sc = ls.sc;
+  if (sc.kind == B2G_SCHED_MAP) {
+    const size_t nv = ls.vals.size(), bytes = nv * (sizeof(double) + sizeof(int32_t));
+    cudaError_t e = cudaMalloc(&l.drop_map, bytes);
+    if (e != cudaSuccess) { l.drop_map = nullptr; return fail(B2G_ERR_OOM, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); }
+    CU(cudaMemcpyAsync(l.drop_map, ls.vals.data(), nv * sizeof(double), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync((char*)l.drop_map + nv * sizeof(double), ls.keys.data(), nv * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    sc.vals = (const double*)l.drop_map; sc.keys = (const int32_t*)((char*)l.drop_map + nv * sizeof(double));
+  }
+  CU(cudaMemcpyAsync(l.drop_sched_dev, &sc, sizeof(sc), cudaMemcpyHostToDevice, s));
+  CU(cudaStreamSynchronize(s));
+  l.drop_sched = sc.kind != B2G_SCHED_NONE;
+  return 0;
+}
+extern "C" int32_t b2g_net_set_dropout_schedule(b2g_net* n, const char* layer, const b2g_lr_schedule* s) {
+  if (!n) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
+  b2g_net::LayerSched ls; B2(parse_schedule(s, &ls));
+  if (layer) { int li = 0; B2(find_dropout_layer(n, layer, &li)); B2(upload_dropout_schedule(n, n->L[li], ls)); }
+  else for (auto& l : n->L) if (l.d.type == B2G_LAYER_DROPOUT && !l.d.frozen) B2(upload_dropout_schedule(n, l, ls));
+  ++n->settings_gen;           // a captured step holds which kernels the layers launch: re-capture
+  return 0;
+}
+extern "C" int32_t b2g_net_get_dropout_value(b2g_net* n, const char* layer, float* out) {
+  if (!n || !layer || !out) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
+  int li = 0; B2(find_dropout_layer(n, layer, &li));
+  const LayerRT& l = n->L[li];
+  k_noise_value(l.d.act, l.d.act_alpha, noise_sched(n, l, nullptr, nullptr), n->lr_out, n->ctx->stream); CHECK_KERNELS();
   CU(cudaMemcpyAsync(out, n->lr_out, sizeof(float), cudaMemcpyDeviceToHost, n->ctx->stream)); CU(cudaStreamSynchronize(n->ctx->stream));
   return 0;
 }
@@ -2015,6 +2115,42 @@ extern "C" int32_t b2g_test_dropout(b2g_ctx* c, int32_t precision, uint64_t seed
   const DropoutArgs a = make_dropout_args(seed, layer, rank, p);
   k_dropout_fwd(prec, tx, ty, mask, n, a, dpass, ticket, 1, s);
   k_dropout_bwd(prec, te, te, mask, n, a.scale, s);
+  unsigned long long p1 = 0;
+  B2(m.downT(y, ty, n)); B2(m.downT(dx, te, n)); CU(cudaMemcpyAsync(&p1, dpass, sizeof(p1), cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s)); CHECK_KERNELS();
+  if (p1 != p0 + 1) return fail(B2G_ERR_CUDA, "dropout test: the forward left the pass counter at %llu, expected %llu", p1, p0 + 1);
+  return 0;
+}
+
+// One DropoutLayer forward and backward of any b2g_dropout_kind, as b2g_test_dropout (include/b200gan.h b2g_test_dropout_kind).
+extern "C" int32_t b2g_test_dropout_kind(b2g_ctx* c, int32_t precision, int32_t kind, uint64_t seed, int32_t layer, int32_t rank, int64_t pass, int32_t rows,
+                                         int32_t h, int32_t w, int32_t ch, float v, const float* x, const float* dy, float* y, float* dx) {
+  if (!c || !x || !dy || !y || !dx) return fail(B2G_ERR_ARG, "null");
+  bool identity = false;
+  switch (kind) {
+    case B2G_DROPOUT: case B2G_DROPOUT_ALPHA: case B2G_DROPOUT_SPATIAL:
+      if (!(v > 0.f && v <= 1.f)) return fail(B2G_ERR_ARG, "dropout retain probability %g outside (0, 1]", (double)v);
+      identity = v >= 1.f; break;
+    case B2G_DROPOUT_GAUSSIAN_DROPOUT: if (!(v >= 0.f && v < 1.f)) return fail(B2G_ERR_ARG, "GaussianDropout rate %g outside [0, 1)", (double)v); identity = v == 0.f; break;
+    case B2G_DROPOUT_GAUSSIAN_NOISE: if (!(v >= 0.f && std::isfinite(v))) return fail(B2G_ERR_ARG, "GaussianNoise stddev %g not finite and >= 0", (double)v); identity = v == 0.f; break;
+    default: return fail(B2G_ERR_ARG, "unknown dropout kind %d", kind);
+  }
+  if (kind == B2G_DROPOUT) return b2g_test_dropout(c, precision, seed, layer, rank, pass, rows, h, w, ch, v, x, dy, y, dx);
+  if (rows < 1 || h < 1 || w < 1 || ch < 1 || layer < 0 || layer > 0xffff || rank < 0 || rank > 0xffff || pass < 0) return fail(B2G_ERR_ARG, "bad dropout test arguments");
+  const size_t n = (size_t)rows * h * w * ch;
+  if (n > 0x7fffffff) return fail(B2G_ERR_UNSUPPORTED, "the dropout test hook takes at most 2^31 - 1 elements (%zu)", n);
+  if (identity) { memcpy(y, x, n * sizeof(float)); memcpy(dx, dy, n * sizeof(float)); return 0; }
+  const int prec = precision == B2G_PREC_BF16 ? PREC_BF16 : PREC_F32; const size_t ts = prec_size(prec);
+  CU(cudaSetDevice(c->device)); cudaStream_t s = c->stream;
+  HookMem m(s, prec);
+  void *tx, *te, *ty; uint32_t* mask; unsigned long long* dpass; NoiseRec* rec; unsigned* ticket;
+  const unsigned long long p0 = (unsigned long long)pass;
+  B2(m.upT(x, n, &tx)); B2(m.upT(dy, n, &te)); B2(m.dev(n, ts, &ty)); B2(m.dev((n + 31) / 32, 4, (void**)&mask));
+  B2(m.dev(1, sizeof(p0), (void**)&dpass)); B2(m.dev(1, sizeof(NoiseRec), (void**)&rec)); B2(m.dev(1, sizeof(unsigned), (void**)&ticket));
+  CU(cudaMemcpyAsync(dpass, &p0, sizeof(p0), cudaMemcpyHostToDevice, s)); CU(cudaMemsetAsync(ticket, 0, sizeof(unsigned), s));
+  const NoiseArgs a = make_noise_args(seed, layer, rank, kind, v, h * w, ch);
+  k_noise_fwd(prec, kind, tx, ty, mask, rec, n, a, NoiseSched{}, dpass, ticket, 1, s);
+  k_noise_bwd(prec, kind, te, te, mask, rec, n, a, NoiseSched{}, s);
   unsigned long long p1 = 0;
   B2(m.downT(y, ty, n)); B2(m.downT(dx, te, n)); CU(cudaMemcpyAsync(&p1, dpass, sizeof(p1), cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s)); CHECK_KERNELS();

@@ -5,6 +5,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <math.h>
 #include <stdint.h>
 
 namespace b2g {
@@ -124,6 +125,42 @@ struct DropoutArgs { uint64_t seed; uint32_t tag; uint32_t threshold; float scal
 void k_dropout_fwd(int prec, const void* x, void* y, uint32_t* mask, size_t n, const DropoutArgs& a, unsigned long long* pass, unsigned* ticket, int bump_pass, cudaStream_t s);
 // Backward: eps_in = eps_out * (1/p) where the forward kept the element, 0 elsewhere (eps_in may equal eps_out)
 void k_dropout_bwd(int prec, const void* eps_out, void* eps_in, const uint32_t* mask, size_t n, float scale, cudaStream_t s);
+// The other IDropout kinds (b2g_dropout_kind; definitions in include/b200gan.h), drawn from the same Philox stream and pass counter, and
+// Dropout(p) with a schedule.  value: the layer's constant value; the rest is derived from a value by noise_derive.  scale: GAUSSIAN_DROPOUT /
+// GAUSSIAN_NOISE sigma, ALPHA_DROPOUT a, DROPOUT / SPATIAL_DROPOUT 1/p; shift: ALPHA_DROPOUT b; fill: ALPHA_DROPOUT a' = -lambda alpha.
+// hw, C: SPATIAL_DROPOUT's map (pixels per row, channels); its keep bit of (row, c) is mask bit j = row * C + c.
+enum DropKind { DROP_BERNOULLI = 0, DROP_GAUSSIAN_DROPOUT = 1, DROP_GAUSSIAN_NOISE = 2, DROP_ALPHA = 3, DROP_SPATIAL = 4 };
+struct NoiseArgs { uint64_t seed; uint32_t tag; uint32_t threshold; float value, scale, shift, fill; int keep_all; int hw, C; };
+// A scheduled value outside its kind's range is clamped into it: p to [2^-32, 1], rate to [0, 1 - 2^-24], sigma to >= 0
+__host__ __device__ inline float noise_clamp(int kind, float v) {
+  if (kind == DROP_GAUSSIAN_DROPOUT) return fminf(fmaxf(v, 0.f), 0x1.fffffep-1f);
+  if (kind == DROP_GAUSSIAN_NOISE) return fmaxf(v, 0.f);
+  return fminf(fmaxf(v, 0x1p-32f), 1.f);
+}
+// The kernels' constants of value v, each computed in double and rounded to fp32 once (include/b200gan.h b2g_dropout_kind)
+__host__ __device__ inline void noise_derive(int kind, float v, NoiseArgs& a) {
+  if (kind == DROP_GAUSSIAN_DROPOUT) { a.scale = (float)sqrt((double)v / (1.0 - (double)v)); return; }
+  if (kind == DROP_GAUSSIAN_NOISE) { a.scale = v; return; }
+  a.keep_all = v >= 1.f ? 1 : 0; a.threshold = a.keep_all ? 0u : (uint32_t)floor((double)v * 4294967296.0);
+  if (kind == DROP_ALPHA) {        // SELU's alpha and lambda
+    const double ap = -1.0507009873554805 * 1.6732632423543772, p = v, A = 1.0 / sqrt(p + ap * ap * p * (1.0 - p));
+    a.scale = (float)A; a.shift = (float)(-A * (1.0 - p) * ap); a.fill = (float)ap;
+  } else a.scale = 1.0f / v;
+}
+// What a forward drew with, for its backward: the pass counter P (GAUSSIAN_DROPOUT draws m again) and the value (scheduled layers)
+struct NoiseRec { unsigned long long P; float v; };
+// A scheduled layer (sched != null): every block takes the value from the schedule at the iteration *step (before the update's increment) or
+// the epoch *epoch, clamps it and derives the constants from it; the forward records the value in rec, the backward reads it from there.
+struct UpdSched;
+struct NoiseSched { const UpdSched* sched; const int* step; const int64_t* epoch; };
+// Forward of a DropoutLayer other than unscheduled Dropout(p).  mask: DROPOUT / ALPHA one bit per element, SPATIAL one per (row, channel).
+void k_noise_fwd(int prec, int kind, const void* x, void* y, uint32_t* mask, NoiseRec* rec, size_t n, const NoiseArgs& a, const NoiseSched& q,
+                 unsigned long long* pass, unsigned* ticket, int bump_pass, cudaStream_t s);
+// Its backward (eps_in may equal eps_out); GAUSSIAN_NOISE is the identity and launches nothing.
+void k_noise_bwd(int prec, int kind, const void* eps_out, void* eps_in, const uint32_t* mask, const NoiseRec* rec, size_t n, const NoiseArgs& a,
+                 const NoiseSched& q, cudaStream_t s);
+// *out = the clamped value the next forward of a layer of this kind uses (one thread, one launch)
+void k_noise_value(int kind, float value, const NoiseSched& q, float* out, cudaStream_t s);
 
 // ---- loss ----------------------------------------------------------------------------------------------
 // LossBinaryXENT on logits z[rows] with labels y[rows]: dz = dL/dz (sum form, not /mb), loss_sums[g] = sum of losses per group.
@@ -218,6 +255,24 @@ void k_updater(float* params, const float* grads, float* st0, float* st1, float*
 // *out = the fp32 learning rate the updater kernel would use for segment seg at the current *step_dev / *epoch_dev (one thread, one launch)
 void k_sched_lr(const UpdSeg* segs_dev, const UpdSched* sched, int seg, const int* step_dev, const int64_t* epoch_dev, float* out, cudaStream_t s);
 static const int UPD_CHUNK = 4096;
+// The learning rate of a segment at iteration `it` (the counter before this update's increment) / epoch `ep`: DL4J's ISchedule.valueAt in
+// double, rounded to fp32 once (include/b200gan.h, b2g_lr_schedule); kind 0 = the constant lr.  Also the scheduled DropoutLayer value.
+__device__ inline float sched_lr(const UpdSched& sc, float lr, int it, long long ep) {
+  if (sc.kind == 0) return lr;
+  const long long ii = sc.type == 1 ? ep : (long long)it;
+  const double i = (double)ii;
+  double v;
+  if (sc.kind == 1) v = sc.initial * pow(sc.gamma, i);
+  else if (sc.kind == 2) v = sc.initial / pow(1.0 + sc.gamma * i, sc.power);
+  else if (sc.kind == 3) v = sc.initial / (1.0 + exp(-sc.gamma * (i - sc.step)));
+  else if (sc.kind == 4) v = sc.initial * pow(sc.decay, floor(i / sc.step));
+  else {          // MAP: the largest key <= i (keys strictly increase, keys[0] <= 0 <= i)
+    int lo = 0, hi = sc.n_map - 1;
+    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if ((long long)sc.keys[mid] <= ii) lo = mid; else hi = mid - 1; }
+    v = sc.vals[lo];
+  }
+  return (float)v;
+}
 
 // ---- L2 gradient normalization (DL4J GradientNormalization.{Renormalize,Clip}L2Per{Layer,ParamType}; kernels_gradnorm.cu) ---------
 // A norm group is a run of updater segments: one layer's segments, or one segment.  Its chunks are [chunk_begin, chunk_end) of the updater's

@@ -1,6 +1,7 @@
 // kernels_dropout.cu -- DropoutLayer (DL4J 1.0.0-beta3 inverted dropout): the masked forward with its on-device Philox4x32-10 mask and
 // pass counter, and the backward that applies the stored mask.  Mask definition: include/b200gan.h (B2G_LAYER_DROPOUT); oracle restatement:
-// tests/dropout_ref.py dropout_mask.
+// tests/dropout_ref.py dropout_mask.  Below them, the other IDropout kinds of a DropoutLayer (GaussianDropout, GaussianNoise, AlphaDropout,
+// SpatialDropout; include/b200gan.h b2g_dropout_kind) from the same Philox stream and pass counter.
 //
 // A translation unit of its own: compiled inside kernels_ew.cu these kernels changed the code nvcc generated for the updater kernel there
 // (register allocation and scheduling of the unchanged source), and the C2 step, which has no DropoutLayer, ran about 1% slower on an H100.
@@ -106,6 +107,247 @@ void k_dropout_bwd(int prec, const void* eo, void* ei, const uint32_t* mask, siz
   const int vec = aligned16(eo, ei) ? 1 : 0;
   DISPATCH_PREC(prec, T, (launch_pdl(dropout_bwd_kernel<T>, dim3(ew_blocks((n + 16 / sizeof(T) - 1) / (16 / sizeof(T)))), dim3(256), (size_t)0, s,
                                      (const T*)eo, (T*)ei, mask, n, scale, vec))); LAUNCHED();
+}
+
+// ---- GaussianDropout, GaussianNoise, AlphaDropout, SpatialDropout, and scheduled Dropout (b2g_dropout_kind) ---------------------------------
+// The vector loops take one 16-byte vector per thread and iteration: one Philox call per 4 elements and one Box-Muller per 2.  The tails run
+// one element per thread.  The per-element masks are written the way dropout_fwd_kernel writes them (a warp assembles whole words).
+
+// Box-Muller of one Philox word pair (include/b200gan.h b2g_dropout_kind): u and v are exact, so the draw depends only on logf / sqrtf / sincospif
+__device__ __forceinline__ void box_muller(uint32_t xe, uint32_t xo, float& ze, float& zo) {
+  const float u = ((float)(xe >> 9) + 0.5f) * 0x1p-23f, v = (float)(xo >> 8) * 0x1p-24f;
+  const float r = sqrtf(-2.0f * logf(u));
+  float sn, cs; sincospif(2.0f * v, &sn, &cs);
+  ze = r * cs; zo = r * sn;
+}
+__device__ __forceinline__ void normals4(const Philox4& r, float (&z)[4]) { box_muller(r.x[0], r.x[1], z[0], z[1]); box_muller(r.x[2], r.x[3], z[2], z[3]); }
+__device__ __forceinline__ float normal1(const Philox4& r, unsigned j) {
+  float ze, zo; box_muller(pick4(r, j & 2u), pick4(r, (j & 2u) + 1u), ze, zo);
+  return (j & 1u) ? zo : ze;
+}
+// GaussianNoise: y = x + sigma z;  GaussianDropout: y = x * m, m = 1 + sigma z (also its backward, with x = dy)
+template <int K> __device__ __forceinline__ float gauss_apply(float x, float z, float sigma) {
+  if (K == DROP_GAUSSIAN_NOISE) return fmaf(sigma, z, x);
+  return x * fmaf(sigma, z, 1.0f);
+}
+// the pass counter bump of dropout_fwd_kernel: the last block to finish advances *pass
+__device__ __forceinline__ void bump_pass_counter(unsigned long long* pass, unsigned* ticket, unsigned long long P) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    const unsigned done = atomicAdd(ticket, 1u);
+    if (done == gridDim.x - 1) { *pass = P + 1; *ticket = 0u; __threadfence(); }
+  }
+}
+// A scheduled layer's constants (NoiseSched): the forward evaluates the schedule, clamps the value and records it; the backward reads the record
+template <int K> __device__ __forceinline__ void scheduled_args(NoiseArgs& a, const NoiseSched& q, NoiseRec* rec, int bwd) {
+  if (!q.sched) return;
+  const float v = bwd ? rec->v : noise_clamp(K, sched_lr(*q.sched, a.value, *q.step, (long long)*q.epoch));
+  noise_derive(K, v, a);
+  if (!bwd && blockIdx.x == 0 && threadIdx.x == 0) rec->v = v;
+}
+
+// Forward of GaussianNoise / GaussianDropout and GaussianDropout's backward (bwd = 1: P and the value from *rec, no bump)
+template <typename T, int K>
+__global__ void __launch_bounds__(256) gauss_kernel(const T* x, T* y, size_t n, int vec, NoiseArgs a, const NoiseSched q, unsigned long long* pass,
+                                                    NoiseRec* rec, unsigned* ticket, int bump, int bwd) { pdl_enter();
+  constexpr int V = 16 / sizeof(T);
+  const unsigned long long P = bwd ? rec->P : *(volatile unsigned long long*)pass;
+  scheduled_args<K>(a, q, rec, bwd);
+  const uint32_t c1 = (uint32_t)P, c2 = (uint32_t)(P >> 32), k0 = (uint32_t)a.seed, k1 = (uint32_t)(a.seed >> 32);
+  const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
+  if (!bwd && tid == 0) rec->P = P;
+  const size_t nv = vec ? n / V : 0;
+  for (size_t i = tid; i < nv; i += stride) {
+    const size_t e0 = i * V;
+    float v[V]; ld16(x + e0, v);
+#pragma unroll
+    for (int h = 0; h < V / 4; ++h) {
+      float z[4]; normals4(philox4x32_10((uint32_t)(e0 >> 2) + h, c1, c2, a.tag, k0, k1), z);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) v[4 * h + j] = gauss_apply<K>(v[4 * h + j], z[j], a.scale);
+    }
+    st16(y + e0, v);
+  }
+  for (size_t e = nv * V + tid; e < n; e += stride)
+    stf(y, e, gauss_apply<K>(ldf(x, e), normal1(philox4x32_10((uint32_t)(e >> 2), c1, c2, a.tag, k0, k1), (unsigned)(e & 3)), a.scale));
+  if (bump) bump_pass_counter(pass, ticket, P);
+}
+
+// Per-element Bernoulli forward: Dropout's y = keep ? x * (1/p) : 0 (scheduled Dropout) or AlphaDropout's y = fmaf(a, keep ? x : a', b), the
+// keep bits into mask as dropout_fwd_kernel writes them
+template <int K> __device__ __forceinline__ float bern_apply(float x, bool keep, const NoiseArgs& a) {
+  if (K == DROP_ALPHA) return fmaf(a.scale, keep ? x : a.fill, a.shift);
+  return keep ? x * a.scale : 0.f;
+}
+template <typename T, int K>
+__global__ void __launch_bounds__(256) bern_fwd_kernel(const T* __restrict__ x, T* __restrict__ y, uint32_t* __restrict__ mask, size_t n, int vec,
+                                                       NoiseArgs a, const NoiseSched q, NoiseRec* rec, unsigned long long* pass, unsigned* ticket, int bump) { pdl_enter();
+  constexpr int V = 16 / sizeof(T);
+  const unsigned long long P = *(volatile unsigned long long*)pass;
+  scheduled_args<K>(a, q, rec, 0);
+  const uint32_t c1 = (uint32_t)P, c2 = (uint32_t)(P >> 32), k0 = (uint32_t)a.seed, k1 = (uint32_t)(a.seed >> 32);
+  const int lane = threadIdx.x & 31;
+  const size_t warp = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((size_t)gridDim.x * blockDim.x) >> 5;
+  const size_t n_main = vec ? n / (32 * V) * (32 * V) : 0;
+  for (size_t base = warp * 32 * V; base < n_main; base += nwarps * 32 * V) {
+    const size_t e0 = base + (size_t)lane * V;
+    float v[V]; ld16(x + e0, v);
+    uint32_t bits = 0;
+#pragma unroll
+    for (int h = 0; h < V / 4; ++h) {
+      const Philox4 r = philox4x32_10((uint32_t)(e0 >> 2) + h, c1, c2, a.tag, k0, k1);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const bool keep = a.keep_all || r.x[j] < a.threshold;
+        bits |= (uint32_t)keep << (4 * h + j); v[4 * h + j] = bern_apply<K>(v[4 * h + j], keep, a);
+      }
+    }
+    st16(y + e0, v);
+    uint32_t w = bits << ((lane * V) & 31);
+#pragma unroll
+    for (int o = 1; o < 32 / V; o <<= 1) w |= __shfl_xor_sync(0xffffffffu, w, o);
+    if ((lane & (32 / V - 1)) == 0) mask[e0 >> 5] = w;
+  }
+  for (size_t base = n_main + warp * 32; base < n; base += nwarps * 32) {
+    const size_t e = base + lane;
+    bool keep = false;
+    if (e < n) {
+      const Philox4 r = philox4x32_10((uint32_t)(e >> 2), c1, c2, a.tag, k0, k1);
+      keep = a.keep_all || pick4(r, (unsigned)(e & 3)) < a.threshold;
+      stf(y, e, bern_apply<K>(ldf(x, e), keep, a));
+    }
+    const uint32_t w = __ballot_sync(0xffffffffu, keep);
+    if (lane == 0) mask[base >> 5] = w;
+  }
+  if (bump) bump_pass_counter(pass, ticket, P);
+}
+
+// SpatialDropout: one keep bit per (row, channel), j = row * C + c.  The forward writes the R*C-bit mask (one word per thread and iteration,
+// 8 Philox calls) and applies the keep bits to the elements, drawing them again per element (one Philox call per 4 consecutive j).
+// (row, pixel, channel) of a vector's first element is divided out once and then stepped.
+struct SpatialPos {
+  size_t row; int pix, c;
+  __device__ __forceinline__ SpatialPos(size_t e, int hw, int C) { const size_t per = (size_t)hw * C, q = e % per; row = e / per; pix = (int)(q / C); c = (int)(q % C); }
+  __device__ __forceinline__ size_t j(int C) const { return row * C + c; }
+  __device__ __forceinline__ void next(int hw, int C) { if (++c == C) { c = 0; if (++pix == hw) { pix = 0; ++row; } } }
+};
+template <typename T>
+__global__ void __launch_bounds__(256) spatial_fwd_kernel(const T* __restrict__ x, T* __restrict__ y, uint32_t* __restrict__ mask, size_t n, int vec,
+                                                          NoiseArgs a, const NoiseSched q, NoiseRec* rec, unsigned long long* pass, unsigned* ticket, int bump) { pdl_enter();
+  constexpr int V = 16 / sizeof(T);
+  const unsigned long long P = *(volatile unsigned long long*)pass;
+  scheduled_args<DROP_SPATIAL>(a, q, rec, 0);
+  const uint32_t c1 = (uint32_t)P, c2 = (uint32_t)(P >> 32), k0 = (uint32_t)a.seed, k1 = (uint32_t)(a.seed >> 32);
+  const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
+  const size_t nj = n / ((size_t)a.hw * a.C) * a.C, nwords = (nj + 31) / 32;
+  for (size_t wd = tid; wd < nwords; wd += stride) {
+    uint32_t w = 0;
+#pragma unroll
+    for (int h = 0; h < 8; ++h) {
+      const size_t g = wd * 8 + h;
+      if (4 * g >= nj) break;
+      const Philox4 r = philox4x32_10((uint32_t)g, c1, c2, a.tag, k0, k1);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) w |= (uint32_t)(a.keep_all || r.x[j] < a.threshold) << (4 * h + j);
+    }
+    if (nj - wd * 32 < 32) w &= (1u << (nj - wd * 32)) - 1u;
+    mask[wd] = w;
+  }
+  const size_t nv = vec ? n / V : 0;
+  for (size_t i = tid; i < nv; i += stride) {
+    const size_t e0 = i * V;
+    float v[V]; ld16(x + e0, v);
+    SpatialPos sp(e0, a.hw, a.C);
+    size_t g = ~(size_t)0; Philox4 r{};
+#pragma unroll
+    for (int k = 0; k < V; ++k) {
+      const size_t j = sp.j(a.C);
+      if ((j >> 2) != g) { g = j >> 2; r = philox4x32_10((uint32_t)g, c1, c2, a.tag, k0, k1); }
+      const bool keep = a.keep_all || pick4(r, (unsigned)(j & 3)) < a.threshold;
+      v[k] = keep ? v[k] * a.scale : 0.f;
+      sp.next(a.hw, a.C);
+    }
+    st16(y + e0, v);
+  }
+  for (size_t e = nv * V + tid; e < n; e += stride) {
+    const size_t j = SpatialPos(e, a.hw, a.C).j(a.C);
+    const bool keep = a.keep_all || pick4(philox4x32_10((uint32_t)(j >> 2), c1, c2, a.tag, k0, k1), (unsigned)(j & 3)) < a.threshold;
+    stf(y, e, keep ? ldf(x, e) * a.scale : 0.f);
+  }
+  if (bump) bump_pass_counter(pass, ticket, P);
+}
+// Backward of the mask kinds: dx = dy * scale where the forward kept, 0 elsewhere (scale: 1/p, AlphaDropout's a); mask bit j = e, or
+// j = row * C + c for SpatialDropout
+template <typename T, int K>
+__global__ void __launch_bounds__(256) mask_bwd_kernel(const T* eo, T* ei, const uint32_t* __restrict__ mask, size_t n, int vec, NoiseArgs a,
+                                                       const NoiseSched q, NoiseRec* rec) { pdl_enter();
+  constexpr int V = 16 / sizeof(T);
+  scheduled_args<K>(a, q, rec, 1);
+  const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
+  const size_t nv = vec ? n / V : 0;
+  for (size_t i = tid; i < nv; i += stride) {
+    const size_t e0 = i * V;
+    float v[V]; ld16(eo + e0, v);
+    if (K == DROP_SPATIAL) {
+      SpatialPos sp(e0, a.hw, a.C);
+#pragma unroll
+      for (int k = 0; k < V; ++k) { const size_t j = sp.j(a.C); v[k] = ((mask[j >> 5] >> (j & 31)) & 1u) ? v[k] * a.scale : 0.f; sp.next(a.hw, a.C); }
+    } else {
+      const uint32_t bits = mask[e0 >> 5] >> (e0 & 31);
+#pragma unroll
+      for (int k = 0; k < V; ++k) v[k] = ((bits >> k) & 1u) ? v[k] * a.scale : 0.f;
+    }
+    st16(ei + e0, v);
+  }
+  for (size_t e = nv * V + tid; e < n; e += stride) {
+    const size_t j = K == DROP_SPATIAL ? SpatialPos(e, a.hw, a.C).j(a.C) : e;
+    stf(ei, e, ((mask[j >> 5] >> (j & 31)) & 1u) ? ldf(eo, e) * a.scale : 0.f);
+  }
+}
+__global__ void noise_value_kernel(int kind, float value, const NoiseSched q, float* out) {
+  if (threadIdx.x || blockIdx.x) return;
+  float v = value;
+  if (q.sched) {
+    v = sched_lr(*q.sched, value, *q.step, (long long)*q.epoch);
+    v = kind == DROP_GAUSSIAN_DROPOUT ? noise_clamp(DROP_GAUSSIAN_DROPOUT, v) : kind == DROP_GAUSSIAN_NOISE ? noise_clamp(DROP_GAUSSIAN_NOISE, v) : noise_clamp(DROP_ALPHA, v);
+  }
+  *out = v;
+}
+
+void k_noise_fwd(int prec, int kind, const void* x, void* y, uint32_t* mask, NoiseRec* rec, size_t n, const NoiseArgs& a, const NoiseSched& q,
+                 unsigned long long* pass, unsigned* ticket, int bump_pass, cudaStream_t s) {
+  if (!n) return;
+  const int vec = aligned16(x, y) ? 1 : 0;
+  DISPATCH_PREC(prec, T, {
+    const dim3 grid(ew_blocks((n + 16 / sizeof(T) - 1) / (16 / sizeof(T))));
+    switch (kind) {
+      case DROP_GAUSSIAN_DROPOUT: launch_pdl(gauss_kernel<T, DROP_GAUSSIAN_DROPOUT>, grid, dim3(256), (size_t)0, s, (const T*)x, (T*)y, n, vec, a, q, pass, rec, ticket, bump_pass, 0); break;
+      case DROP_GAUSSIAN_NOISE: launch_pdl(gauss_kernel<T, DROP_GAUSSIAN_NOISE>, grid, dim3(256), (size_t)0, s, (const T*)x, (T*)y, n, vec, a, q, pass, rec, ticket, bump_pass, 0); break;
+      case DROP_ALPHA: launch_pdl(bern_fwd_kernel<T, DROP_ALPHA>, grid, dim3(256), (size_t)0, s, (const T*)x, (T*)y, mask, n, vec, a, q, rec, pass, ticket, bump_pass); break;
+      case DROP_BERNOULLI: launch_pdl(bern_fwd_kernel<T, DROP_BERNOULLI>, grid, dim3(256), (size_t)0, s, (const T*)x, (T*)y, mask, n, vec, a, q, rec, pass, ticket, bump_pass); break;
+      default: launch_pdl(spatial_fwd_kernel<T>, grid, dim3(256), (size_t)0, s, (const T*)x, (T*)y, mask, n, vec, a, q, rec, pass, ticket, bump_pass); break;
+    }
+  }); LAUNCHED();
+}
+void k_noise_bwd(int prec, int kind, const void* eo, void* ei, const uint32_t* mask, const NoiseRec* rec, size_t n, const NoiseArgs& a, const NoiseSched& q,
+                 cudaStream_t s) {
+  if (!n || kind == DROP_GAUSSIAN_NOISE) return;
+  const int vec = aligned16(eo, ei) ? 1 : 0;
+  NoiseRec* r = const_cast<NoiseRec*>(rec);
+  DISPATCH_PREC(prec, T, {
+    const dim3 grid(ew_blocks((n + 16 / sizeof(T) - 1) / (16 / sizeof(T))));
+    switch (kind) {
+      case DROP_GAUSSIAN_DROPOUT: launch_pdl(gauss_kernel<T, DROP_GAUSSIAN_DROPOUT>, grid, dim3(256), (size_t)0, s, (const T*)eo, (T*)ei, n, vec, a, q,
+                                             (unsigned long long*)nullptr, r, (unsigned*)nullptr, 0, 1); break;
+      case DROP_ALPHA: launch_pdl(mask_bwd_kernel<T, DROP_ALPHA>, grid, dim3(256), (size_t)0, s, (const T*)eo, (T*)ei, mask, n, vec, a, q, r); break;
+      case DROP_BERNOULLI: launch_pdl(mask_bwd_kernel<T, DROP_BERNOULLI>, grid, dim3(256), (size_t)0, s, (const T*)eo, (T*)ei, mask, n, vec, a, q, r); break;
+      default: launch_pdl(mask_bwd_kernel<T, DROP_SPATIAL>, grid, dim3(256), (size_t)0, s, (const T*)eo, (T*)ei, mask, n, vec, a, q, r); break;
+    }
+  }); LAUNCHED();
+}
+void k_noise_value(int kind, float value, const NoiseSched& q, float* out, cudaStream_t s) {
+  noise_value_kernel<<<1, 32, 0, s>>>(kind, value, q, out); LAUNCHED();
 }
 
 }  // namespace b2g

@@ -977,24 +977,6 @@ __device__ __forceinline__ float upd_elem(const UpdSeg& sg, float g, float p, fl
   if (sg.l2 != 0.f) u = fmaf(sg.l2, p, u);
   return p - u;
 }
-// The learning rate of a segment at iteration `it` (the counter before this update's increment) / epoch `ep`: DL4J's ISchedule.valueAt in
-// double, rounded to fp32 once (include/b200gan.h, b2g_lr_schedule); kind 0 = the constant lr.
-__device__ float sched_lr(const UpdSched& sc, float lr, int it, long long ep) {
-  if (sc.kind == 0) return lr;
-  const long long ii = sc.type == 1 ? ep : (long long)it;
-  const double i = (double)ii;
-  double v;
-  if (sc.kind == 1) v = sc.initial * pow(sc.gamma, i);
-  else if (sc.kind == 2) v = sc.initial / pow(1.0 + sc.gamma * i, sc.power);
-  else if (sc.kind == 3) v = sc.initial / (1.0 + exp(-sc.gamma * (i - sc.step)));
-  else if (sc.kind == 4) v = sc.initial * pow(sc.decay, floor(i / sc.step));
-  else {          // MAP: the largest key <= i (keys strictly increase, keys[0] <= 0 <= i)
-    int lo = 0, hi = sc.n_map - 1;
-    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if ((long long)sc.keys[mid] <= ii) lo = mid; else hi = mid - 1; }
-    v = sc.vals[lo];
-  }
-  return (float)v;
-}
 // SCHED: the segment's lr comes from its schedule (thread 0 evaluates it once per block, at *step before the increment or at *epoch)
 // EXT: kinds 4-9 (upd_elem); st2 (AMSGrad's v-hat, allocated only for nets with an AMSGrad segment) is read by EXT instantiations only
 template <bool SCALED, bool SCHED, bool EXT>

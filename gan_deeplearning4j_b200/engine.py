@@ -205,6 +205,25 @@ def resolve_vertices(specs: Sequence[Dict]) -> List[Optional[tuple]]:
     return out
 
 
+# IDropout of a "dropout" spec (b2g_dropout_kind in include/b200gan.h): kind -> (code, the key of its value).  No "kind": Dropout(p).
+DROPOUT_KINDS = {"dropout": (0, "p"), "gaussian_dropout": (1, "rate"), "gaussian_noise": (2, "stddev"), "alpha_dropout": (3, "p"),
+                 "spatial_dropout": (4, "p")}
+
+
+def dropout_kind_value(spec: Dict):
+    """(b2g_dropout_kind code, value) of a "dropout" spec; the value is the retain probability p, the rate or the stddev: a number, or a
+    schedule dict (new GaussianNoise(ISchedule)) whose value at 0 the desc carries, as for a scheduled lr; the schedule is set after creation."""
+    kind = spec.get("kind", "dropout")
+    if kind not in DROPOUT_KINDS:
+        raise ValueError(f"dropout layer {spec.get('name', '')!r}: unknown kind {kind!r}; one of {sorted(DROPOUT_KINDS)}")
+    code, key = DROPOUT_KINDS[kind]
+    return code, constant_lr(spec[key])
+
+
+def dropout_value_key(spec: Dict) -> str:
+    return DROPOUT_KINDS[spec.get("kind", "dropout")][1]
+
+
 def layer_desc(spec: Dict, skip: Optional[tuple] = None) -> LayerDesc:
     """skip: the vertex's (j, order) from resolve_vertices."""
     d = LayerDesc()
@@ -219,8 +238,8 @@ def layer_desc(spec: Dict, skip: Optional[tuple] = None) -> LayerDesc:
     act = spec.get("activation", "identity")
     d.act = ACTS[act]
     d.act_alpha = spec.get("alpha", ACT_ALPHA_DEFAULTS.get(act, 0.01))
-    if spec["type"] == "dropout":       # DropoutLayer.Builder(p): p = retain probability, carried in act_alpha
-        d.act_alpha = spec["p"]
+    if spec["type"] == "dropout":       # DropoutLayer.Builder(IDropout): the b2g_dropout_kind in act, its value in act_alpha
+        d.act, d.act_alpha = dropout_kind_value(spec)
     if spec["type"] in ("subsampling", "global_pooling"):      # the pooling kind in act, PNORM's p in act_alpha (0 = none given: refused)
         d.act = POOLINGS[spec.get("pooling", "max")]
         d.act_alpha = float(spec.get("pnorm", GLOBAL_PNORM_DEFAULT if spec["type"] == "global_pooling" else 0))
@@ -345,6 +364,10 @@ class Net:
             for sp in self.specs:
                 if sp.get("constraints"):
                     self._push_constraints(sp, {})
+            self.dropout_constants = {sp["name"]: dropout_kind_value(sp)[1] for sp in self.specs if sp["type"] == "dropout" and sp.get("name")}
+            for sp in self.specs:         # new GaussianNoise(ISchedule) and the other IDropout schedule constructors
+                if sp["type"] == "dropout" and is_schedule(sp[dropout_value_key(sp)]):
+                    self.set_dropout_schedule(sp[dropout_value_key(sp)], sp["name"])
         except Exception:
             self.close()
             raise
@@ -475,6 +498,24 @@ class Net:
     def apply_constraints(self):
         """Model.applyConstraints: every constraint of the net once, now (the updates apply them by themselves)."""
         check(self.lib.b2g_net_apply_constraints(self.h))
+
+    def set_dropout_schedule(self, schedule: Optional[Dict], layer: Optional[str] = None):
+        """An ISchedule in place of a DropoutLayer's value (p, rate or stddev; b2g_net_set_dropout_schedule): layer None = every non-frozen
+        DropoutLayer; schedule None = back to the value from creation.  The specs a checkpoint writes follow."""
+        s, _arrays = schedule_struct(schedule)
+        check(self.lib.b2g_net_set_dropout_schedule(self.h, None if layer is None else layer.encode(), C.byref(s)))
+        for sp in self.specs:
+            if sp["type"] != "dropout" or (layer is None and sp.get("frozen", False)) or (layer is not None and sp.get("name") != layer):
+                continue
+            sp[dropout_value_key(sp)] = copy.deepcopy(schedule) if schedule is not None else self.dropout_constants[sp["name"]]
+            if layer is not None:
+                break
+
+    def dropout_value(self, layer: str) -> float:
+        """The value (p, rate or stddev) the DropoutLayer's next train-mode forward uses, evaluated and clamped on the device."""
+        v = C.c_float()
+        check(self.lib.b2g_net_get_dropout_value(self.h, layer.encode(), C.byref(v)))
+        return v.value
 
     def learning_rate(self, layer: str) -> float:
         """ComputationGraph.getLearningRate(layer): the fp32 learning rate the layer's next update uses (before Adam's bias correction),
@@ -695,6 +736,16 @@ def test_bn(ctx: Context, precision: int, path: int, x, eps_out, gamma, beta, ru
     check(ctx.lib.b2g_test_bn(ctx.h, precision, path, groups, rows, ch, _fp(x), _fp(e), *[_fp(v) for v in par], ACTS[act], alpha, eps, decay,
                               int(want_param_grads), *[_fp(r[k]) for k in ("y", "eps_in", "g_gamma", "g_beta", "g_mean", "g_var", "mean", "invstd")]))
     return r
+
+
+def test_dropout_kind(ctx: Context, precision: int, kind: str, x, dy, value: float, *, seed: int = 666, layer: int = 0, rank: int = 0, pass_: int = 0):
+    """One DropoutLayer forward and backward of an IDropout kind (a DROPOUT_KINDS name) and its value (b2g_test_dropout_kind); as test_dropout."""
+    x, e = _f32(x), _f32(dy)
+    rows = x.shape[0]
+    h, w, c = (x.shape[1:] if x.ndim == 4 else (1, 1, int(np.prod(x.shape[1:]))))
+    y, dx = np.empty_like(x), np.empty_like(x)
+    check(ctx.lib.b2g_test_dropout_kind(ctx.h, precision, DROPOUT_KINDS[kind][0], seed, layer, rank, pass_, rows, h, w, c, value, _fp(x), _fp(e), _fp(y), _fp(dx)))
+    return y, dx
 
 
 def test_dropout(ctx: Context, precision: int, x, dy, p: float, *, seed: int = 666, layer: int = 0, rank: int = 0, pass_: int = 0):

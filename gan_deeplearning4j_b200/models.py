@@ -110,6 +110,33 @@ def non_negative(on="weights") -> Dict:
     return {"constraint": "non_negative", "on": on}
 
 
+# ------------------------------------------------------------------ IDropout kinds of a DropoutLayer ---------------------
+# DropoutLayer.Builder(IDropout) (b2g_dropout_kind in include/b200gan.h); a "dropout" spec without "kind" is DropoutLayer.Builder(p).  Each value
+# may be a schedule (exponential_schedule, ...): new GaussianNoise(ISchedule), evaluated on the device at every train-mode forward.
+def _value(v):
+    return v if isinstance(v, dict) else float(v)
+
+
+def gaussian_noise(stddev, name="") -> Dict:
+    """new DropoutLayer.Builder(new GaussianNoise(stddev)): y = x + stddev * N(0, 1) in training."""
+    return {"type": "dropout", "name": name, "kind": "gaussian_noise", "stddev": _value(stddev)}
+
+
+def gaussian_dropout(rate, name="") -> Dict:
+    """new DropoutLayer.Builder(new GaussianDropout(rate)): y = x * (1 + sqrt(rate / (1 - rate)) * N(0, 1)) in training."""
+    return {"type": "dropout", "name": name, "kind": "gaussian_dropout", "rate": _value(rate)}
+
+
+def alpha_dropout(p, name="") -> Dict:
+    """new DropoutLayer.Builder(new AlphaDropout(p)), p = the retain probability: the dropout that keeps SELU's mean and variance."""
+    return {"type": "dropout", "name": name, "kind": "alpha_dropout", "p": _value(p)}
+
+
+def spatial_dropout(p, name="") -> Dict:
+    """new DropoutLayer.Builder(new SpatialDropout(p)), p = the retain probability: whole (example, channel) maps kept or zeroed."""
+    return {"type": "dropout", "name": name, "kind": "spatial_dropout", "p": _value(p)}
+
+
 # ------------------------------------------------------------------ pooling layers ---------------------
 # SubsamplingLayer / GlobalPoolingLayer (b2g_pooling in include/b200gan.h).  SubsamplingLayer(MAX) is the "maxpool" spec (unpadded).
 def subsampling(pooling, kernel=(1, 1), stride=(2, 2), padding=(0, 0), pnorm=None, name="") -> Dict:
@@ -298,7 +325,7 @@ def _loss_keys(loss, out_activation) -> Dict:
 
 
 def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", out_activation="identity", activation="lrelu", alpha=None,
-                        global_pooling=None, patch=False, residual=False) -> List[Dict]:
+                        global_pooling=None, patch=False, residual=False, instance_noise=None) -> List[Dict]:
     """Conv(4x4 s2 p1)+LeakyReLU(0.2); (Conv+BatchNorm+LeakyReLU)*; Conv(4x4 s1 p0) -> logit; LossLayer(loss).  Input (nc,size,size).
     loss: "xent" (sigmoid implied), or "mse" (least-squares GAN), "hinge", "wasserstein", ... applied to out_activation(logit).
     activation / alpha: the hidden activation in place of LeakyReLU(0.2) (as in _act).
@@ -307,7 +334,8 @@ def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", o
     patch: a PatchGAN critic -- the down-sampling stages stop at the max(4, size/16) map (at most four stride-2 convs), and a 3x3 s1 p1 conv onto
     1 channel and a CnnLossLayer(loss) take the place of the last conv and its LossLayer: one logit and one label per patch (a 4x4 map up to
     64x64, 8x8 at 128x128).
-    residual: one identity residual_block after each down-sampling stage (a ResNet-style critic)."""
+    residual: one identity residual_block after each down-sampling stage (a ResNet-style critic).
+    instance_noise = stddev: a GaussianNoise(stddev) DropoutLayer on the input (instance noise: real and fake images both get the noise)."""
     if patch and global_pooling is not None:
         raise ValueError("patch and global_pooling are two different heads")
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
@@ -315,7 +343,8 @@ def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", o
     if patch:
         n_down = min(n_down, 4)
     block = lambda k, c, skip: residual_block(f"dis_res_{k}", c, skip, lr, beta1, activation, alpha) if residual else []
-    L = [{"type": "conv2d", "name": "dis_conv_1", "n_in": nc, "n_out": nf, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), **_act(activation, alpha), "updater": u()}]
+    L = [] if instance_noise is None else [gaussian_noise(instance_noise, name="dis_instance_noise")]
+    L += [{"type": "conv2d", "name": "dis_conv_1", "n_in": nc, "n_out": nf, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), **_act(activation, alpha), "updater": u()}]
     ch = nf
     L += block(1, ch, "dis_conv_1")
     for i in range(n_down - 1):
@@ -344,11 +373,12 @@ def mlp_generator(z=100, hidden=1024, d=256, lr=2e-4, beta1=0.5, activation="rel
 
 
 def mlp_discriminator(d=256, hidden=1024, lr=2e-4, beta1=0.5, dropout=None, loss="xent", out_activation="identity", activation="lrelu",
-                      alpha=None) -> List[Dict]:
+                      alpha=None, instance_noise=None) -> List[Dict]:
     """dropout = p: a DropoutLayer(p) (p = retain probability) after each hidden LeakyReLU, the DL4J MNIST GAN example's discriminator shape.
-    loss / out_activation: the OutputLayer's loss, as for dcgan_discriminator.  activation / alpha: the hidden activation (as in _act)."""
+    loss / out_activation: the OutputLayer's loss, as for dcgan_discriminator.  activation / alpha: the hidden activation (as in _act).
+    instance_noise = stddev: a GaussianNoise(stddev) DropoutLayer on the input, as for dcgan_discriminator."""
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
-    L = []
+    L = [] if instance_noise is None else [gaussian_noise(instance_noise, name="dis_instance_noise")]
     for i in (1, 2):
         L.append({"type": "dense", "name": f"dis_dense_{i}", "n_out": hidden, **_act(activation, alpha), "updater": u()})
         if dropout is not None:

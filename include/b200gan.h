@@ -113,7 +113,36 @@ typedef enum {
  * P is a 64-bit word in device memory, 0 at b2g_net_create.  Every train-mode forward of a net with at least one masking DropoutLayer
  * (train, not frozen, p < 1) uses the current P for all of them and then advances P by 1 on the device (so a replayed CUDA graph draws new
  * masks); other forwards leave it unchanged.  In the GAN step D's real|fake pass (2N rows) uses P and the generator step's D pass P + 1.
- * A pass may hold at most 2^34 elements (max_batch * layer size; B2G_ERR_UNSUPPORTED at b2g_net_create). */
+ * A pass may hold at most 2^34 elements (max_batch * layer size; B2G_ERR_UNSUPPORTED at b2g_net_create).
+ * The rest of this comment is b2g_dropout_kind: the other IDropout kinds of a DropoutLayer. */
+
+/* The IDropout of a B2G_LAYER_DROPOUT layer (DL4J 1.0.0-beta3, recalled; parity unpinned like the rest of the DL4J semantics).  The kind is
+ * carried in b2g_layer_desc.act (a DropoutLayer has no activation), its value in act_alpha:
+ *   DROPOUT           retain probability p in (0, 1]      as above (B2G_LAYER_DROPOUT)
+ *   GAUSSIAN_DROPOUT  rate in [0, 1)                      y = x * m, m = fmaf(s, z, 1.0f), s = sqrt(rate / (1 - rate)) in double, then fp32;
+ *                                                         dx = dy * m, m drawn again from the forward's (S, r, L, P, e): no noise buffer
+ *   GAUSSIAN_NOISE    stddev s >= 0, finite               y = fmaf(s, z, x);  dx = dy (no launch)
+ *   ALPHA_DROPOUT     retain probability p in (0, 1]      y = fmaf(a, keep ? x : a', b);  dx = keep ? dy * a : 0;  a' = -lambda * alpha
+ *                                                         (SELU's alpha = 1.6732632423543772, lambda = 1.0507009873554805), a = 1 / sqrt(p +
+ *                                                         a'^2 p (1 - p)), b = -a (1 - p) a', each computed in double and rounded to fp32 once
+ *   SPATIAL_DROPOUT   retain probability p in (0, 1]      Dropout's x * (1/p) or +0 with one keep bit per (row, channel) of a [rows][H][W][C] map
+ * Another kind or a value outside its range is B2G_ERR_ARG at b2g_net_create; SPATIAL_DROPOUT on a 1 x 1 map (a feed-forward input) is
+ * B2G_ERR_SHAPE.  Train mode only, in fp32 from the stored activation, each result rounded once to the activation type.
+ * Draws: the Philox4x32-10 words of B2G_LAYER_DROPOUT with the counter word j >> 2, where j = e (the element's NHWC index in the pass) for
+ * every kind except SPATIAL_DROPOUT, and j = row * C + c for it.  The Bernoulli kinds keep where x[j & 3] < floor(p * 2^32), p >= 1 keeps all.
+ * The Gaussian kinds turn the four words of one counter into four normals, pair (x0, x1) into z0, z1 and pair (x2, x3) into z2, z3; element e
+ * takes z[e & 3].  In fp32, with IEEE sqrtf and the library's logf / sincospif (no fast-math):
+ *   u = ((x_even >> 9) + 0.5f) * 2^-23 (exact, in [2^-24, 1)),  v = (x_odd >> 8) * 2^-24 (exact),  r = sqrtf(-2 logf(u)),
+ *   sincospif(2v, &s, &c),  z_even = r * c,  z_odd = r * s.
+ * So |z| <= sqrt(-2 ln 2^-24), about 5.8: a truncated normal, a documented deviation (DL4J draws from its own generator).
+ * Identity cases launch nothing, report their input as their activation and do not count as a masking pass for P: inference, a FrozenLayer,
+ * p = 1, rate = 0 and stddev = 0.  Every other train-mode DropoutLayer of any kind is stochastic: the pass uses one P for all of them and the
+ * last one's forward advances it.  Buffers: DROPOUT and ALPHA_DROPOUT keep one bit per element, SPATIAL_DROPOUT one per (row, channel),
+ * GAUSSIAN_DROPOUT the P of its latest forward (one device word, written by the forward, read by the backward), GAUSSIAN_NOISE nothing.
+ * Any kind, Dropout included, may take a schedule in place of its value: b2g_net_set_dropout_schedule. */
+typedef enum {
+  B2G_DROPOUT = 0, B2G_DROPOUT_GAUSSIAN_DROPOUT = 1, B2G_DROPOUT_GAUSSIAN_NOISE = 2, B2G_DROPOUT_ALPHA = 3, B2G_DROPOUT_SPATIAL = 4
+} b2g_dropout_kind;
 
 /* org.deeplearning4j.nn.conf.layers.PoolingType of SUBSAMPLING and GLOBAL_POOLING layers (DL4J 1.0.0-beta3, recalled; parity unpinned like the
  * rest of the DL4J semantics).  The kind is carried in b2g_layer_desc.act (pooling layers have no activation), PNORM's p in act_alpha: a whole
@@ -246,9 +275,9 @@ typedef struct {
   int32_t n_in, n_out;          /* channels / features (n_in may be 0 = infer, like setInputTypes) */
   int32_t k_h, k_w, s_h, s_w, p_h, p_w;   /* conv / deconv / pool geometry; upsample factor in k_h */
   int32_t has_bias;             /* hasBias(true) default */
-  int32_t act;                  /* b2g_activation; b2g_pooling on SUBSAMPLING / GLOBAL_POOLING layers */
+  int32_t act;                  /* b2g_activation; b2g_pooling on SUBSAMPLING / GLOBAL_POOLING layers; b2g_dropout_kind on DROPOUT layers */
   float act_alpha;              /* ActivationLReLU alpha: DL4J default 0.01, DCGAN passes 0.2; ELU alpha / ThresholdedReLU theta (DL4J 1.0);
-                                   DropoutLayer retain probability p; PNORM pooling's p */
+                                   DropoutLayer value (b2g_dropout_kind); PNORM pooling's p */
   int32_t updater;              /* b2g_updater; "frozen" in the reference = RMSPROP with lr 0 (J:84) */
   float lr, beta1, beta2, eps;  /* RmsProp: beta1 = rmsDecay (ctor order lr, rmsDecay, epsilon; J:133 passes 1e-8, 1e-8) */
   float l2;                     /* .l2(1e-4) (J:125): weights only, applied AFTER the updater, not lr-scaled */
@@ -424,6 +453,16 @@ int32_t b2g_net_set_lr_schedule(b2g_net* net, const char* layer, const b2g_lr_sc
 /* ComputationGraph.getLearningRate(String): the fp32 learning rate the layer's next update will use (before Adam's bias correction), computed
  * on the device by the function the updater kernel calls.  Sync point. */
 int32_t b2g_net_get_learning_rate(b2g_net* net, const char* layer, float* out);
+/* IDropout with an ISchedule in place of its constant (b2g_dropout_kind): layer NULL = every non-frozen DropoutLayer, else the named one
+ * (B2G_ERR_ARG if it is not a DropoutLayer); s NULL or kind NONE: back to the constant from b2g_net_create.  The schedule checks of
+ * b2g_net_set_lr_schedule apply.  Each train-mode forward evaluates it on the device, by the function the updater calls, at the owning net's
+ * iteration counter (before the update's increment) or epoch word -- in b2g_gan_step the generator step's pass through D at the generator's --
+ * and clamps the value into its kind's range (p to [2^-32, 1], rate to [0, 1 - 2^-24], stddev to >= 0; a documented deviation), then derives
+ * the kernels' constants from it; its backward uses the forward's value.  A scheduled layer is stochastic whatever its value.  Bumps the
+ * settings generation (a captured GAN step is re-captured); a replay reads the counters from device memory. */
+int32_t b2g_net_set_dropout_schedule(b2g_net* net, const char* layer, const b2g_lr_schedule* s);
+/* The value (p, rate or stddev) the named DropoutLayer's next train-mode forward uses, clamped, computed on the device.  Sync point. */
+int32_t b2g_net_get_dropout_value(b2g_net* net, const char* layer, float* out);
 /* ComputationGraph.getEpochCount / setEpochCount: the 64-bit device word EPOCH schedules read, 0 at b2g_net_create.  The host sets it, nothing
  * increments it; a new value takes effect at the next update, also in a replayed CUDA graph.  Sync points.  B2G_ERR_ARG for epoch < 0. */
 int32_t b2g_net_get_epoch(b2g_net* net, int64_t* out);
@@ -569,6 +608,11 @@ int32_t b2g_test_net_shadow(b2g_net* net, int32_t layer, int32_t which, float* o
  * B2G_LAYER_DROPOUT.  Out: y, dx (same order).  Fails unless the forward advanced its pass counter from pass to pass + 1. */
 int32_t b2g_test_dropout(b2g_ctx* ctx, int32_t precision, uint64_t seed, int32_t layer, int32_t rank, int64_t pass, int32_t rows, int32_t h, int32_t w,
                          int32_t c, float p, const float* x, const float* dy, float* y, float* dx);
+/* The same for a DropoutLayer of any b2g_dropout_kind with its value (p, rate or stddev; the ranges of b2g_dropout_kind, else B2G_ERR_ARG).
+ * An identity case (p = 1, rate = 0, stddev = 0) launches nothing and leaves the pass counter alone: y = x, dx = dy.  Otherwise it fails unless
+ * the forward advanced the pass counter from pass to pass + 1. */
+int32_t b2g_test_dropout_kind(b2g_ctx* ctx, int32_t precision, int32_t kind, uint64_t seed, int32_t layer, int32_t rank, int64_t pass, int32_t rows,
+                              int32_t h, int32_t w, int32_t c, float value, const float* x, const float* dy, float* y, float* dx);
 
 /* One reduction, loss or element-wise kernel of the training step on host tensors, through its production launch wrapper (tests).
  * T tensors are fp32 on the host, rounded to bf16 on the device when precision is BF16 and widened back on the way out; the others are fp32.

@@ -37,6 +37,8 @@ public final class Native {
     public static native int netSetConstraints(long net, long layerNameAddr, long paramNameAddr, long constraintsAddr, int n);   // b2g_constraint[n]
     public static native int netApplyConstraints(long net);
     public static native int netGetLearningRate(long net, long layerNameAddr, long outAddr);
+    public static native int netSetDropoutSchedule(long net, long layerNameAddr, long scheduleAddr);   // layerNameAddr 0: every DropoutLayer; scheduleAddr 0: constant
+    public static native int netGetDropoutValue(long net, long layerNameAddr, long outAddr);
     public static native int netGetEpoch(long net, long outAddr);
     public static native int netSetEpoch(long net, long epoch);
     public static native int netSimtGemmCalls(long net, long outAddr);

@@ -13,6 +13,7 @@ public class Layer {
     public int type, nIn, nOut, kH = 1, kW = 1, sH = 1, sW = 1, pH, pW, hasBias = 1, act = -1, preH, preW, preC, loss, frozen;
     public float alpha = 0.01f, l2 = Float.NaN, bnDecay = 0.9f, bnEps = 1e-5f;
     public IUpdater updater; public String name = "";
+    public org.nd4j.linalg.schedule.ISchedule dropSchedule;   // DropoutLayer.Builder(IDropout) with an ISchedule: applied by ComputationGraph.init
     /** constrainAllParameters / constrainWeights / constrainBias; all null: the global builder's lists apply. */
     public List<LayerConstraint> constrainAll, constrainW, constrainB;
     public boolean alphaSet;   // alpha given by leakyReluAlpha(..) or activation(IActivation); else ELU / ThresholdedReLU write DL4J's 1.0
@@ -28,7 +29,7 @@ public class Layer {
     }
     public Layer copy() { Layer c = new Layer(); c.type = type; c.nIn = nIn; c.nOut = nOut; c.kH = kH; c.kW = kW; c.sH = sH; c.sW = sW; c.pH = pH; c.pW = pW; c.hasBias = hasBias; c.act = act;
         c.preH = preH; c.preW = preW; c.preC = preC; c.loss = loss; c.frozen = frozen; c.alpha = alpha; c.l2 = l2; c.bnDecay = bnDecay; c.bnEps = bnEps; c.updater = updater; c.name = name; c.alphaSet = alphaSet;
-        c.constrainAll = constrainAll; c.constrainW = constrainW; c.constrainB = constrainB; return c; }
+        c.constrainAll = constrainAll; c.constrainW = constrainW; c.constrainB = constrainB; c.dropSchedule = dropSchedule; return c; }
     protected int defaultAct(Activation g) { return g.code; }   // conv / dense inherit the global .activation(..) (J:126)
 
     @SuppressWarnings("unchecked")

@@ -32,6 +32,8 @@ public class ComputationGraph {
         for (Layer l : layers)            // new Adam(ISchedule) / RmsProp(ISchedule) / Sgd(ISchedule): evaluated on the device at every update
             if (l.updater != null && l.updater.lrSchedule() != null && hasLearningRate(l)) setLearningRate(l.name, l.updater.lrSchedule());
         for (Layer l : layers) applyConstraints(l);
+        for (Layer l : layers)            // new GaussianNoise(ISchedule) etc.: evaluated on the device at every train-mode forward
+            if (l.type == 11 && l.dropSchedule != null) setDropoutSchedule(l.name, l.dropSchedule);
     }
     /** The parameters a constrainAllParameters / constrainWeights / constrainBias list reaches on a layer (the library's rule, include/b200gan.h
      *  b2g_constraint, and engine.py constraint_params): weights = W of conv, deconv, dense and output layers, nothing on BatchNorm; bias = b
@@ -83,7 +85,15 @@ public class ComputationGraph {
     /** setLearningRate(ISchedule): every layer whose updater has a learning rate, from the next update on (null: back to the constant lr). */
     public void setLearningRate(ISchedule s) { applySchedule(null, s); }
     public void setLearningRate(String layerName, ISchedule s) { applySchedule(layerName, s); }
-    private void applySchedule(String layerName, ISchedule s) {
+    /** An IDropout's ISchedule for one DropoutLayer (layerName null: every non-frozen DropoutLayer; s null: back to its constant). */
+    public void setDropoutSchedule(String layerName, ISchedule s) { applySchedule(layerName, s, true); }
+    /** The value (p, rate or stddev) the DropoutLayer's next train-mode forward uses. */
+    public double getDropoutValue(String layerName) {
+        ByteBuffer o = Native.direct(4); ByteBuffer name = Native.cstr(layerName);
+        Native.check(Native.netGetDropoutValue(net, Native.address(name), Native.address(o))); return o.getFloat(0);
+    }
+    private void applySchedule(String layerName, ISchedule s) { applySchedule(layerName, s, false); }
+    private void applySchedule(String layerName, ISchedule s, boolean dropout) {
         ByteBuffer st = null, keys = null, vals = null;      // b2g_lr_schedule (72 bytes) and a MapSchedule's entries
         if (s != null) {
             int[] k = s.mapKeys(); double[] v = s.mapValues(); double[] p = s.parameters();
@@ -95,7 +105,8 @@ public class ComputationGraph {
             st.putInt(48, k.length).putLong(56, Native.address(keys)).putLong(64, Native.address(vals));
         }
         ByteBuffer name = layerName == null ? null : Native.cstr(layerName);
-        Native.check(Native.netSetLrSchedule(net, name == null ? 0 : Native.address(name), st == null ? 0 : Native.address(st)));
+        final long nameAddr = name == null ? 0 : Native.address(name), stAddr = st == null ? 0 : Native.address(st);
+        Native.check(dropout ? Native.netSetDropoutSchedule(net, nameAddr, stAddr) : Native.netSetLrSchedule(net, nameAddr, stAddr));
         java.lang.ref.Reference.reachabilityFence(st); java.lang.ref.Reference.reachabilityFence(keys); java.lang.ref.Reference.reachabilityFence(vals);
         java.lang.ref.Reference.reachabilityFence(name);   // the native side reads these buffers only through their addresses
     }

@@ -59,6 +59,13 @@ FN(netApplyConstraints)(JNIEnv_*, jclass, jlong net) { return b2g_net_apply_cons
 FN(netGetLearningRate)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong outAddr) {
   return b2g_net_get_learning_rate(P(b2g_net*, net), P(const char*, layerNameAddr), P(float*, outAddr));
 }
+// the DropoutLayer's IDropout schedule, laid out as for netSetLrSchedule (layerNameAddr 0: every non-frozen DropoutLayer; scheduleAddr 0: constant)
+FN(netSetDropoutSchedule)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong scheduleAddr) {
+  return b2g_net_set_dropout_schedule(P(b2g_net*, net), P(const char*, layerNameAddr), P(const b2g_lr_schedule*, scheduleAddr));
+}
+FN(netGetDropoutValue)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong outAddr) {
+  return b2g_net_get_dropout_value(P(b2g_net*, net), P(const char*, layerNameAddr), P(float*, outAddr));
+}
 FN(netGetEpoch)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_get_epoch(P(b2g_net*, net), P(int64_t*, outAddr)); }
 FN(netSetEpoch)(JNIEnv_*, jclass, jlong net, jlong epoch) { return b2g_net_set_epoch(P(b2g_net*, net), epoch); }
 FN(netSimtGemmCalls)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_simt_gemm_calls(P(b2g_net*, net), P(uint64_t*, outAddr)); }

@@ -233,7 +233,29 @@ def constraint(ctx):
     return replicated_matches_one_gpu(ctx, dict(constraints=[m.max_norm(2.0, ())]), dict(constraints=[m.max_norm(0.5, (1,))]))
 
 
-CHECKS = {"core": core, "updater": updater, "dropout": dropout, "gradnorm": gradnorm, "constraint": constraint}
+def noise(ctx):
+    """The dropout check with the other IDropout kinds: an Exponential-scheduled GaussianNoise on D's input and GaussianDropout and
+    AlphaDropout after its hidden LeakyReLUs.  The ranks draw different noise (the rank enters the counter), the all-reduced gradients keep D's
+    parameters identical, and every rank evaluates the same scheduled value."""
+    n, z, hid, d = 128, 128, 256, 128
+    G = b.Net(ctx, m.mlp_generator(z, hid, d, lr=1e-3), (z,), max_batch=n, precision=b.BF16, xent_clip_eps=0.0, seed=1)
+    ds = m.mlp_discriminator(d, hid, lr=1e-3, instance_noise=m.exponential_schedule(0.2, 0.9))
+    ds = ds[:2] + [m.gaussian_dropout(0.3, "gd")] + ds[2:3] + [m.alpha_dropout(0.9, "ad")] + ds[3:]
+    D = b.Net(ctx, ds, (d,), max_batch=2 * n, precision=b.BF16, xent_clip_eps=0.0, bn_groups=2, seed=2)
+    gan = b.Gan(G, D, use_cuda_graph=True)
+    data = replicated_data(n, z, d)
+    for _ in range(3):
+        gan.step(*data)
+    acts = np.concatenate([D.activation(i, n).ravel() for i, s in enumerate(ds) if s["type"] == "dropout"])
+    allv = gather(np.concatenate([D.params(), [D.dropout_value("dis_instance_noise")], acts]))
+    npar = D.num_params()
+    gan.close(); G.close(); D.close()
+    return {"world": world, "d_params_identical": all(np.array_equal(allv[0][:npar + 1], v[:npar + 1]) for v in allv[1:]),
+            "noise_differs": all(not np.array_equal(allv[0][npar + 1:], v[npar + 1:]) for v in allv[1:]),
+            "scheduled_value": float(allv[0][npar])}
+
+
+CHECKS = {"core": core, "updater": updater, "dropout": dropout, "noise": noise, "gradnorm": gradnorm, "constraint": constraint}
 
 
 def main():

@@ -65,7 +65,7 @@ def build(ctx, cfg_name, variant):
         gin, din = (cfg["z"],), (cfg["nc"], cfg["size"], cfg["size"])
     swap = variant.get("swap", list)
     G = b.Net(ctx, swap(gs), gin, max_batch=n, precision=b.BF16, xent_clip_eps=0.0, seed=666)
-    D = b.Net(ctx, swap(ds), din, max_batch=2 * n, precision=b.BF16, xent_clip_eps=0.0, bn_groups=2, seed=667)
+    D = b.Net(ctx, variant.get("d_swap", list)(swap(ds)), din, max_batch=2 * n, precision=b.BF16, xent_clip_eps=0.0, bn_groups=2, seed=667)
     gan = b.Gan(G, D, fake_bn_train=False, use_cuda_graph=True)
     if "hook" in variant:
         variant["hook"](G); variant["hook"](D)
@@ -214,6 +214,32 @@ def dropout_model(cfg, G, D, n):
     elems = 2 * (2 * n + n) * cfg["hidden"]          # masked elements per step, forward (the backward handles the same)
     each_way = elems * (2 + 2 + 1 / 8)
     return {"masked_elements_per_step": elems, "kernel_bytes_per_step": {"dropout_fwd_kernel": each_way, "dropout_bwd_kernel": each_way}}
+
+
+# ---------------------------------------------------------------- noise: instance noise on D's input (C5, C2); GaussianDropout(0.5) or
+# AlphaDropout(0.9) after each hidden LeakyReLU of D (C5), beside C5's DropoutLayer(0.5) in the same session
+def after_lrelu(make):
+    def swap(specs):
+        out = []
+        for s in specs:
+            out.append(s)
+            if s.get("activation") == "lrelu":
+                out.append(make(s["name"] + "_noise"))
+        return out
+    return swap
+
+
+def noise_model(fwd_kernel, fwd_bytes, bwd_kernel, bwd_bytes):
+    """Algorithmic bytes per element of D's DropoutLayers, bf16: GaussianNoise reads x and writes y (4 B) and has no backward;
+    GaussianDropout 4 B each way (its backward draws m again); AlphaDropout 4 B and one mask bit each way (bern_fwd_kernel, mask_bwd_kernel).  Per step D runs them on its 2N-row
+    pass and on the generator step's N-row pass.  GaussianDropout's forward and backward are one kernel (gauss_kernel)."""
+    def model(cfg, G, D, n):
+        elems = 3 * n * sum(D.layer_output_size(i) for i, s in enumerate(D.specs) if s["type"] == "dropout")
+        kb = {fwd_kernel: elems * fwd_bytes}
+        if bwd_bytes:
+            kb[bwd_kernel] = kb.get(bwd_kernel, 0) + elems * bwd_bytes
+        return {"noisy_elements_per_step": elems, "kernel_bytes_per_step": kb}
+    return model
 
 
 # ---------------------------------------------------------------- gradnorm: RenormalizeL2PerLayer on C5, ClipL2PerLayer(1.0) on C2
@@ -432,6 +458,13 @@ FEATURES = {
     "constraint": dict(configs="c5,c2", variants=[{}, dict(name="maxnorm", hook=constrain, kernels=CONSTRAINT, model=constraint_model)]),
     "dropout": dict(configs="c5", variants=[{}, dict(name="dropout", d=dict(dropout=0.5), kernels=("dropout_fwd_kernel", "dropout_bwd_kernel"),
                                                      model=dropout_model)]),
+    "noise": dict(configs="c5,c2", variants=[
+        {}, dict(name="instance_noise", d=dict(instance_noise=0.1), kernels=("gauss_kernel",), model=noise_model("gauss_kernel", 4, None, 0)),
+        dict(name="gaussian_dropout", only=("c5",), d_swap=after_lrelu(lambda nm: m.gaussian_dropout(0.5, nm)), kernels=("gauss_kernel",),
+             model=noise_model("gauss_kernel", 4, "gauss_kernel", 4)),
+        dict(name="alpha_dropout", only=("c5",), d_swap=after_lrelu(lambda nm: m.alpha_dropout(0.9, nm)), kernels=("bern_fwd_kernel", "mask_bwd_kernel"),
+             model=noise_model("bern_fwd_kernel", 4.125, "mask_bwd_kernel", 4.125)),
+        dict(name="dropout", only=("c5",), d=dict(dropout=0.5), kernels=("dropout_fwd_kernel", "dropout_bwd_kernel"), model=dropout_model)]),
     "gradnorm": dict(configs="c5,c2", variants=[{}, dict(gradnorm("renormalize_l2_per_layer"), only=("c5",)),
                                                 dict(gradnorm("clip_l2_per_layer"), only=("c2",))]),
     "graph": dict(configs="c2", steps=50, variants=[{}, dict(name="residual", g=dict(residual=True), d=dict(residual=True))],
