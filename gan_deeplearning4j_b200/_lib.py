@@ -44,6 +44,12 @@ class LrSchedule(C.Structure):
                 ("map_values", C.POINTER(C.c_double))]
 
 
+class WeightNoise(C.Structure):
+    """b2g_weight_noise: DropConnect (p, or an ISchedule copied during the call) or WeightNoise (a distribution's two parameters)."""
+    _fields_ = [("kind", C.c_int32), ("apply_to_bias", C.c_int32), ("p", C.c_float), ("p_schedule", C.POINTER(LrSchedule)), ("dist", C.c_int32),
+                ("a", C.c_float), ("b", C.c_float), ("additive", C.c_int32)]
+
+
 class Constraint(C.Structure):
     """b2g_constraint: one DL4J LayerConstraint on one parameter tensor (kind, DL4J dimensions as a bit mask, bounds, MinMaxNorm's rate)."""
     _fields_ = [("kind", C.c_int32), ("dims_mask", C.c_int32), ("max_norm", C.c_double), ("min_norm", C.c_double), ("rate", C.c_double)]
@@ -129,6 +135,7 @@ PROTOTYPES = {
     "b2g_net_get_learning_rate": (_i32, [_vp, C.c_char_p, _fp]),
     "b2g_net_set_dropout_schedule": (_i32, [_vp, C.c_char_p, C.POINTER(LrSchedule)]),
     "b2g_net_get_dropout_value": (_i32, [_vp, C.c_char_p, _fp]),
+    "b2g_net_set_weight_noise": (_i32, [_vp, C.c_char_p, C.POINTER(WeightNoise)]),
     "b2g_net_get_epoch": (_i32, [_vp, C.POINTER(_i64)]),
     "b2g_net_set_epoch": (_i32, [_vp, _i64]),
     "b2g_net_simt_gemm_calls": (_i32, [_vp, C.POINTER(C.c_uint64)]),
@@ -154,6 +161,7 @@ PROTOTYPES = {
     "b2g_test_bn": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _fp, _fp, _fp, _fp, _fp, _fp, _i32, C.c_float, C.c_float, C.c_float,
                            _i32, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
     "b2g_test_net_shadow": (_i32, [_vp, _i32, _i32, _fp, _i64]),
+    "b2g_test_net_noisy_operand": (_i32, [_vp, _i32, _i32, _fp, _i64]),
     "b2g_test_dropout": (_i32, [_vp, _i32, C.c_uint64, _i32, _i32, _i64, _i32, _i32, _i32, _i32, C.c_float, _fp, _fp, _fp, _fp]),
     "b2g_test_dropout_kind": (_i32, [_vp, _i32, _i32, C.c_uint64, _i32, _i32, _i64, _i32, _i32, _i32, _i32, C.c_float, _fp, _fp, _fp, _fp]),
     "b2g_test_ew": (_i32, [_vp, _i32, C.POINTER(TestEwOpts), _fp, _fp, _fp, _fp, _fp]),

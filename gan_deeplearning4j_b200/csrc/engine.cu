@@ -124,6 +124,17 @@ struct LayerRT {
     return d.act == B2G_DROPOUT_GAUSSIAN_DROPOUT || d.act == B2G_DROPOUT_GAUSSIAN_NOISE ? d.act_alpha > 0.f : d.act_alpha < 1.f;
   }
   bool has_gemm() const { return d.type == B2G_LAYER_CONV2D || d.type == B2G_LAYER_DECONV2D || d.type == B2G_LAYER_DENSE || d.type == B2G_LAYER_OUTPUT; }
+  // Weight noise (b2g_net_set_weight_noise; wn.p_schedule is never kept): the layer's DropConnect schedule on the device (MAP entries in
+  // wn_map).  Its noisy operands, allocated when the layer first gets noise: wn_w = W' (fp32 in FP32 nets; in BF16 nets the bf16 straight
+  // copy, and the packed pixel-shuffle copy from element wn_ps on), wn_b = b' (fp32).  wn_live: the latest forward was a train-mode pass that
+  // drew, so the pass's GEMMs read the noisy operands; wn_drawn: some train-mode pass has drawn them
+  b2g_weight_noise wn{}; bool wn_sched = false; UpdSched* wn_sched_dev = nullptr; void* wn_map = nullptr;
+  void* wn_w = nullptr; int64_t wn_ps = -1; float* wn_b = nullptr; bool wn_live = false, wn_drawn = false;
+  // a layer whose train-mode passes draw: FrozenLayer never, constant DropConnect(1) is the identity
+  bool wn_active() const {
+    if (wn.kind == B2G_WEIGHT_NOISE_NONE || d.frozen) return false;
+    return wn.kind != B2G_WEIGHT_NOISE_DROPCONNECT || wn_sched || wn.p < 1.f;
+  }
 };
 
 struct b2g_net {
@@ -173,6 +184,8 @@ struct b2g_net {
   struct ConRound { int j0, j1, onepass_blocks, t0, t1, norm_blocks, scale_blocks; };
   std::vector<ConTensor> con; std::vector<ConRound> con_rounds;
   ConJob* con_jobs = nullptr; double* con_partial = nullptr; float* con_mult = nullptr; unsigned* con_ticket = nullptr;
+  // Weight noise: the job table of every drawing layer's noisy tensors (device, room for two per layer) and its block count; empty: no launch
+  WnJob* wn_jobs = nullptr; int wn_njobs = 0, wn_blocks = 0;
   ReduceList pending{};                                           // split-K partial sums queued by this backward pass
   uint64_t simt_gemm_calls = 0;                                    // BF16 nets: GEMM-shaped ops that ran on the SIMT kernels (skinny / unsupported shapes) -- reported, never silent
   float* scratch = nullptr; size_t scratch_floats = 0;
@@ -581,9 +594,10 @@ static void net_refresh_shadow(b2g_net* n, int only_layer = -1) {
 // sched_step / sched_epoch: the counters scheduled DropoutLayers read (null: the net's own)
 struct FwdOpts { int rows; int groups; bool train; bool update_running; void* out_override; const int* sched_step = nullptr; const int64_t* sched_epoch = nullptr; };
 
+// The weight operand of every GEMM route: the noisy W' while the layer's latest forward drew one (b2g_weight_noise), else the clean weights
 static const void* w_ptr(const b2g_net* n, const LayerRT& l, int* wprec) {
-  if (n->prec == PREC_BF16) { *wprec = PREC_BF16; return n->shadow + l.off_W_bf; }
-  *wprec = PREC_F32; return n->params + l.off_W;
+  if (n->prec == PREC_BF16) { *wprec = PREC_BF16; return l.wn_live ? l.wn_w : n->shadow + l.off_W_bf; }
+  *wprec = PREC_F32; return l.wn_live ? l.wn_w : n->params + l.off_W;
 }
 
 static inline bool tc_on(const b2g_net* n) { return n->prec == PREC_BF16 && n->ctx->tc_ok; }
@@ -626,7 +640,8 @@ static int32_t gemm_dgrad(b2g_net* n, const LayerRT& l, const ConvGeom& g, const
   }
   if (tc_on(n) && l.off_Wps_bf >= 0 && tc_deconv_ps_supported(g)) {
     const TcEpi* f = (fuse && fuse->mode == EPI_ACTBWD) ? fuse : nullptr;
-    if (k_tc_deconv_ps(g, (const __nv_bfloat16*)dy, n->shadow + l.off_Wps_bf, bias, (__nv_bfloat16*)dx, act, alpha, s, f) == 0) { if (fused) *fused = f != nullptr; return 0; }
+    const __nv_bfloat16* wps = l.wn_live ? (const __nv_bfloat16*)l.wn_w + l.wn_ps : n->shadow + l.off_Wps_bf;
+    if (k_tc_deconv_ps(g, (const __nv_bfloat16*)dy, wps, bias, (__nv_bfloat16*)dx, act, alpha, s, f) == 0) { if (fused) *fused = f != nullptr; return 0; }
     return fail(B2G_ERR_CUDA, "tensor-core pixel-shuffle deconv launch failed");
   }
   if (edge_deconv_small_c_supported(g)) { note_simt(n); k_edge_deconv_small_c(n->prec, wp, g, dy, w, bias, dx, act, alpha, s); return 0; }
@@ -702,11 +717,19 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
   // every stochastic DropoutLayer of a train-mode pass draws with the same pass counter P; the last one's kernel advances P on the device
   int last_drop = -1;
   if (o.train) for (size_t i = 0; i < n->L.size(); ++i) if (n->L[i].drop_active()) last_drop = (int)i;
+  // weight noise: one launch at the top of a train-mode pass draws every noisy tensor with the same P; it advances P itself only when no
+  // DropoutLayer of the pass will
+  for (auto& l : n->L) l.wn_live = o.train && l.wn_active();
+  if (o.train && n->wn_njobs) {
+    k_weight_noise(n->wn_jobs, n->wn_njobs, n->wn_blocks, n->cfg.seed ? n->cfg.seed : 666, n->ctx->rank, o.sched_step ? o.sched_step : n->step_dev,
+                   o.sched_epoch ? o.sched_epoch : n->epoch_dev, n->drop_pass, n->drop_ticket, last_drop < 0 ? 1 : 0, s);
+    for (auto& l : n->L) l.wn_drawn = l.wn_drawn || l.wn_live;
+  }
   for (size_t i = 0; i < n->L.size(); ++i) {
     LayerRT& l = n->L[i]; const b2g_layer_desc& d = l.d;
     void* out = l.out;
     if (i + 1 == n->L.size() && o.out_override && !l.out_alias) out = o.out_override;
-    const float* bias = l.off_b >= 0 ? n->params + l.off_b : nullptr;
+    const float* bias = l.off_b >= 0 ? (l.wn_live && l.wn.apply_to_bias ? l.wn_b : n->params + l.off_b) : nullptr;
     const bool gemm_then_bn = (d.type == B2G_LAYER_CONV2D || d.type == B2G_LAYER_DECONV2D || d.type == B2G_LAYER_DENSE) && i + 1 < n->L.size() && n->L[i + 1].d.type == B2G_LAYER_BATCHNORM;
     // a 1x1-input deconv is computed as the 1x1 problem with taps*C output channels: its columns are not the BatchNorm's channels
     const bool remapped = d.type == B2G_LAYER_DECONV2D && l.geom.KH == 1 && l.geom.C != l.oc;
@@ -1083,7 +1106,7 @@ extern "C" int32_t b2g_net_destroy(b2g_net* n) {
   for (auto e : n->ev_fork) if (e) cudaEventDestroy(e); for (auto e : n->ev_done) if (e) cudaEventDestroy(e); if (n->ev_join) cudaEventDestroy(n->ev_join);
   if (n->p2p) for (int r = 0; r < n->ctx->world; ++r) if (r != n->ctx->rank && n->p2p_peer_grads[r]) cudaIpcCloseMemHandle(n->p2p_peer_grads[r]);
   if (n->sched_map) cudaFree(n->sched_map);
-  for (auto& l : n->L) if (l.drop_map) cudaFree(l.drop_map);
+  for (auto& l : n->L) { if (l.drop_map) cudaFree(l.drop_map); if (l.wn_map) cudaFree(l.wn_map); }
   cudaFree(n->con_jobs); cudaFree(n->con_partial); cudaFree(n->con_mult);
   for (void* p : n->allocs) cudaFree(p); delete n; return 0;
 }
@@ -1712,23 +1735,27 @@ static int32_t find_dropout_layer(const b2g_net* n, const char* layer, int* li) 
   }
   return fail(B2G_ERR_ARG, "no layer named %s", layer);
 }
-// The layer's schedule to its device slot, MAP entries (values, then keys) to a buffer of its own
-static int32_t upload_dropout_schedule(b2g_net* n, LayerRT& l, const b2g_net::LayerSched& ls) {
+// A layer's schedule to its device slot `dev`, MAP entries (values, then keys) to a buffer of its own (*map, replaced)
+static int32_t upload_schedule(b2g_net* n, UpdSched* dev, void** map, const b2g_net::LayerSched& ls) {
   cudaStream_t s = n->ctx->stream;
   CU(cudaStreamSynchronize(s));                  // nothing in flight reads the old schedule or map
-  if (l.drop_map) { CU(cudaFree(l.drop_map)); l.drop_map = nullptr; }
+  if (*map) { CU(cudaFree(*map)); *map = nullptr; }
   UpdSched sc = ls.sc;
   if (sc.kind == B2G_SCHED_MAP) {
     const size_t nv = ls.vals.size(), bytes = nv * (sizeof(double) + sizeof(int32_t));
-    cudaError_t e = cudaMalloc(&l.drop_map, bytes);
-    if (e != cudaSuccess) { l.drop_map = nullptr; return fail(B2G_ERR_OOM, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); }
-    CU(cudaMemcpyAsync(l.drop_map, ls.vals.data(), nv * sizeof(double), cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync((char*)l.drop_map + nv * sizeof(double), ls.keys.data(), nv * sizeof(int32_t), cudaMemcpyHostToDevice, s));
-    sc.vals = (const double*)l.drop_map; sc.keys = (const int32_t*)((char*)l.drop_map + nv * sizeof(double));
+    cudaError_t e = cudaMalloc(map, bytes);
+    if (e != cudaSuccess) { *map = nullptr; return fail(B2G_ERR_OOM, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); }
+    CU(cudaMemcpyAsync(*map, ls.vals.data(), nv * sizeof(double), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync((char*)*map + nv * sizeof(double), ls.keys.data(), nv * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+    sc.vals = (const double*)*map; sc.keys = (const int32_t*)((char*)*map + nv * sizeof(double));
   }
-  CU(cudaMemcpyAsync(l.drop_sched_dev, &sc, sizeof(sc), cudaMemcpyHostToDevice, s));
+  CU(cudaMemcpyAsync(dev, &sc, sizeof(sc), cudaMemcpyHostToDevice, s));
   CU(cudaStreamSynchronize(s));
-  l.drop_sched = sc.kind != B2G_SCHED_NONE;
+  return 0;
+}
+static int32_t upload_dropout_schedule(b2g_net* n, LayerRT& l, const b2g_net::LayerSched& ls) {
+  B2(upload_schedule(n, l.drop_sched_dev, &l.drop_map, ls));
+  l.drop_sched = ls.sc.kind != B2G_SCHED_NONE;
   return 0;
 }
 extern "C" int32_t b2g_net_set_dropout_schedule(b2g_net* n, const char* layer, const b2g_lr_schedule* s) {
@@ -1747,6 +1774,89 @@ extern "C" int32_t b2g_net_get_dropout_value(b2g_net* n, const char* layer, floa
   CU(cudaMemcpyAsync(out, n->lr_out, sizeof(float), cudaMemcpyDeviceToHost, n->ctx->stream)); CU(cudaStreamSynchronize(n->ctx->stream));
   return 0;
 }
+// ------------------------------------------------------------------ weight noise (b2g_net_set_weight_noise) --------------------------------
+static int32_t check_weight_noise(const b2g_weight_noise& w) {
+  if (w.kind == B2G_WEIGHT_NOISE_NONE) return 0;
+  if (w.kind == B2G_WEIGHT_NOISE_DROPCONNECT) {
+    if (!(w.p > 0.f && w.p <= 1.f)) return fail(B2G_ERR_ARG, "DropConnect retain probability %g outside (0, 1]", (double)w.p);
+    return 0;
+  }
+  if (w.kind != B2G_WEIGHT_NOISE_WEIGHTNOISE) return fail(B2G_ERR_ARG, "unknown weight noise kind %d", w.kind);
+  if (!std::isfinite(w.a) || !std::isfinite(w.b)) return fail(B2G_ERR_ARG, "WeightNoise distribution parameters must be finite");
+  if (w.dist == B2G_DIST_NORMAL) { if (w.b < 0.f) return fail(B2G_ERR_ARG, "NormalDistribution std %g < 0", (double)w.b); }
+  else if (w.dist == B2G_DIST_UNIFORM) { if (w.b < w.a) return fail(B2G_ERR_ARG, "UniformDistribution upper %g < lower %g", (double)w.b, (double)w.a); }
+  else return fail(B2G_ERR_ARG, "unknown distribution %d (NORMAL or UNIFORM)", w.dist);
+  return 0;
+}
+// The layer's noisy operands, once: W' (fp32, or bf16 straight | packed pixel-shuffle copy) and b' when the bias is perturbed
+static int32_t wn_alloc(b2g_net* n, LayerRT& l) {
+  cudaStream_t s = n->ctx->stream;
+  if (!l.wn_w) {
+    if (n->prec == PREC_BF16) {
+      const int64_t straight = (l.n_W + 63) / 64 * 64, ps = l.off_Wps_bf >= 0 ? (int64_t)k_tc_deconv_ps_weight_elems(l.geom) : 0;
+      B2(dalloc(n, &l.wn_w, sizeof(__nv_bfloat16) * (straight + ps)));
+      // the packed operand's slots no weight element maps to stay zero, as k_pack_deconv_ps leaves them
+      CU(cudaMemsetAsync(l.wn_w, 0, sizeof(__nv_bfloat16) * (straight + ps), s));
+      l.wn_ps = ps ? straight : -1;
+    } else B2(dalloc(n, &l.wn_w, sizeof(float) * l.n_W));
+  }
+  if (l.wn.apply_to_bias && l.off_b >= 0 && !l.wn_b) B2(dalloc(n, &l.wn_b, sizeof(float) * l.d.n_out));
+  return 0;
+}
+// The job table of one draw: a W job per drawing layer and a b job per perturbed bias, each of ceil(n / WN_CHUNK) blocks
+static int32_t wn_build_jobs(b2g_net* n) {
+  if (!n->wn_jobs) B2(dalloc(n, &n->wn_jobs, sizeof(WnJob) * 2 * n->L.size()));
+  std::vector<WnJob> jobs; int blocks = 0;
+  for (size_t i = 0; i < n->L.size(); ++i) {
+    const LayerRT& l = n->L[i];
+    if (!l.wn_active()) continue;
+    WnJob j{}; j.layer = (int)i; j.kind = l.wn.kind; j.dist = l.wn.dist; j.additive = l.wn.additive; j.p = l.wn.p; j.a = l.wn.a; j.b = l.wn.b;
+    j.sched = l.wn_sched ? l.wn_sched_dev : nullptr; j.sg.off_bf = 0; j.sg.off_ps = -1;
+    WnJob w = j; w.src = n->params + l.off_W; w.n = l.n_W; w.j0 = 0;
+    if (n->prec == PREC_BF16) { w.dst_bf16 = (__nv_bfloat16*)l.wn_w; w.sg.len = l.n_W; w.sg.off_ps = l.wn_ps; w.sg.ps_O = l.geom.O; w.sg.ps_C = l.geom.C; }
+    else w.dst_f32 = (float*)l.wn_w;
+    w.blk_begin = blocks; w.blocks = (int)((w.n + WN_CHUNK - 1) / WN_CHUNK); blocks += w.blocks; jobs.push_back(w);
+    if (l.wn.apply_to_bias && l.off_b >= 0) {
+      WnJob b = j; b.src = n->params + l.off_b; b.n = l.d.n_out; b.j0 = 4 * ((l.n_W + 3) / 4); b.dst_f32 = l.wn_b;
+      b.blk_begin = blocks; b.blocks = (int)((b.n + WN_CHUNK - 1) / WN_CHUNK); blocks += b.blocks; jobs.push_back(b);
+    }
+  }
+  if (!jobs.empty()) { CU(cudaMemcpyAsync(n->wn_jobs, jobs.data(), sizeof(WnJob) * jobs.size(), cudaMemcpyHostToDevice, n->ctx->stream)); CU(cudaStreamSynchronize(n->ctx->stream)); }
+  n->wn_njobs = (int)jobs.size(); n->wn_blocks = blocks;
+  return 0;
+}
+extern "C" int32_t b2g_net_set_weight_noise(b2g_net* n, const char* layer, const b2g_weight_noise* wn) {
+  if (!n) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
+  b2g_weight_noise w{}; if (wn && wn->kind != B2G_WEIGHT_NOISE_NONE) w = *wn;
+  B2(check_weight_noise(w));
+  b2g_net::LayerSched ls;
+  if (w.kind == B2G_WEIGHT_NOISE_DROPCONNECT) B2(parse_schedule(w.p_schedule, &ls));
+  w.p_schedule = nullptr;
+  std::vector<int> targets;
+  if (layer) {
+    for (size_t i = 0; i < n->L.size() && targets.empty(); ++i) if (!strncmp(n->L[i].d.name, layer, B2G_NAME_LEN)) {
+      if (!n->L[i].has_gemm()) return fail(B2G_ERR_ARG, "layer %s has no W (weight noise needs a conv, deconv, dense or output layer)", layer);
+      targets.push_back((int)i);
+    }
+    if (targets.empty()) return fail(B2G_ERR_ARG, "no layer named %s", layer);
+  } else for (size_t i = 0; i < n->L.size(); ++i) if (n->L[i].has_gemm() && !n->L[i].d.frozen) targets.push_back((int)i);
+  CU(cudaStreamSynchronize(n->ctx->stream));      // nothing in flight reads the old job table or operands
+  for (int i : targets) {
+    LayerRT& l = n->L[i];
+    l.wn = w; l.wn_drawn = false; l.wn_sched = false;
+    if (w.kind == B2G_WEIGHT_NOISE_NONE) continue;
+    B2(wn_alloc(n, l));
+    if (w.kind == B2G_WEIGHT_NOISE_DROPCONNECT && ls.sc.kind != B2G_SCHED_NONE) {
+      if (!l.wn_sched_dev) B2(dalloc(n, &l.wn_sched_dev, sizeof(UpdSched)));
+      B2(upload_schedule(n, l.wn_sched_dev, &l.wn_map, ls));
+      l.wn_sched = true;
+    }
+  }
+  B2(wn_build_jobs(n));
+  ++n->settings_gen;           // a captured step holds the launch and its job count: re-capture
+  return 0;
+}
+
 // The epoch word lives on the device like the iteration counter: a replayed graph reads the value set last, no re-capture needed.
 extern "C" int32_t b2g_net_get_epoch(b2g_net* n, int64_t* out) {
   if (!n || !out) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
@@ -2450,6 +2560,32 @@ extern "C" int32_t b2g_test_net_shadow(b2g_net* n, int32_t layer, int32_t which,
   if ((size_t)len > n->stage_floats) return fail(B2G_ERR_SHAPE, "operand larger than the staging buffer");
   k_nhwc_to_nchw_f32(PREC_BF16, n->shadow + off, n->stage_f32, 1, 1, (int)len, s);
   CU(cudaMemcpyAsync(out, n->stage_f32, sizeof(float) * len, cudaMemcpyDeviceToHost, s)); CU(cudaStreamSynchronize(s)); CHECK_KERNELS();
+  return 0;
+}
+
+// The noisy operands of the layer's latest drawing pass (b2g_weight_noise), widened to fp32: which = 0 W' (fp32 or the bf16 straight copy),
+// 1 the packed pixel-shuffle W', 2 b'.
+extern "C" int32_t b2g_test_net_noisy_operand(b2g_net* n, int32_t layer, int32_t which, float* out, int64_t count) {
+  if (!n || !out) return fail(B2G_ERR_ARG, "null");
+  if (layer < 0 || layer >= (int)n->L.size()) return fail(B2G_ERR_ARG, "layer %d out of range", layer);
+  const LayerRT& l = n->L[layer];
+  if (!l.wn_drawn) return fail(B2G_ERR_UNSUPPORTED, "layer %d drew no weight noise", layer);
+  const void* src = nullptr; int64_t len = 0; int prec = PREC_F32;
+  if (which == 0) { src = l.wn_w; len = l.n_W; prec = n->prec; }
+  else if (which == 1) {
+    if (l.wn_ps < 0) return fail(B2G_ERR_UNSUPPORTED, "layer %d has no pixel-shuffle operand", layer);
+    src = (const __nv_bfloat16*)l.wn_w + l.wn_ps; len = (int64_t)k_tc_deconv_ps_weight_elems(l.geom); prec = PREC_BF16;
+  } else if (which == 2) {
+    if (!l.wn.apply_to_bias || !l.wn_b) return fail(B2G_ERR_UNSUPPORTED, "layer %d perturbs no bias", layer);
+    src = l.wn_b; len = l.d.n_out;
+  } else return fail(B2G_ERR_ARG, "which = %d (0 W', 1 pixel-shuffle W', 2 b')", which);
+  if (count != len) return fail(B2G_ERR_SHAPE, "layer %d operand has %lld elements, %lld requested", layer, (long long)len, (long long)count);
+  CU(cudaSetDevice(n->ctx->device)); cudaStream_t s = n->ctx->stream;
+  if (prec == PREC_BF16) {
+    if ((size_t)len > n->stage_floats) return fail(B2G_ERR_SHAPE, "operand larger than the staging buffer");
+    k_nhwc_to_nchw_f32(PREC_BF16, src, n->stage_f32, 1, 1, (int)len, s); src = n->stage_f32;
+  }
+  CU(cudaMemcpyAsync(out, src, sizeof(float) * len, cudaMemcpyDeviceToHost, s)); CU(cudaStreamSynchronize(s)); CHECK_KERNELS();
   return 0;
 }
 

@@ -162,6 +162,7 @@ void k_noise_bwd(int prec, int kind, const void* eps_out, void* eps_in, const ui
 // *out = the clamped value the next forward of a layer of this kind uses (one thread, one launch)
 void k_noise_value(int kind, float value, const NoiseSched& q, float* out, cudaStream_t s);
 
+
 // ---- loss ----------------------------------------------------------------------------------------------
 // LossBinaryXENT on logits z[rows] with labels y[rows]: dz = dL/dz (sum form, not /mb), loss_sums[g] = sum of losses per group.
 void k_xent(int prec, const void* z, const float* y, void* dz, float* loss_sums, int rows_per_group, int groups, float clip_eps, cudaStream_t s);
@@ -273,6 +274,27 @@ __device__ inline float sched_lr(const UpdSched& sc, float lr, int it, long long
   }
   return (float)v;
 }
+
+// ---- weight noise (DL4J DropConnect / WeightNoise; definitions at b2g_weight_noise in include/b200gan.h) ------------------------------
+// One job = one noisy tensor: n fp32 master elements src[0, n) drawn with indices j = j0 + i and counter word 3 = layer | rank << 16.  Output:
+// dst_f32[i] (FP32 nets' W, every b), or for BF16 W the bf16 value through upd_shadow(sg, dst_bf16, i, .) (sg.off = 0: the straight copy at
+// sg.off_bf, and the packed pixel-shuffle slot at sg.off_ps >= 0).  Blocks [blk_begin, blk_begin + blocks) of the launch serve the job,
+// WN_CHUNK elements each (4 per thread, one Philox call).  sched (DROPCONNECT, may be null): thread 0 of each block evaluates p.
+enum { WN_DROPCONNECT = 1, WN_WEIGHTNOISE = 2 };   // b2g_weight_noise_kind
+enum { WN_NORMAL = 0, WN_UNIFORM = 1 };            // b2g_distribution_kind
+static const int WN_CHUNK = 1024;
+struct WnJob {
+  const float* src; int64_t n, j0;
+  float* dst_f32; __nv_bfloat16* dst_bf16; UpdSeg sg;
+  int layer, kind, dist, additive;
+  float p, a, b;                 // DROPCONNECT p; WEIGHTNOISE NORMAL (mean, std) / UNIFORM (lower, upper)
+  const UpdSched* sched;
+  int blk_begin, blocks;
+};
+// jobs: device table of njobs jobs, nblocks blocks in all.  P = *pass read on the device; bump_pass: the last block advances *pass (ticket as
+// k_dropout_fwd).  step / epoch: the counters scheduled jobs read.
+void k_weight_noise(const WnJob* jobs, int njobs, int nblocks, uint64_t seed, int rank, const int* step, const int64_t* epoch, unsigned long long* pass,
+                    unsigned* ticket, int bump_pass, cudaStream_t s);
 
 // ---- L2 gradient normalization (DL4J GradientNormalization.{Renormalize,Clip}L2Per{Layer,ParamType}; kernels_gradnorm.cu) ---------
 // A norm group is a run of updater segments: one layer's segments, or one segment.  Its chunks are [chunk_begin, chunk_end) of the updater's

@@ -350,4 +350,65 @@ void k_noise_value(int kind, float value, const NoiseSched& q, float* out, cudaS
   noise_value_kernel<<<1, 32, 0, s>>>(kind, value, q, out); LAUNCHED();
 }
 
+// ---- weight noise (DropConnect, WeightNoise; b2g_weight_noise) ------------------------------------------------------------------------
+// One launch per train-mode pass over the job table: each block finds its job (the largest blk_begin <= blockIdx.x), each thread draws 4
+// consecutive elements with one Philox call (j0 is a multiple of 4, so they share a counter).  Loads are 16-byte where the tensor starts on a
+// 16-byte boundary (a conv W follows its nOut biases, so it may not), scalar otherwise.
+__global__ void __launch_bounds__(256) weight_noise_kernel(const WnJob* __restrict__ jobs, int njobs, uint64_t seed, int rank, const int* step,
+                                                           const int64_t* epoch, unsigned long long* pass, unsigned* ticket, int bump) { pdl_enter();
+  const unsigned long long P = *(volatile unsigned long long*)pass;
+  int lo = 0, hi = njobs - 1;
+  while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (jobs[mid].blk_begin <= (int)blockIdx.x) lo = mid; else hi = mid - 1; }
+  const WnJob& jb = jobs[lo];
+  __shared__ uint32_t s_threshold; __shared__ int s_keep_all;
+  if (jb.kind == WN_DROPCONNECT && threadIdx.x == 0) {        // Dropout's keep rule at p, or at the schedule's clamped value
+    NoiseArgs a{};
+    noise_derive(DROP_BERNOULLI, jb.sched ? noise_clamp(DROP_BERNOULLI, sched_lr(*jb.sched, jb.p, *step, (long long)*epoch)) : jb.p, a);
+    s_threshold = a.threshold; s_keep_all = a.keep_all;
+  }
+  __syncthreads();
+  const int64_t i0 = (int64_t)(blockIdx.x - jb.blk_begin) * WN_CHUNK + 4 * (int64_t)threadIdx.x, n = jb.n;
+  if (i0 < n) {
+    const Philox4 r = philox4x32_10((uint32_t)((jb.j0 + i0) >> 2), (uint32_t)P, (uint32_t)(P >> 32), (uint32_t)jb.layer | ((uint32_t)rank << 16),
+                                    (uint32_t)seed, (uint32_t)(seed >> 32));
+    const bool full = i0 + 4 <= n;
+    float w[4];
+    if (full && (reinterpret_cast<uintptr_t>(jb.src) & 15) == 0) ld16(jb.src + i0, w);
+    else {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) w[k] = i0 + k < n ? jb.src[i0 + k] : 0.f;
+    }
+    if (jb.kind == WN_DROPCONNECT) {
+      const uint32_t thr = s_threshold; const int all = s_keep_all;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) w[k] = (all || r.x[k] < thr) ? w[k] : 0.f;
+    } else {
+      float nz[4];
+      if (jb.dist == WN_NORMAL) {
+        normals4(r, nz);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) nz[k] = fmaf(jb.b, nz[k], jb.a);
+      } else {
+        const float span = jb.b - jb.a;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) nz[k] = fmaf(span, (float)(r.x[k] >> 8) * 0x1p-24f, jb.a);
+      }
+#pragma unroll
+      for (int k = 0; k < 4; ++k) w[k] = jb.additive ? w[k] + nz[k] : w[k] * nz[k];
+    }
+    if (jb.dst_f32) {
+      if (full) st16(jb.dst_f32 + i0, w);
+      else for (int k = 0; k < 4 && i0 + k < n; ++k) jb.dst_f32[i0 + k] = w[k];
+    } else {
+      for (int k = 0; k < 4 && i0 + k < n; ++k) upd_shadow(jb.sg, jb.dst_bf16, i0 + k, __float2bfloat16_rn(w[k]));
+    }
+  }
+  if (bump) bump_pass_counter(pass, ticket, P);
+}
+void k_weight_noise(const WnJob* jobs, int njobs, int nblocks, uint64_t seed, int rank, const int* step, const int64_t* epoch, unsigned long long* pass,
+                    unsigned* ticket, int bump_pass, cudaStream_t s) {
+  if (!njobs || !nblocks) return;
+  launch_pdl(weight_noise_kernel, dim3(nblocks), dim3(256), (size_t)0, s, jobs, njobs, seed, rank, step, epoch, pass, ticket, bump_pass); LAUNCHED();
+}
+
 }  // namespace b2g

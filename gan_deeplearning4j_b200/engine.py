@@ -224,6 +224,37 @@ def dropout_value_key(spec: Dict) -> str:
     return DROPOUT_KINDS[spec.get("kind", "dropout")][1]
 
 
+# Weight noise of a GEMM layer spec's "weight_noise" (b2g_weight_noise in include/b200gan.h; models.drop_connect / models.weight_noise)
+WEIGHT_NOISE_KINDS = {"drop_connect": 1, "weight_noise": 2}
+DISTRIBUTIONS = {"normal": (0, "mean", "std"), "uniform": (1, "lower", "upper")}
+
+
+def weight_noise_struct(wn: Optional[Dict]):
+    """A weight-noise dict (models.py) -> (b2g_weight_noise, what it points into).  None -> kind NONE."""
+    s = _lib.WeightNoise()
+    if wn is None:
+        return s, ()
+    kind = wn.get("weight_noise")
+    if kind not in WEIGHT_NOISE_KINDS:
+        raise ValueError(f"unknown weight noise {kind!r}; one of {sorted(WEIGHT_NOISE_KINDS)}")
+    s.kind, s.apply_to_bias = WEIGHT_NOISE_KINDS[kind], int(bool(wn.get("apply_to_bias", False)))
+    keep = ()
+    if kind == "drop_connect":
+        s.p = constant_lr(wn["p"])
+        if is_schedule(wn["p"]):
+            sched, arrays = schedule_struct(wn["p"])
+            s.p_schedule = C.pointer(sched)
+            keep = (sched, arrays)
+    else:
+        dist = wn["distribution"]
+        if dist.get("distribution") not in DISTRIBUTIONS:
+            raise ValueError(f"unknown distribution {dist.get('distribution')!r}; one of {sorted(DISTRIBUTIONS)}")
+        code, ka, kb = DISTRIBUTIONS[dist["distribution"]]
+        s.dist, s.a, s.b = code, float(dist[ka]), float(dist[kb])
+        s.additive = int(bool(wn.get("additive", True)))
+    return s, keep
+
+
 def layer_desc(spec: Dict, skip: Optional[tuple] = None) -> LayerDesc:
     """skip: the vertex's (j, order) from resolve_vertices."""
     d = LayerDesc()
@@ -330,15 +361,20 @@ class Net:
     def __init__(self, ctx: Context, specs: Sequence[Dict], input_shape, max_batch: int, precision: int = FP32,
                  grad_clip: float = 0.0, xent_clip_eps: float = 1e-5, bn_groups: int = 1, seed: int = 666,
                  gradient_normalization: str = "none", gradient_normalization_threshold: float = 1.0,
-                 constraints: Optional[Sequence[Dict]] = None):
+                 constraints: Optional[Sequence[Dict]] = None, weight_noise: Optional[Dict] = None):
         """constraints: the global builder's constraints (models.max_norm, ...), for every layer whose own "constraints" reach none of its
         parameters (none given, or e.g. only bias constraints on a BatchNorm), as DL4J's builder fills them in; the specs the net keeps (and a
-        checkpoint saves) carry them per layer."""
+        checkpoint saves) carry them per layer.  weight_noise: the global builder's weightNoise (models.drop_connect / models.weight_noise) for
+        every non-frozen conv, deconv, dense and output layer without a "weight_noise" of its own; the kept specs carry it per layer."""
         self.ctx, self.lib, self.specs = ctx, ctx.lib, copy.deepcopy(list(specs))
         if constraints:
             for sp in self.specs:
                 if sp["type"] in GEMM_TYPES + ("batchnorm",) and not resolve_constraints(sp):
                     sp["constraints"] = copy.deepcopy(list(constraints))
+        if weight_noise is not None:
+            for sp in self.specs:
+                if sp["type"] in GEMM_TYPES and not sp.get("frozen", False) and "weight_noise" not in sp:
+                    sp["weight_noise"] = copy.deepcopy(weight_noise)
         # each layer's b2g_layer_desc.lr: what the engine uses again when a schedule is cleared
         self.lr_constants = [constant_lr((sp.get("updater") or {}).get("lr", 0.0)) for sp in self.specs]
         c, h, w = input_shape if len(input_shape) == 3 else (input_shape[0], 1, 1)
@@ -368,6 +404,9 @@ class Net:
             for sp in self.specs:         # new GaussianNoise(ISchedule) and the other IDropout schedule constructors
                 if sp["type"] == "dropout" and is_schedule(sp[dropout_value_key(sp)]):
                     self.set_dropout_schedule(sp[dropout_value_key(sp)], sp["name"])
+            for sp in self.specs:         # Layer.Builder.weightNoise
+                if sp.get("weight_noise") is not None:
+                    self.set_weight_noise(sp["weight_noise"], sp["name"])
         except Exception:
             self.close()
             raise
@@ -510,6 +549,28 @@ class Net:
             sp[dropout_value_key(sp)] = copy.deepcopy(schedule) if schedule is not None else self.dropout_constants[sp["name"]]
             if layer is not None:
                 break
+
+    def set_weight_noise(self, weight_noise: Optional[Dict], layer: Optional[str] = None):
+        """DropConnect or WeightNoise on a layer's weights (b2g_net_set_weight_noise; models.drop_connect / models.weight_noise): layer None =
+        every non-frozen conv, deconv, dense and output layer; None clears it.  Drawn anew in every train-mode pass from the next one on; the
+        specs a checkpoint writes follow."""
+        s, _keep = weight_noise_struct(weight_noise)
+        check(self.lib.b2g_net_set_weight_noise(self.h, None if layer is None else layer.encode(), C.byref(s)))
+        for sp in self.specs:
+            if sp["type"] not in GEMM_TYPES or (layer is None and sp.get("frozen", False)) or (layer is not None and sp.get("name") != layer):
+                continue
+            sp.pop("weight_noise", None)
+            if weight_noise is not None:
+                sp["weight_noise"] = copy.deepcopy(weight_noise)
+            if layer is not None:
+                break
+
+    def noisy_operand(self, layer: int, which: int, size: int) -> np.ndarray:
+        """What the latest train-mode pass of a weight-noise layer drew (b2g_test_net_noisy_operand): which 0 = W' in the internal order, 1 = the
+        packed pixel-shuffle W' (BF16), 2 = b'."""
+        out = np.empty(size, np.float32)
+        check(self.lib.b2g_test_net_noisy_operand(self.h, layer, which, _fp(out), size))
+        return out
 
     def dropout_value(self, layer: str) -> float:
         """The value (p, rate or stddev) the DropoutLayer's next train-mode forward uses, evaluated and clamped on the device."""

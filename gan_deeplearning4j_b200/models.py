@@ -137,6 +137,29 @@ def spatial_dropout(p, name="") -> Dict:
     return {"type": "dropout", "name": name, "kind": "spatial_dropout", "p": _value(p)}
 
 
+# ------------------------------------------------------------------ weight noise ----------------------
+# Layer.Builder.weightNoise / NeuralNetConfiguration.Builder.weightNoise (b2g_weight_noise in include/b200gan.h): the value of a GEMM layer
+# spec's "weight_noise" key, or of Net(..., weight_noise=...) for every GEMM layer without its own.
+def drop_connect(p, apply_to_biases=False) -> Dict:
+    """new DropConnect(p[, applyToBiases]), p = the retain probability of each weight (a number or a schedule); W' = keep ? W : 0, not rescaled."""
+    return {"weight_noise": "drop_connect", "p": _value(p), "apply_to_bias": bool(apply_to_biases)}
+
+
+def normal(mean, std) -> Dict:
+    """new NormalDistribution(mean, std)"""
+    return {"distribution": "normal", "mean": float(mean), "std": float(std)}
+
+
+def uniform(lower, upper) -> Dict:
+    """new UniformDistribution(lower, upper)"""
+    return {"distribution": "uniform", "lower": float(lower), "upper": float(upper)}
+
+
+def weight_noise(distribution, apply_to_bias=False, additive=True) -> Dict:
+    """new WeightNoise(distribution, applyToBias, additive): W' = W + n (additive) or W * n, n drawn from normal(..) or uniform(..)."""
+    return {"weight_noise": "weight_noise", "distribution": dict(distribution), "apply_to_bias": bool(apply_to_bias), "additive": bool(additive)}
+
+
 # ------------------------------------------------------------------ pooling layers ---------------------
 # SubsamplingLayer / GlobalPoolingLayer (b2g_pooling in include/b200gan.h).  SubsamplingLayer(MAX) is the "maxpool" spec (unpadded).
 def subsampling(pooling, kernel=(1, 1), stride=(2, 2), padding=(0, 0), pnorm=None, name="") -> Dict:
@@ -325,7 +348,7 @@ def _loss_keys(loss, out_activation) -> Dict:
 
 
 def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", out_activation="identity", activation="lrelu", alpha=None,
-                        global_pooling=None, patch=False, residual=False, instance_noise=None) -> List[Dict]:
+                        global_pooling=None, patch=False, residual=False, instance_noise=None, drop_connect=None) -> List[Dict]:
     """Conv(4x4 s2 p1)+LeakyReLU(0.2); (Conv+BatchNorm+LeakyReLU)*; Conv(4x4 s1 p0) -> logit; LossLayer(loss).  Input (nc,size,size).
     loss: "xent" (sigmoid implied), or "mse" (least-squares GAN), "hinge", "wasserstein", ... applied to out_activation(logit).
     activation / alpha: the hidden activation in place of LeakyReLU(0.2) (as in _act).
@@ -335,7 +358,8 @@ def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", o
     1 channel and a CnnLossLayer(loss) take the place of the last conv and its LossLayer: one logit and one label per patch (a 4x4 map up to
     64x64, 8x8 at 128x128).
     residual: one identity residual_block after each down-sampling stage (a ResNet-style critic).
-    instance_noise = stddev: a GaussianNoise(stddev) DropoutLayer on the input (instance noise: real and fake images both get the noise)."""
+    instance_noise = stddev: a GaussianNoise(stddev) DropoutLayer on the input (instance noise: real and fake images both get the noise).
+    drop_connect = p: DropConnect(p) weight noise on every conv and output layer (see _with_drop_connect)."""
     if patch and global_pooling is not None:
         raise ValueError("patch and global_pooling are two different heads")
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
@@ -353,14 +377,21 @@ def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", o
         ch *= 2
         L += block(i + 2, ch, f"dis_act_{i + 2}")
     if global_pooling is not None:
-        return L + [_global_pooling_spec(global_pooling, name="dis_global_pool"),
-                    dict({"type": "output", "name": "dis_output", "n_out": 1, "updater": u()}, **_loss_keys(loss, out_activation))]
+        return _with_drop_connect(L + [_global_pooling_spec(global_pooling, name="dis_global_pool"),
+                                       dict({"type": "output", "name": "dis_output", "n_out": 1, "updater": u()}, **_loss_keys(loss, out_activation))], drop_connect)
     if patch:
-        return L + [{"type": "conv2d", "name": f"dis_conv_{n_down + 1}", "n_in": ch, "n_out": 1, "kernel": (3, 3), "stride": (1, 1), "padding": (1, 1), "updater": u()},
-                    dict({"type": "cnn_loss", "name": "dis_loss"}, **_loss_keys(loss, out_activation))]
+        return _with_drop_connect(L + [{"type": "conv2d", "name": f"dis_conv_{n_down + 1}", "n_in": ch, "n_out": 1, "kernel": (3, 3), "stride": (1, 1), "padding": (1, 1), "updater": u()},
+                                       dict({"type": "cnn_loss", "name": "dis_loss"}, **_loss_keys(loss, out_activation))], drop_connect)
     L += [{"type": "conv2d", "name": f"dis_conv_{n_down + 1}", "n_in": ch, "n_out": 1, "kernel": (4, 4), "stride": (1, 1), "padding": (0, 0), "updater": u()},
           dict({"type": "loss", "name": "dis_loss"}, **_loss_keys(loss, out_activation))]
-    return L
+    return _with_drop_connect(L, drop_connect)
+
+
+def _with_drop_connect(specs: List[Dict], p) -> List[Dict]:
+    """p None: the specs unchanged; else each GEMM layer spec gets "weight_noise": drop_connect(p) (the global builder's weightNoise)."""
+    if p is None:
+        return specs
+    return [dict(s, weight_noise=drop_connect(p)) if s["type"] in ("conv2d", "deconv2d", "dense", "output") else s for s in specs]
 
 
 # ------------------------------------------------------------------ C5: MLP-GAN --------------------------
@@ -373,17 +404,18 @@ def mlp_generator(z=100, hidden=1024, d=256, lr=2e-4, beta1=0.5, activation="rel
 
 
 def mlp_discriminator(d=256, hidden=1024, lr=2e-4, beta1=0.5, dropout=None, loss="xent", out_activation="identity", activation="lrelu",
-                      alpha=None, instance_noise=None) -> List[Dict]:
+                      alpha=None, instance_noise=None, drop_connect=None) -> List[Dict]:
     """dropout = p: a DropoutLayer(p) (p = retain probability) after each hidden LeakyReLU, the DL4J MNIST GAN example's discriminator shape.
     loss / out_activation: the OutputLayer's loss, as for dcgan_discriminator.  activation / alpha: the hidden activation (as in _act).
-    instance_noise = stddev: a GaussianNoise(stddev) DropoutLayer on the input, as for dcgan_discriminator."""
+    instance_noise = stddev: a GaussianNoise(stddev) DropoutLayer on the input, as for dcgan_discriminator.
+    drop_connect = p: DropConnect(p) weight noise on every dense and output layer, as for dcgan_discriminator."""
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
     L = [] if instance_noise is None else [gaussian_noise(instance_noise, name="dis_instance_noise")]
     for i in (1, 2):
         L.append({"type": "dense", "name": f"dis_dense_{i}", "n_out": hidden, **_act(activation, alpha), "updater": u()})
         if dropout is not None:
             L.append({"type": "dropout", "name": f"dis_dropout_{i}", "p": dropout})
-    return L + [dict({"type": "output", "name": "dis_output", "n_out": 1, "updater": u()}, **_loss_keys(loss, out_activation))]
+    return _with_drop_connect(L + [dict({"type": "output", "name": "dis_output", "n_out": 1, "updater": u()}, **_loss_keys(loss, out_activation))], drop_connect)
 
 
 # algorithmic MACs per image of the conv/deconv/dense layers (SURVEY.md 8d: F = 2*(4*G_f + 8*D_f))

@@ -463,6 +463,49 @@ int32_t b2g_net_get_learning_rate(b2g_net* net, const char* layer, float* out);
 int32_t b2g_net_set_dropout_schedule(b2g_net* net, const char* layer, const b2g_lr_schedule* s);
 /* The value (p, rate or stddev) the named DropoutLayer's next train-mode forward uses, clamped, computed on the device.  Sync point. */
 int32_t b2g_net_get_dropout_value(b2g_net* net, const char* layer, float* out);
+
+/* Weight noise (DL4J 1.0.0-beta3 org.deeplearning4j.nn.conf.weightnoise: Layer.Builder.weightNoise / NeuralNetConfiguration.Builder.weightNoise
+ * with DropConnect or WeightNoise, recalled; parity unpinned like the rest of the DL4J semantics).
+ * Which layers: CONV2D, DECONV2D, DENSE and OUTPUT; W always, b only with apply_to_bias.  BatchNorm parameters are never perturbed.
+ * When: in the train-mode passes of a non-frozen layer, exactly the passes in which the net's DropoutLayers draw (b2g_net_fit,
+ * b2g_net_compute_gradient_and_score, b2g_net_output with train = 1, the GAN step's real|fake pass of D and its generator pass through D, the
+ * generator's train-mode pass).  A FrozenLayer draws nothing; a layer with lr 0 does draw.  Inference passes use the clean parameters (DL4J's
+ * `train && isWeight || (applyToBias && isBias)` would also perturb biases at inference: a documented deviation).
+ * One pass, one draw: the forward and the input gradient of a pass use the same W' and b'.  The weight and bias gradients are computed from x
+ * and dy as without noise and applied to the clean W and b (straight through; DL4J does not multiply dW by the mask).  The l2 score, the
+ * updater, the constraints and b2g_net_get_param see the clean parameters.
+ * Draws: element j of a noisy tensor takes word x[j & 3] of Philox4x32-10(ctr = {j >> 2, lo32(P), hi32(P), L | r << 16}, key = {lo32(S), hi32(S)})
+ * with S, r and P of B2G_LAYER_DROPOUT and L the GEMM layer's own index (no DropoutLayer mask uses a GEMM layer's index).  For W, j is the
+ * element's index in the fp32 master as stored (the internal [A][taps][B] order of b2g_test_net_shadow); bias element k takes
+ * j = 4 * ceil(n_W / 4) + k.  Each result is computed in fp32 and rounded once to the operand type (fp32, or bf16 in BF16 nets):
+ *   DROPCONNECT(p)   keep = p >= 1 || x[j & 3] < floor(p * 2^32);  W' = keep ? w : +0.  Not rescaled by 1/p (DL4J applies the DropOut op, not
+ *                    DropOutInverted).  p in (0, 1]; p_schedule (may be NULL) replaces it with an ISchedule evaluated on the device at each
+ *                    train-mode pass, at the owning net's iteration counter or epoch word (in b2g_gan_step's generator pass through D at the
+ *                    generator's, as for DropoutLayer schedules), clamped to [2^-32, 1].
+ *   WEIGHTNOISE      n = fmaf(b, z, a) for NORMAL(mean a, std b >= 0), z = z[j & 3] of the Box-Muller normals of b2g_dropout_kind (truncated
+ *                    at |z| <= 5.8); n = fmaf(b - a, u, a) for UNIFORM(lower a, upper b >= a), u = (x[j & 3] >> 8) * 2^-24.
+ *                    W' = additive ? w + n : w * n.
+ * Pass counter: a train-mode pass with at least one noisy layer issues one launch at its top, before any layer, for every noisy tensor of the
+ * net.  It reads P; when the pass has no stochastic DropoutLayer its last block advances P, otherwise the last DropoutLayer does as before, so
+ * adding weight noise changes no DropoutLayer mask.  DROPCONNECT with a constant p = 1 is the identity: no launch, no pass counted; a scheduled
+ * DROPCONNECT draws whatever its value.  One GPU runs the reference's two worker minibatches of the D step (real | fake) as one pass: they share
+ * one W', as they share DropoutLayer masks.  Buffers: the noisy operands of a layer are allocated when it first gets weight noise. */
+typedef enum { B2G_WEIGHT_NOISE_NONE = 0, B2G_WEIGHT_NOISE_DROPCONNECT = 1, B2G_WEIGHT_NOISE_WEIGHTNOISE = 2 } b2g_weight_noise_kind;
+typedef enum { B2G_DIST_NORMAL = 0, B2G_DIST_UNIFORM = 1 } b2g_distribution_kind;    /* NormalDistribution(mean, std), UniformDistribution(lower, upper) */
+typedef struct {
+  int32_t kind;                     /* b2g_weight_noise_kind */
+  int32_t apply_to_bias;            /* DropConnect's applyToBiases / WeightNoise's applyToBias */
+  float p;                          /* DROPCONNECT: retain probability in (0, 1] */
+  const b2g_lr_schedule* p_schedule;   /* DROPCONNECT: an ISchedule in place of p (NULL: none; copied during the call) */
+  int32_t dist;                     /* WEIGHTNOISE: b2g_distribution_kind */
+  float a, b;                       /* WEIGHTNOISE: NORMAL mean, std; UNIFORM lower, upper */
+  int32_t additive;                 /* WEIGHTNOISE: W' = w + n (1) or w * n (0) */
+} b2g_weight_noise;
+/* Layer.Builder.weightNoise (layer named) or NeuralNetConfiguration.Builder.weightNoise (layer NULL: every non-frozen CONV2D, DECONV2D, DENSE
+ * and OUTPUT layer).  wn NULL or kind NONE clears it.  Bumps the settings generation (a captured GAN step is re-captured).  B2G_ERR_ARG for an
+ * unknown kind or distribution, p outside (0, 1], std < 0, upper < lower, a non-finite value, a schedule b2g_net_set_dropout_schedule refuses,
+ * or a named layer that does not exist or has no W. */
+int32_t b2g_net_set_weight_noise(b2g_net* net, const char* layer, const b2g_weight_noise* wn);
 /* ComputationGraph.getEpochCount / setEpochCount: the 64-bit device word EPOCH schedules read, 0 at b2g_net_create.  The host sets it, nothing
  * increments it; a new value takes effect at the next update, also in a replayed CUDA graph.  Sync points.  B2G_ERR_ARG for epoch < 0. */
 int32_t b2g_net_get_epoch(b2g_net* net, int64_t* out);
@@ -603,6 +646,10 @@ int32_t b2g_test_bn(b2g_ctx* ctx, int32_t precision, int32_t path, int32_t group
  * which = 0: the straight copy of W in the internal [A][taps][B] order; 1: the packed [(py,px,c)][(dyr,dxc)][O] operand of the
  * pixel-shuffle transposed conv onto <= 4 channels (B2G_ERR_UNSUPPORTED if the layer has none). */
 int32_t b2g_test_net_shadow(b2g_net* net, int32_t layer, int32_t which, float* out, int64_t n);
+/* The noisy operands the latest train-mode pass of a weight-noise layer drew (b2g_weight_noise), widened to fp32 (n = the element count).
+ * which = 0: W' in the internal [A][taps][B] order (the fp32 copy in FP32 nets, the bf16 straight copy in BF16 nets); 1: the packed
+ * pixel-shuffle W' (BF16 nets, layers that have that operand); 2: b' (apply_to_bias).  B2G_ERR_UNSUPPORTED if the layer drew nothing. */
+int32_t b2g_test_net_noisy_operand(b2g_net* net, int32_t layer, int32_t which, float* out, int64_t n);
 /* One DropoutLayer forward and backward on host tensors x, dy of rows*h*w*c elements in NHWC element order (fp32; rounded to bf16 on the
  * device when precision is BF16), through the kernels of the training step, with the mask of (seed, layer, rank, pass) as defined at
  * B2G_LAYER_DROPOUT.  Out: y, dx (same order).  Fails unless the forward advanced its pass counter from pass to pass + 1. */

@@ -39,6 +39,9 @@ public class NeuralNetConfiguration {
         public Builder constrainAllParameters(LayerConstraint... c) { constrainAll = List.of(c); return this; }
         public Builder constrainWeights(LayerConstraint... c) { constrainW = List.of(c); return this; }
         public Builder constrainBias(LayerConstraint... c) { constrainB = List.of(c); return this; }
+        /** The global weight noise: every non-frozen conv, deconv, dense and output layer without its own takes it. */
+        public org.deeplearning4j.nn.conf.weightnoise.IWeightNoise weightNoise;
+        public Builder weightNoise(org.deeplearning4j.nn.conf.weightnoise.IWeightNoise w) { weightNoise = w; return this; }
         public GraphBuilder graphBuilder() { return new GraphBuilder(this); }
     }
 

@@ -34,6 +34,11 @@ public class ComputationGraph {
         for (Layer l : layers) applyConstraints(l);
         for (Layer l : layers)            // new GaussianNoise(ISchedule) etc.: evaluated on the device at every train-mode forward
             if (l.type == 11 && l.dropSchedule != null) setDropoutSchedule(l.name, l.dropSchedule);
+        for (Layer l : layers) {          // DropConnect / WeightNoise: drawn on the device at every train-mode pass
+            boolean gemm = l.type == 0 || l.type == 1 || l.type == 3 || l.type == 7;
+            org.deeplearning4j.nn.conf.weightnoise.IWeightNoise w = l.weightNoise != null ? l.weightNoise : (l.frozen == 0 ? conf.b.g.weightNoise : null);
+            if (gemm && w != null) setWeightNoise(l.name, w);
+        }
     }
     /** The parameters a constrainAllParameters / constrainWeights / constrainBias list reaches on a layer (the library's rule, include/b200gan.h
      *  b2g_constraint, and engine.py constraint_params): weights = W of conv, deconv, dense and output layers, nothing on BatchNorm; bias = b
@@ -93,8 +98,9 @@ public class ComputationGraph {
         Native.check(Native.netGetDropoutValue(net, Native.address(name), Native.address(o))); return o.getFloat(0);
     }
     private void applySchedule(String layerName, ISchedule s) { applySchedule(layerName, s, false); }
-    private void applySchedule(String layerName, ISchedule s, boolean dropout) {
-        ByteBuffer st = null, keys = null, vals = null;      // b2g_lr_schedule (72 bytes) and a MapSchedule's entries
+    /** b2g_lr_schedule (72 bytes) of s in buf[0], a MapSchedule's keys and values in buf[1], buf[2]; all null for s null. */
+    private static ByteBuffer[] scheduleStruct(ISchedule s) {
+        ByteBuffer st = null, keys = null, vals = null;
         if (s != null) {
             int[] k = s.mapKeys(); double[] v = s.mapValues(); double[] p = s.parameters();
             keys = Native.direct(4 * Math.max(1, k.length)); vals = Native.direct(8 * Math.max(1, v.length));
@@ -104,11 +110,29 @@ public class ComputationGraph {
             for (int i = 0; i < 5; ++i) st.putDouble(8 + 8 * i, p[i]);
             st.putInt(48, k.length).putLong(56, Native.address(keys)).putLong(64, Native.address(vals));
         }
+        return new ByteBuffer[] { st, keys, vals };
+    }
+    private void applySchedule(String layerName, ISchedule s, boolean dropout) {
+        ByteBuffer[] sb = scheduleStruct(s); ByteBuffer st = sb[0];
         ByteBuffer name = layerName == null ? null : Native.cstr(layerName);
         final long nameAddr = name == null ? 0 : Native.address(name), stAddr = st == null ? 0 : Native.address(st);
         Native.check(dropout ? Native.netSetDropoutSchedule(net, nameAddr, stAddr) : Native.netSetLrSchedule(net, nameAddr, stAddr));
-        java.lang.ref.Reference.reachabilityFence(st); java.lang.ref.Reference.reachabilityFence(keys); java.lang.ref.Reference.reachabilityFence(vals);
+        java.lang.ref.Reference.reachabilityFence(sb);
         java.lang.ref.Reference.reachabilityFence(name);   // the native side reads these buffers only through their addresses
+    }
+    /** Layer.Builder.weightNoise after init: DropConnect or WeightNoise on one layer (layerName null: every non-frozen conv, deconv, dense and
+     *  output layer; w null: none). */
+    public void setWeightNoise(String layerName, org.deeplearning4j.nn.conf.weightnoise.IWeightNoise w) {
+        ByteBuffer b = null; ByteBuffer[] sb = scheduleStruct(w == null ? null : w.pSchedule());
+        if (w != null) {                    // b2g_weight_noise: kind, apply_to_bias, p, (pad), p_schedule, dist, a, b, additive (40 bytes)
+            b = Native.direct(40);
+            b.putInt(0, w.kind()).putInt(4, w.applyToBias() ? 1 : 0).putFloat(8, (float) w.p()).putLong(16, sb[0] == null ? 0 : Native.address(sb[0]));
+            if (w.distribution() != null) b.putInt(24, w.distribution().kind()).putFloat(28, (float) w.distribution().a()).putFloat(32, (float) w.distribution().b());
+            b.putInt(36, w.additive() ? 1 : 0);
+        }
+        ByteBuffer name = layerName == null ? null : Native.cstr(layerName);
+        Native.check(Native.netSetWeightNoise(net, name == null ? 0 : Native.address(name), b == null ? 0 : Native.address(b)));
+        java.lang.ref.Reference.reachabilityFence(b); java.lang.ref.Reference.reachabilityFence(sb); java.lang.ref.Reference.reachabilityFence(name);
     }
     /** The learning rate the layer's next update uses (its schedule's value at the current iteration / epoch, or its constant lr). */
     public double getLearningRate(String layerName) {

@@ -66,6 +66,10 @@ FN(netSetDropoutSchedule)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlon
 FN(netGetDropoutValue)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong outAddr) {
   return b2g_net_get_dropout_value(P(b2g_net*, net), P(const char*, layerNameAddr), P(float*, outAddr));
 }
+// b2g_weight_noise (40 bytes, its p_schedule laid out as for netSetLrSchedule); layerNameAddr 0: every non-frozen layer with a W; 0: none
+FN(netSetWeightNoise)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong wnAddr) {
+  return b2g_net_set_weight_noise(P(b2g_net*, net), P(const char*, layerNameAddr), P(const b2g_weight_noise*, wnAddr));
+}
 FN(netGetEpoch)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_get_epoch(P(b2g_net*, net), P(int64_t*, outAddr)); }
 FN(netSetEpoch)(JNIEnv_*, jclass, jlong net, jlong epoch) { return b2g_net_set_epoch(P(b2g_net*, net), epoch); }
 FN(netSimtGemmCalls)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_simt_gemm_calls(P(b2g_net*, net), P(uint64_t*, outAddr)); }

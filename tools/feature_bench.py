@@ -242,6 +242,31 @@ def noise_model(fwd_kernel, fwd_bytes, bwd_kernel, bwd_bytes):
     return model
 
 
+# ---------------------------------------------------------------- weightnoise: DropConnect(0.9) on every GEMM layer of D (C5, C2); on C5 also
+# WeightNoise(Normal(0, 0.01)) on every layer of G
+def g_normal_noise(net):
+    if net.specs[0]["name"].startswith("gen"):
+        net.set_weight_noise(m.weight_noise(m.normal(0.0, 0.01)))
+
+
+def weight_noise_model(cfg, G, D, n):
+    """Bytes per noisy bf16 weight and draw: read the fp32 master (4 B), write the bf16 straight copy (2 B), and 2 B more for a layer with the
+    packed pixel-shuffle copy (a 4x4 s2 p1 conv from or transposed conv onto <= 4 channels, 64k units: C2's D-first and G-last).  D draws in
+    both of its passes per step, G in its one train-mode pass; biases are not perturbed."""
+    def per_draw(net):
+        tot = 0
+        for sp in with_n_in(net):
+            if sp.get("weight_noise") is None:
+                continue
+            k = sp.get("kernel", (1, 1)) if sp["type"] in ("conv2d", "deconv2d") else (1, 1)
+            nw = sp["n_in"] * sp["n_out"] * k[0] * k[1]
+            img, units = (sp["n_out"], sp["n_in"]) if sp["type"] == "deconv2d" else (sp["n_in"], sp["n_out"])
+            packed = tuple(k) == (4, 4) and tuple(sp.get("stride", ())) == (2, 2) and tuple(sp.get("padding", ())) == (1, 1) and img <= 4 and units % 64 == 0
+            tot += nw * (8 if packed else 6)
+        return tot
+    return {"bytes_per_draw_D": per_draw(D), "bytes_per_draw_G": per_draw(G), "bytes_per_step": 2 * per_draw(D) + per_draw(G)}
+
+
 # ---------------------------------------------------------------- gradnorm: RenormalizeL2PerLayer on C5, ClipL2PerLayer(1.0) on C2
 def gradnorm_model(cfg, G, D, n):
     """The norm kernel reads every gradient once, 4 B per parameter of G and D per step (it writes one double per 4096 parameters and one
@@ -477,6 +502,10 @@ FEATURES = {
     "schedule": dict(configs="c5,c2", variants=[dict(kernels=UPDATER, model=params_model),
                                                 dict(name="exponential_schedule", hook=schedule, kernels=UPDATER, model=params_model)]),
     "updater": dict(configs="c5,c2", variants=[updater(k) for k in ("adam", "nesterovs", "adagrad", "adamax", "nadam", "amsgrad", "adadelta")]),
+    "weightnoise": dict(configs="c5,c2", variants=[
+        {}, dict(name="dropconnect", d=dict(drop_connect=0.9), kernels=("weight_noise_kernel",), model=weight_noise_model),
+        dict(name="dropconnect+g_normal", only=("c5",), d=dict(drop_connect=0.9), hook=g_normal_noise, kernels=("weight_noise_kernel",),
+             model=weight_noise_model)]),
 }
 
 
