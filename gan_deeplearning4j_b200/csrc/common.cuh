@@ -68,6 +68,17 @@ __device__ __forceinline__ Philox4 philox4x32_10(uint32_t c0, uint32_t c1, uint3
   }
   return Philox4{{c0, c1, c2, c3}};
 }
+__device__ __forceinline__ uint32_t pick4(const Philox4& r, unsigned j) { return j == 0 ? r.x[0] : j == 1 ? r.x[1] : j == 2 ? r.x[2] : r.x[3]; }
+
+// Box-Muller of one Philox word pair (DropoutLayer kinds, weight noise, weight initialization) (include/b200gan.h
+// b2g_dropout_kind): u and v are exact, so the draw depends only on logf / sqrtf / sincospif
+__device__ __forceinline__ void box_muller(uint32_t xe, uint32_t xo, float& ze, float& zo) {
+  const float u = ((float)(xe >> 9) + 0.5f) * 0x1p-23f, v = (float)(xo >> 8) * 0x1p-24f;
+  const float r = sqrtf(-2.0f * logf(u));
+  float sn, cs; sincospif(2.0f * v, &sn, &cs);
+  ze = r * cs; zo = r * sn;
+}
+__device__ __forceinline__ void normals4(const Philox4& r, float (&z)[4]) { box_muller(r.x[0], r.x[1], z[0], z[1]); box_muller(r.x[2], r.x[3], z[2], z[3]); }
 
 #define DISPATCH_PREC(prec, T, ...)                                   \
   do {                                                                \

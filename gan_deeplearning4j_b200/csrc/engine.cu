@@ -1857,6 +1857,91 @@ extern "C" int32_t b2g_net_set_weight_noise(b2g_net* n, const char* layer, const
   return 0;
 }
 
+// ------------------------------------------------------------------ weight initialization (b2g_net_init_weights) --------------------------
+static int32_t check_weight_init(const b2g_weight_init& w) {
+  if (w.scheme < B2G_WI_DISTRIBUTION || w.scheme > B2G_WI_VAR_SCALING_UNIFORM_FAN_AVG) return fail(B2G_ERR_ARG, "unknown weight init scheme %d", w.scheme);
+  if (!std::isfinite(w.bias_init)) return fail(B2G_ERR_ARG, "biasInit %g is not finite", (double)w.bias_init);
+  if (w.scheme != B2G_WI_DISTRIBUTION) return 0;
+  if (w.dist < B2G_DIST_NORMAL || w.dist > B2G_DIST_ORTHOGONAL) return fail(B2G_ERR_ARG, "unknown distribution %d", w.dist);
+  if (w.dist == B2G_DIST_ORTHOGONAL) return fail(B2G_ERR_UNSUPPORTED, "OrthogonalDistribution is not supported (it needs an SVD)");
+  if (!std::isfinite(w.a) || (w.dist != B2G_DIST_CONSTANT && !std::isfinite(w.b))) return fail(B2G_ERR_ARG, "distribution parameters must be finite");
+  switch (w.dist) {
+    case B2G_DIST_NORMAL: case B2G_DIST_TRUNCATED_NORMAL: case B2G_DIST_LOG_NORMAL:
+      if (w.b < 0.f) return fail(B2G_ERR_ARG, "distribution std %g < 0", (double)w.b);
+      break;
+    case B2G_DIST_UNIFORM: if (w.b < w.a) return fail(B2G_ERR_ARG, "UniformDistribution upper %g < lower %g", (double)w.b, (double)w.a); break;
+    case B2G_DIST_BINOMIAL:
+      if (!(w.a >= 0.f && w.a <= 65536.f && w.a == floorf(w.a))) return fail(B2G_ERR_ARG, "BinomialDistribution nTrials %g is not a whole number in [0, 65536]", (double)w.a);
+      if (!(w.b >= 0.f && w.b <= 1.f)) return fail(B2G_ERR_ARG, "BinomialDistribution p %g outside [0, 1]", (double)w.b);
+      break;
+    default: break;
+  }
+  return 0;
+}
+// The draw of one layer's W under the scheme, from the desc's fans (the internal geometry of a 1x1-map deconv or whole-input conv aside)
+static int32_t weight_init_draw(const b2g_weight_init& w, const LayerRT& l, WiDraw* out) {
+  const b2g_layer_desc& d = l.d;
+  const bool conv = d.type == B2G_LAYER_CONV2D || d.type == B2G_LAYER_DECONV2D;
+  const double fi = (double)d.n_in * l.wTaps, fo = (double)d.n_out * l.wTaps / (conv ? (double)(d.s_h * d.s_w) : 1.0);
+  WiDraw r{}; double sd = -1.0, lim = -1.0, tsd = -1.0;
+  switch (w.scheme) {
+    case B2G_WI_DISTRIBUTION:
+      r.kind = w.dist; r.a = w.a; r.b = w.b;
+      if (w.dist == B2G_DIST_BINOMIAL) { r.trials = (int)w.a; r.thr = (uint64_t)floor((double)w.b * 4294967296.0); }
+      break;
+    case B2G_WI_ZERO: r.kind = WI_CONSTANT; r.a = 0.f; break;
+    case B2G_WI_ONES: r.kind = WI_CONSTANT; r.a = 1.f; break;
+    case B2G_WI_SIGMOID_UNIFORM: lim = 4.0 * sqrt(6.0 / (fi + fo)); break;
+    case B2G_WI_NORMAL: case B2G_WI_LECUN_NORMAL: case B2G_WI_XAVIER_FAN_IN: sd = 1.0 / sqrt(fi); break;
+    case B2G_WI_UNIFORM: lim = 1.0 / sqrt(fi); break;
+    case B2G_WI_XAVIER: sd = sqrt(2.0 / (fi + fo)); break;
+    case B2G_WI_XAVIER_UNIFORM: lim = sqrt(6.0) / sqrt(fi + fo); break;
+    case B2G_WI_XAVIER_LEGACY: sd = 1.0 / sqrt((double)d.n_in + d.n_out); break;
+    case B2G_WI_RELU: sd = sqrt(2.0 / fi); break;
+    case B2G_WI_RELU_UNIFORM: lim = sqrt(6.0 / fi); break;
+    case B2G_WI_IDENTITY:
+      if (conv) return fail(B2G_ERR_SHAPE, "layer %s: WeightInit.IDENTITY needs a dense or output layer, not a convolution", d.name);
+      if (d.n_in != d.n_out) return fail(B2G_ERR_SHAPE, "layer %s: WeightInit.IDENTITY needs a square W, got nIn %d != nOut %d", d.name, d.n_in, d.n_out);
+      r.kind = WI_IDENTITY; break;
+    case B2G_WI_LECUN_UNIFORM: case B2G_WI_VAR_SCALING_UNIFORM_FAN_IN: lim = 3.0 / sqrt(fi); break;
+    case B2G_WI_VAR_SCALING_NORMAL_FAN_IN: tsd = sqrt(1.0 / fi); break;
+    case B2G_WI_VAR_SCALING_NORMAL_FAN_OUT: tsd = sqrt(1.0 / fo); break;
+    case B2G_WI_VAR_SCALING_NORMAL_FAN_AVG: tsd = sqrt(2.0 / (fi + fo)); break;
+    case B2G_WI_VAR_SCALING_UNIFORM_FAN_OUT: lim = 3.0 / sqrt(fo); break;
+    case B2G_WI_VAR_SCALING_UNIFORM_FAN_AVG: lim = 3.0 / sqrt((fi + fo) / 2.0); break;
+    default: return fail(B2G_ERR_ARG, "unknown weight init scheme %d", w.scheme);
+  }
+  if (sd >= 0.0) { r.kind = WI_NORMAL; r.a = 0.f; r.b = (float)sd; }
+  if (tsd >= 0.0) { r.kind = WI_TRUNCATED_NORMAL; r.a = 0.f; r.b = (float)tsd; }
+  if (lim >= 0.0) { r.kind = WI_UNIFORM; r.a = -(float)lim; r.b = (float)lim; }
+  *out = r;
+  return 0;
+}
+extern "C" int32_t b2g_net_init_weights(b2g_net* n, const char* layer, const b2g_weight_init* wi) {
+  if (!n || !wi) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
+  const b2g_weight_init w = *wi;
+  B2(check_weight_init(w));
+  std::vector<int> targets;
+  if (layer) {
+    for (size_t i = 0; i < n->L.size() && targets.empty(); ++i) if (!strncmp(n->L[i].d.name, layer, B2G_NAME_LEN)) {
+      if (!n->L[i].has_gemm()) return fail(B2G_ERR_ARG, "layer %s has no W (weight init needs a conv, deconv, dense or output layer)", layer);
+      targets.push_back((int)i);
+    }
+    if (targets.empty()) return fail(B2G_ERR_ARG, "no layer named %s", layer);
+  } else for (size_t i = 0; i < n->L.size(); ++i) if (n->L[i].has_gemm()) targets.push_back((int)i);
+  std::vector<WiDraw> draws(targets.size());
+  for (size_t k = 0; k < targets.size(); ++k) B2(weight_init_draw(w, n->L[targets[k]], &draws[k]));    // every target checked before any write
+  cudaStream_t s = n->ctx->stream;
+  const uint64_t seed = n->cfg.seed ? n->cfg.seed : 666;
+  for (size_t k = 0; k < targets.size(); ++k) {
+    const LayerRT& l = n->L[targets[k]];
+    k_weight_init(n->params + l.off_W, l.wA, l.wTaps, l.wB, draws[k], l.off_b >= 0 ? n->params + l.off_b : nullptr, l.d.n_out, w.bias_init, seed, targets[k], s);
+    net_refresh_shadow(n, targets[k]);
+  }
+  CU(cudaStreamSynchronize(s)); CHECK_KERNELS();
+  return 0;
+}
+
 // The epoch word lives on the device like the iteration counter: a replayed graph reads the value set last, no re-capture needed.
 extern "C" int32_t b2g_net_get_epoch(b2g_net* n, int64_t* out) {
   if (!n || !out) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));

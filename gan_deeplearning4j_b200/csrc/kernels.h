@@ -296,6 +296,18 @@ struct WnJob {
 void k_weight_noise(const WnJob* jobs, int njobs, int nblocks, uint64_t seed, int rank, const int* step, const int64_t* epoch, unsigned long long* pass,
                     unsigned* ticket, int bump_pass, cudaStream_t s);
 
+// ---- weight initialization (DL4J WeightInit / Distribution / biasInit; definitions at b2g_weight_init in include/b200gan.h; kernels_init.cu) ----
+// What a scheme draws, resolved on the host: a b2g_distribution_kind (not ORTHOGONAL) with its fp32 parameters, or WI_IDENTITY.
+enum { WI_NORMAL = 0, WI_UNIFORM = 1, WI_TRUNCATED_NORMAL = 2, WI_LOG_NORMAL = 3, WI_BINOMIAL = 4, WI_CONSTANT = 5, WI_IDENTITY = 6 };
+struct WiDraw {
+  int kind;
+  float a, b;                    // NORMAL / TRUNCATED_NORMAL / LOG_NORMAL (mean, std); UNIFORM (lower, upper); CONSTANT a
+  int trials; uint64_t thr;      // BINOMIAL: nTrials and floor(p 2^32) (up to 2^32)
+};
+// W (the fp32 master of A*taps*B elements in the internal [A][taps][B] order) drawn element by element at its DL4J view index j =
+// (a*B + b)*taps + t, with counter word 3 = layer | 0x80000000; bias[0, n_bias) = bias_init (bias may be null).  One launch.
+void k_weight_init(float* w, int A, int taps, int B, const WiDraw& d, float* bias, int n_bias, float bias_init, uint64_t seed, int layer, cudaStream_t s);
+
 // ---- L2 gradient normalization (DL4J GradientNormalization.{Renormalize,Clip}L2Per{Layer,ParamType}; kernels_gradnorm.cu) ---------
 // A norm group is a run of updater segments: one layer's segments, or one segment.  Its chunks are [chunk_begin, chunk_end) of the updater's
 // chunk map, its segments [seg_begin, seg_end).

@@ -32,7 +32,6 @@ __device__ __forceinline__ void ld16(const float* p, float (&v)[4]) { const floa
 __device__ __forceinline__ void ld16(const __nv_bfloat16* p, float (&v)[8]) { unpack8(*reinterpret_cast<const uint4*>(p), v); }
 __device__ __forceinline__ void st16(float* p, const float (&v)[4]) { *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]); }
 __device__ __forceinline__ void st16(__nv_bfloat16* p, const float (&v)[8]) { *reinterpret_cast<uint4*>(p) = pack8(v); }
-__device__ __forceinline__ uint32_t pick4(const Philox4& r, unsigned j) { return j == 0 ? r.x[0] : j == 1 ? r.x[1] : j == 2 ? r.x[2] : r.x[3]; }
 
 template <typename T>
 __global__ void __launch_bounds__(256) dropout_fwd_kernel(const T* __restrict__ x, T* __restrict__ y, uint32_t* __restrict__ mask, size_t n, int vec,
@@ -113,14 +112,6 @@ void k_dropout_bwd(int prec, const void* eo, void* ei, const uint32_t* mask, siz
 // The vector loops take one 16-byte vector per thread and iteration: one Philox call per 4 elements and one Box-Muller per 2.  The tails run
 // one element per thread.  The per-element masks are written the way dropout_fwd_kernel writes them (a warp assembles whole words).
 
-// Box-Muller of one Philox word pair (include/b200gan.h b2g_dropout_kind): u and v are exact, so the draw depends only on logf / sqrtf / sincospif
-__device__ __forceinline__ void box_muller(uint32_t xe, uint32_t xo, float& ze, float& zo) {
-  const float u = ((float)(xe >> 9) + 0.5f) * 0x1p-23f, v = (float)(xo >> 8) * 0x1p-24f;
-  const float r = sqrtf(-2.0f * logf(u));
-  float sn, cs; sincospif(2.0f * v, &sn, &cs);
-  ze = r * cs; zo = r * sn;
-}
-__device__ __forceinline__ void normals4(const Philox4& r, float (&z)[4]) { box_muller(r.x[0], r.x[1], z[0], z[1]); box_muller(r.x[2], r.x[3], z[2], z[3]); }
 __device__ __forceinline__ float normal1(const Philox4& r, unsigned j) {
   float ze, zo; box_muller(pick4(r, j & 2u), pick4(r, (j & 2u) + 1u), ze, zo);
   return (j & 1u) ? zo : ze;

@@ -255,6 +255,54 @@ def weight_noise_struct(wn: Optional[Dict]):
     return s, keep
 
 
+# Weight initialization of a GEMM layer spec's "weight_init" (b2g_weight_init in include/b200gan.h; models.weight_init): DL4J's WeightInit
+# ordinals, and every b2g_distribution_kind with its two parameter keys (ORTHOGONAL is refused)
+WEIGHT_INIT_SCHEMES = {"distribution": 0, "zero": 1, "ones": 2, "sigmoid_uniform": 3, "normal": 4, "lecun_normal": 5, "uniform": 6, "xavier": 7,
+                       "xavier_uniform": 8, "xavier_fan_in": 9, "xavier_legacy": 10, "relu": 11, "relu_uniform": 12, "identity": 13,
+                       "lecun_uniform": 14, "var_scaling_normal_fan_in": 15, "var_scaling_normal_fan_out": 16, "var_scaling_normal_fan_avg": 17,
+                       "var_scaling_uniform_fan_in": 18, "var_scaling_uniform_fan_out": 19, "var_scaling_uniform_fan_avg": 20}
+INIT_DISTRIBUTIONS = {"normal": (0, "mean", "std"), "uniform": (1, "lower", "upper"), "truncated_normal": (2, "mean", "std"),
+                      "log_normal": (3, "mean", "std"), "binomial": (4, "n_trials", "p"), "constant": (5, "value", None),
+                      "orthogonal": (6, "gain", None)}
+
+
+def weight_init_struct(wi: Dict, spec: Optional[Dict] = None):
+    """A weight-init dict (models.weight_init) -> b2g_weight_init, with ValueError for whatever b2g_net_init_weights refuses: an unknown
+    scheme or distribution, OrthogonalDistribution, DISTRIBUTION without a distribution or with a non-finite or out-of-range parameter, a
+    non-finite bias_init; with the layer's spec also IDENTITY on a convolution or on a dense layer whose given nIn != nOut."""
+    scheme = wi.get("weight_init")
+    if scheme not in WEIGHT_INIT_SCHEMES:
+        raise ValueError(f"unknown weight init {scheme!r}; one of {sorted(WEIGHT_INIT_SCHEMES)}")
+    s = _lib.WeightInit()
+    s.scheme, s.bias_init = WEIGHT_INIT_SCHEMES[scheme], float(wi.get("bias_init", 0.0))
+    if not np.isfinite(np.float32(s.bias_init)):
+        raise ValueError(f"bias_init {wi.get('bias_init')!r} is not finite")
+    if scheme == "distribution":
+        dist = wi.get("distribution") or {}
+        kind = dist.get("distribution")
+        if kind not in INIT_DISTRIBUTIONS:
+            raise ValueError(f"weight init 'distribution' needs a distribution; got {kind!r}, one of {sorted(INIT_DISTRIBUTIONS)}")
+        if kind == "orthogonal":
+            raise ValueError("OrthogonalDistribution is not supported (it needs an SVD)")
+        code, ka, kb = INIT_DISTRIBUTIONS[kind]
+        s.dist, s.a, s.b = code, float(dist[ka]), float(dist[kb]) if kb else 0.0
+        a, b = np.float32(s.a), np.float32(s.b)
+        if not (np.isfinite(a) and np.isfinite(b)):
+            raise ValueError(f"{kind} distribution parameters must be finite: {dist}")
+        if kind in ("normal", "truncated_normal", "log_normal") and b < 0:
+            raise ValueError(f"{kind} distribution std {dist['std']} < 0")
+        if kind == "uniform" and b < a:
+            raise ValueError(f"uniform distribution upper {dist['upper']} < lower {dist['lower']}")
+        if kind == "binomial" and not (0 <= a <= 65536 and a == np.floor(a) and 0 <= b <= 1):
+            raise ValueError(f"binomial distribution needs a whole n_trials in [0, 65536] and p in [0, 1]: {dist}")
+    if scheme == "identity" and spec is not None:
+        if spec["type"] not in ("dense", "output"):
+            raise ValueError(f"layer {spec.get('name', '')!r}: weight init 'identity' needs a dense or output layer")
+        if spec.get("n_in") and spec["n_in"] != spec.get("n_out"):
+            raise ValueError(f"layer {spec.get('name', '')!r}: weight init 'identity' needs nIn == nOut, got {spec['n_in']} and {spec.get('n_out')}")
+    return s
+
+
 def layer_desc(spec: Dict, skip: Optional[tuple] = None) -> LayerDesc:
     """skip: the vertex's (j, order) from resolve_vertices."""
     d = LayerDesc()
@@ -361,12 +409,20 @@ class Net:
     def __init__(self, ctx: Context, specs: Sequence[Dict], input_shape, max_batch: int, precision: int = FP32,
                  grad_clip: float = 0.0, xent_clip_eps: float = 1e-5, bn_groups: int = 1, seed: int = 666,
                  gradient_normalization: str = "none", gradient_normalization_threshold: float = 1.0,
-                 constraints: Optional[Sequence[Dict]] = None, weight_noise: Optional[Dict] = None):
+                 constraints: Optional[Sequence[Dict]] = None, weight_noise: Optional[Dict] = None, weight_init: Optional[Dict] = None):
         """constraints: the global builder's constraints (models.max_norm, ...), for every layer whose own "constraints" reach none of its
         parameters (none given, or e.g. only bias constraints on a BatchNorm), as DL4J's builder fills them in; the specs the net keeps (and a
         checkpoint saves) carry them per layer.  weight_noise: the global builder's weightNoise (models.drop_connect / models.weight_noise) for
-        every non-frozen conv, deconv, dense and output layer without a "weight_noise" of its own; the kept specs carry it per layer."""
+        every non-frozen conv, deconv, dense and output layer without a "weight_noise" of its own; the kept specs carry it per layer.
+        weight_init: the global builder's weightInit / dist / biasInit (models.weight_init) for every conv, deconv, dense and output layer
+        without a "weight_init" of its own, drawn right after creation; the kept specs carry it per layer.  Layers with neither keep
+        b2g_net_create's Xavier draw."""
         self.ctx, self.lib, self.specs = ctx, ctx.lib, copy.deepcopy(list(specs))
+        if weight_init is not None:
+            for sp in self.specs:
+                if sp["type"] in GEMM_TYPES and "weight_init" not in sp:
+                    sp["weight_init"] = copy.deepcopy(weight_init)
+        inits = [(sp["name"], weight_init_struct(sp["weight_init"], sp)) for sp in self.specs if sp["type"] in GEMM_TYPES and sp.get("weight_init") is not None]
         if constraints:
             for sp in self.specs:
                 if sp["type"] in GEMM_TYPES + ("batchnorm",) and not resolve_constraints(sp):
@@ -391,6 +447,8 @@ class Net:
         check(self.lib.b2g_net_output_size(self.h, C.byref(n)))
         self.out_elems = n.value
         try:
+            for name, s in inits:         # Layer.Builder.weightInit / dist / biasInit, at init()
+                check(self.lib.b2g_net_init_weights(self.h, name.encode(), C.byref(s)))
             if gradient_normalization != "none":
                 self.set_gradient_normalization(gradient_normalization, gradient_normalization_threshold)
             for sp in self.specs:         # an updater constructed with an ISchedule: new Adam(new StepSchedule(...))
@@ -564,6 +622,19 @@ class Net:
                 sp["weight_noise"] = copy.deepcopy(weight_noise)
             if layer is not None:
                 break
+
+    def init_weights(self, weight_init: Dict, layer: Optional[str] = None):
+        """Redraws W and sets b = bias_init now (b2g_net_init_weights; models.weight_init): layer None = every conv, deconv, dense and output
+        layer.  Nothing else changes.  The specs a checkpoint writes follow."""
+        targets = [sp for sp in self.specs if sp["type"] in GEMM_TYPES and (layer is None or sp.get("name") == layer)]
+        if layer is not None:
+            targets = targets[:1]
+        s = weight_init_struct(weight_init)
+        for sp in targets:
+            weight_init_struct(weight_init, sp)          # the IDENTITY shape checks, before anything changes
+        check(self.lib.b2g_net_init_weights(self.h, None if layer is None else layer.encode(), C.byref(s)))
+        for sp in targets:
+            sp["weight_init"] = copy.deepcopy(weight_init)
 
     def noisy_operand(self, layer: int, which: int, size: int) -> np.ndarray:
         """What the latest train-mode pass of a weight-noise layer drew (b2g_test_net_noisy_operand): which 0 = W' in the internal order, 1 = the

@@ -160,6 +160,43 @@ def weight_noise(distribution, apply_to_bias=False, additive=True) -> Dict:
     return {"weight_noise": "weight_noise", "distribution": dict(distribution), "apply_to_bias": bool(apply_to_bias), "additive": bool(additive)}
 
 
+# ------------------------------------------------------------------ weight initialization ---------------
+# Layer.Builder / NeuralNetConfiguration.Builder .weightInit, .dist and .biasInit (b2g_weight_init in include/b200gan.h): the value of a GEMM
+# layer spec's "weight_init" key, or of Net(..., weight_init=...) for every GEMM layer without its own.  The distributions below, with normal
+# and uniform above, are DISTRIBUTION's.
+def truncated_normal(mean, std) -> Dict:
+    """new TruncatedNormalDistribution(mean, std): values beyond 2 std are redrawn"""
+    return {"distribution": "truncated_normal", "mean": float(mean), "std": float(std)}
+
+
+def log_normal(mean, std) -> Dict:
+    """new LogNormalDistribution(mean, std): exp of a normal(mean, std)"""
+    return {"distribution": "log_normal", "mean": float(mean), "std": float(std)}
+
+
+def binomial(n_trials, p) -> Dict:
+    """new BinomialDistribution(nTrials, p): ValueError for an nTrials that is not a whole number."""
+    if not math.isfinite(float(n_trials)) or float(n_trials) != math.floor(float(n_trials)):
+        raise ValueError(f"BinomialDistribution nTrials {n_trials!r} is not a whole number")
+    return {"distribution": "binomial", "n_trials": int(n_trials), "p": float(p)}
+
+
+def constant(value) -> Dict:
+    """new ConstantDistribution(value)"""
+    return {"distribution": "constant", "value": float(value)}
+
+
+def weight_init(scheme, dist=None, bias_init=0.0) -> Dict:
+    """.weightInit(WeightInit.<SCHEME>) with .dist(dist) for "distribution" and .biasInit(bias_init): scheme is the lower-case WeightInit name
+    ("xavier", "relu", "var_scaling_normal_fan_avg", ...).  ValueError for what the engine refuses (engine.weight_init_struct)."""
+    from .engine import weight_init_struct
+    wi = {"weight_init": scheme, "bias_init": float(bias_init)}
+    if dist is not None:
+        wi["distribution"] = dict(dist)
+    weight_init_struct(wi)
+    return wi
+
+
 # ------------------------------------------------------------------ pooling layers ---------------------
 # SubsamplingLayer / GlobalPoolingLayer (b2g_pooling in include/b200gan.h).  SubsamplingLayer(MAX) is the "maxpool" spec (unpadded).
 def subsampling(pooling, kernel=(1, 1), stride=(2, 2), padding=(0, 0), pnorm=None, name="") -> Dict:

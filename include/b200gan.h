@@ -315,7 +315,8 @@ int32_t b2g_device_info(b2g_ctx* ctx, int32_t* sm_count, int32_t* cc_major, int3
 
 /* ---------------------------------------------------------------- nets ---------------------------- */
 /* new ComputationGraph(conf).init() (J:118-166): infers nIn, allocates the flattened params/grads/
- * updater-state arena and every activation buffer; Xavier-normal weights, BN gamma=1 beta=0 mean=0 var=1. */
+ * updater-state arena and every activation buffer; Xavier-normal weights, BN gamma=1 beta=0 mean=0 var=1 (b2g_net_init_weights redraws
+ * W and b with any other WeightInit). */
 int32_t b2g_net_create(b2g_ctx* ctx, const b2g_net_config* cfg, const b2g_layer_desc* layers, int32_t n_layers, b2g_net** out);
 int32_t b2g_net_destroy(b2g_net* net);
 int32_t b2g_net_num_params(b2g_net* net, int64_t* out);                       /* ComputationGraph.numParams() */
@@ -492,6 +493,10 @@ int32_t b2g_net_get_dropout_value(b2g_net* net, const char* layer, float* out);
  * one W', as they share DropoutLayer masks.  Buffers: the noisy operands of a layer are allocated when it first gets weight noise. */
 typedef enum { B2G_WEIGHT_NOISE_NONE = 0, B2G_WEIGHT_NOISE_DROPCONNECT = 1, B2G_WEIGHT_NOISE_WEIGHTNOISE = 2 } b2g_weight_noise_kind;
 typedef enum { B2G_DIST_NORMAL = 0, B2G_DIST_UNIFORM = 1 } b2g_distribution_kind;    /* NormalDistribution(mean, std), UniformDistribution(lower, upper) */
+/* The further b2g_distribution_kind values, for weight initialization (b2g_weight_init; weight noise takes NORMAL and UNIFORM only):
+ * TruncatedNormalDistribution(mean, std), LogNormalDistribution(mean, std), BinomialDistribution(nTrials, p), ConstantDistribution(value),
+ * OrthogonalDistribution(gain) (refused).  GaussianDistribution is NORMAL under another name. */
+enum { B2G_DIST_TRUNCATED_NORMAL = 2, B2G_DIST_LOG_NORMAL = 3, B2G_DIST_BINOMIAL = 4, B2G_DIST_CONSTANT = 5, B2G_DIST_ORTHOGONAL = 6 };
 typedef struct {
   int32_t kind;                     /* b2g_weight_noise_kind */
   int32_t apply_to_bias;            /* DropConnect's applyToBiases / WeightNoise's applyToBias */
@@ -506,6 +511,62 @@ typedef struct {
  * unknown kind or distribution, p outside (0, 1], std < 0, upper < lower, a non-finite value, a schedule b2g_net_set_dropout_schedule refuses,
  * or a named layer that does not exist or has no W. */
 int32_t b2g_net_set_weight_noise(b2g_net* net, const char* layer, const b2g_weight_noise* wn);
+
+/* Weight initialization (DL4J 1.0.0-beta3 WeightInitUtil.initWeights with Layer.Builder / NeuralNetConfiguration.Builder .weightInit, .dist and
+ * .biasInit, recalled; parity unpinned like the rest of the DL4J semantics).  The scheme numbers are DL4J's WeightInit ordinals.  Each scheme
+ * draws W from a distribution of the layer's fans:
+ *    0 DISTRIBUTION     the b2g_weight_init's own dist(a, b)          11 RELU                  N(0, sqrt(2 / fanIn))
+ *    1 ZERO             0                                            12 RELU_UNIFORM          U(+-sqrt(6 / fanIn))
+ *    2 ONES             1                                            13 IDENTITY              the identity (square DENSE / OUTPUT only)
+ *    3 SIGMOID_UNIFORM  U(+-4 sqrt(6 / (fanIn + fanOut)))             14 LECUN_UNIFORM         U(+-3 / sqrt(fanIn))
+ *    4 NORMAL           N(0, 1 / sqrt(fanIn))                         15 VAR_SCALING_NORMAL_FAN_IN    T(0, sqrt(1 / fanIn))
+ *    5 LECUN_NORMAL     N(0, 1 / sqrt(fanIn))                         16 VAR_SCALING_NORMAL_FAN_OUT   T(0, sqrt(1 / fanOut))
+ *    6 UNIFORM          U(+-1 / sqrt(fanIn))                          17 VAR_SCALING_NORMAL_FAN_AVG   T(0, sqrt(2 / (fanIn + fanOut)))
+ *    7 XAVIER           N(0, sqrt(2 / (fanIn + fanOut)))              18 VAR_SCALING_UNIFORM_FAN_IN   U(+-3 / sqrt(fanIn))
+ *    8 XAVIER_UNIFORM   U(+-sqrt(6) / sqrt(fanIn + fanOut))           19 VAR_SCALING_UNIFORM_FAN_OUT  U(+-3 / sqrt(fanOut))
+ *    9 XAVIER_FAN_IN    N(0, 1 / sqrt(fanIn))                         20 VAR_SCALING_UNIFORM_FAN_AVG  U(+-3 / sqrt((fanIn + fanOut) / 2))
+ *   10 XAVIER_LEGACY    N(0, 1 / sqrt(nIn + nOut))
+ * N(mean, std) is NORMAL, U(+-r) UNIFORM(-r, r), T(mean, std) TRUNCATED_NORMAL below.  Fans come from the layer desc, whatever geometry the
+ * engine computes the layer with (the 1x1-map deconv, the whole-input conv): CONV2D and DECONV2D fanIn = nIn kH kW, fanOut = nOut kH kW /
+ * (sH sW); DENSE and OUTPUT fanIn = nIn, fanOut = nOut.  Each std or bound is computed in double and rounded to fp32 once.
+ * Draws: S = b2g_net_config.seed (0: 666), L = the layer's index in the desc array, j = the element's index in DL4J's view order of W (what
+ * b2g_net_get_param(layer, "W") returns, so the draw does not depend on the internal layout).  Round k of element j uses word x[j & 3] of
+ * Philox4x32-10(ctr = {j >> 2, k, 0, L | 0x80000000}, key = {lo32(S), hi32(S)}); the top bit keeps these streams apart from every
+ * DropoutLayer and weight-noise draw.  No rank input: every data-parallel replica draws the same W.  Values are fp32:
+ *   NORMAL(mean a, std b >= 0)            fmaf(b, z, a), z = z[j & 3] of round 0's Box-Muller normals of b2g_dropout_kind (|z| <= 5.8)
+ *   UNIFORM(lower a, upper b >= a)        fmaf(b - a, u, a) (b - a in fp32), u = (x >> 8) 2^-24 of round 0
+ *   TRUNCATED_NORMAL(mean a, std b >= 0)  fmaf(b, z, a) with z of the first round k < 16 whose |z| <= 2; none: round 15's z clamped to +-2
+ *   LOG_NORMAL(mean a, std b >= 0)        expf(fmaf(b, z, a)), z as for NORMAL
+ *   BINOMIAL(nTrials a, p b)              the count over rounds t < nTrials of x_t < floor(p 2^32) (p = 1: nTrials); nTrials a whole number
+ *                                         in [0, 65536], p in [0, 1]
+ *   CONSTANT(value a)                     a, no draw (ZERO, ONES and IDENTITY draw nothing either)
+ *   ORTHOGONAL                            refused with B2G_ERR_UNSUPPORTED: it needs an SVD, and DL4J's bits could not be matched anyway.
+ * b2g_net_create's own draw is unchanged: Xavier-normal weights from a host generator and zero biases.  An explicit XAVIER through
+ * b2g_net_init_weights draws the same distribution from the stream above, so it gives other bits. */
+typedef enum {
+  B2G_WI_DISTRIBUTION = 0, B2G_WI_ZERO = 1, B2G_WI_ONES = 2, B2G_WI_SIGMOID_UNIFORM = 3, B2G_WI_NORMAL = 4, B2G_WI_LECUN_NORMAL = 5,
+  B2G_WI_UNIFORM = 6, B2G_WI_XAVIER = 7, B2G_WI_XAVIER_UNIFORM = 8, B2G_WI_XAVIER_FAN_IN = 9, B2G_WI_XAVIER_LEGACY = 10, B2G_WI_RELU = 11,
+  B2G_WI_RELU_UNIFORM = 12, B2G_WI_IDENTITY = 13, B2G_WI_LECUN_UNIFORM = 14, B2G_WI_VAR_SCALING_NORMAL_FAN_IN = 15,
+  B2G_WI_VAR_SCALING_NORMAL_FAN_OUT = 16, B2G_WI_VAR_SCALING_NORMAL_FAN_AVG = 17, B2G_WI_VAR_SCALING_UNIFORM_FAN_IN = 18,
+  B2G_WI_VAR_SCALING_UNIFORM_FAN_OUT = 19, B2G_WI_VAR_SCALING_UNIFORM_FAN_AVG = 20
+} b2g_weight_init_scheme;
+typedef struct {
+  int32_t scheme;       /* b2g_weight_init_scheme */
+  int32_t dist;         /* DISTRIBUTION: a b2g_distribution_kind, B2G_DIST_NORMAL .. B2G_DIST_ORTHOGONAL (the typedef's two and the enum after it) */
+  float a, b;           /* DISTRIBUTION: NORMAL / TRUNCATED_NORMAL / LOG_NORMAL mean, std; UNIFORM lower, upper; BINOMIAL nTrials, p; CONSTANT value */
+  float bias_init;      /* biasInit: every element of b */
+} b2g_weight_init;
+/* DL4J's per-layer initialization at init(): redraws W as above and sets b = bias_init, now.  layer named: Layer.Builder's weightInit / dist /
+ * biasInit; layer NULL: every CONV2D, DECONV2D, DENSE and OUTPUT layer (the global builder's).  Nothing else changes: BatchNorm parameters,
+ * other layers, the updater state, the iteration counter, the dropout pass counter and the epoch word stay as they are.  BF16 nets get the
+ * layer's bf16 operand copy (and its packed pixel-shuffle operand) refreshed.  Call it right after b2g_net_create, as DL4J initializes at
+ * init(); a captured GAN step reads the new weights at its next replay.  Every target is checked before anything is written: a failed call
+ * leaves the net unchanged.  Sync point.
+ * B2G_ERR_ARG: an unknown scheme or distribution; DISTRIBUTION with a non-finite or out-of-range parameter (std < 0, upper < lower, p outside
+ * [0, 1], nTrials not a whole number in [0, 65536]); a non-finite bias_init; a named layer that does not exist or has no W.
+ * B2G_ERR_SHAPE: IDENTITY on a CONV2D or DECONV2D layer, or on a DENSE / OUTPUT layer with nIn != nOut (DL4J throws).
+ * B2G_ERR_UNSUPPORTED: DISTRIBUTION with ORTHOGONAL. */
+int32_t b2g_net_init_weights(b2g_net* net, const char* layer, const b2g_weight_init* wi);
 /* ComputationGraph.getEpochCount / setEpochCount: the 64-bit device word EPOCH schedules read, 0 at b2g_net_create.  The host sets it, nothing
  * increments it; a new value takes effect at the next update, also in a replayed CUDA graph.  Sync points.  B2G_ERR_ARG for epoch < 0. */
 int32_t b2g_net_get_epoch(b2g_net* net, int64_t* out);

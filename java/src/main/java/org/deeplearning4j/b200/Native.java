@@ -40,6 +40,7 @@ public final class Native {
     public static native int netSetDropoutSchedule(long net, long layerNameAddr, long scheduleAddr);   // layerNameAddr 0: every DropoutLayer; scheduleAddr 0: constant
     public static native int netGetDropoutValue(long net, long layerNameAddr, long outAddr);
     public static native int netSetWeightNoise(long net, long layerNameAddr, long weightNoiseAddr);   // b2g_weight_noise; layerNameAddr 0: every layer with a W
+    public static native int netInitWeights(long net, long layerNameAddr, long weightInitAddr);   // b2g_weight_init; layerNameAddr 0: every layer with a W
     public static native int netGetEpoch(long net, long outAddr);
     public static native int netSetEpoch(long net, long epoch);
     public static native int netSimtGemmCalls(long net, long outAddr);

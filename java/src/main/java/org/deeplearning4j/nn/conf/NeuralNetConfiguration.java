@@ -33,7 +33,12 @@ public class NeuralNetConfiguration {
         public Builder gradientNormalizationThreshold(double t) { gradNormThreshold = (float) t; if (!gradNorm.isL2()) clip = (float) t; return this; }
         public Builder l2(double v) { l2 = (float) v; return this; }
         public Builder activation(Activation a) { act = a; return this; }
-        public Builder weightInit(WeightInit w) { return this; }
+        /** The global weightInit / dist / biasInit (null: not given): every conv, deconv, dense and output layer takes what it does not set
+         *  itself.  With none of the three given anywhere a layer keeps the library's default draw. */
+        public WeightInit weightInit; public org.deeplearning4j.nn.conf.distribution.Distribution dist; public Double biasInit;
+        public Builder weightInit(WeightInit w) { weightInit = w; return this; }
+        public Builder dist(org.deeplearning4j.nn.conf.distribution.Distribution d) { dist = d; return this; }
+        public Builder biasInit(double b) { biasInit = b; return this; }
         /** The global constraints: a layer whose own lists reach none of its parameters takes these. */
         public List<LayerConstraint> constrainAll, constrainW, constrainB;
         public Builder constrainAllParameters(LayerConstraint... c) { constrainAll = List.of(c); return this; }

@@ -15,6 +15,8 @@ public class Layer {
     public IUpdater updater; public String name = "";
     public org.nd4j.linalg.schedule.ISchedule dropSchedule;   // DropoutLayer.Builder(IDropout) with an ISchedule: applied by ComputationGraph.init
     public org.deeplearning4j.nn.conf.weightnoise.IWeightNoise weightNoise;   // Layer.Builder.weightNoise (null: the global builder's): applied by ComputationGraph.init
+    /** Layer.Builder.weightInit / dist / biasInit (null: the global builder's): applied by ComputationGraph.init. */
+    public org.deeplearning4j.nn.weights.WeightInit weightInit; public org.deeplearning4j.nn.conf.distribution.Distribution dist; public Double biasInit;
     /** constrainAllParameters / constrainWeights / constrainBias; all null: the global builder's lists apply. */
     public List<LayerConstraint> constrainAll, constrainW, constrainB;
     public boolean alphaSet;   // alpha given by leakyReluAlpha(..) or activation(IActivation); else ELU / ThresholdedReLU write DL4J's 1.0
@@ -30,7 +32,8 @@ public class Layer {
     }
     public Layer copy() { Layer c = new Layer(); c.type = type; c.nIn = nIn; c.nOut = nOut; c.kH = kH; c.kW = kW; c.sH = sH; c.sW = sW; c.pH = pH; c.pW = pW; c.hasBias = hasBias; c.act = act;
         c.preH = preH; c.preW = preW; c.preC = preC; c.loss = loss; c.frozen = frozen; c.alpha = alpha; c.l2 = l2; c.bnDecay = bnDecay; c.bnEps = bnEps; c.updater = updater; c.name = name; c.alphaSet = alphaSet;
-        c.constrainAll = constrainAll; c.constrainW = constrainW; c.constrainB = constrainB; c.dropSchedule = dropSchedule; c.weightNoise = weightNoise; return c; }
+        c.constrainAll = constrainAll; c.constrainW = constrainW; c.constrainB = constrainB; c.dropSchedule = dropSchedule; c.weightNoise = weightNoise;
+        c.weightInit = weightInit; c.dist = dist; c.biasInit = biasInit; return c; }
     protected int defaultAct(Activation g) { return g.code; }   // conv / dense inherit the global .activation(..) (J:126)
 
     @SuppressWarnings("unchecked")
@@ -51,6 +54,9 @@ public class Layer {
         public T constrainWeights(LayerConstraint... c) { l.constrainW = List.of(c); return (T) this; }
         public T constrainBias(LayerConstraint... c) { l.constrainB = List.of(c); return (T) this; }
         public T weightNoise(org.deeplearning4j.nn.conf.weightnoise.IWeightNoise w) { l.weightNoise = w; return (T) this; }
+        public T weightInit(org.deeplearning4j.nn.weights.WeightInit w) { l.weightInit = w; return (T) this; }
+        public T dist(org.deeplearning4j.nn.conf.distribution.Distribution d) { l.dist = d; return (T) this; }
+        public T biasInit(double b) { l.biasInit = b; return (T) this; }
         public Layer build() { return l; }
     }
 }

@@ -7,8 +7,11 @@ import java.util.List;
 import org.deeplearning4j.b200.Native;
 import org.deeplearning4j.nn.api.layers.LayerConstraint;
 import org.deeplearning4j.nn.conf.GradientNormalization;
+import org.deeplearning4j.nn.conf.NeuralNetConfiguration;
 import org.deeplearning4j.nn.conf.NeuralNetConfiguration.ComputationGraphConfiguration;
+import org.deeplearning4j.nn.conf.distribution.Distribution;
 import org.deeplearning4j.nn.conf.layers.Layer;
+import org.deeplearning4j.nn.weights.WeightInit;
 import org.nd4j.linalg.api.ndarray.INDArray;
 import org.nd4j.linalg.dataset.DataSet;
 import org.nd4j.linalg.schedule.ISchedule;
@@ -27,6 +30,13 @@ public class ComputationGraph {
         ByteBuffer h = Native.direct(8);
         Native.check(Native.netCreate(Native.context(), Native.address(cfg), Native.address(desc), layers.size(), Native.address(h)));
         net = h.getLong(0);
+        NeuralNetConfiguration.Builder g = conf.b.g;     // weightInit / dist / biasInit, resolved per layer: its own, else the global builder's
+        boolean global = g.weightInit != null || g.dist != null || g.biasInit != null;
+        for (Layer l : layers) {
+            boolean gemm = l.type == 0 || l.type == 1 || l.type == 3 || l.type == 7;
+            if (gemm && (global || l.weightInit != null || l.dist != null || l.biasInit != null))
+                initWeights(l.name, l.weightInit != null ? l.weightInit : g.weightInit, l.dist != null ? l.dist : g.dist, l.biasInit != null ? l.biasInit : g.biasInit);
+        }
         GradientNormalization gn = conf.b.g.gradNorm;      // RenormalizeL2* / ClipL2*: on-device norms before every update
         if (gn.isL2()) Native.check(Native.netSetGradientNormalization(net, gn.ordinal(), conf.b.g.gradNormThreshold));
         for (Layer l : layers)            // new Adam(ISchedule) / RmsProp(ISchedule) / Sgd(ISchedule): evaluated on the device at every update
@@ -133,6 +143,16 @@ public class ComputationGraph {
         ByteBuffer name = layerName == null ? null : Native.cstr(layerName);
         Native.check(Native.netSetWeightNoise(net, name == null ? 0 : Native.address(name), b == null ? 0 : Native.address(b)));
         java.lang.ref.Reference.reachabilityFence(b); java.lang.ref.Reference.reachabilityFence(sb); java.lang.ref.Reference.reachabilityFence(name);
+    }
+    /** WeightInitUtil.initWeights at init(): redraws W and sets b on one layer (layerName null: every conv, deconv, dense and output layer).
+     *  w null is DL4J's default XAVIER, biasInit null its 0; DISTRIBUTION draws from d. */
+    public void initWeights(String layerName, WeightInit w, Distribution d, Double biasInit) {
+        ByteBuffer b = Native.direct(20);   // b2g_weight_init: scheme, dist, a, b, bias_init (20 bytes)
+        b.putInt(0, (w == null ? WeightInit.XAVIER : w).ordinal()).putInt(4, d == null ? -1 : d.kind()).putFloat(8, d == null ? 0f : (float) d.a())
+         .putFloat(12, d == null ? 0f : (float) d.b()).putFloat(16, biasInit == null ? 0f : biasInit.floatValue());
+        ByteBuffer name = layerName == null ? null : Native.cstr(layerName);
+        Native.check(Native.netInitWeights(net, name == null ? 0 : Native.address(name), Native.address(b)));
+        java.lang.ref.Reference.reachabilityFence(b); java.lang.ref.Reference.reachabilityFence(name);
     }
     /** The learning rate the layer's next update uses (its schedule's value at the current iteration / epoch, or its constant lr). */
     public double getLearningRate(String layerName) {

@@ -70,6 +70,10 @@ FN(netGetDropoutValue)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong o
 FN(netSetWeightNoise)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong wnAddr) {
   return b2g_net_set_weight_noise(P(b2g_net*, net), P(const char*, layerNameAddr), P(const b2g_weight_noise*, wnAddr));
 }
+// b2g_weight_init (20 bytes); layerNameAddr 0: every layer with a W
+FN(netInitWeights)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong wiAddr) {
+  return b2g_net_init_weights(P(b2g_net*, net), P(const char*, layerNameAddr), P(const b2g_weight_init*, wiAddr));
+}
 FN(netGetEpoch)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_get_epoch(P(b2g_net*, net), P(int64_t*, outAddr)); }
 FN(netSetEpoch)(JNIEnv_*, jclass, jlong net, jlong epoch) { return b2g_net_set_epoch(P(b2g_net*, net), epoch); }
 FN(netSimtGemmCalls)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_simt_gemm_calls(P(b2g_net*, net), P(uint64_t*, outAddr)); }

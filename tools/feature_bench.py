@@ -473,6 +473,51 @@ def updater(kind):
     return dict(name=kind, swap=lambda s: with_kind(s, kind), kernels=UPDATER, model=model)
 
 
+# ---------------------------------------------------------------- weightinit: b2g_net_init_weights over bench.py's nets
+INIT_SCHEMES = (("distribution_normal_0.02", m.weight_init("distribution", m.normal(0, 0.02))), ("xavier", m.weight_init("xavier")),
+                ("xavier_uniform", m.weight_init("xavier_uniform")), ("var_scaling_normal_fan_avg", m.weight_init("var_scaling_normal_fan_avg")))
+
+
+def init_weights_times(ctx, configs):
+    """Per config, on G and D as bench.make_gan builds them (BF16): the host time of b2g_net_create, and for a few schemes one
+    b2g_net_init_weights call (layer NULL) on each net, measured two ways after one warm-up pair of calls:
+      call_ms        CUDA events on the library stream around the two calls, median of 5: what a caller waits, host-side checks, one launch
+                     per layer and the closing stream synchronisation included -- a latency, not a kernel time;
+      kernel_us      torch.profiler device time of the weight_init_kernel launches of one pair of calls (mean of 5), and refresh_us that of the
+                     bf16 operand refresh (cast_f32_to_bf16_kernel, pack_deconv_ps_kernel) that follows them.
+    hbm_fraction: the kernel's algorithmic bytes, 4 B written per parameter (BatchNorm's few included), over kernel_us, as a fraction of the
+    3.35 TB/s data sheet."""
+    out = {}
+    for cfg_name in configs:
+        cfg = bench.CONFIGS[cfg_name]
+        t0 = time.perf_counter()
+        G, D, gan = bench.make_gan(b, ctx, cfg, cfg["batch"])
+        create_ms = (time.perf_counter() - t0) * 1e3
+        gan.close()
+        params = G.num_params() + D.num_params()
+        rows = {}
+        for name, wi in INIT_SCHEMES:
+            G.init_weights(wi); D.init_weights(wi)          # warm-up
+            ms = []
+            for _ in range(5):
+                ctx.sync(); ctx.timer_start()
+                G.init_weights(wi); D.init_weights(wi)
+                ms.append(ctx.timer_stop_ms())
+            ctx.sync()
+            with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+                for _ in range(5):
+                    G.init_weights(wi); D.init_weights(wi)
+                ctx.sync()
+            k = kernel_us(prof, "weight_init_kernel")
+            refresh = sum(kernel_us(prof, "cast_f32_to_bf16_kernel")) + sum(kernel_us(prof, "pack_deconv_ps_kernel"))
+            kus = sum(k) / 5
+            rows[name] = {"call_ms": float(np.median(ms)), "kernel_launches": len(k) / 5, "kernel_us": kus, "refresh_us": refresh / 5,
+                          "hbm_fraction": fraction(params * 4, kus)}
+        out[cfg_name] = {"params": params, "net_create_host_ms": create_ms, "init_weights": rows}
+        G.close(); D.close()
+    return out
+
+
 ACT_EXT = ("act_ext_fwd_kernel", "act_ext_bwd_kernel")
 CONSTRAINT = ("constraint_onepass_kernel", "constraint_norm_kernel", "constraint_scale_kernel")
 # each feature: default configs, steps, rounds; its variants ("only": the configs it runs on; "kernels": the in-step kernels to profile);
@@ -502,6 +547,7 @@ FEATURES = {
     "schedule": dict(configs="c5,c2", variants=[dict(kernels=UPDATER, model=params_model),
                                                 dict(name="exponential_schedule", hook=schedule, kernels=UPDATER, model=params_model)]),
     "updater": dict(configs="c5,c2", variants=[updater(k) for k in ("adam", "nesterovs", "adagrad", "adamax", "nadam", "amsgrad", "adadelta")]),
+    "weightinit": dict(configs="c4,c2", variants=[], extras=lambda ctx, configs, steps: {"init_weights": init_weights_times(ctx, configs)}),
     "weightnoise": dict(configs="c5,c2", variants=[
         {}, dict(name="dropconnect", d=dict(drop_connect=0.9), kernels=("weight_noise_kernel",), model=weight_noise_model),
         dict(name="dropconnect+g_normal", only=("c5",), d=dict(drop_connect=0.9), hook=g_normal_noise, kernels=("weight_noise_kernel",),
