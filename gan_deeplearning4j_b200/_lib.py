@@ -55,6 +55,11 @@ class WeightInit(C.Structure):
     _fields_ = [("scheme", C.c_int32), ("dist", C.c_int32), ("a", C.c_float), ("b", C.c_float), ("bias_init", C.c_float)]
 
 
+class Regularization(C.Structure):
+    """b2g_regularization: l1 and l2 on W, l1_bias and l2_bias on b."""
+    _fields_ = [("l1", C.c_float), ("l2", C.c_float), ("l1_bias", C.c_float), ("l2_bias", C.c_float)]
+
+
 class Constraint(C.Structure):
     """b2g_constraint: one DL4J LayerConstraint on one parameter tensor (kind, DL4J dimensions as a bit mask, bounds, MinMaxNorm's rate)."""
     _fields_ = [("kind", C.c_int32), ("dims_mask", C.c_int32), ("max_norm", C.c_double), ("min_norm", C.c_double), ("rate", C.c_double)]
@@ -142,6 +147,9 @@ PROTOTYPES = {
     "b2g_net_get_dropout_value": (_i32, [_vp, C.c_char_p, _fp]),
     "b2g_net_set_weight_noise": (_i32, [_vp, C.c_char_p, C.POINTER(WeightNoise)]),
     "b2g_net_init_weights": (_i32, [_vp, C.c_char_p, C.POINTER(WeightInit)]),
+    "b2g_net_set_regularization": (_i32, [_vp, C.c_char_p, C.POINTER(Regularization)]),
+    "b2g_net_get_regularization": (_i32, [_vp, C.c_char_p, C.POINTER(Regularization)]),
+    "b2g_net_calc_regularization": (_i32, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "b2g_net_get_epoch": (_i32, [_vp, C.POINTER(_i64)]),
     "b2g_net_set_epoch": (_i32, [_vp, _i64]),
     "b2g_net_simt_gemm_calls": (_i32, [_vp, C.POINTER(C.c_uint64)]),

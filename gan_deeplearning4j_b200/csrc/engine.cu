@@ -83,6 +83,7 @@ struct LayerRT {
   size_t in_elems = 0, out_elems = 0;
   ConvGeom geom{};                                             // conv-equivalent geometry (N filled per call)
   int64_t off_W = -1, n_W = 0, off_b = -1, off_gamma = -1, off_beta = -1, off_mean = -1, off_var = -1;
+  b2g_regularization reg{};                                    // l1, l2 (W), l1_bias, l2_bias (b) of a GEMM layer (b2g_net_set_regularization)
   int64_t off_W_bf = -1;                                       // bf16 operand copy [A][taps][B] (written by the updater itself); serves fprop, dgrad (MN-major tiles) and wgrad
   int64_t off_Wps_bf = -1;                                     // packed [16][9][O] weights of the tensor-core pixel-shuffle transposed conv (<= 4 image channels)
   int wA = 0, wTaps = 0, wB = 0;                               // internal weight layout [A][taps][B]
@@ -148,7 +149,10 @@ struct b2g_net {
   bool upd_ext = false;                // some segment has a kind >= 4: the updater runs its extended instantiations
   __nv_bfloat16* shadow = nullptr; int64_t n_shadow = 0;
   std::vector<UpdSeg> segs; UpdSeg* segs_dev = nullptr; int32_t* chunk_seg_dev = nullptr; int64_t* chunk_off_dev = nullptr; int nchunks = 0;
-  int64_t *l2_off_dev = nullptr, *l2_len_dev = nullptr; float* l2_coef_dev = nullptr; int n_l2 = 0;
+  // Regularization score: one entry per W and b of every non-frozen GEMM layer, in segment order (reg_seg: the entry's segment), with the
+  // fp32 coefficients of its l2 term (0.5 * l2) and l1 term on the host and the device; n_l2 / n_l1: entries with a non-zero coefficient
+  std::vector<int> reg_seg; std::vector<float> reg_l2c, reg_l1c;
+  int64_t *reg_off_dev = nullptr, *reg_len_dev = nullptr; float *reg_l2c_dev = nullptr, *reg_l1c_dev = nullptr; int n_l2 = 0, n_l1 = 0;
   int* step_dev = nullptr;
   int max_rows = 0;                    // cfg.max_batch
   size_t in_elems = 0;
@@ -191,7 +195,7 @@ struct b2g_net {
   float* scratch = nullptr; size_t scratch_floats = 0;
   float* loss_dev = nullptr;           // [8]
   double* loss_partial = nullptr; unsigned* loss_ticket = nullptr;   // k_loss's per-block sums and its ticket
-  double* l2_dev = nullptr;
+  double* reg_dev = nullptr;          // [2]: the score's L2 and L1 sums
   void* input_grad = nullptr;          // where the last backward left d(loss)/d(input), or null
   int last_rows = 0;
   cudaStream_t fwd_stream = nullptr;   // when set, net_forward launches here instead of ctx->stream
@@ -414,7 +418,7 @@ static int32_t net_alloc(b2g_net* n) {
   B2(dalloc(n, &n->upd_ticket, sizeof(unsigned))); CU(cudaMemsetAsync(n->upd_ticket, 0, sizeof(unsigned), n->ctx->stream));
   B2(dalloc(n, &n->drop_pass, sizeof(unsigned long long))); CU(cudaMemsetAsync(n->drop_pass, 0, sizeof(unsigned long long), n->ctx->stream));
   B2(dalloc(n, &n->drop_ticket, sizeof(unsigned))); CU(cudaMemsetAsync(n->drop_ticket, 0, sizeof(unsigned), n->ctx->stream));
-  B2(dalloc(n, &n->step_dev, sizeof(int))); B2(dalloc(n, &n->loss_dev, sizeof(float) * 8)); B2(dalloc(n, &n->l2_dev, sizeof(double)));
+  B2(dalloc(n, &n->step_dev, sizeof(int))); B2(dalloc(n, &n->loss_dev, sizeof(float) * 8)); B2(dalloc(n, &n->reg_dev, 2 * sizeof(double)));
   B2(dalloc(n, &n->labels_dev, sizeof(float) * R * std::max<size_t>(1, n->L.back().out_elems)));
   {  // k_loss's per-block sums for one group of max_batch rows (fit) or two of max_batch / 2 (the GAN step's D pass)
     const size_t per = n->L.back().out_elems;
@@ -504,19 +508,20 @@ static int32_t net_init_params_and_updater(b2g_net* n) {
   cudaStream_t s = n->ctx->stream;
   std::vector<float> hp(n->n_params, 0.f), h0(n->n_params, 0.f);
   uint64_t seed = n->cfg.seed ? n->cfg.seed : 666;
-  std::vector<int64_t> l2o, l2l; std::vector<float> l2c;
+  std::vector<int64_t> rego, regl;
   std::vector<int> seg_layer;      // layer index of every segment (the norm groups of the PerLayer modes)
   for (auto& l : n->L) {
     const b2g_layer_desc& d = l.d;
     auto add_seg = [&](int64_t off, int64_t len, bool weight, bool noop) {
       if (d.frozen) return;      // FrozenLayer: no update, no l2 decay, no l2 score (calcL2() == 0)
       UpdSeg sg{}; sg.off = off; sg.len = len; sg.kind = noop ? 3 : updater_kind(d.updater);
-      sg.lr = d.lr; sg.b1 = d.beta1; sg.b2 = d.beta2; sg.eps = d.eps; sg.l2 = weight ? d.l2 : 0.f; sg.clip = n->cfg.grad_clip; sg.div_mb = noop ? 0 : 1;
+      sg.lr = d.lr; sg.b1 = d.beta1; sg.b2 = d.beta2; sg.eps = d.eps; sg.l2 = weight ? d.l2 : 0.f; sg.l1 = 0.f; sg.clip = n->cfg.grad_clip; sg.div_mb = noop ? 0 : 1;
       sg.off_bf = (weight && l.off_W_bf >= 0) ? l.off_W_bf : -1; sg.off_ps = (weight && l.off_Wps_bf >= 0) ? l.off_Wps_bf : -1; sg.ps_O = l.geom.O; sg.ps_C = l.geom.C; n->segs.push_back(sg); seg_layer.push_back((int)(&l - n->L.data()));
       if (!noop && (sg.kind == 1 || sg.kind == 5)) for (int64_t i = 0; i < len; ++i) h0[off + i] = d.eps;     // RmsProp cache / AdaGrad history initialised to epsilon
-      if (weight && d.l2 != 0.f) { l2o.push_back(off); l2l.push_back(len); l2c.push_back(0.5f * d.l2); }
+      if (l.has_gemm()) { n->reg_seg.push_back((int)n->segs.size() - 1); rego.push_back(off); regl.push_back(len); n->reg_l2c.push_back(0.5f * sg.l2); n->reg_l1c.push_back(0.f); }
     };
     if (l.has_gemm()) {
+      l.reg.l2 = d.l2;
       // WeightInit.XAVIER (J:127): N(0, 2/(fanIn+fanOut)); conv fanIn = nIn*kH*kW, fanOut = nOut*kH*kW/(sH*sW)
       double fi = (double)d.n_in * l.wTaps, fo = (double)d.n_out * l.wTaps / ((d.type == B2G_LAYER_CONV2D || d.type == B2G_LAYER_DECONV2D) ? (double)(d.s_h * d.s_w) : 1.0);
       float sd = (float)sqrt(2.0 / (fi + fo));
@@ -567,12 +572,17 @@ static int32_t net_init_params_and_updater(b2g_net* n) {
     B2(dalloc(n, &n->epoch_dev, sizeof(int64_t))); CU(cudaMemsetAsync(n->epoch_dev, 0, sizeof(int64_t), s));
     B2(dalloc(n, &n->lr_out, sizeof(float)));
   }
-  n->n_l2 = (int)l2o.size();
-  if (n->n_l2) {
-    B2(dalloc(n, &n->l2_off_dev, sizeof(int64_t) * n->n_l2)); B2(dalloc(n, &n->l2_len_dev, sizeof(int64_t) * n->n_l2)); B2(dalloc(n, &n->l2_coef_dev, sizeof(float) * n->n_l2));
-    CU(cudaMemcpyAsync(n->l2_off_dev, l2o.data(), sizeof(int64_t) * n->n_l2, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(n->l2_len_dev, l2l.data(), sizeof(int64_t) * n->n_l2, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(n->l2_coef_dev, l2c.data(), sizeof(float) * n->n_l2, cudaMemcpyHostToDevice, s));
+  {  // regularization score table: every W and b of a non-frozen GEMM layer, so that b2g_net_set_regularization only rewrites coefficients
+    const size_t nr = std::max<size_t>(1, rego.size());
+    B2(dalloc(n, &n->reg_off_dev, sizeof(int64_t) * nr)); B2(dalloc(n, &n->reg_len_dev, sizeof(int64_t) * nr));
+    B2(dalloc(n, &n->reg_l2c_dev, sizeof(float) * nr)); B2(dalloc(n, &n->reg_l1c_dev, sizeof(float) * nr));
+    if (!rego.empty()) {
+      CU(cudaMemcpyAsync(n->reg_off_dev, rego.data(), sizeof(int64_t) * rego.size(), cudaMemcpyHostToDevice, s));
+      CU(cudaMemcpyAsync(n->reg_len_dev, regl.data(), sizeof(int64_t) * regl.size(), cudaMemcpyHostToDevice, s));
+      CU(cudaMemcpyAsync(n->reg_l2c_dev, n->reg_l2c.data(), sizeof(float) * rego.size(), cudaMemcpyHostToDevice, s));
+      CU(cudaMemcpyAsync(n->reg_l1c_dev, n->reg_l1c.data(), sizeof(float) * rego.size(), cudaMemcpyHostToDevice, s));
+    }
+    n->n_l2 = (int)std::count_if(n->reg_l2c.begin(), n->reg_l2c.end(), [](float c) { return c != 0.f; }); n->n_l1 = 0;
   }
   CU(cudaStreamSynchronize(s));
   return 0;
@@ -1276,6 +1286,15 @@ static int32_t upload_labels(b2g_net* n, const float* y, int batch, float* dst, 
   CU(cudaMemcpyAsync(dst, y, sizeof(float) * cnt, cudaMemcpyHostToDevice, s));
   return 0;
 }
+// The score's regularization sums L1 and L2 (b2g_regularization): one launch per term that has a non-zero coefficient, copied back on the
+// net's stream (complete at its next synchronization); a term without one stays 0 and launches nothing
+static int32_t net_reg_sums(b2g_net* n, double* l1, double* l2) {
+  cudaStream_t s = n->ctx->stream;
+  const int nr = (int)n->reg_seg.size();
+  if (n->n_l2) { k_sumsq_segments(n->params, n->reg_off_dev, n->reg_len_dev, n->reg_l2c_dev, nr, n->reg_dev, s); CU(cudaMemcpyAsync(l2, n->reg_dev, sizeof(double), cudaMemcpyDeviceToHost, s)); }
+  if (n->n_l1) { k_sumabs_segments(n->params, n->reg_off_dev, n->reg_len_dev, n->reg_l1c_dev, nr, n->reg_dev + 1, s); CU(cudaMemcpyAsync(l1, n->reg_dev + 1, sizeof(double), cudaMemcpyDeviceToHost, s)); }
+  return 0;
+}
 static int32_t train_pass(b2g_net* n, const float* x, const float* y, int batch, bool do_update, float* score) {
   cudaStream_t s = n->ctx->stream;
   if (batch < 1 || batch > n->max_rows) return fail(B2G_ERR_SHAPE, "batch %d outside [1,%d]", batch, n->max_rows);
@@ -1289,10 +1308,10 @@ static int32_t train_pass(b2g_net* n, const float* x, const float* y, int batch,
   net_loss(n, logits, n->labels_dev, n->epsA, n->loss_dev, batch, 1);
   B2(net_backward(n, n->input, n->epsA, batch, 1, true, false, /*allreduce_follows=*/do_update && !score));
   if (score) {
-    double l2 = 0.0; float ls = 0.f;
-    if (n->n_l2) { k_sumsq_segments(n->params, n->l2_off_dev, n->l2_len_dev, n->l2_coef_dev, n->n_l2, n->l2_dev, s); CU(cudaMemcpyAsync(&l2, n->l2_dev, sizeof(double), cudaMemcpyDeviceToHost, s)); }
+    double l2 = 0.0, l1 = 0.0; float ls = 0.f;
+    B2(net_reg_sums(n, &l1, &l2));
     CU(cudaMemcpyAsync(&ls, n->loss_dev, sizeof(float), cudaMemcpyDeviceToHost, s)); CU(cudaStreamSynchronize(s));
-    *score = ls / batch + (float)l2;
+    *score = ls / batch + (float)(l2 + l1);
   }
   if (do_update) { B2(net_allreduce_grads(n)); B2(net_update(n, batch)); }
   return 0;
@@ -1939,6 +1958,56 @@ extern "C" int32_t b2g_net_init_weights(b2g_net* n, const char* layer, const b2g
     net_refresh_shadow(n, targets[k]);
   }
   CU(cudaStreamSynchronize(s)); CHECK_KERNELS();
+  return 0;
+}
+
+// ------------------------------------------------------------------ regularization (b2g_net_set_regularization) --------------------------
+// The coefficients live in the updater's segment table and the score table, both read from device memory at run time: a new value needs
+// no new launch, and a captured GAN step picks it up at its next replay without a re-capture.
+static int32_t find_gemm_layer(const b2g_net* n, const char* layer, int* li) {
+  for (size_t i = 0; i < n->L.size(); ++i) if (!strncmp(n->L[i].d.name, layer, B2G_NAME_LEN)) {
+    if (!n->L[i].has_gemm()) return fail(B2G_ERR_ARG, "layer %s has no W (regularization needs a conv, deconv, dense or output layer)", layer);
+    *li = (int)i; return 0;
+  }
+  return fail(B2G_ERR_ARG, "no layer named %s", layer);
+}
+extern "C" int32_t b2g_net_set_regularization(b2g_net* n, const char* layer, const b2g_regularization* r) {
+  if (!n || !r) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
+  const float v[4] = {r->l1, r->l2, r->l1_bias, r->l2_bias};
+  for (float x : v) if (!(std::isfinite(x) && x >= 0.f)) return fail(B2G_ERR_ARG, "regularization coefficient %g: must be finite and >= 0", (double)x);
+  if (layer) { int li = 0; B2(find_gemm_layer(n, layer, &li)); n->L[li].reg = *r; }
+  else for (auto& l : n->L) if (l.has_gemm() && !l.d.frozen) l.reg = *r;
+  for (size_t i = 0; i < n->segs.size(); ++i) {        // frozen layers own no segment: they take no term
+    const LayerRT& l = n->L[n->seg_layer[i]];
+    if (!l.has_gemm()) continue;
+    const bool weight = n->segs[i].off == l.off_W;
+    n->segs[i].l2 = weight ? l.reg.l2 : l.reg.l2_bias; n->segs[i].l1 = weight ? l.reg.l1 : l.reg.l1_bias;
+  }
+  n->n_l2 = n->n_l1 = 0;
+  for (size_t k = 0; k < n->reg_seg.size(); ++k) {
+    const UpdSeg& sg = n->segs[n->reg_seg[k]];
+    n->reg_l2c[k] = 0.5f * sg.l2; n->reg_l1c[k] = sg.l1; n->n_l2 += sg.l2 != 0.f; n->n_l1 += sg.l1 != 0.f;
+  }
+  cudaStream_t s = n->ctx->stream;
+  CU(cudaStreamSynchronize(s));                  // nothing in flight reads the old tables
+  if (!n->segs.empty()) CU(cudaMemcpyAsync(n->segs_dev, n->segs.data(), sizeof(UpdSeg) * n->segs.size(), cudaMemcpyHostToDevice, s));
+  if (!n->reg_seg.empty()) {
+    CU(cudaMemcpyAsync(n->reg_l2c_dev, n->reg_l2c.data(), sizeof(float) * n->reg_seg.size(), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(n->reg_l1c_dev, n->reg_l1c.data(), sizeof(float) * n->reg_seg.size(), cudaMemcpyHostToDevice, s));
+  }
+  CU(cudaStreamSynchronize(s));
+  return 0;
+}
+extern "C" int32_t b2g_net_get_regularization(b2g_net* n, const char* layer, b2g_regularization* out) {
+  if (!n || !layer || !out) return fail(B2G_ERR_ARG, "null");
+  int li = 0; B2(find_gemm_layer(n, layer, &li)); *out = n->L[li].reg; return 0;
+}
+extern "C" int32_t b2g_net_calc_regularization(b2g_net* n, double* l1, double* l2) {
+  if (!n) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
+  double a = 0.0, b = 0.0;
+  B2(net_reg_sums(n, &a, &b)); CU(cudaStreamSynchronize(n->ctx->stream));
+  if (l1) *l1 = a;
+  if (l2) *l2 = b;
   return 0;
 }
 

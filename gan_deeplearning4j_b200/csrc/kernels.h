@@ -203,8 +203,10 @@ void k_skip_add(int prec, void* eps, const float* acc, size_t n, cudaStream_t s)
 // out[c] (+)= sum_rows x[row][c]
 void k_colsum(int prec, const void* x, int rows, int C, float* scratch, float* out, int accumulate, cudaStream_t s);
 size_t k_colsum_scratch_floats(int C);
-// out[0] = sum_i coef[i] * x[i]^2 over the listed segments (l2 score)
+// out[0] = sum_i coef[i] * x[i]^2 over the listed segments (l2 score); segments with coef 0 are skipped
 void k_sumsq_segments(const float* p, const int64_t* seg_off, const int64_t* seg_len, const float* seg_coef, int nseg, double* out, cudaStream_t s);
+// out[0] = sum_i coef[i] * |x[i]| over the listed segments (l1 score), in the order of k_sumsq_segments; segments with coef 0 are skipped
+void k_sumabs_segments(const float* p, const int64_t* seg_off, const int64_t* seg_len, const float* seg_coef, int nseg, double* out, cudaStream_t s);
 // dst[i] = sum_s src[s*stride + i]
 void k_reduce_splits(const float* src, float* dst, size_t n, int splits, size_t stride, int accumulate, cudaStream_t s);
 // the same for a whole list of (src, dst) pairs in ONE launch: the split-K partials of every weight gradient of a backward pass
@@ -218,7 +220,8 @@ struct UpdSeg {            // one parameter tensor
   int64_t off, len;
   int kind;                // b2g_updater: 0 sgd, 1 rmsprop, 2 adam, 3 noop, 4 nesterovs, 5 adagrad, 6 adamax, 7 nadam, 8 amsgrad, 9 adadelta
   float lr, b1, b2, eps;   // rmsprop: b1 = rmsDecay; nesterovs: b1 = momentum; adadelta: b1 = rho (lr unused)
-  float l2;                // post-updater, not lr-scaled (pre-beta4)
+  float l2;                // post-updater, not lr-scaled (pre-beta4): u = fmaf(l2, p, u)
+  float l1;                // then u += l1 * sign(p), sign(+-0) = 0; W takes the layer's l1 / l2, b its l1Bias / l2Bias
   float clip;              // elementwise clip threshold, 0 = off
   int div_mb;              // 0 for BN mean/var pseudo-gradients
   // bf16 shadow of a conv/deconv/dense weight: shadow[off_bf..] same layout [A][taps][B]; off_ps >= 0: also the packed [16][9][ps_O] operand of

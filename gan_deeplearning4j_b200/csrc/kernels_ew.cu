@@ -1,6 +1,6 @@
 // kernels_ew.cu -- the HBM-bound kernels of the GAN step: layout conversion, BatchNorm statistics /
 // apply / backward, activations, max-pool, upsampling, binary cross-entropy, column sums, and the
-// one-pass updater (divide-by-minibatch -> clip -> RmsProp/Adam -> +l2*W -> theta -= g).
+// one-pass updater (divide-by-minibatch -> clip -> RmsProp/Adam -> +l2*W + l1*sign(W) -> theta -= g).
 //
 // Semantics follow DL4J 1.0.0-beta3 as restated in oracle/dl4j_oracle.py (SURVEY.md section 8a rows
 // a3-a6, a8, a9); the reference call sites are J:123-125,132-134,141-144,159-163,201-202 where
@@ -865,12 +865,16 @@ void k_colsum(int prec, const void* x, int rows, int C, float* scratch, float* o
   LAUNCHED();
   launch_pdl(colsum_final_kernel, dim3((C + 31) / 32), dim3(512), (size_t)(0), s, scratch, C, S, out, accumulate); LAUNCHED();
 }
-__global__ void sumsq_segments_kernel(const float* __restrict__ p, const int64_t* off, const int64_t* len, const float* coef, int nseg, double* out) { pdl_enter();
+// The regularization score terms, in an order fixed by the segment table: each thread walks every segment with a non-zero coefficient in
+// turn and adds coef * its own double sum over the segment; then a warp butterfly and the warps in order.  ABS: |x| (l1), else x^2 (l2).
+template <bool ABS>
+__device__ __forceinline__ void segments_norm(const float* __restrict__ p, const int64_t* off, const int64_t* len, const float* coef, int nseg, double* out) {
   __shared__ double red[32];
   double acc = 0.0;
   for (int sgi = 0; sgi < nseg; ++sgi) {
+    if (coef[sgi] == 0.f) continue;
     const float* q = p + off[sgi]; double a = 0.0;
-    for (int64_t i = threadIdx.x; i < len[sgi]; i += blockDim.x) a += (double)q[i] * q[i];
+    for (int64_t i = threadIdx.x; i < len[sgi]; i += blockDim.x) a += ABS ? fabs((double)q[i]) : (double)q[i] * q[i];
     acc += coef[sgi] * a;
   }
   for (int o = 16; o; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
@@ -878,9 +882,19 @@ __global__ void sumsq_segments_kernel(const float* __restrict__ p, const int64_t
   __syncthreads();
   if (threadIdx.x == 0) { double t = 0; for (int w = 0; w < (blockDim.x + 31) / 32; ++w) t += red[w]; *out = t; }
 }
+__global__ void sumsq_segments_kernel(const float* __restrict__ p, const int64_t* off, const int64_t* len, const float* coef, int nseg, double* out) { pdl_enter();
+  segments_norm<false>(p, off, len, coef, nseg, out);
+}
+__global__ void sumabs_segments_kernel(const float* __restrict__ p, const int64_t* off, const int64_t* len, const float* coef, int nseg, double* out) { pdl_enter();
+  segments_norm<true>(p, off, len, coef, nseg, out);
+}
 void k_sumsq_segments(const float* p, const int64_t* so, const int64_t* sl, const float* sc, int nseg, double* out, cudaStream_t s) {
   launch_pdl(sumsq_segments_kernel, dim3(1), dim3(1024), (size_t)(0), s, p, so, sl, sc, nseg, out); LAUNCHED();
   g_ew_last_kernel = "sumsq_segments_kernel";
+}
+void k_sumabs_segments(const float* p, const int64_t* so, const int64_t* sl, const float* sc, int nseg, double* out, cudaStream_t s) {
+  launch_pdl(sumabs_segments_kernel, dim3(1), dim3(1024), (size_t)(0), s, p, so, sl, sc, nseg, out); LAUNCHED();
+  g_ew_last_kernel = "sumabs_segments_kernel";
 }
 __global__ void reduce_splits_kernel(const float* __restrict__ src, float* __restrict__ dst, size_t n, int splits, size_t stride, int accumulate) { pdl_enter();
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -975,6 +989,7 @@ __device__ __forceinline__ float upd_elem(const UpdSeg& sg, float g, float p, fl
   else { s0 = sg.b1 * s0 + (1.0f - sg.b1) * g * g; u = sqrtf(s1 + sg.eps) / sqrtf(s0 + sg.eps) * g;                              // AdaDelta
          s1 = sg.b1 * s1 + (1.0f - sg.b1) * u * u; }
   if (sg.l2 != 0.f) u = fmaf(sg.l2, p, u);
+  if (sg.l1 != 0.f) u = fmaf(sg.l1, (float)((p > 0.f) - (p < 0.f)), u);     // + l1 * sign(p), exact: sign(+-0) = 0
   return p - u;
 }
 // SCHED: the segment's lr comes from its schedule (thread 0 evaluates it once per block, at *step before the increment or at *epoch)

@@ -163,6 +163,54 @@ def resolve_constraints(spec: Dict) -> Dict[str, List[Dict]]:
     return out
 
 
+# Regularization of a GEMM layer spec (b2g_regularization in include/b200gan.h): "l1" and "l2" on W, "l1_bias" and "l2_bias" on b, applied
+# after the updater and added to the score.  "l2" travels in b2g_layer_desc; a spec with any of the other three gets them all set at creation.
+REGULARIZATION_KEYS = ("l1", "l2", "l1_bias", "l2_bias")
+
+
+def check_regularization(values: Dict, where: str = "regularization") -> Dict[str, float]:
+    """The coefficients of a regularization dict, each a finite number >= 0 as b2g_net_set_regularization requires (DL4J ignores a value
+    <= 0; refusing negatives is a deliberate deviation).  ValueError for an unknown key or a bad value."""
+    unknown = set(values) - set(REGULARIZATION_KEYS)
+    if unknown:
+        raise ValueError(f"{where}: unknown key(s) {sorted(unknown)}; one of {list(REGULARIZATION_KEYS)}")
+    out = {}
+    for k, v in values.items():
+        f = np.float32(v)
+        if not (np.isfinite(f) and f >= 0):
+            raise ValueError(f"{where}: {k} = {v!r} must be finite and >= 0")
+        out[k] = float(v)
+    return out
+
+
+def spec_regularization(spec: Dict) -> Dict[str, float]:
+    """The four coefficients a GEMM layer spec carries (a missing key is 0)."""
+    return {k: float(spec.get(k, 0.0)) for k in REGULARIZATION_KEYS}
+
+
+def resolve_regularization(specs: List[Dict], regularization: Optional[Dict] = None) -> List[Dict]:
+    """Fills in the global builder's coefficients (regularization, may be None) in place: every non-frozen conv, deconv, dense and output spec
+    takes each key it does not set itself, as DL4J's builder fills in a layer's NaN fields.  Then checks each GEMM spec's "l1", "l1_bias" and
+    "l2_bias" ("l2" is the desc's, as before).  Returns specs."""
+    if regularization is not None:
+        glob = check_regularization(regularization)
+        for sp in specs:
+            if sp["type"] in GEMM_TYPES and not sp.get("frozen", False):
+                for k, v in glob.items():
+                    sp.setdefault(k, v)
+    for sp in specs:
+        if sp["type"] in GEMM_TYPES:
+            check_regularization({k: sp[k] for k in REGULARIZATION_KEYS if k in sp and k != "l2"}, f"layer {sp.get('name', '')!r}")
+    return specs
+
+
+def regularization_struct(values: Dict) -> "_lib.Regularization":
+    r = _lib.Regularization()
+    for k in REGULARIZATION_KEYS:
+        setattr(r, k, float(values.get(k, 0.0)))
+    return r
+
+
 def _fp(a: np.ndarray):
     return a.ctypes.data_as(C.POINTER(C.c_float))
 
@@ -409,15 +457,19 @@ class Net:
     def __init__(self, ctx: Context, specs: Sequence[Dict], input_shape, max_batch: int, precision: int = FP32,
                  grad_clip: float = 0.0, xent_clip_eps: float = 1e-5, bn_groups: int = 1, seed: int = 666,
                  gradient_normalization: str = "none", gradient_normalization_threshold: float = 1.0,
-                 constraints: Optional[Sequence[Dict]] = None, weight_noise: Optional[Dict] = None, weight_init: Optional[Dict] = None):
+                 constraints: Optional[Sequence[Dict]] = None, weight_noise: Optional[Dict] = None, weight_init: Optional[Dict] = None,
+                 regularization: Optional[Dict] = None):
         """constraints: the global builder's constraints (models.max_norm, ...), for every layer whose own "constraints" reach none of its
         parameters (none given, or e.g. only bias constraints on a BatchNorm), as DL4J's builder fills them in; the specs the net keeps (and a
         checkpoint saves) carry them per layer.  weight_noise: the global builder's weightNoise (models.drop_connect / models.weight_noise) for
         every non-frozen conv, deconv, dense and output layer without a "weight_noise" of its own; the kept specs carry it per layer.
         weight_init: the global builder's weightInit / dist / biasInit (models.weight_init) for every conv, deconv, dense and output layer
         without a "weight_init" of its own, drawn right after creation; the kept specs carry it per layer.  Layers with neither keep
-        b2g_net_create's Xavier draw."""
+        b2g_net_create's Xavier draw.  regularization: the global builder's l1 / l2 / l1Bias / l2Bias ({"l1": .., "l2": .., "l1_bias": ..,
+        "l2_bias": ..}): every non-frozen conv, deconv, dense and output layer takes each key its spec does not set, as DL4J's builder fills
+        them in; the kept specs carry them per layer."""
         self.ctx, self.lib, self.specs = ctx, ctx.lib, copy.deepcopy(list(specs))
+        resolve_regularization(self.specs, regularization)
         if weight_init is not None:
             for sp in self.specs:
                 if sp["type"] in GEMM_TYPES and "weight_init" not in sp:
@@ -436,7 +488,7 @@ class Net:
         c, h, w = input_shape if len(input_shape) == 3 else (input_shape[0], 1, 1)
         self.input_shape = tuple(input_shape)
         cfg = NetConfig(h, w, c, max_batch, precision, grad_clip, xent_clip_eps, bn_groups, seed)
-        arr = (LayerDesc * len(specs))(*[layer_desc(s, v) for s, v in zip(specs, resolve_vertices(specs))])
+        arr = (LayerDesc * len(specs))(*[layer_desc(s, v) for s, v in zip(self.specs, resolve_vertices(specs))])     # the kept specs: a global l2 included
         hnd = C.c_void_p()
         check(self.lib.b2g_net_create(ctx.h, C.byref(cfg), arr, len(specs), C.byref(hnd)))
         self.h = hnd
@@ -449,6 +501,10 @@ class Net:
         try:
             for name, s in inits:         # Layer.Builder.weightInit / dist / biasInit, at init()
                 check(self.lib.b2g_net_init_weights(self.h, name.encode(), C.byref(s)))
+            for sp in self.specs:         # Layer.Builder.l1 / l1Bias / l2Bias (l2 alone travels in the desc)
+                r = spec_regularization(sp)
+                if sp["type"] in GEMM_TYPES and (r["l1"] or r["l1_bias"] or r["l2_bias"]):
+                    check(self.lib.b2g_net_set_regularization(self.h, sp["name"].encode(), C.byref(regularization_struct(r))))
             if gradient_normalization != "none":
                 self.set_gradient_normalization(gradient_normalization, gradient_normalization_threshold)
             for sp in self.specs:         # an updater constructed with an ISchedule: new Adam(new StepSchedule(...))
@@ -635,6 +691,35 @@ class Net:
         check(self.lib.b2g_net_init_weights(self.h, None if layer is None else layer.encode(), C.byref(s)))
         for sp in targets:
             sp["weight_init"] = copy.deepcopy(weight_init)
+
+    def set_regularization(self, l1: float = 0.0, l2: float = 0.0, l1_bias: float = 0.0, l2_bias: float = 0.0, layer: Optional[str] = None):
+        """l1 / l2 on W and l1Bias / l2Bias on b (b2g_net_set_regularization): layer None = every non-frozen conv, deconv, dense and output
+        layer.  Replaces all four coefficients (the spec's "l2" too), from the next update and score on.  The specs a checkpoint writes
+        follow: a coefficient of 0 leaves no key."""
+        r = check_regularization({"l1": l1, "l2": l2, "l1_bias": l1_bias, "l2_bias": l2_bias})
+        check(self.lib.b2g_net_set_regularization(self.h, None if layer is None else layer.encode(), C.byref(regularization_struct(r))))
+        for sp in self.specs:
+            if sp["type"] not in GEMM_TYPES or (layer is None and sp.get("frozen", False)) or (layer is not None and sp.get("name") != layer):
+                continue
+            for k, v in r.items():
+                if v:
+                    sp[k] = v
+                else:
+                    sp.pop(k, None)
+            if layer is not None:
+                break
+
+    def get_regularization(self, layer: str) -> Dict[str, float]:
+        """The four coefficients of a conv, deconv, dense or output layer, as the engine holds them (fp32)."""
+        r = _lib.Regularization()
+        check(self.lib.b2g_net_get_regularization(self.h, layer.encode(), C.byref(r)))
+        return {k: getattr(r, k) for k in REGULARIZATION_KEYS}
+
+    def calc_regularization(self):
+        """(calcL1(true), calcL2(true)): the score's L1 and L2 terms over the current parameters, in double (b2g_net_calc_regularization)."""
+        l1, l2 = C.c_double(), C.c_double()
+        check(self.lib.b2g_net_calc_regularization(self.h, C.byref(l1), C.byref(l2)))
+        return l1.value, l2.value
 
     def noisy_operand(self, layer: int, which: int, size: int) -> np.ndarray:
         """What the latest train-mode pass of a weight-noise layer drew (b2g_test_net_noisy_operand): which 0 = W' in the internal order, 1 = the

@@ -200,7 +200,8 @@ typedef enum {
 } b2g_activation;
 
 /* org.nd4j.linalg.learning.config.*  J:133 (RmsProp), north_star (Adam); the others as in DL4J 1.0.0-beta3 (recalled, parity unpinned like
- * the rest of the DL4J semantics).  One update is  g /= mb -> [normalization] -> [clip] -> u = updater(g) -> u += l2*W -> theta -= u,  in fp32.
+ * the rest of the DL4J semantics).  One update is  g /= mb -> [normalization] -> [clip] -> u = updater(g) -> u += l2*W [+ l1*sign(W)] -> theta -= u,
+ * in fp32 (the regularization terms: b2g_regularization).
  * t = iteration + 1 (b2g_net_get_iteration before the update's increment); lr = b2g_layer_desc.lr or the layer's schedule value (b2g_lr_schedule);
  * the bias-correction factors are computed once per updater block in fp32.  Desc fields: beta1, beta2, eps as named, except where noted.
  *   SGD (0)        u = lr*g
@@ -280,7 +281,7 @@ typedef struct {
                                    DropoutLayer value (b2g_dropout_kind); PNORM pooling's p */
   int32_t updater;              /* b2g_updater; "frozen" in the reference = RMSPROP with lr 0 (J:84) */
   float lr, beta1, beta2, eps;  /* RmsProp: beta1 = rmsDecay (ctor order lr, rmsDecay, epsilon; J:133 passes 1e-8, 1e-8) */
-  float l2;                     /* .l2(1e-4) (J:125): weights only, applied AFTER the updater, not lr-scaled */
+  float l2;                     /* .l2(1e-4) (J:125): weights only, applied AFTER the updater, not lr-scaled (b2g_net_set_regularization) */
   float bn_decay, bn_eps;       /* BatchNormalization defaults 0.9 / 1e-5 */
   int32_t pre_h, pre_w, pre_c;  /* FF_TO_CNN target shape */
   int32_t loss;                 /* OUTPUT / LOSS layer: b2g_loss (0 = LossFunction.XENT + sigmoid J:159-163, 1 = MCXENT + softmax J:357-362, 2-8 on act) */
@@ -342,7 +343,7 @@ int32_t b2g_net_output(b2g_net* net, const float* x, int32_t batch, int32_t trai
 /* Activations of one layer from the most recent forward (parity tests): NCHW fp32. */
 int32_t b2g_net_get_activation(b2g_net* net, int32_t layer, int32_t batch, float* host);
 /* computeGradientAndScore(): train-mode forward, the last layer's loss (b2g_loss) vs labels y, backprop.
- * score = sum(loss)/batch + 0.5*l2*||W||^2 ; gradients stay on device (b2g_net_get_gradients).
+ * score = sum(loss)/batch + 0.5*l2*||W||^2 (+ the other terms of b2g_regularization); gradients stay on device (b2g_net_get_gradients).
  * Labels y are [batch, nOut] (nOut = 1 for XENT; one-hot rows for MCXENT; targets for codes 2-8). */
 int32_t b2g_net_compute_gradient_and_score(b2g_net* net, const float* x, const float* y, int32_t batch, float* score);
 /* epsilon w.r.t. the network input from the last backward (NCHW fp32; what the stacked gan graph feeds the generator). */
@@ -567,6 +568,33 @@ typedef struct {
  * B2G_ERR_SHAPE: IDENTITY on a CONV2D or DECONV2D layer, or on a DENSE / OUTPUT layer with nIn != nOut (DL4J throws).
  * B2G_ERR_UNSUPPORTED: DISTRIBUTION with ORTHOGONAL. */
 int32_t b2g_net_init_weights(b2g_net* net, const char* layer, const b2g_weight_init* wi);
+
+/* Regularization (DL4J 1.0.0-beta3 Layer.Builder / NeuralNetConfiguration.Builder .l1, .l2, .l1Bias, .l2Bias, resolved per parameter by
+ * getL1ByParam / getL2ByParam, recalled; parity unpinned like the rest of the DL4J semantics).
+ * Which tensors: on CONV2D, DECONV2D, DENSE and OUTPUT layers l1 and l2 apply to W, l1_bias and l2_bias to b.  BatchNorm parameters are never
+ * regularized (beta3's BatchNormalization returns 0 for every parameter).  A FrozenLayer takes no term, in the update or in the score; a layer
+ * with lr 0 still decays.
+ * Update (UpdaterBlock.postApply): after the updater, with the coefficients as set (no schedule, not lr-scaled; the normalization of
+ * b2g_net_set_gradient_normalization and grad_clip never see the term):
+ *   u = fmaf(l2, theta, u);  then  u = u + l1 * sign(theta),  sign(+0) = sign(-0) = 0;  theta -= u
+ * (l2_bias / l1_bias on b), in the updater's one pass, wherever the net's updater runs (b2g_net_fit, the D and G updates of b2g_gan_step,
+ * local fits in parameter-averaging mode).  BF16 nets get the bf16 weight operands from the same pass, as always.
+ * Score (calcL2 / calcL1): score = sum(loss) / minibatch + (float)(L2 + L1), where over the layers
+ *   L2 = sum of 0.5 * l2 * ||W||^2 + 0.5 * l2_bias * ||b||^2        L1 = sum of l1 * ||W||_1 + l1_bias * ||b||_1
+ * each norm summed in double over the fp32 master values (never the weight-noise operands) in an order fixed by the shape, and multiplied by
+ * the fp32 coefficient (0.5f * l2 for the squares).  A term whose coefficients are all 0 launches nothing: a net with l2 only launches what it
+ * launched before and scores the same bits.
+ * b2g_layer_desc.l2 is the initial l2 of W; every other coefficient starts at 0. */
+typedef struct { float l1, l2, l1_bias, l2_bias; } b2g_regularization;
+/* Layer.Builder.l1 / l2 / l1Bias / l2Bias (layer named) or NeuralNetConfiguration.Builder's (layer NULL: every non-frozen CONV2D, DECONV2D,
+ * DENSE and OUTPUT layer).  Replaces all four coefficients of the layer (the desc's l2 too).  Takes effect at the next update, also in a replayed
+ * CUDA graph of the GAN step (the updater reads the coefficients from device memory).  B2G_ERR_ARG for a value that is not finite and >= 0
+ * (DL4J silently ignores a value <= 0: refusing negatives is a deliberate deviation), or a named layer that does not exist or has no W. */
+int32_t b2g_net_set_regularization(b2g_net* net, const char* layer, const b2g_regularization* r);
+/* The four coefficients of a named CONV2D, DECONV2D, DENSE or OUTPUT layer (B2G_ERR_ARG for any other name). */
+int32_t b2g_net_get_regularization(b2g_net* net, const char* layer, b2g_regularization* out);
+/* ComputationGraph.calcL1(true) and calcL2(true): L1 and L2 of the score above, now, in double.  Either pointer may be NULL.  Sync point. */
+int32_t b2g_net_calc_regularization(b2g_net* net, double* l1, double* l2);
 /* ComputationGraph.getEpochCount / setEpochCount: the 64-bit device word EPOCH schedules read, 0 at b2g_net_create.  The host sets it, nothing
  * increments it; a new value takes effect at the next update, also in a replayed CUDA graph.  Sync points.  B2G_ERR_ARG for epoch < 0. */
 int32_t b2g_net_get_epoch(b2g_net* net, int64_t* out);

@@ -41,6 +41,8 @@ public final class Native {
     public static native int netGetDropoutValue(long net, long layerNameAddr, long outAddr);
     public static native int netSetWeightNoise(long net, long layerNameAddr, long weightNoiseAddr);   // b2g_weight_noise; layerNameAddr 0: every layer with a W
     public static native int netInitWeights(long net, long layerNameAddr, long weightInitAddr);   // b2g_weight_init; layerNameAddr 0: every layer with a W
+    public static native int netSetRegularization(long net, long layerNameAddr, long regAddr);   // b2g_regularization; layerNameAddr 0: every non-frozen layer with a W
+    public static native int netCalcRegularization(long net, long l1Addr, long l2Addr);          // two doubles: calcL1(true), calcL2(true)
     public static native int netGetEpoch(long net, long outAddr);
     public static native int netSetEpoch(long net, long epoch);
     public static native int netSimtGemmCalls(long net, long outAddr);

@@ -32,6 +32,11 @@ public class NeuralNetConfiguration {
         }
         public Builder gradientNormalizationThreshold(double t) { gradNormThreshold = (float) t; if (!gradNorm.isL2()) clip = (float) t; return this; }
         public Builder l2(double v) { l2 = (float) v; return this; }
+        /** The global l1 (W), l1Bias and l2Bias (b): every conv, deconv, dense and output layer takes each one it does not set itself. */
+        public float l1 = 0f, l1Bias = 0f, l2Bias = 0f;
+        public Builder l1(double v) { l1 = (float) v; return this; }
+        public Builder l1Bias(double v) { l1Bias = (float) v; return this; }
+        public Builder l2Bias(double v) { l2Bias = (float) v; return this; }
         public Builder activation(Activation a) { act = a; return this; }
         /** The global weightInit / dist / biasInit (null: not given): every conv, deconv, dense and output layer takes what it does not set
          *  itself.  With none of the three given anywhere a layer keeps the library's default draw. */

@@ -12,6 +12,8 @@ public class Layer {
     public static final int DESC_BYTES = 4 + 64 + 4 * 2 + 4 * 6 + 4 + 4 + 4 + 4 + 4 * 4 + 4 + 4 * 2 + 4 * 3 + 4 * 2;   // == sizeof(b2g_layer_desc) = 164
     public int type, nIn, nOut, kH = 1, kW = 1, sH = 1, sW = 1, pH, pW, hasBias = 1, act = -1, preH, preW, preC, loss, frozen;
     public float alpha = 0.01f, l2 = Float.NaN, bnDecay = 0.9f, bnEps = 1e-5f;
+    /** l1 (W), l1Bias and l2Bias (b); NaN: the global builder's.  Applied by ComputationGraph.init (l2 travels in the desc). */
+    public float l1 = Float.NaN, l1Bias = Float.NaN, l2Bias = Float.NaN;
     public IUpdater updater; public String name = "";
     public org.nd4j.linalg.schedule.ISchedule dropSchedule;   // DropoutLayer.Builder(IDropout) with an ISchedule: applied by ComputationGraph.init
     public org.deeplearning4j.nn.conf.weightnoise.IWeightNoise weightNoise;   // Layer.Builder.weightNoise (null: the global builder's): applied by ComputationGraph.init
@@ -31,7 +33,7 @@ public class Layer {
         b.putFloat(Float.isNaN(l2) ? globalL2 : l2).putFloat(bnDecay).putFloat(bnEps).putInt(preH).putInt(preW).putInt(preC).putInt(loss).putInt(frozen);
     }
     public Layer copy() { Layer c = new Layer(); c.type = type; c.nIn = nIn; c.nOut = nOut; c.kH = kH; c.kW = kW; c.sH = sH; c.sW = sW; c.pH = pH; c.pW = pW; c.hasBias = hasBias; c.act = act;
-        c.preH = preH; c.preW = preW; c.preC = preC; c.loss = loss; c.frozen = frozen; c.alpha = alpha; c.l2 = l2; c.bnDecay = bnDecay; c.bnEps = bnEps; c.updater = updater; c.name = name; c.alphaSet = alphaSet;
+        c.preH = preH; c.preW = preW; c.preC = preC; c.loss = loss; c.frozen = frozen; c.alpha = alpha; c.l2 = l2; c.l1 = l1; c.l1Bias = l1Bias; c.l2Bias = l2Bias; c.bnDecay = bnDecay; c.bnEps = bnEps; c.updater = updater; c.name = name; c.alphaSet = alphaSet;
         c.constrainAll = constrainAll; c.constrainW = constrainW; c.constrainB = constrainB; c.dropSchedule = dropSchedule; c.weightNoise = weightNoise;
         c.weightInit = weightInit; c.dist = dist; c.biasInit = biasInit; return c; }
     protected int defaultAct(Activation g) { return g.code; }   // conv / dense inherit the global .activation(..) (J:126)
@@ -50,6 +52,9 @@ public class Layer {
         public T activation(IActivation a) { l.act = a.code(); l.alpha = a.alpha(); l.alphaSet = true; return (T) this; }   // ActivationELU(alpha), ActivationThresholdedReLU(theta)
         public T leakyReluAlpha(double a) { l.alpha = (float) a; l.alphaSet = true; return (T) this; }
         public T l2(double v) { l.l2 = (float) v; return (T) this; }
+        public T l1(double v) { l.l1 = (float) v; return (T) this; }
+        public T l1Bias(double v) { l.l1Bias = (float) v; return (T) this; }
+        public T l2Bias(double v) { l.l2Bias = (float) v; return (T) this; }
         public T constrainAllParameters(LayerConstraint... c) { l.constrainAll = List.of(c); return (T) this; }
         public T constrainWeights(LayerConstraint... c) { l.constrainW = List.of(c); return (T) this; }
         public T constrainBias(LayerConstraint... c) { l.constrainB = List.of(c); return (T) this; }

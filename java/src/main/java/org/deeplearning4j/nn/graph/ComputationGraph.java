@@ -37,6 +37,11 @@ public class ComputationGraph {
             if (gemm && (global || l.weightInit != null || l.dist != null || l.biasInit != null))
                 initWeights(l.name, l.weightInit != null ? l.weightInit : g.weightInit, l.dist != null ? l.dist : g.dist, l.biasInit != null ? l.biasInit : g.biasInit);
         }
+        for (Layer l : layers) {          // l1 / l1Bias / l2Bias, resolved per layer like l2: its own, else the global builder's
+            boolean gemm = l.type == 0 || l.type == 1 || l.type == 3 || l.type == 7;
+            float l1 = Float.isNaN(l.l1) ? g.l1 : l.l1, l1b = Float.isNaN(l.l1Bias) ? g.l1Bias : l.l1Bias, l2b = Float.isNaN(l.l2Bias) ? g.l2Bias : l.l2Bias;
+            if (gemm && (l1 != 0f || l1b != 0f || l2b != 0f)) setRegularization(l.name, l1, Float.isNaN(l.l2) ? g.l2 : l.l2, l1b, l2b);
+        }
         GradientNormalization gn = conf.b.g.gradNorm;      // RenormalizeL2* / ClipL2*: on-device norms before every update
         if (gn.isL2()) Native.check(Native.netSetGradientNormalization(net, gn.ordinal(), conf.b.g.gradNormThreshold));
         for (Layer l : layers)            // new Adam(ISchedule) / RmsProp(ISchedule) / Sgd(ISchedule): evaluated on the device at every update
@@ -153,6 +158,22 @@ public class ComputationGraph {
         ByteBuffer name = layerName == null ? null : Native.cstr(layerName);
         Native.check(Native.netInitWeights(net, name == null ? 0 : Native.address(name), Native.address(b)));
         java.lang.ref.Reference.reachabilityFence(b); java.lang.ref.Reference.reachabilityFence(name);
+    }
+    /** l1 / l2 on W and l1Bias / l2Bias on b of one layer (layerName null: every non-frozen conv, deconv, dense and output layer), applied
+     *  after the updater from the next update on; replaces all four. */
+    public void setRegularization(String layerName, float l1, float l2, float l1Bias, float l2Bias) {
+        ByteBuffer b = Native.direct(16);   // b2g_regularization: l1, l2, l1_bias, l2_bias (16 bytes)
+        b.putFloat(0, l1).putFloat(4, l2).putFloat(8, l1Bias).putFloat(12, l2Bias);
+        ByteBuffer name = layerName == null ? null : Native.cstr(layerName);
+        Native.check(Native.netSetRegularization(net, name == null ? 0 : Native.address(name), Native.address(b)));
+        java.lang.ref.Reference.reachabilityFence(b); java.lang.ref.Reference.reachabilityFence(name);
+    }
+    /** ComputationGraph.calcL1(true) / calcL2(true): the score's regularization terms over the current parameters. */
+    public double calcL1(boolean backpropParamsOnly) { return calcRegularization()[0]; }
+    public double calcL2(boolean backpropParamsOnly) { return calcRegularization()[1]; }
+    private double[] calcRegularization() {
+        ByteBuffer o = Native.direct(16);
+        Native.check(Native.netCalcRegularization(net, Native.address(o), Native.address(o) + 8)); return new double[] { o.getDouble(0), o.getDouble(8) };
     }
     /** The learning rate the layer's next update uses (its schedule's value at the current iteration / epoch, or its constant lr). */
     public double getLearningRate(String layerName) {

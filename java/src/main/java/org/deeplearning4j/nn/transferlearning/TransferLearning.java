@@ -20,7 +20,7 @@ public final class TransferLearning {
         public GraphBuilder removeVertexKeepConnections(String name) { removed.add(name); return this; }
         public GraphBuilder addLayer(String name, Layer l, String... inputs) { l.name = name; added.add(l); return this; }
         public ComputationGraph build() {
-            NeuralNetConfiguration.Builder b = new NeuralNetConfiguration.Builder().seed(ft.seed).gradientNormalizationThreshold(ft.clip).l2(ft.l2).activation(ft.act);
+            NeuralNetConfiguration.Builder b = new NeuralNetConfiguration.Builder().seed(ft.seed).gradientNormalizationThreshold(ft.clip).l2(ft.l2).l1(ft.l1).l1Bias(ft.l1Bias).l2Bias(ft.l2Bias).activation(ft.act);
             if (ft.gradNorm.isL2()) b.gradientNormalization(ft.gradNorm).gradientNormalizationThreshold(ft.gradNormThreshold);
             NeuralNetConfiguration.GraphBuilder g = b.graphBuilder().setInputTypes(src.configuration().b.in);
             boolean frozen = frozenUpTo != null;

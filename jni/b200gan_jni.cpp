@@ -74,6 +74,13 @@ FN(netSetWeightNoise)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong wn
 FN(netInitWeights)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong wiAddr) {
   return b2g_net_init_weights(P(b2g_net*, net), P(const char*, layerNameAddr), P(const b2g_weight_init*, wiAddr));
 }
+// b2g_regularization (16 bytes); layerNameAddr 0: every non-frozen layer with a W
+FN(netSetRegularization)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong regAddr) {
+  return b2g_net_set_regularization(P(b2g_net*, net), P(const char*, layerNameAddr), P(const b2g_regularization*, regAddr));
+}
+FN(netCalcRegularization)(JNIEnv_*, jclass, jlong net, jlong l1Addr, jlong l2Addr) {
+  return b2g_net_calc_regularization(P(b2g_net*, net), P(double*, l1Addr), P(double*, l2Addr));
+}
 FN(netGetEpoch)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_get_epoch(P(b2g_net*, net), P(int64_t*, outAddr)); }
 FN(netSetEpoch)(JNIEnv_*, jclass, jlong net, jlong epoch) { return b2g_net_set_epoch(P(b2g_net*, net), epoch); }
 FN(netSimtGemmCalls)(JNIEnv_*, jclass, jlong net, jlong outAddr) { return b2g_net_simt_gemm_calls(P(b2g_net*, net), P(uint64_t*, outAddr)); }

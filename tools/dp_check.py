@@ -255,7 +255,15 @@ def noise(ctx):
             "scheduled_value": float(allv[0][npar])}
 
 
-CHECKS = {"core": core, "updater": updater, "dropout": dropout, "noise": noise, "gradnorm": gradnorm, "constraint": constraint}
+def regularization(ctx):
+    """l1, l2, l1Bias and l2Bias on every layer of G and D (the global builder's): the terms act on the all-reduced update, on parameters the
+    ranks hold identically."""
+    reg = dict(regularization={"l1": 1e-3, "l2": 1e-2, "l1_bias": 5e-4, "l2_bias": 5e-3})
+    return replicated_matches_one_gpu(ctx, reg, reg)
+
+
+CHECKS = {"core": core, "updater": updater, "dropout": dropout, "noise": noise, "gradnorm": gradnorm, "constraint": constraint,
+          "regularization": regularization}
 
 
 def main():

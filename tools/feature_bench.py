@@ -473,6 +473,12 @@ def updater(kind):
     return dict(name=kind, swap=lambda s: with_kind(s, kind), kernels=UPDATER, model=model)
 
 
+# ---------------------------------------------------------------- regularization: the reference's l2 1e-4 on every W, against l1, l2, l1Bias
+# and l2Bias on every layer (the same one updater pass; the score sums are not part of the step)
+def regularize(**coefs):
+    return lambda net: net.set_regularization(**coefs)
+
+
 # ---------------------------------------------------------------- weightinit: b2g_net_init_weights over bench.py's nets
 INIT_SCHEMES = (("distribution_normal_0.02", m.weight_init("distribution", m.normal(0, 0.02))), ("xavier", m.weight_init("xavier")),
                 ("xavier_uniform", m.weight_init("xavier_uniform")), ("var_scaling_normal_fan_avg", m.weight_init("var_scaling_normal_fan_avg")))
@@ -544,6 +550,9 @@ FEATURES = {
     "patchgan": dict(configs="c2,c4", steps=50, variants=[{}, dict(name="patch", d=dict(patch=True))], kernels=cnn_loss_kernels, extras=head_conv),
     "pooling": dict(configs="c2", variants=[dict(name="base"), dict(name="sum", d=dict(global_pooling="sum")),
                                             dict(name="avg", d=dict(global_pooling="avg"))], kernels=pooling_kernels),
+    "regularization": dict(configs="c5,c2", variants=[
+        dict(name="l2", hook=regularize(l2=1e-4), kernels=UPDATER, model=params_model),
+        dict(name="l1+l2+l1bias+l2bias", hook=regularize(l1=1e-4, l2=1e-4, l1_bias=1e-4, l2_bias=1e-4), kernels=UPDATER, model=params_model)]),
     "schedule": dict(configs="c5,c2", variants=[dict(kernels=UPDATER, model=params_model),
                                                 dict(name="exponential_schedule", hook=schedule, kernels=UPDATER, model=params_model)]),
     "updater": dict(configs="c5,c2", variants=[updater(k) for k in ("adam", "nesterovs", "adagrad", "adamax", "nadam", "amsgrad", "adadelta")]),
