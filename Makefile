@@ -4,7 +4,7 @@ ARCH := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall,-Wno-unused-function -Xptxas -v
 SRC := gan_deeplearning4j_b200/csrc
 OUT := gan_deeplearning4j_b200/lib
-OBJS := $(OUT)/kernels_ew.o $(OUT)/kernels_dropout.o $(OUT)/kernels_act.o $(OUT)/kernels_pool.o $(OUT)/kernels_cnnloss.o $(OUT)/kernels_head.o $(OUT)/kernels_graph.o $(OUT)/kernels_gradnorm.o $(OUT)/kernels_constraint.o $(OUT)/kernels_init.o $(OUT)/kernels_simt.o $(OUT)/kernels_tc.o $(OUT)/kernels_edge.o $(OUT)/engine.o $(OUT)/jni_shim.o
+OBJS := $(OUT)/kernels_ew.o $(OUT)/kernels_dropout.o $(OUT)/kernels_act.o $(OUT)/kernels_pool.o $(OUT)/kernels_cnnloss.o $(OUT)/kernels_head.o $(OUT)/kernels_graph.o $(OUT)/kernels_prelu.o $(OUT)/kernels_gradnorm.o $(OUT)/kernels_constraint.o $(OUT)/kernels_init.o $(OUT)/kernels_simt.o $(OUT)/kernels_tc.o $(OUT)/kernels_edge.o $(OUT)/engine.o $(OUT)/jni_shim.o
 
 all: $(OUT)/libb200gan.so
 

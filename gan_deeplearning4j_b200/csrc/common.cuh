@@ -91,6 +91,43 @@ __device__ __forceinline__ float ldf(const __nv_bfloat16* p, size_t i) { return 
 __device__ __forceinline__ void stf(float* p, size_t i, float v) { p[i] = v; }
 __device__ __forceinline__ void stf(__nv_bfloat16* p, size_t i, float v) { p[i] = __float2bfloat16_rn(v); }
 
+// One 16-byte chunk of V elements of T, widened to fp32 (the element-wise streams of kernels_graph.cu and kernels_prelu.cu)
+template <typename T> struct GVec;
+template <> struct GVec<float> {
+  static constexpr int V = 4;
+  static __device__ __forceinline__ void load(const float* p, float* v) { const float4 q = *reinterpret_cast<const float4*>(p); v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w; }
+  static __device__ __forceinline__ void store(float* p, const float* v) { *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]); }
+};
+template <> struct GVec<__nv_bfloat16> {
+  static constexpr int V = 8;
+  static __device__ __forceinline__ void load(const __nv_bfloat16* p, float* v) {
+    const uint4 q = *reinterpret_cast<const uint4*>(p); const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&q);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) { const float2 f = __bfloat1622float2(h[k]); v[2 * k] = f.x; v[2 * k + 1] = f.y; }
+  }
+  static __device__ __forceinline__ void store(__nv_bfloat16* p, const float* v) {
+    uint4 q; __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&q);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) h[k] = __floats2bfloat162_rn(v[2 * k], v[2 * k + 1]);
+    *reinterpret_cast<uint4*>(p) = q;
+  }
+};
+// Load / store V elements starting at e: the 16-byte path when VEC and the chunk is whole, else element by element (clipped to n)
+template <typename T, bool VEC>
+__device__ __forceinline__ void ld_chunk(const T* p, size_t e, size_t n, float* v) {
+  constexpr int V = GVec<T>::V;
+  if (VEC && e + V <= n) { GVec<T>::load(p + e, v); return; }
+#pragma unroll
+  for (int k = 0; k < V; ++k) v[k] = e + k < n ? ldf(p, e + k) : 0.f;
+}
+template <typename T, bool VEC>
+__device__ __forceinline__ void st_chunk(T* p, size_t e, size_t n, const float* v) {
+  constexpr int V = GVec<T>::V;
+  if (VEC && e + V <= n) { GVec<T>::store(p + e, v); return; }
+#pragma unroll
+  for (int k = 0; k < V; ++k) if (e + k < n) stf(p, e + k, v[k]);
+}
+
 // org.nd4j.linalg.activations.impl.Activation{Identity,TanH,Sigmoid,ReLU,LReLU}
 __device__ __forceinline__ float act_fwd(int act, float z, float alpha) {
   switch (act) {

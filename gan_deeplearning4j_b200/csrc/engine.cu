@@ -118,6 +118,8 @@ struct LayerRT {
   // consumer of j the backward visits (it writes j's accumulator; the later ones add).  A skip source: its consumer count and fp32 accumulator.
   int vsrc = -1, vorder = 0; bool vfirst = false;
   int n_skip = 0; float* skip_acc = nullptr;
+  // PRELU (kernels_prelu.cu): the map and shared-axes mask; the slope gradient's row-group partials (non-frozen layers)
+  PreluGeom pg{}; float* prelu_part = nullptr;
   // a stochastic DropoutLayer: train mode draws from the pass counter.  FrozenLayer: test mode, identity; p = 1, rate = 0, stddev = 0: identity
   bool drop_active() const {
     if (d.type != B2G_LAYER_DROPOUT || d.frozen) return false;
@@ -125,6 +127,8 @@ struct LayerRT {
     return d.act == B2G_DROPOUT_GAUSSIAN_DROPOUT || d.act == B2G_DROPOUT_GAUSSIAN_NOISE ? d.act_alpha > 0.f : d.act_alpha < 1.f;
   }
   bool has_gemm() const { return d.type == B2G_LAYER_CONV2D || d.type == B2G_LAYER_DECONV2D || d.type == B2G_LAYER_DENSE || d.type == B2G_LAYER_OUTPUT; }
+  // a layer whose W takes l1 / l2 (b2g_regularization): the GEMM layers and PReLU's slopes
+  bool has_reg() const { return has_gemm() || d.type == B2G_LAYER_PRELU; }
   // Weight noise (b2g_net_set_weight_noise; wn.p_schedule is never kept): the layer's DropConnect schedule on the device (MAP entries in
   // wn_map).  Its noisy operands, allocated when the layer first gets noise: wn_w = W' (fp32 in FP32 nets; in BF16 nets the bf16 straight
   // copy, and the packed pixel-shuffle copy from element wn_ps on), wn_b = b' (fp32).  wn_live: the latest forward was a train-mode pass that
@@ -383,6 +387,17 @@ static int32_t net_build(b2g_net* n, const b2g_layer_desc* layers, int32_t nl) {
         l.vsrc = j; l.vorder = d.pre_w;
         l.oh = h; l.ow = w; l.oc = d.type == B2G_LAYER_MERGE ? ch + src.oc : ch;
       } break;
+      case B2G_LAYER_PRELU: {        // PReLULayer: the shared-axes mask in act, inputShape (0 = not given) in pre_c, pre_h, pre_w
+        // a 1x1 map is a feed-forward input [F] (axis 1 only) unless inputShape says [C, 1, 1]
+        const bool ff = h == 1 && w == 1 && !(d.pre_h == 1 && d.pre_w == 1);
+        if (d.act < 0 || (d.act >> (ff ? 1 : 3)) != 0) return fail(B2G_ERR_ARG, "layer %s: shared axes mask 0x%x outside the input's %d dimension(s)", d.name, d.act, ff ? 1 : 3);
+        if ((d.pre_c || d.pre_h || d.pre_w) && (d.pre_c != ch || (ff ? (d.pre_h || d.pre_w) : (d.pre_h != h || d.pre_w != w))))
+          return fail(B2G_ERR_SHAPE, "layer %s: inputShape [%d,%d,%d] != the inferred input [%d,%d,%d] (a feed-forward input is [%d])", d.name, d.pre_c, d.pre_h, d.pre_w, ch, h, w, ch);
+        l.oh = h; l.ow = w; l.oc = ch;
+        l.pg = PreluGeom{h, w, ch, d.act};
+        l.wA = 1; l.wTaps = 1; l.n_W = (int64_t)prelu_slopes(l.pg); l.wB = (int)l.n_W;
+        l.off_W = off; off += l.n_W;           // "W" in DL4J's [C][H][W] order with the shared axes of extent 1
+      } break;
       default: return fail(B2G_ERR_ARG, "layer %d: unknown type %d", i, d.type);
     }
     l.out_elems = (size_t)l.oh * l.ow * l.oc;
@@ -447,6 +462,7 @@ static int32_t net_alloc(b2g_net* n) {
     if (l.ext_act && l.has_gemm() && l.d.type != B2G_LAYER_OUTPUT) B2(dalloc(n, (char**)&l.ext_z, ts * R * l.out_elems));
     if (l.d.type == B2G_LAYER_MAXPOOL) B2(dalloc(n, &l.argmax, (size_t)R * l.out_elems));
     if (l.n_skip) B2(dalloc(n, &l.skip_acc, sizeof(float) * R * l.out_elems));
+    if (l.d.type == B2G_LAYER_PRELU && !l.d.frozen) B2(dalloc(n, &l.prelu_part, sizeof(float) * k_prelu_part_floats(R, l.pg)));
     if (l.d.type == B2G_LAYER_GLOBAL_POOLING) {
       if (l.pool == B2G_POOL_MAX) B2(dalloc(n, &l.pool_idx, sizeof(int32_t) * R * l.oc));
       const size_t part = k_global_pool_partial_elems(n->prec, R, l.ih * l.iw, l.ic);
@@ -518,7 +534,7 @@ static int32_t net_init_params_and_updater(b2g_net* n) {
       sg.lr = d.lr; sg.b1 = d.beta1; sg.b2 = d.beta2; sg.eps = d.eps; sg.l2 = weight ? d.l2 : 0.f; sg.l1 = 0.f; sg.clip = n->cfg.grad_clip; sg.div_mb = noop ? 0 : 1;
       sg.off_bf = (weight && l.off_W_bf >= 0) ? l.off_W_bf : -1; sg.off_ps = (weight && l.off_Wps_bf >= 0) ? l.off_Wps_bf : -1; sg.ps_O = l.geom.O; sg.ps_C = l.geom.C; n->segs.push_back(sg); seg_layer.push_back((int)(&l - n->L.data()));
       if (!noop && (sg.kind == 1 || sg.kind == 5)) for (int64_t i = 0; i < len; ++i) h0[off + i] = d.eps;     // RmsProp cache / AdaGrad history initialised to epsilon
-      if (l.has_gemm()) { n->reg_seg.push_back((int)n->segs.size() - 1); rego.push_back(off); regl.push_back(len); n->reg_l2c.push_back(0.5f * sg.l2); n->reg_l1c.push_back(0.f); }
+      if (l.has_reg()) { n->reg_seg.push_back((int)n->segs.size() - 1); rego.push_back(off); regl.push_back(len); n->reg_l2c.push_back(0.5f * sg.l2); n->reg_l1c.push_back(0.f); }
     };
     if (l.has_gemm()) {
       l.reg.l2 = d.l2;
@@ -533,6 +549,9 @@ static int32_t net_init_params_and_updater(b2g_net* n) {
       for (int c = 0; c < l.oc; ++c) { hp[l.off_gamma + c] = 1.f; hp[l.off_var + c] = 1.f; }
       add_seg(l.off_gamma, l.oc, false, false); add_seg(l.off_beta, l.oc, false, false);
       add_seg(l.off_mean, l.oc, false, true); add_seg(l.off_var, l.oc, false, true);
+    } else if (d.type == B2G_LAYER_PRELU) {      // alpha starts at 0 (hp): a new PReLU is a ReLU
+      l.reg.l2 = d.l2;
+      add_seg(l.off_W, l.n_W, true, false);
     }
   }
   CU(cudaMemcpyAsync(n->params, hp.data(), sizeof(float) * n->n_params, cudaMemcpyHostToDevice, s));
@@ -814,6 +833,7 @@ static int32_t net_forward(b2g_net* n, const void* in, const FwdOpts& o, const v
         if (l.vorder) k_merge_fwd(n->prec, src.out, cur, out, px, src.oc, l.ic, s);
         else k_merge_fwd(n->prec, cur, src.out, out, px, l.ic, src.oc, s);
       } break;
+      case B2G_LAYER_PRELU: k_prelu_fwd(n->prec, cur, out, n->params + l.off_W, R, l.pg, s); break;     // the same function in both modes
     }
     if (l.ext_z) k_act_ext_fwd(n->prec, l.ext_act, l.ext_alpha, l.ext_z, out, (size_t)R * l.out_elems, s);
     if (fuse) n->L[i + 1].stats_by_producer = fused;
@@ -893,7 +913,7 @@ static int32_t net_backward(b2g_net* n, const void* net_in, void* eps, int rows,
     const void* lin = i == 0 ? net_in : n->L[i - 1].out;
     // the epsilon w.r.t. this layer's input is needed only if a trainable layer sits below it (or the caller wants d/d input)
     bool need_in = need_input_grad;
-    if (!need_in) for (int j = 0; j < i; ++j) if (!n->L[j].d.frozen && (n->L[j].has_gemm() || n->L[j].d.type == B2G_LAYER_BATCHNORM)) need_in = true;
+    if (!need_in) for (int j = 0; j < i; ++j) if (!n->L[j].d.frozen && (n->L[j].has_reg() || n->L[j].d.type == B2G_LAYER_BATCHNORM)) need_in = true;
     const bool want_wgrad_l = want_wgrad && !d.frozen;
     // a skip source: its vertices' shares join the spine epsilon before anything of its own backward runs
     if (l.skip_acc) k_skip_add(n->prec, cur, l.skip_acc, (size_t)R * l.out_elems, s);
@@ -973,6 +993,16 @@ static int32_t net_backward(b2g_net* n, const void* net_in, void* eps, int rows,
         if (need_in && l.drop_live) {
           if (d.act == B2G_DROPOUT && !l.drop_sched) k_dropout_bwd(n->prec, cur, cur, l.drop_mask, (size_t)R * l.out_elems, 1.0f / d.act_alpha, s);
           else k_noise_bwd(n->prec, d.act, cur, cur, l.drop_mask, l.drop_rec, (size_t)R * l.out_elems, noise_args(n, i), noise_sched(n, l, nullptr, nullptr), s);
+        }
+        break;
+      case B2G_LAYER_PRELU:         // dx in place from the layer's input x; a trainable layer also leaves its slope partials for the reduce list
+        if (need_in || want_wgrad_l) {
+          k_prelu_bwd(n->prec, lin, cur, n->params + l.off_W, want_wgrad_l ? l.prelu_part : nullptr, need_in ? 1 : 0, R, l.pg, s);
+          if (want_wgrad_l) {
+            fork_wgrad(i, cur);             // the side stream, which runs the pass's reduce list, starts after the partials
+            if (n->pending.count == ReduceList::MAX_JOBS) flush_pending_reduce(n, s2);
+            prelu_queue_reduce(&n->pending, l.prelu_part, n->grads + l.off_W, R, l.pg);
+          }
         }
         break;
     }
@@ -1627,6 +1657,7 @@ extern "C" int32_t b2g_net_set_constraints(b2g_net* n, const char* layer, const 
   if (cnt > 4) return fail(B2G_ERR_ARG, "%s.%s: %d constraints, at most 4 per tensor", layer, param, cnt);
   CU(cudaSetDevice(n->ctx->device));
   ParamRef r; B2(find_param(n, layer, param, &r));
+  if (n->L[r.layer].d.type == B2G_LAYER_PRELU) return fail(B2G_ERR_ARG, "layer %s: constraints on a PReLU's slopes are not supported", layer);
   const ConAxes a = con_axes(n, r, param);
   for (int i = 0; i < cnt; ++i) {
     const b2g_constraint& k = list[i];
@@ -1854,7 +1885,7 @@ extern "C" int32_t b2g_net_set_weight_noise(b2g_net* n, const char* layer, const
   std::vector<int> targets;
   if (layer) {
     for (size_t i = 0; i < n->L.size() && targets.empty(); ++i) if (!strncmp(n->L[i].d.name, layer, B2G_NAME_LEN)) {
-      if (!n->L[i].has_gemm()) return fail(B2G_ERR_ARG, "layer %s has no W (weight noise needs a conv, deconv, dense or output layer)", layer);
+      if (!n->L[i].has_gemm()) return fail(B2G_ERR_ARG, "layer %s: weight noise needs a conv, deconv, dense or output layer (not supported on a PReLU's slopes)", layer);
       targets.push_back((int)i);
     }
     if (targets.empty()) return fail(B2G_ERR_ARG, "no layer named %s", layer);
@@ -1900,6 +1931,8 @@ static int32_t check_weight_init(const b2g_weight_init& w) {
 // The draw of one layer's W under the scheme, from the desc's fans (the internal geometry of a 1x1-map deconv or whole-input conv aside)
 static int32_t weight_init_draw(const b2g_weight_init& w, const LayerRT& l, WiDraw* out) {
   const b2g_layer_desc& d = l.d;
+  if (d.type == B2G_LAYER_PRELU && w.scheme != B2G_WI_ZERO && w.scheme != B2G_WI_ONES && w.scheme != B2G_WI_DISTRIBUTION)
+    return fail(B2G_ERR_ARG, "layer %s: weight init %d needs fans, which a PReLU's slopes do not have (ZERO, ONES or DISTRIBUTION)", d.name, w.scheme);
   const bool conv = d.type == B2G_LAYER_CONV2D || d.type == B2G_LAYER_DECONV2D;
   const double fi = (double)d.n_in * l.wTaps, fo = (double)d.n_out * l.wTaps / (conv ? (double)(d.s_h * d.s_w) : 1.0);
   WiDraw r{}; double sd = -1.0, lim = -1.0, tsd = -1.0;
@@ -1943,7 +1976,7 @@ extern "C" int32_t b2g_net_init_weights(b2g_net* n, const char* layer, const b2g
   std::vector<int> targets;
   if (layer) {
     for (size_t i = 0; i < n->L.size() && targets.empty(); ++i) if (!strncmp(n->L[i].d.name, layer, B2G_NAME_LEN)) {
-      if (!n->L[i].has_gemm()) return fail(B2G_ERR_ARG, "layer %s has no W (weight init needs a conv, deconv, dense or output layer)", layer);
+      if (!n->L[i].has_reg()) return fail(B2G_ERR_ARG, "layer %s has no W (weight init needs a conv, deconv, dense, output or PReLU layer)", layer);
       targets.push_back((int)i);
     }
     if (targets.empty()) return fail(B2G_ERR_ARG, "no layer named %s", layer);
@@ -1964,9 +1997,9 @@ extern "C" int32_t b2g_net_init_weights(b2g_net* n, const char* layer, const b2g
 // ------------------------------------------------------------------ regularization (b2g_net_set_regularization) --------------------------
 // The coefficients live in the updater's segment table and the score table, both read from device memory at run time: a new value needs
 // no new launch, and a captured GAN step picks it up at its next replay without a re-capture.
-static int32_t find_gemm_layer(const b2g_net* n, const char* layer, int* li) {
+static int32_t find_reg_layer(const b2g_net* n, const char* layer, int* li) {
   for (size_t i = 0; i < n->L.size(); ++i) if (!strncmp(n->L[i].d.name, layer, B2G_NAME_LEN)) {
-    if (!n->L[i].has_gemm()) return fail(B2G_ERR_ARG, "layer %s has no W (regularization needs a conv, deconv, dense or output layer)", layer);
+    if (!n->L[i].has_reg()) return fail(B2G_ERR_ARG, "layer %s has no W (regularization needs a conv, deconv, dense, output or PReLU layer)", layer);
     *li = (int)i; return 0;
   }
   return fail(B2G_ERR_ARG, "no layer named %s", layer);
@@ -1975,11 +2008,11 @@ extern "C" int32_t b2g_net_set_regularization(b2g_net* n, const char* layer, con
   if (!n || !r) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
   const float v[4] = {r->l1, r->l2, r->l1_bias, r->l2_bias};
   for (float x : v) if (!(std::isfinite(x) && x >= 0.f)) return fail(B2G_ERR_ARG, "regularization coefficient %g: must be finite and >= 0", (double)x);
-  if (layer) { int li = 0; B2(find_gemm_layer(n, layer, &li)); n->L[li].reg = *r; }
-  else for (auto& l : n->L) if (l.has_gemm() && !l.d.frozen) l.reg = *r;
+  if (layer) { int li = 0; B2(find_reg_layer(n, layer, &li)); n->L[li].reg = *r; }
+  else for (auto& l : n->L) if (l.has_reg() && !l.d.frozen) l.reg = *r;
   for (size_t i = 0; i < n->segs.size(); ++i) {        // frozen layers own no segment: they take no term
     const LayerRT& l = n->L[n->seg_layer[i]];
-    if (!l.has_gemm()) continue;
+    if (!l.has_reg()) continue;
     const bool weight = n->segs[i].off == l.off_W;
     n->segs[i].l2 = weight ? l.reg.l2 : l.reg.l2_bias; n->segs[i].l1 = weight ? l.reg.l1 : l.reg.l1_bias;
   }
@@ -2000,7 +2033,7 @@ extern "C" int32_t b2g_net_set_regularization(b2g_net* n, const char* layer, con
 }
 extern "C" int32_t b2g_net_get_regularization(b2g_net* n, const char* layer, b2g_regularization* out) {
   if (!n || !layer || !out) return fail(B2G_ERR_ARG, "null");
-  int li = 0; B2(find_gemm_layer(n, layer, &li)); *out = n->L[li].reg; return 0;
+  int li = 0; B2(find_reg_layer(n, layer, &li)); *out = n->L[li].reg; return 0;
 }
 extern "C" int32_t b2g_net_calc_regularization(b2g_net* n, double* l1, double* l2) {
   if (!n) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
@@ -2661,6 +2694,29 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
       k_upsample_fwd(prec, x, y, o->N, o->H, o->W, o->C, f, s); ran();
       k_upsample_bwd(prec, eo, ei, o->N, o->H, o->W, o->C, f, s); ran();
       B2(m.downT(out0, y, no)); B2(m.downT(out1, ei, ni));
+      break;
+    }
+    case B2G_EW_PRELU_FWD: case B2G_EW_PRELU_BWD: {      // in0 = [x | alpha], act = the shared-axes mask, the map in N, H, W, C
+      const bool bwd = o->op == B2G_EW_PRELU_BWD;
+      if (!in0 || (bwd && !in1) || o->N < 1 || o->H < 1 || o->W < 1 || o->C < 1 || o->act < 0 || o->act > 7) return fail(B2G_ERR_ARG, "bad PRELU arguments");
+      const PreluGeom g{o->H, o->W, o->C, o->act};
+      const size_t n = (size_t)o->N * o->H * o->W * o->C, K = prelu_slopes(g);
+      if (n > (size_t)lim) return fail(B2G_ERR_ARG, "PRELU tensors too large");
+      void* x = nullptr; float* alpha = nullptr; B2(m.upT(in0, n, &x, off)); B2(m.upF(in0 + n, K, &alpha, off));
+      if (!bwd) {
+        void* y = nullptr; B2(m.dev(n, ts, &y, off)); B2(poison(y, ts * n));
+        k_prelu_fwd(prec, x, y, alpha, o->N, g, s); ran();
+        B2(m.downT(out0, y, n));
+      } else {        // out0 = dx in eps's buffer (in place; NULL: not written), out1 = dalpha (NULL: no slope gradient)
+        void* e = nullptr; float *part = nullptr, *da = nullptr; B2(m.upT(in1, n, &e, off));
+        if (out1) {
+          const size_t np = k_prelu_part_floats(o->N, g);
+          B2(m.upF(nullptr, np, &part, off)); B2(m.upF(nullptr, K, &da, off)); B2(poison(part, 4 * np)); B2(poison(da, 4 * K));
+        }
+        k_prelu_bwd(prec, x, e, alpha, part, out0 ? 1 : 0, o->N, g, s); ran();
+        if (out1) { ReduceList rl{}; prelu_queue_reduce(&rl, part, da, o->N, g); k_reduce_multi(rl, s); ran(); }
+        B2(m.downT(out0, e, n)); B2(m.downF(out1, da, K));
+      }
       break;
     }
     case B2G_EW_SUMSQ: {

@@ -199,6 +199,26 @@ void k_merge_bwd(int prec, const void* eps, void* dst, float* acc, size_t P, int
 // eps = eps + acc in fp32, rounded once to T (the skip gradient joining the spine at its source)
 void k_skip_add(int prec, void* eps, const float* acc, size_t n, cudaStream_t s);
 
+// ---- PReLULayer (kernels_prelu.cu; semantics and summation order at B2G_LAYER_PRELU in include/b200gan.h) ---------------------------
+// A [rows][H][W][C] map (a feed-forward input: H = W = 1, C = F).  The slopes alpha are in DL4J's order [C][H][W] with every axis whose bit is
+// set in `shared` (1 = C, 2 = H, 4 = W) of extent 1: K = prelu_slopes slopes, each shared by S = H*W*C / K positions of a row.
+struct PreluGeom { int H, W, C, shared; };
+__host__ __device__ inline size_t prelu_slopes(const PreluGeom& g) {
+  return (size_t)((g.shared & 1) ? 1 : g.C) * ((g.shared & 2) ? 1 : g.H) * ((g.shared & 4) ? 1 : g.W);
+}
+// The backward's row groups for `rows` rows (a function of the shape only): *groups groups of *rows_per_group consecutive rows, the last ragged
+void prelu_row_groups(int rows, const PreluGeom& g, int* groups, int* rows_per_group);
+// fp32 partial sums the backward of a pass of up to max_rows rows writes
+size_t k_prelu_part_floats(int max_rows, const PreluGeom& g);
+// y = x < 0 ? alpha*x : x (one launch)
+void k_prelu_fwd(int prec, const void* x, void* y, const float* alpha, int rows, const PreluGeom& g, cudaStream_t s);
+// One launch: eps = x < 0 ? alpha*eps : eps in place (write_dx); part (may be null): part[(grp*S + s)*K + k] = the fp32 sum, over the rows of
+// row group grp in ascending order, of x*eps (x < 0) at the position s of slope k
+void k_prelu_bwd(int prec, const void* x, void* eps, const float* alpha, float* part, int write_dx, int rows, const PreluGeom& g, cudaStream_t s);
+// Queues dalpha[k] = sum over t < groups*S of part[t*K + k] as one job of a reduce list (k_reduce_multi sums it)
+struct ReduceList;
+void prelu_queue_reduce(ReduceList* rl, const float* part, float* dalpha, int rows, const PreluGeom& g);
+
 // ---- reductions ------------------------------------------------------------------------------------
 // out[c] (+)= sum_rows x[row][c]
 void k_colsum(int prec, const void* x, int rows, int C, float* scratch, float* out, int accumulate, cudaStream_t s);

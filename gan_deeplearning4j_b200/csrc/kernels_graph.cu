@@ -16,26 +16,6 @@ namespace {
 
 constexpr int GR_THREADS = 256;
 
-template <typename T> struct GVec;       // one 16-byte chunk of V elements of T, widened to fp32
-template <> struct GVec<float> {
-  static constexpr int V = 4;
-  static __device__ __forceinline__ void load(const float* p, float* v) { const float4 q = *reinterpret_cast<const float4*>(p); v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w; }
-  static __device__ __forceinline__ void store(float* p, const float* v) { *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]); }
-};
-template <> struct GVec<__nv_bfloat16> {
-  static constexpr int V = 8;
-  static __device__ __forceinline__ void load(const __nv_bfloat16* p, float* v) {
-    const uint4 q = *reinterpret_cast<const uint4*>(p); const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&q);
-#pragma unroll
-    for (int k = 0; k < 4; ++k) { const float2 f = __bfloat1622float2(h[k]); v[2 * k] = f.x; v[2 * k + 1] = f.y; }
-  }
-  static __device__ __forceinline__ void store(__nv_bfloat16* p, const float* v) {
-    uint4 q; __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&q);
-#pragma unroll
-    for (int k = 0; k < 4; ++k) h[k] = __floats2bfloat162_rn(v[2 * k], v[2 * k + 1]);
-    *reinterpret_cast<uint4*>(p) = q;
-  }
-};
 // V fp32 values of the accumulator (V = 4 or 8: one or two float4)
 template <int V> __device__ __forceinline__ void acc_load(const float* p, float* v) {
 #pragma unroll
@@ -46,21 +26,6 @@ template <int V> __device__ __forceinline__ void acc_store(float* p, const float
   for (int k = 0; k < V; k += 4) *reinterpret_cast<float4*>(p + k) = make_float4(v[k], v[k + 1], v[k + 2], v[k + 3]);
 }
 
-// Load / store V elements starting at e: the 16-byte path when VEC and the chunk is whole, else element by element (clipped to n)
-template <typename T, bool VEC>
-__device__ __forceinline__ void ld_chunk(const T* p, size_t e, size_t n, float* v) {
-  constexpr int V = GVec<T>::V;
-  if (VEC && e + V <= n) { GVec<T>::load(p + e, v); return; }
-#pragma unroll
-  for (int k = 0; k < V; ++k) v[k] = e + k < n ? ldf(p, e + k) : 0.f;
-}
-template <typename T, bool VEC>
-__device__ __forceinline__ void st_chunk(T* p, size_t e, size_t n, const float* v) {
-  constexpr int V = GVec<T>::V;
-  if (VEC && e + V <= n) { GVec<T>::store(p + e, v); return; }
-#pragma unroll
-  for (int k = 0; k < V; ++k) if (e + k < n) stf(p, e + k, v[k]);
-}
 template <int V, bool VEC>
 __device__ __forceinline__ void ld_acc(const float* p, size_t e, size_t n, float* v) {
   if (VEC && e + V <= n) { acc_load<V>(p + e, v); return; }

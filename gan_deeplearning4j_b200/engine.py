@@ -18,7 +18,7 @@ from ._lib import GanConfig, LayerDesc, LrSchedule, NetConfig, check
 
 LAYER_TYPES = {"conv2d": 0, "deconv2d": 1, "batchnorm": 2, "dense": 3, "activation": 4, "maxpool": 5, "upsample2d": 6,
                "output": 7, "loss": 8, "ff_to_cnn": 9, "cnn_to_ff": 10, "dropout": 11, "subsampling": 12, "global_pooling": 13,
-               "cnn_loss": 14, "elementwise": 15, "merge": 16}
+               "cnn_loss": 14, "elementwise": 15, "merge": 16, "prelu": 17}
 # ElementWiseVertex.Op -> b2g_elementwise_op, carried in b2g_layer_desc.act of "elementwise" specs (semantics in include/b200gan.h)
 ELEMENTWISE_OPS = {"add": 0, "subtract": 1, "product": 2, "average": 3, "max": 4}
 VERTEX_TYPES = ("elementwise", "merge")
@@ -94,11 +94,33 @@ def schedule_struct(sched: Optional[Dict]):
     return s, keep
 
 
+# PReLULayer (B2G_LAYER_PRELU in include/b200gan.h): DL4J's 1-based sharedAxes (1 = C, 2 = H, 3 = W) -> the bit mask b2g_layer_desc.act carries
+def prelu_shared_mask(spec: Dict) -> int:
+    """The shared-axes bit mask of a "prelu" spec; ValueError for an axis outside 1-3 (the engine refuses a bit outside the input's rank)."""
+    axes = [int(a) for a in spec.get("shared_axes", ())]
+    if any(a not in (1, 2, 3) for a in axes):
+        raise ValueError(f"prelu layer {spec.get('name', '')!r}: shared axes {axes}; DL4J's axes are 1 (C), 2 (H) and 3 (W)")
+    return sum(1 << (a - 1) for a in set(axes))
+
+
+def prelu_groups(rows: int, row_elems: int) -> int:
+    """The row groups of a PReLU backward over `rows` rows of `row_elems` elements (the summation order at B2G_LAYER_PRELU in
+    include/b200gan.h): each writes one fp32 slope partial per row element."""
+    bx = -(-row_elems // 2048)
+    g0 = max(1, min(rows, 64, max(1, 1024 // bx)))
+    rpg = -(-rows // g0)
+    return -(-rows // rpg)
+
+
+# a PReLU layer's slopes take ZERO, ONES and DISTRIBUTION (the other schemes need fans it does not have)
+PRELU_WEIGHT_INITS = ("zero", "ones", "distribution")
+
+
 def layer_has_lr(spec: Dict) -> bool:
     """A layer whose updater has a learning rate: it has parameters, is not frozen and its updater is neither NoOp nor AdaDelta.  A spec
     without an updater is Sgd with lr 0 (layer_desc), so it has one.  The engine applies the same rule (engine.cu layer_has_lr)."""
     u = spec.get("updater") or {"kind": "sgd"}
-    return spec["type"] in ("conv2d", "deconv2d", "dense", "output", "batchnorm") and not spec.get("frozen", False) and u["kind"] not in NO_LR_UPDATERS
+    return spec["type"] in ("conv2d", "deconv2d", "dense", "output", "batchnorm", "prelu") and not spec.get("frozen", False) and u["kind"] not in NO_LR_UPDATERS
 
 
 def follow_lr_schedule(specs: List[Dict], constant: List[float], schedule: Optional[Dict], layer: Optional[str] = None):
@@ -120,6 +142,8 @@ def follow_lr_schedule(specs: List[Dict], constant: List[float], schedule: Optio
 CONSTRAINT_KINDS = {"max_norm": 0, "min_max_norm": 1, "unit_norm": 2, "non_negative": 3}
 CONSTRAINT_ON = ("all", "weights", "bias")      # also the order a layer's lists apply in: constrainAllParameters, Weights, Bias
 GEMM_TYPES = ("conv2d", "deconv2d", "dense", "output")
+# the layers whose W takes l1 / l2: the GEMM layers and PReLU's slopes
+REG_TYPES = GEMM_TYPES + ("prelu",)
 
 
 def constraint_params(spec: Dict, on: str) -> List[str]:
@@ -189,17 +213,17 @@ def spec_regularization(spec: Dict) -> Dict[str, float]:
 
 
 def resolve_regularization(specs: List[Dict], regularization: Optional[Dict] = None) -> List[Dict]:
-    """Fills in the global builder's coefficients (regularization, may be None) in place: every non-frozen conv, deconv, dense and output spec
-    takes each key it does not set itself, as DL4J's builder fills in a layer's NaN fields.  Then checks each GEMM spec's "l1", "l1_bias" and
-    "l2_bias" ("l2" is the desc's, as before).  Returns specs."""
+    """Fills in the global builder's coefficients (regularization, may be None) in place: every non-frozen conv, deconv, dense, output and
+    prelu spec takes each key it does not set itself, as DL4J's builder fills in a layer's NaN fields.  Then checks each such spec's "l1",
+    "l1_bias" and "l2_bias" ("l2" is the desc's, as before).  Returns specs."""
     if regularization is not None:
         glob = check_regularization(regularization)
         for sp in specs:
-            if sp["type"] in GEMM_TYPES and not sp.get("frozen", False):
+            if sp["type"] in REG_TYPES and not sp.get("frozen", False):
                 for k, v in glob.items():
                     sp.setdefault(k, v)
     for sp in specs:
-        if sp["type"] in GEMM_TYPES:
+        if sp["type"] in REG_TYPES:
             check_regularization({k: sp[k] for k in REGULARIZATION_KEYS if k in sp and k != "l2"}, f"layer {sp.get('name', '')!r}")
     return specs
 
@@ -343,6 +367,8 @@ def weight_init_struct(wi: Dict, spec: Optional[Dict] = None):
             raise ValueError(f"uniform distribution upper {dist['upper']} < lower {dist['lower']}")
         if kind == "binomial" and not (0 <= a <= 65536 and a == np.floor(a) and 0 <= b <= 1):
             raise ValueError(f"binomial distribution needs a whole n_trials in [0, 65536] and p in [0, 1]: {dist}")
+    if spec is not None and spec["type"] == "prelu" and scheme not in PRELU_WEIGHT_INITS:
+        raise ValueError(f"layer {spec.get('name', '')!r}: weight init {scheme!r} needs fans, which a PReLU's slopes do not have; one of {list(PRELU_WEIGHT_INITS)}")
     if scheme == "identity" and spec is not None:
         if spec["type"] not in ("dense", "output"):
             raise ValueError(f"layer {spec.get('name', '')!r}: weight init 'identity' needs a dense or output layer")
@@ -392,6 +418,12 @@ def layer_desc(spec: Dict, skip: Optional[tuple] = None) -> LayerDesc:
     if spec["type"] in VERTEX_TYPES:       # the op in act, the skip source and the input order in pre_h / pre_w
         d.act = ELEMENTWISE_OPS[spec["op"]] if spec["type"] == "elementwise" else 0
         d.pre_h, d.pre_w = skip
+    if spec["type"] == "prelu":            # the shared-axes mask in act, inputShape [C, H, W] or [F] in pre_c, pre_h, pre_w (0: not given)
+        d.act, d.act_alpha = prelu_shared_mask(spec), 0.0
+        shape = [int(v) for v in spec.get("input_shape", ())]
+        if len(shape) not in (0, 1, 3):
+            raise ValueError(f"prelu layer {spec.get('name', '')!r}: input_shape {shape} is neither [C, H, W] nor [F]")
+        d.pre_c, d.pre_h, d.pre_w = (shape + [0, 0, 0])[:3] if len(shape) != 3 else shape
     return d
 
 
@@ -474,7 +506,7 @@ class Net:
             for sp in self.specs:
                 if sp["type"] in GEMM_TYPES and "weight_init" not in sp:
                     sp["weight_init"] = copy.deepcopy(weight_init)
-        inits = [(sp["name"], weight_init_struct(sp["weight_init"], sp)) for sp in self.specs if sp["type"] in GEMM_TYPES and sp.get("weight_init") is not None]
+        inits = [(sp["name"], weight_init_struct(sp["weight_init"], sp)) for sp in self.specs if sp["type"] in REG_TYPES and sp.get("weight_init") is not None]
         if constraints:
             for sp in self.specs:
                 if sp["type"] in GEMM_TYPES + ("batchnorm",) and not resolve_constraints(sp):
@@ -503,7 +535,7 @@ class Net:
                 check(self.lib.b2g_net_init_weights(self.h, name.encode(), C.byref(s)))
             for sp in self.specs:         # Layer.Builder.l1 / l1Bias / l2Bias (l2 alone travels in the desc)
                 r = spec_regularization(sp)
-                if sp["type"] in GEMM_TYPES and (r["l1"] or r["l1_bias"] or r["l2_bias"]):
+                if sp["type"] in REG_TYPES and (r["l1"] or r["l1_bias"] or r["l2_bias"]):
                     check(self.lib.b2g_net_set_regularization(self.h, sp["name"].encode(), C.byref(regularization_struct(r))))
             if gradient_normalization != "none":
                 self.set_gradient_normalization(gradient_normalization, gradient_normalization_threshold)
@@ -681,8 +713,9 @@ class Net:
 
     def init_weights(self, weight_init: Dict, layer: Optional[str] = None):
         """Redraws W and sets b = bias_init now (b2g_net_init_weights; models.weight_init): layer None = every conv, deconv, dense and output
-        layer.  Nothing else changes.  The specs a checkpoint writes follow."""
-        targets = [sp for sp in self.specs if sp["type"] in GEMM_TYPES and (layer is None or sp.get("name") == layer)]
+        layer; a named prelu layer takes "zero", "ones" and "distribution" for its slopes.  Nothing else changes.  The specs a checkpoint
+        writes follow."""
+        targets = [sp for sp in self.specs if (sp["type"] in GEMM_TYPES or (layer is not None and sp["type"] == "prelu")) and (layer is None or sp.get("name") == layer)]
         if layer is not None:
             targets = targets[:1]
         s = weight_init_struct(weight_init)
@@ -693,13 +726,13 @@ class Net:
             sp["weight_init"] = copy.deepcopy(weight_init)
 
     def set_regularization(self, l1: float = 0.0, l2: float = 0.0, l1_bias: float = 0.0, l2_bias: float = 0.0, layer: Optional[str] = None):
-        """l1 / l2 on W and l1Bias / l2Bias on b (b2g_net_set_regularization): layer None = every non-frozen conv, deconv, dense and output
-        layer.  Replaces all four coefficients (the spec's "l2" too), from the next update and score on.  The specs a checkpoint writes
-        follow: a coefficient of 0 leaves no key."""
+        """l1 / l2 on W and l1Bias / l2Bias on b (b2g_net_set_regularization): layer None = every non-frozen conv, deconv, dense, output and
+        prelu layer (a prelu layer's W is its slopes; it has no b).  Replaces all four coefficients (the spec's "l2" too), from the next update
+        and score on.  The specs a checkpoint writes follow: a coefficient of 0 leaves no key."""
         r = check_regularization({"l1": l1, "l2": l2, "l1_bias": l1_bias, "l2_bias": l2_bias})
         check(self.lib.b2g_net_set_regularization(self.h, None if layer is None else layer.encode(), C.byref(regularization_struct(r))))
         for sp in self.specs:
-            if sp["type"] not in GEMM_TYPES or (layer is None and sp.get("frozen", False)) or (layer is not None and sp.get("name") != layer):
+            if sp["type"] not in REG_TYPES or (layer is None and sp.get("frozen", False)) or (layer is not None and sp.get("name") != layer):
                 continue
             for k, v in r.items():
                 if v:
@@ -710,7 +743,7 @@ class Net:
                 break
 
     def get_regularization(self, layer: str) -> Dict[str, float]:
-        """The four coefficients of a conv, deconv, dense or output layer, as the engine holds them (fp32)."""
+        """The four coefficients of a conv, deconv, dense, output or prelu layer, as the engine holds them (fp32)."""
         r = _lib.Regularization()
         check(self.lib.b2g_net_get_regularization(self.h, layer.encode(), C.byref(r)))
         return {k: getattr(r, k) for k in REGULARIZATION_KEYS}
@@ -978,7 +1011,8 @@ def test_dropout(ctx: Context, precision: int, x, dy, p: float, *, seed: int = 6
 
 EW_OPS = {"reduce_splits": 0, "reduce_multi": 1, "colsum": 2, "xent": 3, "softmax_xent": 4, "act_fwd": 5, "act_bwd": 6, "maxpool": 7,
           "upsample": 8, "sumsq": 9, "loss": 10, "act_ext_fwd": 11, "act_ext_bwd": 12,
-          "cnn_xent": 13, "cnn_softmax_xent": 14, "vertex_fwd": 15, "vertex_bwd": 16, "merge_fwd": 17, "merge_bwd": 18, "skip_add": 19}
+          "cnn_xent": 13, "cnn_softmax_xent": 14, "vertex_fwd": 15, "vertex_bwd": 16, "merge_fwd": 17, "merge_bwd": 18, "skip_add": 19,
+          "prelu_fwd": 20, "prelu_bwd": 21}
 
 
 def test_ew(ctx: Context, precision: int, op: str, in0, in1=None, out_sizes=(0, 0, 0), *, act: str = "identity", jobs=None, segments=None,
@@ -986,12 +1020,16 @@ def test_ew(ctx: Context, precision: int, op: str, in0, in1=None, out_sizes=(0, 
     """One reduction / loss / element-wise kernel through its production wrapper (b2g_test_ew; operands per op in include/b200gan.h).
     vertex_fwd / vertex_bwd: act is an ELEMENTWISE_OPS name and groups the input order.
     act_ext_fwd / act_ext_bwd (act: a name of codes 5-16): in0 = z, in1 = eps_out, out0 = f(z) / eps_out * f'(z).
+    prelu_fwd / prelu_bwd: in0 = x then alpha, in1 = dy; shared = the shared-axes bit mask (1 = C, 2 = H, 4 = W), the map in N, H, W, C;
+    out0 = y / dx, out1 = dalpha (0: not asked for).
     out_sizes: element counts of out0..out2 (0: not asked for).  opts: the b2g_test_ew_opts sizes and switches (n, rows, cols, groups, splits,
     stride, N, H, W, C, KH, KW, SH, SW, alpha, clip_eps, offset, in_place, accumulate, poison).  jobs (reduce_multi): dicts of n, splits,
     stride, src_off, dst_off.  segments (sumsq): (offsets, lengths, coefficients).  loss (op "loss"): a LOSSES name of codes 2-8.
     Returns ([out0, out1, out2] with None where not asked for, {"kernel": names, "sumsq": float, "wide": [per job]})."""
     o = _lib.TestEwOpts()
     o.op, o.act, o.loss = EW_OPS[op], ELEMENTWISE_OPS[act] if op in ("vertex_fwd", "vertex_bwd") else ACTS[act], LOSSES[loss]
+    if op in ("prelu_fwd", "prelu_bwd"):
+        o.act = int(opts.pop("shared", 0))
     for k, v in opts.items():
         setattr(o, k, int(v) if isinstance(v, bool) else v)
     keep = []

@@ -240,6 +240,28 @@ def cnn_loss(loss="xent", activation="identity", name="", alpha=None) -> Dict:
     return spec
 
 
+# ------------------------------------------------------------------ learned activation -----------------
+def prelu(shared_axes=(), name="", input_shape=None) -> Dict:
+    """new PReLULayer.Builder().sharedAxes(shared_axes).inputShape(input_shape) (B2G_LAYER_PRELU in include/b200gan.h): y = x < 0 ? alpha*x : x
+    with learned slopes alpha ("W", starting at 0), one per element of the input shape except along DL4J's shared axes (1 = C, 2 = H, 3 = W):
+    (2, 3) is one slope per channel.  input_shape ([C, H, W] or [F]), when given, must be the inferred input.  Add "updater", "l1" / "l2",
+    "weight_init" (zero, ones, distribution) or "frozen" like on any layer with parameters."""
+    spec = {"type": "prelu", "name": name, "shared_axes": sorted({int(a) for a in shared_axes})}
+    if input_shape is not None:
+        spec["input_shape"] = [int(v) for v in input_shape]
+    from .engine import prelu_shared_mask
+    prelu_shared_mask(spec)
+    return spec
+
+
+def _act_layer(name, activation, alpha, updater) -> Dict:
+    """The activation of a BatchNorm block: an ActivationLayer, or for activation "prelu" a PReLULayer shared over H and W (one slope per channel)
+    on the block's updater."""
+    if activation == "prelu":
+        return dict(prelu((2, 3), name), updater=updater())
+    return dict({"type": "activation", "name": name}, **_act(activation, alpha))
+
+
 # ------------------------------------------------------------------ skip connections -------------------
 # ElementWiseVertex / MergeVertex (B2G_LAYER_ELEMENTWISE / B2G_LAYER_MERGE in include/b200gan.h).  A vertex's inputs are layer names: one of them
 # must be the layer right before it (the spine), the other any earlier layer (engine.resolve_vertices).
@@ -261,13 +283,14 @@ def merge(inputs, name="") -> Dict:
 
 def residual_block(prefix, ch, skip, lr=2e-4, beta1=0.5, activation="relu", alpha=None) -> List[Dict]:
     """An identity residual block on the ch-channel map of layer `skip`, which must be the layer right before the block:
-    conv3x3 -> BatchNorm -> act -> conv3x3 -> BatchNorm -> ElementWiseVertex(Add)(., skip) -> act (the convolutions stride 1, pad 1, no bias)."""
+    conv3x3 -> BatchNorm -> act -> conv3x3 -> BatchNorm -> ElementWiseVertex(Add)(., skip) -> act (the convolutions stride 1, pad 1, no bias;
+    activation "prelu": PReLULayers shared over H and W)."""
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
     conv = lambda k: {"type": "conv2d", "name": f"{prefix}_conv_{k}", "n_in": ch, "n_out": ch, "kernel": (3, 3), "stride": (1, 1), "padding": (1, 1),
                       "has_bias": False, "updater": u()}
-    return [conv(1), {"type": "batchnorm", "name": f"{prefix}_bn_1", "updater": u()}, dict({"type": "activation", "name": f"{prefix}_act_1"}, **_act(activation, alpha)),
+    return [conv(1), {"type": "batchnorm", "name": f"{prefix}_bn_1", "updater": u()}, _act_layer(f"{prefix}_act_1", activation, alpha, u),
             conv(2), {"type": "batchnorm", "name": f"{prefix}_bn_2", "updater": u()},
-            elementwise("add", [f"{prefix}_bn_2", skip], name=f"{prefix}_add"), dict({"type": "activation", "name": f"{prefix}_act_2"}, **_act(activation, alpha))]
+            elementwise("add", [f"{prefix}_bn_2", skip], name=f"{prefix}_add"), _act_layer(f"{prefix}_act_2", activation, alpha, u)]
 
 
 def unet(size=64, nc=3, n_classes=2, nf=32, depth=2, loss="mcxent", lr=1e-3, beta1=0.9, activation="relu", alpha=None) -> List[Dict]:
@@ -356,7 +379,8 @@ def _act(activation, alpha=None) -> Dict:
 def dcgan_generator(size=64, z=100, nf=64, nc=3, lr=2e-4, beta1=0.5, activation="relu", out_activation="tanh", alpha=None,
                     residual=False) -> List[Dict]:
     """ConvolutionTranspose2D(4x4)+BatchNorm+ReLU stack, tanh output (SURVEY.md Appendix B).  Input (z,).
-    activation: the ActivationLayers' kind (any engine.ACTS name; alpha as in _act), out_activation: the last deconv's.
+    activation: the ActivationLayers' kind (any engine.ACTS name; alpha as in _act), or "prelu": a PReLULayer shared over H and W in place of
+    each ActivationLayer; out_activation: the last deconv's.
     residual: one identity residual_block after each up-sampling stage (a ResNet-style generator)."""
     u = lambda: adam(lr, beta1, 0.999, 1e-8)
     n_up = int(math.log2(size)) - 2
@@ -364,11 +388,11 @@ def dcgan_generator(size=64, z=100, nf=64, nc=3, lr=2e-4, beta1=0.5, activation=
     block = lambda k, c: residual_block(f"gen_res_{k}", c, f"gen_act_{k}", lr, beta1, activation, alpha) if residual else []
     L = [{"type": "ff_to_cnn", "name": "gen_ff2cnn", "to": (1, 1, z)},
          {"type": "deconv2d", "name": "gen_deconv_1", "n_in": z, "n_out": ch, "kernel": (4, 4), "stride": (1, 1), "padding": (0, 0), "has_bias": False, "updater": u()},
-         {"type": "batchnorm", "name": "gen_bn_1", "updater": u()}, dict({"type": "activation", "name": "gen_act_1"}, **_act(activation, alpha))]
+         {"type": "batchnorm", "name": "gen_bn_1", "updater": u()}, _act_layer("gen_act_1", activation, alpha, u)]
     L += block(1, ch)
     for i in range(n_up - 1):
         L += [{"type": "deconv2d", "name": f"gen_deconv_{i + 2}", "n_in": ch, "n_out": ch // 2, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "has_bias": False, "updater": u()},
-              {"type": "batchnorm", "name": f"gen_bn_{i + 2}", "updater": u()}, dict({"type": "activation", "name": f"gen_act_{i + 2}"}, **_act(activation, alpha))]
+              {"type": "batchnorm", "name": f"gen_bn_{i + 2}", "updater": u()}, _act_layer(f"gen_act_{i + 2}", activation, alpha, u)]
         ch //= 2
         L += block(i + 2, ch)
     L += [{"type": "deconv2d", "name": f"gen_deconv_{n_up + 1}", "n_in": ch, "n_out": nc, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "updater": u(), **_act(out_activation)}]
@@ -388,7 +412,8 @@ def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", o
                         global_pooling=None, patch=False, residual=False, instance_noise=None, drop_connect=None) -> List[Dict]:
     """Conv(4x4 s2 p1)+LeakyReLU(0.2); (Conv+BatchNorm+LeakyReLU)*; Conv(4x4 s1 p0) -> logit; LossLayer(loss).  Input (nc,size,size).
     loss: "xent" (sigmoid implied), or "mse" (least-squares GAN), "hinge", "wasserstein", ... applied to out_activation(logit).
-    activation / alpha: the hidden activation in place of LeakyReLU(0.2) (as in _act).
+    activation / alpha: the hidden activation in place of LeakyReLU(0.2) (as in _act); "prelu": each ActivationLayer becomes a PReLULayer shared
+    over H and W, and the first conv becomes identity followed by such a layer ("dis_act_1").
     global_pooling: a pooling kind ("sum" for the projected / ResNet-style head, "avg", "max", "pnorm"): GlobalPoolingLayer + OutputLayer(nOut 1,
     loss) in place of the last conv and its LossLayer.
     patch: a PatchGAN critic -- the down-sampling stages stop at the max(4, size/16) map (at most four stride-2 convs), and a 3x3 s1 p1 conv onto
@@ -405,12 +430,14 @@ def dcgan_discriminator(size=64, nf=64, nc=3, lr=2e-4, beta1=0.5, loss="xent", o
         n_down = min(n_down, 4)
     block = lambda k, c, skip: residual_block(f"dis_res_{k}", c, skip, lr, beta1, activation, alpha) if residual else []
     L = [] if instance_noise is None else [gaussian_noise(instance_noise, name="dis_instance_noise")]
-    L += [{"type": "conv2d", "name": "dis_conv_1", "n_in": nc, "n_out": nf, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), **_act(activation, alpha), "updater": u()}]
+    p = activation == "prelu"
+    L += [{"type": "conv2d", "name": "dis_conv_1", "n_in": nc, "n_out": nf, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), **({} if p else _act(activation, alpha)), "updater": u()}]
+    L += [_act_layer("dis_act_1", activation, alpha, u)] if p else []
     ch = nf
-    L += block(1, ch, "dis_conv_1")
+    L += block(1, ch, "dis_act_1" if p else "dis_conv_1")
     for i in range(n_down - 1):
         L += [{"type": "conv2d", "name": f"dis_conv_{i + 2}", "n_in": ch, "n_out": ch * 2, "kernel": (4, 4), "stride": (2, 2), "padding": (1, 1), "has_bias": False, "updater": u()},
-              {"type": "batchnorm", "name": f"dis_bn_{i + 2}", "updater": u()}, dict({"type": "activation", "name": f"dis_act_{i + 2}"}, **_act(activation, alpha))]
+              {"type": "batchnorm", "name": f"dis_bn_{i + 2}", "updater": u()}, _act_layer(f"dis_act_{i + 2}", activation, alpha, u)]
         ch *= 2
         L += block(i + 2, ch, f"dis_act_{i + 2}")
     if global_pooling is not None:

@@ -68,8 +68,40 @@ typedef enum {
   B2G_LAYER_GLOBAL_POOLING = 13, /* GlobalPoolingLayer.Builder(PoolingType).pnorm(): b2g_pooling, output [mb, C] (H = W = 1)                 */
   B2G_LAYER_CNN_LOSS = 14,       /* CnnLossLayer.Builder(LossFunction).activation(..): the loss per pixel of a [mb, C, H, W] map; no parameters  */
   B2G_LAYER_ELEMENTWISE = 15,    /* ElementWiseVertex(Op) of the spine and an earlier entry's output: b2g_elementwise_op; no parameters       */
-  B2G_LAYER_MERGE = 16           /* MergeVertex: concatenation of the two inputs along dimension 1 (channels / features); no parameters        */
+  B2G_LAYER_MERGE = 16,          /* MergeVertex: concatenation of the two inputs along dimension 1 (channels / features); no parameters        */
+  B2G_LAYER_PRELU = 17           /* PReLULayer.Builder().inputShape(..).sharedAxes(..): learned negative slopes "W" (alpha), shared-axes mask in act */
 } b2g_layer_type;
+
+/* PReLULayer (DL4J 1.0.0-beta3 org.deeplearning4j.nn.conf.layers.PReLULayer with libnd4j prelu / prelu_bp, recalled; parity unpinned like the
+ * rest of the DL4J semantics).  Output shape = input shape.
+ *   Parameter "W" = alpha, DL4J's weight shape: the input shape [C, H, W] ([F] for a feed-forward input, H = W = 1) with every shared axis of
+ *   extent 1, flattened in 'c' order at the layer's place in the parameter vector, so get_param / set_param / get_params and a checkpoint are
+ *   plain copies.  sharedAxes (DL4J's 1-based axes 1 = C, 2 = H, 3 = W) travel as a bit mask in b2g_layer_desc.act: bit 0 = C (or F), bit 1 = H,
+ *   bit 2 = W; 0 = one slope per element, 6 = sharedAxes(2, 3) = one slope per channel.  inputShape, when given, in pre_c, pre_h, pre_w (a
+ *   feed-forward input: pre_c = F, pre_h = pre_w = 0; all 0 = not given).  A 1 x 1 map is a feed-forward input unless inputShape is [C, 1, 1];
+ *   then it is a [C, 1, 1] map, whose H and W bits are accepted and change nothing.
+ *   B2G_ERR_ARG at b2g_net_create for a mask bit outside the input's rank (bit 0 only on a feed-forward input); B2G_ERR_SHAPE for an inputShape
+ *   other than the inferred input.
+ *   Arithmetic, in fp32 from the stored activations, each result rounded once to the activation type:
+ *     y = x < 0 ? alpha*x : x;    dx = x < 0 ? alpha*dy : dy;    dalpha[k] = sum over the examples and the positions of slope k of (x < 0 ? x*dy : 0)
+ *   x = +-0 is not negative (dy passes, no slope term); NaN passes.  dalpha is summed, not divided by the minibatch (the updater's division is
+ *   the only one, as for W and b).
+ *   Summation order of dalpha, fixed by the shape: a pass of R rows of M = H*W*C elements is cut into G row groups of rpg consecutive rows
+ *   (bx = ceil(M / 2048), G0 = max(1, min(R, 64, 1024 / bx)) with integer division, rpg = ceil(R / G0), G = ceil(R / rpg); G is not monotone
+ *   in R, and the partials of a net are sized for min(max_batch, 64, 1024 / bx) groups, which bounds G for every batch up to max_batch).  The partial of
+ *   group g at row element j is the fp32 sum over the group's rows, ascending, from +0, of the products x*dy (rounded, no fused multiply-add) with
+ *   x < 0.  Element j = (h*W + w)*C + c belongs to slope k = ((c')*aH + h')*aW + w' and position s = ((c")*sH + h")*sW + w" among the S = M / K
+ *   positions sharing it, where a primed coordinate is 0 on a shared axis, a double-primed one 0 on a kept axis, aX = 1 on a shared axis (else X)
+ *   and sX = X on a shared axis (else 1).  dalpha[k] is then the sum over t < G*S of partial[t] (t = g*S + s) as a reduce-list job does it: from
+ *   +0 in ascending t, or, when G*S >= 64 and K <= 65536, as 32 lane sums (lane l takes t = l, l + 32, ... ascending) folded by a butterfly
+ *   (xor 16, 8, 4, 2, 1).
+ *   Launches: one forward and one backward per PReLU layer and pass; a trainable layer's slope gradient is one job of the backward pass's
+ *   reduce-list launch (kernels_ew.cu reduce_multi_kernel), which a pass that queues no other job launches for it alone.  A FrozenLayer (or the
+ *   generator step's pass through D) computes dx only.  Never fused into a BatchNorm or GEMM epilogue.
+ *   Training: alpha takes the layer's updater, learning rate, schedule and gradient normalization like any parameter; l1 / l2 of
+ *   b2g_regularization apply to it (the desc's l2 included; l1_bias / l2_bias have no tensor); it starts at 0 (a new PReLU is a ReLU) and
+ *   b2g_net_init_weights on the named layer takes ZERO, ONES and DISTRIBUTION (the global form leaves it alone).  Not supported (documented
+ *   deviations): constraints and weight noise on alpha -- the named setters return B2G_ERR_ARG. */
 
 /* Spine-plus-skip graphs (DL4J 1.0.0-beta3 ElementWiseVertex / MergeVertex, recalled; parity unpinned like the rest of the DL4J semantics).
  * Entry i of the b2g_layer_desc array takes entry i-1's output as its input (entry 0 the net input): the spine.  ELEMENTWISE and MERGE
@@ -191,8 +223,8 @@ typedef enum { B2G_POOL_MAX = 0, B2G_POOL_AVG = 1, B2G_POOL_SUM = 2, B2G_POOL_PN
  * Codes 0-16 are valid on CONV2D, DECONV2D, DENSE and ACTIVATION layers and on OUTPUT / LOSS layers with loss codes 2-8 (XENT / MCXENT ignore
  * act); any other code there is B2G_ERR_ARG at b2g_net_create.  A GEMM layer with a code of 5-16 keeps its pre-activation z in a buffer of its own
  * and applies f in a separate element-wise kernel; it is never fused into a GEMM or BatchNorm epilogue.
- * Not provided: RRELU (random slopes per element in train mode), SOFTMAX as a hidden activation (implied by MCXENT), and GELU / MISH / PReLU
- * (later DL4J versions). */
+ * Not provided: RRELU (random slopes per element in train mode), SOFTMAX as a hidden activation (implied by MCXENT), GELU / MISH (later DL4J
+ * versions), and PReLU as an activation code (it is a layer with parameters: B2G_LAYER_PRELU). */
 typedef enum {
   B2G_ACT_IDENTITY = 0, B2G_ACT_TANH = 1, B2G_ACT_SIGMOID = 2, B2G_ACT_RELU = 3, B2G_ACT_LRELU = 4,
   B2G_ACT_ELU = 5, B2G_ACT_SELU = 6, B2G_ACT_SOFTPLUS = 7, B2G_ACT_SOFTSIGN = 8, B2G_ACT_HARDTANH = 9, B2G_ACT_HARDSIGMOID = 10,
@@ -514,7 +546,9 @@ typedef struct {
 int32_t b2g_net_set_weight_noise(b2g_net* net, const char* layer, const b2g_weight_noise* wn);
 
 /* Weight initialization (DL4J 1.0.0-beta3 WeightInitUtil.initWeights with Layer.Builder / NeuralNetConfiguration.Builder .weightInit, .dist and
- * .biasInit, recalled; parity unpinned like the rest of the DL4J semantics).  The scheme numbers are DL4J's WeightInit ordinals.  Each scheme
+ * .biasInit, recalled; parity unpinned like the rest of the DL4J semantics).  A named PRELU layer takes ZERO, ONES and DISTRIBUTION for its slopes,
+ * element j = the slope's index in DL4J's order (the other schemes need fans: B2G_ERR_ARG); the global form leaves PReLU layers alone.  The
+ * scheme numbers are DL4J's WeightInit ordinals.  Each scheme
  * draws W from a distribution of the layer's fans:
  *    0 DISTRIBUTION     the b2g_weight_init's own dist(a, b)          11 RELU                  N(0, sqrt(2 / fanIn))
  *    1 ZERO             0                                            12 RELU_UNIFORM          U(+-sqrt(6 / fanIn))
@@ -571,7 +605,8 @@ int32_t b2g_net_init_weights(b2g_net* net, const char* layer, const b2g_weight_i
 
 /* Regularization (DL4J 1.0.0-beta3 Layer.Builder / NeuralNetConfiguration.Builder .l1, .l2, .l1Bias, .l2Bias, resolved per parameter by
  * getL1ByParam / getL2ByParam, recalled; parity unpinned like the rest of the DL4J semantics).
- * Which tensors: on CONV2D, DECONV2D, DENSE and OUTPUT layers l1 and l2 apply to W, l1_bias and l2_bias to b.  BatchNorm parameters are never
+ * Which tensors: on CONV2D, DECONV2D, DENSE and OUTPUT layers l1 and l2 apply to W, l1_bias and l2_bias to b; on PRELU layers l1 and l2 apply to
+ * the slopes W.  BatchNorm parameters are never
  * regularized (beta3's BatchNormalization returns 0 for every parameter).  A FrozenLayer takes no term, in the update or in the score; a layer
  * with lr 0 still decays.
  * Update (UpdaterBlock.postApply): after the updater, with the coefficients as set (no schedule, not lr-scaled; the normalization of
@@ -587,11 +622,11 @@ int32_t b2g_net_init_weights(b2g_net* net, const char* layer, const b2g_weight_i
  * b2g_layer_desc.l2 is the initial l2 of W; every other coefficient starts at 0. */
 typedef struct { float l1, l2, l1_bias, l2_bias; } b2g_regularization;
 /* Layer.Builder.l1 / l2 / l1Bias / l2Bias (layer named) or NeuralNetConfiguration.Builder's (layer NULL: every non-frozen CONV2D, DECONV2D,
- * DENSE and OUTPUT layer).  Replaces all four coefficients of the layer (the desc's l2 too).  Takes effect at the next update, also in a replayed
+ * DENSE, OUTPUT and PRELU layer).  Replaces all four coefficients of the layer (the desc's l2 too).  Takes effect at the next update, also in a replayed
  * CUDA graph of the GAN step (the updater reads the coefficients from device memory).  B2G_ERR_ARG for a value that is not finite and >= 0
  * (DL4J silently ignores a value <= 0: refusing negatives is a deliberate deviation), or a named layer that does not exist or has no W. */
 int32_t b2g_net_set_regularization(b2g_net* net, const char* layer, const b2g_regularization* r);
-/* The four coefficients of a named CONV2D, DECONV2D, DENSE or OUTPUT layer (B2G_ERR_ARG for any other name). */
+/* The four coefficients of a named CONV2D, DECONV2D, DENSE, OUTPUT or PRELU layer (B2G_ERR_ARG for any other name). */
 int32_t b2g_net_get_regularization(b2g_net* net, const char* layer, b2g_regularization* out);
 /* ComputationGraph.calcL1(true) and calcL2(true): L1 and L2 of the score above, now, in double.  Either pointer may be NULL.  Sync point. */
 int32_t b2g_net_calc_regularization(b2g_net* net, double* l1, double* l2);
@@ -783,12 +818,18 @@ int32_t b2g_test_dropout_kind(b2g_ctx* ctx, int32_t precision, int32_t kind, uin
  *   MERGE_BWD      in0 eps [rows][cols + C] T, in1 acc's initial value [rows][C] fp32 (when accumulate)
  *                                                                                     -> out0 the spine's slice [rows][cols] T, out1 acc [rows][C]
  *   SKIP_ADD       in0 eps [n] T, in1 acc [n] fp32                                    -> out0 eps + acc T (in place)
+ * PReLU (B2G_LAYER_PRELU; act = the shared-axes mask, the map N x H x W x C, K = the slope count):
+ *   PRELU_FWD      in0 [x [n] T | alpha [K] fp32]                                     -> out0 y T
+ *   PRELU_BWD      in0 [x [n] T | alpha [K] fp32], in1 dy [n] T                       -> out0 dx T (dy's buffer, in place; NULL: not written),
+ *                                                                                        out1 dalpha [K] (NULL: no slope gradient), summed by
+ *                                                                                        one reduce-list launch
  * Every output buffer not asked for may be NULL. */
 typedef enum {
   B2G_EW_REDUCE_SPLITS = 0, B2G_EW_REDUCE_MULTI = 1, B2G_EW_COLSUM = 2, B2G_EW_XENT = 3, B2G_EW_SOFTMAX_XENT = 4,
   B2G_EW_ACT_FWD = 5, B2G_EW_ACT_BWD = 6, B2G_EW_MAXPOOL = 7, B2G_EW_UPSAMPLE = 8, B2G_EW_SUMSQ = 9, B2G_EW_LOSS = 10,
   B2G_EW_ACT_EXT_FWD = 11, B2G_EW_ACT_EXT_BWD = 12, B2G_EW_CNN_XENT = 13, B2G_EW_CNN_SOFTMAX_XENT = 14,
-  B2G_EW_VERTEX_FWD = 15, B2G_EW_VERTEX_BWD = 16, B2G_EW_MERGE_FWD = 17, B2G_EW_MERGE_BWD = 18, B2G_EW_SKIP_ADD = 19
+  B2G_EW_VERTEX_FWD = 15, B2G_EW_VERTEX_BWD = 16, B2G_EW_MERGE_FWD = 17, B2G_EW_MERGE_BWD = 18, B2G_EW_SKIP_ADD = 19,
+  B2G_EW_PRELU_FWD = 20, B2G_EW_PRELU_BWD = 21
 } b2g_ew_op;
 typedef struct {          /* one split-K sum of a reduce list: dst[i] = sum_s src[s*stride + i], i < n, all offsets in elements of in0 */
   int64_t n, stride, src_off, dst_off;

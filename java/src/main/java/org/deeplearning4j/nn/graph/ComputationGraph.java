@@ -36,11 +36,12 @@ public class ComputationGraph {
             boolean gemm = l.type == 0 || l.type == 1 || l.type == 3 || l.type == 7;
             if (gemm && (global || l.weightInit != null || l.dist != null || l.biasInit != null))
                 initWeights(l.name, l.weightInit != null ? l.weightInit : g.weightInit, l.dist != null ? l.dist : g.dist, l.biasInit != null ? l.biasInit : g.biasInit);
+            if (l.type == 17 && l.weightInit != null) preluSlopeInit(l);      // PReLU: its own weightInit only (ZERO otherwise)
         }
         for (Layer l : layers) {          // l1 / l1Bias / l2Bias, resolved per layer like l2: its own, else the global builder's
-            boolean gemm = l.type == 0 || l.type == 1 || l.type == 3 || l.type == 7;
+            boolean reg = l.type == 0 || l.type == 1 || l.type == 3 || l.type == 7 || l.type == 17;    // PReLU's slopes are a weight
             float l1 = Float.isNaN(l.l1) ? g.l1 : l.l1, l1b = Float.isNaN(l.l1Bias) ? g.l1Bias : l.l1Bias, l2b = Float.isNaN(l.l2Bias) ? g.l2Bias : l.l2Bias;
-            if (gemm && (l1 != 0f || l1b != 0f || l2b != 0f)) setRegularization(l.name, l1, Float.isNaN(l.l2) ? g.l2 : l.l2, l1b, l2b);
+            if (reg && (l1 != 0f || l1b != 0f || l2b != 0f)) setRegularization(l.name, l1, Float.isNaN(l.l2) ? g.l2 : l.l2, l1b, l2b);
         }
         GradientNormalization gn = conf.b.g.gradNorm;      // RenormalizeL2* / ClipL2*: on-device norms before every update
         if (gn.isL2()) Native.check(Native.netSetGradientNormalization(net, gn.ordinal(), conf.b.g.gradNormThreshold));
@@ -98,7 +99,7 @@ public class ComputationGraph {
     public void applyConstraints(int iteration, int epoch) { Native.check(Native.netApplyConstraints(net)); }
     /** The library's rule (include/b200gan.h, b2g_net_set_lr_schedule): parameters, not frozen, updater neither NoOp nor AdaDelta. */
     private static boolean hasLearningRate(Layer l) {
-        boolean params = l.type == 0 || l.type == 1 || l.type == 2 || l.type == 3 || l.type == 7;    // conv, deconv, BatchNorm, dense, output
+        boolean params = l.type == 0 || l.type == 1 || l.type == 2 || l.type == 3 || l.type == 7 || l.type == 17;    // conv, deconv, BatchNorm, dense, output, PReLU
         return params && l.frozen == 0 && l.updater.kind() != 3 && l.updater.kind() != 9;
     }
 
@@ -149,6 +150,8 @@ public class ComputationGraph {
         Native.check(Native.netSetWeightNoise(net, name == null ? 0 : Native.address(name), b == null ? 0 : Native.address(b)));
         java.lang.ref.Reference.reachabilityFence(b); java.lang.ref.Reference.reachabilityFence(sb); java.lang.ref.Reference.reachabilityFence(name);
     }
+    /** A PReLULayer's weightInit(ZERO / ONES / DISTRIBUTION) with its dist: the slopes redrawn at init(); the global builder's is not inherited. */
+    private void preluSlopeInit(Layer l) { initWeights(l.name, l.weightInit, l.dist, null); }
     /** WeightInitUtil.initWeights at init(): redraws W and sets b on one layer (layerName null: every conv, deconv, dense and output layer).
      *  w null is DL4J's default XAVIER, biasInit null its 0; DISTRIBUTION draws from d. */
     public void initWeights(String layerName, WeightInit w, Distribution d, Double biasInit) {

@@ -524,6 +524,23 @@ def init_weights_times(ctx, configs):
     return out
 
 
+# ---------------------------------------------------------------- prelu: C2 with activation="prelu" in both nets (PReLULayers shared over H
+# and W in place of the ActivationLayers, D's first conv identity + PReLU) against plain C2
+def prelu_model(cfg, G, D, n):
+    """Algorithmic bytes of the PReLU kernels per step, bf16: the forward reads x and writes y (4 B / element); the backward reads x and dy and
+    writes dx (6 B / element), and in a trainable pass also its fp32 slope partials (4 B per row group and row element; the reduce-list job
+    that folds them is not counted).  G runs its layers forward on z_d and z_g (N rows each) and backward on N; D forward on real|fake (2N)
+    and on G's output (N), backward on both.  The fp32 slopes (one per channel) are left out."""
+    def elems(net):
+        return [net.layer_output_size(i) for i, s in enumerate(net.specs) if s["type"] == "prelu"]
+    def parts(net, rows):
+        return sum(4 * engine.prelu_groups(rows, e) * e for e in elems(net))
+    g, d = sum(elems(G)), sum(elems(D))
+    return {"prelu_elements_per_row_G": g, "prelu_elements_per_row_D": d,
+            "kernel_bytes_per_step": {"prelu_fwd_kernel": 4 * (2 * n * g + 3 * n * d),
+                                      "prelu_bwd_kernel": 6 * (n * g + 3 * n * d) + parts(G, n) + parts(D, 2 * n)}}
+
+
 ACT_EXT = ("act_ext_fwd_kernel", "act_ext_bwd_kernel")
 CONSTRAINT = ("constraint_onepass_kernel", "constraint_norm_kernel", "constraint_scale_kernel")
 # each feature: default configs, steps, rounds; its variants ("only": the configs it runs on; "kernels": the in-step kernels to profile);
@@ -550,6 +567,8 @@ FEATURES = {
     "patchgan": dict(configs="c2,c4", steps=50, variants=[{}, dict(name="patch", d=dict(patch=True))], kernels=cnn_loss_kernels, extras=head_conv),
     "pooling": dict(configs="c2", variants=[dict(name="base"), dict(name="sum", d=dict(global_pooling="sum")),
                                             dict(name="avg", d=dict(global_pooling="avg"))], kernels=pooling_kernels),
+    "prelu": dict(configs="c2", variants=[{}, dict(name="prelu", g=dict(activation="prelu"), d=dict(activation="prelu"),
+                                                   kernels=("prelu_fwd_kernel", "prelu_bwd_kernel", "reduce_multi_kernel"), model=prelu_model)]),
     "regularization": dict(configs="c5,c2", variants=[
         dict(name="l2", hook=regularize(l2=1e-4), kernels=UPDATER, model=params_model),
         dict(name="l1+l2+l1bias+l2bias", hook=regularize(l1=1e-4, l2=1e-4, l1_bias=1e-4, l2_bias=1e-4), kernels=UPDATER, model=params_model)]),
