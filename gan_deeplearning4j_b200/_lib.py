@@ -101,6 +101,12 @@ class TestPoolOpts(C.Structure):
                 ("kernel", C.c_char * 64), ("splits", C.c_int32)]
 
 
+class TestLossOpts(C.Structure):
+    """b2g_test_loss_opts: which weighted / masked loss kernel to run, its sizes and options, and what ran."""
+    _fields_ = [(k, C.c_int32) for k in ("kernel", "rows", "cols", "groups", "loss", "act")] + [("alpha", C.c_float), ("clip_eps", C.c_float)] + [
+                (k, C.c_int32) for k in ("mask_width", "offset", "poison")] + [("kernel_name", C.c_char * 64)]
+
+
 _vp, _i32, _i64, _fp = C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_float)
 _pvp = C.POINTER(C.c_void_p)
 
@@ -134,6 +140,10 @@ PROTOTYPES = {
     "b2g_net_compute_gradient_and_score": (_i32, [_vp, _fp, _fp, _i32, _fp]),
     "b2g_net_get_input_gradient": (_i32, [_vp, _i32, _fp]),
     "b2g_net_fit": (_i32, [_vp, _fp, _fp, _i32, _fp]),
+    "b2g_net_fit_masked": (_i32, [_vp, _fp, _fp, _i32, _fp, _fp, _i32]),
+    "b2g_net_compute_gradient_and_score_masked": (_i32, [_vp, _fp, _fp, _i32, _fp, _fp, _i32]),
+    "b2g_net_set_loss_weights": (_i32, [_vp, C.c_char_p, _fp, _i32]),
+    "b2g_net_loss_columns": (_i32, [_vp, C.POINTER(C.c_int32)]),
     "b2g_net_get_iteration": (_i32, [_vp, C.POINTER(_i64)]),
     "b2g_net_set_iteration": (_i32, [_vp, _i64]),
     "b2g_net_get_dropout_pass": (_i32, [_vp, C.POINTER(_i64)]),
@@ -158,6 +168,7 @@ PROTOTYPES = {
     "b2g_gan_step": (_i32, [_vp, _fp, _fp, _fp, _fp, _fp, _fp, _i32, _fp]),
     "b2g_gan_upload": (_i32, [_vp, _fp, _fp, _fp, _fp, _fp, _fp, _i32]),
     "b2g_gan_step_resident": (_i32, [_vp, _i32]),
+    "b2g_gan_set_label_masks": (_i32, [_vp, _fp, _fp, _fp, _i32, _i32]),
     "b2g_gan_read_losses": (_i32, [_vp, _fp]),
     "b2g_gan_last_step_ms": (_i32, [_vp, _fp]),
     "b2g_comm_unique_id": (_i32, [_vp]),
@@ -180,6 +191,7 @@ PROTOTYPES = {
     "b2g_test_dropout_kind": (_i32, [_vp, _i32, _i32, C.c_uint64, _i32, _i32, _i64, _i32, _i32, _i32, _i32, C.c_float, _fp, _fp, _fp, _fp]),
     "b2g_test_ew": (_i32, [_vp, _i32, C.POINTER(TestEwOpts), _fp, _fp, _fp, _fp, _fp]),
     "b2g_test_pool": (_i32, [_vp, _i32, C.POINTER(TestPoolOpts), _fp, _fp, _fp, _fp, _fp]),
+    "b2g_test_loss": (_i32, [_vp, _i32, C.POINTER(TestLossOpts), _fp, _fp, _fp, _fp, _fp, _fp]),
 }
 
 _lib = None

@@ -55,6 +55,13 @@ __device__ __forceinline__ double block_sum(double v, double* red) {
   return t;
 }
 
+// The factor of element (label row r, column j) of a weighted / masked loss (LossWM): w_j * m_rj in fp32, 1 for what is absent
+__device__ __forceinline__ float loss_wm_scale(const LossWM& q, size_t r, int j) {
+  float s = q.w ? q.w[j] : 1.0f;
+  if (q.m) s *= q.m[r * q.mw + (q.mw > 1 ? j : 0)];
+  return s;
+}
+
 // Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC'11; the Random123 constants): a counter-based generator,
 // so a mask element's random word is a pure function of (counter, key) and needs no state beyond the counter the caller forms.
 struct Philox4 { uint32_t x[4]; };

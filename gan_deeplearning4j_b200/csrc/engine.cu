@@ -163,6 +163,8 @@ struct b2g_net {
   void* input = nullptr;               // T NHWC [max_rows][in_elems]
   float* stage_f32 = nullptr; size_t stage_floats = 0;   // host<->device fp32 staging (inputs, outputs, params)
   float* labels_dev = nullptr;         // [max_rows]
+  float* mask_dev = nullptr;           // the masked fit's label mask: [max_rows][output size] at most
+  float* loss_w = nullptr; bool loss_w_on = false;   // the loss's per-output weights (b2g_net_set_loss_weights): [loss columns]
   void *epsA = nullptr, *epsB = nullptr, *epsC = nullptr; size_t eps_elems = 0;
   float* scratch2 = nullptr;           // split-K / colsum partials of the side stream
   std::vector<cudaEvent_t> ev_fork, ev_done; cudaEvent_t ev_join = nullptr;
@@ -435,6 +437,8 @@ static int32_t net_alloc(b2g_net* n) {
   B2(dalloc(n, &n->drop_ticket, sizeof(unsigned))); CU(cudaMemsetAsync(n->drop_ticket, 0, sizeof(unsigned), n->ctx->stream));
   B2(dalloc(n, &n->step_dev, sizeof(int))); B2(dalloc(n, &n->loss_dev, sizeof(float) * 8)); B2(dalloc(n, &n->reg_dev, 2 * sizeof(double)));
   B2(dalloc(n, &n->labels_dev, sizeof(float) * R * std::max<size_t>(1, n->L.back().out_elems)));
+  B2(dalloc(n, &n->mask_dev, sizeof(float) * R * std::max<size_t>(1, n->L.back().out_elems)));
+  B2(dalloc(n, &n->loss_w, sizeof(float) * std::max<size_t>(1, n->L.back().out_elems)));
   {  // k_loss's per-block sums for one group of max_batch rows (fit) or two of max_batch / 2 (the GAN step's D pass)
     const size_t per = n->L.back().out_elems;
     // CnnLossLayer: every slicing of kernels_cnnloss.cu and loss_kernel stays within LOSS_MAX_GRID = 1024 blocks
@@ -1274,43 +1278,76 @@ extern "C" int32_t b2g_net_get_activation(b2g_net* n, int32_t layer, int32_t bat
   return download_act(n, l.out, batch, l.oc, l.oh * l.ow, host);
 }
 
+// The columns of the last layer's loss: the channels of a CnnLossLayer (its rows are pixels), else the outputs per example
+static int loss_cols(const LayerRT& l) { return l.d.type == B2G_LAYER_CNN_LOSS ? l.oc : (int)std::max<size_t>(1, l.out_elems); }
+static bool is_loss_layer(const LayerRT& l) { return l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS || l.d.type == B2G_LAYER_CNN_LOSS; }
+
 // The loss of the net's last layer (b2g_loss) on its logits, one launch: dz = dL/dz, loss_sums[g] = the summed scores of group g's rows.  The only
 // place that dispatches on the loss: fit, computeGradientAndScore and both losses of the GAN step come here.  A net that does not end in an
-// OUTPUT or LOSS layer runs XENT.
-static void net_loss(b2g_net* n, const void* logits, const float* labels, void* dz, float* loss_sums, int rows_per_group, int groups) {
+// OUTPUT or LOSS layer runs XENT.  mask: [rows][mask_width] in the labels' rows (null: none); with neither a mask nor the net's loss weights the
+// unweighted instantiations run, else their weighted / masked ones (the same launches).
+static void net_loss(b2g_net* n, const void* logits, const float* labels, void* dz, float* loss_sums, int rows_per_group, int groups,
+                     const float* mask = nullptr, int mask_width = 0) {
   const LayerRT& l = n->L.back();
+  const bool wm = n->loss_w_on || mask;
+  const LossWM q{n->loss_w_on ? n->loss_w : nullptr, mask, mask_width, loss_cols(l)};
   if (l.d.type == B2G_LAYER_CNN_LOSS) {      // rows = the group's pixels, columns = the channels
     const int px = rows_per_group * l.oh * l.ow; cudaStream_t s = n->ctx->stream;
-    if (l.d.loss == B2G_LOSS_XENT) k_cnn_xent(n->prec, logits, labels, dz, loss_sums, (size_t)rows_per_group * l.out_elems, groups, n->cfg.xent_clip_eps, n->loss_partial, n->loss_ticket, s);
-    else if (l.d.loss == B2G_LOSS_MCXENT) k_cnn_softmax_xent(n->prec, logits, labels, dz, nullptr, loss_sums, px, l.oc, groups, n->loss_partial, n->loss_ticket, s);
+    if (l.d.loss == B2G_LOSS_XENT) {
+      if (wm) k_cnn_xent_wm(n->prec, logits, labels, dz, loss_sums, (size_t)rows_per_group * l.out_elems, groups, n->cfg.xent_clip_eps, n->loss_partial, n->loss_ticket, q, s);
+      else k_cnn_xent(n->prec, logits, labels, dz, loss_sums, (size_t)rows_per_group * l.out_elems, groups, n->cfg.xent_clip_eps, n->loss_partial, n->loss_ticket, s);
+    }
+    else if (l.d.loss == B2G_LOSS_MCXENT) {
+      if (wm) k_cnn_softmax_xent_wm(n->prec, logits, labels, dz, loss_sums, px, l.oc, groups, n->loss_partial, n->loss_ticket, q, s);
+      else k_cnn_softmax_xent(n->prec, logits, labels, dz, nullptr, loss_sums, px, l.oc, groups, n->loss_partial, n->loss_ticket, s);
+    }
     else if (l.ext_act) {
       const size_t cnt = (size_t)rows_per_group * groups * l.out_elems;
       k_act_ext_fwd(n->prec, l.ext_act, l.ext_alpha, logits, l.probs, cnt, s);
-      k_loss(n->prec, l.d.loss, ACT_IDENTITY, 0.f, l.probs, labels, dz, loss_sums, px, l.oc, groups, n->loss_partial, n->loss_ticket, s);
+      if (wm) k_loss_wm(n->prec, l.d.loss, ACT_IDENTITY, 0.f, l.probs, labels, dz, loss_sums, px, l.oc, groups, n->loss_partial, n->loss_ticket, q, s);
+      else k_loss(n->prec, l.d.loss, ACT_IDENTITY, 0.f, l.probs, labels, dz, loss_sums, px, l.oc, groups, n->loss_partial, n->loss_ticket, s);
       k_act_ext_bwd(n->prec, l.ext_act, l.ext_alpha, logits, dz, cnt, s);
     }
+    else if (wm) k_loss_wm(n->prec, l.d.loss, l.loss_act, l.loss_alpha, logits, labels, dz, loss_sums, px, l.oc, groups, n->loss_partial, n->loss_ticket, q, s);
     else k_loss(n->prec, l.d.loss, l.loss_act, l.loss_alpha, logits, labels, dz, loss_sums, px, l.oc, groups, n->loss_partial, n->loss_ticket, s);
     return;
   }
   const int loss = (l.d.type == B2G_LAYER_OUTPUT || l.d.type == B2G_LAYER_LOSS) ? l.d.loss : B2G_LOSS_XENT;
-  if (loss == B2G_LOSS_MCXENT) k_softmax_xent(n->prec, logits, labels, dz, nullptr, loss_sums, rows_per_group * groups, l.oc, n->ctx->stream);
-  else if (loss == B2G_LOSS_XENT) k_xent(n->prec, logits, labels, dz, loss_sums, rows_per_group, groups, n->cfg.xent_clip_eps, n->ctx->stream);
+  cudaStream_t s = n->ctx->stream;
+  if (loss == B2G_LOSS_MCXENT) {
+    if (wm) k_softmax_xent_wm(n->prec, logits, labels, dz, loss_sums, rows_per_group * groups, l.oc, q, s);
+    else k_softmax_xent(n->prec, logits, labels, dz, nullptr, loss_sums, rows_per_group * groups, l.oc, s);
+  }
+  else if (loss == B2G_LOSS_XENT) {
+    if (wm) k_xent_wm(n->prec, logits, labels, dz, loss_sums, rows_per_group, groups, n->cfg.xent_clip_eps, q, s);
+    else k_xent(n->prec, logits, labels, dz, loss_sums, rows_per_group, groups, n->cfg.xent_clip_eps, s);
+  }
   else if (l.ext_act) {      // activation of codes 5-16: a = f(z) into probs, the loss on a with the identity, then dL/dz = dL/da * f'(z)
     const size_t cnt = (size_t)rows_per_group * groups * l.out_elems;
-    k_act_ext_fwd(n->prec, l.ext_act, l.ext_alpha, logits, l.probs, cnt, n->ctx->stream);
-    k_loss(n->prec, loss, ACT_IDENTITY, 0.f, l.probs, labels, dz, loss_sums, rows_per_group, (int)l.out_elems, groups, n->loss_partial, n->loss_ticket, n->ctx->stream);
-    k_act_ext_bwd(n->prec, l.ext_act, l.ext_alpha, logits, dz, cnt, n->ctx->stream);
+    k_act_ext_fwd(n->prec, l.ext_act, l.ext_alpha, logits, l.probs, cnt, s);
+    if (wm) k_loss_wm(n->prec, loss, ACT_IDENTITY, 0.f, l.probs, labels, dz, loss_sums, rows_per_group, (int)l.out_elems, groups, n->loss_partial, n->loss_ticket, q, s);
+    else k_loss(n->prec, loss, ACT_IDENTITY, 0.f, l.probs, labels, dz, loss_sums, rows_per_group, (int)l.out_elems, groups, n->loss_partial, n->loss_ticket, s);
+    k_act_ext_bwd(n->prec, l.ext_act, l.ext_alpha, logits, dz, cnt, s);
   }
-  else k_loss(n->prec, loss, l.loss_act, l.loss_alpha, logits, labels, dz, loss_sums, rows_per_group, (int)l.out_elems, groups, n->loss_partial, n->loss_ticket, n->ctx->stream);
+  else if (wm) k_loss_wm(n->prec, loss, l.loss_act, l.loss_alpha, logits, labels, dz, loss_sums, rows_per_group, (int)l.out_elems, groups, n->loss_partial, n->loss_ticket, q, s);
+  else k_loss(n->prec, loss, l.loss_act, l.loss_alpha, logits, labels, dz, loss_sums, rows_per_group, (int)l.out_elems, groups, n->loss_partial, n->loss_ticket, s);
 }
-// host labels [batch][out_elems] -> dst on s.  A CnnLossLayer's labels are NCHW: permuted to the engine's NHWC through `stage` when C > 1 and
-// the map is wider than one pixel (otherwise the two orders coincide).
-static int32_t upload_labels(b2g_net* n, const float* y, int batch, float* dst, float* stage, cudaStream_t s) {
-  const LayerRT& l = n->L.back(); const size_t cnt = (size_t)batch * l.out_elems;
-  if (l.d.type == B2G_LAYER_CNN_LOSS && l.oc > 1 && l.oh * l.ow > 1) {
+// A label mask of width mask_width for the net's loss (b2g_loss): 1 (per example / pixel) or the loss columns (per output)
+static int32_t check_loss_mask(const b2g_net* n, int mask_width) {
+  const LayerRT& l = n->L.back(); const int cols = loss_cols(l);
+  if (mask_width != 1 && mask_width != cols) return fail(B2G_ERR_SHAPE, "label mask width %d: 1 or %d", mask_width, cols);
+  if (mask_width > 1 && is_loss_layer(l) && l.d.loss == B2G_LOSS_MCXENT) return fail(B2G_ERR_UNSUPPORTED, "per-output masking for MCXENT + softmax is not supported");
+  return 0;
+}
+// host rows [batch][chans x the map] -> dst on s: labels (chans = 0: the loss columns) or a label mask (chans = its width).  A CnnLossLayer's
+// are NCHW: permuted to the engine's NHWC through `stage` when chans > 1 and the map is wider than one pixel (otherwise the orders coincide).
+static int32_t upload_labels(b2g_net* n, const float* y, int batch, float* dst, float* stage, cudaStream_t s, int chans = 0) {
+  const LayerRT& l = n->L.back(); const int cols = loss_cols(l); if (!chans) chans = cols;
+  const size_t cnt = (size_t)batch * (std::max<size_t>(1, l.out_elems) / cols) * chans;
+  if (l.d.type == B2G_LAYER_CNN_LOSS && chans > 1 && l.oh * l.ow > 1) {
     if (cnt > n->stage_floats) return fail(B2G_ERR_SHAPE, "labels larger than staging");
     CU(cudaMemcpyAsync(stage, y, sizeof(float) * cnt, cudaMemcpyHostToDevice, s));
-    k_nchw_f32_to_nhwc(PREC_F32, stage, dst, batch, l.oc, l.oh * l.ow, s);
+    k_nchw_f32_to_nhwc(PREC_F32, stage, dst, batch, chans, l.oh * l.ow, s);
     return 0;
   }
   CU(cudaMemcpyAsync(dst, y, sizeof(float) * cnt, cudaMemcpyHostToDevice, s));
@@ -1325,17 +1362,18 @@ static int32_t net_reg_sums(b2g_net* n, double* l1, double* l2) {
   if (n->n_l1) { k_sumabs_segments(n->params, n->reg_off_dev, n->reg_len_dev, n->reg_l1c_dev, nr, n->reg_dev + 1, s); CU(cudaMemcpyAsync(l1, n->reg_dev + 1, sizeof(double), cudaMemcpyDeviceToHost, s)); }
   return 0;
 }
-static int32_t train_pass(b2g_net* n, const float* x, const float* y, int batch, bool do_update, float* score) {
+static int32_t train_pass(b2g_net* n, const float* x, const float* y, int batch, bool do_update, float* score, const float* mask = nullptr, int mask_width = 0) {
   cudaStream_t s = n->ctx->stream;
   if (batch < 1 || batch > n->max_rows) return fail(B2G_ERR_SHAPE, "batch %d outside [1,%d]", batch, n->max_rows);
   int lt = n->L.back().d.type;
   if (lt != B2G_LAYER_OUTPUT && lt != B2G_LAYER_LOSS && lt != B2G_LAYER_CNN_LOSS) return fail(B2G_ERR_UNSUPPORTED, "fit needs a net ending in OutputLayer/LossLayer/CnnLossLayer");
   B2(upload_input(n, x, batch, n->input));
   B2(upload_labels(n, y, batch, n->labels_dev, n->stage_f32, s));
+  if (mask) { B2(check_loss_mask(n, mask_width)); B2(upload_labels(n, mask, batch, n->mask_dev, n->stage_f32, s, mask_width)); }
   CU(cudaMemsetAsync(n->grads, 0, sizeof(float) * n->n_params, s));
   const void* logits = nullptr; FwdOpts o{batch, 1, true, true, nullptr};
   B2(net_forward(n, n->input, o, &logits));
-  net_loss(n, logits, n->labels_dev, n->epsA, n->loss_dev, batch, 1);
+  net_loss(n, logits, n->labels_dev, n->epsA, n->loss_dev, batch, 1, mask ? n->mask_dev : nullptr, mask_width);
   B2(net_backward(n, n->input, n->epsA, batch, 1, true, false, /*allreduce_follows=*/do_update && !score));
   if (score) {
     double l2 = 0.0, l1 = 0.0; float ls = 0.f;
@@ -1351,6 +1389,32 @@ extern "C" int32_t b2g_net_compute_gradient_and_score(b2g_net* n, const float* x
 }
 extern "C" int32_t b2g_net_fit(b2g_net* n, const float* x, const float* y, int32_t batch, float* score) {
   if (!n || !x || !y) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device)); B2(train_pass(n, x, y, batch, true, score)); CU(cudaStreamSynchronize(n->ctx->stream)); return 0;
+}
+extern "C" int32_t b2g_net_compute_gradient_and_score_masked(b2g_net* n, const float* x, const float* y, int32_t batch, float* score, const float* mask, int32_t mask_width) {
+  if (!n || !x || !y) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device)); B2(train_pass(n, x, y, batch, false, score, mask, mask_width)); CU(cudaStreamSynchronize(n->ctx->stream)); return 0;
+}
+extern "C" int32_t b2g_net_fit_masked(b2g_net* n, const float* x, const float* y, int32_t batch, float* score, const float* mask, int32_t mask_width) {
+  if (!n || !x || !y) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device)); B2(train_pass(n, x, y, batch, true, score, mask, mask_width)); CU(cudaStreamSynchronize(n->ctx->stream)); return 0;
+}
+extern "C" int32_t b2g_net_loss_columns(b2g_net* n, int32_t* cols) {
+  if (!n || !cols) return fail(B2G_ERR_ARG, "null");
+  *cols = loss_cols(n->L.back()); return 0;
+}
+extern "C" int32_t b2g_net_set_loss_weights(b2g_net* n, const char* layer, const float* w, int32_t count) {
+  if (!n) return fail(B2G_ERR_ARG, "null");
+  const LayerRT& l = n->L.back();
+  if (!w && !layer) { if (n->loss_w_on) { n->loss_w_on = false; ++n->settings_gen; } return 0; }     // clearing: a no-op on any net without weights
+  if (layer && strncmp(l.d.name, layer, B2G_NAME_LEN)) return fail(B2G_ERR_ARG, "layer '%s' is not the net's loss layer", layer);
+  if (!is_loss_layer(l)) return fail(B2G_ERR_ARG, "loss weights need a net ending in OutputLayer / LossLayer / CnnLossLayer");
+  if (!w) { if (n->loss_w_on) { n->loss_w_on = false; ++n->settings_gen; } return 0; }
+  CU(cudaSetDevice(n->ctx->device));
+  if (l.d.loss == B2G_LOSS_HINGE || l.d.loss == B2G_LOSS_SQUARED_HINGE || l.d.loss == B2G_LOSS_WASSERSTEIN)
+    return fail(B2G_ERR_UNSUPPORTED, "loss %d takes no per-output weights", l.d.loss);
+  if (count != loss_cols(l)) return fail(B2G_ERR_SHAPE, "%d loss weights for %d outputs", count, loss_cols(l));
+  for (int j = 0; j < count; ++j) if (!isfinite(w[j])) return fail(B2G_ERR_ARG, "loss weight %d is not finite", j);
+  CU(cudaMemcpyAsync(n->loss_w, w, sizeof(float) * count, cudaMemcpyHostToDevice, n->ctx->stream)); CU(cudaStreamSynchronize(n->ctx->stream));
+  n->loss_w_on = true; ++n->settings_gen;      // a captured step holds which instantiation the loss launches: re-capture
+  return 0;
 }
 extern "C" int32_t b2g_net_get_input_gradient(b2g_net* n, int32_t batch, float* host) {
   if (!n || !host) return fail(B2G_ERR_ARG, "null"); CU(cudaSetDevice(n->ctx->device));
@@ -1368,6 +1432,8 @@ struct b2g_gan {
   float* stage = nullptr; size_t stage_floats = 0;
   cudaGraph_t graph = nullptr, graph1 = nullptr; cudaGraphExec_t exec = nullptr, exec1 = nullptr; int graph_batch = 0; uint64_t graph_launches = 0, graph_simt_g = 0, graph_simt_d = 0;
   uint64_t graph_settings_g = 0, graph_settings_d = 0;   // the nets' updater settings generations the captured graph was made with
+  float *m_d = nullptr, *m_g = nullptr;   // label masks (b2g_gan_set_label_masks): [2N][mw x map] = m_real | m_fake ; [N][mw x map]; allocated once
+  int mask_width = 0, mask_batch = 0, graph_mask_width = 0;   // 0: no masks; graph_mask_width: what the captured graph was made with
   cudaEvent_t ev0 = nullptr, ev1 = nullptr; float last_ms = 0.f; int last_batch = 1; bool nccl_warm = false;
   cudaStream_t copy_stream = nullptr; cudaEvent_t ev_x = nullptr; bool ev1_valid = false;   // x_real's H2D runs under the generator's forward
   std::vector<void*> allocs;
@@ -1406,7 +1472,7 @@ static int32_t gan_step_part2(b2g_gan* g, int N) {
   CU(cudaMemsetAsync(D->grads, 0, sizeof(float) * D->n_params, s));
   const void* logits = nullptr; FwdOpts od{2 * N, 2, true, true, nullptr};
   B2(net_forward(D, D->input, od, &logits));
-  net_loss(D, logits, g->y_d, D->epsA, g->loss_dev, N, 2);
+  net_loss(D, logits, g->y_d, D->epsA, g->loss_dev, N, 2, g->mask_width ? g->m_d : nullptr, g->mask_width);
   B2(net_backward(D, D->input, D->epsA, 2 * N, 2, true, false, /*allreduce_follows=*/true));
   if (under_allreduce) B2(hoisted_g_forward());
   B2(net_allreduce_grads(D));
@@ -1416,7 +1482,7 @@ static int32_t gan_step_part2(b2g_gan* g, int N) {
   // a scheduled DropoutLayer of D reads G's counters here: this pass belongs to the generator's fit (the stacked gan graph counts its own)
   FwdOpts od2{N, 1, true, false, nullptr, G->step_dev, G->epoch_dev};
   B2(net_forward(D, xg, od2, &logits));
-  net_loss(D, logits, g->y_g, D->epsA, g->loss_dev + 2, N, 1);
+  net_loss(D, logits, g->y_g, D->epsA, g->loss_dev + 2, N, 1, g->mask_width ? g->m_g : nullptr, g->mask_width);
   // the generator's output activation (tanh) is differentiated inside D's last input-gradient kernel when that kernel can (EPI_ACTBWD)
   TcEpi ga{}; const LayerRT& gl = G->L.back(); bool ga_done = false;
   const bool ga_can = gl.has_gemm() && gl.d.act != B2G_ACT_IDENTITY && gl.d.type != B2G_LAYER_OUTPUT;
@@ -1494,11 +1560,13 @@ extern "C" int32_t b2g_gan_step_resident(b2g_gan* g, int32_t batch) {
   static int graph_nccl = -1; if (graph_nccl < 0) { const char* e = getenv("B2G_GRAPH_NCCL"); graph_nccl = (e && e[0] == '0') ? 0 : 1; }
   bool use_graph = g->cfg.use_cuda_graph && (!c->comm || (graph_nccl && g->nccl_warm));
   if (c->comm) g->nccl_warm = true;
+  if (g->mask_width && batch != g->mask_batch) return fail(B2G_ERR_SHAPE, "step batch %d, label masks set for %d", batch, g->mask_batch);
   g->last_batch = batch;
   CU(cudaEventRecord(g->ev0, s));
   if (!use_graph) { B2(gan_step_part1(g, batch)); CU(cudaStreamWaitEvent(s, g->ev_x, 0)); B2(gan_step_part2(g, batch)); }
   else {
-    if (!g->exec || g->graph_batch != batch || g->graph_settings_g != g->G->settings_gen || g->graph_settings_d != g->D->settings_gen) {
+    if (!g->exec || g->graph_batch != batch || g->graph_settings_g != g->G->settings_gen || g->graph_settings_d != g->D->settings_gen ||
+        g->graph_mask_width != g->mask_width) {
       if (g->exec) { cudaGraphExecDestroy(g->exec); g->exec = nullptr; } if (g->graph) { cudaGraphDestroy(g->graph); g->graph = nullptr; }
       if (g->exec1) { cudaGraphExecDestroy(g->exec1); g->exec1 = nullptr; } if (g->graph1) { cudaGraphDestroy(g->graph1); g->graph1 = nullptr; }
       uint64_t before = g_launch_count; const uint64_t sg0 = g->G->simt_gemm_calls, sd0 = g->D->simt_gemm_calls;
@@ -1513,13 +1581,37 @@ extern "C" int32_t b2g_gan_step_resident(b2g_gan* g, int32_t batch) {
       g->graph_simt_g = g->G->simt_gemm_calls - sg0; g->graph_simt_d = g->D->simt_gemm_calls - sd0; g->G->simt_gemm_calls = sg0; g->D->simt_gemm_calls = sd0;
       if (r) return r; if (e != cudaSuccess) return fail(B2G_ERR_CUDA, "graph capture: %s", cudaGetErrorString(e));
       CU(cudaGraphInstantiate(&g->exec1, g->graph1, 0)); CU(cudaGraphInstantiate(&g->exec, g->graph, 0)); g->graph_batch = batch;
-      g->graph_settings_g = g->G->settings_gen; g->graph_settings_d = g->D->settings_gen;
+      g->graph_settings_g = g->G->settings_gen; g->graph_settings_d = g->D->settings_gen; g->graph_mask_width = g->mask_width;
     }
     CU(cudaGraphLaunch(g->exec1, s));
     CU(cudaStreamWaitEvent(s, g->ev_x, 0));
     CU(cudaGraphLaunch(g->exec, s)); g_launch_count += g->graph_launches; g->G->simt_gemm_calls += g->graph_simt_g; g->D->simt_gemm_calls += g->graph_simt_d;
   }
   CU(cudaEventRecord(g->ev1, s)); g->ev1_valid = true;
+  return 0;
+}
+extern "C" int32_t b2g_gan_set_label_masks(b2g_gan* g, const float* m_real, const float* m_fake, const float* m_gen, int32_t mask_width, int32_t batch) {
+  if (!g) return fail(B2G_ERR_ARG, "null");
+  if (!m_real && !m_fake && !m_gen) { g->mask_width = 0; g->mask_batch = 0; return 0; }
+  if (!m_real || !m_fake || !m_gen) return fail(B2G_ERR_ARG, "label masks: all three or none");
+  if (batch < 1 || batch > g->N) return fail(B2G_ERR_SHAPE, "batch %d outside [1,%d]", batch, g->N);
+  b2g_net* D = g->D; cudaStream_t s = g->G->ctx->stream; CU(cudaSetDevice(D->ctx->device));
+  B2(check_loss_mask(D, mask_width));
+  const size_t oe = D->L.back().out_elems;
+  if (!g->m_d) {
+    for (float** p : {&g->m_d, &g->m_g}) {
+      cudaError_t e = cudaMalloc((void**)p, sizeof(float) * (p == &g->m_d ? 2 : 1) * g->N * std::max<size_t>(1, oe));
+      if (e != cudaSuccess) return fail(B2G_ERR_OOM, "cudaMalloc: %s", cudaGetErrorString(e));
+      g->allocs.push_back(*p);
+    }
+  }
+  // the previous step may still read the masks (and D's staging buffer): the copies wait for it on the step's stream
+  const size_t per = (size_t)batch * (std::max<size_t>(1, oe) / loss_cols(D->L.back())) * mask_width;
+  B2(upload_labels(D, m_real, batch, g->m_d, D->stage_f32, s, mask_width));
+  B2(upload_labels(D, m_fake, batch, g->m_d + per, D->stage_f32, s, mask_width));
+  B2(upload_labels(D, m_gen, batch, g->m_g, D->stage_f32, s, mask_width));
+  CU(cudaStreamSynchronize(s));
+  g->mask_width = mask_width; g->mask_batch = batch;
   return 0;
 }
 extern "C" int32_t b2g_gan_read_losses(b2g_gan* g, float* losses) {
@@ -2739,6 +2831,42 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
 }
 extern "C" int32_t b2g_test_ew(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, const float* in0, const float* in1, float* out0, float* out1, float* out2) {
   return test_ew_impl(c, precision, o, nullptr, in0, in1, out0, out1, out2);
+}
+extern "C" int32_t b2g_test_loss(b2g_ctx* c, int32_t precision, b2g_test_loss_opts* o, const float* zh, const float* yh, const float* wh, const float* mh,
+                                  float* dzh, float* lossh) {
+  if (!c || !o || !zh || !yh) return fail(B2G_ERR_ARG, "null");
+  const int prec = precision == B2G_PREC_BF16 ? PREC_BF16 : PREC_F32; const size_t ts = prec_size(prec);
+  const int off = o->offset, k = o->kernel;
+  if (off < 0 || off > 64) return fail(B2G_ERR_ARG, "offset %d outside [0, 64]", off);
+  if (k < B2G_TEST_LOSS_XENT || k > B2G_TEST_LOSS_CNN_SOFTMAX_XENT || o->rows < 1 || o->cols < 1 || o->groups < 1 ||
+      (k == B2G_TEST_LOSS_XENT && o->cols != 1) || (k == B2G_TEST_LOSS_SOFTMAX_XENT && o->groups != 1) ||
+      (int64_t)o->rows * o->cols * o->groups > 0x7fffffff) return fail(B2G_ERR_ARG, "bad loss test arguments");
+  if (k == B2G_TEST_LOSS_CODES && (o->loss < B2G_LOSS_MSE || o->loss > B2G_LOSS_WASSERSTEIN || o->act < B2G_ACT_IDENTITY || o->act > B2G_ACT_LRELU))
+    return fail(B2G_ERR_ARG, "bad loss / activation");
+  if (mh && o->mask_width != 1 && o->mask_width != o->cols) return fail(B2G_ERR_SHAPE, "mask width %d: 1 or %d", o->mask_width, o->cols);
+  CU(cudaSetDevice(c->device)); cudaStream_t s = c->stream;
+  HookMem m(s, prec);
+  const size_t per = (size_t)o->rows * o->cols, n = per * o->groups, rows = (size_t)o->rows * o->groups;
+  void *z = nullptr, *dz = nullptr; float *y = nullptr, *w = nullptr, *mk = nullptr, *loss = nullptr; double* partial = nullptr; unsigned* ticket = nullptr;
+  B2(m.upT(zh, n, &z, off)); B2(m.upF(yh, n, &y, off)); B2(m.dev(n, ts, &dz, off)); B2(m.upF(nullptr, (size_t)o->groups, &loss, off));
+  if (wh) B2(m.upF(wh, (size_t)o->cols, &w, off));
+  if (mh) B2(m.upF(mh, rows * o->mask_width, &mk, off));
+  B2(m.dev((size_t)1024 + (size_t)o->groups, 8, (void**)&partial, off)); B2(m.dev(1, 4, (void**)&ticket, off)); CU(cudaMemsetAsync(ticket, 0, 4, s));
+  if (o->poison) { CU(cudaMemsetAsync(dz, 0xFF, ts * n, s)); CU(cudaMemsetAsync(loss, 0xFF, 4 * (size_t)o->groups, s)); }
+  const LossWM q{w, mk, mh ? o->mask_width : 0, o->cols};
+  g_ew_last_kernel = "";
+  switch (k) {
+    case B2G_TEST_LOSS_XENT: k_xent_wm(prec, z, y, dz, loss, o->rows, o->groups, o->clip_eps, q, s); break;
+    case B2G_TEST_LOSS_SOFTMAX_XENT: k_softmax_xent_wm(prec, z, y, dz, loss, o->rows, o->cols, q, s); break;
+    case B2G_TEST_LOSS_CODES: k_loss_wm(prec, o->loss, o->act, o->alpha, z, y, dz, loss, o->rows, o->cols, o->groups, partial, ticket, q, s); break;
+    case B2G_TEST_LOSS_CNN_XENT: k_cnn_xent_wm(prec, z, y, dz, loss, per, o->groups, o->clip_eps, partial, ticket, q, s); break;
+    default: k_cnn_softmax_xent_wm(prec, z, y, dz, loss, o->rows, o->cols, o->groups, partial, ticket, q, s); break;
+  }
+  snprintf(o->kernel_name, sizeof(o->kernel_name), "%s", g_ew_last_kernel); g_ew_last_kernel = "";
+  B2(m.downT(dzh, dz, n)); B2(m.downF(lossh, loss, (size_t)o->groups));
+  unsigned t = 1; CU(cudaMemcpyAsync(&t, ticket, 4, cudaMemcpyDeviceToHost, s)); CU(cudaStreamSynchronize(s));
+  if (t != 0) return fail(B2G_ERR_CUDA, "loss test: the kernel left its ticket word at %u", t);
+  return 0;
 }
 extern "C" int32_t b2g_test_pool(b2g_ctx* c, int32_t precision, b2g_test_pool_opts* po, const float* in0, const float* in1, float* out0, float* out1, float* out2) {
   if (!c || !po) return fail(B2G_ERR_ARG, "null");

@@ -184,6 +184,19 @@ void k_cnn_xent(int prec, const void* z, const float* y, void* dz, float* loss_s
 int k_cnn_softmax_blocks(int rows_per_group, int groups);
 void k_cnn_softmax_xent(int prec, const void* z, const float* y, void* dz, void* p_out, float* loss_sums, int rows_per_group, int C, int groups,
                         double* partial, unsigned* ticket, cudaStream_t s);
+// Per-output weights and label mask of a loss (b2g_net_set_loss_weights / the masked fit; semantics at b2g_loss).  w: [C] or null; m: the
+// mask, [rows][mw] in the rows of the labels (examples, or NHWC pixels of a CnnLossLayer) with mw = 1 or C, or null; C: the columns (nOut,
+// or the channels of a CnnLossLayer).  A wrapper given null (or a LossWM with neither) launches its unweighted instantiation.
+struct LossWM { const float* w; const float* m; int mw; int C; };
+// The weighted / masked instantiations of the five loss kernels: the same launch, slicing and summation order as the wrappers above.
+void k_xent_wm(int prec, const void* z, const float* y, void* dz, float* loss_sums, int rows_per_group, int groups, float clip_eps, const LossWM& wm, cudaStream_t s);
+void k_softmax_xent_wm(int prec, const void* z, const float* y, void* dz, float* loss_sums, int rows, int K, const LossWM& wm, cudaStream_t s);
+void k_loss_wm(int prec, int loss, int act, float alpha, const void* z, const float* y, void* dz, float* loss_sums, int rows_per_group, int n_out, int groups,
+               double* partial, unsigned* ticket, const LossWM& wm, cudaStream_t s);
+void k_cnn_xent_wm(int prec, const void* z, const float* y, void* dz, float* loss_sums, size_t n_per_group, int groups, float clip_eps, double* partial,
+                   unsigned* ticket, const LossWM& wm, cudaStream_t s);
+void k_cnn_softmax_xent_wm(int prec, const void* z, const float* y, void* dz, float* loss_sums, int rows_per_group, int C, int groups,
+                           double* partial, unsigned* ticket, const LossWM& wm, cudaStream_t s);
 
 // ---- skip-connection vertices (kernels_graph.cu; semantics at b2g_elementwise_op in include/b200gan.h) ----------------------------
 // One launch each.  a, b: the vertex's inputs in its input order.  The fp32 accumulator acc of a skip source is written (accumulate = 0, the

@@ -72,9 +72,12 @@ template <> struct Vec<__nv_bfloat16> {
 // (k = 0, 1, ...) of V = 16 / sizeof(T) elements each, [jV, jV + V) clipped to n; its double sum adds the elements' fp32 scores in element
 // order, chunk after chunk.  VEC: 16-byte loads and stores of the full chunks (z, y, dz aligned and every group starting aligned); a partial
 // chunk, and every chunk of the scalar instantiation, goes element by element in the same order -- the bits do not depend on the path.
-template <typename T, bool VEC>
+// WM: element e (of the whole launch) is scaled by sc = loss_wm_scale(wm, e / C, e % C): its score enters as (double)score * (double)sc and its
+// dz is grad * sc, in the same order.
+template <typename T, bool VEC, bool WM>
 __global__ void __launch_bounds__(CL_THREADS) cnn_xent_kernel(const T* __restrict__ z, const float* __restrict__ y, T* __restrict__ dz,
-                                                              float* __restrict__ loss_sums, size_t n, int bpg, float clip, double* partial, unsigned* ticket) {
+                                                              float* __restrict__ loss_sums, size_t n, int bpg, float clip, double* partial, unsigned* ticket,
+                                                              LossWM wm) {
   pdl_enter();
   __shared__ double red[CL_THREADS / 32];
   constexpr int V = Vec<T>::V;
@@ -89,11 +92,20 @@ __global__ void __launch_bounds__(CL_THREADS) cnn_xent_kernel(const T* __restric
 #pragma unroll
       for (int k = 0; k < V; k += 4) { const float4 q = *reinterpret_cast<const float4*>(y + base + e0 + k); yv[k] = q.x; yv[k + 1] = q.y; yv[k + 2] = q.z; yv[k + 3] = q.w; }
 #pragma unroll
-      for (int k = 0; k < V; ++k) acc += (double)xent_elem(zv[k], yv[k], clip, &gv[k]);
+      for (int k = 0; k < V; ++k) {
+        const float l = xent_elem(zv[k], yv[k], clip, &gv[k]);
+        if (WM) { const size_t e = base + e0 + k; const float sc = loss_wm_scale(wm, e / wm.C, (int)(e % wm.C)); acc += __dmul_rn((double)l, (double)sc); gv[k] *= sc; }
+        else acc += (double)l;
+      }
       Vec<T>::store(dz + base + e0, gv);
     } else {
       const size_t e1 = e0 + V < n ? e0 + V : n;
-      for (size_t e = e0; e < e1; ++e) { float gr; acc += (double)xent_elem(ldf(z, base + e), y[base + e], clip, &gr); stf(dz, base + e, gr); }
+      for (size_t e = e0; e < e1; ++e) {
+        float gr; const float l = xent_elem(ldf(z, base + e), y[base + e], clip, &gr);
+        if (WM) { const float sc = loss_wm_scale(wm, (base + e) / wm.C, (int)((base + e) % wm.C)); acc += __dmul_rn((double)l, (double)sc); gr *= sc; }
+        else acc += (double)l;
+        stf(dz, base + e, gr);
+      }
     }
   }
   const double tot = block_sum(acc, red);
@@ -103,10 +115,12 @@ __global__ void __launch_bounds__(CL_THREADS) cnn_xent_kernel(const T* __restric
 // Softmax MCXENT per pixel: z, y, dz, p_out [groups][rows][C] (NHWC pixels).  One thread per pixel, thread t of block b of group g taking
 // the pixels r = b*256 + t + k*bpg*256 of its group: m = max over c in channel order; den = sum over c of expf(z - m) in fp32, channel order;
 // p_c = expf(z_c - m) / den; dz_c = p_c - y_c; the thread's double sum subtracts y_c * log((double)clamp(p_c, 1e-10, 1 - 1e-10)) channel after
-// channel, pixel after pixel.  Without labels (y = null) it writes p_out only and sums nothing.
-template <typename T>
+// channel, pixel after pixel.  Without labels (y = null) it writes p_out only and sums nothing.  WM (labels given, a mask per pixel): the
+// weighted softmax gradient of kernels_ew.cu softmax_xent_kernel, m_r the mask of pixel g*rows + r.
+template <typename T, bool WM>
 __global__ void __launch_bounds__(CL_THREADS) cnn_softmax_xent_kernel(const T* __restrict__ z, const float* __restrict__ y, T* __restrict__ dz, T* __restrict__ p_out,
-                                                                      float* __restrict__ loss_sums, int rows, int C, int bpg, double* partial, unsigned* ticket) {
+                                                                      float* __restrict__ loss_sums, int rows, int C, int bpg, double* partial, unsigned* ticket,
+                                                                      LossWM wm) {
   pdl_enter();
   __shared__ double red[CL_THREADS / 32];
   const int g = blockIdx.x / bpg, b = blockIdx.x % bpg;
@@ -115,10 +129,19 @@ __global__ void __launch_bounds__(CL_THREADS) cnn_softmax_xent_kernel(const T* _
     const size_t i0 = ((size_t)g * rows + r) * C;
     float m = -INFINITY; for (int c = 0; c < C; ++c) m = fmaxf(m, ldf(z, i0 + c));
     float den = 0.f; for (int c = 0; c < C; ++c) den += expf(ldf(z, i0 + c) - m);
+    float sy = 0.f, mr = 1.f;
+    if (WM) {
+      if (wm.w) for (int c = 0; c < C; ++c) sy += __fmul_rn(wm.w[c], y[i0 + c]);
+      if (wm.m) mr = wm.m[(size_t)g * rows + r];
+    }
     for (int c = 0; c < C; ++c) {
       const float p = expf(ldf(z, i0 + c) - m) / den;
       if (p_out) stf(p_out, i0 + c, p);
-      if (y) { const float yc = y[i0 + c]; stf(dz, i0 + c, p - yc); acc -= (double)yc * log((double)fminf(fmaxf(p, 1e-10f), 1.0f - 1e-10f)); }
+      if (WM) {
+        const float yc = y[i0 + c], wy = wm.w ? wm.w[c] * yc : yc;
+        stf(dz, i0 + c, mr * (wm.w ? __fmul_rn(p, sy) - wy : p - yc)); acc -= __dmul_rn((double)(mr * wy), log((double)fminf(fmaxf(p, 1e-10f), 1.0f - 1e-10f)));
+      }
+      else if (y) { const float yc = y[i0 + c]; stf(dz, i0 + c, p - yc); acc -= (double)yc * log((double)fminf(fmaxf(p, 1e-10f), 1.0f - 1e-10f)); }
     }
   }
   if (!y) return;
@@ -134,8 +157,19 @@ void k_cnn_xent(int prec, const void* z, const float* y, void* dz, float* loss_s
   const int V = prec == PREC_F32 ? 4 : 8;     // elements per 16-byte chunk of z / dz
   const bool vec = (uintptr_t)z % 16 == 0 && (uintptr_t)dz % 16 == 0 && (uintptr_t)y % 16 == 0 && (groups == 1 || n_per_group % V == 0);
   DISPATCH_PREC(prec, T, {
-    if (vec) { launch_pdl(cnn_xent_kernel<T, true>, dim3(groups * bpg), dim3(CL_THREADS), (size_t)0, s, (const T*)z, y, (T*)dz, loss_sums, n_per_group, bpg, clip, partial, ticket); g_ew_last_kernel = "cnn_xent_kernel<vec>"; }
-    else { launch_pdl(cnn_xent_kernel<T, false>, dim3(groups * bpg), dim3(CL_THREADS), (size_t)0, s, (const T*)z, y, (T*)dz, loss_sums, n_per_group, bpg, clip, partial, ticket); g_ew_last_kernel = "cnn_xent_kernel<scalar>"; }
+    if (vec) { launch_pdl(cnn_xent_kernel<T, true, false>, dim3(groups * bpg), dim3(CL_THREADS), (size_t)0, s, (const T*)z, y, (T*)dz, loss_sums, n_per_group, bpg, clip, partial, ticket, LossWM{}); g_ew_last_kernel = "cnn_xent_kernel<vec>"; }
+    else { launch_pdl(cnn_xent_kernel<T, false, false>, dim3(groups * bpg), dim3(CL_THREADS), (size_t)0, s, (const T*)z, y, (T*)dz, loss_sums, n_per_group, bpg, clip, partial, ticket, LossWM{}); g_ew_last_kernel = "cnn_xent_kernel<scalar>"; }
+  });
+  LAUNCHED();
+}
+void k_cnn_xent_wm(int prec, const void* z, const float* y, void* dz, float* loss_sums, size_t n_per_group, int groups, float clip, double* partial, unsigned* ticket,
+                   const LossWM& wm, cudaStream_t s) {
+  const int bpg = k_loss_blocks(n_per_group, groups);
+  const int V = prec == PREC_F32 ? 4 : 8;
+  const bool vec = (uintptr_t)z % 16 == 0 && (uintptr_t)dz % 16 == 0 && (uintptr_t)y % 16 == 0 && (groups == 1 || n_per_group % V == 0);
+  DISPATCH_PREC(prec, T, {
+    if (vec) { launch_pdl(cnn_xent_kernel<T, true, true>, dim3(groups * bpg), dim3(CL_THREADS), (size_t)0, s, (const T*)z, y, (T*)dz, loss_sums, n_per_group, bpg, clip, partial, ticket, wm); g_ew_last_kernel = "cnn_xent_kernel<vec,wm>"; }
+    else { launch_pdl(cnn_xent_kernel<T, false, true>, dim3(groups * bpg), dim3(CL_THREADS), (size_t)0, s, (const T*)z, y, (T*)dz, loss_sums, n_per_group, bpg, clip, partial, ticket, wm); g_ew_last_kernel = "cnn_xent_kernel<scalar,wm>"; }
   });
   LAUNCHED();
 }
@@ -145,10 +179,18 @@ int k_cnn_softmax_blocks(int rows_per_group, int groups) { return k_loss_blocks(
 void k_cnn_softmax_xent(int prec, const void* z, const float* y, void* dz, void* p_out, float* loss_sums, int rows_per_group, int C, int groups, double* partial,
                         unsigned* ticket, cudaStream_t s) {
   const int bpg = k_cnn_softmax_blocks(rows_per_group, groups);
-  DISPATCH_PREC(prec, T, (launch_pdl(cnn_softmax_xent_kernel<T>, dim3(groups * bpg), dim3(CL_THREADS), (size_t)0, s, (const T*)z, y, (T*)dz, (T*)p_out, loss_sums,
-                                     rows_per_group, C, bpg, partial, ticket)));
+  DISPATCH_PREC(prec, T, (launch_pdl(cnn_softmax_xent_kernel<T, false>, dim3(groups * bpg), dim3(CL_THREADS), (size_t)0, s, (const T*)z, y, (T*)dz, (T*)p_out, loss_sums,
+                                     rows_per_group, C, bpg, partial, ticket, LossWM{})));
   LAUNCHED();
   g_ew_last_kernel = "cnn_softmax_xent_kernel";
+}
+void k_cnn_softmax_xent_wm(int prec, const void* z, const float* y, void* dz, float* loss_sums, int rows_per_group, int C, int groups, double* partial,
+                           unsigned* ticket, const LossWM& wm, cudaStream_t s) {
+  const int bpg = k_cnn_softmax_blocks(rows_per_group, groups);
+  DISPATCH_PREC(prec, T, (launch_pdl(cnn_softmax_xent_kernel<T, true>, dim3(groups * bpg), dim3(CL_THREADS), (size_t)0, s, (const T*)z, y, (T*)dz, (T*)nullptr, loss_sums,
+                                     rows_per_group, C, bpg, partial, ticket, wm)));
+  LAUNCHED();
+  g_ew_last_kernel = "cnn_softmax_xent_kernel<wm>";
 }
 
 }  // namespace b2g

@@ -667,9 +667,11 @@ void k_upsample_bwd(int prec, const void* eo, void* ei, int N, int H, int W, int
 }
 
 // ---------------------------------------------------------------- XENT ---------------------------------
-// LossBinaryXENT + sigmoid on the logit (J:159-163): clip_eps>0 DL4J-exact, 0 = BCE-with-logits.
-template <typename T>
-__global__ void xent_kernel(const T* __restrict__ z, const float* __restrict__ y, T* __restrict__ dz, float* __restrict__ loss_sums, int rows, float clip) { pdl_enter();
+// LossBinaryXENT + sigmoid on the logit (J:159-163): clip_eps>0 DL4J-exact, 0 = BCE-with-logits.  WM: row i's score and dz scaled by
+// loss_wm_scale(wm, i, 0) (the score in double: (double)loss * (double)scale), summed in the unweighted order.
+template <typename T, bool WM>
+__global__ void xent_kernel(const T* __restrict__ z, const float* __restrict__ y, T* __restrict__ dz, float* __restrict__ loss_sums, int rows, float clip,
+                            LossWM wm) { pdl_enter();
   int g = blockIdx.x;
   __shared__ double red[32];
   double acc = 0.0;
@@ -685,7 +687,9 @@ __global__ void xent_kernel(const T* __restrict__ z, const float* __restrict__ y
       loss = fmaxf(zi, 0.f) + log1pf(expf(-fabsf(zi))) - yi * zi;
       grad = sg - yi;
     }
-    acc += loss; stf(dz, i, grad);
+    if (WM) { const float sc = loss_wm_scale(wm, i, 0); acc += __dmul_rn((double)loss, (double)sc); grad *= sc; }
+    else acc += loss;
+    stf(dz, i, grad);
   }
   for (int o = 16; o; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
   if (threadIdx.x % 32 == 0) red[threadIdx.x / 32] = acc;
@@ -693,22 +697,38 @@ __global__ void xent_kernel(const T* __restrict__ z, const float* __restrict__ y
   if (threadIdx.x == 0) { double t = 0; for (int w = 0; w < (blockDim.x + 31) / 32; ++w) t += red[w]; loss_sums[g] = (float)t; }
 }
 void k_xent(int prec, const void* z, const float* y, void* dz, float* loss_sums, int rows, int groups, float clip, cudaStream_t s) {
-  DISPATCH_PREC(prec, T, (launch_pdl(xent_kernel<T>, dim3(groups), dim3(1024), (size_t)(0), s, (const T*)z, y, (T*)dz, loss_sums, rows, clip))); LAUNCHED();
+  DISPATCH_PREC(prec, T, (launch_pdl(xent_kernel<T, false>, dim3(groups), dim3(1024), (size_t)(0), s, (const T*)z, y, (T*)dz, loss_sums, rows, clip, LossWM{}))); LAUNCHED();
   g_ew_last_kernel = "xent_kernel";
 }
+void k_xent_wm(int prec, const void* z, const float* y, void* dz, float* loss_sums, int rows, int groups, float clip, const LossWM& wm, cudaStream_t s) {
+  DISPATCH_PREC(prec, T, (launch_pdl(xent_kernel<T, true>, dim3(groups), dim3(1024), (size_t)(0), s, (const T*)z, y, (T*)dz, loss_sums, rows, clip, wm))); LAUNCHED();
+  g_ew_last_kernel = "xent_kernel<wm>";
+}
 
-// LossMCXENT with softmax (J:357-362), K classes per row: one thread per row, block-level loss sum
-template <typename T>
-__global__ void softmax_xent_kernel(const T* __restrict__ z, const float* __restrict__ y, T* __restrict__ dz, T* __restrict__ p_out, float* __restrict__ loss_sum, int rows, int K) { pdl_enter();
+// LossMCXENT with softmax (J:357-362), K classes per row: one thread per row, block-level loss sum.  WM (labels given; mask per row, mw = 1):
+// m_r = the row's mask (1 without one); with weights sy = sum_k w_k y_k in fp32, class order, and dz_k = m_r * (p_k * sy - w_k y_k)
+// (LossMCXENT's weighted gradient), without them dz_k = m_r * (p_k - y_k); the score term is (double)(m_r * w_k y_k) * log(clamp(p_k)).
+template <typename T, bool WM>
+__global__ void softmax_xent_kernel(const T* __restrict__ z, const float* __restrict__ y, T* __restrict__ dz, T* __restrict__ p_out, float* __restrict__ loss_sum, int rows, int K,
+                                    LossWM wm) { pdl_enter();
   __shared__ double red[32];
   double acc = 0.0;
   for (int r = threadIdx.x; r < rows; r += blockDim.x) {
     float m = -INFINITY; for (int k = 0; k < K; ++k) m = fmaxf(m, ldf(z, (size_t)r * K + k));
     float den = 0.f; for (int k = 0; k < K; ++k) den += expf(ldf(z, (size_t)r * K + k) - m);
+    float sy = 0.f, mr = 1.f;
+    if (WM) {
+      if (wm.w) for (int k = 0; k < K; ++k) sy += __fmul_rn(wm.w[k], y[(size_t)r * K + k]);
+      if (wm.m) mr = wm.m[r];
+    }
     for (int k = 0; k < K; ++k) {
       const float p = expf(ldf(z, (size_t)r * K + k) - m) / den;
       if (p_out) stf(p_out, (size_t)r * K + k, p);
-      if (dz) { const float yk = y[(size_t)r * K + k]; stf(dz, (size_t)r * K + k, p - yk); acc -= (double)yk * log((double)fminf(fmaxf(p, 1e-10f), 1.0f - 1e-10f)); }
+      if (WM) {
+        const float yk = y[(size_t)r * K + k], wy = wm.w ? wm.w[k] * yk : yk;
+        stf(dz, (size_t)r * K + k, mr * (wm.w ? __fmul_rn(p, sy) - wy : p - yk)); acc -= __dmul_rn((double)(mr * wy), log((double)fminf(fmaxf(p, 1e-10f), 1.0f - 1e-10f)));
+      }
+      else if (dz) { const float yk = y[(size_t)r * K + k]; stf(dz, (size_t)r * K + k, p - yk); acc -= (double)yk * log((double)fminf(fmaxf(p, 1e-10f), 1.0f - 1e-10f)); }
     }
   }
   for (int o = 16; o; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
@@ -717,8 +737,12 @@ __global__ void softmax_xent_kernel(const T* __restrict__ z, const float* __rest
   if (threadIdx.x == 0 && loss_sum) { double t = 0; for (int w = 0; w < (blockDim.x + 31) / 32; ++w) t += red[w]; loss_sum[0] = (float)t; }
 }
 void k_softmax_xent(int prec, const void* z, const float* y, void* dz, void* p_out, float* loss_sums, int rows, int K, cudaStream_t s) {
-  DISPATCH_PREC(prec, T, (launch_pdl(softmax_xent_kernel<T>, dim3(1), dim3(1024), (size_t)0, s, (const T*)z, y, (T*)dz, (T*)p_out, loss_sums, rows, K))); LAUNCHED();
+  DISPATCH_PREC(prec, T, (launch_pdl(softmax_xent_kernel<T, false>, dim3(1), dim3(1024), (size_t)0, s, (const T*)z, y, (T*)dz, (T*)p_out, loss_sums, rows, K, LossWM{}))); LAUNCHED();
   g_ew_last_kernel = "softmax_xent_kernel";
+}
+void k_softmax_xent_wm(int prec, const void* z, const float* y, void* dz, float* loss_sums, int rows, int K, const LossWM& wm, cudaStream_t s) {
+  DISPATCH_PREC(prec, T, (launch_pdl(softmax_xent_kernel<T, true>, dim3(1), dim3(1024), (size_t)0, s, (const T*)z, y, (T*)dz, (T*)nullptr, loss_sums, rows, K, wm))); LAUNCHED();
+  g_ew_last_kernel = "softmax_xent_kernel<wm>";
 }
 
 // ---------------------------------------------------------------- regression / margin losses ----------------
@@ -733,9 +757,11 @@ int k_loss_blocks(size_t n_per_group, int groups) {
   const size_t b = (n_per_group + LOSS_ELEMS_PER_BLOCK - 1) / LOSS_ELEMS_PER_BLOCK;
   return (int)std::min<size_t>(std::max<size_t>(b, 1), std::max(1, LOSS_MAX_GRID / groups));
 }
-template <typename T>
+// WM: element i's score and dz scaled by sc = loss_wm_scale(wm, i / n_out, i % n_out): the score l * (double)sc, dz = (dL/da * act'(a)) * sc.
+template <typename T, bool WM>
 __global__ void __launch_bounds__(LOSS_THREADS) loss_kernel(const T* __restrict__ z, const float* __restrict__ y, T* __restrict__ dz, float* __restrict__ loss_sums,
-                                                           size_t n_per_group, int n_out, int bpg, int loss, int act, float alpha, double* partial, unsigned* ticket) {
+                                                           size_t n_per_group, int n_out, int bpg, int loss, int act, float alpha, double* partial, unsigned* ticket,
+                                                           LossWM wm) {
   pdl_enter();
   __shared__ double red[LOSS_THREADS / 32];
   __shared__ int last;
@@ -756,8 +782,8 @@ __global__ void __launch_bounds__(LOSS_THREADS) loss_kernel(const T* __restrict_
       case LOSS_SQUARED_HINGE: l = m > 0.0 ? m * m : 0.0; ga = m > 0.0 ? -2.0f * yi * (float)m : 0.f; break;
       default: l = (double)yi * (double)a; ga = yi / nf; break;                   // LOSS_WASSERSTEIN
     }
-    acc += l;
-    stf(dz, i, ga * act_grad_from_out(act, a, alpha));
+    if (WM) { const float sc = loss_wm_scale(wm, i / n_out, (int)(i % n_out)); acc += __dmul_rn(l, (double)sc); stf(dz, i, ga * act_grad_from_out(act, a, alpha) * sc); }
+    else { acc += l; stf(dz, i, ga * act_grad_from_out(act, a, alpha)); }
   }
   const double tot = block_sum(acc, red);
   if (threadIdx.x == 0) {
@@ -782,9 +808,16 @@ __global__ void __launch_bounds__(LOSS_THREADS) loss_kernel(const T* __restrict_
 void k_loss(int prec, int loss, int act, float alpha, const void* z, const float* y, void* dz, float* loss_sums, int rows_per_group, int n_out, int groups,
             double* partial, unsigned* ticket, cudaStream_t s) {
   const size_t n = (size_t)rows_per_group * n_out; const int bpg = k_loss_blocks(n, groups);
-  DISPATCH_PREC(prec, T, (launch_pdl(loss_kernel<T>, dim3(groups * bpg), dim3(LOSS_THREADS), (size_t)0, s, (const T*)z, y, (T*)dz, loss_sums, n, n_out, bpg,
-                                     loss, act, alpha, partial, ticket))); LAUNCHED();
+  DISPATCH_PREC(prec, T, (launch_pdl(loss_kernel<T, false>, dim3(groups * bpg), dim3(LOSS_THREADS), (size_t)0, s, (const T*)z, y, (T*)dz, loss_sums, n, n_out, bpg,
+                                     loss, act, alpha, partial, ticket, LossWM{}))); LAUNCHED();
   g_ew_last_kernel = "loss_kernel";
+}
+void k_loss_wm(int prec, int loss, int act, float alpha, const void* z, const float* y, void* dz, float* loss_sums, int rows_per_group, int n_out, int groups,
+               double* partial, unsigned* ticket, const LossWM& wm, cudaStream_t s) {
+  const size_t n = (size_t)rows_per_group * n_out; const int bpg = k_loss_blocks(n, groups);
+  DISPATCH_PREC(prec, T, (launch_pdl(loss_kernel<T, true>, dim3(groups * bpg), dim3(LOSS_THREADS), (size_t)0, s, (const T*)z, y, (T*)dz, loss_sums, n, n_out, bpg,
+                                     loss, act, alpha, partial, ticket, wm))); LAUNCHED();
+  g_ew_last_kernel = "loss_kernel<wm>";
 }
 
 // ---------------------------------------------------------------- column sum / misc reductions -----------

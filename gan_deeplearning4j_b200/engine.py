@@ -553,6 +553,11 @@ class Net:
             for sp in self.specs:         # Layer.Builder.weightNoise
                 if sp.get("weight_noise") is not None:
                     self.set_weight_noise(sp["weight_noise"], sp["name"])
+            for sp in self.specs[:-1]:
+                if sp.get("loss_weights") is not None:
+                    raise ValueError(f"layer {sp.get('name')!r}: loss_weights belong to the net's last (loss) layer")
+            if self.specs and self.specs[-1].get("loss_weights") is not None:     # new LossMCXENT(weights), ...
+                self.set_loss_weights(self.specs[-1]["loss_weights"])
         except Exception:
             self.close()
             raise
@@ -628,17 +633,52 @@ class Net:
         check(self.lib.b2g_net_get_activation(self.h, layer, batch, _fp(out)))
         return out
 
-    def compute_gradient_and_score(self, x, y) -> float:
+    def _mask(self, mask, batch: int):
+        """A labels mask as (contiguous fp32, width): [batch] or [batch, 1] per example, [batch, nOut] per output, NCHW [batch, 1 or C, H, W]
+        on a CnnLossLayer; the width is its second dimension, and the mask holds exactly what the engine reads for it."""
+        m = _f32(mask)
+        width = m.shape[1] if m.ndim >= 2 else 1
+        cols = C.c_int32()
+        check(self.lib.b2g_net_loss_columns(self.h, C.byref(cols)))
+        per = self.out_elems // max(1, cols.value) * width
+        if m.shape[0] != batch or m.size != batch * per:
+            raise ValueError(f"labels mask of shape {m.shape}: {batch} examples of {self.out_elems // max(1, cols.value)} values per column of "
+                             f"its width {width} (1 or {cols.value})")
+        return m, width
+
+    def compute_gradient_and_score(self, x, y, mask=None) -> float:
+        """mask: DataSet's labels mask (semantics at b2g_loss in include/b200gan.h), or None."""
         x, y = _f32(x), _f32(y)
         s = C.c_float()
-        check(self.lib.b2g_net_compute_gradient_and_score(self.h, _fp(x), _fp(y), x.shape[0], C.byref(s)))
+        if mask is None:
+            check(self.lib.b2g_net_compute_gradient_and_score(self.h, _fp(x), _fp(y), x.shape[0], C.byref(s)))
+        else:
+            m, width = self._mask(mask, x.shape[0])
+            check(self.lib.b2g_net_compute_gradient_and_score_masked(self.h, _fp(x), _fp(y), x.shape[0], C.byref(s), _fp(m), width))
         return s.value
 
-    def fit(self, x, y) -> float:
+    def fit(self, x, y, mask=None) -> float:
+        """mask: DataSet's labels mask (semantics at b2g_loss in include/b200gan.h), or None."""
         x, y = _f32(x), _f32(y)
         s = C.c_float()
-        check(self.lib.b2g_net_fit(self.h, _fp(x), _fp(y), x.shape[0], C.byref(s)))
+        if mask is None:
+            check(self.lib.b2g_net_fit(self.h, _fp(x), _fp(y), x.shape[0], C.byref(s)))
+        else:
+            m, width = self._mask(mask, x.shape[0])
+            check(self.lib.b2g_net_fit_masked(self.h, _fp(x), _fp(y), x.shape[0], C.byref(s), _fp(m), width))
         return s.value
+
+    def set_loss_weights(self, weights, layer: Optional[str] = None):
+        """The per-output weights of the net's loss layer (new LossMCXENT(weights), new LossBinaryXENT(weights), new LossMSE(weights), ...):
+        nOut (C on a CnnLossLayer) finite floats, None clears.  The kept specs (and so checkpoints) carry them."""
+        name = layer.encode() if layer is not None else None
+        if weights is None:
+            check(self.lib.b2g_net_set_loss_weights(self.h, name, None, 0))
+            self.specs[-1].pop("loss_weights", None)
+            return
+        w = _f32(weights).ravel()
+        check(self.lib.b2g_net_set_loss_weights(self.h, name, _fp(w), w.size))
+        self.specs[-1]["loss_weights"] = [float(v) for v in w]
 
     def set_gradient_normalization(self, mode: str, threshold: float = 1.0):
         """DL4J's GradientNormalization for every layer of the net, applied from the next update on: "none", "renormalize_l2_per_layer",
@@ -895,6 +935,20 @@ class Gan:
         check(self.lib.b2g_gan_upload(self.h, *[_fp(v) for v in a], a[0].shape[0]))
         self.gen.ctx.sync()
 
+    def set_label_masks(self, m_real, m_fake, m_gen):
+        """Labels masks of the discriminator's loss for every later step (b2g_gan_set_label_masks): [batch, 1] per example, or NCHW
+        [batch, 1 or C, H, W] on a CnnLossLayer discriminator.  All three None clears."""
+        if m_real is None and m_fake is None and m_gen is None:
+            check(self.lib.b2g_gan_set_label_masks(self.h, None, None, None, 0, 0))
+            return
+        ms = [_f32(m) for m in (m_real, m_fake, m_gen)]
+        batch = ms[0].shape[0]
+        width = self.dis._mask(ms[0], batch)[1]
+        for m in ms[1:]:
+            if m.shape != ms[0].shape:
+                raise ValueError(f"labels masks of shapes {[v.shape for v in ms]}")
+        check(self.lib.b2g_gan_set_label_masks(self.h, *[_fp(m) for m in ms], width, batch))
+
     def step_resident(self, batch: int):
         check(self.lib.b2g_gan_step_resident(self.h, batch))
 
@@ -1048,6 +1102,28 @@ def test_ew(ctx: Context, precision: int, op: str, in0, in1=None, out_sizes=(0, 
     check(ctx.lib.b2g_test_ew(ctx.h, precision, C.byref(o), *[ptr(a) for a in ins], *[ptr(a) for a in outs]))
     info = {"kernel": o.kernel.decode(), "sumsq": o.sumsq, "wide": [o.jobs[i].wide for i in range(o.n_jobs)] if jobs is not None else []}
     return outs, info
+
+
+LOSS_TEST_KERNELS = {"xent": 0, "softmax_xent": 1, "codes": 2, "cnn_xent": 3, "cnn_softmax_xent": 4}
+
+
+def test_loss(ctx: Context, precision: int, kernel: str, z, y, w=None, mask=None, *, rows: int, cols: int, groups: int = 1, loss: str = "mse",
+              act: str = "identity", alpha: float = 0.0, clip_eps: float = 0.0, offset: int = 0, poison: bool = False):
+    """A weighted / masked loss kernel through its production wrapper (b2g_test_loss; operands in include/b200gan.h).  mask: [groups * rows,
+    width].  Returns (dz, loss_sums, kernel name)."""
+    o = _lib.TestLossOpts()
+    o.kernel, o.rows, o.cols, o.groups, o.loss, o.act = LOSS_TEST_KERNELS[kernel], rows, cols, groups, LOSSES[loss], ACTS[act]
+    o.alpha, o.clip_eps, o.offset, o.poison = alpha, clip_eps, offset, int(poison)
+    zz, yy = _f32(z).ravel(), _f32(y).ravel()
+    ww = None if w is None else _f32(w).ravel()
+    mm = None if mask is None else _f32(mask)
+    if mm is not None:
+        o.mask_width = mm.shape[1] if mm.ndim > 1 else 1
+        mm = mm.ravel()
+    dz, ls = np.empty(zz.size, np.float32), np.empty(groups, np.float32)
+    ptr = lambda a: None if a is None else _fp(a)
+    check(ctx.lib.b2g_test_loss(ctx.h, precision, C.byref(o), _fp(zz), _fp(yy), ptr(ww), ptr(mm), _fp(dz), _fp(ls)))
+    return dz, ls, o.kernel_name.decode()
 
 
 POOL_TEST_OPS = {"pool2d": 0, "global_pool": 1}

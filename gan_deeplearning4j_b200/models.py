@@ -226,10 +226,10 @@ _global_pooling_spec = global_pooling       # dcgan_discriminator's argument of 
 
 
 # ------------------------------------------------------------------ per-pixel loss ---------------------
-def cnn_loss(loss="xent", activation="identity", name="", alpha=None) -> Dict:
+def cnn_loss(loss="xent", activation="identity", name="", alpha=None, loss_weights=None) -> Dict:
     """new CnnLossLayer.Builder(LossFunction).activation(act): the loss on every pixel of a [mb, C, H, W] map, labels [mb, C, H, W]
     (B2G_LAYER_CNN_LOSS in include/b200gan.h).  XENT implies a sigmoid per element, MCXENT a softmax over the channels of each pixel; the
-    others apply `activation`."""
+    others apply `activation`.  loss_weights: the loss's per-channel weights (new LossMCXENT(weights), ...; C finite floats), or None."""
     if loss not in ("xent", "mcxent", "mse", "l1", "l2", "mae", "hinge", "squared_hinge", "wasserstein"):
         raise ValueError(f"unknown loss {loss!r}")
     if loss in ("xent", "mcxent") and activation != "identity":
@@ -237,6 +237,8 @@ def cnn_loss(loss="xent", activation="identity", name="", alpha=None) -> Dict:
     spec = {"type": "cnn_loss", "name": name, "loss": loss}
     if loss not in ("xent", "mcxent"):
         spec.update(_act(activation, alpha))
+    if loss_weights is not None:
+        spec["loss_weights"] = [float(v) for v in loss_weights]
     return spec
 
 

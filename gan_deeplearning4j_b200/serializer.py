@@ -108,4 +108,7 @@ def restore_into(net, path, load_updater: bool = True) -> Dict:
     # the epoch count EPOCH learning-rate schedules read
     if "epoch" in m["meta"] and hasattr(net, "set_epoch"):
         net.set_epoch(int(m["meta"]["epoch"]))
+    # the loss layer's per-output weights (new LossMCXENT(weights), ...) are part of its configuration
+    if m["specs"] and m["specs"][-1].get("type") in ("output", "loss", "cnn_loss") and hasattr(net, "set_loss_weights"):
+        net.set_loss_weights(m["specs"][-1].get("loss_weights"))
     return m

@@ -279,6 +279,26 @@ typedef enum { B2G_PREC_FP32 = 0, B2G_PREC_BF16 = 1 } b2g_precision;
  * With an activation of codes 5-16 (b2g_activation) a = f(z) is formed by its own kernel and rounded to the activation type, the loss takes a
  * with the identity, and dL/dz = dL/da * f'(z) with the derivative taken from z.
  *
+ * Per-output weights and label masks (b2g_net_set_loss_weights, b2g_net_fit_masked, b2g_gan_set_label_masks; DL4J 1.0.0-beta3 ILossFunction
+ * weights and DataSet labels masks, recalled).  Row r is an example (a pixel of a CnnLossLayer), column j an output (a channel of a
+ * CnnLossLayer), w_j the weight (1 without weights), m_rj the mask (1 without one; a [rows, 1] mask gives every column of its row one value):
+ *   XENT, codes 2-8   the row's score terms become w_j m_rj l(a_rj, y_rj) and dz_rj = w_j m_rj (dz_rj unweighted)
+ *   MCXENT            score -m_r sum_j w_j y_rj log clamp(p_rj);  dz_rj = m_r (p_rj sum_k w_k y_rk - w_j y_rj) with weights (LossMCXENT's
+ *                     weighted softmax gradient), m_r (p_rj - y_rj) without
+ *   The score stays the sum divided by the minibatch (not by the mask count); MSE, MAE and WASSERSTEIN still divide by nOut / C.  Masks are
+ *   multiplicative fp32 values taken as given, like labels: [N, 1] or [N, nOut] on OUTPUT / LOSS layers, NCHW [N, 1, H, W] or [N, C, H, W] on a
+ *   CnnLossLayer.  Weights are nOut (C) finite floats.  b2g_net_output ignores both.
+ *   Refused: weights on HINGE, SQUARED_HINGE or WASSERSTEIN (DL4J has no weights constructor for them) and a per-output mask with MCXENT
+ *   (LossMCXENT: "Per output masking for MCXENT + softmax: not supported"): B2G_ERR_UNSUPPORTED; a weight count or mask width other than
+ *   those above: B2G_ERR_SHAPE; a non-finite weight, or weights on a net whose last layer is not OUTPUT / LOSS / CNN_LOSS: B2G_ERR_ARG.
+ *   Arithmetic (no product below is fused into an add): s = w_j * m_rj in fp32 (w first; what is absent is 1); the score term enters the
+ *   loss's double sum as (double)l * (double)s (the loss kernel's double l times (double)s) and dz is the unweighted fp32 dz times s, in the
+ *   unweighted kernels' slicing and summation order.  MCXENT forms sy = sum_k w_k y_rk in fp32 in class order (each product rounded, then
+ *   added); dz = m_r * (p * sy - w_j y_j) with p * sy rounded before the subtraction; its term is (double)(m_r * w_j y_rj) *
+ *   log((double)clamp(p)), subtracted from the double sum.  A net with neither
+ *   weights nor a mask launches the unweighted instantiations; a weighted or masked loss is the same single launch.  All-ones weights and
+ *   mask give the unweighted bits (for MCXENT with one-hot labels).
+ *
  * B2G_LAYER_CNN_LOSS (DL4J 1.0.0-beta3 CnnLossLayer, recalled; parity unpinned like the rest of the DL4J semantics).  No parameters.
  *   Rows and columns: the input is the layer below's [N, C, H, W]; the rows are its N*H*W pixels and the columns its C channels (DL4J's
  *   reshape4dTo2d, which in the engine's NHWC layout is the buffer as it is).  A 1x1 map is accepted and then equals a LOSS layer on the same
@@ -293,7 +313,7 @@ typedef enum { B2G_PREC_FP32 = 0, B2G_PREC_BF16 = 1 } b2g_precision;
  *   fixed by the shape (kernels_cnnloss.cu for XENT / MCXENT, loss_kernel for codes 2-8) and rounded to fp32 once.
  *   Labels: [N, C, H, W] fp32 in DL4J's NCHW order, b2g_net_output_size elements per example (fit, computeGradientAndScore and the GAN step).
  *   b2g_net_output returns the activated map in NCHW: the sigmoid (XENT), the per-pixel softmax (MCXENT) or act(z).
- *   Not supported: label masks, per-output weights, and the NHWC CNN2DFormat of later DL4J versions.
+ *   Not supported: the NHWC CNN2DFormat of later DL4J versions.
  *   The adversarial step (b2g_gan_create) takes a discriminator ending in CNN_LOSS with XENT or codes 2-8 (a PatchGAN critic: one logit and
  *   one label per patch); MCXENT there is B2G_ERR_UNSUPPORTED. */
 typedef enum {
@@ -383,6 +403,20 @@ int32_t b2g_net_get_input_gradient(b2g_net* net, int32_t batch, float* host);
 /* ComputationGraph.fit(DataSet) (J:426,471 via SparkComputationGraph): one minibatch =
  * computeGradientAndScore + [gradient all-reduce if a communicator is attached] + updater + params.subi. */
 int32_t b2g_net_fit(b2g_net* net, const float* x, const float* y, int32_t batch, float* score);
+/* fit / computeGradientAndScore of a DataSet with a labels mask (DataSet(features, labels, null, labelsMask)); semantics at b2g_loss.
+ * mask: fp32 host, [batch, mask_width] on OUTPUT / LOSS layers (mask_width 1 = per example, nOut = per output), NCHW [batch, mask_width, H, W]
+ * on a CnnLossLayer (mask_width 1 = per pixel, C = per output); null = no mask (mask_width ignored). */
+int32_t b2g_net_fit_masked(b2g_net* net, const float* x, const float* y, int32_t batch, float* score, const float* mask, int32_t mask_width);
+int32_t b2g_net_compute_gradient_and_score_masked(b2g_net* net, const float* x, const float* y, int32_t batch, float* score, const float* mask,
+                                                  int32_t mask_width);
+/* new LossMCXENT(weights), new LossBinaryXENT(weights), new LossMSE(weights), ...: the per-output weights of the net's loss layer (semantics at
+ * b2g_loss), kept in device memory and used by every later fit, computeGradientAndScore and GAN step.  layer: null = the net's loss layer, or
+ * its name; w: n = nOut (C on a CnnLossLayer) finite floats, null = clear (with layer null a no-op on a net that has none, whatever its last
+ * layer).  Setting or clearing re-captures a captured GAN step. */
+int32_t b2g_net_set_loss_weights(b2g_net* net, const char* layer, const float* w, int32_t n);
+/* The columns of the net's loss: nOut (the outputs per example), or the channels C of a CnnLossLayer.  A mask of width 1 holds
+ * b2g_net_output_size / columns values per example, one of width = columns b2g_net_output_size. */
+int32_t b2g_net_loss_columns(b2g_net* net, int32_t* cols);
 /* The updater's iteration counter (BaseMultiLayerUpdater's iteration; Adam's t = iteration + 1).  ModelSerializer keeps it in
  * configuration.json ("iterationCount"); a restore that drops it restarts Adam's bias correction with warm moments (J:606-618). */
 int32_t b2g_net_get_iteration(b2g_net* net, int64_t* out);
@@ -658,6 +692,11 @@ int32_t b2g_gan_step(b2g_gan* gan, const float* x_real, const float* z_d, const 
 int32_t b2g_gan_upload(b2g_gan* gan, const float* x_real, const float* z_d, const float* z_g,
                        const float* y_real, const float* y_fake, const float* y_gen, int32_t batch);
 int32_t b2g_gan_step_resident(b2g_gan* gan, int32_t batch);
+/* Label masks of the discriminator's loss for every later b2g_gan_step / b2g_gan_step_resident (semantics at b2g_loss): m_real / m_fake for the
+ * D update's two halves, m_gen for the G update through D, each [batch, mask_width(, H, W)] fp32 host laid out like b2g_net_fit_masked's mask,
+ * copied to the device here.  A step with another batch is B2G_ERR_SHAPE.  All three null clears.  New contents reach a replayed graph
+ * without re-capture; turning masks on or off, or changing the width, re-captures. */
+int32_t b2g_gan_set_label_masks(b2g_gan* gan, const float* m_real, const float* m_fake, const float* m_gen, int32_t mask_width, int32_t batch);
 int32_t b2g_gan_read_losses(b2g_gan* gan, float* losses);   /* syncs */
 /* CUDA-event time of the last b2g_gan_step_resident call, in ms (measured on the launching stream). */
 int32_t b2g_gan_last_step_ms(b2g_gan* gan, float* ms);
@@ -877,6 +916,30 @@ typedef struct {
   int32_t splits;         /* out, GLOBAL_POOL: the number of blocks each example's pixel range was split over (1: no split) */
 } b2g_test_pool_opts;
 int32_t b2g_test_pool(b2g_ctx* ctx, int32_t precision, b2g_test_pool_opts* opts, const float* in0, const float* in1, float* out0, float* out1, float* out2);
+
+/* The weighted / masked instantiations of the five loss kernels (semantics and order at b2g_loss) through their production wrappers on host
+ * tensors (z rounded to bf16 on the device when precision is BF16; offset and poison as b2g_test_ew's):
+ *   XENT               xent_kernel: z, y, dz [groups][rows] (cols = 1)
+ *   SOFTMAX_XENT       softmax_xent_kernel: z, y, dz [rows][cols] (groups = 1)
+ *   CODES              loss_kernel: z, y, dz [groups][rows][cols], loss b2g_loss 2-8 on act (b2g_activation 0-4, alpha)
+ *   CNN_XENT           cnn_xent_kernel: z, y, dz [groups][rows][cols] (NHWC pixels x channels)
+ *   CNN_SOFTMAX_XENT   cnn_softmax_xent_kernel: as CNN_XENT
+ * w: [cols] or NULL; mask: [groups * rows][mask_width] or NULL (mask_width 1 or cols); out dz (T, widened to fp32) and loss_sums [groups].
+ * The weighted / masked instantiation runs even with neither. */
+typedef enum { B2G_TEST_LOSS_XENT = 0, B2G_TEST_LOSS_SOFTMAX_XENT = 1, B2G_TEST_LOSS_CODES = 2, B2G_TEST_LOSS_CNN_XENT = 3,
+               B2G_TEST_LOSS_CNN_SOFTMAX_XENT = 4 } b2g_test_loss_kernel;
+typedef struct {
+  int32_t kernel;         /* b2g_test_loss_kernel */
+  int32_t rows, cols, groups;
+  int32_t loss, act; float alpha;       /* CODES */
+  float clip_eps;                       /* XENT, CNN_XENT: 0 = BCE with logits */
+  int32_t mask_width;     /* with a mask: 1 or cols */
+  int32_t offset;         /* every device operand starts this many elements past a 256-byte aligned address (reaches the misaligned paths) */
+  int32_t poison;         /* fill dz and the loss sums with NaN before the launch */
+  char kernel_name[64];   /* out: the kernel the wrapper dispatched */
+} b2g_test_loss_opts;
+int32_t b2g_test_loss(b2g_ctx* ctx, int32_t precision, b2g_test_loss_opts* opts, const float* z, const float* y, const float* w, const float* mask,
+                      float* dz, float* loss_sums);
 
 #ifdef __cplusplus
 }

@@ -32,5 +32,14 @@ public final class GanTrainer implements AutoCloseable {
             Native.address(Native.floats(yr)), Native.address(Native.floats(yf)), Native.address(Native.floats(yg)), (int) mb, Native.address(l)));
         return new float[] { l.getFloat(0), l.getFloat(4), l.getFloat(8) };
     }
+    /** Labels masks of the discriminator's loss for every later step ([mb, 1] per example, or [mb, 1 | C, H, W] on a CnnLossLayer
+     *  discriminator; semantics at b2g_loss); all three null clears. */
+    public void setLabelMasks(INDArray mReal, INDArray mFake, INDArray mGen) {
+        if (mReal == null && mFake == null && mGen == null) { Native.check(Native.ganSetLabelMasks(gan, 0L, 0L, 0L, 0, 0)); return; }
+        long[] sh = mReal.shape(); int width = sh.length > 1 ? (int) sh[1] : 1;
+        java.nio.FloatBuffer r = Native.floats(mReal.data), f = Native.floats(mFake.data), g = Native.floats(mGen.data);
+        Native.check(Native.ganSetLabelMasks(gan, Native.address(r), Native.address(f), Native.address(g), width, (int) sh[0]));
+        java.lang.ref.Reference.reachabilityFence(r); java.lang.ref.Reference.reachabilityFence(f); java.lang.ref.Reference.reachabilityFence(g);
+    }
     @Override public void close() { Native.ganDestroy(gan); }
 }

@@ -51,6 +51,9 @@ public final class Native {
     public static native int netEnableP2pAllreduce(long net, long outEnabledAddr);   // collective over the communicator: b2g_net_enable_p2p_allreduce
     public static native int netOutput(long net, long xAddr, int batch, int train, long outAddr);
     public static native int netFit(long net, long xAddr, long yAddr, int batch, long scoreAddr);
+    public static native int netFitMasked(long net, long xAddr, long yAddr, int batch, long scoreAddr, long maskAddr, int maskWidth);
+    public static native int netSetLossWeights(long net, long layerNameAddr, long wAddr, int n);
+    public static native int ganSetLabelMasks(long gan, long mReal, long mFake, long mGen, int maskWidth, int batch);
     public static native int ganCreate(long gen, long dis, int fakeBnTrain, int useGraph, long outHandleAddr);
     public static native int ganDestroy(long gan);
     public static native int ganStep(long gan, long xReal, long zD, long zG, long yReal, long yFake, long yGen, int batch, long lossesAddr);

@@ -7,5 +7,7 @@ public final class CnnLossLayer {
         // XENT implies a sigmoid per element and MCXENT a softmax over the channels of each pixel; the other losses apply .activation(..),
         // identity by default
         public Builder(org.nd4j.linalg.lossfunctions.LossFunctions.LossFunction f) { l.type = TYPE; l.loss = f.code; l.act = 0; }
+        /** new LossMCXENT(weights), ...: the loss and its per-channel weights. */
+        public Builder(org.nd4j.linalg.lossfunctions.ILossFunction f) { this(f.lossFunction()); l.lossWeights = f.getWeights(); }
     }
 }

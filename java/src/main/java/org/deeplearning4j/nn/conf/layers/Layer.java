@@ -22,6 +22,8 @@ public class Layer {
     /** constrainAllParameters / constrainWeights / constrainBias; all null: the global builder's lists apply. */
     public List<LayerConstraint> constrainAll, constrainW, constrainB;
     public boolean alphaSet;   // alpha given by leakyReluAlpha(..) or activation(IActivation); else ELU / ThresholdedReLU write DL4J's 1.0
+    /** The loss's per-output weights of an OutputLayer / LossLayer / CnnLossLayer built from an ILossFunction (null: none): applied by ComputationGraph.init. */
+    public org.nd4j.linalg.api.ndarray.INDArray lossWeights;
 
     /** Serialise into the C struct layout (little-endian, no padding: every field is 4-byte aligned). */
     public void write(ByteBuffer b, Activation globalAct, float globalL2) {
@@ -35,7 +37,7 @@ public class Layer {
     public Layer copy() { Layer c = new Layer(); c.type = type; c.nIn = nIn; c.nOut = nOut; c.kH = kH; c.kW = kW; c.sH = sH; c.sW = sW; c.pH = pH; c.pW = pW; c.hasBias = hasBias; c.act = act;
         c.preH = preH; c.preW = preW; c.preC = preC; c.loss = loss; c.frozen = frozen; c.alpha = alpha; c.l2 = l2; c.l1 = l1; c.l1Bias = l1Bias; c.l2Bias = l2Bias; c.bnDecay = bnDecay; c.bnEps = bnEps; c.updater = updater; c.name = name; c.alphaSet = alphaSet;
         c.constrainAll = constrainAll; c.constrainW = constrainW; c.constrainB = constrainB; c.dropSchedule = dropSchedule; c.weightNoise = weightNoise;
-        c.weightInit = weightInit; c.dist = dist; c.biasInit = biasInit; return c; }
+        c.weightInit = weightInit; c.dist = dist; c.biasInit = biasInit; c.lossWeights = lossWeights; return c; }
     protected int defaultAct(Activation g) { return g.code; }   // conv / dense inherit the global .activation(..) (J:126)
 
     @SuppressWarnings("unchecked")

@@ -48,6 +48,9 @@ public class ComputationGraph {
         for (Layer l : layers)            // new Adam(ISchedule) / RmsProp(ISchedule) / Sgd(ISchedule): evaluated on the device at every update
             if (l.updater != null && l.updater.lrSchedule() != null && hasLearningRate(l)) setLearningRate(l.name, l.updater.lrSchedule());
         for (Layer l : layers) applyConstraints(l);
+        Layer last = layers.get(layers.size() - 1);     // new LossMCXENT(weights), ...: device-resident, used by every later fit
+        if (last.lossWeights != null)
+            Native.check(Native.netSetLossWeights(net, 0L, Native.address(Native.floats(last.lossWeights.data)), (int) last.lossWeights.length()));
         for (Layer l : layers)            // new GaussianNoise(ISchedule) etc.: evaluated on the device at every train-mode forward
             if (l.type == 11 && l.dropSchedule != null) setDropoutSchedule(l.name, l.dropSchedule);
         for (Layer l : layers) {          // DropConnect / WeightNoise: drawn on the device at every train-mode pass
@@ -206,7 +209,12 @@ public class ComputationGraph {
     /** fit(DataSet): one minibatch = computeGradientAndScore + updater + params.subi (what SparkComputationGraph.fit reaches, SURVEY.md 3.3). */
     public void fit(DataSet ds) {
         int batch = (int) ds.getFeatures().shape()[0]; ByteBuffer score = Native.direct(4);
-        Native.check(Native.netFit(net, Native.address(Native.floats(ds.getFeatures().data)), Native.address(Native.floats(ds.getLabels().data)), batch, Native.address(score)));
+        INDArray mask = ds.getLabelsMaskArray();
+        if (mask == null)
+            Native.check(Native.netFit(net, Native.address(Native.floats(ds.getFeatures().data)), Native.address(Native.floats(ds.getLabels().data)), batch, Native.address(score)));
+        else                              // the mask's width is its second dimension: 1 (per example / pixel) or nOut / C (per output)
+            Native.check(Native.netFitMasked(net, Native.address(Native.floats(ds.getFeatures().data)), Native.address(Native.floats(ds.getLabels().data)), batch,
+                                             Native.address(score), Native.address(Native.floats(mask.data)), mask.shape().length > 1 ? (int) mask.shape()[1] : 1));
     }
     public INDArray params() { int n = (int) numParams(); FloatBuffer b = Native.direct(4 * n).asFloatBuffer(); Native.check(Native.netGetParams(net, Native.address(b), n)); float[] d = new float[n]; b.get(d); return new INDArray(d, 1, n); }
     /** Updater state in the library's [state0 | state1] order (RmsProp cache / Adam m, then Adam v), 2 x numParams values, plus | state2

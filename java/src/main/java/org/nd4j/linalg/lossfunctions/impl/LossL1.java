@@ -1,0 +1,12 @@
+package org.nd4j.linalg.lossfunctions.impl;
+import org.nd4j.linalg.api.ndarray.INDArray;
+import org.nd4j.linalg.lossfunctions.ILossFunction;
+import org.nd4j.linalg.lossfunctions.LossFunctions;
+/** LossL1, with optional per-output weights (a row vector of nOut finite values; C on a CnnLossLayer). */
+public class LossL1 implements ILossFunction {
+    private final INDArray weights;
+    public LossL1() { this(null); }
+    public LossL1(INDArray weights) { this.weights = weights; }
+    public LossFunctions.LossFunction lossFunction() { return LossFunctions.LossFunction.L1; }
+    public INDArray getWeights() { return weights; }
+}

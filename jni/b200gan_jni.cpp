@@ -93,6 +93,15 @@ FN(netOutput)(JNIEnv_*, jclass, jlong net, jlong xAddr, jint batch, jint train, 
 FN(netFit)(JNIEnv_*, jclass, jlong net, jlong xAddr, jlong yAddr, jint batch, jlong scoreAddr) {
   return b2g_net_fit(P(b2g_net*, net), P(const float*, xAddr), P(const float*, yAddr), batch, P(float*, scoreAddr));
 }
+FN(netFitMasked)(JNIEnv_*, jclass, jlong net, jlong xAddr, jlong yAddr, jint batch, jlong scoreAddr, jlong maskAddr, jint maskWidth) {
+  return b2g_net_fit_masked(P(b2g_net*, net), P(const float*, xAddr), P(const float*, yAddr), batch, P(float*, scoreAddr), P(const float*, maskAddr), maskWidth);
+}
+FN(netSetLossWeights)(JNIEnv_*, jclass, jlong net, jlong layerNameAddr, jlong wAddr, jint n) {
+  return b2g_net_set_loss_weights(P(b2g_net*, net), P(const char*, layerNameAddr), P(const float*, wAddr), n);
+}
+FN(ganSetLabelMasks)(JNIEnv_*, jclass, jlong gan, jlong mReal, jlong mFake, jlong mGen, jint maskWidth, jint batch) {
+  return b2g_gan_set_label_masks(P(b2g_gan*, gan), P(const float*, mReal), P(const float*, mFake), P(const float*, mGen), maskWidth, batch);
+}
 FN(ganCreate)(JNIEnv_*, jclass, jlong gen, jlong dis, jint fakeBnTrain, jint useGraph, jlong outHandleAddr) {
   b2g_gan_config c{fakeBnTrain, useGraph};
   return b2g_gan_create(P(b2g_net*, gen), P(b2g_net*, dis), &c, P(b2g_gan**, outHandleAddr));

@@ -69,6 +69,8 @@ def build(ctx, cfg_name, variant):
     gan = b.Gan(G, D, fake_bn_train=False, use_cuda_graph=True)
     if "hook" in variant:
         variant["hook"](G); variant["hook"](D)
+    if "gan_hook" in variant:
+        variant["gan_hook"](gan, D, n)
     data = bench.synthetic(cfg, n, 666)
     if "labels" in variant:
         data = data[:3] + [np.full((n, 1), v, np.float32) for v in variant["labels"]]
@@ -280,19 +282,23 @@ def gradnorm(mode):
 
 
 # ---------------------------------------------------------------- graph: residual C2, a U-Net fit and the vertex kernels
-def unet_step(ctx, steps):
+def unet_step(ctx, steps, weighted=False):
+    """weighted: class weights (0.5, 2) and a per-pixel labels mask (a quarter of the pixels 0), as a segmentation run with void pixels has."""
     n, size = 128, 64
     net = b.Net(ctx, m.unet(size, 3, 2, 32, 2), (3, size, size), max_batch=n, precision=b.BF16)
     rng = np.random.default_rng(1)
     x = rng.uniform(-1, 1, (n, 3, size, size)).astype(np.float32)
     lab = rng.integers(0, 2, (n, size, size))
     y = np.ascontiguousarray(np.moveaxis(np.eye(2, dtype=np.float32)[lab], -1, 1))
+    mask = (rng.uniform(0, 1, (n, 1, size, size)) > 0.25).astype(np.float32) if weighted else None
+    if weighted:
+        net.set_loss_weights([0.5, 2.0])
     for _ in range(3):
-        net.fit(x, y)
+        net.fit(x, y, mask=mask)
     s0, l0 = net.simt_gemm_calls(), ctx.launch_count()
     t0 = time.perf_counter()
     for _ in range(steps):
-        net.fit(x, y)                    # returns after a device synchronise
+        net.fit(x, y, mask=mask)         # returns after a device synchronise
     ms = (time.perf_counter() - t0) * 1e3 / steps
     res = {"ms_per_fit_incl_host_copies": round(ms, 3), "simt_calls_per_fit": (net.simt_gemm_calls() - s0) / steps,
            "launches_per_fit": (ctx.launch_count() - l0) / steps}
@@ -385,6 +391,45 @@ def cnn_loss_kernels(ctx):
         _, t = hook_kernel(ctx, lambda: b.test_ew(ctx, b.BF16, op, z, y, (0, 0, 0), rows=rows, cols=c, groups=groups), (f"{op}_kernel",), 5, False, np.mean)
         byts = n * (2 + 2 + 4)
         res[name] = dict(t[f"{op}_kernel"], algorithmic_bytes=byts, fraction_of_3_35_TBps=fraction(byts, t[f"{op}_kernel"]["us"]))
+    return res
+
+
+# ---------------------------------------------------------------- lossmask: per-output loss weights and labels masks
+def patch_masks(gan, D, n):
+    """Per-patch labels masks on the C2 patch step: the border patches of the 4 x 4 map masked out, the inner ones 1."""
+    mk = np.zeros((n, 1, 4, 4), np.float32)
+    mk[:, :, 1:3, 1:3] = 1
+    gan.set_label_masks(mk, mk, mk)
+
+
+def loss_mask_kernels(ctx):
+    """The MCXENT and XENT CnnLossLayer kernels at a segmentation size, 16 x 128 x 128 pixels x 21 classes, unweighted and with class weights and
+    a per-pixel mask: a net of one identity ActivationLayer into the CnnLossLayer, fit 5 times under torch.profiler.  Algorithmic bytes per
+    element: z + dz (2 B each, bf16) + labels (4 B); the mask adds 4 B per pixel and the weights are left out."""
+    n, c, hw = 16, 21, 128
+    rng = np.random.default_rng(3)
+    x = rng.uniform(-3, 3, (n, c, hw, hw)).astype(np.float32)
+    lab = rng.integers(0, c, (n, hw, hw))
+    y1 = np.ascontiguousarray(np.moveaxis(np.eye(c, dtype=np.float32)[lab], -1, 1))
+    mask = (rng.uniform(0, 1, (n, 1, hw, hw)) > 0.25).astype(np.float32)
+    res = {}
+    for loss, kern in (("mcxent", "cnn_softmax_xent_kernel"), ("xent", "cnn_xent_kernel")):
+        for weighted in (False, True):
+            net = b.Net(ctx, [{"type": "activation", "name": "a", "activation": "identity"}, m.cnn_loss(loss, name="cl")], (c, hw, hw), max_batch=n,
+                        precision=b.BF16)
+            if weighted:
+                net.set_loss_weights(np.linspace(0.5, 2.0, c))
+            for _ in range(2):
+                net.fit(x, y1, mask=mask if weighted else None)
+            with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+                for _ in range(5):
+                    net.fit(x, y1, mask=mask if weighted else None)
+            t = kernel_us(prof, kern)
+            us = float(np.mean(t)) if t else None
+            byts = n * hw * hw * (c * (2 + 2 + 4) + (4 if weighted else 0))
+            res[f"{kern} {'weights + mask' if weighted else 'plain'}"] = {"us": us, "launches_per_fit": len(t) / 5, "algorithmic_bytes": byts,
+                                                                          "fraction_of_3_35_TBps": fraction(byts, us)}
+            net.close()
     return res
 
 
@@ -564,6 +609,11 @@ FEATURES = {
                   kernels=vertex_kernels, extras=lambda ctx, configs, steps: {"unet": unet_step(ctx, max(5, steps // 5))}),
     "loss": dict(configs="c5,c2", variants=[dict(name="xent", kernels=("xent_kernel",))] + [
         dict(name=k, d=dict(loss=k), labels=lab, kernels=("loss_kernel",)) for k, lab in LOSS_LABELS.items()], kernels=loss_fit_output),
+    "lossmask": dict(configs="c2", steps=50, variants=[dict(name="patch", d=dict(patch=True), kernels=("cnn_xent_kernel",)),
+                                                       dict(name="patch+mask", d=dict(patch=True), gan_hook=patch_masks, kernels=("cnn_xent_kernel",))],
+                     kernels=loss_mask_kernels,
+                     extras=lambda ctx, configs, steps: {"unet": unet_step(ctx, max(5, steps // 5)),
+                                                          "unet_weights_mask": unet_step(ctx, max(5, steps // 5), weighted=True)}),
     "patchgan": dict(configs="c2,c4", steps=50, variants=[{}, dict(name="patch", d=dict(patch=True))], kernels=cnn_loss_kernels, extras=head_conv),
     "pooling": dict(configs="c2", variants=[dict(name="base"), dict(name="sum", d=dict(global_pooling="sum")),
                                             dict(name="avg", d=dict(global_pooling="avg"))], kernels=pooling_kernels),
