@@ -101,6 +101,13 @@ class TestPoolOpts(C.Structure):
                 ("kernel", C.c_char * 64), ("splits", C.c_int32)]
 
 
+class TestBnOpts(C.Structure):
+    """b2g_test_bn_opts: the accumulator path, replica count, per-replica shape, fused activation and BatchNorm constants of a cross-replica
+    BatchNorm test."""
+    _fields_ = [(k, C.c_int32) for k in ("path", "replicas", "groups", "rows", "C", "act")] + [
+                ("alpha", C.c_float), ("eps", C.c_float), ("decay", C.c_float), ("want_param_grads", C.c_int32)]
+
+
 class TestLossOpts(C.Structure):
     """b2g_test_loss_opts: which weighted / masked loss kernel to run, its sizes and options, and what ran."""
     _fields_ = [(k, C.c_int32) for k in ("kernel", "rows", "cols", "groups", "loss", "act")] + [("alpha", C.c_float), ("clip_eps", C.c_float)] + [
@@ -185,6 +192,7 @@ PROTOTYPES = {
     "b2g_test_conv_ex": (_i32, [_vp, _i32, _i32, _i32, C.POINTER(ConvGeom), _fp, _fp, _fp, _i32, _fp, C.POINTER(TestConvOpts)]),
     "b2g_test_bn": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _fp, _fp, _fp, _fp, _fp, _fp, _i32, C.c_float, C.c_float, C.c_float,
                            _i32, _fp, _fp, _fp, _fp, _fp, _fp, _fp, _fp]),
+    "b2g_test_bn_ex": (_i32, [_vp, C.POINTER(TestBnOpts)] + [_fp] * 16),
     "b2g_test_net_shadow": (_i32, [_vp, _i32, _i32, _fp, _i64]),
     "b2g_test_net_noisy_operand": (_i32, [_vp, _i32, _i32, _fp, _i64]),
     "b2g_test_dropout": (_i32, [_vp, _i32, C.c_uint64, _i32, _i32, _i64, _i32, _i32, _i32, _i32, C.c_float, _fp, _fp, _fp, _fp]),

@@ -2484,6 +2484,67 @@ extern "C" int32_t b2g_test_bn(b2g_ctx* c, int32_t precision, int32_t path, int3
   return 0;
 }
 
+// Cross-replica BatchNorm on one device (include/b200gan.h b2g_test_bn_ex): every replica's accumulator kernels on its own rows, the
+// replicas' 128-bit words summed on the host as the ncclUint64 sum all-reduce sums them (uint64, modulo 2^64), the sum handed back to every
+// replica's buffer, the apply kernels run with replicas = R.
+extern "C" int32_t b2g_test_bn_ex(b2g_ctx* c, const b2g_test_bn_opts* o, const float* x, const float* eps_out, const float* gamma, const float* beta,
+                                  const float* run_mean, const float* run_var, const float* g_gamma0, const float* g_beta0, float* y, float* eps_in,
+                                  float* g_gamma, float* g_beta, float* g_mean, float* g_var, float* mean, float* invstd) {
+  if (!c || !o || !x || !eps_out || !gamma || !beta || !run_mean || !run_var || !g_gamma0 || !g_beta0 || !y || !eps_in || !g_gamma || !g_beta || !g_mean ||
+      !g_var || !mean || !invstd) return fail(B2G_ERR_ARG, "null");
+  const int R = o->replicas, groups = o->groups, rows = o->rows, C = o->C, path = o->path;
+  if (R < 1 || groups < 1 || rows < 1 || C < 1 || path < 1 || path > 2) return fail(B2G_ERR_ARG, "bad cross-replica BatchNorm test arguments");
+  if (!k_bn_vec_ok(PREC_BF16, C)) return fail(B2G_ERR_UNSUPPORTED, "the accumulator BatchNorm kernels need C %% 8 == 0 with 256 %% (C/8) == 0 (C = %d)", C);
+  if ((int64_t)R * groups * rows * C > 0x7fffffff) return fail(B2G_ERR_ARG, "the cross-replica BatchNorm test takes at most 2^31 - 1 elements");
+  CU(cudaSetDevice(c->device)); cudaStream_t s = c->stream;
+  const size_t per = (size_t)groups * rows * C, n = per * R, gc = (size_t)groups * C, na = k_bn_acc_elems(C, groups);
+  HookMem m(s, PREC_BF16);
+  float *d_gamma, *d_beta, *d_rm, *d_rv, *d_gg, *d_gb, *d_gm, *d_gv, *coef, *unit; void *tx, *te, *ty, *tei; unsigned long long *acc_f, *acc_b;
+  B2(m.upT(x, n, &tx)); B2(m.upT(eps_out, n, &te)); B2(m.dev(n, 2, &ty)); B2(m.dev(n, 2, &tei));
+  B2(m.upF(gamma, C, &d_gamma)); B2(m.upF(beta, C, &d_beta)); B2(m.upF(run_mean, C, &d_rm)); B2(m.upF(run_var, C, &d_rv));
+  B2(m.upF(nullptr, (size_t)R * C, &d_gg)); B2(m.upF(nullptr, (size_t)R * C, &d_gb)); B2(m.upF(nullptr, (size_t)R * C, &d_gm)); B2(m.upF(nullptr, (size_t)R * C, &d_gv));
+  for (int r = 0; r < R; ++r) {
+    CU(cudaMemcpyAsync(d_gg + (size_t)r * C, g_gamma0, 4 * C, cudaMemcpyHostToDevice, s)); CU(cudaMemcpyAsync(d_gb + (size_t)r * C, g_beta0, 4 * C, cudaMemcpyHostToDevice, s));
+  }
+  B2(m.upF(nullptr, 4 * gc * R, &coef)); B2(m.upF(nullptr, 4 * gc, &unit));
+  B2(m.dev(na * R, 8, (void**)&acc_f)); B2(m.dev(na * R, 8, (void**)&acc_b)); CU(cudaMemsetAsync(acc_f, 0, 8 * na * R, s)); CU(cudaMemsetAsync(acc_b, 0, 8 * na * R, s));
+  auto X = [&](void* t, int r) { return (void*)((__nv_bfloat16*)t + per * r); };
+  auto CF = [&](int r) { return coef + 4 * gc * r; };
+  std::vector<unsigned long long> words(na * R), sum(na);
+  auto allreduce = [&](unsigned long long* acc) -> int32_t {      // every replica's buffer <- the word-wise sum of all of them
+    CU(cudaMemcpyAsync(words.data(), acc, 8 * na * R, cudaMemcpyDeviceToHost, s)); CU(cudaStreamSynchronize(s));
+    std::fill(sum.begin(), sum.end(), 0ull);
+    for (int r = 0; r < R; ++r) for (size_t i = 0; i < na; ++i) sum[i] += words[na * r + i];
+    for (int r = 0; r < R; ++r) CU(cudaMemcpyAsync(acc + na * r, sum.data(), 8 * na, cudaMemcpyHostToDevice, s));
+    return 0;
+  };
+  const int want = o->want_param_grads ? 1 : 0;
+  for (int r = 0; r < R; ++r) k_bn_stats_acc(X(tx, r), rows, C, groups, acc_f + na * r, s);
+  B2(allreduce(acc_f));
+  for (int r = 0; r < R; ++r)
+    k_bn_apply_acc(X(tx, r), X(ty, r), rows, C, groups, acc_f + na * r, d_gamma, d_beta, o->act, o->alpha, o->eps, CF(r), d_rm, d_rv, d_gm + (size_t)r * C,
+                   d_gv + (size_t)r * C, o->decay, s, R);
+  if (path == 2)      // (scale 1, shift 0, mean 0, invstd 1): the accumulator receives (sum dy', sum dy'*z), as b2g_test_bn's path 2
+    for (int g = 0; g < groups; ++g) for (int k = 0; k < 4; ++k) k_fill_f32(unit + (size_t)(g * 4 + k) * C, (k == 0 || k == 3) ? 1.f : 0.f, C, s);
+  for (int r = 0; r < R; ++r) {
+    if (path == 1) k_bn_bwd_stats_acc(X(tx, r), X(te, r), rows, C, groups, CF(r), o->act, o->alpha, acc_b + na * r, s);
+    else k_bn_bwd_stats_acc(X(tx, r), X(te, r), rows, C, groups, unit, ACT_IDENTITY, 0.f, acc_b + na * r, s);
+  }
+  B2(allreduce(acc_b));
+  for (int r = 0; r < R; ++r)
+    k_bn_bwd_apply_acc(X(tx, r), X(te, r), X(tei, r), rows, C, groups, CF(r), o->act, o->alpha, path == 2 ? 1 : 0, acc_b + na * r, d_gg + (size_t)r * C,
+                       d_gb + (size_t)r * C, want, s, R);
+  B2(m.downT(y, ty, n)); B2(m.downT(eps_in, tei, n));
+  B2(m.downF(g_gamma, d_gg, (size_t)R * C)); B2(m.downF(g_beta, d_gb, (size_t)R * C)); B2(m.downF(g_mean, d_gm, (size_t)R * C)); B2(m.downF(g_var, d_gv, (size_t)R * C));
+  std::vector<float> cf(4 * gc * R); CU(cudaMemcpyAsync(cf.data(), coef, 4 * 4 * gc * R, cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s)); CHECK_KERNELS();
+  for (int r = 0; r < R; ++r) for (int g = 0; g < groups; ++g) {      // coef rows per group: scale, beta, mean, invstd
+    memcpy(mean + ((size_t)r * groups + g) * C, cf.data() + 4 * gc * r + (size_t)(g * 4 + 2) * C, 4 * C);
+    memcpy(invstd + ((size_t)r * groups + g) * C, cf.data() + 4 * gc * r + (size_t)(g * 4 + 3) * C, 4 * C);
+  }
+  return 0;
+}
+
 // One DropoutLayer forward (pass counter `pass`, advanced by the kernel) and backward on rows*h*w*c host tensors in NHWC element order,
 // through the kernels the training step uses.
 extern "C" int32_t b2g_test_dropout(b2g_ctx* c, int32_t precision, uint64_t seed, int32_t layer, int32_t rank, int64_t pass, int32_t rows, int32_t h, int32_t w, int32_t ch,
@@ -2821,6 +2882,40 @@ static int32_t test_ew_impl(b2g_ctx* c, int32_t precision, b2g_test_ew_opts* o, 
       B2(poison(res, 8));
       k_sumsq_segments(p, so, sl, coef, o->n_seg, res, s); ran();
       CU(cudaMemcpyAsync(&o->sumsq, res, 8, cudaMemcpyDeviceToHost, s));
+      break;
+    }
+    case B2G_EW_NCHW_TO_NHWC: case B2G_EW_NHWC_TO_NCHW: case B2G_EW_PERMUTE: {
+      const size_t n = (size_t)o->N * o->C * o->H * o->W;
+      if (!in0 || o->N < 1 || o->C < 1 || o->H < 1 || o->W < 1 || n > (size_t)lim || (o->op == B2G_EW_PERMUTE && o->groups != 0 && o->groups != 1))
+        return fail(B2G_ERR_ARG, "bad layout arguments");
+      const int HW = o->H * o->W;
+      if (o->op == B2G_EW_NCHW_TO_NHWC) {
+        float* x = nullptr; void* y = nullptr; B2(m.upF(in0, n, &x, off)); B2(m.dev(n, ts, &y, off)); B2(poison(y, ts * n));
+        k_nchw_f32_to_nhwc(prec, x, y, o->N, o->C, HW, s); ran();
+        B2(m.downT(out0, y, n));
+      } else if (o->op == B2G_EW_NHWC_TO_NCHW) {
+        void* x = nullptr; float* y = nullptr; B2(m.upT(in0, n, &x, off)); B2(m.upF(nullptr, n, &y, off)); B2(poison(y, 4 * n));
+        k_nhwc_to_nchw_f32(prec, x, y, o->N, o->C, HW, s); ran();
+        B2(m.downF(out0, y, n));
+      } else {
+        void *x = nullptr, *y = nullptr; B2(m.upT(in0, n, &x, off)); B2(m.dev(n, ts, &y, off)); B2(poison(y, ts * n));
+        k_permute(prec, x, y, o->N, o->C, HW, o->groups, s); ran();
+        B2(m.downT(out0, y, n));
+      }
+      break;
+    }
+    case B2G_EW_CAST_BF16: {      // the bf16 result comes back raw (widened on the host), and through the device widen the gradient payload uses
+      const size_t n = (size_t)o->n;
+      if (!in0 || o->n < 1 || o->n > lim) return fail(B2G_ERR_ARG, "bad CAST_BF16 arguments");
+      float *x = nullptr, *w = nullptr; __nv_bfloat16* y = nullptr;
+      B2(m.upF(in0, n, &x, off)); B2(m.dev(n, 2, (void**)&y, off)); B2(m.upF(nullptr, n, &w, off)); B2(poison(y, 2 * n)); B2(poison(w, 4 * n));
+      k_cast_f32_to_bf16(x, y, n, s); ran();
+      k_nhwc_to_nchw_f32(PREC_BF16, y, w, 1, 1, (int)n, s); ran();
+      if (out0) {
+        std::vector<uint16_t> h(n); CU(cudaMemcpyAsync(h.data(), y, 2 * n, cudaMemcpyDeviceToHost, s)); CU(cudaStreamSynchronize(s));
+        for (size_t i = 0; i < n; ++i) { const uint32_t u = (uint32_t)h[i] << 16; memcpy(out0 + i, &u, 4); }
+      }
+      B2(m.downF(out1, w, n));
       break;
     }
     default: return fail(B2G_ERR_ARG, "unknown op %d", o->op);

@@ -63,20 +63,24 @@ static inline int ew_blocks(size_t n, int per = 256) { const size_t cap = (size_
 void k_nchw_f32_to_nhwc(int prec, const float* src, void* dst, int N, int C, int HW, cudaStream_t s) {
   size_t n = (size_t)N * C * HW; if (!n) return;
   DISPATCH_PREC(prec, T, (launch_pdl(nchw_f32_to_nhwc_kernel<T>, dim3(ew_blocks(n)), dim3(256), (size_t)(0), s, src, (T*)dst, N, C, HW))); LAUNCHED();
+  g_ew_last_kernel = "nchw_f32_to_nhwc_kernel";
 }
 void k_nhwc_to_nchw_f32(int prec, const void* src, float* dst, int N, int C, int HW, cudaStream_t s) {
   size_t n = (size_t)N * C * HW; if (!n) return;
   DISPATCH_PREC(prec, T, (launch_pdl(nhwc_to_nchw_f32_kernel<T>, dim3(ew_blocks(n)), dim3(256), (size_t)(0), s, (const T*)src, dst, N, C, HW))); LAUNCHED();
+  g_ew_last_kernel = "nhwc_to_nchw_f32_kernel";
 }
 void k_permute(int prec, const void* src, void* dst, int N, int C, int HW, int to_nhwc, cudaStream_t s) {
   size_t n = (size_t)N * C * HW; if (!n) return;
   DISPATCH_PREC(prec, T, (launch_pdl(permute_kernel<T>, dim3(ew_blocks(n)), dim3(256), (size_t)(0), s, (const T*)src, (T*)dst, N, C, HW, to_nhwc))); LAUNCHED();
+  g_ew_last_kernel = "permute_kernel";
 }
 __global__ void cast_f32_to_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, size_t n) { pdl_enter();
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) dst[i] = __float2bfloat16_rn(src[i]);
 }
 void k_cast_f32_to_bf16(const float* src, __nv_bfloat16* dst, size_t n, cudaStream_t s) {
   if (!n) return; launch_pdl(cast_f32_to_bf16_kernel, dim3(ew_blocks(n)), dim3(256), (size_t)(0), s, src, dst, n); LAUNCHED();
+  g_ew_last_kernel = "cast_f32_to_bf16_kernel";
 }
 // ---------------------------------------------------------------- sliced column reductions ---------------
 // Thread idx -> (slice s = idx / C, channel c = idx % C); it sums rows s, s+S, s+2S, ... so that a warp

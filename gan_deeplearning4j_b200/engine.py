@@ -1025,13 +1025,27 @@ def test_conv_ex(ctx: Context, kind: int, geom: Dict[str, int], a, b, out_size: 
 
 
 def test_bn(ctx: Context, precision: int, path: int, x, eps_out, gamma, beta, run_mean, run_var, *, act: str = "identity", alpha: float = 0.0,
-            eps: float = 1e-5, decay: float = 0.9, g_gamma=None, g_beta=None, want_param_grads: bool = True):
+            eps: float = 1e-5, decay: float = 0.9, g_gamma=None, g_beta=None, want_param_grads: bool = True, replicas: int | None = None):
     """One BatchNorm(+activation) forward and backward through the training-step kernels (b2g_test_bn).  x, eps_out: [groups, rows, C].
     Returns a dict with y, eps_in ([groups, rows, C]), g_gamma, g_beta (accumulated into the given initial values), g_mean, g_var ([C]) and
-    mean, invstd ([groups, C])."""
+    mean, invstd ([groups, C]).
+    replicas=R: cross-replica BatchNorm as R data-parallel ranks run it (b2g_test_bn_ex; BF16, path 1 or 2).  x, eps_out: [R, groups, rows, C],
+    replica r's rows at [r]; every result gains a leading replica axis (g_gamma, g_beta, g_mean, g_var [R, C]; mean, invstd [R, groups, C])."""
     x, e = _f32(x), _f32(eps_out)
-    groups, rows, ch = x.shape
     par = [_f32(v).ravel() for v in (gamma, beta, run_mean, run_var)]
+    if replicas is not None:
+        R, groups, rows, ch = x.shape
+        if R != replicas or precision != BF16:
+            raise ValueError(f"replicas={replicas}: x must be [replicas, groups, rows, C] ({x.shape}) and the precision BF16")
+        o = _lib.TestBnOpts(path, replicas, groups, rows, ch, ACTS[act], alpha, eps, decay, int(want_param_grads))
+        g0 = [_f32(np.zeros(ch) if v is None else v).ravel() for v in (g_gamma, g_beta)]
+        r = {k: np.empty(x.shape, np.float32) for k in ("y", "eps_in")}
+        r.update({k: np.empty((R, ch), np.float32) for k in ("g_gamma", "g_beta", "g_mean", "g_var")})
+        r.update({k: np.empty((R, groups, ch), np.float32) for k in ("mean", "invstd")})
+        check(ctx.lib.b2g_test_bn_ex(ctx.h, C.byref(o), _fp(x), _fp(e), *[_fp(v) for v in par + g0],
+                                     *[_fp(r[k]) for k in ("y", "eps_in", "g_gamma", "g_beta", "g_mean", "g_var", "mean", "invstd")]))
+        return r
+    groups, rows, ch = x.shape
     r = {k: np.empty(x.shape, np.float32) for k in ("y", "eps_in")}
     r["g_gamma"] = _f32(np.zeros(ch) if g_gamma is None else g_gamma).copy()
     r["g_beta"] = _f32(np.zeros(ch) if g_beta is None else g_beta).copy()
@@ -1066,7 +1080,7 @@ def test_dropout(ctx: Context, precision: int, x, dy, p: float, *, seed: int = 6
 EW_OPS = {"reduce_splits": 0, "reduce_multi": 1, "colsum": 2, "xent": 3, "softmax_xent": 4, "act_fwd": 5, "act_bwd": 6, "maxpool": 7,
           "upsample": 8, "sumsq": 9, "loss": 10, "act_ext_fwd": 11, "act_ext_bwd": 12,
           "cnn_xent": 13, "cnn_softmax_xent": 14, "vertex_fwd": 15, "vertex_bwd": 16, "merge_fwd": 17, "merge_bwd": 18, "skip_add": 19,
-          "prelu_fwd": 20, "prelu_bwd": 21}
+          "prelu_fwd": 20, "prelu_bwd": 21, "nchw_to_nhwc": 22, "nhwc_to_nchw": 23, "permute": 24, "cast_bf16": 25}
 
 
 def test_ew(ctx: Context, precision: int, op: str, in0, in1=None, out_sizes=(0, 0, 0), *, act: str = "identity", jobs=None, segments=None,

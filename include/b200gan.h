@@ -805,6 +805,23 @@ int32_t b2g_test_hbm_kernels(b2g_net* net, int32_t rows, int32_t channels, int32
 int32_t b2g_test_bn(b2g_ctx* ctx, int32_t precision, int32_t path, int32_t groups, int32_t rows, int32_t C, const float* x, const float* eps_out,
                     const float* gamma, const float* beta, const float* run_mean, const float* run_var, int32_t act, float alpha, float eps, float decay,
                     int32_t want_param_grads, float* y, float* eps_in, float* g_gamma, float* g_beta, float* g_mean, float* g_var, float* mean, float* invstd);
+/* Cross-replica (sync) BatchNorm on one device: what `replicas` ranks of a data-parallel step run on the 128-bit accumulator kernels (path 1
+ * or 2 of b2g_test_bn, bf16, the same channel rule).  x, eps_out are [replicas][groups][rows][C]: replica r's rows, as rank r holds them.
+ * Each replica fills its own zeroed accumulators from its own rows (k_bn_stats_acc); the replicas' words are summed as uint64 modulo 2^64,
+ * as an ncclUint64 sum all-reduce leaves them; every replica then applies the sum with replicas = R (k_bn_apply_acc), and the backward runs
+ * the same way (k_bn_bwd_stats_acc, the word sum, k_bn_bwd_apply_acc).  Out, per replica: y, eps_in [R][groups][rows][C]; g_gamma / g_beta
+ * [R][C], each replica's row accumulated into from the shared initial value [C] (the (global sum) / R the gradient all-reduce sums back);
+ * g_mean / g_var [R][C]; mean / invstd [R][groups][C].  replicas = 1 runs exactly b2g_test_bn's launches. */
+typedef struct {
+  int32_t path;           /* 1: backward statistics from k_bn_bwd_stats_acc; 2: as the fused BatchNorm-backward epilogue leaves them */
+  int32_t replicas;       /* R >= 1 */
+  int32_t groups, rows, C;                /* rows per replica and group */
+  int32_t act; float alpha, eps, decay;
+  int32_t want_param_grads;
+} b2g_test_bn_opts;
+int32_t b2g_test_bn_ex(b2g_ctx* ctx, const b2g_test_bn_opts* opts, const float* x, const float* eps_out, const float* gamma, const float* beta,
+                       const float* run_mean, const float* run_var, const float* g_gamma0, const float* g_beta0, float* y, float* eps_in,
+                       float* g_gamma, float* g_beta, float* g_mean, float* g_var, float* mean, float* invstd);
 /* BF16 nets: the bf16 weight operand the next forward reads instead of the fp32 master, widened to fp32 (n = its element count).
  * which = 0: the straight copy of W in the internal [A][taps][B] order; 1: the packed [(py,px,c)][(dyr,dxc)][O] operand of the
  * pixel-shuffle transposed conv onto <= 4 channels (B2G_ERR_UNSUPPORTED if the layer has none). */
@@ -862,13 +879,21 @@ int32_t b2g_test_dropout_kind(b2g_ctx* ctx, int32_t precision, int32_t kind, uin
  *   PRELU_BWD      in0 [x [n] T | alpha [K] fp32], in1 dy [n] T                       -> out0 dx T (dy's buffer, in place; NULL: not written),
  *                                                                                        out1 dalpha [K] (NULL: no slope gradient), summed by
  *                                                                                        one reduce-list launch
+ * Layout conversion and casts (the map N x C x HW, HW = H * W):
+ *   NCHW_TO_NHWC   in0 x [N][C][HW] fp32                                              -> out0 [N][HW][C] T
+ *   NHWC_TO_NCHW   in0 x [N][HW][C] T                                                 -> out0 [N][C][HW] fp32
+ *   PERMUTE        in0 x T, groups = 1: [N][C][HW] -> [N][HW][C], 0: the reverse      -> out0 T
+ *   CAST_BF16      in0 x [n] fp32 (any precision)                                     -> out0 the bf16 result, widened on the host, out1 the
+ *                                                                                        same widened on the device (nhwc_to_nchw_f32 at
+ *                                                                                        1 x 1 x n, the bf16 gradient payload's round trip)
  * Every output buffer not asked for may be NULL. */
 typedef enum {
   B2G_EW_REDUCE_SPLITS = 0, B2G_EW_REDUCE_MULTI = 1, B2G_EW_COLSUM = 2, B2G_EW_XENT = 3, B2G_EW_SOFTMAX_XENT = 4,
   B2G_EW_ACT_FWD = 5, B2G_EW_ACT_BWD = 6, B2G_EW_MAXPOOL = 7, B2G_EW_UPSAMPLE = 8, B2G_EW_SUMSQ = 9, B2G_EW_LOSS = 10,
   B2G_EW_ACT_EXT_FWD = 11, B2G_EW_ACT_EXT_BWD = 12, B2G_EW_CNN_XENT = 13, B2G_EW_CNN_SOFTMAX_XENT = 14,
   B2G_EW_VERTEX_FWD = 15, B2G_EW_VERTEX_BWD = 16, B2G_EW_MERGE_FWD = 17, B2G_EW_MERGE_BWD = 18, B2G_EW_SKIP_ADD = 19,
-  B2G_EW_PRELU_FWD = 20, B2G_EW_PRELU_BWD = 21
+  B2G_EW_PRELU_FWD = 20, B2G_EW_PRELU_BWD = 21,
+  B2G_EW_NCHW_TO_NHWC = 22, B2G_EW_NHWC_TO_NCHW = 23, B2G_EW_PERMUTE = 24, B2G_EW_CAST_BF16 = 25
 } b2g_ew_op;
 typedef struct {          /* one split-K sum of a reduce list: dst[i] = sum_s src[s*stride + i], i < n, all offsets in elements of in0 */
   int64_t n, stride, src_off, dst_off;
@@ -877,11 +902,11 @@ typedef struct {          /* one split-K sum of a reduce list: dst[i] = sum_s sr
 } b2g_ew_reduce_job;
 typedef struct {
   int32_t op;             /* b2g_ew_op */
-  int64_t n;              /* REDUCE_SPLITS outputs, REDUCE_MULTI buffer length, ACT_* / SUMSQ elements */
+  int64_t n;              /* REDUCE_SPLITS outputs, REDUCE_MULTI buffer length, ACT_* / SUMSQ / CAST_BF16 elements */
   int32_t rows, cols;     /* COLSUM rows x channels; XENT rows per group; SOFTMAX_XENT rows x classes; CNN_* pixels per group x channels */
-  int32_t groups;         /* XENT, LOSS, CNN_* */
+  int32_t groups;         /* XENT, LOSS, CNN_*; PERMUTE: 1 = to NHWC */
   int32_t splits; int64_t stride;       /* REDUCE_SPLITS */
-  int32_t N, H, W, C, KH, KW, SH, SW;  /* MAXPOOL input and window; UPSAMPLE input and factor KH */
+  int32_t N, H, W, C, KH, KW, SH, SW;  /* MAXPOOL input and window; UPSAMPLE input and factor KH; layout ops: the map */
   int32_t act; float alpha;             /* ACT_*: b2g activation */
   float clip_eps;                       /* XENT: 0 = BCE with logits */
   int32_t offset;         /* every device operand starts this many elements past a 256-byte aligned address (reaches the misaligned fallbacks) */

@@ -57,7 +57,9 @@ def test_struct_layouts_match_the_c_header(tmp_path):
                     'printf("%zu %zu\\n", offsetof(b2g_test_conv_opts,param_offset), offsetof(b2g_test_conv_opts,splits));'
                     'printf("%zu %zu %zu\\n", sizeof(b2g_ew_reduce_job), offsetof(b2g_ew_reduce_job,splits), offsetof(b2g_ew_reduce_job,wide));'
                     + "".join(f'printf("%zu\\n", offsetof(b2g_test_ew_opts,{f}));' for f, _ in _lib.TestEwOpts._fields_) +
-                    'printf("%zu\\n", sizeof(b2g_test_ew_opts));return 0;}')
+                    'printf("%zu\\n", sizeof(b2g_test_ew_opts));'
+                    + "".join(f'printf("%zu\\n", offsetof(b2g_test_bn_opts,{f}));' for f, _ in _lib.TestBnOpts._fields_) +
+                    'printf("%zu\\n", sizeof(b2g_test_bn_opts));return 0;}')
     exe = tmp_path / "layout"
     subprocess.run(["gcc", "-I", os.path.join(ROOT, "include"), str(prog), "-o", str(exe)], check=True)
     got = [int(v) for v in subprocess.run([str(exe)], capture_output=True, text=True).stdout.split()]
@@ -66,7 +68,8 @@ def test_struct_layouts_match_the_c_header(tmp_path):
                    C.sizeof(T), T.stats.offset, T.kernel.offset, T.bn.offset, T.max_ctas.offset, T.poison.offset, T.w_mn.offset,
                    T.per_tap.offset, T.slab.offset, T.defer.offset, T.db.offset, T.param_offset.offset, T.splits.offset,
                    C.sizeof(J), J.splits.offset, J.wide.offset] + \
-        [getattr(E, f).offset for f, _ in E._fields_] + [C.sizeof(E)]
+        [getattr(E, f).offset for f, _ in E._fields_] + [C.sizeof(E)] + \
+        [getattr(_lib.TestBnOpts, f).offset for f, _ in _lib.TestBnOpts._fields_] + [C.sizeof(_lib.TestBnOpts)]
     assert (T.stats.offset, T.kernel.offset, T.bn.offset, T.slab.offset) == (56, 64, 128, 148)       # the fields older callers fill keep their offsets
     assert (T.defer.offset, T.db.offset) == (152, 160)
     assert (T.param_offset.offset, T.splits.offset, C.sizeof(T)) == (168, 172, 176)                 # appended after db

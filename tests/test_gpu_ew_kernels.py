@@ -414,3 +414,96 @@ def test_sumsq_segments_against_float64(b200):
     assert info["kernel"] == "sumsq_segments_kernel"
     ref = math.fsum(float(c) * math.fsum((p[o:o + k].astype(np.float64) ** 2).tolist()) for o, k, c in zip(off, ln, coef))
     assert abs(info["sumsq"] - ref) <= 1e-12 * abs(ref), (info["sumsq"], ref)
+
+
+# ---------------------------------------------------------------- layout conversion and the bf16 cast ---------------------------------------
+def _pass_elems(ctx):
+    """Elements one grid-stride pass of the layout and cast kernels covers: ew_blocks caps their grid at 16 blocks of 256 threads per SM."""
+    return 16 * ctx.device_info()["sm_count"] * 256
+
+
+LAYOUT_SHAPES = [
+    # N, C, H, W (HW = H * W), offset
+    (1, 1, 1, 1, 0), (1, 5, 1, 1, 0), (3, 1, 7, 5, 0), (1, 7, 3, 3, 1), (2, 3, 5, 7, 3), (4, 64, 8, 8, 0),
+    (7, 131, 43, 47, 0), (7, 131, 43, 47, 1),      # 1.85M elements: more than three grid-stride passes on an H100
+]
+
+
+@pytest.mark.parametrize("prec", PRECS)
+@pytest.mark.parametrize("shape", LAYOUT_SHAPES, ids=[f"{s[0]}x{s[1]}x{s[2]}x{s[3]}-off{s[4]}" for s in LAYOUT_SHAPES])
+def test_layout_kernels_exact(b200, prec, shape):
+    """NCHW fp32 -> NHWC T (input staging), NHWC T -> NCHW fp32 (output read-back) and the T -> T permutes of the FF <-> CNN preprocessors: numpy's
+    transpose of the stored values, bit for bit, every element written (NaN-poisoned outputs)."""
+    b, ctx = b200
+    N, C, H, W, offset = shape
+    HW, n = H * W, N * C * H * W
+    if n > 1_000_000:
+        assert n > 3 * _pass_elems(ctx)
+    rng = np.random.default_rng(n + offset)
+    x = (rng.standard_normal(n) * np.exp(rng.uniform(-8, 8, n))).astype(np.float32)        # many binades: a misplaced element shows
+    nchw, nhwc = x.reshape(N, C, HW), x.reshape(N, HW, C)
+    geom = dict(N=N, C=C, H=H, W=W, offset=offset, poison=True)
+    P = _P(b, prec)
+    (got, _, _), info = b.test_ew(ctx, P, "nchw_to_nhwc", x, None, (n, 0, 0), **geom)
+    assert info["kernel"] == "nchw_f32_to_nhwc_kernel"
+    assert np.array_equal(_bits(got), _bits(_rnd(prec, nchw.transpose(0, 2, 1)).ravel()))
+    (got, _, _), info = b.test_ew(ctx, P, "nhwc_to_nchw", x, None, (n, 0, 0), **geom)
+    assert info["kernel"] == "nhwc_to_nchw_f32_kernel"
+    assert np.array_equal(_bits(got), _bits(_rnd(prec, nhwc).transpose(0, 2, 1).ravel()))
+    for to_nhwc, want in ((1, _rnd(prec, nchw).transpose(0, 2, 1)), (0, _rnd(prec, nhwc).transpose(0, 2, 1))):
+        (got, _, _), info = b.test_ew(ctx, P, "permute", x, None, (n, 0, 0), groups=to_nhwc, **geom)
+        assert info["kernel"] == "permute_kernel"
+        assert np.array_equal(_bits(got), _bits(want.ravel())), f"permute to_nhwc={to_nhwc}"
+
+
+def _cast_specials():
+    """fp32 bit patterns where a bf16 rounding can go wrong: exact ties between bf16 neighbours (even and odd upper halves, both signs), one ulp
+    either side of a tie, +-0, subnormals (the largest rounds up to the smallest normal), the largest finite values (round to inf), +-inf and NaNs
+    (quiet, and signalling ones whose payload is only in the low 16 bits)"""
+    hi = np.array([0x3F80, 0x3F81, 0x4049, 0x404A, 0x7F7E, 0x0080, 0x0001, 0x4B00], np.uint32)
+    ties = [(h << 16) | lo for h in hi for lo in (0x8000, 0x7FFF, 0x8001, 0x0000, 0xFFFF)]
+    bits = ties + [0x00000000, 0x00000001, 0x00008000, 0x00018000, 0x007FFFFF, 0x00800000, 0x7F7FFFFF, 0x7F7F7FFF, 0x7F800000,
+                   0x7FC00000, 0x7F800001, 0x7F808000, 0x7FFFFFFF]
+    bits = np.array(bits, np.uint32)
+    return np.concatenate([bits, bits | np.uint32(0x80000000)]).view(np.float32)
+
+
+def _bf16_rne(x):
+    """fp32 -> bf16 -> fp32, round to nearest even, in integer arithmetic on the bits (NaNs excepted): helpers.bf16_round's rounding, without
+    depending on which conversion the host CPU's torch build uses for subnormals"""
+    u = _bits(x).astype(np.uint64)
+    r = ((u + 0x7FFF + ((u >> 16) & 1)) >> 16) << 16
+    return r.astype(np.uint32).view(np.float32)
+
+
+def _check_cast(x, got, round_trip):
+    want = _bf16_rne(x)
+    nan = np.isnan(x)
+    normal = (np.abs(x) >= 2.0 ** -126) & (np.abs(x) < 1e38)          # the same rounding as helpers.bf16_round where no host can differ
+    assert np.array_equal(_bits(bf16_round(x[normal])), _bits(want[normal]))
+    assert np.isnan(got[nan]).all(), "a NaN must stay NaN"
+    assert np.array_equal(_bits(got[~nan]), _bits(want[~nan])), f"{int((_bits(got[~nan]) != _bits(want[~nan])).sum())} elements not rounded to nearest even"
+    assert np.array_equal(_bits(round_trip), _bits(got)), "the device widen of the bf16 payload differs from its bits"
+
+
+@pytest.mark.parametrize("case", ["specials", "random-bits", "wrap"])
+@pytest.mark.parametrize("offset", [0, 1])
+def test_cast_f32_to_bf16_rounds_to_nearest_even(b200, case, offset):
+    """k_cast_f32_to_bf16 (the bf16 gradient payload, the hooks' bf16 uploads) against round-to-nearest-even, and the payload's widen back to fp32
+    through nhwc_to_nchw_f32_kernel at 1 x 1 x n: the cast's bits, NaN-poisoned outputs, n not a multiple of 4 or 8."""
+    b, ctx = b200
+    rng = np.random.default_rng(len(case) + offset)
+    if case == "specials":
+        x = _cast_specials()
+    elif case == "random-bits":        # every binade, subnormals, infinities and NaNs in proportion to their bit patterns
+        x = rng.integers(0, 2 ** 32, 12347, dtype=np.uint64).astype(np.uint32).view(np.float32)
+    else:                              # more than two grid-stride passes, the specials spread through every pass
+        n = 2 * _pass_elems(ctx) + 4099
+        x = (rng.standard_normal(n) * np.exp(rng.uniform(-30, 30, n))).astype(np.float32)
+        sp = _cast_specials()
+        x[rng.choice(n, 40 * sp.size, replace=False)] = np.tile(sp, 40)
+    n = x.size
+    assert n % 4 != 0
+    (got, rt, _), info = b.test_ew(ctx, b.BF16, "cast_bf16", x, None, (n, n, 0), n=n, offset=offset, poison=True)
+    assert info["kernel"] == "cast_f32_to_bf16_kernel,nhwc_to_nchw_f32_kernel"
+    _check_cast(x, got, rt)
