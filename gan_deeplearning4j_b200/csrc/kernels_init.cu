@@ -1,6 +1,6 @@
 // kernels_init.cu -- weight initialization (DL4J WeightInit / Distribution / biasInit): a layer's W drawn on the device from the counter-based
 // generator, element by element at its DL4J view index, and its bias filled.  Definitions: include/b200gan.h b2g_weight_init; restatement:
-// tests/weight_init_ref.py.  A translation unit of its own, so that no other kernel's generated code changes.
+// oracle/dl4j_oracle.py (weight_init_draw).  A translation unit of its own, so that no other kernel's generated code changes.
 #include <stdint.h>
 #include <algorithm>
 #include "kernels.h"

@@ -33,7 +33,15 @@ include/b200gan.h):
   * activations of b2g_activation codes 5-16       -> ``forward`` / ``derivative`` (reached through ``act_forward`` / ``act_backward``)
   * losses of b2g_loss codes 2-8                   -> ``score_and_grad`` (``Output`` / ``LossLayer`` with a loss other than XENT)
   * SubsamplingLayer AVG / SUM / PNORM, GlobalPoolingLayer (b2g_pooling)  -> ``Subsampling`` / ``GlobalPooling``
-  * DropoutLayer (B2G_LAYER_DROPOUT; the mask is the library's Philox draw) -> ``Dropout``, ``dropout_mask``
+  * DropoutLayer (B2G_LAYER_DROPOUT; b2g_dropout_kind: Dropout, GaussianDropout, GaussianNoise, AlphaDropout, SpatialDropout; scheduled
+    values; the draws are the library's Philox draws)  -> ``Dropout``, ``dropout_mask``, ``dropout_normals``, ``spatial_mask``,
+                                                          ``Net.set_dropout_schedule``
+  * weight noise (b2g_weight_noise: DropConnect, WeightNoise)  -> ``noisy_operands``, ``Net.set_weight_noise``
+  * weight initialization (b2g_weight_init)        -> ``resolve``, ``weights``, ``init_layer``
+  * l1, l2, l1Bias, l2Bias (b2g_regularization)    -> ``Net.layer_regularization``, ``Net.reg_coefs``, ``Net.calc_l1`` / ``calc_l2``
+  * PReLULayer (B2G_LAYER_PRELU)                   -> ``PReLU``
+  * per-output loss weights and labels masks (b2g_loss)  -> ``rows_score_and_grad``, ``Net.set_loss_weights``, the ``mask`` of
+                                                            ``Net.fit`` / ``compute_gradient_and_score`` and ``gan_step``'s three
   * the updaters of b2g_updater                    -> ``UpdaterCfg``, ``init_state``, ``update``
   * L2 gradient normalization                      -> ``Net.set_gradient_normalization``, ``normalize``
   * learning-rate schedules (ISchedule)            -> ``Net.set_lr_schedule``, ``value``, ``lr_at``
@@ -90,6 +98,30 @@ class Quirks:
     # weight constraints
     constraint_eps: float = 1e-6                  # BaseConstraint.DEFAULT_EPSILON
     unit_norm_zero_group_unchanged: bool = True   # UnitNorm leaves an all-zero group as it is (DL4J: 0/0 = NaN)
+    # the library's Box-Muller: u = ((x_even >> 9) + 0.5) 2^-23 and v = (x_odd >> 8) 2^-24, so |z| <= sqrt(-2 ln 2^-24); DL4J draws its own
+    box_muller_u_shift: int = 9
+    box_muller_v_shift: int = 8
+    # weight noise
+    dropconnect_inverted: bool = False            # DropConnect applies ND4J's DropOut op, not DropOutInverted: W' = keep ? W : 0, not / p
+    # DL4J's `train && isWeight || (applyToBias && isBias)` also perturbs biases at inference; the library perturbs nothing there (a deviation)
+    noise_on_bias_in_inference: bool = False
+    # weight initialization
+    lecun_uniform_three_over_sqrt: bool = True    # LECUN_UNIFORM's bound 3 / sqrt(fanIn), recalled from WeightInitUtil (not sqrt(3 / fanIn))
+    var_scaling_uniform_three_over_sqrt: bool = True  # VAR_SCALING_UNIFORM_FAN_{IN,OUT,AVG} bounds 3 / sqrt(fan), recalled the same way
+    xavier_legacy_shape01: bool = True            # XAVIER_LEGACY's std 1 / sqrt(shape[0] + shape[1]) = 1 / sqrt(nIn + nOut) for every GEMM W
+    truncation_sigmas: float = 2.0                # TruncatedNormalDistribution and VAR_SCALING_NORMAL_*: values beyond this many std are redrawn
+    normal_scaled_by_fan_in: bool = True          # NORMAL is N(0, 1 / sqrt(fanIn)), not unit variance
+    # regularization
+    batchnorm_unregularized: bool = True          # beta3's BatchNormalization.getL1ByParam / getL2ByParam return 0 for all four parameters
+    # PReLULayer
+    prelu_alpha_init_zero: bool = True            # PReLULayer.Builder sets weightInit(ZERO) itself (a new PReLU is a ReLU), not the global init
+    prelu_alpha_regularized: bool = True          # "W" is a weight parameter: the layer's l1 / l2 (and the global builder's) regularize alpha
+    prelu_zero_is_negative: bool = False          # libnd4j prelu compares x < 0: x = +-0 is not negative (dy passes, no slope term)
+    # loss weights and labels masks
+    masked_score_per_minibatch: bool = True       # BaseOutputLayer.computeScore divides the masked sum by the minibatch, not the unmasked count
+    mcxent_per_output_mask_refused: bool = True   # LossMCXENT throws "Per output masking for MCXENT + softmax: not supported"
+    weightless_losses: tuple = ("hinge", "squared_hinge", "wasserstein")     # the losses without a weights constructor in beta3
+    cnn_mask_channels: tuple = ("one", "all")     # a CnnLossLayer's NCHW masks: one value per pixel [N, 1, H, W], or one per output [N, C, H, W]
 
 
 DEFAULT_QUIRKS = Quirks()
@@ -490,12 +522,14 @@ def apply_constraint(w: np.ndarray, c: Dict, q: Quirks = DEFAULT_QUIRKS) -> np.n
 
 def constraints_by_param(layer: Layer, constraints: Sequence[Dict]) -> Dict[str, List[Dict]]:
     """One layer's constraints as parameter name -> the ordered list its tensor runs (DL4J initializeConstraints): on a layer with parameters
-    that is not frozen, "weights" reaches W, "bias" b and "all" every parameter, where the layer has them; each list runs the all-parameter
-    constraints, then the weight, then the bias ones, each in the order given.  ValueError for an unknown target or kind."""
+    that is not frozen, "weights" reaches W, "bias" b and "all" every parameter, where the layer has them (a PReLU's alpha takes none: the
+    library refuses them); each list runs the all-parameter constraints, then the weight, then the bias ones, each in the order given.
+    ValueError for an unknown target or kind."""
     for c in constraints:
         if c.get("on", "weights") not in CONSTRAINT_ON or c.get("constraint") not in CONSTRAINT_KINDS:
             raise ValueError(f"constraint {c!r}: targets {CONSTRAINT_ON}, kinds {CONSTRAINT_KINDS}")
-    names = [p for p, _, _ in layer.param_specs()] if layer.has_params and not getattr(layer, "frozen", False) else []
+    live = layer.has_params and not getattr(layer, "frozen", False) and not isinstance(layer, PReLU)
+    names = [p for p, _, _ in layer.param_specs()] if live else []
     reach = {"all": names, "weights": [p for p in names if p == "W"], "bias": [p for p in names if p == "b"]}
     out: Dict[str, List[Dict]] = {}
     for c in sorted(constraints, key=lambda c: CONSTRAINT_ON.index(c.get("on", "weights"))):    # stable: the given order within a target
@@ -539,8 +573,11 @@ def col2im(cols: np.ndarray, x_shape, kh, kw, sh, sw, ph, pw) -> np.ndarray:
 # --------------------------------------------------------------------------------------------------
 class Layer:
     name: str = ""
+    index: int = 0                  # the layer's chain index in the CUDA library's layer array (its spec position): the draws' L
     updater: Optional[UpdaterCfg] = None
     l2: float = 0.0
+    weight_noise: Optional[Dict] = None     # a conv, deconv or dense layer's DropConnect / WeightNoise
+    noisy: Optional[Dict] = None            # its W' (and b') of the current train-mode pass, in W's shape, or None
     has_params = False
     q: Quirks = DEFAULT_QUIRKS      # a Net gives its quirks to the layers that have none of their own
 
@@ -548,7 +585,12 @@ class Layer:
         return []
 
     def l2_names(self) -> Tuple[str, ...]:
+        """The parameters the layer's l2 reaches."""
         return ()
+
+    def _p(self, name):
+        """The parameter a forward or an input gradient reads: the pass's noisy operand if it has one."""
+        return self.noisy[name] if self.noisy is not None and name in self.noisy else self.params[name]
 
     def noop_names(self) -> Tuple[str, ...]:
         return ()
@@ -601,10 +643,10 @@ class Conv2D(Layer):
         oh, ow = cols.shape[1], cols.shape[2]
         self._x_shape = x.shape
         self._cols2d = np.ascontiguousarray(cols).reshape(n * oh * ow, -1)
-        w2d = self.params["W"].reshape(self.n_out, -1)
+        w2d = self._p("W").reshape(self.n_out, -1)
         z2d = self._cols2d @ w2d.T
         if self.has_bias:
-            z2d = z2d + self.params["b"]
+            z2d = z2d + self._p("b")
         self._z = z2d.reshape(n, oh, ow, self.n_out).transpose(0, 3, 1, 2)
         return _layer_act_forward(self.activation, self._z, self.alpha, self.q)
 
@@ -615,7 +657,7 @@ class Conv2D(Layer):
         self.grads["W"] = (d2d.T @ self._cols2d).reshape(self.params["W"].shape)
         if self.has_bias:
             self.grads["b"] = d2d.sum(0)
-        w2d = self.params["W"].reshape(o, -1)
+        w2d = self._p("W").reshape(o, -1)
         dcols = (d2d @ w2d).reshape(n, oh, ow, self.n_in, *self.k)
         return col2im(dcols, self._x_shape, *self.k, *self.s, *self.p)
 
@@ -658,11 +700,11 @@ class Deconv2D(Layer):
         self._x2d = x.transpose(0, 2, 3, 1).reshape(-1, c)
         self._x_shape = x.shape
         osh = self.out_shape(x.shape)
-        w2d = self.params["W"].reshape(self.n_in, -1)               # [Cin, Cout*kH*kW]
+        w2d = self._p("W").reshape(self.n_in, -1)               # [Cin, Cout*kH*kW]
         cols = (self._x2d @ w2d).reshape(n, h, w, self.n_out, *self.k)
         z = col2im(cols, osh, *self.k, *self.s, *self.p)
         if self.has_bias:
-            z = z + self.params["b"][None, :, None, None]
+            z = z + self._p("b")[None, :, None, None]
         self._z = z
         return _layer_act_forward(self.activation, z, self.alpha, self.q)
 
@@ -673,7 +715,7 @@ class Deconv2D(Layer):
         self.grads["W"] = (self._x2d.T @ dcols).reshape(self.params["W"].shape)
         if self.has_bias:
             self.grads["b"] = delta.sum((0, 2, 3))
-        w2d = self.params["W"].reshape(self.n_in, -1)
+        w2d = self._p("W").reshape(self.n_in, -1)
         return (dcols @ w2d.T).reshape(n, h, w, c).transpose(0, 3, 1, 2)
 
 
@@ -693,6 +735,9 @@ class Dense(Layer):
     def l2_names(self):
         return ("W",)
 
+    def fans(self):
+        return self.n_in, self.n_out
+
     def init(self, rng, dtype):
         super().init(rng, dtype)
         self.params["W"] = (rng.standard_normal((self.n_in, self.n_out)) * np.sqrt(2.0 / (self.n_in + self.n_out))).astype(dtype)
@@ -704,9 +749,9 @@ class Dense(Layer):
 
     def forward(self, x, train):
         self._x = x
-        self._z = x @ self.params["W"]
+        self._z = x @ self._p("W")
         if self.has_bias:
-            self._z = self._z + self.params["b"]
+            self._z = self._z + self._p("b")
         return _layer_act_forward(self.activation, self._z, self.alpha, self.q)
 
     def backward(self, eps):
@@ -715,7 +760,10 @@ class Dense(Layer):
         self.grads["W"] = self._x.T @ delta
         if self.has_bias:
             self.grads["b"] = delta.sum(0)
-        return delta @ self.params["W"].T
+        return delta @ self._p("W").T
+
+
+GEMM = (Conv2D, Deconv2D, Dense)          # the layers with a W: Output and OutputSoftmax are Dense
 
 
 class BatchNorm(Layer):
@@ -787,6 +835,51 @@ class ActivationLayer(Layer):
 
     def backward(self, eps):
         return _layer_act_backward(self.activation, self._z, eps, self.alpha, self.q)
+
+
+class PReLU(Layer):
+    """PReLULayer.Builder().inputShape(in_shape).sharedAxes(shared_axes) (B2G_LAYER_PRELU): in_shape (C, H, W) or (F,), shared_axes DL4J's
+    1-based axes.
+      forward   y = x < 0 ? alpha * x : x
+      backward  dx = x < 0 ? alpha * eps : eps;  dalpha = sum over the minibatch and the shared axes of (x < 0 ? x * eps : 0)
+    alpha ("W") has DL4J's weight shape: in_shape with every shared axis of extent 1, so in the NCHW layout it broadcasts over the minibatch
+    and the shared axes as it is.  A FrozenLayer PReLU is the same function in both modes and passes an input gradient (Net's backward walk
+    goes through it)."""
+    has_params = True
+
+    def __init__(self, in_shape, shared_axes=(), updater=None, l2=0.0, name=""):
+        self.in_shape = tuple(int(d) for d in in_shape)
+        self.shared = tuple(sorted({int(a) for a in shared_axes}))
+        if any(a < 1 or a > len(self.in_shape) for a in self.shared):
+            raise ValueError(f"prelu {name!r}: shared axes {self.shared} outside the input's {len(self.in_shape)} dimension(s)")
+        self.alpha_shape = tuple(1 if i + 1 in self.shared else d for i, d in enumerate(self.in_shape))
+        self.updater, self.l2, self.name = updater, l2, name
+
+    def param_specs(self):
+        return [("W", self.alpha_shape, "c")]
+
+    def l2_names(self):
+        return ("W",) if self.q.prelu_alpha_regularized else ()
+
+    def init(self, rng, dtype):
+        super().init(rng, dtype)
+        if not self.q.prelu_alpha_init_zero:
+            raise NotImplementedError("only beta3's ZERO initial alpha is restated")
+        self.params["W"] = np.zeros(self.alpha_shape, dtype)
+
+    def _neg(self, x):
+        return x <= 0 if self.q.prelu_zero_is_negative else x < 0
+
+    def forward(self, x, train):
+        self._x = x
+        return np.where(self._neg(x), self.params["W"][None] * x, x)
+
+    def backward(self, eps):
+        x, neg = self._x, self._neg(self._x)
+        if not getattr(self, "frozen", False):
+            axes = (0,) + self.shared           # DL4J axis a is array axis a of the [N, ...] activation
+            self.grads["W"] = np.where(neg, x * eps, 0.0).sum(axis=axes, keepdims=True).reshape(self.alpha_shape)
+        return np.where(neg, self.params["W"][None] * eps, eps)
 
 
 class MaxPool(Layer):
@@ -994,10 +1087,18 @@ class Reshape(Layer):
         return eps.reshape(self._in_shape)
 
 
-# DropoutLayer.Builder(p), p = the RETAIN probability: training forward y = x * m, m = 1/p with probability p else 0; backward dx = dy * m;
-# inference and a FrozenLayer are the identity.  ND4J's random stream cannot be restated, so the mask is the CUDA library's own definition
-# (include/b200gan.h, B2G_LAYER_DROPOUT), restated exactly: parity with DL4J holds in distribution, with the library element for element.
+# --------------------------------------------------------------------------------------------------
+# The library's random draws.  ND4J's random stream cannot be restated, so every draw is the CUDA library's own definition (include/b200gan.h),
+# restated exactly: parity with DL4J holds in distribution, with the library element for element.  Draw index j takes word j & 3 of
+# Philox4x32-10(ctr = {j >> 2, c1, c2, c3}, key = {lo32(S), hi32(S)}), S = the net's seed (0 -> 666), with counter words 1-3
+#   DropoutLayers and weight noise  {lo32(P), hi32(P), L | r << 16}   (pass P, layer L, rank r < 2^15)
+#   weight initialization           {k, 0, L | 2^31}                  (round k)
+# so the two streams never share a counter.  A keep bit is x < floor(p 2^32); a normal pairs words (x0, x1) -> z0, z1 and (x2, x3) -> z2, z3
+# through box_muller; a uniform is fmaf(upper - lower, (x >> 8) 2^-24, lower).
+# --------------------------------------------------------------------------------------------------
 _M32 = np.uint64(0xFFFFFFFF)
+WEIGHT_INIT_TAG = 0x80000000
+Z_MAX = math.sqrt(-2.0 * math.log(2.0 ** -24))          # the largest |z| box_muller gives
 
 
 def philox4x32_10(ctr, key):
@@ -1013,35 +1114,138 @@ def philox4x32_10(ctr, key):
     return [v.astype(np.uint32) for v in c]
 
 
+def philox_words(seed, j0, j1, c1, c2, c3):
+    """The word of each draw index j in [j0, j1) (uint32): word j & 3 of Philox4x32-10({j >> 2, c1, c2, c3}, {lo32(S), hi32(S)})."""
+    seed = int(seed) or 666
+    g = np.arange(j0 >> 2, ((j1 - 1) >> 2) + 1, dtype=np.uint64)
+    words = np.stack(philox4x32_10((g, c1, c2, c3), (seed & 0xFFFFFFFF, seed >> 32)), -1).ravel()
+    return words[j0 - 4 * (j0 >> 2):][:j1 - j0]
+
+
+def dropout_counter(rank, layer, pass_):
+    """Counter words 1-3 of the DropoutLayer and weight-noise draws: {lo32(P), hi32(P), L | r << 16}."""
+    pass_ = int(pass_)
+    return pass_ & 0xFFFFFFFF, pass_ >> 32, int(layer) | (int(rank) << 16)
+
+
+def keep_bits(words, p):
+    """x < floor(p 2^32) of each word, p taken as fp32."""
+    return words < np.uint64(math.floor(float(np.float32(p)) * 2.0 ** 32))
+
+
+def box_muller(x_even, x_odd, q: Quirks = DEFAULT_QUIRKS):
+    """float64 normals (z_even, z_odd) of Philox word pairs, from the library's exact u and v."""
+    u = ((np.asarray(x_even, np.uint64) >> np.uint64(q.box_muller_u_shift)).astype(np.float64) + 0.5) * 2.0 ** -23
+    v = (np.asarray(x_odd, np.uint64) >> np.uint64(q.box_muller_v_shift)).astype(np.float64) * 2.0 ** -24
+    r = np.sqrt(-2.0 * np.log(u))
+    return r * np.cos(2 * np.pi * v), r * np.sin(2 * np.pi * v)
+
+
+def normals(words, q: Quirks = DEFAULT_QUIRKS):
+    """The float64 normal of each word of whole counters (a multiple of 4 words): pair (x0, x1) -> z0, z1, pair (x2, x3) -> z2, z3."""
+    w4 = words.reshape(-1, 4)
+    z = np.empty(w4.shape)
+    z[:, 0], z[:, 1] = box_muller(w4[:, 0], w4[:, 1], q)
+    z[:, 2], z[:, 3] = box_muller(w4[:, 2], w4[:, 3], q)
+    return z.ravel()
+
+
+def fmaf(a, b, c):
+    """fp32 fmaf(a, b, c) for fp32 a, c and float64 b: exact in double where a * b fits (uniform draws), one rounding to fp32."""
+    return (np.float64(np.float32(a)) * np.asarray(b, np.float64) + np.float64(np.float32(c))).astype(np.float32)
+
+
+def uniform_fmaf(lower, upper, words):
+    """The fp32 uniform of each word: fmaf(upper - lower, (x >> 8) 2^-24, lower), upper - lower in fp32."""
+    u = (words >> np.uint64(8)).astype(np.float64) * 2.0 ** -24
+    return fmaf(np.float32(upper) - np.float32(lower), u, lower)
+
+
+# DropoutLayer.Builder(IDropout) (B2G_LAYER_DROPOUT, b2g_dropout_kind), with the retain probability p, GaussianDropout's rate or GaussianNoise's
+# stddev, each taken as fp32; inference and a FrozenLayer are the identity.  Element e = ((row*h + y)*w + x)*c + ch (its NHWC index in the
+# pass) draws with j = e, SpatialDropout's (row, channel) with j = row * C + ch:
+#   dropout          y = x * m,  m = keep / p                          dx = dy * m
+#   gaussian_dropout y = x * m,  m = 1 + sqrt(rate / (1 - rate)) z     dx = dy * m
+#   gaussian_noise   y = x + stddev z                                  dx = dy
+#   alpha_dropout    y = a (keep ? x : alpha') + b                     dx = dy * keep * a   (alpha_coefficients)
+#   spatial_dropout  the dropout of each whole [H, W] map
+DROPOUT_KINDS = ("dropout", "gaussian_dropout", "gaussian_noise", "alpha_dropout", "spatial_dropout")
+VALUE_KEY = {"dropout": "p", "gaussian_dropout": "rate", "gaussian_noise": "stddev", "alpha_dropout": "p", "spatial_dropout": "p"}
+
+
 def dropout_mask(seed, rank, layer, pass_, rows, h, w, c, p, row0=0):
-    """Keep mask of a DropoutLayer (True = kept) for rows [row0, row0 + rows) of pass `pass_`, returned NCHW [rows, c, h, w].  Element
-    e = ((row*h + y)*w + x)*c + ch (NHWC index in the pass) keeps iff p >= 1 or Philox4x32-10(ctr = {e >> 2, lo32(P), hi32(P), layer | rank << 16},
-    key = {lo32(S), hi32(S)})[e & 3] < floor(p * 2^32), with p taken as fp32 and S = seed (0 -> 666)."""
-    p = np.float32(p)
+    """Keep mask of a DropoutLayer (True = kept) for rows [row0, row0 + rows) of pass `pass_`, returned NCHW [rows, c, h, w]; all kept at
+    p >= 1."""
     per = h * w * c
     e0, e1 = row0 * per, (row0 + rows) * per
-    if p >= 1:
+    if np.float32(p) >= 1:
         keep = np.ones(e1 - e0, bool)
     else:
-        seed, pass_ = int(seed) or 666, int(pass_)
-        g = np.arange(e0 >> 2, ((e1 - 1) >> 2) + 1, dtype=np.uint64)
-        words = np.stack(philox4x32_10((g, pass_ & 0xFFFFFFFF, pass_ >> 32, int(layer) | (int(rank) << 16)), (seed & 0xFFFFFFFF, seed >> 32)), -1).ravel()
-        keep = words[e0 - 4 * (e0 >> 2):][:e1 - e0] < np.uint64(math.floor(float(p) * 2.0 ** 32))
+        keep = keep_bits(philox_words(seed, e0, e1, *dropout_counter(rank, layer, pass_)), p)
     return keep.reshape(rows, h, w, c).transpose(0, 3, 1, 2)
 
 
-class DropoutState:
-    """The mask inputs a net's DropoutLayers share: seed (the library's b2g_net_config.seed), rank, pass counter P, explicit draws.  Like the
-    library, the last masking DropoutLayer of a train-mode forward advances P once it has drawn its mask; `queue` holds explicit (pass, first
-    row) draws that replace the counter for the next forwards without advancing it."""
+def dropout_normals(seed, rank, layer, pass_, rows, h, w, c, row0=0, q: Quirks = DEFAULT_QUIRKS):
+    """The normal z of each element of rows [row0, row0 + rows) of pass `pass_`, in float64, NCHW [rows, c, h, w]."""
+    per = h * w * c
+    e0, e1 = row0 * per, (row0 + rows) * per
+    g0 = e0 >> 2
+    z = normals(philox_words(seed, 4 * g0, 4 * (((e1 - 1) >> 2) + 1), *dropout_counter(rank, layer, pass_)), q)
+    return z[e0 - 4 * g0:][:e1 - e0].reshape(rows, h, w, c).transpose(0, 3, 1, 2)
 
-    def __init__(self, seed=666, rank=0):
-        self.seed, self.rank, self.pass_, self.queue = seed, rank, 0, []
+
+def spatial_mask(seed, rank, layer, pass_, rows, c, p, row0=0):
+    """SpatialDropout's keep bit of each (row, channel) of rows [row0, row0 + rows), [rows, c]."""
+    if np.float32(p) >= 1:
+        return np.ones((rows, c), bool)
+    return keep_bits(philox_words(seed, row0 * c, (row0 + rows) * c, *dropout_counter(rank, layer, pass_)), p).reshape(rows, c)
+
+
+def clamp_value(kind, v) -> np.float32:
+    """A scheduled value clamped into its kind's range (the library's documented deviation): rate to [0, 1 - 2^-24], stddev to >= 0, p to
+    [2^-32, 1]."""
+    v = np.float32(v)
+    if kind == "gaussian_dropout":
+        return np.float32(min(max(v, np.float32(0)), np.float32(1 - 2.0 ** -24)))
+    if kind == "gaussian_noise":
+        return np.float32(max(v, np.float32(0)))
+    return np.float32(min(max(v, np.float32(2.0 ** -32)), np.float32(1)))
+
+
+def gaussian_sigma(rate) -> np.float32:
+    """GaussianDropout's stddev sqrt(rate / (1 - rate)), in double from the fp32 rate, rounded to fp32 once."""
+    r = float(np.float32(rate))
+    return np.float32(math.sqrt(r / (1.0 - r)))
+
+
+def alpha_coefficients(p):
+    """AlphaDropout's (a, b, alpha') for the fp32 retain probability p: alpha' = -lambda alpha (SELU's constants),
+    a = 1 / sqrt(p + alpha'^2 p (1 - p)), b = -a (1 - p) alpha', each in double and rounded to fp32 once."""
+    p = float(np.float32(p))
+    ap = -SELU_LAMBDA * SELU_ALPHA
+    a = 1.0 / math.sqrt(p + ap * ap * p * (1.0 - p))
+    return np.float32(a), np.float32(-a * (1.0 - p) * ap), np.float32(ap)
+
+
+class DropoutState:
+    """The draw inputs a net's DropoutLayers and noisy layers share: seed (the library's b2g_net_config.seed), rank, pass counter P, explicit
+    draws.  Like the library, the last stochastic DropoutLayer of a train-mode forward advances P once it has drawn (weight noise does when the
+    pass has no such layer); `queue` holds explicit (pass, first row) draws that replace the counter for the next forwards without advancing
+    it.  `net`: the owning Net; `lead`: None, or the Net whose counters the next passes read their scheduled values at (gan_step's G pass
+    through D reads G's)."""
+
+    def __init__(self, seed=666, rank=0, net=None):
+        self.seed, self.rank, self.pass_, self.queue, self.net, self.lead = seed, rank, 0, [], net, None
+
+    def counters(self):
+        """The (iteration, epoch) a pass reads scheduled dropout values and DropConnect p at: the lead's, else the owning net's, else (0, 0)."""
+        net = self.lead if self.lead is not None else self.net
+        return (net.iteration, net.epoch) if net is not None else (0, 0)
 
     def current(self):
         return self.queue[0] if self.queue else (self.pass_, 0)
 
-    def finish(self):          # end of a masking train-mode forward
+    def finish(self):          # end of a stochastic train-mode forward
         if self.queue:
             self.queue.pop(0)
         else:
@@ -1049,47 +1253,292 @@ class DropoutState:
 
 
 class Dropout(Layer):
-    """DropoutLayer.Builder(p).  `index` = the layer's chain index in the CUDA library's layer array (the mask's L).  A Net shares its
-    DropoutState among its DropoutLayers."""
+    """DropoutLayer.Builder(IDropout): `kind` one of DROPOUT_KINDS with its value (VALUE_KEY: p, rate or stddev) and an optional schedule of
+    it.  A Net shares its DropoutState among its DropoutLayers.  Train mode draws from that state; the identity cases (p = 1, rate = 0 or
+    stddev = 0 without a schedule, frozen, inference) draw nothing and count no pass."""
 
-    def __init__(self, p, name="", index=0, state=None, frozen=False):
-        self.p, self.name, self.index, self.state, self.frozen, self.last = float(np.float32(p)), name, index, state, frozen, False
-        self._m = None
+    def __init__(self, value, name="", index=0, state=None, frozen=False, kind="dropout", schedule=None):
+        assert kind in DROPOUT_KINDS, kind
+        self.value, self.name, self.index, self.state, self.frozen = float(np.float32(value)), name, index, state, frozen
+        self.kind, self.schedule, self.last, self._m = kind, schedule, False, None
 
     def active(self):
-        return self.p < 1 and not self.frozen
+        if self.frozen:
+            return False
+        if self.schedule is not None:          # a scheduled layer is stochastic whatever its value
+            return True
+        return self.value > 0 if self.kind in ("gaussian_dropout", "gaussian_noise") else self.value < 1
+
+    def value_at(self, iteration, epoch) -> float:
+        """The value a train-mode pass at (iteration, epoch) uses: the schedule's fp32 value clamped into the kind's range, or the constant."""
+        if self.schedule is None:
+            return self.value
+        return float(clamp_value(self.kind, lr_at(self.schedule, iteration, epoch)))
 
     def forward(self, x, train):
         self._m = None
-        if not train or self.p >= 1:
+        if not train or not self.active():
             return x
+        value = self.value_at(*self.state.counters())
         pass_, row0 = self.state.current()
         _, c, h, w = x.shape if x.ndim == 4 else (x.shape[0], x.shape[1], 1, 1)
-        keep = dropout_mask(self.state.seed, self.state.rank, self.index, pass_, x.shape[0], h, w, c, self.p, row0).reshape(x.shape)
-        self._m = keep * x.dtype.type(np.float32(1) / np.float32(self.p))
+        args = (self.state.seed, self.state.rank, self.index, pass_, x.shape[0])
+        t = x.dtype.type
+        if self.kind == "dropout":
+            keep = dropout_mask(*args, h, w, c, value, row0).reshape(x.shape)
+            self._m = keep * t(np.float32(1) / np.float32(value)); y = x * self._m
+        elif self.kind in ("gaussian_noise", "gaussian_dropout"):
+            z = dropout_normals(*args, h, w, c, row0, self.q).reshape(x.shape)
+            if self.kind == "gaussian_noise":
+                y = x + t(np.float32(value)) * z
+            else:
+                self._m = 1 + t(gaussian_sigma(value)) * z; y = x * self._m
+        elif self.kind == "alpha_dropout":
+            keep = dropout_mask(*args, h, w, c, value, row0).reshape(x.shape)
+            a, b, ap = (t(v) for v in alpha_coefficients(value))
+            self._m = keep * a; y = a * np.where(keep, x, ap) + b
+        else:
+            if x.ndim != 4 or h * w == 1:
+                raise ValueError("SpatialDropout needs a [N, C, H, W] input")
+            keep = spatial_mask(*args[:4], x.shape[0], c, value, row0)[:, :, None, None]
+            self._m = np.broadcast_to(keep * t(np.float32(1) / np.float32(value)), x.shape); y = x * self._m
         if self.last:
             self.state.finish()
-        return x * self._m
+        return y
 
     def backward(self, eps):
         return eps if self._m is None else eps * self._m
 
 
-def xent_score_and_grad(z: np.ndarray, y: np.ndarray, clip_eps: float):
-    """LossBinaryXENT with a sigmoid activation (J:159-163).  Returns (sum of per-example losses, dL/dz).
+# Weight noise (b2g_weight_noise: DL4J's DropConnect and WeightNoise) on a conv, deconv or dense layer's `weight_noise` dict.  A train-mode
+# pass draws W' (and b' with apply_to_bias) of every noisy layer once at its top (Net.forward), from the clean parameters in the net's dtype;
+# that layer's forward and input gradient run on them, and its weight and bias gradients are taken straight through.  The draw index j is the
+# element's index in the library's internal [A][taps][B] order (internal_w), b's from bias_j0 on:
+#   DropConnect   W' = keep ? W : 0                     WeightNoise   n = NORMAL fmaf(std, z, mean) or UNIFORM (uniform_fmaf);
+#                                                                     W' = W + n (additive) or W * n
+def internal_w(W):
+    """W (DL4J's shape) in the library's internal [A][taps][B] order, flattened: conv [nOut][kH*kW][nIn], transposed conv [nIn][kH*kW][nOut],
+    dense [nOut][nIn]."""
+    W = np.asarray(W)
+    if W.ndim == 2:
+        return W.T.ravel()
+    return W.reshape(W.shape[0], W.shape[1], -1).transpose(0, 2, 1).ravel()
+
+
+def dl4j_w(flat, shape):
+    """The inverse of internal_w: the internal order back to W's shape."""
+    flat = np.asarray(flat)
+    if len(shape) == 2:
+        return flat.reshape(shape[1], shape[0]).T
+    return flat.reshape(shape[0], -1, shape[1]).transpose(0, 2, 1).reshape(shape)
+
+
+def bias_j0(n_w: int) -> int:
+    """Draw index of bias element 0: 4 * ceil(n_W / 4), so W and b never share a Philox counter."""
+    return 4 * ((n_w + 3) // 4)
+
+
+def drop_connect_p(wn, counters=(0, 0)) -> np.float32:
+    """DropConnect's retain probability of a pass: the constant, or the schedule's fp32 value at the pass's (iteration, epoch) clamped to
+    [2^-32, 1]."""
+    p = wn["p"]
+    if isinstance(p, dict):
+        return clamp_value("dropout", lr_at(p, *counters))
+    return np.float32(p)
+
+
+def weight_noise_draw(wn, n, j0, seed, rank, layer, pass_, p=None, q: Quirks = DEFAULT_QUIRKS):
+    """The draws of n elements with indices j0 .. j0 + n - 1 (j0 a multiple of 4): DropConnect's keep bits (bool), or WeightNoise's noise in
+    fp32."""
+    assert j0 % 4 == 0
+    words = philox_words(seed, j0, ((j0 + n + 3) // 4) * 4, *dropout_counter(rank, layer, pass_))
+    if wn["weight_noise"] == "drop_connect":
+        if np.float32(p) >= 1:
+            return np.ones(n, bool)
+        return keep_bits(words[:n], p)
+    d = wn["distribution"]
+    if d["distribution"] == "normal":
+        return fmaf(d["std"], normals(words, q)[:n], d["mean"])
+    return uniform_fmaf(d["lower"], d["upper"], words[:n])
+
+
+def weight_noise_apply(wn, w, d, p=None, q: Quirks = DEFAULT_QUIRKS):
+    """W' from the clean values w and the draws d, in w's dtype (float32: the library's fp32 operand, each result rounded once)."""
+    t = w.dtype.type
+    if wn["weight_noise"] == "drop_connect":
+        kept = w / t(np.float32(p)) if q.dropconnect_inverted else w
+        return np.where(d, kept, t(0))
+    n = d.astype(w.dtype)
+    return (w + n if wn.get("additive", True) else w * n).astype(w.dtype)
+
+
+def noisy_operands(layer, wn, index, seed, rank, pass_, counters=(0, 0), dtype=np.float32, q: Quirks = DEFAULT_QUIRKS):
+    """(W' in the internal order, b' or None) of one layer for pass `pass_`, from its parameters taken as `dtype`."""
+    p = drop_connect_p(wn, counters) if wn["weight_noise"] == "drop_connect" else None
+    w = internal_w(layer.params["W"]).astype(dtype)
+    w_n = weight_noise_apply(wn, w, weight_noise_draw(wn, w.size, 0, seed, rank, index, pass_, p, q), p, q)
+    b_n = None
+    if wn.get("apply_to_bias", False) and getattr(layer, "has_bias", False):
+        b = np.asarray(layer.params["b"]).astype(dtype)
+        b_n = weight_noise_apply(wn, b, weight_noise_draw(wn, b.size, bias_j0(w.size), seed, rank, index, pass_, p, q), p, q)
+    return w_n, b_n
+
+
+def weight_noise_active(layer) -> bool:
+    """A layer whose train-mode passes draw: it has weight noise, is not frozen, and is not a constant DropConnect(1)."""
+    wn = layer.weight_noise
+    if wn is None or getattr(layer, "frozen", False):
+        return False
+    return wn["weight_noise"] != "drop_connect" or isinstance(wn["p"], dict) or np.float32(wn["p"]) < 1
+
+
+# Weight initialization (b2g_weight_init: DL4J's WeightInit, Distribution and biasInit), each scheme's distribution from the layer's fans().
+# The draw: L = the layer's index in the library's desc array, j = the element's index in DL4J's view order of W (b2g_net_get_param's);
+# round k draws from counter {j >> 2, k, 0, L | 2^31}.  NORMAL: fmaf(std, z, mean), z of round 0's Box-Muller pairs (float64 here; the
+# device's is fp32, so normal draws agree within its tolerance).  UNIFORM: uniform_fmaf.  TRUNCATED_NORMAL: z of the first round k < 16 with
+# |z| <= truncation_sigmas, else round 15's z clamped.  LOG_NORMAL: exp of the NORMAL value.  BINOMIAL: the count over rounds t < nTrials of
+# keep_bits(x_t, p).  CONSTANT, ZERO, ONES, IDENTITY: no draw.
+SCHEMES = ("distribution", "zero", "ones", "sigmoid_uniform", "normal", "lecun_normal", "uniform", "xavier", "xavier_uniform", "xavier_fan_in",
+           "xavier_legacy", "relu", "relu_uniform", "identity", "lecun_uniform", "var_scaling_normal_fan_in", "var_scaling_normal_fan_out",
+           "var_scaling_normal_fan_avg", "var_scaling_uniform_fan_in", "var_scaling_uniform_fan_out", "var_scaling_uniform_fan_avg")
+DISTRIBUTIONS = ("normal", "uniform", "truncated_normal", "log_normal", "binomial", "constant", "orthogonal")
+WEIGHT_INIT_ROUNDS = 16
+
+
+def resolve(wi, layer, q: Quirks = DEFAULT_QUIRKS):
+    """What the scheme draws on the layer: (kind, a, b) with kind a distribution name or "identity"; a, b fp32, each computed in double and
+    rounded once (binomial: (nTrials, p))."""
+    scheme = wi["weight_init"]
+    fi, fo = (float(v) for v in layer.fans())
+    N = lambda sd: ("normal", np.float32(0), np.float32(sd))
+    U = lambda r: ("uniform", -np.float32(r), np.float32(r))
+    T = lambda sd: ("truncated_normal", np.float32(0), np.float32(sd))
+    u3 = lambda fan: 3.0 / math.sqrt(fan) if q.var_scaling_uniform_three_over_sqrt else math.sqrt(3.0 / fan)
+    if scheme == "distribution":
+        d = wi["distribution"]
+        kind = d["distribution"]
+        if kind in ("normal", "truncated_normal", "log_normal"):
+            return kind, np.float32(d["mean"]), np.float32(d["std"])
+        if kind == "uniform":
+            return kind, np.float32(d["lower"]), np.float32(d["upper"])
+        if kind == "binomial":
+            return kind, int(d["n_trials"]), np.float32(d["p"])
+        if kind == "constant":
+            return kind, np.float32(d["value"]), np.float32(0)
+        raise ValueError(kind)
+    table = {
+        "zero": lambda: ("constant", np.float32(0), np.float32(0)),
+        "ones": lambda: ("constant", np.float32(1), np.float32(0)),
+        "sigmoid_uniform": lambda: U(4.0 * math.sqrt(6.0 / (fi + fo))),
+        "normal": lambda: N(1.0 / math.sqrt(fi) if q.normal_scaled_by_fan_in else 1.0),
+        "lecun_normal": lambda: N(1.0 / math.sqrt(fi)),
+        "uniform": lambda: U(1.0 / math.sqrt(fi)),
+        "xavier": lambda: N(math.sqrt(2.0 / (fi + fo))),
+        "xavier_uniform": lambda: U(math.sqrt(6.0) / math.sqrt(fi + fo)),
+        "xavier_fan_in": lambda: N(1.0 / math.sqrt(fi)),
+        "xavier_legacy": lambda: N(1.0 / math.sqrt(layer.n_in + layer.n_out) if q.xavier_legacy_shape01 else 1.0 / math.sqrt(fi + fo)),
+        "relu": lambda: N(math.sqrt(2.0 / fi)),
+        "relu_uniform": lambda: U(math.sqrt(6.0 / fi)),
+        "identity": lambda: ("identity", np.float32(0), np.float32(0)),
+        "lecun_uniform": lambda: U(3.0 / math.sqrt(fi) if q.lecun_uniform_three_over_sqrt else math.sqrt(3.0 / fi)),
+        "var_scaling_normal_fan_in": lambda: T(math.sqrt(1.0 / fi)),
+        "var_scaling_normal_fan_out": lambda: T(math.sqrt(1.0 / fo)),
+        "var_scaling_normal_fan_avg": lambda: T(math.sqrt(2.0 / (fi + fo))),
+        "var_scaling_uniform_fan_in": lambda: U(u3(fi)),
+        "var_scaling_uniform_fan_out": lambda: U(u3(fo)),
+        "var_scaling_uniform_fan_avg": lambda: U(u3((fi + fo) / 2.0)),
+    }
+    return table[scheme]()
+
+
+def weight_init_words(seed, layer_index, n, k):
+    """Round k's Philox word of every view index j < n."""
+    return philox_words(seed, 0, n, int(k), 0, int(layer_index) | WEIGHT_INIT_TAG)
+
+
+def weight_init_normals(seed, layer_index, n, k=0, q: Quirks = DEFAULT_QUIRKS):
+    """Round k's float64 normal of every view index j < n (a tail element's pair partner exists past n)."""
+    return normals(weight_init_words(seed, layer_index, 4 * ((n + 3) // 4), k), q)[:n]
+
+
+def truncated_z(seed, layer_index, n, q: Quirks = DEFAULT_QUIRKS):
+    """The z of the first round k < 16 with |z| <= the truncation, else round 15's z clamped."""
+    lim = q.truncation_sigmas
+    z = np.zeros(n)
+    todo = np.ones(n, bool)
+    for k in range(WEIGHT_INIT_ROUNDS):
+        t = weight_init_normals(seed, layer_index, n, k, q)
+        hit = todo & (np.abs(t) <= lim)
+        z[hit] = t[hit]
+        todo &= ~hit
+        if k == WEIGHT_INIT_ROUNDS - 1:
+            z[todo] = np.clip(t[todo], -lim, lim)
+        if not todo.any():
+            break
+    return z
+
+
+def weight_init_draw(kind, a, b, n, seed, layer_index, n_in=None, q: Quirks = DEFAULT_QUIRKS):
+    """n fp32 values in view order.  identity: n_in = nIn of the square dense W (view index j = o nIn + i)."""
+    if kind == "normal":
+        return fmaf(b, weight_init_normals(seed, layer_index, n, 0, q), a)
+    if kind == "log_normal":
+        return np.exp(fmaf(b, weight_init_normals(seed, layer_index, n, 0, q), a).astype(np.float64)).astype(np.float32)
+    if kind == "truncated_normal":
+        return fmaf(b, truncated_z(seed, layer_index, n, q), a)
+    if kind == "uniform":
+        return uniform_fmaf(a, b, weight_init_words(seed, layer_index, n, 0))
+    if kind == "binomial":
+        c = np.zeros(n, np.int64)
+        for t in range(int(a)):
+            c += keep_bits(weight_init_words(seed, layer_index, n, t), b)
+        return c.astype(np.float32)
+    if kind == "constant":
+        return np.full(n, np.float32(a), np.float32)
+    if kind == "identity":
+        j = np.arange(n)
+        return (j // n_in == j % n_in).astype(np.float32)
+    raise ValueError(kind)
+
+
+def weights(wi, layer, seed, layer_index, q: Quirks = DEFAULT_QUIRKS):
+    """W of a conv, deconv or dense layer in DL4J's flattened view order (b2g_net_get_param's), fp32."""
+    kind, a, b = resolve(wi, layer, q)
+    if kind == "identity" and (not isinstance(layer, Dense) or layer.n_in != layer.n_out):
+        raise ValueError("IDENTITY needs a square dense W")
+    n = layer.n_in * layer.n_out * int(np.prod(getattr(layer, "k", (1, 1))))
+    return weight_init_draw(kind, a, b, n, seed, layer_index, layer.n_in, q)
+
+
+def init_layer(layer, wi, seed, layer_index, q: Quirks = DEFAULT_QUIRKS):
+    """The layer's W and b (if it has one) as b2g_net_init_weights leaves them, in the layer's dtype."""
+    flat = weights(wi, layer, seed, layer_index, q)
+    order = next(o for p, _, o in layer.param_specs() if p == "W")
+    W = layer.params["W"]
+    layer.params["W"] = flat.astype(W.dtype).reshape(W.shape, order=order.upper())
+    if "b" in layer.params:
+        layer.params["b"] = np.full(layer.params["b"].shape, np.float32(wi.get("bias_init", 0.0)), layer.params["b"].dtype)
+    return layer
+
+
+def xent_score_and_grad(z: np.ndarray, y: np.ndarray, clip_eps: float, s=None):
+    """LossBinaryXENT with a sigmoid activation (J:159-163).  Returns (sum of per-example losses, dL/dz); s: the per-element weight and mask
+    product both are scaled by (None: unweighted).
 
     clip_eps > 0: p = clip(sigmoid(z), eps, 1-eps); grad = (p-y)/(p(1-p)) * sigmoid'(z)   (DL4J-exact)
     clip_eps = 0: BCE-with-logits (north_star): loss = softplus(z) - y z; grad = sigmoid(z) - y.
     """
     if clip_eps > 0:
-        s = _sigmoid(z)
-        p = np.clip(s, clip_eps, 1 - clip_eps)
+        sg = _sigmoid(z)
+        p = np.clip(sg, clip_eps, 1 - clip_eps)
         loss = -(y * np.log(p) + (1 - y) * np.log(1 - p))
-        grad = (p - y) / (p * (1 - p)) * s * (1 - s)
+        grad = (p - y) / (p * (1 - p)) * sg * (1 - sg)
     else:
         loss = np.maximum(z, 0) + np.log1p(np.exp(-np.abs(z))) - y * z
         grad = _sigmoid(z) - y
-    return loss.sum(), grad
+    if s is None:
+        return loss.sum(), grad
+    return float((loss * s).sum()), grad * s
 
 
 # Regression and margin losses (b2g_loss codes 2-8; org.nd4j.linalg.lossfunctions.impl.*).  Each is ILossFunction.computeGradient(labels,
@@ -1127,35 +1576,102 @@ def per_output(loss: str, q: Quirks = DEFAULT_QUIRKS) -> bool:
     return loss in ("mse", "mae") or (loss == "wasserstein" and q.wasserstein_per_output)
 
 
-def score_and_grad(loss: str, act: str, alpha: float, z: np.ndarray, y: np.ndarray, q: Quirks = DEFAULT_QUIRKS):
-    """z, y: [N, nOut].  Returns (sum over the N examples of the per-example scores, dL/dz [N, nOut])."""
+def _elem_score_and_grad(loss, act, alpha, z, y, q):
+    """The per-element scores (before the / nOut of the per-output losses) and dL/dz of a loss of codes 2-8."""
     if act in EXT_ACTS:
-        s, g = score_and_grad(loss, "identity", 0.0, forward(act, z, alpha, q), y, q)
-        return s, g * derivative(act, z, alpha, q)
+        l, g = _elem_score_and_grad(loss, "identity", 0.0, forward(act, z, alpha, q), y, q)
+        return l, g * derivative(act, z, alpha, q)
     a = act_forward(act, z, alpha)
     e, m = a - y, 1 - y * a
     if loss in ("mse", "l2"):
-        s, g = (e * e).sum(), 2 * e
+        l, g = e * e, 2 * e
     elif loss in ("l1", "mae"):
-        s, g = np.abs(e).sum(), np.sign(e)
+        l, g = np.abs(e), np.sign(e)
     elif loss == "hinge":
-        s, g = np.maximum(m, 0).sum(), np.where(m > 0, -y, 0.0)
+        l, g = np.maximum(m, 0), np.where(m > 0, -y, 0.0)
     elif loss == "squared_hinge":
-        s, g = (np.maximum(m, 0) ** 2).sum(), -2 * y * np.maximum(m, 0)
+        l, g = np.maximum(m, 0) ** 2, -2 * y * np.maximum(m, 0)
     elif loss == "wasserstein":
-        s, g = (y * a).sum(), y * np.ones_like(a)
+        l, g = y * a, y * np.ones_like(a)
     else:
         raise ValueError(loss)
     if per_output(loss, q):
-        n = z.shape[1]
-        s, g = s / n, g / n
-    return float(s), g * act_grad_from_out(act, a, alpha)
+        g = g / z.shape[1]
+    return l, g * act_grad_from_out(act, a, alpha)
 
 
-def _loss_score_and_grad(layer, z, y):
-    if layer.loss == "xent":
-        return xent_score_and_grad(z, y, layer.q.xent_clip_eps)
-    return score_and_grad(layer.loss, layer.loss_act, layer.loss_alpha, z, y, layer.q)
+def score_and_grad(loss: str, act: str, alpha: float, z: np.ndarray, y: np.ndarray, q: Quirks = DEFAULT_QUIRKS, s=None):
+    """z, y: [N, nOut].  Returns (sum over the N examples of the per-example scores, dL/dz [N, nOut]); s: the per-element weight and mask
+    product both are scaled by (None: unweighted)."""
+    l, g = _elem_score_and_grad(loss, act, alpha, z, y, q)
+    score = l.sum() if s is None else (l * s).sum()
+    if per_output(loss, q):
+        score = score / z.shape[1]
+    return float(score), g if s is None else g * s
+
+
+# Per-output loss weights w_j and labels masks m_rj (semantics at b2g_loss).  For row r (an example, or a pixel of a CnnLossLayer) and
+# column j (an output, or a channel):
+#   XENT, codes 2-8   score terms w_j m_rj l(a_rj, y_rj), dz_rj = w_j m_rj dz_rj
+#   MCXENT            score -m_r sum_j w_j y_rj log clamp(p_rj), dz_rj = m_r (p_rj sum_k w_k y_rk - w_j y_rj) (weighted), m_r (p_rj - y_rj)
+# The score stays the loss sum over the minibatch; MSE, MAE and Wasserstein still divide by nOut / C.  A mask is [N, 1] or [N, nOut] on
+# OUTPUT / LOSS layers and NCHW [N, 1, H, W] or [N, C, H, W] on a CnnLossLayer.
+def check_weights(loss, weights, cols, q: Quirks = DEFAULT_QUIRKS):
+    """The loss weights as float64 [cols] (None stays None), refused as the library refuses them."""
+    if weights is None:
+        return None
+    w = np.asarray(weights, np.float64).ravel()
+    if loss in q.weightless_losses:
+        raise NotImplementedError(f"{loss} takes no per-output weights")
+    if w.size != cols:
+        raise ValueError(f"{w.size} loss weights for {cols} outputs")
+    if not np.all(np.isfinite(w)):
+        raise ValueError("loss weights must be finite")
+    return w
+
+
+def check_mask(loss, mask, rows, cols, q: Quirks = DEFAULT_QUIRKS):
+    """The mask as float64 rows: [rows, 1] or [rows, cols] (None stays None)."""
+    if mask is None:
+        return None
+    m = np.asarray(mask, np.float64).reshape(rows, -1)
+    if m.shape[1] not in (1, cols):
+        raise ValueError(f"mask width {m.shape[1]}: 1 or {cols}")
+    if m.shape[1] > 1 and loss == "mcxent" and q.mcxent_per_output_mask_refused:
+        raise NotImplementedError("per-output masking for MCXENT + softmax is not supported")
+    return m
+
+
+def loss_scale(z, w, m):
+    """The per-element product of the weights w [C] and the mask m [R, 1 | C] on rows z [R, C]; None when both are absent."""
+    if w is None and m is None:
+        return None
+    s = np.ones_like(z)
+    if w is not None:
+        s = s * w[None, :]
+    if m is not None:
+        s = s * m
+    return s
+
+
+def rows_score_and_grad(loss, act, alpha, z, y, w=None, m=None, q: Quirks = DEFAULT_QUIRKS):
+    """The loss on rows z, y [R, C], weighted by w [C] and masked by m [R, 1 | C] (None: that part absent): (summed score, dL/dz [R, C])."""
+    if loss == "mcxent":
+        return mcxent_softmax_score_and_grad(z, y, w=w, m=m)
+    s = loss_scale(z, w, m)
+    if loss == "xent":
+        return xent_score_and_grad(z, y, q.xent_clip_eps, s)
+    return score_and_grad(loss, act, alpha, z, y, q, s)
+
+
+def _score_and_eps(layer, loss, y, weights, mask):
+    """(summed score, dL/dz) of an OutputLayer or LossLayer on its pre-activations as [N, nOut] rows."""
+    z = layer._z
+    y = np.asarray(y, z.dtype)
+    zr = z.reshape(y.shape)
+    w, m = check_weights(loss, weights, zr.shape[1], layer.q), check_mask(loss, mask, zr.shape[0], zr.shape[1], layer.q)
+    s, g = rows_score_and_grad(loss, layer.loss_act, layer.loss_alpha, zr, y, w, m, layer.q)
+    return s, g.reshape(z.shape)
 
 
 class LossLayer(Layer):
@@ -1172,10 +1688,9 @@ class LossLayer(Layer):
         self._z = x
         return _layer_act_forward(self.loss_act, x, self.loss_alpha, self.q)
 
-    def score_and_eps(self, y):
-        z = self._z
-        s, g = _loss_score_and_grad(self, z.reshape(y.shape), y)
-        return s, g.reshape(z.shape)
+    def score_and_eps(self, y, weights=None, mask=None):
+        """(summed score, dL/dz) on labels y, with per-output weights and a labels mask (None: that part absent)."""
+        return _score_and_eps(self, self.loss, y, weights, mask)
 
 
 def to_rows(a):
@@ -1214,13 +1729,17 @@ class CnnLossLayer(LossLayer):
             return softmax_channels(x)
         return _layer_act_forward(self.loss_act, x, self.loss_alpha, self.q)
 
-    def score_and_eps(self, y):
+    def score_and_eps(self, y, weights=None, mask=None):
         z = self._z
+        n, c, h, w = z.shape
         zr, yr = to_rows(z), to_rows(np.asarray(y, z.dtype).reshape(z.shape))
-        if self.loss == "mcxent":
-            s, g = mcxent_softmax_score_and_grad(zr, yr)
-        else:
-            s, g = _loss_score_and_grad(self, zr, yr)
+        if mask is not None:
+            mask = np.asarray(mask, np.float64).reshape(n, -1, h, w)
+            if mask.shape[1] not in (1, c):
+                raise ValueError(f"mask channels {mask.shape[1]}: 1 or {c}")
+            mask = to_rows(mask)
+        wt, m = check_weights(self.loss, weights, c, self.q), check_mask(self.loss, mask, zr.shape[0], c, self.q)
+        s, g = rows_score_and_grad(self.loss, self.loss_act, self.loss_alpha, zr, yr, wt, m, self.q)
         g = from_rows(g, z.shape)
         if not self.q.cnn_loss_score_per_minibatch:
             hw = z.shape[2] * z.shape[3]
@@ -1243,27 +1762,37 @@ class Output(Dense):
         z = super().forward(x, train)          # the identity Dense: z; the loss applies the activation
         return _layer_act_forward(self.loss_act, z, self.loss_alpha, self.q)
 
-    def score_and_eps(self, y):
-        return _loss_score_and_grad(self, self._z, y)
+    def score_and_eps(self, y, weights=None, mask=None):
+        return _score_and_eps(self, self.loss, y, weights, mask)
 
     def backward(self, eps):   # eps is already dL/dz
         self.grads["W"] = self._x.T @ eps
         self.grads["b"] = eps.sum(0)
-        return eps @ self.params["W"].T
+        return eps @ self._p("W").T
 
 
-def mcxent_softmax_score_and_grad(z: np.ndarray, y: np.ndarray, clip_eps: float = 1e-10):
+def mcxent_softmax_score_and_grad(z: np.ndarray, y: np.ndarray, clip_eps: float = 1e-10, w=None, m=None):
     """LossMCXENT with a softmax activation (J:357-362): p = softmax(z) clipped to [eps, 1-eps] for the log
-    (softmaxClipEps default 1e-10); loss = -sum y log p; dL/dz = p - y (DL4J's softmax+MCXENT shortcut)."""
+    (softmaxClipEps default 1e-10); loss = -sum y log p; dL/dz = p - y (DL4J's softmax+MCXENT shortcut).  w [C], m [R, 1]: the class
+    weights and the row mask (None: absent)."""
     zs = z - z.max(1, keepdims=True)
     e = np.exp(zs)
     p = e / e.sum(1, keepdims=True)
     pc = np.clip(p, clip_eps, 1 - clip_eps) if clip_eps > 0 else p
-    return float(-(y * np.log(pc)).sum()), p - y
+    s = loss_scale(z, w, m)
+    if s is None:
+        return float(-(y * np.log(pc)).sum()), p - y
+    mr = m if m is not None else 1.0
+    if w is not None:
+        wy = w[None, :] * y
+        return float(-((y * np.log(pc)) * s).sum()), mr * (p * wy.sum(1, keepdims=True) - wy)
+    return float(-((y * np.log(pc)) * s).sum()), mr * (p - y)
 
 
 class OutputSoftmax(Dense):
     """OutputLayer.Builder(LossFunction.MCXENT).activation(Activation.SOFTMAX).nOut(10) (J:357-362): the transfer-learning head."""
+
+    loss, loss_act, loss_alpha = "mcxent", "softmax", None
 
     def __init__(self, n_in, n_out, updater=None, l2=0.0, name=""):
         super().__init__(n_in, n_out, activation="identity", updater=updater, l2=l2, name=name)
@@ -1271,13 +1800,13 @@ class OutputSoftmax(Dense):
     def forward(self, x, train):
         return softmax_channels(super().forward(x, train))
 
-    def score_and_eps(self, y):
-        return mcxent_softmax_score_and_grad(self._z, y)
+    def score_and_eps(self, y, weights=None, mask=None):
+        return _score_and_eps(self, self.loss, y, weights, mask)
 
     def backward(self, eps):
         self.grads["W"] = self._x.T @ eps
         self.grads["b"] = eps.sum(0)
-        return eps @ self.params["W"].T
+        return eps @ self._p("W").T
 
 
 # --------------------------------------------------------------------------------------------------
@@ -1375,19 +1904,16 @@ class Net:
         self.gradient_normalization, self.gradient_normalization_threshold, self.grad_norm_last_norms = "none", 1.0, []
         self.schedules: Dict[str, dict] = {}      # layer name -> schedule (None: the constant lr)
         self.layer_constraints: Dict[str, Dict[str, List[Dict]]] = {}     # layer name -> parameter -> its ordered constraints
-        self.dropout = DropoutState(mask_seed, rank)
+        self.layer_regularization: Dict[str, Tuple[float, float, float]] = {}     # layer name -> (l1, l1Bias, l2Bias) beside its l2
+        self.dropout = DropoutState(mask_seed, rank, self)
+        self.loss_weights: Optional[np.ndarray] = None      # the loss layer's per-output weights (None: unweighted)
         self._skip_acc: Dict[int, np.ndarray] = {}    # skip source index -> the skip shares the current backward has met
         rng = np.random.default_rng(seed)
         for l in self.layers:
             if "q" not in vars(l):        # a layer built with its own quirks, or already in a net, keeps them
                 l.q = quirks
             l.init(rng, dtype)
-        drops = [l for l in self.layers if isinstance(l, Dropout)]
-        for l in drops:
-            l.state, l.last = self.dropout, False
-        active = [l for l in drops if l.active()]
-        if active:
-            active[-1].last = True
+        self._link_dropout()
         self.state: Dict[Tuple[int, str], List[np.ndarray]] = {}
         for li, l in enumerate(self.layers):
             if not l.has_params:
@@ -1439,15 +1965,46 @@ class Net:
                     for c in lst:
                         l.params[p] = apply_constraint(l.params[p], c, self.q)
 
+    def _link_dropout(self):
+        """The DropoutLayers' shared state, and the last-stochastic-layer flag: the last active DropoutLayer of a pass advances P."""
+        drops = [l for l in self.layers if isinstance(l, Dropout)]
+        for l in drops:
+            l.state, l.last = self.dropout, False
+        active = [l for l in drops if l.active()]
+        if active:
+            active[-1].last = True
+
+    def set_dropout_schedule(self, schedule: Optional[dict], layer: Optional[str] = None):
+        """The library Net's set_dropout_schedule: layer None = every non-frozen DropoutLayer; schedule None = the constant."""
+        for l in self.layers:
+            if isinstance(l, Dropout) and (l.name == layer if layer is not None else not l.frozen):
+                l.schedule = schedule
+        self._link_dropout()
+
+    def dropout_value(self, layer: str) -> float:
+        """The value the DropoutLayer's next train-mode pass uses, at the net's own counters."""
+        return self.layer(layer).value_at(self.iteration, self.epoch)
+
+    def set_weight_noise(self, wn: Optional[Dict], layer: Optional[str] = None):
+        """The library Net's set_weight_noise: layer None = every non-frozen conv, deconv or dense layer; wn None clears."""
+        for l in self.layers:
+            if isinstance(l, GEMM) and (l.name == layer if layer is not None else not getattr(l, "frozen", False)):
+                l.weight_noise = wn
+
+    def set_loss_weights(self, weights):
+        """The loss layer's per-output weights (None: unweighted), checked against its outputs at every score."""
+        self.loss_weights = None if weights is None else np.asarray(weights, np.float64).ravel()
+
     def dropout_pass(self) -> int:
-        """The dropout pass counter P: train-mode forwards that applied a DropoutLayer mask."""
+        """The dropout pass counter P: train-mode forwards that drew a DropoutLayer mask or weight noise."""
         return self.dropout.pass_
 
     def set_dropout_pass(self, p: int):
         self.dropout.pass_ = p
 
     def _has_active_dropout(self) -> bool:
-        return any(isinstance(l, Dropout) and l.active() for l in self.layers)
+        """A stochastic pass: a DropoutLayer or a noisy layer draws."""
+        return any((isinstance(l, Dropout) and l.active()) or weight_noise_active(l) for l in self.layers)
 
     # ---- DL4J flattened parameter vector -------------------------------------------------------
     def param_table(self):
@@ -1484,6 +2041,17 @@ class Net:
     # ---- forward / backward --------------------------------------------------------------------
     def forward(self, x, train: bool, collect: bool = False):
         self._skip_acc = {}
+        for l in self.layers:
+            l.noisy = None
+        noisy = [l for l in self.layers if weight_noise_active(l)] if train else []
+        if noisy:               # W' (and b') of every noisy layer at the top of the pass
+            pass_, _ = self.dropout.current()
+            for l in noisy:
+                w, b = noisy_operands(l, l.weight_noise, l.index, self.dropout.seed, self.dropout.rank, pass_, self.dropout.counters(), self.dtype,
+                                      l.q)
+                l.noisy = {"W": dl4j_w(w, l.params["W"].shape)} | ({"b": b} if b is not None else {})
+            if not any(isinstance(l, Dropout) and l.active() for l in self.layers):
+                self.dropout.finish()
         acts = []
         a = np.asarray(x, self.dtype)
         for l in self.layers:
@@ -1521,45 +2089,85 @@ class Net:
         """Back-propagate eps (w.r.t. the output of the last non-loss layer handled by the caller)."""
         return self._backward(eps, stop_at, len(self.layers), collect)
 
-    def l2_score(self):
-        s = 0.0
-        for l in self.layers:
-            if l.has_params and l.l2 and not getattr(l, "frozen", False):     # FrozenLayer.calcL2() == 0
-                for p in l.l2_names():
-                    s += 0.5 * l.l2 * float((l.params[p].astype(np.float64) ** 2).sum())
-        return s
+    # Regularization (b2g_regularization: DL4J's l1, l2, l1Bias and l2Bias), per parameter as beta3's getL1ByParam / getL2ByParam:
+    #   update  theta -= updater(g) + l2 * theta (W);  then theta -= l2Bias * theta (b) + l1 * sign(theta_before),  sign(+-0) = 0;  then the
+    #           constraints.  The two subtractions are rounded to the net's dtype one after the other, as the library applies them.
+    #   score   sum(loss) / mb + calc_l2() + calc_l1()
+    def reg_coefs(self, layer: Layer, param: str) -> Tuple[float, float]:
+        """(l1, l2) of one parameter: a conv, deconv, dense or output layer's W takes its l1 and l2, its b l1Bias and l2Bias, a PReLU's alpha
+        ("W") its l1 and l2 as a weight; everything else (BatchNorm, every other layer) (0, 0).  l1, l1Bias and l2Bias are the net's
+        layer_regularization, l2 the layer's."""
+        if isinstance(layer, BatchNorm) and not layer.q.batchnorm_unregularized:
+            raise NotImplementedError("only beta3's unregularized BatchNorm is restated")
+        l1, l1_bias, l2_bias = self.layer_regularization.get(layer.name, (0.0, 0.0, 0.0))
+        if isinstance(layer, PReLU):
+            return (l1, float(layer.l2)) if param == "W" and layer.q.prelu_alpha_regularized else (0.0, 0.0)
+        if not isinstance(layer, GEMM):
+            return 0.0, 0.0
+        if param == "W":
+            return l1, float(layer.l2)
+        if param == "b":
+            return l1_bias, l2_bias
+        return 0.0, 0.0
 
-    def compute_gradient_and_score(self, x, y, collect=False, pass_=None, row0=0):
+    def _reg_sum(self, which, norm):
+        s = [0.0, 0.0]          # the PReLU terms are summed apart and added last, as the library sums them
+        for l in self.layers:
+            if l.has_params and not getattr(l, "frozen", False):     # FrozenLayer.calcL1() == calcL2() == 0
+                for p, _, _ in l.param_specs():
+                    c = self.reg_coefs(l, p)[which]
+                    if c:
+                        s[isinstance(l, PReLU)] += norm(c, l.params[p].astype(np.float64))
+        return s[0] + s[1]
+
+    def calc_l2(self) -> float:
+        """ComputationGraph.calcL2(true): sum of 0.5 * l2 * ||W||^2 + 0.5 * l2_bias * ||b||^2 over the live layers."""
+        return self._reg_sum(1, lambda c, v: 0.5 * c * float((v ** 2).sum()))
+
+    def calc_l1(self) -> float:
+        """ComputationGraph.calcL1(true): sum of l1 * ||W||_1 + l1_bias * ||b||_1 over the live layers."""
+        return self._reg_sum(0, lambda c, v: c * float(np.abs(v).sum()))
+
+    def l2_score(self):
+        """The score's whole regularization term."""
+        return self.calc_l2() + self.calc_l1()
+
+    def compute_gradient_and_score(self, x, y, collect=False, pass_=None, row0=0, mask=None):
         """ComputationGraph.computeGradientAndScore: train-mode forward, loss, backprop.
-        Gradients are minibatch *sums*; score = sum(loss)/mb + 0.5*l2*||W||^2.
-        pass_: the DropoutLayers draw rows [row0, row0 + mb) of that pass, and the pass counter is left alone."""
+        Gradients are minibatch *sums*; score = sum(loss)/mb + l2_score().
+        pass_: the DropoutLayers draw rows [row0, row0 + mb) of that pass, and the pass counter is left alone.  mask: the labels mask."""
+        if mask is not None and not self.q.masked_score_per_minibatch:
+            raise NotImplementedError("only the minibatch divisor is restated")
         if pass_ is not None and self._has_active_dropout():
             self.dropout.queue.append((pass_, row0))
         out, acts = self.forward(x, train=True, collect=True)
-        loss_sum, eps_in, epss = self._loss_backward(y)
+        loss_sum, eps_in, epss = self._loss_backward(y) if mask is None else self._loss_backward(y, mask)
         score = float(loss_sum) / x.shape[0] + self.l2_score()
         if collect:
             return score, acts, epss, eps_in
         return score
 
-    def _loss_backward(self, y):
-        """After a forward: the last layer's score on labels y, then the backward of its own parameters (an OutputLayer's) and the prefix.
-        Returns (loss sum, eps at the prefix's input, the prefix's epsilons)."""
+    def _loss_backward(self, y, mask=None):
+        """After a forward: the last layer's score on labels y (weighted by loss_weights, masked by mask), then the backward of its own
+        parameters (an OutputLayer's) and the prefix.  Returns (loss sum, eps at the prefix's input, the prefix's epsilons).  Unmasked
+        callers pass y alone, so a subclass that scores its own way may override the one-argument form."""
         last = self.layers[-1]
-        loss_sum, eps = last.score_and_eps(np.asarray(y, self.dtype))
+        loss_sum, eps = last.score_and_eps(np.asarray(y, self.dtype), self.loss_weights, mask)
         if last.has_params:
             eps = last.backward(eps)
         return (loss_sum,) + self.backward_from_prefix(eps, collect=True)
 
     def backward_from_prefix(self, eps, collect=False):
-        """Backprop through all layers except the final loss-bearing one; stops at the frozen feature extractor."""
+        """Backprop through all layers except the final loss-bearing one; stops at the frozen feature extractor (a frozen PReLU passes its
+        input gradient)."""
         hi = len(self.layers) - 1
-        lo = max((i + 1 for i in range(hi) if getattr(self.layers[i], "frozen", False)), default=0)
+        lo = max((i + 1 for i in range(hi) if getattr(self.layers[i], "frozen", False) and not isinstance(self.layers[i], PReLU)), default=0)
         return self._backward(eps, lo, hi, collect)
 
     # ---- updater: BaseMultiLayerUpdater.update + UpdaterBlock + params.subi ----------------------
     def apply_update(self, mb: int, grads: Optional[Dict[Tuple[int, str], np.ndarray]] = None, frozen_from: Optional[int] = None):
-        """g/=mb -> L2 normalization -> clip -> updater at the layer's lr -> +l2*W -> theta -= g -> constraints.  (SURVEY.md 8a row a9.)"""
+        """g/=mb -> L2 normalization -> clip -> updater at the layer's lr -> +l2*W -> theta -= g -> theta -= the l1 and l2Bias terms ->
+        constraints.  (SURVEY.md 8a row a9.)"""
         t = self.iteration + 1
         live = [(li, l) for li, l in enumerate(self.layers)
                 if l.has_params and not getattr(l, "frozen", False)]     # FrozenLayer: no gradient, no update, no l2 decay
@@ -1582,19 +2190,25 @@ class Net:
                 if self.grad_clip > 0 and (not noop or self.q.bn_stats_clipped):
                     g = np.clip(g, -self.grad_clip, self.grad_clip)
                 upd = g if noop else update(u, self.state.get((li, pname)), g, t, self.q, lr)
+                l1, l2 = self.reg_coefs(l, pname)
+                l2_bias = l2 if pname == "b" else 0.0
+                before = l.params[pname]
                 if l.l2 and pname in l.l2_names():
                     if self.q.l2_after_updater:
-                        upd = upd + l.l2 * l.params[pname]
+                        upd = upd + l.l2 * before
                     else:
                         raise NotImplementedError("only the pre-beta4 post-updater l2 form is restated")
-                l.params[pname] = (l.params[pname] - upd).astype(self.dtype)
+                l.params[pname] = (before - upd).astype(self.dtype)
+                if l1 or l2_bias:
+                    t_reg = (l2_bias * before if l2_bias else 0.0) + (l1 * np.sign(before) if l1 else 0.0)
+                    l.params[pname] = (l.params[pname] - t_reg).astype(self.dtype)
         self.iteration += 1
         if self.layer_constraints:
             self.apply_constraints()
 
-    def fit(self, x, y):
-        """ComputationGraph.fit(DataSet) for one minibatch (Solver -> StochasticGradientDescent.optimize)."""
-        score = self.compute_gradient_and_score(x, y)
+    def fit(self, x, y, mask=None):
+        """ComputationGraph.fit(DataSet) for one minibatch (Solver -> StochasticGradientDescent.optimize); mask: the labels mask."""
+        score = self.compute_gradient_and_score(x, y, mask=mask)
         self.apply_update(x.shape[0])
         return score
 
@@ -1617,7 +2231,7 @@ def parameter_average(nets: Sequence[Net], into: Net):
 # --------------------------------------------------------------------------------------------------
 # The GAN step.
 # --------------------------------------------------------------------------------------------------
-def gan_step(G: Net, D: Net, x_real, z_d, z_g, y_real, y_fake, y_gen, fake_bn_train: bool = False):
+def gan_step(G: Net, D: Net, x_real, z_d, z_g, y_real, y_fake, y_gen, fake_bn_train: bool = False, *, m_real=None, m_fake=None, m_gen=None):
     """The aliased G+D adversarial step the CUDA path executes (what J:408-471 computes for one real batch
     when the three graphs dis / gan / gen share storage instead of exchanging 28 setParam copies, and the
     two D minibatches are combined as one averaged update instead of two Spark workers):
@@ -1630,8 +2244,10 @@ def gan_step(G: Net, D: Net, x_real, z_d, z_g, y_real, y_fake, y_gen, fake_bn_tr
       3. G grads through D on z_g with labels y_gen (J:465-471): G and D both run train-mode BN; D's
          parameters, running stats and updater state are NOT touched (the reference's lr-0 "frozen" copy
          is overwritten from dis next iteration, J:429-460); one G updater step.
-    D's DropoutLayers draw as the library draws them, which runs the two D minibatches as one 2N-row pass: the real and fake minibatches are
-    rows [0, N) and [N, 2N) of pass P, and the G step's D pass is P + 1 (the counter ends at P + 2).
+    D's DropoutLayers and weight noise draw as the library draws them, which runs the two D minibatches as one 2N-row pass: the real and fake
+    minibatches are rows [0, N) and [N, 2N) of pass P, and the G step's D pass is P + 1 (the counter ends at P + 2).  D's scheduled dropout
+    values and DropConnect p are read at D's counters in the D step and at G's in the G step's pass through D (the reference's stacked gan graph
+    counts its own fits).  m_real, m_fake, m_gen: the labels masks of the three loss evaluations (None: unmasked).
     Returns dict(loss_d_real, loss_d_fake, loss_g, x_fake).
     """
     n = x_real.shape[0]
@@ -1641,9 +2257,9 @@ def gan_step(G: Net, D: Net, x_real, z_d, z_g, y_real, y_fake, y_gen, fake_bn_tr
         D.dropout.pass_ = P + 1
     x_fake = G.forward(z_d, train=fake_bn_train)
     # --- D step
-    s_real = D.compute_gradient_and_score(x_real, y_real) - D.l2_score()
+    s_real = D.compute_gradient_and_score(x_real, y_real, mask=m_real) - D.l2_score()
     g_real = {(li, p): l.grads[p].copy() for li, l in enumerate(D.layers) if l.has_params for p, _, _ in l.param_specs()}
-    s_fake = D.compute_gradient_and_score(x_fake, y_fake) - D.l2_score()
+    s_fake = D.compute_gradient_and_score(x_fake, y_fake, mask=m_fake) - D.l2_score()
     g_sum = {}
     for li, l in enumerate(D.layers):
         if not l.has_params:
@@ -1656,9 +2272,13 @@ def gan_step(G: Net, D: Net, x_real, z_d, z_g, y_real, y_fake, y_gen, fake_bn_tr
     D.apply_update(2 * n, grads=g_sum)
     # --- G step (through D, D untouched)
     xg = G.forward(z_g, train=True)
-    D.forward(xg, train=True)
+    D.dropout.lead = G
+    try:
+        D.forward(xg, train=True)
+    finally:
+        D.dropout.lead = None
     d_params_before = {(li, p): l.params[p] for li, l in enumerate(D.layers) if l.has_params for p, _, _ in l.param_specs()}
-    loss_sum, eps_x, _ = D._loss_backward(y_gen)
+    loss_sum, eps_x, _ = D._loss_backward(y_gen) if m_gen is None else D._loss_backward(y_gen, m_gen)
     G.backward_from(eps_x.reshape(xg.shape))
     G.apply_update(n)
     for (li, p), v in d_params_before.items():
@@ -1820,17 +2440,23 @@ def net_from_specs(specs, input_shape, *, quirks: Quirks = DEFAULT_QUIRKS, dtype
                    mask_seed=666, rank=0, constraints: Optional[Sequence[Dict]] = None) -> Net:
     """The Net of the layer specs the CUDA engine consumes.  input_shape: (C,H,W) or (F,).  flat_input: prepend the convolutionalFlat
     reshape (the oracle's layer indices are then the specs' + 1).  A spec's scheduled lr becomes the layer's schedule; its constant lr is
-    the schedule's value at 0, as the library keeps it.  An activation's alpha defaults as engine.layer_desc fills it.  A DropoutLayer's
-    mask index is its position in `specs` (the library's index).  A vertex's inputs are resolved by vertex_inputs.  mask_seed, rank: see Net.
-    A spec's "constraints" are its layer's; constraints: the global builder's, for every layer whose own reach none of its parameters, as
-    DL4J's builder fills them in."""
+    the schedule's value at 0, as the library keeps it.  An activation's alpha defaults as engine.layer_desc fills it.  Each layer's `index`
+    is its position in `specs` (the library's index, the L of its draws).  A vertex's inputs are resolved by vertex_inputs.  mask_seed, rank:
+    see Net.  A spec's "constraints" are its layer's; constraints: the global builder's, for every layer whose own reach none of its
+    parameters, as DL4J's builder fills them in.  A GEMM or PReLU spec's "l1", "l1_bias" and "l2_bias" are the net's layer_regularization
+    (its "l2" the layer's); a GEMM
+    spec's "weight_noise" is its layer's, and its "weight_init" replaces the seeded draw as b2g_net_init_weights does right after creation
+    (seed mask_seed).  The last spec's "loss_weights" are the net's."""
     layers, by_layer = [], {}
     shape = (1,) + tuple(input_shape)
     if len(input_shape) == 3 and flat_input:
         layers.append(Reshape(tuple(input_shape), name="in_reshape"))      # convolutionalFlat accepts [N,784] or [N,1,28,28]
     shapes = [shape] * len(layers)          # each layer's output shape
     skips = vertex_inputs(specs, len(layers))
-    schedules = {}
+    schedules, inits, regs = {}, [], {}
+    for s in specs[:-1]:
+        if s.get("loss_weights") is not None:
+            raise ValueError("loss_weights belong to the net's last (loss) layer")
     for i, s in enumerate(specs):
         t, name = s["type"], s.get("name", "")
         u = updater_cfg(s.get("updater"))
@@ -1872,16 +2498,31 @@ def net_from_specs(specs, input_shape, *, quirks: Quirks = DEFAULT_QUIRKS, dtype
             l = GlobalPooling(s.get("pooling", "max"), s.get("pnorm", 2), name)
         elif t == "upsample2d":
             l = Upsample2D(s.get("size", 2), name)
+        elif t == "prelu":
+            l = PReLU(shape[1:], s.get("shared_axes", ()), u, s.get("l2", 0.0), name)
         elif t == "dropout":
-            l = Dropout(s["p"], name, index=i)
+            kind = s.get("kind", "dropout")
+            v = s[VALUE_KEY[kind]]
+            sched = v if isinstance(v, dict) else None
+            l = Dropout(value(sched, 0) if sched else v, name, kind=kind, schedule=sched)
         elif t == "ff_to_cnn":
             h, w, c = s["to"]; l = Reshape((c, h, w), name)
         elif t == "cnn_to_ff":
             l = Reshape((int(np.prod(shape[1:])),), name)
         else:
             raise ValueError(t)
+        l.index = i
         if s.get("frozen", False):
             l.frozen = True
+        reg = tuple(float(s.get(k, 0.0)) for k in ("l1", "l1_bias", "l2_bias"))
+        if isinstance(l, GEMM + (PReLU,)) and any(reg):
+            regs[name] = reg
+        if isinstance(l, GEMM):
+            l.weight_noise = s.get("weight_noise")
+        if s.get("weight_init") is not None:
+            if not isinstance(l, GEMM):
+                raise NotImplementedError(f"{t} {name!r}: weight_init is restated on conv, deconv and dense layers")
+            inits.append((l, s["weight_init"]))
         per = constraints_by_param(l, s.get("constraints", ())) or constraints_by_param(l, constraints or ())
         if per:
             by_layer[name] = per
@@ -1889,9 +2530,14 @@ def net_from_specs(specs, input_shape, *, quirks: Quirks = DEFAULT_QUIRKS, dtype
         shape = l.out_shape(shape, shapes[l.src]) if isinstance(l, Vertex) else l.out_shape(shape)
         shapes.append(shape)
     net = Net(layers, seed=seed, dtype=dtype, grad_clip=grad_clip, quirks=quirks, mask_seed=mask_seed, rank=rank)
+    for l, wi in inits:
+        init_layer(l, wi, mask_seed, l.index, quirks)
     for name, sched in schedules.items():
         net.set_lr_schedule(sched, name)
-    net.layer_constraints = by_layer
+    net.layer_constraints, net.layer_regularization = by_layer, regs
+    if specs and specs[-1].get("loss_weights") is not None:
+        last = net.layers[-1]
+        net.set_loss_weights(check_weights(last.loss, specs[-1]["loss_weights"], shape[1], quirks))
     return net
 
 

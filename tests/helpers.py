@@ -263,15 +263,13 @@ def inject_forward(onet, bnet, specs, x_in, batch, what):
 
 
 def w_internal(spec, w_dl4j):
-    """A GEMM layer's W from DL4J's flattened view to the engine's internal [A][taps][B] order (conv [nOut][kH*kW][nIn], transposed conv
-    [nIn][kH*kW][nOut]; dense 'f'-order [nIn,nOut] already is [nOut][nIn])."""
+    """A GEMM layer's W from DL4J's flattened view to the engine's internal order (o.internal_w; dense 'f'-order [nIn,nOut] already is
+    [nOut][nIn])."""
     w = np.asarray(w_dl4j).ravel()
-    k = spec.get("kernel", (1, 1))
-    taps = k[0] * k[1]
-    if spec["type"] in ("dense", "output") or taps == 1:
+    if spec["type"] in ("dense", "output"):
         return w
-    a = spec["n_out"] if spec["type"] == "conv2d" else spec["n_in"]
-    return w.reshape(a, -1, taps).transpose(0, 2, 1).ravel()
+    a, b = (spec["n_out"], spec["n_in"]) if spec["type"] == "conv2d" else (spec["n_in"], spec["n_out"])
+    return o.internal_w(w.reshape((a, b) + tuple(spec.get("kernel", (1, 1)))))
 
 
 def pack_deconv_ps(w):

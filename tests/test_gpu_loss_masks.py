@@ -1,5 +1,5 @@
-"""Per-output loss weights and labels masks on the GPU (semantics at b2g_loss in include/b200gan.h): FP32 nets against the restatement
-(loss_mask_ref) over 3 fits with a ragged batch -- a weighted MCXENT classifier, a U-Net with weighted MCXENT and a per-pixel mask, a PatchGAN
+"""Per-output loss weights and labels masks on the GPU (semantics at b2g_loss in include/b200gan.h): FP32 nets against the oracle
+over 3 fits with a ragged batch -- a weighted MCXENT classifier, a U-Net with weighted MCXENT and a per-pixel mask, a PatchGAN
 discriminator with a mask, every loss code on OutputLayer / LossLayer / CnnLossLayer with per-example and per-output masks; all-ones weights and
 mask give the unweighted bits; the masked PatchGAN step against the restatement, BF16 graph replay against eager, new mask contents without
 re-capture, the unmasked step's launch count; and the refusals."""
@@ -8,7 +8,6 @@ import copy
 import numpy as np
 import pytest
 
-import loss_mask_ref as lm
 from gan_deeplearning4j_b200 import models as m
 from helpers import b200, launches_per_step, oracle_gan_pair, pclose, push_params, randomize, rel_err
 from oracle import dl4j_oracle as o
@@ -54,7 +53,7 @@ def test_weighted_mcxent_classifier(b200):
     specs = [{"type": "dense", "name": "d", "n_out": 16, "activation": "tanh", "updater": m.adam(0.01)},
              {"type": "output", "name": "out", "n_out": 5, "loss": "mcxent", "updater": m.adam(0.01), "loss_weights": [0.5, 1.0, 2.0, 0.25, 1.5]}]
     rng = np.random.default_rng(1)
-    onet = lm.net_from_specs(specs, (12,), seed=2); randomize(onet, rng)
+    onet = o.net_from_specs(specs, (12,), seed=2); randomize(onet, rng)
     bnet = b.Net(ctx, specs, (12,), max_batch=6, precision=b.FP32)
     push_params(onet, bnet)
     mask = lambda r, s: np.where(r.uniform(0, 1, (s[0], 1)) < 0.3, 0.0, r.uniform(0.2, 1.0, (s[0], 1)))
@@ -70,7 +69,7 @@ def test_unet_weighted_mcxent_per_pixel_mask(b200):
             sp["updater"] = m.sgd(0.01)
     specs[-1]["loss_weights"] = [0.2, 1.0, 3.0]
     rng = np.random.default_rng(2)
-    onet = lm.net_from_specs(specs, (3, 16, 16), seed=2, flat_input=False); randomize(onet, rng)
+    onet = o.net_from_specs(specs, (3, 16, 16), seed=2, flat_input=False); randomize(onet, rng)
     bnet = b.Net(ctx, specs, (3, 16, 16), max_batch=6, precision=b.FP32)
     push_params(onet, bnet)
     mask = lambda r, s: (r.uniform(0, 1, (s[0], 1) + s[2:]) > 0.25).astype(np.float64)      # "void" pixels
@@ -109,11 +108,11 @@ def test_every_loss_weighted_and_masked(b200, kind, loss, act):
     b, ctx = b200
     c = 1 if loss == "xent" and kind != "cnn_loss" else 3
     specs, shape = _small_specs(kind, loss, act, c)
-    if loss not in lm.MQ.weightless_losses:
+    if loss not in o.DEFAULT_QUIRKS.weightless_losses:
         specs[-1]["loss_weights"] = [0.5, 2.0, 1.25][:c]
     rng = np.random.default_rng(len(kind) * 10 + len(loss))
     for per_output in ((False, True) if loss != "mcxent" else (False,)):
-        onet = lm.net_from_specs(specs, shape, seed=2, flat_input=False); randomize(onet, rng)
+        onet = o.net_from_specs(specs, shape, seed=2, flat_input=False); randomize(onet, rng)
         bnet = b.Net(ctx, specs, shape, max_batch=6, precision=b.FP32)
         push_params(onet, bnet)
         mask = lambda r, s: r.uniform(0, 1, s if per_output else (s[0], 1) + tuple(s[2:]))
@@ -162,7 +161,7 @@ def test_patch_discriminator_fit_with_mask(b200):
     b, ctx = b200
     _, ds = _patch_gan()
     rng = np.random.default_rng(6)
-    onet = lm.net_from_specs(ds, (3, 16, 16), seed=2); randomize(onet, rng)
+    onet = o.net_from_specs(ds, (3, 16, 16), seed=2); randomize(onet, rng)
     bnet = b.Net(ctx, ds, (3, 16, 16), max_batch=6, precision=b.FP32)
     push_params(onet, bnet)
     mask = lambda r, s: (r.uniform(0, 1, s) > 0.4).astype(np.float64)
@@ -171,7 +170,7 @@ def test_patch_discriminator_fit_with_mask(b200):
 
 
 def test_fp32_masked_patch_gan_step_matches_restatement(b200):
-    """3 masked steps: losses and both nets' parameters against loss_mask_ref.gan_step, graph replay and eager, the two bit for bit."""
+    """3 masked steps: losses and both nets' parameters against the oracle's gan_step, graph replay and eager, the two bit for bit."""
     b, ctx = b200
     size, z, n, lr_ = 16, 12, 8, 2e-3
     gs, ds = _patch_gan(size, z, lr_)
@@ -182,7 +181,7 @@ def test_fp32_masked_patch_gan_step_matches_restatement(b200):
     masks = [(rng.uniform(0, 1, (n, 1, 4, 4)) > 0.3) * rng.uniform(0.5, 1.0, (n, 1, 4, 4)) for _ in range(3)]
     results = {}
     for graph in (True, False):
-        Gc, Dc = copy.deepcopy(G), lm.to_mask_net(copy.deepcopy(D))
+        Gc, Dc = copy.deepcopy(G), copy.deepcopy(D)
         bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
         bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, precision=b.FP32, bn_groups=2)
         push_params(Gc, bG); push_params(Dc, bD)
@@ -190,7 +189,7 @@ def test_fp32_masked_patch_gan_step_matches_restatement(b200):
         gan.set_label_masks(*masks)
         ls = []
         for it in range(3):
-            r = lm.gan_step(Gc, Dc, *data[:3], *maps, *masks)
+            r = o.gan_step(Gc, Dc, *data[:3], *maps, m_real=masks[0], m_fake=masks[1], m_gen=masks[2])
             lo = gan.step(*data)
             ls.append(lo)
             want = np.array([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]])

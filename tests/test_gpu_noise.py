@@ -7,7 +7,6 @@ from fractions import Fraction
 import numpy as np
 import pytest
 
-import noise_ref as nr
 from gan_deeplearning4j_b200 import models as m
 from helpers import b200, bf16_round, push_params, randomize, rel_err
 from oracle import dl4j_oracle as o
@@ -63,7 +62,7 @@ def test_gaussian_kernels(b200, kind, sigma, prec, n):
     P = b.BF16 if prec == "bf16" else b.FP32
     rnd = bf16_round if prec == "bf16" else (lambda a: np.asarray(a, np.float32))
     x, dy = _inputs(n)
-    z64 = nr.dropout_normals(SEED, RANK, LAYER, PASS, 1, 1, 1, n).ravel()
+    z64 = o.dropout_normals(SEED, RANK, LAYER, PASS, 1, 1, 1, n).ravel()
     if kind == "gaussian_noise":
         z_dev, _ = _hook(b, ctx, b.FP32, kind, np.zeros_like(x), dy, 1.0)      # fmaf(1, z, 0) = z: the device's own draws
         noise, _ = _hook(b, ctx, b.FP32, kind, np.zeros_like(x), dy, sigma)    # read through x = 0
@@ -71,7 +70,7 @@ def test_gaussian_kernels(b200, kind, sigma, prec, n):
         ref = s * z64
     else:
         noise, _ = _hook(b, ctx, b.FP32, kind, np.ones_like(x), dy, sigma)     # y = 1 * m: read through x = 1
-        s = nr.gaussian_sigma(sigma)
+        s = o.gaussian_sigma(sigma)
         ref = 1 + np.float64(s) * z64
     noise = noise.ravel()
     tol = 8 * np.spacing(np.maximum(1, np.abs(z64)).astype(np.float32) * s).astype(np.float64)
@@ -94,7 +93,7 @@ def test_gaussian_kernels(b200, kind, sigma, prec, n):
 
 
 def _check_alpha(y, dx, x, dy, keep, p, rnd):
-    a, bb, ap = nr.alpha_coefficients(p)
+    a, bb, ap = o.alpha_coefficients(p)
     xs, es = rnd(x).ravel(), rnd(dy).ravel()
     assert np.array_equal(dx.ravel() != 0, keep)
     assert np.array_equal(dx.ravel(), np.where(keep, rnd(es * a), 0).astype(np.float32))
@@ -117,7 +116,7 @@ def test_bernoulli_kernels(b200, kind, p, prec, n):
         keep = o.dropout_mask(SEED, RANK, LAYER, PASS, 1, 1, 1, n, p).ravel()
         _check_alpha(y, dx, x, dy, keep, p, rnd)
     else:
-        keep = nr.spatial_mask(SEED, RANK, LAYER, PASS, 1, n, p).ravel()         # one row of n channels: j = c
+        keep = o.spatial_mask(SEED, RANK, LAYER, PASS, 1, n, p).ravel()         # one row of n channels: j = c
         s = np.float32(1) / np.float32(p)
         assert np.array_equal(y.ravel(), np.where(keep, rnd(rnd(x).ravel() * s), 0).astype(np.float32))
         assert np.array_equal(dx.ravel(), np.where(keep, rnd(rnd(dy).ravel() * s), 0).astype(np.float32))
@@ -134,7 +133,7 @@ def test_spatial_kernels_on_odd_maps(b200, C, prec):
     rows, h, w, p = 37, 5, 3, 0.6
     x, dy = _inputs(rows * h * w * C, (rows, h, w, C))
     y, dx = _hook(b, ctx, P, "spatial_dropout", x, dy, p)
-    keep = nr.spatial_mask(SEED, RANK, LAYER, PASS, rows, C, p)[:, None, None, :]
+    keep = o.spatial_mask(SEED, RANK, LAYER, PASS, rows, C, p)[:, None, None, :]
     s = np.float32(1) / np.float32(p)
     assert np.array_equal(y, np.where(keep, rnd(rnd(x) * s), 0).astype(np.float32))
     assert np.array_equal(dx, np.where(keep, rnd(rnd(dy) * s), 0).astype(np.float32))
@@ -155,7 +154,7 @@ def test_hook_identity_and_bad_arguments(b200):
                 _hook(b, ctx, b.FP32, kind, x, dy, v)
             assert e.value.code == -1
             with pytest.raises(b.B200GanError) as e:
-                b.Net(ctx, [{"type": "conv2d", "n_out": 4, "kernel": (1, 1)}, {"type": "dropout", "kind": kind, nr.VALUE_KEY[kind]: v},
+                b.Net(ctx, [{"type": "conv2d", "n_out": 4, "kernel": (1, 1)}, {"type": "dropout", "kind": kind, o.VALUE_KEY[kind]: v},
                             {"type": "cnn_to_ff"}, {"type": "output", "n_out": 1}], (3, 4, 4), max_batch=2)
             assert e.value.code == -1
     with pytest.raises(b.B200GanError) as e:          # SpatialDropout on a feed-forward input
@@ -166,7 +165,7 @@ def test_hook_identity_and_bad_arguments(b200):
 def _chain_specs(kind, value, frozen=False):
     u = m.adam(1e-2)
     noise = lambda name, where: ([] if kind is None or (kind == "spatial_dropout" and where == "ff") else
-                                 [{"type": "dropout", "name": name, "kind": kind, nr.VALUE_KEY[kind]: value, "frozen": frozen}])
+                                 [{"type": "dropout", "name": name, "kind": kind, o.VALUE_KEY[kind]: value, "frozen": frozen}])
     return (noise("n0", "map") +
             [{"type": "conv2d", "name": "c1", "n_out": 8, "kernel": (3, 3), "stride": (2, 2), "padding": (1, 1), "updater": u},
              {"type": "activation", "name": "a1", "activation": "lrelu", "alpha": 0.2}] + noise("n1", "map") +
@@ -187,7 +186,7 @@ def test_fp32_chain_matches_oracle_under_identical_draws(b200, kind, value):
     b, ctx = b200
     specs = _chain_specs(kind, value)
     rng = np.random.default_rng(3)
-    onet = nr.net_from_specs(specs, (3, 8, 8), mask_seed=41, seed=2); randomize(onet, rng)
+    onet = o.net_from_specs(specs, (3, 8, 8), mask_seed=41, seed=2); randomize(onet, rng)
     bnet = b.Net(ctx, specs, (3, 8, 8), max_batch=6, precision=b.FP32, seed=41)
     push_params(onet, bnet)
     x = rng.uniform(-1, 1, (6, 3, 8, 8)); y = rng.uniform(0, 1, (6, 1))
@@ -238,7 +237,7 @@ def test_identity_cases_launch_nothing_and_match_the_plain_net(b200):
 
 def _bf16_grad_err(b, ctx, specs, in_shape, n, seed, rng_seed):
     rng = np.random.default_rng(rng_seed)
-    onet = nr.net_from_specs(specs, in_shape, mask_seed=seed, quirks=o.Quirks(xent_clip_eps=0.0), seed=2); randomize(onet, rng)
+    onet = o.net_from_specs(specs, in_shape, mask_seed=seed, quirks=o.Quirks(xent_clip_eps=0.0), seed=2); randomize(onet, rng)
     bnet = b.Net(ctx, specs, in_shape, max_batch=n, precision=b.BF16, xent_clip_eps=0.0, seed=seed)
     push_params(onet, bnet)
     x = rng.uniform(-1, 1, (n,) + tuple(in_shape)); y = rng.uniform(0, 1, (n, 1))
@@ -294,7 +293,7 @@ def test_fp32_gan_step_with_instance_noise_graph_eager_and_oracle(b200):
     for graph in (False, True):
         rng = np.random.default_rng(5)
         G = o.net_from_specs(gs, (z,), seed=1)
-        D = nr.net_from_specs(ds, (3, size, size), seed=2, mask_seed=667)
+        D = o.net_from_specs(ds, (3, size, size), seed=2, mask_seed=667)
         randomize(G, rng); randomize(D, rng)
         bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
         bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, bn_groups=2, precision=b.FP32, seed=667)
@@ -357,7 +356,7 @@ def test_scheduled_instance_noise_gan_step(b200):
     for graph in (False, True):
         rng = np.random.default_rng(5)
         G = o.net_from_specs(gs, (z,), seed=1)
-        D = nr.net_from_specs(ds, (3, size, size), seed=2, mask_seed=667)
+        D = o.net_from_specs(ds, (3, size, size), seed=2, mask_seed=667)
         randomize(G, rng); randomize(D, rng)
         bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.FP32)
         bD = b.Net(ctx, ds, (3, size, size), max_batch=2 * n, bn_groups=2, precision=b.FP32, seed=667)
@@ -366,8 +365,8 @@ def test_scheduled_instance_noise_gan_step(b200):
         gan = b.Gan(bG, bD, use_cuda_graph=graph)
 
         def step(it, what):
-            assert bD.dropout_value("dis_instance_noise") == nr.dropout_value(D, "dis_instance_noise"), (graph, what, it)
-            r = nr.gan_step(G, D, *data)
+            assert bD.dropout_value("dis_instance_noise") == D.dropout_value("dis_instance_noise"), (graph, what, it)
+            r = o.gan_step(G, D, *data)
             lo = gan.step(*data)
             want = np.array([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]])
             assert np.all(np.abs(lo - want) < TOL * np.maximum(1, np.abs(want))), (graph, what, it, lo, want)
@@ -383,7 +382,7 @@ def test_scheduled_instance_noise_gan_step(b200):
         assert not np.array_equal(acts[0], acts[1]) and not np.array_equal(acts[1], acts[2])
         # EPOCH schedule: set once (a re-capture), then set_epoch on both nets moves the value inside the replays
         sched = m.step_schedule(0.25, 0.5, 1, type="epoch")
-        bD.set_dropout_schedule(sched, "dis_instance_noise"); nr.set_dropout_schedule(D, sched, "dis_instance_noise")
+        bD.set_dropout_schedule(sched, "dis_instance_noise"); D.set_dropout_schedule(sched, "dis_instance_noise")
         assert bD.specs[0]["stddev"] == sched
         for ep in (0, 2):
             for net in (bD, bG, D, G):
@@ -407,14 +406,14 @@ def test_scheduled_dropout_kinds_match_the_oracle(b200):
         specs = _chain_specs(kind, 0.5)
         for sp in specs:
             if sp["type"] == "dropout":
-                sp[nr.VALUE_KEY[kind]] = sched
+                sp[o.VALUE_KEY[kind]] = sched
         rng = np.random.default_rng(3)
-        onet = nr.net_from_specs(specs, (3, 8, 8), mask_seed=41, seed=2); randomize(onet, rng)
+        onet = o.net_from_specs(specs, (3, 8, 8), mask_seed=41, seed=2); randomize(onet, rng)
         bnet = b.Net(ctx, specs, (3, 8, 8), max_batch=6, precision=b.FP32, seed=41)
         push_params(onet, bnet)
         x = rng.uniform(-1, 1, (6, 3, 8, 8)); y = rng.uniform(0, 1, (6, 1))
         for it in range(2):
-            assert bnet.dropout_value("n1") == nr.dropout_value(onet, "n1"), (kind, it)
+            assert bnet.dropout_value("n1") == onet.dropout_value("n1"), (kind, it)
             so, sb = onet.fit(x, y), bnet.fit(x, y)
             assert abs(sb - so) < TOL * max(1, abs(so)), (kind, it, sb, so)
             assert rel_err(bnet.params(), onet.params_flat()) < 2 * TOL, (kind, it)

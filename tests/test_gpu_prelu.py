@@ -1,5 +1,5 @@
 """DL4J's PReLULayer on the device: the forward and backward kernels bit for bit against a CPU emulation of the documented order (every mask,
-both paths, FP32 and BF16, ragged shapes, poisoned outputs); FP32 fit against the oracle's restatement (prelu_ref) on MLP and conv + BatchNorm
+both paths, FP32 and BF16, ragged shapes, poisoned outputs); FP32 fit against the oracle's restatement on MLP and conv + BatchNorm
 nets with several updaters, l1 / l2 and a schedule, frozen PReLUs, parameter round trips and the engine's refusals; BF16 nets; the GAN step
 against the oracle (graph replay == eager), D's slopes untouched by the G step, a generator ending in a PReLU, and the launch count."""
 import copy
@@ -12,8 +12,6 @@ from gan_deeplearning4j_b200 import _lib, engine, models as m
 from helpers import (b200, bf16_round, check_weight_operands, compare_params_and_state, gan_step_parity, launches_per_step,  # noqa: F401
                      pclose, push_params, randomize, rel_err)
 from oracle import dl4j_oracle as o
-import prelu_ref as pr
-import weight_init_ref as wr
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
@@ -151,10 +149,10 @@ def _specs(net, kind, reg=True):
 
 def _oracle(specs, shape, seed):
     rng = np.random.default_rng(seed)
-    onet = pr.net_from_specs(specs, shape, seed=2)
+    onet = o.net_from_specs(specs, shape, seed=2)
     randomize(onet, rng)
     for l in onet.layers:
-        if isinstance(l, pr.PReLU):
+        if isinstance(l, o.PReLU):
             l.params["W"] = rng.uniform(-0.3, 0.6, l.alpha_shape)
     return onet, rng
 
@@ -247,7 +245,7 @@ def test_weight_init_and_refusals(b200):
     bnet.init_weights(m.weight_init("ones"), "p2")
     assert np.all(bnet.get_param("p2", "W", 12) == 1)
     bnet.init_weights(m.weight_init("distribution", m.uniform(0.1, 0.3)), "p1")
-    np.testing.assert_array_equal(bnet.get_param("p1", "W", 128), wr.draw("uniform", 0.1, 0.3, 128, 666, 1))
+    np.testing.assert_array_equal(bnet.get_param("p1", "W", 128), o.weight_init_draw("uniform", 0.1, 0.3, 128, 666, 1))
     bnet.init_weights(m.weight_init("xavier"))             # the global form leaves PReLU layers alone
     assert np.all(bnet.get_param("p2", "W", 12) == 1) and not np.array_equal(bnet.get_param("c1", "W", w_c1.size), w_c1)
     wi = engine.weight_init_struct(m.weight_init("relu"))
@@ -280,11 +278,11 @@ def test_bf16_nets(b200):
 # ------------------------------------------------------------------ the GAN step -------------------------------------------------------------
 def _gan_pair(gs, ds, size=16, z=12):
     rng = np.random.default_rng(5)
-    G = pr.net_from_specs(gs, (z,), seed=1); D = pr.net_from_specs(ds, (3, size, size), seed=2)
+    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
     randomize(G, rng); randomize(D, rng)
     for net in (G, D):
         for l in net.layers:
-            if isinstance(l, pr.PReLU):
+            if isinstance(l, o.PReLU):
                 l.params["W"] = rng.uniform(0.05, 0.3, l.alpha_shape)
     return G, D
 

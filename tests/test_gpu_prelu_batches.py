@@ -6,7 +6,7 @@ import pytest
 
 from gan_deeplearning4j_b200 import models as m
 from helpers import b200, compare_params_and_state, push_params, randomize  # noqa: F401
-import prelu_ref as pr
+from oracle import dl4j_oracle as o
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
@@ -15,10 +15,10 @@ LR = 2e-3
 
 def _oracle(specs, shape, seed):
     rng = np.random.default_rng(seed)
-    onet = pr.net_from_specs(specs, shape, seed=2)
+    onet = o.net_from_specs(specs, shape, seed=2)
     randomize(onet, rng)
     for l in onet.layers:
-        if isinstance(l, pr.PReLU):
+        if isinstance(l, o.PReLU):
             l.params["W"] = rng.uniform(-0.3, 0.6, l.alpha_shape)
     return onet, rng
 

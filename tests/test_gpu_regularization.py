@@ -7,9 +7,8 @@ import pytest
 
 from gan_deeplearning4j_b200 import models as m
 from helpers import (b200, bf16_gan, check_weight_operands, compare_params_and_state, gan_step_parity, launches_per_step,  # noqa: F401
-                     mlp_convbn_specs, pclose, push_params, randomize, rel_err, run_two_ranks)
+                     mlp_convbn_specs, oracle_gan_pair, pclose, push_params, randomize, rel_err, run_two_ranks)
 from oracle import dl4j_oracle as o
-import regularization_ref as rr
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
@@ -60,7 +59,7 @@ def _specs(net, kind, reg=REG):
 def _oracle(specs, shape, seed, grad_clip):
     """The oracle net with random biases / BatchNorm parameters and every 11th weight exactly 0 (sign 0)."""
     rng = np.random.default_rng(seed)
-    onet = rr.net_from_specs(specs, shape, seed=2, grad_clip=grad_clip)
+    onet = o.net_from_specs(specs, shape, seed=2, grad_clip=grad_clip)
     randomize(onet, rng)
     for l in onet.layers:
         if getattr(l, "params", None) and "W" in l.params:
@@ -192,15 +191,6 @@ def test_rejections(b200):
     net.close()
 
 
-def oracle_gan_pair(gs, ds, size=16, z=12):
-    """helpers.oracle_gan_pair with the regularized oracle nets: G (seed 1) and D (seed 2), both randomized from default_rng(5), G first."""
-    rng = np.random.default_rng(5)
-    G = rr.net_from_specs(gs, (z,), seed=1)
-    D = rr.net_from_specs(ds, (3, size, size), seed=2)
-    randomize(G, rng); randomize(D, rng)
-    return G, D
-
-
 def _reg_gan_specs(reg_g, reg_d):
     gs, ds = m.dcgan_generator(16, 12, 8, 3, lr=2e-3), m.dcgan_discriminator(16, 8, 3, lr=2e-3)
     for specs, reg in ((gs, reg_g), (ds, reg_d)):
@@ -232,8 +222,9 @@ def test_a_change_between_replays_takes_effect(b200):
             bD.set_regularization(**REG); bG.set_regularization(l1=5e-3, layer=last)
             for l in D.layers:
                 if isinstance(l, (o.Conv2D, o.Dense)):
-                    l.l1, l.l2, l.l1_bias, l.l2_bias = REG["l1"], REG["l2"], REG["l1_bias"], REG["l2_bias"]
-            G.layer(last).l1 = 5e-3
+                    l.l2 = REG["l2"]
+                    D.layer_regularization[l.name] = (REG["l1"], REG["l1_bias"], REG["l2_bias"])
+            G.layer_regularization[last] = (5e-3,) + G.layer_regularization.get(last, (0.0, 0.0, 0.0))[1:]
         o.gan_step(G, D, *data)
         gan.step(*data)
         assert pclose(bD.params(), D.params_flat(), 2 * (2e-3 + REG["l1"])), (it, rel_err(bD.params(), D.params_flat()))

@@ -1,4 +1,4 @@
-"""Weight initialization (b2g_net_init_weights; b2g_weight_init in include/b200gan.h) on the GPU against tests/weight_init_ref.py: every
+"""Weight initialization (b2g_net_init_weights; b2g_weight_init in include/b200gan.h) on the GPU against the oracle's restatement: every
 scheme and distribution drawn on conv, deconv, dense and output layers in both precisions (bit for bit, the normal families within the fp32
 Box-Muller tolerance), the bf16 operands, what a call leaves alone, what a failed call leaves alone, determinism, and DCGAN training from
 Normal(0, 0.02) weights, eager and graph-replayed."""
@@ -10,7 +10,6 @@ import pytest
 
 from helpers import b200, check_weight_operands, gan_step_parity
 from oracle import dl4j_oracle as o
-import weight_init_ref as ir
 
 pytestmark = pytest.mark.gpu
 _ = b200
@@ -42,7 +41,7 @@ DISTS = {"normal": {"distribution": "normal", "mean": 0.01, "std": 0.02},
          "log_normal": {"distribution": "log_normal", "mean": -2.0, "std": 0.5},
          "binomial": {"distribution": "binomial", "n_trials": 5, "p": 0.25},
          "constant": {"distribution": "constant", "value": -0.125}}
-CASES = [(s, {"weight_init": s, "bias_init": 0.0625}) for s in ir.SCHEMES if s not in ("distribution", "identity")] + \
+CASES = [(s, {"weight_init": s, "bias_init": 0.0625}) for s in o.SCHEMES if s not in ("distribution", "identity")] + \
         [("dist_" + k, {"weight_init": "distribution", "distribution": d, "bias_init": -0.5}) for k, d in DISTS.items()]
 
 
@@ -50,13 +49,23 @@ def _gemm(specs):
     return [(i, s) for i, s in enumerate(specs) if s["type"] in ("conv2d", "deconv2d", "dense", "output")]
 
 
+def layer_of(spec):
+    """The oracle layer of a GEMM spec (n_in given): what fans() and the W shape come from."""
+    k, s, p = spec.get("kernel", (1, 1)), spec.get("stride", (1, 1)), spec.get("padding", (0, 0))
+    if spec["type"] == "conv2d":
+        return o.Conv2D(spec["n_in"], spec["n_out"], tuple(k), tuple(s), tuple(p))
+    if spec["type"] == "deconv2d":
+        return o.Deconv2D(spec["n_in"], spec["n_out"], tuple(k), tuple(s), tuple(p))
+    return o.Dense(spec["n_in"], spec["n_out"])
+
+
 def _check_layer(net, spec, li, wi, what):
     """get_param("W") against the restatement (bit for bit; normal families within 8 fp32 ulps of |std z| <= 6 std plus the rounding of the
     result; log-normal relative to its value), and every bias element equal to bias_init."""
-    layer = ir.layer_of(spec)
-    want = ir.weights(wi, layer, SEED, li)
+    layer = layer_of(spec)
+    want = o.weights(wi, layer, SEED, li)
     got = net.get_param(spec["name"], "W", want.size)
-    kind, a, b = ir.resolve(wi, layer)
+    kind, a, b = o.resolve(wi, layer)
     if kind in ("normal", "truncated_normal"):
         tol = 8 * np.spacing(np.float32(6 * float(b))) + 2 * np.spacing(np.abs(want))
         assert np.all(np.abs(got - want) <= tol), (what, spec["name"], np.max(np.abs(got - want)))

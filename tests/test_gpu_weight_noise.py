@@ -1,4 +1,4 @@
-"""Weight noise (DropConnect, WeightNoise; b2g_weight_noise in include/b200gan.h) on the GPU against tests/weight_noise_ref.py: the noisy
+"""Weight noise (DropConnect, WeightNoise; b2g_weight_noise in include/b200gan.h) on the GPU against the oracle's restatement: the noisy
 operands bit for bit (the Normal draws within the fp32 Box-Muller tolerance), FP32 training parity through every GEMM route of a small chain,
 the BF16 nets loosely, the adversarial step graph-replayed, eager and restated, and the launches and pass counter of the identity cases."""
 import numpy as np
@@ -7,7 +7,6 @@ import pytest
 from helpers import (b200, bf16_gan, bf16_round, fp32_gan_pair, gan_step_parity, launches_per_step, oracle_gan_pair, pack_deconv_ps, pclose,
                      push_params, randomize, rel_err, w_internal)
 from oracle import dl4j_oracle as o
-import weight_noise_ref as wr
 
 pytestmark = pytest.mark.gpu
 _ = b200
@@ -57,9 +56,9 @@ def test_noisy_operands_match_the_restatement(b200, prec, name, wn):
         nw, nb = _sizes(s)
         w = w_internal(s, theta[s["name"]][0]).astype(np.float32)
         bias = theta[s["name"]][1].astype(np.float32)
-        p = wr.drop_connect_p(wn, (1, 0)) if wn["weight_noise"] == "drop_connect" else None
-        ref_w = wr.apply(wn, w, wr.draw(wn, nw, 0, 21, 0, li, 1, p), p)
-        ref_b = wr.apply(wn, bias, wr.draw(wn, nb, wr.bias_j0(nw), 21, 0, li, 1, p), p)
+        p = o.drop_connect_p(wn, (1, 0)) if wn["weight_noise"] == "drop_connect" else None
+        ref_w = o.weight_noise_apply(wn, w, o.weight_noise_draw(wn, nw, 0, 21, 0, li, 1, p), p)
+        ref_b = o.weight_noise_apply(wn, bias, o.weight_noise_draw(wn, nb, o.bias_j0(nw), 21, 0, li, 1, p), p)
         got_w, got_b = net.noisy_operand(li, 0, nw), net.noisy_operand(li, 2, nb)
         for got, ref, what, bf in ((got_w, ref_w, "W", prec == "bf16"), (got_b, ref_b, "b", False)):
             want = bf16_round(ref) if bf else ref
@@ -97,7 +96,7 @@ def test_fp32_chain_follows_the_restatement(b200, name, wn):
     b, ctx = b200
     specs = _chain(wn)
     rng = np.random.default_rng(5)
-    onet = wr.net_from_specs(specs, (2, 8, 8), seed=3, mask_seed=11); randomize(onet, rng)
+    onet = o.net_from_specs(specs, (2, 8, 8), seed=3, mask_seed=11); randomize(onet, rng)
     net = b.Net(ctx, specs, (2, 8, 8), max_batch=6, precision=b.FP32, seed=11)
     push_params(onet, net)
     x = rng.uniform(-1, 1, (6, 2, 8, 8)); y = rng.uniform(0, 1, (6, 1))
@@ -117,7 +116,7 @@ def test_bf16_chain_follows_the_restatement_loosely(b200):
     b, ctx = b200
     specs = _operand_specs(DC)
     rng = np.random.default_rng(6)
-    onet = wr.net_from_specs(specs, (3, 8, 8), seed=3, mask_seed=21); randomize(onet, rng)
+    onet = o.net_from_specs(specs, (3, 8, 8), seed=3, mask_seed=21); randomize(onet, rng)
     net = b.Net(ctx, specs, (3, 8, 8), max_batch=8, precision=b.BF16, seed=21)
     push_params(onet, net)
     x = rng.uniform(-1, 1, (8, 3, 8, 8)); y = rng.uniform(0, 1, (8, 1))
@@ -128,15 +127,14 @@ def test_bf16_chain_follows_the_restatement_loosely(b200):
     net.close()
 
 
-def test_gan_step_graph_eager_and_restatement_agree(b200):
-    """FP32 16x16 GAN, DropConnect(0.9) on D and WeightNoise(Normal(0, 0.01)) on G: graph replay, eager and the restatement over 3 steps,
-    each step drawing anew (D's real | fake pass P, the generator pass P + 1)."""
+def test_gan_step_graph_eager_and_oracle_agree(b200):
+    """FP32 16x16 GAN, DropConnect(0.9) on D and WeightNoise(Normal(0, 0.01)) on G, both read from the specs: graph replay, eager and the
+    oracle over 3 steps, each step drawing anew (D's real | fake pass P, the generator pass P + 1)."""
     from gan_deeplearning4j_b200 import models as m
     b, ctx = b200
     gs = [dict(s, weight_noise=m.weight_noise(m.normal(0, 0.01))) if s["type"] in ("deconv2d", "dense") else s for s in m.dcgan_generator(16, 12, 8, 3, lr=2e-3)]
     ds = m.dcgan_discriminator(16, 8, 3, lr=2e-3, drop_connect=0.9)
     G, D = oracle_gan_pair(gs, ds)
-    wr.attach(G, gs); wr.attach(D, ds)
     data = [a.astype(np.float64) for a in o.synthetic_batch(8, 16, 3, 12, seed=3)]
     labels = tuple(data[3:])
     gan_step_parity(b, ctx, gs, ds, G, D, data, labels, 2e-3, "weight noise")

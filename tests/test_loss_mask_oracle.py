@@ -1,4 +1,4 @@
-"""The weighted / masked loss restatement (loss_mask_ref) on the CPU: finite differences for every (loss, activation) pair on OutputLayer,
+"""The oracle's weighted / masked losses on the CPU: finite differences for every (loss, activation) pair on OutputLayer,
 LossLayer, a CnnLossLayer on an odd map and a conv -> CnnLossLayer net; float64 torch for one-hot MCXENT and for XENT; hand-computed two-row
 answers; all-ones weights and mask reproduce the unweighted oracle bit for bit; the refusals; the spec key and a checkpoint round trip."""
 import copy
@@ -6,7 +6,6 @@ import copy
 import numpy as np
 import pytest
 
-import loss_mask_ref as lm
 from gan_deeplearning4j_b200 import models as m
 from gan_deeplearning4j_b200 import serializer
 from oracle import dl4j_oracle as o
@@ -29,7 +28,7 @@ def _labels(loss, rng, shape, axis=1):
 
 
 def _weights(loss, rng, c):
-    return None if loss in lm.MQ.weightless_losses else rng.uniform(0.2, 2.0, c)
+    return None if loss in o.DEFAULT_QUIRKS.weightless_losses else rng.uniform(0.2, 2.0, c)
 
 
 def _masks(loss, rng, rows_shape, full_shape):
@@ -90,9 +89,9 @@ def test_finite_differences_on_the_logits(kind, loss, act):
     for mk in _masks(loss, rng, rows_shape, full_shape) + [None]:
         def score(zz):
             layer._z = zz
-            return lm.layer_score_and_eps(layer, y, wts, mk)[0]
+            return layer.score_and_eps(y, wts, mk)[0]
         layer._z = z
-        _, g = lm.layer_score_and_eps(layer, y, wts, mk)
+        _, g = layer.score_and_eps(y, wts, mk)
         _fd_check(score, z.copy(), g)
 
 
@@ -107,7 +106,7 @@ def test_finite_differences_conv_to_cnn_loss_net(loss):
               "updater": m.sgd(0.1)},
              m.cnn_loss(loss, "tanh" if loss in ("mse", "l2") else "identity", name="cl", loss_weights=[0.5, 1.5, 1.0])]
     rng = np.random.default_rng(11)
-    net = lm.net_from_specs(specs, (2, 3, 5), seed=2, flat_input=False)
+    net = o.net_from_specs(specs, (2, 3, 5), seed=2, flat_input=False)
     x = rng.uniform(-1, 1, (2, 2, 3, 5)); y = _labels(loss, rng, (2, c, 3, 5))
     mk = rng.uniform(0, 1, (2, 1, 3, 5))
     net.compute_gradient_and_score(x, y, mask=mk)
@@ -130,13 +129,13 @@ def test_mcxent_one_hot_against_torch_cross_entropy():
     zt = torch.tensor(z, requires_grad=True)
     l = torch.nn.functional.cross_entropy(zt, torch.tensor(k), weight=torch.tensor(w), reduction="none")
     (l * torch.tensor(mk[:, 0])).sum().backward()
-    s, g = lm.rows_score_and_grad("mcxent", None, None, z, y, w, mk)
+    s, g = o.rows_score_and_grad("mcxent", None, None, z, y, w, mk)
     assert abs(s - float((l * torch.tensor(mk[:, 0])).sum().detach())) < 1e-12 * max(1, abs(s))
     assert np.allclose(g, zt.grad.numpy(), rtol=1e-12, atol=1e-14)
     # the plain weighted form, reduction="sum"
     zt.grad = None
     torch.nn.functional.cross_entropy(zt, torch.tensor(k), weight=torch.tensor(w), reduction="sum").backward()
-    s2, g2 = lm.rows_score_and_grad("mcxent", None, None, z, y, w, None)
+    s2, g2 = o.rows_score_and_grad("mcxent", None, None, z, y, w, None)
     assert np.allclose(g2, zt.grad.numpy(), rtol=1e-12, atol=1e-14)
 
 
@@ -147,7 +146,7 @@ def test_xent_with_logits_against_torch():
     zt = torch.tensor(z, requires_grad=True)
     l = torch.nn.functional.binary_cross_entropy_with_logits(zt, torch.tensor(y), weight=torch.tensor(w[None, :] * mk), reduction="sum")
     l.backward()
-    s, g = lm.rows_score_and_grad("xent", None, None, z, y, w, mk, o.Quirks(xent_clip_eps=0.0))
+    s, g = o.rows_score_and_grad("xent", None, None, z, y, w, mk, o.Quirks(xent_clip_eps=0.0))
     assert abs(s - float(l)) < 1e-12 * abs(s)
     assert np.allclose(g, zt.grad.numpy(), rtol=1e-12, atol=1e-14)
 
@@ -156,14 +155,14 @@ def test_hand_computed_two_rows():
     # MSE, nOut 2, identity: a = z.  Row scores (a - y)^2 / 2 per element, weights (2, 0.5), row mask (1, 0.5).
     z = np.array([[1.0, 2.0], [0.0, -1.0]]); y = np.array([[0.0, 0.0], [1.0, 1.0]])
     w = np.array([2.0, 0.5]); mk = np.array([[1.0], [0.5]])
-    s, g = lm.rows_score_and_grad("mse", "identity", 0.0, z, y, w, mk)
+    s, g = o.rows_score_and_grad("mse", "identity", 0.0, z, y, w, mk)
     # row 0: 2*1 + 0.5*4 = 4; row 1: 0.5 * (2*1 + 0.5*4) = 2; sum 6, / nOut = 3
     assert s == 3.0
     # dz = w m 2 (a - y) / 2
     assert np.array_equal(g, np.array([[2.0, 1.0], [-1.0, -0.5]]))
     # MCXENT, two classes, equal logits: p = 0.5.  Row 0 label class 0, row 1 label class 1; weights (3, 1); row 1 masked out.
     z = np.zeros((2, 2)); y = np.array([[1.0, 0.0], [0.0, 1.0]]); w = np.array([3.0, 1.0]); mk = np.array([[1.0], [0.0]])
-    s, g = lm.rows_score_and_grad("mcxent", None, None, z, y, w, mk)
+    s, g = o.rows_score_and_grad("mcxent", None, None, z, y, w, mk)
     assert abs(s - 3 * np.log(2)) < 1e-15
     # row 0: p * (sum w y = 3) - w y = (1.5 - 3, 1.5 - 0)
     assert np.array_equal(g, np.array([[-1.5, 1.5], [0.0, 0.0]]))
@@ -180,9 +179,9 @@ def test_all_ones_reproduce_the_oracle_bit_for_bit(loss):
     x = rng.uniform(-1, 1, (2, 2, 3, 5)); y = _labels(loss, rng, (2, 3, 3, 5))
     ref = o.net_from_specs(specs, (2, 3, 5), seed=2, flat_input=False)
     wspecs = copy.deepcopy(specs)
-    if loss not in lm.MQ.weightless_losses:
+    if loss not in o.DEFAULT_QUIRKS.weightless_losses:
         wspecs[-1]["loss_weights"] = [1.0, 1.0, 1.0]
-    net = lm.net_from_specs(wspecs, (2, 3, 5), seed=2, flat_input=False)
+    net = o.net_from_specs(wspecs, (2, 3, 5), seed=2, flat_input=False)
     for it in range(2):
         s0 = ref.fit(x, y)
         s1 = net.fit(x, y, mask=np.ones((2, 1, 3, 5)))
@@ -192,22 +191,22 @@ def test_all_ones_reproduce_the_oracle_bit_for_bit(loss):
 
 def test_refusals():
     with pytest.raises(NotImplementedError):
-        lm.check_weights("hinge", [1.0], 1)
+        o.check_weights("hinge", [1.0], 1)
     with pytest.raises(NotImplementedError):
-        lm.check_weights("wasserstein", [1.0], 1)
+        o.check_weights("wasserstein", [1.0], 1)
     with pytest.raises(ValueError):
-        lm.check_weights("mse", [1.0, 2.0], 3)
+        o.check_weights("mse", [1.0, 2.0], 3)
     with pytest.raises(ValueError):
-        lm.check_weights("mse", [1.0, np.inf], 2)
+        o.check_weights("mse", [1.0, np.inf], 2)
     with pytest.raises(NotImplementedError):
-        lm.check_mask("mcxent", np.ones((4, 3)), 4, 3)
+        o.check_mask("mcxent", np.ones((4, 3)), 4, 3)
     with pytest.raises(ValueError):
-        lm.check_mask("mse", np.ones((4, 2)), 4, 3)
+        o.check_mask("mse", np.ones((4, 2)), 4, 3)
     layer = o.CnnLossLayer("cl", loss="xent"); layer._z = np.zeros((2, 3, 3, 5))
     with pytest.raises(ValueError):
-        lm.layer_score_and_eps(layer, np.zeros((2, 3, 3, 5)), None, np.ones((2, 2, 3, 5)))
+        layer.score_and_eps(np.zeros((2, 3, 3, 5)), None, np.ones((2, 2, 3, 5)))
     with pytest.raises(ValueError):
-        lm.net_from_specs([{"type": "dense", "name": "d", "n_out": 2, "loss_weights": [1, 1]}, m.cnn_loss("xent")], (4,))
+        o.net_from_specs([{"type": "dense", "name": "d", "n_out": 2, "loss_weights": [1, 1]}, m.cnn_loss("xent")], (4,))
 
 
 def test_spec_key_and_checkpoint_round_trip(tmp_path):
@@ -238,22 +237,21 @@ def test_spec_key_and_checkpoint_round_trip(tmp_path):
 
 
 def test_gan_step_masks_reach_each_pass():
-    """The restatement's gan_step hands m_real, m_fake and m_gen to the D update's real and fake passes and to the G update, in that order:
-    zero masks on one pass zero its loss, and masks of ones reproduce o.gan_step bit for bit."""
+    """gan_step hands m_real, m_fake and m_gen to the D update's real and fake passes and to the G update, in that order: zero masks on one
+    pass zero its loss, masks of ones reproduce the unmasked step bit for bit, and no mask outlives its step."""
     size, z, n = 8, 4, 3
     gs = m.dcgan_generator(size, z, 4, 3, lr=1e-3)
     ds = m.dcgan_discriminator(size, 4, 3, lr=1e-3, patch=True)
     rng = np.random.default_rng(5)
     G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (3, size, size), seed=2)
     data = [a.astype(np.float64) for a in o.synthetic_batch(n, size, 3, z, seed=3)]
-    D2 = lm.to_mask_net(copy.deepcopy(D))
-    G2 = copy.deepcopy(G)
+    D2, G2 = copy.deepcopy(D), copy.deepcopy(G)
     out = o.net_from_specs(ds, (3, size, size), seed=2).output(data[0])
     maps = [np.broadcast_to(v.reshape(n, 1, 1, 1), (n,) + out.shape[1:]).copy() for v in data[3:]]
     ones = np.ones((n, 1) + out.shape[2:])
     r0 = o.gan_step(copy.deepcopy(G), copy.deepcopy(D), *data[:3], *maps)
-    r1 = lm.gan_step(copy.deepcopy(G2), copy.deepcopy(D2), *data[:3], *maps, ones, ones, ones)
+    r1 = o.gan_step(copy.deepcopy(G2), copy.deepcopy(D2), *data[:3], *maps, m_real=ones, m_fake=ones, m_gen=ones)
     assert (r0["loss_d_real"], r0["loss_d_fake"], r0["loss_g"]) == (r1["loss_d_real"], r1["loss_d_fake"], r1["loss_g"])
-    r2 = lm.gan_step(G2, D2, *data[:3], *maps, ones, 0 * ones, ones)
+    r2 = o.gan_step(G2, D2, *data[:3], *maps, m_real=ones, m_fake=0 * ones, m_gen=ones)
     assert r2["loss_d_fake"] == 0.0 and r2["loss_d_real"] == r0["loss_d_real"] and r2["loss_g"] != 0.0
-    assert D2.pass_masks == [] and not D2.in_gan_step
+    assert o.gan_step(G2, D2, *data[:3], *maps)["loss_d_fake"] != 0.0

@@ -8,7 +8,6 @@ import subprocess
 import numpy as np
 import pytest
 
-import noise_ref as nr
 from helpers import ROOT, randomize
 from oracle import dl4j_oracle as o
 
@@ -20,36 +19,36 @@ from oracle import dl4j_oracle as o
     (0xFFFFFFFF, 0x00000000, (0.00034526698814612303, 0.0)),       # u = 1 - 2^-24, the smallest r
 ], ids=["half", "quarter_turn", "tail", "center"])
 def test_box_muller_known_answers(xe, xo, want):
-    ze, zo = nr.box_muller(np.array([xe]), np.array([xo]))
+    ze, zo = o.box_muller(np.array([xe]), np.array([xo]))
     assert abs(ze[0] - want[0]) < 1e-12 and abs(zo[0] - want[1]) < 1e-12
-    assert abs(-5.768107546403532) == pytest.approx(nr.Z_MAX, rel=1e-15)
+    assert abs(-5.768107546403532) == pytest.approx(o.Z_MAX, rel=1e-15)
 
 
 def test_normals_follow_the_pairing_and_nchw_order():
     """Element e takes z[e & 3] of counter e >> 2: pair (x0, x1) gives z0, z1 and pair (x2, x3) z2, z3; NCHW result of the NHWC order."""
     seed, rank, layer, pass_ = 5, 1, 3, 9
-    z = nr.dropout_normals(seed, rank, layer, pass_, 2, 3, 5, 7)
+    z = o.dropout_normals(seed, rank, layer, pass_, 2, 3, 5, 7)
     assert z.shape == (2, 7, 3, 5)
     e = ((1 * 3 + 2) * 5 + 4) * 7 + 6             # (row 1, c 6, y 2, x 4)
     w = [int(v) for v in o.philox4x32_10((e >> 2, pass_, 0, layer | rank << 16), (seed, 0))]
     pair = (e & 3) >> 1
-    ze, zo = nr.box_muller(np.array([w[2 * pair]]), np.array([w[2 * pair + 1]]))
+    ze, zo = o.box_muller(np.array([w[2 * pair]]), np.array([w[2 * pair + 1]]))
     assert z[1, 6, 2, 4] == (zo if e & 1 else ze)[0]
-    assert np.array_equal(nr.dropout_normals(seed, rank, layer, pass_, 1, 3, 5, 7, row0=1), z[1:])
-    assert np.abs(z).max() <= nr.Z_MAX
+    assert np.array_equal(o.dropout_normals(seed, rank, layer, pass_, 1, 3, 5, 7, row0=1), z[1:])
+    assert np.abs(z).max() <= o.Z_MAX
 
 
 @pytest.mark.parametrize("p,a,b", [(0.5, 0.8864048946659319, 0.7791939305180315), (0.9, 0.9212845161497115, 0.16197097005757016)])
 def test_alpha_dropout_coefficients(p, a, b):
     """a = 1 / sqrt(p + a'^2 p (1 - p)) and b = -a (1 - p) a' with a' = -1.0507009873554805 * 1.6732632423543772 = -1.7580993408473766, the
     hand values at the decimal p; the layer takes p as fp32 (0.9 -> 0.899999976), hence the 1e-6 relative tolerance."""
-    ga, gb, gap = nr.alpha_coefficients(p)
+    ga, gb, gap = o.alpha_coefficients(p)
     assert gap == np.float32(-1.7580993408473766)
     assert abs(ga - a) <= 1e-6 * a and abs(gb - b) <= 1e-6 * b
 
 
 def _layer(kind, value, layer=2, seed=11):
-    l = nr.NoiseDropout(kind, value, "n", index=layer, state=o.DropoutState(seed))
+    l = o.Dropout(value, "n", index=layer, state=o.DropoutState(seed), kind=kind)
     l.last = True
     return l
 
@@ -77,7 +76,7 @@ def test_gaussian_noise_adds_sigma_z():
     x = np.random.default_rng(1).standard_normal((4, 3, 5, 6))
     l = _layer("gaussian_noise", 0.25)
     y = l.forward(x, True)
-    z = nr.dropout_normals(11, 0, 2, 0, 4, 5, 6, 3)
+    z = o.dropout_normals(11, 0, 2, 0, 4, 5, 6, 3)
     assert np.allclose(y, x + np.float32(0.25) * z, rtol=0, atol=1e-15)
     assert l.state.pass_ == 1 and np.array_equal(l.backward(x), x)
 
@@ -86,7 +85,7 @@ def test_spatial_dropout_zeroes_whole_maps():
     x = np.random.default_rng(2).uniform(0.5, 1.5, (16, 8, 5, 3))
     l = _layer("spatial_dropout", 0.5)
     y = l.forward(x, True)
-    keep = nr.spatial_mask(11, 0, 2, 0, 16, 8, 0.5)
+    keep = o.spatial_mask(11, 0, 2, 0, 16, 8, 0.5)
     assert 0 < keep.sum() < keep.size
     for r in range(16):
         for c in range(8):
@@ -111,7 +110,7 @@ def test_identity_cases_draw_nothing():
 
 def _chain(kind, value, first):
     """conv -> lrelu -> [noise] -> conv -> BN -> tanh -> cnn_to_ff -> dense -> [noise] -> output, or the noise as entry 0."""
-    noise = lambda name: {"type": "dropout", "name": name, "kind": kind, nr.VALUE_KEY[kind]: value}
+    noise = lambda name: {"type": "dropout", "name": name, "kind": kind, o.VALUE_KEY[kind]: value}
     dense_noise = [] if kind == "spatial_dropout" else [noise("n2")]
     return (([noise("n0")] if first else []) +
             [{"type": "conv2d", "name": "c1", "n_out": 4, "kernel": (3, 3), "stride": (2, 2), "padding": (1, 1)},
@@ -129,8 +128,8 @@ def test_finite_differences_with_fixed_draws(kind, value, first):
     max relative error 1e-3 and min absolute error 1e-8, over 30 parameters."""
     rng = np.random.default_rng(7)
     specs = _chain(kind, value, first)
-    net = nr.net_from_specs(specs, (2, 6, 6), mask_seed=3, seed=3); randomize(net, rng)
-    drops = [l for l in net.layers if isinstance(l, nr.NoiseDropout)]
+    net = o.net_from_specs(specs, (2, 6, 6), mask_seed=3, seed=3); randomize(net, rng)
+    drops = [l for l in net.layers if isinstance(l, o.Dropout)]
     assert drops and all(l.kind == kind for l in drops) and drops[-1].last
     x = rng.uniform(-1, 1, (4, 2, 6, 6)); y = rng.uniform(0, 1, (4, 1))
     net.compute_gradient_and_score(x, y, pass_=2)
@@ -201,13 +200,13 @@ def test_net_from_specs_agrees_with_the_library_specs():
     from gan_deeplearning4j_b200 import engine, models as m
     specs = m.dcgan_discriminator(16, 8, 3, instance_noise=0.1)
     specs = specs[:3] + [m.alpha_dropout(0.9, "ad"), m.spatial_dropout(0.7, "sd")] + specs[3:6] + [m.gaussian_dropout(0.3, "gd")] + specs[6:]
-    net = nr.net_from_specs(specs, (3, 16, 16))
+    net = o.net_from_specs(specs, (3, 16, 16))
     off = len(net.layers) - len(specs)
     for i, s in enumerate(specs):
         if s["type"] != "dropout":
             continue
         l, d = net.layers[off + i], engine.layer_desc(s)
-        assert isinstance(l, nr.NoiseDropout) and l.index == i
+        assert isinstance(l, o.Dropout) and l.index == i
         assert engine.DROPOUT_KINDS[l.kind][0] == d.act and np.float32(l.value) == np.float32(d.act_alpha)
     assert [l.last for l in net.layers if isinstance(l, o.Dropout)] == [False, False, False, True]
 
@@ -219,22 +218,19 @@ def test_schedule_values_at_chosen_iterations_and_epochs():
     l = _layer("gaussian_noise", 0.5)
     l.schedule = m.exponential_schedule(0.5, 0.9)
     for it in (0, 1, 7, 100):
-        l.state.counters = lambda it=it: (it, 0)
-        assert l.current_value() == np.float32(0.5 * 0.9 ** it) and l.active()
+        assert l.value_at(it, 0) == np.float32(0.5 * 0.9 ** it) and l.active()
     l.schedule = m.step_schedule(0.4, 0.5, 2, type="epoch")
     for ep, want in ((0, 0.4), (1, 0.4), (2, 0.2), (5, 0.1)):
-        l.state.counters = lambda ep=ep: (1000, ep)
-        assert l.current_value() == np.float32(want)
+        assert l.value_at(1000, ep) == np.float32(want)
     # clamping: rate to [0, 1 - 2^-24], p to [2^-32, 1], stddev to >= 0
-    assert nr.clamp_value("gaussian_dropout", 2.0) == np.float32(1 - 2.0 ** -24) and nr.clamp_value("gaussian_dropout", -1) == 0
-    assert nr.clamp_value("alpha_dropout", 0.0) == np.float32(2.0 ** -32) and nr.clamp_value("spatial_dropout", 3.0) == 1
-    assert nr.clamp_value("gaussian_noise", -0.5) == 0 and nr.clamp_value("dropout", 0.25) == np.float32(0.25)
+    assert o.clamp_value("gaussian_dropout", 2.0) == np.float32(1 - 2.0 ** -24) and o.clamp_value("gaussian_dropout", -1) == 0
+    assert o.clamp_value("alpha_dropout", 0.0) == np.float32(2.0 ** -32) and o.clamp_value("spatial_dropout", 3.0) == 1
+    assert o.clamp_value("gaussian_noise", -0.5) == 0 and o.clamp_value("dropout", 0.25) == np.float32(0.25)
     # a scheduled value of 0 still draws: the layer is stochastic whatever its value
     l = _layer("gaussian_noise", 0.0)
     assert not l.active()
     l.schedule = m.map_schedule({0: 0.0})
-    l.state.counters = lambda: (0, 0)
-    assert l.active() and l.current_value() == 0
+    assert l.active() and l.value_at(0, 0) == 0
 
 
 def test_gan_step_reads_g_counters_in_the_generator_pass():
@@ -244,18 +240,18 @@ def test_gan_step_reads_g_counters_in_the_generator_pass():
     gs = m.mlp_generator(z, hid, d, lr=1e-2)
     ds = m.mlp_discriminator(d, hid, lr=1e-2, instance_noise=m.exponential_schedule(0.4, 0.5))
     rng = np.random.default_rng(3)
-    G = o.net_from_specs(gs, (z,), seed=1); D = nr.net_from_specs(ds, (d,), seed=2)
+    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (d,), seed=2)
     randomize(G, rng); randomize(D, rng)
     seen = []
-    l = next(x for x in D.layers if isinstance(x, nr.NoiseDropout))
-    orig = l.current_value
-    l.current_value = lambda: (seen.append(orig()), seen[-1])[1]
+    l = next(x for x in D.layers if isinstance(x, o.Dropout))
+    orig = l.value_at
+    l.value_at = lambda it, ep: (seen.append(orig(it, ep)), seen[-1])[1]
     data = [rng.uniform(-1, 1, (n, d)), rng.uniform(-1, 1, (n, z)), rng.uniform(-1, 1, (n, z)), np.ones((n, 1)), np.zeros((n, 1)), np.ones((n, 1))]
     for _ in range(2):
-        nr.gan_step(G, D, *data)
+        o.gan_step(G, D, *data)
     # per step: the real and fake minibatches at D's counters, then the generator pass at G's (D's counter has already moved: 0.2, 0.1)
     assert seen == [np.float32(0.4)] * 3 + [np.float32(0.2)] * 3
-    assert nr.dropout_value(D, "dis_instance_noise") == np.float32(0.1)
+    assert D.dropout_value("dis_instance_noise") == np.float32(0.1)
 
 
 def test_schedule_symbols_are_exported_and_bound_and_specs_carry_schedules():

@@ -23,20 +23,19 @@ def fd_check(net, x, y, eps=1e-6, max_rel=1e-3, min_abs=1e-8, n_probe=60, seed=0
     net.compute_gradient_and_score(x, y, **kw)
     mb = x.shape[0]
     g = net.grads_flat() / mb
-    # l2 contributes l2*W to d(score)/dW; add analytically (DL4J's check includes it via the score)
+    # the regularization contributes l2 theta + l1 sign(theta) to d(score)/dtheta; added analytically (DL4J's check includes it via the score)
     p0 = net.params_flat().copy()
     rng = np.random.default_rng(seed)
     table = net.param_table()
     # skip BN mean/var slots (pseudo-gradients are not derivatives)
     mask = np.ones_like(p0, bool)
-    l2 = np.zeros_like(p0)
+    l1, l2 = np.zeros_like(p0), np.zeros_like(p0)
     off = 0
     for li, _, p, shape, _ in table:
         n = int(np.prod(shape))
         if p in net.layers[li].noop_names():
             mask[off:off + n] = False
-        if net.layers[li].l2 and p in net.layers[li].l2_names():
-            l2[off:off + n] = net.layers[li].l2
+        l1[off:off + n], l2[off:off + n] = net.reg_coefs(net.layers[li], p)
         off += n
     idx = rng.choice(np.flatnonzero(mask), size=min(n_probe, mask.sum()), replace=False)
     worst = 0.0
@@ -44,7 +43,7 @@ def fd_check(net, x, y, eps=1e-6, max_rel=1e-3, min_abs=1e-8, n_probe=60, seed=0
         pp = p0.copy(); pp[i] += eps; net.set_params_flat(pp); sp = net.compute_gradient_and_score(x, y, **kw)
         pm = p0.copy(); pm[i] -= eps; net.set_params_flat(pm); sm = net.compute_gradient_and_score(x, y, **kw)
         num = (sp - sm) / (2 * eps)
-        ana = g[i] + l2[i] * p0[i]
+        ana = g[i] + l2[i] * p0[i] + l1[i] * np.sign(p0[i])
         if abs(num - ana) < min_abs:
             continue
         rel = abs(num - ana) / (abs(num) + abs(ana))
@@ -105,6 +104,36 @@ def test_finite_differences_of_a_net_composing_the_later_features():
     assert net.iteration == 2 and net.dropout_pass() == 2
     assert net.learning_rate("c1") == net.learning_rate("d1") == np.float32(0.0125) and net.learning_rate("out") == 1e-2
     assert len(net.state[(0, "W")]) == 1 and np.all(np.isfinite(net.params_flat())) and not np.any(net.params_flat() == p0)
+
+
+def test_one_spec_list_mixes_regularization_weight_noise_prelu_scheduled_noise_and_masks():
+    """A conv with l1 / l1Bias / l2Bias and additive WeightNoise -> PReLU on shared axes -> scheduled GaussianDropout -> a weighted MCXENT
+    output with a labels mask, from one spec list: GradientCheckUtil's tolerances with every draw pinned to one pass (the conv's parameters
+    away from l1's kink), and one masked GAN step with it as D moves D's pass counter by two."""
+    from gan_deeplearning4j_b200 import models as m
+    specs = [{"type": "conv2d", "name": "c", "n_out": 3, "kernel": (3, 3), "padding": (1, 1), "activation": "tanh", "updater": m.sgd(0.1),
+              "l1": 1e-2, "l1_bias": 2e-2, "l2_bias": 3e-2, "weight_noise": m.weight_noise(m.normal(0.0, 0.05), apply_to_bias=True)},
+             dict(m.prelu((2, 3), "p"), updater=m.sgd(0.1), l1=1e-2, l2=2e-2),
+             m.gaussian_dropout(m.exponential_schedule(0.3, 0.5), "gd"),
+             {"type": "cnn_to_ff", "name": "f"},
+             {"type": "output", "name": "out", "n_out": 3, "loss": "mcxent", "updater": m.sgd(0.1), "loss_weights": [0.5, 1.0, 2.0]}]
+    D = o.net_from_specs(specs, (2, 5, 5), seed=4, mask_seed=9)
+    rng = np.random.default_rng(8)
+    for l in D.layers:
+        for p, shape, _ in l.param_specs():
+            v = rng.uniform(-0.5, 0.5, shape)
+            l.params[p] = v + 0.05 * np.sign(v)
+    assert [type(l) for l in D.layers[1:4]] == [o.Conv2D, o.PReLU, o.Dropout] and D.layers[1].weight_noise and D.loss_weights is not None
+    n = 4
+    x, y = rng.uniform(-1, 1, (n, 2, 5, 5)), np.eye(3)[rng.integers(0, 3, n)]
+    mask = rng.uniform(0.2, 1.0, (n, 1))
+    fd_check(D, x, y, n_probe=80, pass_=3, mask=mask)
+    assert D.dropout_pass() == 0
+    G = o.net_from_specs([{"type": "dense", "name": "g", "n_out": 50, "activation": "tanh", "updater": m.sgd(0.1)}], (6,), seed=5)
+    D.set_dropout_pass(5)
+    masks = [rng.uniform(0.2, 1.0, (n, 1)) for _ in range(3)]
+    r = o.gan_step(G, D, x, *rng.uniform(-1, 1, (2, n, 6)), y, y[::-1], y, m_real=masks[0], m_fake=masks[1], m_gen=masks[2])
+    assert np.isfinite([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]]).all() and D.dropout_pass() == 7
 
 
 def test_finite_differences_dcgan_tiny():

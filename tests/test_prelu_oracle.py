@@ -1,4 +1,4 @@
-"""PReLULayer on the CPU: the restatement (prelu_ref) against finite differences at GradientCheckUtil's tolerances for every shared-axes mask,
+"""PReLULayer on the CPU: the oracle's restatement against finite differences at GradientCheckUtil's tolerances for every shared-axes mask,
 in nets around it (conv -> PReLU -> dense, conv -> BatchNorm -> PReLU, PReLU first, a residual block of PReLUs) and against float64
 torch.autograd; known answers at the signed zeros and NaN; hand-computed updates with l1 / l2 and a schedule on alpha; the spec builders and
 their refusals."""
@@ -9,7 +9,6 @@ import torch.nn.functional as F
 
 from gan_deeplearning4j_b200 import engine, models as m
 from oracle import dl4j_oracle as o
-import prelu_ref as pr
 
 # GradientCheckUtil: epsilon 1e-6, max relative error 1e-3, min absolute error 1e-8
 EPS, MAX_REL, MIN_ABS = 1e-6, 1e-3, 1e-8
@@ -18,7 +17,7 @@ CONV_MASKS = [(), (1,), (2,), (3,), (1, 2), (1, 3), (2, 3), (1, 2, 3)]
 
 def _randomize_alpha(net, rng):
     for l in net.layers:
-        if isinstance(l, pr.PReLU):
+        if isinstance(l, o.PReLU):
             l.params["W"] = rng.uniform(-0.5, 0.8, l.alpha_shape)
         elif l.has_params:
             for p, shape, _ in l.param_specs():
@@ -55,7 +54,7 @@ def _grad_check(net, x, y):
 
 def _net(specs, shape, seed=3):
     rng = np.random.default_rng(seed)
-    net = pr.net_from_specs(specs, shape, seed=2)
+    net = o.net_from_specs(specs, shape, seed=2)
     _randomize_alpha(net, rng)
     return net, rng
 
@@ -102,7 +101,7 @@ def test_finite_differences_batchnorm_first_layer_and_residual():
 @pytest.mark.parametrize("axes", CONV_MASKS)
 def test_float64_autograd(axes):
     rng = np.random.default_rng(len(axes) + 10 * sum(axes))
-    l = pr.PReLU((3, 4, 5), axes)
+    l = o.PReLU((3, 4, 5), axes)
     l.init(rng, np.float64)
     l.params["W"] = rng.uniform(-0.5, 0.8, l.alpha_shape)
     x, e = rng.uniform(-1, 1, (2, 3, 4, 5)), rng.standard_normal((2, 3, 4, 5))
@@ -116,7 +115,7 @@ def test_float64_autograd(axes):
 
 
 def test_known_answers_signed_zero_and_nan():
-    l = pr.PReLU((6,), ())
+    l = o.PReLU((6,), ())
     l.init(np.random.default_rng(0), np.float64)
     l.params["W"] = np.full(6, 0.25)
     x = np.array([[0.0, -0.0, -2.0, 3.0, np.nan, -4.0]])
@@ -129,7 +128,7 @@ def test_known_answers_signed_zero_and_nan():
 
 
 def test_new_prelu_is_a_relu():
-    net = pr.net_from_specs([_prelu((1,)), {"type": "output", "name": "out", "n_out": 1, "updater": m.sgd(0.1)}], (5,), seed=1)
+    net = o.net_from_specs([_prelu((1,)), {"type": "output", "name": "out", "n_out": 1, "updater": m.sgd(0.1)}], (5,), seed=1)
     assert np.all(net.layers[0].params["W"] == 0) and net.layers[0].alpha_shape == (1,)
     x = np.linspace(-2, 2, 10).reshape(2, 5)
     np.testing.assert_array_equal(net.layers[0].forward(x, True), np.maximum(x, 0))
@@ -139,7 +138,7 @@ def test_new_prelu_is_a_relu():
 def test_hand_computed_update_with_l1_l2(l1, l2):
     lr, mb = 0.1, 2
     specs = [dict(_prelu((), l1=l1, l2=l2), updater=m.sgd(lr)), {"type": "output", "name": "out", "n_out": 1, "updater": m.sgd(0.0)}]
-    net = pr.net_from_specs(specs, (3,), seed=1)
+    net = o.net_from_specs(specs, (3,), seed=1)
     a0 = np.array([0.3, -0.2, 0.0])
     net.layers[0].params["W"] = a0.copy()
     x, y = np.array([[-1.0, -2.0, 3.0], [-0.5, 1.0, -1.0]]), np.array([[1.0], [0.0]])
@@ -156,7 +155,7 @@ def test_hand_computed_update_with_l1_l2(l1, l2):
 def test_schedule_value_on_the_prelu_layer():
     sched = m.exponential_schedule(0.1, 0.5)
     specs = [dict(m.prelu((), "p"), updater=m.sgd(sched)), {"type": "output", "name": "out", "n_out": 1, "updater": m.sgd(0.0)}]
-    net = pr.net_from_specs(specs, (2,), seed=1)
+    net = o.net_from_specs(specs, (2,), seed=1)
     assert net.schedules == {"p": sched}
     x, y = np.array([[-1.0, -2.0]]), np.array([[1.0]])
     for it in range(3):
@@ -204,7 +203,7 @@ def test_refusals():
         engine.weight_init_struct(m.weight_init(scheme), m.prelu(name="p"))
     engine.weight_init_struct(m.weight_init("distribution", m.normal(0.25, 0.01)), m.prelu(name="p"))
     with pytest.raises(ValueError):
-        pr.PReLU((5,), (2,))
+        o.PReLU((5,), (2,))
 
 
 def test_dcgan_prelu_specs_resolve_and_count():
@@ -217,17 +216,17 @@ def test_dcgan_prelu_specs_resolve_and_count():
             engine.resolve_vertices(specs)
             base = m.dcgan_generator(16, 12, 8, 3, residual=residual) if shape == (12,) else m.dcgan_discriminator(16, 8, 3, residual=residual)
             assert m.forward_macs(specs, shape) == m.forward_macs(base, shape)
-            net = pr.net_from_specs(specs, shape, seed=1)
-            assert sum(isinstance(l, pr.PReLU) for l in net.layers) == sum(s["type"] == "prelu" for s in specs)
+            net = o.net_from_specs(specs, shape, seed=1)
+            assert sum(isinstance(l, o.PReLU) for l in net.layers) == sum(s["type"] == "prelu" for s in specs)
         assert ds[0].get("activation", "identity") == "identity" and ds[1]["name"] == "dis_act_1" and ds[1]["type"] == "prelu"
 
 
 def test_oracle_gan_step_trains_both_nets_slopes():
     gs, ds = m.dcgan_generator(16, 12, 8, 3, lr=2e-3, activation="prelu"), m.dcgan_discriminator(16, 8, 3, lr=2e-3, activation="prelu")
-    G = pr.net_from_specs(gs, (12,), seed=1); D = pr.net_from_specs(ds, (3, 16, 16), seed=2)
+    G = o.net_from_specs(gs, (12,), seed=1); D = o.net_from_specs(ds, (3, 16, 16), seed=2)
     rng = np.random.default_rng(4)
     _randomize_alpha(G, rng); _randomize_alpha(D, rng)
-    before = {(net_i, l.name): l.params["W"].copy() for net_i, net in enumerate((G, D)) for l in net.layers if isinstance(l, pr.PReLU)}
+    before = {(net_i, l.name): l.params["W"].copy() for net_i, net in enumerate((G, D)) for l in net.layers if isinstance(l, o.PReLU)}
     r = o.gan_step(G, D, *[a.astype(np.float64) for a in o.synthetic_batch(4, 16, 3, 12, seed=3)])
     assert np.isfinite([r["loss_d_real"], r["loss_d_fake"], r["loss_g"]]).all()
     for (net_i, name), w in before.items():
@@ -237,7 +236,7 @@ def test_oracle_gan_step_trains_both_nets_slopes():
 def test_checkpoint_specs_round_trip(tmp_path):
     from gan_deeplearning4j_b200 import serializer
     ds = m.dcgan_discriminator(16, 8, 3, activation="prelu") + [dict(m.prelu((1,), "extra", input_shape=(4,)), l1=1e-3, frozen=True)]
-    net = pr.net_from_specs(ds[:-1], (3, 16, 16), seed=1)
+    net = o.net_from_specs(ds[:-1], (3, 16, 16), seed=1)
     serializer.write_model(tmp_path / "d.zip", ds, (3, 16, 16), net.params_flat().astype(np.float32))
     back = serializer.read_model(tmp_path / "d.zip")
     assert back["specs"] == [json_like(s) for s in ds]

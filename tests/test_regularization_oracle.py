@@ -1,7 +1,6 @@
-"""The restated regularization (tests/regularization_ref.py: l1, l2, l1Bias and l2Bias on top of the oracle; b2g_regularization in
-include/b200gan.h): hand-computed one-element updates for every updater kind and every sign of theta, the term apply_update adds against
-finite differences and float64 torch.autograd of the score's terms, BatchNorm and frozen layers, which take none, and l2-only nets, which
-train exactly as the oracle's own."""
+"""The oracle's regularization (l1, l2, l1Bias and l2Bias; b2g_regularization in include/b200gan.h): hand-computed one-element updates for
+every updater kind and every sign of theta, the term apply_update adds against finite differences and float64 torch.autograd of the score's
+terms, BatchNorm and frozen layers, which take none, and l2-only nets, which train exactly as specs without the other coefficients."""
 import copy
 import math
 
@@ -11,7 +10,6 @@ import torch
 
 from gan_deeplearning4j_b200 import models as m
 from oracle import dl4j_oracle as o
-import regularization_ref as rr
 
 KINDS = ("sgd", "rmsprop", "adam", "noop") + o.EXT_UPDATERS
 REG = {"l1": 0.03, "l2": 0.2, "l1_bias": 0.05, "l2_bias": 0.4}
@@ -49,7 +47,7 @@ def first_step(kind, g):
 
 
 def one_element_net(kind, reg):
-    return rr.net_from_specs([{"type": "output", "name": "out", "n_in": 1, "n_out": 1, "updater": copy.deepcopy(UPD[kind]), **reg}], (1,))
+    return o.net_from_specs([{"type": "output", "name": "out", "n_in": 1, "n_out": 1, "updater": copy.deepcopy(UPD[kind]), **reg}], (1,))
 
 
 @pytest.mark.parametrize("kind", KINDS)
@@ -90,7 +88,7 @@ def reg_net(frozen_first=False):
         if s["type"] in ("conv2d", "deconv2d", "dense", "output"):
             s.update(REG, updater=m.sgd(0.1))
     specs[0]["frozen"] = frozen_first
-    net = rr.net_from_specs(specs, (2, 6, 6), seed=4)
+    net = o.net_from_specs(specs, (2, 6, 6), seed=4)
     rng = np.random.default_rng(1)
     for l in net.layers:
         for p, shape, _ in l.param_specs():
@@ -110,8 +108,9 @@ def live_gemm(net):
 def test_added_term_is_the_gradient_of_the_score_terms():
     net = reg_net()
     plain = copy.deepcopy(net)
+    plain.layer_regularization = {}
     for l in plain.layers:
-        l.l1 = l.l2 = l.l1_bias = l.l2_bias = 0.0
+        l.l2 = 0.0
     grads = {(li, p): np.zeros(shape) for li, l in enumerate(net.layers) for p, shape, _ in l.param_specs()}
     net.apply_update(1, grads=copy.deepcopy(grads)); plain.apply_update(1, grads=copy.deepcopy(grads))
     fresh = reg_net()
@@ -136,7 +135,7 @@ def test_score_terms_against_torch_autograd():
     for li, l in live_gemm(net):
         for p in ("W", "b"):
             t = torch.tensor(net.layers[li].params[p], dtype=torch.float64, requires_grad=True)
-            c1, c2 = (l.l1, l.l2) if p == "W" else (l.l1_bias, l.l2_bias)
+            c1, c2 = net.reg_coefs(l, p)
             a, q = c1 * t.abs().sum(), 0.5 * c2 * (t * t).sum()
             (a + q).backward()
             l1, l2 = l1 + a.item(), l2 + q.item()
@@ -152,7 +151,7 @@ def test_score_terms_against_torch_autograd():
 def test_batchnorm_and_frozen_layers_take_no_term():
     net = reg_net()
     bn = net.layer("bn")
-    assert all(rr.reg_coefs(bn, p) == (0.0, 0.0) for p, _, _ in bn.param_specs())
+    assert all(net.reg_coefs(bn, p) == (0.0, 0.0) for p, _, _ in bn.param_specs())
     before = {p: v.copy() for p, v in bn.params.items()}
     zeros = {(li, p): np.zeros(s) for li, l in enumerate(net.layers) for p, s, _ in l.param_specs()}
     net.apply_update(1, grads=copy.deepcopy(zeros))
@@ -169,8 +168,7 @@ def test_batchnorm_and_frozen_layers_take_no_term():
 def test_l2_only_nets_keep_their_update_and_score():
     """With l1 = l1Bias = l2Bias = 0 the update and the score are the l2-only ones: W -= lr g + l2 W, b -= lr g, score term 0.5 l2 ||W||^2."""
     net = reg_net()
-    for l in net.layers:
-        l.l1 = l.l1_bias = l.l2_bias = 0.0
+    net.layer_regularization = {}
     want = sum(0.5 * l.l2 * float((l.params["W"] ** 2).sum()) for _, l in live_gemm(net))
     assert net.l2_score() == want and net.calc_l1() == 0.0
     fc = net.layer("fc")
@@ -181,12 +179,14 @@ def test_l2_only_nets_keep_their_update_and_score():
 
 
 def test_l2_only_specs_train_bit_for_bit_as_the_oracle():
+    """Zero l1, l1Bias and l2Bias train exactly as specs that leave them out."""
     specs = copy.deepcopy(SPECS)
     for s in specs:
         if s["type"] in ("conv2d", "deconv2d", "dense", "output"):
             s.update(l2=0.2, updater=m.adam(0.01), constraints=[m.max_norm(0.5, ())])
     specs[1].pop("l1")
-    a, c = rr.net_from_specs(specs, (2, 6, 6), seed=4, grad_clip=0.5), o.net_from_specs(specs, (2, 6, 6), seed=4, grad_clip=0.5)
+    zeros = [dict(s, l1=0.0, l1_bias=0.0, l2_bias=0.0) if s["type"] in ("conv2d", "deconv2d", "dense", "output") else s for s in specs]
+    a, c = o.net_from_specs(zeros, (2, 6, 6), seed=4, grad_clip=0.5), o.net_from_specs(specs, (2, 6, 6), seed=4, grad_clip=0.5)
     assert np.array_equal(a.params_flat(), c.params_flat()) and a.layer_constraints == c.layer_constraints
     rng = np.random.default_rng(2)
     for _ in range(3):

@@ -1,5 +1,5 @@
 """Regularization in the layer specs: the global builder's coefficients and each layer's own (engine.resolve_regularization), argument
-errors, the restated net_from_specs (tests/regularization_ref.py), a checkpoint's specs, and the names across the header, Python, the JNI shim and the Java facade."""
+errors, the oracle's net_from_specs, a checkpoint's specs, and the names across the header, Python, the JNI shim and the Java facade."""
 import copy
 import os
 import re
@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 
 from gan_deeplearning4j_b200 import _lib, engine, models as m, serializer
-import regularization_ref as rr
+from oracle import dl4j_oracle as o
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REG = {"l1": 1e-3, "l2": 1e-4, "l1_bias": 2e-3, "l2_bias": 3e-4}
@@ -59,23 +59,24 @@ def test_unknown_key_and_zero():
 
 def test_oracle_reads_the_spec_keys():
     s = engine.resolve_regularization(specs(), REG)
-    net = rr.net_from_specs(s, (3, 8, 8))
+    net = o.net_from_specs(s, (3, 8, 8))
     for name in ("c1", "c2", "fc", "out"):
         l, sp = net.layer(name), next(x for x in s if x["name"] == name)
-        assert (l.l1, l.l2, l.l1_bias, l.l2_bias) == tuple(float(sp.get(k, 0.0)) for k in engine.REGULARIZATION_KEYS)
-        assert rr.reg_coefs(l, "W") == (l.l1, l.l2) and rr.reg_coefs(l, "b") == (l.l1_bias, l.l2_bias)
+        l1, l1_bias, l2_bias = net.layer_regularization.get(name, (0.0, 0.0, 0.0))
+        assert (l1, l.l2, l1_bias, l2_bias) == tuple(float(sp.get(k, 0.0)) for k in engine.REGULARIZATION_KEYS)
+        assert net.reg_coefs(l, "W") == (l1, l.l2) and net.reg_coefs(l, "b") == (l1_bias, l2_bias)
     assert net.layer("c1").frozen
 
 
 def test_checkpoint_carries_the_specs(tmp_path):
     s = engine.resolve_regularization(specs(), REG)
-    onet = rr.net_from_specs(s, (3, 8, 8))
+    onet = o.net_from_specs(s, (3, 8, 8))
     path = str(tmp_path / "reg.zip")
     serializer.write_model(path, s, (3, 8, 8), onet.params_flat().astype(np.float32))
     back = serializer.read_model(path)["specs"]
     for a, c in zip(s, back):
         assert engine.spec_regularization(a) == engine.spec_regularization(c), a["name"]
-    again = rr.net_from_specs(back, (3, 8, 8))
+    again = o.net_from_specs(back, (3, 8, 8))
     onet.set_params_flat(onet.params_flat())
     again.set_params_flat(onet.params_flat())
     assert again.calc_l1() == onet.calc_l1() and again.calc_l2() == onet.calc_l2() and onet.calc_l1() > 0

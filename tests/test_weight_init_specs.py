@@ -1,5 +1,5 @@
 """Weight initialization's host-side plumbing (b2g_weight_init in include/b200gan.h): the scheme and distribution numbers agree across the
-header, the Python dicts, the restatement and the Java facade; the builders refuse what the engine refuses, before any library call; a checkpoint round-trips the settings; the symbols are exported and
+header, the Python dicts, the oracle's restatement and the Java facade; the builders refuse what the engine refuses, before any library call; a checkpoint round-trips the settings; the symbols are exported and
 bound.  No GPU needed."""
 import os
 import re
@@ -8,7 +8,7 @@ import subprocess
 import numpy as np
 import pytest
 
-import weight_init_ref as ir
+from oracle import dl4j_oracle as o
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 JAVA = os.path.join(ROOT, "java", "src", "main", "java", "org", "deeplearning4j")
@@ -28,9 +28,9 @@ def test_scheme_numbers_agree_across_header_python_and_java():
     from gan_deeplearning4j_b200 import engine
     body = re.search(r"typedef enum \{([^}]*)\} b2g_weight_init_scheme;", _header()).group(1)
     header = {k.lower(): int(v) for k, v in re.findall(r"B2G_WI_(\w+) = (\d+)", body)}
-    assert header == {s: i for i, s in enumerate(ir.SCHEMES)} == engine.WEIGHT_INIT_SCHEMES
+    assert header == {s: i for i, s in enumerate(o.SCHEMES)} == engine.WEIGHT_INIT_SCHEMES
     java = re.search(r"enum WeightInit \{([^}]*)\}", _read("nn", "weights", "WeightInit.java")).group(1)
-    assert [w.strip().lower() for w in java.split(",")] == list(ir.SCHEMES)
+    assert [w.strip().lower() for w in java.split(",")] == list(o.SCHEMES)
 
 
 def test_distribution_numbers_agree_across_header_python_and_java():
@@ -39,7 +39,7 @@ def test_distribution_numbers_agree_across_header_python_and_java():
     body = re.search(r"typedef enum \{([^}]*)\} b2g_distribution_kind;", h).group(1)
     assert re.findall(r"B2G_DIST_(\w+) = (\d+)", body) == [("NORMAL", "0"), ("UNIFORM", "1")]     # weight noise's two, then the rest
     header = {k.lower(): int(v) for k, v in re.findall(r"B2G_DIST_(\w+) = (\d+)", h)}
-    assert header == {d: i for i, d in enumerate(ir.DISTRIBUTIONS)}
+    assert header == {d: i for i, d in enumerate(o.DISTRIBUTIONS)}
     assert {k: v[0] for k, v in engine.INIT_DISTRIBUTIONS.items()} == header
     # weight noise keeps its two
     assert {k: v[0] for k, v in engine.DISTRIBUTIONS.items()} == {"normal": 0, "uniform": 1}

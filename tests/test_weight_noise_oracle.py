@@ -1,4 +1,4 @@
-"""Weight noise (DropConnect, WeightNoise; b2g_weight_noise in include/b200gan.h) in the restatement tests/weight_noise_ref.py: known answers,
+"""Weight noise (DropConnect, WeightNoise; b2g_weight_noise in include/b200gan.h) in the oracle's restatement: known answers,
 the draws' statistics, straight-through gradients by finite differences with W' fixed, the pass counter shared with DropoutLayers, and the
 host-side plumbing (kind numbers, specs, models, checkpoints, exported symbols).  No GPU needed."""
 import copy
@@ -11,8 +11,6 @@ import pytest
 
 from helpers import randomize
 from oracle import dl4j_oracle as o
-import noise_ref as nr
-import weight_noise_ref as wr
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DC = {"weight_noise": "drop_connect", "p": 0.75, "apply_to_bias": False}
@@ -22,7 +20,8 @@ def _dense(n_in=6, n_out=5, wn=DC, seed=0):
     l = o.Dense(n_in, n_out, name="d")
     l.init(np.random.default_rng(seed), np.float64)
     l.params["b"] = np.arange(n_out, dtype=np.float64) / 10
-    net = wr.set_weight_noise(o.Net([l], mask_seed=9), wn)
+    net = o.Net([l], mask_seed=9)
+    net.set_weight_noise(wn)
     return net, l
 
 
@@ -30,35 +29,35 @@ def test_drop_connect_known_answer():
     """W' = keep ? W : +0 with keep = x[j & 3] < floor(p 2^32) of counter {j >> 2, P, L}, j the internal index; not rescaled by 1 / p; b' only
     with apply_to_bias, from j = 4 ceil(n_W / 4) on."""
     net, l = _dense()
-    w_int = wr.internal_w(l, l.params["W"]).astype(np.float32)
-    words = nr.philox_words(9, 0, 0, 0, 0, 40)
+    w_int = o.internal_w(l.params["W"]).astype(np.float32)
+    words = o.philox_words(9, 0, 40, *o.dropout_counter(0, 0, 0))
     thr = int(np.float32(0.75) * 2.0 ** 32)
     want = np.array([w if words[j] < thr else 0.0 for j, w in enumerate(w_int)], np.float32)
-    got, b = wr.noisy_operands(l, DC, 0, 9, 0, 0)
+    got, b = o.noisy_operands(l, DC, 0, 9, 0, 0)
     assert np.array_equal(got, want) and b is None
-    assert np.array_equal(wr.internal_w(l, wr.dl4j_w(l, got)), got)
+    assert np.array_equal(o.internal_w(o.dl4j_w(got, l.params["W"].shape)), got)
     wn = dict(DC, apply_to_bias=True)
-    _, b = wr.noisy_operands(l, wn, 0, 9, 0, 0)
+    _, b = o.noisy_operands(l, wn, 0, 9, 0, 0)
     bw = l.params["b"].astype(np.float32)
     assert np.array_equal(b, np.where(words[32:37] < thr, bw, np.float32(0)))        # j0 = 4 * ceil(30 / 4) = 32
-    inv = wr.WeightNoiseQuirks(dropconnect_inverted=True)
-    got_inv, _ = wr.noisy_operands(l, DC, 0, 9, 0, 0, q=inv)
+    inv = o.Quirks(dropconnect_inverted=True)
+    got_inv, _ = o.noisy_operands(l, DC, 0, 9, 0, 0, q=inv)
     assert np.array_equal(got_inv[want != 0], want[want != 0] / np.float32(0.75))
 
 
 def test_weight_noise_known_answers():
     """NORMAL n = std z + mean with z of the Box-Muller pairs; UNIFORM n = fmaf(upper - lower, (x >> 8) 2^-24, lower); additive or multiplicative."""
     _, l = _dense()
-    w = wr.internal_w(l, l.params["W"]).astype(np.float32)
-    words = nr.philox_words(9, 0, 3, 5, 0, 32).reshape(-1, 4)
+    w = o.internal_w(l.params["W"]).astype(np.float32)
+    words = o.philox_words(9, 0, 32, *o.dropout_counter(0, 3, 5)).reshape(-1, 4)
     z = np.empty(words.shape)
-    z[:, 0], z[:, 1] = nr.box_muller(words[:, 0], words[:, 1])
-    z[:, 2], z[:, 3] = nr.box_muller(words[:, 2], words[:, 3])
+    z[:, 0], z[:, 1] = o.box_muller(words[:, 0], words[:, 1])
+    z[:, 2], z[:, 3] = o.box_muller(words[:, 2], words[:, 3])
     wn = {"weight_noise": "weight_noise", "distribution": {"distribution": "normal", "mean": 0.5, "std": 0.01}, "additive": True}
-    got, _ = wr.noisy_operands(l, wn, 3, 9, 0, 5)
+    got, _ = o.noisy_operands(l, wn, 3, 9, 0, 5)
     assert np.array_equal(got, (w + (0.01 * z.ravel()[:30] + 0.5).astype(np.float32)).astype(np.float32))
     wn = {"weight_noise": "weight_noise", "distribution": {"distribution": "uniform", "lower": 0.9, "upper": 1.1}, "additive": False}
-    got, _ = wr.noisy_operands(l, wn, 3, 9, 0, 5)
+    got, _ = o.noisy_operands(l, wn, 3, 9, 0, 5)
     u = (words.ravel()[:30] >> np.uint64(8)).astype(np.float64) / 2 ** 24
     n = (float(np.float32(1.1) - np.float32(0.9)) * u + float(np.float32(0.9))).astype(np.float32)
     assert np.array_equal(got, w * n) and np.all((n >= np.float32(0.9)) & (n <= np.float32(1.1)))
@@ -67,11 +66,11 @@ def test_weight_noise_known_answers():
 def test_drop_connect_keep_fraction_is_the_counters():
     """Over 10^6 draws the kept count is exactly the number of words below the threshold, and within 5 sigma of p n."""
     n, p = 1 << 20, 0.9
-    keep = wr.draw(DC, n, 0, 7, 0, 2, 11, p)
-    words = nr.philox_words(7, 0, 2, 11, 0, n)
+    keep = o.weight_noise_draw(DC, n, 0, 7, 0, 2, 11, p)
+    words = o.philox_words(7, 0, n, *o.dropout_counter(0, 2, 11))
     assert keep.sum() == (words < np.uint64(int(np.float32(p) * 2.0 ** 32))).sum()
     assert abs(keep.sum() - p * n) < 5 * np.sqrt(n * p * (1 - p))
-    assert wr.draw(DC, 8, 0, 7, 0, 2, 11, 1.0).all()
+    assert o.weight_noise_draw(DC, 8, 0, 7, 0, 2, 11, 1.0).all()
 
 
 @pytest.mark.parametrize("dist", ["normal", "uniform"])
@@ -82,7 +81,7 @@ def test_noise_moments(dist):
         d, mean, var = {"distribution": "normal", "mean": 0.25, "std": 2.0}, 0.25, 4.0
     else:
         d, mean, var = {"distribution": "uniform", "lower": -1.0, "upper": 3.0}, 1.0, 16.0 / 12
-    x = wr.draw({"weight_noise": "weight_noise", "distribution": d}, n, 0, 666, 0, 1, 4).astype(np.float64)
+    x = o.weight_noise_draw({"weight_noise": "weight_noise", "distribution": d}, n, 0, 666, 0, 1, 4).astype(np.float64)
     assert abs(x.mean() - mean) < 5 * np.sqrt(var / n)
     fourth = 3 * var ** 2 if dist == "normal" else 9.0 / 5 * var ** 2
     assert abs(x.var() - var) < 5 * np.sqrt((fourth - var ** 2) / n)
@@ -113,7 +112,7 @@ def test_straight_through_gradients_by_finite_differences(wn):
     relative error 1e-3 and min absolute error 1e-8."""
     rng = np.random.default_rng(7)
     specs = _chain(wn)
-    net = wr.net_from_specs(specs, (2, 6, 6), mask_seed=3, seed=3); randomize(net, rng)
+    net = o.net_from_specs(specs, (2, 6, 6), mask_seed=3, seed=3); randomize(net, rng)
     x = rng.uniform(-1, 1, (4, 2, 6, 6)); y = rng.uniform(0, 1, (4, 1))
     theta = net.params_flat().copy()
     net.compute_gradient_and_score(x, y)
@@ -125,8 +124,8 @@ def test_straight_through_gradients_by_finite_differences(wn):
     off = len(net.layers) - len(specs)
     for i, s in enumerate(specs):
         l = net.layers[off + i]
-        if isinstance(l, wr.NoisyLayerMixin):
-            for k, v in l._wn_live.items():
+        if l.noisy is not None:
+            for k, v in l.noisy.items():
                 plain.layers[off + i].params[k] = v.copy()
     assert not np.array_equal(plain.params_flat(), theta)
     assert np.array_equal(net.params_flat(), theta)                     # the clean parameters are untouched
@@ -160,23 +159,25 @@ def test_inference_and_frozen_layers_draw_nothing():
     net, l = _dense()
     x = np.ones((2, 6))
     y0 = net.output(x)
-    assert net.dropout.pass_ == 0 and l._wn_live is None
-    assert np.array_equal(y0, o.Net.forward(net, x, False))
+    assert net.dropout.pass_ == 0 and l.noisy is None
+    clean = copy.deepcopy(net)
+    clean.set_weight_noise(None)
+    assert np.array_equal(y0, clean.forward(x, False))
     net.forward(x, True)
-    assert net.dropout.pass_ == 1 and l._wn_live is not None
+    assert net.dropout.pass_ == 1 and l.noisy is not None
     net.output(x)
-    assert l._wn_live is None
+    assert l.noisy is None
     l.frozen = True
     net.forward(x, True)
     assert net.dropout.pass_ == 1
     l.frozen = False
-    wr.set_weight_noise(net, dict(DC, p=1.0))
+    net.set_weight_noise(dict(DC, p=1.0))
     net.forward(x, True)
-    assert net.dropout.pass_ == 1 and not wr.active(l)
+    assert net.dropout.pass_ == 1 and not o.weight_noise_active(l)
     sched = {"schedule": "map", "values": [(0, 1.0)], "type": "iteration"}
-    wr.set_weight_noise(net, dict(DC, p=sched))
+    net.set_weight_noise(dict(DC, p=sched))
     net.forward(x, True)
-    assert net.dropout.pass_ == 2 and wr.active(l)             # a scheduled DropConnect draws whatever its value
+    assert net.dropout.pass_ == 2 and o.weight_noise_active(l)             # a scheduled DropConnect draws whatever its value
 
 
 def test_adding_weight_noise_leaves_dropout_masks_unchanged():
@@ -184,8 +185,8 @@ def test_adding_weight_noise_leaves_dropout_masks_unchanged():
     same with and without weight noise."""
     rng = np.random.default_rng(2)
     plain_specs = [{k: v for k, v in s.items() if k != "weight_noise"} for s in _chain(DC, dropout=True)]
-    a = nr.net_from_specs(plain_specs, (2, 6, 6), mask_seed=4, seed=3); randomize(a, rng)
-    b = wr.net_from_specs(_chain(DC, dropout=True), (2, 6, 6), mask_seed=4, seed=3); b.set_params_flat(a.params_flat())
+    a = o.net_from_specs(plain_specs, (2, 6, 6), mask_seed=4, seed=3); randomize(a, rng)
+    b = o.net_from_specs(_chain(DC, dropout=True), (2, 6, 6), mask_seed=4, seed=3); b.set_params_flat(a.params_flat())
     x = rng.uniform(-1, 1, (3, 2, 6, 6))
     da = next(l for l in a.layers if isinstance(l, o.Dropout)); db = next(l for l in b.layers if isinstance(l, o.Dropout))
     for step in range(3):
@@ -193,8 +194,8 @@ def test_adding_weight_noise_leaves_dropout_masks_unchanged():
         assert np.array_equal(da._m, db._m) and a.dropout.pass_ == b.dropout.pass_ == step + 1
     # each pass drew with the pass's P: the W' of the last pass is that of P = 2
     c1 = next(l for l in b.layers if l.name == "c1")
-    w, _ = wr.noisy_operands(c1, DC, 0, 4, 0, 2, dtype=np.float64)
-    assert np.array_equal(c1._wn_live["W"], wr.dl4j_w(c1, w))
+    w, _ = o.noisy_operands(c1, DC, 0, 4, 0, 2, dtype=np.float64)
+    assert np.array_equal(c1.noisy["W"], o.dl4j_w(w, c1.params["W"].shape))
 
 
 def test_gan_step_pass_bookkeeping():
@@ -205,23 +206,23 @@ def test_gan_step_pass_bookkeeping():
     gs = [dict(s, weight_noise=m.weight_noise(m.normal(0, 0.01))) for s in m.mlp_generator(z, hid, d, lr=1e-2)]
     ds = m.mlp_discriminator(d, hid, lr=1e-2, drop_connect=0.9)
     rng = np.random.default_rng(3)
-    G = wr.net_from_specs(gs, (z,), seed=1); D = wr.net_from_specs(ds, (d,), seed=2)
+    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (d,), seed=2)
     randomize(G, rng); randomize(D, rng)
     seen = []
-    orig = wr.noisy_operands
+    orig = o.noisy_operands
     l0 = D.layers[-3]
 
     def spy(layer, wn, index, seed, rank, pass_, *a, **k):
         if layer is l0:
             seen.append(pass_)
         return orig(layer, wn, index, seed, rank, pass_, *a, **k)
-    wr.noisy_operands = spy
+    o.noisy_operands = spy
     try:
         data = [rng.uniform(-1, 1, (n, d)), rng.uniform(-1, 1, (n, z)), rng.uniform(-1, 1, (n, z)), np.ones((n, 1)), np.zeros((n, 1)), np.ones((n, 1))]
         for _ in range(2):
-            wr.gan_step(G, D, *data)
+            o.gan_step(G, D, *data)
     finally:
-        wr.noisy_operands = orig
+        o.noisy_operands = orig
     assert seen == [0, 0, 1, 2, 2, 3] and D.dropout.pass_ == 4
     assert G.dropout.pass_ == 2                                   # one train-mode pass of G per step (x_fake is an inference pass)
 
@@ -232,16 +233,16 @@ def test_gan_step_reads_g_counters_for_a_scheduled_drop_connect():
     gs = m.mlp_generator(z, hid, d, lr=1e-2)
     ds = m.mlp_discriminator(d, hid, lr=1e-2, drop_connect=m.exponential_schedule(0.8, 0.5))
     rng = np.random.default_rng(3)
-    G = wr.net_from_specs(gs, (z,), seed=1); D = wr.net_from_specs(ds, (d,), seed=2)
+    G = o.net_from_specs(gs, (z,), seed=1); D = o.net_from_specs(ds, (d,), seed=2)
     seen = []
-    orig = wr.drop_connect_p
-    wr.drop_connect_p = lambda wn, c=(0, 0): (seen.append(orig(wn, c)), seen[-1])[1]
+    orig = o.drop_connect_p
+    o.drop_connect_p = lambda wn, c=(0, 0): (seen.append(orig(wn, c)), seen[-1])[1]
     try:
         data = [rng.uniform(-1, 1, (n, d)), rng.uniform(-1, 1, (n, z)), rng.uniform(-1, 1, (n, z)), np.ones((n, 1)), np.zeros((n, 1)), np.ones((n, 1))]
         for _ in range(2):
-            wr.gan_step(G, D, *data)
+            o.gan_step(G, D, *data)
     finally:
-        wr.drop_connect_p = orig
+        o.drop_connect_p = orig
     # three noisy layers per pass; per step the real and fake passes at D's counters, then the generator pass at G's, which lag D's by the
     # D update (at D's the first step's generator pass would read 0.4)
     assert seen[::3] == [np.float32(0.8)] * 3 + [np.float32(0.4)] * 3
