@@ -5,7 +5,10 @@
 - Builders: mlp_convbn_specs (the small MLP and conv + BatchNorm nets), oracle_gan_pair / fp32_gan_pair (the 16x16 DCGAN pair of the
   oracle, and of the library with the oracle's parameters), bf16_gan (the BF16 pair of the launch-count tests).
 - Comparisons: pclose, compare_params_and_state, assert_close_up_to_sign_flips, gan_step_parity, check_bf16, inject_forward and
-  check_weight_operands; launches_per_step counts a GAN step's kernel launches; run_two_ranks runs a tools/ script on two GPUs."""
+  check_weight_operands; launches_per_step counts a GAN step's kernel launches; run_two_ranks runs a tools/ script on two GPUs.
+- Flat vectors and the oracle: push_params / push_state load parameters into the library net and a library updater state into the oracle,
+  state_flat flattens an oracle state slot, grads_by_tensor splits a library gradient vector per oracle tensor, flat_order flattens an oracle
+  gradient like the library; weight_operands reads a BF16 net's bf16 weight copies."""
 import json
 import os
 import subprocess
@@ -47,6 +50,86 @@ def randomize(net, rng, scale=None):
 def push_params(onet, bnet):
     """Copy the oracle's parameters into the CUDA net through getParam/setParam-style calls (DL4J flattened order)."""
     bnet.set_params(onet.params_flat().astype(np.float32))
+
+
+def push_state(onet, st):
+    """Load a library net's updater state vector st (Net.updater_state(): [state0 | state1 (| state2)], each slot in DL4J flattened order)
+    into the oracle's state slots: the inverse of state_flat.  A parameter the oracle keeps no state for must hold zeros in every slot."""
+    n = onet.num_params()
+    slots = st.size // n
+    assert st.size == slots * n, (st.size, n)
+    off = 0
+    for li, name, p, shape, order in onet.param_table():
+        k = int(np.prod(shape))
+        have = onet.state.get((li, p), [])
+        for j in range(slots):
+            v = st[j * n + off:j * n + off + k]
+            if j < len(have):
+                have[j][...] = v.reshape(shape, order=order.upper())
+            else:
+                assert np.all(v == 0), (name, p, "slot", j)
+        off += k
+
+
+def grads_by_tensor(onet, flat, shaped=False):
+    """A flat gradient vector (Net.gradients(), DL4J flattened order) per oracle tensor: {(layer index, param): the tensor's slice}, or with
+    shaped the slice in the tensor's shape (dense W is 'f'-order), what Net.apply_update(grads=...) takes."""
+    out, off = {}, 0
+    for li, l in enumerate(onet.layers):
+        if not l.has_params:
+            continue
+        for pname, shp, order in l.param_specs():
+            n = int(np.prod(shp)); v = flat[off:off + n]; off += n
+            out[(li, pname)] = v.reshape(shp, order=order.upper()) if shaped else v
+    assert off == flat.size
+    return out
+
+
+def flat_order(l, pname):
+    """oracle gradient tensor -> the element order of DL4J's flattened view (dense W is 'f'-order)."""
+    g = np.asarray(l.grads[pname], np.float64)
+    return g.ravel(order="F") if (isinstance(l, o.Dense) and pname == "W") else g.ravel()
+
+
+def rel_fro(a, b):
+    """Relative Frobenius error of a against b."""
+    a = np.asarray(a, np.float64).ravel(); b = np.asarray(b, np.float64).ravel()
+    return float(np.linalg.norm(a - b) / (np.linalg.norm(b) + 1e-30))
+
+
+def check_grads_against_oracle(onet, got_flat, specs, what):
+    """A library gradient vector against the oracle's gradients after its backward, tensor by tensor (the running-stat pseudo-gradients
+    excepted): relative Frobenius error < 3e-2 (about ten bf16-rounded epsilon tensors deep) and cosine > 0.999."""
+    for (li, pname), gv in grads_by_tensor(onet, got_flat).items():
+        if pname in ("mean", "var"):
+            continue
+        ref = flat_order(onet.layers[li], pname)
+        fro = rel_fro(gv, ref); cos = float(np.dot(gv, ref) / (np.linalg.norm(gv) * np.linalg.norm(ref) + 1e-30))
+        assert fro < 3e-2 and cos > 0.999, (f"{what} grad {specs[li].get('name')}.{pname}", fro, cos)
+
+
+def bf16_weights(onet):
+    """Every W of a float32 oracle net rounded to bf16 in place: the operands a BF16 library net's forward reads instead of its fp32 master."""
+    for l in onet.layers:
+        if l.has_params and "W" in l.params:
+            l.params["W"] = bf16_round(l.params["W"]).astype(np.float32)
+
+
+def check_generator_step_grads(G, D, bG, bD, gs, ds, z_g, y_gen, what=""):
+    """After an adversarial step of the library nets bG, bD: G's gradient against the oracle's exact backward of the G step, on the activations
+    of that step's pass injected layer by layer (inject_forward; the pass is each library net's most recent forward), by
+    check_grads_against_oracle.  G, D: the oracle nets (float32) holding the parameters that pass ran with, W rounded to bf16.  what: a prefix
+    of the messages."""
+    n = z_g.shape[0]
+    xg = inject_forward(G, bG, gs, bf16_round(z_g), n, f"{what}G (train, z_g)")
+    inject_forward(D, bD, ds, xg, n, f"{what}D (G step)")
+    _, eps = D.layers[-1].score_and_eps(np.asarray(y_gen, np.float32))
+    if isinstance(D.layers[-1], o.Output):
+        eps = D.layers[-1].backward(eps)
+    eps_g = D.backward_from_prefix(eps).reshape(xg.shape)
+    for l in reversed(G.layers):
+        eps_g = l.backward(eps_g)
+    check_grads_against_oracle(G, bG.gradients(), gs, f"{what}G")
 
 
 def rel_err(a, b):
@@ -301,6 +384,20 @@ def _ps_operand_O(spec):
         return 0
     O, C = (spec["n_in"], spec["n_out"]) if spec["type"] == "deconv2d" else (spec["n_out"], spec["n_in"])
     return O if C <= 4 and O % 64 == 0 else 0
+
+
+def weight_operands(net, specs):
+    """Every bf16 weight operand of a BF16 net, widened to fp32: {(layer name, which): operand}, which 0 the straight copy of W and 1 the
+    packed pixel-shuffle operand of a layer that has one (Net.weight_operand)."""
+    out = {}
+    for li, s in enumerate(specs):
+        if s["type"] not in ("conv2d", "deconv2d", "dense", "output"):
+            continue
+        k = s.get("kernel", (1, 1))
+        out[(s["name"], 0)] = net.weight_operand(li, 0, s["n_in"] * s["n_out"] * k[0] * k[1])
+        if _ps_operand_O(s):
+            out[(s["name"], 1)] = net.weight_operand(li, 1, 144 * _ps_operand_O(s))
+    return out
 
 
 def check_weight_operands(b, net, specs, what):

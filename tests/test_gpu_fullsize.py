@@ -18,7 +18,8 @@ import pytest
 
 import conv_ref
 import tc_schedule
-from helpers import b200, bf16_round, check_bf16, inject_forward
+from helpers import (b200, bf16_round, bf16_weights, check_bf16, check_generator_step_grads, check_grads_against_oracle, flat_order,
+                     grads_by_tensor, inject_forward, rel_fro)
 from oracle import dl4j_oracle as o
 from tc_schedule import pick_row_tile as _pick_row_tile
 
@@ -238,28 +239,6 @@ def test_edge_kernels_full_size(b200):
 # every layer's oracle is evaluated on the GPU's OWN input to that layer, so one layer's bf16 rounding never hides in the next one's
 # tolerance; the backward pass is the oracle's exact backward through the layers whose caches hold those injected activations.
 # ------------------------------------------------------------------------------------------------
-def _fro(a, b):
-    a = np.asarray(a, np.float64).ravel(); b = np.asarray(b, np.float64).ravel()
-    return float(np.linalg.norm(a - b) / (np.linalg.norm(b) + 1e-30))
-
-
-def _grads_by_tensor(onet, flat):
-    out, off = {}, 0
-    for li, l in enumerate(onet.layers):
-        if not l.has_params:
-            continue
-        for pname, shp, _ in l.param_specs():
-            n = int(np.prod(shp)); out[(li, pname)] = flat[off:off + n]; off += n
-    assert off == flat.size
-    return out
-
-
-def _flat_order(l, pname):
-    """oracle gradient tensor -> the element order of DL4J's flattened view (dense W is 'f'-order)."""
-    g = np.asarray(l.grads[pname], np.float64)
-    return g.ravel(order="F") if (isinstance(l, o.Dense) and pname == "W") else g.ravel()
-
-
 STEP_CASES = [("c2", 64, 100, 64, 128), ("c4", 128, 100, 64, 32), ("c5", 0, 128, 1024, 8192)]
 
 
@@ -291,48 +270,22 @@ def test_bf16_whole_step_layer_by_layer(b200, case):
     x2 = np.concatenate([data[0], rng.uniform(-1, 1, data[0].shape).astype(np.float32)]); y2 = np.concatenate([data[3], data[4]])
     bD.compute_gradient_and_score(x2, y2)
     # the tensor-core path holds bf16 weights: the oracle must see the same operands
-    for net in (G, D):
-        for l in net.layers:
-            if l.has_params and "W" in l.params:
-                l.params["W"] = bf16_round(l.params["W"]).astype(np.float32)
+    bf16_weights(G); bf16_weights(D)
     inject_forward(D, bD, ds, bf16_round(x2), 2 * n, "D (2N)")
     loss_sum, eps = D.layers[-1].score_and_eps(y2.astype(np.float32))
     if isinstance(D.layers[-1], o.Output):
         eps = D.layers[-1].backward(eps)
     D.backward_from_prefix(eps)
-    got = _grads_by_tensor(D, bD.gradients())
-    for (li, pname), gv in got.items():
-        if pname in ("mean", "var"):
-            continue
-        ref = _flat_order(D.layers[li], pname)
-        fro = _fro(gv, ref); cos = float(np.dot(gv, ref) / (np.linalg.norm(gv) * np.linalg.norm(ref) + 1e-30))
-        assert fro < 3e-2 and cos > 0.999, (f"D grad {ds[li].get('name')}.{pname}", fro, cos)
+    check_grads_against_oracle(D, bD.gradients(), ds, "D")
     # ---- the adversarial step: afterwards the nets hold the G-step pass (G train forward on z_g, D train forward on G's output)
     pD_before = bD.params()
     gan = b.Gan(bG, bD, use_cuda_graph=False)
     gan.step(*data)
     # D was updated once before the G step ran through it: give the oracle those parameters (G's are still the pre-update ones it ran with)
     D.set_params_flat(bD.params().astype(np.float32))
-    for l in D.layers:
-        if l.has_params and "W" in l.params:
-            l.params["W"] = bf16_round(l.params["W"]).astype(np.float32)
+    bf16_weights(D)
     assert np.abs(bD.params() - pD_before).max() > 0
-    xg = inject_forward(G, bG, gs, bf16_round(data[2]), n, "G (train, z_g)")
-    inject_forward(D, bD, ds, xg, n, "D (G step)")
-    loss_sum, eps = D.layers[-1].score_and_eps(data[5].astype(np.float32))
-    if isinstance(D.layers[-1], o.Output):
-        eps = D.layers[-1].backward(eps)
-    eps_x = D.backward_from_prefix(eps)
-    eps_g = eps_x.reshape(xg.shape)
-    for l in reversed(G.layers):
-        eps_g = l.backward(eps_g)
-    got = _grads_by_tensor(G, bG.gradients())
-    for (li, pname), gv in got.items():
-        if pname in ("mean", "var"):
-            continue
-        ref = _flat_order(G.layers[li], pname)
-        fro = _fro(gv, ref); cos = float(np.dot(gv, ref) / (np.linalg.norm(gv) * np.linalg.norm(ref) + 1e-30))
-        assert fro < 3e-2 and cos > 0.999, (f"G grad {gs[li].get('name')}.{pname}", fro, cos)
+    check_generator_step_grads(G, D, bG, bD, gs, ds, data[2], data[5])
     assert bD.simt_gemm_calls() > 0        # the skinny layers (the logit; z -> 4x4 in the DCGANs) are SIMT by design, and counted
     gan.close(); bG.close(); bD.close()
 
@@ -418,21 +371,21 @@ def _oracle_grads(onet):
     for li, l in enumerate(onet.layers):
         if l.has_params:
             for pname, _, _ in l.param_specs():
-                out[(li, pname)] = _flat_order(l, pname)
+                out[(li, pname)] = flat_order(l, pname)
     return out
 
 
 def _check_grads(got_flat, want, onet, specs, what, fro_bound, errs, injected=True):
     """injected: the oracle ran on the GPU's own activations, so the running-statistic pseudo-gradients (1 - decay) * (running - batch
     statistic) must match to 1e-4 relative; otherwise they are held to the Frobenius bound like every other gradient."""
-    got = _grads_by_tensor(onet, got_flat)
+    got = grads_by_tensor(onet, got_flat)
     for (li, pname), gv in got.items():
         ref = want[(li, pname)]
         if injected and pname in ("mean", "var"):
             e = float(np.abs(gv - ref).max() / (np.abs(ref).max() + 1e-30))
             assert e <= 1e-4, (f"{what}: {specs[li].get('name')}.{pname}", e)
             continue
-        fro = _fro(gv, ref); errs.append(fro)
+        fro = rel_fro(gv, ref); errs.append(fro)
         if fro_bound is not None:
             assert fro <= fro_bound, (f"{what}: {specs[li].get('name')}.{pname}", fro, fro_bound)
 
@@ -452,10 +405,7 @@ def test_bf16_ragged_batch_routes_layer_by_layer(b200, n):
     bG = b.Net(ctx, gs, (z,), max_batch=n, precision=b.BF16, xent_clip_eps=0.0)
     bD = b.Net(ctx, ds, dshape, max_batch=2 * n, precision=b.BF16, xent_clip_eps=0.0, bn_groups=2)
     push_params(G, bG); push_params(D, bD)
-    for net in (G, D):
-        for l in net.layers:
-            if l.has_params and "W" in l.params:
-                l.params["W"] = bf16_round(l.params["W"]).astype(np.float32)
+    bf16_weights(G); bf16_weights(D)
     routes = _sweep_routes(n)
     errs = []
     # ---- the SIMT count of a train-mode forward is the table's (the D pass and D.output see the same 2N rows)
@@ -506,9 +456,7 @@ def test_bf16_ragged_batch_routes_layer_by_layer(b200, n):
     # ---- the generator step: G train forward on z_g and D forward on its output, injected; every G gradient incl. mean / var
     D.layers = [copy.deepcopy(l) for l in D0]
     D.set_params_flat(bD.params().astype(np.float32))
-    for l in D.layers:
-        if l.has_params and "W" in l.params:
-            l.params["W"] = bf16_round(l.params["W"]).astype(np.float32)
+    bf16_weights(D)
     xg = inject_forward(G, bG, gs, bf16_round(data[2]), n, f"G (train, N = {n})")
     inject_forward(D, bD, ds, xg, n, f"D (G step, N = {n})")
     _, eps = D.layers[-1].score_and_eps(data[5].astype(np.float32))
